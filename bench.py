@@ -1,13 +1,15 @@
-"""bench.py -- SAC grad-steps/sec (batch 256, 64x64 depth) on N B200s.
+"""bench.py -- SAC grad-steps/sec (batch 256, 64x64 depth) on N H100s.
 
   python bench.py --gpus N --steps K --warmup W             (N>1: launched under torchrun)
+  python bench.py ... --dump-outputs DIR                    (also writes the last timed step's outputs as DIR/*.npy)
   python bench.py --impl reference ...                      (CPU arm: the oracle restatement of
                                                              SB2.10.1/TF1.14's SAC step, all host cores)
 
 A "step" = one SAC minibatch gradient step (replay sample -> VecNormalize -> 3 CNN fwd, 2 CNN bwd,
 heads, losses -> [all-reduce] -> 3x Adam -> Polyak) at batch 256 per GPU on synthetic 64x64x2 depth
 observations (BASELINE.json configs[1]).  `value` times K steps with the replay already resident in
-HBM (CUDA events, max over ranks); `e2e` times the same step through the C-ABI parity entry point
+HBM (CUDA events, max over ranks; the K steps are split into timed regions and the median region rate is
+reported; K is exactly the number of steps behind `value`, the secondary figures use counts derived from it, see --help); `e2e` times the same step through the C-ABI parity entry point
 with HOST (pinned) batches, i.e. host->device copies of the batch and device->host read of the
 losses inside the timed region.  Weak scaling: every rank processes its own 256-sample minibatch
 and one NCCL all-reduce averages the gradients, so N ranks = one step on a global batch of N*256;
@@ -36,9 +38,10 @@ sys.path.insert(0, ROOT)
 GOLD = os.path.join(ROOT, "tests", "golden")
 FLOP_PER_STEP_B256 = 2 * 256 * 18_923_328          # SURVEY.md section 8d: 9.689 GFLOP
 LR = 3e-4
-KERNEL_DESC = ("cg_kernel (TMA-fed tcgen05 contraction engine, csrc/cg.cu): converged producer warps issue cp.async.bulk.tensor boxes -- "
+KERNEL_DESC = ("cg_kernel (TMA-fed wgmma contraction engine, csrc/cg.cu): converged producer warps issue cp.async.bulk.tensor boxes -- "
                "implicit-im2col / shifted-window / zero-bordered tensor-map views of the BF16 activation planes, all planes of an operand in one "
-               "box -- into a 128B-swizzled smem ring; tcgen05.mma kind::f16 with fp32 TMEM accumulators, one wide MMA per operand plane; "
+               "box -- into a 128B-swizzled smem ring; two consumer warpgroups issue wgmma.mma_async with fp32 register accumulators, one wide "
+               "MMA per operand plane; "
                "forward = 6-product 3-plane split, backward = 3-product 2-plane split; TWO persistent launches per step (forward chain "
                "conv1..fc0, backward chain heads dgrad..conv wgrads), layers chained tile by tile through arrival counters")
 WORKLOAD = "SAC depth CNN (config/gripper_grasp.yaml), batch 256/GPU, 64x64x2 obs, 1M-slot replay"
@@ -49,7 +52,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d["bf16_tflops"], d["hbm_gbs"], "measured (MEASURED_PEAKS.json, burst)"
-    return 1590.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, "NVIDIA H100 SXM data sheet (dense BF16, HBM3; 700 W card)"
 
 
 class ClockSampler:
@@ -172,6 +175,17 @@ def run_reference(args):
     emit(json.dumps(line))
 
 
+def dump_outputs(out_dir, metrics, params):
+    """The last timed step's results as out_dir/<name>.npy: every loss / metric it returned (float64 scalars) and every
+    parameter tensor it left behind (float32; 7.4 MB for the depth CNN).  The inputs are fixed by the seeds, so two builds run
+    with the same arguments can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in metrics.items():
+        np.save(os.path.join(out_dir, f"metric_{k}.npy"), np.asarray(v, np.float64))
+    for k, v in params.items():
+        np.save(os.path.join(out_dir, "param_" + k.replace("/", "__") + ".npy"), np.asarray(v, np.float32))
+
+
 def numa_bind(dev):
     """Binds this process to the host CPUs local to GPU `dev` (sysfs local_cpulist of its PCI function) BEFORE the
     pinned e2e buffers are allocated, so that their pages and the copy-issuing thread sit on the GPU's NUMA node.
@@ -214,25 +228,34 @@ def fill_replay(L, vn, n_fill, rank, distinct_chunks=8, chunk=2048):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=200,
+                    help="K: the exact number of timed steps behind `value` (device-resident, graph mode). The secondary measurements "
+                         "derive their own counts from K: e2e, unpipelined and learn-loop paths max(10, min(K, 200)) steps per run, "
+                         "the RGB-D extra (c3) max(20, K // 4) steps per region")
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--batch", type=int, default=256)
-    ap.add_argument("--replay-filled", type=int, default=65536, help="transitions resident in HBM (2 x 32 KiB each: 4 GiB >> 126 MB L2)")
+    ap.add_argument("--replay-filled", type=int, default=65536, help="transitions resident in HBM (2 x 32 KiB each: 4 GiB >> 50 MB L2)")
     ap.add_argument("--buffer-size", type=int, default=1_000_000)
-    ap.add_argument("--regions", type=int, default=7, help="timed K-step regions; the MEDIAN region is reported")
+    ap.add_argument("--regions", type=int, default=7, help="the K timed steps are split into this many regions; the MEDIAN region is reported")
     ap.add_argument("--cpu-seconds", type=float, default=12.0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--dp", default="p2p", choices=["p2p", "nccl"],
                     help="N > 1: p2p = the optimiser launch reduces / updates / broadcasts over NVLink peer memory; nccl = all-reduce + replicated Adam")
     ap.add_argument("--no-c3", action="store_true", help="skip the RGB-D B=1024 extra measurement (config.extra.c3)")
     ap.add_argument("--precision", default="bf16x3", choices=["fp32", "bf16x3", "bf16"],
-                    help="bf16x3 = tcgen05 BF16 hi/lo split, the mode that passes the 1e-4 parity tests (default)")
+                    help="bf16x3 = wgmma BF16 hi/lo split, the mode that passes the 1e-4 parity tests (default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (its losses and metrics) and the parameters it "
+                         "left, as DIR/<name>.npy (float64 / float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
     args.warmup = max(args.warmup, 3)
-    args.regions = max(args.regions, 5)
+    args.steps = max(args.steps, 1)
+    args.regions = max(1, min(args.regions, args.steps))
+    # exactly K timed steps: region i runs K // R steps, the first K % R regions one more
+    region_steps = [args.steps // args.regions + (1 if i < args.steps % args.regions else 0) for i in range(args.regions)]
 
     import torch
     import torch.distributed as dist
@@ -303,23 +326,28 @@ def main():
             parity = {"oracle_batch": B * world, "rel_err": {k: float(f"{v:.3g}") for k, v in errs.items()}, "q1_rel_err_rank0": float(f"{q_err:.3g}"),
                       "tol": 1e-4, "first_step_ok": bool(max(errs.values()) <= 1e-4 and q_err <= 1e-4)}
 
-    # ---- device-resident throughput: R regions of exactly K graph replays each, CUDA events on the learner's stream
+    # ---- device-resident throughput: K graph replays in R regions, CUDA events on the learner's stream
     # (b2g_sac_step brackets the K launches with events), barrier + synchronize on both sides of every region, max over
     # ranks per region, MEDIAN over regions.  Inputs: random slots of a replay working set far larger than L2.
     L.step(args.warmup, lr=LR)
     barrier()
     region_ms = []
+    last_metrics = None
     with ClockSampler(local) as clk:
         time.sleep(0.25)                       # let the sampler stream before the timed regions start
-        for _ in range(args.regions):
+        for k in region_steps:
             barrier()
-            L.step(args.steps, lr=LR)          # one timed region: exactly K steps
+            last_metrics = L.step(k, lr=LR)    # one timed region of k steps; returns the losses of its last step
             region_ms.append(L.last_step_ms())
         barrier()
     region_ms = max_over_ranks(region_ms)
-    ms = float(np.median(region_ms))
-    sync_steps_per_s = args.steps / (ms * 1e-3)
+    ms_per_step_regions = [m / k for m, k in zip(region_ms, region_steps)]
+    ms_step = float(np.median(ms_per_step_regions))
+    ms = ms_step * args.steps                  # K steps at the median region rate
+    sync_steps_per_s = 1e3 / ms_step
     value = world * sync_steps_per_s
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_metrics, L.get_parameters())
 
     # ---- end to end through the C ABI with pinned HOST batches (H2D of the batch + D2H of the losses per step)
     tr = synth.make_transitions(B, vn["obs_mean"], vn["obs_var"], seed=77 + rank)
@@ -394,7 +422,7 @@ def main():
 
     c3 = None
     if rank == 0 and world == 1 and not args.no_c3 and prec != 0:
-        # BASELINE.json configs[2]: SAC RGB-D (64x64x4 image + feature plane), batch 1024, one B200
+        # BASELINE.json configs[2]: SAC RGB-D (64x64x4 image + feature plane), batch 1024, one GPU
         vn5 = dict(np.load(os.path.join(GOLD, "vecnorm_sac_rgbd.npz")))
         L3 = b200grasp.Learner((64, 64, 5), n_act=5, batch_size=1024, buffer_size=8192, seed=99, device=local, precision=prec)
         L3.set_norm_stats(vn5["obs_mean"], vn5["obs_var"], float(vn5["ret_var"]), float(vn5["clip_obs"]), float(vn5["clip_reward"]),
@@ -422,22 +450,12 @@ def main():
                        or k.startswith("heads_fc0") or k == "heads_dgrad" or (k == "heads_wgrad" and "fwd_fused" not in prof)}
         gemm_serial = sum(gemm_groups.values())
         share = gemm_serial / sum(prof.values())
-        ms_step = ms / args.steps
         gemm_ms = share * ms_step
         peak_tf, peak_hbm, peak_src = peaks()
         flops = FLOP_PER_STEP_B256 * B / 256
         achieved = flops / (gemm_ms * 1e-3) / 1e12
-        traffic = None
-        tnote = None
-        for tname in ("traffic_r2.json", "traffic_r1.json"):
-            tpath = os.path.join(ROOT, "profiles", tname)
-            if os.path.exists(tpath):          # dram read+write per tensor-engine launch from the committed ncu --set full capture
-                tj = json.load(open(tpath))
-                traffic = tj.get("dram_bytes_per_launch", tj.get("gg_tc_kernel_dram_bytes_per_launch"))
-                tnote = f"profiles/{tname}: ncu dram__bytes_read.sum + dram__bytes_write.sum per tensor-engine launch (mean over the step's launches)"
-                break
         roofline = {"bound": "tensor", "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf,
-                    "traffic": traffic, "traffic_unit": tnote,
+                    "traffic": None,
                     "kernel": KERNEL_DESC if prec else "gg_simt_kernel (fp32 FFMA engine)",
                     "peak_source": peak_src, "launch_ms": gemm_ms, "launches": len(gemm_groups),
                     "launch_ms_note": "tensor-engine share of the serial per-launch profile x graph-mode ms_per_step",
@@ -455,9 +473,9 @@ def main():
             "scaling": "weak", "vs_baseline": None, "dtype": {"fp32": "f32", "bf16x3": "bf16x3 (fp32-faithful split, f32 accumulate)", "bf16": "bf16"}[args.precision], "data": "synthetic",
             "config": {"workload": WORKLOAD,
                        "global_batch": B * world, "replay_capacity": args.buffer_size, "replay_filled": args.replay_filled,
-                       "l2": f"inputs larger than L2: replay working set {args.replay_filled * 2 * 32768 / 2**30:.1f} GiB >> 126 MB; minibatch slots are random per step",
-                       "timing": f"median of {args.regions} regions of {args.steps} steps (CUDA events on the learner's stream, max over ranks per region); regions_ms={[round(x, 3) for x in region_ms]}",
-                       "precision": {"fp32": "fp32 FFMA (B2G_PREC_FP32_SIMT)", "bf16x3": "tcgen05 BF16 hi/lo split x3, fp32 TMEM accumulate (B2G_PREC_BF16X3; passes 1e-4 parity)", "bf16": "tcgen05 single-pass BF16 (fast mode, ~5e-4 on Q)"}[args.precision], "parallelism": f"dp{world}" + ("" if world == 1 else (" (gradients reduced, slices updated and parameters broadcast by one kernel over NVLink peer memory)" if args.dp == "p2p" else " (NCCL all-reduce, replicated Adam)")),
+                       "l2": f"inputs larger than L2: replay working set {args.replay_filled * 2 * 32768 / 2**30:.1f} GiB >> 50 MB; minibatch slots are random per step",
+                       "timing": f"{args.steps} steps in {args.regions} regions of {region_steps} steps, median region rate (CUDA events on the learner's stream, max over ranks per region); regions_ms={[round(x, 3) for x in region_ms]}",
+                       "precision": {"fp32": "fp32 FFMA (B2G_PREC_FP32_SIMT)", "bf16x3": "wgmma BF16 hi/lo split x3, fp32 accumulate (B2G_PREC_BF16X3; passes 1e-4 parity)", "bf16": "wgmma single-pass BF16 (fast mode, ~5e-4 on Q)"}[args.precision], "parallelism": f"dp{world}" + ("" if world == 1 else (" (gradients reduced, slices updated and parameters broadcast by one kernel over NVLink peer memory)" if args.dp == "p2p" else " (NCCL all-reduce, replicated Adam)")),
                        "sync_steps_per_s": sync_steps_per_s, "numa": numa,
                        "extra": {"c3": c3}},
             "clocks": clk.summary(),

@@ -1,9 +1,9 @@
 #!/bin/bash
-# Builds libb200grasp.so (sm_100a only) in-tree.  nvcc cross-compiles without a GPU.
+# Builds libb200grasp.so (sm_90a only) in-tree.  nvcc cross-compiles without a GPU.
 set -e
 cd "$(dirname "$0")/deep-rl-grasping_b200"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -Wall -Xcompiler -fopenmp"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -Wall -Xcompiler -fopenmp"
 mkdir -p build
 objs=""
 pids=""
@@ -21,5 +21,5 @@ for f in csrc/*.cu; do
   objs="$objs $o"
 done
 for p in $pids; do wait $p || { echo "build.sh: compilation failed" >&2; exit 1; }; done
-$NVCC -gencode arch=compute_100a,code=sm_100a -shared -o libb200grasp.so $objs -ldl -lgomp
+$NVCC -gencode arch=compute_90a,code=sm_90a -shared -o libb200grasp.so $objs -ldl -lgomp
 echo "built $(pwd)/libb200grasp.so"

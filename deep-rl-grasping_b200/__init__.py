@@ -1,4 +1,4 @@
-"""b200grasp -- B200-native SAC learner behind the stable-baselines model API used by
+"""b200grasp -- H100-native SAC learner behind the stable-baselines model API used by
 BarisYazici/deep-rl-grasping (manipulation_main/training/sb_helper.py:104-128,175).
 
 Import as ``b200grasp`` (``b200grasp.py`` at the repo root aliases this directory, whose name

@@ -1,7 +1,7 @@
 """ctypes binding of libb200grasp.so (the C ABI in include/b200grasp.h).
 
 The product path has NO CPU fallback: if the shared library is missing this raises, and if it
-loads on a box without an sm_100 GPU ``b2g_sac_create`` fails with B2G_ECUDA.
+loads on a machine without an sm_90 (Hopper) GPU ``b2g_sac_create`` fails with B2G_ECUDA.
 """
 from __future__ import annotations
 

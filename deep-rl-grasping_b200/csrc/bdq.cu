@@ -508,7 +508,7 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
   BCK(cudaSetDevice(cfg->device));
   cudaDeviceProp prop{};
   BCK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) return bfail(B2G_ECUDA, std::string("libb200grasp is built for sm_100a only; found ") + prop.name);
+  if (prop.major != 9) return bfail(B2G_ECUDA, std::string("libb200grasp is built for sm_90a only; found ") + prop.name);
   b2g_bdq* h = new b2g_bdq();
   h->cfg = *cfg;
   h->cfg.nccl_id = nullptr; h->cfg.nccl_lib = nullptr;

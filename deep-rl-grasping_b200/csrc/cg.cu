@@ -1,17 +1,16 @@
-// TMA-fed tcgen05 contraction engine (sm_100a).  See cg.cuh for the problem description.
+// TMA-fed wgmma contraction engine (sm_90a).  See cg.cuh for the problem description.
 //
 // Persistent, warp-specialised kernel, one CTA per SM, grid = min(#tiles, #SMs):
-//   warps 0..1  : TMA producers (whole warps, converged; one elected lane issues).  The cp.async.bulk.tensor boxes of a K-chunk
-//                 (operands x planes) are dealt round-robin to the two warps; warp 0 posts the chunk's expect_tx.  More issuing
-//                 warps do not help: with 2 or 4 the 72 KB of a 3-plane chunk take ~1400 cycles to land either way (51 B/clk
-//                 per SM, ~14 TB/s chip-wide out of L2 -- profiles/cg_trace_r2.txt), which is the fabric, not the issue rate;
-//   warp 2      : owns the TMEM allocation; converged warp, one elected lane issues tcgen05.mma.cta_group::1.kind::f16 (BF16
-//                 planes, fp32 accumulation in TMEM, two accumulator buffers so the epilogue of tile i overlaps the mainloop
-//                 of tile i+1).  Precision modes per problem: 1 product (hi*hi), 3 products (2-plane split) or 6 products
-//                 (3-plane split hi/mid/lo: everything down to 2^-24), issued as 1..3 WIDE MMAs per k-step (see the issue
-//                 loop) -- profiles/precision_r2.md explains why the forward pass needs the 6-product mode;
-//   warps 3..10 : epilogue.  tcgen05.ld one accumulator row per thread, apply bias/ReLU or the ReLU mask (+ the bias-gradient column
-//                 sums), split into BF16 planes and store the row's 32 columns of every plane directly (16-byte vectors).
+//   warps 0..7  : two consumer warpgroups.  Warpgroup w issues wgmma.mma_async for rows [64w, 64w + 64) of the 128-row tile
+//                 (BF16 planes from the swizzled ring, fp32 accumulators in registers).  Precision modes per problem: 1 product
+//                 (hi*hi), 3 products (2-plane split) or 6 products (3-plane split hi/mid/lo: everything down to 2^-24), issued as
+//                 1..3 WIDE MMAs per k-step (see mma_tile).  After the last K-chunk the same warps run the epilogue: the
+//                 accumulator columns pass, 16 at a time, through a small shared-memory staging block so that every lane ends up
+//                 with one output row; then bias/ReLU or the ReLU mask (+ the bias-gradient column sums), the split into BF16
+//                 planes and the row's 32-column stores of every plane (16-byte vectors).  The producers keep filling the ring
+//                 for the next tile meanwhile;
+//   warps 8..9  : TMA producers (whole warps, converged; one elected lane issues).  The cp.async.bulk.tensor boxes of a K-chunk
+//                 (operands x planes) are dealt round-robin to the two warps; warp 8 posts the chunk's expect_tx.
 #include <cuda_bf16.h>
 
 #include <cstdio>
@@ -19,15 +18,15 @@
 
 #include "cg.cuh"
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace b2g {
 namespace {
 
-// warps 0..1: TMA producers, warp 2: MMA issuer (owns TMEM), warps 3..10: epilogue
-constexpr int NPROD_WARPS = 2, MMA_WARP = NPROD_WARPS;
-constexpr int EPI_WARP0 = NPROD_WARPS + 1, NEPI_WARPS = CG_EPI_WARPS;
-constexpr int NTHREADS = 32 * (EPI_WARP0 + NEPI_WARPS);
-constexpr int TMEM_COLS = 512;          // two accumulators of up to 256 fp32 columns
+// warps 0..7: consumer warpgroups (MMA + epilogue), warps 8..9: TMA producers
+constexpr int NEPI_WARPS = CG_EPI_WARPS, NPROD_WARPS = 2, PROD_WARP0 = NEPI_WARPS;
+constexpr int NTHREADS = 32 * (NEPI_WARPS + NPROD_WARPS);
+constexpr int STG_BYTES = 2 * 64 * 16 * 4;    // epilogue staging: per warpgroup 64 rows x 16 fp32 columns (rows of 64 B)
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -49,10 +48,9 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "}" ::"r"(bar), "r"(parity)
       : "memory");
 }
-// one lane of a CONVERGED warp.  The producer and MMA roles run their loops with all 32 lanes so that every address,
-// descriptor and coordinate is warp-uniform and lives in the uniform register file UTMALDG / UTCHMMA read; a role entered
-// by one lane only (if (lane == 0) {...}) made the compiler wrap every such instruction in an R2UR + ELECT/BRA.U.ANY
-// value-serialisation loop -- ~75 cycles per MMA issued (profiles/cg_trace_r2.txt).
+// one lane of a CONVERGED warp.  The producer warps run their loops with all 32 lanes so that every address and coordinate
+// is warp-uniform and can live in the uniform registers the TMA instruction reads; a role entered by one lane only
+// (if (lane == 0) {...}) lets the compiler wrap each such instruction in a value-serialisation loop.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -64,35 +62,11 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// shared-memory matrix descriptors (cute::UMMA::SmemDescriptor): start >> 4 in [0,14), LBO >> 4 in [16,30), SBO >> 4 in
-// [32,46), version 1 in [46,48), layout type 2 = SWIZZLE_128B in [61,64).  K-major: rows of 128 B, 8-row groups 1024 B
-// apart (SBO), LBO unused.  MN-major: rows = K, 128 B = 64 elements along M|N; SBO = stride between 8-row K groups
-// (1024 B inside a TMA box), LBO = stride between 64-element atoms along M|N (one box each).
-__device__ __forceinline__ uint64_t desc_k(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ uint64_t desc_mn(uint32_t saddr, uint32_t lbo) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// kind::f16 instruction descriptor: D = f32 (bit 4), A = B = BF16 (bits 7, 10), MN-major A / B (bits 15, 16), N >> 3 at 17, M >> 4 at 24
-__device__ __forceinline__ uint32_t make_idesc(int m, int n, bool mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (mn_major ? (3u << 15) : 0u) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
+// shared-memory matrix descriptors (SWIZZLE_128B, wgmma.cuh).  K-major: rows of 128 B, 8-row groups 1024 B apart (SBO), LBO
+// unused.  MN-major: rows = K, 128 B = 64 elements along M|N; SBO = stride between 8-row K groups (1024 B inside a TMA box),
+// LBO = stride between 64-element atoms along M|N (one box each).
+__device__ __forceinline__ uint64_t desc_k(uint32_t saddr) { return wg_desc(saddr, 16, 1024); }
+__device__ __forceinline__ uint64_t desc_mn(uint32_t saddr, uint32_t lbo) { return wg_desc(saddr, lbo, 1024); }
 
 __device__ __forceinline__ void tma_load(uint32_t dst, const CUtensorMap* map, uint32_t bar, int rank, const int (&c)[5]) {
   switch (rank) {
@@ -121,8 +95,7 @@ __device__ __forceinline__ void tma_load(uint32_t dst, const CUtensorMap* map, u
 }
 
 // The problem list lives in the kernel-parameter constant bank: every role re-reads descriptor fields per tile, and a
-// constant-cache hit costs tens of cycles where a global-memory descriptor cost a dependent L2 round trip per field
-// group (the "skeleton" of the round-1 engine: profiles/tc_ablation_r1.txt).
+// constant-cache hit costs far less than the dependent L2 round trip per field group of a descriptor in global memory.
 struct CgPack { CgProblem p[CG_MAX_PROBLEMS]; };
 struct Tile { int p, tm, tn, c_begin, c_end; };
 // Tile walker: a CTA's tiles increase monotonically, so the problem index only moves forward and the tile-grid fields of
@@ -160,35 +133,138 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {    // lo -
   return d;
 }
 
+// The MMAs of one K-chunk for this warpgroup's m64 block: `planes` wide MMAs per k-step, A_p x [B_0 | .. | B_(planes-1-p)] ->
+// accumulator columns [p*n, planes*n).  Column group g therefore collects the products of order 2^(-8g): g0 = hi*hi,
+// g1 = hi*mid + mid*hi, g2 = hi*lo + mid*mid + lo*hi; keeping each order in its own columns keeps the accumulator's rounding
+// 2^-8g smaller on the correction terms, and the epilogue adds the groups small-to-large in fp32.  One wide MMA reads the A plane
+// from shared memory once for up to three products.  Column offset n is register offset n / 2 of the fragment (wgmma.cuh).
+// Tile width, product count and operand major-ness are template parameters: a run-time choice between wgmma sequences puts the
+// instructions on divergent paths, where the compiler serialises them.
+template <int NT, int NPROD, int TRANS, int NACC>
+__device__ __forceinline__ void mma_chunk(float (&acc)[NACC], uint32_t sbase, int ksteps, uint32_t a_off, uint32_t b_off, uint32_t a_ks,
+                                          uint32_t b_ks, uint32_t a_lbo, uint32_t b_lbo, uint32_t a_ps, uint32_t m_off) {
+  static_assert(NACC == NT / 2 * (NPROD >= 6 ? 3 : (NPROD >= 3 ? 2 : 1)) && (NPROD >= 6 ? 3 : (NPROD >= 3 ? 2 : 1)) * NT <= 256,
+                "accumulator of `planes` column groups of NT columns, at most 256 columns wide");
+  for (int k = 0; k < ksteps; ++k) {
+    const uint32_t pb = sbase + b_off + (uint32_t)k * b_ks;
+    const uint64_t db = TRANS ? desc_mn(pb, b_lbo) : desc_k(pb);
+    uint64_t da[3];
+#pragma unroll
+    for (int pl = 0; pl < 3; ++pl) {
+      const uint32_t pa = sbase + (uint32_t)pl * a_ps + a_off + (uint32_t)k * a_ks + m_off;
+      da[pl] = TRANS ? desc_mn(pa, a_lbo) : desc_k(pa);
+    }
+    if constexpr (NPROD >= 6) {
+      Wgmma<3 * NT, TRANS>::mma(acc, da[0], db);
+      Wgmma<2 * NT, TRANS>::mma(acc + NT / 2, da[1], db);
+      Wgmma<NT, TRANS>::mma(acc + NT, da[2], db);
+    } else if constexpr (NPROD >= 3) {
+      Wgmma<2 * NT, TRANS>::mma(acc, da[0], db);
+      Wgmma<NT, TRANS>::mma(acc + NT / 2, da[1], db);
+    } else {
+      Wgmma<NT, TRANS>::mma(acc, da[0], db);
+    }
+  }
+}
+
+// Consumer side of one tile with tile width NT, NPROD products per k-step and TRANS = MN-major operands: mainloop over the
+// tile's K-chunks, then the accumulators to one row per lane.  `s` / `ph`: ring slot and per-slot phase bits, carried by the
+// caller across tiles.  body(g, x) runs the epilogue of column group g of this thread's row (x = its 32 accumulator sums).
+template <int NT, int NPROD, int TRANS, class Body>
+__device__ __forceinline__ void consume_tile(const CgProblem& P, const Tile& ti, uint32_t ring, uint32_t stg, int slot_bytes, int nstages, uint32_t& s,
+                                             uint32_t& ph, uint64_t* bar_full, uint64_t* bar_empty, bool nomma, Body&& body) {
+  constexpr int NGRP = NPROD >= 6 ? 3 : (NPROD >= 3 ? 2 : 1);     // accumulator column groups (product orders)
+  constexpr int NACC = NT / 2 * NGRP;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int wg = warp >> 2, wl = warp & 3, half = wl >> 1;
+  float acc[NACC];
+#pragma unroll
+  for (int j = 0; j < NACC; ++j) acc[j] = 0.f;
+  const uint32_t a_ps = (uint32_t)P.a_pstride, a_off = P.a_off, b_off = P.b_off, a_ks = P.a_kstep, b_ks = P.b_kstep;
+  const uint32_t a_lbo = P.a_lbo, b_lbo = P.b_lbo;
+  const uint32_t m_off = TRANS ? (uint32_t)wg * a_lbo : (uint32_t)wg * 8192u;     // rows [64 wg, 64 wg + 64) of the A tile
+  const int ksteps = nomma ? 0 : P.ksteps;
+  for (int c = ti.c_begin; c < ti.c_end; ++c) {
+    mbar_wait(smem_u32(&bar_full[s]), (ph >> s) & 1u);
+    const uint32_t sbase = ring + s * (uint32_t)slot_bytes;
+    wg_arrive();
+    mma_chunk<NT, NPROD, TRANS>(acc, sbase, ksteps, a_off, b_off, a_ks, b_ks, a_lbo, b_lbo, a_ps, m_off);
+    wg_commit();
+    wg_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(&bar_empty[s]));      // the slot may be refilled
+    ph ^= 1u << s;
+    if (++s == (uint32_t)nstages) s = 0;
+  }
+  // correction column groups, smallest order first
+  if constexpr (NGRP > 2) {
+#pragma unroll
+    for (int j = 0; j < NT / 2; ++j) acc[j] = acc[j] + (acc[j + NT / 2] + acc[j + NT]);
+  } else if constexpr (NGRP > 1) {
+#pragma unroll
+    for (int j = 0; j < NT / 2; ++j) acc[j] = acc[j] + acc[j + NT / 2];
+  }
+  // Fragments -> one row per lane, 16 columns at a time through the warpgroup's staging block (rows of 64 B, 16-byte chunks
+  // XOR-swizzled by row pair).  Warp wl & 1 of a warpgroup owns rows 32 (wl & 1) .. + 31 and `half` the parity of its column
+  // groups; a pair of column groups (64 columns) is gathered in four steps, then every warp runs the epilogue of its group.
+  const int rrow = 32 * (wl & 1) + lane;
+  const uint32_t wstg = stg + (uint32_t)wg * 4096u;
+#pragma unroll
+  for (int R = 0; R < (NT + 63) / 64; ++R) {
+    float x[32];
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const int c0 = 64 * R + 16 * t;              // first column of this step: group 2R + (t >> 1), columns 16 (t & 1) .. of it
+      if (c0 < NT) {
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");     // the previous step's readers are done
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = 16 * wl + (lane >> 2) + 8 * h, chunk = 2 * jj + ((lane & 3) >> 1);
+            const int j = c0 / 8 + jj;
+            const uint32_t a = wstg + (uint32_t)row * 64u + (uint32_t)((chunk ^ ((row >> 1) & 3)) << 4) + (uint32_t)((lane & 1) * 8);
+            asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(a), "f"(acc[4 * j + 2 * h]), "f"(acc[4 * j + 2 * h + 1]) : "memory");
+          }
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+        if (half == (t >> 1)) {
+#pragma unroll
+          for (int cc = 0; cc < 4; ++cc) {
+            const uint32_t a = wstg + (uint32_t)rrow * 64u + (uint32_t)((cc ^ ((rrow >> 1) & 3)) << 4);
+            float* xd = x + 16 * (t & 1) + 4 * cc;
+            asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(xd[0]), "=f"(xd[1]), "=f"(xd[2]), "=f"(xd[3]) : "r"(a));
+          }
+        }
+      }
+    }
+    const int g = 2 * R + half;
+    if (32 * g < NT) body(g, x);
+  }
+}
+
+// 10 warps per CTA: the SM sub-partition that holds three of them caps the kernel at 168 registers per thread.
 __global__ void __launch_bounds__(NTHREADS, 1)
 cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const CUtensorMap* __restrict__ maps, int max_stages,
-          int dbg, long long* __restrict__ trace, int epi_tiles) {
+          int dbg, long long* __restrict__ trace) {
   const CgProblem* __restrict__ probs = pk.p;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_full[CG_MAX_STAGES], bar_empty[CG_MAX_STAGES], bar_acc_full[2], bar_acc_empty[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t bar_full[CG_MAX_STAGES], bar_empty[CG_MAX_STAGES];
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);          // warp-uniform for the compiler, not just in fact
   const int trace_cta = dbg >> 8;                    // bring-up: the CTA whose roles write clock stamps
   const bool dbg_noload = dbg & 1, dbg_nomma = dbg & 2, dbg_nostore = dbg & 4, dbg_nost = dbg & 16;    // 16: epilogue math without the global stores
   if (tid == 0) {
-    for (int s = 0; s < max_stages; ++s) { mbar_init(smem_u32(&bar_full[s]), 1); mbar_init(smem_u32(&bar_empty[s]), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(smem_u32(&bar_acc_full[b]), 1); mbar_init(smem_u32(&bar_acc_empty[b]), epi_tiles ? NEPI_WARPS / 2 : NEPI_WARPS); }
+    for (int s = 0; s < max_stages; ++s) { mbar_init(smem_u32(&bar_full[s]), 1); mbar_init(smem_u32(&bar_empty[s]), NEPI_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t ring = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t stg = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t ring = stg + STG_BYTES;
   pdl_trigger();
   pdl_wait();
 
-  if (warp < NPROD_WARPS) {
+  if (warp >= PROD_WARP0) {
+    const int pw = warp - PROD_WARP0;
     // ============================================================================================ TMA producers
     {
       // Ring slot s and the phase parity of every slot (bit s of ph): the partition of the ring (slot size, slot count) belongs
@@ -215,7 +291,7 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
           const int* __restrict__ ctr = P.dep_ctr;
           const int x0 = P.dep_by_chunk ? ti.c_begin : ti.tm, x1 = P.dep_by_chunk ? ti.c_end : ti.tm + 1;
           const int lo = x0 * P.dep_rows / P.dep_rows_tile, hi = min(P.dep_tiles - 1, (x1 * P.dep_rows - 1) / P.dep_rows_tile);
-          const int expect = P.dep_expect * (epi_tiles ? NEPI_WARPS / 2 : NEPI_WARPS);
+          const int expect = P.dep_expect * NEPI_WARPS;
           for (int j = lo + lane; j <= hi; j += 32) {
             int seen;
             do {
@@ -239,15 +315,15 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
         }
         int c1 = n2 > 1 ? ti.c_begin / n2 : 0, c2 = ti.c_begin - c1 * n2;
         for (int c = ti.c_begin; c < ti.c_end; ++c, ++gc) {
-          const bool tr = trace && blockIdx.x == trace_cta && warp == 0 && gc < 64 && lane == 0;
+          const bool tr = trace && blockIdx.x == trace_cta && pw == 0 && gc < 64 && lane == 0;
           if (tr) trace[gc * 8 + 0] = clock64();
           mbar_wait(smem_u32(&bar_empty[s]), ((ph >> s) & 1u) ^ 1u);
           if (tr) trace[gc * 8 + 1] = clock64();
           const uint32_t full = smem_u32(&bar_full[s]);
           const bool leader = elect_one();
-          if (dbg_noload) { if (warp == 0 && leader) mbar_arrive(full); }
+          if (dbg_noload) { if (pw == 0 && leader) mbar_arrive(full); }
           else {
-            if (warp == 0 && leader) mbar_expect_tx(full, (uint32_t)tx);        // the one arrival of the phase; boxes may land before it
+            if (pw == 0 && leader) mbar_expect_tx(full, (uint32_t)tx);        // the one arrival of the phase; boxes may land before it
             const uint32_t sbase = ring + s * (uint32_t)slot_bytes;
             int j = 0;                                                 // box index inside the chunk, dealt round-robin to the producer warps
 #pragma unroll
@@ -258,13 +334,13 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
 #pragma unroll
                 for (int d = 0; d < 5; ++d) crd[d] = base[l][d] + c1 * L.d_c1[d] + c2 * L.d_c2[d];
                 if (L.plane_box) {                               // all planes in one box (plane = outermost coordinate, 0)
-                  if ((j & (NPROD_WARPS - 1)) == warp && leader) tma_load(sbase + (uint32_t)L.smem_off, maps + L.map, full, L.rank, crd);
+                  if ((j & (NPROD_WARPS - 1)) == pw && leader) tma_load(sbase + (uint32_t)L.smem_off, maps + L.map, full, L.rank, crd);
                   ++j;
                 } else {
                   for (int pl = 0; pl < planes; ++pl, ++j) {
 #pragma unroll
                     for (int d = 2; d < 5; ++d) if (d == L.rank - 1) crd[d] = pl;
-                    if ((j & (NPROD_WARPS - 1)) == warp && leader)
+                    if ((j & (NPROD_WARPS - 1)) == pw && leader)
                       tma_load(sbase + (uint32_t)(pl * L.plane_stride + L.smem_off), maps + L.map, full, L.rank, crd);
                   }
                 }
@@ -278,94 +354,20 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
         }
       }
     }
-  } else if (warp == MMA_WARP) {
-    // ============================================================================================ MMA issuer
-    {
-      uint32_t it = 0, s = 0, ph = 0, gcm = 0;
-      int slot_bytes = 0, nstages = 1;
-      Walker w;
-      bool mnm = false;
-      uint32_t idesc[3] = {0, 0, 0}, a_off = 0, b_off = 0, a_ks = 0, b_ks = 0, a_lbo = 0, b_lbo = 0, a_ps = 0, ncol = 0;
-      int ksteps = 0, nprod = 1;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        if (w.advance(probs, nprob, tile)) {
-          const CgProblem& P = probs[w.p];
-          mnm = P.mn_major != 0;
-          ncol = (uint32_t)P.umma_n;
-#pragma unroll
-          for (int j = 0; j < 3; ++j) idesc[j] = make_idesc(128, P.umma_n * (j + 1), mnm);      // N = n, 2n, 3n
-          ksteps = P.ksteps; nprod = P.nprod; a_ps = (uint32_t)P.a_pstride;
-          a_off = P.a_off; b_off = P.b_off; a_ks = P.a_kstep; b_ks = P.b_kstep; a_lbo = P.a_lbo; b_lbo = P.b_lbo;
-          if (P.slot_bytes != slot_bytes || P.nstages != nstages) { slot_bytes = P.slot_bytes; nstages = P.nstages; s = 0; }
-        }
-        const Tile ti = w.tile(tile);
-        if (ti.c_end <= ti.c_begin) continue;
-        const uint32_t buf = it & 1;
-        if (it >= 2) mbar_wait(smem_u32(&bar_acc_empty[buf]), ((it >> 1) - 1) & 1);
-        tc_fence_after();
-        const uint32_t acc = tmem + buf * 256u;
-        for (int c = ti.c_begin; c < ti.c_end; ++c) {
-          const bool tr = trace && blockIdx.x == trace_cta && gcm < 64 && lane == 0;
-          if (tr) trace[gcm * 8 + 3] = clock64();
-          mbar_wait(smem_u32(&bar_full[s]), (ph >> s) & 1u);
-          if (tr) trace[gcm * 8 + 4] = clock64();
-          tc_fence_after();
-          const uint32_t sbase = ring + s * (uint32_t)slot_bytes;
-          const bool leader = elect_one();
-          if (!dbg_nomma) {
-            for (int k = 0; k < ksteps; ++k) {
-// `planes` wide MMAs per k-step: A_p x [B_0 | .. | B_(planes-1-p)] -> accumulator columns [p*n, planes*n).
-              // Column group g therefore collects the products of order 2^(-8g): g0 = hi*hi, g1 = hi*mid + mid*hi,
-              // g2 = hi*lo + mid*mid + lo*hi.  The tensor core truncates the fp32 accumulator at every MMA (measured:
-              // tools/tc_accum_probe.py, ~2^-25 relative per accumulation), so keeping each order in its own columns keeps that
-              // truncation 2^-8g smaller on the correction terms; the epilogue adds the groups small-to-large in fp32.
-              // One wide MMA reads the A plane from shared memory once for up to three products -- at N = 64 the SS-mode
-              // MMA is shared-memory bound (55 cycles where the tensor floor is 32: profiles/cg_trace_r2.txt).
-              const uint32_t pb = sbase + b_off + (uint32_t)k * b_ks;
-              const uint64_t db = mnm ? desc_mn(pb, b_lbo) : desc_k(pb);
-              uint64_t da[3];
-#pragma unroll
-              for (int pl = 0; pl < 3; ++pl) {
-                const uint32_t pa = sbase + (uint32_t)pl * a_ps + a_off + (uint32_t)k * a_ks;
-                da[pl] = mnm ? desc_mn(pa, a_lbo) : desc_k(pa);
-              }
-              const uint32_t first = (c == ti.c_begin && k == 0) ? 0u : 1u;
-              if (leader) {
-                if (nprod >= 6) {
-                  umma(acc, da[0], db, idesc[2], first); umma(acc + ncol, da[1], db, idesc[1], 1u); umma(acc + 2u * ncol, da[2], db, idesc[0], 1u);
-                } else if (nprod >= 3) {
-                  umma(acc, da[0], db, idesc[1], first); umma(acc + ncol, da[1], db, idesc[0], 1u);
-                } else {
-                  umma(acc, da[0], db, idesc[0], first);
-                }
-              }
-            }
-          }
-          if (leader) umma_commit(smem_u32(&bar_empty[s]));
-          __syncwarp();
-          if (tr) trace[gcm * 8 + 5] = clock64();
-          ++gcm;
-          ph ^= 1u << s;
-          if (++s == (uint32_t)nstages) s = 0;
-        }
-        if (elect_one()) umma_commit(smem_u32(&bar_acc_full[buf]));
-        __syncwarp();
-        ++it;
-      }
-    }
-    __syncwarp();
   } else {
-    // ============================================================================================ epilogue
-    const int ew = warp - EPI_WARP0, q = warp & 3, half = ew >> 2;
-    uint32_t it = 0;
+    // ============================================================================================ consumers: MMA + epilogue
+    const int ew = warp, half = (ew & 3) >> 1, q = 2 * (ew >> 2) + (ew & 1);
+    uint32_t it = 0, s = 0, ph = 0;
+    int slot_bytes = 0, nstages = 1;
     Walker w;
-    const int r = q * 32 + lane;                         // accumulator row of this thread
+    const int r = q * 32 + lane;                         // output row of this thread in the epilogue
     // per-problem constants of this thread, recomputed only when the CTA moves to another problem: the row's offset
     // inside a tile (the r -> (i0, i1, i2) decomposition needs integer divisions) and every descriptor field the tile loop reads
     int epi = 0, rows_tile = 0, lim_rows = 0, umma_n = 0, out_planes = 0, grp_stride = 32, n_valid = 0;
     long long roff = 0, rmoff = 0, o_tm = 0, m_tm = 0;
     int ri0 = 0, ri1 = 0, grp_tab = 0;
-    int ngrp_acc = 1;
+    int nprod = 1;
+    bool mnm = false;
     const float* __restrict__ bias = nullptr;
     const uint16_t* __restrict__ mask = nullptr;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -377,47 +379,38 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
         const int i0 = r % d0, i12 = r / d0, i1 = i12 % d1, i2 = i12 / d1;
         roff = Q.o_base + (long long)i0 * Q.o0 + (long long)i1 * Q.o1 + (long long)i2 * Q.o2;
         rmoff = Q.m_base + (long long)i0 * Q.m0 + (long long)i1 * Q.m1 + (long long)i2 * Q.m2;
-        ri0 = i0; ri1 = i1; grp_tab = Q.grp_tab; ngrp_acc = Q.nprod >= 6 ? 3 : (Q.nprod >= 3 ? 2 : 1);
+        ri0 = i0; ri1 = i1; grp_tab = Q.grp_tab; nprod = Q.nprod;
+        mnm = Q.mn_major != 0;
+        if (Q.slot_bytes != slot_bytes || Q.nstages != nstages) { slot_bytes = Q.slot_bytes; nstages = Q.nstages; s = 0; }
       }
       const Tile ti = w.tile(tile);
       if (ti.c_end <= ti.c_begin) continue;
       const CgProblem& P = probs[ti.p];
-      const uint32_t buf = it & 1;
-      // epi_tiles: the two warp quads alternate TILES (quad h owns accumulator buffer h) instead of splitting the column groups of
-      // one tile, so that one quad's TMEM / ALU phase overlaps the other's store phase
-      if (epi_tiles && (int)buf != half) { ++it; continue; }
       const bool valid0 = r < rows_tile && ti.tm * rows_tile + r < lim_rows;
       const long long off0 = roff + (long long)ti.tm * o_tm, moff0 = rmoff + (long long)ti.tm * m_tm;
       const int n0 = ti.tn * umma_n, ngroups = umma_n >> 5;
-      const bool tre = trace && blockIdx.x == trace_cta && (ew & 3) == 0 && lane == 0 && it < 16 && (epi_tiles || ew == 0);
+      const bool tre = trace && blockIdx.x == trace_cta && ew == 0 && lane == 0 && it < 16;
       if (tre) trace[512 + it * 4 + 0] = clock64();
-      mbar_wait(smem_u32(&bar_acc_full[buf]), (it >> 1) & 1);
-      if (tre) trace[512 + it * 4 + 1] = clock64();
-      tc_fence_after();
       const bool split_fin = P.ws != nullptr;          // split-K tile of an ACT problem: partial sums first, the last arriver finishes
       float* __restrict__ wsrow = split_fin ? P.ws + ((size_t)(ti.tm * w.tiles_n + ti.tn) * 128 + r) * umma_n : nullptr;
-      bool last_arriver = !split_fin;
-      for (int pass = 0; pass < (split_fin ? 2 : 1); ++pass) {
-      if (pass == 1) {
-        __syncwarp();
-        int old = 0;
-        if (lane == 0) { __threadfence(); old = atomicAdd(P.ws_cnt + (ti.tm * w.tiles_n + ti.tn) * NEPI_WARPS + ew, 1); }
-        old = __shfl_sync(0xffffffffu, old, 0);
-        last_arriver = old == w.splits - 1;
-        if (!last_arriver) break;
-        __threadfence();
-        if (lane == 0) P.ws_cnt[(ti.tm * w.tiles_n + ti.tn) * NEPI_WARPS + ew] = 0;     // next step starts from zero
-      }
-      for (int g = epi_tiles ? 0 : half; g < ngroups; g += epi_tiles ? 1 : 2) {
+      // epilogue of column group g of this thread's row; pass 0: x = this tile's accumulator sums, pass 1: x = the finished
+      // split-K sums read back by the last arriver
+      auto body = [&](int g, float (&x)[32], int pass) {
         const int ng = n0 + 32 * g;                      // first problem column of the group
-        // ---- everything that does not depend on the accumulator is fetched BEFORE the TMEM loads are waited for: the epilogue of
-        //      a tile is a dependent chain of long-latency operations on 8 warps, so latency, not bandwidth, sets its length
         bool valid = valid0;
         long long off = off0, moff = moff0;
         if (grp_tab) {
           const int gg = ng >> 5;
           valid = valid0 && ri0 < P.grp_lim0[gg] && ri1 < P.grp_lim1[gg];
           off = off0 + P.grp_off[gg]; moff = moff0 + P.grp_moff[gg] - ng;     // (the mask load below adds ng)
+        }
+        if (pass == 0 && split_fin) {                    // partial sums of this split -> workspace
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(wsrow + 32 * g + 4 * j), "f"(x[4 * j]), "f"(x[4 * j + 1]), "f"(x[4 * j + 2]),
+                         "f"(x[4 * j + 3])
+                         : "memory");
+          return;
         }
         const bool live = !dbg_nostore && ng < n_valid;
         float4 bv[8];
@@ -430,55 +423,8 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
 #pragma unroll
           for (int j = 0; j < 4; ++j) mk[j] = valid ? __ldg(reinterpret_cast<const uint4*>(mask + moff + ng) + j) : make_uint4(0, 0, 0, 0);
         }
-        float x[32];
-        if (pass == 0) {
-        uint32_t v[32], u[32], t[32];
-        const uint32_t taddr = tmem + buf * 256u + ((uint32_t)(q * 32) << 16) + (uint32_t)(32 * g);
-#define CG_TMEM_LD32(dst, addr)                                                                                                              \
-  asm volatile(                                                                                                                             \
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                                                                             \
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"     \
-      : "=r"(dst[0]), "=r"(dst[1]), "=r"(dst[2]), "=r"(dst[3]), "=r"(dst[4]), "=r"(dst[5]), "=r"(dst[6]), "=r"(dst[7]), "=r"(dst[8]),       \
-        "=r"(dst[9]), "=r"(dst[10]), "=r"(dst[11]), "=r"(dst[12]), "=r"(dst[13]), "=r"(dst[14]), "=r"(dst[15]), "=r"(dst[16]),              \
-        "=r"(dst[17]), "=r"(dst[18]), "=r"(dst[19]), "=r"(dst[20]), "=r"(dst[21]), "=r"(dst[22]), "=r"(dst[23]), "=r"(dst[24]),             \
-        "=r"(dst[25]), "=r"(dst[26]), "=r"(dst[27]), "=r"(dst[28]), "=r"(dst[29]), "=r"(dst[30]), "=r"(dst[31])                             \
-      : "r"(addr))
-        CG_TMEM_LD32(v, taddr);
-        if (ngrp_acc > 1) CG_TMEM_LD32(u, taddr + (uint32_t)umma_n);
-        if (ngrp_acc > 2) CG_TMEM_LD32(t, taddr + 2u * (uint32_t)umma_n);
-#undef CG_TMEM_LD32
-        if (tre && g == 0) trace[576 + it * 4 + 0] = clock64();
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (tre && g == 0) trace[576 + it * 4 + 1] = clock64();
-        if (ngrp_acc > 2) {                                // correction column groups, smallest order first
-#pragma unroll
-          for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(v[j]) + (__uint_as_float(u[j]) + __uint_as_float(t[j]));
-        } else if (ngrp_acc > 1) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(v[j]) + __uint_as_float(u[j]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(v[j]);
-        }
-        if (split_fin) {                                   // partial sums of this split -> workspace
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(wsrow + 32 * g + 4 * j), "f"(x[4 * j]), "f"(x[4 * j + 1]), "f"(x[4 * j + 2]),
-                         "f"(x[4 * j + 3])
-                         : "memory");
-          continue;
-        }
-        } else {                                           // last arriver: the complete sums, and a clean workspace for the next step
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 sum = __ldcg(reinterpret_cast<const float4*>(wsrow + 32 * g) + j);
-            x[4 * j] = sum.x; x[4 * j + 1] = sum.y; x[4 * j + 2] = sum.z; x[4 * j + 3] = sum.w;
-            __stcg(reinterpret_cast<float4*>(wsrow + 32 * g) + j, make_float4(0.f, 0.f, 0.f, 0.f));
-          }
-        }
-        if (!live) continue;
-        // Every lane owns one output row and writes its 32 columns itself (64 B per BF16 plane, 128 B of fp32): 16-byte vector
-        // stores, no shared-memory transpose -- partial-sector writes are cheap next to the staging round trips they replace.
+        if (!live) return;
+        // Every lane owns one output row and writes its 32 columns itself (64 B per BF16 plane, 128 B of fp32): 16-byte vector stores.
         if (epi == CG_EPI_RAW) {
           if (valid) {
             float* dst = P.out_f + off + (long long)(ng >> 5) * P.f_grp;
@@ -493,7 +439,7 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
               for (int j = 0; j < 8; ++j) *reinterpret_cast<float4*>(dst + 4 * j) = make_float4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
             }
           }
-          continue;
+          return;
         }
         if (epi == CG_EPI_WGRAD) {
           if (valid) {
@@ -521,7 +467,7 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
               }
             }
           }
-          continue;
+          return;
         }
         if (epi == CG_EPI_ACT) {
 #pragma unroll
@@ -532,10 +478,7 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
           if (P.f0 > 0 && valid && !dbg_nost) {        // optional fp32 copy (cnn_fc1 features for the head kernels)
             float* dst = P.out_f + (long long)ti.tm * P.f_tm + (long long)r * P.f0 + (long long)(ng >> 5) * P.f_grp;
 #pragma unroll
-            for (int j = 0; j < 4; ++j)
-              asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst + 8 * j), "f"(x[8 * j]), "f"(x[8 * j + 1]), "f"(x[8 * j + 2]),
-                           "f"(x[8 * j + 3]), "f"(x[8 * j + 4]), "f"(x[8 * j + 5]), "f"(x[8 * j + 6]), "f"(x[8 * j + 7])
-                           : "memory");
+            for (int j = 0; j < 8; ++j) *reinterpret_cast<float4*>(dst + 4 * j) = make_float4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
           }
         } else {   // CG_EPI_DGRAD: ReLU mask = hi plane of the forward activation at the same position
 #pragma unroll
@@ -565,7 +508,6 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
             atomicAdd(P.colsum + ((ng + lane) & P.colsum_mask), cs[0]);
           }
         }
-        if (tre && g == 0) trace[576 + it * 4 + 2] = clock64();
         // ---- BF16 planes: hi = bf16(x), then the residual feeds the next plane
         const long long gcol = grp_tab ? 0 : (long long)(ng >> 5) * grp_stride;
 #pragma unroll 1
@@ -577,35 +519,58 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
             x[2 * j] -= __uint_as_float(pk[j] << 16);
             x[2 * j + 1] -= __uint_as_float(pk[j] & 0xFFFF0000u);
           }
-          if (valid && !dbg_nost) {              // 2 x 256-bit stores: every lane writes whole 32-byte sectors
+          if (valid && !dbg_nost) {              // 4 x 128-bit stores: every lane writes whole 32-byte sectors
             uint16_t* dst = P.out_p[pl] + off + gcol;
 #pragma unroll
-            for (int j = 0; j < 2; ++j)
-              asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst + 16 * j), "r"(pk[8 * j]), "r"(pk[8 * j + 1]), "r"(pk[8 * j + 2]),
-                           "r"(pk[8 * j + 3]), "r"(pk[8 * j + 4]), "r"(pk[8 * j + 5]), "r"(pk[8 * j + 6]), "r"(pk[8 * j + 7])
-                           : "memory");
+            for (int j = 0; j < 4; ++j) *reinterpret_cast<uint4*>(dst + 8 * j) = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
+          }
+        }
+      };
+      auto body0 = [&](int g, float (&x)[32]) { body(g, x, 0); };
+#define CG_CONSUME(NT, NPROD, TRANS) \
+  consume_tile<NT, NPROD, TRANS>(P, ti, ring, stg, slot_bytes, nstages, s, ph, bar_full, bar_empty, dbg_nomma, body0)
+      // the (width, products, major-ness) combinations cg_shape_supported() admits on the host; anything else is a bug: trap
+      switch (cg_shape_key(umma_n, nprod, mnm)) {
+        case cg_shape_key(32, 6, false): CG_CONSUME(32, 6, 0); break;
+        case cg_shape_key(64, 6, false): CG_CONSUME(64, 6, 0); break;
+        case cg_shape_key(64, 3, false): CG_CONSUME(64, 3, 0); break;
+        case cg_shape_key(128, 3, false): CG_CONSUME(128, 3, 0); break;
+        case cg_shape_key(64, 3, true): CG_CONSUME(64, 3, 1); break;
+        case cg_shape_key(128, 3, true): CG_CONSUME(128, 3, 1); break;
+        default: __trap();
+      }
+#undef CG_CONSUME
+      if (tre) trace[512 + it * 4 + 1] = clock64();
+      bool last_arriver = !split_fin;
+      if (split_fin) {
+        __syncwarp();
+        int old = 0;
+        if (lane == 0) { __threadfence(); old = atomicAdd(P.ws_cnt + (ti.tm * w.tiles_n + ti.tn) * NEPI_WARPS + ew, 1); }
+        old = __shfl_sync(0xffffffffu, old, 0);
+        last_arriver = old == w.splits - 1;
+        if (last_arriver) {                              // the complete sums, and a clean workspace for the next step
+          __threadfence();
+          if (lane == 0) P.ws_cnt[(ti.tm * w.tiles_n + ti.tn) * NEPI_WARPS + ew] = 0;     // next step starts from zero
+          for (int g = half; g < ngroups; g += 2) {
+            float x[32];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const float4 sum = __ldcg(reinterpret_cast<const float4*>(wsrow + 32 * g) + j);
+              x[4 * j] = sum.x; x[4 * j + 1] = sum.y; x[4 * j + 2] = sum.z; x[4 * j + 3] = sum.w;
+              __stcg(reinterpret_cast<float4*>(wsrow + 32 * g) + j, make_float4(0.f, 0.f, 0.f, 0.f));
+            }
+            body(g, x, 1);
           }
         }
       }
-      }   // pass
-      tc_fence_before();
       __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(smem_u32(&bar_acc_empty[buf]));
-        if (P.done_ctr && last_arriver) {                                // this warp's rows of the tile are in global memory
-          __threadfence();
-          atomicAdd(P.done_ctr + ti.tm, 1);
-        }
+      if (lane == 0 && P.done_ctr && last_arriver) {     // this warp's rows of the tile are in global memory
+        __threadfence();
+        atomicAdd(P.done_ctr + ti.tm, 1);
       }
       if (tre) { trace[512 + it * 4 + 2] = clock64(); trace[512 + it * 4 + 3] = ti.p * 100000 + ti.tm * 10 + ti.tn; }
       ++it;
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS));
   }
 }
 
@@ -615,7 +580,17 @@ EncodeTiledFn g_encode = nullptr;
 
 }  // namespace
 
-int cg_smem_limit() { return 226 * 1024; }   // dynamic part; the kernel's static shared memory (barriers) takes < 1 KiB of the 227 KiB
+// ring budget (cg_finalize): the dynamic part minus the epilogue staging; the kernel's static shared memory (barriers) takes < 1 KiB
+// of the 227 KiB
+bool cg_shape_supported(int umma_n, int nprod, bool mn_major) {
+  switch (cg_shape_key(umma_n, nprod, mn_major)) {
+    case cg_shape_key(32, 6, false): case cg_shape_key(64, 6, false): case cg_shape_key(64, 3, false): case cg_shape_key(128, 3, false):
+    case cg_shape_key(64, 3, true): case cg_shape_key(128, 3, true): return true;
+    default: return false;
+  }
+}
+
+int cg_smem_limit() { return 226 * 1024 - STG_BYTES; }
 
 int cg_encode_map(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box,
                   const uint32_t* elem_strides) {
@@ -673,18 +648,16 @@ cudaError_t cg_launch(const CgGroup& g, const CUtensorMap* dev_maps, int num_sms
   if (g.total_tiles <= 0 || (debug_flags & 8)) return cudaSuccess;     // bit 3: skip the launch (timing ablation)
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(cg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cg_smem_limit());
+    cudaError_t e = cudaFuncSetAttribute(cg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  static int epi_tiles = -1;
-  if (epi_tiles < 0) { const char* e = getenv("B2G_EPI_TILES"); epi_tiles = (e && e[0] == '1') ? 1 : 0; }
-  const int smem = 1024 + g.ring_bytes;
+  const int smem = 1024 + STG_BYTES + g.ring_bytes;
   const int grid = g.total_tiles < num_sms ? g.total_tiles : num_sms;
   CgPack pk;              // (host staging; the launch copies it into the parameter buffer)
-  static_assert(sizeof(CgPack) < 28 * 1024, "problem list must fit the kernel parameter space (32,764 B on sm_100)");
+  static_assert(sizeof(CgPack) < 28 * 1024, "problem list must fit the kernel parameter space (32,764 B)");
   for (int i = 0; i < g.n; ++i) pk.p[i] = g.host[i];
-  cudaError_t e = launch_pdl(cg_kernel, dim3(grid), dim3(NTHREADS), (size_t)smem, s, pdl, pk, g.n, g.total_tiles, dev_maps, g.nstages, debug_flags, g_cg_trace, epi_tiles);
+  cudaError_t e = launch_pdl(cg_kernel, dim3(grid), dim3(NTHREADS), (size_t)smem, s, pdl, pk, g.n, g.total_tiles, dev_maps, g.nstages, debug_flags, g_cg_trace);
   if (e != cudaSuccess) fprintf(stderr, "cg_launch %s: %s (grid %d, %d threads, smem %d)\n", g.name, cudaGetErrorString(e), grid, NTHREADS, smem);
   return e;
 }

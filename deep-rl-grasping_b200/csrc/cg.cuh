@@ -1,7 +1,7 @@
-// TMA-fed tcgen05 contraction engine ("cg"): declarations shared by cg.cu (kernel) and sac.cu (problem builders).
+// TMA-fed wgmma contraction engine ("cg"): declarations shared by cg.cu (kernel) and sac.cu (problem builders).
 //
 // Every dense contraction of the step is a list of 128-row output tiles; the operands of a tile are fetched, K-chunk by
-// K-chunk, by cp.async.bulk.tensor (TMA) boxes over BF16 plane tensors straight into 128B-swizzled shared-memory UMMA
+// K-chunk, by cp.async.bulk.tensor (TMA) boxes over BF16 plane tensors straight into 128B-swizzled shared-memory wgmma
 // tiles.  Convolutions need no im2col buffer: their patches / shifted windows / zero borders are expressed as tensor-map
 // VIEWS (overlapping strides, element strides, out-of-bound zero fill) of the NHWC activation planes, so two elected
 // lanes feed the whole ring (tools/tma_probe.cu checks each view behaviour on the device).  A launch is a list of problems;
@@ -45,7 +45,7 @@ struct CgProblem {
   // ---- operand fetch
   int nloads, planes;
   int a_pstride, b_pstride;   // stage layout: [A plane 0 | A plane 1 | ..][B plane 0 | B plane 1 | ..]; bytes of one A / B plane.
-                              // The B planes are CONTIGUOUS so that one UMMA descriptor spans [B0|B1|B2] (see nprod)
+                              // The B planes are CONTIGUOUS so that one wgmma descriptor spans [B0|B1|B2] (see nprod)
   int tx_bytes;               // bytes all boxes of one stage deliver (planes x sum of box bytes)
   int slot_bytes, nstages;    // stage ring geometry of THIS problem (cg_finalize): the problems of a launch share the ring's bytes, not
                               // its partition -- the ring is drained when the partition changes
@@ -53,11 +53,11 @@ struct CgProblem {
   const int* tm_tab;          // optional [tiles_m][CG_MAX_LOADS][2]: extra offsets of coordinates 1 and 2 per (tm, load)
   // ---- MMA
   int mn_major;               // 0: K-major A and B (rows = M|N, 128 B of K); 1: MN-major (rows = K, 128 B of M|N)
-  int ksteps;                 // UMMA K = 16 steps per chunk
+  int ksteps;                 // wgmma K = 16 steps per chunk
   int a_off, b_off;           // region offsets inside a stage (b_off = planes * a_pstride)
   int a_kstep, b_kstep;       // descriptor start-address advance per k-step (bytes)
   int a_lbo, b_lbo;           // MN-major: byte stride between 64-element atoms along M|N
-  int umma_n;                 // tile width (multiple of 16, <= 256)
+  int umma_n;                 // tile width: 32, 64 or 128 (the widths cg_kernel is instantiated for)
   int nprod;                  // products per k-step: 1 (hi*hi), 3 (+hi*lo, lo*hi), 6 (+mid terms of the 3-plane split), issued as
                               // `planes` wide MMAs: A_p x [B_0 | .. | B_(planes-1-p)] into accumulator columns [p*n, planes*n), so
                               // column group g collects the products of order 2^(-8g) (planes * umma_n <= 256)
@@ -93,7 +93,7 @@ struct CgProblem {
   int* done_ctr;              // arrival counters of THIS problem, one per tm (nullptr: nobody waits on it); zeroed before the launch
   const int* dep_ctr;         // counters of the producing problem (nullptr: no dependency)
   int dep_rows, dep_rows_tile, dep_tiles, dep_expect;
-  // ---- split-K with in-kernel finalisation (ACT problems with splits > 1; the late layers have too few tiles for 148 SMs): every
+  // ---- split-K with in-kernel finalisation (ACT problems with splits > 1; the late layers have too few tiles for 132 SMs): every
   //      split tile adds its fp32 partial sums into ws[tile][128][umma_n] (red.add), then each epilogue warp bumps its own arrival
   //      counter of the tile; the warp that arrives LAST reads the sums back, clears them for the next step, and runs the normal
   //      bias / ReLU / plane-split / store path (and alone signals done_ctr)
@@ -124,5 +124,9 @@ int cg_encode_map(CUtensorMap* out, const void* base, int rank, const uint64_t* 
 int cg_finalize(CgGroup& g, int smem_budget);
 cudaError_t cg_launch(const CgGroup& g, const CUtensorMap* dev_maps, int num_sms, cudaStream_t s, bool pdl, int debug_flags);
 int cg_smem_limit();
+// cg_kernel is compiled for a fixed set of (tile width, products per k-step, MN-major) shapes; a problem of any other shape is
+// rejected when its group is built
+__host__ __device__ constexpr int cg_shape_key(int umma_n, int nprod, bool mn_major) { return umma_n * 16 + nprod * 2 + (mn_major ? 1 : 0); }
+bool cg_shape_supported(int umma_n, int nprod, bool mn_major);
 
 }  // namespace b2g

@@ -1,4 +1,4 @@
-// Shared declarations of libb200grasp (sm_100a only).
+// Shared declarations of libb200grasp (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -10,7 +10,7 @@ namespace b2g {
 
 // ---------------------------------------------------------------------------------------------
 // Programmatic dependent launch: a kernel launched through launch_pdl() may start (smem carve-up,
-// barrier init, TMEM allocation) while its predecessor on the stream is still running; it must call
+// barrier init) while its predecessor on the stream is still running; it must call
 // pdl_wait() before touching global memory, and pdl_trigger() lets ITS successor start early.
 // ---------------------------------------------------------------------------------------------
 #ifdef __CUDACC__
@@ -55,7 +55,7 @@ enum GemmFlags : int {
   GG_A_ROWLANES = 1 << 14, // planes K-major producer: lanes walk 8 consecutive rows of one 16-byte column group (conv1: adjacent
                            // output pixels overlap in the image, so a warp copy touches 4-8 lines instead of 32)
   GG_EPI_BIAS_LRELU = 1 << 13, // C = leaky_relu(acc + bias[n], slope alpha)   (Keras LeakyReLU; encoder.cu)
-  GG_MN_MAJOR = 1 << 9,   // planes mode, wgrad: both operands contiguous along their M / N index -> MN-major UMMA tiles
+  GG_MN_MAJOR = 1 << 9,   // planes mode, wgrad: both operands contiguous along their M / N index -> MN-major wgmma tiles
   GG_CN_AFFINE4 = 1 << 8, // host-verified: cN / kN contiguous inside aligned 4-column groups, outputs 16-byte aligned
 };
 
@@ -82,7 +82,7 @@ struct GemmDesc {
   int tiles_m, tiles_n;
   int tile_start;   // first flattened CTA index of this problem inside a grouped launch
   int tile_count;
-  int col_id;       // tcgen05 engine: identity of (cN, kN, bias, N); equal ids share the staged column tables
+  int col_id;       // wgmma engine: identity of (cN, kN, bias, N); equal ids share the staged column tables
   int layer;        // host side: layer index inside a fused (layer-synchronised) launch
   int need_done;    // fused launch: tiles [0, need_done) of the launch must be complete before this problem's operands are read
 };
@@ -93,9 +93,9 @@ struct GemmGroup {          // one grouped launch
   GemmDesc* dev = nullptr;
   int total_tiles = 0;
   double flops = 0;
-  bool tc = false;          // run on the tcgen05 engine
+  bool tc = false;          // run on the wgmma engine
   bool tc_eligible = false; // large dense contraction (convs, cnn_fc1)
-  int* dev_ranges = nullptr; // tcgen05 engine: contiguous tile range per CTA (gg_tc_ranges)
+  int* dev_ranges = nullptr; // wgmma engine: contiguous tile range per CTA (gg_tc_ranges)
   int ranges_grid = 0;
   bool layer_sync = false;   // several dependent layers in ONE persistent launch (in-kernel completion counter)
 };
@@ -103,7 +103,7 @@ struct GemmGroup {          // one grouped launch
 // engines (gg_simt.cu / gg_tc.cu)
 void gg_simt_launch(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaStream_t s);
 constexpr int GG_SIMT_BM = 64, GG_SIMT_BN = 64, GG_SIMT_BK = 16;
-// tcgen05 engine: 128 x 64 output tile, 64-wide r-chunks; x3 != 0 -> BF16 hi/lo split (3 MMAs)
+// wgmma engine: 128 x 64 output tile, 64-wide r-chunks; x3 != 0 -> BF16 hi/lo split (3 MMAs)
 cudaError_t gg_tc_launch(const GemmDesc* host_descs, int ndesc, int total_tiles, int mode_flags, int x3, int num_sms, cudaStream_t s,
                          const int* dev_ranges = nullptr, int ranges_grid = 0, unsigned* sync_ctr = nullptr);
 // host side of the contiguous tile schedule: cost-balanced range boundaries [grid + 1] for a finalized group

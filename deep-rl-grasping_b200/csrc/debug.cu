@@ -1,8 +1,8 @@
 // Bring-up / measurement hooks of libb200grasp (not on the product path).
 //
-// b2g_debug_gemm: one dense C[M,N] = A[M,K] * B[N,K]^T through the tcgen05 gather-GEMM engine (register-staged fp32
+// b2g_debug_gemm: one dense C[M,N] = A[M,K] * B[N,K]^T through the wgmma gather-GEMM engine (register-staged fp32
 // operands, BF16 hi/lo split when x3 != 0), used by tools/tc_accum_probe.py to measure what the tensor core's fp32
-// accumulation in TMEM does to long, cancelling reductions -- independently of the operand split.
+// accumulation in registers does to long, cancelling reductions -- independently of the operand split.
 #include <cuda_runtime.h>
 
 #include <string>

@@ -263,7 +263,7 @@ int b2g_encoder_encode(b2g_encoder* h, const float* imgs, int n, float* out) {
   const size_t in_numel = (size_t)n * h->cfg.height * h->cfg.width * h->cfg.channels;
   memcpy(h->pin_in, imgs, in_numel * sizeof(float));
   ECK(cudaMemcpyAsync(h->stage_in, h->pin_in, in_numel * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  const int blocks = (int)std::min<size_t>((in_numel + 255) / 256, 148 * 8);
+  const int blocks = (int)std::min<size_t>((in_numel + 255) / 256, 132 * 8);
   enc_pad_copy<<<blocks, 256, 0, h->stream>>>(h->stage_in, y0.in, n, h->cfg.height, h->cfg.width, h->cfg.channels, y0.hp, y0.wp,
                                               y0.pad_t, y0.pad_l);
   for (auto& g : h->groups) gg_simt_launch(g.dev, 1, g.total_tiles, h->stream);

@@ -1,4 +1,4 @@
-// Engine v2: the CNN / head contractions of the SAC step on the TMA-fed tcgen05 engine (cg.cu).
+// Engine v2: the CNN / head contractions of the SAC step on the TMA-fed wgmma engine (cg.cu).
 //
 // This file owns (i) the BF16 plane tensors the engine reads and writes, (ii) the tensor-map VIEWS that turn NHWC
 // activation planes into implicit-im2col / shifted-window / zero-bordered operand tiles (one map per tensor: plane = outermost
@@ -7,7 +7,7 @@
 //   gather2_kernel : replay slot draw + compact-row gather + float64 VecNormalize + clip + /255 (replay.cu semantics,
 //                    [SB2] ReplayBuffer.sample(env=VecNormalize), observation_input(scale=True)), the 3-plane BF16 split and the
 //                    conv1 patch rows (8x8 stride-4 patches of the normalised image; the one view TMA cannot express, see
-//                    profiles/tma_r2.md) so that conv1 forward and its wgrad are plain 2-D TMA tiles;
+//                    tools/tma_probe.cu) so that conv1 forward and its wgrad are plain 2-D TMA tiles;
 //   compact_kernel : full observation rows -> compact replay rows (image planes | actuator value);
 //   planes2_kernel : weights -> BF16 planes in the layouts the tensor maps expect (transposed / packed per consumer);
 //   colsum2_kernel : bias gradients as column sums of the gradient-map planes -- only with B2G_BIAS_EPI=0: by default the DGRAD
@@ -60,8 +60,7 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
   const bool norm_obs = g.normc[3] != 0.0;
   const float scale = g.scale;
   // shared-memory planes with a padded row pitch (+8 elements = +4 banks per image row): the patch pass below reads 16-byte runs
-  // of 8 consecutive image rows at once, which a 128-byte pitch puts on the same four banks (8-way conflicts: 2.5 M conflict
-  // cycles per launch in profiles/ncu_aux_r2.md)
+  // of 8 consecutive image rows at once, which a 128-byte pitch puts on the same four banks (8-way conflicts)
   const int rowe = g.W * Ci, pitch = rowe + 8, plane_e = g.H * pitch;
   uint16_t* xh = a.xp[which][0]; uint16_t* xl = a.xp[which][1];
   (void)Cfull;
@@ -167,8 +166,7 @@ struct Plane2Job {
 // consecutive r values per plane (the 2-byte scattered stores of the first version made this the longest leaf kernel).
 __global__ void __launch_bounds__(256) planes2_kernel(const Plane2Job* __restrict__ jobs, const int* __restrict__ cta_job) {
   __shared__ float tile[64][33];
-  // (the job of a CTA comes from a table: walking the job list cost up to 30 DEPENDENT global loads before the first useful one --
-  //  19.5 long-scoreboard stalls per issue in profiles/ncu_aux_r2.md)
+  // (the job of a CTA comes from a table: walking the job list cost up to 30 DEPENDENT global loads before the first useful one)
   const Plane2Job job = jobs[cta_job[blockIdx.x]];
   const int t = blockIdx.x - job.tile_start;
   const int tiles_n = (job.N + 31) / 32;
@@ -274,7 +272,7 @@ int valloc(b2g_sac* h, T** ptr, size_t count) {
 // ONE map over the np equidistant planes of a tensor: the given geometry plus an outermost plane dimension.  The box covers all
 // planes (one instruction fetches them, stacked plane after plane in shared memory) when one plane's box is a whole number of
 // 1024-byte swizzle atoms, else one plane (an instruction per plane, plane = last coordinate).  Distinct maps per plane cost a
-// descriptor fetch per instruction: ~375 cycles each whatever the box size (profiles/cg_trace_r2.txt).  Returns the map index or -1.
+// descriptor fetch per instruction, whatever the box size.  Returns the map index or -1.
 int add_maps(V2State& v, uint16_t* const* planes, int np, int rank, std::initializer_list<uint64_t> dims, std::initializer_list<uint64_t> strides_b,
              std::initializer_list<uint32_t> box, std::initializer_list<uint32_t> estr = {}, bool allow_whole = true) {
   uint64_t d[5] = {1, 1, 1, 1, 1}, s[5] = {0, 0, 0, 0, 0};
@@ -360,6 +358,8 @@ int push_group(b2g_sac* h, std::vector<CgGroup>& list, CgGroup& g, const char* n
   for (int i = 0; i < g.n; ++i) {
     const CgProblem& P = g.host[i];
     if (P.planes * P.umma_n > 256) return b2g_fail(B2G_EINVAL, std::string("engine v2: planes x tile width exceeds one accumulator buffer (group ") + name + ")");
+    if (!cg_shape_supported(P.umma_n, P.nprod, P.mn_major != 0))
+      return b2g_fail(B2G_EINVAL, std::string("engine v2: no cg_kernel instance for the tile shape of a problem in group ") + name);
     g.flops += 2.0 * P.tiles_m * 128.0 * P.tiles_n * P.umma_n * P.chunks * 64.0;      // issued (tile-padded) work
   }
   list.push_back(g);
@@ -612,7 +612,7 @@ int v2_create(b2g_sac* h) {
       P.bias = h->p(std::string(nets[n]) + "/cnn_fc1/b"); P.bias_grp = 32;
       P.out_f = h->F[n]; P.f_tm = (long long)128 * FS; P.f0 = FS; P.f_grp = 32;
       if (v.split_fc1 > 1) {
-        // 48 tiles of 16 K-chunks would hold 48 of the 148 SMs for the longest stretch of the forward launch: three K-splits per
+        // 48 tiles of 16 K-chunks would hold 48 of the 132 SMs for the longest stretch of the forward launch: three K-splits per
         // tile, fp32 partial sums in a workspace, the last split to arrive finishes the tile (cg.cuh: ws)
         P.splits = v.split_fc1;
         if (int rc = valloc(h, &P.ws, (size_t)P.tiles_m * P.tiles_n * 128 * 64)) return rc;
@@ -866,9 +866,8 @@ int v2_create(b2g_sac* h) {
   }
   // ================================================================================ fused launches
   // One persistent launch for the forward chain (conv1 -> conv2 -> conv3 -> cnn_fc1 -> head fc0) and one for the backward chain up
-  // to the conv2 dgrad: a launch boundary costs ~7 us of an ~20 us layer (launch + TMEM allocation, first-fetch latency, the last
-  // tile's epilogue and the ragged last wave: profiles/cg_trace_r2.txt), a counter wait between dependent TILES costs nothing
-  // once the pipeline is full.  The stage ring is re-partitioned per problem (the conv2 wgrad needs 108 KB stages, the rest 64 - 72 KB).
+  // to the conv2 dgrad: a launch boundary costs a sizeable share of a layer (launch, first-fetch latency, the last tile's
+  // epilogue and the ragged last wave), a counter wait between dependent TILES costs nothing once the pipeline is full.  The stage ring is re-partitioned per problem (the conv2 wgrad needs 108 KB stages, the rest 64 - 72 KB).
   {
     const char* ef = getenv("B2G_FUSE");
     v.fuse = !(ef && ef[0] == '0');

@@ -1,7 +1,7 @@
 // fp32 CUDA-core gather-GEMM engine (precision mode B2G_PREC_FP32_SIMT).
 //
 // Bit-faithful fp32 FFMA arithmetic for every dense contraction on the SAC step; it is the
-// on-device numerical reference the tcgen05 engine (gg_tc.cu) is validated against, and the
+// on-device numerical reference the wgmma engine (gg_tc.cu) is validated against, and the
 // engine used for the small head-side contractions in every mode.
 // Tile: 64(m) x 64(n) x 16(r), 256 threads, 4x4 outputs per thread, register-prefetched smem.
 #include <cuda_bf16.h>

@@ -1,49 +1,51 @@
-// tcgen05 gather-GEMM engine (sm_100a): the dense contractions of the SAC step on the 5th-gen
-// tensor cores with fp32 accumulation in TMEM.
+// wgmma gather-GEMM engine (sm_90a): the dense contractions of the SAC step on the Hopper tensor
+// cores with fp32 accumulation in registers.
 //
 //   C[cM[m] + cN[n]] (=|+=) epi( sum_r A[aM[m] + aR[r]] * B[bR[r] + bN[n]] )       (common.cuh)
 //
 // Persistent, warp-specialised kernel: grid = min(#tiles, #SMs); every CTA walks the flattened tile
-// list of a grouped launch (tile = 128(m) x <=64(n) x its r-range) with three concurrent roles:
-//   * 16 producer warps gather fp32 operands through the offset tables (implicit im2col / wgrad /
+// list of a grouped launch (tile = 128(m) x <=64(n) x its r-range) with two concurrent roles:
+//   * producer warps gather fp32 operands through the offset tables (implicit im2col / wgrad /
 //     dgrad views), split every value into BF16 hi + BF16 lo (x = hi + lo to ~2^-17) and write both
-//     as K-major, 128B-swizzled UMMA tiles into a 4-stage shared-memory ring that runs continuously
+//     as K-major, 128B-swizzled wgmma tiles into a 3-stage shared-memory ring that runs continuously
 //     across tiles (generic-proxy stores -> fence.proxy.async -> mbarrier arrive);
-//   * 1 MMA warp (one thread) issues tcgen05.mma.cta_group::1.kind::f16 over the ring into one of
-//     two TMEM accumulators: mode BF16X3 = hi*hi + hi*lo + lo*hi (fp32-faithful to ~1e-5, the parity
-//     mode), mode BF16 = hi*hi only (fast mode); tcgen05.commit frees ring slots and publishes the
-//     accumulator;
-//   * 4 epilogue warps tcgen05.ld the finished accumulator (one row per thread), release it to the
-//     MMA warp at once, then apply bias+ReLU / ReLU-mask / split-R atomics and store, overlapping the
-//     next tile's mainloop.
-// TMEM: 2 x (128 lanes x 64 fp32 columns).  Shared memory: 4 x 48 KiB ring.
+//   * consumer warpgroups issue wgmma.mma_async over the ring into register accumulators: mode
+//     BF16X3 = hi*hi + hi*lo + lo*hi (fp32-faithful to ~1e-5, the parity mode), mode BF16 = hi*hi
+//     only (fast mode); each finished chunk frees its ring slot.  After the last chunk of a tile the
+//     accumulators go to a shared-memory tile (one row per thread from there on), and the same warps
+//     apply bias+ReLU / ReLU-mask / split-R atomics and store while the producers already fill the
+//     ring for the next tile.
+// Shared memory: 3 x 48 KiB ring, 32 KiB accumulator tile, 32 KiB store staging.
 #include <cuda_bf16.h>
 
 #include <algorithm>
 #include <vector>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace b2g {
 namespace {
 
 constexpr int TM = GG_TC_BM, TN = GG_TC_BN, TK = GG_TC_BK;   // tile: 128 x 64 x 64
-constexpr int STAGES = 4;
-// warp roles.  register-staged operands (fp32 sources): 16 producer warps, MMA warp, 4 epilogue warps (672 threads);
-// BF16-plane operands (cp.async): 8 producer warps, MMA warp, 8 epilogue warps (544 threads).
+constexpr int STAGES = 3;
+// warp roles.  register-staged operands (fp32 sources): 16 producer warps, one consumer warpgroup (640 threads);
+// BF16-plane operands (cp.async): 8 producer warps, two consumer warpgroups (512 threads).  Consumers run the MMAs and the
+// epilogue; warpgroups start at a warp index that is a multiple of 4.
 template <bool planes> struct Roles {
   static constexpr int NPROD = planes ? 256 : 512;
-  static constexpr int MMA_WARP = NPROD / 32;
+  static constexpr int MMA_WARP = NPROD / 32;            // first consumer warp
   static constexpr int NEPI = planes ? 256 : 128;
-  static constexpr int NTHREADS = NPROD + 32 + NEPI;
-  static constexpr int EPI_COLS = planes ? 32 : 64;      // accumulator columns handled by one epilogue warp
+  static constexpr int NTHREADS = NPROD + NEPI;
+  static constexpr int EPI_COLS = planes ? 32 : 64;      // accumulator columns handled by one consumer warp in the epilogue
+  static constexpr int MB = planes ? 1 : 2;              // m64 blocks of the 128-row tile per consumer warpgroup
 };
 constexpr int A_BYTES = TM * TK * 2;                    // 16 KiB per (hi | lo)
 constexpr int B_BYTES = TN * TK * 2;                    // 8 KiB
 constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;  // 48 KiB
 constexpr int STG_BYTES = TM * TN * 4;                   // fp32 output staging tile (32 KiB): coalesced epilogue stores
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STG_BYTES + 1024;
-constexpr int TMEM_COLS = 2 * TN;
+constexpr int ACC_BYTES = TM * TN * 4;                   // fp32 accumulator tile (32 KiB), rows of 256 B, 16-byte chunks XOR-swizzled by row
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STG_BYTES + ACC_BYTES + 1024;
 
 struct DescPack {
   GemmDesc d[GG_TC_MAX_DESCS];
@@ -75,37 +77,28 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 in
-// [0,14), LBO (ignored for swizzled K-major) in [16,30), SBO = 1024 B between 8-row groups in
-// [32,46), version 1 in [46,48), layout type 2 (SWIZZLE_128B) in [61,64).
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// MN-major, SWIZZLE_128B descriptor: atoms of 64 (M|N) x 8 (K) elements = 8 rows of 128 B; LBO = byte stride
-// between 64-element atoms along M|N, SBO = byte stride between 8-element atoms along K.
-__device__ __forceinline__ uint64_t umma_desc_mn(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-// kind::f16 instruction descriptor: D=f32 (bits 4-5 = 1), A=B=BF16 (bits 7-9, 10-12 = 1), K-major A/B,
-// N>>3 at bit 17, M>>4 at bit 24.
-__device__ __forceinline__ uint32_t umma_idesc(int m, int n, bool mn_major = false) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (mn_major ? (3u << 15) : 0u) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// The wgmmas of one ring chunk for the MB m64 blocks of this warpgroup (rows 64 * (m_first + mb)), N = tile width rounded up to
+// 32 or 64.  K-major tiles: rows of 128 B, 8-row groups 1024 B apart, 16 k = 32 bytes along the row.  MN-major tiles (wgrad):
+// 8-row K atoms of two 64-element M atoms (A, 1024 B apart) or one N atom (B); 16 k = two K atoms.
+template <int N, int TRANS, int MB>
+__device__ __forceinline__ void mma_chunk(float (&acc)[MB][32], uint32_t sA_hi, uint32_t sA_lo, uint32_t sB_hi, uint32_t sB_lo, int m_first, int x3) {
+#pragma unroll
+  for (int k = 0; k < TK / 16; ++k) {
+    const uint64_t bh = TRANS ? wg_desc(sB_hi + k * 2048, 1024, 1024) : wg_desc(sB_hi + k * 32, 16, 1024);
+    const uint64_t bl = TRANS ? wg_desc(sB_lo + k * 2048, 1024, 1024) : wg_desc(sB_lo + k * 32, 16, 1024);
+#pragma unroll
+    for (int mb = 0; mb < MB; ++mb) {
+      const uint32_t ao = TRANS ? (uint32_t)(k * 4096 + (m_first + mb) * 1024) : (uint32_t)((m_first + mb) * 8192 + k * 32);
+      const uint64_t ah = TRANS ? wg_desc(sA_hi + ao, 1024, 2048) : wg_desc(sA_hi + ao, 16, 1024);
+      Wgmma<N, TRANS>::mma(acc[mb], ah, bh);
+      if (x3) {
+        const uint64_t al = TRANS ? wg_desc(sA_lo + ao, 1024, 2048) : wg_desc(sA_lo + ao, 16, 1024);
+        Wgmma<N, TRANS>::mma(acc[mb], ah, bl);
+        Wgmma<N, TRANS>::mma(acc[mb], al, bh);
+      }
+    }
+  }
 }
 
 // 8 fp32 -> 8 bf16 hi (4 x b32) + 8 bf16 lo.  cvt.rn.bf16x2.f32 d, a, b packs a into the upper half.
@@ -174,7 +167,7 @@ __device__ __forceinline__ TileInfo tile_info(const DescPack& pk, int tile) {
   ti.r_begin = split * chunk_r;
   ti.r_end = min(R, ti.r_begin + chunk_r);
   ti.nchunks = ti.r_end > ti.r_begin ? (ti.r_end - ti.r_begin + TK - 1) / TK : 0;
-  ti.un = min(TN, ((d.N - ti.n0) + 15) / 16 * 16);   // UMMA N for this tile (multiple of 16)
+  ti.un = min(TN, ((d.N - ti.n0) + 15) / 16 * 16);   // MMA N for this tile (multiple of 16; the wgmma issues 32 or 64)
   return ti;
 }
 
@@ -184,8 +177,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
   constexpr int NPROD = Roles<planes>::NPROD, MMA_WARP = Roles<planes>::MMA_WARP, NEPI = Roles<planes>::NEPI;
   constexpr int EPI_COLS = Roles<planes>::EPI_COLS;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_full[STAGES], bar_empty[STAGES], bar_acc_full[2], bar_acc_empty[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t bar_full[STAGES], bar_empty[STAGES];
   __shared__ int s_cn[TN], s_kn[TN];
   __shared__ __align__(16) float s_bias[TN];
 
@@ -195,22 +187,11 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(smem_u32(&bar_full[s]), NPROD);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(smem_u32(&bar_acc_full[b]), 1);
-      mbar_init(smem_u32(&bar_acc_empty[b]), NEPI);
+      mbar_init(smem_u32(&bar_empty[s]), NEPI / 32);     // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == MMA_WARP) {   // MMA warp owns the TMEM allocation
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
   const uint32_t ring = (smem_u32(smem_raw) + 1023u) & ~1023u;
   pdl_trigger();      // the next kernel on the stream may begin its own prologue now
   pdl_wait();         // everything above overlapped the predecessor; its results are visible from here on
@@ -223,7 +204,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
 
   if (planes && warp < MMA_WARP) {
     // =========================================================================== producers (BF16 planes, cp.async)
-    // Operands are already split into BF16 hi/lo planes in HBM: every 16-byte chunk of a UMMA tile is one
+    // Operands are already split into BF16 hi/lo planes in HBM: every 16-byte chunk of a wgmma tile is one
     // cp.async straight into its swizzled slot -- no registers, no conversion; the ring depth is the prefetch
     // depth, and the slot's mbarrier is signalled by the copies themselves (cp.async.mbarrier.arrive.noinc).
     const int c8 = tid & 7, q = tid >> 3;      // 16-byte chunk, row group: A rows q + 32 i (i < 4), B rows q + 32 i (i < 2)
@@ -591,61 +572,22 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
         if (nb + 3 < d.N) atomicAdd(d.colsum + nb + 3, csum.w);
       }
     }
-  } else if (warp == MMA_WARP) {
-    // =========================================================================== MMA issuer
-    if (lane == 0) {
-      uint32_t gc = 0, it = 0;
-      for (int tile = t_begin; tile < t_end; tile += t_step) {
-        const TileInfo ti = tile_info(pk, tile);
-        if (ti.nchunks == 0) continue;
-        const uint32_t buf = it & 1;
-        if (it >= 2) mbar_wait(smem_u32(&bar_acc_empty[buf]), ((it >> 1) - 1) & 1);
-        tc_fence_after();
-        const bool mnm = planes && (pk.d[ti.p].flags & GG_MN_MAJOR);
-        const uint32_t idesc = umma_idesc(TM, ti.un, mnm);
-        const uint32_t acc = tmem + buf * TN;
-        for (int ch = 0; ch < ti.nchunks; ++ch, ++gc) {
-          const int s = gc % STAGES;
-          mbar_wait(smem_u32(&bar_full[s]), (gc / STAGES) & 1);
-          if (pk.trace && blockIdx.x == 0 && ch == 0 && it < 64) pk.trace[it * 8 + 2] = clock64();
-          if (planes) fence_proxy_async();       // cp.async (generic proxy) writes -> tensor-core (async proxy) reads
-          tc_fence_after();
-          const uint32_t sA_hi = ring + s * STAGE_BYTES, sA_lo = sA_hi + A_BYTES;
-          const uint32_t sB_hi = sA_lo + A_BYTES, sB_lo = sB_hi + B_BYTES;
-#pragma unroll
-          for (int k = 0; k < TK / 16; ++k) {
-            if (dbg_nomma) break;
-            // K-major: 16 k = 32 bytes inside the 128-byte row.  MN-major: 16 k = two 8-row K-atoms.
-            const uint64_t ah = mnm ? umma_desc_mn(sA_hi + k * 4096, 1024, 2048) : umma_desc(sA_hi + k * 32);
-            const uint64_t bh = mnm ? umma_desc_mn(sB_hi + k * 2048, 1024, 1024) : umma_desc(sB_hi + k * 32);
-            umma_bf16(acc, ah, bh, idesc, (ch | k) ? 1u : 0u);
-            if (x3) {
-              const uint64_t al = mnm ? umma_desc_mn(sA_lo + k * 4096, 1024, 2048) : umma_desc(sA_lo + k * 32);
-              const uint64_t bl = mnm ? umma_desc_mn(sB_lo + k * 2048, 1024, 1024) : umma_desc(sB_lo + k * 32);
-              umma_bf16(acc, ah, bl, idesc, 1u);
-              umma_bf16(acc, al, bh, idesc, 1u);
-            }
-          }
-          umma_commit(smem_u32(&bar_empty[s]));        // frees the ring slot when these MMAs retire
-        }
-        umma_commit(smem_u32(&bar_acc_full[buf]));     // accumulator complete -> epilogue
-        if (pk.trace && blockIdx.x == 0 && it < 64) pk.trace[it * 8 + 3] = clock64();
-        ++it;
-      }
-    }
-    __syncwarp();
   } else {
-    // =========================================================================== epilogue warps
-    // Each warp owns 32 accumulator rows (its TMEM lane quarter) x EPI_COLS columns.  Column-side tables (cN, kN,
-    // bias) of the tile are staged in shared memory BEFORE the accumulator is waited for.  Phase A: TMEM -> (+bias,
-    // ReLU) -> the warp's private fp32 staging rows; the accumulator is handed back to the MMA warp right after the
-    // last tcgen05.ld.  Phase B: staging rows -> (ReLU mask) -> global, fully coalesced: LPR lanes cover one row's
+    // =========================================================================== consumers: MMA + epilogue
+    // Mainloop: every consumer warpgroup issues the wgmmas of its m64 blocks for each ring chunk, waits for them and frees the
+    // slot (one arrival per warp).  Epilogue: the accumulators go to the shared accumulator tile, after which each warp owns 32
+    // rows (its lane quarter) x EPI_COLS columns.  Column-side tables (cN, kN, bias) of the tile are staged in shared memory
+    // BEFORE the mainloop.  Phase A: accumulator tile -> (+bias, ReLU) -> the warp's private fp32 staging rows.  Phase B: staging rows -> (ReLU mask) -> global, fully coalesced: LPR lanes cover one row's
     // contiguous run (fp32 float4 + BF16 hi/lo uint2), 32/LPR rows per instruction, loads batched ahead of stores.
     // Fast-path contract (GG_CN_AFFINE4, verified on the host): inside every aligned group of 4 columns cN / kN are
     // contiguous and the output offset is 16-byte aligned.
-    const int ew = warp - (MMA_WARP + 1);          // epilogue warp index
-    const int lq = warp & 3;                       // TMEM lane quarter this warp may access
-    const int et = tid - (MMA_WARP + 1) * 32;      // 0..NEPI-1
+    const int ew = warp - MMA_WARP;                // consumer warp index
+    const int lq = warp & 3;                       // row quarter of the tile this warp stores
+    const int et = tid - MMA_WARP * 32;            // 0..NEPI-1
+    constexpr int MB = Roles<planes>::MB;
+    const int m_first = (ew >> 2) * MB;            // first m64 block of this warpgroup
+    const uint32_t accs = ring + STAGES * STAGE_BYTES + STG_BYTES;
+    uint32_t gcm = 0;                              // ring chunk counter, continuous across tiles
     int pinned_p = -1, dflags = 0, dN = 0;
     float* dC = nullptr; uint16_t* dChi = nullptr; uint16_t* dClo = nullptr; const float* dmask = nullptr;
     const uint32_t stg = ring + STAGES * STAGE_BYTES + (uint32_t)ew * (32 * EPI_COLS * 4);
@@ -702,7 +644,6 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
       const int cm = cur.cm, km = cur.km_same ? cur.cm : cur.km;
       const bool m_ok = cur.ok;
       const GemmDesc& d = pk.d[ti.p];
-      const uint32_t buf = it & 1;
       if (cur.col_id != st_col || ti.n0 != staged_n0) {   // block-uniform: every epilogue warp walks the same tiles
         asm volatile("bar.sync 2, %0;" ::"n"(NEPI));  // previous readers of the staged tables are done
         if (et < TN) {
@@ -719,7 +660,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
         dC = pin(d.C); dChi = pin(d.C_hi); dClo = pin(d.C_lo); dmask = pin(d.mask);
         pinned_p = ti.p;
       }
-      // column split between the two warps of a TMEM lane quarter (8 epilogue warps, planes mode): 32 + 32 columns,
+      // column split between the two warps of a row quarter (8 epilogue warps, planes mode): 32 + 32 columns,
       // or 16 + 16 when the tile is at most 32 wide (conv1 fwd / wgrad, conv2 dgrad) so that no warp idles
       const int ecols = (NEPI == 256 && ti.un <= 32) ? 16 : EPI_COLS;
       const int col0 = (ew >> 2) * ecols;            // first accumulator column of this warp
@@ -745,19 +686,57 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
           if (early_mask && pact && ok_r && row < 32) mk0[u] = ldg4(dmask + km_r + kn);
         }
       }
-      mbar_wait(smem_u32(&bar_acc_full[buf]), (it >> 1) & 1);
-      tc_fence_after();
+      {
+        float acc[MB][32];
+#pragma unroll
+        for (int mb = 0; mb < MB; ++mb)
+#pragma unroll
+          for (int j = 0; j < 32; ++j) acc[mb][j] = 0.f;
+        const bool mnm = planes && (dflags & GG_MN_MAJOR);
+        for (int ch = 0; ch < ti.nchunks; ++ch, ++gcm) {
+          const int s = gcm % STAGES;
+          mbar_wait(smem_u32(&bar_full[s]), (gcm / STAGES) & 1);
+          if (planes) fence_proxy_async();       // cp.async (generic proxy) writes -> tensor-core (async proxy) reads
+          const uint32_t sA_hi = ring + s * STAGE_BYTES, sA_lo = sA_hi + A_BYTES;
+          const uint32_t sB_hi = sA_lo + A_BYTES, sB_lo = sB_hi + B_BYTES;
+          wg_arrive();
+          if (!dbg_nomma) {
+            if (mnm) mma_chunk<64, 1, MB>(acc, sA_hi, sA_lo, sB_hi, sB_lo, m_first, x3);
+            else if (ti.un <= 32) mma_chunk<32, 0, MB>(acc, sA_hi, sA_lo, sB_hi, sB_lo, m_first, x3);
+            else mma_chunk<64, 0, MB>(acc, sA_hi, sA_lo, sB_hi, sB_lo, m_first, x3);
+          }
+          wg_commit();
+          wg_wait<0>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(smem_u32(&bar_empty[s]));     // the ring slot may be refilled
+        }
+        // accumulator fragments -> the shared accumulator tile (every consumer has read the previous tile's rows)
+        asm volatile("bar.sync 3, %0;" ::"n"(NEPI));
+#pragma unroll
+        for (int mb = 0; mb < MB; ++mb)
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = 64 * (m_first + mb) + 16 * (ew & 3) + (lane >> 2) + 8 * h;
+              const int chunk = 2 * j + ((lane & 3) >> 1);
+              const uint32_t a = accs + (uint32_t)row * 256u + (uint32_t)((chunk ^ (row & 7)) << 4) + (uint32_t)((lane & 1) * 8);
+              asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(a), "f"(acc[mb][4 * j + 2 * h]), "f"(acc[mb][4 * j + 2 * h + 1]) : "memory");
+            }
+        asm volatile("bar.sync 3, %0;" ::"n"(NEPI));
+      }
       if (tr) pk.trace[it * 8 + 4] = clock64();
 #pragma unroll 1
       for (int cb = col0; cb < col0 + ncols_w; cb += 16) {
         uint32_t v[16];
-        const uint32_t taddr = tmem + buf * TN + ((uint32_t)(lq * 32) << 16) + (uint32_t)cb;
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-            : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        {
+          const int row = lq * 32 + lane;
+#pragma unroll
+          for (int g = 0; g < 4; ++g) {
+            const uint32_t a = accs + (uint32_t)row * 256u + (uint32_t)((((cb >> 2) + g) ^ (row & 7)) << 4);
+            asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v[4 * g]), "=r"(v[4 * g + 1]), "=r"(v[4 * g + 2]), "=r"(v[4 * g + 3]) : "r"(a));
+          }
+        }
         if (dbg_nostore) continue;
         if (fastp) {
           // phase A: accumulator row -> (+bias, ReLU) -> this warp's staging rows (16-byte chunks XOR-swizzled by row)
@@ -793,8 +772,6 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
           }
         }
       }
-      tc_fence_before();
-      mbar_arrive(smem_u32(&bar_acc_empty[buf]));   // this thread's TMEM reads of the tile are done
       if (tr) pk.trace[it * 8 + 5] = clock64();
       if (fastp && !dbg_nostore && ncols_w > 0) {
         __syncwarp();
@@ -853,12 +830,6 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
       if (tr) pk.trace[it * 8 + 6] = clock64();
       ++it;
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS));
   }
 }
 

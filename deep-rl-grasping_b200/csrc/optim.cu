@@ -353,7 +353,7 @@ void optim_launch(const OptimArgs& a, cudaStream_t s) {
   if (a.r_hi[0] > 0 || a.r_hi[1] > 0) n4 = ((a.r_hi[0] - a.r_lo[0]) + (a.r_hi[1] - a.r_lo[1])) >> 2;
   if (n4 <= 0) return;
   int grid = (n4 + 255) / 256;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   optim_kernel<<<grid, 256, 0, s>>>(a);
 }
 

@@ -251,7 +251,7 @@ int finalize_group(b2g_sac* h, GemmGroup& g) {
     }
     if (d.flags & GG_EPI_ATOMIC) {     // split-R sized for this engine's tile grid
       const int tiles = d.tiles_m * d.tiles_n;
-      int sp = std::max(1, (g.tc ? 148 : 148) / std::max(1, tiles));
+      int sp = std::max(1, h->num_sms / std::max(1, tiles));
       sp = std::min(sp, std::max(1, d.R / (2 * bk)));
       d.splitR = sp;
     }
@@ -273,7 +273,7 @@ int finalize_group(b2g_sac* h, GemmGroup& g) {
     for (auto& d : g.host) { auto it = first.find(d.layer); if (it == first.end() || d.tile_start < it->second) first[d.layer] = d.tile_start; }
     for (auto& d : g.host) d.need_done = d.layer > 0 ? first[d.layer] : 0;
   }
-  if (g.tc && h->tc_ranges && start > 0 && !g.layer_sync) {     // contiguous cost-balanced tile schedule of the tcgen05 engine
+  if (g.tc && h->tc_ranges && start > 0 && !g.layer_sync) {     // contiguous cost-balanced tile schedule of the wgmma engine
     g.ranges_grid = std::min(start, h->num_sms);
     const std::vector<int> rg = gg_tc_ranges(g.host.data(), (int)g.host.size(), start, g.ranges_grid);
     if (int rc = dalloc(h, &g.dev_ranges, rg.size(), false)) return rc;
@@ -286,7 +286,7 @@ int finalize_group(b2g_sac* h, GemmGroup& g) {
   return 0;
 }
 
-int split_for(int tiles, int R, int target_ctas = 148) {
+int split_for(int tiles, int R, int target_ctas = 132) {
   int s = std::max(1, target_ctas / std::max(1, tiles));
   const int max_s = std::max(1, R / (4 * GG_SIMT_BK));
   return std::min(s, max_s);
@@ -616,7 +616,7 @@ int build_groups(b2g_sac* h) {
     }
     GemmGroup a = g;
     // training step: the 516-deep reduction of each head is split over several CTAs (atomic accumulation into the
-    // pre-zeroed z0 block) -- 10 tiles would otherwise each walk 9 r-chunks serially on 10 of the 148 SMs
+    // pre-zeroed z0 block) -- 10 tiles would otherwise each walk 9 r-chunks serially on 10 of the 132 SMs
     if (h->fc0_split) for (auto& d : g.host) d.flags |= GG_EPI_ATOMIC;
     h->fwd_groups.push_back(g);
     a.name = "act_heads_fc0";
@@ -666,7 +666,7 @@ int build_groups(b2g_sac* h) {
     CK(cudaMemcpyAsync(h->d_jobs, jobs.data(), jobs.size() * sizeof(PlaneJob), cudaMemcpyHostToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));
   }
-  // one operand-contiguity mode per launch (the tcgen05 kernel is specialised on it): split mixed groups
+  // one operand-contiguity mode per launch (the wgmma kernel is specialised on it): split mixed groups
   {
     std::vector<GemmGroup> split;
     for (auto& g : h->bwd_groups) {
@@ -686,7 +686,7 @@ int build_groups(b2g_sac* h) {
     }
     h->bwd_groups.swap(split);
   }
-  // engine selection: the large dense contractions go to the tcgen05 engine unless fp32 SIMT is asked for
+  // engine selection: the large dense contractions go to the wgmma engine unless fp32 SIMT is asked for
   const char* sel = getenv("B2G_TC_GROUPS");   // debugging: comma-separated group names, "all" or "none"
   auto pick = [&](GemmGroup& g) {
     g.tc_eligible = g.name.find("conv") != std::string::npos || g.name.find("fc1_") != std::string::npos;
@@ -1328,7 +1328,7 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
   CK(cudaSetDevice(cfg->device));
   cudaDeviceProp prop{};
   CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) return fail(B2G_ECUDA, std::string("libb200grasp is built for sm_100a only; found ") + prop.name);
+  if (prop.major != 9) return fail(B2G_ECUDA, std::string("libb200grasp is built for sm_90a only; found ") + prop.name);
 
   b2g_sac* h = new b2g_sac();
   h->cfg = *cfg;
@@ -1795,10 +1795,8 @@ int b2g_sac_step_host_pipelined(b2g_sac* h, const float* obs, const float* act, 
   // (1) copy stream: this step's observations into staging slot j (free once the gather of step k-2 has run)
   // staging slot j is free once step k-2 has run (its losses' event: the step replays as a graph, so no event from inside it)
   if (k >= 2) CK(cudaStreamWaitEvent(h->cstream, h->use_graph ? h->ev_met[j] : h->ev_consumed[j], 0));
-  // Copy k+1 may or may not overlap the kernels of step k.  Measured on B200 boxes (tools/e2e_diag.py): on some, the 16.8 MB
-  // host-to-device copy and the step run side by side at full speed (2300 steps/s against 1140 back to back); on others they
-  // starve each other -- the copy takes 0.7 - 1.0 ms instead of 0.31, the step 0.45 - 0.70 ms instead of 0.26 -- and back to back
-  // wins (1750 against 1020).  So the first calls time both schedules (eight calls each, host clock, pipeline full) and the
+  // Copy k+1 may or may not overlap the kernels of step k: on some machines the host-to-device copy and the step run side by side
+  // at full speed, on others they starve each other and back to back wins.  So the first calls time both schedules (eight calls each, host clock, pipeline full) and the
   // faster one stays.  B2G_PIPE_MODE=overlap|serial pins it.  Either way the HOST stays pipelined: a call returns while its
   // copies and kernels are still queued.
   {

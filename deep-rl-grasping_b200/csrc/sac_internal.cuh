@@ -1,4 +1,4 @@
-// Internal declarations shared by sac.cu (handle, step orchestration, C ABI) and engine_v2.cu (TMA-fed tcgen05 engine).
+// Internal declarations shared by sac.cu (handle, step orchestration, C ABI) and engine_v2.cu (TMA-fed wgmma engine).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -99,7 +99,7 @@ using namespace b2g;   // (internal header: only library translation units inclu
 struct b2g_sac {
   b2g_sac_cfg cfg{};
   bool cnn = false;
-  int num_sms = 148;
+  int num_sms = 132;
   int B = 0, A = 0, H = 0, E = 0, Cimg = 0, feat_dim = 0, FS = 0;
   int Hi = 0, Wi = 0, H1 = 0, W1 = 0, H2 = 0, W2 = 0, H3 = 0, W3 = 0;
   std::vector<Tensor> tensors;

@@ -143,7 +143,7 @@ __global__ void __launch_bounds__(WARPS * 32) tail_kernel(TailArgs t) {
   pdl_wait();
   const float* k1s[S_NW] = {t.pi.k1, t.vf.k1, t.q1.k1, t.q2.k1, t.vt.k1};
   // stage the five 64x64 fc1 kernels (row stride 65) with 4-byte cp.async: all 80 copies of a thread are in flight
-  // at once (a load->store loop serialises into ~80 round trips and dominated this kernel, profiles/ncu_tail_r1.md)
+  // at once (a load->store loop serialises into ~80 round trips and dominated this kernel)
   for (int w = 0; w < S_NW; ++w)
     for (int i = tid; i < H * H; i += blockDim.x) {
       const uint32_t dst = (uint32_t)__cvta_generic_to_shared(&Wk1[w * H * LD + (i >> 6) * LD + (i & 63)]);

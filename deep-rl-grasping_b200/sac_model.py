@@ -1,7 +1,7 @@
 """``SAC`` -- the stable-baselines model object the reference constructs and drives
 (/root/reference/manipulation_main/training/sb_helper.py:104-128,175,186-198,241-247;
 train_stable_baselines.py:95-106; utils.py:71; base_callbacks.py:84-111,145-146), re-hosted on the
-B200 learner.  Same constructor keywords, ``learn / predict / save / load / get_parameters /
+H100 learner.  Same constructor keywords, ``learn / predict / save / load / get_parameters /
 load_parameters / get_env / get_vec_normalize_env``, same callback protocol, same zip format.
 
 What runs where: env stepping (PyBullet) and this loop stay on host cores; replay storage,

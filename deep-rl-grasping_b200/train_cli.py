@@ -1,4 +1,4 @@
-"""``train`` / ``run`` command line of the reference, re-hosted on the B200 learner.
+"""``train`` / ``run`` command line of the reference, re-hosted on the H100 learner.
 
 Mirrors /root/reference/manipulation_main/training/train_stable_baselines.py:26-148 (same sub-commands, flags,
 ``model_dir`` layout: ``config.yaml``, ``best_model/``, ``logs/rl_model_*`` checkpoints, ``vecnormalize.pkl``,
@@ -123,7 +123,7 @@ def train(args):
         if args.load_dir:
             model.load_parameters(BDQ.load(args.load_dir, env).get_parameters())
     else:
-        raise NotImplementedError(f"--algo {algo}: the B200 learner builds the SAC and BDQ branches of SBPolicy.learn (sb_helper.py:85-226)")
+        raise NotImplementedError(f"--algo {algo}: the H100 learner builds the SAC and BDQ branches of SBPolicy.learn (sb_helper.py:85-226)")
     model.learn(total_timesteps=int(c["total_timesteps"]), callback=callbacks)
     model.save(os.path.join(args.model_dir, "final_model" if algo != "BDQ" else "bdq_model"))   # sb_helper.py:228-247
     vn = model.get_vec_normalize_env()
@@ -170,7 +170,7 @@ def run(args):
     elif algo == "bdq":
         agent = BDQ.load(args.model)
     else:
-        raise NotImplementedError(f"algorithm '{algo}': only sac / bdq zips run on the B200 learner")
+        raise NotImplementedError(f"algorithm '{algo}': only sac / bdq zips run on the H100 learner")
     print("Run the agent")
     out = run_agent(task, agent, args.stochastic, n_episodes=args.episodes)
     task.close()

@@ -1,5 +1,5 @@
 /*
- * b200grasp.h -- C ABI of the B200-native SAC learner (libb200grasp.so).
+ * b200grasp.h -- C ABI of the H100-native SAC learner (libb200grasp.so).
  *
  * Drop-in boundary for the ONE hot path of BarisYazici/deep-rl-grasping: the replay-buffer
  * minibatch gradient step that the reference delegates to stable_baselines.SAC (TF1) --
@@ -34,8 +34,8 @@ extern "C" {
 
 /* precision modes of the dense contractions (convs, cnn_fc1, fc0 layers) */
 #define B2G_PREC_FP32_SIMT 0   /* fp32 FFMA on CUDA cores: bit-faithful fp32 arithmetic            */
-#define B2G_PREC_BF16X3 1      /* tcgen05 BF16 hi/lo split, 3 MMAs, fp32 TMEM accumulate (~2^-16)  */
-#define B2G_PREC_BF16 2        /* tcgen05 single-pass BF16 (fast mode; tolerance reported)         */
+#define B2G_PREC_BF16X3 1      /* wgmma BF16 hi/lo split, 3 MMAs, fp32 accumulate (~2^-16)        */
+#define B2G_PREC_BF16 2        /* wgmma single-pass BF16 (fast mode; tolerance reported)           */
 
 typedef struct b2g_sac b2g_sac;
 
@@ -246,7 +246,7 @@ int b2g_encoder_set_weights(b2g_encoder* h, int layer, const float* kernel, size
 int b2g_encoder_encode(b2g_encoder* h, const float* imgs, int n, float* out);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Bring-up hook (not on the product path): C[M,N] = A[M,K] * B[N,K]^T through the tcgen05 engine; host pointers,
+ * Bring-up hook (not on the product path): C[M,N] = A[M,K] * B[N,K]^T through the wgmma engine; host pointers,
  * K a multiple of 8; x3 != 0 -> BF16 hi/lo split (3 MMAs); split_k > 1 -> that many partial accumulators summed
  * with fp32 atomics.  tools/tc_accum_probe.py uses it to measure the accumulation behaviour of the tensor core.
  * ------------------------------------------------------------------------------------------------------------ */

@@ -45,8 +45,8 @@ def _check_step(cfg, params, vn, B, tol=TOL, precision=0):
     # per-tensor gradients, conditioning-aware: a tensor whose per-sample contributions cancel amplifies the unit
     # round-off of whatever arithmetic formed it, and the fp32 oracle's own distance from float64 measures that
     # amplification: <= max(1e-3, 3 x fp32-oracle error) for BOTH engines.  (Round 1 needed 1e-2 / 192x for the tensor
-    # engine: its 2-plane BF16 forward and the truncating TMEM accumulation cost two decimal digits; the 3-plane forward
-    # with separate leading / correction accumulators is at fp32 level, profiles/precision_r2.md.)
+    # engine: its 2-plane BF16 forward and the truncating tensor-core accumulation cost two decimal digits; the 3-plane forward
+    # with separate leading / correction accumulators is at fp32 level, tools/precision_emulation.py.)
     gtol = 10 * tol
     gbar = {n: max(gtol, 3.0 * rel_err(grads[n], grads64[n])) for n in grads64}
     worst_g = max(gerr, key=lambda n: gerr[n] / gbar[n])
@@ -114,7 +114,7 @@ def test_depth_cnn_fresh_init_b256():
 
 @pytest.mark.parametrize("B", [32, 256])
 def test_tcgen05_bf16x3_parity_mode(B):
-    """Tensor-core engine (parity mode: BF16 plane split, fp32 TMEM accumulate): held to the SAME bars as the fp32 engine."""
+    """Tensor-core engine (parity mode: BF16 plane split, fp32 accumulate): held to the SAME bars as the fp32 engine."""
     cfg, params, vn = load_case("sac_depth")
     _check_step(cfg, params, vn, B, precision=1)
 

@@ -1,5 +1,5 @@
 """CPU emulation of the tensor engine's split-precision arithmetic on the REAL SAC step (oracle/sac_ref_np.py with every
-matmul replaced), used to decide which operand split each contraction needs (profiles/precision_r2.md).
+matmul replaced), used to decide which operand split each contraction needs.
 
 Every matmul operand is split into `n` BF16 (or scaled FP16) terms; the chosen products are summed in float64, i.e. with an
 IDEAL accumulator, so what is measured is the operand split alone.  FWD / BWD select the mode of the forward and the

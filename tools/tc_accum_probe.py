@@ -1,6 +1,6 @@
-"""How exact is the tensor core's fp32 accumulation (TMEM) on cancelling reductions?
+"""How exact is the tensor core's fp32 accumulation on cancelling reductions?
 
-C = A B^T through the tcgen05 engine (b2g_debug_gemm) against float64 evaluated on the SAME bf16-split operands
+C = A B^T through the wgmma engine (b2g_debug_gemm) against float64 evaluated on the SAME bf16-split operands
 (hi*hi + hi*lo + lo*hi in float64), so the operand split drops out and what is left is the accumulation itself.
 Rows of A / B are built so that the products cancel to a chosen fraction of their absolute sum."""
 import ctypes as C

@@ -1,4 +1,4 @@
-// tma_rate: how fast can ONE SM (and all 148 together) pull L2-resident data with cp.async.bulk.tensor?
+// tma_rate: how fast can ONE SM (and all 132 of an H100 together) pull L2-resident data with cp.async.bulk.tensor?
 // Each CTA streams `iters` boxes of [rows x 128 B] from a 32 MB bf16 matrix (L2 resident after the warm-up pass) into a ring of
 // `stages` shared-memory slots; a box is re-armed as soon as it lands (no consumer).  Reports GB/s per SM and aggregate
 // for several (grid, stages, rows-per-box, issuing-thread count).
@@ -58,7 +58,7 @@ int main() {
     CUtensorMap m;
     cuuint64_t gd[2] = {NC, NR}, gs[1] = {NC * 2}; cuuint32_t bx[2] = {64, (cuuint32_t)rows}, es[2] = {1, 1};
     if (enc(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, d, gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) { printf("encode failed\n"); return 1; }
-    const int grids[2] = {1, 148};
+    const int grids[2] = {1, 132};
     for (int gi = 0; gi < 2; ++gi)
       for (int stages = 2; stages <= 8; stages *= 2) {
         for (int issuers = 1; issuers <= 4; issuers *= 2) {
