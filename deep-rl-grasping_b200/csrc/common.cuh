@@ -83,8 +83,6 @@ struct GemmDesc {
   int tile_start;   // first flattened CTA index of this problem inside a grouped launch
   int tile_count;
   int col_id;       // wgmma engine: identity of (cN, kN, bias, N); equal ids share the staged column tables
-  int layer;        // host side: layer index inside a fused (layer-synchronised) launch
-  int need_done;    // fused launch: tiles [0, need_done) of the launch must be complete before this problem's operands are read
 };
 
 struct GemmGroup {          // one grouped launch
@@ -94,23 +92,15 @@ struct GemmGroup {          // one grouped launch
   int total_tiles = 0;
   double flops = 0;
   bool tc = false;          // run on the wgmma engine
-  bool tc_eligible = false; // large dense contraction (convs, cnn_fc1)
-  int* dev_ranges = nullptr; // wgmma engine: contiguous tile range per CTA (gg_tc_ranges)
-  int ranges_grid = 0;
-  bool layer_sync = false;   // several dependent layers in ONE persistent launch (in-kernel completion counter)
 };
 
 // engines (gg_simt.cu / gg_tc.cu)
 void gg_simt_launch(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaStream_t s);
 constexpr int GG_SIMT_BM = 64, GG_SIMT_BN = 64, GG_SIMT_BK = 16;
 // wgmma engine: 128 x 64 output tile, 64-wide r-chunks; x3 != 0 -> BF16 hi/lo split (3 MMAs)
-cudaError_t gg_tc_launch(const GemmDesc* host_descs, int ndesc, int total_tiles, int mode_flags, int x3, int num_sms, cudaStream_t s,
-                         const int* dev_ranges = nullptr, int ranges_grid = 0, unsigned* sync_ctr = nullptr);
-// host side of the contiguous tile schedule: cost-balanced range boundaries [grid + 1] for a finalized group
-std::vector<int> gg_tc_ranges(const GemmDesc* host_descs, int ndesc, int total_tiles, int grid);
+cudaError_t gg_tc_launch(const GemmDesc* host_descs, int ndesc, int total_tiles, int mode_flags, int x3, int num_sms, cudaStream_t s);
 constexpr int GG_TC_MAX_DESCS = 16;
 int gg_tc_smem_bytes();
-extern long long* g_tc_trace;   // bring-up hook (gg_tc.cu)
 constexpr int GG_TC_BM = 128, GG_TC_BN = 64, GG_TC_BK = 64;
 
 // ---------------------------------------------------------------------------------------------

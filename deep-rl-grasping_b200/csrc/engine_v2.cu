@@ -9,9 +9,8 @@
 //                    conv1 patch rows (8x8 stride-4 patches of the normalised image; the one view TMA cannot express, see
 //                    tools/tma_probe.cu) so that conv1 forward and its wgrad are plain 2-D TMA tiles;
 //   compact_kernel : full observation rows -> compact replay rows (image planes | actuator value);
-//   planes2_kernel : weights -> BF16 planes in the layouts the tensor maps expect (transposed / packed per consumer);
-//   colsum2_kernel : bias gradients as column sums of the gradient-map planes -- only with B2G_BIAS_EPI=0: by default the DGRAD
-//                    epilogues of cg.cu produce them.
+//   planes2_kernel : weights -> BF16 planes in the layouts the tensor maps expect (transposed / packed per consumer).
+// The bias gradients of the conv and cnn_fc1 layers come from the DGRAD epilogues of cg.cu (column sums of the gradient maps).
 // Reference shapes: custom_obs_policy.py:34-40 (conv 8x8/4 -> 4x4/2 -> 3x3/1, fc 1024->512), SURVEY.md Appendix A.
 #include <cuda_bf16.h>
 
@@ -29,7 +28,6 @@ namespace {
 struct Gather2Args {
   GatherArgs g;                 // sources, statistics, F rows (fp32), reward / done outputs, slot draw
   uint16_t* a1[2][3];           // patch matrices [B*225][64*Ci] (obs, next_obs) x 3 planes
-  uint16_t* xp[2][2];           // plain NHWC planes hi / lo (conv1 wgrad of the v1 backward); may be null
   uint16_t* fp[3][3];           // feature-row planes [net][plane] [B][KF]
   int KF, Ci, OH, OW;           // OH = OW = 15
 };
@@ -62,7 +60,6 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
   // shared-memory planes with a padded row pitch (+8 elements = +4 banks per image row): the patch pass below reads 16-byte runs
   // of 8 consecutive image rows at once, which a 128-byte pitch puts on the same four banks (8-way conflicts)
   const int rowe = g.W * Ci, pitch = rowe + 8, plane_e = g.H * pitch;
-  uint16_t* xh = a.xp[which][0]; uint16_t* xl = a.xp[which][1];
   (void)Cfull;
   // image block: exactly the NHWC image with Ci channels -> no index arithmetic; float64 VecNormalize chain per element
   for (int e4 = tid; e4 < (npx >> 2); e4 += blockDim.x) {
@@ -84,7 +81,6 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
       const uint2 w = make_uint2((uint32_t)p[pl][0] | ((uint32_t)p[pl][1] << 16), (uint32_t)p[pl][2] | ((uint32_t)p[pl][3] << 16));
       const int e = 4 * e4, row = e / rowe, col = e - row * rowe;          // (rowe is a multiple of 4: a group never straddles rows)
       *reinterpret_cast<uint2*>(sm_planes + pl * plane_e + row * pitch + col) = w;
-      if (xh && pl < 2) reinterpret_cast<uint2*>((pl ? xl : xh) + (size_t)b * npx)[e4] = w;
     }
   }
   if (tid == 0) {                                            // direct feature -> column 512 of the feature rows
@@ -217,45 +213,6 @@ __global__ void __launch_bounds__(256) planes2_kernel(const Plane2Job* __restric
       }
     }
   }
-}
-
-// ------------------------------------------------------------------------------------------------ colsum2
-// bias gradients: dst[n] += sum over rows of (hi + lo)[row * pitch + col0 + n].  Thread = (row group, 8-column group).
-struct Colsum2Job { const uint16_t* hi; const uint16_t* lo; float* dst; int rows, pitch, col0, N; int cta_start; };
-
-__global__ void __launch_bounds__(256) colsum2_kernel(const Colsum2Job* __restrict__ jobs, int njobs) {
-  __shared__ float red[512];
-  int j = 0;
-  while (j + 1 < njobs && (int)blockIdx.x >= jobs[j + 1].cta_start) ++j;
-  const Colsum2Job job = jobs[j];
-  const int N = job.N, N8 = N >> 3, tid = threadIdx.x;
-  const int groups = 256 / N8;                 // N <= 512 -> N8 <= 64
-  const int rows_per_cta = 16 * groups;
-  const int r0 = (blockIdx.x - job.cta_start) * rows_per_cta;
-  for (int i = tid; i < N; i += 256) red[i] = 0.f;
-  __syncthreads();
-  const int g = tid / N8, c8 = tid - g * N8;
-  if (g < groups) {
-    float s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-#pragma unroll 4
-    for (int i = 0; i < 16; ++i) {
-      const int r = r0 + g + i * groups;
-      if (r < job.rows) {
-        const size_t o = (size_t)r * job.pitch + job.col0 + 8 * c8;
-        const uint4 h = *reinterpret_cast<const uint4*>(job.hi + o), l = *reinterpret_cast<const uint4*>(job.lo + o);
-        const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lw[4] = {l.x, l.y, l.z, l.w};
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          s[2 * u] += __uint_as_float(hw[u] << 16) + __uint_as_float(lw[u] << 16);
-          s[2 * u + 1] += __uint_as_float(hw[u] & 0xFFFF0000u) + __uint_as_float(lw[u] & 0xFFFF0000u);
-        }
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < 8; ++u) atomicAdd(&red[8 * c8 + u], s[u]);
-  }
-  __syncthreads();
-  for (int i = tid; i < N; i += 256) atomicAdd(job.dst + i, red[i]);
 }
 
 // ------------------------------------------------------------------------------------------------ host helpers
@@ -494,17 +451,15 @@ int v2_create(b2g_sac* h) {
   add_job(h->p("model/values_fn/qf1/fc0/kernel"), h->feat_dim + h->A, 64, v.K0T[1], 3, 1, KF, 64);
   add_job(h->p("model/values_fn/qf2/fc0/kernel"), h->feat_dim + h->A, 64, v.K0T[1], 3, 1, KF, 128);
   add_job(h->p("target/values_fn/vf/fc0/kernel"), h->feat_dim, 64, v.K0T[2], 3, 1, KF, 0);
-  if (v.bwd) {
-    for (int n = 0; n < 2; ++n) {
-      add_job(h->p(std::string(nets[n]) + "/cnn2/w"), 512, 64, v.W2n[n], 2, 0, 64, 0);
-      add_job(h->p(std::string(nets[n]) + "/cnn3/w"), 576, 64, v.W3n[n], 2, 0, 64, 0);
-      add_job(h->p(std::string(nets[n]) + "/cnn_fc1/w"), 1024, 512, v.Wfn[n], 2, 0, 512, 0);
-    }
-    add_job(h->p("model/pi/fc0/kernel"), h->feat_dim, 64, v.K0n[0], 2, 0, 64, 0);
-    add_job(h->p("model/values_fn/vf/fc0/kernel"), h->feat_dim, 64, v.K0n[1], 2, 0, 192, 0);
-    add_job(h->p("model/values_fn/qf1/fc0/kernel"), h->feat_dim + h->A, 64, v.K0n[1], 2, 0, 192, 64);
-    add_job(h->p("model/values_fn/qf2/fc0/kernel"), h->feat_dim + h->A, 64, v.K0n[1], 2, 0, 192, 128);
+  for (int n = 0; n < 2; ++n) {
+    add_job(h->p(std::string(nets[n]) + "/cnn2/w"), 512, 64, v.W2n[n], 2, 0, 64, 0);
+    add_job(h->p(std::string(nets[n]) + "/cnn3/w"), 576, 64, v.W3n[n], 2, 0, 64, 0);
+    add_job(h->p(std::string(nets[n]) + "/cnn_fc1/w"), 1024, 512, v.Wfn[n], 2, 0, 512, 0);
   }
+  add_job(h->p("model/pi/fc0/kernel"), h->feat_dim, 64, v.K0n[0], 2, 0, 64, 0);
+  add_job(h->p("model/values_fn/vf/fc0/kernel"), h->feat_dim, 64, v.K0n[1], 2, 0, 192, 0);
+  add_job(h->p("model/values_fn/qf1/fc0/kernel"), h->feat_dim + h->A, 64, v.K0n[1], 2, 0, 192, 64);
+  add_job(h->p("model/values_fn/qf2/fc0/kernel"), h->feat_dim + h->A, 64, v.K0n[1], 2, 0, 192, 128);
   v.n_plane_jobs = (int)jobs.size();
   v.plane_ctas = start;
   Plane2Job* dj = nullptr;
@@ -547,7 +502,6 @@ int v2_create(b2g_sac* h) {
       for (int p = 0; p < 3; ++p) P.out_p[p] = v.H1[net0][p];
       P.bias = h->p(std::string(nets[net0]) + "/cnn1/b");
       P.bias_grp = w == 0 ? (int)(h->p("model/values_fn/cnn1/b") - h->p("model/pi/cnn1/b")) : 32;
-      if (!v.bwd) { P.out_f = h->h1[net0]; P.f_tm = 128 * 32; P.f0 = 32; P.f_grp = w == 0 ? (long long)(h->h1[1] - h->h1[0]) : 32; }
       g.host[g.n++] = P;
     }
     if (int rc = push_group(h, v.fwd, g, "conv1_fwd")) return rc;
@@ -568,7 +522,6 @@ int v2_create(b2g_sac* h) {
       P.o_tm = 108 * 64; P.o0 = 64; P.n_valid = 64; P.out_planes = 3;
       for (int p = 0; p < 3; ++p) P.out_p[p] = v.H2[n][p];
       P.bias = h->p(std::string(nets[n]) + "/cnn2/b"); P.bias_grp = 32;
-      if (!v.bwd) { P.out_f = h->h2[n]; P.f_tm = 108 * 64; P.f0 = 64; P.f_grp = 32; }
       g.host[g.n++] = P;
     }
     if (int rc = push_group(h, v.fwd, g, "conv2_fwd")) return rc;
@@ -589,7 +542,6 @@ int v2_create(b2g_sac* h) {
       P.o_tm = 128 * 64; P.o0 = 64; P.n_valid = 64; P.out_planes = 3;
       for (int p = 0; p < 3; ++p) P.out_p[p] = v.H3[n][p];
       P.bias = h->p(std::string(nets[n]) + "/cnn3/b"); P.bias_grp = 32;
-      if (!v.bwd) { P.out_f = h->h3[n]; P.f_tm = 128 * 64; P.f0 = 64; P.f_grp = 32; }
       g.host[g.n++] = P;
     }
     if (int rc = push_group(h, v.fwd, g, "conv3_fwd")) return rc;
@@ -646,282 +598,246 @@ int v2_create(b2g_sac* h) {
   }
 
   // ================================================================================ backward problems (3-product mode)
-  { const char* e = getenv("B2G_BIAS_EPI"); v.epi_colsum = !(e && e[0] == '0'); }
-  if (v.bwd) {
-    const int NB = 2;
-    // ---- heads dgrad: dZ4 = dz0 . K0^T, masked by the cnn_fc1 ReLU (F > 0)
-    {
-      CgGroup g;
-      for (int n = 0; n < 2; ++n) {
-        const int Kd = n == 0 ? 64 : 192;
-        uint16_t* const* dz = n == 0 ? v.dz0pi : v.dz0v;
-        const int mA = add_maps(v, dz, NB, 2, {(uint64_t)Kd, (uint64_t)B}, {(uint64_t)Kd * 2}, {64, 128});
-        const int mB = add_maps(v, v.K0n[n], NB, 2, {(uint64_t)Kd, (uint64_t)KF}, {(uint64_t)Kd * 2}, {64, 128});
-        if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (heads dgrad)");
-        CgProblem P = kmajor(NB, 128, Kd / 64, Kd / 64, 128);
+  const int NB = 2;
+  // ---- heads dgrad: dZ4 = dz0 . K0^T, masked by the cnn_fc1 ReLU (F > 0)
+  {
+    CgGroup g;
+    for (int n = 0; n < 2; ++n) {
+      const int Kd = n == 0 ? 64 : 192;
+      uint16_t* const* dz = n == 0 ? v.dz0pi : v.dz0v;
+      const int mA = add_maps(v, dz, NB, 2, {(uint64_t)Kd, (uint64_t)B}, {(uint64_t)Kd * 2}, {64, 128});
+      const int mB = add_maps(v, v.K0n[n], NB, 2, {(uint64_t)Kd, (uint64_t)KF}, {(uint64_t)Kd * 2}, {64, 128});
+      if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (heads dgrad)");
+      CgProblem P = kmajor(NB, 128, Kd / 64, Kd / 64, 128);
+      P.nloads = 2;
+      P.ld[0] = mk_load(mA, 2, 0); P.ld[0].d_tm[1] = 128; P.ld[0].d_c2[0] = 64;
+      P.ld[1] = mk_load(mB, 2, P.b_off); P.ld[1].d_tn[1] = 128; P.ld[1].d_c2[0] = 64;
+      P.tiles_m = (B + 127) / 128; P.tiles_n = 4;
+      P.epi = CG_EPI_DGRAD; P.rows_tile = 128; P.lim_rows = B;
+      P.o_tm = 128 * 512; P.o0 = 512; P.n_valid = 512; P.out_planes = 2;
+      for (int p = 0; p < 2; ++p) P.out_p[p] = v.dZ4[n][p];
+      P.mask = v.F[n][0]; P.m_tm = (long long)128 * KF; P.m0 = KF;
+      P.colsum = h->g(std::string(nets[n]) + "/cnn_fc1/b"); P.colsum_mask = 511;
+      g.host[g.n++] = P;
+    }
+    if (int rc = push_group(h, v.bwd_groups, g, "heads_dgrad")) return rc;
+  }
+  // ---- cnn_fc1 backward: dgrad dZ3 = dZ4 . Wf^T (masked by h3 > 0) and wgrad G_Wf = h3^T . dZ4 (MN-major, K = batch)
+  {
+    CgGroup g;
+    for (int n = 0; n < 2; ++n) {
+      {
+        const int mA = add_maps(v, v.dZ4[n], NB, 2, {512, (uint64_t)B}, {1024}, {64, 128});
+        const int mB = add_maps(v, v.Wfn[n], NB, 2, {512, 1024}, {1024}, {64, 128});
+        if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (fc1 dgrad)");
+        CgProblem P = kmajor(NB, 128, 8, 8, 128);
         P.nloads = 2;
         P.ld[0] = mk_load(mA, 2, 0); P.ld[0].d_tm[1] = 128; P.ld[0].d_c2[0] = 64;
         P.ld[1] = mk_load(mB, 2, P.b_off); P.ld[1].d_tn[1] = 128; P.ld[1].d_c2[0] = 64;
-        P.tiles_m = (B + 127) / 128; P.tiles_n = 4;
+        P.tiles_m = (B + 127) / 128; P.tiles_n = 8;
         P.epi = CG_EPI_DGRAD; P.rows_tile = 128; P.lim_rows = B;
-        P.o_tm = 128 * 512; P.o0 = 512; P.n_valid = 512; P.out_planes = 2;
-        for (int p = 0; p < 2; ++p) P.out_p[p] = v.dZ4[n][p];
-        P.mask = v.F[n][0]; P.m_tm = (long long)128 * KF; P.m0 = KF;
-        if (v.epi_colsum) { P.colsum = h->g(std::string(nets[n]) + "/cnn_fc1/b"); P.colsum_mask = 511; }
-        g.host[g.n++] = P;
-      }
-      if (int rc = push_group(h, v.bwd_groups, g, "heads_dgrad")) return rc;
-    }
-    // ---- cnn_fc1 backward: dgrad dZ3 = dZ4 . Wf^T (masked by h3 > 0) and wgrad G_Wf = h3^T . dZ4 (MN-major, K = batch)
-    {
-      CgGroup g;
-      for (int n = 0; n < 2; ++n) {
-        {
-          const int mA = add_maps(v, v.dZ4[n], NB, 2, {512, (uint64_t)B}, {1024}, {64, 128});
-          const int mB = add_maps(v, v.Wfn[n], NB, 2, {512, 1024}, {1024}, {64, 128});
-          if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (fc1 dgrad)");
-          CgProblem P = kmajor(NB, 128, 8, 8, 128);
-          P.nloads = 2;
-          P.ld[0] = mk_load(mA, 2, 0); P.ld[0].d_tm[1] = 128; P.ld[0].d_c2[0] = 64;
-          P.ld[1] = mk_load(mB, 2, P.b_off); P.ld[1].d_tn[1] = 128; P.ld[1].d_c2[0] = 64;
-          P.tiles_m = (B + 127) / 128; P.tiles_n = 8;
-          P.epi = CG_EPI_DGRAD; P.rows_tile = 128; P.lim_rows = B;
-          P.o_tm = 128 * 1024; P.o0 = 1024; P.n_valid = 1024; P.out_planes = 2;
-          for (int p = 0; p < 2; ++p) P.out_p[p] = v.dZ3[n][p];
-          P.mask = v.H3[n][0]; P.m_tm = 128 * 1024; P.m0 = 1024;
-          if (v.epi_colsum) { P.colsum = h->g(std::string(nets[n]) + "/cnn3/b"); P.colsum_mask = 63; }     // dZ3 row = [16 pixels][64 channels]
-          if (v.split_fc1_dgrad > 1) {         // 32 tiles of 8 K-chunks at the head of the backward chain: split-K with finalisation
-            P.splits = v.split_fc1_dgrad;
-            if (int rc = valloc(h, &P.ws, (size_t)P.tiles_m * P.tiles_n * 128 * 128)) return rc;
-            if (int rc = valloc(h, &P.ws_cnt, (size_t)P.tiles_m * P.tiles_n * CG_EPI_WARPS)) return rc;
-          }
-          g.host[g.n++] = P;
+        P.o_tm = 128 * 1024; P.o0 = 1024; P.n_valid = 1024; P.out_planes = 2;
+        for (int p = 0; p < 2; ++p) P.out_p[p] = v.dZ3[n][p];
+        P.mask = v.H3[n][0]; P.m_tm = 128 * 1024; P.m0 = 1024;
+        P.colsum = h->g(std::string(nets[n]) + "/cnn3/b"); P.colsum_mask = 63;     // dZ3 row = [16 pixels][64 channels]
+        if (v.split_fc1_dgrad > 1) {         // 32 tiles of 8 K-chunks at the head of the backward chain: split-K with finalisation
+          P.splits = v.split_fc1_dgrad;
+          if (int rc = valloc(h, &P.ws, (size_t)P.tiles_m * P.tiles_n * 128 * 128)) return rc;
+          if (int rc = valloc(h, &P.ws_cnt, (size_t)P.tiles_m * P.tiles_n * CG_EPI_WARPS)) return rc;
         }
-        {
-          const int mA = add_maps(v, v.H3[n], NB, 2, {1024, (uint64_t)B}, {2048}, {64, 64});
-          const int mB = add_maps(v, v.dZ4[n], NB, 2, {512, (uint64_t)B}, {1024}, {64, 64}, {}, false);     // two B atoms per plane
-          if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (fc1 wgrad)");
-          CgProblem P = mnmajor(NB, 64, 2, 2, (B + 63) / 64);
-          P.nloads = 4;
-          for (int a = 0; a < 2; ++a) {
-            P.ld[a] = mk_load(mA, 2, a * P.a_lbo); P.ld[a].c0[0] = 64 * a; P.ld[a].d_tm[0] = 128; P.ld[a].d_c2[1] = 64;
-            P.ld[2 + a] = mk_load(mB, 2, P.b_off + a * 8192); P.ld[2 + a].c0[0] = 64 * a; P.ld[2 + a].d_tn[0] = 128; P.ld[2 + a].d_c2[1] = 64;
-          }
-          P.tiles_m = 8; P.tiles_n = 4;
-          P.lim_rows = 1024; P.o_tm = 128 * 512; P.o0 = 512; P.n_valid = 512;
-          P.out_f = h->g(std::string(nets[n]) + "/cnn_fc1/w"); P.atomic = 0;
-          g.host[g.n++] = P;
-        }
-      }
-      if (int rc = push_group(h, v.bwd_groups, g, "fc1_bwd")) return rc;
-    }
-    // ---- conv3 backward: dgrad over the zero-bordered dZ3 (TMA out-of-bound fill) and wgrad (two kernel positions per M tile)
-    {
-      CgGroup g;
-      std::vector<int> tab(5 * CG_MAX_LOADS * 2, 0);
-      for (int tm = 0; tm < 5; ++tm)
-        for (int a = 0; a < 2; ++a) {
-          const int pos = 2 * tm + a;
-          tab[(tm * CG_MAX_LOADS + a) * 2] = pos % 3; tab[(tm * CG_MAX_LOADS + a) * 2 + 1] = pos / 3;
-        }
-      int* dtab = nullptr;
-      if (int rc = valloc(h, &dtab, tab.size())) return rc;
-      B2G_CK(cudaMemcpy(dtab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice));
-      for (int n = 0; n < 2; ++n) {
-        {
-          const int mA = add_maps(v, v.dZ3[n], NB, 4, {64, 4, 4, (uint64_t)B}, {128, 512, 2048}, {64, 6, 6, 3});
-          const int mB = add_maps(v, v.W3n[n], NB, 2, {64, 576}, {128}, {64, 64});
-          if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (conv3 dgrad)");
-          CgProblem P = kmajor(NB, 64, 9, 3, 108);
-          P.nloads = 2;
-          P.ld[0] = mk_load(mA, 4, 0); P.ld[0].d_tm[3] = 3; P.ld[0].d_c1[2] = -1; P.ld[0].d_c2[1] = -1;
-          P.ld[1] = mk_load(mB, 2, P.b_off); P.ld[1].d_c1[1] = 192; P.ld[1].d_c2[1] = 64;
-          P.tiles_m = (B + 2) / 3;
-          P.epi = CG_EPI_DGRAD; P.rows_tile = 108; P.lim_rows = B * 36;
-          P.o_tm = 108 * 64; P.o0 = 64; P.n_valid = 64; P.out_planes = 2;
-          for (int p = 0; p < 2; ++p) P.out_p[p] = v.dZ2[n][p];
-          P.mask = v.H2[n][0]; P.m_tm = 108 * 64; P.m0 = 64;
-          if (v.epi_colsum) { P.colsum = h->g(std::string(nets[n]) + "/cnn2/b"); P.colsum_mask = 63; }
-          g.host[g.n++] = P;
-        }
-        {
-          const int mA = add_maps(v, v.H2[n], NB, 4, {64, 6, 6, (uint64_t)B}, {128, 768, 4608}, {64, 4, 4, 4});
-          const int mB = add_maps(v, v.dZ3[n], NB, 2, {64, (uint64_t)B * 16}, {128}, {64, 64});
-          if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (conv3 wgrad)");
-          CgProblem P = mnmajor(NB, 64, 2, 1, (B + 3) / 4);
-          P.nloads = 3;
-          for (int a = 0; a < 2; ++a) { P.ld[a] = mk_load(mA, 4, a * P.a_lbo); P.ld[a].d_c2[3] = 4; }
-          P.ld[2] = mk_load(mB, 2, P.b_off); P.ld[2].d_c2[1] = 64;
-          P.tm_tab = dtab;
-          P.tiles_m = 5; P.tiles_n = 1;
-          P.splits = std::max(1, std::min(P.chunks, std::max(14, (P.chunks + 15) / 16)));     // <= 16 chunks (64 k-steps) per accumulator chain
-          P.lim_rows = 576; P.o_tm = 128 * 64; P.o0 = 64; P.n_valid = 64;
-          P.out_f = h->g(std::string(nets[n]) + "/cnn3/w"); P.atomic = 1;
-          g.host[g.n++] = P;
-        }
-      }
-      if (int rc = push_group(h, v.bwd_groups, g, "conv3_bwd")) return rc;
-    }
-    // ---- conv2 dgrad: the four output-parity classes of the stride-2 convolution share their A operand (the gradient map
-    // shifted by (-jy, -jx), zero-filled outside), so ONE tile computes all four: B = [W(py,px)] stacked along N
-    // (4 x 32 input channels = 128 accumulator columns, two boxes of 64 rows), one 32-column group per class, each with
-    // its own output offset and row limits (classes with 7 rows / columns mask the 8th).
-    {
-      CgGroup g;
-      for (int n = 0; n < 2; ++n) {
-        const int mA = add_maps(v, v.dZ2[n], NB, 4, {64, 6, 6, (uint64_t)B}, {128, 768, 4608}, {64, 8, 8, 2});
-        const int mB = add_maps(v, v.W2n[n], NB, 2, {64, 512}, {128}, {64, 64}, {}, false);      // two boxes (py) per plane
-        if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (conv2 dgrad)");
-        CgProblem P = kmajor(NB, 128, 4, 2, 128);
-        P.tx_bytes = NB * (128 * 128 + 2 * 64 * 128);
-        P.nloads = 3;
-        P.ld[0] = mk_load(mA, 4, 0); P.ld[0].d_tm[3] = 2; P.ld[0].d_c1[2] = -1; P.ld[0].d_c2[1] = -1;
-        // kernel positions (ky, kx) = (py + 2 jy, px + 2 jx): rows ((2 jy) * 4 + 2 jx) * 32 .. hold (py = 0; px = 0, 1), + 128 rows (py = 1)
-        for (int py = 0; py < 2; ++py) {
-          P.ld[1 + py] = mk_load(mB, 2, P.b_off + py * 64 * 128);
-          P.ld[1 + py].c0[1] = py * 128; P.ld[1 + py].d_c1[1] = 256; P.ld[1 + py].d_c2[1] = 64;
-        }
-        P.tiles_m = (B + 1) / 2;
-        P.epi = CG_EPI_DGRAD; P.rows_tile = 128; P.lim_rows = B * 64;
-        P.d0 = 8; P.d1 = 8;
-        P.o_tm = 2 * 225 * 64; P.o0 = 2 * 64; P.o1 = 2 * 15 * 64; P.o2 = 225 * 64; P.o_base = n * 32;
-        P.m_tm = 2 * 225 * 32; P.m0 = 2 * 32; P.m1 = 2 * 15 * 32; P.m2 = 225 * 32; P.m_base = 0;
-        P.grp_tab = 1;
-        for (int py = 0; py < 2; ++py)
-          for (int px = 0; px < 2; ++px) {
-            const int gg = py * 2 + px;
-            P.grp_off[gg] = (py * 15 + px) * 64; P.grp_moff[gg] = (py * 15 + px) * 32;
-            P.grp_lim0[gg] = (15 - px + 1) / 2; P.grp_lim1[gg] = (15 - py + 1) / 2;
-          }
-        P.n_valid = 128; P.out_planes = 2;
-        for (int p = 0; p < 2; ++p) P.out_p[p] = v.dZ1[p];
-        P.mask = v.H1[n][0];
-        if (v.epi_colsum) { P.colsum = h->g(std::string(nets[n]) + "/cnn1/b"); P.colsum_mask = 31; }       // four parity classes x 32 channels
-        g.host[g.n++] = P;
-      }
-      if (int rc = push_group(h, v.bwd_groups, g, "conv2_dgrad")) return rc;
-    }
-    // ---- conv2 + conv1 wgrad (MN-major, reduction over batch x pixels, split-K with fp32 red.add)
-    {
-      CgGroup g;
-      for (int n = 0; n < 2; ++n) {
-        const int mA = add_maps(v, v.H1[n], NB, 4, {64, 14, 15, (uint64_t)B}, {64, 15 * 64, 225 * 64}, {64, 12, 12, 4}, {1, 2, 2, 1});
-        const int mB = add_maps(v, v.dZ2[n], NB, 2, {64, (uint64_t)B * 36}, {128}, {64, 144});
-        if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (conv2 wgrad)");
-        CgProblem P = mnmajor(NB, 144, 2, 1, (B + 3) / 4);
-        P.nloads = 3;
-        for (int a = 0; a < 2; ++a) { P.ld[a] = mk_load(mA, 4, a * P.a_lbo); P.ld[a].c0[1] = 2 * a; P.ld[a].d_tm[2] = 1; P.ld[a].d_c2[3] = 4; }
-        P.ld[2] = mk_load(mB, 2, P.b_off); P.ld[2].d_c2[1] = 144;
-        P.tiles_m = 4; P.tiles_n = 1;
-        P.splits = std::max(1, std::min(P.chunks, std::max(8, (P.chunks + 7) / 8)));           // <= 8 chunks (72 k-steps) per chain
-        P.lim_rows = 512; P.o_tm = 128 * 64; P.o0 = 64; P.n_valid = 64;
-        P.out_f = h->g(std::string(nets[n]) + "/cnn2/w"); P.atomic = 1;
         g.host[g.n++] = P;
       }
       {
-        const int mA = add_maps(v, v.A1[0], NB, 2, {(uint64_t)K1, (uint64_t)B * 225}, {(uint64_t)K1 * 2}, {64, 64});
-        const int mB = add_maps(v, v.dZ1, NB, 2, {64, (uint64_t)B * 225}, {128}, {64, 64});
-        if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (conv1 wgrad)");
-        CgProblem P = mnmajor(NB, 64, 2, 1, (B * 225 + 63) / 64);
-        P.nloads = 3;
-        // both 64-wide atoms of the M tile are always fetched; an atom beyond K1 (one image channel: K1 = 64) is out of
-        // bounds and arrives as zeros, its output rows are masked by lim_rows
-        for (int a = 0; a < 2; ++a) { P.ld[a] = mk_load(mA, 2, a * P.a_lbo); P.ld[a].c0[0] = 64 * a; P.ld[a].d_tm[0] = 128; P.ld[a].d_c2[1] = 64; }
-        P.ld[2] = mk_load(mB, 2, P.b_off); P.ld[2].d_c2[1] = 64;
-        P.tiles_m = (K1 + 127) / 128; P.tiles_n = 1;
-        P.splits = std::max(1, std::min(P.chunks, std::max(84 / P.tiles_m, (P.chunks + 15) / 16)));
-        P.lim_rows = K1; P.o_tm = 128 * 32; P.o0 = 32; P.n_valid = 64;
-        P.out_f = h->g("model/pi/cnn1/w"); P.f_grp = (long long)(h->g("model/values_fn/cnn1/w") - h->g("model/pi/cnn1/w")); P.atomic = 1;
+        const int mA = add_maps(v, v.H3[n], NB, 2, {1024, (uint64_t)B}, {2048}, {64, 64});
+        const int mB = add_maps(v, v.dZ4[n], NB, 2, {512, (uint64_t)B}, {1024}, {64, 64}, {}, false);     // two B atoms per plane
+        if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (fc1 wgrad)");
+        CgProblem P = mnmajor(NB, 64, 2, 2, (B + 63) / 64);
+        P.nloads = 4;
+        for (int a = 0; a < 2; ++a) {
+          P.ld[a] = mk_load(mA, 2, a * P.a_lbo); P.ld[a].c0[0] = 64 * a; P.ld[a].d_tm[0] = 128; P.ld[a].d_c2[1] = 64;
+          P.ld[2 + a] = mk_load(mB, 2, P.b_off + a * 8192); P.ld[2 + a].c0[0] = 64 * a; P.ld[2 + a].d_tn[0] = 128; P.ld[2 + a].d_c2[1] = 64;
+        }
+        P.tiles_m = 8; P.tiles_n = 4;
+        P.lim_rows = 1024; P.o_tm = 128 * 512; P.o0 = 512; P.n_valid = 512;
+        P.out_f = h->g(std::string(nets[n]) + "/cnn_fc1/w"); P.atomic = 0;
         g.host[g.n++] = P;
       }
-      if (int rc = push_group(h, v.bwd_groups, g, "conv_wgrad")) return rc;
     }
-    // ---- bias gradients from the gradient-map planes
-    {
-      // two launches: [0] the cnn_fc1 biases (need dZ4 only: ready right after heads_dgrad, part of the EARLY all-reduce range),
-      // [1] the conv biases (need every gradient map)
-      for (int part = 0; part < 2; ++part) {
-        std::vector<Colsum2Job> cj;
-        int cstart = 0;
-        auto add_cs = [&](uint16_t* const* pl, float* dst, int rows, int pitch, int col0, int N) {
-          Colsum2Job j{pl[0], pl[1], dst, rows, pitch, col0, N, cstart};
-          const int rows_per_cta = 16 * (256 / (N >> 3));
-          cstart += (rows + rows_per_cta - 1) / rows_per_cta;
-          cj.push_back(j);
-        };
-        for (int n = 0; n < 2; ++n) {
-          if (part == 0) add_cs(v.dZ4[n], h->g(std::string(nets[n]) + "/cnn_fc1/b"), B, 512, 0, 512);
-          else {
-            add_cs(v.dZ1, h->g(std::string(nets[n]) + "/cnn1/b"), B * 225, 64, 32 * n, 32);
-            add_cs(v.dZ2[n], h->g(std::string(nets[n]) + "/cnn2/b"), B * 36, 64, 0, 64);
-            add_cs(v.dZ3[n], h->g(std::string(nets[n]) + "/cnn3/b"), B * 16, 64, 0, 64);
-          }
-        }
-        Colsum2Job* dcj = nullptr;
-        if (int rc = valloc(h, &dcj, cj.size())) return rc;
-        B2G_CK(cudaMemcpy(dcj, cj.data(), cj.size() * sizeof(Colsum2Job), cudaMemcpyHostToDevice));
-        v.colsum_part[part] = dcj; v.n_colsum_part[part] = (int)cj.size(); v.colsum_ctas_part[part] = cstart;
+    if (int rc = push_group(h, v.bwd_groups, g, "fc1_bwd")) return rc;
+  }
+  // ---- conv3 backward: dgrad over the zero-bordered dZ3 (TMA out-of-bound fill) and wgrad (two kernel positions per M tile)
+  {
+    CgGroup g;
+    std::vector<int> tab(5 * CG_MAX_LOADS * 2, 0);
+    for (int tm = 0; tm < 5; ++tm)
+      for (int a = 0; a < 2; ++a) {
+        const int pos = 2 * tm + a;
+        tab[(tm * CG_MAX_LOADS + a) * 2] = pos % 3; tab[(tm * CG_MAX_LOADS + a) * 2 + 1] = pos / 3;
+      }
+    int* dtab = nullptr;
+    if (int rc = valloc(h, &dtab, tab.size())) return rc;
+    B2G_CK(cudaMemcpy(dtab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice));
+    for (int n = 0; n < 2; ++n) {
+      {
+        const int mA = add_maps(v, v.dZ3[n], NB, 4, {64, 4, 4, (uint64_t)B}, {128, 512, 2048}, {64, 6, 6, 3});
+        const int mB = add_maps(v, v.W3n[n], NB, 2, {64, 576}, {128}, {64, 64});
+        if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (conv3 dgrad)");
+        CgProblem P = kmajor(NB, 64, 9, 3, 108);
+        P.nloads = 2;
+        P.ld[0] = mk_load(mA, 4, 0); P.ld[0].d_tm[3] = 3; P.ld[0].d_c1[2] = -1; P.ld[0].d_c2[1] = -1;
+        P.ld[1] = mk_load(mB, 2, P.b_off); P.ld[1].d_c1[1] = 192; P.ld[1].d_c2[1] = 64;
+        P.tiles_m = (B + 2) / 3;
+        P.epi = CG_EPI_DGRAD; P.rows_tile = 108; P.lim_rows = B * 36;
+        P.o_tm = 108 * 64; P.o0 = 64; P.n_valid = 64; P.out_planes = 2;
+        for (int p = 0; p < 2; ++p) P.out_p[p] = v.dZ2[n][p];
+        P.mask = v.H2[n][0]; P.m_tm = 108 * 64; P.m0 = 64;
+        P.colsum = h->g(std::string(nets[n]) + "/cnn2/b"); P.colsum_mask = 63;
+        g.host[g.n++] = P;
+      }
+      {
+        const int mA = add_maps(v, v.H2[n], NB, 4, {64, 6, 6, (uint64_t)B}, {128, 768, 4608}, {64, 4, 4, 4});
+        const int mB = add_maps(v, v.dZ3[n], NB, 2, {64, (uint64_t)B * 16}, {128}, {64, 64});
+        if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (conv3 wgrad)");
+        CgProblem P = mnmajor(NB, 64, 2, 1, (B + 3) / 4);
+        P.nloads = 3;
+        for (int a = 0; a < 2; ++a) { P.ld[a] = mk_load(mA, 4, a * P.a_lbo); P.ld[a].d_c2[3] = 4; }
+        P.ld[2] = mk_load(mB, 2, P.b_off); P.ld[2].d_c2[1] = 64;
+        P.tm_tab = dtab;
+        P.tiles_m = 5; P.tiles_n = 1;
+        P.splits = std::max(1, std::min(P.chunks, std::max(14, (P.chunks + 15) / 16)));     // <= 16 chunks (64 k-steps) per accumulator chain
+        P.lim_rows = 576; P.o_tm = 128 * 64; P.o0 = 64; P.n_valid = 64;
+        P.out_f = h->g(std::string(nets[n]) + "/cnn3/w"); P.atomic = 1;
+        g.host[g.n++] = P;
       }
     }
+    if (int rc = push_group(h, v.bwd_groups, g, "conv3_bwd")) return rc;
+  }
+  // ---- conv2 dgrad: the four output-parity classes of the stride-2 convolution share their A operand (the gradient map
+  // shifted by (-jy, -jx), zero-filled outside), so ONE tile computes all four: B = [W(py,px)] stacked along N
+  // (4 x 32 input channels = 128 accumulator columns, two boxes of 64 rows), one 32-column group per class, each with
+  // its own output offset and row limits (classes with 7 rows / columns mask the 8th).
+  {
+    CgGroup g;
+    for (int n = 0; n < 2; ++n) {
+      const int mA = add_maps(v, v.dZ2[n], NB, 4, {64, 6, 6, (uint64_t)B}, {128, 768, 4608}, {64, 8, 8, 2});
+      const int mB = add_maps(v, v.W2n[n], NB, 2, {64, 512}, {128}, {64, 64}, {}, false);      // two boxes (py) per plane
+      if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (conv2 dgrad)");
+      CgProblem P = kmajor(NB, 128, 4, 2, 128);
+      P.tx_bytes = NB * (128 * 128 + 2 * 64 * 128);
+      P.nloads = 3;
+      P.ld[0] = mk_load(mA, 4, 0); P.ld[0].d_tm[3] = 2; P.ld[0].d_c1[2] = -1; P.ld[0].d_c2[1] = -1;
+      // kernel positions (ky, kx) = (py + 2 jy, px + 2 jx): rows ((2 jy) * 4 + 2 jx) * 32 .. hold (py = 0; px = 0, 1), + 128 rows (py = 1)
+      for (int py = 0; py < 2; ++py) {
+        P.ld[1 + py] = mk_load(mB, 2, P.b_off + py * 64 * 128);
+        P.ld[1 + py].c0[1] = py * 128; P.ld[1 + py].d_c1[1] = 256; P.ld[1 + py].d_c2[1] = 64;
+      }
+      P.tiles_m = (B + 1) / 2;
+      P.epi = CG_EPI_DGRAD; P.rows_tile = 128; P.lim_rows = B * 64;
+      P.d0 = 8; P.d1 = 8;
+      P.o_tm = 2 * 225 * 64; P.o0 = 2 * 64; P.o1 = 2 * 15 * 64; P.o2 = 225 * 64; P.o_base = n * 32;
+      P.m_tm = 2 * 225 * 32; P.m0 = 2 * 32; P.m1 = 2 * 15 * 32; P.m2 = 225 * 32; P.m_base = 0;
+      P.grp_tab = 1;
+      for (int py = 0; py < 2; ++py)
+        for (int px = 0; px < 2; ++px) {
+          const int gg = py * 2 + px;
+          P.grp_off[gg] = (py * 15 + px) * 64; P.grp_moff[gg] = (py * 15 + px) * 32;
+          P.grp_lim0[gg] = (15 - px + 1) / 2; P.grp_lim1[gg] = (15 - py + 1) / 2;
+        }
+      P.n_valid = 128; P.out_planes = 2;
+      for (int p = 0; p < 2; ++p) P.out_p[p] = v.dZ1[p];
+      P.mask = v.H1[n][0];
+      P.colsum = h->g(std::string(nets[n]) + "/cnn1/b"); P.colsum_mask = 31;       // four parity classes x 32 channels
+      g.host[g.n++] = P;
+    }
+    if (int rc = push_group(h, v.bwd_groups, g, "conv2_dgrad")) return rc;
+  }
+  // ---- conv2 + conv1 wgrad (MN-major, reduction over batch x pixels, split-K with fp32 red.add)
+  {
+    CgGroup g;
+    for (int n = 0; n < 2; ++n) {
+      const int mA = add_maps(v, v.H1[n], NB, 4, {64, 14, 15, (uint64_t)B}, {64, 15 * 64, 225 * 64}, {64, 12, 12, 4}, {1, 2, 2, 1});
+      const int mB = add_maps(v, v.dZ2[n], NB, 2, {64, (uint64_t)B * 36}, {128}, {64, 144});
+      if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (conv2 wgrad)");
+      CgProblem P = mnmajor(NB, 144, 2, 1, (B + 3) / 4);
+      P.nloads = 3;
+      for (int a = 0; a < 2; ++a) { P.ld[a] = mk_load(mA, 4, a * P.a_lbo); P.ld[a].c0[1] = 2 * a; P.ld[a].d_tm[2] = 1; P.ld[a].d_c2[3] = 4; }
+      P.ld[2] = mk_load(mB, 2, P.b_off); P.ld[2].d_c2[1] = 144;
+      P.tiles_m = 4; P.tiles_n = 1;
+      P.splits = std::max(1, std::min(P.chunks, std::max(8, (P.chunks + 7) / 8)));           // <= 8 chunks (72 k-steps) per chain
+      P.lim_rows = 512; P.o_tm = 128 * 64; P.o0 = 64; P.n_valid = 64;
+      P.out_f = h->g(std::string(nets[n]) + "/cnn2/w"); P.atomic = 1;
+      g.host[g.n++] = P;
+    }
+    {
+      const int mA = add_maps(v, v.A1[0], NB, 2, {(uint64_t)K1, (uint64_t)B * 225}, {(uint64_t)K1 * 2}, {64, 64});
+      const int mB = add_maps(v, v.dZ1, NB, 2, {64, (uint64_t)B * 225}, {128}, {64, 64});
+      if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (conv1 wgrad)");
+      CgProblem P = mnmajor(NB, 64, 2, 1, (B * 225 + 63) / 64);
+      P.nloads = 3;
+      // both 64-wide atoms of the M tile are always fetched; an atom beyond K1 (one image channel: K1 = 64) is out of
+      // bounds and arrives as zeros, its output rows are masked by lim_rows
+      for (int a = 0; a < 2; ++a) { P.ld[a] = mk_load(mA, 2, a * P.a_lbo); P.ld[a].c0[0] = 64 * a; P.ld[a].d_tm[0] = 128; P.ld[a].d_c2[1] = 64; }
+      P.ld[2] = mk_load(mB, 2, P.b_off); P.ld[2].d_c2[1] = 64;
+      P.tiles_m = (K1 + 127) / 128; P.tiles_n = 1;
+      P.splits = std::max(1, std::min(P.chunks, std::max(84 / P.tiles_m, (P.chunks + 15) / 16)));
+      P.lim_rows = K1; P.o_tm = 128 * 32; P.o0 = 32; P.n_valid = 64;
+      P.out_f = h->g("model/pi/cnn1/w"); P.f_grp = (long long)(h->g("model/values_fn/cnn1/w") - h->g("model/pi/cnn1/w")); P.atomic = 1;
+      g.host[g.n++] = P;
+    }
+    if (int rc = push_group(h, v.bwd_groups, g, "conv_wgrad")) return rc;
   }
   // ================================================================================ fused launches
   // One persistent launch for the forward chain (conv1 -> conv2 -> conv3 -> cnn_fc1 -> head fc0) and one for the backward chain up
   // to the conv2 dgrad: a launch boundary costs a sizeable share of a layer (launch, first-fetch latency, the last tile's
   // epilogue and the ragged last wave), a counter wait between dependent TILES costs nothing once the pipeline is full.  The stage ring is re-partitioned per problem (the conv2 wgrad needs 108 KB stages, the rest 64 - 72 KB).
+  int n_ctr = 0;
   {
-    const char* ef = getenv("B2G_FUSE");
-    v.fuse = !(ef && ef[0] == '0');
-  }
-  if (v.fuse) {
-    int n_ctr = 0;
-    {
-      std::vector<const CgGroup*> parts;
-      for (auto& g : v.fwd) parts.push_back(&g);                 // conv1 (obs, next), conv2 x3, conv3 x3, fc1 x3, fc0 x3
-      std::vector<Wire> w;
-      for (int n = 0; n < 3; ++n) {
-        w.push_back({1, n, 0, n < 2 ? 0 : 1, 3 * 225, 128, 0});  // conv2 tile: 3 samples of H1 (225 rows each; conv1 tiles are 128 rows)
-        w.push_back({2, n, 1, n, 8 * 36, 108, 0});               // conv3 tile: 8 samples of H2 (36 rows each; conv2 tiles are 3 samples)
-        w.push_back({3, n, 2, n, 128 * 16, 128, 0});             // fc1 tile: 128 samples of H3 (16 rows each)
-        w.push_back({4, n, 3, n, 128, 128, 0});                  // fc0 tile: 128 feature rows (all 8 column tiles of them)
-      }
-      if (int rc = fuse_groups(h, parts, w, "fwd_fused", v.fwd_fused, n_ctr)) return rc;
+    std::vector<const CgGroup*> parts;
+    for (auto& g : v.fwd) parts.push_back(&g);                 // conv1 (obs, next), conv2 x3, conv3 x3, fc1 x3, fc0 x3
+    std::vector<Wire> w;
+    for (int n = 0; n < 3; ++n) {
+      w.push_back({1, n, 0, n < 2 ? 0 : 1, 3 * 225, 128, 0});  // conv2 tile: 3 samples of H1 (225 rows each; conv1 tiles are 128 rows)
+      w.push_back({2, n, 1, n, 8 * 36, 108, 0});               // conv3 tile: 8 samples of H2 (36 rows each; conv2 tiles are 3 samples)
+      w.push_back({3, n, 2, n, 128 * 16, 128, 0});             // fc1 tile: 128 samples of H3 (16 rows each)
+      w.push_back({4, n, 3, n, 128, 128, 0});                  // fc0 tile: 128 feature rows (all 8 column tiles of them)
     }
-    if (v.bwd) {
-      std::vector<const CgGroup*> parts;
-      for (auto& g : v.bwd_groups) parts.push_back(&g);          // heads_dgrad, fc1_bwd, conv3_bwd, conv2_dgrad, conv_wgrad
-      std::vector<Wire> w;
-      for (int n = 0; n < 2; ++n) {
-        w.push_back({1, 2 * n, 0, n, 128, 128, 0});              // fc1 dgrad tile: 128 rows of dZ4
-        w.push_back({1, 2 * n + 1, 0, n, 64, 128, 1});           // fc1 wgrad chunk: 64 rows of dZ4
-        w.push_back({2, 2 * n, 1, 2 * n, 3, 128, 0});            // conv3 dgrad tile: 3 samples of dZ3 (fc1 dgrad rows are samples)
-        w.push_back({2, 2 * n + 1, 1, 2 * n, 4, 128, 1});        // conv3 wgrad chunk: 4 samples of dZ3
-        w.push_back({3, n, 2, 2 * n, 72, 108, 0});               // conv2 dgrad tile: 2 samples of dZ2 (36 rows each; conv3 dgrad tiles are 3 samples)
-        w.push_back({4, n, 2, 2 * n, 144, 108, 1});              // conv2 wgrad chunk: 4 samples of dZ2
-      }
-      // conv1 wgrad chunk: 64 rows of dZ1 [B*225][pi | vf]; a conv2 dgrad tile (of EITHER net: both must be done) covers 2 samples = 450 rows
-      w.push_back({4, 2, 3, 0, 64, 450, 1});
-      w.push_back({4, 2, 3, 1, 64, 450, 1});
-      if (int rc = fuse_groups(h, parts, w, "bwd_fused", v.bwd_fused, n_ctr)) return rc;
-      // data parallel: the same chain cut after cnn_fc1, where the gradients of [cnn_fc1 .. end] (84 % of the bytes) are final
-      // and their all-reduce starts on the side stream underneath the conv backward
-      std::vector<const CgGroup*> pa(parts.begin(), parts.begin() + 2), pb(parts.begin() + 2, parts.end());     // pb: conv3_bwd, conv2_dgrad, conv_wgrad
-      std::vector<Wire> wa, wb;
-      for (int n = 0; n < 2; ++n) {
-        wa.push_back({1, 2 * n, 0, n, 128, 128, 0});
-        wa.push_back({1, 2 * n + 1, 0, n, 64, 128, 1});
-        wb.push_back({1, n, 0, 2 * n, 72, 108, 0});
-        wb.push_back({2, n, 0, 2 * n, 144, 108, 1});
-      }
-      wb.push_back({2, 2, 1, 0, 64, 450, 1});
-      wb.push_back({2, 2, 1, 1, 64, 450, 1});
-      if (int rc = fuse_groups(h, pa, wa, "bwd_fused_fc", v.bwd_fused, n_ctr)) return rc;
-      if (int rc = fuse_groups(h, pb, wb, "bwd_fused_conv", v.bwd_fused, n_ctr)) return rc;
-    }
-    if (int rc = valloc(h, &v.dep_ctr, (size_t)n_ctr)) return rc;
-    v.n_dep_ctr = n_ctr;
-    bind_counters(v.fwd_fused, v.dep_ctr);
-    bind_counters(v.bwd_fused, v.dep_ctr);
+    if (int rc = fuse_groups(h, parts, w, "fwd_fused", v.fwd_fused, n_ctr)) return rc;
   }
+  {
+    std::vector<const CgGroup*> parts;
+    for (auto& g : v.bwd_groups) parts.push_back(&g);          // heads_dgrad, fc1_bwd, conv3_bwd, conv2_dgrad, conv_wgrad
+    std::vector<Wire> w;
+    for (int n = 0; n < 2; ++n) {
+      w.push_back({1, 2 * n, 0, n, 128, 128, 0});              // fc1 dgrad tile: 128 rows of dZ4
+      w.push_back({1, 2 * n + 1, 0, n, 64, 128, 1});           // fc1 wgrad chunk: 64 rows of dZ4
+      w.push_back({2, 2 * n, 1, 2 * n, 3, 128, 0});            // conv3 dgrad tile: 3 samples of dZ3 (fc1 dgrad rows are samples)
+      w.push_back({2, 2 * n + 1, 1, 2 * n, 4, 128, 1});        // conv3 wgrad chunk: 4 samples of dZ3
+      w.push_back({3, n, 2, 2 * n, 72, 108, 0});               // conv2 dgrad tile: 2 samples of dZ2 (36 rows each; conv3 dgrad tiles are 3 samples)
+      w.push_back({4, n, 2, 2 * n, 144, 108, 1});              // conv2 wgrad chunk: 4 samples of dZ2
+    }
+    // conv1 wgrad chunk: 64 rows of dZ1 [B*225][pi | vf]; a conv2 dgrad tile (of EITHER net: both must be done) covers 2 samples = 450 rows
+    w.push_back({4, 2, 3, 0, 64, 450, 1});
+    w.push_back({4, 2, 3, 1, 64, 450, 1});
+    if (int rc = fuse_groups(h, parts, w, "bwd_fused", v.bwd_fused, n_ctr)) return rc;
+    // data parallel: the same chain cut after cnn_fc1, where the gradients of [cnn_fc1 .. end] (84 % of the bytes) are final
+    // and their all-reduce starts on the side stream underneath the conv backward
+    std::vector<const CgGroup*> pa(parts.begin(), parts.begin() + 2), pb(parts.begin() + 2, parts.end());     // pb: conv3_bwd, conv2_dgrad, conv_wgrad
+    std::vector<Wire> wa, wb;
+    for (int n = 0; n < 2; ++n) {
+      wa.push_back({1, 2 * n, 0, n, 128, 128, 0});
+      wa.push_back({1, 2 * n + 1, 0, n, 64, 128, 1});
+      wb.push_back({1, n, 0, 2 * n, 72, 108, 0});
+      wb.push_back({2, n, 0, 2 * n, 144, 108, 1});
+    }
+    wb.push_back({2, 2, 1, 0, 64, 450, 1});
+    wb.push_back({2, 2, 1, 1, 64, 450, 1});
+    if (int rc = fuse_groups(h, pa, wa, "bwd_fused_fc", v.bwd_fused, n_ctr)) return rc;
+    if (int rc = fuse_groups(h, pb, wb, "bwd_fused_conv", v.bwd_fused, n_ctr)) return rc;
+  }
+  if (int rc = valloc(h, &v.dep_ctr, (size_t)n_ctr)) return rc;
+  v.n_dep_ctr = n_ctr;
+  bind_counters(v.fwd_fused, v.dep_ctr);
+  bind_counters(v.bwd_fused, v.dep_ctr);
   if (int rc = valloc(h, &v.d_maps, v.maps.size())) return rc;
   B2G_CK(cudaMemcpyAsync(v.d_maps, v.maps.data(), v.maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice, h->stream));
   B2G_CK(cudaStreamSynchronize(h->stream));
@@ -944,10 +860,8 @@ int v2_gather(b2g_sac* h, const GatherArgs& ga, cudaStream_t s) {
   V2State& v = h->v2;
   Gather2Args a{};
   a.g = ga;
-  for (int w = 0; w < 2; ++w) {
+  for (int w = 0; w < 2; ++w)
     for (int p = 0; p < 3; ++p) a.a1[w][p] = v.A1[w][p];
-    a.xp[w][0] = v.bwd ? nullptr : h->xp[w][0]; a.xp[w][1] = v.bwd ? nullptr : h->xp[w][1];
-  }
   for (int n = 0; n < 3; ++n) for (int p = 0; p < 3; ++p) a.fp[n][p] = v.F[n][p];
   a.KF = v.KF; a.Ci = h->Cimg; a.OH = h->H1; a.OW = h->W1;
   const size_t smem = (size_t)3 * h->Hi * (h->Wi * h->Cimg + 8) * sizeof(uint16_t);
@@ -957,14 +871,6 @@ int v2_gather(b2g_sac* h, const GatherArgs& ga, cudaStream_t s) {
     attr = smem;
   }
   gather2_kernel<<<dim3(ga.B, ga.next_obs ? 2 : 1), 512, smem, s>>>(a);
-  return 0;
-}
-
-int v2_colsum(b2g_sac* h, cudaStream_t s, int part) {
-  V2State& v = h->v2;
-  if (v.epi_colsum) return 0;
-  if (v.colsum_ctas_part[part] > 0)
-    colsum2_kernel<<<v.colsum_ctas_part[part], 256, 0, s>>>((const Colsum2Job*)v.colsum_part[part], v.n_colsum_part[part]);
   return 0;
 }
 

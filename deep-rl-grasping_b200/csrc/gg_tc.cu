@@ -18,9 +18,6 @@
 // Shared memory: 3 x 48 KiB ring, 32 KiB accumulator tile, 32 KiB store staging.
 #include <cuda_bf16.h>
 
-#include <algorithm>
-#include <vector>
-
 #include "common.cuh"
 #include "wgmma.cuh"
 
@@ -51,9 +48,6 @@ struct DescPack {
   GemmDesc d[GG_TC_MAX_DESCS];
   int n;
   int total_tiles;
-  long long* trace;   // bring-up: per-tile clock64 stamps of CTA 0 (nullptr in production)
-  const int* ranges;  // [grid + 1] contiguous, cost-balanced tile range per CTA (nullptr: round-robin over the grid)
-  unsigned* sync_ctr; // fused multi-layer launch: epilogue warps that finished a tile (zeroed before the launch; nullptr: none)
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -172,8 +166,7 @@ __device__ __forceinline__ TileInfo tile_info(const DescPack& pk, int tile) {
 }
 
 template <bool a_rvec, bool b_rvec, bool planes>
-__global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const __grid_constant__ DescPack pk, int x3_in) {
-  int x3 = x3_in;
+__global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const __grid_constant__ DescPack pk, int x3) {
   constexpr int NPROD = Roles<planes>::NPROD, MMA_WARP = Roles<planes>::MMA_WARP, NEPI = Roles<planes>::NEPI;
   constexpr int EPI_COLS = Roles<planes>::EPI_COLS;
   extern __shared__ uint8_t smem_raw[];
@@ -182,8 +175,6 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
   __shared__ __align__(16) float s_bias[TN];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const bool dbg_noload = x3 & 0x100, dbg_nomma = x3 & 0x200, dbg_nostore = x3 & 0x400, dbg_nosplit = x3 & 0x800;
-  x3 &= 1;
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(smem_u32(&bar_full[s]), NPROD);
@@ -195,12 +186,8 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
   const uint32_t ring = (smem_u32(smem_raw) + 1023u) & ~1023u;
   pdl_trigger();      // the next kernel on the stream may begin its own prologue now
   pdl_wait();         // everything above overlapped the predecessor; its results are visible from here on
-  // Tile schedule.  With host-built ranges every CTA owns a CONTIGUOUS run of tiles whose summed cost (r-chunks + a
-  // fixed per-tile term) is balanced: consecutive tiles then share their problem and column block, so the per-problem
-  // state (pinned descriptor fields, staged column tables and their barrier pair) is refreshed a few times per CTA
-  // instead of once per tile, and neighbouring rows stay in the same SM's L1/L2 slice.
-  int t_begin = blockIdx.x, t_end = pk.total_tiles, t_step = gridDim.x;
-  if (pk.ranges) { t_begin = pk.ranges[blockIdx.x]; t_end = pk.ranges[blockIdx.x + 1]; t_step = 1; }
+  // Tile schedule: round-robin over the grid
+  const int t_begin = blockIdx.x, t_end = pk.total_tiles, t_step = gridDim.x;
 
   if (planes && warp < MMA_WARP) {
     // =========================================================================== producers (BF16 planes, cp.async)
@@ -252,33 +239,10 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
       return t;
     };
     TState cur = fetch(t_begin);
-    int tcount = 0;
     int pin_p = -1, pflags = 0;
-    // Fused multi-layer launch: a problem of layer L may read its operands only after every tile of the layers before it
-    // has been stored.  Tiles are numbered layer by layer and every CTA walks its tiles in increasing order, so "all
-    // tiles below need_done are complete" is a count: epilogue warps bump one counter per finished tile, producers of a
-    // later layer wait for need_done * (epilogue warps) -- a grid barrier without leaving the kernel.  No cycle is
-    // possible (a tile only ever waits for lower-numbered tiles, all CTAs are co-resident: grid <= #SMs, 1 CTA / SM).
-    unsigned seen_done = 0, pneed = 0;
-    auto layer_wait = [&]() {
-      if (pneed > seen_done) {
-        if (lane == 0) {
-          unsigned v = 0, spins = 0;
-          while (true) {
-            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(pk.sync_ctr) : "memory");
-            if (v >= pneed) break;
-            __nanosleep(40);
-            if (++spins > (1u << 22)) asm volatile("trap;");   // a lost signal must fail loudly, not hang the GPU
-          }
-          seen_done = v;
-        }
-        seen_done = __shfl_sync(0xffffffffu, seen_done, 0);
-      }
-    };
     const uint16_t* pA_hi = nullptr; const uint16_t* pA_lo = nullptr; const uint16_t* pB_hi = nullptr; const uint16_t* pB_lo = nullptr;
     const int* tabA = nullptr; const int* tabB_k = nullptr; const int* tabB_mn = nullptr;
-    for (int tile = t_begin; tile < t_end; tile += t_step, ++tcount) {
-      if (pk.trace && blockIdx.x == 0 && tid == 0 && tcount < 64) pk.trace[tcount * 8 + 0] = clock64();
+    for (int tile = t_begin; tile < t_end; tile += t_step) {
       const TState nxt = fetch(tile + t_step);
       const TileInfo ti = cur.ti;
       if (ti.p != pin_p) {
@@ -286,10 +250,8 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
         pflags = pin(dd.flags);
         pA_hi = pin(dd.A_hi); pA_lo = pin(dd.A_lo); pB_hi = pin(dd.B_hi); pB_lo = pin(dd.B_lo);
         tabA = pin(dd.aR); tabB_mn = pin(dd.bR); tabB_k = pin(dd.bR_p ? dd.bR_p : dd.bR);
-        pneed = pk.sync_ctr ? (unsigned)dd.need_done * (unsigned)(NEPI / 32) : 0u;
         pin_p = ti.p;
       }
-      if (ti.nchunks > 0) layer_wait();
       if (ti.nchunks > 0 && (pflags & GG_MN_MAJOR)) {
         // ---- wgrad: D[k, n] = sum_m act[m -> k] * dZ[m, n]; both operands are contiguous along their M / N
         // index for a fixed reduction index m, so tiles are MN-major: row (r = m) x 16-byte groups along k / n.
@@ -387,7 +349,6 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
           if (ch + 4 < ti.nchunks) { ta3 = tabA[r0a + 4 * TK]; tb3 = tabB[r0 + 4 * TK]; }
         }
       }
-      if (pk.trace && blockIdx.x == 0 && tid == 0 && tcount < 64) pk.trace[tcount * 8 + 1] = clock64();
       cur = nxt;
     }
     asm volatile("cp.async.wait_all;" ::: "memory");
@@ -460,8 +421,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
         for (int i = 0; i < 4; ++i)
 #pragma unroll
           for (int j = 0; j < 8; ++j) xa[i][j] = xb[i][j] = 0.f;
-        if (dbg_noload) {
-        } else if (nr == 8) {
+        if (nr == 8) {
           // ---- fast path: full 8-wide r group, straight-line independent loads
           if (a_rvec) {
 #pragma unroll
@@ -539,7 +499,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
         }
         // ---------------------------------------------------------------- ring slot free?  then split + store
         if (gc >= STAGES) mbar_wait(smem_u32(&bar_empty[s]), ((gc / STAGES) - 1) & 1);
-        if (a_thread && !dbg_nosplit) {
+        if (a_thread) {
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             if (a_rvec && i >= 2) break;
@@ -550,7 +510,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
             if (x3) st_shared16(sA_lo + o, lo);
           }
         }
-        if (b_thread && !dbg_nosplit) {
+        if (b_thread) {
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             if (b_rvec && i >= 1) break;
@@ -591,7 +551,6 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
     int pinned_p = -1, dflags = 0, dN = 0;
     float* dC = nullptr; uint16_t* dChi = nullptr; uint16_t* dClo = nullptr; const float* dmask = nullptr;
     const uint32_t stg = ring + STAGES * STAGE_BYTES + (uint32_t)ew * (32 * EPI_COLS * 4);
-    uint32_t it = 0;
     int staged_n0 = -1, st_col = -2;               // which (column tables, column block) the staged copies belong to
     // Everything a tile's epilogue needs from global memory besides the mask -- tile coordinates, this lane's row
     // offsets (cM / kM), this thread's column-table entry (cN / kN / bias) -- is fetched ONE TILE AHEAD and only
@@ -637,10 +596,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
       const ENext cur = nxt;
       nxt = prefetch(tile + t_step);
       const TileInfo ti = cur.ti;
-      if (ti.nchunks == 0) {
-        if (pk.sync_ctr && lane == 0) atomicAdd(pk.sync_ctr, 1u);   // empty split-R slices still count as finished tiles
-        continue;
-      }
+      if (ti.nchunks == 0) continue;
       const int cm = cur.cm, km = cur.km_same ? cur.cm : cur.km;
       const bool m_ok = cur.ok;
       const GemmDesc& d = pk.d[ti.p];
@@ -665,8 +621,6 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
       const int ecols = (NEPI == 256 && ti.un <= 32) ? 16 : EPI_COLS;
       const int col0 = (ew >> 2) * ecols;            // first accumulator column of this warp
       const int lpr_log = ecols == 16 ? 2 : (EPI_COLS == 64 ? 4 : 3), LPR = 1 << lpr_log, RPI = 32 >> lpr_log;
-      const bool tr = pk.trace && blockIdx.x == 0 && ew == 0 && lane == 0 && it < 64;
-      if (tr) pk.trace[it * 8 + 7] = clock64();
       const bool fastp = (dflags & GG_CN_AFFINE4) && (ti.n0 + ti.un <= dN);
       const int ncols_w = max(0, min(ecols, ti.un - col0));        // warp-uniform, multiple of 16
       // ReLU-mask values of the first store batch: their addresses depend only on the tables, so the loads are issued
@@ -674,7 +628,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
       float4 mk0[4];
       const int pc = lane & (LPR - 1), psub = lane >> lpr_log;
       const bool pact = pc < (ncols_w >> 2);
-      const bool early_mask = planes && fastp && (dflags & GG_EPI_MASK) && ncols_w > 0 && !dbg_nostore;   // (register budget: planes kernel only)
+      const bool early_mask = planes && fastp && (dflags & GG_EPI_MASK) && ncols_w > 0;   // (register budget: planes kernel only)
       {
         const int kn = (early_mask && pact) ? s_kn[col0 + 4 * pc] : 0;
 #pragma unroll
@@ -700,11 +654,9 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
           const uint32_t sA_hi = ring + s * STAGE_BYTES, sA_lo = sA_hi + A_BYTES;
           const uint32_t sB_hi = sA_lo + A_BYTES, sB_lo = sB_hi + B_BYTES;
           wg_arrive();
-          if (!dbg_nomma) {
-            if (mnm) mma_chunk<64, 1, MB>(acc, sA_hi, sA_lo, sB_hi, sB_lo, m_first, x3);
-            else if (ti.un <= 32) mma_chunk<32, 0, MB>(acc, sA_hi, sA_lo, sB_hi, sB_lo, m_first, x3);
-            else mma_chunk<64, 0, MB>(acc, sA_hi, sA_lo, sB_hi, sB_lo, m_first, x3);
-          }
+          if (mnm) mma_chunk<64, 1, MB>(acc, sA_hi, sA_lo, sB_hi, sB_lo, m_first, x3);
+          else if (ti.un <= 32) mma_chunk<32, 0, MB>(acc, sA_hi, sA_lo, sB_hi, sB_lo, m_first, x3);
+          else mma_chunk<64, 0, MB>(acc, sA_hi, sA_lo, sB_hi, sB_lo, m_first, x3);
           wg_commit();
           wg_wait<0>();
           __syncwarp();
@@ -725,7 +677,6 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
             }
         asm volatile("bar.sync 3, %0;" ::"n"(NEPI));
       }
-      if (tr) pk.trace[it * 8 + 4] = clock64();
 #pragma unroll 1
       for (int cb = col0; cb < col0 + ncols_w; cb += 16) {
         uint32_t v[16];
@@ -737,7 +688,6 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
             asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v[4 * g]), "=r"(v[4 * g + 1]), "=r"(v[4 * g + 2]), "=r"(v[4 * g + 3]) : "r"(a));
           }
         }
-        if (dbg_nostore) continue;
         if (fastp) {
           // phase A: accumulator row -> (+bias, ReLU) -> this warp's staging rows (16-byte chunks XOR-swizzled by row)
 #pragma unroll
@@ -772,8 +722,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
           }
         }
       }
-      if (tr) pk.trace[it * 8 + 5] = clock64();
-      if (fastp && !dbg_nostore && ncols_w > 0) {
+      if (fastp && ncols_w > 0) {
         __syncwarp();
         const int c = lane & (LPR - 1), sub = lane >> lpr_log;
         const bool act = c < (ncols_w >> 2);
@@ -822,13 +771,6 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
         }
         __syncwarp();      // staging rows are reused by the next tile
       }
-      if (pk.sync_ctr) {          // this warp's stores of the tile are visible device-wide before the tile counts as done
-        __threadfence();
-        __syncwarp();
-        if (lane == 0) atomicAdd(pk.sync_ctr, 1u);
-      }
-      if (tr) pk.trace[it * 8 + 6] = clock64();
-      ++it;
     }
   }
 }
@@ -848,55 +790,15 @@ cudaError_t launch_mode(const DescPack& pk, int x3, int num_sms, cudaStream_t s)
 
 int gg_tc_smem_bytes() { return SMEM_BYTES; }
 
-// Cost-balanced contiguous tile ranges (mirrors tile_info: tiles of a problem are split-major).  Tile cost = its r-chunk
-// count + a fixed term for the per-tile handshakes and the epilogue.
-std::vector<int> gg_tc_ranges(const GemmDesc* descs, int ndesc, int total_tiles, int grid) {
-  std::vector<float> cost((size_t)total_tiles, 0.f);
-  const float fixed = 3.0f;
-  for (int p = 0; p < ndesc; ++p) {
-    const GemmDesc& d = descs[p];
-    const int per = d.tiles_m * d.tiles_n;
-    const int chunk_r = (((d.R + d.splitR - 1) / d.splitR) + TK - 1) / TK * TK;
-    for (int t = 0; t < d.tile_count; ++t) {
-      const int split = t / per;
-      const int rb = split * chunk_r, re = std::min(d.R, rb + chunk_r);
-      const int nch = re > rb ? (re - rb + TK - 1) / TK : 0;
-      cost[(size_t)d.tile_start + t] = nch > 0 ? nch + fixed : 0.05f;
-    }
-  }
-  double total = 0;
-  for (float c : cost) total += c;
-  std::vector<int> r((size_t)grid + 1, total_tiles);
-  r[0] = 0;
-  double acc = 0;
-  int t = 0;
-  for (int c = 1; c < grid; ++c) {
-    const double target = total * c / grid;
-    // CTA c-1 takes tiles while its share is not exceeded; it gets at least one, and one is left for every later CTA
-    while (t < total_tiles - (grid - c) && (t < r[c - 1] + 1 || acc + 0.5 * cost[t] <= target)) acc += cost[t++];
-    r[c] = t;
-  }
-  r[grid] = total_tiles;
-  return r;
-}
-
 // All problems of one launch share the operand-contiguity mode (flags & (GG_A_RVEC | GG_B_RVEC)).
 // host_descs: the group's descriptors (at most GG_TC_MAX_DESCS), passed as a __grid_constant__ pack.
-long long* g_tc_trace = nullptr;   // set by sac.cu for one traced launch
-
-cudaError_t gg_tc_launch(const GemmDesc* host_descs, int ndesc, int total_tiles, int mode_flags, int x3, int num_sms,
-                         cudaStream_t s, const int* dev_ranges, int ranges_grid, unsigned* sync_ctr) {
+cudaError_t gg_tc_launch(const GemmDesc* host_descs, int ndesc, int total_tiles, int mode_flags, int x3, int num_sms, cudaStream_t s) {
   if (total_tiles <= 0) return cudaSuccess;
   if (ndesc > GG_TC_MAX_DESCS) return cudaErrorInvalidValue;
   DescPack pk;
   for (int i = 0; i < ndesc; ++i) pk.d[i] = host_descs[i];
   pk.n = ndesc;
   pk.total_tiles = total_tiles;
-  pk.trace = g_tc_trace;
-  const int grid = total_tiles < num_sms ? total_tiles : num_sms;
-  pk.ranges = (dev_ranges && ranges_grid == grid) ? dev_ranges : nullptr;   // built for exactly this grid size
-  pk.sync_ctr = sync_ctr;
-  if (sync_ctr && (!(mode_flags & GG_PLANES) || grid > num_sms)) return cudaErrorInvalidValue;   // layer sync: planes kernel, co-resident grid
   const bool ar = mode_flags & GG_A_RVEC, br = mode_flags & GG_B_RVEC;
   if (mode_flags & GG_PLANES) return launch_mode<true, true, true>(pk, x3, num_sms, s);
   if (ar && br) return launch_mode<true, true, false>(pk, x3, num_sms, s);

@@ -8,9 +8,11 @@
 //   batch   : x_obs/x_next [B,H,W,C] (normalised, /255), h1/h2/h3 per network, F rows [B,FS]
 //             (512 CNN features | direct feature | replay action | zero pad), gradient maps with
 //             zero borders (dZ3p, dZ2p) so the dgrad gathers need no bounds logic
-// One gradient step = prep -> gather -> zero G -> grouped gather-GEMM launches (forward) -> tail
-// -> grouped gather-GEMM launches (backward) -> [NCCL all-reduce of G] -> optim; captured once in
-// a CUDA graph and replayed.
+// One gradient step = prep -> gather -> zero G -> forward contractions -> tail -> backward contractions
+// -> [all-reduce of G] -> optim; captured once in a CUDA graph and replayed.  The 64x64 CNN policy in
+// bf16x3 runs its contractions on engine v2 (engine_v2.cu: one fused forward and one fused backward
+// launch); every other configuration, and policy inference, runs them as grouped launches of the
+// round-1 engines (gg_tc.cu, gg_simt.cu).
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <math.h>
@@ -268,18 +270,6 @@ int finalize_group(b2g_sac* h, GemmGroup& g) {
     g.flops += 2.0 * d.M * d.N * d.R;
   }
   g.total_tiles = start;
-  if (g.layer_sync) {       // a layer's problems wait for every tile of the layers before it
-    std::map<int, int> first;
-    for (auto& d : g.host) { auto it = first.find(d.layer); if (it == first.end() || d.tile_start < it->second) first[d.layer] = d.tile_start; }
-    for (auto& d : g.host) d.need_done = d.layer > 0 ? first[d.layer] : 0;
-  }
-  if (g.tc && h->tc_ranges && start > 0 && !g.layer_sync) {     // contiguous cost-balanced tile schedule of the wgmma engine
-    g.ranges_grid = std::min(start, h->num_sms);
-    const std::vector<int> rg = gg_tc_ranges(g.host.data(), (int)g.host.size(), start, g.ranges_grid);
-    if (int rc = dalloc(h, &g.dev_ranges, rg.size(), false)) return rc;
-    CK(cudaMemcpyAsync(g.dev_ranges, rg.data(), rg.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-  }
   if (int rc = dalloc(h, &g.dev, g.host.size(), false)) return rc;
   CK(cudaMemcpyAsync(g.dev, g.host.data(), g.host.size() * sizeof(GemmDesc), cudaMemcpyHostToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));
@@ -343,17 +333,6 @@ int build_groups(b2g_sac* h) {
         if (int rc = upload_table(h, iota_tab(Ns[l], Rs[l]), &wT_n[l])) return rc;
       }
     }
-    // dZ row tables in the zero-bordered layouts
-    std::vector<int> z2row(B * H2 * W2), z3row(B * H3 * W3);
-    for (int b = 0; b < B; ++b) {
-      for (int y = 0; y < H2; ++y)
-        for (int x = 0; x < W2; ++x) z2row[(b * H2 + y) * W2 + x] = ((b * P2h + y + 1) * P2w + x + 1) * 64;
-      for (int y = 0; y < H3; ++y)
-        for (int x = 0; x < W3; ++x) z3row[(b * H3 + y) * W3 + x] = ((b * P3h + y + 2) * P3w + x + 2) * 64;
-    }
-    TAB(dz2row, z2row);
-    TAB(dz3row, z3row);
-
     // ================= forward groups
     const char* cname[3] = {"/cnn1", "/cnn2", "/cnn3"};
     for (int l = 0; l < 3; ++l) {
@@ -369,7 +348,7 @@ int build_groups(b2g_sac* h) {
         if (h->use_planes) {
           uint16_t* const* ip = l == 0 ? h->xp[n == 2 ? 1 : 0] : (l == 1 ? h->h1p[n] : h->h2p[n]);
           uint16_t* const* op = l == 0 ? h->h1p[n] : (l == 1 ? h->h2p[n] : h->h3p[n]);
-          d.flags |= GG_PLANES | GG_B_RVEC | ((l == 0 && (c.Ci & 1)) ? GG_A_ALIGN4 : 0) | ((l == 0 && h->a_rowlanes) ? GG_A_ROWLANES : 0);
+          d.flags |= GG_PLANES | GG_B_RVEC | ((l == 0 && (c.Ci & 1)) ? GG_A_ALIGN4 : 0) | (l == 0 ? GG_A_ROWLANES : 0);
           d.A_hi = ip[0]; d.A_lo = ip[1];
           d.B_hi = h->wp[n][l][2]; d.B_lo = h->wp[n][l][3];
           d.bR_p = wT_r[l]; d.bN_p = wT_n[l];
@@ -405,201 +384,213 @@ int build_groups(b2g_sac* h) {
       h->act_groups.push_back(g);
     }
 
-    // ================= backward groups (pi, values)
-    // head dgrad -> dZ4 (masked by relu of cnn_fc1 output)
-    {
-      GemmGroup g;
-      g.name = "heads_dgrad";
-      TAB(row512, iota_tab(B, 512));
-      // pi
-      GemmDesc d = mk(h->dz0_pi, rowH, i64, h->p("model/pi/fc0/kernel"), i64, kH, h->dZ4[0], row512, i512, B, 512, H,
-                      GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
-      d.mask = h->F[0]; d.kM = rowFS; d.kN = i512;
-      if (h->use_planes) { d.C_hi = h->dZ4p[0][0]; d.C_lo = h->dZ4p[0][1]; }
-      g.host.push_back(d);
-      // values: [dz0_vf | dz0_q1 | dz0_q2] x [K0_vf ; K0_q1 ; K0_q2]^T
-      std::vector<int> br(3 * H);
-      const char* hn[3] = {"/vf/fc0/kernel", "/qf1/fc0/kernel", "/qf2/fc0/kernel"};
-      for (int q = 0; q < 3; ++q)
-        for (int r = 0; r < H; ++r) br[q * H + r] = (int)(h->tensors[h->tindex.at(nn(1, hn[q]))].off) + r;
-      TAB(brv, br);
-      TAB(i3H, iota_tab(3 * H));
-      GemmDesc e = mk(h->dz0_v3, row3H, i3H, h->P, brv, kH, h->dZ4[1], row512, i512, B, 512, 3 * H,
-                      GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
-      e.mask = h->F[1]; e.kM = rowFS; e.kN = i512;
-      if (h->use_planes) { e.C_hi = h->dZ4p[1][0]; e.C_lo = h->dZ4p[1][1]; }
-      g.host.push_back(e);
-      h->bwd_groups.push_back(g);
-      // fc1 wgrad + dgrad
-      GemmGroup f;
-      f.name = "fc1_bwd";
-      std::vector<int> cn(1024), fcT(1024);
-      for (int y = 0; y < H3; ++y)
-        for (int x = 0; x < W3; ++x)
-          for (int c = 0; c < 64; ++c) cn[(y * W3 + x) * 64 + c] = ((y + 2) * P3w + (x + 2)) * 64 + c;
-      TAB(cN3p, cn);
-      TAB(rowP3, iota_tab(B, P3h * P3w * 64));
-      TAB(wfT, iota_tab(1024, 512));
-      for (int n = 0; n < 2; ++n) {
-        GemmDesc w = mk(h->h3[n], i1024, fcA, h->dZ4[n], row512, i512, h->g(nn(n, "/cnn_fc1/w")), fcW, i512, 1024, 512, B,
-                        GG_COLSUM);
-        w.colsum = h->g(nn(n, "/cnn_fc1/b"));
-        if (h->wgrad_planes) {
-          w.flags = (w.flags & ~GG_COLSUM) | GG_PLANES | GG_MN_MAJOR;
-          w.A_hi = h->h3p[n][0]; w.A_lo = h->h3p[n][1]; w.B_hi = h->dZ4p[n][0]; w.B_lo = h->dZ4p[n][1];
-        }
-        f.host.push_back(w);
-        GemmDesc dg = mk(h->dZ4[n], row512, i512, h->p(nn(n, "/cnn_fc1/w")), i512, wfT, h->dZ3p[n], rowP3, cN3p, B, 1024, 512,
-                         GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
-        dg.mask = h->h3[n]; dg.kM = fcA; dg.kN = i1024;
-        if (h->use_planes) {
-          dg.flags |= GG_PLANES;
-          dg.A_hi = h->dZ4p[n][0]; dg.A_lo = h->dZ4p[n][1];
-          dg.B_hi = h->wp[n][3][0]; dg.B_lo = h->wp[n][3][1];
-          dg.C_hi = h->dZ3pp[n][0]; dg.C_lo = h->dZ3pp[n][1];
-        }
-        f.host.push_back(dg);
-      }
-      h->bwd_groups.push_back(f);
-    }
-    // conv3 wgrad + dgrad
-    {
-      GemmGroup g;
-      g.name = "conv3_bwd";
-      std::vector<int> am(B * H2 * W2), ar(9 * 64), br(9 * 64), cm(B * H2 * W2);
-      for (int b = 0; b < B; ++b)
+    if (!h->v2.on) {     // the round-1 backward: built only when the round-1 engines train
+      // dZ row tables in the zero-bordered layouts
+      std::vector<int> z2row(B * H2 * W2), z3row(B * H3 * W3);
+      for (int b = 0; b < B; ++b) {
         for (int y = 0; y < H2; ++y)
-          for (int x = 0; x < W2; ++x) {
-            am[(b * H2 + y) * W2 + x] = ((b * P3h + y + 2) * P3w + x + 2) * 64;
-            cm[(b * H2 + y) * W2 + x] = ((b * P2h + y + 1) * P2w + x + 1) * 64;
-          }
-      for (int ky = 0; ky < 3; ++ky)
-        for (int kx = 0; kx < 3; ++kx)
-          for (int n = 0; n < 64; ++n) {
-            ar[(ky * 3 + kx) * 64 + n] = -(ky * P3w + kx) * 64 + n;
-            br[(ky * 3 + kx) * 64 + n] = (ky * 3 + kx) * 64 * 64 + n;
-          }
-      TAB(t_am, am); TAB(t_ar, ar); TAB(t_br, br); TAB(t_cm, cm);
-      TAB(c64, iota_tab(64, 64));
-      const int R = B * H3 * W3;
-      for (int n = 0; n < 2; ++n) {
-        GemmDesc w = mk(h->h2[n], koff[2], rowoff[2], h->dZ3p[n], dz3row, i64, h->g(nn(n, "/cnn3/w")), wrow[2], i64, 576, 64, R,
-                        GG_COLSUM | GG_EPI_ATOMIC, split_for(9, R));
-        w.colsum = h->g(nn(n, "/cnn3/b"));
-        if (h->wgrad_planes) {
-          w.flags = (w.flags & ~GG_COLSUM) | GG_PLANES | GG_MN_MAJOR;
-          w.A_hi = h->h2p[n][0]; w.A_lo = h->h2p[n][1]; w.B_hi = h->dZ3pp[n][0]; w.B_lo = h->dZ3pp[n][1];
-        }
-        g.host.push_back(w);
-        GemmDesc dg = mk(h->dZ3p[n], t_am, t_ar, h->p(nn(n, "/cnn3/w")), t_br, c64, h->dZ2p[n], t_cm, i64, B * H2 * W2, 64, 576,
-                         GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
-        dg.mask = h->h2[n]; dg.kM = crow[1]; dg.kN = i64;
-        if (h->use_planes) {
-          dg.flags |= GG_PLANES;
-          dg.A_hi = h->dZ3pp[n][0]; dg.A_lo = h->dZ3pp[n][1];
-          dg.B_hi = h->wp[n][2][0]; dg.B_lo = h->wp[n][2][1];
-          dg.C_hi = h->dZ2pp[n][0]; dg.C_lo = h->dZ2pp[n][1];
-        }
-        g.host.push_back(dg);
+          for (int x = 0; x < W2; ++x) z2row[(b * H2 + y) * W2 + x] = ((b * P2h + y + 1) * P2w + x + 1) * 64;
+        for (int y = 0; y < H3; ++y)
+          for (int x = 0; x < W3; ++x) z3row[(b * H3 + y) * W3 + x] = ((b * P3h + y + 2) * P3w + x + 2) * 64;
       }
-      h->bwd_groups.push_back(g);
-    }
-    // conv2 wgrad + 4 parity-class dgrads
-    {
-      GemmGroup g;
-      g.name = "conv2_bwd";
-      const int R = B * H2 * W2;
-      TAB(c64, iota_tab(32, 64));
-      for (int n = 0; n < 2; ++n) {
-        GemmDesc w = mk(h->h1[n], koff[1], rowoff[1], h->dZ2p[n], dz2row, i64, h->g(nn(n, "/cnn2/w")), wrow[1], i64, 512, 64, R,
-                        GG_COLSUM | GG_EPI_ATOMIC, split_for(8, R));
-        w.colsum = h->g(nn(n, "/cnn2/b"));
-        if (h->wgrad_planes) {
-          w.flags = (w.flags & ~GG_COLSUM) | GG_PLANES | GG_MN_MAJOR;
-          w.A_hi = h->h1p[n][0]; w.A_lo = h->h1p[n][1]; w.B_hi = h->dZ2pp[n][0]; w.B_lo = h->dZ2pp[n][1];
+      TAB(dz2row, z2row);
+      TAB(dz3row, z3row);
+      // ================= backward groups (pi, values)
+      // head dgrad -> dZ4 (masked by relu of cnn_fc1 output)
+      {
+        GemmGroup g;
+        g.name = "heads_dgrad";
+        TAB(row512, iota_tab(B, 512));
+        // pi
+        GemmDesc d = mk(h->dz0_pi, rowH, i64, h->p("model/pi/fc0/kernel"), i64, kH, h->dZ4[0], row512, i512, B, 512, H,
+                        GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
+        d.mask = h->F[0]; d.kM = rowFS; d.kN = i512;
+        if (h->use_planes) { d.C_hi = h->dZ4p[0][0]; d.C_lo = h->dZ4p[0][1]; }
+        g.host.push_back(d);
+        // values: [dz0_vf | dz0_q1 | dz0_q2] x [K0_vf ; K0_q1 ; K0_q2]^T
+        std::vector<int> br(3 * H);
+        const char* hn[3] = {"/vf/fc0/kernel", "/qf1/fc0/kernel", "/qf2/fc0/kernel"};
+        for (int q = 0; q < 3; ++q)
+          for (int r = 0; r < H; ++r) br[q * H + r] = (int)(h->tensors[h->tindex.at(nn(1, hn[q]))].off) + r;
+        TAB(brv, br);
+        TAB(i3H, iota_tab(3 * H));
+        GemmDesc e = mk(h->dz0_v3, row3H, i3H, h->P, brv, kH, h->dZ4[1], row512, i512, B, 512, 3 * H,
+                        GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
+        e.mask = h->F[1]; e.kM = rowFS; e.kN = i512;
+        if (h->use_planes) { e.C_hi = h->dZ4p[1][0]; e.C_lo = h->dZ4p[1][1]; }
+        g.host.push_back(e);
+        h->bwd_groups.push_back(g);
+        // fc1 wgrad + dgrad
+        GemmGroup f;
+        f.name = "fc1_bwd";
+        std::vector<int> cn(1024), fcT(1024);
+        for (int y = 0; y < H3; ++y)
+          for (int x = 0; x < W3; ++x)
+            for (int c = 0; c < 64; ++c) cn[(y * W3 + x) * 64 + c] = ((y + 2) * P3w + (x + 2)) * 64 + c;
+        TAB(cN3p, cn);
+        TAB(rowP3, iota_tab(B, P3h * P3w * 64));
+        TAB(wfT, iota_tab(1024, 512));
+        for (int n = 0; n < 2; ++n) {
+          GemmDesc w = mk(h->h3[n], i1024, fcA, h->dZ4[n], row512, i512, h->g(nn(n, "/cnn_fc1/w")), fcW, i512, 1024, 512, B,
+                          GG_COLSUM);
+          w.colsum = h->g(nn(n, "/cnn_fc1/b"));
+          if (h->use_planes) {
+            w.flags = (w.flags & ~GG_COLSUM) | GG_PLANES | GG_MN_MAJOR;
+            w.A_hi = h->h3p[n][0]; w.A_lo = h->h3p[n][1]; w.B_hi = h->dZ4p[n][0]; w.B_lo = h->dZ4p[n][1];
+          }
+          f.host.push_back(w);
+          GemmDesc dg = mk(h->dZ4[n], row512, i512, h->p(nn(n, "/cnn_fc1/w")), i512, wfT, h->dZ3p[n], rowP3, cN3p, B, 1024, 512,
+                           GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
+          dg.mask = h->h3[n]; dg.kM = fcA; dg.kN = i1024;
+          if (h->use_planes) {
+            dg.flags |= GG_PLANES;
+            dg.A_hi = h->dZ4p[n][0]; dg.A_lo = h->dZ4p[n][1];
+            dg.B_hi = h->wp[n][3][0]; dg.B_lo = h->wp[n][3][1];
+            dg.C_hi = h->dZ3pp[n][0]; dg.C_lo = h->dZ3pp[n][1];
+          }
+          f.host.push_back(dg);
         }
-        g.host.push_back(w);
+        h->bwd_groups.push_back(f);
       }
-      for (int py = 0; py < 2; ++py)
-        for (int px = 0; px < 2; ++px) {
-          const int ny = (H1 - py + 1) / 2, nx = (W1 - px + 1) / 2;
-          std::vector<int> am(B * ny * nx), cm(B * ny * nx), ar(4 * 64), br(4 * 64);
-          for (int b = 0; b < B; ++b)
-            for (int yy = 0; yy < ny; ++yy)
-              for (int xx = 0; xx < nx; ++xx) {
-                am[(b * ny + yy) * nx + xx] = ((b * P2h + yy + 1) * P2w + xx + 1) * 64;
-                cm[(b * ny + yy) * nx + xx] = ((b * H1 + 2 * yy + py) * W1 + 2 * xx + px) * 32;
-              }
-          for (int jy = 0; jy < 2; ++jy)
-            for (int jx = 0; jx < 2; ++jx)
-              for (int q = 0; q < 64; ++q) {
-                ar[(jy * 2 + jx) * 64 + q] = -(jy * P2w + jx) * 64 + q;
-                br[(jy * 2 + jx) * 64 + q] = (((py + 2 * jy) * 4 + (px + 2 * jx)) * 32) * 64 + q;
-              }
-          TAB(t_am, am); TAB(t_ar, ar); TAB(t_br, br); TAB(t_cm, cm);
-          for (int n = 0; n < 2; ++n) {
-            GemmDesc dg = mk(h->dZ2p[n], t_am, t_ar, h->p(nn(n, "/cnn2/w")), t_br, c64, h->dZ1[n], t_cm, i64, B * ny * nx, 32, 256,
-                             GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
-            dg.mask = h->h1[n];
-            if (h->use_planes) {
-              dg.flags |= GG_PLANES;
-              dg.A_hi = h->dZ2pp[n][0]; dg.A_lo = h->dZ2pp[n][1];
-              dg.B_hi = h->wp[n][1][0]; dg.B_lo = h->wp[n][1][1];
-              dg.C_hi = h->dZ1p[n][0]; dg.C_lo = h->dZ1p[n][1];
+      // conv3 wgrad + dgrad
+      {
+        GemmGroup g;
+        g.name = "conv3_bwd";
+        std::vector<int> am(B * H2 * W2), ar(9 * 64), br(9 * 64), cm(B * H2 * W2);
+        for (int b = 0; b < B; ++b)
+          for (int y = 0; y < H2; ++y)
+            for (int x = 0; x < W2; ++x) {
+              am[(b * H2 + y) * W2 + x] = ((b * P3h + y + 2) * P3w + x + 2) * 64;
+              cm[(b * H2 + y) * W2 + x] = ((b * P2h + y + 1) * P2w + x + 1) * 64;
             }
-            g.host.push_back(dg);
+        for (int ky = 0; ky < 3; ++ky)
+          for (int kx = 0; kx < 3; ++kx)
+            for (int n = 0; n < 64; ++n) {
+              ar[(ky * 3 + kx) * 64 + n] = -(ky * P3w + kx) * 64 + n;
+              br[(ky * 3 + kx) * 64 + n] = (ky * 3 + kx) * 64 * 64 + n;
+            }
+        TAB(t_am, am); TAB(t_ar, ar); TAB(t_br, br); TAB(t_cm, cm);
+        TAB(c64, iota_tab(64, 64));
+        const int R = B * H3 * W3;
+        for (int n = 0; n < 2; ++n) {
+          GemmDesc w = mk(h->h2[n], koff[2], rowoff[2], h->dZ3p[n], dz3row, i64, h->g(nn(n, "/cnn3/w")), wrow[2], i64, 576, 64, R,
+                          GG_COLSUM | GG_EPI_ATOMIC, split_for(9, R));
+          w.colsum = h->g(nn(n, "/cnn3/b"));
+          if (h->use_planes) {
+            w.flags = (w.flags & ~GG_COLSUM) | GG_PLANES | GG_MN_MAJOR;
+            w.A_hi = h->h2p[n][0]; w.A_lo = h->h2p[n][1]; w.B_hi = h->dZ3pp[n][0]; w.B_lo = h->dZ3pp[n][1];
+          }
+          g.host.push_back(w);
+          GemmDesc dg = mk(h->dZ3p[n], t_am, t_ar, h->p(nn(n, "/cnn3/w")), t_br, c64, h->dZ2p[n], t_cm, i64, B * H2 * W2, 64, 576,
+                           GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
+          dg.mask = h->h2[n]; dg.kM = crow[1]; dg.kN = i64;
+          if (h->use_planes) {
+            dg.flags |= GG_PLANES;
+            dg.A_hi = h->dZ3pp[n][0]; dg.A_lo = h->dZ3pp[n][1];
+            dg.B_hi = h->wp[n][2][0]; dg.B_lo = h->wp[n][2][1];
+            dg.C_hi = h->dZ2pp[n][0]; dg.C_lo = h->dZ2pp[n][1];
+          }
+          g.host.push_back(dg);
+        }
+        h->bwd_groups.push_back(g);
+      }
+      // conv2 wgrad + 4 parity-class dgrads
+      {
+        GemmGroup g;
+        g.name = "conv2_bwd";
+        const int R = B * H2 * W2;
+        TAB(c64, iota_tab(32, 64));
+        for (int n = 0; n < 2; ++n) {
+          GemmDesc w = mk(h->h1[n], koff[1], rowoff[1], h->dZ2p[n], dz2row, i64, h->g(nn(n, "/cnn2/w")), wrow[1], i64, 512, 64, R,
+                          GG_COLSUM | GG_EPI_ATOMIC, split_for(8, R));
+          w.colsum = h->g(nn(n, "/cnn2/b"));
+          if (h->use_planes) {
+            w.flags = (w.flags & ~GG_COLSUM) | GG_PLANES | GG_MN_MAJOR;
+            w.A_hi = h->h1p[n][0]; w.A_lo = h->h1p[n][1]; w.B_hi = h->dZ2pp[n][0]; w.B_lo = h->dZ2pp[n][1];
+          }
+          g.host.push_back(w);
+        }
+        for (int py = 0; py < 2; ++py)
+          for (int px = 0; px < 2; ++px) {
+            const int ny = (H1 - py + 1) / 2, nx = (W1 - px + 1) / 2;
+            std::vector<int> am(B * ny * nx), cm(B * ny * nx), ar(4 * 64), br(4 * 64);
+            for (int b = 0; b < B; ++b)
+              for (int yy = 0; yy < ny; ++yy)
+                for (int xx = 0; xx < nx; ++xx) {
+                  am[(b * ny + yy) * nx + xx] = ((b * P2h + yy + 1) * P2w + xx + 1) * 64;
+                  cm[(b * ny + yy) * nx + xx] = ((b * H1 + 2 * yy + py) * W1 + 2 * xx + px) * 32;
+                }
+            for (int jy = 0; jy < 2; ++jy)
+              for (int jx = 0; jx < 2; ++jx)
+                for (int q = 0; q < 64; ++q) {
+                  ar[(jy * 2 + jx) * 64 + q] = -(jy * P2w + jx) * 64 + q;
+                  br[(jy * 2 + jx) * 64 + q] = (((py + 2 * jy) * 4 + (px + 2 * jx)) * 32) * 64 + q;
+                }
+            TAB(t_am, am); TAB(t_ar, ar); TAB(t_br, br); TAB(t_cm, cm);
+            for (int n = 0; n < 2; ++n) {
+              GemmDesc dg = mk(h->dZ2p[n], t_am, t_ar, h->p(nn(n, "/cnn2/w")), t_br, c64, h->dZ1[n], t_cm, i64, B * ny * nx, 32, 256,
+                               GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
+              dg.mask = h->h1[n];
+              if (h->use_planes) {
+                dg.flags |= GG_PLANES;
+                dg.A_hi = h->dZ2pp[n][0]; dg.A_lo = h->dZ2pp[n][1];
+                dg.B_hi = h->wp[n][1][0]; dg.B_lo = h->wp[n][1][1];
+                dg.C_hi = h->dZ1p[n][0]; dg.C_lo = h->dZ1p[n][1];
+              }
+              g.host.push_back(dg);
+            }
+          }
+        h->bwd_groups.push_back(g);
+      }
+      // conv1 wgrad
+      {
+        GemmGroup g;
+        g.name = "conv1_wgrad";
+        const int R = B * H1 * W1, M = 64 * Ci;
+        for (int n = 0; n < 2; ++n) {
+          GemmDesc w = mk(h->x_obs, koff[0], rowoff[0], h->dZ1[n], crow[0], i64, h->g(nn(n, "/cnn1/w")), wrow[0], i64, M, 32, R,
+                          GG_COLSUM | GG_EPI_ATOMIC, split_for((M + 63) / 64, R, 74));
+          w.colsum = h->g(nn(n, "/cnn1/b"));
+          if (h->use_planes) {
+            w.flags = (w.flags & ~GG_COLSUM) | GG_PLANES | GG_MN_MAJOR | ((Ci & 1) ? GG_A_ALIGN4 : 0) | GG_A_ROWLANES;
+            w.A_hi = h->xp[0][0]; w.A_lo = h->xp[0][1]; w.B_hi = h->dZ1p[n][0]; w.B_lo = h->dZ1p[n][1];
+          }
+          g.host.push_back(w);
+        }
+        h->bwd_groups.push_back(g);
+      }
+      if (h->use_planes) {     // bias gradients (column sums of the gradient maps) as one small launch
+        TAB(row512b, iota_tab(B, 512));
+        std::vector<ColsumJob> jobs, early;
+        int start = 0, estart = 0;
+        for (int n = 0; n < 2; ++n) {
+          const float* srcs[4] = {h->dZ1[n], h->dZ2p[n], h->dZ3p[n], h->dZ4[n]};
+          const int* rows[4] = {crow[0], dz2row, dz3row, row512b};
+          const int nrows[4] = {B * H1 * W1, B * H2 * W2, B * H3 * W3, B};
+          const int Ns[4] = {32, 64, 64, 512};
+          const char* bn[4] = {"/cnn1/b", "/cnn2/b", "/cnn3/b", "/cnn_fc1/b"};
+          for (int l = 0; l < 4; ++l) {
+            const int rows_per_cta = 8 * (256 / (Ns[l] / 4));
+            const int ctas = (nrows[l] + rows_per_cta - 1) / rows_per_cta;
+            if (l == 3) {       // cnn_fc1 bias: ready as soon as dZ4 exists -> part of the early all-reduce range
+              early.push_back(ColsumJob{srcs[l], rows[l], h->g(nn(n, bn[l])), nrows[l], Ns[l], estart});
+              estart += ctas;
+            } else {
+              jobs.push_back(ColsumJob{srcs[l], rows[l], h->g(nn(n, bn[l])), nrows[l], Ns[l], start});
+              start += ctas;
+            }
           }
         }
-      h->bwd_groups.push_back(g);
-    }
-    // conv1 wgrad
-    {
-      GemmGroup g;
-      g.name = "conv1_wgrad";
-      const int R = B * H1 * W1, M = 64 * Ci;
-      for (int n = 0; n < 2; ++n) {
-        GemmDesc w = mk(h->x_obs, koff[0], rowoff[0], h->dZ1[n], crow[0], i64, h->g(nn(n, "/cnn1/w")), wrow[0], i64, M, 32, R,
-                        GG_COLSUM | GG_EPI_ATOMIC, split_for((M + 63) / 64, R, 74));
-        w.colsum = h->g(nn(n, "/cnn1/b"));
-        if (h->wgrad_planes) {
-          w.flags = (w.flags & ~GG_COLSUM) | GG_PLANES | GG_MN_MAJOR | ((Ci & 1) ? GG_A_ALIGN4 : 0) | (h->a_rowlanes ? GG_A_ROWLANES : 0);
-          w.A_hi = h->xp[0][0]; w.A_lo = h->xp[0][1]; w.B_hi = h->dZ1p[n][0]; w.B_lo = h->dZ1p[n][1];
-        }
-        g.host.push_back(w);
+        h->n_colsum_early = (int)early.size();
+        h->colsum_early_ctas = estart;
+        if (int rc = dalloc(h, &h->d_colsum_early, early.size(), false)) return rc;
+        CK(cudaMemcpyAsync(h->d_colsum_early, early.data(), early.size() * sizeof(ColsumJob), cudaMemcpyHostToDevice, h->stream));
+        h->n_colsum = (int)jobs.size();
+        h->colsum_ctas = start;
+        if (int rc = dalloc(h, &h->d_colsum, jobs.size(), false)) return rc;
+        CK(cudaMemcpyAsync(h->d_colsum, jobs.data(), jobs.size() * sizeof(ColsumJob), cudaMemcpyHostToDevice, h->stream));
+        CK(cudaStreamSynchronize(h->stream));
       }
-      h->bwd_groups.push_back(g);
-    }
-    if (h->wgrad_planes) {     // bias gradients (column sums of the gradient maps) as one small launch
-      TAB(row512b, iota_tab(B, 512));
-      std::vector<ColsumJob> jobs, early;
-      int start = 0, estart = 0;
-      for (int n = 0; n < 2; ++n) {
-        const float* srcs[4] = {h->dZ1[n], h->dZ2p[n], h->dZ3p[n], h->dZ4[n]};
-        const int* rows[4] = {crow[0], dz2row, dz3row, row512b};
-        const int nrows[4] = {B * H1 * W1, B * H2 * W2, B * H3 * W3, B};
-        const int Ns[4] = {32, 64, 64, 512};
-        const char* bn[4] = {"/cnn1/b", "/cnn2/b", "/cnn3/b", "/cnn_fc1/b"};
-        for (int l = 0; l < 4; ++l) {
-          const int rows_per_cta = 8 * (256 / (Ns[l] / 4));
-          const int ctas = (nrows[l] + rows_per_cta - 1) / rows_per_cta;
-          if (l == 3) {       // cnn_fc1 bias: ready as soon as dZ4 exists -> part of the early all-reduce range
-            early.push_back(ColsumJob{srcs[l], rows[l], h->g(nn(n, bn[l])), nrows[l], Ns[l], estart});
-            estart += ctas;
-          } else {
-            jobs.push_back(ColsumJob{srcs[l], rows[l], h->g(nn(n, bn[l])), nrows[l], Ns[l], start});
-            start += ctas;
-          }
-        }
-      }
-      h->n_colsum_early = (int)early.size();
-      h->colsum_early_ctas = estart;
-      if (int rc = dalloc(h, &h->d_colsum_early, early.size(), false)) return rc;
-      CK(cudaMemcpyAsync(h->d_colsum_early, early.data(), early.size() * sizeof(ColsumJob), cudaMemcpyHostToDevice, h->stream));
-      h->n_colsum = (int)jobs.size();
-      h->colsum_ctas = start;
-      if (int rc = dalloc(h, &h->d_colsum, jobs.size(), false)) return rc;
-      CK(cudaMemcpyAsync(h->d_colsum, jobs.data(), jobs.size() * sizeof(ColsumJob), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaStreamSynchronize(h->stream));
     }
   }
 
@@ -617,14 +608,14 @@ int build_groups(b2g_sac* h) {
     GemmGroup a = g;
     // training step: the 516-deep reduction of each head is split over several CTAs (atomic accumulation into the
     // pre-zeroed z0 block) -- 10 tiles would otherwise each walk 9 r-chunks serially on 10 of the 132 SMs
-    if (h->fc0_split) for (auto& d : g.host) d.flags |= GG_EPI_ATOMIC;
+    for (auto& d : g.host) d.flags |= GG_EPI_ATOMIC;
     h->fwd_groups.push_back(g);
     a.name = "act_heads_fc0";
     a.host.resize(1);
     h->act_groups.push_back(a);
   }
   // ================= heads wgrad (fc0 and fc1 kernels + their biases through COLSUM)
-  {
+  if (!h->v2.on) {     // (engine v2 steps compute them with heads_wgrad_kernel, tail.cu)
     GemmGroup g;
     g.name = "heads_wgrad";
     const char* hp[4] = {"model/pi", "model/values_fn/vf", "model/values_fn/qf1", "model/values_fn/qf2"};
@@ -676,7 +667,6 @@ int build_groups(b2g_sac* h) {
       // share one launch when every problem of the group is in planes mode
       bool all_planes = true;
       for (auto& d : g.host) all_planes = all_planes && (d.flags & GG_PLANES);
-      if (const char* mg = getenv("B2G_TC_MERGE_BWD")) if (mg[0] == '0') all_planes = false;
       if (wg.empty() || dg.empty() || all_planes) { split.push_back(g); continue; }
       GemmGroup a = g, b = g;
       const std::string base = g.name.substr(0, g.name.find('_'));
@@ -686,43 +676,14 @@ int build_groups(b2g_sac* h) {
     }
     h->bwd_groups.swap(split);
   }
-  // engine selection: the large dense contractions go to the wgmma engine unless fp32 SIMT is asked for
-  const char* sel = getenv("B2G_TC_GROUPS");   // debugging: comma-separated group names, "all" or "none"
+  // engine selection: the large dense contractions (convs, cnn_fc1, head fc0) go to the wgmma engine unless fp32 SIMT is asked for
   auto pick = [&](GemmGroup& g) {
-    g.tc_eligible = g.name.find("conv") != std::string::npos || g.name.find("fc1_") != std::string::npos;
-    {   // head fc0 contractions (fwd / wgrad / dgrad) also run on the tensor engine unless B2G_TC_HEADS=0
-      const char* hd = getenv("B2G_TC_HEADS");
-      if (!(hd && hd[0] == '0') && g.name.find("heads_") != std::string::npos) g.tc_eligible = true;
-    }
-    g.tc = g.tc_eligible && h->cfg.precision != B2G_PREC_FP32_SIMT;
-    if (sel && g.tc_eligible && h->cfg.precision != B2G_PREC_FP32_SIMT) {
-      const std::string s(sel);
-      g.tc = s == "all" || (s != "none" && ("," + s + ",").find("," + g.name + ",") != std::string::npos);
-    }
+    g.tc = h->cfg.precision != B2G_PREC_FP32_SIMT && (g.name.find("conv") != std::string::npos || g.name.find("fc1_") != std::string::npos ||
+                                                        g.name.find("heads_") != std::string::npos);
   };
-  for (auto& g : h->fwd_groups) pick(g);
-  // Fused forward chain: conv1 -> conv2 -> conv3 -> fc1 of all three nets as ONE persistent launch with in-kernel layer
-  // barriers (gg_tc.cu: need_done / sync_ctr) instead of four launches.
-  if (h->fuse_fwd && h->cnn && h->use_planes && h->fwd_groups.size() >= 4) {
-    bool ok = true;
-    size_t ndesc = 0;
-    for (int l = 0; l < 4; ++l) {
-      ok = ok && h->fwd_groups[l].tc;
-      for (auto& d : h->fwd_groups[l].host) ok = ok && (d.flags & GG_PLANES);
-      ndesc += h->fwd_groups[l].host.size();
-    }
-    if (ok && ndesc <= (size_t)GG_TC_MAX_DESCS) {
-      GemmGroup m;
-      m.name = "cnn_fwd";
-      m.tc = m.tc_eligible = true;
-      m.layer_sync = true;
-      for (int l = 0; l < 4; ++l)
-        for (auto d : h->fwd_groups[l].host) { d.layer = l; m.host.push_back(d); }
-      h->fwd_groups.erase(h->fwd_groups.begin(), h->fwd_groups.begin() + 4);
-      h->fwd_groups.insert(h->fwd_groups.begin(), m);
-    }
-  }
-  for (auto& g : h->fwd_groups) { if (int rc = finalize_group(h, g)) return rc; }
+  // engine v2 runs the training forward: of the round-1 forward groups only their policy-inference copies are launched
+  if (h->v2.on) h->fwd_groups.clear();
+  for (auto& g : h->fwd_groups) { pick(g); if (int rc = finalize_group(h, g)) return rc; }
   for (auto& g : h->bwd_groups) { pick(g); if (int rc = finalize_group(h, g)) return rc; }
   for (auto& g : h->act_groups) { pick(g); if (int rc = finalize_group(h, g)) return rc; }
   return 0;
@@ -753,7 +714,7 @@ TailArgs make_tail(b2g_sac* h, bool want_per_sample) {
   t.grad_scale_B = h->B;
   t.z0_pi = h->z0[0]; t.z0_vf = h->z0[1]; t.z0_q1 = h->z0[2]; t.z0_q2 = h->z0[3]; t.z0_vt = h->z0[4];
   t.z0v_ld = h->H;
-  if (h->v2.on && !h->v2_skip) {     // engine v2 writes the three value heads' fc0 outputs as one [B, 3H] block
+  if (h->v2.on) {     // engine v2 writes the three value heads' fc0 outputs as one [B, 3H] block
     t.z0_vf = h->v2.z0v; t.z0_q1 = h->v2.z0v + h->H; t.z0_q2 = h->v2.z0v + 2 * h->H; t.z0v_ld = 3 * h->H;
   }
   t.pi = head_w(h, "model/pi", "dense");
@@ -773,7 +734,7 @@ TailArgs make_tail(b2g_sac* h, bool want_per_sample) {
   t.a0_pi = h->a0[0]; t.a0_vf = h->a0[1]; t.a0_q1 = h->a0[2]; t.a0_q2 = h->a0[3];
   t.dz1_pi = h->dz1[0]; t.dz1_vf = h->dz1[1]; t.dz1_q1 = h->dz1[2]; t.dz1_q2 = h->dz1[3];
   t.dz0_pi = h->dz0_pi; t.dz0_v3 = h->dz0_v3;
-  if (h->v2.bwd) { for (int k = 0; k < 2; ++k) { t.dz0_pi_p[k] = h->v2.dz0pi[k]; t.dz0_v3_p[k] = h->v2.dz0v[k]; } }
+  if (h->v2.on) { for (int k = 0; k < 2; ++k) { t.dz0_pi_p[k] = h->v2.dz0pi[k]; t.dz0_v3_p[k] = h->v2.dz0v[k]; } }
   t.per_sample = want_per_sample ? h->per_sample : nullptr;
   t.pi_out = want_per_sample ? h->pi_out : nullptr;
   t.metrics = h->metrics;
@@ -840,11 +801,10 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
     if (sampled) { ga.indices = nullptr; ga.rng_counters = h->counters; ga.seed = pa.seed; ga.indices_out = h->indices; }
     CK(cudaEventRecord(h->ev_aux[0], s));
     CK(cudaStreamWaitEvent(ax, h->ev_aux[0], 0));
-    if (h->use_planes && !h->v2.bwd) { planes_launch(h->d_jobs, h->n_jobs, h->job_tiles, ax); ++n; }
+    if (h->use_planes && !h->v2.on) { planes_launch(h->d_jobs, h->n_jobs, h->job_tiles, ax); ++n; }
     if (h->v2.on) { if (int rc = v2_planes(h, ax)) return rc; ++n; }
-    if (h->fc0_split || h->v2.on) { CK(cudaMemsetAsync(h->z0[0], 0, (size_t)5 * h->B * h->H * sizeof(float), ax)); ++n_copy; }
+    CK(cudaMemsetAsync(h->z0[0], 0, (size_t)5 * h->B * h->H * sizeof(float), ax)); ++n_copy;
     if (h->v2.on) { CK(cudaMemsetAsync(h->v2.z0v, 0, (size_t)3 * h->B * h->H * sizeof(float), ax)); ++n_copy; }
-    if (h->fuse_fwd) { CK(cudaMemsetAsync(h->sync_ctr, 0, 32 * sizeof(unsigned), ax)); ++n_copy; }
     CK(cudaEventRecord(h->ev_aux[1], ax));
     prep_launch(pa, ax); ++n;
     CK(cudaMemsetAsync(h->G, 0, (size_t)(h->n_train + MET_COUNT) * sizeof(float), ax)); ++n_copy;
@@ -872,56 +832,26 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
   if (fork) CK(cudaStreamWaitEvent(s, h->ev_aux[1], 0));
   else {
     CK(cudaMemsetAsync(h->G, 0, (size_t)(h->n_train + MET_COUNT) * sizeof(float), s)); ++n_copy;
-    if (h->fc0_split || h->v2.on) { CK(cudaMemsetAsync(h->z0[0], 0, (size_t)5 * h->B * h->H * sizeof(float), s)); ++n_copy; }
+    CK(cudaMemsetAsync(h->z0[0], 0, (size_t)5 * h->B * h->H * sizeof(float), s)); ++n_copy;
     if (h->v2.on) { CK(cudaMemsetAsync(h->v2.z0v, 0, (size_t)3 * h->B * h->H * sizeof(float), s)); ++n_copy; }
-    if (h->fuse_fwd) { CK(cudaMemsetAsync(h->sync_ctr, 0, 32 * sizeof(unsigned), s)); ++n_copy; }
     mark("zero_grads");
   }
-  int x3 = h->cfg.precision == B2G_PREC_BF16X3 ? 1 : 0;
-  if (const char* dbg = getenv("B2G_TC_DEBUG")) x3 |= atoi(dbg) << 8;   // kernel bring-up toggles (gg_tc.cu)
-  int sm_reserve = 0;     // SMs left free for a concurrently running collective (persistent GEMM grids are 1 CTA / SM)
+  const int x3 = h->cfg.precision == B2G_PREC_BF16X3 ? 1 : 0;
   auto run_group = [&](GemmGroup& g, cudaStream_t s) -> int {
-    const char* trn = getenv("B2G_TC_TRACE");
-    const bool trace = prof && prof->on && trn && g.name == trn && g.tc;
-    if (trace) {
-      CK(cudaMemsetAsync(h->dbg_trace, 0, 64 * 8 * sizeof(long long), s));
-      g_tc_trace = h->dbg_trace;
-    }
-    struct Reset { ~Reset() { g_tc_trace = nullptr; } } reset_;
-    if (g.tc) CK(gg_tc_launch(g.host.data(), (int)g.host.size(), g.total_tiles, g.host[0].flags, x3, h->num_sms - sm_reserve, s, g.dev_ranges, g.ranges_grid,
-                              g.layer_sync ? h->sync_ctr : nullptr));
+    if (g.tc) CK(gg_tc_launch(g.host.data(), (int)g.host.size(), g.total_tiles, g.host[0].flags, x3, h->num_sms, s));
     else gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
     ++n; mark(g.name.c_str());
-    if (trace) {
-      std::vector<long long> t(64 * 8);
-      CK(cudaStreamSynchronize(s));
-      CK(cudaMemcpy(t.data(), h->dbg_trace, t.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-      const long long t0 = t[0];
-      fprintf(stderr, "trace %s (cycles since first stamp; per tile: prod_start prod_issued | mma_full mma_commit | epi_tables epi_accfull epi_ld epi_stored)\n", g.name.c_str());
-      for (int i = 0; i < 12 && t[i * 8]; ++i)
-        fprintf(stderr, "  tile %2d: %7lld %7lld | %7lld %7lld | %7lld %7lld %7lld %7lld\n", i, t[i * 8] - t0, t[i * 8 + 1] - t0, t[i * 8 + 2] - t0,
-                t[i * 8 + 3] - t0, t[i * 8 + 7] - t0, t[i * 8 + 4] - t0, t[i * 8 + 5] - t0, t[i * 8 + 6] - t0);
-    }
     return 0;
   };
-  const bool fused = h->v2.on && h->v2.fuse && !h->v2.fwd_fused.empty();
-  if (fused) {
+  if (h->v2.on) {
     CK(cudaMemsetAsync(h->v2.dep_ctr, 0, (size_t)h->v2.n_dep_ctr * sizeof(int), s)); ++n_copy;
     if (int rc = v2_launch(h, h->v2.fwd_fused[0], s)) return rc;
     ++n; mark("fwd_fused");
-  } else if (h->v2.on) {
-    for (auto& g : h->v2.fwd) { if (int rc = v2_launch(h, g, s)) return rc; ++n; mark(g.name); }
   } else {
     for (auto& g : h->fwd_groups) if (int rc = run_group(g, s)) return rc;
   }
   if (fork) CK(cudaStreamWaitEvent(s, h->ev_aux[6], 0));
   tail_launch(make_tail(h, want_per_sample), s); ++n; mark("heads_tail");
-  const bool planes_bias = h->wgrad_planes && h->cfg.precision != B2G_PREC_FP32_SIMT;
-  // index of the last backward group that touches cnn_fc1 / the heads: everything up to it produces the gradients of
-  // [cnn_fc1 .. end] of both trainable blocks (+ log_ent_coef + the loss scalars) -- 84 % of the bytes
-  int last_fc1 = -1;
-  for (size_t i = 0; i < h->bwd_groups.size(); ++i)
-    if (h->bwd_groups[i].name.find("fc1") != std::string::npos || h->bwd_groups[i].name.find("heads") != std::string::npos) last_fc1 = (int)i;
   auto make_optim = [&]() {
     OptimArgs oa{};
     oa.P = h->P; oa.Mo = h->Mo; oa.Vo = h->Vo; oa.G = h->G; oa.T = h->P + h->n_train;
@@ -930,52 +860,48 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
     oa.metrics = h->metrics; oa.apply = apply ? 1 : 0;
     return oa;
   };
-  const bool overlap = h->overlap_ar && h->cnn && h->cfg.nranks > 1 && !(h->dp_p2p && apply) && last_fc1 >= 0 && last_fc1 + 1 < (int)h->bwd_groups.size();
+  // N > 1 on engine v2: the gradients of [cnn_fc1 .. end] of both trainable blocks (+ log_ent_coef + the loss scalars: 84 % of
+  // the bytes) are final after cnn_fc1's backward, so their all-reduce runs on a side stream / second communicator underneath the
+  // conv backward (the GEMM grids leave ar_sms SMs to it); only the conv ranges (0.6 MB) are reduced on the critical chain.
+  const bool overlap = h->overlap_ar && h->cfg.nranks > 1 && !(h->dp_p2p && apply);
   const int64_t pi_fc1 = h->tensors[h->tindex.at("model/pi/" + std::string(h->cnn ? "cnn_fc1/w" : "fc0/kernel"))].off;
   const int64_t v_fc1 = h->tensors[h->tindex.at("model/values_fn/" + std::string(h->cnn ? "cnn_fc1/w" : "vf/fc0/kernel"))].off;
-  const bool early_opt = !h->v2.bwd && fork && h->early_opt && h->cfg.nranks == 1 && h->cnn && last_fc1 >= 0 && last_fc1 + 1 < (int)h->bwd_groups.size() &&
-                         (pi_fc1 & 3) == 0 && (v_fc1 & 3) == 0;
   auto nccl_ck = [&](int rc) -> int {
     if (rc != 0) return fail(B2G_ENCCL, std::string("nccl: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "?"));
     return 0;
   };
   bool dp_early_opt = false;
-  if (h->v2.bwd) {
-    // backward chain on engine v2; the small head wgrads (fc0 / fc1 kernels and biases: fp32 operands, register-staged) stay
-    // on the v1 engine and, like the bias column sums, run on the leaf branch.
-    // N > 1: the gradients of [cnn_fc1 .. end] of both trainable blocks (+ log_ent_coef + the loss scalars: 84 % of the
-    // bytes) are final after fc1_bwd, so their all-reduce runs on a side stream / second communicator underneath the conv
-    // backward (the GEMM grids leave ar_sms SMs to it); only the conv ranges (0.6 MB) are reduced on the critical chain.
-    const bool ov = h->overlap_ar && h->cfg.nranks > 1 && !(h->dp_p2p && apply);
+  if (h->v2.on) {
+    // backward chain on engine v2; the small head wgrads (fc0 / fc1 kernels and biases: fp32 operands) run on the CUDA cores
+    // on the leaf branch.
     h->v2.sm_reserve = 0;
     cudaStream_t lx = fork ? ax : s;
-    for (auto& g : h->bwd_groups) {
-      if (g.name != "heads_wgrad") continue;
-      if (fork) { CK(cudaEventRecord(h->ev_aux[2], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[2], 0)); }
-      if (h->heads_wgrad_simt && h->H == 64) {
-        HeadsWgradArgs wa{};
-        const char* hp[4] = {"model/pi", "model/values_fn/vf", "model/values_fn/qf1", "model/values_fn/qf2"};
-        for (int q = 0; q < 4; ++q) {
-          wa.X0[q] = h->F[q == 0 ? 0 : 1];
-          wa.dz0[q] = q == 0 ? h->dz0_pi : h->dz0_v3 + (q - 1) * h->H;
-          wa.dz0_ld[q] = q == 0 ? h->H : 3 * h->H;
-          wa.a0[q] = h->a0[q]; wa.dz1[q] = h->dz1[q];
-          wa.M0[q] = q >= 2 ? h->feat_dim + h->A : h->feat_dim;
-          wa.g_k0[q] = h->g(std::string(hp[q]) + "/fc0/kernel"); wa.g_b0[q] = h->g(std::string(hp[q]) + "/fc0/bias");
-          wa.g_k1[q] = h->g(std::string(hp[q]) + "/fc1/kernel"); wa.g_b1[q] = h->g(std::string(hp[q]) + "/fc1/bias");
-        }
-        wa.x0_ld = h->FS; wa.B = h->B;
-        heads_wgrad_launch(wa, lx); ++n; if (!fork) mark("heads_wgrad");
-      } else if (int rc = run_group(g, lx)) return rc;
+    if (fork) { CK(cudaEventRecord(h->ev_aux[2], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[2], 0)); }
+    HeadsWgradArgs wa{};
+    const char* hp[4] = {"model/pi", "model/values_fn/vf", "model/values_fn/qf1", "model/values_fn/qf2"};
+    for (int q = 0; q < 4; ++q) {
+      wa.X0[q] = h->F[q == 0 ? 0 : 1];
+      wa.dz0[q] = q == 0 ? h->dz0_pi : h->dz0_v3 + (q - 1) * h->H;
+      wa.dz0_ld[q] = q == 0 ? h->H : 3 * h->H;
+      wa.a0[q] = h->a0[q]; wa.dz1[q] = h->dz1[q];
+      wa.M0[q] = q >= 2 ? h->feat_dim + h->A : h->feat_dim;
+      wa.g_k0[q] = h->g(std::string(hp[q]) + "/fc0/kernel"); wa.g_b0[q] = h->g(std::string(hp[q]) + "/fc0/bias");
+      wa.g_k1[q] = h->g(std::string(hp[q]) + "/fc1/kernel"); wa.g_b1[q] = h->g(std::string(hp[q]) + "/fc1/bias");
     }
-    // single GPU: the chain heads_dgrad .. conv2_dgrad is one fused launch.  Data parallel: two (cut after cnn_fc1, where the
-    // early all-reduce starts).
-    const bool fused_bwd = fused && h->v2.bwd_fused.size() == 3;
-    auto early_allreduce = [&]() -> int {
+    wa.x0_ld = h->FS; wa.B = h->B;
+    heads_wgrad_launch(wa, lx); ++n; if (!fork) mark("heads_wgrad");
+    // single GPU: the chain heads_dgrad .. conv wgrads is one fused launch.  Overlapped all-reduce: two (cut after cnn_fc1, where
+    // the early all-reduce starts).
+    if (!overlap) {
+      if (int rc = v2_launch(h, h->v2.bwd_fused[0], s)) return rc;
+      ++n; mark("bwd_fused");
+    } else {
+      if (int rc = v2_launch(h, h->v2.bwd_fused[1], s)) return rc;
+      ++n; mark("bwd_fused_fc");
       CK(cudaMemcpyAsync(h->G + h->n_train, h->metrics, MET_GN_PI * sizeof(float), cudaMemcpyDeviceToDevice, s)); ++n_copy;
       CK(cudaEventRecord(h->ev_fork, s));
       CK(cudaStreamWaitEvent(h->side, h->ev_fork, 0));
-      if (fork) { CK(cudaEventRecord(h->ev_aux[4], ax)); CK(cudaStreamWaitEvent(h->side, h->ev_aux[4], 0)); }   // heads_wgrad (+ fc1 bias sums)
+      if (fork) { CK(cudaEventRecord(h->ev_aux[4], ax)); CK(cudaStreamWaitEvent(h->side, h->ev_aux[4], 0)); }   // heads_wgrad
       if (int rc = nccl_ck(g_nccl.GroupStart())) return rc;
       if (int rc = nccl_ck(g_nccl.AllReduce(h->G + pi_fc1, h->G + pi_fc1, (size_t)(h->n_pi - pi_fc1), 7, 0, h->nccl_comm2, h->side))) return rc;
       if (int rc = nccl_ck(g_nccl.AllReduce(h->G + v_fc1, h->G + v_fc1, (size_t)(h->n_train + MET_COUNT - v_fc1), 7, 0, h->nccl_comm2, h->side))) return rc;
@@ -992,93 +918,37 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
       }
       CK(cudaEventRecord(h->ev_join, h->side));
       h->v2.sm_reserve = h->ar_sms;
-      return 0;
-    };
-    if (fused_bwd) {
-      if (!ov) {
-        if (int rc = v2_launch(h, h->v2.bwd_fused[0], s)) return rc;
-        ++n; mark("bwd_fused");
-      } else {
-        if (int rc = v2_launch(h, h->v2.bwd_fused[1], s)) return rc;
-        ++n; mark("bwd_fused_fc");
-        if (!h->v2.epi_colsum) {
-          if (fork) { CK(cudaEventRecord(h->ev_aux[3], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[3], 0)); }
-          if (int rc = v2_colsum(h, lx, 0)) return rc;
-          ++n;
-        }
-        if (int rc = early_allreduce()) return rc;
-        if (int rc = v2_launch(h, h->v2.bwd_fused[2], s)) return rc;
-        ++n; mark("bwd_fused_conv");
-      }
-      if (!h->v2.epi_colsum) {
-        if (fork) { CK(cudaEventRecord(h->ev_aux[0], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[0], 0)); }
-        if (!ov) { if (int rc = v2_colsum(h, lx, 0)) return rc; ++n; }
-        if (int rc = v2_colsum(h, lx, 1)) return rc;
-        ++n; if (!fork) mark("bias_grads");
-      }
-    }
-    for (auto& g : h->v2.bwd_groups) {
-      if (fused_bwd) break;
-      if (int rc = v2_launch(h, g, s)) return rc;
-      ++n; mark(g.name);
-      const std::string gn(g.name);
-      if (gn == "heads_dgrad") {            // dZ4 exists: cnn_fc1 bias sums on the leaf branch
-        if (fork) { CK(cudaEventRecord(h->ev_aux[3], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[3], 0)); }
-        if (int rc = v2_colsum(h, lx, 0)) return rc;
-        if (!h->v2.epi_colsum) { ++n; if (!fork) mark("bias_grads_fc1"); }
-      }
-      if (gn == "fc1_bwd" && ov) { if (int rc = early_allreduce()) return rc; }
-      if (gn == "conv2_dgrad") {            // every gradient map exists: conv bias sums overlap the conv wgrads
-        if (fork) { CK(cudaEventRecord(h->ev_aux[0], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[0], 0)); }
-        if (int rc = v2_colsum(h, lx, 1)) return rc;
-        if (!h->v2.epi_colsum) { ++n; if (!fork) mark("bias_grads"); }
-      }
+      if (int rc = v2_launch(h, h->v2.bwd_fused[2], s)) return rc;
+      ++n; mark("bwd_fused_conv");
     }
     h->v2.sm_reserve = 0;
-  } else
-  for (size_t i = 0; i < h->bwd_groups.size(); ++i) {
-    const bool leaf = fork && h->bwd_groups[i].name == "heads_wgrad";
-    if (fork && planes_bias && i + 1 == h->bwd_groups.size()) {
-      // every gradient map the conv bias sums read exists once the next-to-last group (conv2_bwd) is issued:
-      // the sums overlap conv1_wgrad
-      CK(cudaEventRecord(h->ev_aux[4], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[4], 0));
-      colsum_launch(h->d_colsum, h->n_colsum, h->colsum_ctas, ax); ++n;
-    }
-    if (leaf) {           // consumes only what the tail wrote; nothing downstream but the optimiser reads its output
-      CK(cudaEventRecord(h->ev_aux[2], s));
-      CK(cudaStreamWaitEvent(ax, h->ev_aux[2], 0));
-    }
-    if (int rc = run_group(h->bwd_groups[i], leaf ? ax : s)) return rc;
-    if ((int)i == last_fc1) {
-      if (fork) { CK(cudaEventRecord(h->ev_aux[3], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[3], 0)); }
-      if (planes_bias && h->n_colsum_early) {
-        colsum_launch(h->d_colsum_early, h->n_colsum_early, h->colsum_early_ctas, ax); ++n; mark("bias_grads_fc1");
+  } else {
+    // index of the last backward group that touches cnn_fc1 / the heads: the cnn_fc1 bias sums can start behind it
+    int last_fc1 = -1;
+    for (size_t i = 0; i < h->bwd_groups.size(); ++i)
+      if (h->bwd_groups[i].name.find("fc1") != std::string::npos || h->bwd_groups[i].name.find("heads") != std::string::npos) last_fc1 = (int)i;
+    for (size_t i = 0; i < h->bwd_groups.size(); ++i) {
+      const bool leaf = fork && h->bwd_groups[i].name == "heads_wgrad";
+      if (fork && h->use_planes && i + 1 == h->bwd_groups.size()) {
+        // every gradient map the conv bias sums read exists once the next-to-last group (conv2_bwd) is issued:
+        // the sums overlap conv1_wgrad
+        CK(cudaEventRecord(h->ev_aux[4], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[4], 0));
+        colsum_launch(h->d_colsum, h->n_colsum, h->colsum_ctas, ax); ++n;
       }
-      if (early_opt) {
-        // Single GPU: every gradient of [cnn_fc1 .. end] of both trainable blocks (84 % of the parameters) is final
-        // here, so their Adam / Polyak pass runs on the leaf branch underneath the conv backward; the closing
-        // optimiser launch only sweeps the conv kernels.
-        OptimArgs oe = make_optim();
-        oe.r_lo[0] = (int)pi_fc1; oe.r_hi[0] = (int)h->n_pi;
-        oe.r_lo[1] = (int)v_fc1; oe.r_hi[1] = (int)(h->n_pi + h->n_values + h->n_ent);
-        optim_launch(oe, ax); ++n;
+      if (leaf) {           // consumes only what the tail wrote; nothing downstream but the optimiser reads its output
+        CK(cudaEventRecord(h->ev_aux[2], s));
+        CK(cudaStreamWaitEvent(ax, h->ev_aux[2], 0));
       }
-      if (overlap) {
-        // early all-reduce on the side stream / second communicator, overlapping the conv backward
-        CK(cudaMemcpyAsync(h->G + h->n_train, h->metrics, MET_GN_PI * sizeof(float), cudaMemcpyDeviceToDevice, s)); ++n_copy;
-        CK(cudaEventRecord(h->ev_fork, s));
-        CK(cudaStreamWaitEvent(h->side, h->ev_fork, 0));
-        if (int rc = nccl_ck(g_nccl.GroupStart())) return rc;
-        if (int rc = nccl_ck(g_nccl.AllReduce(h->G + pi_fc1, h->G + pi_fc1, (size_t)(h->n_pi - pi_fc1), 7, 0, h->nccl_comm2, h->side))) return rc;
-        if (int rc = nccl_ck(g_nccl.AllReduce(h->G + v_fc1, h->G + v_fc1, (size_t)(h->n_train + MET_COUNT - v_fc1), 7, 0, h->nccl_comm2, h->side))) return rc;
-        if (int rc = nccl_ck(g_nccl.GroupEnd())) return rc;
-        ++n;
-        CK(cudaEventRecord(h->ev_join, h->side));
-        sm_reserve = h->ar_sms;
+      if (int rc = run_group(h->bwd_groups[i], leaf ? ax : s)) return rc;
+      if ((int)i == last_fc1) {
+        if (fork) { CK(cudaEventRecord(h->ev_aux[3], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[3], 0)); }
+        if (h->use_planes && h->n_colsum_early) {
+          colsum_launch(h->d_colsum_early, h->n_colsum_early, h->colsum_early_ctas, ax); ++n; mark("bias_grads_fc1");
+        }
       }
     }
+    if (h->use_planes && !fork) { colsum_launch(h->d_colsum, h->n_colsum, h->colsum_ctas, s); ++n; mark("bias_grads"); }
   }
-  if (planes_bias && !fork && !h->v2.bwd) { colsum_launch(h->d_colsum, h->n_colsum, h->colsum_ctas, s); ++n; mark("bias_grads"); }
   if (fork) { CK(cudaEventRecord(h->ev_aux[5], ax)); CK(cudaStreamWaitEvent(s, h->ev_aux[5], 0)); }
   if (h->cfg.nranks > 1 && !(h->dp_p2p && apply)) {
     if (overlap) {
@@ -1100,7 +970,7 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
   }
   OptimArgs oa = make_optim();
   oa.bump_counter = (fork && sampled) ? h->counters + 4 : nullptr;
-  if (early_opt || dp_early_opt) {
+  if (dp_early_opt) {
     oa.r_lo[0] = 0; oa.r_hi[0] = (int)pi_fc1;
     oa.r_lo[1] = (int)h->n_pi; oa.r_hi[1] = (int)v_fc1;
   }
@@ -1116,7 +986,7 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
   } else {     // (a gradient-only step of a connected learner takes the NCCL path above)
     optim_launch(oa, s); ++n; mark("adam_polyak");
   }
-  if (h->use_planes && apply && !h->v2.bwd) {
+  if (h->use_planes && apply && !h->v2.on) {
     // with fork: refreshed on the aux branch at the head of the next step (the API entry points mark them stale)
     if (!fork) { planes_launch(h->d_jobs, h->n_jobs, h->job_tiles, s); ++n; mark("weight_planes"); }
   }
@@ -1128,7 +998,7 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
 // BF16 planes of the CNN weights follow every optimiser step inside the step itself; after a host upload
 // (b2g_set_param) they are refreshed here, outside any graph.
 void refresh_planes(b2g_sac* h, bool for_step = false) {
-  if (for_step && (h->fork_leaves || h->v2.bwd)) {     // the step refreshes the planes itself and leaves them one update behind
+  if (for_step && (h->fork_leaves || h->v2.on)) {     // the step refreshes the planes itself and leaves them one update behind
     h->planes_dirty = true;
     return;
   }
@@ -1252,7 +1122,7 @@ int b2g_sac_dp_connect(b2g_sac* h, const void* all_exports, int nranks) {
   }
   // the cnn_fc1 weight gradients (80 % of the gradient bytes) are final when their tiles are stored: their epilogues push them
   h->dp_skip[0][0] = h->dp_skip[0][1] = h->dp_skip[1][0] = h->dp_skip[1][1] = 0;
-  if (h->v2.bwd && h->cnn && !getenv("B2G_DP_NO_EPI_PUSH")) {
+  if (h->v2.on) {
     const int n_train4 = (int)((h->n_pi + h->n_values + h->n_ent) >> 2), per4 = (n_train4 + nranks - 1) / nranks;
     const char* names[2] = {"model/pi/cnn_fc1/w", "model/values_fn/cnn_fc1/w"};
     for (int k = 0; k < 2; ++k) {
@@ -1269,7 +1139,7 @@ int b2g_sac_dp_connect(b2g_sac* h, const void* all_exports, int nranks) {
             found = true;
           }
       };
-      patch(h->v2.bwd_groups); patch(h->v2.bwd_fused);
+      patch(h->v2.bwd_fused);
       if (found && (t.off & 3) == 0) { h->dp_skip[k][0] = (int)(t.off >> 2); h->dp_skip[k][1] = (int)((t.off + 1024 * 512) >> 2); }
     }
   }
@@ -1362,13 +1232,11 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
   const int B = h->B;
 #define DA(ptr, count) if ((rc = dalloc(h, &(ptr), (size_t)(count)))) return bail(rc)
   DA(h->P, h->n_all); DA(h->Mo, h->n_train); DA(h->Vo, h->n_train); DA(h->G, h->n_train + MET_COUNT);
-  DA(h->dbg_trace, 64 * 8); DA(h->metrics, MET_COUNT); DA(h->counters, 8); DA(h->step_consts, 4); DA(h->d_lr, 1);
+  DA(h->metrics, MET_COUNT); DA(h->counters, 8); DA(h->step_consts, 4); DA(h->d_lr, 1);
   const int64_t cap = cfg->buffer_capacity;
-  {   // engine v2 (TMA-fed, cg.cu) drives the parity mode; B2G_ENGINE=v1 keeps the round-1 engine
-    const char* en = getenv("B2G_ENGINE");
-    h->v2.on = h->cnn && cfg->precision == B2G_PREC_BF16X3 && !(en && en[0] == 'v' && en[1] == '1') && h->Hi == 64 && h->Wi == 64;
+  {   // engine v2 (TMA-fed, cg.cu) trains the 64x64 CNN policy in the parity mode
+    h->v2.on = h->cnn && cfg->precision == B2G_PREC_BF16X3 && h->Hi == 64 && h->Wi == 64;
     if (const char* dbg = getenv("B2G_CG_DEBUG")) h->v2.dbg = atoi(dbg);
-    { const char* eb = getenv("B2G_ENGINE_BWD"); h->v2.bwd = h->v2.on && !(eb && eb[0] == 'v' && eb[1] == '1'); }
     h->compact = h->v2.on;        // the v2 gather reads compact rows only
     h->Ec = h->compact ? h->Hi * h->Wi * h->Cimg + 4 : h->E;
   }
@@ -1390,28 +1258,25 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
     for (int n = 0; n < 3; ++n) {
       DA(h->h1[n], (size_t)B * h->H1 * h->W1 * 32); DA(h->h2[n], (size_t)B * h->H2 * h->W2 * 64); DA(h->h3[n], (size_t)B * 1024);
     }
-    for (int n = 0; n < 2; ++n) {
+    for (int n = 0; n < 2 && !h->v2.on; ++n) {     // gradient maps of the round-1 backward
       DA(h->dZ4[n], (size_t)B * 512); DA(h->dZ3p[n], (size_t)B * (h->H3 + 4) * (h->W3 + 4) * 64);
       DA(h->dZ2p[n], (size_t)B * (h->H2 + 3) * (h->W2 + 3) * 64); DA(h->dZ1[n], (size_t)B * h->H1 * h->W1 * 32);
     }
   }
   h->use_planes = h->cnn && cfg->precision != B2G_PREC_FP32_SIMT;
   if (h->v2.on && (rc = v2_alloc(h))) return bail(rc);
-  if (const char* pl = getenv("B2G_TC_PLANES")) if (pl[0] == '0') h->use_planes = false;
-  h->wgrad_planes = h->use_planes;
-  if (const char* pl = getenv("B2G_TC_WGRAD_PLANES")) h->wgrad_planes = h->use_planes && pl[0] != '0';
   if (h->use_planes) {
     const size_t nx = (size_t)B * h->Hi * h->Wi * h->Cimg;
     for (int k = 0; k < 2; ++k) { DA(h->xp[0][k], nx); DA(h->xp[1][k], nx); }
     for (int n = 0; n < 3; ++n)
       for (int k = 0; k < 2; ++k) {
-        if (h->v2.on) {      // planes 0 / 1 of the v2 activations ARE the hi / lo planes the v1 backward reads
+        if (h->v2.on) {      // policy inference writes its hi / lo activation planes into planes 0 / 1 of the v2 activations
           h->h1p[n][k] = h->v2.H1[n][k]; h->h2p[n][k] = h->v2.H2[n][k]; h->h3p[n][k] = h->v2.H3[n][k];
           continue;
         }
         DA(h->h1p[n][k], (size_t)B * h->H1 * h->W1 * 32); DA(h->h2p[n][k], (size_t)B * h->H2 * h->W2 * 64); DA(h->h3p[n][k], (size_t)B * 1024);
       }
-    for (int n = 0; n < 2; ++n)
+    for (int n = 0; n < 2 && !h->v2.on; ++n)
       for (int k = 0; k < 2; ++k) {
         DA(h->dZ4p[n][k], (size_t)B * 512); DA(h->dZ3pp[n][k], (size_t)B * (h->H3 + 4) * (h->W3 + 4) * 64);
         DA(h->dZ2pp[n][k], (size_t)B * (h->H2 + 3) * (h->W2 + 3) * 64);
@@ -1428,12 +1293,6 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
   for (int n = 0; n < 3; ++n) DA(h->F[n], (size_t)B * h->FS);
   DA(h->z0[0], 5 * B * h->H);                      // one block: zeroed with a single memset per step
   for (int q = 1; q < 5; ++q) h->z0[q] = h->z0[0] + (size_t)q * B * h->H;
-  { const char* e = getenv("B2G_FC0_SPLIT"); h->fc0_split = !(e && atoi(e) == 0) && !h->v2.on; }
-  { const char* e = getenv("B2G_ROWLANES"); h->a_rowlanes = !(e && atoi(e) == 0); }
-  { const char* e = getenv("B2G_FUSE_FWD"); h->fuse_fwd = e && atoi(e) != 0; }
-  DA(h->sync_ctr, 32);
-  { const char* e = getenv("B2G_EARLY_OPT"); h->early_opt = e && atoi(e) != 0; }
-  { const char* e = getenv("B2G_TC_RANGES"); h->tc_ranges = e && atoi(e) != 0; }
   for (int q = 0; q < 4; ++q) { DA(h->a0[q], B * h->H); DA(h->dz1[q], B * h->H); }
   DA(h->dz0_pi, B * h->H); DA(h->dz0_v3, B * 3 * h->H);
   DA(h->per_sample, 7 * B); DA(h->pi_out, B * h->A); DA(h->eps, B * h->A + 4); DA(h->rew_n, B); DA(h->done_n, B);
@@ -1479,12 +1338,9 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
     int nrc = g_nccl.CommInitRank(&h->nccl_comm, cfg->nranks, id, cfg->rank);
     if (nrc != 0) return bail(fail(B2G_ENCCL, std::string("ncclCommInitRank: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(nrc) : "?")));
     {   // second communicator + side stream for the early (overlapped) all-reduce
+      // engine v2 only (B2G_AR_OVERLAP=0 puts the whole all-reduce back on the critical chain)
       const char* ov = getenv("B2G_AR_OVERLAP");
-      // opt-in (B2G_AR_OVERLAP=1): verified bit-correct at N=2, but measured gain is ~1 % because the persistent GEMM
-      // grids occupy every SM (even with SMs reserved the collective's launch latency dominates), see DESIGN.md section 5
-      // default: on for the v2 backward chain (B2G_AR_OVERLAP=0 puts the whole all-reduce back on the critical chain);
-      // the v1 chain keeps it opt-in (B2G_AR_OVERLAP=1)
-      const bool want_ov = h->v2.bwd ? !(ov && ov[0] == '0') : (ov && ov[0] == '1');
+      const bool want_ov = h->v2.on && !(ov && ov[0] == '0');
       if (want_ov && g_nccl.CommSplit && g_nccl.GroupStart && g_nccl.GroupEnd) {
         if (g_nccl.CommSplit(h->nccl_comm, 0, cfg->rank, &h->nccl_comm2, nullptr) == 0 && h->nccl_comm2 &&
             cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking) == cudaSuccess &&
@@ -1816,8 +1672,7 @@ int b2g_sac_step_host_pipelined(b2g_sac* h, const float* obs, const float* act, 
   }
   if (h->pipe_serial && k >= 1) CK(cudaStreamWaitEvent(h->cstream, h->ev_met[j ^ 1], 0));
   if (ptrace) cudaEventRecord(te[j][0], h->cstream);
-  static const bool host_compact = !(getenv("B2G_HOST_COMPACT") && getenv("B2G_HOST_COMPACT")[0] == '0');
-  const bool hc = h->compact && host_compact;
+  const bool hc = h->compact;
   if (hc) {
     // compact on the host (a few threads, ~0.1 ms) into pinned staging, copy half the bytes; the caller's arrays need not be
     // pinned and are free again when this call returns
@@ -1921,7 +1776,7 @@ int b2g_sac_act(b2g_sac* h, const float* obs, int n, int deterministic, float* a
     g.indices = nullptr;
     gather_launch(g, h->stream);
     for (auto& gr : h->act_groups) {
-      if (gr.tc) CK(gg_tc_launch(gr.host.data(), (int)gr.host.size(), gr.total_tiles, gr.host[0].flags, h->cfg.precision == B2G_PREC_BF16X3 ? 1 : 0, h->num_sms, h->stream, gr.dev_ranges, gr.ranges_grid));
+      if (gr.tc) CK(gg_tc_launch(gr.host.data(), (int)gr.host.size(), gr.total_tiles, gr.host[0].flags, h->cfg.precision == B2G_PREC_BF16X3 ? 1 : 0, h->num_sms, h->stream));
       else gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
     }
     b2g::act_launch(make_tail(h, false), chunk, deterministic, h->pi_out, h->stream);

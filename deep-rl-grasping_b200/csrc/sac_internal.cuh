@@ -34,9 +34,8 @@ struct Tensor {
 
 // ---- engine v2 (cg.cu): BF16 plane tensors, tensor maps and problem groups of the TMA-fed path
 struct V2State {
-  bool on = false;               // forward chain on the new engine
-  bool bwd = false;              // backward chain on the new engine
-  int KF = 576;                  // feature-row width of the F planes (513 features + actions, zero padded to 9 x 64)
+  bool on = false;               // the step runs on this engine (CNN policy, 64 x 64 input, bf16x3)
+  int KF = 576;                 // feature-row width of the F planes (513 features + actions, zero padded to 9 x 64)
   // activations: [which / net][plane]
   uint16_t* A1[2][3]{};          // im2col of the normalised image: [B*225][64*Ci]  (0 = obs, 1 = next_obs)
   uint16_t* H1[3][3]{};          // [B*225][32]
@@ -63,19 +62,16 @@ struct V2State {
   float* z0v = nullptr;          // fc0 pre-activations of vf|q1|q2: [B][192]
   void* plane_jobs = nullptr; int n_plane_jobs = 0, plane_ctas = 0;
   int* plane_cta_job = nullptr;  // job index of every CTA of the planes launch
-  void* colsum_part[2]{}; int n_colsum_part[2]{}, colsum_ctas_part[2]{};   // [0] cnn_fc1 biases (early), [1] conv biases
-  int sm_reserve = 0;            // SMs left to a collective that runs concurrently with the persistent GEMM grids
+  int sm_reserve = 0;           // SMs left to a collective that runs concurrently with the persistent GEMM grids
   std::vector<CUtensorMap> maps; // host copy
   std::vector<char> map_whole;   // per map: the box spans every plane
   std::vector<int> map_box_bytes;
   CUtensorMap* d_maps = nullptr;
-  std::vector<CgGroup> fwd, bwd_groups;
+  std::vector<CgGroup> fwd, bwd_groups;   // per-layer problem groups: the parts fuse_groups concatenates
   // fused launches: the layer groups above concatenated into one persistent launch each, chained by arrival counters
   std::vector<CgGroup> fwd_fused, bwd_fused;
-  bool fuse = false;
   int split_fc1 = 3;             // K-splits of the cnn_fc1 forward tiles (1 = none)
   int split_fc1_dgrad = 1;       // K-splits of the cnn_fc1 dgrad tiles (B2G_SPLIT_FC1_DGRAD; opt-in)
-  bool epi_colsum = true;        // conv / cnn_fc1 bias gradients come from the DGRAD epilogues (else: colsum2 launches over the planes)
   int* dep_ctr = nullptr; int n_dep_ctr = 0;
   std::vector<int*> tabs;
   int dbg = 0;
@@ -85,13 +81,12 @@ struct V2State {
 
 struct b2g_sac;
 namespace b2g {
-int v2_alloc(b2g_sac* h);    // plane tensors (before the v1 groups are built: the v1 backward reads planes 0 / 1 of the same buffers)
+int v2_alloc(b2g_sac* h);    // plane tensors (before the v1 groups are built: policy inference writes planes 0 / 1 of the activations)
 int v2_create(b2g_sac* h);   // tensor maps + problem groups
 int v2_planes(b2g_sac* h, cudaStream_t s);
 int v2_gather(b2g_sac* h, const GatherArgs& ga, cudaStream_t s);
 int v2_compact_rows(b2g_sac* h, const float* src_full, float* dst, long long first_row, long long wrap, int n, cudaStream_t s);   // full [n][E] -> compact rows (first_row + i) % wrap
 int v2_launch(b2g_sac* h, const CgGroup& g, cudaStream_t s);
-int v2_colsum(b2g_sac* h, cudaStream_t s, int part);   // bias gradients from the gradient-map planes
 }  // namespace b2g
 
 using namespace b2g;   // (internal header: only library translation units include it)
@@ -119,21 +114,18 @@ struct b2g_sac {
   // batch buffers
   float *x_obs = nullptr, *x_next = nullptr;
   float *h1[3]{}, *h2[3]{}, *h3[3]{}, *F[3]{};
-  float *dZ4[2]{}, *dZ3p[2]{}, *dZ2p[2]{}, *dZ1[2]{};
+  float *dZ4[2]{}, *dZ3p[2]{}, *dZ2p[2]{}, *dZ1[2]{};   // round-1 backward only
   float *z0[5]{}, *a0[4]{}, *dz1[4]{}, *dz0_pi = nullptr, *dz0_v3 = nullptr;
-  bool heads_wgrad_simt = true;  // head weight gradients on the CUDA cores (tail.cu) instead of a v1 tensor-engine launch
-  // BF16 hi/lo planes ([..][0] = hi, [..][1] = lo) of the tensors that feed forward / dgrad contractions
+  // BF16 hi/lo planes ([..][0] = hi, [..][1] = lo) of the tensors that feed forward / dgrad / wgrad contractions
   bool use_planes = false;
   uint16_t *xp[2][2]{}, *h1p[3][2]{}, *h2p[3][2]{}, *h3p[3][2]{};
-  uint16_t *dZ4p[2][2]{}, *dZ3pp[2][2]{}, *dZ2pp[2][2]{}, *dZ1p[2][2]{};
-  bool wgrad_planes = false;
+  uint16_t *dZ4p[2][2]{}, *dZ3pp[2][2]{}, *dZ2pp[2][2]{}, *dZ1p[2][2]{};   // round-1 backward only
   ColsumJob* d_colsum = nullptr;
   int n_colsum = 0, colsum_ctas = 0;
   uint16_t* wp[3][4][4]{};          // [net][cnn1,cnn2,cnn3,fc1][hi, lo, hiT, loT]
   PlaneJob* d_jobs = nullptr;
   int n_jobs = 0, job_tiles = 0;
   bool planes_dirty = true;
-  long long* dbg_trace = nullptr;
   std::map<const int*, std::vector<int>> host_tabs;   // host copies of the offset tables (contract checks at build time)
   float *per_sample = nullptr, *pi_out = nullptr, *eps = nullptr, *rew_n = nullptr, *done_n = nullptr;
   int* indices = nullptr;
@@ -179,15 +171,8 @@ struct b2g_sac {
   cudaEvent_t ev_aux[7]{};
   bool fork_leaves = false;
   std::map<std::tuple<const void*, const void*, const void*, int>, int> col_ids;
-  bool tc_ranges = false;                  // contiguous cost-balanced tile ranges per CTA: measured SLOWER than round-robin
-                                           // (split-R tiles of one output pile their atomics onto one CTA); B2G_TC_RANGES=1 enables
-  bool early_opt = false;                  // early fc1/heads optimiser pass on the leaf branch: measured no gain (B2G_EARLY_OPT=1 enables)
-  bool fuse_fwd = false;                   // B2G_FUSE_FWD=1: the CNN forward chain as one layer-synchronised launch
-  unsigned* sync_ctr = nullptr;            // its completion counter (zeroed every step)
-  bool a_rowlanes = true;                  // conv1 fwd gather with row-major lane order (B2G_ROWLANES=0 disables)
-  bool fc0_split = true;                   // split-R heads_fc0 (needs z0 zeroed every step)
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  bool overlap_ar = false;
+  bool overlap_ar = false;             // engine v2, N > 1: early all-reduce on the side stream (B2G_AR_OVERLAP=0 disables)
   int ar_sms = 8;
   ColsumJob* d_colsum_early = nullptr;
   int n_colsum_early = 0, colsum_early_ctas = 0;
@@ -195,7 +180,6 @@ struct b2g_sac {
   float last_ms = 0.f;
   int launches = 0;
   std::vector<std::string> prof_names;
-  b2g_sac_metrics* h_metrics_pinned = nullptr;
   float* h_met = nullptr;        // pinned MET_COUNT floats
   long long* h_cnt = nullptr;    // pinned counters
 
@@ -210,7 +194,6 @@ struct b2g_sac {
   double* hp_stats[2]{};             // pinned staging of set_norm_stats (asynchronous upload, no stream sync)
   cudaEvent_t ev_stats[2]{};
   int stats_k = 0;
-  bool v2_skip = false;          // (policy inference: the v1 forward groups write the separate z0 blocks)
 
   float* p(const std::string& n) { return P + tensors[tindex.at(n)].off; }
   float* g(const std::string& n) { return G + tensors[tindex.at(n)].off; }

@@ -1,4 +1,4 @@
-// Fused head "tail": everything between the fc0 contractions and their gradients, one warp per
+// Fused head "tail": everything between the fc0 contractions and their gradients, four warps per
 // sample (coalesced HBM/L2 reads, warp-shuffle reductions, no tensor cores: these are 64-wide
 // latency-bound layers).
 //
@@ -64,9 +64,9 @@ __device__ __forceinline__ V2 bwd64(const float* __restrict__ Ws, V2 dz, int lan
   }
   return o;
 }
-// N independent 64x64 mat-vecs advanced in lock step: same arithmetic (and order) per mat-vec as fwd64 / bwd64, but
-// the N dependent FMA chains and their shuffles / shared loads interleave, which is what a one-warp-per-sample kernel
-// needs -- its duration is the length of the dependency chain, not the instruction count.
+// N independent 64x64 mat-vecs advanced in lock step: same arithmetic (and order) per mat-vec as fwd64, but the N
+// dependent FMA chains and their shuffles / shared loads interleave, so the warp's duration is the length of one
+// dependency chain, not N of them.
 template <int N>
 __device__ __forceinline__ void fwd64xN(const float* const (&Ws)[N], const float* const (&bias)[N], const V2 (&a)[N], V2 (&o)[N], int lane) {
 #pragma unroll
@@ -90,29 +90,6 @@ __device__ __forceinline__ void fwd64xN(const float* const (&Ws)[N], const float
     }
   }
 }
-template <int N>
-__device__ __forceinline__ void bwd64xN(const float* const (&Ws)[N], const V2 (&dz)[N], V2 (&o)[N], int lane) {
-#pragma unroll
-  for (int k = 0; k < N; ++k) o[k] = V2{0.f, 0.f};
-#pragma unroll 4
-  for (int j = 0; j < 32; ++j) {
-#pragma unroll
-    for (int k = 0; k < N; ++k) {
-      const float dj = __shfl_sync(0xffffffffu, dz[k].lo, j);
-      o[k].lo = fmaf(dj, Ws[k][lane * LD + j], o[k].lo);
-      o[k].hi = fmaf(dj, Ws[k][(lane + 32) * LD + j], o[k].hi);
-    }
-  }
-#pragma unroll 4
-  for (int j = 0; j < 32; ++j) {
-#pragma unroll
-    for (int k = 0; k < N; ++k) {
-      const float dj = __shfl_sync(0xffffffffu, dz[k].hi, j);
-      o[k].lo = fmaf(dj, Ws[k][lane * LD + j + 32], o[k].lo);
-      o[k].hi = fmaf(dj, Ws[k][(lane + 32) * LD + j + 32], o[k].hi);
-    }
-  }
-}
 __device__ __forceinline__ V2 ld2(const float* p, int lane) { return V2{p[lane], p[lane + 32]}; }
 __device__ __forceinline__ void st2(float* p, int lane, V2 v) { p[lane] = v.lo; p[lane + 32] = v.hi; }
 // BF16 hi / lo planes of a 64-wide row (x = hi + lo to ~2^-17)
@@ -129,270 +106,11 @@ __device__ __forceinline__ float out1(const float* __restrict__ ko, const float*
 
 enum { S_PI = 0, S_VF, S_Q1, S_Q2, S_VT, S_NW };
 
-__global__ void __launch_bounds__(WARPS * 32) tail_kernel(TailArgs t) {
-  extern __shared__ float smem[];
-  float* Wk1 = smem;                              // S_NW x [64][65]
-  float* acc = Wk1 + S_NW * H * LD;               // output-layer gradient accumulators
-  // acc layout: kmu[64*A] ksig[64*A] bmu[A] bsig[A] | vf ko[64] bo | q1 ko[64] bo | q2 ko[64] bo
-  const int A = t.A;
-  const int n_acc = 2 * H * A + 2 * A + 3 * (H + 1);
-  float* red = acc + n_acc;                       // MET_COUNT + 1 (g_log_alpha)
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-
-  pdl_trigger();
-  pdl_wait();
-  const float* k1s[S_NW] = {t.pi.k1, t.vf.k1, t.q1.k1, t.q2.k1, t.vt.k1};
-  // stage the five 64x64 fc1 kernels (row stride 65) with 4-byte cp.async: all 80 copies of a thread are in flight
-  // at once (a load->store loop serialises into ~80 round trips and dominated this kernel)
-  for (int w = 0; w < S_NW; ++w)
-    for (int i = tid; i < H * H; i += blockDim.x) {
-      const uint32_t dst = (uint32_t)__cvta_generic_to_shared(&Wk1[w * H * LD + (i >> 6) * LD + (i & 63)]);
-      asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst), "l"(k1s[w] + i) : "memory");
-    }
-  // Every small parameter the per-sample chain touches (fc0/fc1 biases, output layers, the action rows of the qf fc0
-  // kernels) is staged too: read from global they are ~30 dependent L2 round trips per sample, and a warp owns exactly
-  // one sample, so those round trips were most of this kernel's duration.
-  float* sp = red + ((MET_COUNT + 1 + 3) & ~3);
-  auto stage = [&](float* dst, const float* src, int n) {
-    for (int i = tid; i < n; i += blockDim.x) {
-      const uint32_t d32 = (uint32_t)__cvta_generic_to_shared(dst + i);
-      asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(d32), "l"(src + i) : "memory");
-    }
-  };
-  const HeadW* hw[S_NW] = {&t.pi, &t.vf, &t.q1, &t.q2, &t.vt};
-  float* s_b0[S_NW]; float* s_b1[S_NW];
-  for (int w = 0; w < S_NW; ++w) {
-    s_b0[w] = sp + w * 2 * H; s_b1[w] = s_b0[w] + H;
-    stage(s_b0[w], hw[w]->b0, H); stage(s_b1[w], hw[w]->b1, H);
-  }
-  float* s_pi_ko = sp + S_NW * 2 * H;
-  float* s_ksig = s_pi_ko + H * A;
-  float* s_pi_bo = s_ksig + H * A;
-  float* s_bsig = s_pi_bo + A;
-  float* s_vko[4];                                  // vf, q1, q2, vt output layers: ko[64] then bo
-  s_vko[0] = s_bsig + A;
-  for (int w = 1; w < 4; ++w) s_vko[w] = s_vko[w - 1] + H + 1;
-  float* s_q1act = s_vko[3] + H + 1;                // action rows of the qf fc0 kernels [A][64]
-  float* s_q2act = s_q1act + A * H;
-  stage(s_pi_ko, t.pi.ko, H * A); stage(s_ksig, t.ksig, H * A); stage(s_pi_bo, t.pi.bo, A); stage(s_bsig, t.bsig, A);
-  {
-    const HeadW* vh[4] = {&t.vf, &t.q1, &t.q2, &t.vt};
-    for (int w = 0; w < 4; ++w) { stage(s_vko[w], vh[w]->ko, H); stage(s_vko[w] + H, vh[w]->bo, 1); }
-  }
-  stage(s_q1act, t.q1.k0 + (size_t)t.feat_dim * H, A * H);
-  stage(s_q2act, t.q2.k0 + (size_t)t.feat_dim * H, A * H);
-  for (int i = tid; i < n_acc + MET_COUNT + 1; i += blockDim.x) acc[i] = 0.f;
-  asm volatile("cp.async.wait_all;" ::: "memory");
-  __syncthreads();
-
-  float* a_kmu = acc;
-  float* a_ksig = a_kmu + H * A;
-  float* a_bmu = a_ksig + H * A;
-  float* a_bsig = a_bmu + A;
-  float* a_vf = a_bsig + A;
-  float* a_q1 = a_vf + H + 1;
-  float* a_q2 = a_q1 + H + 1;
-
-  const float invB = 1.0f / (float)t.grad_scale_B;
-  const float log_alpha = t.log_alpha[0];
-  const float alpha = expf(log_alpha);
-
-  for (int b = blockIdx.x * WARPS + warp; b < t.B; b += gridDim.x * WARPS) {
-    // every per-sample global read, issued as one batch
-    const V2 zpi = ld2(t.z0_pi + b * H, lane), zvf = ld2(t.z0_vf + (size_t)b * t.z0v_ld, lane), zvt = ld2(t.z0_vt + b * H, lane);
-    const V2 z0q1 = ld2(t.z0_q1 + (size_t)b * t.z0v_ld, lane), z0q2 = ld2(t.z0_q2 + (size_t)b * t.z0v_ld, lane);
-    const float rew_r = t.rew[b], done_r = t.done[b];
-    float eps_r[AMAX], act_r[AMAX];
-#pragma unroll
-    for (int a = 0; a < AMAX; ++a) {
-      eps_r[a] = a < A ? t.eps[b * A + a] : 0.f;
-      act_r[a] = a < A ? t.act[(size_t)b * t.act_stride + a] : 0.f;
-    }
-    // ------------------------------------------------------------------ actor forward
-    const V2 a0_pi = relu2(V2{zpi.lo + s_b0[S_PI][lane], zpi.hi + s_b0[S_PI][lane + 32]});
-    st2(t.a0_pi + b * H, lane, a0_pi);
-    const V2 g = relu2(fwd64(Wk1 + S_PI * H * LD, s_b1[S_PI], a0_pi, lane));
-    float mu[AMAX], ls_raw[AMAX], ls[AMAX], sd[AMAX], pi[AMAX], tt[AMAX], epsn[AMAX], actv[AMAX];
-    float logp = 0.f, ent = 0.f;
-#pragma unroll
-    for (int a = 0; a < AMAX; ++a) {
-      if (a < A) {
-        mu[a] = warp_sum(g.lo * s_pi_ko[lane * A + a] + g.hi * s_pi_ko[(lane + 32) * A + a]) + s_pi_bo[a];
-        ls_raw[a] = warp_sum(g.lo * s_ksig[lane * A + a] + g.hi * s_ksig[(lane + 32) * A + a]) + s_bsig[a];
-        ls[a] = fminf(fmaxf(ls_raw[a], LS_MIN), LS_MAX);
-        sd[a] = expf(ls[a]);
-        epsn[a] = eps_r[a];
-        actv[a] = act_r[a];
-        const float u = mu[a] + epsn[a] * sd[a];
-        tt[a] = (u - mu[a]) / (sd[a] + EPSF);
-        pi[a] = tanhf(u);
-        logp += -0.5f * (tt[a] * tt[a] + 2.f * ls[a] + 1.8378770664093453f) - logf(1.f - pi[a] * pi[a] + EPSF);
-        ent += ls[a] + 1.4189385332046727f;
-      }
-    }
-    // ------------------------------------------------------------------ critics forward
-    const V2 a0_vf = relu2(V2{zvf.lo + s_b0[S_VF][lane], zvf.hi + s_b0[S_VF][lane + 32]});
-    const V2 a0_vt = relu2(V2{zvt.lo + s_b0[S_VT][lane], zvt.hi + s_b0[S_VT][lane + 32]});
-    V2 z0q1p = z0q1, z0q2p = z0q2;   // fc0 pre-activation at pi: linear in the action columns
-#pragma unroll
-    for (int a = 0; a < AMAX; ++a) {
-      if (a < A) {
-        const float dlt = pi[a] - actv[a];
-        const float* r1 = s_q1act + a * H;
-        const float* r2 = s_q2act + a * H;
-        z0q1p.lo = fmaf(dlt, r1[lane], z0q1p.lo); z0q1p.hi = fmaf(dlt, r1[lane + 32], z0q1p.hi);
-        z0q2p.lo = fmaf(dlt, r2[lane], z0q2p.lo); z0q2p.hi = fmaf(dlt, r2[lane + 32], z0q2p.hi);
-      }
-    }
-    const V2 b0q1 = ld2(s_b0[S_Q1], lane), b0q2 = ld2(s_b0[S_Q2], lane);
-    const V2 a0_q1 = relu2(V2{z0q1.lo + b0q1.lo, z0q1.hi + b0q1.hi});
-    const V2 a0_q2 = relu2(V2{z0q2.lo + b0q2.lo, z0q2.hi + b0q2.hi});
-    const V2 a0_q1p = relu2(V2{z0q1p.lo + b0q1.lo, z0q1p.hi + b0q1.hi});
-    const V2 a0_q2p = relu2(V2{z0q2p.lo + b0q2.lo, z0q2p.hi + b0q2.hi});
-    V2 a1_vf, a1_vt, a1_q1, a1_q2, a1_q1p, a1_q2p;
-    {   // six independent fc1 layers, interleaved
-      const float* const Wn[6] = {Wk1 + S_VF * H * LD, Wk1 + S_VT * H * LD, Wk1 + S_Q1 * H * LD, Wk1 + S_Q2 * H * LD,
-                                  Wk1 + S_Q1 * H * LD, Wk1 + S_Q2 * H * LD};
-      const float* const bn[6] = {s_b1[S_VF], s_b1[S_VT], s_b1[S_Q1], s_b1[S_Q2], s_b1[S_Q1], s_b1[S_Q2]};
-      const V2 an[6] = {a0_vf, a0_vt, a0_q1, a0_q2, a0_q1p, a0_q2p};
-      V2 on[6];
-      fwd64xN<6>(Wn, bn, an, on, lane);
-      a1_vf = relu2(on[0]); a1_vt = relu2(on[1]); a1_q1 = relu2(on[2]); a1_q2 = relu2(on[3]);
-      a1_q1p = relu2(on[4]); a1_q2p = relu2(on[5]);
-    }
-    const float v = out1(s_vko[0], s_vko[0] + H, a1_vf, lane);
-    const float v_targ = out1(s_vko[3], s_vko[3] + H, a1_vt, lane);
-    const float q1 = out1(s_vko[1], s_vko[1] + H, a1_q1, lane), q2 = out1(s_vko[2], s_vko[2] + H, a1_q2, lane);
-    const float q1p = out1(s_vko[1], s_vko[1] + H, a1_q1p, lane), q2p = out1(s_vko[2], s_vko[2] + H, a1_q2p, lane);
-
-    // ------------------------------------------------------------------ losses + seeds
-    const float q_backup = rew_r + (1.f - done_r) * t.gamma * v_targ;
-    const float v_backup = fminf(q1p, q2p) - alpha * logp;
-    const float e1 = q1 - q_backup, e2 = q2 - q_backup, ev = v - v_backup;
-    if (lane == 0) {
-      atomicAdd(&red[MET_POLICY_LOSS], (alpha * logp - q1p) * invB);
-      atomicAdd(&red[MET_QF1_LOSS], 0.5f * e1 * e1 * invB);
-      atomicAdd(&red[MET_QF2_LOSS], 0.5f * e2 * e2 * invB);
-      atomicAdd(&red[MET_VALUE_LOSS], 0.5f * ev * ev * invB);
-      atomicAdd(&red[MET_ENT_COEF_LOSS], -log_alpha * (logp + t.target_entropy) * invB);
-      atomicAdd(&red[MET_ENTROPY], ent * invB);
-      atomicAdd(&red[MET_MEAN_Q1], q1 * invB);
-      atomicAdd(&red[MET_MEAN_Q2], q2 * invB);
-      atomicAdd(&red[MET_MEAN_V], v * invB);
-      atomicAdd(&red[MET_MEAN_LOGP], logp * invB);
-      atomicAdd(&red[MET_COUNT], -(logp + t.target_entropy) * invB);   // d ent_coef_loss / d log_alpha
-      if (t.per_sample) {
-        float* ps = t.per_sample;
-        ps[0 * t.B + b] = q1; ps[1 * t.B + b] = q2; ps[2 * t.B + b] = v; ps[3 * t.B + b] = logp;
-        ps[4 * t.B + b] = v_targ; ps[5 * t.B + b] = q1p; ps[6 * t.B + b] = q2p;
-      }
-    }
-    if (t.pi_out && lane < A) {
-      float pv = 0.f;
-#pragma unroll
-      for (int a = 0; a < AMAX; ++a) if (a == lane) pv = pi[a];
-      t.pi_out[b * A + lane] = pv;
-    }
-
-    // ------------------------------------------------------------------ value heads + d(-Q1(s,pi))/d pi backward
-    st2(t.a0_vf + b * H, lane, a0_vf);
-    st2(t.a0_q1 + b * H, lane, a0_q1);
-    st2(t.a0_q2 + b * H, lane, a0_q2);
-    float dpi[AMAX];
-    {
-      // output-layer gradients and the fc1 backward seeds of the three value heads, plus the qf1-at-pi path of the policy
-      // loss (its weights held constant); the four fc1 transposed mat-vecs are independent and run interleaved
-      const float douts[3] = {ev * invB, e1 * invB, e2 * invB};
-      const V2 a1s[3] = {a1_vf, a1_q1, a1_q2};
-      float* const accs[3] = {a_vf, a_q1, a_q2};
-      float* const dz1o[3] = {t.dz1_vf + b * H, t.dz1_q1 + b * H, t.dz1_q2 + b * H};
-      V2 dzn[4];
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        atomicAdd(&accs[k][lane], a1s[k].lo * douts[k]);
-        atomicAdd(&accs[k][lane + 32], a1s[k].hi * douts[k]);
-        if (lane == 0) atomicAdd(&accs[k][H], douts[k]);
-        dzn[k] = V2{a1s[k].lo > 0.f ? douts[k] * s_vko[k][lane] : 0.f, a1s[k].hi > 0.f ? douts[k] * s_vko[k][lane + 32] : 0.f};
-        st2(dz1o[k], lane, dzn[k]);
-      }
-      {
-        const float dout = -invB;
-        dzn[3] = V2{a1_q1p.lo > 0.f ? dout * s_vko[1][lane] : 0.f, a1_q1p.hi > 0.f ? dout * s_vko[1][lane + 32] : 0.f};
-      }
-      const float* const Wn[4] = {Wk1 + S_VF * H * LD, Wk1 + S_Q1 * H * LD, Wk1 + S_Q2 * H * LD, Wk1 + S_Q1 * H * LD};
-      V2 dan[4];
-      bwd64xN<4>(Wn, dzn, dan, lane);
-      const V2 a0s[3] = {a0_vf, a0_q1, a0_q2};
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        const V2 dz0{a0s[k].lo > 0.f ? dan[k].lo : 0.f, a0s[k].hi > 0.f ? dan[k].hi : 0.f};
-        st2(t.dz0_v3 + (size_t)b * 3 * H + k * H, lane, dz0);
-        if (t.dz0_v3_p[0]) st2_planes(t.dz0_v3_p[0] + (size_t)b * 3 * H + k * H, t.dz0_v3_p[1] + (size_t)b * 3 * H + k * H, lane, dz0);
-      }
-      const V2 dz0p{a0_q1p.lo > 0.f ? dan[3].lo : 0.f, a0_q1p.hi > 0.f ? dan[3].hi : 0.f};
-#pragma unroll
-      for (int a = 0; a < AMAX; ++a) {
-        if (a < A) {
-          const float* r1 = s_q1act + a * H;
-          dpi[a] = warp_sum(dz0p.lo * r1[lane] + dz0p.hi * r1[lane + 32]);
-        }
-      }
-    }
-    // ------------------------------------------------------------------ policy backward
-    float dmu[AMAX], dls[AMAX];
-    V2 dg{0.f, 0.f};
-#pragma unroll
-    for (int a = 0; a < AMAX; ++a) {
-      if (a < A) {
-        const float one_m = 1.f - pi[a] * pi[a];
-        const float du = (alpha * invB) * 2.f * pi[a] * one_m / (one_m + EPSF) + dpi[a] * one_m;
-        dmu[a] = du;
-        const float sp = sd[a] + EPSF;
-        float d = du * epsn[a] * sd[a] + (alpha * invB) * (-tt[a] * epsn[a] * sd[a] * EPSF / (sp * sp) - 1.f);
-        dls[a] = (ls_raw[a] >= LS_MIN && ls_raw[a] <= LS_MAX) ? d : 0.f;
-        atomicAdd(&a_kmu[lane * A + a], g.lo * dmu[a]);
-        atomicAdd(&a_kmu[(lane + 32) * A + a], g.hi * dmu[a]);
-        atomicAdd(&a_ksig[lane * A + a], g.lo * dls[a]);
-        atomicAdd(&a_ksig[(lane + 32) * A + a], g.hi * dls[a]);
-        if (lane == 0) { atomicAdd(&a_bmu[a], dmu[a]); atomicAdd(&a_bsig[a], dls[a]); }
-        dg.lo += dmu[a] * s_pi_ko[lane * A + a] + dls[a] * s_ksig[lane * A + a];
-        dg.hi += dmu[a] * s_pi_ko[(lane + 32) * A + a] + dls[a] * s_ksig[(lane + 32) * A + a];
-      }
-    }
-    {
-      V2 dz1{g.lo > 0.f ? dg.lo : 0.f, g.hi > 0.f ? dg.hi : 0.f};
-      st2(t.dz1_pi + b * H, lane, dz1);
-      V2 da0 = bwd64(Wk1 + S_PI * H * LD, dz1, lane);
-      V2 dz0{a0_pi.lo > 0.f ? da0.lo : 0.f, a0_pi.hi > 0.f ? da0.hi : 0.f};
-      st2(t.dz0_pi + b * H, lane, dz0);
-      if (t.dz0_pi_p[0]) st2_planes(t.dz0_pi_p[0] + (size_t)b * H, t.dz0_pi_p[1] + (size_t)b * H, lane, dz0);
-    }
-    // a1 (= g etc.) needed by the fc1 wgrad contractions: store over a0? no -- fc1 wgrad uses a0 (its input)
-  }
-  __syncthreads();
-  // ---- CTA -> global
-  for (int i = tid; i < H * A; i += blockDim.x) {
-    atomicAdd(t.g_pi.ko + i, a_kmu[i]);
-    atomicAdd(t.g_ksig + i, a_ksig[i]);
-  }
-  if (tid < A) { atomicAdd(t.g_pi.bo + tid, a_bmu[tid]); atomicAdd(t.g_bsig + tid, a_bsig[tid]); }
-  if (tid < H) {
-    atomicAdd(t.g_vf.ko + tid, a_vf[tid]); atomicAdd(t.g_q1.ko + tid, a_q1[tid]); atomicAdd(t.g_q2.ko + tid, a_q2[tid]);
-  }
-  if (tid == 0) {
-    atomicAdd(t.g_vf.bo, a_vf[H]); atomicAdd(t.g_q1.bo, a_q1[H]); atomicAdd(t.g_q2.bo, a_q2[H]);
-    atomicAdd(t.g_log_alpha, red[MET_COUNT]);
-  }
-  if (tid < MET_GN_PI) atomicAdd(t.metrics + tid, red[tid]);
-}
-
-
 // ================================================================================================
-// tail4: the same per-sample arithmetic as tail_kernel, with the sample's work split over FOUR warps
-// (actor | vf + target vf | qf1 | qf2) that exchange a handful of scalars through shared memory and three
-// named barriers.  A warp's duration is its dependency chain: 12 serial 64x64 mat-vecs became 4 (actor fc1 ->
-// qf1-at-pi fc1 -> qf1-at-pi fc1^T -> actor fc1^T), and 128 CTAs instead of 32 occupy the GPU.
-// Every expression is evaluated exactly as in tail_kernel (same order inside each mat-vec and reduction).
+// tail4: the per-sample work is split over FOUR warps (actor | vf + target vf | qf1 | qf2) that exchange a
+// handful of scalars through shared memory and three named barriers.  A warp's duration is its dependency
+// chain: with one warp per sample it is 12 serial 64x64 mat-vecs, here 4 (actor fc1 -> qf1-at-pi fc1 ->
+// qf1-at-pi fc1^T -> actor fc1^T), and 128 CTAs instead of 32 occupy the GPU.
 // ================================================================================================
 __device__ __forceinline__ void bar_group(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
@@ -755,19 +473,11 @@ void tail_launch(const TailArgs& a, cudaStream_t s) {
   static bool attr_set = false;
   const size_t smem = tail_smem(a.A);
   if (!attr_set) {
-    cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tail_smem(AMAX));
     cudaFuncSetAttribute(tail4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tail_smem(AMAX));
     attr_set = true;
   }
-  static int v1 = -1;
-  if (v1 < 0) { const char* e = getenv("B2G_TAIL"); v1 = (e && e[0] == 'v' && e[1] == '1') ? 1 : 0; }
-  if (v1) {
-    const int grid = (a.B + WARPS - 1) / WARPS;
-    launch_pdl(tail_kernel, dim3(grid), dim3(WARPS * 32), smem, s, pdl_enabled(), a);
-  } else {
-    const int grid = (a.B + 1) / 2;             // four warps per sample, two samples per CTA
-    launch_pdl(tail4_kernel, dim3(grid), dim3(WARPS * 32), smem, s, pdl_enabled(), a);
-  }
+  const int grid = (a.B + 1) / 2;             // four warps per sample, two samples per CTA
+  launch_pdl(tail4_kernel, dim3(grid), dim3(WARPS * 32), smem, s, pdl_enabled(), a);
 }
 
 }  // namespace b2g

@@ -187,6 +187,22 @@ def test_no_cpu_fallback_create_fails_loudly_without_gpu():
     assert "-2" in str(e.value) or "CUDA" in str(e.value)
 
 
+def test_design_switch_table_lists_every_environment_switch():
+    """DESIGN.md §4 documents exactly the B2G_* environment variables the library reads."""
+    csrc = os.path.join(ROOT, "deep-rl-grasping_b200", "csrc")
+    read = set()
+    for f in os.listdir(csrc):
+        with open(os.path.join(csrc, f)) as fh:
+            read |= set(re.findall(r'getenv\("(B2G_[A-Z_0-9]+)"\)', fh.read()))
+    with open(os.path.join(ROOT, "DESIGN.md")) as fh:
+        design = fh.read()
+    table = design.split("### Switches (environment variables")[1].split("\n\n")[1]
+    documented = set()
+    for row in table.splitlines()[2:]:
+        documented |= set(re.findall(r"`(B2G_[A-Z_0-9]+)", re.split(r"(?<!\\)\|", row)[1]))     # first column; "\|" is a literal bar
+    assert read and read == documented, (sorted(read - documented), sorted(documented - read))
+
+
 def test_product_package_never_imports_the_oracle():
     pkg = os.path.join(ROOT, "deep-rl-grasping_b200")
     for dirpath, _, files in os.walk(pkg):

@@ -1,4 +1,4 @@
-"""A/B of the round-2 design switches on the benchmark workload (depth CNN, B=256, bf16x3, CUDA-graph step), one subprocess per
+"""A/B of the design switches and precision modes on the benchmark workload (depth CNN, B=256, bf16x3, CUDA-graph step), one subprocess per
 setting so that every switch is read at create time:   python tools/ab_r2.py > ab_r2.txt"""
 import os, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -24,11 +24,7 @@ print("%%.1f us/step, %%d kernels/step" %% (float(np.median(ms)) * 1e3, L.launch
 L.close()
 ''' % (ROOT, ROOT)
 VARIANTS = [("default (TMA engine, fused launches, epilogue bias sums, CUDA-core head wgrads)", {}),
-            ("B2G_FUSE=0 (one launch per layer group)", {"B2G_FUSE": "0"}),
-            ("B2G_BIAS_EPI=0 (bias gradients by colsum2 launches)", {"B2G_BIAS_EPI": "0"}),
             ("B2G_FORK=0 (single-branch graph)", {"B2G_FORK": "0"}),
-            ("B2G_ENGINE_BWD=v1 (round-1 engine for the backward)", {"B2G_ENGINE_BWD": "v1"}),
-            ("B2G_ENGINE=v1 (round-1 engine)", {"B2G_ENGINE": "v1"}),
             ("precision fp32 (FFMA engine)", {"PREC": "0"}),
             ("precision bf16 single pass (fast mode, not a parity mode)", {"PREC": "2"})]
 for name, env in VARIANTS:
