@@ -21,16 +21,9 @@
 
 #include "../../include/b200grasp.h"
 #include "common.cuh"
+#include "host.cuh"
 
 using namespace b2g;
-
-extern thread_local std::string g_b2g_err;     // sac.cu
-static int bfail(int code, const std::string& msg) { g_b2g_err = msg; return code; }
-#define BCK(call)                                                                                       \
-  do {                                                                                                  \
-    cudaError_t e_ = (call);                                                                            \
-    if (e_ != cudaSuccess) return bfail(B2G_ECUDA, std::string(#call) + ": " + cudaGetErrorString(e_)); \
-  } while (0)
 
 namespace {
 
@@ -194,12 +187,6 @@ __global__ void bdq_target_copy_kernel(float* __restrict__ P, long long n_train,
   if (freq <= 0 || counters[3] % freq != 0) return;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n_train; i += (long long)gridDim.x * blockDim.x) P[n_train + i] = P[i];
 }
-
-std::vector<int> iota_t(int n, int stride = 1, int base = 0) {
-  std::vector<int> v(n);
-  for (int i = 0; i < n; ++i) v[i] = base + i * stride;
-  return v;
-}
 }  // namespace
 
 struct b2g_bdq {
@@ -237,29 +224,13 @@ struct b2g_bdq {
   long long per_C = 0;
   float *max_prio = nullptr, *d_beta = nullptr, *prio_out = nullptr;
   cudaGraphExec_t graph_exec = nullptr;
+  bool use_graph = true;
   float* p(const std::string& nm) { return P + tensors[tindex.at(nm)].off; }
   float* g(const std::string& nm) { return G + tensors[tindex.at(nm)].off; }
   float* pt(const std::string& nm) { return P + n_train + tensors[tindex.at(nm)].off; }
 };
 
 namespace {
-template <class T>
-int balloc(b2g_bdq* h, T** ptr, size_t count) {
-  void* q = nullptr;
-  BCK(cudaMalloc(&q, std::max<size_t>(count, 1) * sizeof(T)));
-  BCK(cudaMemsetAsync(q, 0, std::max<size_t>(count, 1) * sizeof(T), h->stream));
-  h->allocs.push_back(q);
-  *ptr = (T*)q;
-  return 0;
-}
-int btab(b2g_bdq* h, const std::vector<int>& v, const int** out) {
-  int* d = nullptr;
-  if (int rc = balloc(h, &d, v.size())) return rc;
-  BCK(cudaMemcpyAsync(d, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  BCK(cudaStreamSynchronize(h->stream));
-  *out = d;
-  return 0;
-}
 std::string fcname(int i) { return i == 0 ? "fully_connected" : "fully_connected_" + std::to_string(i); }
 
 void add_t(b2g_bdq* h, const std::string& name, int rows, int cols, bool w, int stride, int64_t& off) {
@@ -269,39 +240,16 @@ void add_t(b2g_bdq* h, const std::string& name, int rows, int cols, bool w, int 
   h->tensors.push_back(t);
 }
 
-GemmDesc mkd(const float* A, const int* aM, const int* aR, const float* B, const int* bR, const int* bN, float* C, const int* cM,
-             const int* cN, int M, int N, int R, int flags) {
-  GemmDesc d{};
-  d.A = A; d.B = B; d.C = C; d.aM = aM; d.aR = aR; d.bR = bR; d.bN = bN; d.cM = cM; d.cN = cN;
-  d.M = M; d.N = N; d.R = R; d.flags = flags; d.splitR = 1; d.alpha = 1.f;
-  return d;
-}
-int fin_group(b2g_bdq* h, GemmGroup& g) {
-  int start = 0;
-  for (auto& d : g.host) {
-    d.tiles_m = (d.M + GG_SIMT_BM - 1) / GG_SIMT_BM;
-    d.tiles_n = (d.N + GG_SIMT_BN - 1) / GG_SIMT_BN;
-    d.tile_start = start;
-    d.tile_count = d.tiles_m * d.tiles_n;
-    start += d.tile_count;
-  }
-  g.total_tiles = start;
-  if (int rc = balloc(h, &g.dev, g.host.size())) return rc;
-  BCK(cudaMemcpyAsync(g.dev, g.host.data(), g.host.size() * sizeof(GemmDesc), cudaMemcpyHostToDevice, h->stream));
-  BCK(cudaStreamSynchronize(h->stream));
-  return 0;
-}
-
 int build(b2g_bdq* h) {
   const int B = h->B, D = h->D, NBS = h->NBS, T0 = h->T0, T1 = h->T1, HB = h->HB, XS = h->XS, obs = h->cfg.obs_dim;
   const int* iT0; const int* iT1; const int* iHB; const int* iNBS; const int* i4; const int* iobs;
   const int* rXS; const int* rT0; const int* rT1; const int* rHB; const int* rNBS; const int* r4; const int* rcat;
   const int* kT0; const int* kT1; const int* kHB; const int* kNBS; const int* k4; const int* icat;
-#define BT(var, vec) if (int rc = btab(h, (vec), &var)) return rc;
-  BT(iT0, iota_t(T0)) BT(iT1, iota_t(T1)) BT(iHB, iota_t(HB)) BT(iNBS, iota_t(NBS)) BT(i4, iota_t(4)) BT(iobs, iota_t(XS))
-  BT(rXS, iota_t(B, XS)) BT(rT0, iota_t(B, T0)) BT(rT1, iota_t(B, T1)) BT(rHB, iota_t(B, HB)) BT(rNBS, iota_t(B, NBS)) BT(r4, iota_t(B, 4))
-  BT(rcat, iota_t(B, (D + 1) * HB)) BT(icat, iota_t((D + 1) * HB))
-  BT(kT0, iota_t(std::max(obs, T0) + 8, T0)) BT(kT1, iota_t(std::max(T0, T1) + 8, T1)) BT(kHB, iota_t(T1 + 8, HB)) BT(kNBS, iota_t(HB + 8, NBS)) BT(k4, iota_t(HB + 8, 4))
+#define BT(var, vec) if (int rc = upload_table(h->allocs, h->stream, (vec), &var)) return rc;
+  BT(iT0, iota_tab(T0)) BT(iT1, iota_tab(T1)) BT(iHB, iota_tab(HB)) BT(iNBS, iota_tab(NBS)) BT(i4, iota_tab(4)) BT(iobs, iota_tab(XS))
+  BT(rXS, iota_tab(B, XS)) BT(rT0, iota_tab(B, T0)) BT(rT1, iota_tab(B, T1)) BT(rHB, iota_tab(B, HB)) BT(rNBS, iota_tab(B, NBS)) BT(r4, iota_tab(B, 4))
+  BT(rcat, iota_tab(B, (D + 1) * HB)) BT(icat, iota_tab((D + 1) * HB))
+  BT(kT0, iota_tab(std::max(obs, T0) + 8, T0)) BT(kT1, iota_tab(std::max(T0, T1) + 8, T1)) BT(kHB, iota_tab(T1 + 8, HB)) BT(kNBS, iota_tab(HB + 8, NBS)) BT(k4, iota_tab(HB + 8, 4))
   const std::string sc[3] = {"bdq/model", "bdq/model", "bdq/target_q_func/model"};
   auto W = [&](int e, const std::string& rel) { return e == 2 ? h->pt("bdq/model" + rel) : h->p("bdq/model" + rel); };
   // ---------------- forward (3 evaluations), also the policy-inference groups (evaluation 0 only)
@@ -312,22 +260,22 @@ int build(b2g_bdq* h) {
       const float* x = e == 0 ? h->X : h->Xn;
       std::vector<GemmDesc> ds;
       if (layer == 0) {
-        GemmDesc d = mkd(x, rXS, iobs, W(e, "/common_net/" + fcname(0) + "/weights"), kT0, iT0, h->h1[e], rT0, iT0, B, T0, obs, GG_A_RVEC | GG_EPI_BIAS_RELU);
+        GemmDesc d = gemm_desc(x, rXS, iobs, W(e, "/common_net/" + fcname(0) + "/weights"), kT0, iT0, h->h1[e], rT0, iT0, B, T0, obs, GG_A_RVEC | GG_EPI_BIAS_RELU);
         d.bias = W(e, "/common_net/" + fcname(0) + "/biases"); ds.push_back(d);
       } else if (layer == 1) {
-        GemmDesc d = mkd(h->h1[e], rT0, iT0, W(e, "/common_net/" + fcname(1) + "/weights"), kT1, iT1, h->h2[e], rT1, iT1, B, T1, T0, GG_A_RVEC | GG_EPI_BIAS_RELU);
+        GemmDesc d = gemm_desc(h->h1[e], rT0, iT0, W(e, "/common_net/" + fcname(1) + "/weights"), kT1, iT1, h->h2[e], rT1, iT1, B, T1, T0, GG_A_RVEC | GG_EPI_BIAS_RELU);
         d.bias = W(e, "/common_net/" + fcname(1) + "/biases"); ds.push_back(d);
       } else if (layer == 2) {
         for (int q = 0; q <= D; ++q) {
           const std::string rel = q < D ? "/action_value/" + fcname(2 * q) : "/state_value/" + fcname(0);
-          GemmDesc d = mkd(h->h2[e], rT1, iT1, W(e, rel + "/weights"), kHB, iHB, q < D ? h->hb[e][q] : h->hv[e], rHB, iHB, B, HB, T1, GG_A_RVEC | GG_EPI_BIAS_RELU);
+          GemmDesc d = gemm_desc(h->h2[e], rT1, iT1, W(e, rel + "/weights"), kHB, iHB, q < D ? h->hb[e][q] : h->hv[e], rHB, iHB, B, HB, T1, GG_A_RVEC | GG_EPI_BIAS_RELU);
           d.bias = W(e, rel + "/biases"); ds.push_back(d);
         }
       } else {
         for (int q = 0; q <= D; ++q) {
           const std::string rel = q < D ? "/action_value/" + fcname(2 * q + 1) : "/state_value/" + fcname(1);
           const int N = q < D ? NBS : 4;
-          GemmDesc d = mkd(q < D ? h->hb[e][q] : h->hv[e], rHB, iHB, W(e, rel + "/weights"), q < D ? kNBS : k4, q < D ? iNBS : i4,
+          GemmDesc d = gemm_desc(q < D ? h->hb[e][q] : h->hv[e], rHB, iHB, W(e, rel + "/weights"), q < D ? kNBS : k4, q < D ? iNBS : i4,
                            q < D ? h->Aout[e][q] : h->Vout[e], q < D ? rNBS : r4, q < D ? iNBS : i4, B, N, HB, GG_A_RVEC | GG_EPI_BIAS);
           d.bias = W(e, rel + "/biases"); ds.push_back(d);
         }
@@ -345,12 +293,12 @@ int build(b2g_bdq* h) {
       const int N = q < D ? NBS : 4;
       const float* dz = q < D ? h->dA[q] : h->dV;
       const float* hin = q < D ? h->hb[0][q] : h->hv[0];
-      GemmDesc w = mkd(hin, iHB, rHB, dz, q < D ? rNBS : r4, q < D ? iNBS : i4, h->g(rel + "/weights"), q < D ? kNBS : k4, q < D ? iNBS : i4, HB, N, B, GG_COLSUM);
+      GemmDesc w = gemm_desc(hin, iHB, rHB, dz, q < D ? rNBS : r4, q < D ? iNBS : i4, h->g(rel + "/weights"), q < D ? kNBS : k4, q < D ? iNBS : i4, HB, N, B, GG_COLSUM);
       w.colsum = h->g(rel + "/biases");
       g.host.push_back(w);
       // d(hidden) = (dz . W_out^T) masked by relu, written into the concatenated buffer [B, (D+1) HB] at column q HB
-      const int* ccol; BT(ccol, iota_t(HB, 1, q * HB))
-      GemmDesc dg = mkd(dz, q < D ? rNBS : r4, q < D ? iNBS : i4, h->p(rel + "/weights"), q < D ? iNBS : i4, q < D ? kNBS : k4, h->dcat, rcat, ccol, B, HB, N,
+      const int* ccol; BT(ccol, iota_tab(HB, 1, q * HB))
+      GemmDesc dg = gemm_desc(dz, q < D ? rNBS : r4, q < D ? iNBS : i4, h->p(rel + "/weights"), q < D ? iNBS : i4, q < D ? kNBS : k4, h->dcat, rcat, ccol, B, HB, N,
                         GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
       dg.mask = hin; dg.kM = rHB; dg.kN = iHB;
       g.host.push_back(dg);
@@ -362,14 +310,14 @@ int build(b2g_bdq* h) {
     std::vector<int> br((D + 1) * HB);
     for (int q = 0; q <= D; ++q) {
       const std::string rel = q < D ? "bdq/model/action_value/" + fcname(2 * q) : "bdq/model/state_value/" + fcname(0);
-      const int* dzcol; BT(dzcol, iota_t(B, (D + 1) * HB, q * HB))
-      GemmDesc w = mkd(h->h2[0], iT1, rT1, h->dcat, dzcol, iHB, h->g(rel + "/weights"), kHB, iHB, T1, HB, B, GG_COLSUM);
+      const int* dzcol; BT(dzcol, iota_tab(B, (D + 1) * HB, q * HB))
+      GemmDesc w = gemm_desc(h->h2[0], iT1, rT1, h->dcat, dzcol, iHB, h->g(rel + "/weights"), kHB, iHB, T1, HB, B, GG_COLSUM);
       w.colsum = h->g(rel + "/biases");
       g.host.push_back(w);
       for (int r = 0; r < HB; ++r) br[q * HB + r] = (int)h->tensors[h->tindex.at(rel + "/weights")].off + r;
     }
     const int* brt; BT(brt, br)
-    GemmDesc dg = mkd(h->dcat, rcat, icat, h->P, brt, kHB, h->dh2, rT1, iT1, B, T1, (D + 1) * HB, GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK | GG_EPI_SCALE);
+    GemmDesc dg = gemm_desc(h->dcat, rcat, icat, h->P, brt, kHB, h->dh2, rT1, iT1, B, T1, (D + 1) * HB, GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK | GG_EPI_SCALE);
     dg.mask = h->h2[0]; dg.kM = rT1; dg.kN = iT1;
     dg.alpha = h->cfg.trunk_grad_rescale ? 1.0f / (float)(D + 1) : 1.0f;
     g.host.push_back(dg);
@@ -377,24 +325,24 @@ int build(b2g_bdq* h) {
   }
   {
     GemmGroup g; g.name = "bdq_trunk2_bwd";
-    GemmDesc w = mkd(h->h1[0], iT0, rT0, h->dh2, rT1, iT1, h->g("bdq/model/common_net/" + fcname(1) + "/weights"), kT1, iT1, T0, T1, B, GG_COLSUM);
+    GemmDesc w = gemm_desc(h->h1[0], iT0, rT0, h->dh2, rT1, iT1, h->g("bdq/model/common_net/" + fcname(1) + "/weights"), kT1, iT1, T0, T1, B, GG_COLSUM);
     w.colsum = h->g("bdq/model/common_net/" + fcname(1) + "/biases");
     g.host.push_back(w);
-    GemmDesc dg = mkd(h->dh2, rT1, iT1, h->p("bdq/model/common_net/" + fcname(1) + "/weights"), iT1, kT1, h->dh1, rT0, iT0, B, T0, T1, GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
+    GemmDesc dg = gemm_desc(h->dh2, rT1, iT1, h->p("bdq/model/common_net/" + fcname(1) + "/weights"), iT1, kT1, h->dh1, rT0, iT0, B, T0, T1, GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
     dg.mask = h->h1[0]; dg.kM = rT0; dg.kN = iT0;
     g.host.push_back(dg);
     h->bwd.push_back(g);
   }
   {
     GemmGroup g; g.name = "bdq_trunk1_wgrad";
-    GemmDesc w = mkd(h->X, iobs, rXS, h->dh1, rT0, iT0, h->g("bdq/model/common_net/" + fcname(0) + "/weights"), kT0, iT0, obs, T0, B, GG_COLSUM);
+    GemmDesc w = gemm_desc(h->X, iobs, rXS, h->dh1, rT0, iT0, h->g("bdq/model/common_net/" + fcname(0) + "/weights"), kT0, iT0, obs, T0, B, GG_COLSUM);
     w.colsum = h->g("bdq/model/common_net/" + fcname(0) + "/biases");
     g.host.push_back(w);
     h->bwd.push_back(g);
   }
-  for (auto& g : h->fwd) if (int rc = fin_group(h, g)) return rc;
-  for (auto& g : h->bwd) if (int rc = fin_group(h, g)) return rc;
-  for (auto& g : h->act) if (int rc = fin_group(h, g)) return rc;
+  for (auto& g : h->fwd) if (int rc = finalize_tiles(g, h->allocs, h->stream)) return rc;
+  for (auto& g : h->bwd) if (int rc = finalize_tiles(g, h->allocs, h->stream)) return rc;
+  for (auto& g : h->act) if (int rc = finalize_tiles(g, h->allocs, h->stream)) return rc;
   (void)sc;
   return 0;
 }
@@ -429,7 +377,7 @@ int bdq_issue(b2g_bdq* h, bool sampled, bool apply, const float* weights) {
     if (sampled) { per_sample_kernel<<<1, ((h->B + 31) / 32) * 32, 0, s>>>(pr); weights = h->weights; }   // overwrites the uniform draw
   }
   gather_launch(bgather(h, sampled, true), s);
-  BCK(cudaMemsetAsync(h->G, 0, (size_t)(h->n_train + MET_COUNT) * sizeof(float), s));
+  CK(cudaMemsetAsync(h->G, 0, (size_t)(h->n_train + MET_COUNT) * sizeof(float), s));
   for (auto& g : h->fwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
   BdqTailArgs t{};
   t.B = h->B; t.D = h->D; t.n = h->n; t.NBS = h->NBS; t.gamma = h->cfg.gamma;
@@ -442,32 +390,24 @@ int bdq_issue(b2g_bdq* h, bool sampled, bool apply, const float* weights) {
   for (auto& g : h->bwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
   if (h->per && sampled) per_write_kernel<<<1, ((h->B + 31) / 32) * 32, 0, s>>>(pr, h->indices, 0, h->cfg.buffer_capacity, h->B, 1);   // update_priorities(|td| + eps)
   if (h->cfg.nranks > 1) {      // gradients + loss scalars averaged over the ranks (each rank sampled its own replay shard)
-    BCK(cudaMemcpyAsync(h->G + h->n_train, h->metrics, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    CK(cudaMemcpyAsync(h->G + h->n_train, h->metrics, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
     if (int rc = nccl_allreduce_sum_f32(h->nccl_comm, h->G, (size_t)(h->n_train + MET_COUNT), s)) return rc;
-    BCK(cudaMemcpyAsync(h->metrics, h->G + h->n_train, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    CK(cudaMemcpyAsync(h->metrics, h->G + h->n_train, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
   }
   OptimArgs oa{};
   oa.P = h->P; oa.Mo = h->Mo; oa.Vo = h->Vo; oa.G = h->G; oa.T = h->P + h->n_train;
   oa.n_pi = (int)h->n_train; oa.n_values = 0; oa.n_ent = 0; oa.n_target = 0;
   oa.step_consts = h->step_consts; oa.tau = 0.f; oa.grad_scale = 1.0f / (float)h->cfg.nranks; oa.metrics = h->metrics; oa.apply = apply ? 1 : 0;
   optim_launch(oa, s);
-  BCK(cudaGetLastError());
+  CK(cudaGetLastError());
   if (apply) bdq_target_copy_kernel<<<64, 256, 0, s>>>(h->P, h->n_train, h->counters, h->cfg.target_update_freq);   // counters[3] = n_updates (prep)
-  BCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return 0;
 }
 
-int bset_lr(b2g_bdq* h, float lr) {
-  if (lr != h->cur_lr) {
-    BCK(cudaStreamSynchronize(h->stream));
-    BCK(cudaMemcpy(h->d_lr, &lr, sizeof(float), cudaMemcpyHostToDevice));
-    h->cur_lr = lr;
-  }
-  return 0;
-}
 int bfetch(b2g_bdq* h, b2g_bdq_metrics* out) {
-  BCK(cudaMemcpyAsync(h->h_met, h->metrics, MET_COUNT * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  BCK(cudaStreamSynchronize(h->stream));
+  CK(cudaMemcpyAsync(h->h_met, h->metrics, MET_COUNT * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   if (out) {
     const float inv = 1.0f / (float)h->cfg.nranks;
     out->loss = h->h_met[BMET_LOSS] * inv; out->mean_q = h->h_met[BMET_MEANQ] * inv; out->grad_norm = sqrtf(h->h_met[BMET_GN]);
@@ -493,31 +433,27 @@ int b2g_bdq_destroy(b2g_bdq* h) {
 }
 
 int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
-  if (!cfg || !out) return bfail(B2G_EINVAL, "cfg/out is NULL");
+  if (!cfg || !out) return b2g_fail(B2G_EINVAL, "cfg/out is NULL");
   *out = nullptr;
-  if (cfg->n_branches < 1 || cfg->n_branches > 8 || cfg->n_bins < 2 || cfg->n_bins > 64) return bfail(B2G_EINVAL, "n_branches in [1,8], n_bins in [2,64]");
+  if (cfg->n_branches < 1 || cfg->n_branches > 8 || cfg->n_bins < 2 || cfg->n_bins > 64) return b2g_fail(B2G_EINVAL, "n_branches in [1,8], n_bins in [2,64]");
   if (cfg->trunk0 % 4 || cfg->trunk1 % 4 || cfg->branch_hidden % 4 || cfg->trunk0 < 4 || cfg->trunk1 < 4 || cfg->branch_hidden < 4)
-    return bfail(B2G_EINVAL, "layer widths must be positive multiples of 4");
-  if (cfg->obs_dim < 1 || cfg->batch < 1 || cfg->buffer_capacity < 1) return bfail(B2G_EINVAL, "obs_dim, batch, buffer_capacity must be positive");
-  if (cfg->nranks < 1 || cfg->rank < 0 || cfg->rank >= cfg->nranks) return bfail(B2G_EINVAL, "bad rank/nranks");
-  if (cfg->nranks > 1 && !cfg->nccl_id) return bfail(B2G_EINVAL, "nranks > 1 needs nccl_id");
-  if (cfg->prioritized_replay && cfg->batch > 1024) return bfail(B2G_EINVAL, "prioritised replay supports batch <= 1024");
-  int ndev = 0;
-  BCK(cudaGetDeviceCount(&ndev));
-  if (cfg->device < 0 || cfg->device >= ndev) return bfail(B2G_ECUDA, "no such CUDA device");
-  BCK(cudaSetDevice(cfg->device));
-  cudaDeviceProp prop{};
-  BCK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 9) return bfail(B2G_ECUDA, std::string("libb200grasp is built for sm_90a only; found ") + prop.name);
+    return b2g_fail(B2G_EINVAL, "layer widths must be positive multiples of 4");
+  if (cfg->obs_dim < 1 || cfg->batch < 1 || cfg->buffer_capacity < 1) return b2g_fail(B2G_EINVAL, "obs_dim, batch, buffer_capacity must be positive");
+  if (cfg->nranks < 1 || cfg->rank < 0 || cfg->rank >= cfg->nranks) return b2g_fail(B2G_EINVAL, "bad rank/nranks");
+  if (cfg->nranks > 1 && !cfg->nccl_id) return b2g_fail(B2G_EINVAL, "nranks > 1 needs nccl_id");
+  if (cfg->prioritized_replay && cfg->batch > 1024) return b2g_fail(B2G_EINVAL, "prioritised replay supports batch <= 1024");
+  if (int rc = check_device(cfg->device)) return rc;
   b2g_bdq* h = new b2g_bdq();
   h->cfg = *cfg;
   h->cfg.nccl_id = nullptr; h->cfg.nccl_lib = nullptr;
   h->per = cfg->prioritized_replay != 0;
+  const char* ng = getenv("B2G_NO_GRAPH");
+  h->use_graph = !(ng && ng[0] == '1');
   h->B = cfg->batch; h->D = cfg->n_branches; h->n = cfg->n_bins; h->NBS = (cfg->n_bins + 3) / 4 * 4;
   h->T0 = cfg->trunk0; h->T1 = cfg->trunk1; h->HB = cfg->branch_hidden; h->E = cfg->obs_dim;
   h->XS = (cfg->obs_dim + cfg->n_branches + 7) / 8 * 8;
   auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_bdq_destroy(h); g_b2g_err = keep; return rc; };
-  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(bfail(B2G_ECUDA, "stream"));
+  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream"));
   // parameter inventory: same names as the zips (oracle/bdq_ref.py param_specs)
   int64_t off = 0;
   for (int d = 0; d < h->D; ++d) {
@@ -537,7 +473,7 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
   h->n_train = off;
   int rc = 0;
   const int B = h->B, D = h->D;
-#define BA(ptr, count) if ((rc = balloc(h, &(ptr), (size_t)(count)))) return bail(rc)
+#define BA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
   BA(h->P, 2 * h->n_train); BA(h->Mo, h->n_train); BA(h->Vo, h->n_train); BA(h->G, h->n_train + MET_COUNT); BA(h->metrics, MET_COUNT);
   BA(h->counters, 8); BA(h->step_consts, 4); BA(h->d_lr, 1);
   const int64_t cap = cfg->buffer_capacity;
@@ -560,10 +496,10 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
     BA(h->t_sum, 2 * h->per_C); BA(h->t_min, 2 * h->per_C);
     per_init_kernel<<<256, 256, 0, h->stream>>>(h->t_sum, h->t_min, 2 * h->per_C, h->max_prio);
     const float beta0 = 0.4f;
-    if (cudaMemcpyAsync(h->d_beta, &beta0, sizeof(float), cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return bail(bfail(B2G_ECUDA, "per init"));
+    if (cudaMemcpyAsync(h->d_beta, &beta0, sizeof(float), cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "per init"));
   }
 #undef BA
-  if (cudaMallocHost((void**)&h->h_met, MET_COUNT * sizeof(float)) != cudaSuccess) return bail(bfail(B2G_ECUDA, "cudaMallocHost"));
+  if (cudaMallocHost((void**)&h->h_met, MET_COUNT * sizeof(float)) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "cudaMallocHost"));
   {
     std::vector<double> ones(h->E, 1.0);
     const double nc[8] = {1.0, 10.0, 10.0, 0.0, 0.0, 0, 0, 0};
@@ -573,14 +509,14 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
         cudaMemcpyAsync(h->d_normc, nc, sizeof(nc), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
         cudaMemcpyAsync(h->d_Aptr, ap, sizeof(ap), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
         cudaStreamSynchronize(h->stream) != cudaSuccess)
-      return bail(bfail(B2G_ECUDA, "init copies"));
+      return bail(b2g_fail(B2G_ECUDA, "init copies"));
   }
   if ((rc = build(h))) return bail(rc);
   if (cfg->nranks > 1) {
     if ((rc = nccl_comm_init(&h->nccl_comm, cfg->nranks, cfg->nccl_id, cfg->rank, cfg->nccl_lib))) return bail(rc);
     if ((rc = nccl_allreduce_sum_f32(h->nccl_comm, h->G, (size_t)(h->n_train + MET_COUNT), h->stream))) return bail(rc);   // warm-up outside capture
   }
-  if (cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(bfail(B2G_ECUDA, "create sync"));
+  if (cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "create sync"));
   *out = h;
   return 0;
 }
@@ -589,7 +525,7 @@ int b2g_bdq_param_count(const b2g_bdq* h) { return h ? 1 + 2 * (int)h->tensors.s
 
 // index 0 = bdq/eps; 1..T = online tensors; T+1..2T = target tensors (names as in the zips)
 int b2g_bdq_param_info(const b2g_bdq* h, int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim) {
-  if (!h || idx < 0 || idx >= b2g_bdq_param_count(h) || !name) return bfail(B2G_EINVAL, "bad tensor index");
+  if (!h || idx < 0 || idx >= b2g_bdq_param_count(h) || !name) return b2g_fail(B2G_EINVAL, "bad tensor index");
   std::string nm = "bdq/eps";
   int64_t r = 1, c = 1;
   int nd = 0;
@@ -607,31 +543,31 @@ int b2g_bdq_param_info(const b2g_bdq* h, int idx, char* name, size_t name_cap, i
 }
 
 static int bdq_copy(b2g_bdq* h, const char* name, float* arena_online, float* host, size_t numel, bool to_host, bool allow_target) {
-  if (!h || !name || !host) return bfail(B2G_EINVAL, "NULL argument");
+  if (!h || !name || !host) return b2g_fail(B2G_EINVAL, "NULL argument");
   std::string nm(name);
   if (nm.size() > 2 && nm.compare(nm.size() - 2, 2, ":0") == 0) nm.resize(nm.size() - 2);
-  BCK(cudaSetDevice(h->cfg.device));
-  BCK(cudaStreamSynchronize(h->stream));
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
   if (nm == "bdq/eps") {
-    if (numel != 1) return bfail(B2G_EINVAL, "bdq/eps is a scalar");
+    if (numel != 1) return b2g_fail(B2G_EINVAL, "bdq/eps is a scalar");
     if (to_host) host[0] = h->eps_value; else h->eps_value = host[0];
     return 0;
   }
   bool target = false;
   const std::string tp = "bdq/target_q_func/model";
   if (nm.compare(0, tp.size(), tp) == 0) { target = true; nm = "bdq/model" + nm.substr(tp.size()); }
-  if (target && !allow_target) return bfail(B2G_EINVAL, "not a trainable variable");
+  if (target && !allow_target) return b2g_fail(B2G_EINVAL, "not a trainable variable");
   auto it = h->tindex.find(nm);
-  if (it == h->tindex.end()) return bfail(B2G_EINVAL, std::string("unknown variable: ") + name);
+  if (it == h->tindex.end()) return b2g_fail(B2G_EINVAL, std::string("unknown variable: ") + name);
   const BTensor& t = h->tensors[it->second];
   const size_t rows = t.is_weight ? t.rows : 1, cols = t.is_weight ? t.cols : (size_t)(t.rows * t.cols);
   const size_t ccount = t.is_weight ? t.cols : (size_t)t.cols;
-  if (numel != rows * ccount) return bfail(B2G_EINVAL, std::string("size mismatch for ") + name);
+  if (numel != rows * ccount) return b2g_fail(B2G_EINVAL, std::string("size mismatch for ") + name);
   float* dev = arena_online + t.off + (target ? h->n_train : 0);
   (void)cols;
   // repack between the zip layout [rows, cols] and the device row stride
-  if (to_host) BCK(cudaMemcpy2D(host, ccount * sizeof(float), dev, t.stride * sizeof(float), ccount * sizeof(float), rows, cudaMemcpyDeviceToHost));
-  else BCK(cudaMemcpy2D(dev, t.stride * sizeof(float), host, ccount * sizeof(float), ccount * sizeof(float), rows, cudaMemcpyHostToDevice));
+  if (to_host) CK(cudaMemcpy2D(host, ccount * sizeof(float), dev, t.stride * sizeof(float), ccount * sizeof(float), rows, cudaMemcpyDeviceToHost));
+  else CK(cudaMemcpy2D(dev, t.stride * sizeof(float), host, ccount * sizeof(float), ccount * sizeof(float), rows, cudaMemcpyHostToDevice));
   return 0;
 }
 int b2g_bdq_get_param(b2g_bdq* h, const char* name, float* dst, size_t numel) { return bdq_copy(h, name, h ? h->P : nullptr, dst, numel, true, true); }
@@ -641,18 +577,18 @@ int b2g_bdq_set_param(b2g_bdq* h, const char* name, const float* src, size_t num
 int b2g_bdq_get_grad(b2g_bdq* h, const char* name, float* dst, size_t numel) { return bdq_copy(h, name, h ? h->G : nullptr, dst, numel, true, false); }
 
 int b2g_bdq_replay_add(b2g_bdq* h, const float* obs, const float* act_idx, const float* rew, const float* next_obs, const float* done, int64_t n) {
-  if (!h || !obs || !act_idx || !rew || !next_obs || !done || n < 0) return bfail(B2G_EINVAL, "NULL argument");
-  BCK(cudaSetDevice(h->cfg.device));
+  if (!h || !obs || !act_idx || !rew || !next_obs || !done || n < 0) return b2g_fail(B2G_EINVAL, "NULL argument");
+  CK(cudaSetDevice(h->cfg.device));
   const int64_t cap = h->cfg.buffer_capacity;
   int64_t done_n = 0;
   while (done_n < n) {
     const int64_t chunk = std::min(n - done_n, cap - h->r_pos);
     const size_t E = h->E, D = h->D;
-    BCK(cudaMemcpyAsync(h->r_obs + h->r_pos * E, obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-    BCK(cudaMemcpyAsync(h->r_next + h->r_pos * E, next_obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-    BCK(cudaMemcpyAsync(h->r_act + h->r_pos * D, act_idx + done_n * D, chunk * D * sizeof(float), cudaMemcpyDefault, h->stream));
-    BCK(cudaMemcpyAsync(h->r_rew + h->r_pos, rew + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
-    BCK(cudaMemcpyAsync(h->r_done + h->r_pos, done + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
+    CK(cudaMemcpyAsync(h->r_obs + h->r_pos * E, obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
+    CK(cudaMemcpyAsync(h->r_next + h->r_pos * E, next_obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
+    CK(cudaMemcpyAsync(h->r_act + h->r_pos * D, act_idx + done_n * D, chunk * D * sizeof(float), cudaMemcpyDefault, h->stream));
+    CK(cudaMemcpyAsync(h->r_rew + h->r_pos, rew + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
+    CK(cudaMemcpyAsync(h->r_done + h->r_pos, done + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
     if (h->per) {        // new transitions enter with the running maximum priority ([SB2] PrioritizedReplayBuffer.add)
       PerArgs pr{};
       pr.tsum = h->t_sum; pr.tmin = h->t_min; pr.C = h->per_C; pr.max_prio = h->max_prio; pr.alpha = h->cfg.per_alpha; pr.eps = h->cfg.per_eps;
@@ -666,49 +602,38 @@ int b2g_bdq_replay_add(b2g_bdq* h, const float* obs, const float* act_idx, const
     done_n += chunk;
   }
   const long long sz = h->r_size;
-  BCK(cudaMemcpyAsync(h->counters + 5, &sz, sizeof(long long), cudaMemcpyHostToDevice, h->stream));
-  BCK(cudaStreamSynchronize(h->stream));
+  CK(cudaMemcpyAsync(h->counters + 5, &sz, sizeof(long long), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   return 0;
 }
 int64_t b2g_bdq_replay_size(const b2g_bdq* h) { return h ? h->r_size : 0; }
 
 int b2g_bdq_set_norm_stats(b2g_bdq* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs, double clip_rew, double eps,
                            int norm_obs, int norm_reward) {
-  if (!h) return bfail(B2G_EINVAL, "NULL handle");
-  if (norm_obs && (!obs_mean || !obs_var)) return bfail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
-  BCK(cudaSetDevice(h->cfg.device));
-  BCK(cudaStreamSynchronize(h->stream));
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  if (norm_obs && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
   if (norm_obs) {
     std::vector<double> istd(h->E);
     for (int i = 0; i < h->E; ++i) istd[i] = 1.0 / sqrt(obs_var[i] + eps);
-    BCK(cudaMemcpy(h->d_mean, obs_mean, h->E * sizeof(double), cudaMemcpyHostToDevice));
-    BCK(cudaMemcpy(h->d_istd, istd.data(), h->E * sizeof(double), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_mean, obs_mean, h->E * sizeof(double), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_istd, istd.data(), h->E * sizeof(double), cudaMemcpyHostToDevice));
   }
   const double nc[8] = {1.0 / sqrt(ret_var + eps), clip_obs, clip_rew, (double)norm_obs, (double)norm_reward, 0, 0, 0};
-  BCK(cudaMemcpy(h->d_normc, nc, sizeof(nc), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(h->d_normc, nc, sizeof(nc), cudaMemcpyHostToDevice));
   return 0;
 }
 
 int b2g_bdq_step(b2g_bdq* h, int n_steps, float lr, b2g_bdq_metrics* out) {
-  if (!h || n_steps < 0) return bfail(B2G_EINVAL, "bad argument");
-  if (h->r_size < 1) return bfail(B2G_ESTATE, "replay buffer is empty");
-  BCK(cudaSetDevice(h->cfg.device));
-  if (int rc = bset_lr(h, lr)) return rc;
-  static int no_graph = -1;
-  if (no_graph < 0) { const char* e = getenv("B2G_NO_GRAPH"); no_graph = (e && e[0] == '1') ? 1 : 0; }
-  if (!no_graph && !h->graph_exec) {       // the whole step (~14 launches of tiny layers) replays as one graph
-    cudaGraph_t graph = nullptr;
-    BCK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-    const int rc = bdq_issue(h, true, true, nullptr);
-    const cudaError_t e = cudaStreamEndCapture(h->stream, &graph);
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (e != cudaSuccess) return bfail(B2G_ECUDA, std::string("BDQ graph capture failed: ") + cudaGetErrorString(e));
-    const cudaError_t e2 = cudaGraphInstantiate(&h->graph_exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (e2 != cudaSuccess) return bfail(B2G_ECUDA, std::string("BDQ graph instantiate failed: ") + cudaGetErrorString(e2));
-  }
+  if (!h || n_steps < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  if (h->r_size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
+  CK(cudaSetDevice(h->cfg.device));
+  if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
+  if (h->use_graph && !h->graph_exec)       // the whole step (~14 launches of tiny layers) replays as one graph
+    if (int rc = capture_graph(h->stream, [&] { return bdq_issue(h, true, true, nullptr); }, &h->graph_exec)) return rc;
   for (int i = 0; i < n_steps; ++i) {
-    if (h->graph_exec) BCK(cudaGraphLaunch(h->graph_exec, h->stream));
+    if (h->graph_exec) CK(cudaGraphLaunch(h->graph_exec, h->stream));
     else if (int rc = bdq_issue(h, true, true, nullptr)) return rc;
     ++h->n_updates;
   }
@@ -716,57 +641,57 @@ int b2g_bdq_step(b2g_bdq* h, int n_steps, float lr, b2g_bdq_metrics* out) {
 }
 
 int b2g_bdq_set_per_beta(b2g_bdq* h, float beta) {
-  if (!h) return bfail(B2G_EINVAL, "NULL handle");
-  BCK(cudaSetDevice(h->cfg.device));
-  BCK(cudaStreamSynchronize(h->stream));
-  BCK(cudaMemcpy(h->d_beta, &beta, sizeof(float), cudaMemcpyHostToDevice));
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  CK(cudaMemcpy(h->d_beta, &beta, sizeof(float), cudaMemcpyHostToDevice));
   return 0;
 }
 
 int b2g_bdq_get_last_per(b2g_bdq* h, int32_t* slots, float* weights, float* priorities) {
-  if (!h) return bfail(B2G_EINVAL, "NULL handle");
-  BCK(cudaSetDevice(h->cfg.device));
-  BCK(cudaStreamSynchronize(h->stream));
-  if (slots) BCK(cudaMemcpy(slots, h->indices, h->B * sizeof(int32_t), cudaMemcpyDeviceToHost));
-  if (weights) BCK(cudaMemcpy(weights, h->weights, h->B * sizeof(float), cudaMemcpyDeviceToHost));
-  if (priorities) BCK(cudaMemcpy(priorities, h->prio_out, h->B * sizeof(float), cudaMemcpyDeviceToHost));
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  if (slots) CK(cudaMemcpy(slots, h->indices, h->B * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  if (weights) CK(cudaMemcpy(weights, h->weights, h->B * sizeof(float), cudaMemcpyDeviceToHost));
+  if (priorities) CK(cudaMemcpy(priorities, h->prio_out, h->B * sizeof(float), cudaMemcpyDeviceToHost));
   return 0;
 }
 
 int b2g_bdq_step_explicit(b2g_bdq* h, const float* obs, const float* act_idx, const float* rew, const float* next_obs, const float* done,
                           const float* weights, float lr, int apply_update, b2g_bdq_metrics* out, float* td_out) {
-  if (!h || !obs || !act_idx || !rew || !next_obs || !done) return bfail(B2G_EINVAL, "NULL argument");
-  BCK(cudaSetDevice(h->cfg.device));
-  if (int rc = bset_lr(h, lr)) return rc;
+  if (!h || !obs || !act_idx || !rew || !next_obs || !done) return b2g_fail(B2G_EINVAL, "NULL argument");
+  CK(cudaSetDevice(h->cfg.device));
+  if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
   const size_t B = h->B, E = h->E, D = h->D;
-  BCK(cudaMemcpyAsync(h->s_obs, obs, B * E * sizeof(float), cudaMemcpyDefault, h->stream));
-  BCK(cudaMemcpyAsync(h->s_next, next_obs, B * E * sizeof(float), cudaMemcpyDefault, h->stream));
-  BCK(cudaMemcpyAsync(h->s_act, act_idx, B * D * sizeof(float), cudaMemcpyDefault, h->stream));
-  BCK(cudaMemcpyAsync(h->s_rew, rew, B * sizeof(float), cudaMemcpyDefault, h->stream));
-  BCK(cudaMemcpyAsync(h->s_done, done, B * sizeof(float), cudaMemcpyDefault, h->stream));
-  if (weights) BCK(cudaMemcpyAsync(h->weights, weights, B * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->s_obs, obs, B * E * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->s_next, next_obs, B * E * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->s_act, act_idx, B * D * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->s_rew, rew, B * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->s_done, done, B * sizeof(float), cudaMemcpyDefault, h->stream));
+  if (weights) CK(cudaMemcpyAsync(h->weights, weights, B * sizeof(float), cudaMemcpyDefault, h->stream));
   if (int rc = bdq_issue(h, false, apply_update != 0, weights ? h->weights : nullptr)) return rc;
   if (apply_update) ++h->n_updates;
-  if (td_out) BCK(cudaMemcpyAsync(td_out, h->td, B * D * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  if (td_out) CK(cudaMemcpyAsync(td_out, h->td, B * D * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   return bfetch(h, out);
 }
 
 // greedy branch actions argmax_n Q_d(s, n) of the online network (the epsilon-greedy mixing is the caller's)
 int b2g_bdq_act(b2g_bdq* h, const float* obs, int n, int32_t* act_idx_out) {
-  if (!h || !obs || !act_idx_out || n < 0) return bfail(B2G_EINVAL, "bad argument");
-  BCK(cudaSetDevice(h->cfg.device));
+  if (!h || !obs || !act_idx_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  CK(cudaSetDevice(h->cfg.device));
   const size_t E = h->E, D = h->D;
   for (int done_n = 0; done_n < n; done_n += h->B) {
     const int chunk = std::min(h->B, n - done_n);
-    BCK(cudaMemcpyAsync(h->s_obs, obs + (size_t)done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
+    CK(cudaMemcpyAsync(h->s_obs, obs + (size_t)done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
     GatherArgs g = bgather(h, false, false);
     gather_launch(g, h->stream);
     for (auto& gr : h->act) gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
     bdq_argmax_kernel<<<(chunk * (int)D + 127) / 128, 128, 0, h->stream>>>(h->d_Aptr, chunk, (int)D, h->n, h->NBS, h->act_idx_out);
-    BCK(cudaMemcpyAsync(act_idx_out + (size_t)done_n * D, h->act_idx_out, chunk * D * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    BCK(cudaStreamSynchronize(h->stream));
+    CK(cudaMemcpyAsync(act_idx_out + (size_t)done_n * D, h->act_idx_out, chunk * D * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
   }
-  BCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return 0;
 }
 

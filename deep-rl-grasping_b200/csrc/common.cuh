@@ -28,10 +28,6 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 }
 #endif
 bool pdl_enabled();   // sac.cu: B2G_PDL != 0
-// NCCL through dlopen (sac.cu); 0 or a negative B2G_E* code with b2g_last_error() set
-int nccl_comm_init(void** comm, int nranks, const void* id128, int rank, const char* lib);
-int nccl_allreduce_sum_f32(void* comm, float* buf, size_t count, cudaStream_t s);
-void nccl_comm_destroy(void* comm);
 
 // ---------------------------------------------------------------------------------------------
 // Gather-GEMM problem descriptor.  One engine serves every dense contraction on the path:

@@ -18,16 +18,9 @@
 
 #include "../../include/b200grasp.h"
 #include "common.cuh"
+#include "host.cuh"
 
 using namespace b2g;
-
-extern thread_local std::string g_b2g_err;     // sac.cu
-static int efail(int code, const std::string& msg) { g_b2g_err = msg; return code; }
-#define ECK(call)                                                                                       \
-  do {                                                                                                  \
-    cudaError_t e_ = (call);                                                                            \
-    if (e_ != cudaSuccess) return efail(B2G_ECUDA, std::string(#call) + ": " + cudaGetErrorString(e_)); \
-  } while (0)
 
 namespace {
 struct EncLayer {
@@ -72,24 +65,6 @@ struct b2g_encoder {
 };
 
 namespace {
-template <class T>
-int ealloc(b2g_encoder* h, T** ptr, size_t count) {
-  void* q = nullptr;
-  ECK(cudaMalloc(&q, std::max<size_t>(count, 1) * sizeof(T)));
-  ECK(cudaMemsetAsync(q, 0, std::max<size_t>(count, 1) * sizeof(T), h->stream));
-  h->allocs.push_back(q);
-  *ptr = (T*)q;
-  return 0;
-}
-int etab(b2g_encoder* h, const std::vector<int>& v, const int** out) {
-  int* d = nullptr;
-  if (int rc = ealloc(h, &d, v.size())) return rc;
-  ECK(cudaMemcpyAsync(d, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  ECK(cudaStreamSynchronize(h->stream));
-  *out = d;
-  return 0;
-}
-
 // Offset tables for the whole capacity; a call with n < max_batch uses the leading n * out_h * out_w rows.
 int build_tables(b2g_encoder* h) {
   const int N = h->cfg.max_batch, L = (int)h->layers.size();
@@ -123,21 +98,21 @@ int build_tables(b2g_encoder* h) {
       bR[r] = r * y.fs;
     }
     for (int n = 0; n < y.f; ++n) bN[n] = cN[n] = n;
-    GemmDesc d{};
-    if (int rc = etab(h, aM, &d.aM)) return rc;
-    if (int rc = etab(h, aR, &d.aR)) return rc;
-    if (int rc = etab(h, bR, &d.bR)) return rc;
-    if (int rc = etab(h, bN, &d.bN)) return rc;
-    if (int rc = etab(h, cM, &d.cM)) return rc;
-    if (int rc = etab(h, cN, &d.cN)) return rc;
-    d.A = y.in; d.B = y.w; d.C = out; d.bias = y.b;
-    d.M = M; d.N = y.f; d.R = R; d.splitR = 1; d.alpha = h->cfg.alpha;
-    d.flags = GG_A_RVEC | GG_EPI_BIAS_LRELU | ((y.in_c & 3) && !dense ? GG_A_SCALAR : 0);
+    GemmDesc d = gemm_desc(y.in, nullptr, nullptr, y.w, nullptr, nullptr, out, nullptr, nullptr, M, y.f, R,
+                           GG_A_RVEC | GG_EPI_BIAS_LRELU | ((y.in_c & 3) && !dense ? GG_A_SCALAR : 0));
+    d.bias = y.b; d.alpha = h->cfg.alpha;
+    if (int rc = upload_table(h->allocs, h->stream, aM, &d.aM)) return rc;
+    if (int rc = upload_table(h->allocs, h->stream, aR, &d.aR)) return rc;
+    if (int rc = upload_table(h->allocs, h->stream, bR, &d.bR)) return rc;
+    if (int rc = upload_table(h->allocs, h->stream, bN, &d.bN)) return rc;
+    if (int rc = upload_table(h->allocs, h->stream, cM, &d.cM)) return rc;
+    if (int rc = upload_table(h->allocs, h->stream, cN, &d.cN)) return rc;
     GemmGroup& g = h->groups[l];
     g.name = dense ? "enc_dense" : "enc_conv" + std::to_string(l);
     g.host = {d};
-    if (int rc = ealloc(h, &g.dev, 1)) return rc;
+    if (int rc = finalize_tiles(g, h->allocs, h->stream)) return rc;
   }
+  h->built_n = N;
   return 0;
 }
 
@@ -145,16 +120,9 @@ int set_batch(b2g_encoder* h, int n) {
   if (h->built_n == n) return 0;
   for (size_t l = 0; l < h->layers.size(); ++l) {
     const EncLayer& y = h->layers[l];
-    GemmGroup& g = h->groups[l];
-    GemmDesc& d = g.host[0];
-    d.M = n * y.out_h * y.out_w;
-    d.tiles_m = (d.M + GG_SIMT_BM - 1) / GG_SIMT_BM;
-    d.tiles_n = (d.N + GG_SIMT_BN - 1) / GG_SIMT_BN;
-    d.tile_start = 0;
-    d.tile_count = g.total_tiles = d.tiles_m * d.tiles_n;
-    ECK(cudaMemcpyAsync(g.dev, &d, sizeof(GemmDesc), cudaMemcpyHostToDevice, h->stream));
+    h->groups[l].host[0].M = n * y.out_h * y.out_w;
+    if (int rc = finalize_tiles(h->groups[l], h->allocs, h->stream)) return rc;
   }
-  ECK(cudaStreamSynchronize(h->stream));     // g.host is pageable
   h->built_n = n;
   return 0;
 }
@@ -163,53 +131,51 @@ int set_batch(b2g_encoder* h, int n) {
 extern "C" {
 
 int b2g_encoder_create(const b2g_encoder_cfg* cfg, b2g_encoder** out) {
-  if (!cfg || !out) return efail(B2G_EINVAL, "null argument");
-  if (cfg->n_layers < 1 || cfg->n_layers > B2G_ENC_MAX_LAYERS) return efail(B2G_EINVAL, "n_layers out of range");
+  if (!cfg || !out) return b2g_fail(B2G_EINVAL, "null argument");
+  if (cfg->n_layers < 1 || cfg->n_layers > B2G_ENC_MAX_LAYERS) return b2g_fail(B2G_EINVAL, "n_layers out of range");
   if (cfg->height < 1 || cfg->width < 1 || cfg->channels < 1 || cfg->encoding_dim < 1 || cfg->max_batch < 1)
-    return efail(B2G_EINVAL, "non-positive dimension");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return efail(B2G_ECUDA, "no CUDA device: libb200grasp has no CPU path");
-  ECK(cudaSetDevice(cfg->device));
+    return b2g_fail(B2G_EINVAL, "non-positive dimension");
+  if (int rc = check_device(cfg->device)) return rc;
   b2g_encoder* h = new b2g_encoder();
   h->cfg = *cfg;
   auto bail = [&](int rc) { b2g_encoder_destroy(h); return rc; };
-  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(efail(B2G_ECUDA, "stream create"));
+  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream create"));
   int ih = cfg->height, iw = cfg->width, ic = cfg->channels;
   for (int l = 0; l < cfg->n_layers; ++l) {
     EncLayer y{};
     y.in_h = ih; y.in_w = iw; y.in_c = ic; y.k = cfg->kernel[l]; y.s = cfg->strides[l]; y.f = cfg->filters[l];
-    if (y.k < 1 || y.s < 1 || y.f < 1) return bail(efail(B2G_EINVAL, "bad conv layer spec"));
+    if (y.k < 1 || y.s < 1 || y.f < 1) return bail(b2g_fail(B2G_EINVAL, "bad conv layer spec"));
     y.out_h = (ih + y.s - 1) / y.s; y.out_w = (iw + y.s - 1) / y.s;
     const int ph = std::max((y.out_h - 1) * y.s + y.k - ih, 0), pw = std::max((y.out_w - 1) * y.s + y.k - iw, 0);
     y.pad_t = ph / 2; y.pad_l = pw / 2; y.hp = ih + ph; y.wp = iw + pw;
     y.fs = (y.f + 3) / 4 * 4;
-    if (l > 0 && (ic & 3)) return bail(efail(B2G_EINVAL, "hidden conv layers need filters % 4 == 0"));
+    if (l > 0 && (ic & 3)) return bail(b2g_fail(B2G_EINVAL, "hidden conv layers need filters % 4 == 0"));
     h->layers.push_back(y);
     ih = y.out_h; iw = y.out_w; ic = y.f;
   }
   EncLayer dn{};
   dn.in_h = ih; dn.in_w = iw; dn.in_c = ic; dn.k = dn.s = 0; dn.f = cfg->encoding_dim; dn.out_h = dn.out_w = 1;
   dn.hp = ih; dn.wp = iw; dn.fs = (dn.f + 3) / 4 * 4;
-  if ((ih * iw * ic) & 3) return bail(efail(B2G_EINVAL, "flattened feature size must be a multiple of 4"));
+  if ((ih * iw * ic) & 3) return bail(b2g_fail(B2G_EINVAL, "flattened feature size must be a multiple of 4"));
   h->layers.push_back(dn);
   const size_t N = cfg->max_batch;
   if (N * (size_t)h->layers[0].hp * h->layers[0].wp * cfg->channels > (1ull << 31) - 1 ||
       N * (size_t)h->layers[0].out_h * h->layers[0].out_w * h->layers[0].fs > (1ull << 31) - 1)
-    return bail(efail(B2G_EINVAL, "max_batch too large for 32-bit offset tables"));
+    return bail(b2g_fail(B2G_EINVAL, "max_batch too large for 32-bit offset tables"));
   int rc;
   for (auto& y : h->layers) {
-    if ((rc = ealloc(h, &y.in, N * y.hp * y.wp * y.in_c))) return bail(rc);
-    if ((rc = ealloc(h, &y.w, (size_t)y.R() * y.fs))) return bail(rc);
-    if ((rc = ealloc(h, &y.b, (size_t)y.fs))) return bail(rc);
+    if ((rc = dev_alloc(h->allocs, h->stream, &y.in, N * y.hp * y.wp * y.in_c))) return bail(rc);
+    if ((rc = dev_alloc(h->allocs, h->stream, &y.w, (size_t)y.R() * y.fs))) return bail(rc);
+    if ((rc = dev_alloc(h->allocs, h->stream, &y.b, (size_t)y.fs))) return bail(rc);
   }
   h->zs = dn.fs;
-  if ((rc = ealloc(h, &h->stage_in, N * cfg->height * cfg->width * cfg->channels))) return bail(rc);
-  if ((rc = ealloc(h, &h->z, N * h->zs))) return bail(rc);
+  if ((rc = dev_alloc(h->allocs, h->stream, &h->stage_in, N * cfg->height * cfg->width * cfg->channels))) return bail(rc);
+  if ((rc = dev_alloc(h->allocs, h->stream, &h->z, N * h->zs))) return bail(rc);
   if (cudaMallocHost(&h->pin_in, N * cfg->height * cfg->width * cfg->channels * sizeof(float)) != cudaSuccess ||
       cudaMallocHost(&h->pin_out, N * cfg->encoding_dim * sizeof(float)) != cudaSuccess)
-    return bail(efail(B2G_ECUDA, "pinned staging allocation failed"));
+    return bail(b2g_fail(B2G_ECUDA, "pinned staging allocation failed"));
   if ((rc = build_tables(h))) return bail(rc);
-  if (cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(efail(B2G_ECUDA, "encoder create sync"));
+  if (cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "encoder create sync"));
   *out = h;
   return 0;
 }
@@ -229,7 +195,7 @@ int b2g_encoder_destroy(b2g_encoder* h) {
 int b2g_encoder_n_layers(const b2g_encoder* h) { return h ? (int)h->layers.size() : -1; }
 
 int b2g_encoder_layer_shape(const b2g_encoder* h, int layer, int64_t* kernel_numel, int64_t* bias_numel) {
-  if (!h || layer < 0 || layer >= (int)h->layers.size()) return efail(B2G_EINVAL, "layer out of range");
+  if (!h || layer < 0 || layer >= (int)h->layers.size()) return b2g_fail(B2G_EINVAL, "layer out of range");
   const EncLayer& y = h->layers[layer];
   if (kernel_numel) *kernel_numel = (int64_t)y.R() * y.f;
   if (bias_numel) *bias_numel = y.f;
@@ -237,40 +203,40 @@ int b2g_encoder_layer_shape(const b2g_encoder* h, int layer, int64_t* kernel_num
 }
 
 int b2g_encoder_set_weights(b2g_encoder* h, int layer, const float* kernel, size_t kernel_numel, const float* bias, size_t bias_numel) {
-  if (!h || !kernel || !bias) return efail(B2G_EINVAL, "null argument");
-  if (layer < 0 || layer >= (int)h->layers.size()) return efail(B2G_EINVAL, "layer out of range");
+  if (!h || !kernel || !bias) return b2g_fail(B2G_EINVAL, "null argument");
+  if (layer < 0 || layer >= (int)h->layers.size()) return b2g_fail(B2G_EINVAL, "layer out of range");
   EncLayer& y = h->layers[layer];
   if (kernel_numel != (size_t)y.R() * y.f || bias_numel != (size_t)y.f)
-    return efail(B2G_EINVAL, "layer " + std::to_string(layer) + ": expected kernel numel " + std::to_string((size_t)y.R() * y.f) +
+    return b2g_fail(B2G_EINVAL, "layer " + std::to_string(layer) + ": expected kernel numel " + std::to_string((size_t)y.R() * y.f) +
                                  ", bias numel " + std::to_string(y.f));
-  ECK(cudaSetDevice(h->cfg.device));
-  ECK(cudaMemcpy2DAsync(y.w, y.fs * sizeof(float), kernel, y.f * sizeof(float), y.f * sizeof(float), y.R(), cudaMemcpyHostToDevice,
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaMemcpy2DAsync(y.w, y.fs * sizeof(float), kernel, y.f * sizeof(float), y.f * sizeof(float), y.R(), cudaMemcpyHostToDevice,
                         h->stream));
-  ECK(cudaMemcpyAsync(y.b, bias, y.f * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  ECK(cudaStreamSynchronize(h->stream));
+  CK(cudaMemcpyAsync(y.b, bias, y.f * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   y.loaded = true;
   return 0;
 }
 
 int b2g_encoder_encode(b2g_encoder* h, const float* imgs, int n, float* out) {
-  if (!h || !imgs || !out) return efail(B2G_EINVAL, "null argument");
-  if (n < 1 || n > h->cfg.max_batch) return efail(B2G_EINVAL, "batch " + std::to_string(n) + " outside [1, max_batch]");
+  if (!h || !imgs || !out) return b2g_fail(B2G_EINVAL, "null argument");
+  if (n < 1 || n > h->cfg.max_batch) return b2g_fail(B2G_EINVAL, "batch " + std::to_string(n) + " outside [1, max_batch]");
   for (size_t l = 0; l < h->layers.size(); ++l)
-    if (!h->layers[l].loaded) return efail(B2G_ESTATE, "encoder layer " + std::to_string(l) + " has no weights (load_weights first)");
-  ECK(cudaSetDevice(h->cfg.device));
+    if (!h->layers[l].loaded) return b2g_fail(B2G_ESTATE, "encoder layer " + std::to_string(l) + " has no weights (load_weights first)");
+  CK(cudaSetDevice(h->cfg.device));
   if (int rc = set_batch(h, n)) return rc;
   const EncLayer& y0 = h->layers[0];
   const size_t in_numel = (size_t)n * h->cfg.height * h->cfg.width * h->cfg.channels;
   memcpy(h->pin_in, imgs, in_numel * sizeof(float));
-  ECK(cudaMemcpyAsync(h->stage_in, h->pin_in, in_numel * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(h->stage_in, h->pin_in, in_numel * sizeof(float), cudaMemcpyHostToDevice, h->stream));
   const int blocks = (int)std::min<size_t>((in_numel + 255) / 256, 132 * 8);
   enc_pad_copy<<<blocks, 256, 0, h->stream>>>(h->stage_in, y0.in, n, h->cfg.height, h->cfg.width, h->cfg.channels, y0.hp, y0.wp,
                                               y0.pad_t, y0.pad_l);
   for (auto& g : h->groups) gg_simt_launch(g.dev, 1, g.total_tiles, h->stream);
-  ECK(cudaGetLastError());
-  ECK(cudaMemcpy2DAsync(h->pin_out, h->cfg.encoding_dim * sizeof(float), h->z, h->zs * sizeof(float),
+  CK(cudaGetLastError());
+  CK(cudaMemcpy2DAsync(h->pin_out, h->cfg.encoding_dim * sizeof(float), h->z, h->zs * sizeof(float),
                         h->cfg.encoding_dim * sizeof(float), n, cudaMemcpyDeviceToHost, h->stream));
-  ECK(cudaStreamSynchronize(h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   memcpy(out, h->pin_out, (size_t)n * h->cfg.encoding_dim * sizeof(float));
   return 0;
 }

@@ -216,16 +216,6 @@ __global__ void __launch_bounds__(256) planes2_kernel(const Plane2Job* __restric
 }
 
 // ------------------------------------------------------------------------------------------------ host helpers
-template <class T>
-int valloc(b2g_sac* h, T** ptr, size_t count) {
-  void* q = nullptr;
-  B2G_CK(cudaMalloc(&q, std::max<size_t>(count, 1) * sizeof(T)));
-  B2G_CK(cudaMemsetAsync(q, 0, std::max<size_t>(count, 1) * sizeof(T), h->stream));
-  h->allocs.push_back(q);
-  *ptr = (T*)q;
-  return 0;
-}
-
 // ONE map over the np equidistant planes of a tensor: the given geometry plus an outermost plane dimension.  The box covers all
 // planes (one instruction fetches them, stacked plane after plane in shared memory) when one plane's box is a whole number of
 // 1024-byte swizzle atoms, else one plane (an instruction per plane, plane = last coordinate).  Distinct maps per plane cost a
@@ -377,24 +367,24 @@ int v2_alloc(b2g_sac* h) {
   const size_t n1 = (size_t)B * 225 * 32, n2 = (size_t)B * 36 * 64, n3 = (size_t)B * 1024, na = (size_t)B * 225 * K1, nf = (size_t)B * KF;
   // ---- activations: one block per layer, [net][plane] with uniform strides (conv1 writes two nets from one tile)
   uint16_t *bH1, *bH2, *bH3, *bF, *bA1;
-  if (int rc = valloc(h, &bH1, 9 * n1)) return rc;
-  if (int rc = valloc(h, &bH2, 9 * n2)) return rc;
-  if (int rc = valloc(h, &bH3, 9 * n3)) return rc;
-  if (int rc = valloc(h, &bF, 9 * nf)) return rc;
-  if (int rc = valloc(h, &bA1, 6 * na)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &bH1, 9 * n1)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &bH2, 9 * n2)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &bH3, 9 * n3)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &bF, 9 * nf)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &bA1, 6 * na)) return rc;
   for (int n = 0; n < 3; ++n)
     for (int p = 0; p < 3; ++p) {
       v.H1[n][p] = bH1 + (n * 3 + p) * n1; v.H2[n][p] = bH2 + (n * 3 + p) * n2; v.H3[n][p] = bH3 + (n * 3 + p) * n3;
       v.F[n][p] = bF + (n * 3 + p) * nf;
     }
   for (int w = 0; w < 2; ++w) for (int p = 0; p < 3; ++p) v.A1[w][p] = bA1 + (w * 3 + p) * na;
-  if (int rc = valloc(h, &v.z0v, (size_t)B * 192)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &v.z0v, (size_t)B * 192)) return rc;
   // ---- gradient maps (2 planes) and natural-layout weight planes of the backward chain.  The planes of a tensor are
   //      equidistant in one allocation: the tensor maps address them through an extra (outermost) plane dimension
   auto palloc = [&](uint16_t** arr, int np, size_t count) -> int {
     const size_t pitch = (count + 63) / 64 * 64;
     uint16_t* base = nullptr;
-    if (int rc = valloc(h, &base, pitch * np)) return rc;
+    if (int rc = dev_alloc(h->allocs, h->stream, &base, pitch * np)) return rc;
     for (int p = 0; p < np; ++p) arr[p] = base + p * pitch;
     return 0;
   };
@@ -463,18 +453,15 @@ int v2_create(b2g_sac* h) {
   v.n_plane_jobs = (int)jobs.size();
   v.plane_ctas = start;
   Plane2Job* dj = nullptr;
-  if (int rc = valloc(h, &dj, jobs.size())) return rc;
-  B2G_CK(cudaMemcpyAsync(dj, jobs.data(), jobs.size() * sizeof(Plane2Job), cudaMemcpyHostToDevice, h->stream));
-  B2G_CK(cudaStreamSynchronize(h->stream));
+  if (int rc = dev_alloc(h->allocs, h->stream, &dj, jobs.size())) return rc;
+  CK(cudaMemcpyAsync(dj, jobs.data(), jobs.size() * sizeof(Plane2Job), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   v.plane_jobs = dj;
   {
     std::vector<int> cj((size_t)start);
     for (size_t k = 0; k < jobs.size(); ++k)
       for (int t = jobs[k].tile_start; t < (k + 1 < jobs.size() ? jobs[k + 1].tile_start : start); ++t) cj[t] = (int)k;
-    int* dcj = nullptr;
-    if (int rc = valloc(h, &dcj, cj.size())) return rc;
-    B2G_CK(cudaMemcpy(dcj, cj.data(), cj.size() * sizeof(int), cudaMemcpyHostToDevice));
-    v.plane_cta_job = dcj;
+    if (int rc = upload_table(h->allocs, h->stream, cj, &v.plane_cta_job)) return rc;
   }
 
   { const char* e = getenv("B2G_SPLIT_FC1"); v.split_fc1 = e ? std::max(1, atoi(e)) : 3; }
@@ -567,8 +554,8 @@ int v2_create(b2g_sac* h) {
         // 48 tiles of 16 K-chunks would hold 48 of the 132 SMs for the longest stretch of the forward launch: three K-splits per
         // tile, fp32 partial sums in a workspace, the last split to arrive finishes the tile (cg.cuh: ws)
         P.splits = v.split_fc1;
-        if (int rc = valloc(h, &P.ws, (size_t)P.tiles_m * P.tiles_n * 128 * 64)) return rc;
-        if (int rc = valloc(h, &P.ws_cnt, (size_t)P.tiles_m * P.tiles_n * CG_EPI_WARPS)) return rc;
+        if (int rc = dev_alloc(h->allocs, h->stream, &P.ws, (size_t)P.tiles_m * P.tiles_n * 128 * 64)) return rc;
+        if (int rc = dev_alloc(h->allocs, h->stream, &P.ws_cnt, (size_t)P.tiles_m * P.tiles_n * CG_EPI_WARPS)) return rc;
       }
       g.host[g.n++] = P;
     }
@@ -642,8 +629,8 @@ int v2_create(b2g_sac* h) {
         P.colsum = h->g(std::string(nets[n]) + "/cnn3/b"); P.colsum_mask = 63;     // dZ3 row = [16 pixels][64 channels]
         if (v.split_fc1_dgrad > 1) {         // 32 tiles of 8 K-chunks at the head of the backward chain: split-K with finalisation
           P.splits = v.split_fc1_dgrad;
-          if (int rc = valloc(h, &P.ws, (size_t)P.tiles_m * P.tiles_n * 128 * 128)) return rc;
-          if (int rc = valloc(h, &P.ws_cnt, (size_t)P.tiles_m * P.tiles_n * CG_EPI_WARPS)) return rc;
+          if (int rc = dev_alloc(h->allocs, h->stream, &P.ws, (size_t)P.tiles_m * P.tiles_n * 128 * 128)) return rc;
+          if (int rc = dev_alloc(h->allocs, h->stream, &P.ws_cnt, (size_t)P.tiles_m * P.tiles_n * CG_EPI_WARPS)) return rc;
         }
         g.host[g.n++] = P;
       }
@@ -674,9 +661,8 @@ int v2_create(b2g_sac* h) {
         const int pos = 2 * tm + a;
         tab[(tm * CG_MAX_LOADS + a) * 2] = pos % 3; tab[(tm * CG_MAX_LOADS + a) * 2 + 1] = pos / 3;
       }
-    int* dtab = nullptr;
-    if (int rc = valloc(h, &dtab, tab.size())) return rc;
-    B2G_CK(cudaMemcpy(dtab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice));
+    const int* dtab = nullptr;
+    if (int rc = upload_table(h->allocs, h->stream, tab, &dtab)) return rc;
     for (int n = 0; n < 2; ++n) {
       {
         const int mA = add_maps(v, v.dZ3[n], NB, 4, {64, 4, 4, (uint64_t)B}, {128, 512, 2048}, {64, 6, 6, 3});
@@ -834,13 +820,13 @@ int v2_create(b2g_sac* h) {
     if (int rc = fuse_groups(h, pa, wa, "bwd_fused_fc", v.bwd_fused, n_ctr)) return rc;
     if (int rc = fuse_groups(h, pb, wb, "bwd_fused_conv", v.bwd_fused, n_ctr)) return rc;
   }
-  if (int rc = valloc(h, &v.dep_ctr, (size_t)n_ctr)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &v.dep_ctr, (size_t)n_ctr)) return rc;
   v.n_dep_ctr = n_ctr;
   bind_counters(v.fwd_fused, v.dep_ctr);
   bind_counters(v.bwd_fused, v.dep_ctr);
-  if (int rc = valloc(h, &v.d_maps, v.maps.size())) return rc;
-  B2G_CK(cudaMemcpyAsync(v.d_maps, v.maps.data(), v.maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice, h->stream));
-  B2G_CK(cudaStreamSynchronize(h->stream));
+  if (int rc = dev_alloc(h->allocs, h->stream, &v.d_maps, v.maps.size())) return rc;
+  CK(cudaMemcpyAsync(v.d_maps, v.maps.data(), v.maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   return 0;
 }
 
@@ -867,7 +853,7 @@ int v2_gather(b2g_sac* h, const GatherArgs& ga, cudaStream_t s) {
   const size_t smem = (size_t)3 * h->Hi * (h->Wi * h->Cimg + 8) * sizeof(uint16_t);
   static size_t attr = 0;
   if (smem > attr) {
-    B2G_CK(cudaFuncSetAttribute(gather2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(cudaFuncSetAttribute(gather2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = smem;
   }
   gather2_kernel<<<dim3(ga.B, ga.next_obs ? 2 : 1), 512, smem, s>>>(a);
@@ -906,7 +892,7 @@ int v2_launch(b2g_sac* h, const CgGroup& g, cudaStream_t s) {
     }
     return 0;
   }
-  B2G_CK(cg_launch(g, h->v2.d_maps, h->num_sms - h->v2.sm_reserve, s, pdl_enabled(), h->v2.dbg));
+  CK(cg_launch(g, h->v2.d_maps, h->num_sms - h->v2.sm_reserve, s, pdl_enabled(), h->v2.dbg));
   return 0;
 }
 

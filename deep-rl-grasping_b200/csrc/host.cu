@@ -1,0 +1,154 @@
+// libb200grasp: host runtime shared by the SAC, BDQ and encoder handles (declarations and contracts in host.cuh), and the
+// library-wide part of the C ABI.
+#include <cuda_runtime.h>
+#include <dlfcn.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include "host.cuh"
+
+thread_local std::string g_b2g_err;
+int b2g_fail(int code, const std::string& msg) { g_b2g_err = msg; return code; }
+
+namespace b2g {
+
+int check_device(int device, int* num_sms) {
+  int ndev = 0;
+  CK(cudaGetDeviceCount(&ndev));
+  if (device < 0 || device >= ndev) return b2g_fail(B2G_ECUDA, "no such CUDA device");
+  CK(cudaSetDevice(device));
+  cudaDeviceProp prop{};
+  CK(cudaGetDeviceProperties(&prop, device));
+  if (prop.major != 9) return b2g_fail(B2G_ECUDA, std::string("libb200grasp is built for sm_90a only; found ") + prop.name);
+  if (num_sms) *num_sms = prop.multiProcessorCount;
+  return 0;
+}
+
+int upload_table(std::vector<void*>& allocs, cudaStream_t s, const std::vector<int>& v, const int** out,
+                 std::map<const int*, std::vector<int>>* host_copy) {
+  int* d = nullptr;
+  if (int rc = dev_alloc(allocs, s, &d, v.size(), false)) return rc;
+  CK(cudaMemcpyAsync(d, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  CK(cudaStreamSynchronize(s));
+  *out = d;
+  if (host_copy) (*host_copy)[d] = v;
+  return 0;
+}
+
+std::vector<int> iota_tab(int n, int stride, int base) {
+  std::vector<int> v(n);
+  for (int i = 0; i < n; ++i) v[i] = base + i * stride;
+  return v;
+}
+
+GemmDesc gemm_desc(const float* A, const int* aM, const int* aR, const float* B, const int* bR, const int* bN, float* C,
+                   const int* cM, const int* cN, int M, int N, int R, int flags, int splitR) {
+  GemmDesc d{};
+  d.A = A; d.B = B; d.C = C; d.aM = aM; d.aR = aR; d.bR = bR; d.bN = bN; d.cM = cM; d.cN = cN;
+  d.M = M; d.N = N; d.R = R; d.flags = flags; d.splitR = splitR; d.alpha = 1.f;
+  return d;
+}
+
+int finalize_tiles(GemmGroup& g, std::vector<void*>& allocs, cudaStream_t s, int bm, int bn) {
+  int start = 0;
+  for (auto& d : g.host) {
+    d.tiles_m = (d.M + bm - 1) / bm;
+    d.tiles_n = (d.N + bn - 1) / bn;
+    d.tile_start = start;
+    d.tile_count = d.tiles_m * d.tiles_n * d.splitR;
+    start += d.tile_count;
+  }
+  g.total_tiles = start;
+  if (!g.dev)
+    if (int rc = dev_alloc(allocs, s, &g.dev, g.host.size(), false)) return rc;
+  CK(cudaMemcpyAsync(g.dev, g.host.data(), g.host.size() * sizeof(GemmDesc), cudaMemcpyHostToDevice, s));
+  CK(cudaStreamSynchronize(s));     // g.host is pageable
+  return 0;
+}
+
+int capture_graph(cudaStream_t s, const std::function<int()>& issue, cudaGraphExec_t* exec) {
+  cudaGraph_t graph = nullptr;
+  CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+  const int rc = issue();
+  const cudaError_t e = cudaStreamEndCapture(s, &graph);
+  if (rc || e != cudaSuccess) {
+    if (graph) cudaGraphDestroy(graph);
+    return rc ? rc : b2g_fail(B2G_ECUDA, std::string("graph capture failed: ") + cudaGetErrorString(e));
+  }
+  const cudaError_t e2 = cudaGraphInstantiate(exec, graph, 0);
+  cudaGraphDestroy(graph);
+  if (e2 != cudaSuccess) return b2g_fail(B2G_ECUDA, std::string("graph instantiate failed: ") + cudaGetErrorString(e2));
+  return 0;
+}
+
+int upload_lr(float* d_lr, float* cur_lr, float lr, cudaStream_t s) {
+  if (lr != *cur_lr) {
+    CK(cudaStreamSynchronize(s));
+    CK(cudaMemcpy(d_lr, &lr, sizeof(float), cudaMemcpyHostToDevice));
+    *cur_lr = lr;
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ NCCL
+NcclApi g_nccl;
+
+int load_nccl(const char* path) {
+  if (g_nccl.lib) return 0;
+  const char* cands[] = {path, "libnccl.so.2", "libnccl.so", "/usr/lib/x86_64-linux-gnu/libnccl.so.2"};
+  for (const char* c : cands) {
+    if (!c || !*c) continue;
+    g_nccl.lib = dlopen(c, RTLD_NOW | RTLD_GLOBAL);
+    if (g_nccl.lib) break;
+  }
+  if (!g_nccl.lib) return b2g_fail(B2G_ENCCL, std::string("cannot dlopen libnccl: ") + dlerror());
+  g_nccl.GetUniqueId = (int (*)(void*))dlsym(g_nccl.lib, "ncclGetUniqueId");
+  g_nccl.CommInitRank = (int (*)(void**, int, NcclUniqueId, int))dlsym(g_nccl.lib, "ncclCommInitRank");
+  g_nccl.AllReduce = (int (*)(const void*, void*, size_t, int, int, void*, cudaStream_t))dlsym(g_nccl.lib, "ncclAllReduce");
+  g_nccl.CommDestroy = (int (*)(void*))dlsym(g_nccl.lib, "ncclCommDestroy");
+  g_nccl.GetErrorString = (const char* (*)(int))dlsym(g_nccl.lib, "ncclGetErrorString");
+  g_nccl.CommSplit = (int (*)(void*, int, int, void**, void*))dlsym(g_nccl.lib, "ncclCommSplit");
+  g_nccl.GroupStart = (int (*)())dlsym(g_nccl.lib, "ncclGroupStart");
+  g_nccl.GroupEnd = (int (*)())dlsym(g_nccl.lib, "ncclGroupEnd");
+  if (!g_nccl.GetUniqueId || !g_nccl.CommInitRank || !g_nccl.AllReduce)
+    return b2g_fail(B2G_ENCCL, "libnccl is missing symbols");
+  return 0;
+}
+
+int nccl_comm_init(void** comm, int nranks, const void* id128, int rank, const char* lib) {
+  if (int rc = load_nccl(lib)) return rc;
+  NcclUniqueId id;
+  memcpy(id.b, id128, 128);
+  // (B2G_AR_SMS also caps NCCL's CTAs: a collective that overlaps the persistent GEMM grids -- one CTA per SM, 226 KB of shared
+  //  memory each, nothing fits beside them -- displaces every GEMM CTA beyond the reserve.  Measured at N = 2: capping at 8 CTAs
+  //  halves the all-reduce bandwidth and costs more than it saves, so the cap is opt-in.)
+  if (!getenv("NCCL_MAX_CTAS")) { if (const char* e = getenv("B2G_AR_SMS")) setenv("NCCL_MAX_CTAS", e, 0); }
+  const int nrc = g_nccl.CommInitRank(comm, nranks, id, rank);
+  if (nrc != 0) return b2g_fail(B2G_ENCCL, std::string("ncclCommInitRank: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(nrc) : "?"));
+  return 0;
+}
+int nccl_allreduce_sum_f32(void* comm, float* buf, size_t count, cudaStream_t s) {
+  const int nrc = g_nccl.AllReduce(buf, buf, count, /*ncclFloat32*/ 7, /*ncclSum*/ 0, comm, s);
+  if (nrc != 0) return b2g_fail(B2G_ENCCL, std::string("ncclAllReduce: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(nrc) : "?"));
+  return 0;
+}
+void nccl_comm_destroy(void* comm) { if (comm && g_nccl.CommDestroy) g_nccl.CommDestroy(comm); }
+
+}  // namespace b2g
+
+using namespace b2g;
+
+extern "C" {
+
+const char* b2g_last_error(void) { return g_b2g_err.c_str(); }
+int b2g_version(void) { return 100; }
+
+int b2g_nccl_unique_id(void* out128, const char* nccl_lib) {
+  if (!out128) return b2g_fail(B2G_EINVAL, "out128 is NULL");
+  if (int rc = load_nccl(nccl_lib)) return rc;
+  int rc = g_nccl.GetUniqueId(out128);
+  if (rc != 0) return b2g_fail(B2G_ENCCL, "ncclGetUniqueId failed");
+  return 0;
+}
+
+}  // extern "C"

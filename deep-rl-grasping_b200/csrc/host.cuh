@@ -1,0 +1,83 @@
+// Host runtime shared by the SAC, BDQ and encoder handles (host.cu): error state, device check, tracked device allocations,
+// offset tables, gather-GEMM descriptor groups, CUDA-graph capture, learning-rate upload and NCCL through dlopen.
+#pragma once
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <functional>
+#include <map>
+#include <string>
+#include <vector>
+
+#include "../../include/b200grasp.h"
+#include "common.cuh"
+
+// Text behind b2g_last_error(): b2g_fail sets it and returns `code`.
+extern thread_local std::string g_b2g_err;
+int b2g_fail(int code, const std::string& msg);
+// Returns B2G_ECUDA from the enclosing function when a CUDA runtime call fails.
+#define CK(call)                                                                                  \
+  do {                                                                                            \
+    cudaError_t e_ = (call);                                                                      \
+    if (e_ != cudaSuccess)                                                                        \
+      return b2g_fail(B2G_ECUDA, std::string(#call) + ": " + cudaGetErrorString(e_) + " @" + __FILE__ + ":" + \
+                                     std::to_string(__LINE__));                                   \
+  } while (0)
+
+namespace b2g {
+
+// The device exists, is made current and is a Hopper part (sm_90); *num_sms receives its SM count when asked for.
+int check_device(int device, int* num_sms = nullptr);
+
+// `count` elements of T (at least one) on the device, zeroed on stream s unless zero == false.  The pointer joins `allocs`,
+// which the owning handle frees on destroy.
+template <class T>
+int dev_alloc(std::vector<void*>& allocs, cudaStream_t s, T** ptr, size_t count, bool zero = true) {
+  void* q = nullptr;
+  CK(cudaMalloc(&q, std::max<size_t>(count, 1) * sizeof(T)));
+  allocs.push_back(q);
+  if (zero) CK(cudaMemsetAsync(q, 0, std::max<size_t>(count, 1) * sizeof(T), s));
+  *ptr = (T*)q;
+  return 0;
+}
+
+// Offset table -> device, synchronously (v may be a temporary).  host_copy, when given, keeps v under the device pointer.
+int upload_table(std::vector<void*>& allocs, cudaStream_t s, const std::vector<int>& v, const int** out,
+                 std::map<const int*, std::vector<int>>* host_copy = nullptr);
+std::vector<int> iota_tab(int n, int stride = 1, int base = 0);     // base + i * stride
+
+// C[cM[m] + cN[n]] = sum_r A[aM[m] + aR[r]] * B[bR[r] + bN[n]] with the given flags; every optional operand unset, alpha = 1
+GemmDesc gemm_desc(const float* A, const int* aM, const int* aR, const float* B, const int* bR, const int* bN, float* C,
+                   const int* cM, const int* cN, int M, int N, int R, int flags, int splitR = 1);
+// Tile grid of every descriptor of a grouped launch (bm x bn output tiles, splitR slices each), their tile_start / tile_count
+// and the group's total_tiles; then the descriptors are copied to g.dev (allocated on the first call), synchronously.
+int finalize_tiles(GemmGroup& g, std::vector<void*>& allocs, cudaStream_t s, int bm = GG_SIMT_BM, int bn = GG_SIMT_BN);
+
+// Captures what issue() enqueues on s into a graph and instantiates it into *exec.  A failing issue() ends the capture and
+// returns its code.
+int capture_graph(cudaStream_t s, const std::function<int()>& issue, cudaGraphExec_t* exec);
+
+// Learning rate -> the device scalar the prep kernel reads; only when it changed (the stream is drained first).
+int upload_lr(float* d_lr, float* cur_lr, float lr, cudaStream_t s);
+
+// ---- NCCL through dlopen (no link-time dependency: the library loads on machines without NCCL or a GPU)
+struct NcclUniqueId { char b[128]; };
+struct NcclApi {
+  void* lib = nullptr;
+  int (*GetUniqueId)(void*) = nullptr;
+  int (*CommInitRank)(void**, int, NcclUniqueId, int) = nullptr;
+  int (*AllReduce)(const void*, void*, size_t, int, int, void*, cudaStream_t) = nullptr;
+  int (*CommDestroy)(void*) = nullptr;
+  int (*CommSplit)(void*, int, int, void**, void*) = nullptr;
+  int (*GroupStart)() = nullptr;
+  int (*GroupEnd)() = nullptr;
+  const char* (*GetErrorString)(int) = nullptr;
+};
+extern NcclApi g_nccl;
+int load_nccl(const char* path);
+// 0 or a negative B2G_E* code with b2g_last_error() set
+int nccl_comm_init(void** comm, int nranks, const void* id128, int rank, const char* lib);
+int nccl_allreduce_sum_f32(void* comm, float* buf, size_t count, cudaStream_t s);
+void nccl_comm_destroy(void* comm);
+
+}  // namespace b2g

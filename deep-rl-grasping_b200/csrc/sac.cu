@@ -14,7 +14,6 @@
 // launch); every other configuration, and policy inference, runs them as grouped launches of the
 // round-1 engines (gg_tc.cu, gg_simt.cu).
 #include <cuda_runtime.h>
-#include <dlfcn.h>
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -40,110 +39,9 @@ bool pdl_enabled() {
 }
 }  // namespace b2g
 
-thread_local std::string g_b2g_err;     // shared with bdq.cu
-#define g_err g_b2g_err
-int b2g_fail(int code, const std::string& msg) { g_b2g_err = msg; return code; }
-static int fail(int code, const std::string& msg) { return b2g_fail(code, msg); }
-#define CK(call)                                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess)                                                                        \
-      return fail(B2G_ECUDA, std::string(#call) + ": " + cudaGetErrorString(e_) + " @" + __FILE__ + ":" + \
-                                 std::to_string(__LINE__));                                       \
-  } while (0)
-
-// ------------------------------------------------------------------------------------------------
-// NCCL through dlopen (no link-time dependency; the library loads on boxes without NCCL/GPU)
-// ------------------------------------------------------------------------------------------------
 namespace {
-struct UId { char b[128]; };   // ncclUniqueId
-struct NcclApi {
-  void* lib = nullptr;
-  int (*GetUniqueId)(void*) = nullptr;
-  int (*CommInitRank)(void**, int, UId, int) = nullptr;
-  int (*AllReduce)(const void*, void*, size_t, int, int, void*, cudaStream_t) = nullptr;
-  int (*CommDestroy)(void*) = nullptr;
-  int (*CommSplit)(void*, int, int, void**, void*) = nullptr;
-  int (*GroupStart)() = nullptr;
-  int (*GroupEnd)() = nullptr;
-  const char* (*GetErrorString)(int) = nullptr;
-};
-NcclApi g_nccl;
-
-int load_nccl(const char* path) {
-  if (g_nccl.lib) return 0;
-  const char* cands[] = {path, "libnccl.so.2", "libnccl.so", "/usr/lib/x86_64-linux-gnu/libnccl.so.2"};
-  for (const char* c : cands) {
-    if (!c || !*c) continue;
-    g_nccl.lib = dlopen(c, RTLD_NOW | RTLD_GLOBAL);
-    if (g_nccl.lib) break;
-  }
-  if (!g_nccl.lib) return fail(B2G_ENCCL, std::string("cannot dlopen libnccl: ") + dlerror());
-  g_nccl.GetUniqueId = (int (*)(void*))dlsym(g_nccl.lib, "ncclGetUniqueId");
-  g_nccl.CommInitRank = (int (*)(void**, int, UId, int))dlsym(g_nccl.lib, "ncclCommInitRank");
-  g_nccl.AllReduce = (int (*)(const void*, void*, size_t, int, int, void*, cudaStream_t))dlsym(g_nccl.lib, "ncclAllReduce");
-  g_nccl.CommDestroy = (int (*)(void*))dlsym(g_nccl.lib, "ncclCommDestroy");
-  g_nccl.GetErrorString = (const char* (*)(int))dlsym(g_nccl.lib, "ncclGetErrorString");
-  g_nccl.CommSplit = (int (*)(void*, int, int, void**, void*))dlsym(g_nccl.lib, "ncclCommSplit");
-  g_nccl.GroupStart = (int (*)())dlsym(g_nccl.lib, "ncclGroupStart");
-  g_nccl.GroupEnd = (int (*)())dlsym(g_nccl.lib, "ncclGroupEnd");
-  if (!g_nccl.GetUniqueId || !g_nccl.CommInitRank || !g_nccl.AllReduce)
-    return fail(B2G_ENCCL, "libnccl is missing symbols");
-  return 0;
-}
 
 int64_t pad32(int64_t n) { return (n + 31) / 32 * 32; }
-}  // namespace
-
-// NCCL plumbing shared with bdq.cu (common.cuh declares these)
-namespace b2g {
-int nccl_comm_init(void** comm, int nranks, const void* id128, int rank, const char* lib) {
-  if (int rc = load_nccl(lib)) return rc;
-  UId id;
-  memcpy(id.b, id128, 128);
-  // (B2G_AR_SMS also caps NCCL's CTAs: a collective that overlaps the persistent GEMM grids -- one CTA per SM, 226 KB of shared
-  //  memory each, nothing fits beside them -- displaces every GEMM CTA beyond the reserve.  Measured at N = 2: capping at 8 CTAs
-  //  halves the all-reduce bandwidth and costs more than it saves, so the cap is opt-in.)
-  if (!getenv("NCCL_MAX_CTAS")) { if (const char* e = getenv("B2G_AR_SMS")) setenv("NCCL_MAX_CTAS", e, 0); }
-  const int nrc = g_nccl.CommInitRank(comm, nranks, id, rank);
-  if (nrc != 0) return fail(B2G_ENCCL, std::string("ncclCommInitRank: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(nrc) : "?"));
-  return 0;
-}
-int nccl_allreduce_sum_f32(void* comm, float* buf, size_t count, cudaStream_t s) {
-  const int nrc = g_nccl.AllReduce(buf, buf, count, /*ncclFloat32*/ 7, /*ncclSum*/ 0, comm, s);
-  if (nrc != 0) return fail(B2G_ENCCL, std::string("ncclAllReduce: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(nrc) : "?"));
-  return 0;
-}
-void nccl_comm_destroy(void* comm) { if (comm && g_nccl.CommDestroy) g_nccl.CommDestroy(comm); }
-}  // namespace b2g
-
-namespace {
-
-template <class T>
-int dalloc(b2g_sac* h, T** ptr, size_t count, bool zero = true) {
-  void* q = nullptr;
-  CK(cudaMalloc(&q, std::max<size_t>(count, 1) * sizeof(T)));
-  if (zero) CK(cudaMemsetAsync(q, 0, std::max<size_t>(count, 1) * sizeof(T), h->stream));
-  h->allocs.push_back(q);
-  *ptr = (T*)q;
-  return 0;
-}
-
-int upload_table(b2g_sac* h, const std::vector<int>& v, const int** out) {
-  int* d = nullptr;
-  if (int rc = dalloc(h, &d, v.size(), false)) return rc;
-  CK(cudaMemcpyAsync(d, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  CK(cudaStreamSynchronize(h->stream));   // v may be a temporary
-  *out = d;
-  h->host_tabs[d] = v;
-  return 0;
-}
-
-std::vector<int> iota_tab(int n, int stride = 1, int base = 0) {
-  std::vector<int> v(n);
-  for (int i = 0; i < n; ++i) v[i] = base + i * stride;
-  return v;
-}
 
 void add_tensor(b2g_sac* h, const std::string& name, std::vector<int64_t> shape, int group) {
   Tensor t;
@@ -217,21 +115,11 @@ void build_params(b2g_sac* h) {
   h->n_all = off;
 }
 
-GemmDesc mk(const float* A, const int* aM, const int* aR, const float* B, const int* bR, const int* bN, float* C,
-            const int* cM, const int* cN, int M, int N, int R, int flags, int splitR = 1) {
-  GemmDesc d{};
-  d.A = A; d.B = B; d.C = C; d.aM = aM; d.aR = aR; d.bR = bR; d.bN = bN; d.cM = cM; d.cN = cN;
-  d.M = M; d.N = N; d.R = R; d.flags = flags; d.splitR = splitR;
-  return d;
-}
-
+// SAC's passes over a group before the shared tile layout: GG_CN_AFFINE4, split-R, column-table ids, flops
 int finalize_group(b2g_sac* h, GemmGroup& g) {
-  int start = 0;
   g.flops = 0;
   const int bm = g.tc ? GG_TC_BM : GG_SIMT_BM, bn = g.tc ? GG_TC_BN : GG_SIMT_BN, bk = g.tc ? GG_TC_BK : GG_SIMT_BK;
   for (auto& d : g.host) {
-    d.tiles_m = (d.M + bm - 1) / bm;
-    d.tiles_n = (d.N + bn - 1) / bn;
     {   // GG_CN_AFFINE4: column tables contiguous in aligned groups of 4, row offsets multiples of 4
       auto grp4 = [&](const int* tab, int n) {
         auto it = h->host_tabs.find(tab);
@@ -252,7 +140,7 @@ int finalize_group(b2g_sac* h, GemmGroup& g) {
       if (ok) d.flags |= GG_CN_AFFINE4;
     }
     if (d.flags & GG_EPI_ATOMIC) {     // split-R sized for this engine's tile grid
-      const int tiles = d.tiles_m * d.tiles_n;
+      const int tiles = ((d.M + bm - 1) / bm) * ((d.N + bn - 1) / bn);
       int sp = std::max(1, h->num_sms / std::max(1, tiles));
       sp = std::min(sp, std::max(1, d.R / (2 * bk)));
       d.splitR = sp;
@@ -264,16 +152,9 @@ int finalize_group(b2g_sac* h, GemmGroup& g) {
       if (it == h->col_ids.end()) it = h->col_ids.emplace(key, (int)h->col_ids.size()).first;
       d.col_id = it->second;
     }
-    d.tile_start = start;
-    d.tile_count = d.tiles_m * d.tiles_n * d.splitR;
-    start += d.tile_count;
     g.flops += 2.0 * d.M * d.N * d.R;
   }
-  g.total_tiles = start;
-  if (int rc = dalloc(h, &g.dev, g.host.size(), false)) return rc;
-  CK(cudaMemcpyAsync(g.dev, g.host.data(), g.host.size() * sizeof(GemmDesc), cudaMemcpyHostToDevice, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return 0;
+  return finalize_tiles(g, h->allocs, h->stream, bm, bn);
 }
 
 int split_for(int tiles, int R, int target_ctas = 132) {
@@ -284,7 +165,7 @@ int split_for(int tiles, int R, int target_ctas = 132) {
 
 #define TAB(var, vec)                                         \
   const int* var = nullptr;                                   \
-  if (int rc_ = upload_table(h, (vec), &var)) return rc_;
+  if (int rc_ = upload_table(h->allocs, h->stream, (vec), &var, &h->host_tabs)) return rc_;
 
 int build_groups(b2g_sac* h) {
   const int B = h->B, A = h->A, H = h->H, FS = h->FS, fd = h->feat_dim;
@@ -317,10 +198,10 @@ int build_groups(b2g_sac* h) {
       for (int ky = 0; ky < c.k; ++ky)
         for (int kx = 0; kx < c.k; ++kx)
           for (int ci = 0; ci < c.Ci; ++ci) ko[(ky * c.k + kx) * c.Ci + ci] = (ky * c.Wi + kx) * c.Ci + ci;
-      if (int rc = upload_table(h, ro, &rowoff[l])) return rc;
-      if (int rc = upload_table(h, ko, &koff[l])) return rc;
-      if (int rc = upload_table(h, iota_tab(c.k * c.k * c.Ci, c.Co), &wrow[l])) return rc;
-      if (int rc = upload_table(h, iota_tab(B * c.Ho * c.Wo, c.Co), &crow[l])) return rc;
+      if (int rc = upload_table(h->allocs, h->stream, ro, &rowoff[l], &h->host_tabs)) return rc;
+      if (int rc = upload_table(h->allocs, h->stream, ko, &koff[l], &h->host_tabs)) return rc;
+      if (int rc = upload_table(h->allocs, h->stream, iota_tab(c.k * c.k * c.Ci, c.Co), &wrow[l], &h->host_tabs)) return rc;
+      if (int rc = upload_table(h->allocs, h->stream, iota_tab(B * c.Ho * c.Wo, c.Co), &crow[l], &h->host_tabs)) return rc;
     }
     TAB(fcA, iota_tab(B, 1024));
     TAB(fcW, iota_tab(1024, 512));
@@ -329,8 +210,8 @@ int build_groups(b2g_sac* h) {
     {
       const int Rs[4] = {64 * Ci, 512, 576, 1024}, Ns[4] = {32, 64, 64, 512};
       for (int l = 0; l < 4; ++l) {
-        if (int rc = upload_table(h, iota_tab(Rs[l]), &wT_r[l])) return rc;
-        if (int rc = upload_table(h, iota_tab(Ns[l], Rs[l]), &wT_n[l])) return rc;
+        if (int rc = upload_table(h->allocs, h->stream, iota_tab(Rs[l]), &wT_r[l], &h->host_tabs)) return rc;
+        if (int rc = upload_table(h->allocs, h->stream, iota_tab(Ns[l], Rs[l]), &wT_n[l], &h->host_tabs)) return rc;
       }
     }
     // ================= forward groups
@@ -342,7 +223,7 @@ int build_groups(b2g_sac* h) {
       for (int n = 0; n < 3; ++n) {
         const float* in = l == 0 ? (n == 2 ? h->x_next : h->x_obs) : (l == 1 ? h->h1[n] : h->h2[n]);
         float* out = l == 0 ? h->h1[n] : (l == 1 ? h->h2[n] : h->h3[n]);
-        GemmDesc d = mk(in, rowoff[l], koff[l], h->p(nn(n, cname[l]) + "/w"), wrow[l], i64, out, crow[l], i64,
+        GemmDesc d = gemm_desc(in, rowoff[l], koff[l], h->p(nn(n, cname[l]) + "/w"), wrow[l], i64, out, crow[l], i64,
                         B * c.Ho * c.Wo, c.Co, c.k * c.k * c.Ci, GG_A_RVEC | GG_EPI_BIAS_RELU);
         d.bias = h->p(nn(n, cname[l]) + "/b");
         if (h->use_planes) {
@@ -362,7 +243,7 @@ int build_groups(b2g_sac* h) {
       GemmGroup g;
       g.name = "fc1_fwd";
       for (int n = 0; n < 3; ++n) {
-        GemmDesc d = mk(h->h3[n], fcA, i1024, h->p(nn(n, "/cnn_fc1/w")), fcW, i512, h->F[n], rowFS, i512, B, 512, 1024,
+        GemmDesc d = gemm_desc(h->h3[n], fcA, i1024, h->p(nn(n, "/cnn_fc1/w")), fcW, i512, h->F[n], rowFS, i512, B, 512, 1024,
                         GG_A_RVEC | GG_EPI_BIAS_RELU);
         d.bias = h->p(nn(n, "/cnn_fc1/b"));
         if (h->use_planes) {
@@ -402,7 +283,7 @@ int build_groups(b2g_sac* h) {
         g.name = "heads_dgrad";
         TAB(row512, iota_tab(B, 512));
         // pi
-        GemmDesc d = mk(h->dz0_pi, rowH, i64, h->p("model/pi/fc0/kernel"), i64, kH, h->dZ4[0], row512, i512, B, 512, H,
+        GemmDesc d = gemm_desc(h->dz0_pi, rowH, i64, h->p("model/pi/fc0/kernel"), i64, kH, h->dZ4[0], row512, i512, B, 512, H,
                         GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
         d.mask = h->F[0]; d.kM = rowFS; d.kN = i512;
         if (h->use_planes) { d.C_hi = h->dZ4p[0][0]; d.C_lo = h->dZ4p[0][1]; }
@@ -414,7 +295,7 @@ int build_groups(b2g_sac* h) {
           for (int r = 0; r < H; ++r) br[q * H + r] = (int)(h->tensors[h->tindex.at(nn(1, hn[q]))].off) + r;
         TAB(brv, br);
         TAB(i3H, iota_tab(3 * H));
-        GemmDesc e = mk(h->dz0_v3, row3H, i3H, h->P, brv, kH, h->dZ4[1], row512, i512, B, 512, 3 * H,
+        GemmDesc e = gemm_desc(h->dz0_v3, row3H, i3H, h->P, brv, kH, h->dZ4[1], row512, i512, B, 512, 3 * H,
                         GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
         e.mask = h->F[1]; e.kM = rowFS; e.kN = i512;
         if (h->use_planes) { e.C_hi = h->dZ4p[1][0]; e.C_lo = h->dZ4p[1][1]; }
@@ -431,7 +312,7 @@ int build_groups(b2g_sac* h) {
         TAB(rowP3, iota_tab(B, P3h * P3w * 64));
         TAB(wfT, iota_tab(1024, 512));
         for (int n = 0; n < 2; ++n) {
-          GemmDesc w = mk(h->h3[n], i1024, fcA, h->dZ4[n], row512, i512, h->g(nn(n, "/cnn_fc1/w")), fcW, i512, 1024, 512, B,
+          GemmDesc w = gemm_desc(h->h3[n], i1024, fcA, h->dZ4[n], row512, i512, h->g(nn(n, "/cnn_fc1/w")), fcW, i512, 1024, 512, B,
                           GG_COLSUM);
           w.colsum = h->g(nn(n, "/cnn_fc1/b"));
           if (h->use_planes) {
@@ -439,7 +320,7 @@ int build_groups(b2g_sac* h) {
             w.A_hi = h->h3p[n][0]; w.A_lo = h->h3p[n][1]; w.B_hi = h->dZ4p[n][0]; w.B_lo = h->dZ4p[n][1];
           }
           f.host.push_back(w);
-          GemmDesc dg = mk(h->dZ4[n], row512, i512, h->p(nn(n, "/cnn_fc1/w")), i512, wfT, h->dZ3p[n], rowP3, cN3p, B, 1024, 512,
+          GemmDesc dg = gemm_desc(h->dZ4[n], row512, i512, h->p(nn(n, "/cnn_fc1/w")), i512, wfT, h->dZ3p[n], rowP3, cN3p, B, 1024, 512,
                            GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
           dg.mask = h->h3[n]; dg.kM = fcA; dg.kN = i1024;
           if (h->use_planes) {
@@ -473,7 +354,7 @@ int build_groups(b2g_sac* h) {
         TAB(c64, iota_tab(64, 64));
         const int R = B * H3 * W3;
         for (int n = 0; n < 2; ++n) {
-          GemmDesc w = mk(h->h2[n], koff[2], rowoff[2], h->dZ3p[n], dz3row, i64, h->g(nn(n, "/cnn3/w")), wrow[2], i64, 576, 64, R,
+          GemmDesc w = gemm_desc(h->h2[n], koff[2], rowoff[2], h->dZ3p[n], dz3row, i64, h->g(nn(n, "/cnn3/w")), wrow[2], i64, 576, 64, R,
                           GG_COLSUM | GG_EPI_ATOMIC, split_for(9, R));
           w.colsum = h->g(nn(n, "/cnn3/b"));
           if (h->use_planes) {
@@ -481,7 +362,7 @@ int build_groups(b2g_sac* h) {
             w.A_hi = h->h2p[n][0]; w.A_lo = h->h2p[n][1]; w.B_hi = h->dZ3pp[n][0]; w.B_lo = h->dZ3pp[n][1];
           }
           g.host.push_back(w);
-          GemmDesc dg = mk(h->dZ3p[n], t_am, t_ar, h->p(nn(n, "/cnn3/w")), t_br, c64, h->dZ2p[n], t_cm, i64, B * H2 * W2, 64, 576,
+          GemmDesc dg = gemm_desc(h->dZ3p[n], t_am, t_ar, h->p(nn(n, "/cnn3/w")), t_br, c64, h->dZ2p[n], t_cm, i64, B * H2 * W2, 64, 576,
                            GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
           dg.mask = h->h2[n]; dg.kM = crow[1]; dg.kN = i64;
           if (h->use_planes) {
@@ -501,7 +382,7 @@ int build_groups(b2g_sac* h) {
         const int R = B * H2 * W2;
         TAB(c64, iota_tab(32, 64));
         for (int n = 0; n < 2; ++n) {
-          GemmDesc w = mk(h->h1[n], koff[1], rowoff[1], h->dZ2p[n], dz2row, i64, h->g(nn(n, "/cnn2/w")), wrow[1], i64, 512, 64, R,
+          GemmDesc w = gemm_desc(h->h1[n], koff[1], rowoff[1], h->dZ2p[n], dz2row, i64, h->g(nn(n, "/cnn2/w")), wrow[1], i64, 512, 64, R,
                           GG_COLSUM | GG_EPI_ATOMIC, split_for(8, R));
           w.colsum = h->g(nn(n, "/cnn2/b"));
           if (h->use_planes) {
@@ -528,7 +409,7 @@ int build_groups(b2g_sac* h) {
                 }
             TAB(t_am, am); TAB(t_ar, ar); TAB(t_br, br); TAB(t_cm, cm);
             for (int n = 0; n < 2; ++n) {
-              GemmDesc dg = mk(h->dZ2p[n], t_am, t_ar, h->p(nn(n, "/cnn2/w")), t_br, c64, h->dZ1[n], t_cm, i64, B * ny * nx, 32, 256,
+              GemmDesc dg = gemm_desc(h->dZ2p[n], t_am, t_ar, h->p(nn(n, "/cnn2/w")), t_br, c64, h->dZ1[n], t_cm, i64, B * ny * nx, 32, 256,
                                GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
               dg.mask = h->h1[n];
               if (h->use_planes) {
@@ -548,7 +429,7 @@ int build_groups(b2g_sac* h) {
         g.name = "conv1_wgrad";
         const int R = B * H1 * W1, M = 64 * Ci;
         for (int n = 0; n < 2; ++n) {
-          GemmDesc w = mk(h->x_obs, koff[0], rowoff[0], h->dZ1[n], crow[0], i64, h->g(nn(n, "/cnn1/w")), wrow[0], i64, M, 32, R,
+          GemmDesc w = gemm_desc(h->x_obs, koff[0], rowoff[0], h->dZ1[n], crow[0], i64, h->g(nn(n, "/cnn1/w")), wrow[0], i64, M, 32, R,
                           GG_COLSUM | GG_EPI_ATOMIC, split_for((M + 63) / 64, R, 74));
           w.colsum = h->g(nn(n, "/cnn1/b"));
           if (h->use_planes) {
@@ -583,11 +464,11 @@ int build_groups(b2g_sac* h) {
         }
         h->n_colsum_early = (int)early.size();
         h->colsum_early_ctas = estart;
-        if (int rc = dalloc(h, &h->d_colsum_early, early.size(), false)) return rc;
+        if (int rc = dev_alloc(h->allocs, h->stream, &h->d_colsum_early, early.size(), false)) return rc;
         CK(cudaMemcpyAsync(h->d_colsum_early, early.data(), early.size() * sizeof(ColsumJob), cudaMemcpyHostToDevice, h->stream));
         h->n_colsum = (int)jobs.size();
         h->colsum_ctas = start;
-        if (int rc = dalloc(h, &h->d_colsum, jobs.size(), false)) return rc;
+        if (int rc = dev_alloc(h->allocs, h->stream, &h->d_colsum, jobs.size(), false)) return rc;
         CK(cudaMemcpyAsync(h->d_colsum, jobs.data(), jobs.size() * sizeof(ColsumJob), cudaMemcpyHostToDevice, h->stream));
         CK(cudaStreamSynchronize(h->stream));
       }
@@ -603,7 +484,7 @@ int build_groups(b2g_sac* h) {
     const int fnet[5] = {0, 1, 1, 1, 2};
     for (int q = 0; q < 5; ++q) {
       const int R = (q == 2 || q == 3) ? fd + A : fd;
-      g.host.push_back(mk(h->F[fnet[q]], rowFS, iFS, h->p(hk[q]), kH, i64, h->z0[q], rowH, i64, B, H, R, GG_A_RVEC));
+      g.host.push_back(gemm_desc(h->F[fnet[q]], rowFS, iFS, h->p(hk[q]), kH, i64, h->z0[q], rowH, i64, B, H, R, GG_A_RVEC));
     }
     GemmGroup a = g;
     // training step: the 516-deep reduction of each head is split over several CTAs (atomic accumulation into the
@@ -626,11 +507,11 @@ int build_groups(b2g_sac* h) {
     for (int q = 0; q < 4; ++q) {
       const int M = (q >= 2) ? fd + A : fd;
       const float* dz0 = q == 0 ? h->dz0_pi : h->dz0_v3;
-      GemmDesc w0 = mk(h->F[q == 0 ? 0 : 1], iFS, rowFS, dz0, dzrow[q], i64, h->g(std::string(hp[q]) + "/fc0/kernel"), kH, i64, M, H, B,
+      GemmDesc w0 = gemm_desc(h->F[q == 0 ? 0 : 1], iFS, rowFS, dz0, dzrow[q], i64, h->g(std::string(hp[q]) + "/fc0/kernel"), kH, i64, M, H, B,
                        GG_COLSUM);
       w0.colsum = h->g(std::string(hp[q]) + "/fc0/bias");
       g.host.push_back(w0);
-      GemmDesc w1 = mk(h->a0[q], i64, rowH, h->dz1[q], rowH, i64, h->g(std::string(hp[q]) + "/fc1/kernel"), kH, i64, H, H, B, GG_COLSUM);
+      GemmDesc w1 = gemm_desc(h->a0[q], i64, rowH, h->dz1[q], rowH, i64, h->g(std::string(hp[q]) + "/fc1/kernel"), kH, i64, H, H, B, GG_COLSUM);
       w1.colsum = h->g(std::string(hp[q]) + "/fc1/bias");
       g.host.push_back(w1);
     }
@@ -653,7 +534,7 @@ int build_groups(b2g_sac* h) {
       }
     h->n_jobs = (int)jobs.size();
     h->job_tiles = start;
-    if (int rc = dalloc(h, &h->d_jobs, jobs.size(), false)) return rc;
+    if (int rc = dev_alloc(h->allocs, h->stream, &h->d_jobs, jobs.size(), false)) return rc;
     CK(cudaMemcpyAsync(h->d_jobs, jobs.data(), jobs.size() * sizeof(PlaneJob), cudaMemcpyHostToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));
   }
@@ -761,6 +642,15 @@ GatherArgs make_gather(b2g_sac* h, bool from_replay, bool with_next) {
   return g;
 }
 
+// prep_kernel arguments: gen != 0 draws the replay slots (when the step samples) and the policy noise
+PrepArgs make_prep(b2g_sac* h, unsigned long long seed, bool gen, bool apply) {
+  PrepArgs pa{};
+  pa.counters = h->counters; pa.step_consts = h->step_consts; pa.lr = h->d_lr; pa.metrics = h->metrics;
+  pa.indices = h->indices; pa.eps = h->eps; pa.B = h->B; pa.A = h->A; pa.replay_size = nullptr;  /* device counter [5] */
+  pa.seed = seed; pa.gen = gen ? 1 : 0; pa.apply = apply ? 1 : 0;
+  return pa;
+}
+
 struct Prof {
   bool on = false;
   std::vector<cudaEvent_t> ev;
@@ -783,10 +673,7 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
     }
   };
   mark("begin");
-  PrepArgs pa{};
-  pa.counters = h->counters; pa.step_consts = h->step_consts; pa.lr = h->d_lr; pa.metrics = h->metrics;
-  pa.indices = h->indices; pa.eps = h->eps; pa.B = h->B; pa.A = h->A; pa.replay_size = nullptr;  /* device counter [5] */
-  pa.seed = h->cfg.seed + 0x9E3779B97F4A7C15ull * (unsigned long long)h->cfg.rank; pa.gen = sampled ? 1 : 0; pa.apply = apply ? 1 : 0;
+  PrepArgs pa = make_prep(h, h->cfg.seed + 0x9E3779B97F4A7C15ull * (unsigned long long)h->cfg.rank, sampled, apply);
   // Leaf work runs on a second stream (parallel branches once captured in the step graph): zeroing the gradient
   // arena and refreshing the BF16 weight planes overlap prep + gather; heads_wgrad and the bias column sums overlap
   // the dgrad chain.  Profiling (per-launch events) keeps everything serial on one stream.
@@ -867,7 +754,7 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
   const int64_t pi_fc1 = h->tensors[h->tindex.at("model/pi/" + std::string(h->cnn ? "cnn_fc1/w" : "fc0/kernel"))].off;
   const int64_t v_fc1 = h->tensors[h->tindex.at("model/values_fn/" + std::string(h->cnn ? "cnn_fc1/w" : "vf/fc0/kernel"))].off;
   auto nccl_ck = [&](int rc) -> int {
-    if (rc != 0) return fail(B2G_ENCCL, std::string("nccl: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "?"));
+    if (rc != 0) return b2g_fail(B2G_ENCCL, std::string("nccl: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "?"));
     return 0;
   };
   bool dp_early_opt = false;
@@ -1008,36 +895,6 @@ void refresh_planes(b2g_sac* h, bool for_step = false) {
   }
 }
 
-int set_lr(b2g_sac* h, float lr) {
-  if (lr != h->cur_lr) {
-    CK(cudaStreamSynchronize(h->stream));
-    CK(cudaMemcpy(h->d_lr, &lr, sizeof(float), cudaMemcpyHostToDevice));
-    h->cur_lr = lr;
-  }
-  return 0;
-}
-
-int fetch_metrics(b2g_sac* h, b2g_sac_metrics* out) {
-  CK(cudaMemcpyAsync(h->h_met, h->metrics, MET_COUNT * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaMemcpyAsync(h->h_cnt, h->counters, 8 * sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
-  float la = 0.f, gla = 0.f;
-  CK(cudaMemcpyAsync(&la, h->p("model/log_ent_coef"), sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaMemcpyAsync(&gla, h->g("model/log_ent_coef"), sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  if (!out) return 0;
-  const float inv = 1.0f / (float)h->cfg.nranks;
-  const float* m = h->h_met;
-  out->policy_loss = m[MET_POLICY_LOSS] * inv; out->qf1_loss = m[MET_QF1_LOSS] * inv; out->qf2_loss = m[MET_QF2_LOSS] * inv;
-  out->value_loss = m[MET_VALUE_LOSS] * inv; out->ent_coef_loss = m[MET_ENT_COEF_LOSS] * inv; out->entropy = m[MET_ENTROPY] * inv;
-  out->mean_q1 = m[MET_MEAN_Q1] * inv; out->mean_q2 = m[MET_MEAN_Q2] * inv; out->mean_v = m[MET_MEAN_V] * inv;
-  out->mean_logp = m[MET_MEAN_LOGP] * inv;
-  out->grad_norm_pi = sqrtf(m[MET_GN_PI]); out->grad_norm_values = sqrtf(m[MET_GN_VALUES]);
-  out->grad_ent = gla * inv;
-  out->ent_coef = expf(la);     // value AFTER the update when apply_update != 0 (SB logs the pre-update value)
-  out->n_updates = h->h_cnt[3];
-  return 0;
-}
-
 void fill_metrics(const b2g_sac* h, const float* m, const long long* cnt, b2g_sac_metrics* out) {
   const float inv = 1.0f / (float)h->cfg.nranks;
   out->policy_loss = m[MET_POLICY_LOSS] * inv; out->qf1_loss = m[MET_QF1_LOSS] * inv; out->qf2_loss = m[MET_QF2_LOSS] * inv;
@@ -1046,8 +903,24 @@ void fill_metrics(const b2g_sac* h, const float* m, const long long* cnt, b2g_sa
   out->mean_logp = m[MET_MEAN_LOGP] * inv;
   out->grad_norm_pi = sqrtf(m[MET_GN_PI]); out->grad_norm_values = sqrtf(m[MET_GN_VALUES]);
   out->grad_ent = m[MET_COUNT + 1] * inv;
-  out->ent_coef = expf(m[MET_COUNT]);
+  out->ent_coef = expf(m[MET_COUNT]);     // value AFTER the update when apply_update != 0 (SB logs the pre-update value)
   out->n_updates = cnt[3];
+}
+
+// the step's metrics -> pinned met[MET_COUNT + 2] (the accumulators, then log_alpha and its gradient) and cnt[8], in stream order
+int copy_metrics_async(b2g_sac* h, float* met, long long* cnt) {
+  CK(cudaMemcpyAsync(met, h->metrics, MET_COUNT * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(met + MET_COUNT, h->p("model/log_ent_coef"), sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(met + MET_COUNT + 1, h->g("model/log_ent_coef"), sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(cnt, h->counters, 8 * sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
+  return 0;
+}
+
+int fetch_metrics(b2g_sac* h, b2g_sac_metrics* out) {
+  if (int rc = copy_metrics_async(h, h->h_met, h->h_cnt)) return rc;
+  CK(cudaStreamSynchronize(h->stream));
+  if (out) fill_metrics(h, h->h_met, h->h_cnt, out);
+  return 0;
 }
 
 int find_tensor(const b2g_sac* h, const char* name) {
@@ -1065,24 +938,13 @@ int find_tensor(const b2g_sac* h, const char* name) {
 // ================================================================================================
 extern "C" {
 
-const char* b2g_last_error(void) { return g_err.c_str(); }
-int b2g_version(void) { return 100; }
-
-int b2g_nccl_unique_id(void* out128, const char* nccl_lib) {
-  if (!out128) return fail(B2G_EINVAL, "out128 is NULL");
-  if (int rc = load_nccl(nccl_lib)) return rc;
-  int rc = g_nccl.GetUniqueId(out128);
-  if (rc != 0) return fail(B2G_ENCCL, "ncclGetUniqueId failed");
-  return 0;
-}
-
 int b2g_sac_dp_export(b2g_sac* h, void* out192) {
-  if (!h || !out192) return fail(B2G_EINVAL, "b2g_sac_dp_export: null argument");
+  if (!h || !out192) return b2g_fail(B2G_EINVAL, "b2g_sac_dp_export: null argument");
   cudaSetDevice(h->cfg.device);
   if (!h->dp_x) {
-    if (int rc = dalloc(h, &h->dp_x, 256)) return rc;
-    if (int rc = dalloc(h, &h->dp_recv, h->n_train + 64 * DP_MAX_RANKS)) return rc;      // [src rank][my slice], slices <= ceil(n/N) + pad
-    if (int rc = dalloc(h, &h->dp_sync, 64)) return rc;
+    if (int rc = dev_alloc(h->allocs, h->stream, &h->dp_x, 256)) return rc;
+    if (int rc = dev_alloc(h->allocs, h->stream, &h->dp_recv, h->n_train + 64 * DP_MAX_RANKS)) return rc;      // [src rank][my slice], slices <= ceil(n/N) + pad
+    if (int rc = dev_alloc(h->allocs, h->stream, &h->dp_sync, 64)) return rc;
     CK(cudaStreamSynchronize(h->stream));
   }
   cudaIpcMemHandle_t hd[3];
@@ -1095,18 +957,18 @@ int b2g_sac_dp_export(b2g_sac* h, void* out192) {
 }
 
 int b2g_debug_dp_stamps(b2g_sac* h, long long* out5) {     /* bring-up: phase timestamps of the last peer-memory optimiser launch */
-  if (!h || !h->dp_sync) return fail(B2G_EINVAL, "b2g_debug_dp_stamps: not connected");
+  if (!h || !h->dp_sync) return b2g_fail(B2G_EINVAL, "b2g_debug_dp_stamps: not connected");
   CK(cudaStreamSynchronize(h->stream));
   CK(cudaMemcpy(out5, h->dp_sync + 8, 5 * sizeof(long long), cudaMemcpyDeviceToHost));
   return 0;
 }
 
 int b2g_sac_dp_connect(b2g_sac* h, const void* all_exports, int nranks) {
-  if (!h || !all_exports) return fail(B2G_EINVAL, "b2g_sac_dp_connect: null argument");
-  if (nranks != h->cfg.nranks || nranks < 2 || nranks > DP_MAX_RANKS) return fail(B2G_EINVAL, "b2g_sac_dp_connect: nranks must equal the learner's (2..8)");
-  if (!h->dp_x) return fail(B2G_EINVAL, "b2g_sac_dp_connect: call b2g_sac_dp_export first");
-  if (h->dp_p2p) return fail(B2G_ESTATE, "b2g_sac_dp_connect: already connected");
-  if (((h->n_pi | h->n_values | h->n_ent | h->n_target) & 3) != 0) return fail(B2G_EINVAL, "b2g_sac_dp_connect: arena segments are not float4 aligned");
+  if (!h || !all_exports) return b2g_fail(B2G_EINVAL, "b2g_sac_dp_connect: null argument");
+  if (nranks != h->cfg.nranks || nranks < 2 || nranks > DP_MAX_RANKS) return b2g_fail(B2G_EINVAL, "b2g_sac_dp_connect: nranks must equal the learner's (2..8)");
+  if (!h->dp_x) return b2g_fail(B2G_EINVAL, "b2g_sac_dp_connect: call b2g_sac_dp_export first");
+  if (h->dp_p2p) return b2g_fail(B2G_ESTATE, "b2g_sac_dp_connect: already connected");
+  if (((h->n_pi | h->n_values | h->n_ent | h->n_target) & 3) != 0) return b2g_fail(B2G_EINVAL, "b2g_sac_dp_connect: arena segments are not float4 aligned");
   cudaSetDevice(h->cfg.device);
   CK(cudaStreamSynchronize(h->stream));
   for (int q = 0; q < nranks; ++q) {
@@ -1156,8 +1018,8 @@ int b2g_sac_destroy(b2g_sac* h) {
   if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
   for (auto& g : h->pipe_graph) if (g) cudaGraphExecDestroy(g);
   for (void* q : h->dp_opened) cudaIpcCloseMemHandle(q);
-  if (h->nccl_comm2 && g_nccl.CommDestroy) g_nccl.CommDestroy(h->nccl_comm2);
-  if (h->nccl_comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->nccl_comm);
+  nccl_comm_destroy(h->nccl_comm2);
+  nccl_comm_destroy(h->nccl_comm);
   if (h->side) cudaStreamDestroy(h->side);
   if (h->aux) { cudaStreamSynchronize(h->aux); cudaStreamDestroy(h->aux); }
   for (auto& e : h->ev_aux) if (e) cudaEventDestroy(e);
@@ -1184,53 +1046,48 @@ int b2g_sac_destroy(b2g_sac* h) {
 }
 
 int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
-  if (!cfg || !out) return fail(B2G_EINVAL, "cfg/out is NULL");
+  if (!cfg || !out) return b2g_fail(B2G_EINVAL, "cfg/out is NULL");
   *out = nullptr;
-  if (cfg->hidden != 64) return fail(B2G_EINVAL, "hidden must be 64 (SAC.layers [64,64], config/gripper_grasp.yaml:81)");
-  if (cfg->n_act < 1 || cfg->n_act > 8) return fail(B2G_EINVAL, "n_act must be in [1,8]");
-  if (cfg->batch < 1 || cfg->buffer_capacity < 1) return fail(B2G_EINVAL, "batch and buffer_capacity must be positive");
-  if (cfg->nranks < 1 || cfg->rank < 0 || cfg->rank >= cfg->nranks) return fail(B2G_EINVAL, "bad rank/nranks");
+  if (cfg->hidden != 64) return b2g_fail(B2G_EINVAL, "hidden must be 64 (SAC.layers [64,64], config/gripper_grasp.yaml:81)");
+  if (cfg->n_act < 1 || cfg->n_act > 8) return b2g_fail(B2G_EINVAL, "n_act must be in [1,8]");
+  if (cfg->batch < 1 || cfg->buffer_capacity < 1) return b2g_fail(B2G_EINVAL, "batch and buffer_capacity must be positive");
+  if (cfg->nranks < 1 || cfg->rank < 0 || cfg->rank >= cfg->nranks) return b2g_fail(B2G_EINVAL, "bad rank/nranks");
   if (cfg->precision < B2G_PREC_FP32_SIMT || cfg->precision > B2G_PREC_BF16)
-    return fail(B2G_EINVAL, "unknown precision mode");
-  int ndev = 0;
-  CK(cudaGetDeviceCount(&ndev));
-  if (cfg->device < 0 || cfg->device >= ndev) return fail(B2G_ECUDA, "no such CUDA device");
-  CK(cudaSetDevice(cfg->device));
-  cudaDeviceProp prop{};
-  CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 9) return fail(B2G_ECUDA, std::string("libb200grasp is built for sm_90a only; found ") + prop.name);
+    return b2g_fail(B2G_EINVAL, "unknown precision mode");
+  int num_sms = 0;
+  if (int rc = check_device(cfg->device, &num_sms)) return rc;
 
   b2g_sac* h = new b2g_sac();
   h->cfg = *cfg;
-  h->num_sms = prop.multiProcessorCount;
+  h->num_sms = num_sms;
   h->cfg.nccl_id = nullptr; h->cfg.nccl_lib = nullptr;
   h->cnn = cfg->obs_h > 0;
   h->B = cfg->batch; h->A = cfg->n_act; h->H = cfg->hidden;
   if (h->cnn) {
-    if (cfg->obs_c < 2) { delete h; return fail(B2G_EINVAL, "CNN policy needs obs_c >= 2 (image planes + feature plane)"); }
+    if (cfg->obs_c < 2) { delete h; return b2g_fail(B2G_EINVAL, "CNN policy needs obs_c >= 2 (image planes + feature plane)"); }
     h->Cimg = cfg->obs_c - 1; h->Hi = cfg->obs_h; h->Wi = cfg->obs_w;
     h->H1 = (h->Hi - 8) / 4 + 1; h->W1 = (h->Wi - 8) / 4 + 1;
     h->H2 = (h->H1 - 4) / 2 + 1; h->W2 = (h->W1 - 4) / 2 + 1;
     h->H3 = h->H2 - 2; h->W3 = h->W2 - 2;
     if (h->H3 * h->W3 * 64 != 1024 || (h->Wi * h->Cimg) % 4 != 0) {
       delete h;
-      return fail(B2G_EINVAL, "observation size must give a 4x4x64 conv3 output (64x64 input; cnn_fc1/w is (1024,512))");
+      return b2g_fail(B2G_EINVAL, "observation size must give a 4x4x64 conv3 output (64x64 input; cnn_fc1/w is (1024,512))");
     }
     h->E = h->Hi * h->Wi * cfg->obs_c;
     h->feat_dim = 513;
   } else {
-    if (cfg->obs_dim < 1) { delete h; return fail(B2G_EINVAL, "obs_dim must be positive for the MLP policy"); }
+    if (cfg->obs_dim < 1) { delete h; return b2g_fail(B2G_EINVAL, "obs_dim must be positive for the MLP policy"); }
     h->E = cfg->obs_dim;
     h->feat_dim = cfg->obs_dim;
   }
   h->FS = (h->feat_dim + h->A + 7) / 8 * 8;
-  auto bail = [&](int rc) { std::string keep = g_err; b2g_sac_destroy(h); g_err = keep; return rc; };
-  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(fail(B2G_ECUDA, "cudaStreamCreate failed"));
+  auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_sac_destroy(h); g_b2g_err = keep; return rc; };
+  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "cudaStreamCreate failed"));
   cudaEventCreate(&h->ev0); cudaEventCreate(&h->ev1);
   build_params(h);
   int rc = 0;
   const int B = h->B;
-#define DA(ptr, count) if ((rc = dalloc(h, &(ptr), (size_t)(count)))) return bail(rc)
+#define DA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
   DA(h->P, h->n_all); DA(h->Mo, h->n_train); DA(h->Vo, h->n_train); DA(h->G, h->n_train + MET_COUNT);
   DA(h->metrics, MET_COUNT); DA(h->counters, 8); DA(h->step_consts, 4); DA(h->d_lr, 1);
   const int64_t cap = cfg->buffer_capacity;
@@ -1250,7 +1107,7 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
   for (int k = 0; k < 2; ++k) {
     if (cudaMallocHost((void**)&h->hp_stats[k], (size_t)(2 * h->E + 2 * h->Ec + 8) * sizeof(double)) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->ev_stats[k], cudaEventDisableTiming) != cudaSuccess)
-      return bail(fail(B2G_ECUDA, "norm-stat staging"));
+      return bail(b2g_fail(B2G_ECUDA, "norm-stat staging"));
   }
   DA(h->s_obs, (size_t)B * h->E); DA(h->s_next, (size_t)B * h->E); DA(h->s_act, B * h->A); DA(h->s_rew, B); DA(h->s_done, B);
   if (h->cnn) {
@@ -1298,25 +1155,25 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
   DA(h->per_sample, 7 * B); DA(h->pi_out, B * h->A); DA(h->eps, B * h->A + 4); DA(h->rew_n, B); DA(h->done_n, B);
   DA(h->indices, B + 4);
 #undef DA
-  if (cudaMallocHost((void**)&h->h_met, MET_COUNT * sizeof(float)) != cudaSuccess ||
+  if (cudaMallocHost((void**)&h->h_met, (MET_COUNT + 2) * sizeof(float)) != cudaSuccess ||
       cudaMallocHost((void**)&h->h_cnt, 8 * sizeof(long long)) != cudaSuccess)
-    return bail(fail(B2G_ECUDA, "cudaMallocHost failed"));
+    return bail(b2g_fail(B2G_ECUDA, "cudaMallocHost failed"));
   for (int j = 0; j < 2; ++j) {
-    if ((rc = dalloc(h, &h->ps_obs[j], (size_t)B * h->E)) || (rc = dalloc(h, &h->ps_next[j], (size_t)B * h->E))) return bail(rc);
+    if ((rc = dev_alloc(h->allocs, h->stream, &h->ps_obs[j], (size_t)B * h->E)) || (rc = dev_alloc(h->allocs, h->stream, &h->ps_next[j], (size_t)B * h->E))) return bail(rc);
     if (cudaEventCreateWithFlags(&h->ev_h2d[j], cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->ev_consumed[j], cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->ev_met[j], cudaEventDisableTiming) != cudaSuccess ||
         cudaMallocHost((void**)&h->pm_met[j], (MET_COUNT + 2) * sizeof(float)) != cudaSuccess ||
         cudaMallocHost((void**)&h->pm_cnt[j], 8 * sizeof(long long)) != cudaSuccess)
-      return bail(fail(B2G_ECUDA, "pipelined-path resources"));
+      return bail(b2g_fail(B2G_ECUDA, "pipelined-path resources"));
   }
-  if (cudaStreamCreateWithFlags(&h->cstream, cudaStreamNonBlocking) != cudaSuccess) return bail(fail(B2G_ECUDA, "copy stream"));
+  if (cudaStreamCreateWithFlags(&h->cstream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "copy stream"));
   {   // leaf branch of the step (B2G_FORK=0 keeps the step on one stream)
     const char* fk = getenv("B2G_FORK");
     if (!(fk && atoi(fk) == 0)) {
-      if (cudaStreamCreateWithFlags(&h->aux, cudaStreamNonBlocking) != cudaSuccess) return bail(fail(B2G_ECUDA, "aux stream"));
+      if (cudaStreamCreateWithFlags(&h->aux, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "aux stream"));
       for (auto& e : h->ev_aux)
-        if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) return bail(fail(B2G_ECUDA, "aux events"));
+        if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "aux events"));
       h->fork_leaves = true;
     }
   }
@@ -1326,17 +1183,13 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
     if ((h->compact && cudaMemcpyAsync(h->d_istd_c, ones.data(), h->Ec * sizeof(double), cudaMemcpyHostToDevice, h->stream) != cudaSuccess) ||
         cudaMemcpyAsync(h->d_istd, ones.data(), h->E * sizeof(double), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
         cudaStreamSynchronize(h->stream) != cudaSuccess)
-      return bail(fail(B2G_ECUDA, "init copy failed"));
+      return bail(b2g_fail(B2G_ECUDA, "init copy failed"));
   }
   if ((rc = build_groups(h))) return bail(rc);
   if (h->v2.on && (rc = v2_create(h))) return bail(rc);
   if (cfg->nranks > 1) {
-    if (!cfg->nccl_id) return bail(fail(B2G_EINVAL, "nranks > 1 needs nccl_id"));
-    if ((rc = load_nccl(cfg->nccl_lib))) return bail(rc);
-    UId id;
-    memcpy(id.b, cfg->nccl_id, 128);
-    int nrc = g_nccl.CommInitRank(&h->nccl_comm, cfg->nranks, id, cfg->rank);
-    if (nrc != 0) return bail(fail(B2G_ENCCL, std::string("ncclCommInitRank: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(nrc) : "?")));
+    if (!cfg->nccl_id) return bail(b2g_fail(B2G_EINVAL, "nranks > 1 needs nccl_id"));
+    if ((rc = nccl_comm_init(&h->nccl_comm, cfg->nranks, cfg->nccl_id, cfg->rank, cfg->nccl_lib))) return bail(rc);
     {   // second communicator + side stream for the early (overlapped) all-reduce
       // engine v2 only (B2G_AR_OVERLAP=0 puts the whole all-reduce back on the critical chain)
       const char* ov = getenv("B2G_AR_OVERLAP");
@@ -1354,18 +1207,18 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
       }
     }
     // warm the communicator up outside any stream capture (NCCL allocates its channels lazily)
-    nrc = g_nccl.AllReduce(h->G, h->G, (size_t)(h->n_train + MET_COUNT), 7, 0, h->nccl_comm, h->stream);
-    if (nrc != 0 || cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(fail(B2G_ENCCL, "NCCL warm-up all-reduce failed"));
+    const int nrc = g_nccl.AllReduce(h->G, h->G, (size_t)(h->n_train + MET_COUNT), 7, 0, h->nccl_comm, h->stream);
+    if (nrc != 0 || cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(b2g_fail(B2G_ENCCL, "NCCL warm-up all-reduce failed"));
   }
   const char* ng = getenv("B2G_NO_GRAPH");
   h->use_graph = !(ng && ng[0] == '1');
-  if (cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(fail(B2G_ECUDA, "create: sync failed"));
+  if (cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "create: sync failed"));
   *out = h;
   return 0;
 }
 
 int b2g_sync(b2g_sac* h) {
-  if (!h) return fail(B2G_EINVAL, "NULL handle");
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
   return 0;
@@ -1374,7 +1227,7 @@ int b2g_sync(b2g_sac* h) {
 int b2g_param_count(const b2g_sac* h) { return h ? (int)h->tensors.size() : 0; }
 
 int b2g_param_info(const b2g_sac* h, int idx, const char** name, int64_t* numel, int32_t* ndim, int64_t shape[4]) {
-  if (!h || idx < 0 || idx >= (int)h->tensors.size()) return fail(B2G_EINVAL, "bad tensor index");
+  if (!h || idx < 0 || idx >= (int)h->tensors.size()) return b2g_fail(B2G_EINVAL, "bad tensor index");
   const Tensor& t = h->tensors[idx];
   if (name) *name = t.name.c_str();
   if (numel) *numel = t.numel;
@@ -1384,12 +1237,12 @@ int b2g_param_info(const b2g_sac* h, int idx, const char** name, int64_t* numel,
 }
 
 static int copy_tensor(b2g_sac* h, const char* name, float* arena, float* host, size_t numel, bool to_host, bool trainable_only) {
-  if (!h || !host) return fail(B2G_EINVAL, "NULL argument");
+  if (!h || !host) return b2g_fail(B2G_EINVAL, "NULL argument");
   const int i = find_tensor(h, name);
-  if (i < 0) return fail(B2G_EINVAL, std::string("unknown variable: ") + (name ? name : "(null)"));
+  if (i < 0) return b2g_fail(B2G_EINVAL, std::string("unknown variable: ") + (name ? name : "(null)"));
   const Tensor& t = h->tensors[i];
-  if ((int64_t)numel != t.numel) return fail(B2G_EINVAL, std::string("size mismatch for ") + t.name);
-  if (trainable_only && t.group == 3) return fail(B2G_EINVAL, std::string("not a trainable variable: ") + t.name);
+  if ((int64_t)numel != t.numel) return b2g_fail(B2G_EINVAL, std::string("size mismatch for ") + t.name);
+  if (trainable_only && t.group == 3) return b2g_fail(B2G_EINVAL, std::string("not a trainable variable: ") + t.name);
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
   if (to_host) CK(cudaMemcpy(host, arena + t.off, numel * sizeof(float), cudaMemcpyDeviceToHost));
@@ -1413,7 +1266,7 @@ int b2g_get_adam(b2g_sac* h, const char* name, float* m, float* v, size_t numel)
   return copy_tensor(h, name, h->Vo, v, numel, true, true);
 }
 int b2g_reset_optimizer(b2g_sac* h) {
-  if (!h) return fail(B2G_EINVAL, "NULL handle");
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaMemsetAsync(h->Mo, 0, h->n_train * sizeof(float), h->stream));
   CK(cudaMemsetAsync(h->Vo, 0, h->n_train * sizeof(float), h->stream));
@@ -1424,7 +1277,7 @@ int b2g_reset_optimizer(b2g_sac* h) {
 
 int b2g_replay_add(b2g_sac* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done,
                    int64_t n) {
-  if (!h || !obs || !act || !rew || !next_obs || !done || n < 0) return fail(B2G_EINVAL, "NULL argument");
+  if (!h || !obs || !act || !rew || !next_obs || !done || n < 0) return b2g_fail(B2G_EINVAL, "NULL argument");
   CK(cudaSetDevice(h->cfg.device));
   const int64_t cap = h->cfg.buffer_capacity;
   int64_t done_n = 0;
@@ -1458,8 +1311,8 @@ int b2g_replay_add(b2g_sac* h, const float* obs, const float* act, const float* 
 int64_t b2g_replay_size(const b2g_sac* h) { return h ? h->r_size : 0; }
 
 int b2g_replay_get(b2g_sac* h, int64_t slot, float* obs, float* act, float* rew, float* next_obs, float* done) {
-  if (!h) return fail(B2G_EINVAL, "NULL handle");
-  if (slot < 0 || slot >= h->r_size) return fail(B2G_EINVAL, "replay slot out of range");
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  if (slot < 0 || slot >= h->r_size) return b2g_fail(B2G_EINVAL, "replay slot out of range");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
   const size_t E = h->E, A = h->A;
@@ -1486,7 +1339,7 @@ int b2g_replay_get(b2g_sac* h, int64_t slot, float* obs, float* act, float* rew,
 }
 
 int b2g_get_last_batch(b2g_sac* h, int32_t* indices, float* eps, float* per_sample, float* pi_out) {
-  if (!h) return fail(B2G_EINVAL, "NULL handle");
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
   const size_t B = h->B, A = h->A;
@@ -1499,8 +1352,8 @@ int b2g_get_last_batch(b2g_sac* h, int32_t* indices, float* eps, float* per_samp
 
 int b2g_set_norm_stats(b2g_sac* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs, double clip_rew,
                        double eps, int norm_obs, int norm_reward) {
-  if (!h) return fail(B2G_EINVAL, "NULL handle");
-  if (norm_obs && (!obs_mean || !obs_var)) return fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  if (norm_obs && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
   CK(cudaSetDevice(h->cfg.device));
   // Called once per environment step by the learn loop (VecNormalize statistics move with every observation): the values
   // are staged in one of two pinned buffers and uploaded asynchronously IN STREAM ORDER -- no stream synchronisation, the
@@ -1534,25 +1387,17 @@ int b2g_set_norm_stats(b2g_sac* h, const double* obs_mean, const double* obs_var
 
 static int ensure_graph(b2g_sac* h) {
   if (h->graph_exec) return 0;
-  cudaGraph_t graph = nullptr;
-  CK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
   int n = 0;
-  int rc = issue_step(h, true, true, true, nullptr, &n);
-  cudaError_t e = cudaStreamEndCapture(h->stream, &graph);
-  if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-  if (e != cudaSuccess) return fail(B2G_ECUDA, std::string("graph capture failed: ") + cudaGetErrorString(e));
-  e = cudaGraphInstantiate(&h->graph_exec, graph, 0);
-  cudaGraphDestroy(graph);
-  if (e != cudaSuccess) return fail(B2G_ECUDA, std::string("graph instantiate failed: ") + cudaGetErrorString(e));
+  if (int rc = capture_graph(h->stream, [&] { return issue_step(h, true, true, true, nullptr, &n); }, &h->graph_exec)) return rc;
   h->launches = n;
   return 0;
 }
 
 int b2g_sac_step_async(b2g_sac* h, int n_steps, float lr) {
-  if (!h || n_steps < 0) return fail(B2G_EINVAL, "bad argument");
-  if (h->r_size < 1) return fail(B2G_ESTATE, "replay buffer is empty");
+  if (!h || n_steps < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  if (h->r_size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
   CK(cudaSetDevice(h->cfg.device));
-  if (int rc = set_lr(h, lr)) return rc;
+  if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
   refresh_planes(h, true);
   if (h->use_graph) if (int rc = ensure_graph(h)) return rc;
   CK(cudaEventRecord(h->ev0, h->stream));
@@ -1573,9 +1418,9 @@ int b2g_sac_step(b2g_sac* h, int n_steps, float lr, b2g_sac_metrics* out) {
 
 int b2g_sac_step_explicit(b2g_sac* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done,
                           const float* eps, float lr, int apply_update, b2g_sac_metrics* out, float* per_sample, float* pi_out) {
-  if (!h || !obs || !act || !rew || !next_obs || !done || !eps) return fail(B2G_EINVAL, "NULL argument");
+  if (!h || !obs || !act || !rew || !next_obs || !done || !eps) return b2g_fail(B2G_EINVAL, "NULL argument");
   CK(cudaSetDevice(h->cfg.device));
-  if (int rc = set_lr(h, lr)) return rc;
+  if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
   const size_t B = h->B, E = h->E, A = h->A;
   refresh_planes(h, true);
   CK(cudaEventRecord(h->ev0, h->stream));
@@ -1618,16 +1463,16 @@ void compact_host(const float* src, float* dst, int n, int HW, int Cfull, int Ec
 
 int b2g_debug_compact_host(const float* src, float* dst, int n, int hw, int cfull, int threads) {
   /* host-only (no device needed): the row compaction b2g_sac_step_host_pipelined applies before its copy */
-  if (!src || !dst || n < 0 || hw < 1 || cfull < 2) return fail(B2G_EINVAL, "b2g_debug_compact_host: bad argument");
+  if (!src || !dst || n < 0 || hw < 1 || cfull < 2) return b2g_fail(B2G_EINVAL, "b2g_debug_compact_host: bad argument");
   compact_host(src, dst, n, hw, cfull, hw * (cfull - 1) + 4, threads > 0 ? threads : 1);
   return 0;
 }
 
 int b2g_sac_step_host_pipelined(b2g_sac* h, const float* obs, const float* act, const float* rew, const float* next_obs,
                                 const float* done, const float* eps, float lr, b2g_sac_metrics* prev_out, int* have_prev) {
-  if (!h || !obs || !act || !rew || !next_obs || !done || !eps) return fail(B2G_EINVAL, "NULL argument");
+  if (!h || !obs || !act || !rew || !next_obs || !done || !eps) return b2g_fail(B2G_EINVAL, "NULL argument");
   CK(cudaSetDevice(h->cfg.device));
-  if (int rc = set_lr(h, lr)) return rc;
+  if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
   refresh_planes(h, true);
   const size_t B = h->B, E = h->E, A = h->A;
   const long long k = h->pipe_k++;
@@ -1710,19 +1555,10 @@ int b2g_sac_step_host_pipelined(b2g_sac* h, const float* obs, const float* act, 
     // were the bottleneck of this path once the copy had shrunk
     if (h->pipe_graph[j] && h->pipe_graph_compact[j] != hc) { cudaGraphExecDestroy(h->pipe_graph[j]); h->pipe_graph[j] = nullptr; }
     if (!h->pipe_graph[j]) {
-      cudaGraph_t graph = nullptr;
-      CK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-      rc = issue_step(h, false, true, false, nullptr, &n);
-      cudaError_t e = cudaStreamEndCapture(h->stream, &graph);
-      if (!rc && e != cudaSuccess) rc = fail(B2G_ECUDA, std::string("graph capture failed: ") + cudaGetErrorString(e));
-      if (!rc) {
-        e = cudaGraphInstantiate(&h->pipe_graph[j], graph, 0);
-        if (e != cudaSuccess) rc = fail(B2G_ECUDA, std::string("graph instantiate failed: ") + cudaGetErrorString(e));
-      }
-      if (graph) cudaGraphDestroy(graph);
+      rc = capture_graph(h->stream, [&] { return issue_step(h, false, true, false, nullptr, &n); }, &h->pipe_graph[j]);
       h->pipe_graph_compact[j] = hc;
     }
-    if (!rc && cudaGraphLaunch(h->pipe_graph[j], h->stream) != cudaSuccess) rc = fail(B2G_ECUDA, "graph launch failed");
+    if (!rc && cudaGraphLaunch(h->pipe_graph[j], h->stream) != cudaSuccess) rc = b2g_fail(B2G_ECUDA, "graph launch failed");
   } else {
     h->record_after_gather = h->ev_consumed[j];
     rc = issue_step(h, false, true, false, nullptr, &n);
@@ -1733,10 +1569,7 @@ int b2g_sac_step_host_pipelined(b2g_sac* h, const float* obs, const float* act, 
   if (rc) return rc;
   if (ptrace) cudaEventRecord(te[j][3], h->stream);
   // (3) this step's losses -> pinned slot j (read back by the NEXT call, or by b2g_sac_pipeline_flush)
-  CK(cudaMemcpyAsync(h->pm_met[j], h->metrics, MET_COUNT * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaMemcpyAsync(h->pm_met[j] + MET_COUNT, h->p("model/log_ent_coef"), sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaMemcpyAsync(h->pm_met[j] + MET_COUNT + 1, h->g("model/log_ent_coef"), sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaMemcpyAsync(h->pm_cnt[j], h->counters, 8 * sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
+  if (int rc = copy_metrics_async(h, h->pm_met[j], h->pm_cnt[j])) return rc;
   CK(cudaEventRecord(h->ev_met[j], h->stream));
   // (4) hand back the PREVIOUS step's losses: blocks only until step k-1 has finished, while step k's copies run
   if (have_prev) *have_prev = h->pipe_pending ? 1 : 0;
@@ -1749,9 +1582,9 @@ int b2g_sac_step_host_pipelined(b2g_sac* h, const float* obs, const float* act, 
 }
 
 int b2g_sac_pipeline_flush(b2g_sac* h, b2g_sac_metrics* last_out) {
-  if (!h) return fail(B2G_EINVAL, "NULL handle");
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   CK(cudaSetDevice(h->cfg.device));
-  if (!h->pipe_pending) return fail(B2G_ESTATE, "no pipelined step in flight");
+  if (!h->pipe_pending) return b2g_fail(B2G_ESTATE, "no pipelined step in flight");
   const int j = (int)((h->pipe_k - 1) & 1);
   CK(cudaEventSynchronize(h->ev_met[j]));
   if (last_out) fill_metrics(h, h->pm_met[j], h->pm_cnt[j], last_out);
@@ -1760,18 +1593,14 @@ int b2g_sac_pipeline_flush(b2g_sac* h, b2g_sac_metrics* last_out) {
 }
 
 int b2g_sac_act(b2g_sac* h, const float* obs, int n, int deterministic, float* act_out) {
-  if (!h || !obs || !act_out || n < 0) return fail(B2G_EINVAL, "bad argument");
+  if (!h || !obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
   CK(cudaSetDevice(h->cfg.device));
   const size_t E = h->E, A = h->A;
   refresh_planes(h);
   for (int done_n = 0; done_n < n; done_n += h->B) {
     const int chunk = std::min(h->B, n - done_n);
     CK(cudaMemcpyAsync(h->s_obs, obs + (size_t)done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-    PrepArgs pa{};
-    pa.counters = h->counters; pa.step_consts = h->step_consts; pa.lr = h->d_lr; pa.metrics = h->metrics;
-    pa.indices = h->indices; pa.eps = h->eps; pa.B = h->B; pa.A = h->A; pa.replay_size = nullptr;
-    pa.seed = h->cfg.seed ^ 0xA5A5A5A5DEADBEEFull; pa.gen = deterministic ? 0 : 1; pa.apply = 0;
-    prep_launch(pa, h->stream);
+    prep_launch(make_prep(h, h->cfg.seed ^ 0xA5A5A5A5DEADBEEFull, !deterministic, false), h->stream);
     GatherArgs g = make_gather(h, false, false);
     g.indices = nullptr;
     gather_launch(g, h->stream);
@@ -1797,10 +1626,10 @@ int b2g_launches_per_step(const b2g_sac* h) {
 float b2g_last_step_ms(const b2g_sac* h) { return h ? h->last_ms : 0.f; }
 
 int b2g_profile_step(b2g_sac* h, float lr, const char** names, float* ms, int cap) {
-  if (!h || !names || !ms) return fail(B2G_EINVAL, "NULL argument");
-  if (h->r_size < 1) return fail(B2G_ESTATE, "replay buffer is empty");
+  if (!h || !names || !ms) return b2g_fail(B2G_EINVAL, "NULL argument");
+  if (h->r_size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
   CK(cudaSetDevice(h->cfg.device));
-  if (int rc = set_lr(h, lr)) return rc;
+  if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
   refresh_planes(h);
   Prof prof;
   prof.on = true;

@@ -10,16 +10,7 @@
 #include "../../include/b200grasp.h"
 #include "cg.cuh"
 #include "common.cuh"
-
-extern thread_local std::string g_b2g_err;
-int b2g_fail(int code, const std::string& msg);
-#define B2G_CK(call)                                                                              \
-  do {                                                                                            \
-    cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess)                                                                        \
-      return b2g_fail(B2G_ECUDA, std::string(#call) + ": " + cudaGetErrorString(e_) + " @" + __FILE__ + ":" + \
-                                     std::to_string(__LINE__));                                   \
-  } while (0)
+#include "host.cuh"
 
 namespace b2g {
 struct Tensor {
@@ -61,7 +52,7 @@ struct V2State {
   uint16_t* K0n[2][2]{};         // [0] pi [513 -> 576 rows][64], [1] values packed [576 rows][192]
   float* z0v = nullptr;          // fc0 pre-activations of vf|q1|q2: [B][192]
   void* plane_jobs = nullptr; int n_plane_jobs = 0, plane_ctas = 0;
-  int* plane_cta_job = nullptr;  // job index of every CTA of the planes launch
+  const int* plane_cta_job = nullptr;  // job index of every CTA of the planes launch
   int sm_reserve = 0;           // SMs left to a collective that runs concurrently with the persistent GEMM grids
   std::vector<CUtensorMap> maps; // host copy
   std::vector<char> map_whole;   // per map: the box spans every plane
@@ -180,7 +171,7 @@ struct b2g_sac {
   float last_ms = 0.f;
   int launches = 0;
   std::vector<std::string> prof_names;
-  float* h_met = nullptr;        // pinned MET_COUNT floats
+  float* h_met = nullptr;        // pinned: MET_COUNT floats + [log_alpha, grad log_alpha]
   long long* h_cnt = nullptr;    // pinned counters
 
   b2g::V2State v2;
