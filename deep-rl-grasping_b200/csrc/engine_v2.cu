@@ -338,6 +338,10 @@ int fuse_groups(b2g_sac* h, const std::vector<const CgGroup*>& parts, const std:
       Pc.dep_expect += Pp.ws ? Pp.tiles_n : Pp.tiles_n * Pp.splits;
       continue;
     }
+    // a split-K producer signals its counters from the tiles of every split (or, finalised, from the last arriver): a split
+    // without chunks skips its tile and would leave the counters short forever
+    if (Pp.splits > 1 && (Pp.splits - 1) * ((Pp.chunks + Pp.splits - 1) / Pp.splits) >= Pp.chunks)
+      return b2g_fail(B2G_EINVAL, std::string("engine v2: a wired split-K producer has an empty split (fused launch ") + name + ")");
     if (ctr_of[pi] < 0) { ctr_of[pi] = n_ctr; n_ctr += Pp.tiles_m; }
     Pc.dep_rows = w.dep_rows; Pc.dep_rows_tile = w.dep_rows_tile; Pc.dep_tiles = Pp.tiles_m; Pc.dep_by_chunk = w.by_chunk;
     Pc.dep_expect = Pp.ws ? Pp.tiles_n : Pp.tiles_n * Pp.splits;   // x the signalling epilogue warps per tile (kernel side); split-K
@@ -356,6 +360,20 @@ void bind_counters(std::vector<CgGroup>& groups, int* base) {
       P.done_ctr = d ? base + (d - 1) : nullptr;
       P.dep_ctr = c ? base + (c - 1) : nullptr;
     }
+}
+
+// A K-split of `chunks` chunks into `splits` takes ceil(chunks / splits) chunks per split, so some counts leave the last
+// splits with none (16 chunks in 5 splits: 4 + 4 + 4 + 4 + 0).  An empty split of a finalised split-K tile never arrives at
+// the tile's ws_cnt, so no split is the last arriver, the tile is never finished and the tiles that wait on it spin forever.
+// Such a count is refused at create, with the counts that do work in the message.
+int check_split(const char* var, int chunks, int splits) {
+  auto empty = [chunks](int s) { return (s - 1) * ((chunks + s - 1) / s) >= chunks; };
+  if (!empty(splits)) return 0;
+  std::string ok;
+  for (int s = 1; s <= chunks; ++s)
+    if (!empty(s)) ok += (ok.empty() ? "" : ", ") + std::to_string(s);
+  return b2g_fail(B2G_EINVAL, std::string(var) + "=" + std::to_string(splits) + " leaves a K-split of " + std::to_string(chunks) +
+                                  " chunks empty; use one of " + ok);
 }
 
 }  // namespace
@@ -554,6 +572,7 @@ int v2_create(b2g_sac* h) {
         // 48 tiles of 16 K-chunks would hold 48 of the 132 SMs for the longest stretch of the forward launch: three K-splits per
         // tile, fp32 partial sums in a workspace, the last split to arrive finishes the tile (cg.cuh: ws)
         P.splits = v.split_fc1;
+        if (int rc = check_split("B2G_SPLIT_FC1", P.chunks, P.splits)) return rc;
         if (int rc = dev_alloc(h->allocs, h->stream, &P.ws, (size_t)P.tiles_m * P.tiles_n * 128 * 64)) return rc;
         if (int rc = dev_alloc(h->allocs, h->stream, &P.ws_cnt, (size_t)P.tiles_m * P.tiles_n * CG_EPI_WARPS)) return rc;
       }
@@ -629,6 +648,7 @@ int v2_create(b2g_sac* h) {
         P.colsum = h->g(std::string(nets[n]) + "/cnn3/b"); P.colsum_mask = 63;     // dZ3 row = [16 pixels][64 channels]
         if (v.split_fc1_dgrad > 1) {         // 32 tiles of 8 K-chunks at the head of the backward chain: split-K with finalisation
           P.splits = v.split_fc1_dgrad;
+          if (int rc = check_split("B2G_SPLIT_FC1_DGRAD", P.chunks, P.splits)) return rc;
           if (int rc = dev_alloc(h->allocs, h->stream, &P.ws, (size_t)P.tiles_m * P.tiles_n * 128 * 128)) return rc;
           if (int rc = dev_alloc(h->allocs, h->stream, &P.ws_cnt, (size_t)P.tiles_m * P.tiles_n * CG_EPI_WARPS)) return rc;
         }

@@ -83,6 +83,8 @@ def _check_step(cfg, params, vn, B, tol=TOL, precision=0):
         assert d.max() <= 2e-2 * LR + 1e-6 * np.abs(newp64[n]).max(), (n, d.max())
     print("errs", {k: f"{v:.2e}" for k, v in errs.items()})
     print("worst grad", worst_g, f"{gerr[worst_g]:.2e} (bar {gbar[worst_g]:.2e})", "worst update/bar", f"{worst_u:.3f}")
+    print(f"B={B} precision={precision} worst err/bar: outputs {max(errs[k] / bars[k] for k in errs):.3f},",
+          f"gradients {gerr[worst_g] / gbar[worst_g]:.3f}, update {worst_u:.3f}")
     L.close()
     bad = {k: (v, bars[k]) for k, v in errs.items() if not v <= bars[k]}
     assert not bad, f"outputs beyond tolerance: {bad}"
@@ -213,11 +215,14 @@ def test_sampled_step_from_replay_and_policy_act():
 def test_pipelined_host_batch_path_equals_explicit_path():
     """b2g_sac_step_host_pipelined (copy/compute overlap, losses one step late) must produce the same
     parameters and losses as b2g_sac_step_explicit on the same two batches."""
+    _check_pipelined_vs_explicit(16)
+
+
+def _check_pipelined_vs_explicit(B, precision=0):
     cfg, params, vn = load_case("sac_depth")
-    B = 16
     batches = [make_batch(vn, B, seed=300 + i) for i in range(3)]
-    A = make_learner(cfg, vn, B, params, precision=0)
-    Bm = make_learner(cfg, vn, B, params, precision=0)
+    A = make_learner(cfg, vn, B, params, precision=precision)
+    Bm = make_learner(cfg, vn, B, params, precision=precision)
     outs_a = [A.step_explicit(r["obs"], r["act"], r["rew"], r["next_obs"], r["done"], e, lr=LR) for r, _, e in batches]
     prev = [Bm.step_host_pipelined(r["obs"], r["act"], r["rew"], r["next_obs"], r["done"], e, lr=LR) for r, _, e in batches]
     assert prev[0] is None
