@@ -356,7 +356,7 @@ GatherArgs bgather(b2g_bdq* h, bool from_replay, bool with_next) {
   g.done = from_replay ? h->r_done : h->s_done;
   g.indices = from_replay ? h->indices : nullptr;
   g.mean = h->d_mean; g.var = h->d_istd; g.normc = h->d_normc;
-  g.B = h->B; g.H = 0; g.W = h->cfg.obs_dim; g.Cfull = 1; g.scale = 1.f;
+  g.B = h->B; g.H = 0; g.W = h->cfg.obs_dim; g.Cimg = 0; g.scale = 1.f;
   g.F_pi = h->Xscratch; g.F_v = h->X; g.F_t = h->Xn; g.FS = h->XS; g.feat_col = 0;
   g.rew_out = h->rew_n; g.done_out = h->done_n; g.n_act = h->D;
   return g;

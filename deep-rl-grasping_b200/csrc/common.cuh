@@ -227,16 +227,20 @@ struct PrepArgs {          // 1-CTA kernel at the head of every step
 void prep_launch(const PrepArgs& a, cudaStream_t s);
 
 // ---------------------------------------------------------------------------------------------
-// replay gather + VecNormalize + /255 (replay.cu)
+// replay row compaction, gather + VecNormalize + /255 (replay.cu)
 // ---------------------------------------------------------------------------------------------
+// full observations [n][HW][Cfull] -> compact rows (first_row + i) % wrap of dst: image planes [HW][Cfull-1] | value at pixel
+// [0,0] of the last plane | 3 zero pads
+void compact_rows(const float* src_full, float* dst, long long first_row, long long wrap, int n, int HW, int Cfull, cudaStream_t s);
+
 struct GatherArgs {
   const float* obs; const float* next_obs; const float* act; const float* rew; const float* done; // replay or staged batch
   const int* indices;        // [B] slot per sample (nullptr: identity)
-  const double* mean; const double* var; // [obs_elems]; var[] holds 1/sqrt(var+eps)
+  const double* mean; const double* var; // [row elems]; var[] holds 1/sqrt(var+eps)
   const double* normc;       // device: {1/sqrt(ret_var+eps), clip_obs, clip_rew, norm_obs, norm_rew}
-  int B, H, W, Cfull;        // CNN: obs [H,W,Cfull]; MLP: H = 0, W = obs_dim
+  int B, H, W, Cimg;         // CNN: compact rows of an [H,W,Cimg] image (replay.cu); MLP: H = 0, W = obs_dim
   float scale;               // 255 for CNN, 1 for MLP
-  float* x_obs; float* x_next;   // CNN: [B,H,W,Cfull-1] image planes (scaled)
+  float* x_obs; float* x_next;   // CNN: [B,H,W,Cimg] image planes (scaled)
   uint16_t* x_obs_hi; uint16_t* x_obs_lo; uint16_t* x_next_hi; uint16_t* x_next_lo;   // optional BF16 planes of x
   float* F_pi; float* F_v; float* F_t; int FS; int feat_col; // feature rows: direct feature -> col feat_col; MLP: whole obs -> cols 0..
   float* rew_out; float* done_out; int n_act;

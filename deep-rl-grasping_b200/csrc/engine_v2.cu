@@ -4,11 +4,10 @@
 // activation planes into implicit-im2col / shifted-window / zero-bordered operand tiles (one map per tensor: plane = outermost
 // dimension), (iii) the problem lists of every layer group and the two FUSED launches built from them (forward chain, backward
 // chain: fuse_groups wires each consumer problem to the producer tiles it reads) and (iv) the HBM-bound helper kernels around them:
-//   gather2_kernel : replay slot draw + compact-row gather + float64 VecNormalize + clip + /255 (replay.cu semantics,
-//                    [SB2] ReplayBuffer.sample(env=VecNormalize), observation_input(scale=True)), the 3-plane BF16 split and the
-//                    conv1 patch rows (8x8 stride-4 patches of the normalised image; the one view TMA cannot express, see
-//                    tools/tma_probe.cu) so that conv1 forward and its wgrad are plain 2-D TMA tiles;
-//   compact_kernel : full observation rows -> compact replay rows (image planes | actuator value);
+//   gather2_kernel : replay slot draw + gather of compact replay rows (the ring layout, replay.cu) + float64 VecNormalize +
+//                    clip + /255 (replay.cu semantics, [SB2] ReplayBuffer.sample(env=VecNormalize), observation_input(scale=True)),
+//                    the 3-plane BF16 split and the conv1 patch rows (8x8 stride-4 patches of the normalised image; the one view
+//                    TMA cannot express, see tools/tma_probe.cu) so that conv1 forward and its wgrad are plain 2-D TMA tiles;
 //   planes2_kernel : weights -> BF16 planes in the layouts the tensor maps expect (transposed / packed per consumer).
 // The bias gradients of the conv and cnn_fc1 layers come from the DGRAD epilogues of cg.cu (column sums of the gradient maps).
 // Reference shapes: custom_obs_policy.py:34-40 (conv 8x8/4 -> 4x4/2 -> 3x3/1, fc 1024->512), SURVEY.md Appendix A.
@@ -45,7 +44,7 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
   extern __shared__ uint16_t sm_planes[];            // [3][H*W*Ci]
   const GatherArgs& g = a.g;
   const int b = blockIdx.x, which = blockIdx.y, tid = threadIdx.x;
-  const int Ci = a.Ci, Cfull = g.Cfull, HW = g.H * g.W, npx = HW * Ci;
+  const int Ci = a.Ci, HW = g.H * g.W, npx = HW * Ci;
   const int Ec = npx + 4;                                  // compact replay row: image planes | actuator value | 3 pad floats
   long long slot = b;
   if (g.indices) slot = g.indices[b];
@@ -60,7 +59,6 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
   // shared-memory planes with a padded row pitch (+8 elements = +4 banks per image row): the patch pass below reads 16-byte runs
   // of 8 consecutive image rows at once, which a 128-byte pitch puts on the same four banks (8-way conflicts)
   const int rowe = g.W * Ci, pitch = rowe + 8, plane_e = g.H * pitch;
-  (void)Cfull;
   // image block: exactly the NHWC image with Ci channels -> no index arithmetic; float64 VecNormalize chain per element
   for (int e4 = tid; e4 < (npx >> 2); e4 += blockDim.x) {
     const float4 v = *reinterpret_cast<const float4*>(src + 4 * e4);
@@ -132,20 +130,6 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
       g.done_out[b] = g.done[slot];
     }
   }
-}
-
-// ------------------------------------------------------------------------------------------------ replay row compaction
-// full observation [HW][Cfull] -> compact row {image planes [HW][Ci] | value at pixel [0,0] of the last plane | 3 pad}
-__global__ void __launch_bounds__(256) compact_kernel(const float* __restrict__ src, float* __restrict__ dst, long long first_row, long long wrap,
-                                                       int HW, int Cfull, int Ec) {
-  const int Ci = Cfull - 1;
-  const float* s = src + (size_t)blockIdx.x * HW * Cfull;
-  float* d = dst + (size_t)((first_row + blockIdx.x) % wrap) * Ec;
-  for (int e = threadIdx.x; e < HW * Ci; e += blockDim.x) {
-    const int pix = e / Ci, c = e - pix * Ci;
-    d[e] = s[(size_t)pix * Cfull + c];
-  }
-  if (threadIdx.x < 4) d[HW * Ci + threadIdx.x] = threadIdx.x == 0 ? s[Ci] : 0.f;
 }
 
 // ------------------------------------------------------------------------------------------------ planes2
@@ -854,11 +838,6 @@ int v2_create(b2g_sac* h) {
 int v2_planes(b2g_sac* h, cudaStream_t s) {
   V2State& v = h->v2;
   planes2_kernel<<<v.plane_ctas, 256, 0, s>>>((const Plane2Job*)v.plane_jobs, v.plane_cta_job);
-  return 0;
-}
-
-int v2_compact_rows(b2g_sac* h, const float* src_full, float* dst, long long first_row, long long wrap, int n, cudaStream_t s) {
-  if (n > 0) compact_kernel<<<n, 256, 0, s>>>(src_full, dst, first_row, wrap, h->Hi * h->Wi, h->Cimg + 1, h->Ec);
   return 0;
 }
 

@@ -1,11 +1,16 @@
-// Replay-buffer minibatch gather fused with VecNormalize and the policy's /255 input scaling.
+// Replay rows: compaction of caller observations into the ring layout, and the minibatch gather fused with VecNormalize and
+// the policy's /255 input scaling.
 //
-// Restates [SB2] ReplayBuffer.sample(batch_size, env=vec_normalize) ->
-// VecNormalize.normalize_obs / normalize_reward (configured at sb_helper.py:118-119: clip_obs=10,
-// clip_reward=10, eps=1e-8; float64 arithmetic like numpy, cast to fp32 by the feed_dict) and
-// observation_input(scale=True) ((x-0)/255 for the Box(0,255) of robot.py:224-228), and the
-// channel split of custom_obs_policy.py:28-32 (last plane pixel [0,0] = direct feature).
-// HBM-bound: one coalesced pass over 2*B observations; no intermediate copies.
+// Ring layout.  MLP policy: a row is the observation vector.  CNN policy: a row is COMPACT, Ec = H*W*Ci + 4 floats -- the
+// image planes [H][W][Ci] (NHWC), then the one value of the constant actuator plane the network reads (pixel [0,0] of the last
+// channel, custom_obs_policy.py:28-32), then 3 zero pads.  Callers pass full [H][W][Ci+1] observations; compact_kernel
+// writes them into the ring, the explicit batch and policy inference's staging.
+//
+// gather_kernel restates [SB2] ReplayBuffer.sample(batch_size, env=vec_normalize) -> VecNormalize.normalize_obs /
+// normalize_reward (configured at sb_helper.py:118-119: clip_obs=10, clip_reward=10, eps=1e-8; float64 arithmetic like numpy,
+// cast to fp32 by the feed_dict) and observation_input(scale=True) ((x-0)/255 for the Box(0,255) of robot.py:224-228).
+// HBM-bound: one coalesced pass over 2*B rows; no intermediate copies.  It serves the round-1 engines and policy inference;
+// engine v2 reads the same rows with gather2_kernel (engine_v2.cu).
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -13,11 +18,43 @@
 namespace b2g {
 namespace {
 
+// full observation [HW][Cfull] -> compact row {image planes [HW][Ci] | value at pixel [0,0] of the last plane | 3 pad}
+__global__ void __launch_bounds__(256) compact_kernel(const float* __restrict__ src, float* __restrict__ dst, long long first_row, long long wrap,
+                                                       int HW, int Cfull, int Ec) {
+  const int Ci = Cfull - 1;
+  const float* s = src + (size_t)blockIdx.x * HW * Cfull;
+  float* d = dst + (size_t)((first_row + blockIdx.x) % wrap) * Ec;
+  for (int e = threadIdx.x; e < HW * Ci; e += blockDim.x) {
+    const int pix = e / Ci, c = e - pix * Ci;
+    d[e] = s[(size_t)pix * Cfull + c];
+  }
+  if (threadIdx.x < 4) d[HW * Ci + threadIdx.x] = threadIdx.x == 0 ? s[Ci] : 0.f;
+}
+
+// float64 VecNormalize of the 4 row elements [e, e + 4) (e % 4 == 0): clip((x - mean) * istd, +-clip_obs)
+__device__ __forceinline__ void load_norm4(const float* __restrict__ src, const GatherArgs& g, int e, bool norm_obs, double clip_obs,
+                                           float y[4]) {
+  const float4 v = *reinterpret_cast<const float4*>(src + e);
+  y[0] = v.x; y[1] = v.y; y[2] = v.z; y[3] = v.w;
+  if (norm_obs) {
+    const double2 m0 = *reinterpret_cast<const double2*>(g.mean + e), m1 = *reinterpret_cast<const double2*>(g.mean + e + 2);
+    const double2 s0 = *reinterpret_cast<const double2*>(g.var + e), s1 = *reinterpret_cast<const double2*>(g.var + e + 2);
+    const double mm[4] = {m0.x, m0.y, m1.x, m1.y}, ss[4] = {s0.x, s0.y, s1.x, s1.y};   // ss = 1/sqrt(var+eps)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      double d = ((double)y[j] - mm[j]) * ss[j];
+      d = fmin(fmax(d, -clip_obs), clip_obs);
+      y[j] = (float)d;
+    }
+  }
+}
+
 __global__ void __launch_bounds__(256) gather_kernel(GatherArgs g) {
   const int b = blockIdx.y;
   const int which = blockIdx.z;               // 0 = obs, 1 = next_obs
   const bool cnn = g.H > 0;
-  const int E = cnn ? g.H * g.W * g.Cfull : g.W;
+  const int npx = g.H * g.W * g.Cimg;         // CNN: image elements of a row (index of the actuator value)
+  const int E = cnn ? npx + 4 : g.W;
   long long slot = b;
   if (g.indices) slot = g.indices[b];
   else if (g.rng_counters) {
@@ -25,101 +62,65 @@ __global__ void __launch_bounds__(256) gather_kernel(GatherArgs g) {
     if (g.indices_out && which == 0 && blockIdx.x == 0 && threadIdx.x == 0) g.indices_out[b] = (int)slot;
   }
   const float* __restrict__ src = (which ? g.next_obs : g.obs) + (size_t)slot * E;
-  const int cimg = g.Cfull - 1;
   const double ret_istd = g.normc[0], clip_obs = g.normc[1], clip_rew = g.normc[2];
   const bool norm_obs = g.normc[3] != 0.0, norm_rew = g.normc[4] != 0.0;
   const float inv_scale_denom = g.scale;
-  float* __restrict__ xdst = (which ? g.x_next : g.x_obs);
-  uint16_t* __restrict__ xhi = which ? g.x_next_hi : g.x_obs_hi;
-  uint16_t* __restrict__ xlo = which ? g.x_next_lo : g.x_obs_lo;
-  // 4 consecutive elements per thread (128-bit loads); E % 4 == 0 for every supported shape except odd MLP sizes
-  const int E4 = (E & 3) == 0 ? E >> 2 : 0;
-  // Fast path for the depth configuration (one image channel + the actuator plane, channel-interleaved): a group of 4
-  // elements is 2 pixels and 2 actuator-plane values of which only pixel 0's is ever used, so the float64 chain, the
-  // IEEE division and the BF16 split run on 2 of the 4 lanes, indices need no run-time div/mod, and the three outputs
-  // are one vector store each.  The kernel is instruction-bound, not byte-bound (about 260 instructions per group before).
-  if (cnn && g.Cfull == 2 && E4 > 0) {
-    for (int e4 = blockIdx.x * blockDim.x + threadIdx.x; e4 < E4; e4 += gridDim.x * blockDim.x) {
-      const float4 v = *reinterpret_cast<const float4*>(src + 4 * e4);
-      float y0 = v.x, y1 = v.z, yf = v.y;
-      if (norm_obs) {
-        const double2 m0 = *reinterpret_cast<const double2*>(g.mean + 4 * e4), m1 = *reinterpret_cast<const double2*>(g.mean + 4 * e4 + 2);
-        const double2 s0 = *reinterpret_cast<const double2*>(g.var + 4 * e4), s1 = *reinterpret_cast<const double2*>(g.var + 4 * e4 + 2);
-        y0 = (float)fmin(fmax(((double)y0 - m0.x) * s0.x, -clip_obs), clip_obs);
-        y1 = (float)fmin(fmax(((double)y1 - m1.x) * s1.x, -clip_obs), clip_obs);
-        if (e4 == 0) yf = (float)fmin(fmax(((double)yf - m0.y) * s0.y, -clip_obs), clip_obs);
-      }
-      y0 = y0 / inv_scale_denom; y1 = y1 / inv_scale_denom;
-      const size_t o = (size_t)b * g.H * g.W + 2 * (size_t)e4;
-      *reinterpret_cast<float2*>(xdst + o) = make_float2(y0, y1);
+  if (cnn) {
+    // the image block is exactly the NHWC input x with Ci channels: 4-element group e4 of the row is group e4 of the sample's x
+    // (and of its BF16 planes).  b2g_sac_create requires (W * Ci) % 4 == 0, so npx and Ec are multiples of 4 and every 128-bit
+    // access here is aligned.
+    const size_t o = (size_t)b * npx;
+    float* __restrict__ xdst = (which ? g.x_next : g.x_obs) + o;
+    uint16_t* __restrict__ xhi = which ? g.x_next_hi : g.x_obs_hi;
+    uint16_t* __restrict__ xlo = which ? g.x_next_lo : g.x_obs_lo;
+    for (int e4 = blockIdx.x * blockDim.x + threadIdx.x; e4 < (npx >> 2); e4 += gridDim.x * blockDim.x) {
+      float y[4];
+      load_norm4(src, g, 4 * e4, norm_obs, clip_obs, y);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) y[j] = y[j] / inv_scale_denom;
+      *reinterpret_cast<float4*>(xdst + 4 * e4) = make_float4(y[0], y[1], y[2], y[3]);
       if (xhi) {
-        const __nv_bfloat16 h0 = __float2bfloat16_rn(y0), h1 = __float2bfloat16_rn(y1);
-        const __nv_bfloat16 l0 = __float2bfloat16_rn(y0 - __bfloat162float(h0)), l1 = __float2bfloat16_rn(y1 - __bfloat162float(h1));
-        *reinterpret_cast<uint32_t*>(xhi + o) = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-        *reinterpret_cast<uint32_t*>(xlo + o) = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-      }
-      if (e4 == 0) {
-        yf = yf / inv_scale_denom;
-        if (which) g.F_t[(size_t)b * g.FS + g.feat_col] = yf;
-        else { g.F_pi[(size_t)b * g.FS + g.feat_col] = yf; g.F_v[(size_t)b * g.FS + g.feat_col] = yf; }
+        uint16_t hi[4], lo[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const __nv_bfloat16 h = __float2bfloat16_rn(y[j]);
+          hi[j] = __bfloat16_as_ushort(h);
+          lo[j] = __bfloat16_as_ushort(__float2bfloat16_rn(y[j] - __bfloat162float(h)));
+        }
+        *reinterpret_cast<uint2*>(xhi + o + 4 * e4) = make_uint2((uint32_t)hi[0] | ((uint32_t)hi[1] << 16), (uint32_t)hi[2] | ((uint32_t)hi[3] << 16));
+        *reinterpret_cast<uint2*>(xlo + o + 4 * e4) = make_uint2((uint32_t)lo[0] | ((uint32_t)lo[1] << 16), (uint32_t)lo[2] | ((uint32_t)lo[3] << 16));
       }
     }
-  } else
-  for (int e4 = blockIdx.x * blockDim.x + threadIdx.x; e4 < E4; e4 += gridDim.x * blockDim.x) {
-    const float4 v = *reinterpret_cast<const float4*>(src + 4 * e4);
-    float y[4] = {v.x, v.y, v.z, v.w};
-    if (norm_obs) {
-      const double2 m0 = *reinterpret_cast<const double2*>(g.mean + 4 * e4), m1 = *reinterpret_cast<const double2*>(g.mean + 4 * e4 + 2);
-      const double2 s0 = *reinterpret_cast<const double2*>(g.var + 4 * e4), s1 = *reinterpret_cast<const double2*>(g.var + 4 * e4 + 2);
-      const double mm[4] = {m0.x, m0.y, m1.x, m1.y}, ss[4] = {s0.x, s0.y, s1.x, s1.y};   // ss = 1/sqrt(var+eps)
+    if (blockIdx.x == 0 && threadIdx.x == 0) {      // the actuator value -> the direct-feature column of the feature rows
+      float y = src[npx];
+      if (norm_obs) y = (float)fmin(fmax(((double)y - g.mean[npx]) * g.var[npx], -clip_obs), clip_obs);
+      y = y / inv_scale_denom;
+      if (which) g.F_t[(size_t)b * g.FS + g.feat_col] = y;
+      else { g.F_pi[(size_t)b * g.FS + g.feat_col] = y; g.F_v[(size_t)b * g.FS + g.feat_col] = y; }
+    }
+  } else {
+    // 4 consecutive elements per thread (128-bit loads) when the observation length allows it
+    const int E4 = (E & 3) == 0 ? E >> 2 : 0;
+    for (int e4 = blockIdx.x * blockDim.x + threadIdx.x; e4 < E4; e4 += gridDim.x * blockDim.x) {
+      float y[4];
+      load_norm4(src, g, 4 * e4, norm_obs, clip_obs, y);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        double d = ((double)y[j] - mm[j]) * ss[j];
-        d = fmin(fmax(d, -clip_obs), clip_obs);
-        y[j] = (float)d;
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int e = 4 * e4 + j;
-      const float yy = y[j] / inv_scale_denom;
-      if (cnn) {
-        const int c = e % g.Cfull, pix = e / g.Cfull;
-        if (c < cimg) {
-          const size_t o = ((size_t)b * g.H * g.W + pix) * cimg + c;
-          xdst[o] = yy;
-          if (xhi) {
-            const __nv_bfloat16 h = __float2bfloat16_rn(yy);
-            xhi[o] = __bfloat16_as_ushort(h);
-            xlo[o] = __bfloat16_as_ushort(__float2bfloat16_rn(yy - __bfloat162float(h)));
-          }
-        } else if (pix == 0) {
-          if (which) g.F_t[(size_t)b * g.FS + g.feat_col] = yy;
-          else { g.F_pi[(size_t)b * g.FS + g.feat_col] = yy; g.F_v[(size_t)b * g.FS + g.feat_col] = yy; }
-        }
-      } else {
+        const int e = 4 * e4 + j;
+        const float yy = y[j] / inv_scale_denom;
         if (which) g.F_t[(size_t)b * g.FS + e] = yy;
         else { g.F_pi[(size_t)b * g.FS + e] = yy; g.F_v[(size_t)b * g.FS + e] = yy; }
       }
     }
-  }
-  if (E4 == 0) {   // generic scalar path
-    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < E; e += gridDim.x * blockDim.x) {
-      float y = src[e];
-      if (norm_obs) {
-        double d = ((double)y - g.mean[e]) * g.var[e];
-        d = fmin(fmax(d, -clip_obs), clip_obs);
-        y = (float)d;
-      }
-      y = y / g.scale;
-      if (cnn) {
-        const int c = e % g.Cfull, pix = e / g.Cfull;
-        if (c < cimg) xdst[((size_t)b * g.H * g.W + pix) * cimg + c] = y;
-        else if (pix == 0) {
-          if (which) g.F_t[(size_t)b * g.FS + g.feat_col] = y;
-          else { g.F_pi[(size_t)b * g.FS + g.feat_col] = y; g.F_v[(size_t)b * g.FS + g.feat_col] = y; }
+    if (E4 == 0) {   // generic scalar path
+      for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < E; e += gridDim.x * blockDim.x) {
+        float y = src[e];
+        if (norm_obs) {
+          double d = ((double)y - g.mean[e]) * g.var[e];
+          d = fmin(fmax(d, -clip_obs), clip_obs);
+          y = (float)d;
         }
-      } else {
+        y = y / g.scale;
         if (which) g.F_t[(size_t)b * g.FS + e] = y;
         else { g.F_pi[(size_t)b * g.FS + e] = y; g.F_v[(size_t)b * g.FS + e] = y; }
       }
@@ -142,8 +143,12 @@ __global__ void __launch_bounds__(256) gather_kernel(GatherArgs g) {
 }
 }  // namespace
 
+void compact_rows(const float* src_full, float* dst, long long first_row, long long wrap, int n, int HW, int Cfull, cudaStream_t s) {
+  if (n > 0) compact_kernel<<<n, 256, 0, s>>>(src_full, dst, first_row, wrap, HW, Cfull, HW * (Cfull - 1) + 4);
+}
+
 void gather_launch(const GatherArgs& a, cudaStream_t s) {
-  const int E = a.H > 0 ? a.H * a.W * a.Cfull : a.W;
+  const int E = a.H > 0 ? a.H * a.W * a.Cimg + 4 : a.W;
   int gx = (E / 4 + 255) / 256;      // one 128-bit group per thread
   if (gx < 1) gx = 1;
   if (gx > 4) gx = 4;

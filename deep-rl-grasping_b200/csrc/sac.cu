@@ -4,7 +4,7 @@
 //   P  : parameter arena  [ model/pi | model/values_fn | log_ent_coef | target/values_fn ], every
 //        tensor padded to 32 floats, tensor order = SB zip parameter_list (SURVEY.md Appendix B)
 //   Mo, Vo, G : Adam moments and gradients, same offsets as the trainable part of P
-//   replay  : obs[cap,E] next_obs[cap,E] act[cap,A] rew[cap] done[cap]   (raw, un-normalised)
+//   replay  : obs[cap,Ec] next_obs[cap,Ec] act[cap,A] rew[cap] done[cap]   (raw, un-normalised; CNN: compact rows, replay.cu)
 //   batch   : x_obs/x_next [B,H,W,C] (normalised, /255), h1/h2/h3 per network, F rows [B,FS]
 //             (512 CNN features | direct feature | replay action | zero pad), gradient maps with
 //             zero borders (dZ3p, dZ2p) so the dgrad gathers need no bounds logic
@@ -633,7 +633,7 @@ GatherArgs make_gather(b2g_sac* h, bool from_replay, bool with_next) {
   g.mean = h->d_mean; g.var = h->d_istd;
   g.normc = h->d_normc;
   g.B = h->B;
-  g.H = h->cnn ? h->Hi : 0; g.W = h->cnn ? h->Wi : h->cfg.obs_dim; g.Cfull = h->cnn ? h->Cimg + 1 : 1;
+  g.H = h->cnn ? h->Hi : 0; g.W = h->cnn ? h->Wi : h->cfg.obs_dim; g.Cimg = h->cnn ? h->Cimg : 0;
   g.scale = h->cnn ? 255.f : 1.f;
   g.x_obs = h->x_obs; g.x_next = h->x_next;
   g.x_obs_hi = h->xp[0][0]; g.x_obs_lo = h->xp[0][1]; g.x_next_hi = h->xp[1][0]; g.x_next_lo = h->xp[1][1];
@@ -701,17 +701,6 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
   }
   if (h->v2.on) {
     if (!fork) { if (int rc = v2_planes(h, s)) return rc; ++n; mark("weight_planes_v2"); }
-    if (h->compact) {
-      if (!sampled && h->staged_compact) {     // host-pipelined batch: compacted on the host, before the copy
-        ga.obs = h->s_obs; ga.next_obs = h->s_next;
-      } else if (!sampled) {       // host-supplied batch (full layout): compact it like replay_add does
-        if (int rc = v2_compact_rows(h, h->s_obs, h->cs_obs, 0, h->B, h->B, s)) return rc;
-        if (int rc = v2_compact_rows(h, h->s_next, h->cs_next, 0, h->B, h->B, s)) return rc;
-        n += 2;
-        ga.obs = h->cs_obs; ga.next_obs = h->cs_next;
-      }
-      ga.mean = h->d_mean_c; ga.var = h->d_istd_c;
-    }
     if (int rc = v2_gather(h, ga, s)) return rc;
   } else gather_launch(ga, s);
   ++n; mark("gather_normalize");
@@ -931,6 +920,31 @@ int find_tensor(const b2g_sac* h, const char* name) {
   return it == h->tindex.end() ? -1 : it->second;
 }
 
+// element of a caller's observation that element e of a ring row holds; -1 for the pads of a compact row
+int full_index(const b2g_sac* h, int e) {
+  if (!h->cnn) return e;
+  const int Ci = h->Cimg, npx = h->Hi * h->Wi * Ci;
+  if (e < npx) return (e / Ci) * (Ci + 1) + e % Ci;
+  return e == npx ? Ci : -1;
+}
+
+// n caller observations (host or device memory) -> rows (first + i) % wrap of dst in the ring layout, on h->stream.  CNN: copied in
+// pieces through the full-layout staging buffer and compacted (stream order frees the buffer for the next piece); MLP: a plain
+// copy, for which first + n <= wrap.
+int load_rows(b2g_sac* h, const float* src, float* dst, long long first, long long wrap, long long n) {
+  const size_t E = h->E;
+  if (!h->cnn) {
+    CK(cudaMemcpyAsync(dst + first * E, src, n * E * sizeof(float), cudaMemcpyDefault, h->stream));
+    return 0;
+  }
+  for (long long i = 0; i < n; i += h->stage_rows) {
+    const int m = (int)std::min<long long>(h->stage_rows, n - i);
+    CK(cudaMemcpyAsync(h->obs_stage, src + i * E, m * E * sizeof(float), cudaMemcpyDefault, h->stream));
+    compact_rows(h->obs_stage, dst, first + i, wrap, m, h->Hi * h->Wi, h->Cimg + 1, h->stream);
+  }
+  return 0;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -1074,10 +1088,11 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
       return b2g_fail(B2G_EINVAL, "observation size must give a 4x4x64 conv3 output (64x64 input; cnn_fc1/w is (1024,512))");
     }
     h->E = h->Hi * h->Wi * cfg->obs_c;
+    h->Ec = h->Hi * h->Wi * h->Cimg + 4;
     h->feat_dim = 513;
   } else {
     if (cfg->obs_dim < 1) { delete h; return b2g_fail(B2G_EINVAL, "obs_dim must be positive for the MLP policy"); }
-    h->E = cfg->obs_dim;
+    h->E = h->Ec = cfg->obs_dim;
     h->feat_dim = cfg->obs_dim;
   }
   h->FS = (h->feat_dim + h->A + 7) / 8 * 8;
@@ -1094,22 +1109,20 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
   {   // engine v2 (TMA-fed, cg.cu) trains the 64x64 CNN policy in the parity mode
     h->v2.on = h->cnn && cfg->precision == B2G_PREC_BF16X3 && h->Hi == 64 && h->Wi == 64;
     if (const char* dbg = getenv("B2G_CG_DEBUG")) h->v2.dbg = atoi(dbg);
-    h->compact = h->v2.on;        // the v2 gather reads compact rows only
-    h->Ec = h->compact ? h->Hi * h->Wi * h->Cimg + 4 : h->E;
   }
-  // replay ring: 2 * cap * Ec * 4 bytes (depth: 32.8 GB at 1M slots in the compact layout, 65.6 GB in the full one)
+  // replay ring: 2 * cap * Ec * 4 bytes (depth: 32.8 GB at 1M slots; full rows would take 65.6 GB)
   DA(h->r_obs, cap * h->Ec); DA(h->r_next, cap * h->Ec); DA(h->r_act, cap * h->A); DA(h->r_rew, cap); DA(h->r_done, cap);
-  DA(h->d_mean, h->E); DA(h->d_istd, h->E); DA(h->d_normc, 8);
-  if (h->compact) {
-    DA(h->cs_obs, (size_t)B * h->Ec); DA(h->cs_next, (size_t)B * h->Ec); DA(h->add_stage, (size_t)2 * 256 * h->E);
-    DA(h->d_mean_c, h->Ec); DA(h->d_istd_c, h->Ec);
+  if (h->cnn) {
+    h->stage_rows = std::max(B, 256);
+    DA(h->obs_stage, (size_t)h->stage_rows * h->E);
   }
+  DA(h->d_mean, h->Ec); DA(h->d_istd, h->Ec); DA(h->d_normc, 8);
   for (int k = 0; k < 2; ++k) {
-    if (cudaMallocHost((void**)&h->hp_stats[k], (size_t)(2 * h->E + 2 * h->Ec + 8) * sizeof(double)) != cudaSuccess ||
+    if (cudaMallocHost((void**)&h->hp_stats[k], (size_t)(2 * h->Ec + 8) * sizeof(double)) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->ev_stats[k], cudaEventDisableTiming) != cudaSuccess)
       return bail(b2g_fail(B2G_ECUDA, "norm-stat staging"));
   }
-  DA(h->s_obs, (size_t)B * h->E); DA(h->s_next, (size_t)B * h->E); DA(h->s_act, B * h->A); DA(h->s_rew, B); DA(h->s_done, B);
+  DA(h->s_obs, (size_t)B * h->Ec); DA(h->s_next, (size_t)B * h->Ec); DA(h->s_act, B * h->A); DA(h->s_rew, B); DA(h->s_done, B);
   if (h->cnn) {
     DA(h->x_obs, (size_t)B * h->Hi * h->Wi * h->Cimg); DA(h->x_next, (size_t)B * h->Hi * h->Wi * h->Cimg);
     for (int n = 0; n < 3; ++n) {
@@ -1159,7 +1172,7 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
       cudaMallocHost((void**)&h->h_cnt, 8 * sizeof(long long)) != cudaSuccess)
     return bail(b2g_fail(B2G_ECUDA, "cudaMallocHost failed"));
   for (int j = 0; j < 2; ++j) {
-    if ((rc = dev_alloc(h->allocs, h->stream, &h->ps_obs[j], (size_t)B * h->E)) || (rc = dev_alloc(h->allocs, h->stream, &h->ps_next[j], (size_t)B * h->E))) return bail(rc);
+    if ((rc = dev_alloc(h->allocs, h->stream, &h->ps_obs[j], (size_t)B * h->Ec)) || (rc = dev_alloc(h->allocs, h->stream, &h->ps_next[j], (size_t)B * h->Ec))) return bail(rc);
     if (cudaEventCreateWithFlags(&h->ev_h2d[j], cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->ev_consumed[j], cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->ev_met[j], cudaEventDisableTiming) != cudaSuccess ||
@@ -1179,9 +1192,8 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
   }
   // identity normalisation until b2g_set_norm_stats is called
   {
-    std::vector<double> ones(std::max(h->E, h->Ec), 1.0);
-    if ((h->compact && cudaMemcpyAsync(h->d_istd_c, ones.data(), h->Ec * sizeof(double), cudaMemcpyHostToDevice, h->stream) != cudaSuccess) ||
-        cudaMemcpyAsync(h->d_istd, ones.data(), h->E * sizeof(double), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
+    std::vector<double> ones(h->Ec, 1.0);
+    if (cudaMemcpyAsync(h->d_istd, ones.data(), h->Ec * sizeof(double), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
         cudaStreamSynchronize(h->stream) != cudaSuccess)
       return bail(b2g_fail(B2G_ECUDA, "init copy failed"));
   }
@@ -1282,19 +1294,10 @@ int b2g_replay_add(b2g_sac* h, const float* obs, const float* act, const float* 
   const int64_t cap = h->cfg.buffer_capacity;
   int64_t done_n = 0;
   while (done_n < n) {
-    int64_t chunk = std::min(n - done_n, cap - h->r_pos);
+    const int64_t chunk = std::min(n - done_n, cap - h->r_pos);
     const size_t E = h->E, A = h->A;
-    if (h->compact) {       // full-layout rows are staged on the device and compacted into the ring
-      chunk = std::min<int64_t>(chunk, 256);
-      float* st0 = h->add_stage; float* st1 = h->add_stage + (size_t)256 * E;
-      CK(cudaMemcpyAsync(st0, obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-      CK(cudaMemcpyAsync(st1, next_obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-      if (int rc = v2_compact_rows(h, st0, h->r_obs, h->r_pos, cap, (int)chunk, h->stream)) return rc;
-      if (int rc = v2_compact_rows(h, st1, h->r_next, h->r_pos, cap, (int)chunk, h->stream)) return rc;
-    } else {
-    CK(cudaMemcpyAsync(h->r_obs + h->r_pos * E, obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_next + h->r_pos * E, next_obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-    }
+    if (int rc = load_rows(h, obs + done_n * E, h->r_obs, h->r_pos, cap, chunk)) return rc;
+    if (int rc = load_rows(h, next_obs + done_n * E, h->r_next, h->r_pos, cap, chunk)) return rc;
     CK(cudaMemcpyAsync(h->r_act + h->r_pos * A, act + done_n * A, chunk * A * sizeof(float), cudaMemcpyDefault, h->stream));
     CK(cudaMemcpyAsync(h->r_rew + h->r_pos, rew + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
     CK(cudaMemcpyAsync(h->r_done + h->r_pos, done + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
@@ -1315,22 +1318,16 @@ int b2g_replay_get(b2g_sac* h, int64_t slot, float* obs, float* act, float* rew,
   if (slot < 0 || slot >= h->r_size) return b2g_fail(B2G_EINVAL, "replay slot out of range");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
-  const size_t E = h->E, A = h->A;
-  if (h->compact) {        // expand: the actuator plane comes back as zeros except pixel [0,0] (all the policy ever reads of it)
-    std::vector<float> row(h->Ec);
-    const int Ci = h->Cimg, Cf = Ci + 1, HW = h->Hi * h->Wi;
-    for (int w = 0; w < 2; ++w) {
-      float* dst = w ? next_obs : obs;
-      if (!dst) continue;
-      CK(cudaMemcpy(row.data(), (w ? h->r_next : h->r_obs) + slot * h->Ec, h->Ec * sizeof(float), cudaMemcpyDeviceToHost));
-      for (int p = 0; p < HW; ++p) {
-        for (int c = 0; c < Ci; ++c) dst[(size_t)p * Cf + c] = row[(size_t)p * Ci + c];
-        dst[(size_t)p * Cf + Ci] = p == 0 ? row[(size_t)HW * Ci] : 0.f;
-      }
-    }
-  } else {
-  if (obs) CK(cudaMemcpy(obs, h->r_obs + slot * E, E * sizeof(float), cudaMemcpyDeviceToHost));
-  if (next_obs) CK(cudaMemcpy(next_obs, h->r_next + slot * E, E * sizeof(float), cudaMemcpyDeviceToHost));
+  const size_t A = h->A;
+  // expand the ring row: for the CNN policy the actuator plane comes back as zeros except pixel [0,0] (all the policy reads of it)
+  std::vector<float> row(h->Ec);
+  for (int w = 0; w < 2; ++w) {
+    float* dst = w ? next_obs : obs;
+    if (!dst) continue;
+    CK(cudaMemcpy(row.data(), (w ? h->r_next : h->r_obs) + slot * h->Ec, h->Ec * sizeof(float), cudaMemcpyDeviceToHost));
+    std::fill(dst, dst + h->E, 0.f);
+    for (int e = 0; e < h->Ec; ++e)
+      if (const int f = full_index(h, e); f >= 0) dst[f] = row[e];
   }
   if (act) CK(cudaMemcpy(act, h->r_act + slot * A, A * sizeof(float), cudaMemcpyDeviceToHost));
   if (rew) CK(cudaMemcpy(rew, h->r_rew + slot, sizeof(float), cudaMemcpyDeviceToHost));
@@ -1361,24 +1358,20 @@ int b2g_set_norm_stats(b2g_sac* h, const double* obs_mean, const double* obs_var
   const int k = h->stats_k++ & 1;
   CK(cudaEventSynchronize(h->ev_stats[k]));
   double* st = h->hp_stats[k];
-  const int E = h->E, Ec = h->Ec;
-  if (norm_obs) {
-    double* m = st; double* is = st + E; double* mc = st + 2 * E; double* isc = mc + Ec;
-    for (int i = 0; i < E; ++i) { m[i] = obs_mean[i]; is[i] = 1.0 / sqrt(obs_var[i] + eps); }
-    CK(cudaMemcpyAsync(h->d_mean, m, E * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_istd, is, E * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    if (h->compact) {
-      const int Ci = h->Cimg, Cf = Ci + 1, npx = h->Hi * h->Wi * Ci;
-      for (int e = 0; e < npx; ++e) { const int f = (e / Ci) * Cf + (e % Ci); mc[e] = m[f]; isc[e] = is[f]; }
-      mc[npx] = m[Ci]; isc[npx] = is[Ci];
-      for (int e = npx + 1; e < Ec; ++e) { mc[e] = 0.0; isc[e] = 1.0; }
-      CK(cudaMemcpyAsync(h->d_mean_c, mc, Ec * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-      CK(cudaMemcpyAsync(h->d_istd_c, isc, Ec * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  const int Ec = h->Ec;
+  if (norm_obs) {     // the caller's full-layout statistics, gathered into the ring layout
+    double* m = st; double* is = st + Ec;
+    for (int e = 0; e < Ec; ++e) {
+      const int f = full_index(h, e);
+      m[e] = f < 0 ? 0.0 : obs_mean[f];
+      is[e] = f < 0 ? 1.0 : 1.0 / sqrt(obs_var[f] + eps);
     }
+    CK(cudaMemcpyAsync(h->d_mean, m, Ec * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_istd, is, Ec * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   }
   h->ret_istd = 1.0 / sqrt(ret_var + eps);
   h->clip_obs = clip_obs; h->clip_rew = clip_rew; h->norm_obs = norm_obs; h->norm_rew = norm_reward;
-  double* nc = st + 2 * E + 2 * Ec;
+  double* nc = st + 2 * Ec;
   nc[0] = h->ret_istd; nc[1] = clip_obs; nc[2] = clip_rew; nc[3] = (double)norm_obs; nc[4] = (double)norm_reward; nc[5] = nc[6] = nc[7] = 0.0;
   CK(cudaMemcpyAsync(h->d_normc, nc, 8 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   CK(cudaEventRecord(h->ev_stats[k], h->stream));
@@ -1421,11 +1414,11 @@ int b2g_sac_step_explicit(b2g_sac* h, const float* obs, const float* act, const 
   if (!h || !obs || !act || !rew || !next_obs || !done || !eps) return b2g_fail(B2G_EINVAL, "NULL argument");
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
-  const size_t B = h->B, E = h->E, A = h->A;
+  const size_t B = h->B, A = h->A;
   refresh_planes(h, true);
   CK(cudaEventRecord(h->ev0, h->stream));
-  CK(cudaMemcpyAsync(h->s_obs, obs, B * E * sizeof(float), cudaMemcpyDefault, h->stream));
-  CK(cudaMemcpyAsync(h->s_next, next_obs, B * E * sizeof(float), cudaMemcpyDefault, h->stream));
+  if (int rc = load_rows(h, obs, h->s_obs, 0, B, B)) return rc;
+  if (int rc = load_rows(h, next_obs, h->s_next, 0, B, B)) return rc;
   CK(cudaMemcpyAsync(h->s_act, act, B * A * sizeof(float), cudaMemcpyDefault, h->stream));
   CK(cudaMemcpyAsync(h->s_rew, rew, B * sizeof(float), cudaMemcpyDefault, h->stream));
   CK(cudaMemcpyAsync(h->s_done, done, B * sizeof(float), cudaMemcpyDefault, h->stream));
@@ -1517,8 +1510,7 @@ int b2g_sac_step_host_pipelined(b2g_sac* h, const float* obs, const float* act, 
   }
   if (h->pipe_serial && k >= 1) CK(cudaStreamWaitEvent(h->cstream, h->ev_met[j ^ 1], 0));
   if (ptrace) cudaEventRecord(te[j][0], h->cstream);
-  const bool hc = h->compact;
-  if (hc) {
+  if (h->cnn) {
     // compact on the host (a few threads, ~0.1 ms) into pinned staging, copy half the bytes; the caller's arrays need not be
     // pinned and are free again when this call returns
     if (!h->hc_obs[0]) {
@@ -1548,23 +1540,17 @@ int b2g_sac_step_host_pipelined(b2g_sac* h, const float* obs, const float* act, 
   if (ptrace) cudaEventRecord(te[j][2], h->stream);
   float* keep_obs = h->s_obs; float* keep_next = h->s_next;
   h->s_obs = h->ps_obs[j]; h->s_next = h->ps_next[j];
-  h->staged_compact = hc;
   int n = 0, rc = 0;
   if (h->use_graph) {
     // one graph per staging slot (the slot's buffers are baked into the nodes): the ~30 runtime calls of an eagerly issued step
     // were the bottleneck of this path once the copy had shrunk
-    if (h->pipe_graph[j] && h->pipe_graph_compact[j] != hc) { cudaGraphExecDestroy(h->pipe_graph[j]); h->pipe_graph[j] = nullptr; }
-    if (!h->pipe_graph[j]) {
-      rc = capture_graph(h->stream, [&] { return issue_step(h, false, true, false, nullptr, &n); }, &h->pipe_graph[j]);
-      h->pipe_graph_compact[j] = hc;
-    }
+    if (!h->pipe_graph[j]) rc = capture_graph(h->stream, [&] { return issue_step(h, false, true, false, nullptr, &n); }, &h->pipe_graph[j]);
     if (!rc && cudaGraphLaunch(h->pipe_graph[j], h->stream) != cudaSuccess) rc = b2g_fail(B2G_ECUDA, "graph launch failed");
   } else {
     h->record_after_gather = h->ev_consumed[j];
     rc = issue_step(h, false, true, false, nullptr, &n);
     h->record_after_gather = nullptr;
   }
-  h->staged_compact = false;
   h->s_obs = keep_obs; h->s_next = keep_next;
   if (rc) return rc;
   if (ptrace) cudaEventRecord(te[j][3], h->stream);
@@ -1599,7 +1585,7 @@ int b2g_sac_act(b2g_sac* h, const float* obs, int n, int deterministic, float* a
   refresh_planes(h);
   for (int done_n = 0; done_n < n; done_n += h->B) {
     const int chunk = std::min(h->B, n - done_n);
-    CK(cudaMemcpyAsync(h->s_obs, obs + (size_t)done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
+    if (int rc = load_rows(h, obs + (size_t)done_n * E, h->s_obs, 0, h->B, chunk)) return rc;
     prep_launch(make_prep(h, h->cfg.seed ^ 0xA5A5A5A5DEADBEEFull, !deterministic, false), h->stream);
     GatherArgs g = make_gather(h, false, false);
     g.indices = nullptr;

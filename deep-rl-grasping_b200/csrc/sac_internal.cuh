@@ -76,7 +76,6 @@ int v2_alloc(b2g_sac* h);    // plane tensors (before the v1 groups are built: p
 int v2_create(b2g_sac* h);   // tensor maps + problem groups
 int v2_planes(b2g_sac* h, cudaStream_t s);
 int v2_gather(b2g_sac* h, const GatherArgs& ga, cudaStream_t s);
-int v2_compact_rows(b2g_sac* h, const float* src_full, float* dst, long long first_row, long long wrap, int n, cudaStream_t s);   // full [n][E] -> compact rows (first_row + i) % wrap
 int v2_launch(b2g_sac* h, const CgGroup& g, cudaStream_t s);
 }  // namespace b2g
 
@@ -95,10 +94,16 @@ struct b2g_sac {
   float* metrics = nullptr;
   cudaStream_t stream = nullptr;
   std::vector<void*> allocs;
-  // replay
+  // replay ring, raw (un-normalised) rows of Ec floats.  MLP policy: Ec = E.  CNN policy: COMPACT rows (replay.cu), Ec = H*W*Cimg
+  // + 4: the image planes, the ONE actuator value the policy reads (pixel [0,0] of the last plane; augmented_nature_cnn never
+  // reads the rest of it, custom_obs_policy.py:28-30) and 3 pad floats.  The explicit batch (s_obs / s_next) and the pipelined
+  // staging (ps_obs / ps_next) hold the same rows.
+  int Ec = 0;
   float *r_obs = nullptr, *r_next = nullptr, *r_act = nullptr, *r_rew = nullptr, *r_done = nullptr;
   int64_t r_size = 0, r_pos = 0;
-  // normalisation
+  float* obs_stage = nullptr;        // CNN: caller observations in the full layout [stage_rows][E] on their way to compact rows
+  int stage_rows = 0;
+  // normalisation, in the ring layout (pads: mean 0, istd 1)
   double *d_mean = nullptr, *d_istd = nullptr, *d_normc = nullptr;   // normc: ret_istd, clip_obs, clip_rew, norm_obs, norm_rew
   double ret_istd = 1.0, clip_obs = 10.0, clip_rew = 10.0;
   int norm_obs = 0, norm_rew = 0;
@@ -125,9 +130,7 @@ struct b2g_sac {
   float *ps_obs[2]{}, *ps_next[2]{};
   // host-pipelined steps, compact transfer: the constant actuator plane never crosses PCIe (b2g_sac_step_host_pipelined)
   float *hc_obs[2]{}, *hc_next[2]{};   // pinned host staging, compact rows [B][Ec]
-  bool staged_compact = false;         // the staged batch already is in compact rows
   cudaGraphExec_t pipe_graph[2]{};     // the step on staging slot j, captured once (b2g_sac_step_host_pipelined)
-  bool pipe_graph_compact[2]{};
   int host_threads = 16;
   cudaStream_t cstream = nullptr;
   cudaEvent_t ev_h2d[2]{}, ev_consumed[2]{}, ev_met[2]{};
@@ -175,13 +178,6 @@ struct b2g_sac {
   long long* h_cnt = nullptr;    // pinned counters
 
   b2g::V2State v2;
-  // compact replay rows (engine v2, CNN policy): image planes + the ONE actuator value the policy reads (pixel [0,0] of the
-  // last plane) + 3 pad floats; the rest of that plane is never read by augmented_nature_cnn (custom_obs_policy.py:28-30)
-  bool compact = false;
-  int Ec = 0;                        // floats per compact row
-  float *cs_obs = nullptr, *cs_next = nullptr;     // compacted explicit batch [B][Ec]
-  float* add_stage = nullptr;        // full-layout staging of replay_add chunks [2][ADD_CHUNK][E]
-  double *d_mean_c = nullptr, *d_istd_c = nullptr; // statistics in the compact layout
   double* hp_stats[2]{};             // pinned staging of set_norm_stats (asynchronous upload, no stream sync)
   cudaEvent_t ev_stats[2]{};
   int stats_k = 0;

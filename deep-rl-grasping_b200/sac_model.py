@@ -320,8 +320,8 @@ class SAC:
                 kw[k] = data[k]
         if isinstance(data.get("learning_rate"), (int, float)):
             kw["learning_rate"] = data["learning_rate"]
-        # The zip's buffer_size (1e6 in every shipped model) is the TRAINING ring: 2 * 1e6 * obs_elems * 4 B = 65.6 GB for
-        # depth, 164 GB for RGB-D.  A loaded model is used for inference or as a parameter donor (sb_helper.py:113-115 builds
+        # The zip's buffer_size (1e6 in every shipped model) is the TRAINING ring: 2 * 1e6 * (H*W*Ci + 4) * 4 B = 32.8 GB for
+        # depth, 131 GB for RGB-D.  A loaded model is used for inference or as a parameter donor (sb_helper.py:113-115 builds
         # a second model just to call get_parameters), so it gets a small ring unless the caller asks for one explicitly.
         kw["buffer_size"] = min(int(kw.get("buffer_size", 1000)), 1000)
         kw.update(kwargs)

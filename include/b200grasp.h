@@ -108,7 +108,9 @@ int b2g_replay_add(b2g_sac* h, const float* obs, const float* act, const float* 
                    const float* done, int64_t n);
 int64_t b2g_replay_size(const b2g_sac* h);
 /* ReplayBuffer.storage[slot] ([SB2] common/buffers.py): one stored (raw) transition back to the host; any output may be
- * NULL.  slot in [0, b2g_replay_size). */
+ * NULL.  slot in [0, b2g_replay_size).  CNN policy: the ring holds compact rows (see b2g_debug_compact_host), so obs and
+ * next_obs come back with the image planes as stored and the actuator plane zero except pixel [0,0], the one value the policy
+ * reads of it. */
 int b2g_replay_get(b2g_sac* h, int64_t slot, float* obs, float* act, float* rew, float* next_obs, float* done);
 /* What the LAST gradient step (any entry point, the CUDA-graph path included) drew and produced: the replay slots
  * indices[batch] (sampled steps only), the policy noise eps[batch, n_act], the per-sample rows q1,q2,v,logp,v_targ,

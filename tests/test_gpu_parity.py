@@ -212,6 +212,31 @@ def test_sampled_step_from_replay_and_policy_act():
     L.close()
 
 
+@pytest.mark.parametrize("case,precision", [("sac_depth", 0), ("sac_depth", 1), ("sac_rgbd", 0)])
+def test_replay_get_expands_compact_rows(case, precision):
+    """Every CNN handle stores compact replay rows: the image planes and the one actuator value the policy reads (pixel [0,0]
+    of the last plane).  replay_get returns the image planes bit-exact and the actuator plane as zeros except pixel [0,0],
+    which holds the stored value -- also when the caller's actuator plane is constant over the image, as the environment's is.
+    8 transitions into a 6-slot ring: slots 0 and 1 hold the wrapped ones."""
+    vn = dict(np.load(f"{GOLD}/vecnorm_{case}.npz"))
+    cfg = R.SACConfig(obs_shape=tuple(vn["obs_mean"].shape))
+    raw, _, _ = make_batch(vn, 8)
+    for k in ("obs", "next_obs"):
+        raw[k][..., -1] = raw[k][:, :1, :1, -1]            # constant actuator plane
+    L = make_learner(cfg, vn, 4, buffer_size=6, precision=precision)
+    L.replay_add(raw["obs"], raw["act"], raw["rew"], raw["next_obs"], raw["done"])
+    assert L.replay_size() == 6
+    for s in range(6):
+        t = s + 6 if s < 2 else s
+        got = L.replay_get(s)
+        for k in ("obs", "next_obs"):
+            assert np.array_equal(got[k][..., :-1], raw[k][t][..., :-1]), (s, k)
+            plane = got[k][..., -1]
+            assert plane[0, 0] == raw[k][t][0, 0, -1] and not plane.reshape(-1)[1:].any(), (s, k)
+        assert np.array_equal(got["act"], raw["act"][t]) and got["rew"] == raw["rew"][t] and got["done"] == raw["done"][t]
+    L.close()
+
+
 def test_pipelined_host_batch_path_equals_explicit_path():
     """b2g_sac_step_host_pipelined (copy/compute overlap, losses one step late) must produce the same
     parameters and losses as b2g_sac_step_explicit on the same two batches."""
