@@ -3,14 +3,16 @@
 // Persistent, warp-specialised kernel, one CTA per SM, grid = min(#tiles, #SMs):
 //   warps 0..7  : two consumer warpgroups.  Warpgroup w issues wgmma.mma_async for rows [64w, 64w + 64) of the 128-row tile
 //                 (BF16 planes from the swizzled ring, fp32 accumulators in registers).  Precision modes per problem: 1 product
-//                 (hi*hi), 3 products (2-plane split) or 6 products (3-plane split hi/mid/lo: everything down to 2^-24), issued as
-//                 1..3 WIDE MMAs per k-step (see mma_tile).  After the last K-chunk the same warps run the epilogue: the
+//                 (hi*hi), 3 products (2-plane split) or 6 products (3-plane split hi/mid/lo: everything down to 2^-24), one
+//                 MMA per product into the accumulator of its order (see mma_chunk), one K-chunk of them in flight while the
+//                 next chunk is awaited.  After the last K-chunk the same warps run the epilogue: the
 //                 accumulator columns pass, 16 at a time, through a small shared-memory staging block so that every lane ends up
 //                 with one output row; then bias/ReLU or the ReLU mask (+ the bias-gradient column sums), the split into BF16
 //                 planes and the row's 32-column stores of every plane (16-byte vectors).  The producers keep filling the ring
 //                 for the next tile meanwhile;
 //   warps 8..9  : TMA producers (whole warps, converged; one elected lane issues).  The cp.async.bulk.tensor boxes of a K-chunk
 //                 (operands x planes) are dealt round-robin to the two warps; warp 8 posts the chunk's expect_tx.
+//   warps 10..11: complete the producer warpgroup for setmaxnreg and exit.
 #include <cuda_bf16.h>
 
 #include <cstdio>
@@ -23,9 +25,14 @@
 namespace b2g {
 namespace {
 
-// warps 0..7: consumer warpgroups (MMA + epilogue), warps 8..9: TMA producers
+// warps 0..7: consumer warpgroups (MMA + epilogue), warps 8..11: producer warpgroup, of which warps 8..9 issue the TMA loads and
+// warps 10..11 only hand their registers over (setmaxnreg acts on whole warpgroups)
 constexpr int NEPI_WARPS = CG_EPI_WARPS, NPROD_WARPS = 2, PROD_WARP0 = NEPI_WARPS;
-constexpr int NTHREADS = 32 * (NEPI_WARPS + NPROD_WARPS);
+constexpr int NTHREADS = 32 * (NEPI_WARPS + 4);
+// registers per thread after setmaxnreg: 2 x 232 + 40 = 512 per SM sub-partition lane (each holds two consumer warps and one
+// producer warp), i.e. the whole 64K register file.  The consumers hold up to 128 accumulator registers across a mainloop in which
+// one chunk's wgmmas are always in flight; at the launch-time 168 they spilled inside it.
+constexpr int PROD_REGS = 40, CONS_REGS = 232;
 constexpr int STG_BYTES = 2 * 64 * 16 * 4;    // epilogue staging: per warpgroup 64 rows x 16 fp32 columns (rows of 64 B)
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -133,46 +140,72 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {    // lo -
   return d;
 }
 
-// The MMAs of one K-chunk for this warpgroup's m64 block: `planes` wide MMAs per k-step, A_p x [B_0 | .. | B_(planes-1-p)] ->
-// accumulator columns [p*n, planes*n).  Column group g therefore collects the products of order 2^(-8g): g0 = hi*hi,
-// g1 = hi*mid + mid*hi, g2 = hi*lo + mid*mid + lo*hi; keeping each order in its own columns keeps the accumulator's rounding
-// 2^-8g smaller on the correction terms, and the epilogue adds the groups small-to-large in fp32.  One wide MMA reads the A plane
-// from shared memory once for up to three products.  Column offset n is register offset n / 2 of the fragment (wgmma.cuh).
-// Tile width, product count and operand major-ness are template parameters: a run-time choice between wgmma sequences puts the
-// instructions on divergent paths, where the compiler serialises them.
-template <int NT, int NPROD, int TRANS, int NACC>
-__device__ __forceinline__ void mma_chunk(float (&acc)[NACC], uint32_t sbase, int ksteps, uint32_t a_off, uint32_t b_off, uint32_t a_ks,
-                                          uint32_t b_ks, uint32_t a_lbo, uint32_t b_lbo, uint32_t a_ps, uint32_t m_off) {
-  static_assert(NACC == NT / 2 * (NPROD >= 6 ? 3 : (NPROD >= 3 ? 2 : 1)) && (NPROD >= 6 ? 3 : (NPROD >= 3 ? 2 : 1)) * NT <= 256,
-                "accumulator of `planes` column groups of NT columns, at most 256 columns wide");
-  for (int k = 0; k < ksteps; ++k) {
-    const uint32_t pb = sbase + b_off + (uint32_t)k * b_ks;
-    const uint64_t db = TRANS ? desc_mn(pb, b_lbo) : desc_k(pb);
-    uint64_t da[3];
+// The MMAs of one K-chunk (KS k-steps) for this warpgroup's m64 block: one m64 x NT MMA per product, A_p x B_q accumulating into
+// order group g = p + q (NT / 2 registers each: g0 = hi*hi, g1 = hi*mid + mid*hi, g2 = hi*lo + mid*mid + lo*hi).  Keeping each
+// order in its own accumulator keeps the accumulator's rounding 2^-8g smaller on the correction terms, and the epilogue adds the
+// groups small-to-large in fp32.  Every MMA writes exactly one group's registers: ptxas only keeps wgmmas in flight back to back
+// when their accumulator ranges are identical or disjoint (partly overlapping ranges get a wait after every instruction).
+// Tile width, product count, operand major-ness and k-step count are template parameters: a run-time choice between wgmma
+// sequences, or a run-time trip count, puts the instructions on paths where the compiler serialises them.
+template <int NT, int NPROD, int TRANS, int KS, int NACC>
+__device__ __forceinline__ void mma_chunk(float (&acc)[NACC], uint32_t sbase, uint32_t a_off, uint32_t b_off, uint32_t a_ks, uint32_t b_ks,
+                                          uint32_t a_lbo, uint32_t b_lbo, uint32_t a_ps, uint32_t b_ps, uint32_t m_off) {
+  constexpr int NPL = NPROD >= 6 ? 3 : (NPROD >= 3 ? 2 : 1), G = NT / 2;      // planes = order groups; registers per group
+  static_assert(NACC == G * NPL, "one accumulator group of NT columns per product order");
 #pragma unroll
-    for (int pl = 0; pl < 3; ++pl) {
+  for (int k = 0; k < KS; ++k) {
+    uint64_t da[NPL], db[NPL];
+#pragma unroll
+    for (int pl = 0; pl < NPL; ++pl) {
       const uint32_t pa = sbase + (uint32_t)pl * a_ps + a_off + (uint32_t)k * a_ks + m_off;
+      const uint32_t pb = sbase + (uint32_t)pl * b_ps + b_off + (uint32_t)k * b_ks;
       da[pl] = TRANS ? desc_mn(pa, a_lbo) : desc_k(pa);
+      db[pl] = TRANS ? desc_mn(pb, b_lbo) : desc_k(pb);
     }
-    if constexpr (NPROD >= 6) {
-      Wgmma<3 * NT, TRANS>::mma(acc, da[0], db);
-      Wgmma<2 * NT, TRANS>::mma(acc + NT / 2, da[1], db);
-      Wgmma<NT, TRANS>::mma(acc + NT, da[2], db);
-    } else if constexpr (NPROD >= 3) {
-      Wgmma<2 * NT, TRANS>::mma(acc, da[0], db);
-      Wgmma<NT, TRANS>::mma(acc + NT / 2, da[1], db);
-    } else {
-      Wgmma<NT, TRANS>::mma(acc, da[0], db);
+    // per group, the products in the order of a wide A_p x [B_0 | ..] issue: g1 = A0 B1, A1 B0; g2 = A0 B2, A1 B1, A2 B0
+    Wgmma<NT, TRANS>::mma(acc, da[0], db[0]);
+    if constexpr (NPL >= 2) Wgmma<NT, TRANS>::mma(acc + G, da[0], db[1]);
+    if constexpr (NPL >= 3) Wgmma<NT, TRANS>::mma(acc + 2 * G, da[0], db[2]);
+    if constexpr (NPL >= 2) Wgmma<NT, TRANS>::mma(acc + G, da[1], db[0]);
+    if constexpr (NPL >= 3) {
+      Wgmma<NT, TRANS>::mma(acc + 2 * G, da[1], db[1]);
+      Wgmma<NT, TRANS>::mma(acc + 2 * G, da[2], db[0]);
     }
   }
 }
 
-// Consumer side of one tile with tile width NT, NPROD products per k-step and TRANS = MN-major operands: mainloop over the
-// tile's K-chunks, then the accumulators to one row per lane.  `s` / `ph`: ring slot and per-slot phase bits, carried by the
-// caller across tiles.  body(g, x) runs the epilogue of column group g of this thread's row (x = its 32 accumulator sums).
-template <int NT, int NPROD, int TRANS, class Body>
+// all lanes run it, lane `pred` arrives: a predicated instruction, not a branch (a divergent block between the wgmmas of a chunk
+// makes the compiler wait for every wgmma)
+__device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.u32 p, %1, 0;\n\t"
+      "@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t"
+      "}" ::"r"(bar), "r"((uint32_t)pred)
+      : "memory");
+}
+// trace stamp with the same rule: every lane reads the clock, lane `pred` stores
+__device__ __forceinline__ void stamp_if(long long* dst, bool pred) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      ".reg .u64 t;\n\t"
+      "mov.u64 t, %%clock64;\n\t"
+      "setp.ne.u32 p, %1, 0;\n\t"
+      "@p st.global.u64 [%0], t;\n\t"
+      "}" ::"l"(dst), "r"((uint32_t)pred)
+      : "memory");
+}
+
+// Consumer side of one tile with tile width NT, NPROD products and KS k-steps per K-chunk and TRANS = MN-major operands: mainloop
+// over the tile's K-chunks, then the accumulators to one row per lane.  `s` / `ph`: ring slot and per-slot phase bits, carried by
+// the caller across tiles.  body(g, x) runs the epilogue of column group g of this thread's row (x = its 32 accumulator sums).
+// ctrace: this warp's chunk stamps (nullptr: none), gc: the CTA's chunk counter, the index the producer stamps use.
+template <int NT, int NPROD, int TRANS, int KS, class Body>
 __device__ __forceinline__ void consume_tile(const CgProblem& P, const Tile& ti, uint32_t ring, uint32_t stg, int slot_bytes, int nstages, uint32_t& s,
-                                             uint32_t& ph, uint64_t* bar_full, uint64_t* bar_empty, bool nomma, Body&& body) {
+                                             uint32_t& ph, uint64_t* bar_full, uint64_t* bar_empty, bool nomma, long long* ctrace, uint32_t& gc,
+                                             Body&& body) {
   constexpr int NGRP = NPROD >= 6 ? 3 : (NPROD >= 3 ? 2 : 1);     // accumulator column groups (product orders)
   constexpr int NACC = NT / 2 * NGRP;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -180,21 +213,40 @@ __device__ __forceinline__ void consume_tile(const CgProblem& P, const Tile& ti,
   float acc[NACC];
 #pragma unroll
   for (int j = 0; j < NACC; ++j) acc[j] = 0.f;
-  const uint32_t a_ps = (uint32_t)P.a_pstride, a_off = P.a_off, b_off = P.b_off, a_ks = P.a_kstep, b_ks = P.b_kstep;
+  const uint32_t a_ps = (uint32_t)P.a_pstride, b_ps = (uint32_t)P.b_pstride, a_off = P.a_off, b_off = P.b_off, a_ks = P.a_kstep, b_ks = P.b_kstep;
   const uint32_t a_lbo = P.a_lbo, b_lbo = P.b_lbo;
   const uint32_t m_off = TRANS ? (uint32_t)wg * a_lbo : (uint32_t)wg * 8192u;     // rows [64 wg, 64 wg + 64) of the A tile
-  const int ksteps = nomma ? 0 : P.ksteps;
-  for (int c = ti.c_begin; c < ti.c_end; ++c) {
-    mbar_wait(smem_u32(&bar_full[s]), (ph >> s) & 1u);
-    const uint32_t sbase = ring + s * (uint32_t)slot_bytes;
-    wg_arrive();
-    mma_chunk<NT, NPROD, TRANS>(acc, sbase, ksteps, a_off, b_off, a_ks, b_ks, a_lbo, b_lbo, a_ps, m_off);
-    wg_commit();
+  // One chunk's MMAs stay in flight while the next chunk is awaited and issued; the slot of chunk c - 1 is released once
+  // wait_group 1 in chunk c has seen them finish.  Every lane runs the same instructions from the fence to the release: the
+  // release and the stamps are predicated, not branched on (see mbar_arrive_if).
+  // B2G_CG_DEBUG=2 (no MMA) takes a loop of its own: a branch inside the chunk loop would serialise the wgmmas as well.
+  uint32_t prev = 0;
+  if (nomma) {
+    for (int c = ti.c_begin; c < ti.c_end; ++c, ++gc) {
+      mbar_wait(smem_u32(&bar_full[s]), (ph >> s) & 1u);
+      mbar_arrive_if(smem_u32(&bar_empty[s]), lane == 0);
+      ph ^= 1u << s;
+      if (++s == (uint32_t)nstages) s = 0;
+    }
+  } else {
+    for (int c = ti.c_begin; c < ti.c_end; ++c, ++gc) {
+      long long* const tr = ctrace + gc * 8;
+      const bool stamp = ctrace != nullptr && lane == 0 && gc < 64;
+      stamp_if(tr + 3, stamp);
+      mbar_wait(smem_u32(&bar_full[s]), (ph >> s) & 1u);
+      stamp_if(tr + 4, stamp);
+      wg_arrive();
+      mma_chunk<NT, NPROD, TRANS, KS>(acc, ring + s * (uint32_t)slot_bytes, a_off, b_off, a_ks, b_ks, a_lbo, b_lbo, a_ps, b_ps, m_off);
+      wg_commit();
+      wg_wait<1>();
+      mbar_arrive_if(smem_u32(&bar_empty[prev]), lane == 0 && c > ti.c_begin);      // chunk c - 1's slot may be refilled
+      stamp_if(tr + 5, stamp);
+      prev = s;
+      ph ^= 1u << s;
+      if (++s == (uint32_t)nstages) s = 0;
+    }
     wg_wait<0>();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(smem_u32(&bar_empty[s]));      // the slot may be refilled
-    ph ^= 1u << s;
-    if (++s == (uint32_t)nstages) s = 0;
+    mbar_arrive_if(smem_u32(&bar_empty[prev]), lane == 0);
   }
   // correction column groups, smallest order first
   if constexpr (NGRP > 2) {
@@ -242,7 +294,7 @@ __device__ __forceinline__ void consume_tile(const CgProblem& P, const Tile& ti,
   }
 }
 
-// 10 warps per CTA: the SM sub-partition that holds three of them caps the kernel at 168 registers per thread.
+// 12 warps per CTA: 168 registers per thread at launch, then PROD_REGS / CONS_REGS.
 __global__ void __launch_bounds__(NTHREADS, 1)
 cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const CUtensorMap* __restrict__ maps, int max_stages,
           int dbg, long long* __restrict__ trace) {
@@ -264,7 +316,9 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
   pdl_wait();
 
   if (warp >= PROD_WARP0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PROD_REGS));
     const int pw = warp - PROD_WARP0;
+    if (pw >= NPROD_WARPS) return;
     // ============================================================================================ TMA producers
     {
       // Ring slot s and the phase parity of every slot (bit s of ph): the partition of the ring (slot size, slot count) belongs
@@ -356,18 +410,19 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
     }
   } else {
     // ============================================================================================ consumers: MMA + epilogue
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONS_REGS));
     const int ew = warp, half = (ew & 3) >> 1, q = 2 * (ew >> 2) + (ew & 1);
-    uint32_t it = 0, s = 0, ph = 0;
+    uint32_t it = 0, s = 0, ph = 0, gc = 0;
     int slot_bytes = 0, nstages = 1;
     Walker w;
+    long long* const ctrace = trace && blockIdx.x == trace_cta && ew == 0 ? trace : nullptr;     // chunk stamps: first consumer warp
     const int r = q * 32 + lane;                         // output row of this thread in the epilogue
     // per-problem constants of this thread, recomputed only when the CTA moves to another problem: the row's offset
     // inside a tile (the r -> (i0, i1, i2) decomposition needs integer divisions) and every descriptor field the tile loop reads
     int epi = 0, rows_tile = 0, lim_rows = 0, umma_n = 0, out_planes = 0, grp_stride = 32, n_valid = 0;
     long long roff = 0, rmoff = 0, o_tm = 0, m_tm = 0;
     int ri0 = 0, ri1 = 0, grp_tab = 0;
-    int nprod = 1;
-    bool mnm = false;
+    int shape = 0;
     const float* __restrict__ bias = nullptr;
     const uint16_t* __restrict__ mask = nullptr;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -379,8 +434,8 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
         const int i0 = r % d0, i12 = r / d0, i1 = i12 % d1, i2 = i12 / d1;
         roff = Q.o_base + (long long)i0 * Q.o0 + (long long)i1 * Q.o1 + (long long)i2 * Q.o2;
         rmoff = Q.m_base + (long long)i0 * Q.m0 + (long long)i1 * Q.m1 + (long long)i2 * Q.m2;
-        ri0 = i0; ri1 = i1; grp_tab = Q.grp_tab; nprod = Q.nprod;
-        mnm = Q.mn_major != 0;
+        ri0 = i0; ri1 = i1; grp_tab = Q.grp_tab;
+        shape = cg_shape_key(Q.umma_n, Q.nprod, Q.mn_major != 0, Q.ksteps);
         if (Q.slot_bytes != slot_bytes || Q.nstages != nstages) { slot_bytes = Q.slot_bytes; nstages = Q.nstages; s = 0; }
       }
       const Tile ti = w.tile(tile);
@@ -527,16 +582,17 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
         }
       };
       auto body0 = [&](int g, float (&x)[32]) { body(g, x, 0); };
-#define CG_CONSUME(NT, NPROD, TRANS) \
-  consume_tile<NT, NPROD, TRANS>(P, ti, ring, stg, slot_bytes, nstages, s, ph, bar_full, bar_empty, dbg_nomma, body0)
-      // the (width, products, major-ness) combinations cg_shape_supported() admits on the host; anything else is a bug: trap
-      switch (cg_shape_key(umma_n, nprod, mnm)) {
-        case cg_shape_key(32, 6, false): CG_CONSUME(32, 6, 0); break;
-        case cg_shape_key(64, 6, false): CG_CONSUME(64, 6, 0); break;
-        case cg_shape_key(64, 3, false): CG_CONSUME(64, 3, 0); break;
-        case cg_shape_key(128, 3, false): CG_CONSUME(128, 3, 0); break;
-        case cg_shape_key(64, 3, true): CG_CONSUME(64, 3, 1); break;
-        case cg_shape_key(128, 3, true): CG_CONSUME(128, 3, 1); break;
+#define CG_CONSUME(NT, NPROD, TRANS, KS) \
+  consume_tile<NT, NPROD, TRANS, KS>(P, ti, ring, stg, slot_bytes, nstages, s, ph, bar_full, bar_empty, dbg_nomma, ctrace, gc, body0)
+      // the (width, products, major-ness, k-steps) combinations cg_shape_supported() admits on the host; anything else is a bug: trap
+      switch (shape) {
+        case cg_shape_key(32, 6, false, 4): CG_CONSUME(32, 6, 0, 4); break;
+        case cg_shape_key(64, 6, false, 4): CG_CONSUME(64, 6, 0, 4); break;
+        case cg_shape_key(64, 3, false, 4): CG_CONSUME(64, 3, 0, 4); break;
+        case cg_shape_key(128, 3, false, 4): CG_CONSUME(128, 3, 0, 4); break;
+        case cg_shape_key(64, 3, true, 4): CG_CONSUME(64, 3, 1, 4); break;
+        case cg_shape_key(64, 3, true, 9): CG_CONSUME(64, 3, 1, 9); break;
+        case cg_shape_key(128, 3, true, 4): CG_CONSUME(128, 3, 1, 4); break;
         default: __trap();
       }
 #undef CG_CONSUME
@@ -582,10 +638,10 @@ EncodeTiledFn g_encode = nullptr;
 
 // ring budget (cg_finalize): the dynamic part minus the epilogue staging; the kernel's static shared memory (barriers) takes < 1 KiB
 // of the 227 KiB
-bool cg_shape_supported(int umma_n, int nprod, bool mn_major) {
-  switch (cg_shape_key(umma_n, nprod, mn_major)) {
-    case cg_shape_key(32, 6, false): case cg_shape_key(64, 6, false): case cg_shape_key(64, 3, false): case cg_shape_key(128, 3, false):
-    case cg_shape_key(64, 3, true): case cg_shape_key(128, 3, true): return true;
+bool cg_shape_supported(int umma_n, int nprod, bool mn_major, int ksteps) {
+  switch (cg_shape_key(umma_n, nprod, mn_major, ksteps)) {
+    case cg_shape_key(32, 6, false, 4): case cg_shape_key(64, 6, false, 4): case cg_shape_key(64, 3, false, 4): case cg_shape_key(128, 3, false, 4):
+    case cg_shape_key(64, 3, true, 4): case cg_shape_key(64, 3, true, 9): case cg_shape_key(128, 3, true, 4): return true;
     default: return false;
   }
 }

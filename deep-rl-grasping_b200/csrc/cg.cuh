@@ -44,8 +44,7 @@ struct CgProblem {
   int chunks, n2;
   // ---- operand fetch
   int nloads, planes;
-  int a_pstride, b_pstride;   // stage layout: [A plane 0 | A plane 1 | ..][B plane 0 | B plane 1 | ..]; bytes of one A / B plane.
-                              // The B planes are CONTIGUOUS so that one wgmma descriptor spans [B0|B1|B2] (see nprod)
+  int a_pstride, b_pstride;   // stage layout: [A plane 0 | A plane 1 | ..][B plane 0 | B plane 1 | ..]; bytes of one A / B plane
   int tx_bytes;               // bytes all boxes of one stage deliver (planes x sum of box bytes)
   int slot_bytes, nstages;    // stage ring geometry of THIS problem (cg_finalize): the problems of a launch share the ring's bytes, not
                               // its partition -- the ring is drained when the partition changes
@@ -53,14 +52,14 @@ struct CgProblem {
   const int* tm_tab;          // optional [tiles_m][CG_MAX_LOADS][2]: extra offsets of coordinates 1 and 2 per (tm, load)
   // ---- MMA
   int mn_major;               // 0: K-major A and B (rows = M|N, 128 B of K); 1: MN-major (rows = K, 128 B of M|N)
-  int ksteps;                 // wgmma K = 16 steps per chunk
+  int ksteps;                 // wgmma K = 16 steps per chunk (a template parameter of the kernel's mainloop: part of the shape key)
   int a_off, b_off;           // region offsets inside a stage (b_off = planes * a_pstride)
   int a_kstep, b_kstep;       // descriptor start-address advance per k-step (bytes)
   int a_lbo, b_lbo;           // MN-major: byte stride between 64-element atoms along M|N
   int umma_n;                 // tile width: 32, 64 or 128 (the widths cg_kernel is instantiated for)
-  int nprod;                  // products per k-step: 1 (hi*hi), 3 (+hi*lo, lo*hi), 6 (+mid terms of the 3-plane split), issued as
-                              // `planes` wide MMAs: A_p x [B_0 | .. | B_(planes-1-p)] into accumulator columns [p*n, planes*n), so
-                              // column group g collects the products of order 2^(-8g) (planes * umma_n <= 256)
+  int nprod;                  // products per k-step: 1 (hi*hi), 3 (+hi*lo, lo*hi), 6 (+mid terms of the 3-plane split), one MMA
+                              // each: A_p x B_q into accumulator group p + q, so group g collects the products of order 2^(-8g)
+                              // (planes * umma_n <= 256 accumulator columns)
   // ---- epilogue
   int epi;
   int rows_tile;              // real rows of a full tile (<= 128)
@@ -124,9 +123,11 @@ int cg_encode_map(CUtensorMap* out, const void* base, int rank, const uint64_t* 
 int cg_finalize(CgGroup& g, int smem_budget);
 cudaError_t cg_launch(const CgGroup& g, const CUtensorMap* dev_maps, int num_sms, cudaStream_t s, bool pdl, int debug_flags);
 int cg_smem_limit();
-// cg_kernel is compiled for a fixed set of (tile width, products per k-step, MN-major) shapes; a problem of any other shape is
-// rejected when its group is built
-__host__ __device__ constexpr int cg_shape_key(int umma_n, int nprod, bool mn_major) { return umma_n * 16 + nprod * 2 + (mn_major ? 1 : 0); }
-bool cg_shape_supported(int umma_n, int nprod, bool mn_major);
+// cg_kernel is compiled for a fixed set of (tile width, products per k-step, MN-major, k-steps per chunk) shapes; a problem of
+// any other shape is rejected when its group is built
+__host__ __device__ constexpr int cg_shape_key(int umma_n, int nprod, bool mn_major, int ksteps) {
+  return ksteps * 8192 + umma_n * 16 + nprod * 2 + (mn_major ? 1 : 0);
+}
+bool cg_shape_supported(int umma_n, int nprod, bool mn_major, int ksteps);
 
 }  // namespace b2g

@@ -289,7 +289,7 @@ int push_group(b2g_sac* h, std::vector<CgGroup>& list, CgGroup& g, const char* n
   for (int i = 0; i < g.n; ++i) {
     const CgProblem& P = g.host[i];
     if (P.planes * P.umma_n > 256) return b2g_fail(B2G_EINVAL, std::string("engine v2: planes x tile width exceeds one accumulator buffer (group ") + name + ")");
-    if (!cg_shape_supported(P.umma_n, P.nprod, P.mn_major != 0))
+    if (!cg_shape_supported(P.umma_n, P.nprod, P.mn_major != 0, P.ksteps))
       return b2g_fail(B2G_EINVAL, std::string("engine v2: no cg_kernel instance for the tile shape of a problem in group ") + name);
     g.flops += 2.0 * P.tiles_m * 128.0 * P.tiles_n * P.umma_n * P.chunks * 64.0;      // issued (tile-padded) work
   }
