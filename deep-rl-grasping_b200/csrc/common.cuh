@@ -139,23 +139,24 @@ struct TailArgs {
   float* pi_out;                               // [B,A]
   float* metrics;                              // accumulators (see MET_* in sac.cu)
 };
-void tail_launch(const TailArgs& a, cudaStream_t s);
+cudaError_t tail_launch(const TailArgs& a, cudaStream_t s);
 
 // Weight gradients of the head MLPs (fc0 / fc1 kernels and biases of pi, vf, qf1, qf2) in fp32 on the CUDA cores: 76 MFLOP
 // of [B]-deep reductions, too small for a tensor-engine launch (which would also hold every SM while it runs).
 struct HeadsWgradArgs {
   const float* X0[4];     // fc0 inputs: feature rows [B][x0_ld] (pi: F_pi; vf, qf1, qf2: F_values incl. the action columns)
   const float* dz0[4];    // fc0 pre-activation gradients [B][dz0_ld[q]] (column offset applied)
-  const float* a0[4];     // fc0 activations [B][64]
-  const float* dz1[4];    // fc1 pre-activation gradients [B][64]
+  const float* a0[4];     // fc0 activations [B][H]
+  const float* dz1[4];    // fc1 pre-activation gradients [B][H]
   float* g_k0[4]; float* g_b0[4]; float* g_k1[4]; float* g_b1[4];
   int M0[4];              // fc0 input width of head q (kernel rows)
   int dz0_ld[4];
   int x0_ld, B;
+  int H;                  // head width (a multiple of 64)
 };
 void heads_wgrad_launch(const HeadsWgradArgs& a, cudaStream_t s);
 // policy inference tail: tanh(mu) or tanh(mu + eps*std) for the first n rows of z0_pi
-void act_launch(const TailArgs& t, int n, int deterministic, float* act_out, cudaStream_t s);
+cudaError_t act_launch(const TailArgs& t, int n, int deterministic, float* act_out, cudaStream_t s);
 
 enum Metric : int {
   MET_POLICY_LOSS = 0, MET_QF1_LOSS, MET_QF2_LOSS, MET_VALUE_LOSS, MET_ENT_COEF_LOSS, MET_ENTROPY,

@@ -380,7 +380,7 @@ int v2_alloc(b2g_sac* h) {
       v.F[n][p] = bF + (n * 3 + p) * nf;
     }
   for (int w = 0; w < 2; ++w) for (int p = 0; p < 3; ++p) v.A1[w][p] = bA1 + (w * 3 + p) * na;
-  if (int rc = dev_alloc(h->allocs, h->stream, &v.z0v, (size_t)B * 192)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &v.z0v, (size_t)B * 3 * h->H)) return rc;
   // ---- gradient maps (2 planes) and natural-layout weight planes of the backward chain.  The planes of a tensor are
   //      equidistant in one allocation: the tensor maps address them through an extra (outermost) plane dimension
   auto palloc = [&](uint16_t** arr, int np, size_t count) -> int {
@@ -390,8 +390,8 @@ int v2_alloc(b2g_sac* h) {
     for (int p = 0; p < np; ++p) arr[p] = base + p * pitch;
     return 0;
   };
-  if (int rc = palloc(v.dz0pi, 2, (size_t)B * 64)) return rc;
-  if (int rc = palloc(v.dz0v, 2, (size_t)B * 192)) return rc;
+  if (int rc = palloc(v.dz0pi, 2, (size_t)B * h->H)) return rc;
+  if (int rc = palloc(v.dz0v, 2, (size_t)B * 3 * h->H)) return rc;
   if (int rc = palloc(v.dZ1, 2, (size_t)B * 225 * 64)) return rc;
   for (int n = 0; n < 2; ++n) {
     if (int rc = palloc(v.dZ4[n], 2, (size_t)B * 512)) return rc;
@@ -400,7 +400,7 @@ int v2_alloc(b2g_sac* h) {
     if (int rc = palloc(v.W2n[n], 2, 512 * 64)) return rc;
     if (int rc = palloc(v.W3n[n], 2, 576 * 64)) return rc;
     if (int rc = palloc(v.Wfn[n], 2, 1024 * 512)) return rc;
-    if (int rc = palloc(v.K0n[n], 2, (size_t)KF * (n == 1 ? 192 : 64))) return rc;
+    if (int rc = palloc(v.K0n[n], 2, (size_t)KF * (n == 1 ? 3 : 1) * h->H)) return rc;
   }
   // ---- weight planes
   if (int rc = palloc(v.W1T[0], 3, (size_t)64 * K1)) return rc;
@@ -409,7 +409,7 @@ int v2_alloc(b2g_sac* h) {
     if (int rc = palloc(v.W2T[n], 3, 64 * 512)) return rc;
     if (int rc = palloc(v.W3T[n], 3, 64 * 576)) return rc;
     if (int rc = palloc(v.WfT[n], 3, 512 * 1024)) return rc;
-    if (int rc = palloc(v.K0T[n], 3, (size_t)(n == 1 ? 192 : 64) * KF)) return rc;
+    if (int rc = palloc(v.K0T[n], 3, (size_t)(n == 1 ? 3 : 1) * h->H * KF)) return rc;
   }
   return 0;
 }
@@ -417,7 +417,7 @@ int v2_alloc(b2g_sac* h) {
 int v2_create(b2g_sac* h) {
   V2State& v = h->v2;
   g_mk_state = &v;
-  const int B = h->B, Ci = h->Cimg, K1 = 64 * Ci, KF = v.KF, FS = h->FS;
+  const int B = h->B, Ci = h->Cimg, K1 = 64 * Ci, KF = v.KF, FS = h->FS, H = h->H;
   const size_t n1 = (size_t)B * 225 * 32;
   // ---- plane jobs (weights change every step)
   const char* nets[3] = {"model/pi", "model/values_fn", "target/values_fn"};
@@ -438,20 +438,20 @@ int v2_create(b2g_sac* h) {
     add_job(h->p(std::string(nets[n]) + "/cnn3/w"), 576, 64, v.W3T[n], 3, 1, 576, 0);
     add_job(h->p(std::string(nets[n]) + "/cnn_fc1/w"), 1024, 512, v.WfT[n], 3, 1, 1024, 0);
   }
-  add_job(h->p("model/pi/fc0/kernel"), h->feat_dim, 64, v.K0T[0], 3, 1, KF, 0);
-  add_job(h->p("model/values_fn/vf/fc0/kernel"), h->feat_dim, 64, v.K0T[1], 3, 1, KF, 0);
-  add_job(h->p("model/values_fn/qf1/fc0/kernel"), h->feat_dim + h->A, 64, v.K0T[1], 3, 1, KF, 64);
-  add_job(h->p("model/values_fn/qf2/fc0/kernel"), h->feat_dim + h->A, 64, v.K0T[1], 3, 1, KF, 128);
-  add_job(h->p("target/values_fn/vf/fc0/kernel"), h->feat_dim, 64, v.K0T[2], 3, 1, KF, 0);
+  add_job(h->p("model/pi/fc0/kernel"), h->feat_dim, H, v.K0T[0], 3, 1, KF, 0);
+  add_job(h->p("model/values_fn/vf/fc0/kernel"), h->feat_dim, H, v.K0T[1], 3, 1, KF, 0);
+  add_job(h->p("model/values_fn/qf1/fc0/kernel"), h->feat_dim + h->A, H, v.K0T[1], 3, 1, KF, H);
+  add_job(h->p("model/values_fn/qf2/fc0/kernel"), h->feat_dim + h->A, H, v.K0T[1], 3, 1, KF, 2 * H);
+  add_job(h->p("target/values_fn/vf/fc0/kernel"), h->feat_dim, H, v.K0T[2], 3, 1, KF, 0);
   for (int n = 0; n < 2; ++n) {
     add_job(h->p(std::string(nets[n]) + "/cnn2/w"), 512, 64, v.W2n[n], 2, 0, 64, 0);
     add_job(h->p(std::string(nets[n]) + "/cnn3/w"), 576, 64, v.W3n[n], 2, 0, 64, 0);
     add_job(h->p(std::string(nets[n]) + "/cnn_fc1/w"), 1024, 512, v.Wfn[n], 2, 0, 512, 0);
   }
-  add_job(h->p("model/pi/fc0/kernel"), h->feat_dim, 64, v.K0n[0], 2, 0, 64, 0);
-  add_job(h->p("model/values_fn/vf/fc0/kernel"), h->feat_dim, 64, v.K0n[1], 2, 0, 192, 0);
-  add_job(h->p("model/values_fn/qf1/fc0/kernel"), h->feat_dim + h->A, 64, v.K0n[1], 2, 0, 192, 64);
-  add_job(h->p("model/values_fn/qf2/fc0/kernel"), h->feat_dim + h->A, 64, v.K0n[1], 2, 0, 192, 128);
+  add_job(h->p("model/pi/fc0/kernel"), h->feat_dim, H, v.K0n[0], 2, 0, H, 0);
+  add_job(h->p("model/values_fn/vf/fc0/kernel"), h->feat_dim, H, v.K0n[1], 2, 0, 3 * H, 0);
+  add_job(h->p("model/values_fn/qf1/fc0/kernel"), h->feat_dim + h->A, H, v.K0n[1], 2, 0, 3 * H, H);
+  add_job(h->p("model/values_fn/qf2/fc0/kernel"), h->feat_dim + h->A, H, v.K0n[1], 2, 0, 3 * H, 2 * H);
   v.n_plane_jobs = (int)jobs.size();
   v.plane_ctas = start;
   Plane2Job* dj = nullptr;
@@ -564,12 +564,12 @@ int v2_create(b2g_sac* h) {
     }
     if (int rc = push_group(h, v.fwd, g, "fc1_fwd")) return rc;
   }
-  // ---- head fc0 layers: pi [513->64], values vf|q1|q2 [518->192] on the shared feature rows, target vf
+  // ---- head fc0 layers: pi [513->H], values vf|q1|q2 [518->3H] on the shared feature rows, target vf
   {
     CgGroup g;
     float* z0out[3] = {h->z0[0], v.z0v, h->z0[4]};
     for (int n = 0; n < 3; ++n) {
-      const int Nn = n == 1 ? 192 : 64;
+      const int Nn = n == 1 ? 3 * H : H;
       const int mA = add_maps(v, v.F[n], NP, 2, {(uint64_t)KF, (uint64_t)B}, {(uint64_t)KF * 2}, {64, 128});
       const int mB = add_maps(v, v.K0T[n], NP, 2, {(uint64_t)KF, (uint64_t)Nn}, {(uint64_t)KF * 2}, {64, 64});
       if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (fc0)");
@@ -593,7 +593,7 @@ int v2_create(b2g_sac* h) {
   {
     CgGroup g;
     for (int n = 0; n < 2; ++n) {
-      const int Kd = n == 0 ? 64 : 192;
+      const int Kd = n == 0 ? H : 3 * H;
       uint16_t* const* dz = n == 0 ? v.dz0pi : v.dz0v;
       const int mA = add_maps(v, dz, NB, 2, {(uint64_t)Kd, (uint64_t)B}, {(uint64_t)Kd * 2}, {64, 128});
       const int mB = add_maps(v, v.K0n[n], NB, 2, {(uint64_t)Kd, (uint64_t)KF}, {(uint64_t)Kd * 2}, {64, 128});

@@ -177,7 +177,8 @@ int build_groups(b2g_sac* h) {
   TAB(rowFS, iota_tab(B, FS));
   TAB(row3H, iota_tab(B, 3 * H));
   TAB(iFS, iota_tab(FS));
-  TAB(kH, iota_tab(FS, H));         // j*H  (fc0 kernel rows)
+  TAB(iH, iota_tab(H));             // head columns
+  TAB(kH, iota_tab(std::max(FS, H), H));   // j*H  (fc0 / fc1 kernel rows)
 
   auto nn = [&](int net, const char* s) { return std::string(nets[net]) + s; };
 
@@ -283,7 +284,7 @@ int build_groups(b2g_sac* h) {
         g.name = "heads_dgrad";
         TAB(row512, iota_tab(B, 512));
         // pi
-        GemmDesc d = gemm_desc(h->dz0_pi, rowH, i64, h->p("model/pi/fc0/kernel"), i64, kH, h->dZ4[0], row512, i512, B, 512, H,
+        GemmDesc d = gemm_desc(h->dz0_pi, rowH, iH, h->p("model/pi/fc0/kernel"), iH, kH, h->dZ4[0], row512, i512, B, 512, H,
                         GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
         d.mask = h->F[0]; d.kM = rowFS; d.kN = i512;
         if (h->use_planes) { d.C_hi = h->dZ4p[0][0]; d.C_lo = h->dZ4p[0][1]; }
@@ -484,7 +485,7 @@ int build_groups(b2g_sac* h) {
     const int fnet[5] = {0, 1, 1, 1, 2};
     for (int q = 0; q < 5; ++q) {
       const int R = (q == 2 || q == 3) ? fd + A : fd;
-      g.host.push_back(gemm_desc(h->F[fnet[q]], rowFS, iFS, h->p(hk[q]), kH, i64, h->z0[q], rowH, i64, B, H, R, GG_A_RVEC));
+      g.host.push_back(gemm_desc(h->F[fnet[q]], rowFS, iFS, h->p(hk[q]), kH, iH, h->z0[q], rowH, iH, B, H, R, GG_A_RVEC));
     }
     GemmGroup a = g;
     // training step: the 516-deep reduction of each head is split over several CTAs (atomic accumulation into the
@@ -507,11 +508,11 @@ int build_groups(b2g_sac* h) {
     for (int q = 0; q < 4; ++q) {
       const int M = (q >= 2) ? fd + A : fd;
       const float* dz0 = q == 0 ? h->dz0_pi : h->dz0_v3;
-      GemmDesc w0 = gemm_desc(h->F[q == 0 ? 0 : 1], iFS, rowFS, dz0, dzrow[q], i64, h->g(std::string(hp[q]) + "/fc0/kernel"), kH, i64, M, H, B,
+      GemmDesc w0 = gemm_desc(h->F[q == 0 ? 0 : 1], iFS, rowFS, dz0, dzrow[q], iH, h->g(std::string(hp[q]) + "/fc0/kernel"), kH, iH, M, H, B,
                        GG_COLSUM);
       w0.colsum = h->g(std::string(hp[q]) + "/fc0/bias");
       g.host.push_back(w0);
-      GemmDesc w1 = gemm_desc(h->a0[q], i64, rowH, h->dz1[q], rowH, i64, h->g(std::string(hp[q]) + "/fc1/kernel"), kH, i64, H, H, B, GG_COLSUM);
+      GemmDesc w1 = gemm_desc(h->a0[q], iH, rowH, h->dz1[q], rowH, iH, h->g(std::string(hp[q]) + "/fc1/kernel"), kH, iH, H, H, B, GG_COLSUM);
       w1.colsum = h->g(std::string(hp[q]) + "/fc1/bias");
       g.host.push_back(w1);
     }
@@ -727,7 +728,7 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
     for (auto& g : h->fwd_groups) if (int rc = run_group(g, s)) return rc;
   }
   if (fork) CK(cudaStreamWaitEvent(s, h->ev_aux[6], 0));
-  tail_launch(make_tail(h, want_per_sample), s); ++n; mark("heads_tail");
+  CK(tail_launch(make_tail(h, want_per_sample), s)); ++n; mark("heads_tail");
   auto make_optim = [&]() {
     OptimArgs oa{};
     oa.P = h->P; oa.Mo = h->Mo; oa.Vo = h->Vo; oa.G = h->G; oa.T = h->P + h->n_train;
@@ -764,7 +765,7 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
       wa.g_k0[q] = h->g(std::string(hp[q]) + "/fc0/kernel"); wa.g_b0[q] = h->g(std::string(hp[q]) + "/fc0/bias");
       wa.g_k1[q] = h->g(std::string(hp[q]) + "/fc1/kernel"); wa.g_b1[q] = h->g(std::string(hp[q]) + "/fc1/bias");
     }
-    wa.x0_ld = h->FS; wa.B = h->B;
+    wa.x0_ld = h->FS; wa.B = h->B; wa.H = h->H;
     heads_wgrad_launch(wa, lx); ++n; if (!fork) mark("heads_wgrad");
     // single GPU: the chain heads_dgrad .. conv wgrads is one fused launch.  Overlapped all-reduce: two (cut after cnn_fc1, where
     // the early all-reduce starts).
@@ -1062,7 +1063,8 @@ int b2g_sac_destroy(b2g_sac* h) {
 int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
   if (!cfg || !out) return b2g_fail(B2G_EINVAL, "cfg/out is NULL");
   *out = nullptr;
-  if (cfg->hidden != 64) return b2g_fail(B2G_EINVAL, "hidden must be 64 (SAC.layers [64,64], config/gripper_grasp.yaml:81)");
+  if (cfg->hidden != 64 && cfg->hidden != 128 && cfg->hidden != 192 && cfg->hidden != 256)
+    return b2g_fail(B2G_EINVAL, "hidden must be 64, 128, 192 or 256 (SAC.layers [H, H])");
   if (cfg->n_act < 1 || cfg->n_act > 8) return b2g_fail(B2G_EINVAL, "n_act must be in [1,8]");
   if (cfg->batch < 1 || cfg->buffer_capacity < 1) return b2g_fail(B2G_EINVAL, "batch and buffer_capacity must be positive");
   if (cfg->nranks < 1 || cfg->rank < 0 || cfg->rank >= cfg->nranks) return b2g_fail(B2G_EINVAL, "bad rank/nranks");
@@ -1594,7 +1596,7 @@ int b2g_sac_act(b2g_sac* h, const float* obs, int n, int deterministic, float* a
       if (gr.tc) CK(gg_tc_launch(gr.host.data(), (int)gr.host.size(), gr.total_tiles, gr.host[0].flags, h->cfg.precision == B2G_PREC_BF16X3 ? 1 : 0, h->num_sms, h->stream));
       else gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
     }
-    b2g::act_launch(make_tail(h, false), chunk, deterministic, h->pi_out, h->stream);
+    CK(b2g::act_launch(make_tail(h, false), chunk, deterministic, h->pi_out, h->stream));
     CK(cudaMemcpyAsync(act_out + (size_t)done_n * A, h->pi_out, chunk * A * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
   }

@@ -34,8 +34,8 @@ struct V2State {
   uint16_t* H3[3][3]{};          // [B][1024]
   uint16_t* F[3][3]{};           // [B][KF]
   // gradient maps, 2 planes
-  uint16_t* dz0pi[2]{};          // [B][64]
-  uint16_t* dz0v[2]{};           // [B][192]
+  uint16_t* dz0pi[2]{};          // [B][H]
+  uint16_t* dz0v[2]{};           // [B][3H]
   uint16_t* dZ4[2][2]{};         // [net][plane] [B][512]
   uint16_t* dZ3[2][2]{};         // [B*16][64]
   uint16_t* dZ2[2][2]{};         // [B*36][64]
@@ -45,12 +45,12 @@ struct V2State {
   uint16_t* W2T[3][3]{};         // [net][plane] [64][512]
   uint16_t* W3T[3][3]{};         // [64][576]
   uint16_t* WfT[3][3]{};         // [512][1024]
-  uint16_t* K0T[3][3]{};         // [0] pi [64][KF], [1] values vf|q1|q2 [192][KF], [2] target vf [64][KF]
+  uint16_t* K0T[3][3]{};         // [0] pi [H][KF], [1] values vf|q1|q2 [3H][KF], [2] target vf [H][KF]
   uint16_t* W2n[2][2]{};         // natural [512][64] (dgrad B operand), nets pi / values, 2 planes
   uint16_t* W3n[2][2]{};         // [576][64]
   uint16_t* Wfn[2][2]{};         // [1024][512]
-  uint16_t* K0n[2][2]{};         // [0] pi [513 -> 576 rows][64], [1] values packed [576 rows][192]
-  float* z0v = nullptr;          // fc0 pre-activations of vf|q1|q2: [B][192]
+  uint16_t* K0n[2][2]{};         // [0] pi [513 -> 576 rows][H], [1] values packed [576 rows][3H]
+  float* z0v = nullptr;          // fc0 pre-activations of vf|q1|q2: [B][3H]
   void* plane_jobs = nullptr; int n_plane_jobs = 0, plane_ctas = 0;
   const int* plane_cta_job = nullptr;  // job index of every CTA of the planes launch
   int sm_reserve = 0;           // SMs left to a collective that runs concurrently with the persistent GEMM grids

@@ -399,31 +399,490 @@ __global__ void __launch_bounds__(WARPS * 32) act_kernel(TailArgs t, int n, int 
     }
   }
 }
+
+// ================================================================================================
+// Wide heads (H = 128, 192, 256): one fc1 is H*H*4 B (256 KB at H = 256), so the five of them no longer fit shared memory,
+// and a warp per sample re-reading them from L2 would move ~0.8 GB per step.  A CTA of H threads instead takes a group of
+// TW_G samples through the phases of tail4 together; every H x H mat-vec streams its fc1 through a double-buffered
+// shared-memory k-slice (TW_KS rows) that all samples of the group consume, thread c owning output column c for every
+// sample.  The per-sample vectors live in shared memory ([TW_G][H] each), the per-sample scalars are warp reductions.
+// fp32 FFMA throughout, the same formulas and summation order per sample as tail4.
+// ================================================================================================
+// Groups of 4 samples: at B = 256 that is 64 CTAs; groups of 8 (32 CTAs, half the L2 weight traffic) measured 30 % slower.
+constexpr int TW_G = 4, TW_KS = 32;
+enum { V_XPI = 0, V_XVF, V_XQ1, V_XQ2, V_XT, V_XU, V_YPI, V_YVF, V_YQ1, V_YQ2, V_YT, V_YU, V_N };
+// per-sample scalars, AMAX-wide blocks per action: mu (then pi), raw log_std, std, t = (u - mu) / (std + eps), the seeds of mu and
+// log_std, d(-Q1(s, pi))/d pi; then one slot each
+enum { SC_MU = 0, SC_LS = 8, SC_SD = 16, SC_TT = 24, SC_DMU = 32, SC_DLS = 40, SC_DPI = 48, SC_LOGP = 56, SC_ENT, SC_V, SC_VT, SC_Q1,
+       SC_Q2, SC_Q1P, SC_Q2P, SC_DVF, SC_DQ1, SC_DQ2, SC_N = 72 };
+
+template <int H>
+constexpr size_t tw_smem_floats() { return 2 * (size_t)TW_KS * (H + 1) + (size_t)V_N * TW_G * H + TW_G * SC_N + 32; }
+
+// acc[g] += sum_k x[g][k] * M[k][c] for c = threadIdx.x: M = W ([H][H] row-major fc1: forward, out[j] = sum_i a[i] W[i][j]) or,
+// TR, M = W^T (backward, out[i] = sum_j dz[j] W[i][j]).  W streams through wbuf in TW_KS-deep k-slices, double-buffered
+// through registers: slice s + 1 is loaded while slice s is consumed.  The caller orders x's stores before the call; the
+// call ends with a barrier, so wbuf is free again and x may be overwritten afterwards.
+template <int H, bool TR>
+__device__ __forceinline__ void tw_matvec(const float* __restrict__ W, const float* x, float (&acc)[TW_G], float* wbuf) {
+  constexpr int P = TR ? H + 1 : H;            // transposed slices: padded pitch, the scattered stores stay conflict-free
+  constexpr int NS = H / TW_KS, NV = TW_KS / 4;
+  const int c = threadIdx.x;
+  float4 st[NV];
+  auto load = [&](int s) {
+    const int k0 = s * TW_KS;
+#pragma unroll
+    for (int m = 0; m < NV; ++m) {
+      const int f = c + H * m;
+      if (TR) {
+        const int r = f / NV, q = f % NV;           // W[r][k0 + 4q .. + 3]
+        st[m] = __ldg(reinterpret_cast<const float4*>(W + (size_t)r * H + k0 + 4 * q));
+      } else {
+        const int kk = f / (H / 4), c4 = f % (H / 4);
+        st[m] = __ldg(reinterpret_cast<const float4*>(W + (size_t)(k0 + kk) * H + 4 * c4));
+      }
+    }
+  };
+  auto store = [&](float* buf) {
+#pragma unroll
+    for (int m = 0; m < NV; ++m) {
+      const int f = c + H * m;
+      if (TR) {
+        const int r = f / NV, q = f % NV;
+        buf[(4 * q) * P + r] = st[m].x; buf[(4 * q + 1) * P + r] = st[m].y;
+        buf[(4 * q + 2) * P + r] = st[m].z; buf[(4 * q + 3) * P + r] = st[m].w;
+      } else {
+        const int kk = f / (H / 4), c4 = f % (H / 4);
+        *reinterpret_cast<float4*>(buf + kk * P + 4 * c4) = st[m];
+      }
+    }
+  };
+  load(0);
+  store(wbuf);
+  __syncthreads();
+  for (int s = 0; s < NS; ++s) {
+    if (s + 1 < NS) load(s + 1);
+    const float* buf = wbuf + (s & 1) * TW_KS * (H + 1);
+    const int k0 = s * TW_KS;
+#pragma unroll 2
+    for (int kk = 0; kk < TW_KS; kk += 4) {
+      float4 xv[TW_G];
+#pragma unroll
+      for (int g = 0; g < TW_G; ++g) xv[g] = *reinterpret_cast<const float4*>(x + g * H + k0 + kk);
+      const float w0 = buf[kk * P + c], w1 = buf[(kk + 1) * P + c], w2 = buf[(kk + 2) * P + c], w3 = buf[(kk + 3) * P + c];
+#pragma unroll
+      for (int g = 0; g < TW_G; ++g) {
+        acc[g] = fmaf(xv[g].x, w0, acc[g]); acc[g] = fmaf(xv[g].y, w1, acc[g]);
+        acc[g] = fmaf(xv[g].z, w2, acc[g]); acc[g] = fmaf(xv[g].w, w3, acc[g]);
+      }
+    }
+    if (s + 1 < NS) store(wbuf + ((s + 1) & 1) * TW_KS * (H + 1));
+    __syncthreads();
+  }
+}
+
+// sc[g * SC_N + slot(n)] = sum_i x(g, n)[i] * k(n)[i * kld + koff] + bias(n) for the jobs n of every sample, one warp per (g, n)
+template <int H, class F>
+__device__ __forceinline__ void tw_dots(int njobs, F&& job) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int p = warp; p < TW_G * njobs; p += H / 32) {
+    const int g = p / njobs, n = p % njobs;
+    const float* x; const float* k; int kld; float* dst; float bias;
+    job(g, n, x, k, kld, dst, bias);
+    float s = 0.f;
+#pragma unroll
+    for (int i = lane; i < H; i += 32) s = fmaf(x[i], __ldg(k + (size_t)i * kld), s);
+    s = warp_sum(s);
+    if (lane == 0) *dst = s + bias;
+  }
+}
+
+__device__ __forceinline__ void st_planes1(uint16_t* hi, uint16_t* lo, size_t o, float v) {
+  const __nv_bfloat16 h = __float2bfloat16_rn(v);
+  hi[o] = __bfloat16_as_ushort(h);
+  lo[o] = __bfloat16_as_ushort(__float2bfloat16_rn(v - __bfloat162float(h)));
+}
+
+template <int H>
+__global__ void __launch_bounds__(H) tailw_kernel(TailArgs t) {
+  extern __shared__ __align__(16) float smem[];
+  float* wbuf = smem;
+  float* V = wbuf + 2 * TW_KS * (H + 1);
+  float* sc = V + V_N * TW_G * H;
+  float* red = sc + TW_G * SC_N;                  // [MET_COUNT + 1] loss / metric sums of the group
+  auto vec = [&](int v, int g) { return V + (v * TW_G + g) * H; };
+  const int c = threadIdx.x, A = t.A, b_base = blockIdx.x * TW_G;
+  pdl_trigger();
+  pdl_wait();
+  if (c <= MET_COUNT) red[c] = 0.f;
+  const float invB = 1.0f / (float)t.grad_scale_B;
+  const float log_alpha = t.log_alpha[0];
+  const float alpha = expf(log_alpha);
+  const float* K1[S_NW] = {t.pi.k1, t.vf.k1, t.q1.k1, t.q2.k1, t.vt.k1};
+  float acc[TW_G];
+
+  // ---- fc0 activations at the replay action (rows past the batch are zeros and contribute nothing)
+  {
+    const float b0p = t.pi.b0[c], b0v = t.vf.b0[c], b0q1 = t.q1.b0[c], b0q2 = t.q2.b0[c], b0t = t.vt.b0[c];
+    for (int g = 0; g < TW_G; ++g) {
+      const int b = b_base + g;
+      const bool ok = b < t.B;
+      const size_t ov = (size_t)b * t.z0v_ld + c;
+      const float a0p = ok ? fmaxf(t.z0_pi[(size_t)b * H + c] + b0p, 0.f) : 0.f;
+      const float a0v = ok ? fmaxf(t.z0_vf[ov] + b0v, 0.f) : 0.f;
+      const float a0q1 = ok ? fmaxf(t.z0_q1[ov] + b0q1, 0.f) : 0.f;
+      const float a0q2 = ok ? fmaxf(t.z0_q2[ov] + b0q2, 0.f) : 0.f;
+      vec(V_XPI, g)[c] = a0p; vec(V_XVF, g)[c] = a0v; vec(V_XQ1, g)[c] = a0q1; vec(V_XQ2, g)[c] = a0q2;
+      vec(V_XT, g)[c] = ok ? fmaxf(t.z0_vt[(size_t)b * H + c] + b0t, 0.f) : 0.f;
+      if (ok) {
+        const size_t o = (size_t)b * H + c;
+        t.a0_pi[o] = a0p; t.a0_vf[o] = a0v; t.a0_q1[o] = a0q1; t.a0_q2[o] = a0q2;
+      }
+    }
+  }
+  __syncthreads();
+  // ---- fc1 forward of the five heads
+  {
+    const int xin[S_NW] = {V_XPI, V_XVF, V_XQ1, V_XQ2, V_XT}, yout[S_NW] = {V_YPI, V_YVF, V_YQ1, V_YQ2, V_YT};
+    const float* b1s[S_NW] = {t.pi.b1, t.vf.b1, t.q1.b1, t.q2.b1, t.vt.b1};
+    for (int w = 0; w < S_NW; ++w) {
+      const float bias = b1s[w][c];
+#pragma unroll
+      for (int g = 0; g < TW_G; ++g) acc[g] = bias;
+      tw_matvec<H, false>(K1[w], vec(xin[w], 0), acc, wbuf);
+#pragma unroll
+      for (int g = 0; g < TW_G; ++g) vec(yout[w], g)[c] = fmaxf(acc[g], 0.f);
+    }
+  }
+  __syncthreads();
+  // ---- output layers: mu, log_std (raw), v, v_targ, q1, q2
+  tw_dots<H>(2 * A + 4, [&](int g, int n, const float*& x, const float*& k, int& kld, float*& dst, float& bias) {
+    if (n < 2 * A) {
+      const int a = n % A;
+      const bool mu = n < A;
+      x = vec(V_YPI, g); k = (mu ? t.pi.ko : t.ksig) + a; kld = A;
+      dst = sc + g * SC_N + (mu ? SC_MU : SC_LS) + a; bias = (mu ? t.pi.bo : t.bsig)[a];
+      return;
+    }
+    const int m = n - 2 * A;                   // 0 vf, 1 target vf, 2 qf1, 3 qf2
+    const HeadW* hw = m == 0 ? &t.vf : m == 1 ? &t.vt : m == 2 ? &t.q1 : &t.q2;
+    x = vec(m == 0 ? V_YVF : m == 1 ? V_YT : m == 2 ? V_YQ1 : V_YQ2, g); k = hw->ko; kld = 1;
+    dst = sc + g * SC_N + SC_V + m; bias = hw->bo[0];
+  });
+  __syncthreads();
+  // ---- actor outputs (one thread per sample)
+  if (c < TW_G) {
+    const int b = b_base + c;
+    float* s = sc + c * SC_N;
+    float logp = 0.f, ent = 0.f;
+    for (int a = 0; a < A; ++a) {
+      const float e = b < t.B ? t.eps[b * A + a] : 0.f;
+      const float mu = s[SC_MU + a];
+      const float ls = fminf(fmaxf(s[SC_LS + a], LS_MIN), LS_MAX);
+      const float sd = expf(ls);
+      const float u = mu + e * sd;
+      const float tt = (u - mu) / (sd + EPSF);
+      const float pi = tanhf(u);
+      logp += -0.5f * (tt * tt + 2.f * ls + 1.8378770664093453f) - logf(1.f - pi * pi + EPSF);
+      ent += ls + 1.4189385332046727f;
+      s[SC_SD + a] = sd; s[SC_TT + a] = tt; s[SC_MU + a] = pi;      // mu is not needed past here: its slot holds pi
+      if (t.pi_out && b < t.B) t.pi_out[b * A + a] = pi;
+    }
+    s[SC_LOGP] = logp; s[SC_ENT] = ent;
+  }
+  __syncthreads();
+  // ---- qf1, qf2 at pi: z0(pi) = z0(a) + (pi - a) K0[action rows]
+  {
+    const float b0q1 = t.q1.b0[c], b0q2 = t.q2.b0[c];
+    for (int g = 0; g < TW_G; ++g) {
+      const int b = b_base + g;
+      float x1 = 0.f, x2 = 0.f;
+      if (b < t.B) {
+        const size_t ov = (size_t)b * t.z0v_ld + c;
+        float z1 = t.z0_q1[ov], z2 = t.z0_q2[ov];
+        for (int a = 0; a < A; ++a) {
+          const float dlt = sc[g * SC_N + SC_MU + a] - t.act[(size_t)b * t.act_stride + a];
+          const size_t ro = (size_t)(t.feat_dim + a) * H + c;
+          z1 = fmaf(dlt, t.q1.k0[ro], z1); z2 = fmaf(dlt, t.q2.k0[ro], z2);
+        }
+        x1 = fmaxf(z1 + b0q1, 0.f); x2 = fmaxf(z2 + b0q2, 0.f);
+      }
+      vec(V_XT, g)[c] = x1; vec(V_XU, g)[c] = x2;
+    }
+  }
+  __syncthreads();
+  {
+    const float bq1 = t.q1.b1[c], bq2 = t.q2.b1[c];
+#pragma unroll
+    for (int g = 0; g < TW_G; ++g) acc[g] = bq1;
+    tw_matvec<H, false>(t.q1.k1, vec(V_XT, 0), acc, wbuf);
+#pragma unroll
+    for (int g = 0; g < TW_G; ++g) vec(V_YT, g)[c] = fmaxf(acc[g], 0.f);      // (target vf activations are dead)
+#pragma unroll
+    for (int g = 0; g < TW_G; ++g) acc[g] = bq2;
+    tw_matvec<H, false>(t.q2.k1, vec(V_XU, 0), acc, wbuf);
+#pragma unroll
+    for (int g = 0; g < TW_G; ++g) vec(V_YU, g)[c] = fmaxf(acc[g], 0.f);
+  }
+  __syncthreads();
+  tw_dots<H>(2, [&](int g, int n, const float*& x, const float*& k, int& kld, float*& dst, float& bias) {
+    const HeadW* hw = n == 0 ? &t.q1 : &t.q2;
+    x = vec(n == 0 ? V_YT : V_YU, g); k = hw->ko; kld = 1; dst = sc + g * SC_N + SC_Q1P + n; bias = hw->bo[0];
+  });
+  __syncthreads();
+  // ---- losses, metrics and the value / Q backward seeds (one thread per sample)
+  if (c < TW_G) {
+    const int b = b_base + c;
+    float* s = sc + c * SC_N;
+    float dvf = 0.f, dq1 = 0.f, dq2 = 0.f;
+    if (b < t.B) {
+      const float logp = s[SC_LOGP], q1p = s[SC_Q1P], q2p = s[SC_Q2P], v = s[SC_V], v_targ = s[SC_VT];
+      atomicAdd(&red[MET_POLICY_LOSS], (alpha * logp - q1p) * invB);
+      atomicAdd(&red[MET_ENT_COEF_LOSS], -log_alpha * (logp + t.target_entropy) * invB);
+      atomicAdd(&red[MET_ENTROPY], s[SC_ENT] * invB);
+      atomicAdd(&red[MET_MEAN_LOGP], logp * invB);
+      atomicAdd(&red[MET_COUNT], -(logp + t.target_entropy) * invB);
+      const float v_backup = fminf(q1p, q2p) - alpha * logp;
+      const float ev = v - v_backup;
+      atomicAdd(&red[MET_VALUE_LOSS], 0.5f * ev * ev * invB);
+      atomicAdd(&red[MET_MEAN_V], v * invB);
+      dvf = ev * invB;
+      const float q_backup = t.rew[b] + (1.f - t.done[b]) * t.gamma * v_targ;
+      const float e1 = s[SC_Q1] - q_backup, e2 = s[SC_Q2] - q_backup;
+      atomicAdd(&red[MET_QF1_LOSS], 0.5f * e1 * e1 * invB);
+      atomicAdd(&red[MET_QF2_LOSS], 0.5f * e2 * e2 * invB);
+      atomicAdd(&red[MET_MEAN_Q1], s[SC_Q1] * invB);
+      atomicAdd(&red[MET_MEAN_Q2], s[SC_Q2] * invB);
+      dq1 = e1 * invB; dq2 = e2 * invB;
+      if (t.per_sample) {
+        const int B = t.B;
+        t.per_sample[b] = s[SC_Q1]; t.per_sample[B + b] = s[SC_Q2]; t.per_sample[2 * B + b] = v; t.per_sample[3 * B + b] = logp;
+        t.per_sample[4 * B + b] = v_targ; t.per_sample[5 * B + b] = q1p; t.per_sample[6 * B + b] = q2p;
+      }
+    }
+    s[SC_DVF] = dvf; s[SC_DQ1] = dq1; s[SC_DQ2] = dq2;
+  }
+  // d(-Q1(s, pi))/d a1 at pi -> V_YU (the qf2-at-pi activations are dead)
+  {
+    const float k = t.q1.ko[c];
+    for (int g = 0; g < TW_G; ++g)
+      vec(V_YU, g)[c] = (b_base + g < t.B && vec(V_YT, g)[c] > 0.f) ? -invB * k : 0.f;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int g = 0; g < TW_G; ++g) acc[g] = 0.f;
+  tw_matvec<H, true>(t.q1.k1, vec(V_YU, 0), acc, wbuf);
+#pragma unroll
+  for (int g = 0; g < TW_G; ++g) vec(V_XU, g)[c] = vec(V_XT, g)[c] > 0.f ? acc[g] : 0.f;      // dz0 of qf1 at pi
+  __syncthreads();
+  // dpi = dz0(pi) . K0[action rows]^T
+  tw_dots<H>(A, [&](int g, int n, const float*& x, const float*& k, int& kld, float*& dst, float& bias) {
+    x = vec(V_XU, g); k = t.q1.k0 + (size_t)(t.feat_dim + n) * H; kld = 1; dst = sc + g * SC_N + SC_DPI + n; bias = 0.f;
+  });
+  __syncthreads();
+  // ---- actor backward seeds (one thread per sample)
+  if (c < TW_G) {
+    const int b = b_base + c;
+    float* s = sc + c * SC_N;
+    for (int a = 0; a < A; ++a) {
+      float dmu = 0.f, dls = 0.f;
+      if (b < t.B) {
+        const float e = t.eps[b * A + a], pi = s[SC_MU + a], sd = s[SC_SD + a], tt = s[SC_TT + a], ls_raw = s[SC_LS + a];
+        const float one_m = 1.f - pi * pi;
+        const float du = (alpha * invB) * 2.f * pi * one_m / (one_m + EPSF) + s[SC_DPI + a] * one_m;
+        dmu = du;
+        const float spe = sd + EPSF;
+        const float d = du * e * sd + (alpha * invB) * (-tt * e * sd * EPSF / (spe * spe) - 1.f);
+        dls = (ls_raw >= LS_MIN && ls_raw <= LS_MAX) ? d : 0.f;
+      }
+      s[SC_DMU + a] = dmu; s[SC_DLS + a] = dls;
+    }
+  }
+  __syncthreads();
+  // ---- fc1 pre-activation gradients (column c of every sample) and the output-layer gradients of the group
+  float gk_mu[AMAX], gk_sig[AMAX];
+  float gko_vf = 0.f, gko_q1 = 0.f, gko_q2 = 0.f;
+  {
+    float kmu[AMAX], ksg[AMAX];
+#pragma unroll
+    for (int a = 0; a < AMAX; ++a) {
+      kmu[a] = a < A ? t.pi.ko[c * A + a] : 0.f; ksg[a] = a < A ? t.ksig[c * A + a] : 0.f;
+      gk_mu[a] = 0.f; gk_sig[a] = 0.f;
+    }
+    const float kvf = t.vf.ko[c], kq1 = t.q1.ko[c], kq2 = t.q2.ko[c];
+    for (int g = 0; g < TW_G; ++g) {
+      const int b = b_base + g;
+      const float* s = sc + g * SC_N;
+      const float gv = vec(V_YPI, g)[c];
+      float dg = 0.f;
+#pragma unroll
+      for (int a = 0; a < AMAX; ++a) {
+        if (a < A) {
+          const float dmu = s[SC_DMU + a], dls = s[SC_DLS + a];
+          gk_mu[a] = fmaf(gv, dmu, gk_mu[a]); gk_sig[a] = fmaf(gv, dls, gk_sig[a]);
+          dg += dmu * kmu[a] + dls * ksg[a];
+        }
+      }
+      const float dz_pi = gv > 0.f ? dg : 0.f;
+      float* yvf = vec(V_YVF, g); float* yq1 = vec(V_YQ1, g); float* yq2 = vec(V_YQ2, g);
+      const float a1v = yvf[c], a1q1 = yq1[c], a1q2 = yq2[c];
+      const float dvf = s[SC_DVF], dq1 = s[SC_DQ1], dq2 = s[SC_DQ2];
+      gko_vf = fmaf(a1v, dvf, gko_vf); gko_q1 = fmaf(a1q1, dq1, gko_q1); gko_q2 = fmaf(a1q2, dq2, gko_q2);
+      const float dz_vf = a1v > 0.f ? dvf * kvf : 0.f, dz_q1 = a1q1 > 0.f ? dq1 * kq1 : 0.f, dz_q2 = a1q2 > 0.f ? dq2 * kq2 : 0.f;
+      vec(V_YT, g)[c] = dz_pi; yvf[c] = dz_vf; yq1[c] = dz_q1; yq2[c] = dz_q2;      // in place: column c is this thread's own
+      if (b < t.B) {
+        const size_t o = (size_t)b * H + c;
+        t.dz1_pi[o] = dz_pi; t.dz1_vf[o] = dz_vf; t.dz1_q1[o] = dz_q1; t.dz1_q2[o] = dz_q2;
+      }
+    }
+  }
+  __syncthreads();
+  // ---- fc1^T backward of pi, vf, qf1, qf2 -> dz0 (fp32 and, for engine v2, BF16 hi / lo planes)
+  {
+    const int yin[4] = {V_YT, V_YVF, V_YQ1, V_YQ2}, xin[4] = {V_XPI, V_XVF, V_XQ1, V_XQ2};
+    const float* W[4] = {t.pi.k1, t.vf.k1, t.q1.k1, t.q2.k1};
+    for (int w = 0; w < 4; ++w) {
+#pragma unroll
+      for (int g = 0; g < TW_G; ++g) acc[g] = 0.f;
+      tw_matvec<H, true>(W[w], vec(yin[w], 0), acc, wbuf);
+      for (int g = 0; g < TW_G; ++g) {
+        const int b = b_base + g;
+        if (b >= t.B) break;
+        const float dz0 = vec(xin[w], g)[c] > 0.f ? acc[g] : 0.f;
+        if (w == 0) {
+          const size_t o = (size_t)b * H + c;
+          t.dz0_pi[o] = dz0;
+          if (t.dz0_pi_p[0]) st_planes1(t.dz0_pi_p[0], t.dz0_pi_p[1], o, dz0);
+        } else {
+          const size_t o = (size_t)b * 3 * H + (w - 1) * H + c;
+          t.dz0_v3[o] = dz0;
+          if (t.dz0_v3_p[0]) st_planes1(t.dz0_v3_p[0], t.dz0_v3_p[1], o, dz0);
+        }
+      }
+    }
+  }
+  // ---- the group's gradient contributions (tw_matvec ended with a barrier: red is complete)
+#pragma unroll
+  for (int a = 0; a < AMAX; ++a)
+    if (a < A) { atomicAdd(t.g_pi.ko + c * A + a, gk_mu[a]); atomicAdd(t.g_ksig + c * A + a, gk_sig[a]); }
+  atomicAdd(t.g_vf.ko + c, gko_vf); atomicAdd(t.g_q1.ko + c, gko_q1); atomicAdd(t.g_q2.ko + c, gko_q2);
+  if (c < A) {
+    float sm = 0.f, ss = 0.f;
+    for (int g = 0; g < TW_G; ++g) { sm += sc[g * SC_N + SC_DMU + c]; ss += sc[g * SC_N + SC_DLS + c]; }
+    atomicAdd(t.g_pi.bo + c, sm); atomicAdd(t.g_bsig + c, ss);
+  }
+  if (c == 0) {
+    float sv = 0.f, s1 = 0.f, s2 = 0.f;
+    for (int g = 0; g < TW_G; ++g) { sv += sc[g * SC_N + SC_DVF]; s1 += sc[g * SC_N + SC_DQ1]; s2 += sc[g * SC_N + SC_DQ2]; }
+    atomicAdd(t.g_vf.bo, sv); atomicAdd(t.g_q1.bo, s1); atomicAdd(t.g_q2.bo, s2);
+    atomicAdd(t.g_log_alpha, red[MET_COUNT]);
+  }
+  if (c < MET_GN_PI) atomicAdd(t.metrics + c, red[c]);
+}
+
+// policy inference at H >= 128: tanh(mu) or tanh(mu + eps * std) for TW_G rows per CTA, fc1 streamed as in tailw_kernel
+template <int H>
+__global__ void __launch_bounds__(H) actw_kernel(TailArgs t, int n, int deterministic, float* act_out) {
+  extern __shared__ __align__(16) float smem[];
+  float* wbuf = smem;
+  float* X = wbuf + 2 * TW_KS * (H + 1);
+  float* Y = X + TW_G * H;
+  float* sc = Y + TW_G * H;                       // [TW_G][2 * AMAX]: mu, log_std
+  const int c = threadIdx.x, A = t.A, b_base = blockIdx.x * TW_G;
+  const float b0 = t.pi.b0[c];
+  for (int g = 0; g < TW_G; ++g) {
+    const int b = b_base + g;
+    X[g * H + c] = b < n ? fmaxf(t.z0_pi[(size_t)b * H + c] + b0, 0.f) : 0.f;
+  }
+  __syncthreads();
+  float acc[TW_G];
+  const float b1 = t.pi.b1[c];
+#pragma unroll
+  for (int g = 0; g < TW_G; ++g) acc[g] = b1;
+  tw_matvec<H, false>(t.pi.k1, X, acc, wbuf);
+#pragma unroll
+  for (int g = 0; g < TW_G; ++g) Y[g * H + c] = fmaxf(acc[g], 0.f);
+  __syncthreads();
+  tw_dots<H>(2 * A, [&](int g, int m, const float*& x, const float*& k, int& kld, float*& dst, float& bias) {
+    const int a = m % A;
+    const bool mu = m < A;
+    x = Y + g * H; k = (mu ? t.pi.ko : t.ksig) + a; kld = A; dst = sc + g * 2 * AMAX + (mu ? 0 : AMAX) + a; bias = (mu ? t.pi.bo : t.bsig)[a];
+  });
+  __syncthreads();
+  if (c < TW_G * A) {
+    const int g = c / A, a = c % A, b = b_base + g;
+    if (b < n) {
+      float u = sc[g * 2 * AMAX + a];
+      if (!deterministic) u += t.eps[b * A + a] * expf(fminf(fmaxf(sc[g * 2 * AMAX + AMAX + a], LS_MIN), LS_MAX));
+      act_out[b * A + a] = tanhf(u);
+    }
+  }
+}
+
+template <int H>
+size_t tailw_smem() { return sizeof(float) * tw_smem_floats<H>(); }
+template <int H>
+size_t actw_smem() { return sizeof(float) * (2 * (size_t)TW_KS * (H + 1) + 2 * TW_G * H + TW_G * 2 * AMAX); }
+
+// The opt-in to more than 48 KB of dynamic shared memory is a property of the kernel on ONE device: it is set the first time a
+// kernel is launched on each device (done: one bit per device ordinal) and its failure is returned.
+template <class K>
+cudaError_t smem_optin(K* fn, size_t bytes, unsigned long long& done) {
+  int dev = 0;
+  if (cudaError_t e = cudaGetDevice(&dev)) return e;
+  const unsigned long long bit = dev < 64 ? 1ull << dev : 0ull;
+  if (done & bit) return cudaSuccess;
+  if (cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes)) return e;
+  done |= bit;
+  return cudaSuccess;
+}
+
+template <int H>
+cudaError_t tailw_launch(const TailArgs& a, cudaStream_t s) {
+  static unsigned long long done = 0;
+  if (cudaError_t e = smem_optin(tailw_kernel<H>, tailw_smem<H>(), done)) return e;
+  return launch_pdl(tailw_kernel<H>, dim3((a.B + TW_G - 1) / TW_G), dim3(H), tailw_smem<H>(), s, pdl_enabled(), a);
+}
+template <int H>
+cudaError_t actw_launch(const TailArgs& t, int n, int deterministic, float* act_out, cudaStream_t s) {
+  static unsigned long long done = 0;
+  if (cudaError_t e = smem_optin(actw_kernel<H>, actw_smem<H>(), done)) return e;
+  actw_kernel<H><<<(n + TW_G - 1) / TW_G, H, actw_smem<H>(), s>>>(t, n, deterministic, act_out);
+  return cudaPeekAtLastError();
+}
+
 }  // namespace
 
-void act_launch(const TailArgs& t, int n, int deterministic, float* act_out, cudaStream_t s) {
-  if (n <= 0) return;
+cudaError_t act_launch(const TailArgs& t, int n, int deterministic, float* act_out, cudaStream_t s) {
+  if (n <= 0) return cudaSuccess;
+  switch (t.H) {
+    case 128: return actw_launch<128>(t, n, deterministic, act_out, s);
+    case 192: return actw_launch<192>(t, n, deterministic, act_out, s);
+    case 256: return actw_launch<256>(t, n, deterministic, act_out, s);
+  }
   act_kernel<<<(n + WARPS - 1) / WARPS, WARPS * 32, 0, s>>>(t, n, deterministic, act_out);
+  return cudaPeekAtLastError();
 }
 
 namespace {
-// grid (10, 4 heads, HW_KSPLIT batch slices), 256 threads: x = 0..8 -> rows [64x, 64x + 64) of the fc0 kernel gradient
-// X0^T . dz0 (x = 0 also the fc0 bias gradient: column sums of dz0), x = 9 -> the fc1 kernel gradient a0^T . dz1 and the fc1 bias.  Every CTA
+// grid (9 + H/64, 4 heads, HW_KSPLIT batch slices x H/64 column blocks), 256 threads: x = 0..8 -> rows [64x, 64x + 64) of the
+// fc0 kernel gradient X0^T . dz0 (x = 0 also the fc0 bias gradient: column sums of dz0), x = 9.. -> row block x - 9 of the fc1
+// kernel gradient a0^T . dz1 (x = 9 also the fc1 bias); every CTA covers 64 output columns.  Every CTA
 // reduces its batch slice in chunks of 32 samples through shared memory (4 x 4 outputs per thread) and accumulates into the
 // zeroed gradient arena with red.add.
 constexpr int HW_KSPLIT = 4;
 __global__ void __launch_bounds__(256) heads_wgrad_kernel(const HeadsWgradArgs a) {
   __shared__ __align__(16) float As[32][64], Bs[32][64];
-  const int q = blockIdx.y, rb = blockIdx.x, tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const bool fc1 = rb == 9;
-  const int M = fc1 ? 64 : a.M0[q], row0 = fc1 ? 0 : rb * 64;
+  const int q = blockIdx.y, rb = blockIdx.x, tid = threadIdx.x, tx = tid & 15, ty = tid >> 4, H = a.H;
+  const bool fc1 = rb >= 9, sums = rb == 0 || rb == 9;
+  const int M = fc1 ? H : a.M0[q], row0 = (fc1 ? rb - 9 : rb) * 64, n0 = (blockIdx.z / HW_KSPLIT) * 64;
   if (row0 >= M) return;
   const float* __restrict__ X = fc1 ? a.a0[q] : a.X0[q];
-  const float* __restrict__ D = fc1 ? a.dz1[q] : a.dz0[q];
-  const int xld = fc1 ? 64 : a.x0_ld, dld = fc1 ? 64 : a.dz0_ld[q];
-  const int per = (a.B + HW_KSPLIT - 1) / HW_KSPLIT, b0 = blockIdx.z * per, b1 = min(a.B, b0 + per);
+  const float* __restrict__ D = (fc1 ? a.dz1[q] : a.dz0[q]) + n0;
+  const int xld = fc1 ? H : a.x0_ld, dld = fc1 ? H : a.dz0_ld[q];
+  const int per = (a.B + HW_KSPLIT - 1) / HW_KSPLIT, b0 = (blockIdx.z % HW_KSPLIT) * per, b1 = min(a.B, b0 + per);
   float acc[4][4] = {};
-  float cs = 0.f;                         // bias sum: column tid of this CTA's gradient tile (x == 0: fc0 bias from dz0, x == 9: fc1 bias from dz1)
+  float cs = 0.f;                         // bias sum: column n0 + tid (x == 0: fc0 bias from dz0, x == 9: fc1 bias from dz1)
   for (int bb = b0; bb < b1; bb += 32) {
     for (int i = tid; i < 32 * 64; i += 256) {
       const int k = i >> 6, c = i & 63, b = bb + k;
@@ -442,26 +901,28 @@ __global__ void __launch_bounds__(256) heads_wgrad_kernel(const HeadsWgradArgs a
 #pragma unroll
         for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(ar[i], br[j], acc[i][j]);
     }
-    if ((fc1 || rb == 0) && tid < 64) {
+    if (sums && tid < 64) {
 #pragma unroll 8
       for (int k = 0; k < 32; ++k) cs += Bs[k][tid];
     }
     __syncthreads();
   }
-  float* __restrict__ G = fc1 ? a.g_k1[q] : a.g_k0[q];
+  float* __restrict__ G = (fc1 ? a.g_k1[q] : a.g_k0[q]) + n0;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int r = row0 + 4 * ty + i;
     if (r < M)
-      asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(G + (size_t)r * 64 + 4 * tx), "f"(acc[i][0]), "f"(acc[i][1]), "f"(acc[i][2]),
+      asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(G + (size_t)r * H + 4 * tx), "f"(acc[i][0]), "f"(acc[i][1]), "f"(acc[i][2]),
                    "f"(acc[i][3])
                    : "memory");
   }
-  if ((fc1 || rb == 0) && tid < 64) atomicAdd((fc1 ? a.g_b1[q] : a.g_b0[q]) + tid, cs);
+  if (sums && tid < 64) atomicAdd((fc1 ? a.g_b1[q] : a.g_b0[q]) + n0 + tid, cs);
 }
 }  // namespace
 
-void heads_wgrad_launch(const HeadsWgradArgs& a, cudaStream_t s) { heads_wgrad_kernel<<<dim3(10, 4, HW_KSPLIT), 256, 0, s>>>(a); }
+void heads_wgrad_launch(const HeadsWgradArgs& a, cudaStream_t s) {
+  heads_wgrad_kernel<<<dim3(9 + a.H / 64, 4, HW_KSPLIT * (a.H / 64)), 256, 0, s>>>(a);
+}
 
 static size_t tail_smem(int A) {
   return sizeof(float) * (S_NW * H * LD + 2 * H * A + 2 * A + 3 * (H + 1) + MET_COUNT + 1 + 8 +
@@ -469,15 +930,16 @@ static size_t tail_smem(int A) {
                           /* tail4 scratch */ 64);
 }
 
-void tail_launch(const TailArgs& a, cudaStream_t s) {
-  static bool attr_set = false;
-  const size_t smem = tail_smem(a.A);
-  if (!attr_set) {
-    cudaFuncSetAttribute(tail4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tail_smem(AMAX));
-    attr_set = true;
+cudaError_t tail_launch(const TailArgs& a, cudaStream_t s) {
+  switch (a.H) {
+    case 128: return tailw_launch<128>(a, s);
+    case 192: return tailw_launch<192>(a, s);
+    case 256: return tailw_launch<256>(a, s);
   }
+  static unsigned long long done = 0;
+  if (cudaError_t e = smem_optin(tail4_kernel, tail_smem(AMAX), done)) return e;
   const int grid = (a.B + 1) / 2;             // four warps per sample, two samples per CTA
-  launch_pdl(tail4_kernel, dim3(grid), dim3(WARPS * 32), smem, s, pdl_enabled(), a);
+  return launch_pdl(tail4_kernel, dim3(grid), dim3(WARPS * 32), tail_smem(a.A), s, pdl_enabled(), a);
 }
 
 }  // namespace b2g

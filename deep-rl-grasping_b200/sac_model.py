@@ -32,6 +32,15 @@ class MlpPolicy:
 
 
 _PRECISIONS = {"fp32": _lib.B2G_PREC_FP32_SIMT, "bf16x3": _lib.B2G_PREC_BF16X3, "bf16": _lib.B2G_PREC_BF16}
+HEAD_WIDTHS = (64, 128, 192, 256)      # SAC.layers [H, H] the device learner builds (b2g_sac_cfg.hidden)
+
+
+def head_width(layers) -> int:
+    """policy_kwargs['layers'] -> the head width H; anything but two equal widths from HEAD_WIDTHS raises."""
+    layers = [int(x) for x in layers]
+    if len(layers) != 2 or layers[0] != layers[1] or layers[0] not in HEAD_WIDTHS:
+        raise NotImplementedError(f"SAC.layers must be [H, H] with H in {list(HEAD_WIDTHS)} (got {layers})")
+    return layers[0]
 
 
 def _constfn(v):
@@ -67,9 +76,7 @@ class SAC:
             raise NotImplementedError(policy.unsupported)
         self.policy = policy
         self.policy_kwargs = dict(policy_kwargs or {})
-        layers = list(self.policy_kwargs.get("layers", [64, 64]))
-        if layers != [64, 64]:
-            raise NotImplementedError("SAC.layers must be [64, 64] (config/gripper_grasp.yaml:81)")
+        self.hidden = head_width(self.policy_kwargs.get("layers", [64, 64]))
         if self.policy_kwargs.get("layer_norm", False):
             raise NotImplementedError("layer_norm=True is not used by the reference (sb_helper.py:95)")
         self.gamma, self.tau = float(gamma), float(tau)
@@ -120,7 +127,7 @@ class SAC:
                                       "(simplified + depth branch, sb_helper.py:93-95), which is not built; pass "
                                       "cnn_extractor=create_augmented_nature_cnn(1) as sb_helper.py:88-91 does")
         tgt = -float(n_act) if self.target_entropy == "auto" else float(self.target_entropy)
-        self.learner = Learner(obs_shape, n_act=n_act, hidden=64, batch_size=self.batch_size, buffer_size=self.buffer_size,
+        self.learner = Learner(obs_shape, n_act=n_act, hidden=self.hidden, batch_size=self.batch_size, buffer_size=self.buffer_size,
                                gamma=self.gamma, tau=self.tau, target_entropy=tgt, seed=int(self.seed or 0),
                                precision=_PRECISIONS[self.precision], **self._dev)
         self._init_parameters()
@@ -325,8 +332,13 @@ class SAC:
         # a second model just to call get_parameters), so it gets a small ring unless the caller asks for one explicitly.
         kw["buffer_size"] = min(int(kw.get("buffer_size", 1000)), 1000)
         kw.update(kwargs)
+        # the head widths are the zip's own: the actor's fc0 / fc1 kernels give [H1, H2], and SAC's constructor refuses any
+        # layers the learner cannot build (unequal widths included) with the message that names the supported ones
+        layers = [int(params["model/pi/fc0/kernel"].shape[1]), int(params["model/pi/fc1/kernel"].shape[1])]
+        if "model/pi/fc2/kernel" in params:
+            layers.append(int(params["model/pi/fc2/kernel"].shape[1]))
         model = cls(policy=data.get("policy", "CnnPolicy"), env=None, _init_setup_model=False,
-                    policy_kwargs={"layers": [64, 64]}, **kw)
+                    policy_kwargs={"layers": layers}, **kw)
         model._layout_from_zip = True
         model.env = env_like if env is not None else None
         model.n_envs = env_like.num_envs

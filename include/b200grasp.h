@@ -47,7 +47,7 @@ typedef struct b2g_sac_cfg {
                                   (custom_obs_policy.py:28-32).  obs_h == 0 selects the MLP policy */
   int32_t obs_dim;             /* MLP policy: flat observation size (101 for the encoder config)   */
   int32_t n_act;               /* 5 (actuator.py:72-73); <= 8                                      */
-  int32_t hidden;              /* SAC.layers = [hidden, hidden] (config/gripper_grasp.yaml:81); 64 */
+  int32_t hidden;              /* SAC.layers = [hidden, hidden]: 64 (config/gripper_grasp.yaml:81), 128, 192 or 256; else B2G_EINVAL */
   int32_t batch;               /* per-rank minibatch size                                          */
   int64_t buffer_capacity;     /* replay slots on this rank (config/gripper_grasp.yaml:82)         */
   float gamma, tau, target_entropy;
