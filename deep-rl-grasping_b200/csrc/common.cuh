@@ -221,6 +221,7 @@ struct PrepArgs {          // 1-CTA kernel at the head of every step
   float* metrics;          // zeroed
   int* indices; float* eps;// generated when gen != 0
   int B, A; const long long* replay_size;   // nullptr -> counters[5]
+  long long ring_cap;      // > 0: slots are (counters[6] + u) % ring_cap (replay that lost transitions early starts mid-ring)
   unsigned long long seed; int gen; int apply;
   int defer_bump;          // 1: the rng step counter [4] is advanced by the optimiser kernel at the end of the step
   int skip_indices;        // 1: the gather kernel draws the replay slots itself (same Philox stream)
@@ -234,8 +235,51 @@ void prep_launch(const PrepArgs& a, cudaStream_t s);
 // [0,0] of the last plane | 3 zero pads
 void compact_rows(const float* src_full, float* dst, long long first_row, long long wrap, int n, int HW, int Cfull, cudaStream_t s);
 
+// How a replay frame stores one compact row of Ec floats: npx image elements [HW][Ci] (NHWC), then a tail of Ec - npx floats
+// (CNN: the actuator value and 3 pads; MLP: npx = 0 and the tail is the whole observation).  Image channel c lives in the
+// pixel's uint8 block when ch[c] >= 0 (byte ch[c] of [HW][n8] at offset 0) and in its fp32 block otherwise (float -1 - ch[c] of
+// [HW][n32] at byte f32_off).  n8 == 0 is the plain fp32 compact row (ch unused).
+struct FrameFmt {
+  int n8, n32;
+  int f32_off, tail;         // byte offsets of the fp32 image block and of the tail
+  signed char ch[8];
+};
+#ifdef __CUDACC__
+// element e of the compact row stored in frame f (decoded values are exactly the values the caller passed)
+__device__ __forceinline__ float frame_elem(const unsigned char* __restrict__ f, const FrameFmt& m, int npx, int Ci, int e) {
+  if (e >= npx) return reinterpret_cast<const float*>(f + m.tail)[e - npx];
+  if (m.n8 == 0) return reinterpret_cast<const float*>(f)[e];
+  const int pix = e / Ci, k = m.ch[e - pix * Ci];
+  return k >= 0 ? (float)f[pix * m.n8 + k] : reinterpret_cast<const float*>(f + m.f32_off)[pix * m.n32 - 1 - k];
+}
+// image elements [e, e + 4) (e % 4 == 0): one 128-bit load for fp32 frames
+__device__ __forceinline__ float4 frame_load4(const unsigned char* __restrict__ f, const FrameFmt& m, int npx, int Ci, int e) {
+  if (m.n8 == 0) return *reinterpret_cast<const float4*>(f + 4 * (size_t)e);
+  return make_float4(frame_elem(f, m, npx, Ci, e), frame_elem(f, m, npx, Ci, e + 1), frame_elem(f, m, npx, Ci, e + 2),
+                     frame_elem(f, m, npx, Ci, e + 3));
+}
+#endif
+
+// Replay frame pool writes (replay.cu).  frame_check: flags[i] bit 0 = compact row c_obs[i] equals frame prev[i] bit for bit
+// (prev[i] < 0: no candidate), bit 1 = a value of c_obs[i] or c_next[i] in a uint8 channel is not an integer in [0, 255].
+// frame_commit: c_obs[i] -> frame plan[i] when plan[m + i] != 0, c_next[i] -> frame plan[2m + i], and transition slot
+// (first + i) % cap records both frame indices.  plan == nullptr: row i takes the new frames fid0 + 2i, fid0 + 2i + 1
+// (mod fcap), which needs no upload when no frame is shared.
+struct FrameIo {
+  const float* c_obs; const float* c_next;   // compact rows [m][Ec]
+  unsigned char* frames; long long frame_bytes;
+  FrameFmt fmt; int npx, Ci, Ec;
+};
+void frame_check_launch(const FrameIo& io, const int* prev, int* flags, int m, cudaStream_t s);
+void frame_commit_launch(const FrameIo& io, const int* plan, long long fid0, long long fcap, int m, int* r_ofr, int* r_nfr,
+                         long long first, long long cap, cudaStream_t s);
+
 struct GatherArgs {
   const float* obs; const float* next_obs; const float* act; const float* rew; const float* done; // replay or staged batch
+  // replay frame pool: when obs_frame != nullptr, sample slot s reads frames obs_frame[s] / next_frame[s] instead of obs / next_obs
+  const unsigned char* frames; long long frame_bytes; const int* obs_frame; const int* next_frame;
+  FrameFmt fmt;              // layout of the rows read (frames, or the fp32 compact rows of obs / next_obs)
+  long long ring_cap;        // in-kernel slot draw: slot = (rng_counters[6] + u) % ring_cap, u uniform in [0, size)
   const int* indices;        // [B] slot per sample (nullptr: identity)
   const double* mean; const double* var; // [row elems]; var[] holds 1/sqrt(var+eps)
   const double* normc;       // device: {1/sqrt(ret_var+eps), clip_obs, clip_rew, norm_obs, norm_rew}
@@ -246,7 +290,7 @@ struct GatherArgs {
   float* F_pi; float* F_v; float* F_t; int FS; int feat_col; // feature rows: direct feature -> col feat_col; MLP: whole obs -> cols 0..
   float* rew_out; float* done_out; int n_act;
   // in-kernel slot draw (indices == nullptr && rng_counters != nullptr): Philox stream 0 of prep_kernel, same values
-  const long long* rng_counters;   // [4] = rng step, [5] = replay size
+  const long long* rng_counters;   // [4] = rng step, [5] = replay size, [6] = first live slot (ring_cap > 0)
   unsigned long long seed;
   int* indices_out;                // optional record of the drawn slots
 };
@@ -271,6 +315,11 @@ __device__ __forceinline__ int philox_slot(unsigned long long seed, unsigned lon
                                 make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
   const unsigned v = (b & 3) == 0 ? r.x : (b & 3) == 1 ? r.y : (b & 3) == 2 ? r.z : r.w;
   return (int)(((unsigned long long)v * rsz) >> 32);
+}
+// u-th live slot of a ring whose live range starts at slot base (u < cap)
+__device__ __forceinline__ int ring_slot(long long base, int u, long long cap) {
+  const long long s = base + u;
+  return (int)(s >= cap ? s - cap : s);
 }
 #endif
 

@@ -4,7 +4,7 @@
 // activation planes into implicit-im2col / shifted-window / zero-bordered operand tiles (one map per tensor: plane = outermost
 // dimension), (iii) the problem lists of every layer group and the two FUSED launches built from them (forward chain, backward
 // chain: fuse_groups wires each consumer problem to the producer tiles it reads) and (iv) the HBM-bound helper kernels around them:
-//   gather2_kernel : replay slot draw + gather of compact replay rows (the ring layout, replay.cu) + float64 VecNormalize +
+//   gather2_kernel : replay slot draw + gather of replay frames (compact rows, replay.cu) + float64 VecNormalize +
 //                    clip + /255 (replay.cu semantics, [SB2] ReplayBuffer.sample(env=VecNormalize), observation_input(scale=True)),
 //                    the 3-plane BF16 split and the conv1 patch rows (8x8 stride-4 patches of the normalised image; the one view
 //                    TMA cannot express, see tools/tma_probe.cu) so that conv1 forward and its wgrad are plain 2-D TMA tiles;
@@ -50,9 +50,12 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
   if (g.indices) slot = g.indices[b];
   else if (g.rng_counters) {
     slot = philox_slot(g.seed, (unsigned long long)g.rng_counters[4], b, (unsigned long long)g.rng_counters[5]);
+    if (g.ring_cap > 0) slot = ring_slot(g.rng_counters[6], (int)slot, g.ring_cap);
     if (g.indices_out && which == 0 && tid == 0) g.indices_out[b] = (int)slot;
   }
-  const float* __restrict__ src = (which ? g.next_obs : g.obs) + (size_t)slot * Ec;
+  const unsigned char* __restrict__ src =
+      g.obs_frame ? g.frames + (size_t)(which ? g.next_frame : g.obs_frame)[slot] * g.frame_bytes
+                  : reinterpret_cast<const unsigned char*>((which ? g.next_obs : g.obs) + (size_t)slot * Ec);
   const double clip_obs = g.normc[1];
   const bool norm_obs = g.normc[3] != 0.0;
   const float scale = g.scale;
@@ -61,7 +64,7 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
   const int rowe = g.W * Ci, pitch = rowe + 8, plane_e = g.H * pitch;
   // image block: exactly the NHWC image with Ci channels -> no index arithmetic; float64 VecNormalize chain per element
   for (int e4 = tid; e4 < (npx >> 2); e4 += blockDim.x) {
-    const float4 v = *reinterpret_cast<const float4*>(src + 4 * e4);
+    const float4 v = frame_load4(src, g.fmt, npx, Ci, 4 * e4);
     float y[4] = {v.x, v.y, v.z, v.w};
     if (norm_obs) {
       const double2 m0 = *reinterpret_cast<const double2*>(g.mean + 4 * e4), m1 = *reinterpret_cast<const double2*>(g.mean + 4 * e4 + 2);
@@ -82,7 +85,7 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
     }
   }
   if (tid == 0) {                                            // direct feature -> column 512 of the feature rows
-    float yy = src[npx];
+    float yy = frame_elem(src, g.fmt, npx, Ci, npx);
     if (norm_obs) yy = (float)fmin(fmax(((double)yy - g.mean[npx]) * g.var[npx], -clip_obs), clip_obs);
     yy = yy / scale;
     uint16_t p0, p1, p2;
@@ -855,7 +858,7 @@ int v2_gather(b2g_sac* h, const GatherArgs& ga, cudaStream_t s) {
     CK(cudaFuncSetAttribute(gather2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = smem;
   }
-  gather2_kernel<<<dim3(ga.B, ga.next_obs ? 2 : 1), 512, smem, s>>>(a);
+  gather2_kernel<<<dim3(ga.B, ga.next_obs || ga.next_frame ? 2 : 1), 512, smem, s>>>(a);
   return 0;
 }
 

@@ -46,7 +46,9 @@ __global__ void prep_kernel(PrepArgs a) {
     const unsigned v[4] = {r.x, r.y, r.z, r.w};
     for (int j = 0; j < 4; ++j) {
       const int b = 4 * i + j;
-      if (b < a.B) a.indices[b] = (int)(((unsigned long long)v[j] * rsz) >> 32);
+      if (b >= a.B) continue;
+      const int u = (int)(((unsigned long long)v[j] * rsz) >> 32);
+      a.indices[b] = a.ring_cap > 0 ? ring_slot(a.counters[6], u, a.ring_cap) : u;
     }
   }
   const int n_eps = a.B * a.A;

@@ -1,10 +1,11 @@
-// Replay rows: compaction of caller observations into the ring layout, and the minibatch gather fused with VecNormalize and
-// the policy's /255 input scaling.
+// Replay rows: compaction of caller observations into compact rows, the frame pool's writes (frame_check / frame_commit), and
+// the minibatch gather fused with VecNormalize and the policy's /255 input scaling.
 //
-// Ring layout.  MLP policy: a row is the observation vector.  CNN policy: a row is COMPACT, Ec = H*W*Ci + 4 floats -- the
+// Row layout.  MLP policy: a row is the observation vector.  CNN policy: a row is COMPACT, Ec = H*W*Ci + 4 floats -- the
 // image planes [H][W][Ci] (NHWC), then the one value of the constant actuator plane the network reads (pixel [0,0] of the last
 // channel, custom_obs_policy.py:28-32), then 3 zero pads.  Callers pass full [H][W][Ci+1] observations; compact_kernel
-// writes them into the ring, the explicit batch and policy inference's staging.
+// writes them into replay_add's staging, the explicit batch and policy inference's staging.  Replay frames hold such rows,
+// optionally with 8-bit image channels (FrameFmt, common.cuh); the gathers decode them into the same fp32 values.
 //
 // gather_kernel restates [SB2] ReplayBuffer.sample(batch_size, env=vec_normalize) -> VecNormalize.normalize_obs /
 // normalize_reward (configured at sb_helper.py:118-119: clip_obs=10, clip_reward=10, eps=1e-8; float64 arithmetic like numpy,
@@ -32,9 +33,9 @@ __global__ void __launch_bounds__(256) compact_kernel(const float* __restrict__ 
 }
 
 // float64 VecNormalize of the 4 row elements [e, e + 4) (e % 4 == 0): clip((x - mean) * istd, +-clip_obs)
-__device__ __forceinline__ void load_norm4(const float* __restrict__ src, const GatherArgs& g, int e, bool norm_obs, double clip_obs,
-                                           float y[4]) {
-  const float4 v = *reinterpret_cast<const float4*>(src + e);
+__device__ __forceinline__ void load_norm4(const unsigned char* __restrict__ src, const GatherArgs& g, int npx, int e, bool norm_obs,
+                                           double clip_obs, float y[4]) {
+  const float4 v = frame_load4(src, g.fmt, npx, g.Cimg, e);
   y[0] = v.x; y[1] = v.y; y[2] = v.z; y[3] = v.w;
   if (norm_obs) {
     const double2 m0 = *reinterpret_cast<const double2*>(g.mean + e), m1 = *reinterpret_cast<const double2*>(g.mean + e + 2);
@@ -59,9 +60,13 @@ __global__ void __launch_bounds__(256) gather_kernel(GatherArgs g) {
   if (g.indices) slot = g.indices[b];
   else if (g.rng_counters) {
     slot = philox_slot(g.seed, (unsigned long long)g.rng_counters[4], b, (unsigned long long)g.rng_counters[5]);
+    if (g.ring_cap > 0) slot = ring_slot(g.rng_counters[6], (int)slot, g.ring_cap);
     if (g.indices_out && which == 0 && blockIdx.x == 0 && threadIdx.x == 0) g.indices_out[b] = (int)slot;
   }
-  const float* __restrict__ src = (which ? g.next_obs : g.obs) + (size_t)slot * E;
+  const unsigned char* __restrict__ fsrc =
+      g.obs_frame ? g.frames + (size_t)(which ? g.next_frame : g.obs_frame)[slot] * g.frame_bytes
+                  : reinterpret_cast<const unsigned char*>((which ? g.next_obs : g.obs) + (size_t)slot * E);
+  const float* __restrict__ src = reinterpret_cast<const float*>(fsrc);   // MLP rows: always fp32
   const double ret_istd = g.normc[0], clip_obs = g.normc[1], clip_rew = g.normc[2];
   const bool norm_obs = g.normc[3] != 0.0, norm_rew = g.normc[4] != 0.0;
   const float inv_scale_denom = g.scale;
@@ -75,7 +80,7 @@ __global__ void __launch_bounds__(256) gather_kernel(GatherArgs g) {
     uint16_t* __restrict__ xlo = which ? g.x_next_lo : g.x_obs_lo;
     for (int e4 = blockIdx.x * blockDim.x + threadIdx.x; e4 < (npx >> 2); e4 += gridDim.x * blockDim.x) {
       float y[4];
-      load_norm4(src, g, 4 * e4, norm_obs, clip_obs, y);
+      load_norm4(fsrc, g, npx, 4 * e4, norm_obs, clip_obs, y);
 #pragma unroll
       for (int j = 0; j < 4; ++j) y[j] = y[j] / inv_scale_denom;
       *reinterpret_cast<float4*>(xdst + 4 * e4) = make_float4(y[0], y[1], y[2], y[3]);
@@ -92,7 +97,7 @@ __global__ void __launch_bounds__(256) gather_kernel(GatherArgs g) {
       }
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) {      // the actuator value -> the direct-feature column of the feature rows
-      float y = src[npx];
+      float y = frame_elem(fsrc, g.fmt, npx, g.Cimg, npx);
       if (norm_obs) y = (float)fmin(fmax(((double)y - g.mean[npx]) * g.var[npx], -clip_obs), clip_obs);
       y = y / inv_scale_denom;
       if (which) g.F_t[(size_t)b * g.FS + g.feat_col] = y;
@@ -103,7 +108,7 @@ __global__ void __launch_bounds__(256) gather_kernel(GatherArgs g) {
     const int E4 = (E & 3) == 0 ? E >> 2 : 0;
     for (int e4 = blockIdx.x * blockDim.x + threadIdx.x; e4 < E4; e4 += gridDim.x * blockDim.x) {
       float y[4];
-      load_norm4(src, g, 4 * e4, norm_obs, clip_obs, y);
+      load_norm4(fsrc, g, 0, 4 * e4, norm_obs, clip_obs, y);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const int e = 4 * e4 + j;
@@ -141,7 +146,73 @@ __global__ void __launch_bounds__(256) gather_kernel(GatherArgs g) {
     }
   }
 }
+__device__ __forceinline__ bool u8_channel(const FrameIo& io, int e) {
+  return io.fmt.n8 > 0 && e < io.npx && io.fmt.ch[e % io.Ci] >= 0;
+}
+
+// one CTA per row (see frame_check_launch)
+__global__ void __launch_bounds__(256) frame_check_kernel(FrameIo io, const int* __restrict__ prev, int* __restrict__ flags) {
+  __shared__ int s_neq, s_bad;
+  const int i = blockIdx.x;
+  if (threadIdx.x == 0) { s_neq = 0; s_bad = 0; }
+  __syncthreads();
+  const float* o = io.c_obs + (size_t)i * io.Ec;
+  const float* nx = io.c_next + (size_t)i * io.Ec;
+  const int p = prev[i];
+  const unsigned char* f = p >= 0 ? io.frames + (size_t)p * io.frame_bytes : nullptr;
+  int neq = 0, bad = 0;
+  for (int e = threadIdx.x; e < io.Ec; e += blockDim.x) {
+    const float v = o[e];
+    if (f && __float_as_uint(frame_elem(f, io.fmt, io.npx, io.Ci, e)) != __float_as_uint(v)) neq = 1;
+    if (u8_channel(io, e)) {
+      // -0.0 would come back as +0.0: refused with the fractions, negatives, values > 255 and NaNs
+      const float w = nx[e];
+      if (!(v >= 0.f && v <= 255.f && v == rintf(v) && !signbit(v))) bad = 1;
+      if (!(w >= 0.f && w <= 255.f && w == rintf(w) && !signbit(w))) bad = 1;
+    }
+  }
+  if (neq) atomicOr(&s_neq, 1);
+  if (bad) atomicOr(&s_bad, 1);
+  __syncthreads();
+  if (threadIdx.x == 0) flags[i] = (f && !s_neq ? 1 : 0) | (s_bad ? 2 : 0);
+}
+
+// grid (m, 2): y = 0 writes the obs row (when it takes a new frame) and the transition's frame indices, y = 1 the next_obs row.
+// plan == nullptr: every row takes two new frames, ids fid0 + 2i and fid0 + 2i + 1.
+__global__ void __launch_bounds__(256) frame_commit_kernel(FrameIo io, const int* __restrict__ plan, long long fid0, long long fcap,
+                                                           int m, int* __restrict__ r_ofr, int* __restrict__ r_nfr, long long first,
+                                                           long long cap) {
+  const int i = blockIdx.x, which = blockIdx.y;
+  const int of = plan ? plan[i] : (int)((fid0 + 2 * i) % fcap);
+  const int nf = plan ? plan[2 * m + i] : (int)((fid0 + 2 * i + 1) % fcap);
+  if (which == 0 && threadIdx.x == 0) {
+    const long long slot = (first + i) % cap;
+    r_ofr[slot] = of;
+    r_nfr[slot] = nf;
+  }
+  if (which == 0 && plan && !plan[m + i]) return;
+  const float* src = (which ? io.c_next : io.c_obs) + (size_t)i * io.Ec;
+  unsigned char* f = io.frames + (size_t)(which ? nf : of) * io.frame_bytes;
+  const FrameFmt& fm = io.fmt;
+  for (int e = threadIdx.x; e < io.Ec; e += blockDim.x) {
+    const float v = src[e];
+    if (e >= io.npx) { reinterpret_cast<float*>(f + fm.tail)[e - io.npx] = v; continue; }
+    if (fm.n8 == 0) { reinterpret_cast<float*>(f)[e] = v; continue; }
+    const int pix = e / io.Ci, k = fm.ch[e - pix * io.Ci];
+    if (k >= 0) f[pix * fm.n8 + k] = (unsigned char)v;
+    else reinterpret_cast<float*>(f + fm.f32_off)[pix * fm.n32 - 1 - k] = v;
+  }
+}
 }  // namespace
+
+void frame_check_launch(const FrameIo& io, const int* prev, int* flags, int m, cudaStream_t s) {
+  if (m > 0) frame_check_kernel<<<m, 256, 0, s>>>(io, prev, flags);
+}
+
+void frame_commit_launch(const FrameIo& io, const int* plan, long long fid0, long long fcap, int m, int* r_ofr, int* r_nfr,
+                         long long first, long long cap, cudaStream_t s) {
+  if (m > 0) frame_commit_kernel<<<dim3(m, 2), 256, 0, s>>>(io, plan, fid0, fcap, m, r_ofr, r_nfr, first, cap);
+}
 
 void compact_rows(const float* src_full, float* dst, long long first_row, long long wrap, int n, int HW, int Cfull, cudaStream_t s) {
   if (n > 0) compact_kernel<<<n, 256, 0, s>>>(src_full, dst, first_row, wrap, HW, Cfull, HW * (Cfull - 1) + 4);
@@ -152,7 +223,7 @@ void gather_launch(const GatherArgs& a, cudaStream_t s) {
   int gx = (E / 4 + 255) / 256;      // one 128-bit group per thread
   if (gx < 1) gx = 1;
   if (gx > 4) gx = 4;
-  dim3 grid(gx, a.B, a.next_obs ? 2 : 1);
+  dim3 grid(gx, a.B, a.next_obs || a.next_frame ? 2 : 1);
   gather_kernel<<<grid, 256, 0, s>>>(a);
 }
 

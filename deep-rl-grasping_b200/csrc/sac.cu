@@ -4,7 +4,8 @@
 //   P  : parameter arena  [ model/pi | model/values_fn | log_ent_coef | target/values_fn ], every
 //        tensor padded to 32 floats, tensor order = SB zip parameter_list (SURVEY.md Appendix B)
 //   Mo, Vo, G : Adam moments and gradients, same offsets as the trainable part of P
-//   replay  : obs[cap,Ec] next_obs[cap,Ec] act[cap,A] rew[cap] done[cap]   (raw, un-normalised; CNN: compact rows, replay.cu)
+//   replay  : frames[frame_cap][frame_bytes] (raw, un-normalised compact rows, RGB planes optionally uint8; replay.cu)
+//             obs_frame[cap] next_frame[cap] (int32) act[cap,A] rew[cap] done[cap]
 //   batch   : x_obs/x_next [B,H,W,C] (normalised, /255), h1/h2/h3 per network, F rows [B,FS]
 //             (512 CNN features | direct feature | replay action | zero pad), gradient maps with
 //             zero borders (dZ3p, dZ2p) so the dgrad gathers need no bounds logic
@@ -625,8 +626,13 @@ TailArgs make_tail(b2g_sac* h, bool want_per_sample) {
 
 GatherArgs make_gather(b2g_sac* h, bool from_replay, bool with_next) {
   GatherArgs g{};
-  g.obs = from_replay ? h->r_obs : h->s_obs;
-  g.next_obs = with_next ? (from_replay ? h->r_next : h->s_next) : nullptr;
+  g.obs = from_replay ? nullptr : h->s_obs;
+  g.next_obs = with_next ? (from_replay ? nullptr : h->s_next) : nullptr;
+  if (from_replay) {
+    g.frames = h->frames; g.frame_bytes = h->frame_bytes; g.obs_frame = h->r_ofr; g.next_frame = with_next ? h->r_nfr : nullptr;
+    g.ring_cap = h->cfg.buffer_capacity;
+  }
+  g.fmt = from_replay ? h->fmt : h->row_fmt;
   g.act = with_next ? (from_replay ? h->r_act : h->s_act) : nullptr;
   g.rew = from_replay ? h->r_rew : h->s_rew;
   g.done = from_replay ? h->r_done : h->s_done;
@@ -648,6 +654,7 @@ PrepArgs make_prep(b2g_sac* h, unsigned long long seed, bool gen, bool apply) {
   PrepArgs pa{};
   pa.counters = h->counters; pa.step_consts = h->step_consts; pa.lr = h->d_lr; pa.metrics = h->metrics;
   pa.indices = h->indices; pa.eps = h->eps; pa.B = h->B; pa.A = h->A; pa.replay_size = nullptr;  /* device counter [5] */
+  pa.ring_cap = h->cfg.buffer_capacity;
   pa.seed = seed; pa.gen = gen ? 1 : 0; pa.apply = apply ? 1 : 0;
   return pa;
 }
@@ -1044,6 +1051,8 @@ int b2g_sac_destroy(b2g_sac* h) {
   for (int q = 0; q < 2; ++q) { if (h->hc_obs[q]) cudaFreeHost(h->hc_obs[q]); if (h->hc_next[q]) cudaFreeHost(h->hc_next[q]); }
   if (h->h_met) cudaFreeHost(h->h_met);
   if (h->h_cnt) cudaFreeHost(h->h_cnt);
+  if (h->h_plan) cudaFreeHost(h->h_plan);
+  if (h->h_rc) cudaFreeHost(h->h_rc);
   for (int k = 0; k < 2; ++k) { if (h->hp_stats[k]) cudaFreeHost(h->hp_stats[k]); if (h->ev_stats[k]) cudaEventDestroy(h->ev_stats[k]); }
   for (int j = 0; j < 2; ++j) {
     if (h->ev_h2d[j]) cudaEventDestroy(h->ev_h2d[j]);
@@ -1060,9 +1069,17 @@ int b2g_sac_destroy(b2g_sac* h) {
   return 0;
 }
 
-int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
+int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) { return b2g_sac_create2(cfg, nullptr, out); }
+
+int b2g_sac_create2(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, b2g_sac** out) {
   if (!cfg || !out) return b2g_fail(B2G_EINVAL, "cfg/out is NULL");
   *out = nullptr;
+  if (replay && replay->frame_capacity < cfg->buffer_capacity + 1)
+    return b2g_fail(B2G_EINVAL, "frame_capacity must be at least buffer_capacity + 1");
+  if (replay && replay->u8_plane_mask && cfg->obs_h <= 0) return b2g_fail(B2G_EINVAL, "the MLP policy has no 8-bit image planes");
+  if (replay && replay->u8_plane_mask &&
+      (cfg->obs_c < 2 || cfg->obs_c - 1 > 8 || (replay->u8_plane_mask >> (cfg->obs_c - 1)) != 0))
+    return b2g_fail(B2G_EINVAL, "u8_plane_mask may only name image planes, at most 8 (the actuator plane is the last channel)");
   if (cfg->hidden != 64 && cfg->hidden != 128 && cfg->hidden != 192 && cfg->hidden != 256)
     return b2g_fail(B2G_EINVAL, "hidden must be 64, 128, 192 or 256 (SAC.layers [H, H])");
   if (cfg->n_act < 1 || cfg->n_act > 8) return b2g_fail(B2G_EINVAL, "n_act must be in [1,8]");
@@ -1112,12 +1129,33 @@ int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) {
     h->v2.on = h->cnn && cfg->precision == B2G_PREC_BF16X3 && h->Hi == 64 && h->Wi == 64;
     if (const char* dbg = getenv("B2G_CG_DEBUG")) h->v2.dbg = atoi(dbg);
   }
-  // replay ring: 2 * cap * Ec * 4 bytes (depth: 32.8 GB at 1M slots; full rows would take 65.6 GB)
-  DA(h->r_obs, cap * h->Ec); DA(h->r_next, cap * h->Ec); DA(h->r_act, cap * h->A); DA(h->r_rew, cap); DA(h->r_done, cap);
-  if (h->cnn) {
-    h->stage_rows = std::max(B, 256);
-    DA(h->obs_stage, (size_t)h->stage_rows * h->E);
+  {   // frame formats: the fp32 compact row, and the replay frames (8-bit planes first, then the fp32 planes, then the tail)
+    const int npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0, HW = h->Hi * h->Wi;
+    h->row_fmt.n32 = h->Cimg; h->row_fmt.tail = 4 * npx;
+    h->u8_mask = replay ? replay->u8_plane_mask : 0;
+    h->fmt = h->row_fmt;
+    h->frame_bytes = (int64_t)h->Ec * 4;
+    if (h->u8_mask) {
+      FrameFmt& f = h->fmt;
+      f.n8 = f.n32 = 0;
+      for (int c = 0; c < h->Cimg; ++c) f.ch[c] = (h->u8_mask >> c & 1) ? (signed char)f.n8++ : (signed char)(-1 - f.n32++);
+      f.f32_off = HW * f.n8;
+      f.tail = f.f32_off + 4 * HW * f.n32;
+      if (f.f32_off % 16 != 0) return bail(b2g_fail(B2G_EINVAL, "8-bit planes need H * W * (8-bit planes) to be a multiple of 16"));
+      h->frame_bytes = (f.tail + 16 + 15) / 16 * 16;      // 16-byte frame stride: the gathers' 128-bit loads stay aligned
+    }
+    h->frame_cap = replay ? replay->frame_capacity : 2 * cap;
+    if (h->frame_cap > INT32_MAX) return bail(b2g_fail(B2G_EINVAL, "frame_capacity must fit in int32 (frame indices)"));
+    h->dedup = h->frame_cap < 2 * cap;     // at 2 cap every transition has two frames of its own: sharing would save nothing
   }
+  if ((rc = dev_alloc(h->allocs, h->stream, &h->frames, (size_t)(h->frame_cap * h->frame_bytes)))) return bail(rc);
+  DA(h->r_ofr, cap); DA(h->r_nfr, cap); DA(h->r_act, cap * h->A); DA(h->r_rew, cap); DA(h->r_done, cap);
+  h->stage_rows = std::max(B, 256);
+  if (h->cnn) DA(h->obs_stage, (size_t)h->stage_rows * h->E);
+  DA(h->c_obs, (size_t)h->stage_rows * h->Ec); DA(h->c_next, (size_t)h->stage_rows * h->Ec); DA(h->d_plan, 4 * h->stage_rows);
+  if (cudaMallocHost((void**)&h->h_plan, 4 * h->stage_rows * sizeof(int)) != cudaSuccess ||
+      cudaMallocHost((void**)&h->h_rc, 2 * sizeof(long long)) != cudaSuccess)
+    return bail(b2g_fail(B2G_ECUDA, "replay staging"));
   DA(h->d_mean, h->Ec); DA(h->d_istd, h->Ec); DA(h->d_normc, 8);
   for (int k = 0; k < 2; ++k) {
     if (cudaMallocHost((void**)&h->hp_stats[k], (size_t)(2 * h->Ec + 8) * sizeof(double)) != cudaSuccess ||
@@ -1292,44 +1330,138 @@ int b2g_reset_optimizer(b2g_sac* h) {
 int b2g_replay_add(b2g_sac* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done,
                    int64_t n) {
   if (!h || !obs || !act || !rew || !next_obs || !done || n < 0) return b2g_fail(B2G_EINVAL, "NULL argument");
+  if (h->dedup && 2 * n > h->frame_cap) return b2g_fail(B2G_EINVAL, "replay_add: 2 n rows exceed frame_capacity");
   CK(cudaSetDevice(h->cfg.device));
-  const int64_t cap = h->cfg.buffer_capacity;
-  int64_t done_n = 0;
-  while (done_n < n) {
-    const int64_t chunk = std::min(n - done_n, cap - h->r_pos);
-    const size_t E = h->E, A = h->A;
-    if (int rc = load_rows(h, obs + done_n * E, h->r_obs, h->r_pos, cap, chunk)) return rc;
-    if (int rc = load_rows(h, next_obs + done_n * E, h->r_next, h->r_pos, cap, chunk)) return rc;
-    CK(cudaMemcpyAsync(h->r_act + h->r_pos * A, act + done_n * A, chunk * A * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_rew + h->r_pos, rew + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_done + h->r_pos, done + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
-    h->r_pos = (h->r_pos + chunk) % cap;
-    h->r_size = std::min(cap, h->r_size + chunk);
-    done_n += chunk;
+  const int64_t cap = h->cfg.buffer_capacity, FC = h->frame_cap;
+  // rows per chunk: one commit launch writes distinct transition slots and distinct frames
+  const int64_t R = std::min<int64_t>({(int64_t)h->stage_rows, cap, FC / 2});
+  const size_t E = h->E, A = h->A;
+  FrameIo io{};
+  io.c_obs = h->c_obs; io.c_next = h->c_next; io.frames = h->frames; io.frame_bytes = h->frame_bytes;
+  io.fmt = h->fmt; io.npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0; io.Ci = h->cnn ? h->Cimg : 1; io.Ec = h->Ec;
+  int* flags = h->h_plan + 3 * R;
+  // rows [c0, c0 + m) -> compact staging, then (when sharing frames or checking 8-bit values) frame_check -> flags, synchronised
+  auto stage_check = [&](int64_t c0, int m, bool check) -> int {
+    if (c0 > 0) CK(cudaStreamSynchronize(h->stream));        // the previous chunk's plan upload has left h_plan
+    if (int rc = load_rows(h, obs + c0 * E, h->c_obs, 0, R, m)) return rc;
+    if (int rc = load_rows(h, next_obs + c0 * E, h->c_next, 0, R, m)) return rc;
+    if (!check) return 0;
+    for (int i = 0; i < m; ++i) {      // candidate frame of row i: the previous call's next_obs of row i, while it still exists
+      const int64_t p = c0 + i < (int64_t)h->prev_next.size() ? h->prev_next[c0 + i] : -1;
+      h->h_plan[i] = h->dedup && p >= 0 && p > h->next_fid - FC ? (int)(p % FC) : -1;
+    }
+    CK(cudaMemcpyAsync(h->d_plan, h->h_plan, m * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    frame_check_launch(io, h->d_plan, h->d_plan + 3 * R, m, h->stream);
+    CK(cudaMemcpyAsync(flags, h->d_plan + 3 * R, m * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < m; ++i)
+      if (flags[i] & 2) return b2g_fail(B2G_EINVAL, "replay_add: a value of an 8-bit plane is not an integer in [0, 255]");
+    return 0;
+  };
+  // a call larger than the staging validates every row before it stores the first one
+  if (h->u8_mask && n > R)
+    for (int64_t c0 = 0; c0 < n; c0 += R)
+      if (int rc = stage_check(c0, (int)std::min<int64_t>(R, n - c0), true)) return rc;
+  // next frame id; a frame that would overwrite one a live transition references drops the oldest transitions first
+  auto alloc_frame = [&]() -> int64_t {
+    const int64_t f = h->next_fid++, over = f - FC;
+    while (h->head_seq > h->tail_seq) {
+      while (h->lw.front().first < h->tail_seq) h->lw.pop_front();
+      if (h->lw.front().second > over) break;
+      ++h->tail_seq; ++h->evicted;
+    }
+    return f;
+  };
+  std::vector<int64_t> next_ids((size_t)n);
+  for (int64_t c0 = 0; c0 < n; c0 += R) {
+    const int m = (int)std::min<int64_t>(R, n - c0);
+    if (int rc = stage_check(c0, m, h->dedup || (h->u8_mask && n <= R))) return rc;
+    const int64_t first = h->head_seq, fid0 = h->next_fid;
+    for (int i = 0; i < m; ++i) {
+      if (h->head_seq - h->tail_seq == cap) ++h->tail_seq;                       // the ring's own replacement
+      const int64_t p = c0 + i < (int64_t)h->prev_next.size() ? h->prev_next[c0 + i] : -1;
+      // shared only while the frame outlives the allocation of this row's next_obs frame
+      const bool share = h->dedup && (flags[i] & 1) && p >= h->next_fid + 1 - FC;
+      const int64_t of = share ? p : alloc_frame();
+      const int64_t nf = alloc_frame();
+      while (!h->lw.empty() && h->lw.back().second >= of) h->lw.pop_back();
+      h->lw.emplace_back(h->head_seq++, of);
+      h->h_plan[i] = (int)(of % FC); h->h_plan[m + i] = share ? 0 : 1; h->h_plan[2 * m + i] = (int)(nf % FC);
+      next_ids[c0 + i] = nf;
+    }
+    if (h->dedup) CK(cudaMemcpyAsync(h->d_plan, h->h_plan, 3 * m * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    frame_commit_launch(io, h->dedup ? h->d_plan : nullptr, fid0, FC, m, h->r_ofr, h->r_nfr, first, cap, h->stream);
+    for (int64_t k = 0; k < m;) {          // act / rew / done into slots (first + k) % cap, in at most two pieces
+      const int64_t pos = (first + k) % cap, len = std::min<int64_t>(m - k, cap - pos);
+      CK(cudaMemcpyAsync(h->r_act + pos * A, act + (c0 + k) * A, len * A * sizeof(float), cudaMemcpyDefault, h->stream));
+      CK(cudaMemcpyAsync(h->r_rew + pos, rew + c0 + k, len * sizeof(float), cudaMemcpyDefault, h->stream));
+      CK(cudaMemcpyAsync(h->r_done + pos, done + c0 + k, len * sizeof(float), cudaMemcpyDefault, h->stream));
+      k += len;
+    }
   }
-  h->h_cnt[7] = h->r_size;
-  CK(cudaMemcpyAsync(h->counters + 5, h->h_cnt + 7, sizeof(long long), cudaMemcpyHostToDevice, h->stream));
+  h->prev_next.swap(next_ids);
+  h->r_size = h->head_seq - h->tail_seq;
+  // sampling draws u in [0, size) and reads slot (first live + u) % cap; the first live slot is 0 unless transitions went early
+  h->h_rc[0] = h->r_size;
+  h->h_rc[1] = h->r_size == cap ? 0 : h->tail_seq % cap;
+  CK(cudaMemcpyAsync(h->counters + 5, h->h_rc, 2 * sizeof(long long), cudaMemcpyHostToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));     // host arrays are caller-owned: copied before return
   return 0;
 }
 
 int64_t b2g_replay_size(const b2g_sac* h) { return h ? h->r_size : 0; }
 
+int b2g_replay_info(const b2g_sac* h, int64_t* capacity, int64_t* size, int64_t* frame_capacity, int64_t* live_frames,
+                    int64_t* bytes, int64_t* evicted_early) {
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  const int64_t cap = h->cfg.buffer_capacity;
+  int64_t live = 0;
+  if (h->r_size > 0) {
+    int64_t lo = h->next_fid;
+    for (const auto& q : h->lw) if (q.first >= h->tail_seq) { lo = q.second; break; }
+    live = h->next_fid - lo;
+  }
+  if (capacity) *capacity = cap;
+  if (size) *size = h->r_size;
+  if (frame_capacity) *frame_capacity = h->frame_cap;
+  if (live_frames) *live_frames = live;
+  if (bytes) *bytes = h->frame_cap * h->frame_bytes + cap * (int64_t)(2 * sizeof(int) + (h->A + 2) * sizeof(float));
+  if (evicted_early) *evicted_early = h->evicted;
+  return 0;
+}
+
 int b2g_replay_get(b2g_sac* h, int64_t slot, float* obs, float* act, float* rew, float* next_obs, float* done) {
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  if (slot < 0 || slot >= h->r_size) return b2g_fail(B2G_EINVAL, "replay slot out of range");
+  const int64_t cap = h->cfg.buffer_capacity;
+  if (slot < 0 || slot >= cap || ((slot - h->tail_seq % cap) % cap + cap) % cap >= h->r_size)
+    return b2g_fail(B2G_EINVAL, "replay slot is not live");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
   const size_t A = h->A;
-  // expand the ring row: for the CNN policy the actuator plane comes back as zeros except pixel [0,0] (all the policy reads of it)
-  std::vector<float> row(h->Ec);
+  // expand the frames: for the CNN policy the actuator plane comes back as zeros except pixel [0,0] (all the policy reads of it)
+  std::vector<unsigned char> fr(h->frame_bytes);
+  const FrameFmt& fm = h->fmt;
+  const int npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0;
   for (int w = 0; w < 2; ++w) {
     float* dst = w ? next_obs : obs;
     if (!dst) continue;
-    CK(cudaMemcpy(row.data(), (w ? h->r_next : h->r_obs) + slot * h->Ec, h->Ec * sizeof(float), cudaMemcpyDeviceToHost));
+    int fi = 0;
+    CK(cudaMemcpy(&fi, (w ? h->r_nfr : h->r_ofr) + slot, sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(fr.data(), h->frames + (size_t)fi * h->frame_bytes, h->frame_bytes, cudaMemcpyDeviceToHost));
     std::fill(dst, dst + h->E, 0.f);
-    for (int e = 0; e < h->Ec; ++e)
-      if (const int f = full_index(h, e); f >= 0) dst[f] = row[e];
+    for (int e = 0; e < h->Ec; ++e) {
+      const int f = full_index(h, e);
+      if (f < 0) continue;
+      float v;
+      if (e >= npx) memcpy(&v, fr.data() + fm.tail + 4 * (e - npx), 4);
+      else if (fm.n8 == 0) memcpy(&v, fr.data() + 4 * e, 4);
+      else {
+        const int pix = e / h->Cimg, k = fm.ch[e % h->Cimg];
+        if (k >= 0) v = (float)fr[pix * fm.n8 + k];
+        else memcpy(&v, fr.data() + fm.f32_off + 4 * (pix * fm.n32 - 1 - k), 4);
+      }
+      dst[f] = v;
+    }
   }
   if (act) CK(cudaMemcpy(act, h->r_act + slot * A, A * sizeof(float), cudaMemcpyDeviceToHost));
   if (rew) CK(cudaMemcpy(rew, h->r_rew + slot, sizeof(float), cudaMemcpyDeviceToHost));

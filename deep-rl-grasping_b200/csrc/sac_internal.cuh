@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <deque>
 #include <map>
 #include <string>
 #include <tuple>
@@ -94,13 +95,27 @@ struct b2g_sac {
   float* metrics = nullptr;
   cudaStream_t stream = nullptr;
   std::vector<void*> allocs;
-  // replay ring, raw (un-normalised) rows of Ec floats.  MLP policy: Ec = E.  CNN policy: COMPACT rows (replay.cu), Ec = H*W*Cimg
-  // + 4: the image planes, the ONE actuator value the policy reads (pixel [0,0] of the last plane; augmented_nature_cnn never
-  // reads the rest of it, custom_obs_policy.py:28-30) and 3 pad floats.  The explicit batch (s_obs / s_next) and the pipelined
-  // staging (ps_obs / ps_next) hold the same rows.
+  // Raw (un-normalised) observations travel as compact rows of Ec floats.  MLP policy: Ec = E.  CNN policy: COMPACT rows
+  // (replay.cu), Ec = H*W*Cimg + 4: the image planes, the ONE actuator value the policy reads (pixel [0,0] of the last plane;
+  // augmented_nature_cnn never reads the rest of it, custom_obs_policy.py:28-30) and 3 pad floats.  The explicit batch
+  // (s_obs / s_next) and the pipelined staging (ps_obs / ps_next) hold such rows.
   int Ec = 0;
-  float *r_obs = nullptr, *r_next = nullptr, *r_act = nullptr, *r_rew = nullptr, *r_done = nullptr;
-  int64_t r_size = 0, r_pos = 0;
+  // Replay: a ring of cap transition slots {obs frame, next_obs frame, act, rew, done} over a pool of frame_cap frames (one
+  // compact row each, stored in format fmt) allocated in FIFO order with monotone 64-bit ids; frame id f sits at f % frame_cap.
+  // Transitions are numbered too: the live ones are [tail_seq, head_seq), transition t sits at slot t % cap.
+  unsigned char* frames = nullptr;
+  int64_t frame_cap = 0, frame_bytes = 0;
+  FrameFmt fmt{}, row_fmt{};         // frame format; format of an fp32 compact row (explicit batch, staging)
+  uint32_t u8_mask = 0;
+  bool dedup = false;                // obs may share the previous call's next_obs frame (frame_cap < 2 cap)
+  int *r_ofr = nullptr, *r_nfr = nullptr;
+  float *r_act = nullptr, *r_rew = nullptr, *r_done = nullptr;
+  int64_t r_size = 0, head_seq = 0, tail_seq = 0, next_fid = 0, evicted = 0;
+  std::deque<std::pair<int64_t, int64_t>> lw;   // (transition, obs frame id): sliding-window minimum of the live obs frames
+  std::vector<int64_t> prev_next;    // frame ids of the last replay_add's next_obs rows
+  float *c_obs = nullptr, *c_next = nullptr;    // replay_add staging: compact rows [stage_rows][Ec]
+  int *d_plan = nullptr, *h_plan = nullptr;     // [4][stage_rows]: frame plan (3 rows) + check flags; h_plan pinned
+  long long* h_rc = nullptr;         // pinned: replay size, first live slot -> counters[5..6]
   float* obs_stage = nullptr;        // CNN: caller observations in the full layout [stage_rows][E] on their way to compact rows
   int stage_rows = 0;
   // normalisation, in the ring layout (pads: mean 0, istd 1)

@@ -27,7 +27,11 @@ class Learner:
     def __init__(self, obs_shape: Sequence[int], n_act: int = 5, hidden: int = 64, batch_size: int = 64,
                  buffer_size: int = 100000, gamma: float = 0.99, tau: float = 0.005,
                  target_entropy: Optional[float] = None, seed: int = 0, precision: int = _lib.B2G_PREC_FP32_SIMT,
-                 device: int = 0, rank: int = 0, nranks: int = 1, nccl_id: Optional[bytes] = None):
+                 device: int = 0, rank: int = 0, nranks: int = 1, nccl_id: Optional[bytes] = None,
+                 frame_capacity: Optional[int] = None, u8_planes: Sequence[int] = ()):
+        """frame_capacity / u8_planes: replay storage (include/b200grasp.h, b2g_replay_cfg).  None and () keep two fp32
+        frames per replay slot; a smaller frame budget shares each obs with the previous row's next_obs when they are
+        equal, and u8_planes lists image channels stored as one byte per pixel (values must be integers in [0, 255])."""
         self.lib = _lib.load()
         self.obs_shape = tuple(int(s) for s in obs_shape)
         self.n_act, self.batch_size = int(n_act), int(batch_size)
@@ -53,7 +57,15 @@ class Learner:
             lib_path = _lib.default_nccl_lib()
             cfg.nccl_lib = lib_path.encode() if lib_path else None
         self.h = C.c_void_p()
-        _lib.check(self.lib.b2g_sac_create(C.byref(cfg), C.byref(self.h)))
+        self.frame_capacity = None if frame_capacity is None else int(frame_capacity)
+        self.u8_planes = tuple(int(c) for c in u8_planes)
+        rcfg = None
+        if self.frame_capacity is not None or self.u8_planes:
+            if any(not 0 <= c < 32 for c in self.u8_planes):
+                raise ValueError(f"u8_planes must be channel indices (got {self.u8_planes})")
+            rcfg = _lib.ReplayCfg(2 * int(buffer_size) if self.frame_capacity is None else self.frame_capacity,
+                                  sum(1 << c for c in set(self.u8_planes)))
+        _lib.check(self.lib.b2g_sac_create2(C.byref(cfg), None if rcfg is None else C.byref(rcfg), C.byref(self.h)))
         self.obs_elems = int(np.prod(self.obs_shape))
         self._info = OrderedDict()
         name, numel, ndim = C.c_char_p(), C.c_int64(), C.c_int32()
@@ -165,6 +177,13 @@ class Learner:
 
     def replay_size(self) -> int:
         return int(self.lib.b2g_replay_size(self.h))
+
+    def replay_info(self) -> dict:
+        """capacity, size, frame_capacity, live_frames, bytes (device memory of the replay), evicted_early."""
+        keys = ("capacity", "size", "frame_capacity", "live_frames", "bytes", "evicted_early")
+        vals = [C.c_int64() for _ in keys]
+        _lib.check(self.lib.b2g_replay_info(self.h, *[C.byref(v) for v in vals]))
+        return {k: int(v.value) for k, v in zip(keys, vals)}
 
     def replay_get(self, slot: int) -> dict:
         """One stored (raw) transition, like ``ReplayBuffer.storage[slot]``."""

@@ -65,7 +65,7 @@ class SAC:
                  batch_size=64, tau=0.005, ent_coef="auto", target_update_interval=1, gradient_steps=1,
                  target_entropy="auto", action_noise=None, random_exploration=0.0, verbose=0, tensorboard_log=None,
                  _init_setup_model=True, policy_kwargs=None, full_tensorboard_log=False, seed=None, n_cpu_tf_sess=None,
-                 precision="bf16x3", device=0, rank=0, nranks=1, nccl_id=None):
+                 precision="bf16x3", device=0, rank=0, nranks=1, nccl_id=None, replay_frames=None, replay_u8_planes=()):
         if ent_coef != "auto":
             raise NotImplementedError("only ent_coef='auto' (every shipped zip; SURVEY.md section 8c) is built")
         if target_update_interval != 1:
@@ -87,6 +87,9 @@ class SAC:
         self.verbose, self.tensorboard_log, self.seed = verbose, tensorboard_log, seed
         self.ent_coef, self.target_entropy = ent_coef, target_entropy
         self.precision = precision
+        # replay storage (Learner: frame_capacity, u8_planes); None / () = two fp32 frames per replay slot
+        self.replay_frames = None if replay_frames is None else int(replay_frames)
+        self.replay_u8_planes = tuple(int(c) for c in replay_u8_planes)
         self._dev = dict(device=device, rank=rank, nranks=nranks, nccl_id=nccl_id)
         self._layout_from_zip = False
         self.num_timesteps, self.n_updates = 0, 0
@@ -129,7 +132,8 @@ class SAC:
         tgt = -float(n_act) if self.target_entropy == "auto" else float(self.target_entropy)
         self.learner = Learner(obs_shape, n_act=n_act, hidden=self.hidden, batch_size=self.batch_size, buffer_size=self.buffer_size,
                                gamma=self.gamma, tau=self.tau, target_entropy=tgt, seed=int(self.seed or 0),
-                               precision=_PRECISIONS[self.precision], **self._dev)
+                               precision=_PRECISIONS[self.precision], frame_capacity=self.replay_frames,
+                               u8_planes=self.replay_u8_planes, **self._dev)
         self._init_parameters()
         self._sync_norm_stats()
 
@@ -154,7 +158,7 @@ class SAC:
         self.learner.load_parameters(p)
 
     def close(self):
-        """Releases the device learner (replay ring included: 2 * buffer_size * obs_elems * 4 bytes of HBM)."""
+        """Releases the device learner (replay included: Learner.replay_info()["bytes"] of HBM)."""
         if self.learner is not None:
             self.learner.close()
             self.learner = None
@@ -289,7 +293,8 @@ class SAC:
                                   "high": float(np.max(self.observation_space.high))},
             "action_space": {"shape": list(self.action_space.shape), "low": [float(x) for x in np.ravel(self.action_space.low)],
                              "high": [float(x) for x in np.ravel(self.action_space.high)]},
-            "b200grasp": {"precision": self.precision, "n_updates": self.n_updates},
+            "b200grasp": {"precision": self.precision, "n_updates": self.n_updates, "replay_frames": self.replay_frames,
+                          "replay_u8_planes": list(self.replay_u8_planes)},
         }
 
     def save(self, save_path, cloudpickle=False):

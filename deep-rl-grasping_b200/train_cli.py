@@ -107,8 +107,14 @@ def train(args):
             policy, kw = CnnPolicy, {"layers": c["layers"], "cnn_extractor": "augmented_nature_cnn"}
         else:
             policy, kw = MlpPolicy, {"layers": c["layers"], "layer_norm": False}
+        replay = {}
+        if args.replay_spare is not None:
+            # every transition holds one frame of its own plus one per episode end; n_envs more for the rows in flight
+            replay["replay_frames"] = int(c["buffer_size"] * (1.0 + args.replay_spare)) + n_envs
+        if _is_image_obs(env) and config.get("full_observation", False):
+            replay["replay_u8_planes"] = (0, 1, 2)        # RGB renders as uint8 (gripperEnv/sensor.py), depth stays fp32
         model = SAC(policy, env, policy_kwargs=kw, verbose=1, gamma=config["discount_factor"], buffer_size=c["buffer_size"],
-                    batch_size=c["batch_size"], learning_rate=c["step_size"], precision=args.precision)
+                    batch_size=c["batch_size"], learning_rate=c["step_size"], precision=args.precision, **replay)
         if args.load_dir:
             old = SAC.load(args.load_dir, env, buffer_size=1)
             model.load_parameters(old.get_parameters(), exact_match=False)
@@ -193,6 +199,9 @@ def build_parser():
     t.add_argument("--env", type=str, default=None, help="module:callable environment factory (default: the reference's gripper-env-v0)")
     t.add_argument("--n_envs", type=int, default=1, help=">1: SubprocVecEnv actor loop on host cores feeding the device replay")
     t.add_argument("--precision", default="bf16x3", choices=["fp32", "bf16x3", "bf16"])
+    t.add_argument("--replay_spare", type=float, default=None,
+                   help="SAC replay frame budget buffer_size * (1 + F) + n_envs (observations shared between consecutive "
+                        "transitions; 0.125 covers episodes down to ~9 steps); default: two frames per replay slot")
     t.add_argument("--eval_freq", type=int, default=50000)
     t.add_argument("--checkpoint_freq", type=int, default=25000)
     t.set_defaults(func=train)

@@ -73,7 +73,24 @@ int b2g_version(void);
 /* writes a fresh 128-byte ncclUniqueId (rank 0 calls this, then shares it out of band) */
 int b2g_nccl_unique_id(void* out128, const char* nccl_lib);
 
-int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out);
+/* Replay storage.  The replay keeps a pool of frame_capacity observation frames; a transition references the frame of its obs
+ * and of its next_obs.  b2g_replay_add stores every next_obs as a new frame, and row i's obs shares the frame of row i's next_obs
+ * of the previous call when the two are bitwise equal (the learn loop's next_obs(t) == obs(t+1) within an episode), so
+ * episodic streams need about cap * (1 + episode ends / transitions) + n_envs frames.  When a new frame would overwrite one a
+ * live transition still references, the oldest transitions are dropped early (b2g_replay_info counts them) and sampling stays
+ * uniform over the live ones.
+ * u8_plane_mask: bit c declares image channel c (CNN policy, c < obs_c - 1) an 8-bit plane, stored as one byte per pixel;
+ * b2g_replay_add then refuses (B2G_EINVAL, nothing stored) any value there that is not an integer in [0, 255].
+ * NULL (the default) = frame_capacity 2 * buffer_capacity and no 8-bit planes.  From 2 * buffer_capacity frames on, every
+ * transition keeps two frames of its own (sharing would save nothing): the bytes of two rows per transition, and nothing is
+ * ever dropped early. */
+typedef struct b2g_replay_cfg {
+  int64_t frame_capacity;      /* >= buffer_capacity + 1 */
+  uint32_t u8_plane_mask;
+} b2g_replay_cfg;
+
+int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out);   /* = b2g_sac_create2(cfg, NULL, out) */
+int b2g_sac_create2(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay /* NULL = default */, b2g_sac** out);
 int b2g_sac_destroy(b2g_sac* h);
 /* Peer-memory data parallelism (nranks > 1, one process per GPU of one NVLink node).  Every rank exports B2G_DP_EXPORT_BYTES
  * (CUDA IPC handles of its parameter arena, gradient receive arena and exchange block), the caller gathers the nranks blobs in rank
@@ -104,14 +121,20 @@ int b2g_reset_optimizer(b2g_sac* h);   /* zero Adam moments and step counters (f
 /* ---- replay buffer (ReplayBuffer.add; stores UN-normalised obs/reward as SB does when a
  *      VecNormalize wraps the env) and VecNormalize statistics used at sample time
  *      (sb_helper.py:118-119; float64 like numpy) */
+/* n rows of full observations (host or device memory).  With frame_capacity < 2 * buffer_capacity, 2 n <= frame_capacity;
+ * otherwise a call larger than the ring keeps its last buffer_capacity rows, like any ring. */
 int b2g_replay_add(b2g_sac* h, const float* obs, const float* act, const float* rew, const float* next_obs,
                    const float* done, int64_t n);
 int64_t b2g_replay_size(const b2g_sac* h);
 /* ReplayBuffer.storage[slot] ([SB2] common/buffers.py): one stored (raw) transition back to the host; any output may be
- * NULL.  slot in [0, b2g_replay_size).  CNN policy: the ring holds compact rows (see b2g_debug_compact_host), so obs and
- * next_obs come back with the image planes as stored and the actuator plane zero except pixel [0,0], the one value the policy
- * reads of it. */
+ * NULL.  slot must be live: one of the b2g_replay_size slots starting at the oldest transition (slot 0 unless transitions
+ * were dropped early).  CNN policy: frames hold compact rows (see b2g_debug_compact_host), so obs and next_obs come back with
+ * the image planes as stored and the actuator plane zero except pixel [0,0], the one value the policy reads of it. */
 int b2g_replay_get(b2g_sac* h, int64_t slot, float* obs, float* act, float* rew, float* next_obs, float* done);
+/* replay counters; any output may be NULL.  live_frames = frames from the oldest one a live transition references to the newest;
+ * bytes = device memory of the replay (frames, frame indices, actions, rewards, dones) */
+int b2g_replay_info(const b2g_sac* h, int64_t* capacity, int64_t* size, int64_t* frame_capacity, int64_t* live_frames,
+                    int64_t* bytes, int64_t* evicted_early);
 /* What the LAST gradient step (any entry point, the CUDA-graph path included) drew and produced: the replay slots
  * indices[batch] (sampled steps only), the policy noise eps[batch, n_act], the per-sample rows q1,q2,v,logp,v_targ,
  * q1_pi,q2_pi (7 x [batch]) and the squashed actions pi[batch, n_act].  Any pointer may be NULL.  This is what lets a
