@@ -1,18 +1,21 @@
 // TMA-fed wgmma contraction engine (sm_90a).  See cg.cuh for the problem description.
 //
 // Persistent, warp-specialised kernel, one CTA per SM, grid = min(#tiles, #SMs):
-//   warps 0..7  : two consumer warpgroups.  Warpgroup w issues wgmma.mma_async for rows [64w, 64w + 64) of the 128-row tile
+//   warps 0..7  : two MMA warpgroups.  Warpgroup w issues wgmma.mma_async for rows [64w, 64w + 64) of the 128-row tile
 //                 (BF16 planes from the swizzled ring, fp32 accumulators in registers).  Precision modes per problem: 1 product
 //                 (hi*hi), 3 products (2-plane split) or 6 products (3-plane split hi/mid/lo: everything down to 2^-24), one
 //                 MMA per product into the accumulator of its order (see mma_chunk), one K-chunk of them in flight while the
-//                 next chunk is awaited.  After the last K-chunk the same warps run the epilogue: the
-//                 accumulator columns pass, 16 at a time, through a small shared-memory staging block so that every lane ends up
-//                 with one output row; then bias/ReLU or the ReLU mask (+ the bias-gradient column sums), the split into BF16
-//                 planes and the row's 32-column stores of every plane (16-byte vectors).  The producers keep filling the ring
-//                 for the next tile meanwhile;
-//   warps 8..9  : TMA producers (whole warps, converged; one elected lane issues).  The cp.async.bulk.tensor boxes of a K-chunk
-//                 (operands x planes) are dealt round-robin to the two warps; warp 8 posts the chunk's expect_tx.
-//   warps 10..11: complete the producer warpgroup for setmaxnreg and exit.
+//                 next chunk is awaited.  After the last K-chunk an ACT / DGRAD tile's sums go to the shared-memory handoff
+//                 buffer (acc_full / acc_empty barriers) and the warps start the next tile; a RAW / WGRAD tile is finished in
+//                 place: its columns pass, 16 at a time, through a small staging block so that every lane holds one output row,
+//                 then the fp32 stores or red.adds;
+//   warps 8..11 : the epilogue warpgroup.  Lane l of warp e reads row 32e + l of a handed-off tile (all its columns), then
+//                 bias/ReLU or the ReLU mask (+ the bias-gradient column sums), the split into BF16 planes and the row's
+//                 32-column stores of every plane (16-byte vectors), the split-K finalisation and the dependency arrivals -- while
+//                 the MMA warps run the next tile's mainloop;
+//   warps 12..13: TMA producers (whole warps, converged; one elected lane issues).  The cp.async.bulk.tensor boxes of a K-chunk
+//                 (operands x planes) are dealt round-robin to the two warps; warp 12 posts the chunk's expect_tx.
+//   warps 14..15: complete the producer warpgroup for setmaxnreg and exit.
 #include <cuda_bf16.h>
 
 #include <cstdio>
@@ -25,15 +28,18 @@
 namespace b2g {
 namespace {
 
-// warps 0..7: consumer warpgroups (MMA + epilogue), warps 8..11: producer warpgroup, of which warps 8..9 issue the TMA loads and
-// warps 10..11 only hand their registers over (setmaxnreg acts on whole warpgroups)
-constexpr int NEPI_WARPS = CG_EPI_WARPS, NPROD_WARPS = 2, PROD_WARP0 = NEPI_WARPS;
-constexpr int NTHREADS = 32 * (NEPI_WARPS + 4);
-// registers per thread after setmaxnreg: 2 x 232 + 40 = 512 per SM sub-partition lane (each holds two consumer warps and one
-// producer warp), i.e. the whole 64K register file.  The consumers hold up to 128 accumulator registers across a mainloop in which
-// one chunk's wgmmas are always in flight; at the launch-time 168 they spilled inside it.
-constexpr int PROD_REGS = 40, CONS_REGS = 232;
-constexpr int STG_BYTES = 2 * 64 * 16 * 4;    // epilogue staging: per warpgroup 64 rows x 16 fp32 columns (rows of 64 B)
+// warps 0..7: MMA warpgroups, warps 8..11: epilogue warpgroup, warps 12..15: producer warpgroup, of which warps 12..13 issue the
+// TMA loads and warps 14..15 only hand their registers over (setmaxnreg acts on whole warpgroups)
+constexpr int NMMA_WARPS = 8, NEPI_WARPS = CG_EPI_WARPS, NPROD_WARPS = 2;
+constexpr int EPI_WARP0 = NMMA_WARPS, PROD_WARP0 = NMMA_WARPS + NEPI_WARPS;
+static_assert(NEPI_WARPS == 4, "the epilogue is one warpgroup: one row of the 128-row tile per lane");
+constexpr int NTHREADS = 32 * (PROD_WARP0 + 4);
+// registers per thread after setmaxnreg: 2 x MMA + EPI + PROD <= 512 per SM sub-partition lane (each holds two MMA warps, one
+// epilogue warp and one producer warp), i.e. the whole 64K register file.  The MMA warps hold up to 128 accumulator registers
+// across a mainloop in which one chunk's wgmmas are always in flight.
+constexpr int MMA_REGS = 176, EPI_REGS = 136, PROD_REGS = 24;
+static_assert(2 * MMA_REGS + EPI_REGS + PROD_REGS <= 512, "register file");
+constexpr int STG_BYTES = 2 * 64 * 16 * 4;    // in-place epilogue staging: per warpgroup 64 rows x 16 fp32 columns (rows of 64 B)
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -198,14 +204,15 @@ __device__ __forceinline__ void stamp_if(long long* dst, bool pred) {
       : "memory");
 }
 
-// Consumer side of one tile with tile width NT, NPROD products and KS k-steps per K-chunk and TRANS = MN-major operands: mainloop
-// over the tile's K-chunks, then the accumulators to one row per lane.  `s` / `ph`: ring slot and per-slot phase bits, carried by
-// the caller across tiles.  body(g, x) runs the epilogue of column group g of this thread's row (x = its 32 accumulator sums).
+// MMA side of one tile with tile width NT, NPROD products and KS k-steps per K-chunk and TRANS = MN-major operands: mainloop
+// over the tile's K-chunks, then the sums either into the handoff buffer `acc_buf` (handoff: nb = tiles handed off so far) or,
+// in place, to one row per lane.  `s` / `ph`: ring slot and per-slot phase bits, carried by the caller across tiles.  body(g, x)
+// runs the in-place epilogue of column group g of this thread's row (x = its 32 accumulator sums).
 // ctrace: this warp's chunk stamps (nullptr: none), gc: the CTA's chunk counter, the index the producer stamps use.
 template <int NT, int NPROD, int TRANS, int KS, class Body>
 __device__ __forceinline__ void consume_tile(const CgProblem& P, const Tile& ti, uint32_t ring, uint32_t stg, int slot_bytes, int nstages, uint32_t& s,
                                              uint32_t& ph, uint64_t* bar_full, uint64_t* bar_empty, bool nomma, long long* ctrace, uint32_t& gc,
-                                             Body&& body) {
+                                             bool handoff, uint32_t acc_buf, uint32_t& nb, uint64_t* acc_full, uint64_t* acc_empty, Body&& body) {
   constexpr int NGRP = NPROD >= 6 ? 3 : (NPROD >= 3 ? 2 : 1);     // accumulator column groups (product orders)
   constexpr int NACC = NT / 2 * NGRP;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -256,7 +263,26 @@ __device__ __forceinline__ void consume_tile(const CgProblem& P, const Tile& ti,
 #pragma unroll
     for (int j = 0; j < NT / 2; ++j) acc[j] = acc[j] + acc[j + NT / 2];
   }
-  // Fragments -> one row per lane, 16 columns at a time through the warpgroup's staging block (rows of 64 B, 16-byte chunks
+  if (handoff) {
+    // Buffer rows of NT fp32, the 16-byte chunks of row R XOR-swizzled by R & 7: the fragment stores (8 rows x 2 chunks per
+    // instruction) and the epilogue's row reads (8 rows per 128-byte phase) both spread over all banks.  The buffer is free once
+    // the epilogue warpgroup has read the previous handed-off tile.
+    mbar_wait(smem_u32(acc_empty), (nb & 1u) ^ 1u);
+    const uint32_t R = 64u * wg + 16u * wl + (uint32_t)(lane >> 2), sw = (uint32_t)(lane >> 2);      // sw = R & 7 (= (R + 8) & 7)
+    const uint32_t rowa = acc_buf + R * (uint32_t)(NT * 4) + (uint32_t)((lane & 1) * 8);
+#pragma unroll
+    for (int j = 0; j < NT / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t a = rowa + (uint32_t)h * (8u * NT * 4) + ((((uint32_t)(2 * j) + (uint32_t)((lane & 3) >> 1)) ^ sw) << 4);
+        asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(a), "f"(acc[4 * j + 2 * h]), "f"(acc[4 * j + 2 * h + 1]) : "memory");
+      }
+    __syncwarp();
+    mbar_arrive_if(smem_u32(acc_full), lane == 0);
+    ++nb;
+    return;
+  }
+  // In place: fragments -> one row per lane, 16 columns at a time through the warpgroup's staging block (rows of 64 B, 16-byte chunks
   // XOR-swizzled by row pair).  Warp wl & 1 of a warpgroup owns rows 32 (wl & 1) .. + 31 and `half` the parity of its column
   // groups; a pair of column groups (64 columns) is gathered in four steps, then every warp runs the epilogue of its group.
   const int rrow = 32 * (wl & 1) + lane;
@@ -294,19 +320,35 @@ __device__ __forceinline__ void consume_tile(const CgProblem& P, const Tile& ti,
   }
 }
 
-// 12 warps per CTA: 168 registers per thread at launch, then PROD_REGS / CONS_REGS.
+// per-problem constants of one output row r of a tile: the row's offsets inside a tile (the r -> (i0, i1, i2) decomposition needs
+// integer divisions), recomputed only when a role moves to another problem
+struct RowOff {
+  long long roff = 0, rmoff = 0;
+  int ri0 = 0, ri1 = 0;
+  __device__ __forceinline__ void set(const CgProblem& Q, int r) {
+    const int d0 = Q.d0, d1 = Q.d1;
+    const int i0 = r % d0, i12 = r / d0, i1 = i12 % d1, i2 = i12 / d1;
+    roff = Q.o_base + (long long)i0 * Q.o0 + (long long)i1 * Q.o1 + (long long)i2 * Q.o2;
+    rmoff = Q.m_base + (long long)i0 * Q.m0 + (long long)i1 * Q.m1 + (long long)i2 * Q.m2;
+    ri0 = i0; ri1 = i1;
+  }
+};
+
+// 16 warps per CTA: 128 registers per thread at launch, then MMA_REGS / EPI_REGS / PROD_REGS.
 __global__ void __launch_bounds__(NTHREADS, 1)
 cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const CUtensorMap* __restrict__ maps, int max_stages,
           int dbg, long long* __restrict__ trace) {
   const CgProblem* __restrict__ probs = pk.p;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_full[CG_MAX_STAGES], bar_empty[CG_MAX_STAGES];
+  __shared__ __align__(8) uint64_t bar_full[CG_MAX_STAGES], bar_empty[CG_MAX_STAGES], acc_full, acc_empty;
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);          // warp-uniform for the compiler, not just in fact
   const int trace_cta = dbg >> 8;                    // bring-up: the CTA whose roles write clock stamps
   const bool dbg_noload = dbg & 1, dbg_nomma = dbg & 2, dbg_nostore = dbg & 4, dbg_nost = dbg & 16;    // 16: epilogue math without the global stores
   if (tid == 0) {
-    for (int s = 0; s < max_stages; ++s) { mbar_init(smem_u32(&bar_full[s]), 1); mbar_init(smem_u32(&bar_empty[s]), NEPI_WARPS); }
+    for (int s = 0; s < max_stages; ++s) { mbar_init(smem_u32(&bar_full[s]), 1); mbar_init(smem_u32(&bar_empty[s]), NMMA_WARPS); }
+    mbar_init(smem_u32(&acc_full), NMMA_WARPS);
+    mbar_init(smem_u32(&acc_empty), NEPI_WARPS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -323,24 +365,33 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
     {
       // Ring slot s and the phase parity of every slot (bit s of ph): the partition of the ring (slot size, slot count) belongs
       // to the problem, so a slot's barrier may have completed a different number of phases than its neighbours'.
-      uint32_t gc = 0, s = 0, ph = 0;
+      uint32_t gc = 0, s = 0, ph = 0, nbuf = 0;        // nbuf: handed-off tiles so far
       int slot_bytes = 0, nstages = 1;
+      bool handoff = false;
       Walker w;
       int n2 = 1, nloads = 0, planes = 0, tx = 0;
       const int* tab = nullptr;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         if (w.advance(probs, nprob, tile)) {
           const CgProblem& P = probs[w.p];
-          n2 = P.n2; nloads = P.nloads; planes = P.planes; tx = P.tx_bytes; tab = P.tm_tab;
+          n2 = P.n2; nloads = P.nloads; planes = P.planes; tx = P.tx_bytes; tab = P.tm_tab; handoff = cg_epi_handoff(P.epi);
           if (P.slot_bytes != slot_bytes || P.nstages != nstages) {
             // new partition: every slot of the old one must have been consumed before its bytes are overwritten (a fresh
-            // barrier passes the parity-1 wait at once, so never-used slots cost nothing)
+            // barrier passes the parity-1 wait at once, so never-used slots cost nothing), and the new ring may cover the
+            // old handoff buffer: wait until the MMA warps have handed off the last tile (acc_full has completed nbuf phases;
+            // with the ring drained it is at most one behind) and the epilogue warpgroup has read it (acc_empty likewise)
             for (int q = 0; q < nstages; ++q) mbar_wait(smem_u32(&bar_empty[q]), ((ph >> q) & 1u) ^ 1u);
+            if (nbuf) {
+              mbar_wait(smem_u32(&acc_full), (nbuf - 1) & 1u);
+              mbar_wait(smem_u32(&acc_empty), (nbuf - 1) & 1u);
+              asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // its generic reads before our TMA writes
+            }
             slot_bytes = P.slot_bytes; nstages = P.nstages; s = 0;
           }
         }
         const Tile ti = w.tile(tile);
         const CgProblem& P = probs[ti.p];
+        if (handoff && ti.c_end > ti.c_begin) ++nbuf;
         if (P.dep_ctr) {                                                 // fused layers: wait for the tiles this one reads
           const int* __restrict__ ctr = P.dep_ctr;
           const int x0 = P.dep_by_chunk ? ti.c_begin : ti.tm, x1 = P.dep_by_chunk ? ti.c_end : ti.tm + 1;
@@ -408,57 +459,185 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
         }
       }
     }
-  } else {
-    // ============================================================================================ consumers: MMA + epilogue
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONS_REGS));
-    const int ew = warp, half = (ew & 3) >> 1, q = 2 * (ew >> 2) + (ew & 1);
-    uint32_t it = 0, s = 0, ph = 0, gc = 0;
+  } else if (warp < NMMA_WARPS) {
+    // ============================================================================================ MMA warpgroups
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(MMA_REGS));
+    const int q = 2 * (warp >> 2) + (warp & 1);
+    uint32_t it = 0, s = 0, ph = 0, gc = 0, nb = 0;      // nb: tiles handed off to the epilogue warpgroup so far
     int slot_bytes = 0, nstages = 1;
     Walker w;
-    long long* const ctrace = trace && blockIdx.x == trace_cta && ew == 0 ? trace : nullptr;     // chunk stamps: first consumer warp
-    const int r = q * 32 + lane;                         // output row of this thread in the epilogue
-    // per-problem constants of this thread, recomputed only when the CTA moves to another problem: the row's offset
-    // inside a tile (the r -> (i0, i1, i2) decomposition needs integer divisions) and every descriptor field the tile loop reads
-    int epi = 0, rows_tile = 0, lim_rows = 0, umma_n = 0, out_planes = 0, grp_stride = 32, n_valid = 0;
-    long long roff = 0, rmoff = 0, o_tm = 0, m_tm = 0;
-    int ri0 = 0, ri1 = 0, grp_tab = 0;
-    int shape = 0;
+    long long* const ctrace = trace && blockIdx.x == trace_cta && warp == 0 ? trace : nullptr;     // chunk stamps: first MMA warp
+    const int r = q * 32 + lane;                         // output row of this thread in the in-place epilogue
+    int epi = 0, rows_tile = 0, lim_rows = 0, umma_n = 0, n_valid = 0, shape = 0;
+    bool handoff = false;
+    uint32_t acc_buf = 0;
+    long long o_tm = 0;
+    RowOff ro;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      if (w.advance(probs, nprob, tile)) {
+        const CgProblem& Q = probs[w.p];
+        epi = Q.epi; rows_tile = Q.rows_tile; lim_rows = Q.lim_rows; umma_n = Q.umma_n; n_valid = Q.n_valid; o_tm = Q.o_tm;
+        ro.set(Q, r);
+        shape = cg_shape_key(Q.umma_n, Q.nprod, Q.mn_major != 0, Q.ksteps);
+        if (Q.slot_bytes != slot_bytes || Q.nstages != nstages) { slot_bytes = Q.slot_bytes; nstages = Q.nstages; s = 0; }
+        handoff = cg_epi_handoff(epi);
+        acc_buf = ring + (uint32_t)(nstages * slot_bytes);
+      }
+      const Tile ti = w.tile(tile);
+      if (ti.c_end <= ti.c_begin) continue;
+      const CgProblem& P = probs[ti.p];
+      const bool valid0 = r < rows_tile && ti.tm * rows_tile + r < lim_rows;
+      const long long off0 = ro.roff + (long long)ti.tm * o_tm;
+      const int n0 = ti.tn * umma_n;
+      const bool tre = trace && blockIdx.x == trace_cta && warp == 0 && lane == 0 && it < 16;
+      if (tre) trace[512 + it * 4 + 0] = clock64();
+      // in-place epilogue (RAW / WGRAD) of column group g of this thread's row.  Every lane owns one output row and writes its
+      // 32 columns itself (128 B of fp32): 16-byte vector stores or red.adds.
+      auto body = [&](int g, float (&x)[32]) {
+        const int ng = n0 + 32 * g;                      // first problem column of the group
+        if (dbg_nostore || ng >= n_valid || !valid0) return;
+        float* dst = P.out_f + off0 + (long long)(ng >> 5) * P.f_grp;
+        if (epi == CG_EPI_RAW) {
+          if (P.atomic) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+              asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(dst + 4 * j), "f"(x[4 * j]), "f"(x[4 * j + 1]), "f"(x[4 * j + 2]),
+                           "f"(x[4 * j + 3])
+                           : "memory");
+          } else {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) *reinterpret_cast<float4*>(dst + 4 * j) = make_float4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
+          }
+          return;
+        }
+        // CG_EPI_WGRAD
+        const float sc = P.scale;
+        if (P.atomic) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(dst + 4 * j), "f"(x[4 * j] * sc), "f"(x[4 * j + 1] * sc),
+                         "f"(x[4 * j + 2] * sc), "f"(x[4 * j + 3] * sc)
+                         : "memory");
+        } else {
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<float4*>(dst + 4 * j) = make_float4(x[4 * j] * sc, x[4 * j + 1] * sc, x[4 * j + 2] * sc, x[4 * j + 3] * sc);
+          if (P.dp_n > 1) {                          // final values: push them to their owner now (posted NVLink stores)
+            const int i4 = (int)((dst - P.dp_gbase) >> 2), per4 = P.dp_per4;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int owner = (i4 + j) / per4;
+              if (owner != P.dp_rank)
+                reinterpret_cast<float4*>(P.dp_recv[owner])[(size_t)P.dp_rank * per4 + (i4 + j - owner * per4)] =
+                    make_float4(x[4 * j] * sc, x[4 * j + 1] * sc, x[4 * j + 2] * sc, x[4 * j + 3] * sc);
+            }
+          }
+        }
+      };
+#define CG_CONSUME(NT, NPROD, TRANS, KS)                                                                                                      \
+  consume_tile<NT, NPROD, TRANS, KS>(P, ti, ring, stg, slot_bytes, nstages, s, ph, bar_full, bar_empty, dbg_nomma, ctrace, gc, handoff, acc_buf, \
+                                     nb, &acc_full, &acc_empty, body)
+      // the (width, products, major-ness, k-steps) combinations cg_shape_supported() admits on the host; anything else is a bug: trap
+      switch (shape) {
+        case cg_shape_key(32, 6, false, 4): CG_CONSUME(32, 6, 0, 4); break;
+        case cg_shape_key(64, 6, false, 4): CG_CONSUME(64, 6, 0, 4); break;
+        case cg_shape_key(64, 3, false, 4): CG_CONSUME(64, 3, 0, 4); break;
+        case cg_shape_key(128, 3, false, 4): CG_CONSUME(128, 3, 0, 4); break;
+        case cg_shape_key(64, 3, true, 4): CG_CONSUME(64, 3, 1, 4); break;
+        case cg_shape_key(64, 3, true, 9): CG_CONSUME(64, 3, 1, 9); break;
+        case cg_shape_key(128, 3, true, 4): CG_CONSUME(128, 3, 1, 4); break;
+        default: __trap();
+      }
+#undef CG_CONSUME
+      if (tre) {
+        trace[512 + it * 4 + 1] = clock64();
+        trace[512 + it * 4 + 2] = handoff;
+        trace[512 + it * 4 + 3] = ti.p * 100000 + ti.tm * 10 + ti.tn;
+      }
+      ++it;
+    }
+  } else {
+    // ============================================================================================ epilogue warpgroup
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(EPI_REGS));
+    const int ew = warp - EPI_WARP0;
+    const int r = ew * 32 + lane;                        // output row of this thread
+    uint32_t ne = 0;                                     // handed-off tiles finished so far
+    int slot_bytes = 0, nstages = 1;
+    Walker w;
+    // per-problem constants of this thread, recomputed only when the CTA moves to another problem
+    int epi = 0, rows_tile = 0, lim_rows = 0, umma_n = 0, out_planes = 0, grp_stride = 32, n_valid = 0, grp_tab = 0;
+    bool handoff = false;
+    uint32_t acc_buf = 0;
+    long long o_tm = 0, m_tm = 0;
+    RowOff ro;
     const float* __restrict__ bias = nullptr;
     const uint16_t* __restrict__ mask = nullptr;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       if (w.advance(probs, nprob, tile)) {
         const CgProblem& Q = probs[w.p];
         epi = Q.epi; rows_tile = Q.rows_tile; lim_rows = Q.lim_rows; umma_n = Q.umma_n; out_planes = Q.out_planes;
-        grp_stride = Q.grp_stride; n_valid = Q.n_valid; o_tm = Q.o_tm; m_tm = Q.m_tm; bias = Q.bias; mask = Q.mask;
-        const int d0 = Q.d0, d1 = Q.d1;
-        const int i0 = r % d0, i12 = r / d0, i1 = i12 % d1, i2 = i12 / d1;
-        roff = Q.o_base + (long long)i0 * Q.o0 + (long long)i1 * Q.o1 + (long long)i2 * Q.o2;
-        rmoff = Q.m_base + (long long)i0 * Q.m0 + (long long)i1 * Q.m1 + (long long)i2 * Q.m2;
-        ri0 = i0; ri1 = i1; grp_tab = Q.grp_tab;
-        shape = cg_shape_key(Q.umma_n, Q.nprod, Q.mn_major != 0, Q.ksteps);
-        if (Q.slot_bytes != slot_bytes || Q.nstages != nstages) { slot_bytes = Q.slot_bytes; nstages = Q.nstages; s = 0; }
+        grp_stride = Q.grp_stride; n_valid = Q.n_valid; o_tm = Q.o_tm; m_tm = Q.m_tm; bias = Q.bias; mask = Q.mask; grp_tab = Q.grp_tab;
+        ro.set(Q, r);
+        if (Q.slot_bytes != slot_bytes || Q.nstages != nstages) { slot_bytes = Q.slot_bytes; nstages = Q.nstages; }
+        handoff = cg_epi_handoff(epi);
+        acc_buf = ring + (uint32_t)(nstages * slot_bytes);
       }
       const Tile ti = w.tile(tile);
-      if (ti.c_end <= ti.c_begin) continue;
+      if (ti.c_end <= ti.c_begin || !handoff) continue;
       const CgProblem& P = probs[ti.p];
       const bool valid0 = r < rows_tile && ti.tm * rows_tile + r < lim_rows;
-      const long long off0 = roff + (long long)ti.tm * o_tm, moff0 = rmoff + (long long)ti.tm * m_tm;
+      const long long off0 = ro.roff + (long long)ti.tm * o_tm, moff0 = ro.rmoff + (long long)ti.tm * m_tm;
       const int n0 = ti.tn * umma_n, ngroups = umma_n >> 5;
-      const bool tre = trace && blockIdx.x == trace_cta && ew == 0 && lane == 0 && it < 16;
-      if (tre) trace[512 + it * 4 + 0] = clock64();
+      // the row limits and output / mask offsets of column group g (per group from the tables for grp_tab problems)
+      auto group_at = [&](int g, bool& valid, long long& off, long long& moff) {
+        const int ng = n0 + 32 * g;
+        valid = valid0; off = off0; moff = moff0;
+        if (grp_tab) {
+          const int gg = ng >> 5;
+          valid = valid0 && ro.ri0 < P.grp_lim0[gg] && ro.ri1 < P.grp_lim1[gg];
+          off = off0 + P.grp_off[gg]; moff = moff0 + P.grp_moff[gg] - ng;     // (the mask load adds ng)
+        }
+      };
+      const bool tre = trace && blockIdx.x == trace_cta && ew == 0 && lane == 0 && ne < 16;
+      if (tre) trace[576 + ne * 4 + 0] = clock64();
+      // DGRAD: the ReLU mask does not depend on the sums, so its loads are issued before the handoff wait, while the MMA
+      // warps are still in the mainloop; bit c of mbits[g] = column 32g + c of this row is kept (an invalid row keeps none).
+      // Four groups: the instantiated tile widths are at most 128.
+      uint32_t mbits[4] = {0u, 0u, 0u, 0u};
+      if (epi == CG_EPI_DGRAD && !dbg_nostore) {
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+          bool valid;
+          long long off, moff;
+          group_at(g, valid, off, moff);
+          const int ng = n0 + 32 * g;
+          if (g < ngroups && valid && ng < n_valid) {
+            uint4 mk[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) mk[j] = __ldg(reinterpret_cast<const uint4*>(mask + moff + ng) + j);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const uint32_t wd[4] = {mk[j].x, mk[j].y, mk[j].z, mk[j].w};
+#pragma unroll
+              for (int uu = 0; uu < 4; ++uu) {
+                if (wd[uu] & 0x00007FFFu) mbits[g] |= 1u << (8 * j + 2 * uu);
+                if (wd[uu] & 0x7FFF0000u) mbits[g] |= 1u << (8 * j + 2 * uu + 1);
+              }
+            }
+          }
+        }
+      }
+      mbar_wait(smem_u32(&acc_full), ne & 1u);
+      if (tre) trace[576 + ne * 4 + 1] = clock64();
       const bool split_fin = P.ws != nullptr;          // split-K tile of an ACT problem: partial sums first, the last arriver finishes
       float* __restrict__ wsrow = split_fin ? P.ws + ((size_t)(ti.tm * w.tiles_n + ti.tn) * 128 + r) * umma_n : nullptr;
       // epilogue of column group g of this thread's row; pass 0: x = this tile's accumulator sums, pass 1: x = the finished
       // split-K sums read back by the last arriver
       auto body = [&](int g, float (&x)[32], int pass) {
         const int ng = n0 + 32 * g;                      // first problem column of the group
-        bool valid = valid0;
-        long long off = off0, moff = moff0;
-        if (grp_tab) {
-          const int gg = ng >> 5;
-          valid = valid0 && ri0 < P.grp_lim0[gg] && ri1 < P.grp_lim1[gg];
-          off = off0 + P.grp_off[gg]; moff = moff0 + P.grp_moff[gg] - ng;     // (the mask load below adds ng)
-        }
+        bool valid;
+        long long off, moff;
+        group_at(g, valid, off, moff);
         if (pass == 0 && split_fin) {                    // partial sums of this split -> workspace
 #pragma unroll
           for (int j = 0; j < 8; ++j)
@@ -469,61 +648,11 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
         }
         const bool live = !dbg_nostore && ng < n_valid;
         float4 bv[8];
-        uint4 mk[4];
         if (epi == CG_EPI_ACT && live) {
 #pragma unroll
           for (int j = 0; j < 8; ++j) bv[j] = __ldg(reinterpret_cast<const float4*>(bias + (long long)(ng >> 5) * P.bias_grp) + j);
         }
-        if (epi == CG_EPI_DGRAD && live) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) mk[j] = valid ? __ldg(reinterpret_cast<const uint4*>(mask + moff + ng) + j) : make_uint4(0, 0, 0, 0);
-        }
         if (!live) return;
-        // Every lane owns one output row and writes its 32 columns itself (64 B per BF16 plane, 128 B of fp32): 16-byte vector stores.
-        if (epi == CG_EPI_RAW) {
-          if (valid) {
-            float* dst = P.out_f + off + (long long)(ng >> 5) * P.f_grp;
-            if (P.atomic) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(dst + 4 * j), "f"(x[4 * j]), "f"(x[4 * j + 1]), "f"(x[4 * j + 2]),
-                             "f"(x[4 * j + 3])
-                             : "memory");
-            } else {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) *reinterpret_cast<float4*>(dst + 4 * j) = make_float4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
-            }
-          }
-          return;
-        }
-        if (epi == CG_EPI_WGRAD) {
-          if (valid) {
-            const float sc = P.scale;
-            float* dst = P.out_f + off + (long long)(ng >> 5) * P.f_grp;
-            if (P.atomic) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(dst + 4 * j), "f"(x[4 * j] * sc), "f"(x[4 * j + 1] * sc),
-                             "f"(x[4 * j + 2] * sc), "f"(x[4 * j + 3] * sc)
-                             : "memory");
-            } else {
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                *reinterpret_cast<float4*>(dst + 4 * j) = make_float4(x[4 * j] * sc, x[4 * j + 1] * sc, x[4 * j + 2] * sc, x[4 * j + 3] * sc);
-              if (P.dp_n > 1) {                          // final values: push them to their owner now (posted NVLink stores)
-                const int i4 = (int)((dst - P.dp_gbase) >> 2), per4 = P.dp_per4;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const int owner = (i4 + j) / per4;
-                  if (owner != P.dp_rank)
-                    reinterpret_cast<float4*>(P.dp_recv[owner])[(size_t)P.dp_rank * per4 + (i4 + j - owner * per4)] =
-                        make_float4(x[4 * j] * sc, x[4 * j + 1] * sc, x[4 * j + 2] * sc, x[4 * j + 3] * sc);
-                }
-              }
-            }
-          }
-          return;
-        }
         if (epi == CG_EPI_ACT) {
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
@@ -536,15 +665,10 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
             for (int j = 0; j < 8; ++j) *reinterpret_cast<float4*>(dst + 4 * j) = make_float4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
           }
         } else {   // CG_EPI_DGRAD: ReLU mask = hi plane of the forward activation at the same position
+          const uint32_t mb = g == 0 ? mbits[0] : g == 1 ? mbits[1] : g == 2 ? mbits[2] : mbits[3];
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint32_t w[4] = {mk[j].x, mk[j].y, mk[j].z, mk[j].w};
-#pragma unroll
-            for (int uu = 0; uu < 4; ++uu) {
-              if (!(w[uu] & 0x00007FFFu)) x[8 * j + 2 * uu] = 0.f;
-              if (!(w[uu] & 0x7FFF0000u)) x[8 * j + 2 * uu + 1] = 0.f;
-            }
-          }
+          for (int j = 0; j < 32; ++j)
+            if (!((mb >> j) & 1u)) x[j] = 0.f;
           if (P.colsum) {
             // bias gradient: column sums over this warp's 32 rows (invalid rows are zero: their mask words were not loaded) by a
             // transposing butterfly -- 31 shuffles leave lane c with the sum of column c -- then one 128-byte red.add per warp
@@ -581,22 +705,23 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
           }
         }
       };
-      auto body0 = [&](int g, float (&x)[32]) { body(g, x, 0); };
-#define CG_CONSUME(NT, NPROD, TRANS, KS) \
-  consume_tile<NT, NPROD, TRANS, KS>(P, ti, ring, stg, slot_bytes, nstages, s, ph, bar_full, bar_empty, dbg_nomma, ctrace, gc, body0)
-      // the (width, products, major-ness, k-steps) combinations cg_shape_supported() admits on the host; anything else is a bug: trap
-      switch (shape) {
-        case cg_shape_key(32, 6, false, 4): CG_CONSUME(32, 6, 0, 4); break;
-        case cg_shape_key(64, 6, false, 4): CG_CONSUME(64, 6, 0, 4); break;
-        case cg_shape_key(64, 3, false, 4): CG_CONSUME(64, 3, 0, 4); break;
-        case cg_shape_key(128, 3, false, 4): CG_CONSUME(128, 3, 0, 4); break;
-        case cg_shape_key(64, 3, true, 4): CG_CONSUME(64, 3, 1, 4); break;
-        case cg_shape_key(64, 3, true, 9): CG_CONSUME(64, 3, 1, 9); break;
-        case cg_shape_key(128, 3, true, 4): CG_CONSUME(128, 3, 1, 4); break;
-        default: __trap();
+      // this thread's row of the handoff buffer (16-byte chunk c of row r at c ^ (r & 7), see consume_tile), one 32-column group
+      // at a time; the buffer is released as soon as the last group is in registers
+      const uint32_t rowa = acc_buf + (uint32_t)(r * umma_n * 4), sw = (uint32_t)(r & 7);
+      for (int g = 0; g < ngroups; ++g) {
+        float x[32];
+#pragma unroll
+        for (int cc = 0; cc < 8; ++cc) {
+          const uint32_t a = rowa + ((((uint32_t)(8 * g + cc)) ^ sw) << 4);
+          asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(x[4 * cc]), "=f"(x[4 * cc + 1]), "=f"(x[4 * cc + 2]), "=f"(x[4 * cc + 3]) : "r"(a));
+        }
+        if (g == ngroups - 1) {
+          __syncwarp();
+          mbar_arrive_if(smem_u32(&acc_empty), lane == 0);
+        }
+        body(g, x, 0);
       }
-#undef CG_CONSUME
-      if (tre) trace[512 + it * 4 + 1] = clock64();
+      ++ne;
       bool last_arriver = !split_fin;
       if (split_fin) {
         __syncwarp();
@@ -607,7 +732,7 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
         if (last_arriver) {                              // the complete sums, and a clean workspace for the next step
           __threadfence();
           if (lane == 0) P.ws_cnt[(ti.tm * w.tiles_n + ti.tn) * NEPI_WARPS + ew] = 0;     // next step starts from zero
-          for (int g = half; g < ngroups; g += 2) {
+          for (int g = 0; g < ngroups; ++g) {
             float x[32];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
@@ -624,8 +749,7 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
         __threadfence();
         atomicAdd(P.done_ctr + ti.tm, 1);
       }
-      if (tre) { trace[512 + it * 4 + 2] = clock64(); trace[512 + it * 4 + 3] = ti.p * 100000 + ti.tm * 10 + ti.tn; }
-      ++it;
+      if (tre) { trace[576 + (ne - 1) * 4 + 2] = clock64(); trace[576 + (ne - 1) * 4 + 3] = ti.p * 100000 + ti.tm * 10 + ti.tn; }
     }
   }
 }
@@ -636,7 +760,7 @@ EncodeTiledFn g_encode = nullptr;
 
 }  // namespace
 
-// ring budget (cg_finalize): the dynamic part minus the epilogue staging; the kernel's static shared memory (barriers) takes < 1 KiB
+// ring budget (cg_finalize): the dynamic part minus the in-place epilogue staging; the kernel's static shared memory (barriers) takes < 1 KiB
 // of the 227 KiB
 bool cg_shape_supported(int umma_n, int nprod, bool mn_major, int ksteps) {
   switch (cg_shape_key(umma_n, nprod, mn_major, ksteps)) {
@@ -687,12 +811,14 @@ int cg_finalize(CgGroup& g, int smem_budget) {
   int ring = 0;
   for (int i = 0; i < g.n; ++i) {
     CgProblem& P = g.host[i];
-    P.nstages = P.slot_bytes > 0 ? avail / P.slot_bytes : 0;
+    const int acc = cg_epi_handoff(P.epi) ? cg_acc_bytes(P.umma_n) : 0;     // the handoff buffer follows the problem's ring
+    const int avail_ring = avail - acc;
+    P.nstages = P.slot_bytes > 0 ? avail_ring / P.slot_bytes : 0;
     if (P.nstages > CG_MAX_STAGES) P.nstages = CG_MAX_STAGES;
     if (P.nstages < 2) return -1;
-    P.slot_bytes = avail / P.nstages / 1024 * 1024;        // one slot size per stage count: problems with equal depth share the partition
+    P.slot_bytes = avail_ring / P.nstages / 1024 * 1024;   // one slot size per stage count: problems with equal depth share the partition
     g.nstages = g.nstages > P.nstages ? g.nstages : P.nstages;
-    ring = ring > P.nstages * P.slot_bytes ? ring : P.nstages * P.slot_bytes;
+    ring = ring > P.nstages * P.slot_bytes + acc ? ring : P.nstages * P.slot_bytes + acc;
   }
   g.ring_bytes = ring;
   return 0;

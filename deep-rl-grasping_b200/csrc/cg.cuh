@@ -17,7 +17,8 @@ constexpr int CG_MAX_LOADS = 4;     // TMA boxes per K-chunk and plane (A atoms 
 constexpr int CG_MAX_PROBLEMS = 16; // problems per grouped launch (the whole list travels as a __grid_constant__ kernel parameter)
 constexpr int CG_MAX_STAGES = 8;
 constexpr int CG_MAX_PLANES = 3;
-constexpr int CG_EPI_WARPS = 8;    // epilogue warps of a CTA; each signals a finished tile once (dependency counters)
+constexpr int CG_EPI_WARPS = 4;    // the epilogue warpgroup's warps (one output row per lane); each signals a finished tile once
+                                   // (dependency counters, split-K arrival counters)
 
 enum CgEpiKind : int {
   CG_EPI_ACT = 0,     // relu(acc + bias[n]) -> BF16 planes (activations; optional fp32 copy)
@@ -25,6 +26,12 @@ enum CgEpiKind : int {
   CG_EPI_DGRAD = 2,   // acc * (mask[row, n] > 0) -> BF16 planes (gradient maps)
   CG_EPI_WGRAD = 3,   // acc -> fp32 weight gradient, plain store or atomic accumulation (split-K)
 };
+// ACT / DGRAD tiles hand their fp32 sums to the epilogue warpgroup through a 128 x umma_n fp32 buffer in shared memory (carved
+// out of the problem's ring budget) and the MMA warps go on to the next tile; RAW / WGRAD tiles (plain stores or red.adds, and
+// the conv2 wgrad's 108 KB stages leave no room for a buffer) are finished in place by the MMA warps.  Only the epilogue
+// warpgroup signals dependency counters, so only ACT / DGRAD problems may be wired as producers.
+__host__ __device__ constexpr bool cg_epi_handoff(int epi) { return epi == CG_EPI_ACT || epi == CG_EPI_DGRAD; }
+__host__ __device__ constexpr int cg_acc_bytes(int umma_n) { return 128 * umma_n * 4; }
 
 struct CgLoad {
   int map;            // index of the tensor map (all planes of the tensor: plane = outermost dimension)
@@ -47,7 +54,8 @@ struct CgProblem {
   int a_pstride, b_pstride;   // stage layout: [A plane 0 | A plane 1 | ..][B plane 0 | B plane 1 | ..]; bytes of one A / B plane
   int tx_bytes;               // bytes all boxes of one stage deliver (planes x sum of box bytes)
   int slot_bytes, nstages;    // stage ring geometry of THIS problem (cg_finalize): the problems of a launch share the ring's bytes, not
-                              // its partition -- the ring is drained when the partition changes
+                              // its partition -- the ring is drained when the partition changes.  The handoff buffer of an ACT / DGRAD
+                              // problem follows its ring (byte nstages * slot_bytes)
   CgLoad ld[CG_MAX_LOADS];
   const int* tm_tab;          // optional [tiles_m][CG_MAX_LOADS][2]: extra offsets of coordinates 1 and 2 per (tm, load)
   // ---- MMA
@@ -87,7 +95,7 @@ struct CgProblem {
   // ---- dependencies between the problems of ONE launch (fused layers).  Tiles are dealt to the CTAs in increasing order and
   //      every CTA of the grid is resident, so a tile may wait for lower-numbered tiles of an earlier problem: the producers of
   //      tile tm spin until the row-tiles [tm * dep_rows / dep_rows_tile, ((tm + 1) * dep_rows - 1) / dep_rows_tile] of the
-  //      producing problem have each collected dep_expect arrivals (one per epilogue warp and (tn, split) tile), then order the
+  //      producing problem have each collected dep_expect arrivals (x CG_EPI_WARPS: one per epilogue warp and (tn, split) tile), then order the
   //      generic-proxy stores they observed before their own async-proxy (TMA) reads.
   int* done_ctr;              // arrival counters of THIS problem, one per tm (nullptr: nobody waits on it); zeroed before the launch
   const int* dep_ctr;         // counters of the producing problem (nullptr: no dependency)
@@ -111,7 +119,7 @@ struct CgGroup {               // one launch
   CgProblem host[CG_MAX_PROBLEMS];
   int n = 0;
   int total_tiles = 0;
-  int slot_bytes = 0, nstages = 0, ring_bytes = 0;     // largest slot / most stages of any problem; bytes of the ring
+  int slot_bytes = 0, nstages = 0, ring_bytes = 0;     // largest slot / most stages of any problem; bytes of the ring (with the handoff buffer)
   const char* name = "";
   double flops = 0;
 };

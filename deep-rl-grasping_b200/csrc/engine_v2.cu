@@ -319,6 +319,8 @@ int fuse_groups(b2g_sac* h, const std::vector<const CgGroup*>& parts, const std:
     const int pi = first[w.prod] + w.pi, qi = first[w.cons] + w.ci;
     CgProblem& Pp = f.host[pi];
     CgProblem& Pc = f.host[qi];
+    if (!cg_epi_handoff(Pp.epi))       // only the epilogue warpgroup signals finished tiles (cg.cuh: cg_epi_handoff)
+      return b2g_fail(B2G_EINVAL, std::string("engine v2: a wired producer must have an ACT or DGRAD epilogue (fused launch ") + name + ")");
     if (Pc.dep_ctr && ctr_of[pi] < 0) {
       // a second producer of the same consumer (the two nets' conv2 dgrads both write dZ1): it signals the first one's counters
       ctr_of[pi] = (int)(intptr_t)Pc.dep_ctr - 1;
@@ -887,10 +889,12 @@ int v2_launch(b2g_sac* h, const CgGroup& g, cudaStream_t s) {
       for (int i = 0; i < 64 && t[i * 8 + 2]; ++i)
         fprintf(stderr, "  chunk %2d (p %lld tm %lld): %7lld %7lld %7lld | %7lld %7lld %7lld\n", i, t[i * 8 + 6] / 100000, t[i * 8 + 6] % 100000 / 10, t[i * 8] - t0,
                 t[i * 8 + 1] - t0, t[i * 8 + 2] - t0, t[i * 8 + 3] - t0, t[i * 8 + 4] - t0, t[i * 8 + 5] - t0);
-      for (int i = 0; i < 16 && t[512 + i * 4 + 2]; ++i)
-        fprintf(stderr, "  tile %d (p %lld tm %lld) epilogue: wait_start %7lld acc_full %7lld done %7lld | first group: ld issued %7lld ld done %7lld math done %7lld\n", i,
-                t[512 + i * 4 + 3] / 100000, t[512 + i * 4 + 3] % 100000 / 10, t[512 + i * 4] - t0, t[512 + i * 4 + 1] - t0, t[512 + i * 4 + 2] - t0,
-                t[576 + i * 4] - t0, t[576 + i * 4 + 1] - t0, t[576 + i * 4 + 2] - t0);
+      for (int i = 0; i < 16 && t[512 + i * 4 + 1]; ++i)
+        fprintf(stderr, "  tile %d (p %lld tm %lld) mma: start %7lld sums out %7lld (%s)\n", i, t[512 + i * 4 + 3] / 100000, t[512 + i * 4 + 3] % 100000 / 10,
+                t[512 + i * 4] - t0, t[512 + i * 4 + 1] - t0, t[512 + i * 4 + 2] ? "handed off" : "in place");
+      for (int i = 0; i < 16 && t[576 + i * 4 + 2]; ++i)
+        fprintf(stderr, "  handoff %d (p %lld tm %lld) epilogue warpgroup: buffer wait %7lld start %7lld end %7lld\n", i, t[576 + i * 4 + 3] / 100000,
+                t[576 + i * 4 + 3] % 100000 / 10, t[576 + i * 4] - t0, t[576 + i * 4 + 1] - t0, t[576 + i * 4 + 2] - t0);
     }
     return 0;
   }
