@@ -75,11 +75,8 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-// shared-memory matrix descriptors (SWIZZLE_128B, wgmma.cuh).  K-major: rows of 128 B, 8-row groups 1024 B apart (SBO), LBO
-// unused.  MN-major: rows = K, 128 B = 64 elements along M|N; SBO = stride between 8-row K groups (1024 B inside a TMA box),
-// LBO = stride between 64-element atoms along M|N (one box each).
-__device__ __forceinline__ uint64_t desc_k(uint32_t saddr) { return wg_desc(saddr, 16, 1024); }
-__device__ __forceinline__ uint64_t desc_mn(uint32_t saddr, uint32_t lbo) { return wg_desc(saddr, lbo, 1024); }
+// shared-memory matrix descriptor: the problem's constant bits (cg_desc_bits: swizzle span, LBO, SBO) | the start address
+__device__ __forceinline__ uint64_t desc_at(uint64_t bits, uint32_t saddr) { return bits | (uint64_t)((saddr & 0x3FFFFu) >> 4); }
 
 __device__ __forceinline__ void tma_load(uint32_t dst, const CUtensorMap* map, uint32_t bar, int rank, const int (&c)[5]) {
   switch (rank) {
@@ -155,7 +152,7 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {    // lo -
 // sequences, or a run-time trip count, puts the instructions on paths where the compiler serialises them.
 template <int NT, int NPROD, int TRANS, int KS, int NACC>
 __device__ __forceinline__ void mma_chunk(float (&acc)[NACC], uint32_t sbase, uint32_t a_off, uint32_t b_off, uint32_t a_ks, uint32_t b_ks,
-                                          uint32_t a_lbo, uint32_t b_lbo, uint32_t a_ps, uint32_t b_ps, uint32_t m_off) {
+                                          uint32_t a_ks2, uint64_t a_desc, uint64_t b_desc, uint32_t a_ps, uint32_t b_ps, uint32_t m_off) {
   constexpr int NPL = NPROD >= 6 ? 3 : (NPROD >= 3 ? 2 : 1), G = NT / 2;      // planes = order groups; registers per group
   static_assert(NACC == G * NPL, "one accumulator group of NT columns per product order");
 #pragma unroll
@@ -163,10 +160,10 @@ __device__ __forceinline__ void mma_chunk(float (&acc)[NACC], uint32_t sbase, ui
     uint64_t da[NPL], db[NPL];
 #pragma unroll
     for (int pl = 0; pl < NPL; ++pl) {
-      const uint32_t pa = sbase + (uint32_t)pl * a_ps + a_off + (uint32_t)k * a_ks + m_off;
+      const uint32_t pa = sbase + (uint32_t)pl * a_ps + a_off + (uint32_t)(k & 1) * a_ks + (uint32_t)(k >> 1) * a_ks2 + m_off;
       const uint32_t pb = sbase + (uint32_t)pl * b_ps + b_off + (uint32_t)k * b_ks;
-      da[pl] = TRANS ? desc_mn(pa, a_lbo) : desc_k(pa);
-      db[pl] = TRANS ? desc_mn(pb, b_lbo) : desc_k(pb);
+      da[pl] = desc_at(a_desc, pa);
+      db[pl] = desc_at(b_desc, pb);
     }
     // per group, the products in the order of a wide A_p x [B_0 | ..] issue: g1 = A0 B1, A1 B0; g2 = A0 B2, A1 B1, A2 B0
     Wgmma<NT, TRANS>::mma(acc, da[0], db[0]);
@@ -221,8 +218,9 @@ __device__ __forceinline__ void consume_tile(const CgProblem& P, const Tile& ti,
 #pragma unroll
   for (int j = 0; j < NACC; ++j) acc[j] = 0.f;
   const uint32_t a_ps = (uint32_t)P.a_pstride, b_ps = (uint32_t)P.b_pstride, a_off = P.a_off, b_off = P.b_off, a_ks = P.a_kstep, b_ks = P.b_kstep;
-  const uint32_t a_lbo = P.a_lbo, b_lbo = P.b_lbo;
-  const uint32_t m_off = TRANS ? (uint32_t)wg * a_lbo : (uint32_t)wg * 8192u;     // rows [64 wg, 64 wg + 64) of the A tile
+  const uint32_t a_ks2 = P.a_kstep2;
+  const uint64_t a_desc = P.a_desc, b_desc = P.b_desc;
+  const uint32_t m_off = (uint32_t)wg * (uint32_t)P.a_moff;     // rows [64 wg, 64 wg + 64) of the A tile
   // One chunk's MMAs stay in flight while the next chunk is awaited and issued; the slot of chunk c - 1 is released once
   // wait_group 1 in chunk c has seen them finish.  Every lane runs the same instructions from the fence to the release: the
   // release and the stamps are predicated, not branched on (see mbar_arrive_if).
@@ -243,7 +241,7 @@ __device__ __forceinline__ void consume_tile(const CgProblem& P, const Tile& ti,
       mbar_wait(smem_u32(&bar_full[s]), (ph >> s) & 1u);
       stamp_if(tr + 4, stamp);
       wg_arrive();
-      mma_chunk<NT, NPROD, TRANS, KS>(acc, ring + s * (uint32_t)slot_bytes, a_off, b_off, a_ks, b_ks, a_lbo, b_lbo, a_ps, b_ps, m_off);
+      mma_chunk<NT, NPROD, TRANS, KS>(acc, ring + s * (uint32_t)slot_bytes, a_off, b_off, a_ks, b_ks, a_ks2, a_desc, b_desc, a_ps, b_ps, m_off);
       wg_commit();
       wg_wait<1>();
       mbar_arrive_if(smem_u32(&bar_empty[prev]), lane == 0 && c > ti.c_begin);      // chunk c - 1's slot may be refilled
@@ -325,12 +323,15 @@ __device__ __forceinline__ void consume_tile(const CgProblem& P, const Tile& ti,
 struct RowOff {
   long long roff = 0, rmoff = 0;
   int ri0 = 0, ri1 = 0;
+  bool ok = true;                                    // not cut by lim_i0
   __device__ __forceinline__ void set(const CgProblem& Q, int r) {
     const int d0 = Q.d0, d1 = Q.d1;
     const int i0 = r % d0, i12 = r / d0, i1 = i12 % d1, i2 = i12 / d1;
     roff = Q.o_base + (long long)i0 * Q.o0 + (long long)i1 * Q.o1 + (long long)i2 * Q.o2;
+    if (Q.rgrp_rows > 0) roff += Q.rgrp_off[min(r / Q.rgrp_rows, 7)];
     rmoff = Q.m_base + (long long)i0 * Q.m0 + (long long)i1 * Q.m1 + (long long)i2 * Q.m2;
     ri0 = i0; ri1 = i1;
+    ok = Q.lim_i0 <= 0 || i0 < Q.lim_i0;
   }
 };
 
@@ -486,7 +487,7 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
       const Tile ti = w.tile(tile);
       if (ti.c_end <= ti.c_begin) continue;
       const CgProblem& P = probs[ti.p];
-      const bool valid0 = r < rows_tile && ti.tm * rows_tile + r < lim_rows;
+      const bool valid0 = r < rows_tile && ti.tm * rows_tile + r < lim_rows && ro.ok;
       const long long off0 = ro.roff + (long long)ti.tm * o_tm;
       const int n0 = ti.tn * umma_n;
       const bool tre = trace && blockIdx.x == trace_cta && warp == 0 && lane == 0 && it < 16;
@@ -585,8 +586,14 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
       const Tile ti = w.tile(tile);
       if (ti.c_end <= ti.c_begin || !handoff) continue;
       const CgProblem& P = probs[ti.p];
-      const bool valid0 = r < rows_tile && ti.tm * rows_tile + r < lim_rows;
-      const long long off0 = ro.roff + (long long)ti.tm * o_tm, moff0 = ro.rmoff + (long long)ti.tm * m_tm;
+      bool valid0 = r < rows_tile && ti.tm * rows_tile + r < lim_rows && ro.ok;
+      long long off0 = ro.roff + (long long)ti.tm * o_tm;
+      const long long moff0 = ro.rmoff + (long long)ti.tm * m_tm;
+      if (P.tm_sub > 1) {                              // band tr of block tq (cg.cuh: tm_sub)
+        const int tq = ti.tm / P.tm_sub, tr = ti.tm - tq * P.tm_sub;
+        off0 = ro.roff + (long long)tq * o_tm + (long long)tr * P.o_sub;
+        valid0 = valid0 && tr * P.d1 + ro.ri1 < P.lim_i1;
+      }
       const int n0 = ti.tn * umma_n, ngroups = umma_n >> 5;
       // the row limits and output / mask offsets of column group g (per group from the tables for grp_tab problems)
       auto group_at = [&](int g, bool& valid, long long& off, long long& moff) {
@@ -773,7 +780,8 @@ bool cg_shape_supported(int umma_n, int nprod, bool mn_major, int ksteps) {
 int cg_smem_limit() { return 226 * 1024 - STG_BYTES; }
 
 int cg_encode_map(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box,
-                  const uint32_t* elem_strides) {
+                  const uint32_t* elem_strides, int swizzle) {
+  if (swizzle != 128 && swizzle != 64) return -1;
   if (!g_encode) {
     cudaDriverEntryPointQueryResult q;
     void* fn = nullptr;
@@ -785,8 +793,17 @@ int cg_encode_map(CUtensorMap* out, const void* base, int rank, const uint64_t* 
   for (int i = 0; i < rank; ++i) { gd[i] = dims[i]; bx[i] = box[i]; es[i] = elem_strides ? elem_strides[i] : 1; }
   for (int i = 0; i + 1 < rank; ++i) gs[i] = strides_bytes[i];
   const CUresult r = g_encode(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                              swizzle == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : (int)r;
+}
+
+// wgmma descriptor (wgmma.cuh): LBO >> 4 in [16,30), SBO >> 4 in [32,46), swizzle mode in [62,64) (1 = 128 B, 2 = 64 B).  Rows of
+// `swizzle` bytes in 8-row groups: SBO = 8 rows.  K-major: LBO unused (the k16 slice lies inside one row); MN-major: LBO = stride
+// between the swizzle / 2-element atoms along M|N (one TMA box each)
+unsigned long long cg_desc_bits(int swizzle, bool mn_major, int lbo) {
+  const unsigned long long l = mn_major ? (unsigned)lbo : 16u, sbo = 8u * (unsigned)swizzle;
+  return ((l >> 4) & 0x3FFF) << 16 | ((sbo >> 4) & 0x3FFF) << 32 | (unsigned long long)(swizzle == 128 ? 1 : 2) << 62;
 }
 
 int cg_finalize(CgGroup& g, int smem_budget) {

@@ -1,8 +1,8 @@
 // TMA-fed wgmma contraction engine ("cg"): declarations shared by cg.cu (kernel) and sac.cu (problem builders).
 //
 // Every dense contraction of the step is a list of 128-row output tiles; the operands of a tile are fetched, K-chunk by
-// K-chunk, by cp.async.bulk.tensor (TMA) boxes over BF16 plane tensors straight into 128B-swizzled shared-memory wgmma
-// tiles.  Convolutions need no im2col buffer: their patches / shifted windows / zero borders are expressed as tensor-map
+// K-chunk, by cp.async.bulk.tensor (TMA) boxes over BF16 plane tensors straight into swizzled (128B; 64B for conv1's A at one
+// image channel) shared-memory wgmma tiles.  Convolutions need no im2col buffer: their patches / shifted windows / zero borders are expressed as tensor-map
 // VIEWS (overlapping strides, element strides, out-of-bound zero fill) of the NHWC activation planes, so two elected
 // lanes feed the whole ring (tools/tma_probe.cu checks each view behaviour on the device).  A launch is a list of problems;
 // problems of one launch may depend on each other tile by tile (fused layers) and may split K with in-kernel finalisation.
@@ -60,9 +60,13 @@ struct CgProblem {
   const int* tm_tab;          // optional [tiles_m][CG_MAX_LOADS][2]: extra offsets of coordinates 1 and 2 per (tm, load)
   // ---- MMA
   int mn_major;               // 0: K-major A and B (rows = M|N, 128 B of K); 1: MN-major (rows = K, 128 B of M|N)
+  unsigned long long a_desc, b_desc;  // shared-memory descriptor bits of the A / B operand except the start address (cg_desc_bits:
+                                      // swizzle span, LBO, SBO); B is always 128B-swizzled, A's rows may be 64 B (conv1, one channel)
+  int a_moff;                 // byte offset of the second warpgroup's 64 rows of A inside the A region
   int ksteps;                 // wgmma K = 16 steps per chunk (a template parameter of the kernel's mainloop: part of the shape key)
   int a_off, b_off;           // region offsets inside a stage (b_off = planes * a_pstride)
   int a_kstep, b_kstep;       // descriptor start-address advance per k-step (bytes)
+  int a_kstep2;               // A's advance per PAIR of k-steps (2 a_kstep, or the next box when a box row holds two k16 slices)
   int a_lbo, b_lbo;           // MN-major: byte stride between 64-element atoms along M|N
   int umma_n;                 // tile width: 32, 64 or 128 (the widths cg_kernel is instantiated for)
   int nprod;                  // products per k-step: 1 (hi*hi), 3 (+hi*lo, lo*hi), 6 (+mid terms of the 3-plane split), one MMA
@@ -74,6 +78,12 @@ struct CgProblem {
   int lim_rows;               // tm * rows_tile + r < lim_rows
   int d0, d1;                 // r -> i0 = r % d0, i1 = (r / d0) % d1, i2 = r / (d0 * d1)
   long long o_tm; int o0, o1, o2; long long o_base;    // output element offset of (tm, r)
+  int rgrp_rows;              // > 0: row r also adds rgrp_off[r / rgrp_rows] (conv1 wgrad: one base offset per M atom)
+  int rgrp_off[8];
+  int lim_i0;                 // > 0: rows with i0 >= lim_i0 are not stored (junk columns of conv1, padded channels of its wgrad)
+  int tm_sub;                 // > 1 (ACT / DGRAD): row-tile tm is band tm % tm_sub of block tm / tm_sub -- its output starts at
+  long long o_sub;            //   (tm / tm_sub) * o_tm + (tm % tm_sub) * o_sub, and rows with (tm % tm_sub) * d1 + i1 >= lim_i1
+  int lim_i1;                 //   are not stored (conv1: two 8 x 16 bands of a sample's 15 x 15 output map)
   long long m_tm; int m0, m1, m2; long long m_base;    // mask element offset of (tm, r)
   int n_valid;                // columns < n_valid are stored (N of the problem)
   int grp_stride;             // element distance between consecutive 32-column groups of the output (32 = contiguous)
@@ -124,9 +134,14 @@ struct CgGroup {               // one launch
   double flops = 0;
 };
 
-// encodes a BF16 tiled tensor map (SWIZZLE_128B, zero OOB fill); dims/box innermost first, strides in BYTES for dims 1..rank-1
+// encodes a BF16 tiled tensor map (zero OOB fill, SWIZZLE_<swizzle>B: 128 or 64, the bytes of the box's innermost dimension);
+// dims/box innermost first, strides in BYTES for dims 1..rank-1
 int cg_encode_map(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box,
-                  const uint32_t* elem_strides);
+                  const uint32_t* elem_strides, int swizzle = 128);
+// descriptor bits of a wgmma shared-memory operand (everything but the start address) whose rows are `swizzle` bytes (128 or 64)
+// swizzled: K-major (rows = M|N; SBO = 8 rows, LBO unused) or MN-major (rows = K; SBO = 8 rows, LBO = stride between atoms
+// of swizzle / 2 elements along M|N)
+unsigned long long cg_desc_bits(int swizzle, bool mn_major, int lbo);
 // finalises tile_start / total_tiles / ring geometry of a group (host side)
 int cg_finalize(CgGroup& g, int smem_budget);
 cudaError_t cg_launch(const CgGroup& g, const CUtensorMap* dev_maps, int num_sms, cudaStream_t s, bool pdl, int debug_flags);

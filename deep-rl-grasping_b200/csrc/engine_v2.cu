@@ -6,8 +6,8 @@
 // chain: fuse_groups wires each consumer problem to the producer tiles it reads) and (iv) the HBM-bound helper kernels around them:
 //   gather2_kernel : replay slot draw + gather of replay frames (compact rows, replay.cu) + float64 VecNormalize +
 //                    clip + /255 (replay.cu semantics, [SB2] ReplayBuffer.sample(env=VecNormalize), observation_input(scale=True)),
-//                    the 3-plane BF16 split and the conv1 patch rows (8x8 stride-4 patches of the normalised image; the one view
-//                    TMA cannot express, see tools/tma_probe.cu) so that conv1 forward and its wgrad are plain 2-D TMA tiles;
+//                    the 3-plane BF16 split, stored space-to-depth (S, below) so that conv1's 8x8 stride-4 patches become a
+//                    2x2 stride-1 window over S: four shifted boxes of a monotonic tensor-map view;
 //   planes2_kernel : weights -> BF16 planes in the layouts the tensor maps expect (transposed / packed per consumer).
 // The bias gradients of the conv and cnn_fc1 layers come from the DGRAD epilogues of cg.cu (column sums of the gradient maps).
 // Reference shapes: custom_obs_policy.py:34-40 (conv 8x8/4 -> 4x4/2 -> 3x3/1, fc 1024->512), SURVEY.md Appendix A.
@@ -26,9 +26,9 @@ namespace {
 // ------------------------------------------------------------------------------------------------ gather2
 struct Gather2Args {
   GatherArgs g;                 // sources, statistics, F rows (fp32), reward / done outputs, slot draw
-  uint16_t* a1[2][3];           // patch matrices [B*225][64*Ci] (obs, next_obs) x 3 planes
+  uint16_t* s1[2][3];           // space-to-depth images [B][16][16][4][4][Cp] (obs, next_obs) x 3 planes
   uint16_t* fp[3][3];           // feature-row planes [net][plane] [B][KF]
-  int KF, Ci, OH, OW;           // OH = OW = 15
+  int KF;
 };
 
 __device__ __forceinline__ void split3(float y, uint16_t& p0, uint16_t& p1, uint16_t& p2) {
@@ -39,12 +39,72 @@ __device__ __forceinline__ void split3(float y, uint16_t& p0, uint16_t& p1, uint
   p0 = __bfloat16_as_ushort(h0); p1 = __bfloat16_as_ushort(h1); p2 = __bfloat16_as_ushort(__float2bfloat16_rn(r2));
 }
 
-// one CTA per (sample, obs | next_obs): normalise into shared-memory planes, then emit the patch matrix rows
+// Half a 4x4 block of the space-to-depth image S[Y][X][b][c][ci] (pixel (4Y + b, 4X + c), channel ci < CP; ci >= Ci is a zero
+// pad): image rows b = 2h, 2h + 1 of the block, 4 pixels each.  The 4 CP values of a row are contiguous in S (8 CP bytes) and the
+// threads of a warp cover consecutive half blocks, so its stores fill whole sectors.  Normalise / clip / scale / split as the
+// round-1 gather does, element by element.
+template <int Ci>
+__device__ __forceinline__ void s2d_half_block(const Gather2Args& a, const unsigned char* __restrict__ src, int it, int which, size_t b) {
+  constexpr int CP = s2d_channels(Ci);
+  const GatherArgs& g = a.g;
+  const int npx = g.H * g.W * Ci;
+  const int h = it & 1, X = (it >> 1) & 15, Y = it >> 5;
+  const double clip_obs = g.normc[1];
+  const bool norm_obs = g.normc[3] != 0.0;
+  const float scale = g.scale;
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const int e0 = ((4 * Y + 2 * h + rr) * g.W + 4 * X) * Ci;      // 4 pixels x Ci channels, a multiple of 4 elements
+    float y[4 * Ci];
+#pragma unroll
+    for (int q = 0; q < Ci; ++q) {
+      const int e = e0 + 4 * q;
+      const float4 v = frame_load4(src, g.fmt, npx, Ci, e);
+      float t[4] = {v.x, v.y, v.z, v.w};
+      if (norm_obs) {
+        const double2 m0 = *reinterpret_cast<const double2*>(g.mean + e), m1 = *reinterpret_cast<const double2*>(g.mean + e + 2);
+        const double2 i0 = *reinterpret_cast<const double2*>(g.var + e), i1 = *reinterpret_cast<const double2*>(g.var + e + 2);
+        t[0] = (float)fmin(fmax(((double)t[0] - m0.x) * i0.x, -clip_obs), clip_obs);
+        t[1] = (float)fmin(fmax(((double)t[1] - m0.y) * i0.y, -clip_obs), clip_obs);
+        t[2] = (float)fmin(fmax(((double)t[2] - m1.x) * i1.x, -clip_obs), clip_obs);
+        t[3] = (float)fmin(fmax(((double)t[3] - m1.y) * i1.y, -clip_obs), clip_obs);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) y[4 * q + j] = t[j];
+    }
+    uint32_t p[3][2 * CP];                                   // the row's 4 CP values per plane, packed in pairs
+#pragma unroll
+    for (int k = 0; k < 4 * CP; k += 2) {
+      uint16_t q[3][2];
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const int c = (k + u) / CP, ci = (k + u) % CP;
+        if (ci < Ci) split3(y[c * Ci + ci] / scale, q[0][u], q[1][u], q[2][u]);
+        else q[0][u] = q[1][u] = q[2][u] = 0;
+      }
+#pragma unroll
+      for (int pl = 0; pl < 3; ++pl) p[pl][k / 2] = (uint32_t)q[pl][0] | ((uint32_t)q[pl][1] << 16);
+    }
+    const size_t o = b * 4096 * CP + (size_t)((Y * 16 + X) * 16 + 4 * (2 * h + rr)) * CP;
+#pragma unroll
+    for (int pl = 0; pl < 3; ++pl) {
+      if constexpr (CP == 1) {
+        *reinterpret_cast<uint2*>(a.s1[which][pl] + o) = make_uint2(p[pl][0], p[pl][1]);
+      } else {
+        uint4* d = reinterpret_cast<uint4*>(a.s1[which][pl] + o);
+        d[0] = make_uint4(p[pl][0], p[pl][1], p[pl][2], p[pl][3]);
+        d[1] = make_uint4(p[pl][4], p[pl][5], p[pl][6], p[pl][7]);
+      }
+    }
+  }
+}
+
+// one CTA per (sample, obs | next_obs), one thread per half 4x4 block of the 64 x 64 image (Ci image channels)
+template <int Ci>
 __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
-  extern __shared__ uint16_t sm_planes[];            // [3][H*W*Ci]
   const GatherArgs& g = a.g;
   const int b = blockIdx.x, which = blockIdx.y, tid = threadIdx.x;
-  const int Ci = a.Ci, HW = g.H * g.W, npx = HW * Ci;
+  const int HW = g.H * g.W, npx = HW * Ci;
   const int Ec = npx + 4;                                  // compact replay row: image planes | actuator value | 3 pad floats
   long long slot = b;
   if (g.indices) slot = g.indices[b];
@@ -59,31 +119,7 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
   const double clip_obs = g.normc[1];
   const bool norm_obs = g.normc[3] != 0.0;
   const float scale = g.scale;
-  // shared-memory planes with a padded row pitch (+8 elements = +4 banks per image row): the patch pass below reads 16-byte runs
-  // of 8 consecutive image rows at once, which a 128-byte pitch puts on the same four banks (8-way conflicts)
-  const int rowe = g.W * Ci, pitch = rowe + 8, plane_e = g.H * pitch;
-  // image block: exactly the NHWC image with Ci channels -> no index arithmetic; float64 VecNormalize chain per element
-  for (int e4 = tid; e4 < (npx >> 2); e4 += blockDim.x) {
-    const float4 v = frame_load4(src, g.fmt, npx, Ci, 4 * e4);
-    float y[4] = {v.x, v.y, v.z, v.w};
-    if (norm_obs) {
-      const double2 m0 = *reinterpret_cast<const double2*>(g.mean + 4 * e4), m1 = *reinterpret_cast<const double2*>(g.mean + 4 * e4 + 2);
-      const double2 i0 = *reinterpret_cast<const double2*>(g.var + 4 * e4), i1 = *reinterpret_cast<const double2*>(g.var + 4 * e4 + 2);
-      y[0] = (float)fmin(fmax(((double)y[0] - m0.x) * i0.x, -clip_obs), clip_obs);
-      y[1] = (float)fmin(fmax(((double)y[1] - m0.y) * i0.y, -clip_obs), clip_obs);
-      y[2] = (float)fmin(fmax(((double)y[2] - m1.x) * i1.x, -clip_obs), clip_obs);
-      y[3] = (float)fmin(fmax(((double)y[3] - m1.y) * i1.y, -clip_obs), clip_obs);
-    }
-    uint16_t p[3][4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) split3(y[j] / scale, p[0][j], p[1][j], p[2][j]);
-#pragma unroll
-    for (int pl = 0; pl < 3; ++pl) {
-      const uint2 w = make_uint2((uint32_t)p[pl][0] | ((uint32_t)p[pl][1] << 16), (uint32_t)p[pl][2] | ((uint32_t)p[pl][3] << 16));
-      const int e = 4 * e4, row = e / rowe, col = e - row * rowe;          // (rowe is a multiple of 4: a group never straddles rows)
-      *reinterpret_cast<uint2*>(sm_planes + pl * plane_e + row * pitch + col) = w;
-    }
-  }
+  for (int it = tid; it < 512; it += blockDim.x) s2d_half_block<Ci>(a, src, it, which, b);
   if (tid == 0) {                                            // direct feature -> column 512 of the feature rows
     float yy = frame_elem(src, g.fmt, npx, Ci, npx);
     if (norm_obs) yy = (float)fmin(fmax(((double)yy - g.mean[npx]) * g.var[npx], -clip_obs), clip_obs);
@@ -96,24 +132,6 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
       g.F_pi[fo] = yy; g.F_v[fo] = yy;
       a.fp[0][0][po] = p0; a.fp[0][1][po] = p1; a.fp[0][2][po] = p2;
       a.fp[1][0][po] = p0; a.fp[1][1][po] = p1; a.fp[1][2][po] = p2;
-    }
-  }
-  __syncthreads();
-  // patch rows: for output pixel (oy, ox) and kernel row ky the 8*Ci elements (kx, ci) are contiguous in the NHWC plane
-  const int seg = 8 * Ci;                                     // elements per (patch, ky) run: 16 B (Ci = 1) .. 64 B (Ci = 4)
-  const int K1 = 64 * Ci, nruns = a.OH * a.OW * 8;
-  const size_t img = (size_t)b * a.OH * a.OW * K1;
-  for (int i = tid; i < nruns * (seg / 8); i += blockDim.x) {
-    const int part = i % (seg / 8), run = i / (seg / 8);      // 16-byte pieces of a run
-    const int ky = run & 7, patch = run >> 3;
-    const int oy = patch / a.OW, ox = patch - oy * a.OW;
-    const int so = (4 * oy + ky) * pitch + 4 * ox * Ci + 8 * part;         // 8-byte aligned at least
-    const size_t go = img + (size_t)patch * K1 + ky * seg + 8 * part;
-#pragma unroll
-    for (int pl = 0; pl < 3; ++pl) {
-      const uint16_t* sp = sm_planes + pl * plane_e + so;
-      const uint2 lo = *reinterpret_cast<const uint2*>(sp), hi = *reinterpret_cast<const uint2*>(sp + 4);
-      *reinterpret_cast<uint4*>(a.a1[which][pl] + go) = make_uint4(lo.x, lo.y, hi.x, hi.y);
     }
   }
   if (which == 0 && g.act) {
@@ -142,6 +160,7 @@ struct Plane2Job {
   int R, N, np;
   int transpose;             // 1: dst[(n + off0) * ld + r]   0: dst[r * ld + n + off0]
   int ld, off0;
+  int k1_ci;                 // > 0 (transposed conv1 weights of k1_ci channels): row r goes to K row conv1_krow(r, k1_ci)
   int tile_start;
 };
 
@@ -192,7 +211,9 @@ __global__ void __launch_bounds__(256) planes2_kernel(const Plane2Job* __restric
       const size_t o = (size_t)(n + job.off0) * job.ld + rb;
       for (int k = 0; k < job.np; ++k) {
         uint16_t* d = job.dst[k] + o;
-        if (rb + 7 < job.R && (o & 7) == 0)
+        if (job.k1_ci) {
+          for (int u = 0; u < 8; ++u) if (rb + u < job.R) d[conv1_krow(rb + u, job.k1_ci) - rb] = p[k][u];
+        } else if (rb + 7 < job.R && (o & 7) == 0)
           *reinterpret_cast<uint4*>(d) = make_uint4((uint32_t)p[k][0] | ((uint32_t)p[k][1] << 16), (uint32_t)p[k][2] | ((uint32_t)p[k][3] << 16),
                                                     (uint32_t)p[k][4] | ((uint32_t)p[k][5] << 16), (uint32_t)p[k][6] | ((uint32_t)p[k][7] << 16));
         else
@@ -208,7 +229,7 @@ __global__ void __launch_bounds__(256) planes2_kernel(const Plane2Job* __restric
 // 1024-byte swizzle atoms, else one plane (an instruction per plane, plane = last coordinate).  Distinct maps per plane cost a
 // descriptor fetch per instruction, whatever the box size.  Returns the map index or -1.
 int add_maps(V2State& v, uint16_t* const* planes, int np, int rank, std::initializer_list<uint64_t> dims, std::initializer_list<uint64_t> strides_b,
-             std::initializer_list<uint32_t> box, std::initializer_list<uint32_t> estr = {}, bool allow_whole = true) {
+             std::initializer_list<uint32_t> box, std::initializer_list<uint32_t> estr = {}, bool allow_whole = true, int swizzle = 128) {
   uint64_t d[5] = {1, 1, 1, 1, 1}, s[5] = {0, 0, 0, 0, 0};
   uint32_t bx[5] = {1, 1, 1, 1, 1}, es[5] = {1, 1, 1, 1, 1};
   int i = 0; for (auto x : dims) d[i++] = x;
@@ -226,7 +247,7 @@ int add_maps(V2State& v, uint16_t* const* planes, int np, int rank, std::initial
   if (pitch <= 0 || pitch % 16) return -1;
   d[rank] = (uint64_t)np; s[rank - 1] = (uint64_t)pitch; bx[rank] = whole ? (uint32_t)np : 1u; es[rank] = 1;
   CUtensorMap m;
-  if (cg_encode_map(&m, planes[0], rank + 1, d, s, bx, es) != 0) return -1;
+  if (cg_encode_map(&m, planes[0], rank + 1, d, s, bx, es, swizzle) != 0) return -1;
   v.maps.push_back(m);
   v.map_whole.push_back(whole ? 1 : 0);
   v.map_box_bytes.push_back((int)box_bytes);
@@ -253,7 +274,8 @@ CgProblem kmajor(int planes, int n_tile, int chunks, int n2, int a_box_rows) {
   P.a_off = 0; P.a_pstride = 128 * 128;
   P.b_off = planes * P.a_pstride; P.b_pstride = n_tile * 128;
   P.tx_bytes = planes * (a_box_rows * 128 + n_tile * 128);
-  P.mn_major = 0; P.ksteps = 4; P.a_kstep = P.b_kstep = 32;
+  P.mn_major = 0; P.ksteps = 4; P.a_kstep = P.b_kstep = 32; P.a_kstep2 = 64;
+  P.a_desc = P.b_desc = cg_desc_bits(128, false, 0); P.a_moff = 64 * 128;
   P.umma_n = n_tile;
   P.nprod = planes == 3 ? 6 : (planes == 2 ? 3 : 1);
   P.d0 = 1 << 20; P.d1 = 1;
@@ -275,8 +297,9 @@ CgProblem mnmajor(int planes, int kr, int a_atoms, int b_atoms, int chunks) {
   P.a_off = 0; P.a_pstride = atom;
   P.b_off = 2 * planes * atom; P.b_pstride = b_atoms * atom;
   P.tx_bytes = planes * (a_atoms + b_atoms) * atom;
-  P.mn_major = 1; P.ksteps = kr / 16; P.a_kstep = P.b_kstep = 2048;
+  P.mn_major = 1; P.ksteps = kr / 16; P.a_kstep = P.b_kstep = 2048; P.a_kstep2 = 4096;
   P.a_lbo = planes * atom; P.b_lbo = atom;
+  P.a_desc = cg_desc_bits(128, true, P.a_lbo); P.b_desc = cg_desc_bits(128, true, P.b_lbo); P.a_moff = P.a_lbo;
   P.umma_n = 64 * b_atoms;
   P.nprod = planes == 3 ? 6 : (planes == 2 ? 3 : 1);
   P.d0 = 1 << 20; P.d1 = 1;
@@ -294,6 +317,8 @@ int push_group(b2g_sac* h, std::vector<CgGroup>& list, CgGroup& g, const char* n
     if (P.planes * P.umma_n > 256) return b2g_fail(B2G_EINVAL, std::string("engine v2: planes x tile width exceeds one accumulator buffer (group ") + name + ")");
     if (!cg_shape_supported(P.umma_n, P.nprod, P.mn_major != 0, P.ksteps))
       return b2g_fail(B2G_EINVAL, std::string("engine v2: no cg_kernel instance for the tile shape of a problem in group ") + name);
+    if (P.tm_sub > 1 && !cg_epi_handoff(P.epi))     // only the epilogue warpgroup maps bands (cg.cuh: tm_sub)
+      return b2g_fail(B2G_EINVAL, std::string("engine v2: a banded problem must have an ACT or DGRAD epilogue (group ") + name + ")");
     g.flops += 2.0 * P.tiles_m * 128.0 * P.tiles_n * P.umma_n * P.chunks * 64.0;      // issued (tile-padded) work
   }
   list.push_back(g);
@@ -370,21 +395,21 @@ int check_split(const char* var, int chunks, int splits) {
 // ================================================================================================ create
 int v2_alloc(b2g_sac* h) {
   V2State& v = h->v2;
-  const int B = h->B, Ci = h->Cimg, K1 = 64 * Ci, KF = v.KF;
-  const size_t n1 = (size_t)B * 225 * 32, n2 = (size_t)B * 36 * 64, n3 = (size_t)B * 1024, na = (size_t)B * 225 * K1, nf = (size_t)B * KF;
+  const int B = h->B, Cp = s2d_channels(h->Cimg), K1 = 64 * Cp, KF = v.KF;
+  const size_t n1 = (size_t)B * 225 * 32, n2 = (size_t)B * 36 * 64, n3 = (size_t)B * 1024, ns = (size_t)B * 4096 * Cp, nf = (size_t)B * KF;
   // ---- activations: one block per layer, [net][plane] with uniform strides (conv1 writes two nets from one tile)
-  uint16_t *bH1, *bH2, *bH3, *bF, *bA1;
+  uint16_t *bH1, *bH2, *bH3, *bF, *bS;
   if (int rc = dev_alloc(h->allocs, h->stream, &bH1, 9 * n1)) return rc;
   if (int rc = dev_alloc(h->allocs, h->stream, &bH2, 9 * n2)) return rc;
   if (int rc = dev_alloc(h->allocs, h->stream, &bH3, 9 * n3)) return rc;
   if (int rc = dev_alloc(h->allocs, h->stream, &bF, 9 * nf)) return rc;
-  if (int rc = dev_alloc(h->allocs, h->stream, &bA1, 6 * na)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &bS, 6 * ns)) return rc;
   for (int n = 0; n < 3; ++n)
     for (int p = 0; p < 3; ++p) {
       v.H1[n][p] = bH1 + (n * 3 + p) * n1; v.H2[n][p] = bH2 + (n * 3 + p) * n2; v.H3[n][p] = bH3 + (n * 3 + p) * n3;
       v.F[n][p] = bF + (n * 3 + p) * nf;
     }
-  for (int w = 0; w < 2; ++w) for (int p = 0; p < 3; ++p) v.A1[w][p] = bA1 + (w * 3 + p) * na;
+  for (int w = 0; w < 2; ++w) for (int p = 0; p < 3; ++p) v.S[w][p] = bS + (w * 3 + p) * ns;
   if (int rc = dev_alloc(h->allocs, h->stream, &v.z0v, (size_t)B * 3 * h->H)) return rc;
   // ---- gradient maps (2 planes) and natural-layout weight planes of the backward chain.  The planes of a tensor are
   //      equidistant in one allocation: the tensor maps address them through an extra (outermost) plane dimension
@@ -422,7 +447,7 @@ int v2_alloc(b2g_sac* h) {
 int v2_create(b2g_sac* h) {
   V2State& v = h->v2;
   g_mk_state = &v;
-  const int B = h->B, Ci = h->Cimg, K1 = 64 * Ci, KF = v.KF, FS = h->FS, H = h->H;
+  const int B = h->B, Ci = h->Cimg, Cp = s2d_channels(Ci), K1 = 64 * Cp, KF = v.KF, FS = h->FS, H = h->H;
   const size_t n1 = (size_t)B * 225 * 32;
   // ---- plane jobs (weights change every step)
   const char* nets[3] = {"model/pi", "model/values_fn", "target/values_fn"};
@@ -435,9 +460,12 @@ int v2_create(b2g_sac* h) {
     start += ((R + 63) / 64) * ((N + 31) / 32);
     jobs.push_back(j);
   };
-  add_job(h->p("model/pi/cnn1/w"), K1, 32, v.W1T[0], 3, 1, K1, 0);
-  add_job(h->p("model/values_fn/cnn1/w"), K1, 32, v.W1T[0], 3, 1, K1, 32);
-  add_job(h->p("target/values_fn/cnn1/w"), K1, 32, v.W1T[1], 3, 1, K1, 0);
+  add_job(h->p("model/pi/cnn1/w"), 64 * Ci, 32, v.W1T[0], 3, 1, K1, 0);
+  jobs.back().k1_ci = Ci;
+  add_job(h->p("model/values_fn/cnn1/w"), 64 * Ci, 32, v.W1T[0], 3, 1, K1, 32);
+  jobs.back().k1_ci = Ci;
+  add_job(h->p("target/values_fn/cnn1/w"), 64 * Ci, 32, v.W1T[1], 3, 1, K1, 0);
+  jobs.back().k1_ci = Ci;
   for (int n = 0; n < 3; ++n) {
     add_job(h->p(std::string(nets[n]) + "/cnn2/w"), 512, 64, v.W2T[n], 3, 1, 512, 0);
     add_job(h->p(std::string(nets[n]) + "/cnn3/w"), 576, 64, v.W3T[n], 3, 1, 576, 0);
@@ -476,21 +504,44 @@ int v2_create(b2g_sac* h) {
   // ================================================================================ forward problems (6-product mode)
   const int NP = 3;
   const long long h1_net = (long long)3 * n1;       // element distance between the same plane of consecutive nets
-  // ---- conv1: [obs -> pi | vf] (N = 64, two output tensors) and [next_obs -> target] (N = 32)
+  // ---- conv1: [obs -> pi | vf] (N = 64, two output tensors) and [next_obs -> target] (N = 32), a 2x2 stride-1 convolution over S.
+  //      The sample is folded into the block row (monotonic strides): row tile tm = 2 s + t (output rows oy 8t .. 8t + 7, ox 0 .. 15 of
+  //      sample s) reads block rows 8 tm + a.  Block row 16 s + 16 belongs to the next sample (the last sample's is out of bounds);
+  //      like X = 15 + 1 it only reaches the junk rows ox = 15 and oy = 15, which the epilogue does not store.
+  //      Cp = 4: S as {64, 16 X, 16 B Y}; K-chunk = window (c1, c2) = (a, a'), the box {64, 16, 8} at (0, a', 8 tm + a).
+  //      Cp = 1: S as {32, 15 X, 16 B Y} with a 32-byte X stride, so that a row holds blocks X and X + 1 = windows (a, 0) and (a, 1)
+  //      (the view overlaps itself along X, like conv2's); the box {32, 16, 8} at (0, 0, 8 tm + a) holds k-steps 2a and 2a + 1
+  //      (64-byte rows, X = 15 out of bounds), one K-chunk of two such boxes.
   {
     CgGroup g;
     for (int w = 0; w < 2; ++w) {
       const int N = w == 0 ? 64 : 32;
-      const int mA = add_maps(v, v.A1[w], NP, 2, {(uint64_t)K1, (uint64_t)B * 225}, {(uint64_t)K1 * 2}, {64, 128});
+      const int mA = Cp == 1 ? add_maps(v, v.S[w], NP, 3, {32, 15, (uint64_t)B * 16}, {32, 512}, {32, 16, 8}, {}, true, 64)
+                             : add_maps(v, v.S[w], NP, 3, {64, 16, (uint64_t)B * 16}, {128, 2048}, {64, 16, 8});
       const int mB = add_maps(v, v.W1T[w], NP, 2, {(uint64_t)K1, (uint64_t)N}, {(uint64_t)K1 * 2}, {64, (uint32_t)N});
       if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (conv1)");
-      CgProblem P = kmajor(NP, N, Ci, Ci, 128);
-      P.nloads = 2;
-      P.ld[0] = mk_load(mA, 2, 0); P.ld[0].d_tm[1] = 128; P.ld[0].d_c2[0] = 64;
-      P.ld[1] = mk_load(mB, 2, P.b_off); P.ld[1].d_c2[0] = 64;
-      P.tiles_m = (B * 225 + 127) / 128;
-      P.epi = CG_EPI_ACT; P.rows_tile = 128; P.lim_rows = B * 225;
-      P.o_tm = 128 * 32; P.o0 = 32; P.n_valid = N; P.out_planes = 3;
+      CgProblem P;
+      if (Cp == 1) {
+        // k-step 2a + a' = box a, bytes [32 a', 32 a' + 32) of its 64-byte rows
+        P = kmajor(NP, N, 1, 1, 128);
+        P.a_pstride = 128 * 64; P.a_kstep = 32; P.a_kstep2 = NP * P.a_pstride;
+        P.b_off = 2 * P.a_kstep2;
+        P.tx_bytes = NP * (2 * 128 * 64 + N * 128);
+        P.a_desc = cg_desc_bits(64, false, 0); P.a_moff = 64 * 64;
+        P.nloads = 3;
+        for (int a = 0; a < 2; ++a) { P.ld[a] = mk_load(mA, 3, a * P.a_kstep2); P.ld[a].c0[2] = a; P.ld[a].d_tm[2] = 8; }
+        P.ld[2] = mk_load(mB, 2, P.b_off);
+      } else {
+        P = kmajor(NP, N, 4, 2, 128);
+        P.nloads = 2;
+        P.ld[0] = mk_load(mA, 3, 0); P.ld[0].d_tm[2] = 8; P.ld[0].d_c1[2] = 1; P.ld[0].d_c2[1] = 1;
+        P.ld[1] = mk_load(mB, 2, P.b_off); P.ld[1].d_c1[0] = 128; P.ld[1].d_c2[0] = 64;
+      }
+      P.tiles_m = 2 * B;
+      P.epi = CG_EPI_ACT; P.rows_tile = 128; P.lim_rows = 2 * B * 128;
+      P.d0 = 16; P.d1 = 8; P.o0 = 32; P.o1 = 15 * 32; P.o_tm = 225 * 32;      // row (oy - 8t, ox) of band t of sample s
+      P.tm_sub = 2; P.o_sub = 8 * 15 * 32; P.lim_i0 = 15; P.lim_i1 = 15;
+      P.n_valid = N; P.out_planes = 3;
       P.grp_stride = (int)h1_net;
       const int net0 = w == 0 ? 0 : 2;
       for (int p = 0; p < 3; ++p) P.out_p[p] = v.H1[net0][p];
@@ -764,18 +815,45 @@ int v2_create(b2g_sac* h) {
       g.host[g.n++] = P;
     }
     {
-      const int mA = add_maps(v, v.A1[0], NB, 2, {(uint64_t)K1, (uint64_t)B * 225}, {(uint64_t)K1 * 2}, {64, 64});
-      const int mB = add_maps(v, v.dZ1, NB, 2, {64, (uint64_t)B * 225}, {128}, {64, 64});
+      // M = conv1's K rows (window (a, a'), then (b, c, ci)): the M atoms are the shifted S boxes of the forward's views, MN-major.
+      // K-chunk (c1, c2) = (sample, band of 4 output rows): the S boxes {.., 16, 4} at block row 16 c1 + 4 c2 + a, and dZ1 viewed
+      // as {64, 15 ox, 15 oy, B}, box {64, 16, 4, 1} at (0, 0, 4 c2, c1).  The junk pixels (ox = 15, oy = 15) may be in bounds of
+      // S; their dZ1 rows are out of bounds, so they add zeros.
+      const int mA = Cp == 1 ? add_maps(v, v.S[0], NB, 3, {32, 15, (uint64_t)B * 16}, {32, 512}, {32, 16, 4}, {}, true, 64)
+                             : add_maps(v, v.S[0], NB, 3, {64, 16, (uint64_t)B * 16}, {128, 2048}, {64, 16, 4});
+      const int mB = add_maps(v, v.dZ1, NB, 4, {64, 15, 15, (uint64_t)B}, {128, 15 * 128, 225 * 128}, {64, 16, 4, 1});
       if (mA < 0 || mB < 0) return b2g_fail(B2G_ECUDA, "engine v2: cuTensorMapEncodeTiled failed (conv1 wgrad)");
-      CgProblem P = mnmajor(NB, 64, 2, 1, (B * 225 + 63) / 64);
-      P.nloads = 3;
-      // both 64-wide atoms of the M tile are always fetched; an atom beyond K1 (one image channel: K1 = 64) is out of
-      // bounds and arrives as zeros, its output rows are masked by lim_rows
-      for (int a = 0; a < 2; ++a) { P.ld[a] = mk_load(mA, 2, a * P.a_lbo); P.ld[a].c0[0] = 64 * a; P.ld[a].d_tm[0] = 128; P.ld[a].d_c2[1] = 64; }
-      P.ld[2] = mk_load(mB, 2, P.b_off); P.ld[2].d_c2[1] = 64;
-      P.tiles_m = (K1 + 127) / 128; P.tiles_n = 1;
+      CgProblem P = mnmajor(NB, 64, 2, 1, 4 * B);
+      P.n2 = 4;
+      if (Cp == 1) {
+        // all four windows (64 rows of M) in one tile: two 32-element atoms (windows (a, 0) | (a, 1)) of 64-byte rows; the second
+        // warpgroup repeats the first one's rows (rows 64 .. 127 are not stored)
+        P.a_pstride = 64 * 64; P.a_lbo = NB * P.a_pstride;
+        P.b_off = 2 * P.a_lbo;
+        P.tx_bytes = NB * (2 * 64 * 64 + 64 * 128);
+        P.a_kstep = 16 * 64; P.a_kstep2 = 2 * P.a_kstep; P.a_desc = cg_desc_bits(64, true, P.a_lbo); P.a_moff = 0;
+        P.nloads = 3;
+        for (int a = 0; a < 2; ++a) { P.ld[a] = mk_load(mA, 3, a * P.a_lbo); P.ld[a].c0[2] = a; P.ld[a].d_c1[2] = 16; P.ld[a].d_c2[2] = 4; }
+        P.tiles_m = 1;
+        P.d0 = 4; P.d1 = 4; P.o0 = 32; P.o1 = 8 * 32;          // row (l, b, c) of window l = 2a + a'
+        P.rgrp_rows = 16;
+        for (int l = 0; l < 4; ++l) P.rgrp_off[l] = (32 * (l >> 1) + 4 * (l & 1)) * 32;
+      } else {
+        // tile tm = window row a: the windows (a, 0), (a, 1) as the two 64-wide atoms of the M tile
+        for (int l = 0; l < 2; ++l) {
+          P.ld[l] = mk_load(mA, 3, l * P.a_lbo); P.ld[l].c0[1] = l; P.ld[l].d_tm[2] = 1; P.ld[l].d_c1[2] = 16; P.ld[l].d_c2[2] = 4;
+        }
+        P.nloads = 3;
+        P.tiles_m = 2;
+        P.d0 = 4; P.d1 = 4; P.o0 = 32; P.o1 = Ci * 32; P.o_tm = 32 * Ci * 32;     // row (a', b, c, ci) of window (tm, a')
+        P.lim_i0 = Ci;                                         // pad channels
+        P.rgrp_rows = 16;
+        for (int j = 0; j < 8; ++j) P.rgrp_off[j] = (8 * Ci * (j & 3) + 4 * Ci * (j >> 2)) * 32;
+      }
+      P.ld[P.nloads - 1] = mk_load(mB, 4, P.b_off); P.ld[P.nloads - 1].d_c1[3] = 1; P.ld[P.nloads - 1].d_c2[2] = 4;
+      P.tiles_n = 1;
       P.splits = std::max(1, std::min(P.chunks, std::max(84 / P.tiles_m, (P.chunks + 15) / 16)));
-      P.lim_rows = K1; P.o_tm = 128 * 32; P.o0 = 32; P.n_valid = 64;
+      P.lim_rows = 64 * Cp; P.n_valid = 64;
       P.out_f = h->g("model/pi/cnn1/w"); P.f_grp = (long long)(h->g("model/values_fn/cnn1/w") - h->g("model/pi/cnn1/w")); P.atomic = 1;
       g.host[g.n++] = P;
     }
@@ -791,7 +869,7 @@ int v2_create(b2g_sac* h) {
     for (auto& g : v.fwd) parts.push_back(&g);                 // conv1 (obs, next), conv2 x3, conv3 x3, fc1 x3, fc0 x3
     std::vector<Wire> w;
     for (int n = 0; n < 3; ++n) {
-      w.push_back({1, n, 0, n < 2 ? 0 : 1, 3 * 225, 128, 0});  // conv2 tile: 3 samples of H1 (225 rows each; conv1 tiles are 128 rows)
+      w.push_back({1, n, 0, n < 2 ? 0 : 1, 6, 1, 0});          // conv2 tile: 3 samples of H1 = 6 conv1 tiles (two bands per sample)
       w.push_back({2, n, 1, n, 8 * 36, 108, 0});               // conv3 tile: 8 samples of H2 (36 rows each; conv2 tiles are 3 samples)
       w.push_back({3, n, 2, n, 128 * 16, 128, 0});             // fc1 tile: 128 samples of H3 (16 rows each)
       w.push_back({4, n, 3, n, 128, 128, 0});                  // fc0 tile: 128 feature rows (all 8 column tiles of them)
@@ -810,9 +888,9 @@ int v2_create(b2g_sac* h) {
       w.push_back({3, n, 2, 2 * n, 72, 108, 0});               // conv2 dgrad tile: 2 samples of dZ2 (36 rows each; conv3 dgrad tiles are 3 samples)
       w.push_back({4, n, 2, 2 * n, 144, 108, 1});              // conv2 wgrad chunk: 4 samples of dZ2
     }
-    // conv1 wgrad chunk: 64 rows of dZ1 [B*225][pi | vf]; a conv2 dgrad tile (of EITHER net: both must be done) covers 2 samples = 450 rows
-    w.push_back({4, 2, 3, 0, 64, 450, 1});
-    w.push_back({4, 2, 3, 1, 64, 450, 1});
+    // conv1 wgrad chunk: a quarter sample of dZ1 [B*225][pi | vf]; a conv2 dgrad tile (of EITHER net: both must be done) covers 2 samples
+    w.push_back({4, 2, 3, 0, 1, 8, 1});
+    w.push_back({4, 2, 3, 1, 1, 8, 1});
     if (int rc = fuse_groups(h, parts, w, "bwd_fused", v.bwd_fused, n_ctr)) return rc;
     // data parallel: the same chain cut after cnn_fc1, where the gradients of [cnn_fc1 .. end] (84 % of the bytes) are final
     // and their all-reduce starts on the side stream underneath the conv backward
@@ -824,8 +902,8 @@ int v2_create(b2g_sac* h) {
       wb.push_back({1, n, 0, 2 * n, 72, 108, 0});
       wb.push_back({2, n, 0, 2 * n, 144, 108, 1});
     }
-    wb.push_back({2, 2, 1, 0, 64, 450, 1});
-    wb.push_back({2, 2, 1, 1, 64, 450, 1});
+    wb.push_back({2, 2, 1, 0, 1, 8, 1});
+    wb.push_back({2, 2, 1, 1, 1, 8, 1});
     if (int rc = fuse_groups(h, pa, wa, "bwd_fused_fc", v.bwd_fused, n_ctr)) return rc;
     if (int rc = fuse_groups(h, pb, wb, "bwd_fused_conv", v.bwd_fused, n_ctr)) return rc;
   }
@@ -851,16 +929,16 @@ int v2_gather(b2g_sac* h, const GatherArgs& ga, cudaStream_t s) {
   Gather2Args a{};
   a.g = ga;
   for (int w = 0; w < 2; ++w)
-    for (int p = 0; p < 3; ++p) a.a1[w][p] = v.A1[w][p];
+    for (int p = 0; p < 3; ++p) a.s1[w][p] = v.S[w][p];
   for (int n = 0; n < 3; ++n) for (int p = 0; p < 3; ++p) a.fp[n][p] = v.F[n][p];
-  a.KF = v.KF; a.Ci = h->Cimg; a.OH = h->H1; a.OW = h->W1;
-  const size_t smem = (size_t)3 * h->Hi * (h->Wi * h->Cimg + 8) * sizeof(uint16_t);
-  static size_t attr = 0;
-  if (smem > attr) {
-    CK(cudaFuncSetAttribute(gather2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = smem;
+  a.KF = v.KF;
+  const dim3 grid(ga.B, ga.next_obs || ga.next_frame ? 2 : 1);
+  switch (h->Cimg) {      // v2 runs 1 .. 4 image channels (sac.cu)
+    case 1: gather2_kernel<1><<<grid, 512, 0, s>>>(a); break;
+    case 2: gather2_kernel<2><<<grid, 512, 0, s>>>(a); break;
+    case 3: gather2_kernel<3><<<grid, 512, 0, s>>>(a); break;
+    default: gather2_kernel<4><<<grid, 512, 0, s>>>(a); break;
   }
-  gather2_kernel<<<dim3(ga.B, ga.next_obs || ga.next_frame ? 2 : 1), 512, smem, s>>>(a);
   return 0;
 }
 

@@ -1125,8 +1125,8 @@ int b2g_sac_create2(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, b2g_sa
   DA(h->P, h->n_all); DA(h->Mo, h->n_train); DA(h->Vo, h->n_train); DA(h->G, h->n_train + MET_COUNT);
   DA(h->metrics, MET_COUNT); DA(h->counters, 8); DA(h->step_consts, 4); DA(h->d_lr, 1);
   const int64_t cap = cfg->buffer_capacity;
-  {   // engine v2 (TMA-fed, cg.cu) trains the 64x64 CNN policy in the parity mode
-    h->v2.on = h->cnn && cfg->precision == B2G_PREC_BF16X3 && h->Hi == 64 && h->Wi == 64;
+  {   // engine v2 (TMA-fed, cg.cu) trains the 64x64 CNN policy of up to 4 image channels (conv1's S layout) in the parity mode
+    h->v2.on = h->cnn && cfg->precision == B2G_PREC_BF16X3 && h->Hi == 64 && h->Wi == 64 && h->Cimg <= 4;
     if (const char* dbg = getenv("B2G_CG_DEBUG")) h->v2.dbg = atoi(dbg);
   }
   {   // frame formats: the fp32 compact row, and the replay frames (8-bit planes first, then the fp32 planes, then the tail)

@@ -25,11 +25,20 @@ struct Tensor {
 
 
 // ---- engine v2 (cg.cu): BF16 plane tensors, tensor maps and problem groups of the TMA-fed path
+// conv1 reads the normalised image space-to-depth: S[sample][Y 16][X 16][b 4][c 4][ci < Cp] holds pixel (4Y + b, 4X + c), so the
+// 8x8 stride-4 convolution is a 2x2 stride-1 one over S.  Cp = 1 for one channel, else 4 (zero pad channels): conv1's operand
+// rows are two neighbouring blocks (64 bytes) or one block (128 bytes), swizzle spans that TMA and wgmma share.
+__host__ __device__ constexpr int s2d_channels(int Ci) { return Ci == 1 ? 1 : 4; }
+// conv1's K index (window (a, a') = (ky / 4, kx / 4), then (b, c, ci) = (ky % 4, kx % 4, ci)) of HWIO weight row (ky * 8 + kx) * Ci + ci
+__host__ __device__ inline int conv1_krow(int r, int Ci) {
+  const int ci = r % Ci, kx = (r / Ci) % 8, ky = r / (8 * Ci);
+  return ((((ky >> 2) * 2 + (kx >> 2)) * 4 + (ky & 3)) * 4 + (kx & 3)) * s2d_channels(Ci) + ci;
+}
 struct V2State {
   bool on = false;               // the step runs on this engine (CNN policy, 64 x 64 input, bf16x3)
   int KF = 576;                 // feature-row width of the F planes (513 features + actions, zero padded to 9 x 64)
   // activations: [which / net][plane]
-  uint16_t* A1[2][3]{};          // im2col of the normalised image: [B*225][64*Ci]  (0 = obs, 1 = next_obs)
+  uint16_t* S[2][3]{};           // the normalised image space-to-depth: [B][16][16][4][4][Cp]  (0 = obs, 1 = next_obs)
   uint16_t* H1[3][3]{};          // [B*225][32]
   uint16_t* H2[3][3]{};          // [B*36][64]
   uint16_t* H3[3][3]{};          // [B][1024]
@@ -42,7 +51,7 @@ struct V2State {
   uint16_t* dZ2[2][2]{};         // [B*36][64]
   uint16_t* dZ1[2]{};            // [plane] [B*225][2 nets][32]
   // weights as planes (refreshed every step by planes2_kernel)
-  uint16_t* W1T[2][3]{};         // [0]: obs [64 = pi|vf][64*Ci], [1]: target [32][64*Ci]
+  uint16_t* W1T[2][3]{};         // [0]: obs [64 = pi|vf][64*Cp], [1]: target [32][64*Cp]; K in conv1_krow order (pad rows zero)
   uint16_t* W2T[3][3]{};         // [net][plane] [64][512]
   uint16_t* W3T[3][3]{};         // [64][576]
   uint16_t* WfT[3][3]{};         // [512][1024]
