@@ -1,7 +1,8 @@
 """Seeded synthetic replay data of the reference's shapes and statistics (SURVEY.md §8d).
 
 Raw (un-normalised) transitions as ``replay_buffer.add`` would store them when VecNormalize wraps
-the env: depth plane ~ clip(N(mean_ij, var_ij), 0.02, 2.0) from the shipped ``obs_rms``; the pad
+the env: depth plane ~ clip(N(mean_ij, var_ij), 0.02, 2.0) from the shipped ``obs_rms`` (the last
+image plane; with 2 or more image planes the ones before it are integer colour 0..255); the pad
 plane is zero except pixel [0,0] = gripper width (robot.py:199-200); reward mixture from
 config/gripper_grasp.yaml:42-46 / rewards.py:128-138; done ~ Bernoulli(1/15).
 """
@@ -21,11 +22,9 @@ def make_transitions(n: int, obs_mean: np.ndarray, obs_var: np.ndarray, seed: in
         o = rng.standard_normal((n,) + shape) * sd + obs_mean
         if len(shape) == 3:
             c = shape[2] - 1
-            if c == 1:
-                o[..., :c] = np.clip(o[..., :c], 0.02, 2.0)
-            else:                                   # RGB-D: rgb 0..255, depth metres
-                o[..., :3] = np.clip(np.round(o[..., :3]), 0, 255)
-                o[..., 3] = np.clip(o[..., 3], 0.02, 2.0)
+            if c >= 2:                              # colour planes 0..255 before the depth plane (RGB-D when c = 4)
+                o[..., :c - 1] = np.clip(np.round(o[..., :c - 1]), 0, 255)
+            o[..., c - 1] = np.clip(o[..., c - 1], 0.02, 2.0)   # depth metres, the last image plane
             pad = np.zeros((n,) + shape[:2])
             pad[:, 0, 0] = rng.uniform(0, 1, n)
             o[..., c] = pad

@@ -131,11 +131,11 @@ def _other_side(params, kinks):
     return sets + ([moved(kinks)] if len(kinks) > 1 else [])
 
 
-def _graph_steps_vs_oracle(cfg, params, vn, B, data_seed=9101):
+def _graph_steps_vs_oracle(cfg, params, vn, B, data_seed=9101, precision=1):
     """K_GRAPH graph-path steps; every step's outputs against the float64 oracle on the batch the device reports, from the
     parameters it held before that step (the bars of test_graph_path_ten_steps_vs_oracle_bf16x3_b256).  -> the steps' rows"""
-    tr = synth.make_transitions(NS, vn["obs_mean"], vn["obs_var"], seed=data_seed)
-    rows, _ = _run_graph_steps(cfg, params, vn, tr, B, K_GRAPH, precision=1, keep_params=True)
+    tr = synth.make_transitions(NS, vn["obs_mean"], vn["obs_var"], seed=data_seed, n_act=cfg.n_act)
+    rows, _ = _run_graph_steps(cfg, params, vn, tr, B, K_GRAPH, precision=precision, keep_params=True)
     worst = {}
     for it, (m, lb, pre) in enumerate(rows):
         assert lb["indices"].min() >= 0 and lb["indices"].max() < NS

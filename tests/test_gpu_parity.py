@@ -243,12 +243,19 @@ def test_pipelined_host_batch_path_equals_explicit_path():
     _check_pipelined_vs_explicit(16)
 
 
-def _check_pipelined_vs_explicit(B, precision=0):
-    cfg, params, vn = load_case("sac_depth")
-    batches = [make_batch(vn, B, seed=300 + i) for i in range(3)]
-    A = make_learner(cfg, vn, B, params, precision=precision)
-    Bm = make_learner(cfg, vn, B, params, precision=precision)
-    outs_a = [A.step_explicit(r["obs"], r["act"], r["rew"], r["next_obs"], r["done"], e, lr=LR) for r, _, e in batches]
+def _check_pipelined_vs_explicit(B, precision=0, cfg=None, params=None, vn=None):
+    """Three batches through both paths; the depth case's trained weights unless (cfg, params, vn) are given."""
+    if cfg is None:
+        cfg, params, vn = load_case("sac_depth")
+    batches = [make_batch(vn, B, seed=300 + i, n_act=cfg.n_act) for i in range(3)]
+    A = make_learner(cfg, vn, B, params, precision=precision, hidden=cfg.layers[0])
+    Bm = make_learner(cfg, vn, B, params, precision=precision, hidden=cfg.layers[0])
+    outs_a, well = [], {}
+    for r, _, e in batches:
+        outs_a.append(A.step_explicit(r["obs"], r["act"], r["rew"], r["next_obs"], r["done"], e, lr=LR))
+        for n, g in A.get_gradients().items():
+            ok = np.abs(g) > 1e-4 * max(1e-30, float(np.abs(g).max()))
+            well[n] = well.get(n, ok) & ok
     prev = [Bm.step_host_pipelined(r["obs"], r["act"], r["rew"], r["next_obs"], r["done"], e, lr=LR) for r, _, e in batches]
     assert prev[0] is None
     outs_b = prev[1:] + [Bm.pipeline_flush()]
@@ -257,5 +264,10 @@ def _check_pipelined_vs_explicit(B, precision=0):
             assert abs(a[k] - b[k]) <= 2e-5 * max(1.0, abs(a[k])), (k, a[k], b[k])
     pa, pb = A.get_parameters(), Bm.get_parameters()
     for n in pa:
-        assert np.abs(pa[n] - pb[n]).max() <= 1e-6 + 1e-5 * np.abs(pa[n]).max(), n
+        # Element-wise where every step's gradient is well away from zero (the rule of _check_step's update check): the
+        # engines accumulate with fp32 atomics, so two runs agree to summation-order noise (test_graph_path_fork_branches_
+        # are_race_free), and Adam's first steps turn that noise in a near-zero element into a move of up to lr.
+        d = np.abs(pa[n] - pb[n])[well.get(n, Ellipsis)]
+        bar = 1e-6 + 1e-5 * np.abs(pa[n]).max()
+        assert d.size == 0 or d.max() <= bar, (n, float(d.max()), bar)
     A.close(); Bm.close()

@@ -42,9 +42,11 @@ def test_train_cli_replay_spare_flag():
 # ---------------------------------------------------------------------------------------------------- GPU
 def _learner(obs_shape, B, cap, precision, **kw):
     import b200grasp
-    from tests.util import load_case
-    key = {(64, 64, 2): "sac_depth", (64, 64, 5): "sac_rgbd", (101,): "sac_encoder"}[tuple(obs_shape)]
-    vn = dict(np.load(os.path.join(ROOT, "tests", "golden", f"vecnorm_{key}.npz")))
+    from tests.test_gpu_configs import vecnorm_for
+    if len(obs_shape) == 1:
+        vn = dict(np.load(os.path.join(ROOT, "tests", "golden", "vecnorm_sac_encoder.npz")))
+    else:
+        vn = vecnorm_for(obs_shape[2] - 1)
     L = b200grasp.Learner(obs_shape, n_act=N_ACT, batch_size=B, buffer_size=cap, seed=11, precision=precision, **kw)
     L.set_norm_stats(vn["obs_mean"], vn["obs_var"], float(vn["ret_var"]), float(vn["clip_obs"]), float(vn["clip_reward"]),
                      float(vn["epsilon"]))
@@ -54,23 +56,24 @@ def _learner(obs_shape, B, cap, precision, **kw):
     return L
 
 
-def _fresh_obs(rng, obs_shape, n):
-    """n observations: integer RGB (channels 0-2 of RGB-D), float depth, a constant actuator plane; MLP: floats."""
+def _fresh_obs(rng, obs_shape, n, u8=()):
+    """n observations: integers 0..255 in exactly the 8-bit planes `u8`, floats in [0, 1) in the other image planes, a
+    constant actuator plane; MLP: floats."""
     if len(obs_shape) == 1:
         return rng.standard_normal((n,) + tuple(obs_shape)).astype(np.float32)
     h, w, c = obs_shape
     o = rng.random((n, h, w, c), dtype=np.float32)
-    if c == 5:
-        o[..., :3] = rng.integers(0, 256, (n, h, w, 3)).astype(np.float32)
+    if u8:
+        o[..., sorted(u8)] = rng.integers(0, 256, (n, h, w, len(u8))).astype(np.float32)
     o[..., -1] = rng.random((n, 1, 1), dtype=np.float32)
     return o
 
 
-def _episodic_stream(rng, obs_shape, lanes, calls, p_done):
+def _episodic_stream(rng, obs_shape, lanes, calls, p_done, u8=()):
     """(obs, act, rew, next_obs, done) per call: lane i's next_obs is its obs of the next call unless the episode ended."""
-    cur = _fresh_obs(rng, obs_shape, lanes)
+    cur = _fresh_obs(rng, obs_shape, lanes, u8)
     for _ in range(calls):
-        nxt = _fresh_obs(rng, obs_shape, lanes)
+        nxt = _fresh_obs(rng, obs_shape, lanes, u8)
         done = (rng.random(lanes) < p_done).astype(np.float32)
         act = rng.uniform(-1, 1, (lanes, N_ACT)).astype(np.float32)
         rew = rng.standard_normal(lanes).astype(np.float32)
@@ -78,7 +81,7 @@ def _episodic_stream(rng, obs_shape, lanes, calls, p_done):
         cur = nxt.copy()
         ends = np.nonzero(done)[0]
         if len(ends):
-            cur[ends] = _fresh_obs(rng, obs_shape, len(ends))
+            cur[ends] = _fresh_obs(rng, obs_shape, len(ends), u8)
 
 
 def _same_row(a, b):
@@ -93,6 +96,8 @@ EXACT_CASES = [
     ((64, 64, 5), 0, (0, 1, 2)),   # round-1 gather, fp32
     ((64, 64, 2), 2, ()),          # round-1 gather, bf16
     ((101,), 0, ()),               # MLP policy
+    ((64, 64, 4), 1, (0, 1, 2)),   # engine v2 gather, every image plane 8-bit (no fp32 image block), one pad channel
+    ((64, 64, 3), 1, (1,)),        # engine v2 gather, an 8-bit plane after an fp32 one, two pad channels
 ]
 
 
@@ -107,7 +112,7 @@ def test_shared_frames_sample_and_compute_what_two_frames_do(obs_shape, precisio
     dones = []
     calls = 2 * cap // lanes + 40                    # the ring wraps more than twice
     bar = 5e-3 if precision == 2 else 1e-4           # test_gpu_parity.py: the bf16 fast mode's bar, the parity bar
-    for t, (o, a, r, nx, d) in enumerate(_episodic_stream(rng, obs_shape, lanes, calls, p_done=0.04)):
+    for t, (o, a, r, nx, d) in enumerate(_episodic_stream(rng, obs_shape, lanes, calls, p_done=0.04, u8=u8)):
         ref.replay_add(o, a, r, nx, d)
         bud.replay_add(o, a, r, nx, d)
         dones.extend(d.tolist())
@@ -182,7 +187,7 @@ def test_refusals():
     cap, B = 32, 8
     L = _learner((64, 64, 5), B, cap, 0, frame_capacity=cap + cap // 8, u8_planes=(0, 1, 2))
     rng = np.random.default_rng(3)
-    o, nx = _fresh_obs(rng, (64, 64, 5), 4), _fresh_obs(rng, (64, 64, 5), 4)
+    o, nx = _fresh_obs(rng, (64, 64, 5), 4, (0, 1, 2)), _fresh_obs(rng, (64, 64, 5), 4, (0, 1, 2))
     a, r, d = np.zeros((4, N_ACT), np.float32), np.zeros(4, np.float32), np.zeros(4, np.float32)
     L.replay_add(o, a, r, nx, d)
     assert L.replay_size() == 4

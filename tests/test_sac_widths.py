@@ -115,10 +115,10 @@ def test_create_rejects_unsupported_hidden_width():
 
 def _check_step(cfg, params, vn, B, tol=TOL, precision=0):
     """One explicit step on the GPU vs the oracle (the helper of tests/test_gpu_parity.py, with the head width taken from
-    cfg.layers).  Bars: ``tol`` against float64, or 3x the fp32 oracle's own distance from float64 where fp32 arithmetic
+    cfg.layers and the action count from cfg.n_act).  Bars: ``tol`` against float64, or 3x the fp32 oracle's own distance from float64 where fp32 arithmetic
     itself does not resolve ``tol``; gradients per tensor max(10 tol, 3x fp32 oracle); the Adam / Polyak update checked on the
     GPU's own gradients."""
-    raw, norm, eps = make_batch(vn, B)
+    raw, norm, eps = make_batch(vn, B, n_act=cfg.n_act)
     L = make_learner(cfg, vn, B, params, precision=precision, hidden=cfg.layers[0])
     out = L.step_explicit(raw["obs"], raw["act"], raw["rew"], raw["next_obs"], raw["done"], eps, lr=LR, apply_update=True)
     ref, grads, newp, newopt = R.sac_step(params, R.OptState.zeros(params), norm, eps, LR, cfg, torch.float32)
@@ -169,9 +169,13 @@ def _check_step(cfg, params, vn, B, tol=TOL, precision=0):
     for n in ("model/values_fn/cnn_fc1/w", "model/pi/fc0/kernel", "model/log_ent_coef"):
         if n not in grads64:
             continue
+        # Element-wise, or 3x the fp32 oracle's own distance from the float64 update where that is larger: at saturated actions
+        # and clamped log_std fp32 does not resolve every element's gradient, and Adam's first step turns its sign into +-lr.
         well = np.abs(grads64[n]) > 1e-4 * max(1e-30, float(np.abs(grads64[n]).max()))
         d = np.abs(p2[n].astype(np.float64) - newp64[n])[well]
-        assert d.max() <= 2e-2 * LR + 1e-6 * np.abs(newp64[n]).max(), (n, d.max())
+        d32 = np.abs(np.asarray(newp[n], np.float64) - newp64[n])[well]
+        bar = np.maximum(2e-2 * LR + 1e-6 * np.abs(newp64[n]).max(), 3.0 * d32)
+        assert (d <= bar).all(), (n, d.max(), float((d / bar).max()))
     print("errs", {k: f"{v:.2e}" for k, v in errs.items()})
     print("worst grad", worst_g, f"{gerr[worst_g]:.2e} (bar {gbar[worst_g]:.2e})", "worst update/bar", f"{worst_u:.3f}")
     print(f"H={cfg.layers[0]} B={B} precision={precision} worst err/bar: outputs {max(errs[k] / bars[k] for k in errs):.3f},",

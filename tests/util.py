@@ -19,19 +19,37 @@ def load_case(key):
     return cfg, params, vn
 
 
-def make_batch(vn, B, seed=synth.DATA_SEED):
-    raw = synth.make_transitions(B, vn["obs_mean"], vn["obs_var"], seed=seed)
-    norm = dict(obs=R.normalize_obs(raw["obs"], vn["obs_mean"], vn["obs_var"]),
-                next_obs=R.normalize_obs(raw["next_obs"], vn["obs_mean"], vn["obs_var"]),
-                act=raw["act"], rew=R.normalize_reward(raw["rew"], float(vn["ret_var"])), done=raw["done"])
-    return raw, norm, synth.make_eps(B, seed=seed + 1)
+def _switch(vn, key):
+    return bool(vn[key]) if key in vn else True
+
+
+def normalize(tr, vn, idx=slice(None)):
+    """What the learner feeds the step for the raw transitions ``tr[idx]`` under the VecNormalize statistics ``vn``: its own
+    clip_obs, clip_reward and epsilon, and each of norm_obs / norm_reward (absent = on) switching its half off."""
+    clip_o, clip_r, e = float(vn["clip_obs"]), float(vn["clip_reward"]), float(vn["epsilon"])
+
+    def obs(o):
+        if not _switch(vn, "norm_obs"):
+            return np.asarray(o, np.float32)
+        return R.normalize_obs(o, vn["obs_mean"], vn["obs_var"], clip=clip_o, eps=e)
+
+    rew = tr["rew"][idx]
+    if _switch(vn, "norm_reward"):
+        rew = R.normalize_reward(rew, float(vn["ret_var"]), clip=clip_r, eps=e)
+    return dict(obs=obs(tr["obs"][idx]), next_obs=obs(tr["next_obs"][idx]), act=tr["act"][idx],
+                rew=np.asarray(rew, np.float32), done=tr["done"][idx])
+
+
+def make_batch(vn, B, seed=synth.DATA_SEED, n_act=5):
+    raw = synth.make_transitions(B, vn["obs_mean"], vn["obs_var"], seed=seed, n_act=n_act)
+    return raw, normalize(raw, vn), synth.make_eps(B, n_act=n_act, seed=seed + 1)
 
 
 def make_learner(cfg, vn, B, params=None, buffer_size=1024, precision=0, **kw):
     L = b200grasp.Learner(cfg.obs_shape, n_act=cfg.n_act, batch_size=B, buffer_size=buffer_size, gamma=cfg.gamma,
                           tau=cfg.tau, target_entropy=cfg.target_entropy, precision=precision, **kw)
     L.set_norm_stats(vn["obs_mean"], vn["obs_var"], float(vn["ret_var"]), float(vn["clip_obs"]), float(vn["clip_reward"]),
-                     float(vn["epsilon"]))
+                     float(vn["epsilon"]), norm_obs=_switch(vn, "norm_obs"), norm_reward=_switch(vn, "norm_reward"))
     if params is not None:
         L.load_parameters(params)
     return L
