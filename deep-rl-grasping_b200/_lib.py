@@ -25,6 +25,10 @@ SYMBOLS = [
     "b2g_bdq_step_explicit", "b2g_bdq_act", "b2g_bdq_set_per_beta", "b2g_bdq_get_last_per",
     "b2g_encoder_create", "b2g_encoder_destroy", "b2g_encoder_n_layers", "b2g_encoder_layer_shape", "b2g_encoder_set_weights",
     "b2g_encoder_encode", "b2g_debug_gemm",
+    "b2g_autoencoder_create", "b2g_autoencoder_destroy", "b2g_autoencoder_n_layers", "b2g_autoencoder_layer_shape",
+    "b2g_autoencoder_set_weights", "b2g_autoencoder_get_weights", "b2g_autoencoder_get_grad", "b2g_autoencoder_reset_optimizer",
+    "b2g_autoencoder_set_dataset", "b2g_autoencoder_train_epoch", "b2g_autoencoder_evaluate", "b2g_autoencoder_predict",
+    "b2g_autoencoder_step",
 ]
 
 ENC_MAX_LAYERS = 8
@@ -151,6 +155,18 @@ def load():
     lib.b2g_encoder_layer_shape.argtypes = [vp, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     lib.b2g_encoder_set_weights.argtypes = [vp, C.c_int, fp, C.c_size_t, fp, C.c_size_t]
     lib.b2g_encoder_encode.argtypes = [vp, fp, C.c_int, fp]
+    lib.b2g_autoencoder_create.argtypes = [C.POINTER(EncoderCfg), C.POINTER(vp)]
+    lib.b2g_autoencoder_destroy.argtypes = [vp]
+    lib.b2g_autoencoder_n_layers.argtypes = [vp]
+    lib.b2g_autoencoder_layer_shape.argtypes = [vp, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    for f in ("b2g_autoencoder_set_weights", "b2g_autoencoder_get_weights", "b2g_autoencoder_get_grad"):
+        getattr(lib, f).argtypes = [vp, C.c_int, fp, C.c_size_t, fp, C.c_size_t]
+    lib.b2g_autoencoder_reset_optimizer.argtypes = [vp]
+    lib.b2g_autoencoder_set_dataset.argtypes = [vp, fp, fp, C.c_int64]
+    lib.b2g_autoencoder_train_epoch.argtypes = [vp, C.POINTER(C.c_int32), C.c_int64, C.c_int, C.c_float, dp]
+    lib.b2g_autoencoder_evaluate.argtypes = [vp, C.c_int64, C.c_int64, dp]
+    lib.b2g_autoencoder_predict.argtypes = [vp, fp, C.c_int, fp]
+    lib.b2g_autoencoder_step.argtypes = [vp, fp, fp, C.c_int, C.c_float, C.c_int, dp]
     lib.b2g_debug_gemm.argtypes = [C.c_int, C.c_int, C.c_int, fp, fp, fp, C.c_int, C.c_int]
     _lib = lib
     return lib

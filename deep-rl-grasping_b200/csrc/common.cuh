@@ -47,12 +47,15 @@ enum GemmFlags : int {
   GG_A_ALIGN4 = 1 << 7,   // plane A rows are only 8-byte aligned (conv1 with one image channel)
   GG_EPI_BIAS = 1 << 10,  // C = acc + bias[n] (no activation; output layers)
   GG_EPI_SCALE = 1 << 11, // C = acc * alpha (after mask)
-  GG_A_SCALAR = 1 << 12,  // fp32 engine, with GG_A_RVEC: no 4-element contiguity along r -> element-wise gather (1-channel convs)
+  GG_A_SCALAR = 1 << 12,  // fp32 engine, with GG_A_RVEC: no 4-element contiguity along r -> element-wise gather (1-channel convs);
+                          // gg_simt_launch_ext also without GG_A_RVEC (no contiguity along m)
   GG_A_ROWLANES = 1 << 14, // planes K-major producer: lanes walk 8 consecutive rows of one 16-byte column group (conv1: adjacent
                            // output pixels overlap in the image, so a warp copy touches 4-8 lines instead of 32)
   GG_EPI_BIAS_LRELU = 1 << 13, // C = leaky_relu(acc + bias[n], slope alpha)   (Keras LeakyReLU; encoder.cu)
   GG_MN_MAJOR = 1 << 9,   // planes mode, wgrad: both operands contiguous along their M / N index -> MN-major wgmma tiles
   GG_CN_AFFINE4 = 1 << 8, // host-verified: cN / kN contiguous inside aligned 4-column groups, outputs 16-byte aligned
+  GG_EPI_LRELU_GRAD = 1 << 15, // gg_simt_launch_ext: C = acc * g(mask[kM[m] + kN[n]]), g = 1 / alpha / 0 for a post-LeakyReLU value
+                               // > 0 / < 0 / == 0 (Keras' relu(x) - alpha * relu(-x) has gradient 0 at x = 0)
 };
 
 struct GemmDesc {
@@ -92,6 +95,9 @@ struct GemmGroup {          // one grouped launch
 
 // engines (gg_simt.cu / gg_tc.cu)
 void gg_simt_launch(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaStream_t s);
+// the same engine with GG_EPI_LRELU_GRAD and m-contiguous GG_A_SCALAR gathers, summing in double, with GG_EPI_ATOMIC /
+// GG_COLSUM accumulating into double arrays behind C / colsum (auto-encoder training, autoencoder.cu)
+void gg_simt_launch_ext(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaStream_t s);
 constexpr int GG_SIMT_BM = 64, GG_SIMT_BN = 64, GG_SIMT_BK = 16;
 // wgmma engine: 128 x 64 output tile, 64-wide r-chunks; x3 != 0 -> BF16 hi/lo split (3 MMAs)
 cudaError_t gg_tc_launch(const GemmDesc* host_descs, int ndesc, int total_tiles, int mode_flags, int x3, int num_sms, cudaStream_t s);

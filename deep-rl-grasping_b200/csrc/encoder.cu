@@ -5,10 +5,9 @@
 // (manipulation_main/gripperEnv/sensor.py:218-222): Conv2D(filters, k, strides, padding='same') + LeakyReLU(alpha)
 // per entry of config.yaml's `network`, Flatten, Dense(encoding_dim), LeakyReLU(alpha).
 //
-// Every layer is one gather-GEMM on the fp32 engine (gg_simt.cu).  TensorFlow 'same' padding
-// (pad_total = max((ceil(in/s)-1)*s + k - in, 0), floor(pad_total/2) in front) is realised by keeping each layer's
-// input in a zero-bordered NHWC buffer, so the im2col offset tables need no bounds tests: layer l's epilogue
-// writes straight into the interior of layer l+1's bordered buffer.  Kernels keep Keras' HWIO layout.
+// Every layer is one gather-GEMM on the fp32 engine (gg_simt.cu).  TensorFlow 'same' padding is realised by keeping each
+// layer's input in a zero-bordered NHWC buffer (enc_tables.cuh): layer l's epilogue writes straight into the interior of
+// layer l+1's bordered buffer.  Kernels keep Keras' HWIO layout.
 #include <cuda_runtime.h>
 #include <string.h>
 
@@ -18,24 +17,12 @@
 
 #include "../../include/b200grasp.h"
 #include "common.cuh"
+#include "enc_tables.cuh"
 #include "host.cuh"
 
 using namespace b2g;
 
 namespace {
-struct EncLayer {
-  int in_h, in_w, in_c;        // logical input
-  int k, s, f;                 // kernel, stride, filters (dense: k = s = 0, f = encoding_dim)
-  int pad_t, pad_l, hp, wp;    // bordered input geometry
-  int out_h, out_w;
-  int fs;                      // filter stride of the stored kernel (f rounded up to 4)
-  float* in = nullptr;         // bordered input  [N, hp, wp, in_c]
-  float* w = nullptr;          // [R, fs]
-  float* b = nullptr;          // [fs]
-  bool loaded = false;
-  int R() const { return k ? k * k * in_c : in_h * in_w * in_c; }
-};
-
 __global__ void enc_pad_copy(const float* __restrict__ src, float* __restrict__ dst, int n, int h, int w, int c, int hp, int wp,
                              int pt, int pl) {
   const long long total = (long long)n * h * w * c;
@@ -81,25 +68,9 @@ int build_tables(b2g_encoder* h) {
       out = nx.in; o_hp = nx.hp; o_wp = nx.wp; o_pt = nx.pad_t; o_pl = nx.pad_l; o_c = y.f;
     }
     const int M = N * y.out_h * y.out_w, R = y.R();
-    std::vector<int> aM(M), cM(M), aR(R), bR(R), bN(y.f), cN(y.f);
-    for (int b = 0; b < N; ++b)
-      for (int oy = 0; oy < y.out_h; ++oy)
-        for (int ox = 0; ox < y.out_w; ++ox) {
-          const int m = (b * y.out_h + oy) * y.out_w + ox;
-          aM[m] = dense ? b * R : ((b * y.hp + oy * y.s) * y.wp + ox * y.s) * y.in_c;
-          cM[m] = ((b * o_hp + oy + o_pt) * o_wp + ox + o_pl) * o_c;
-        }
-    for (int r = 0; r < R; ++r) {
-      if (dense) aR[r] = r;
-      else {
-        const int c = r % y.in_c, kx = (r / y.in_c) % y.k, ky = r / (y.in_c * y.k);
-        aR[r] = (ky * y.wp + kx) * y.in_c + c;
-      }
-      bR[r] = r * y.fs;
-    }
-    for (int n = 0; n < y.f; ++n) bN[n] = cN[n] = n;
-    GemmDesc d = gemm_desc(y.in, nullptr, nullptr, y.w, nullptr, nullptr, out, nullptr, nullptr, M, y.f, R,
-                           GG_A_RVEC | GG_EPI_BIAS_LRELU | ((y.in_c & 3) && !dense ? GG_A_SCALAR : 0));
+    std::vector<int> aM, cM, aR, bR, bN, cN;
+    enc_fwd_tables(y, N, o_hp, o_wp, o_pt, o_pl, o_c, aM, cM, aR, bR, bN, cN);
+    GemmDesc d = gemm_desc(y.in, nullptr, nullptr, y.w, nullptr, nullptr, out, nullptr, nullptr, M, y.f, R, enc_fwd_flags(y));
     d.bias = y.b; d.alpha = h->cfg.alpha;
     if (int rc = upload_table(h->allocs, h->stream, aM, &d.aM)) return rc;
     if (int rc = upload_table(h->allocs, h->stream, aR, &d.aR)) return rc;
@@ -140,24 +111,8 @@ int b2g_encoder_create(const b2g_encoder_cfg* cfg, b2g_encoder** out) {
   h->cfg = *cfg;
   auto bail = [&](int rc) { b2g_encoder_destroy(h); return rc; };
   if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream create"));
-  int ih = cfg->height, iw = cfg->width, ic = cfg->channels;
-  for (int l = 0; l < cfg->n_layers; ++l) {
-    EncLayer y{};
-    y.in_h = ih; y.in_w = iw; y.in_c = ic; y.k = cfg->kernel[l]; y.s = cfg->strides[l]; y.f = cfg->filters[l];
-    if (y.k < 1 || y.s < 1 || y.f < 1) return bail(b2g_fail(B2G_EINVAL, "bad conv layer spec"));
-    y.out_h = (ih + y.s - 1) / y.s; y.out_w = (iw + y.s - 1) / y.s;
-    const int ph = std::max((y.out_h - 1) * y.s + y.k - ih, 0), pw = std::max((y.out_w - 1) * y.s + y.k - iw, 0);
-    y.pad_t = ph / 2; y.pad_l = pw / 2; y.hp = ih + ph; y.wp = iw + pw;
-    y.fs = (y.f + 3) / 4 * 4;
-    if (l > 0 && (ic & 3)) return bail(b2g_fail(B2G_EINVAL, "hidden conv layers need filters % 4 == 0"));
-    h->layers.push_back(y);
-    ih = y.out_h; iw = y.out_w; ic = y.f;
-  }
-  EncLayer dn{};
-  dn.in_h = ih; dn.in_w = iw; dn.in_c = ic; dn.k = dn.s = 0; dn.f = cfg->encoding_dim; dn.out_h = dn.out_w = 1;
-  dn.hp = ih; dn.wp = iw; dn.fs = (dn.f + 3) / 4 * 4;
-  if ((ih * iw * ic) & 3) return bail(b2g_fail(B2G_EINVAL, "flattened feature size must be a multiple of 4"));
-  h->layers.push_back(dn);
+  if (int rc = enc_geometry(*cfg, h->layers)) return bail(rc);
+  const EncLayer& dn = h->layers.back();
   const size_t N = cfg->max_batch;
   if (N * (size_t)h->layers[0].hp * h->layers[0].wp * cfg->channels > (1ull << 31) - 1 ||
       N * (size_t)h->layers[0].out_h * h->layers[0].out_w * h->layers[0].fs > (1ull << 31) - 1)

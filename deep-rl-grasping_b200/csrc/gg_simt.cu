@@ -6,6 +6,8 @@
 // Tile: 64(m) x 64(n) x 16(r), 256 threads, 4x4 outputs per thread, register-prefetched smem.
 #include <cuda_bf16.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace b2g {
@@ -14,11 +16,18 @@ constexpr int BM = GG_SIMT_BM, BN = GG_SIMT_BN, BK = GG_SIMT_BK, PAD = 4;
 
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
+// EXT: the auto-encoder's variant, which adds element-wise m-contiguous A gathers (GG_A_SCALAR without GG_A_RVEC) and the
+// GG_EPI_LRELU_GRAD epilogue, and sums in double: fp32 products are exact in double, so a long reduction whose terms cancel
+// (a weight or bias gradient over every pixel of a batch) keeps its accuracy; its GG_EPI_ATOMIC and GG_COLSUM destinations
+// are double arrays (C and colsum reinterpreted), accumulated without rounding to fp32.  The plain instantiation is the
+// engine every other path launches, unchanged.
+template <bool EXT>
 __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict__ descs, int ndesc) {
   __shared__ GemmDesc sd;
   __shared__ __align__(16) float As[BK][BM + PAD];
   __shared__ __align__(16) float Bs[BK][BN + PAD];
-  __shared__ float cs[BN];
+  using Acc = typename std::conditional<EXT, double, float>::type;
+  __shared__ Acc cs[BN];
   const int tid = threadIdx.x;
   if (tid == 0) {
     int p = 0;
@@ -26,7 +35,7 @@ __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict
     while (p + 1 < ndesc && t >= descs[p + 1].tile_start) ++p;
     sd = descs[p];
   }
-  if (tid < BN) cs[tid] = 0.f;
+  if (tid < BN) cs[tid] = 0;
   pdl_trigger();
   pdl_wait();
   __syncthreads();
@@ -82,7 +91,7 @@ __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict
   }
 
   float4 ra = make_float4(0, 0, 0, 0), rb = make_float4(0, 0, 0, 0);
-  float4 csum = make_float4(0, 0, 0, 0);
+  Acc csum[4] = {0, 0, 0, 0};
 
   auto load_tiles = [&](int rk) {
     // ---- A
@@ -104,7 +113,7 @@ __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict
       ra = make_float4(0, 0, 0, 0);
       if (r < r_end) {
         const int ar = d.aR[r];
-        if (a_ok[3]) {
+        if (a_ok[3] && !(EXT && a_scalar)) {
           ra = ld4(A + a_off[0] + ar);
         } else {
           float v[4] = {0, 0, 0, 0};
@@ -157,16 +166,16 @@ __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict
       Bs[b_r + 0][b_n] = rb.x; Bs[b_r + 1][b_n] = rb.y; Bs[b_r + 2][b_n] = rb.z; Bs[b_r + 3][b_n] = rb.w;
     } else {
       *reinterpret_cast<float4*>(&Bs[b_r][b_n]) = rb;
-      if (do_colsum) { csum.x += rb.x; csum.y += rb.y; csum.z += rb.z; csum.w += rb.w; }
+      if (do_colsum) { csum[0] += rb.x; csum[1] += rb.y; csum[2] += rb.z; csum[3] += rb.w; }
     }
   };
 
   const int tx = tid & 15, ty = tid >> 4;
-  float acc[4][4];
+  Acc acc[4][4];
 #pragma unroll
   for (int i = 0; i < 4; ++i)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0;
 
   if (r_begin < r_end) load_tiles(r_begin);
   for (int rk = r_begin; rk < r_end; rk += BK) {
@@ -181,7 +190,10 @@ __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+        for (int j = 0; j < 4; ++j) {
+          if constexpr (EXT) acc[i][j] = fma((double)av[i], (double)bv[j], acc[i][j]);
+          else acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+        }
     }
     __syncthreads();
   }
@@ -193,13 +205,13 @@ __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict
     const int m = m0 + ty * 4 + i;
     if (m >= d.M) continue;
     const int cm = d.cM[m];
-    const int km = (d.flags & GG_EPI_MASK) ? (d.kM ? d.kM[m] : cm) : 0;
+    const int km = (d.flags & (EXT ? GG_EPI_MASK | GG_EPI_LRELU_GRAD : GG_EPI_MASK)) ? (d.kM ? d.kM[m] : cm) : 0;
     float v[4];
     int co[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int n = nb + j;
-      v[j] = acc[i][j];
+      v[j] = (float)acc[i][j];
       co[j] = -1;
       if (n < d.N) {
         const int cn = d.cN[n];
@@ -213,6 +225,10 @@ __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict
         if (d.flags & GG_EPI_MASK) {
           const int kn = d.kN ? d.kN[n] : cn;
           v[j] = d.mask[km + kn] > 0.f ? v[j] : 0.f;
+        }
+        if (EXT && (d.flags & GG_EPI_LRELU_GRAD)) {
+          const float a = d.mask[km + (d.kN ? d.kN[n] : cn)];
+          v[j] *= a > 0.f ? 1.f : (a < 0.f ? d.alpha : 0.f);
         }
         if (d.flags & GG_EPI_SCALE) v[j] *= d.alpha;
       }
@@ -229,7 +245,10 @@ __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict
     if (d.flags & GG_EPI_ATOMIC) {
 #pragma unroll
       for (int j = 0; j < 4; ++j)
-        if (co[j] >= 0) atomicAdd(d.C + co[j], v[j]);
+        if (co[j] >= 0) {
+          if constexpr (EXT) atomicAdd(reinterpret_cast<double*>(d.C) + co[j], acc[i][j]);
+          else atomicAdd(d.C + co[j], v[j]);
+        }
     } else if (co[3] >= 0 && co[1] == co[0] + 1 && co[2] == co[0] + 2 && co[3] == co[0] + 3 && (co[0] & 3) == 0) {
       *reinterpret_cast<float4*>(d.C + co[0]) = make_float4(v[0], v[1], v[2], v[3]);
     } else {
@@ -239,17 +258,25 @@ __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict
     }
   }
   if (do_colsum) {   // block-uniform branch
-    atomicAdd(&cs[b_n + 0], csum.x); atomicAdd(&cs[b_n + 1], csum.y);
-    atomicAdd(&cs[b_n + 2], csum.z); atomicAdd(&cs[b_n + 3], csum.w);
+    atomicAdd(&cs[b_n + 0], csum[0]); atomicAdd(&cs[b_n + 1], csum[1]);
+    atomicAdd(&cs[b_n + 2], csum[2]); atomicAdd(&cs[b_n + 3], csum[3]);
     __syncthreads();
-    if (tid < BN && n0 + tid < d.N) atomicAdd(d.colsum + n0 + tid, cs[tid]);
+    if (tid < BN && n0 + tid < d.N) {
+      if constexpr (EXT) atomicAdd(reinterpret_cast<double*>(d.colsum) + n0 + tid, cs[tid]);
+      else atomicAdd(d.colsum + n0 + tid, cs[tid]);
+    }
   }
 }
 }  // namespace
 
 void gg_simt_launch(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaStream_t s) {
   if (total_tiles <= 0) return;
-  launch_pdl(gg_simt_kernel, dim3(total_tiles), dim3(256), 0, s, pdl_enabled(), dev_descs, ndesc);
+  launch_pdl(gg_simt_kernel<false>, dim3(total_tiles), dim3(256), 0, s, pdl_enabled(), dev_descs, ndesc);
+}
+
+void gg_simt_launch_ext(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaStream_t s) {
+  if (total_tiles <= 0) return;
+  gg_simt_kernel<true><<<total_tiles, 256, 0, s>>>(dev_descs, ndesc);
 }
 
 }  // namespace b2g

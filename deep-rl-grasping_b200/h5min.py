@@ -146,3 +146,211 @@ def load_keras_weights(path: str) -> Dict[str, np.ndarray]:
         if parts[-1].endswith(":0") and len(parts) >= 2:
             out[parts[-2] + "/" + parts[-1][:-2]] = v
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------- attributes
+def _attr_value(f: H5File, body: int):
+    """Decodes one attribute message (version 1): fixed- or variable-length strings and float arrays."""
+    ver, nsz, tsz, ssz = f.b[body], f._u16(body + 2), f._u16(body + 4), f._u16(body + 6)
+    if ver != 1:
+        raise NotImplementedError(f"attribute message version {ver}")
+    pad = lambda n: (n + 7) // 8 * 8
+    name = f.b[body + 8:body + 8 + nsz - 1].decode()
+    t = body + 8 + pad(nsz)
+    s = t + pad(tsz)
+    d = s + pad(ssz)
+    rank = f.b[s + 1]
+    shape = tuple(f._u64(s + 8 + 8 * i) for i in range(rank))
+    n = int(np.prod(shape)) if shape else 1
+    cls, size = f.b[t] & 0x0F, f._u32(t + 4)
+    if cls == 3:                                   # fixed-length string
+        vals = [f.b[d + i * size:d + (i + 1) * size].rstrip(b"\x00") for i in range(n)]
+    elif cls == 9:                                 # variable-length string: (length, global heap address, object index)
+        vals = []
+        for i in range(n):
+            q = d + 16 * i
+            ln, gaddr, idx = f._u32(q), f._u64(q + 4), f._u32(q + 12)
+            vals.append(_global_heap_object(f, gaddr, idx)[:ln])
+    elif cls == 1:
+        dt = {4: np.float32, 8: np.float64}[size]
+        return name, np.frombuffer(f.b, dtype=dt, count=n, offset=d).reshape(shape).copy()
+    else:
+        raise NotImplementedError(f"attribute datatype class {cls}")
+    return name, (vals if shape else vals[0])
+
+
+def _global_heap_object(f: H5File, addr: int, index: int) -> bytes:
+    assert f.b[addr:addr + 4] == b"GCOL"
+    size = f._u64(addr + 8)
+    p, end = addr + 16, addr + size
+    while p + 16 <= end:
+        idx, osz = f._u16(p), f._u64(p + 8)
+        if idx == index:
+            return f.b[p + 16:p + 16 + osz]
+        if idx == 0:
+            break
+        p += 16 + (osz + 7) // 8 * 8
+    raise ValueError(f"global heap object {index} not found")
+
+
+def read_structure(path: str):
+    """{'/': attrs, 'encoder': attrs, 'encoder/conv2d_1/kernel:0': (shape, dtype), ...}: every group with its attributes
+    (names -> values; strings as bytes) and every dataset with its shape and dtype."""
+    f = H5File(path)
+    out = {}
+
+    def walk(hdr, cached, prefix):
+        msgs = f._messages(hdr)
+        ch = f._children(hdr, cached)
+        if ch is None:
+            d = f._dataset(hdr)
+            if d is not None:
+                out[prefix] = (d.shape, d.dtype)
+            return
+        out[prefix or "/"] = dict(_attr_value(f, body) for t, body, _ in msgs if t == 0x0C)
+        for name, (h2, c2) in ch.items():
+            walk(h2, c2, f"{prefix}/{name}" if prefix else name)
+    walk(f.root_header, (f.root_btree, f.root_heap), "")
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------------- writer
+_UNDEF = 0xFFFFFFFFFFFFFFFF
+_LEAF_K, _NODE_K = 4, 16                # symbol-node and group B-tree K, as libhdf5 writes them
+
+
+class _Writer:
+    """Superblock 0 / object header 1 / symbol-table groups / contiguous datasets: the subset Keras 2.2.4's save_weights
+    produced (h5py on libhdf5 1.10 with default settings).  Strings are stored as fixed-length, null-padded arrays."""
+
+    def __init__(self):
+        self.buf = bytearray(96)        # superblock, patched at the end
+
+    def alloc(self, data: bytes) -> int:
+        addr = len(self.buf)
+        self.buf += data
+        self.buf += b"\x00" * (-len(self.buf) % 8)
+        return addr
+
+    @staticmethod
+    def _msg(t: int, body: bytes) -> bytes:
+        body += b"\x00" * (-len(body) % 8)
+        return struct.pack("<HHB3x", t, len(body), 0) + body
+
+    def header(self, msgs) -> int:
+        body = b"".join(msgs)
+        return self.alloc(struct.pack("<BBHII4x", 1, 0, len(msgs), 1, len(body)) + body)
+
+    @staticmethod
+    def _space(shape) -> bytes:
+        dims = b"".join(struct.pack("<Q", d) for d in shape)
+        return struct.pack("<BBB5x", 1, len(shape), 1 if shape else 0) + dims + (dims if shape else b"")
+
+    @staticmethod
+    def _ftype(size: int) -> bytes:
+        if size == 4:
+            return bytes.fromhex("11201f00") + struct.pack("<I", 4) + bytes.fromhex("00002000170800177f000000")
+        return bytes.fromhex("11203f00") + struct.pack("<I", 8) + bytes.fromhex("00004000340b0034ff030000")
+
+    def _attr(self, name: str, value) -> bytes:
+        nm = name.encode() + b"\x00"
+        if isinstance(value, np.ndarray):
+            a = np.ascontiguousarray(value, dtype=value.dtype.newbyteorder("<"))
+            dtype, space, data = self._ftype(a.dtype.itemsize), self._space(a.shape), a.tobytes()
+        else:
+            vals = [value] if isinstance(value, bytes) else list(value)
+            size = max([len(v) for v in vals] + [1])
+            dtype = struct.pack("<BBBBI", 0x13, 0x01, 0, 0, size)
+            space = self._space(() if isinstance(value, bytes) else (len(vals),))
+            data = b"".join(v.ljust(size, b"\x00") for v in vals)
+        pad = lambda b: b + b"\x00" * (-len(b) % 8)
+        body = struct.pack("<BBHHH", 1, 0, len(nm), len(dtype), len(space)) + pad(nm) + pad(dtype) + pad(space) + data
+        return self._msg(0x0C, body)
+
+    def dataset(self, arr: np.ndarray) -> int:
+        a = np.ascontiguousarray(arr, dtype=arr.dtype.newbyteorder("<"))
+        addr = self.alloc(a.tobytes())
+        msgs = [self._msg(0x01, self._space(a.shape)), self._msg(0x03, self._ftype(a.dtype.itemsize)),
+                self._msg(0x05, bytes.fromhex("0202020100000000")),
+                self._msg(0x08, struct.pack("<BBQQ", 3, 1, addr, a.nbytes))]
+        return self.header(msgs)
+
+    def group(self, children, attrs=()):
+        """children: {name: (header address, (btree, heap) or None)}.  Returns (header, btree, heap)."""
+        names = sorted(children)
+        heap_data = bytearray(8)                   # offset 0: the empty name
+        offs = {}
+        for n in names:
+            offs[n] = len(heap_data)
+            heap_data += n.encode() + b"\x00"
+            heap_data += b"\x00" * (-len(heap_data) % 8)
+        data_addr = self.alloc(bytes(heap_data))
+        heap = self.alloc(b"HEAP" + bytes(4) + struct.pack("<QQQ", len(heap_data), _UNDEF, data_addr))
+        snods, keys = [], [0]
+        for i in range(0, max(len(names), 1), 2 * _LEAF_K):
+            chunk = names[i:i + 2 * _LEAF_K]
+            ents = b""
+            for n in chunk:
+                hdr, cache = children[n]
+                ents += struct.pack("<QQII", offs[n], hdr, 1 if cache else 0, 0) + (struct.pack("<QQ", *cache) if cache else bytes(16))
+            ents += bytes(40 * (2 * _LEAF_K - len(chunk)))
+            snods.append(self.alloc(b"SNOD" + struct.pack("<BBH", 1, 0, len(chunk)) + ents))
+            keys.append(offs[chunk[-1]] if chunk else 0)
+        if len(snods) > 2 * _NODE_K:
+            raise NotImplementedError("group too large for one B-tree node")
+        node = b"TREE" + struct.pack("<BBHQQ", 0, 0, len(snods), _UNDEF, _UNDEF)
+        for i, s in enumerate(snods):
+            node += struct.pack("<QQ", keys[i], s)
+        node += struct.pack("<Q", keys[len(snods)])
+        node += bytes(8 * (2 * _NODE_K + 1) + 8 * 2 * _NODE_K - (len(node) - 24))
+        btree = self.alloc(node)
+        msgs = [self._msg(0x11, struct.pack("<QQ", btree, heap))] + [self._attr(k, v) for k, v in attrs]
+        return self.header(msgs), btree, heap
+
+    def finish(self, root) -> bytes:
+        hdr, btree, heap = root
+        sb = b"\x89HDF\r\n\x1a\n" + bytes([0, 0, 0, 0, 0, 8, 8, 0]) + struct.pack("<HHI", _LEAF_K, _NODE_K, 0)
+        sb += struct.pack("<QQQQ", 0, _UNDEF, len(self.buf), _UNDEF)
+        sb += struct.pack("<QQII", 0, hdr, 1, 0) + struct.pack("<QQ", btree, heap)
+        assert len(sb) == 96
+        self.buf[:96] = sb
+        return bytes(self.buf)
+
+
+def write_keras_weights(path: str, layers) -> None:
+    """Writes a Keras 2.2.4 ``save_weights`` file of a model whose top-level layers are ``layers``:
+    [(layer name, [(weight name, array), ...])], e.g. ('encoder', [('conv2d_1/kernel:0', k), ...]); a layer without weights
+    gets an empty ``weight_names``.  Root attributes: layer_names, backend = tensorflow, keras_version = 2.2.4."""
+    w = _Writer()
+    top = {}
+    for lname, weights in layers:
+        # nested groups for 'sub/name:0' paths
+        tree = {}
+        for wname, arr in weights:
+            parts = wname.split("/")
+            node = tree
+            for p in parts[:-1]:
+                node = node.setdefault(p, {})
+            node[parts[-1]] = w.dataset(np.asarray(arr))
+
+        def build(node, attrs=()):
+            ch = {}
+            for k, v in node.items():
+                if isinstance(v, dict):
+                    hdr, bt, hp = build(v)
+                    ch[k] = (hdr, (bt, hp))
+                else:
+                    ch[k] = (v, None)
+            return w.group(ch, attrs)
+        names = [n.encode() for n, _ in weights]
+        wn = names if names else np.zeros((0,), np.float64)
+        hdr, bt, hp = build(tree, [("weight_names", wn)])
+        top[lname] = (hdr, (bt, hp))
+    root = w.group(top, [("layer_names", [n.encode() for n, _ in layers]), ("backend", b"tensorflow"),
+                         ("keras_version", b"2.2.4")])
+    data = w.finish(root)
+    tmp = path + ".tmp"
+    with open(tmp, "wb") as fh:
+        fh.write(data)
+    import os
+    os.replace(tmp, path)

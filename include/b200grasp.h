@@ -271,6 +271,41 @@ int b2g_encoder_set_weights(b2g_encoder* h, int layer, const float* kernel, size
 int b2g_encoder_encode(b2g_encoder* h, const float* imgs, int n, float* out);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Auto-encoder TRAINING (encoders.py:40-61 train / test / predict, graph :84-136): the full Keras model
+ * encoder -> decoder on one handle, trained with mean_squared_error and Keras Adam (eps 1e-7) in fp32 on the GPU.
+ * Decoder: Dense(h*w*c) + LeakyReLU, Reshape, then for i = L-1..1 UpSampling2D(strides_i) + Conv2D(filters_{i-1},
+ * kernel_i, 'same') + LeakyReLU, then UpSampling2D(strides_0) + Conv2D(1, kernel_0, 'same').
+ * Layers are numbered in model.h5 order: encoder convs, encoder dense, decoder dense, decoder convs, output conv
+ * (2 * n_layers + 2); weights use the Keras layouts of b2g_encoder_set_weights.  Requires channels == 1, every filter
+ * count a multiple of 4 and a decoder that returns to height x width (else B2G_EINVAL).  max_batch is the largest
+ * batch of any call.  Calls that run the model return B2G_ESTATE until every layer has weights.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct b2g_autoencoder b2g_autoencoder;
+int b2g_autoencoder_create(const b2g_encoder_cfg* cfg, b2g_autoencoder** out);
+int b2g_autoencoder_destroy(b2g_autoencoder* h);
+int b2g_autoencoder_n_layers(const b2g_autoencoder* h);
+int b2g_autoencoder_layer_shape(const b2g_autoencoder* h, int layer, int64_t* kernel_numel, int64_t* bias_numel);
+int b2g_autoencoder_set_weights(b2g_autoencoder* h, int layer, const float* kernel, size_t kernel_numel, const float* bias,
+                                size_t bias_numel);
+int b2g_autoencoder_get_weights(b2g_autoencoder* h, int layer, float* kernel, size_t kernel_numel, float* bias, size_t bias_numel);
+/* gradients of the last b2g_autoencoder_step (mean squared error over the batch) */
+int b2g_autoencoder_get_grad(b2g_autoencoder* h, int layer, float* kernel, size_t kernel_numel, float* bias, size_t bias_numel);
+/* zeroes Adam's moments and its step count */
+int b2g_autoencoder_reset_optimizer(b2g_autoencoder* h);
+/* copies n images [n, height, width, 1] to the device; targets == NULL trains towards the inputs themselves */
+int b2g_autoencoder_set_dataset(b2g_autoencoder* h, const float* inputs, const float* targets, int64_t n);
+/* one pass over dataset rows order[0..n_order) in batches of `batch` (the last one may be partial): one Adam step per batch;
+ * *mean_loss = sample-weighted mean of the batch losses, each taken before its update */
+int b2g_autoencoder_train_epoch(b2g_autoencoder* h, const int32_t* order, int64_t n_order, int batch, float lr, double* mean_loss);
+/* mean squared error over dataset rows [start, start + count) */
+int b2g_autoencoder_evaluate(b2g_autoencoder* h, int64_t start, int64_t count, double* mean_loss);
+/* imgs: host [n, height, width, 1] -> out: host [n, height, width, 1] reconstructions */
+int b2g_autoencoder_predict(b2g_autoencoder* h, const float* imgs, int n, float* out);
+/* one step on a host batch (targets == NULL: the inputs); apply_update == 0 only computes loss and gradients */
+int b2g_autoencoder_step(b2g_autoencoder* h, const float* inputs, const float* targets, int n, float lr, int apply_update,
+                         double* loss);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Bring-up hook (not on the product path): C[M,N] = A[M,K] * B[N,K]^T through the wgmma engine; host pointers,
  * K a multiple of 8; x3 != 0 -> BF16 hi/lo split (3 MMAs); split_k > 1 -> that many partial accumulators summed
  * with fp32 atomics.  tools/tc_accum_probe.py uses it to measure the accumulation behaviour of the tensor core.
