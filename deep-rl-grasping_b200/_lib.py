@@ -12,6 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200grasp.so")
 
 B2G_PREC_FP32_SIMT, B2G_PREC_BF16X3, B2G_PREC_BF16 = 0, 1, 2
+B2G_EINVAL, B2G_ECUDA, B2G_ESTATE = -1, -2, -3
 
 #: every symbol include/b200grasp.h declares (tests check the .so exports each of them)
 SYMBOLS = [
@@ -19,10 +20,10 @@ SYMBOLS = [
     "b2g_sac_create2", "b2g_param_count", "b2g_param_info", "b2g_get_param", "b2g_set_param", "b2g_get_grad", "b2g_get_adam",
     "b2g_reset_optimizer", "b2g_replay_add", "b2g_replay_size", "b2g_replay_get", "b2g_replay_info", "b2g_get_last_batch", "b2g_set_norm_stats", "b2g_sac_step",
     "b2g_sac_step_async", "b2g_sac_step_explicit", "b2g_sac_step_host_pipelined", "b2g_sac_pipeline_flush", "b2g_sac_act", "b2g_launches_per_step", "b2g_last_step_ms",
-    "b2g_profile_step",
+    "b2g_profile_step", "b2g_sac_state_save", "b2g_sac_state_load",
     "b2g_bdq_create", "b2g_bdq_destroy", "b2g_bdq_param_count", "b2g_bdq_param_info", "b2g_bdq_get_param", "b2g_bdq_set_param",
     "b2g_bdq_get_grad", "b2g_bdq_replay_add", "b2g_bdq_replay_size", "b2g_bdq_set_norm_stats", "b2g_bdq_step",
-    "b2g_bdq_step_explicit", "b2g_bdq_act", "b2g_bdq_set_per_beta", "b2g_bdq_get_last_per",
+    "b2g_bdq_step_explicit", "b2g_bdq_act", "b2g_bdq_set_per_beta", "b2g_bdq_get_last_per", "b2g_bdq_state_save", "b2g_bdq_state_load",
     "b2g_encoder_create", "b2g_encoder_destroy", "b2g_encoder_n_layers", "b2g_encoder_layer_shape", "b2g_encoder_set_weights",
     "b2g_encoder_encode", "b2g_debug_gemm",
     "b2g_autoencoder_create", "b2g_autoencoder_destroy", "b2g_autoencoder_n_layers", "b2g_autoencoder_layer_shape",
@@ -84,7 +85,9 @@ class SacMetrics(C.Structure):
 
 
 class B2GError(RuntimeError):
-    pass
+    def __init__(self, msg, code=None):
+        super().__init__(msg)
+        self.code = code
 
 
 _lib = None
@@ -134,6 +137,8 @@ def load():
     lib.b2g_last_step_ms.argtypes = [vp]
     lib.b2g_last_step_ms.restype = C.c_float
     lib.b2g_profile_step.argtypes = [vp, C.c_float, C.POINTER(C.c_char_p), fp, C.c_int]
+    for f in ("b2g_sac_state_save", "b2g_sac_state_load", "b2g_bdq_state_save", "b2g_bdq_state_load"):
+        getattr(lib, f).argtypes = [vp, C.c_char_p]
     lib.b2g_bdq_create.argtypes = [C.POINTER(BdqCfg), C.POINTER(vp)]
     lib.b2g_bdq_destroy.argtypes = [vp]
     lib.b2g_bdq_param_count.argtypes = [vp]
@@ -174,7 +179,7 @@ def load():
 
 def check(rc: int):
     if rc < 0:
-        raise B2GError(f"libb200grasp error {rc}: {load().b2g_last_error().decode(errors='replace')}")
+        raise B2GError(f"libb200grasp error {rc}: {load().b2g_last_error().decode(errors='replace')}", rc)
     return rc
 
 

@@ -16,7 +16,7 @@ from typing import Optional
 
 import numpy as np
 
-from . import _lib, sb_io
+from . import _lib, sb_io, training_state
 from .callbacks import as_callback
 from .learner import _f32, _fp
 from .vec_env import DummyVecEnv
@@ -110,6 +110,14 @@ class BDQLearner:
 
     def replay_size(self):
         return int(self.lib.b2g_bdq_replay_size(self.h))
+
+    def save_state(self, path: str):
+        """Parameters, Adam moments, counters, the live replay rows and the prioritised-replay trees -> ``path``."""
+        _lib.check(self.lib.b2g_bdq_state_save(self.h, os.fsencode(path)))
+
+    def load_state(self, path: str):
+        """Restores a ``save_state`` file into this learner, which must have the same configuration."""
+        _lib.check(self.lib.b2g_bdq_state_load(self.h, os.fsencode(path)))
 
     def step(self, n_steps=1, lr=1e-4):
         m = _lib.BdqMetrics()
@@ -211,8 +219,12 @@ class BDQ:
         obs = self.env.reset()
         n_env, D = self.env.num_envs, self.learner.n_branches
         lr = self.learning_rate if not callable(self.learning_rate) else self.learning_rate(1.0)
+        # reset_num_timesteps=False continues a run: epsilon and beta follow num_timesteps over the schedule of a run that ends
+        # total_timesteps from now (the stable-baselines DQN rule)
+        resume = not reset_num_timesteps
+        horizon = self.num_timesteps + total_timesteps if resume else total_timesteps
         for t in range(0, total_timesteps, n_env):
-            eps = self._epsilon(t, total_timesteps)
+            eps = self._epsilon(self.num_timesteps if resume else t, horizon)
             idx = self.learner.act(np.asarray(obs, np.float32))
             explore = self._rng.random((n_env, D)) < eps                       # independent epsilon-greedy per branch
             idx = np.where(explore, self._rng.integers(0, self.num_actions_pad, (n_env, D)), idx)
@@ -229,7 +241,7 @@ class BDQ:
             if self.num_timesteps > self.learning_starts and self.num_timesteps % self.train_freq == 0 and \
                     self.learner.replay_size() >= self.batch_size:
                 if self.prioritized_replay:          # [SB2] LinearSchedule(beta_iters, initial_p=beta0, final_p=1.0)
-                    iters = self.per_beta_iters or total_timesteps
+                    iters = self.per_beta_iters or horizon
                     self.learner.set_per_beta(self.per_beta0 + min(1.0, self.num_timesteps / iters) * (1.0 - self.per_beta0))
                 self.learner.step(1, lr)
         callback.on_training_end()
@@ -260,6 +272,45 @@ class BDQ:
                 "prioritized_replay_alpha": self.per_alpha, "prioritized_replay_beta0": self.per_beta0, "double_q": True,
                 "epsilon_greedy": True, "policy_kwargs": {"layers": self.layers}}
         sb_io.save_sb_zip(save_path, data, self.learner.get_parameters())
+
+    def get_vec_normalize_env(self):
+        from .sac_model import unwrap_vec_normalize
+        return unwrap_vec_normalize(self.env)
+
+    # ------------------------------------------------------------------ training state (training_state.py)
+    def _host_state(self):
+        if callable(self.learning_rate):
+            raise NotImplementedError("save_training_state needs a constant learning_rate")
+        init = dict(gamma=self.gamma, learning_rate=self.learning_rate, buffer_size=self.buffer_size,
+                    exploration_fraction=self.exploration_fraction, exploration_final_eps=self.exploration_final_eps,
+                    train_freq=self.train_freq, batch_size=self.batch_size, learning_starts=self.learning_starts,
+                    target_network_update_freq=self.target_network_update_freq, num_actions_pad=self.num_actions_pad,
+                    prioritized_replay=self.prioritized_replay, prioritized_replay_alpha=self.per_alpha,
+                    prioritized_replay_beta0=self.per_beta0, prioritized_replay_beta_iters=self.per_beta_iters,
+                    prioritized_replay_eps=self.per_eps, policy_kwargs=self.policy_kwargs, verbose=self.verbose, seed=self.seed,
+                    device=self.device)
+        return {"algo": "BDQ", "init": init, "num_timesteps": int(self.num_timesteps), "rng": training_state.rng_state(self._rng)}
+
+    def save_training_state(self, path):
+        """Writes directory ``path``: model.zip, learner.state (parameters, Adam moments, counters, the replay and its
+        priority trees), vecnormalize.pkl and host.json.  The previous contents stay loadable until the new one is complete."""
+        return training_state.save_training_state(self, path)
+
+    @classmethod
+    def load_training_state(cls, path, env, **kwargs):
+        """Rebuilds the model ``save_training_state`` wrote into ``path`` on ``env``; ``learn(n, reset_num_timesteps=False)``
+        then continues with epsilon and beta taken from ``num_timesteps``."""
+        path = training_state.resolve(path)
+        host = training_state.read_host(path)
+        if host.get("algo") != "BDQ":
+            raise ValueError(f"{path} holds a {host.get('algo')} training state")
+        model = cls("MlpActPolicy", env, **dict(host["init"], **kwargs))
+        training_state.restore_vec_normalize(path, model.env)
+        model.load_parameters(os.path.join(path, training_state.MODEL_FILE))
+        model.learner.load_state(os.path.join(path, training_state.STATE_FILE))
+        model.num_timesteps = int(host["num_timesteps"])
+        training_state.set_rng_state(model._rng, host["rng"])
+        return model
 
     @classmethod
     def load(cls, load_path, env=None, **kwargs):

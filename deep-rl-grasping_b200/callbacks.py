@@ -161,6 +161,23 @@ class CheckpointCallback(BaseCallback):
         return True
 
 
+class TrainingStateCallback(BaseCallback):
+    """Every ``save_freq`` calls, writes the model's whole training state (``save_training_state``: parameters, optimiser
+    moments, replay, VecNormalize statistics, counters) to ``save_dir``.  Only the latest checkpoint is kept, because the
+    replay makes each one large; a new one replaces the old only once it is complete."""
+
+    def __init__(self, save_freq: int, save_dir: str, verbose: int = 0):
+        super().__init__(verbose)
+        self.save_freq, self.save_dir = int(save_freq), save_dir
+
+    def _on_step(self) -> bool:
+        if self.save_freq > 0 and self.n_calls % self.save_freq == 0:
+            self.model.save_training_state(self.save_dir)
+            if self.verbose > 1:
+                print("Saving training state to {}".format(self.save_dir))
+        return True
+
+
 class EveryNTimesteps(EventCallback):
     """[SB2] trigger the child callback every ``n_steps`` environment timesteps."""
 

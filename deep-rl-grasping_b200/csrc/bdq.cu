@@ -22,6 +22,7 @@
 #include "../../include/b200grasp.h"
 #include "common.cuh"
 #include "host.cuh"
+#include "state.cuh"
 
 using namespace b2g;
 
@@ -225,6 +226,7 @@ struct b2g_bdq {
   float *max_prio = nullptr, *d_beta = nullptr, *prio_out = nullptr;
   cudaGraphExec_t graph_exec = nullptr;
   bool use_graph = true;
+  bool broken = false;         // a training-state load failed after it began writing: only destroy / load are accepted
   float* p(const std::string& nm) { return P + tensors[tindex.at(nm)].off; }
   float* g(const std::string& nm) { return G + tensors[tindex.at(nm)].off; }
   float* pt(const std::string& nm) { return P + n_train + tensors[tindex.at(nm)].off; }
@@ -521,10 +523,11 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
   return 0;
 }
 
-int b2g_bdq_param_count(const b2g_bdq* h) { return h ? 1 + 2 * (int)h->tensors.size() : 0; }
+int b2g_bdq_param_count(const b2g_bdq* h) { B2G_USABLE(h); return h ? 1 + 2 * (int)h->tensors.size() : 0; }
 
 // index 0 = bdq/eps; 1..T = online tensors; T+1..2T = target tensors (names as in the zips)
 int b2g_bdq_param_info(const b2g_bdq* h, int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim) {
+  B2G_USABLE(h);
   if (!h || idx < 0 || idx >= b2g_bdq_param_count(h) || !name) return b2g_fail(B2G_EINVAL, "bad tensor index");
   std::string nm = "bdq/eps";
   int64_t r = 1, c = 1;
@@ -570,13 +573,15 @@ static int bdq_copy(b2g_bdq* h, const char* name, float* arena_online, float* ho
   else CK(cudaMemcpy2D(dev, t.stride * sizeof(float), host, ccount * sizeof(float), ccount * sizeof(float), rows, cudaMemcpyHostToDevice));
   return 0;
 }
-int b2g_bdq_get_param(b2g_bdq* h, const char* name, float* dst, size_t numel) { return bdq_copy(h, name, h ? h->P : nullptr, dst, numel, true, true); }
+int b2g_bdq_get_param(b2g_bdq* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return bdq_copy(h, name, h ? h->P : nullptr, dst, numel, true, true); }
 int b2g_bdq_set_param(b2g_bdq* h, const char* name, const float* src, size_t numel) {
+  B2G_USABLE(h);
   return bdq_copy(h, name, h ? h->P : nullptr, const_cast<float*>(src), numel, false, true);
 }
-int b2g_bdq_get_grad(b2g_bdq* h, const char* name, float* dst, size_t numel) { return bdq_copy(h, name, h ? h->G : nullptr, dst, numel, true, false); }
+int b2g_bdq_get_grad(b2g_bdq* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return bdq_copy(h, name, h ? h->G : nullptr, dst, numel, true, false); }
 
 int b2g_bdq_replay_add(b2g_bdq* h, const float* obs, const float* act_idx, const float* rew, const float* next_obs, const float* done, int64_t n) {
+  B2G_USABLE(h);
   if (!h || !obs || !act_idx || !rew || !next_obs || !done || n < 0) return b2g_fail(B2G_EINVAL, "NULL argument");
   CK(cudaSetDevice(h->cfg.device));
   const int64_t cap = h->cfg.buffer_capacity;
@@ -606,10 +611,11 @@ int b2g_bdq_replay_add(b2g_bdq* h, const float* obs, const float* act_idx, const
   CK(cudaStreamSynchronize(h->stream));
   return 0;
 }
-int64_t b2g_bdq_replay_size(const b2g_bdq* h) { return h ? h->r_size : 0; }
+int64_t b2g_bdq_replay_size(const b2g_bdq* h) { B2G_USABLE(h); return h ? h->r_size : 0; }
 
 int b2g_bdq_set_norm_stats(b2g_bdq* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs, double clip_rew, double eps,
                            int norm_obs, int norm_reward) {
+  B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   if (norm_obs && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
   CK(cudaSetDevice(h->cfg.device));
@@ -626,6 +632,7 @@ int b2g_bdq_set_norm_stats(b2g_bdq* h, const double* obs_mean, const double* obs
 }
 
 int b2g_bdq_step(b2g_bdq* h, int n_steps, float lr, b2g_bdq_metrics* out) {
+  B2G_USABLE(h);
   if (!h || n_steps < 0) return b2g_fail(B2G_EINVAL, "bad argument");
   if (h->r_size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
   CK(cudaSetDevice(h->cfg.device));
@@ -641,6 +648,7 @@ int b2g_bdq_step(b2g_bdq* h, int n_steps, float lr, b2g_bdq_metrics* out) {
 }
 
 int b2g_bdq_set_per_beta(b2g_bdq* h, float beta) {
+  B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
@@ -649,6 +657,7 @@ int b2g_bdq_set_per_beta(b2g_bdq* h, float beta) {
 }
 
 int b2g_bdq_get_last_per(b2g_bdq* h, int32_t* slots, float* weights, float* priorities) {
+  B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
@@ -660,6 +669,7 @@ int b2g_bdq_get_last_per(b2g_bdq* h, int32_t* slots, float* weights, float* prio
 
 int b2g_bdq_step_explicit(b2g_bdq* h, const float* obs, const float* act_idx, const float* rew, const float* next_obs, const float* done,
                           const float* weights, float lr, int apply_update, b2g_bdq_metrics* out, float* td_out) {
+  B2G_USABLE(h);
   if (!h || !obs || !act_idx || !rew || !next_obs || !done) return b2g_fail(B2G_EINVAL, "NULL argument");
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
@@ -678,6 +688,7 @@ int b2g_bdq_step_explicit(b2g_bdq* h, const float* obs, const float* act_idx, co
 
 // greedy branch actions argmax_n Q_d(s, n) of the online network (the epsilon-greedy mixing is the caller's)
 int b2g_bdq_act(b2g_bdq* h, const float* obs, int n, int32_t* act_idx_out) {
+  B2G_USABLE(h);
   if (!h || !obs || !act_idx_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
   CK(cudaSetDevice(h->cfg.device));
   const size_t E = h->E, D = h->D;
@@ -692,6 +703,107 @@ int b2g_bdq_act(b2g_bdq* h, const float* obs, int n, int32_t* act_idx_out) {
     CK(cudaStreamSynchronize(h->stream));
   }
   CK(cudaGetLastError());
+  return 0;
+}
+
+}  // extern "C"
+
+// ================================================================================================
+// Training state (b2g_bdq_state_save / _load; container format in state.cuh)
+// ================================================================================================
+namespace {
+
+std::vector<FpField> bdq_fingerprint(const b2g_bdq* h) {
+  const b2g_bdq_cfg& c = h->cfg;
+  return {fp_int("obs_dim", c.obs_dim), fp_int("n_branches", c.n_branches), fp_int("n_bins", c.n_bins), fp_int("trunk0", c.trunk0),
+          fp_int("trunk1", c.trunk1), fp_int("branch_hidden", c.branch_hidden), fp_int("batch", c.batch),
+          fp_int("buffer_capacity", c.buffer_capacity), fp_real("gamma", c.gamma), fp_int("target_update_freq", c.target_update_freq),
+          fp_int("trunk_grad_rescale", c.trunk_grad_rescale), fp_int("seed", (int64_t)c.seed),
+          fp_int("prioritized_replay", c.prioritized_replay), fp_real("per_alpha", c.per_alpha), fp_real("per_eps", c.per_eps)};
+}
+
+const uint32_t kBdqTags[] = {state_tag("HOST"), state_tag("CNTR"), state_tag("PARM"), state_tag("ADMM"), state_tag("ADMV"),
+                             state_tag("ROBS"), state_tag("RNXT"), state_tag("RACT"), state_tag("RREW"), state_tag("RDON"),
+                             state_tag("PERT"), state_tag("PERS")};
+
+StatePiece bdev(void* p, size_t bytes) { StatePiece s; s.dev = p; s.bytes = bytes; return s; }
+
+// sections 2.. (parameters .. prioritised-replay scalars) of a handle holding `live` replay rows
+std::vector<StateSection> bdq_device_sections(b2g_bdq* h, int64_t live) {
+  const size_t cap = (size_t)h->cfg.buffer_capacity, E = h->E, D = h->D;
+  std::vector<StateSection> s(10);
+  s[0].pieces = {bdev(h->P, 2 * h->n_train * sizeof(float))};
+  s[1].pieces = {bdev(h->Mo, h->n_train * sizeof(float))};
+  s[2].pieces = {bdev(h->Vo, h->n_train * sizeof(float))};
+  s[3].pieces = {bdev(h->r_obs, live * E * sizeof(float))};       // rows [0, size) are the live ones
+  s[4].pieces = {bdev(h->r_next, live * E * sizeof(float))};
+  s[5].pieces = {bdev(h->r_act, cap * D * sizeof(float))};
+  s[6].pieces = {bdev(h->r_rew, cap * sizeof(float))};
+  s[7].pieces = {bdev(h->r_done, cap * sizeof(float))};
+  if (h->per) s[8].pieces = {bdev(h->t_sum, 2 * h->per_C * sizeof(double)), bdev(h->t_min, 2 * h->per_C * sizeof(double))};
+  s[9].pieces = {bdev(h->max_prio, sizeof(float)), bdev(h->d_beta, sizeof(float))};
+  for (int i = 0; i < 10; ++i) s[i].tag = kBdqTags[i + 2];
+  return s;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b2g_bdq_state_save(b2g_bdq* h, const char* path) {
+  if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
+  B2G_USABLE(h);
+  if (h->cfg.nranks > 1)
+    return b2g_fail(B2G_ESTATE, "training-state files of data-parallel learners (nranks > 1) are not built: each rank holds its own replay shard");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  long long cnt[8];
+  CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
+  uint32_t eps_bits;
+  memcpy(&eps_bits, &h->eps_value, sizeof eps_bits);
+  int64_t hv[4] = {h->r_size, h->r_pos, h->n_updates, (int64_t)eps_bits};
+  std::vector<StateSection> secs(2);
+  secs[0].tag = kBdqTags[0]; secs[0].pieces = {StatePiece{hv, nullptr, sizeof hv}};
+  secs[1].tag = kBdqTags[1]; secs[1].pieces = {StatePiece{cnt, nullptr, sizeof cnt}};
+  for (auto& s : bdq_device_sections(h, h->r_size)) secs.push_back(std::move(s));
+  return state_write(path, STATE_KIND_BDQ, bdq_fingerprint(h), secs);
+}
+
+int b2g_bdq_state_load(b2g_bdq* h, const char* path) {
+  if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
+  if (h->cfg.nranks > 1) return b2g_fail(B2G_ESTATE, "training-state files of data-parallel learners (nranks > 1) are not built");
+  CK(cudaSetDevice(h->cfg.device));
+  // ---- everything is checked before the handle changes
+  StateReader rd;
+  if (int rc = rd.open(path, STATE_KIND_BDQ, bdq_fingerprint(h))) return rc;
+  const int n_sec = (int)(sizeof kBdqTags / sizeof kBdqTags[0]);
+  if (rd.n_sections() != n_sec) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a BDQ learner");
+  for (int i = 0; i < n_sec; ++i)
+    if (rd.tag(i) != kBdqTags[i]) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a BDQ learner");
+  int64_t hv[4];
+  long long cnt[8];
+  if (rd.bytes(0) != sizeof hv || rd.bytes(1) != sizeof cnt)
+    return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  if (int rc = rd.read_host(0, hv, sizeof hv)) return rc;
+  const int64_t cap = h->cfg.buffer_capacity;
+  if (hv[0] < 0 || hv[0] > cap || hv[1] < 0 || hv[1] >= cap || (hv[0] < cap && hv[1] != hv[0]) || hv[2] < 0)
+    return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
+  std::vector<StateSection> dev = bdq_device_sections(h, hv[0]);
+  for (int i = 0; i < (int)dev.size(); ++i)
+    if (rd.bytes(i + 2) != dev[i].bytes())
+      return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
+  // ---- from here on a failure leaves the handle unusable until a load succeeds
+  CK(cudaStreamSynchronize(h->stream));
+  h->broken = true;
+  for (int i = 0; i < (int)dev.size(); ++i)
+    if (int rc = rd.read_pieces(i + 2, dev[i].pieces)) return rc;
+  CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
+  h->r_size = hv[0]; h->r_pos = hv[1]; h->n_updates = hv[2];
+  const uint32_t eps_bits = (uint32_t)hv[3];
+  memcpy(&h->eps_value, &eps_bits, sizeof eps_bits);
+  // the captured step graph stays valid: it holds device pointers and configuration; size and Philox step are device counters
+  h->broken = false;
   return 0;
 }
 

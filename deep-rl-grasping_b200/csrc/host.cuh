@@ -24,6 +24,13 @@ int b2g_fail(int code, const std::string& msg);
                                      std::to_string(__LINE__));                                   \
   } while (0)
 
+// Returns B2G_ESTATE from the enclosing entry point when a failed training-state load left handle h unusable.
+#define B2G_USABLE(h)                                                                                        \
+  do {                                                                                                       \
+    if ((h) && (h)->broken)                                                                                  \
+      return b2g_fail(B2G_ESTATE, "handle unusable: a training-state load failed part way (load a state again or destroy it)"); \
+  } while (0)
+
 namespace b2g {
 
 // The device exists, is made current and is a Hopper part (sm_90); *num_sms receives its SM count when asked for.

@@ -29,6 +29,7 @@
 #include "../../include/b200grasp.h"
 #include "common.cuh"
 #include "sac_internal.cuh"
+#include "state.cuh"
 
 using namespace b2g;
 
@@ -961,6 +962,7 @@ int load_rows(b2g_sac* h, const float* src, float* dst, long long first, long lo
 extern "C" {
 
 int b2g_sac_dp_export(b2g_sac* h, void* out192) {
+  B2G_USABLE(h);
   if (!h || !out192) return b2g_fail(B2G_EINVAL, "b2g_sac_dp_export: null argument");
   cudaSetDevice(h->cfg.device);
   if (!h->dp_x) {
@@ -986,6 +988,7 @@ int b2g_debug_dp_stamps(b2g_sac* h, long long* out5) {     /* bring-up: phase ti
 }
 
 int b2g_sac_dp_connect(b2g_sac* h, const void* all_exports, int nranks) {
+  B2G_USABLE(h);
   if (!h || !all_exports) return b2g_fail(B2G_EINVAL, "b2g_sac_dp_connect: null argument");
   if (nranks != h->cfg.nranks || nranks < 2 || nranks > DP_MAX_RANKS) return b2g_fail(B2G_EINVAL, "b2g_sac_dp_connect: nranks must equal the learner's (2..8)");
   if (!h->dp_x) return b2g_fail(B2G_EINVAL, "b2g_sac_dp_connect: call b2g_sac_dp_export first");
@@ -1270,15 +1273,17 @@ int b2g_sac_create2(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, b2g_sa
 }
 
 int b2g_sync(b2g_sac* h) {
+  B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
   return 0;
 }
 
-int b2g_param_count(const b2g_sac* h) { return h ? (int)h->tensors.size() : 0; }
+int b2g_param_count(const b2g_sac* h) { B2G_USABLE(h); return h ? (int)h->tensors.size() : 0; }
 
 int b2g_param_info(const b2g_sac* h, int idx, const char** name, int64_t* numel, int32_t* ndim, int64_t shape[4]) {
+  B2G_USABLE(h);
   if (!h || idx < 0 || idx >= (int)h->tensors.size()) return b2g_fail(B2G_EINVAL, "bad tensor index");
   const Tensor& t = h->tensors[idx];
   if (name) *name = t.name.c_str();
@@ -1302,22 +1307,26 @@ static int copy_tensor(b2g_sac* h, const char* name, float* arena, float* host, 
   return 0;
 }
 
-int b2g_get_param(b2g_sac* h, const char* name, float* dst, size_t numel) { return copy_tensor(h, name, h ? h->P : nullptr, dst, numel, true, false); }
+int b2g_get_param(b2g_sac* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return copy_tensor(h, name, h ? h->P : nullptr, dst, numel, true, false); }
 int b2g_set_param(b2g_sac* h, const char* name, const float* src, size_t numel) {
+  B2G_USABLE(h);
   int rc = copy_tensor(h, name, h ? h->P : nullptr, const_cast<float*>(src), numel, false, false);
   if (rc == 0) h->planes_dirty = true;
   return rc;
 }
 int b2g_get_grad(b2g_sac* h, const char* name, float* dst, size_t numel) {
+  B2G_USABLE(h);
   int rc = copy_tensor(h, name, h ? h->G : nullptr, dst, numel, true, true);
   if (rc == 0 && h->cfg.nranks > 1) for (size_t i = 0; i < numel; ++i) dst[i] /= (float)h->cfg.nranks;
   return rc;
 }
 int b2g_get_adam(b2g_sac* h, const char* name, float* m, float* v, size_t numel) {
+  B2G_USABLE(h);
   if (int rc = copy_tensor(h, name, h ? h->Mo : nullptr, m, numel, true, true)) return rc;
   return copy_tensor(h, name, h->Vo, v, numel, true, true);
 }
 int b2g_reset_optimizer(b2g_sac* h) {
+  B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaMemsetAsync(h->Mo, 0, h->n_train * sizeof(float), h->stream));
@@ -1329,6 +1338,7 @@ int b2g_reset_optimizer(b2g_sac* h) {
 
 int b2g_replay_add(b2g_sac* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done,
                    int64_t n) {
+  B2G_USABLE(h);
   if (!h || !obs || !act || !rew || !next_obs || !done || n < 0) return b2g_fail(B2G_EINVAL, "NULL argument");
   if (h->dedup && 2 * n > h->frame_cap) return b2g_fail(B2G_EINVAL, "replay_add: 2 n rows exceed frame_capacity");
   CK(cudaSetDevice(h->cfg.device));
@@ -1409,10 +1419,11 @@ int b2g_replay_add(b2g_sac* h, const float* obs, const float* act, const float* 
   return 0;
 }
 
-int64_t b2g_replay_size(const b2g_sac* h) { return h ? h->r_size : 0; }
+int64_t b2g_replay_size(const b2g_sac* h) { B2G_USABLE(h); return h ? h->r_size : 0; }
 
 int b2g_replay_info(const b2g_sac* h, int64_t* capacity, int64_t* size, int64_t* frame_capacity, int64_t* live_frames,
                     int64_t* bytes, int64_t* evicted_early) {
+  B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   const int64_t cap = h->cfg.buffer_capacity;
   int64_t live = 0;
@@ -1431,6 +1442,7 @@ int b2g_replay_info(const b2g_sac* h, int64_t* capacity, int64_t* size, int64_t*
 }
 
 int b2g_replay_get(b2g_sac* h, int64_t slot, float* obs, float* act, float* rew, float* next_obs, float* done) {
+  B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   const int64_t cap = h->cfg.buffer_capacity;
   if (slot < 0 || slot >= cap || ((slot - h->tail_seq % cap) % cap + cap) % cap >= h->r_size)
@@ -1470,6 +1482,7 @@ int b2g_replay_get(b2g_sac* h, int64_t slot, float* obs, float* act, float* rew,
 }
 
 int b2g_get_last_batch(b2g_sac* h, int32_t* indices, float* eps, float* per_sample, float* pi_out) {
+  B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
@@ -1483,6 +1496,7 @@ int b2g_get_last_batch(b2g_sac* h, int32_t* indices, float* eps, float* per_samp
 
 int b2g_set_norm_stats(b2g_sac* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs, double clip_rew,
                        double eps, int norm_obs, int norm_reward) {
+  B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   if (norm_obs && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
   CK(cudaSetDevice(h->cfg.device));
@@ -1521,6 +1535,7 @@ static int ensure_graph(b2g_sac* h) {
 }
 
 int b2g_sac_step_async(b2g_sac* h, int n_steps, float lr) {
+  B2G_USABLE(h);
   if (!h || n_steps < 0) return b2g_fail(B2G_EINVAL, "bad argument");
   if (h->r_size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
   CK(cudaSetDevice(h->cfg.device));
@@ -1537,6 +1552,7 @@ int b2g_sac_step_async(b2g_sac* h, int n_steps, float lr) {
 }
 
 int b2g_sac_step(b2g_sac* h, int n_steps, float lr, b2g_sac_metrics* out) {
+  B2G_USABLE(h);
   if (int rc = b2g_sac_step_async(h, n_steps, lr)) return rc;
   if (int rc = fetch_metrics(h, out)) return rc;
   cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1);
@@ -1545,6 +1561,7 @@ int b2g_sac_step(b2g_sac* h, int n_steps, float lr, b2g_sac_metrics* out) {
 
 int b2g_sac_step_explicit(b2g_sac* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done,
                           const float* eps, float lr, int apply_update, b2g_sac_metrics* out, float* per_sample, float* pi_out) {
+  B2G_USABLE(h);
   if (!h || !obs || !act || !rew || !next_obs || !done || !eps) return b2g_fail(B2G_EINVAL, "NULL argument");
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
@@ -1597,6 +1614,7 @@ int b2g_debug_compact_host(const float* src, float* dst, int n, int hw, int cful
 
 int b2g_sac_step_host_pipelined(b2g_sac* h, const float* obs, const float* act, const float* rew, const float* next_obs,
                                 const float* done, const float* eps, float lr, b2g_sac_metrics* prev_out, int* have_prev) {
+  B2G_USABLE(h);
   if (!h || !obs || !act || !rew || !next_obs || !done || !eps) return b2g_fail(B2G_EINVAL, "NULL argument");
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
@@ -1702,6 +1720,7 @@ int b2g_sac_step_host_pipelined(b2g_sac* h, const float* obs, const float* act, 
 }
 
 int b2g_sac_pipeline_flush(b2g_sac* h, b2g_sac_metrics* last_out) {
+  B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   CK(cudaSetDevice(h->cfg.device));
   if (!h->pipe_pending) return b2g_fail(B2G_ESTATE, "no pipelined step in flight");
@@ -1713,6 +1732,7 @@ int b2g_sac_pipeline_flush(b2g_sac* h, b2g_sac_metrics* last_out) {
 }
 
 int b2g_sac_act(b2g_sac* h, const float* obs, int n, int deterministic, float* act_out) {
+  B2G_USABLE(h);
   if (!h || !obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
   CK(cudaSetDevice(h->cfg.device));
   const size_t E = h->E, A = h->A;
@@ -1737,15 +1757,17 @@ int b2g_sac_act(b2g_sac* h, const float* obs, int n, int deterministic, float* a
 }
 
 int b2g_launches_per_step(const b2g_sac* h) {
+  B2G_USABLE(h);
   if (!h) return 0;
   if (h->launches) return h->launches;
   // prep + gather + memset + groups + tail + optim (+3 with a collective)
   return 3 + (int)h->fwd_groups.size() + 1 + (int)h->bwd_groups.size() + 1 + (h->cfg.nranks > 1 ? 3 : 0);
 }
 
-float b2g_last_step_ms(const b2g_sac* h) { return h ? h->last_ms : 0.f; }
+float b2g_last_step_ms(const b2g_sac* h) { B2G_USABLE(h); return h ? h->last_ms : 0.f; }
 
 int b2g_profile_step(b2g_sac* h, float lr, const char** names, float* ms, int cap) {
+  B2G_USABLE(h);
   if (!h || !names || !ms) return b2g_fail(B2G_EINVAL, "NULL argument");
   if (h->r_size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
   CK(cudaSetDevice(h->cfg.device));
@@ -1764,6 +1786,158 @@ int b2g_profile_step(b2g_sac* h, float lr, const char** names, float* ms, int ca
   }
   for (auto e : prof.ev) cudaEventDestroy(e);
   return k;
+}
+
+}  // extern "C"
+
+// ================================================================================================
+// Training state (b2g_sac_state_save / _load; container format in state.cuh)
+// ================================================================================================
+namespace {
+
+std::vector<FpField> sac_fingerprint(const b2g_sac* h) {
+  const b2g_sac_cfg& c = h->cfg;
+  return {fp_int("obs_h", c.obs_h), fp_int("obs_w", c.obs_w), fp_int("obs_c", c.obs_c), fp_int("obs_dim", c.obs_dim),
+          fp_int("n_act", c.n_act), fp_int("hidden", c.hidden), fp_int("batch", c.batch),
+          fp_int("buffer_capacity", c.buffer_capacity), fp_int("frame_capacity", h->frame_cap),
+          fp_int("u8_plane_mask", h->u8_mask), fp_real("gamma", c.gamma), fp_real("tau", c.tau),
+          fp_real("target_entropy", c.target_entropy), fp_int("seed", (int64_t)c.seed)};
+}
+
+// Host replay bookkeeping as stored: r_size, head_seq, tail_seq, next_fid, evicted, |lw|, |prev_next|, lw pairs, prev_next.
+struct SacHostState {
+  int64_t r_size = 0, head_seq = 0, tail_seq = 0, next_fid = 0, evicted = 0;
+  std::vector<std::pair<int64_t, int64_t>> lw;
+  std::vector<int64_t> prev_next;
+  // oldest frame the file must hold: the oldest one a live transition references, or a previous next_obs frame the next
+  // b2g_replay_add may still share
+  int64_t frame_lo(int64_t fcap) const {
+    int64_t lo = next_fid;
+    if (r_size > 0)
+      for (const auto& q : lw) if (q.first >= tail_seq) { lo = q.second; break; }
+    for (int64_t p : prev_next) if (p > next_fid - fcap) lo = std::min(lo, p);
+    return lo;
+  }
+};
+
+StatePiece host_piece(void* p, size_t bytes) { StatePiece s; s.host = p; s.bytes = bytes; return s; }
+StatePiece dev_piece(void* p, size_t bytes) { StatePiece s; s.dev = p; s.bytes = bytes; return s; }
+
+// frames [lo, hi) of the ring: at most two contiguous ranges, each stored at id % frame_cap
+std::vector<StatePiece> frame_pieces(b2g_sac* h, int64_t lo, int64_t hi) {
+  std::vector<StatePiece> v;
+  for (int64_t f = lo; f < hi;) {
+    const int64_t pos = f % h->frame_cap, n = std::min(hi - f, h->frame_cap - pos);
+    v.push_back(dev_piece(h->frames + pos * h->frame_bytes, (size_t)(n * h->frame_bytes)));
+    f += n;
+  }
+  return v;
+}
+
+const uint32_t kSacTags[] = {state_tag("HOST"), state_tag("CNTR"), state_tag("PARM"), state_tag("ADMM"), state_tag("ADMV"),
+                             state_tag("ROFR"), state_tag("RNFR"), state_tag("RACT"), state_tag("RREW"), state_tag("RDON"),
+                             state_tag("FRMS")};
+
+// the device-resident sections 2..10 (parameters .. frames) of a handle whose frame window is [lo, hi)
+std::vector<StateSection> sac_device_sections(b2g_sac* h, int64_t lo, int64_t hi) {
+  const size_t cap = (size_t)h->cfg.buffer_capacity;
+  std::vector<StateSection> s(9);
+  s[0].pieces = {dev_piece(h->P, h->n_all * sizeof(float))};
+  s[1].pieces = {dev_piece(h->Mo, h->n_train * sizeof(float))};
+  s[2].pieces = {dev_piece(h->Vo, h->n_train * sizeof(float))};
+  s[3].pieces = {dev_piece(h->r_ofr, cap * sizeof(int))};
+  s[4].pieces = {dev_piece(h->r_nfr, cap * sizeof(int))};
+  s[5].pieces = {dev_piece(h->r_act, cap * h->A * sizeof(float))};
+  s[6].pieces = {dev_piece(h->r_rew, cap * sizeof(float))};
+  s[7].pieces = {dev_piece(h->r_done, cap * sizeof(float))};
+  s[8].pieces = frame_pieces(h, lo, hi);
+  for (int i = 0; i < 9; ++i) s[i].tag = kSacTags[i + 2];
+  return s;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b2g_sac_state_save(b2g_sac* h, const char* path) {
+  if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
+  B2G_USABLE(h);
+  if (h->cfg.nranks > 1)
+    return b2g_fail(B2G_ESTATE, "training-state files of data-parallel learners (nranks > 1) are not built: each rank holds only its "
+                                "slice of the Adam moments");
+  if (h->pipe_pending)
+    return b2g_fail(B2G_ESTATE, "a host-pipelined step is in flight: call b2g_sac_pipeline_flush first (its losses would be lost)");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));     // every enqueued step (b2g_sac_step_async included) has run
+  if (h->aux) CK(cudaStreamSynchronize(h->aux));
+  long long cnt[8];
+  CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
+  SacHostState hs;
+  hs.r_size = h->r_size; hs.head_seq = h->head_seq; hs.tail_seq = h->tail_seq; hs.next_fid = h->next_fid; hs.evicted = h->evicted;
+  hs.lw.assign(h->lw.begin(), h->lw.end());
+  hs.prev_next = h->prev_next;
+  std::vector<int64_t> hv = {hs.r_size, hs.head_seq, hs.tail_seq, hs.next_fid, hs.evicted, (int64_t)hs.lw.size(), (int64_t)hs.prev_next.size()};
+  for (const auto& q : hs.lw) { hv.push_back(q.first); hv.push_back(q.second); }
+  hv.insert(hv.end(), hs.prev_next.begin(), hs.prev_next.end());
+  std::vector<StateSection> secs(2);
+  secs[0].tag = kSacTags[0]; secs[0].pieces = {host_piece(hv.data(), hv.size() * sizeof(int64_t))};
+  secs[1].tag = kSacTags[1]; secs[1].pieces = {host_piece(cnt, sizeof cnt)};
+  for (auto& s : sac_device_sections(h, hs.frame_lo(h->frame_cap), hs.next_fid)) secs.push_back(std::move(s));
+  return state_write(path, STATE_KIND_SAC, sac_fingerprint(h), secs);
+}
+
+int b2g_sac_state_load(b2g_sac* h, const char* path) {
+  if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
+  if (h->cfg.nranks > 1)
+    return b2g_fail(B2G_ESTATE, "training-state files of data-parallel learners (nranks > 1) are not built");
+  if (h->pipe_pending)
+    return b2g_fail(B2G_ESTATE, "a host-pipelined step is in flight: call b2g_sac_pipeline_flush first");
+  CK(cudaSetDevice(h->cfg.device));
+  // ---- everything is checked before the handle changes
+  StateReader rd;
+  if (int rc = rd.open(path, STATE_KIND_SAC, sac_fingerprint(h))) return rc;
+  const int n_sec = (int)(sizeof kSacTags / sizeof kSacTags[0]);
+  if (rd.n_sections() != n_sec) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a SAC learner");
+  for (int i = 0; i < n_sec; ++i)
+    if (rd.tag(i) != kSacTags[i]) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a SAC learner");
+  const int64_t cap = h->cfg.buffer_capacity, FC = h->frame_cap;
+  if (rd.bytes(0) % 8 || rd.bytes(0) < 7 * 8 || rd.bytes(0) > (uint64_t)(7 + 2 * cap + 4 * FC) * 8)
+    return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
+  std::vector<int64_t> hv(rd.bytes(0) / 8);
+  if (int rc = rd.read_host(0, hv.data(), hv.size() * 8)) return rc;
+  SacHostState hs;
+  hs.r_size = hv[0]; hs.head_seq = hv[1]; hs.tail_seq = hv[2]; hs.next_fid = hv[3]; hs.evicted = hv[4];
+  const int64_t n_lw = hv[5], n_prev = hv[6];
+  if (n_lw < 0 || n_prev < 0 || (int64_t)hv.size() != 7 + 2 * n_lw + n_prev || hs.r_size != hs.head_seq - hs.tail_seq || hs.r_size < 0 ||
+      hs.r_size > cap || hs.tail_seq < 0 || hs.next_fid < 0 || hs.evicted < 0)
+    return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
+  for (int64_t i = 0; i < n_lw; ++i) hs.lw.emplace_back(hv[7 + 2 * i], hv[8 + 2 * i]);
+  hs.prev_next.assign(hv.begin() + 7 + 2 * n_lw, hv.end());
+  const int64_t lo = hs.frame_lo(FC);
+  if (lo < 0 || lo > hs.next_fid || hs.next_fid - lo > FC) return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
+  std::vector<StateSection> dev = sac_device_sections(h, lo, hs.next_fid);
+  for (int i = 0; i < (int)dev.size(); ++i)
+    if (rd.bytes(i + 2) != dev[i].bytes())
+      return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  long long cnt[8];
+  if (rd.bytes(1) != sizeof cnt) return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
+  // ---- from here on a failure leaves the handle unusable until a load succeeds
+  CK(cudaStreamSynchronize(h->stream));
+  if (h->aux) CK(cudaStreamSynchronize(h->aux));
+  h->broken = true;
+  for (int i = 0; i < (int)dev.size(); ++i)
+    if (int rc = rd.read_pieces(i + 2, dev[i].pieces)) return rc;
+  CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
+  h->r_size = hs.r_size; h->head_seq = hs.head_seq; h->tail_seq = hs.tail_seq; h->next_fid = hs.next_fid; h->evicted = hs.evicted;
+  h->lw.assign(hs.lw.begin(), hs.lw.end());
+  h->prev_next = hs.prev_next;
+  // The BF16 weight planes follow the restored arena at the next step or act.  The captured step graphs (graph_exec, pipe_graph)
+  // stay valid: their kernel parameters hold device pointers and configuration only, and the replay size, first live slot and
+  // Philox step they depend on are read from the device counters restored above.
+  h->planes_dirty = true;
+  h->broken = false;
+  return 0;
 }
 
 }  // extern "C"

@@ -202,6 +202,7 @@ struct b2g_sac {
   long long* h_cnt = nullptr;    // pinned counters
 
   b2g::V2State v2;
+  bool broken = false;               // a training-state load failed after it began writing: only destroy / load are accepted
   double* hp_stats[2]{};             // pinned staging of set_norm_stats (asynchronous upload, no stream sync)
   cudaEvent_t ev_stats[2]{};
   int stats_k = 0;

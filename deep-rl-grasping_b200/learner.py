@@ -6,6 +6,7 @@ bench.py also use it directly because it maps 1:1 onto the C ABI entry points.
 from __future__ import annotations
 
 import ctypes as C
+import os
 from collections import OrderedDict
 from typing import Dict, Optional, Sequence
 
@@ -216,6 +217,16 @@ class Learner:
             mp = vp = None
         _lib.check(self.lib.b2g_set_norm_stats(self.h, mp, vp, float(ret_var), float(clip_obs), float(clip_reward),
                                                 float(epsilon), int(bool(norm_obs)), int(bool(norm_reward))))
+
+    # ---- training state (include/b200grasp.h: b2g_sac_state_save / _load)
+    def save_state(self, path: str):
+        """Writes parameters, Adam moments, counters and the whole replay to ``path`` (waits for enqueued steps)."""
+        _lib.check(self.lib.b2g_sac_state_save(self.h, os.fsencode(path)))
+
+    def load_state(self, path: str):
+        """Restores a ``save_state`` file into this learner, which must have the same configuration (precision aside).
+        Normalisation statistics are not part of the file: set them again with ``set_norm_stats``."""
+        _lib.check(self.lib.b2g_sac_state_load(self.h, os.fsencode(path)))
 
     # ---- hot path
     def step(self, n_steps: int = 1, lr: float = 3e-4) -> dict:

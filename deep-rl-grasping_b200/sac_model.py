@@ -17,7 +17,7 @@ from typing import Optional
 
 import numpy as np
 
-from . import _lib, sb_io
+from . import _lib, sb_io, training_state
 from .callbacks import as_callback
 from .learner import Learner
 from .vec_env import DummyVecEnv, VecNormalize
@@ -302,6 +302,49 @@ class SAC:
         if d:
             os.makedirs(d, exist_ok=True)
         sb_io.save_sb_zip(save_path, self._data(), self.learner.get_parameters())
+
+    # ------------------------------------------------------------------ training state (training_state.py)
+    def _host_state(self):
+        kw = self.policy_kwargs.get("cnn_extractor")
+        policy_kwargs = dict(self.policy_kwargs)
+        if kw is not None and not isinstance(kw, str):
+            policy_kwargs["cnn_extractor"] = "augmented_nature_cnn"      # the one extractor the learner builds
+        if callable(self.learning_rate):
+            raise NotImplementedError("save_training_state needs a constant learning_rate")
+        init = dict(gamma=self.gamma, learning_rate=self.learning_rate, buffer_size=self.buffer_size, learning_starts=self.learning_starts,
+                    train_freq=self.train_freq, batch_size=self.batch_size, tau=self.tau, ent_coef=self.ent_coef,
+                    gradient_steps=self.gradient_steps, target_entropy=self.target_entropy, random_exploration=self.random_exploration,
+                    verbose=self.verbose, seed=self.seed, policy_kwargs=policy_kwargs, precision=self.precision,
+                    replay_frames=self.replay_frames, replay_u8_planes=list(self.replay_u8_planes))
+        return {"algo": "SAC", "policy": "CnnPolicy" if len(self.observation_space.shape) == 3 else "MlpPolicy", "init": init,
+                "num_timesteps": int(self.num_timesteps), "n_updates": int(self.n_updates),
+                "episode_rewards": [float(r) for r in self.episode_rewards], "ep_info_buf": list(self.ep_info_buf),
+                "rng": training_state.rng_state(self._rng)}
+
+    def save_training_state(self, path):
+        """Writes directory ``path``: model.zip, learner.state (parameters, Adam moments, counters, the whole replay),
+        vecnormalize.pkl and host.json.  The previous contents stay loadable until the new directory is complete."""
+        return training_state.save_training_state(self, path)
+
+    @classmethod
+    def load_training_state(cls, path, env, **kwargs):
+        """Rebuilds the model ``save_training_state`` wrote into ``path`` on ``env`` and restores the saved VecNormalize
+        statistics into ``env``'s wrapper.  ``learn(n, reset_num_timesteps=False)`` then continues the run."""
+        path = training_state.resolve(path)
+        host = training_state.read_host(path)
+        if host.get("algo") != "SAC":
+            raise ValueError(f"{path} holds a {host.get('algo')} training state")
+        init = dict(host["init"], **kwargs)
+        model = cls({"CnnPolicy": CnnPolicy, "MlpPolicy": MlpPolicy}[host["policy"]], env, **init)
+        training_state.restore_vec_normalize(path, model.env)
+        model.load_parameters(os.path.join(path, training_state.MODEL_FILE))
+        model.learner.load_state(os.path.join(path, training_state.STATE_FILE))
+        model._sync_norm_stats()
+        model.num_timesteps, model.n_updates = int(host["num_timesteps"]), int(host["n_updates"])
+        model.episode_rewards = [float(r) for r in host["episode_rewards"]]
+        model.ep_info_buf = deque(host["ep_info_buf"], maxlen=100)
+        training_state.set_rng_state(model._rng, host["rng"])
+        return model
 
     @classmethod
     def load(cls, load_path, env=None, custom_objects=None, **kwargs):

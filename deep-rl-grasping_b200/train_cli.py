@@ -20,9 +20,9 @@ import os
 import numpy as np
 import yaml
 
-from . import BDQ, SAC
+from . import BDQ, SAC, training_state
 from .bench import Monitor
-from .callbacks import BaseCallback, CheckpointCallback, EvalCallback
+from .callbacks import BaseCallback, CheckpointCallback, EvalCallback, TrainingStateCallback
 from .sac_model import CnnPolicy, MlpPolicy
 from .vec_env import DummyVecEnv, SubprocVecEnv, VecNormalize
 
@@ -64,6 +64,8 @@ def _is_image_obs(env):
 
 
 def train(args):
+    if getattr(args, "resume", None):
+        return resume(args)
     config = yaml.safe_load(open(args.config))
     os.mkdir(args.model_dir)                                   # like the reference: refuses to overwrite a run
     os.mkdir(os.path.join(args.model_dir, "best_model"))
@@ -130,7 +132,11 @@ def train(args):
             model.load_parameters(BDQ.load(args.load_dir, env).get_parameters())
     else:
         raise NotImplementedError(f"--algo {algo}: the H100 learner builds the SAC and BDQ branches of SBPolicy.learn (sb_helper.py:85-226)")
-    model.learn(total_timesteps=int(c["total_timesteps"]), callback=callbacks)
+    if args.state_freq:
+        callbacks.append(TrainingStateCallback(args.state_freq, os.path.join(args.model_dir, STATE_DIR)))
+        _learn_keeping_state(model, int(c["total_timesteps"]), callbacks, os.path.join(args.model_dir, STATE_DIR))
+    else:
+        model.learn(total_timesteps=int(c["total_timesteps"]), callback=callbacks)
     model.save(os.path.join(args.model_dir, "final_model" if algo != "BDQ" else "bdq_model"))   # sb_helper.py:228-247
     vn = model.get_vec_normalize_env()
     if vn is not None:
@@ -138,6 +144,61 @@ def train(args):
     env.close()
     test_env.close()
     return model
+
+
+STATE_DIR = "training_state"
+
+
+def _learn_keeping_state(model, total_timesteps, callbacks, state_dir, reset_num_timesteps=True):
+    """model.learn; an interrupt (Ctrl-C) writes the training state before the run ends, as sb_helper.py:178-181 does
+    for the model."""
+    try:
+        model.learn(total_timesteps=total_timesteps, callback=callbacks, reset_num_timesteps=reset_num_timesteps)
+    except KeyboardInterrupt:
+        model.save_training_state(state_dir)
+
+
+def resume(args):
+    """train --resume <model_dir>: continues the run whose config.yaml and training_state/ sit in model_dir for the
+    remaining total_timesteps - num_timesteps steps.  The environment starts a fresh episode."""
+    model_dir = args.resume
+    config = yaml.safe_load(open(os.path.join(model_dir, "config.yaml")))
+    algo = config["algorithm"].upper()
+    if algo not in ("SAC", "BDQ"):
+        raise NotImplementedError(f"--resume: algorithm '{algo}' has no training state")
+    state_dir = training_state.resolve(os.path.join(model_dir, STATE_DIR))
+    done = int(training_state.read_host(state_dir)["num_timesteps"])
+    make = _factory(args.env)
+    n_envs = max(1, int(args.n_envs))
+    log = os.path.join(model_dir, f"log_file_resume_{done}")        # the original run's monitor file stays as it is
+    if n_envs == 1:
+        env = DummyVecEnv([lambda: Monitor(make(config), log)])
+    else:
+        env = SubprocVecEnv([(lambda i=i: Monitor(make(config), f"{log}_{i}")) for i in range(n_envs)])
+    test_env = DummyVecEnv([lambda: make(config, evaluate=True, validate=True)])
+    eval_path = os.path.join(model_dir, "best_model")
+    if config.get("normalize", False):
+        test_env = VecNormalize(test_env, norm_obs=True, norm_reward=False, clip_obs=10.0)
+        env = VecNormalize(env, norm_obs=True, norm_reward=True, clip_obs=10.0)     # statistics: the saved ones
+    callbacks = [
+        EvalCallback(test_env, best_model_save_path=eval_path, log_path=os.path.join(eval_path, "logs"), eval_freq=args.eval_freq,
+                     n_eval_episodes=10, callback_on_new_best=SaveVecNormalizeCallback(1, eval_path), deterministic=True),
+        CheckpointCallback(save_freq=args.checkpoint_freq, save_path=os.path.join(model_dir, "logs"), name_prefix="rl_model"),
+    ]
+    if args.state_freq:
+        callbacks.append(TrainingStateCallback(args.state_freq, os.path.join(model_dir, STATE_DIR)))
+    model = (SAC if algo == "SAC" else BDQ).load_training_state(state_dir, env)
+    remaining = int(config[algo]["total_timesteps"]) - model.num_timesteps
+    if remaining > 0:
+        _learn_keeping_state(model, remaining, callbacks, os.path.join(model_dir, STATE_DIR), reset_num_timesteps=False)
+    model.save(os.path.join(model_dir, "final_model" if algo != "BDQ" else "bdq_model"))
+    vn = model.get_vec_normalize_env()
+    if vn is not None:
+        vn.save(os.path.join(model_dir, "vecnormalize.pkl"))
+    env.close()
+    test_env.close()
+    return model
+
 
 
 def run_agent(task, agent, stochastic=False, n_episodes=100):
@@ -187,9 +248,9 @@ def build_parser():
     p = argparse.ArgumentParser(prog="b200grasp.train_cli")
     sub = p.add_subparsers()
     t = sub.add_parser("train")
-    t.add_argument("--config", type=str, required=True)
-    t.add_argument("--algo", type=str, required=True)
-    t.add_argument("--model_dir", type=str, required=True)
+    t.add_argument("--config", type=str)           # required unless --resume (checked in main)
+    t.add_argument("--algo", type=str)
+    t.add_argument("--model_dir", type=str)
     t.add_argument("--load_dir", type=str)
     t.add_argument("--timestep", type=str)
     t.add_argument("-s", "--simple", action="store_true")
@@ -204,6 +265,11 @@ def build_parser():
                         "transitions; 0.125 covers episodes down to ~9 steps); default: two frames per replay slot")
     t.add_argument("--eval_freq", type=int, default=50000)
     t.add_argument("--checkpoint_freq", type=int, default=25000)
+    t.add_argument("--state_freq", type=int, default=None,
+                   help="every N steps write the whole training state (replay, optimiser moments, counters) to "
+                        "<model_dir>/training_state, keeping only the latest; an interrupt writes it too")
+    t.add_argument("--resume", type=str, default=None, metavar="MODEL_DIR",
+                   help="continue the run in MODEL_DIR from its training_state/ for the rest of its total_timesteps")
     t.set_defaults(func=train)
     r = sub.add_parser("run")
     r.add_argument("--model", type=str, required=True)
@@ -219,10 +285,15 @@ def build_parser():
 
 def main(argv=None):
     logging.getLogger().setLevel(logging.INFO)
-    args = build_parser().parse_args(argv)
+    parser = build_parser()
+    args = parser.parse_args(argv)
     if not hasattr(args, "func"):
         build_parser().print_help()
         return None
+    if args.func is train and not args.resume:
+        missing = [f"--{k}" for k in ("config", "algo", "model_dir") if getattr(args, k) is None]
+        if missing:
+            parser._subparsers._group_actions[0].choices["train"].error("the following arguments are required: " + ", ".join(missing))
     return args.func(args)
 
 

@@ -172,6 +172,21 @@ int b2g_sac_pipeline_flush(b2g_sac* h, b2g_sac_metrics* last_out);
  * deterministic -> tanh(mu); else tanh(mu + eps*std) with eps from the handle's generator. */
 int b2g_sac_act(b2g_sac* h, const float* obs, int n, int deterministic, float* act_out);
 
+/* ---- training state: stop a run and continue it later.  The file holds what decides the next step / act / replay_add: the
+ *      parameter arena (target network and log_ent_coef included), both Adam moments, the device counters (Adam steps,
+ *      n_updates, the Philox step of the slot and noise draws, replay size and first live slot), the replay bookkeeping, the
+ *      transition arrays and the live window of replay frames.  Not in it: the normalisation statistics (set them again with
+ *      b2g_set_norm_stats; VecNormalize keeps its own file) and the precision mode (a bf16x3 state loads into an fp32 handle).
+ * save: waits for every step enqueued on the handle; B2G_ESTATE while a host-pipelined step awaits b2g_sac_pipeline_flush and
+ *       for nranks > 1 (data-parallel checkpoints are not built).
+ * load: into a handle created with the same configuration.  The header, the configuration fingerprint (shape, n_act, hidden,
+ *       batch, capacities, 8-bit planes, gamma, tau, target_entropy, seed), the section lengths and the file size are checked
+ *       before anything is written: a mismatch returns B2G_EINVAL naming the first field that differs and leaves the handle as
+ *       it was.  A read or checksum failure after that leaves the handle unusable: every call but destroy and another load
+ *       then returns B2G_ESTATE. */
+int b2g_sac_state_save(b2g_sac* h, const char* path);
+int b2g_sac_state_load(b2g_sac* h, const char* path);
+
 /* number of kernel launches one gradient step issues (bench.py's gpu_launches) */
 int b2g_launches_per_step(const b2g_sac* h);
 /* device-time of the last b2g_sac_step call measured with CUDA events on the handle's stream (ms) */
@@ -239,6 +254,11 @@ int b2g_bdq_step_explicit(b2g_bdq* h, const float* obs, const float* act_idx, co
                           float* td_out);
 /* greedy branch indices argmax_n Q_d(s, n) of the online network for n observations */
 int b2g_bdq_act(b2g_bdq* h, const float* obs, int n, int32_t* act_idx_out);
+/* training state, as b2g_sac_state_save / _load: online and target parameters, Adam moments, counters, n_updates, the live
+ * replay rows, the prioritised-replay sum / min trees, max priority and beta, and bdq/eps.  The fingerprint covers every
+ * b2g_bdq_cfg field that decides the layout or the prioritised replay. */
+int b2g_bdq_state_save(b2g_bdq* h, const char* path);
+int b2g_bdq_state_load(b2g_bdq* h, const char* path);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Row a12: auto-encoder ENCODER forward (perception for the `encoded depth` observation, SURVEY.md section 8).
