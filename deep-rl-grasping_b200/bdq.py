@@ -128,7 +128,8 @@ class BDQLearner:
         _lib.check(self.lib.b2g_bdq_set_per_beta(self.h, float(beta)))
 
     def last_per(self):
-        """Slots, importance weights and new priorities (sum_d |TD_d| + eps) of the last sampled step."""
+        """Slots, importance weights and new priorities (sum_d |TD_d| + eps) of the last sampled step.  The slots are valid
+        with uniform replay too (the Philox draw of the step); weights and priorities only with prioritised replay."""
         B = self.batch_size
         idx, w, p = np.empty(B, np.int32), np.empty(B, np.float32), np.empty(B, np.float32)
         _lib.check(self.lib.b2g_bdq_get_last_per(self.h, idx.ctypes.data_as(C.POINTER(C.c_int32)), _fp(w), _fp(p)))

@@ -656,6 +656,8 @@ int b2g_bdq_set_per_beta(b2g_bdq* h, float beta) {
   return 0;
 }
 
+// h->indices holds the slots of the last sampled step with uniform replay too (prep_kernel draws them, per_sample_kernel
+// overwrites them with PER); weights and prio_out are written by PER steps only
 int b2g_bdq_get_last_per(b2g_bdq* h, int32_t* slots, float* weights, float* priorities) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");

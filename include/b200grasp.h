@@ -245,7 +245,8 @@ int b2g_bdq_set_norm_stats(b2g_bdq* h, const double* obs_mean, const double* obs
 int b2g_bdq_step(b2g_bdq* h, int n_steps, float lr, b2g_bdq_metrics* out);
 /* prioritised replay: importance-sampling exponent beta of the NEXT sampled steps (SB anneals beta0 -> 1 over
  * prioritized_replay_beta_iters); last_out (may be NULL) = slots[batch], weights[batch], new priorities[batch] of the last
- * sampled step, for inspection / tests */
+ * sampled step, for inspection / tests.  The slots are valid with uniform replay too (prep_kernel's Philox draw); the
+ * weights and priorities are written by prioritised replay only. */
 int b2g_bdq_set_per_beta(b2g_bdq* h, float beta);
 int b2g_bdq_get_last_per(b2g_bdq* h, int32_t* slots, float* weights, float* priorities);
 /* parity entry point: caller-supplied batch (+ optional importance weights); td_out (may be NULL): [batch, n_branches] */

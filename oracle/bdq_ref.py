@@ -102,9 +102,11 @@ def q_values(p: Dict[str, torch.Tensor], obs: torch.Tensor, cfg: BDQConfig, scop
     return torch.stack(qs, 1)
 
 
-def bdq_step(params: Dict[str, np.ndarray], opt, batch: Dict[str, np.ndarray], lr: float, cfg: BDQConfig, dtype=torch.float32):
+def bdq_step(params: Dict[str, np.ndarray], opt, batch: Dict[str, np.ndarray], lr: float, cfg: BDQConfig, dtype=torch.float32,
+             a_star=None):
     """One train step.  batch: obs [B,obs], act_idx [B,D] (ints), rew [B], next_obs, done [B], weights [B] (IS weights,
-    ones without prioritised replay).  ``opt`` = dict(m, v, t).  Returns (outputs, grads, new_params, new_opt)."""
+    ones without prioritised replay).  ``opt`` = dict(m, v, t).  ``a_star`` [B,D] (optional) replaces the online net's
+    argmax at s' -- for rows whose top two advantages fp32 cannot order.  Returns (outputs, grads, new_params, new_opt)."""
     np_dt = np.float64 if dtype == torch.float64 else np.float32
     tp = {n: torch.tensor(np.asarray(a, np_dt), dtype=dtype, requires_grad=n.startswith("bdq/model/")) for n, a in params.items()}
     obs = torch.tensor(np.asarray(batch["obs"], np_dt), dtype=dtype)
@@ -116,7 +118,10 @@ def bdq_step(params: Dict[str, np.ndarray], opt, batch: Dict[str, np.ndarray], l
     q = q_values(tp, obs, cfg, "bdq/model", rescale=cfg.trunk_grad_rescale)
     q_sa = q.gather(2, act.unsqueeze(2)).squeeze(2)                       # [B, D]
     with torch.no_grad():
-        a_star = q_values(tp, nxt, cfg, "bdq/model").argmax(2)             # online net selects
+        if a_star is None:
+            a_star = q_values(tp, nxt, cfg, "bdq/model").argmax(2)         # online net selects
+        else:
+            a_star = torch.tensor(np.asarray(a_star, np.int64))
         q_t = q_values(tp, nxt, cfg, "bdq/target_q_func/model").gather(2, a_star.unsqueeze(2)).squeeze(2)
         y = rew + cfg.gamma * (1 - done) * q_t.mean(1)
     td = q_sa - y.unsqueeze(1)

@@ -6,7 +6,8 @@ import torch
 
 import b200grasp
 from oracle import bdq_ref as Q
-from tests.util import rel_err
+from tests.test_gpu_bdq_configs import CASES as BDQ_CASES
+from tests.test_gpu_bdq_configs import check_explicit
 
 pytestmark = pytest.mark.gpu
 
@@ -20,50 +21,14 @@ def _batch(cfg, B, seed):
 
 @pytest.mark.parametrize("cfg,B", [(Q.BDQConfig(100, 3, 8, (64, 64), 32, 32, 0.99), 64),
                                    (Q.BDQConfig(100, 5, 33, (64, 64), 32, 32, 0.99), 64),
-                                   (Q.BDQConfig(101, 3, 33, (512, 256), 128, 128, 1.0), 32)])
+                                   (Q.BDQConfig(101, 3, 33, (512, 256), 128, 128, 1.0), 32)]
+                         + [pytest.param(c.cfg, c.B, id=c.name) for c in BDQ_CASES])
 def test_bdq_step_matches_oracle(cfg, B):
-    params = Q.init_params(cfg, seed=1)
-    rng = np.random.default_rng(2)
-    for n in params:                       # non-trivial biases and a target net that differs from the online net
-        if n.endswith("biases"):
-            params[n] = (rng.normal(size=params[n].shape) * 0.1).astype(np.float32)
-        elif n.startswith("bdq/target_q_func") and n.endswith("weights"):
-            params[n] = (params[n] + rng.normal(size=params[n].shape).astype(np.float32) * 0.02).astype(np.float32)
-    L = b200grasp.BDQLearner(cfg.obs_dim, cfg.n_branches, cfg.n_bins, (cfg.trunk, (cfg.branch_hidden,), (cfg.value_hidden,)), batch_size=B,
-                             buffer_size=256, gamma=cfg.gamma, target_network_update_freq=2)
-    assert set(L.param_shapes) == set(n for n, _ in Q.all_specs(cfg))
-    L.load_parameters(params)
-    back = L.get_parameters()
-    for n in params:
-        assert np.array_equal(back[n], np.asarray(params[n], np.float32)), n
-    bt = _batch(cfg, B, 3)
-    w = np.random.default_rng(4).uniform(0.5, 1.5, B).astype(np.float32)
-    out = L.step_explicit(bt["obs"], bt["act_idx"].astype(np.float32), bt["rew"], bt["next_obs"], bt["done"], weights=w, lr=1e-3)
-    ref, grads, newp, opt = Q.bdq_step(params, {"t": 0, "m": {}, "v": {}}, dict(bt, weights=w), 1e-3, cfg, torch.float64)
-    assert abs(out["loss"] - ref["loss"]) <= 1e-4 * abs(ref["loss"])
-    assert abs(out["grad_norm"] - ref["grad_norm"]) <= 1e-4 * ref["grad_norm"]
-    assert rel_err(out["td"], ref["td"]) <= 1e-4
-    g = L.get_gradients()
-    for n in grads:
-        assert rel_err(g[n], grads[n]) <= 1e-3, (n, rel_err(g[n], grads[n]))
-    # second step: Adam state + hard target copy (freq 2)
-    bt2 = _batch(cfg, B, 5)
-    out2 = L.step_explicit(bt2["obs"], bt2["act_idx"].astype(np.float32), bt2["rew"], bt2["next_obs"], bt2["done"], lr=1e-3)
-    p32 = {n: np.asarray(a, np.float32) for n, a in newp.items()}
-    ref2, _, newp2, _ = Q.bdq_step(p32, opt, bt2, 1e-3, cfg, torch.float64)
-    assert abs(out2["loss"] - ref2["loss"]) <= 2e-3 * abs(ref2["loss"]) and out2["n_updates"] == 2
-    got = L.get_parameters()
-    k = "bdq/model/common_net/fully_connected_1/weights"
-    assert np.abs(got[k.replace("bdq/model", "bdq/target_q_func/model")] - got[k]).max() == 0.0          # hard copy happened
-    # greedy actions
-    idx = L.act(bt["obs"][:7])
-    ridx, _ = Q.greedy_action({n: got[n] for n in got}, bt["obs"][:7], cfg)
-    assert (idx == ridx).mean() >= 0.95
-    # sampled steps from the device replay
-    L.replay_add(bt["obs"], bt["act_idx"].astype(np.float32), bt["rew"], bt["next_obs"], bt["done"])
-    m = L.step(3, lr=1e-3)
-    assert m["n_updates"] == 5 and np.isfinite(m["loss"])
-    L.close()
+    """Two explicit steps against the float64 oracle (tests/test_gpu_bdq_configs.py::check_explicit): loss, mean_q, td and
+    grad_norm within 1e-4 relative, every gradient tensor within 1e-3 (or 3x the fp32 oracle's own error where larger), the
+    Adam update element-wise on the GPU's own gradients and against the oracle's update, the second step from the oracle's
+    moments, and the hard target copy.  At the three shipped-size configurations and every case of the BDQ matrix."""
+    check_explicit(cfg, B)
 
 
 def test_bdq_front_end_learn_predict_save_load(tmp_path):
