@@ -29,6 +29,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <map>
 #include <string>
 #include <vector>
@@ -586,6 +587,11 @@ int b2g_autoencoder_create(const b2g_encoder_cfg* cfg, b2g_autoencoder** out) {
   if (cfg->n_layers < 1 || cfg->n_layers > B2G_ENC_MAX_LAYERS) return b2g_fail(B2G_EINVAL, "n_layers out of range");
   if (cfg->height < 1 || cfg->width < 1 || cfg->encoding_dim < 1 || cfg->max_batch < 1)
     return b2g_fail(B2G_EINVAL, "non-positive dimension");
+  // The backward takes the LeakyReLU derivative from the sign of the stored output; with alpha < 0 a negative
+  // pre-activation stores a positive value, so its derivative would come out as 1 instead of alpha.
+  if (!(cfg->alpha >= 0.f) || !std::isfinite(cfg->alpha))
+    return b2g_fail(B2G_EINVAL, "the auto-encoder trains with alpha >= 0 only (alpha = " + std::to_string(cfg->alpha) +
+                                    "): its backward reads the LeakyReLU derivative from the sign of the stored output");
   if (cfg->channels != 1) return b2g_fail(B2G_EINVAL, "the auto-encoder reconstructs one-channel images (channels must be 1)");
   for (int l = 0; l < cfg->n_layers; ++l)
     if (cfg->filters[l] < 1 || (cfg->filters[l] & 3)) return b2g_fail(B2G_EINVAL, "auto-encoder filters must be multiples of 4");
@@ -629,8 +635,13 @@ int b2g_autoencoder_create(const b2g_encoder_cfg* cfg, b2g_autoencoder** out) {
   const int PW = AE_TILE + og.k - 1;
   const size_t smem_fwd = ((size_t)og.k * og.k * og.in_c + (size_t)PW * PW * (og.in_c + 1)) * sizeof(float);
   const size_t smem_wg = (size_t)PW * PW * (og.in_c + 1) * sizeof(float);
-  if ((size_t)og.k * og.k * og.in_c > 256 * AE_WG_OUT || smem_fwd > AE_MAX_SMEM)
-    return b2g_fail(B2G_EINVAL, "output conv too large: kernel_0^2 * filters_0 must be <= 2048");
+  if ((size_t)og.k * og.k * og.in_c > 256 * AE_WG_OUT)
+    return b2g_fail(B2G_EINVAL, "output conv too large: kernel_0^2 * filters_0 = " + std::to_string(og.k * og.k * og.in_c) +
+                                    " must be <= 2048");
+  if (smem_fwd > AE_MAX_SMEM)
+    return b2g_fail(B2G_EINVAL, "output conv too large: its forward needs " + std::to_string(smem_fwd) +
+                                    " B of shared memory ((kernel_0^2 * filters_0 + (kernel_0 + 7)^2 * (filters_0 + 1)) * 4), "
+                                    "more than 98304");
   if (int rc = check_device(cfg->device)) return rc;
 
   b2g_autoencoder* h = new b2g_autoencoder();

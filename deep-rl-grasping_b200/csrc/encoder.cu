@@ -106,17 +106,20 @@ int b2g_encoder_create(const b2g_encoder_cfg* cfg, b2g_encoder** out) {
   if (cfg->n_layers < 1 || cfg->n_layers > B2G_ENC_MAX_LAYERS) return b2g_fail(B2G_EINVAL, "n_layers out of range");
   if (cfg->height < 1 || cfg->width < 1 || cfg->channels < 1 || cfg->encoding_dim < 1 || cfg->max_batch < 1)
     return b2g_fail(B2G_EINVAL, "non-positive dimension");
+  std::vector<EncLayer> layers;
+  if (int rc = enc_geometry(*cfg, layers)) return rc;
+  const size_t N = cfg->max_batch;
+  // every offset table is int: each layer's bordered input (the dense layer's is the flattened last conv output) and z
+  size_t biggest = N * (size_t)layers.back().fs;
+  for (const auto& y : layers) biggest = std::max(biggest, N * y.hp * y.wp * y.in_c);
+  if (biggest > (size_t)((1u << 31) - 1)) return b2g_fail(B2G_EINVAL, "max_batch too large for 32-bit offset tables");
   if (int rc = check_device(cfg->device)) return rc;
   b2g_encoder* h = new b2g_encoder();
   h->cfg = *cfg;
+  h->layers = layers;
   auto bail = [&](int rc) { b2g_encoder_destroy(h); return rc; };
   if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream create"));
-  if (int rc = enc_geometry(*cfg, h->layers)) return bail(rc);
   const EncLayer& dn = h->layers.back();
-  const size_t N = cfg->max_batch;
-  if (N * (size_t)h->layers[0].hp * h->layers[0].wp * cfg->channels > (1ull << 31) - 1 ||
-      N * (size_t)h->layers[0].out_h * h->layers[0].out_w * h->layers[0].fs > (1ull << 31) - 1)
-    return bail(b2g_fail(B2G_EINVAL, "max_batch too large for 32-bit offset tables"));
   int rc;
   for (auto& y : h->layers) {
     if ((rc = dev_alloc(h->allocs, h->stream, &y.in, N * y.hp * y.wp * y.in_c))) return bail(rc);

@@ -267,7 +267,10 @@ int b2g_bdq_state_load(b2g_bdq* h, const char* path);
  * called per env step from EncodedDepthImgSensor.get_state (manipulation_main/gripperEnv/sensor.py:218-222).
  * Layer spec = config.yaml `network` (filters / kernel_size / strides, padding 'same'), LeakyReLU(alpha) after every
  * conv and after Dense(encoding_dim).  Weights are the Keras arrays from model.h5: conv kernels [k,k,in,out], dense
- * kernel [flat,out] (flatten order H,W,C), biases [out].
+ * kernel [flat,out] (flatten order H,W,C), biases [out].  Any alpha is accepted (the forward applies it as given).
+ * b2g_encoder_create returns B2G_EINVAL, before it touches a device, for a bad layer spec, hidden filter counts that are
+ * not multiples of 4, a flattened size that is not a multiple of 4, or a max_batch at which any layer's zero-bordered
+ * input (the dense layer's input included) holds more than 2^31 - 1 floats.
  * ------------------------------------------------------------------------------------------------------------ */
 #define B2G_ENC_MAX_LAYERS 8
 typedef struct b2g_encoder b2g_encoder;
@@ -298,7 +301,11 @@ int b2g_encoder_encode(b2g_encoder* h, const float* imgs, int n, float* out);
  * kernel_i, 'same') + LeakyReLU, then UpSampling2D(strides_0) + Conv2D(1, kernel_0, 'same').
  * Layers are numbered in model.h5 order: encoder convs, encoder dense, decoder dense, decoder convs, output conv
  * (2 * n_layers + 2); weights use the Keras layouts of b2g_encoder_set_weights.  Requires channels == 1, every filter
- * count a multiple of 4 and a decoder that returns to height x width (else B2G_EINVAL).  max_batch is the largest
+ * count a multiple of 4 and a decoder that returns to height x width (else B2G_EINVAL).  alpha must be finite and >= 0:
+ * the backward reads the LeakyReLU derivative from the sign of the stored output, which cannot tell a negative
+ * pre-activation from a positive one when alpha < 0.  The output conv (1 filter, kernel_0, filters_0 inputs) needs
+ * kernel_0^2 * filters_0 <= 2048 and (kernel_0^2 * filters_0 + (kernel_0 + 7)^2 * (filters_0 + 1)) * 4 <= 98304 bytes of
+ * shared memory.  Every one of these refusals comes before any device is touched.  max_batch is the largest
  * batch of any call.  Calls that run the model return B2G_ESTATE until every layer has weights.
  * ------------------------------------------------------------------------------------------------------------ */
 typedef struct b2g_autoencoder b2g_autoencoder;

@@ -43,41 +43,52 @@ def shipped():
     return dict(cfg, learning_rate=2e-4, batch_size=128), arrays
 
 
-def glorot(cfg, seed=3):
-    return glorot_init(model_shapes(cfg["network"], cfg["encoding_dim"]), np.random.default_rng(seed))
+def glorot(cfg, seed=3, input_shape=(64, 64, 1)):
+    return glorot_init(model_shapes(cfg["network"], cfg["encoding_dim"], input_shape), np.random.default_rng(seed))
 
 
-def grad_bars(arrays, x, cfg, ref):
+def grad_bars(arrays, x, cfg, ref, t=None):
     """Gradient bar of each tensor: 1e-4 of its largest element, or 3x the distance of the fp32 oracle from the float64 one
     when fp32 itself cannot resolve the tensor that well: a LeakyReLU input within fp32 rounding of zero takes slope 1 on one
-    side and alpha on the other, and which side an fp32 forward lands on is decided by rounding."""
-    _, r32 = R.loss_and_grads(arrays, x, x, cfg["network"], cfg["alpha"], torch.float32)
+    side and alpha on the other, and which side an fp32 forward lands on is decided by rounding.  t: the targets (None: x)."""
+    _, r32 = R.loss_and_grads(arrays, x, x if t is None else t, cfg["network"], cfg["alpha"], torch.float32)
     return [max(1e-4, 3 * rel_err(a32, a64)) for kb32, kb64 in zip(r32, ref) for a32, a64 in zip(kb32, kb64)]
 
 
-def check_step(cfg, arrays, x):
-    """Loss and every gradient of one explicit step against the float64 oracle."""
-    ae = SimpleAutoEncoder(cfg, max_batch=1)
+def check_step(cfg, arrays, x, t=None, cls=SimpleAutoEncoder):
+    """Loss and every gradient of one explicit step against the float64 oracle.  t: the targets (None: the inputs);
+    cls: the model class, whose input_shape sets the image geometry."""
+    ae = cls(cfg, max_batch=1)
     ae.set_model_weights(arrays)
-    loss, grads = ae.step(x, apply_update=False)
-    ref_loss, ref = R.loss_and_grads(arrays, x, x, cfg["network"], cfg["alpha"])
+    loss, grads = ae.step(x, t, apply_update=False)
+    ref_loss, ref = R.loss_and_grads(arrays, x, x if t is None else t, cfg["network"], cfg["alpha"])
     assert abs(loss - ref_loss) <= 1e-5 * ref_loss, (loss, ref_loss)
-    bars = grad_bars(arrays, x, cfg, ref)
+    bars = grad_bars(arrays, x, cfg, ref, t)
     for i, (a, b) in enumerate(zip((a for kb in grads for a in kb), (b for kb in ref for b in kb))):
         assert rel_err(a, b) <= bars[i], (i, rel_err(a, b), bars[i])
     ae.close()
     return ref
 
 
-def check_updates(cfg, arrays, batches):
+def explicit_step(ae, s, x, t):
+    """The default step of check_updates: one explicit Adam step on the host batch; returns (loss, gradients)."""
+    return ae.step(x, t)
+
+
+def check_updates(cfg, arrays, batches, cls=SimpleAutoEncoder, step=explicit_step):
     """Parameter change of every Adam step and of the whole run, against Keras Adam in float64 applied along the GPU's own
     trajectory: at each step the oracle takes the float64 gradient at the GPU's current parameters (the GPU's gradient must
     be within the gradient bar of it, see grad_bars) and its own moments.  The two updates may then
     differ by 1e-3 of the largest update plus what a gradient error at that bar, carried in Adam's moments, can move:
     Keras Adam moves every weight by about lr whatever the size of its gradient (eps = 1e-7), so a gradient that fp32
     cannot resolve still moves its weight by up to 2 lr.  Anchoring each step at the GPU's parameters keeps the comparison
-    from following two trajectories that drift apart through exactly those weights."""
-    ae = SimpleAutoEncoder(cfg, max_batch=1)
+    from following two trajectories that drift apart through exactly those weights.  One ulp of each fp32 parameter is
+    added to its allowance at every step: the GPU cannot store a change more finely than that.
+
+    batches: host batches x, or (inputs, targets) pairs.  step(ae, s, x, t) makes the GPU's Adam step s on that batch (t is
+    None when the targets are the inputs) and returns (its loss, taken before the update, and its gradients); an epoch
+    whose order covers exactly that batch can stand in for the explicit step."""
+    ae = cls(cfg, max_batch=1)
     ae.set_model_weights(arrays)
     opt = R.Adam(arrays, cfg["learning_rate"])
     p0 = [np.array(a, np.float64) for kb in ae.get_weights() for a in kb]
@@ -86,12 +97,14 @@ def check_updates(cfg, arrays, batches):
     total_ref = [np.zeros(a.shape) for a in p0]
     total_allow = [np.zeros(a.shape) for a in p0]
     cur = p0
-    for s, x in enumerate(batches):
+    for s, b in enumerate(batches):
+        x, t = b if isinstance(b, tuple) else (b, None)
         opt.p = [a.copy() for a in cur]
-        _, g = R.loss_and_grads(opt.arrays(), x, x, cfg["network"], cfg["alpha"])
-        _, gg = ae.step(x)
+        ref_loss, g = R.loss_and_grads(opt.arrays(), x, x if t is None else t, cfg["network"], cfg["alpha"])
+        loss, gg = step(ae, s, x, t)
+        assert abs(loss - ref_loss) <= 1e-5 * ref_loss, (s + 1, loss, ref_loss)
         gflat = [a for kb in g for a in kb]
-        bars = grad_bars(opt.arrays(), x, cfg, g)
+        bars = grad_bars(opt.arrays(), x, cfg, g, t)
         for i, (a, b) in enumerate(zip(gflat, (b for kb in gg for b in kb))):
             assert rel_err(b, a) <= bars[i], (s + 1, i, rel_err(b, a), bars[i])
             d = bars[i] * np.abs(a).max()
@@ -103,11 +116,14 @@ def check_updates(cfg, arrays, batches):
         nxt = [np.array(a, np.float64) for kb in ae.get_weights() for a in kb]
         errs = []
         for i in range(len(p0)):
+            # each parameter is stored in fp32, so its change is resolved only to an ulp of the parameter; that matters
+            # where the gradient is so small that Adam's eps shrinks the whole update to a few ulps (deep, narrow nets)
+            allow[i] = allow[i] + np.spacing(np.maximum(np.abs(cur[i]), np.abs(nxt[i])).astype(np.float32)).astype(np.float64)
             total_ref[i] += u_ref[i]
             total_allow[i] += allow[i]
             for got, ref, al in ((nxt[i] - cur[i], u_ref[i], allow[i]), (nxt[i] - p0[i], total_ref[i], total_allow[i])):
                 over = np.abs(got - ref) - 1e-3 * np.abs(ref).max() - al
-                errs.append((i, float(over.max()), float(np.abs(got - ref).max() / np.abs(ref).max())))
+                errs.append((i, float(over.max()), float(np.abs(got - ref).max() / np.abs(ref).max()), float(np.abs(ref).max())))
         assert all(e[1] <= 0 for e in errs), (s + 1, [e for e in errs if e[1] > 0])
         cur = nxt
     ae.close()
