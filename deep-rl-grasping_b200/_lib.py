@@ -21,6 +21,7 @@ SYMBOLS = [
     "b2g_reset_optimizer", "b2g_replay_add", "b2g_replay_size", "b2g_replay_get", "b2g_replay_info", "b2g_get_last_batch", "b2g_set_norm_stats", "b2g_sac_step",
     "b2g_sac_step_async", "b2g_sac_step_explicit", "b2g_sac_step_host_pipelined", "b2g_sac_pipeline_flush", "b2g_sac_act", "b2g_launches_per_step", "b2g_last_step_ms",
     "b2g_profile_step", "b2g_sac_state_save", "b2g_sac_state_load",
+    "b2g_sac_observe_act", "b2g_sac_observe_add", "b2g_obs_rms_set", "b2g_obs_rms_get", "b2g_upload_bytes",
     "b2g_bdq_create", "b2g_bdq_destroy", "b2g_bdq_param_count", "b2g_bdq_param_info", "b2g_bdq_get_param", "b2g_bdq_set_param",
     "b2g_bdq_get_grad", "b2g_bdq_replay_add", "b2g_bdq_replay_size", "b2g_bdq_set_norm_stats", "b2g_bdq_step",
     "b2g_bdq_step_explicit", "b2g_bdq_act", "b2g_bdq_set_per_beta", "b2g_bdq_get_last_per", "b2g_bdq_state_save", "b2g_bdq_state_load",
@@ -133,6 +134,11 @@ def load():
     lib.b2g_sac_step_host_pipelined.argtypes = [vp, fp, fp, fp, fp, fp, fp, C.c_float, C.POINTER(SacMetrics), C.POINTER(C.c_int)]
     lib.b2g_sac_pipeline_flush.argtypes = [vp, C.POINTER(SacMetrics)]
     lib.b2g_sac_act.argtypes = [vp, fp, C.c_int, C.c_int, fp]
+    lib.b2g_sac_observe_act.argtypes = [vp, fp, C.c_int, C.c_int, C.c_int, fp]
+    lib.b2g_sac_observe_add.argtypes = [vp, fp, fp, fp, fp, fp, C.c_int, C.c_int]
+    lib.b2g_obs_rms_set.argtypes = [vp, dp, dp, C.c_double]
+    lib.b2g_obs_rms_get.argtypes = [vp, dp, dp, dp]
+    lib.b2g_upload_bytes.argtypes = [vp, i64p, i64p]
     lib.b2g_launches_per_step.argtypes = [vp]
     lib.b2g_last_step_ms.argtypes = [vp]
     lib.b2g_last_step_ms.restype = C.c_float

@@ -1,6 +1,7 @@
 // libb200grasp: SAC learner handle, HBM layout, offset tables, step orchestration, C ABI.
 //
-// HBM layout (all fp32 unless noted; everything is allocated once in b2g_sac_create):
+// HBM layout (all fp32 unless noted; everything is allocated once in b2g_sac_create, except the opt-in obs_rms and observe
+// staging of obsnorm.cu, allocated by b2g_obs_rms_set and the first b2g_sac_observe_* call):
 //   P  : parameter arena  [ model/pi | model/values_fn | log_ent_coef | target/values_fn ], every
 //        tensor padded to 32 floats, tensor order = SB zip parameter_list (SURVEY.md Appendix B)
 //   Mo, Vo, G : Adam moments and gradients, same offsets as the trainable part of P
@@ -937,6 +938,71 @@ int full_index(const b2g_sac* h, int e) {
   return e == npx ? Ci : -1;
 }
 
+// next frame id; a frame that would overwrite one a live transition references drops the oldest transitions first
+int64_t alloc_frame(b2g_sac* h) {
+  const int64_t f = h->next_fid++, over = f - h->frame_cap;
+  while (h->head_seq > h->tail_seq) {
+    while (h->lw.front().first < h->tail_seq) h->lw.pop_front();
+    if (h->lw.front().second > over) break;
+    ++h->tail_seq; ++h->evicted;
+  }
+  return f;
+}
+
+FrameIo frame_io(const b2g_sac* h, const float* c_obs, const float* c_next) {
+  FrameIo io{};
+  io.c_obs = c_obs; io.c_next = c_next; io.frames = h->frames; io.frame_bytes = h->frame_bytes;
+  io.fmt = h->fmt; io.npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0; io.Ci = h->cnn ? h->Cimg : 1; io.Ec = h->Ec;
+  return io;
+}
+
+// rows per commit launch: one launch writes distinct transition slots and distinct frames
+int64_t commit_rows(const b2g_sac* h) { return std::min<int64_t>({(int64_t)h->stage_rows, h->cfg.buffer_capacity, h->frame_cap / 2}); }
+
+// Stores m <= commit_rows(h) transitions whose compact rows sit at io.c_obs / io.c_next: plans their frames, commits them and
+// copies act / rew / done (host or device memory) into the ring.  cand[i] >= 0 names a frame that already holds c_obs[i]: it
+// is shared while it outlives the allocation of this row's next_obs frame.  next_ids[i] receives the frame id of c_next[i].
+// h_plan must be free (the previous chunk's upload has run); everything is enqueued on h->stream.
+int commit_chunk(b2g_sac* h, const FrameIo& io, int m, const int64_t* cand, const float* act, const float* rew, const float* done,
+                 int64_t* next_ids) {
+  const int64_t cap = h->cfg.buffer_capacity, FC = h->frame_cap;
+  const size_t A = h->A;
+  const int64_t first = h->head_seq, fid0 = h->next_fid;
+  for (int i = 0; i < m; ++i) {
+    if (h->head_seq - h->tail_seq == cap) ++h->tail_seq;                       // the ring's own replacement
+    const int64_t p = cand[i];
+    const bool share = h->dedup && p >= 0 && p >= h->next_fid + 1 - FC;
+    const int64_t of = share ? p : alloc_frame(h);
+    const int64_t nf = alloc_frame(h);
+    while (!h->lw.empty() && h->lw.back().second >= of) h->lw.pop_back();
+    h->lw.emplace_back(h->head_seq++, of);
+    h->h_plan[i] = (int)(of % FC); h->h_plan[m + i] = share ? 0 : 1; h->h_plan[2 * m + i] = (int)(nf % FC);
+    next_ids[i] = nf;
+  }
+  if (h->dedup) CK(cudaMemcpyAsync(h->d_plan, h->h_plan, 3 * m * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  frame_commit_launch(io, h->dedup ? h->d_plan : nullptr, fid0, FC, m, h->r_ofr, h->r_nfr, first, cap, h->stream);
+  for (int64_t k = 0; k < m;) {          // act / rew / done into slots (first + k) % cap, in at most two pieces
+    const int64_t pos = (first + k) % cap, len = std::min<int64_t>(m - k, cap - pos);
+    CK(cudaMemcpyAsync(h->r_act + pos * A, act + k * A, len * A * sizeof(float), cudaMemcpyDefault, h->stream));
+    CK(cudaMemcpyAsync(h->r_rew + pos, rew + k, len * sizeof(float), cudaMemcpyDefault, h->stream));
+    CK(cudaMemcpyAsync(h->r_done + pos, done + k, len * sizeof(float), cudaMemcpyDefault, h->stream));
+    k += len;
+  }
+  return 0;
+}
+
+// After the last chunk of a call: the next call's sharing candidates, and the replay size / first live slot the sampler reads
+// (it draws u in [0, size) and reads slot (first live + u) % cap; the first live slot is 0 unless transitions went early).
+int commit_finish(b2g_sac* h, std::vector<int64_t>& next_ids) {
+  const int64_t cap = h->cfg.buffer_capacity;
+  h->prev_next.swap(next_ids);
+  h->r_size = h->head_seq - h->tail_seq;
+  h->h_rc[0] = h->r_size;
+  h->h_rc[1] = h->r_size == cap ? 0 : h->tail_seq % cap;
+  CK(cudaMemcpyAsync(h->counters + 5, h->h_rc, 2 * sizeof(long long), cudaMemcpyHostToDevice, h->stream));
+  return 0;
+}
+
 // n caller observations (host or device memory) -> rows (first + i) % wrap of dst in the ring layout, on h->stream.  CNN: copied in
 // pieces through the full-layout staging buffer and compacted (stream order frees the buffer for the next piece); MLP: a plain
 // copy, for which first + n <= wrap.
@@ -955,6 +1021,42 @@ int load_rows(b2g_sac* h, const float* src, float* dst, long long first, long lo
 }
 
 }  // namespace
+
+// ================================================================================================
+// hooks of the observe path (obsnorm.cu; contracts in sac_internal.cuh)
+// ================================================================================================
+namespace b2g {
+
+int sac_act_rows(b2g_sac* h, const float* rows, int chunk, int deterministic) {
+  refresh_planes(h);
+  prep_launch(make_prep(h, h->cfg.seed ^ 0xA5A5A5A5DEADBEEFull, !deterministic, false), h->stream);
+  GatherArgs g = make_gather(h, false, false);
+  g.obs = rows;
+  gather_launch(g, h->stream);
+  for (auto& gr : h->act_groups) {
+    if (gr.tc) CK(gg_tc_launch(gr.host.data(), (int)gr.host.size(), gr.total_tiles, gr.host[0].flags, h->cfg.precision == B2G_PREC_BF16X3 ? 1 : 0, h->num_sms, h->stream));
+    else gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
+  }
+  CK(b2g::act_launch(make_tail(h, false), chunk, deterministic, h->pi_out, h->stream));
+  return 0;
+}
+
+int sac_replay_add_linked(b2g_sac* h, const float* c_obs, const float* c_next, const int64_t* obs_fid, const float* act,
+                          const float* rew, const float* done, int n, int64_t* next_fid) {
+  const int64_t R = commit_rows(h);
+  const size_t A = h->A, Ec = h->Ec;
+  std::vector<int64_t> next_ids((size_t)n);
+  for (int64_t c0 = 0; c0 < n; c0 += R) {
+    const int m = (int)std::min<int64_t>(R, n - c0);
+    if (c0 > 0) CK(cudaStreamSynchronize(h->stream));        // the previous chunk's plan upload has left h_plan
+    if (int rc = commit_chunk(h, frame_io(h, c_obs + c0 * Ec, c_next + c0 * Ec), m, obs_fid + c0, act + c0 * A, rew + c0, done + c0,
+                              next_ids.data() + c0)) return rc;
+  }
+  std::copy(next_ids.begin(), next_ids.end(), next_fid);
+  return commit_finish(h, next_ids);
+}
+
+}  // namespace b2g
 
 // ================================================================================================
 // C ABI
@@ -1342,13 +1444,10 @@ int b2g_replay_add(b2g_sac* h, const float* obs, const float* act, const float* 
   if (!h || !obs || !act || !rew || !next_obs || !done || n < 0) return b2g_fail(B2G_EINVAL, "NULL argument");
   if (h->dedup && 2 * n > h->frame_cap) return b2g_fail(B2G_EINVAL, "replay_add: 2 n rows exceed frame_capacity");
   CK(cudaSetDevice(h->cfg.device));
-  const int64_t cap = h->cfg.buffer_capacity, FC = h->frame_cap;
-  // rows per chunk: one commit launch writes distinct transition slots and distinct frames
-  const int64_t R = std::min<int64_t>({(int64_t)h->stage_rows, cap, FC / 2});
+  const int64_t FC = h->frame_cap;
+  const int64_t R = commit_rows(h);
   const size_t E = h->E, A = h->A;
-  FrameIo io{};
-  io.c_obs = h->c_obs; io.c_next = h->c_next; io.frames = h->frames; io.frame_bytes = h->frame_bytes;
-  io.fmt = h->fmt; io.npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0; io.Ci = h->cnn ? h->Cimg : 1; io.Ec = h->Ec;
+  const FrameIo io = frame_io(h, h->c_obs, h->c_next);
   int* flags = h->h_plan + 3 * R;
   // rows [c0, c0 + m) -> compact staging, then (when sharing frames or checking 8-bit values) frame_check -> flags, synchronised
   auto stage_check = [&](int64_t c0, int m, bool check) -> int {
@@ -1372,49 +1471,18 @@ int b2g_replay_add(b2g_sac* h, const float* obs, const float* act, const float* 
   if (h->u8_mask && n > R)
     for (int64_t c0 = 0; c0 < n; c0 += R)
       if (int rc = stage_check(c0, (int)std::min<int64_t>(R, n - c0), true)) return rc;
-  // next frame id; a frame that would overwrite one a live transition references drops the oldest transitions first
-  auto alloc_frame = [&]() -> int64_t {
-    const int64_t f = h->next_fid++, over = f - FC;
-    while (h->head_seq > h->tail_seq) {
-      while (h->lw.front().first < h->tail_seq) h->lw.pop_front();
-      if (h->lw.front().second > over) break;
-      ++h->tail_seq; ++h->evicted;
-    }
-    return f;
-  };
-  std::vector<int64_t> next_ids((size_t)n);
+  std::vector<int64_t> next_ids((size_t)n), cand((size_t)R);
   for (int64_t c0 = 0; c0 < n; c0 += R) {
     const int m = (int)std::min<int64_t>(R, n - c0);
     if (int rc = stage_check(c0, m, h->dedup || (h->u8_mask && n <= R))) return rc;
-    const int64_t first = h->head_seq, fid0 = h->next_fid;
-    for (int i = 0; i < m; ++i) {
-      if (h->head_seq - h->tail_seq == cap) ++h->tail_seq;                       // the ring's own replacement
+    for (int i = 0; i < m; ++i) {      // the previous call's next_obs of row i, where frame_check found it equal bit for bit
       const int64_t p = c0 + i < (int64_t)h->prev_next.size() ? h->prev_next[c0 + i] : -1;
-      // shared only while the frame outlives the allocation of this row's next_obs frame
-      const bool share = h->dedup && (flags[i] & 1) && p >= h->next_fid + 1 - FC;
-      const int64_t of = share ? p : alloc_frame();
-      const int64_t nf = alloc_frame();
-      while (!h->lw.empty() && h->lw.back().second >= of) h->lw.pop_back();
-      h->lw.emplace_back(h->head_seq++, of);
-      h->h_plan[i] = (int)(of % FC); h->h_plan[m + i] = share ? 0 : 1; h->h_plan[2 * m + i] = (int)(nf % FC);
-      next_ids[c0 + i] = nf;
+      cand[i] = h->dedup && (flags[i] & 1) ? p : -1;
     }
-    if (h->dedup) CK(cudaMemcpyAsync(h->d_plan, h->h_plan, 3 * m * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    frame_commit_launch(io, h->dedup ? h->d_plan : nullptr, fid0, FC, m, h->r_ofr, h->r_nfr, first, cap, h->stream);
-    for (int64_t k = 0; k < m;) {          // act / rew / done into slots (first + k) % cap, in at most two pieces
-      const int64_t pos = (first + k) % cap, len = std::min<int64_t>(m - k, cap - pos);
-      CK(cudaMemcpyAsync(h->r_act + pos * A, act + (c0 + k) * A, len * A * sizeof(float), cudaMemcpyDefault, h->stream));
-      CK(cudaMemcpyAsync(h->r_rew + pos, rew + c0 + k, len * sizeof(float), cudaMemcpyDefault, h->stream));
-      CK(cudaMemcpyAsync(h->r_done + pos, done + c0 + k, len * sizeof(float), cudaMemcpyDefault, h->stream));
-      k += len;
-    }
+    if (int rc = commit_chunk(h, io, m, cand.data(), act + c0 * A, rew + c0, done + c0, next_ids.data() + c0)) return rc;
   }
-  h->prev_next.swap(next_ids);
-  h->r_size = h->head_seq - h->tail_seq;
-  // sampling draws u in [0, size) and reads slot (first live + u) % cap; the first live slot is 0 unless transitions went early
-  h->h_rc[0] = h->r_size;
-  h->h_rc[1] = h->r_size == cap ? 0 : h->tail_seq % cap;
-  CK(cudaMemcpyAsync(h->counters + 5, h->h_rc, 2 * sizeof(long long), cudaMemcpyHostToDevice, h->stream));
+  h->up_other += (int64_t)(n * (2 * E + A + 2) * sizeof(float));
+  if (int rc = commit_finish(h, next_ids)) return rc;
   CK(cudaStreamSynchronize(h->stream));     // host arrays are caller-owned: copied before return
   return 0;
 }
@@ -1498,8 +1566,20 @@ int b2g_set_norm_stats(b2g_sac* h, const double* obs_mean, const double* obs_var
                        double eps, int norm_obs, int norm_reward) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  if (norm_obs && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
+  if (norm_obs && !h->rms_mean && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
   CK(cudaSetDevice(h->cfg.device));
+  const bool eps_changed = eps != h->norm_eps;
+  h->norm_eps = eps;
+  if (h->rms_mean) {
+    // the handle owns obs_rms: statistics passed here replace it (count kept), and the table the gather reads is derived on
+    // the device, again when only epsilon changed
+    if (obs_mean && obs_var) {
+      if (int rc = b2g_obs_rms_set(h, obs_mean, obs_var, h->rms_count)) return rc;
+    } else if (eps_changed) {
+      obs_rms_derive(h);
+    }
+    obs_mean = obs_var = nullptr;
+  }
   // Called once per environment step by the learn loop (VecNormalize statistics move with every observation): the values
   // are staged in one of two pinned buffers and uploaded asynchronously IN STREAM ORDER -- no stream synchronisation, the
   // next gradient step simply sees them.  A buffer is reused only after its previous upload has completed.
@@ -1507,7 +1587,7 @@ int b2g_set_norm_stats(b2g_sac* h, const double* obs_mean, const double* obs_var
   CK(cudaEventSynchronize(h->ev_stats[k]));
   double* st = h->hp_stats[k];
   const int Ec = h->Ec;
-  if (norm_obs) {     // the caller's full-layout statistics, gathered into the ring layout
+  if (norm_obs && obs_mean) {     // the caller's full-layout statistics, gathered into the ring layout
     double* m = st; double* is = st + Ec;
     for (int e = 0; e < Ec; ++e) {
       const int f = full_index(h, e);
@@ -1516,12 +1596,14 @@ int b2g_set_norm_stats(b2g_sac* h, const double* obs_mean, const double* obs_var
     }
     CK(cudaMemcpyAsync(h->d_mean, m, Ec * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_istd, is, Ec * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    h->up_other += (int64_t)(2 * h->E * sizeof(double));
   }
   h->ret_istd = 1.0 / sqrt(ret_var + eps);
   h->clip_obs = clip_obs; h->clip_rew = clip_rew; h->norm_obs = norm_obs; h->norm_rew = norm_reward;
   double* nc = st + 2 * Ec;
   nc[0] = h->ret_istd; nc[1] = clip_obs; nc[2] = clip_rew; nc[3] = (double)norm_obs; nc[4] = (double)norm_reward; nc[5] = nc[6] = nc[7] = 0.0;
   CK(cudaMemcpyAsync(h->d_normc, nc, 8 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  h->up_other += 8 * sizeof(double);
   CK(cudaEventRecord(h->ev_stats[k], h->stream));
   return 0;
 }
@@ -1736,19 +1818,11 @@ int b2g_sac_act(b2g_sac* h, const float* obs, int n, int deterministic, float* a
   if (!h || !obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
   CK(cudaSetDevice(h->cfg.device));
   const size_t E = h->E, A = h->A;
-  refresh_planes(h);
   for (int done_n = 0; done_n < n; done_n += h->B) {
     const int chunk = std::min(h->B, n - done_n);
     if (int rc = load_rows(h, obs + (size_t)done_n * E, h->s_obs, 0, h->B, chunk)) return rc;
-    prep_launch(make_prep(h, h->cfg.seed ^ 0xA5A5A5A5DEADBEEFull, !deterministic, false), h->stream);
-    GatherArgs g = make_gather(h, false, false);
-    g.indices = nullptr;
-    gather_launch(g, h->stream);
-    for (auto& gr : h->act_groups) {
-      if (gr.tc) CK(gg_tc_launch(gr.host.data(), (int)gr.host.size(), gr.total_tiles, gr.host[0].flags, h->cfg.precision == B2G_PREC_BF16X3 ? 1 : 0, h->num_sms, h->stream));
-      else gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
-    }
-    CK(b2g::act_launch(make_tail(h, false), chunk, deterministic, h->pi_out, h->stream));
+    h->up_other += (int64_t)(chunk * E * sizeof(float));
+    if (int rc = sac_act_rows(h, h->s_obs, chunk, deterministic)) return rc;
     CK(cudaMemcpyAsync(act_out + (size_t)done_n * A, h->pi_out, chunk * A * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
   }
@@ -1803,6 +1877,14 @@ std::vector<FpField> sac_fingerprint(const b2g_sac* h) {
           fp_int("u8_plane_mask", h->u8_mask), fp_real("gamma", c.gamma), fp_real("tau", c.tau),
           fp_real("target_entropy", c.target_entropy), fp_int("seed", (int64_t)c.seed)};
 }
+// a handle that owns obs_rms writes one more field and one more section (count, mean[E], var[E] as float64); one that does not
+// reads and writes the files it always did
+std::vector<FpField> sac_fingerprint_rms(const b2g_sac* h) {
+  std::vector<FpField> fp = sac_fingerprint(h);
+  if (h->rms_mean) fp.push_back(fp_int("obs_rms", 1));
+  return fp;
+}
+const uint32_t kRmsTag = state_tag("ORMS");
 
 // Host replay bookkeeping as stored: r_size, head_seq, tail_seq, next_fid, evicted, |lw|, |prev_next|, lw pairs, prev_next.
 struct SacHostState {
@@ -1883,7 +1965,14 @@ int b2g_sac_state_save(b2g_sac* h, const char* path) {
   secs[0].tag = kSacTags[0]; secs[0].pieces = {host_piece(hv.data(), hv.size() * sizeof(int64_t))};
   secs[1].tag = kSacTags[1]; secs[1].pieces = {host_piece(cnt, sizeof cnt)};
   for (auto& s : sac_device_sections(h, hs.frame_lo(h->frame_cap), hs.next_fid)) secs.push_back(std::move(s));
-  return state_write(path, STATE_KIND_SAC, sac_fingerprint(h), secs);
+  if (h->rms_mean) {
+    StateSection r;
+    r.tag = kRmsTag;
+    r.pieces = {host_piece(&h->rms_count, sizeof(double)), dev_piece(h->rms_mean, h->E * sizeof(double)),
+                dev_piece(h->rms_var, h->E * sizeof(double))};
+    secs.push_back(std::move(r));
+  }
+  return state_write(path, STATE_KIND_SAC, sac_fingerprint_rms(h), secs);
 }
 
 int b2g_sac_state_load(b2g_sac* h, const char* path) {
@@ -1895,9 +1984,21 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
   CK(cudaSetDevice(h->cfg.device));
   // ---- everything is checked before the handle changes
   StateReader rd;
-  if (int rc = rd.open(path, STATE_KIND_SAC, sac_fingerprint(h))) return rc;
+  if (int rc = rd.open(path, STATE_KIND_SAC, sac_fingerprint_rms(h))) {
+    // a file with one fingerprint field more or fewer than this handle: say which side owns obs_rms
+    const std::string msg = g_b2g_err;
+    StateReader other;
+    std::vector<FpField> fp = sac_fingerprint(h);
+    if (!h->rms_mean) fp.push_back(fp_int("obs_rms", 1));
+    if (other.open(path, STATE_KIND_SAC, fp) == 0)
+      return b2g_fail(B2G_EINVAL, h->rms_mean ? "the state file has no obs_rms, but this handle owns the observation statistics (b2g_obs_rms_set)"
+                                              : "the state file carries obs_rms: call b2g_obs_rms_set on this handle before loading it");
+    return b2g_fail(rc, msg);
+  }
   const int n_sec = (int)(sizeof kSacTags / sizeof kSacTags[0]);
-  if (rd.n_sections() != n_sec) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a SAC learner");
+  const int n_file = n_sec + (h->rms_mean ? 1 : 0);
+  if (rd.n_sections() != n_file || (h->rms_mean && (rd.tag(n_sec) != kRmsTag || rd.bytes(n_sec) != (uint64_t)(2 * h->E + 1) * sizeof(double))))
+    return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a SAC learner");
   for (int i = 0; i < n_sec; ++i)
     if (rd.tag(i) != kSacTags[i]) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a SAC learner");
   const int64_t cap = h->cfg.buffer_capacity, FC = h->frame_cap;
@@ -1928,6 +2029,14 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
   h->broken = true;
   for (int i = 0; i < (int)dev.size(); ++i)
     if (int rc = rd.read_pieces(i + 2, dev[i].pieces)) return rc;
+  if (h->rms_mean) {
+    double count = 0.0;
+    if (int rc = rd.read_pieces(n_sec, {host_piece(&count, sizeof(double)), dev_piece(h->rms_mean, h->E * sizeof(double)),
+                                        dev_piece(h->rms_var, h->E * sizeof(double))})) return rc;
+    h->rms_count = count;
+    obs_rms_derive(h);
+  }
+  h->ob_n = 0;         // staged observations name frames of the replaced replay: the next b2g_sac_observe_act stages anew
   CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
   h->r_size = hs.r_size; h->head_seq = hs.head_seq; h->tail_seq = hs.tail_seq; h->next_fid = hs.next_fid; h->evicted = hs.evicted;
   h->lw.assign(hs.lw.begin(), hs.lw.end());

@@ -87,6 +87,17 @@ int v2_create(b2g_sac* h);   // tensor maps + problem groups
 int v2_planes(b2g_sac* h, cudaStream_t s);
 int v2_gather(b2g_sac* h, const GatherArgs& ga, cudaStream_t s);
 int v2_launch(b2g_sac* h, const CgGroup& g, cudaStream_t s);
+// sac.cu hooks of the observe path (obsnorm.cu)
+// policy forward on `chunk` <= batch compact rows at `rows` (device), enqueued on h->stream; the actions land in h->pi_out
+int sac_act_rows(b2g_sac* h, const float* rows, int chunk, int deterministic);
+// n <= stage_rows transitions from device memory: compact rows c_obs / c_next, act / rew / done.  obs_fid[i] >= 0 names the
+// replay frame that already holds c_obs[i] (linked instead of stored while it is live and frames are shared); next_fid[i]
+// receives the frame id given to c_next[i].  Enqueues on h->stream; the caller synchronises it before it returns (h_plan and
+// h_rc are pinned and read by the copies enqueued here).
+int sac_replay_add_linked(b2g_sac* h, const float* c_obs, const float* c_next, const int64_t* obs_fid, const float* act,
+                          const float* rew, const float* done, int n, int64_t* next_fid);
+// obsnorm.cu: refreshes d_mean / d_istd from the handle's obs_rms and norm_eps (enqueued on h->stream)
+void obs_rms_derive(b2g_sac* h);
 }  // namespace b2g
 
 using namespace b2g;   // (internal header: only library translation units include it)
@@ -206,6 +217,21 @@ struct b2g_sac {
   double* hp_stats[2]{};             // pinned staging of set_norm_stats (asynchronous upload, no stream sync)
   cudaEvent_t ev_stats[2]{};
   int stats_k = 0;
+  double norm_eps = 1e-8;            // VecNormalize.epsilon of the last b2g_set_norm_stats
+
+  // Device-resident VecNormalize observation statistics (obsnorm.cu; created by b2g_obs_rms_set): float64 mean / var over the
+  // caller's observation layout [E].  The count stays on the host: count + n is the same float64 sum there.
+  double *rms_mean = nullptr, *rms_var = nullptr;
+  double rms_count = 0.0;
+  // b2g_sac_observe_act / _add staging (allocated on first use): the frames of one call in the caller's layout, the current
+  // observation of env i as a compact row, and the replay frame that already holds it (-1: none yet).
+  float* ob_full[2]{};               // [stage_rows][E]: 0 = obs / next_obs, 1 = reset_obs
+  float* ob_rows[2]{};               // compact rows [stage_rows + B][Ec] (the actor's gather reads B rows from any chunk start):
+  int ob_k = 0;                      // ob_rows[ob_k] = current observation of env i; the other takes the next call's next_obs
+  float *ob_act = nullptr, *ob_rew = nullptr, *ob_done = nullptr;
+  std::vector<int64_t> ob_fid;
+  int ob_n = 0;
+  int64_t up_observe = 0, up_other = 0;                   // host->device bytes: observe_* / act + replay_add + set_norm_stats
 
   float* p(const std::string& n) { return P + tensors[tindex.at(n)].off; }
   float* g(const std::string& n) { return G + tensors[tindex.at(n)].off; }

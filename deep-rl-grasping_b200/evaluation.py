@@ -12,13 +12,22 @@ def evaluate_policy(model, env, n_eval_episodes=10, deterministic=True, render=F
         assert env.num_envs == 1, "You must pass only one environment when using this function"
     episode_rewards, episode_lengths = [], []
     obs = None
+    # A model whose own VecNormalize statistics live on its learner (SAC(device_obs_norm=True)) takes RAW observations in
+    # predict and normalises them on the device; an evaluation wrapper that normalises on the host hands over its raw copy.
+    host_vn = None
+    if getattr(model, "predict_takes_raw_obs", False):
+        from .sac_model import unwrap_vec_normalize
+        host_vn = unwrap_vec_normalize(env)
+        if host_vn is not None and (not host_vn.norm_obs or getattr(host_vn, "learner_owns_obs_rms", False)):
+            host_vn = None
     for i in range(n_eval_episodes):
         if not vec or i == 0:            # a VecEnv resets itself at the end of an episode
             obs = env.reset()
         done, state = False, None
         ep_rew, ep_len = 0.0, 0
         while not done:
-            action, state = model.predict(obs, state=state, deterministic=deterministic)
+            action, state = model.predict(obs if host_vn is None else host_vn.get_original_obs(), state=state,
+                                          deterministic=deterministic)
             obs, reward, done, _info = env.step(action)
             if vec:
                 reward, done = float(np.asarray(reward).reshape(-1)[0]), bool(np.asarray(done).reshape(-1)[0])

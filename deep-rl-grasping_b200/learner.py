@@ -208,7 +208,7 @@ class Learner:
     def set_norm_stats(self, obs_mean=None, obs_var=None, ret_var=1.0, clip_obs=10.0, clip_reward=10.0, epsilon=1e-8,
                        norm_obs=True, norm_reward=True):
         dp = C.POINTER(C.c_double)
-        if norm_obs:
+        if norm_obs and obs_mean is not None:      # None: a learner that owns obs_rms keeps its device statistics
             m = np.ascontiguousarray(obs_mean, np.float64).reshape(-1)
             v = np.ascontiguousarray(obs_var, np.float64).reshape(-1)
             assert m.size == self.obs_elems and v.size == self.obs_elems
@@ -218,6 +218,60 @@ class Learner:
         _lib.check(self.lib.b2g_set_norm_stats(self.h, mp, vp, float(ret_var), float(clip_obs), float(clip_reward),
                                                 float(epsilon), int(bool(norm_obs)), int(bool(norm_reward))))
 
+    # ---- device-resident obs_rms and the actor loop on one upload per frame (include/b200grasp.h: b2g_sac_observe_*)
+    #: bumped by every call that may change the device statistics (DeviceRunningMeanStd caches against it)
+    obs_rms_version = 0
+
+    def obs_rms_set(self, mean, var, count):
+        """Creates (first call) or overwrites the device ``obs_rms``: float64 mean / var of the observation shape + count."""
+        dp = C.POINTER(C.c_double)
+        m = np.ascontiguousarray(mean, np.float64).reshape(-1)
+        v = np.ascontiguousarray(var, np.float64).reshape(-1)
+        assert m.size == self.obs_elems and v.size == self.obs_elems
+        _lib.check(self.lib.b2g_obs_rms_set(self.h, m.ctypes.data_as(dp), v.ctypes.data_as(dp), float(count)))
+        self.obs_rms_version += 1
+
+    def obs_rms_get(self):
+        """(mean, var, count) of the device ``obs_rms``; waits for the work enqueued on the handle."""
+        dp = C.POINTER(C.c_double)
+        m, v = np.empty(self.obs_shape, np.float64), np.empty(self.obs_shape, np.float64)
+        cnt = C.c_double()
+        _lib.check(self.lib.b2g_obs_rms_get(self.h, m.ctypes.data_as(dp), v.ctypes.data_as(dp), C.byref(cnt)))
+        return m, v, float(cnt.value)
+
+    def observe_act(self, obs, n=None, update_stats=True, deterministic=False, act=True):
+        """``obs``: n raw observations to upload, merge into ``obs_rms`` (``update_stats``) and stage as the current
+        observation of env i; ``None`` acts on the ones already staged.  Returns the n actions, or None with ``act=False``."""
+        if obs is not None:
+            obs = _f32(obs).reshape(-1, self.obs_elems)
+            n = obs.shape[0]
+            self.obs_rms_version += bool(update_stats)
+        out = np.empty((int(n), self.n_act), np.float32) if act else None
+        _lib.check(self.lib.b2g_sac_observe_act(self.h, None if obs is None else _fp(obs), int(n), int(bool(update_stats)),
+                                                int(deterministic), None if out is None else _fp(out)))
+        return out
+
+    def observe_add(self, act, rew, next_obs, done, reset_obs=None, update_stats=True):
+        """Transition i = (staged obs_i, act_i, rew_i, next_obs_i, done_i); ``reset_obs`` holds, for every finished env,
+        the frame its auto-reset returned (the other rows are not read)."""
+        act, next_obs = _f32(act), _f32(next_obs)
+        rew, done = _f32(np.reshape(rew, -1)), _f32(np.reshape(done, -1))
+        n = rew.shape[0]
+        assert next_obs.size == n * self.obs_elems and act.size == n * self.n_act and done.size == n
+        if reset_obs is not None:
+            reset_obs = _f32(reset_obs)
+            assert reset_obs.size == next_obs.size
+        _lib.check(self.lib.b2g_sac_observe_add(self.h, _fp(act), _fp(rew), _fp(next_obs), _fp(done),
+                                                None if reset_obs is None else _fp(reset_obs), n, int(bool(update_stats))))
+        self.obs_rms_version += bool(update_stats)
+
+    def upload_bytes(self) -> dict:
+        """Bytes copied host -> device so far: by ``observe_*`` / ``obs_rms_set``, and by ``act`` + ``replay_add`` +
+        ``set_norm_stats``."""
+        a, b = C.c_int64(), C.c_int64()
+        _lib.check(self.lib.b2g_upload_bytes(self.h, C.byref(a), C.byref(b)))
+        return {"observe": int(a.value), "other": int(b.value)}
+
     # ---- training state (include/b200grasp.h: b2g_sac_state_save / _load)
     def save_state(self, path: str):
         """Writes parameters, Adam moments, counters and the whole replay to ``path`` (waits for enqueued steps)."""
@@ -225,8 +279,10 @@ class Learner:
 
     def load_state(self, path: str):
         """Restores a ``save_state`` file into this learner, which must have the same configuration (precision aside).
-        Normalisation statistics are not part of the file: set them again with ``set_norm_stats``."""
+        Normalisation statistics are not part of the file (set them again with ``set_norm_stats``), except the device
+        ``obs_rms`` of a learner that owns one."""
         _lib.check(self.lib.b2g_sac_state_load(self.h, os.fsencode(path)))
+        self.obs_rms_version += 1
 
     # ---- hot path
     def step(self, n_steps: int = 1, lr: float = 3e-4) -> dict:

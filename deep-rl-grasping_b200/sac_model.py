@@ -65,7 +65,11 @@ class SAC:
                  batch_size=64, tau=0.005, ent_coef="auto", target_update_interval=1, gradient_steps=1,
                  target_entropy="auto", action_noise=None, random_exploration=0.0, verbose=0, tensorboard_log=None,
                  _init_setup_model=True, policy_kwargs=None, full_tensorboard_log=False, seed=None, n_cpu_tf_sess=None,
-                 precision="bf16x3", device=0, rank=0, nranks=1, nccl_id=None, replay_frames=None, replay_u8_planes=()):
+                 precision="bf16x3", device=0, rank=0, nranks=1, nccl_id=None, replay_frames=None, replay_u8_planes=(),
+                 device_obs_norm=False):
+        if device_obs_norm and nranks > 1:
+            raise NotImplementedError("device_obs_norm=True keeps VecNormalize's obs_rms on one learner handle; with nranks > 1 every "
+                                      "rank would own different statistics")
         if ent_coef != "auto":
             raise NotImplementedError("only ent_coef='auto' (every shipped zip; SURVEY.md section 8c) is built")
         if target_update_interval != 1:
@@ -90,6 +94,9 @@ class SAC:
         # replay storage (Learner: frame_capacity, u8_planes); None / () = two fp32 frames per replay slot
         self.replay_frames = None if replay_frames is None else int(replay_frames)
         self.replay_u8_planes = tuple(int(c) for c in replay_u8_planes)
+        # learn() feeds the actor, the statistics and the replay from one upload per frame, and a VecNormalize with norm_obs
+        # hands its obs_rms to the device learner (Learner.observe_act / observe_add)
+        self.device_obs_norm = bool(device_obs_norm)
         self._dev = dict(device=device, rank=rank, nranks=nranks, nccl_id=nccl_id)
         self._layout_from_zip = False
         self.num_timesteps, self.n_updates = 0, 0
@@ -112,6 +119,9 @@ class SAC:
         self.n_envs = env.num_envs
         self.observation_space, self.action_space = env.observation_space, env.action_space
         self._vec_normalize_env = unwrap_vec_normalize(env)
+        if self.learner is not None:
+            self._attach_device_norm()
+            self._sync_norm_stats()
 
     def get_env(self):
         return self.env
@@ -135,6 +145,7 @@ class SAC:
                                precision=_PRECISIONS[self.precision], frame_capacity=self.replay_frames,
                                u8_planes=self.replay_u8_planes, **self._dev)
         self._init_parameters()
+        self._attach_device_norm()
         self._sync_norm_stats()
 
     def _init_parameters(self):
@@ -158,15 +169,38 @@ class SAC:
         self.learner.load_parameters(p)
 
     def close(self):
-        """Releases the device learner (replay included: Learner.replay_info()["bytes"] of HBM)."""
+        """Releases the device learner (replay included: Learner.replay_info()["bytes"] of HBM).  Observation statistics this
+        learner owned go back to the VecNormalize wrapper first."""
         if self.learner is not None:
+            if self._owns_obs_rms():
+                self._vec_normalize_env.take_obs_rms_back()
             self.learner.close()
             self.learner = None
+
+    def _owns_obs_rms(self) -> bool:
+        vn = self._vec_normalize_env
+        return vn is not None and getattr(vn, "obs_rms_owner", None) is self.learner and self.learner is not None
+
+    @property
+    def predict_takes_raw_obs(self) -> bool:
+        """True while a learner owns the statistics of this model's VecNormalize: that wrapper returns raw observations and
+        ``predict`` normalises them on the device (``evaluate_policy`` feeds an evaluation wrapper's raw copy accordingly)."""
+        return bool(getattr(self._vec_normalize_env, "learner_owns_obs_rms", False))
+
+    def _attach_device_norm(self):
+        """device_obs_norm: the wrapper's obs_rms moves to this learner, unless another learner owns it already (a second
+        model built on the same env, e.g. a parameter donor: it reads the owner's statistics and leaves them where they are)."""
+        vn = self._vec_normalize_env
+        if self.device_obs_norm and isinstance(vn, VecNormalize) and vn.norm_obs and not vn.learner_owns_obs_rms:
+            vn.give_obs_rms_to(self.learner)
 
     def _sync_norm_stats(self):
         vn = self._vec_normalize_env
         if vn is None:
             self.learner.set_norm_stats(norm_obs=False, norm_reward=False)
+        elif self._owns_obs_rms():            # the scalars only: the statistics are this learner's own
+            self.learner.set_norm_stats(None, None, float(vn.ret_rms.var), vn.clip_obs, vn.clip_reward, vn.epsilon,
+                                        norm_obs=vn.norm_obs, norm_reward=vn.norm_reward)
         else:
             self.learner.set_norm_stats(vn.obs_rms.mean, vn.obs_rms.var, float(vn.ret_rms.var), vn.clip_obs, vn.clip_reward,
                                         vn.epsilon, norm_obs=vn.norm_obs, norm_reward=vn.norm_reward)
@@ -193,6 +227,13 @@ class SAC:
         n_env = self.n_envs
         obs = self.env.reset()
         obs_ = vn.get_original_obs() if vn is not None else obs          # un-normalised copy stored in the replay
+        dev = self.device_obs_norm
+        owned = dev and self._owns_obs_rms()
+        if getattr(vn, "learner_owns_obs_rms", False) and not owned:
+            raise RuntimeError("learn: the env's VecNormalize statistics are owned by another model's learner (close that model, "
+                               "or build this one with device_obs_norm=True before it)")
+        if dev:      # the reset frames: uploaded once, merged (VecNormalize.reset's update), staged as every env's current observation
+            self.learner.observe_act(np.asarray(obs_, np.float32), update_stats=owned and vn.training, act=False)
         ep_rew = np.zeros(n_env)
         infos_values = {}
         t_start = time.time()
@@ -204,6 +245,9 @@ class SAC:
             if self.num_timesteps < self.learning_starts or self._rng.random() < self.random_exploration:
                 unscaled = np.stack([np.asarray(self.action_space.sample()) for _ in range(n_env)])
                 action = self._scale_action(unscaled)
+            elif dev:
+                action = self.learner.observe_act(None, n=n_env, deterministic=False)      # the staged frames, current statistics
+                unscaled = self._unscale_action(action)
             else:
                 src = obs_ if vn is not None else obs        # the device normalises raw obs with the same statistics
                 if vn is not None:
@@ -222,8 +266,13 @@ class SAC:
             for i, info in enumerate(infos):
                 if done[i] and isinstance(info, dict) and "terminal_observation" in info:
                     nxt[i] = info["terminal_observation"]
-            self.learner.replay_add(np.asarray(obs_, np.float32), np.asarray(action, np.float32), np.asarray(reward_, np.float32),
-                                    nxt, np.asarray(done, np.float32))
+            if dev:      # next_obs crosses once; a finished env's reset frame is merged and staged, its terminal frame stored
+                self.learner.observe_add(np.asarray(action, np.float32), np.asarray(reward_, np.float32), nxt, np.asarray(done, np.float32),
+                                         reset_obs=np.asarray(new_obs_, np.float32) if np.any(done) else None,
+                                         update_stats=owned and vn.training)      # step_wait's update; a callback may switch it
+            else:
+                self.learner.replay_add(np.asarray(obs_, np.float32), np.asarray(action, np.float32), np.asarray(reward_, np.float32),
+                                        nxt, np.asarray(done, np.float32))
             obs, obs_ = new_obs, new_obs_
             ep_rew += np.asarray(reward_, np.float64).reshape(-1)
             for i in range(n_env):
@@ -262,8 +311,11 @@ class SAC:
         vn = self._vec_normalize_env
         if vn is not None and vn.norm_obs:
             # ``predict`` receives observations ALREADY normalised by the VecNormalize wrapper (utils.py:71 feeds
-            # task.reset()/step() outputs); the device normalises raw ones, so undo the wrapper's transform.
-            obs = obs * np.sqrt(vn.obs_rms.var + vn.epsilon) + vn.obs_rms.mean
+            # task.reset()/step() outputs); the device normalises raw ones, so undo the wrapper's transform.  A wrapper whose
+            # obs_rms a learner owns returns RAW observations: nothing to undo.  (Observations an evaluation wrapper
+            # normalised belong to the model built on that wrapper, or are passed through its ``get_original_obs``.)
+            if not self.predict_takes_raw_obs:
+                obs = obs * np.sqrt(vn.obs_rms.var + vn.epsilon) + vn.obs_rms.mean
             self._sync_norm_stats()
         act = self.learner.act(obs.astype(np.float32), deterministic=deterministic)
         act = self._unscale_action(act.reshape((-1,) + tuple(self.action_space.shape)))
@@ -294,7 +346,7 @@ class SAC:
             "action_space": {"shape": list(self.action_space.shape), "low": [float(x) for x in np.ravel(self.action_space.low)],
                              "high": [float(x) for x in np.ravel(self.action_space.high)]},
             "b200grasp": {"precision": self.precision, "n_updates": self.n_updates, "replay_frames": self.replay_frames,
-                          "replay_u8_planes": list(self.replay_u8_planes)},
+                          "replay_u8_planes": list(self.replay_u8_planes), "device_obs_norm": self.device_obs_norm},
         }
 
     def save(self, save_path, cloudpickle=False):
@@ -316,6 +368,8 @@ class SAC:
                     gradient_steps=self.gradient_steps, target_entropy=self.target_entropy, random_exploration=self.random_exploration,
                     verbose=self.verbose, seed=self.seed, policy_kwargs=policy_kwargs, precision=self.precision,
                     replay_frames=self.replay_frames, replay_u8_planes=list(self.replay_u8_planes))
+        if self.device_obs_norm:
+            init["device_obs_norm"] = True
         return {"algo": "SAC", "policy": "CnnPolicy" if len(self.observation_space.shape) == 3 else "MlpPolicy", "init": init,
                 "num_timesteps": int(self.num_timesteps), "n_updates": int(self.n_updates),
                 "episode_rewards": [float(r) for r in self.episode_rewards], "ep_info_buf": list(self.ep_info_buf),
@@ -337,6 +391,7 @@ class SAC:
         init = dict(host["init"], **kwargs)
         model = cls({"CnnPolicy": CnnPolicy, "MlpPolicy": MlpPolicy}[host["policy"]], env, **init)
         training_state.restore_vec_normalize(path, model.env)
+        model._attach_device_norm()        # the restored statistics go back to the learner; learner.state carries the same ones
         model.load_parameters(os.path.join(path, training_state.MODEL_FILE))
         model.learner.load_state(os.path.join(path, training_state.STATE_FILE))
         model._sync_norm_stats()
@@ -379,6 +434,8 @@ class SAC:
         # depth, 131 GB for RGB-D.  A loaded model is used for inference or as a parameter donor (sb_helper.py:113-115 builds
         # a second model just to call get_parameters), so it gets a small ring unless the caller asks for one explicitly.
         kw["buffer_size"] = min(int(kw.get("buffer_size", 1000)), 1000)
+        if (data.get("b200grasp") or {}).get("device_obs_norm"):
+            kw["device_obs_norm"] = True
         kw.update(kwargs)
         # the head widths are the zip's own: the actor's fc0 / fc1 kernels give [H1, H2], and SAC's constructor refuses any
         # layers the learner cannot build (unequal widths included) with the message that names the supported ones

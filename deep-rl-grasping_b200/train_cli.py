@@ -115,6 +115,8 @@ def train(args):
             replay["replay_frames"] = int(c["buffer_size"] * (1.0 + args.replay_spare)) + n_envs
         if _is_image_obs(env) and config.get("full_observation", False):
             replay["replay_u8_planes"] = (0, 1, 2)        # RGB renders as uint8 (gripperEnv/sensor.py), depth stays fp32
+        if args.device_norm:
+            replay["device_obs_norm"] = True
         model = SAC(policy, env, policy_kwargs=kw, verbose=1, gamma=config["discount_factor"], buffer_size=c["buffer_size"],
                     batch_size=c["batch_size"], learning_rate=c["step_size"], precision=args.precision, **replay)
         if args.load_dir:
@@ -263,6 +265,9 @@ def build_parser():
     t.add_argument("--replay_spare", type=float, default=None,
                    help="SAC replay frame budget buffer_size * (1 + F) + n_envs (observations shared between consecutive "
                         "transitions; 0.125 covers episodes down to ~9 steps); default: two frames per replay slot")
+    t.add_argument("--device_norm", action="store_true",
+                   help="SAC: keep VecNormalize's observation statistics on the GPU and upload every frame once "
+                        "(SAC(device_obs_norm=True)); --resume takes it from the saved run")
     t.add_argument("--eval_freq", type=int, default=50000)
     t.add_argument("--checkpoint_freq", type=int, default=25000)
     t.add_argument("--state_freq", type=int, default=None,

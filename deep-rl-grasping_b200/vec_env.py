@@ -36,6 +36,57 @@ class RunningMeanStd:
         self.mean, self.var, self.count = new_mean, m_2 / tot, tot
 
 
+class DeviceRunningMeanStd:
+    """The ``obs_rms`` of a VecNormalize whose statistics live on the device learner (``SAC(device_obs_norm=True)``).
+    ``owner`` provides ``obs_rms_get() -> (mean, var, count)``, ``obs_rms_set(mean, var, count)`` and a counter
+    ``obs_rms_version`` that moves whenever the device statistics may have changed.  ``mean`` / ``var`` / ``count`` fetch on
+    access (cached until the version moves) and assignment writes through, so everything that reads or copies a
+    RunningMeanStd keeps working: pickling and ``copy.deepcopy`` give a plain RunningMeanStd holding the current numbers."""
+
+    def __init__(self, owner):
+        self.__dict__["_owner"] = owner
+        self.__dict__["_cache"] = None
+
+    def _fetch(self):
+        ver = self._owner.obs_rms_version
+        if self._cache is None or self._cache[0] != ver:
+            self.__dict__["_cache"] = (ver,) + tuple(self._owner.obs_rms_get())
+        return self._cache[1:]
+
+    mean = property(lambda self: self._fetch()[0])
+    var = property(lambda self: self._fetch()[1])
+    count = property(lambda self: self._fetch()[2])
+
+    def __setattr__(self, name, value):
+        if name not in ("mean", "var", "count"):
+            raise AttributeError(name)
+        cur = dict(zip(("mean", "var", "count"), self._fetch()))
+        cur[name] = value
+        self._owner.obs_rms_set(cur["mean"], cur["var"], cur["count"])
+        self.__dict__["_cache"] = None
+
+    def update(self, arr) -> None:
+        raise RuntimeError("the device learner merges observations into these statistics (Learner.observe_act / observe_add)")
+
+    def snapshot(self) -> RunningMeanStd:
+        r = RunningMeanStd.__new__(RunningMeanStd)
+        m, v, c = self._fetch()
+        r.mean, r.var, r.count = np.array(m, np.float64), np.array(v, np.float64), float(c)
+        return r
+
+    def __deepcopy__(self, memo):
+        return self.snapshot()
+
+    def __reduce__(self):
+        return (_rebuild_rms, tuple(self.snapshot().__dict__.items()))
+
+
+def _rebuild_rms(*items):
+    r = RunningMeanStd.__new__(RunningMeanStd)
+    r.__dict__.update(items)
+    return r
+
+
 class VecEnv:
     """Marker base class (``isinstance(env, VecEnv)`` in base_callbacks.py:50 and [SB2] evaluate_policy)."""
     num_envs = 1
@@ -210,6 +261,33 @@ class VecNormalize(VecEnv):
         self.training, self.norm_obs, self.norm_reward = training, norm_obs, norm_reward
         self.old_obs, self.old_rews = np.array([]), np.array([])
 
+    # ---- statistics owned by the device learner (SAC(device_obs_norm=True))
+    @property
+    def learner_owns_obs_rms(self) -> bool:
+        return isinstance(self.obs_rms, DeviceRunningMeanStd)
+
+    def give_obs_rms_to(self, owner) -> None:
+        """Hands the current ``obs_rms`` to ``owner`` (a Learner): from here on ``reset`` / ``step_wait`` return the RAW
+        observation and leave the update and the normalisation of observations to the device; the reward side is unchanged.
+        ``normalize_obs`` called explicitly still works, from the fetched statistics.  A wrapper has one owner at a time:
+        another one must wait for ``take_obs_rms_back``."""
+        if self.learner_owns_obs_rms:
+            if self.obs_rms_owner is owner:
+                return
+            raise RuntimeError("this VecNormalize's obs_rms is already owned by another learner")
+        owner.obs_rms_set(self.obs_rms.mean, self.obs_rms.var, self.obs_rms.count)
+        self.obs_rms = DeviceRunningMeanStd(owner)
+
+    @property
+    def obs_rms_owner(self):
+        return self.obs_rms._owner if self.learner_owns_obs_rms else None
+
+    def take_obs_rms_back(self) -> None:
+        """The statistics return to the host as a plain RunningMeanStd holding the owner's current numbers (the owner is
+        about to go away): the wrapper updates and normalises again itself."""
+        if self.learner_owns_obs_rms:
+            self.obs_rms = self.obs_rms.snapshot()
+
     # ---- VecEnv surface
     @property
     def envs(self):
@@ -226,10 +304,13 @@ class VecNormalize(VecEnv):
         obs, rews, news, infos = self.venv.step_wait()
         self.ret = self.ret * self.gamma + rews
         self.old_obs, self.old_rews = obs, rews
+        owned = self.learner_owns_obs_rms
         if self.training:
-            self.obs_rms.update(obs)
+            if not owned:
+                self.obs_rms.update(obs)
             self.ret_rms.update(self.ret)
-        obs = self.normalize_obs(obs)
+        if not owned:
+            obs = self.normalize_obs(obs)
         rews = self.normalize_reward(rews)
         self.ret[news] = 0
         return obs, rews, news, infos
@@ -242,6 +323,8 @@ class VecNormalize(VecEnv):
         obs = self.venv.reset()
         self.old_obs = obs
         self.ret = np.zeros(self.num_envs)
+        if self.learner_owns_obs_rms:
+            return obs
         if self.training:
             self.obs_rms.update(obs)
         return self.normalize_obs(obs)
@@ -274,6 +357,8 @@ class VecNormalize(VecEnv):
         st = self.__dict__.copy()
         for k in ("venv", "num_envs", "ret"):
             st.pop(k, None)
+        if self.learner_owns_obs_rms:
+            st["obs_rms"] = self.obs_rms.snapshot()
         return st
 
     def __setstate__(self, st):

@@ -140,8 +140,46 @@ int b2g_replay_info(const b2g_sac* h, int64_t* capacity, int64_t* size, int64_t*
  * q1_pi,q2_pi (7 x [batch]) and the squashed actions pi[batch, n_act].  Any pointer may be NULL.  This is what lets a
  * test replay the very batch of a sampled step in the oracle. */
 int b2g_get_last_batch(b2g_sac* h, int32_t* indices, float* eps, float* per_sample, float* pi_out);
+/* On a handle that owns obs_rms (b2g_obs_rms_set, below) obs_mean / obs_var may be NULL with norm_obs != 0: the scalars are
+ * set and the device statistics stay; passing them replaces the device statistics (count kept). */
 int b2g_set_norm_stats(b2g_sac* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs,
                        double clip_rew, double eps, int norm_obs, int norm_reward);
+
+/* ---- VecNormalize's observation statistics on the device, and the actor side of the learn loop fed from one upload per
+ *      frame.  obs_rms = (mean[E], var[E], count), float64, E = H*W*C (or obs_dim) in the caller's observation layout: the
+ *      RunningMeanStd that [SB2] VecNormalize keeps on the host.  b2g_obs_rms_set creates it on the handle (nranks == 1 only:
+ *      each rank would own different statistics); from then on the table that the gather of the gradient step and policy
+ *      inference normalise with is derived from it on the device, in the kernel that merges new frames, on the handle's
+ *      stream: a step sampled after an observe call uses the statistics that call left, with no host round trip.
+ *      Merge rule (RunningMeanStd.update_from_moments): per element, bm = mean and bv = biased variance of the n frames,
+ *      summed in frame order 0 .. n-1; delta = bm - mean; tot = count + n; mean += delta * n / tot;
+ *      var = (var * count + bv * n + delta^2 * count * n / tot) / tot; count = tot.
+ *      Which frames are merged is VecNormalize's rule: reset() merges the reset frames (observe_act with obs), step_wait()
+ *      merges the n frames the VecEnv returned -- for a finished env the frame its auto-reset returned, NOT the terminal
+ *      observation, which goes into the replay only (observe_add).  With 8-bit replay planes the statistics are taken from the
+ *      float frames as uploaded; a value there that is not an integer in [0, 255] is refused (B2G_EINVAL, nothing changed).
+ *      Up to max(batch, 256) frames per call.  Like b2g_replay_add and b2g_sac_act, a call returns once the handle's stream
+ *      has run what it enqueued. */
+/* n raw observations (host, caller-owned, copied before return), or obs == NULL to act on the observations already staged.
+ * update_stats != 0: merge them into the device obs_rms first (VecNormalize.training; B2G_ESTATE without b2g_obs_rms_set).
+ * Then normalise with the CURRENT statistics, run the actor and write n actions; act_out == NULL skips the actor (a step
+ * that explores with random actions).  The frames stay staged in the handle as "the current observation of env i". */
+int b2g_sac_observe_act(b2g_sac* h, const float* obs, int n, int update_stats, int deterministic, float* act_out);
+/* Transition i = (staged obs_i, act_i, rew_i, next_obs_i, done_i).  next_obs is uploaded ONCE: it goes into the replay as this
+ * transition's next frame, is merged into obs_rms when update_stats != 0, and becomes the staged observation of env i unless
+ * done_i, in which case reset_obs_i (the frame the auto-reset returned; merged instead, and the only rows of reset_obs that
+ * are read) does.  With a frame-sharing replay the staged frame is linked, not stored again.  B2G_ESTATE before any
+ * b2g_sac_observe_act; n must equal the number of staged observations. */
+int b2g_sac_observe_add(b2g_sac* h, const float* act, const float* rew, const float* next_obs, const float* done,
+                        const float* reset_obs /* may be NULL when no env finished */, int n, int update_stats);
+/* obs_rms in and out (vecnormalize.pkl, sync_envs_normalization, resume): float64 [H*W*C] each + count.  set refuses a
+ * negative or non-finite count, a negative variance and non-finite values (B2G_EINVAL); get returns B2G_ESTATE on a handle
+ * without statistics; any output may be NULL. */
+int b2g_obs_rms_set(b2g_sac* h, const double* mean, const double* var, double count);
+int b2g_obs_rms_get(b2g_sac* h, double* mean, double* var, double* count);
+/* bytes copied host -> device so far by b2g_sac_observe_* and b2g_obs_rms_set (observe_bytes) and by b2g_sac_act,
+ * b2g_replay_add and b2g_set_norm_stats (other_bytes); either may be NULL */
+int b2g_upload_bytes(const b2g_sac* h, int64_t* observe_bytes, int64_t* other_bytes);
 
 /* ---- the hot path.  One call = n_steps x { sample -> normalise -> fwd -> bwd -> [allreduce] ->
  *      3x Adam -> Polyak }  (SAC._train_step + target_update_op).  Indices and policy noise come
@@ -175,12 +213,15 @@ int b2g_sac_act(b2g_sac* h, const float* obs, int n, int deterministic, float* a
 /* ---- training state: stop a run and continue it later.  The file holds what decides the next step / act / replay_add: the
  *      parameter arena (target network and log_ent_coef included), both Adam moments, the device counters (Adam steps,
  *      n_updates, the Philox step of the slot and noise draws, replay size and first live slot), the replay bookkeeping, the
- *      transition arrays and the live window of replay frames.  Not in it: the normalisation statistics (set them again with
- *      b2g_set_norm_stats; VecNormalize keeps its own file) and the precision mode (a bf16x3 state loads into an fp32 handle).
+ *      transition arrays and the live window of replay frames, and the device obs_rms of a handle that owns one.  Not in it: the
+ *      other normalisation statistics (set them again with b2g_set_norm_stats; VecNormalize keeps its own file), the staged
+ *      observations of b2g_sac_observe_* (a resumed run starts a fresh episode) and the precision mode (a bf16x3 state loads
+ *      into an fp32 handle).
  * save: waits for every step enqueued on the handle; B2G_ESTATE while a host-pipelined step awaits b2g_sac_pipeline_flush and
  *       for nranks > 1 (data-parallel checkpoints are not built).
  * load: into a handle created with the same configuration.  The header, the configuration fingerprint (shape, n_act, hidden,
- *       batch, capacities, 8-bit planes, gamma, tau, target_entropy, seed), the section lengths and the file size are checked
+ *       batch, capacities, 8-bit planes, gamma, tau, target_entropy, seed, and whether obs_rms is carried: a file written with
+ *       it loads only into a handle that owns one, and the reverse), the section lengths and the file size are checked
  *       before anything is written: a mismatch returns B2G_EINVAL naming the first field that differs and leaves the handle as
  *       it was.  A read or checksum failure after that leaves the handle unusable: every call but destroy and another load
  *       then returns B2G_ESTATE. */
