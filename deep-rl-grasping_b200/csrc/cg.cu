@@ -10,9 +10,9 @@
 //                 place: its columns pass, 16 at a time, through a small staging block so that every lane holds one output row,
 //                 then the fp32 stores or red.adds;
 //   warps 8..11 : the epilogue warpgroup.  Lane l of warp e reads row 32e + l of a handed-off tile (all its columns), then
-//                 bias/ReLU or the ReLU mask (+ the bias-gradient column sums), the split into BF16 planes and the row's
-//                 32-column stores of every plane (16-byte vectors), the split-K finalisation and the dependency arrivals -- while
-//                 the MMA warps run the next tile's mainloop;
+//                 bias/ReLU or the ReLU mask (+ the bias-gradient column sums), the split into BF16 planes and their 16-byte
+//                 vector stores (transposed inside lane quads so that each instruction writes whole 64-byte row segments), the
+//                 split-K finalisation and the dependency arrivals -- while the MMA warps run the next tile's mainloop;
 //   warps 12..13: TMA producers (whole warps, converged; one elected lane issues).  The cp.async.bulk.tensor boxes of a K-chunk
 //                 (operands x planes) are dealt round-robin to the two warps; warp 12 posts the chunk's expect_tx.
 //   warps 14..15: complete the producer warpgroup for setmaxnreg and exit.
@@ -37,7 +37,7 @@ constexpr int NTHREADS = 32 * (PROD_WARP0 + 4);
 // registers per thread after setmaxnreg: 2 x MMA + EPI + PROD <= 512 per SM sub-partition lane (each holds two MMA warps, one
 // epilogue warp and one producer warp), i.e. the whole 64K register file.  The MMA warps hold up to 128 accumulator registers
 // across a mainloop in which one chunk's wgmmas are always in flight.
-constexpr int MMA_REGS = 176, EPI_REGS = 136, PROD_REGS = 24;
+constexpr int MMA_REGS = 168, EPI_REGS = 152, PROD_REGS = 24;
 static_assert(2 * MMA_REGS + EPI_REGS + PROD_REGS <= 512, "register file");
 constexpr int STG_BYTES = 2 * 64 * 16 * 4;    // in-place epilogue staging: per warpgroup 64 rows x 16 fp32 columns (rows of 64 B)
 
@@ -696,6 +696,8 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
         }
         // ---- BF16 planes: hi = bf16(x), then the residual feeds the next plane
         const long long gcol = grp_tab ? 0 : (long long)(ng >> 5) * grp_stride;
+        const long long roff = off + gcol;
+        const int q0 = lane & ~3, qi = lane & 3;           // this lane's quad, and its place in it
 #pragma unroll 1
         for (int pl = 0; pl < out_planes; ++pl) {
           uint32_t pk[16];
@@ -705,10 +707,31 @@ cg_kernel(const __grid_constant__ CgPack pk, int nprob, int total_tiles, const C
             x[2 * j] -= __uint_as_float(pk[j] << 16);
             x[2 * j + 1] -= __uint_as_float(pk[j] & 0xFFFF0000u);
           }
-          if (valid && !dbg_nost) {              // 4 x 128-bit stores: every lane writes whole 32-byte sectors
-            uint16_t* dst = P.out_p[pl] + off + gcol;
+          if (dbg_nost) continue;
+          // The row's 64 bytes are 4 16-byte chunks, pk[4c .. 4c + 3] = chunk c.  A 4 x 4 transpose of the chunks inside each quad
+          // of lanes (two shfl_xor exchange steps) leaves lane q0 + i holding chunk i of rows q0 .. q0 + 3 in slots 0 .. 3, so that
+          // store j writes 8 rows (q0 + j of every quad) with 64 contiguous bytes each: 8 whole row segments per instruction instead
+          // of 32 rows' quarter segments (half 32-byte sectors).
 #pragma unroll
-            for (int j = 0; j < 4; ++j) *reinterpret_cast<uint4*>(dst + 8 * j) = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
+          for (int m = 1; m <= 2; m <<= 1) {
+            const bool up = (lane & m) != 0;
+#pragma unroll
+            for (int c0 = 0; c0 < 4; ++c0) {
+              if (c0 & m) continue;
+              const int c1 = c0 | m;                   // slot c of lane i moves to lane i ^ m, slot c ^ m, where bit m of i and c differ
+#pragma unroll
+              for (int u = 0; u < 4; ++u) {
+                const uint32_t got = __shfl_xor_sync(0xffffffffu, up ? pk[4 * c0 + u] : pk[4 * c1 + u], m);
+                if (up) pk[4 * c0 + u] = got; else pk[4 * c1 + u] = got;
+              }
+            }
+          }
+          uint16_t* const base = P.out_p[pl];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {                  // row q0 + j: its owner's offset and limit
+            const long long oj = __shfl_sync(0xffffffffu, roff, q0 + j);
+            const bool vj = __shfl_sync(0xffffffffu, valid ? 1 : 0, q0 + j) != 0;
+            if (vj) *reinterpret_cast<uint4*>(base + oj + 8 * qi) = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
           }
         }
       };
