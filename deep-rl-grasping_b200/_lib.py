@@ -26,7 +26,7 @@ SYMBOLS = [
     "b2g_bdq_get_grad", "b2g_bdq_replay_add", "b2g_bdq_replay_size", "b2g_bdq_set_norm_stats", "b2g_bdq_step",
     "b2g_bdq_step_explicit", "b2g_bdq_act", "b2g_bdq_set_per_beta", "b2g_bdq_get_last_per", "b2g_bdq_state_save", "b2g_bdq_state_load",
     "b2g_encoder_create", "b2g_encoder_destroy", "b2g_encoder_n_layers", "b2g_encoder_layer_shape", "b2g_encoder_set_weights",
-    "b2g_encoder_encode", "b2g_debug_gemm",
+    "b2g_encoder_encode", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor",
     "b2g_autoencoder_create", "b2g_autoencoder_destroy", "b2g_autoencoder_n_layers", "b2g_autoencoder_layer_shape",
     "b2g_autoencoder_set_weights", "b2g_autoencoder_get_weights", "b2g_autoencoder_get_grad", "b2g_autoencoder_reset_optimizer",
     "b2g_autoencoder_set_dataset", "b2g_autoencoder_train_epoch", "b2g_autoencoder_evaluate", "b2g_autoencoder_predict",
@@ -179,6 +179,8 @@ def load():
     lib.b2g_autoencoder_predict.argtypes = [vp, fp, C.c_int, fp]
     lib.b2g_autoencoder_step.argtypes = [vp, fp, fp, C.c_int, C.c_float, C.c_int, dp]
     lib.b2g_debug_gemm.argtypes = [C.c_int, C.c_int, C.c_int, fp, fp, fp, C.c_int, C.c_int]
+    lib.b2g_debug_tensor_info.argtypes = [vp, C.c_char_p, i64p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    lib.b2g_debug_tensor.argtypes = [vp, C.c_char_p, C.c_int, vp, C.c_size_t]
     _lib = lib
     return lib
 

@@ -381,6 +381,38 @@ int b2g_autoencoder_step(b2g_autoencoder* h, const float* inputs, const float* t
  * ------------------------------------------------------------------------------------------------------------ */
 int b2g_debug_gemm(int M, int N, int K, const float* A, const float* B, float* C, int x3, int split_k);
 
+/* Bring-up hook (not on the product path): one plane of one named device tensor of a SAC handle, copied to the host after the
+ * handle's stream is synchronised.  BF16 planes come back as raw uint16 (elem_bytes 2), fp32 buffers as float (elem_bytes 4);
+ * bytes must be numel * elem_bytes.  Returns B2G_EINVAL for an unknown name, a plane out of range or a size mismatch, and
+ * B2G_ESTATE for an engine-v2 name (every BF16 name, and z0v) on a handle that does not run engine v2 (CNN policy, 64 x 64
+ * image, 1 to 4 image channels, bf16x3).  The tensors hold what the LAST step left: read them right after the step, since
+ * b2g_sac_act overwrites planes 0 and 1 of the policy's activations (S/obs, H1/pi .. F/pi).
+ * <net> is pi, values or target; the backward tensors and natural weight planes exist for pi and values only.  B = batch,
+ * Ci = image channels, Cp = 1 if Ci == 1 else 4, K1 = 64 Cp, KF = 576, FS = feature-row stride of the fp32 rows, H = hidden.
+ *   S/obs, S/next_obs   3 planes  [B][16 Y][16 X][4 b][4 c][Cp]: normalised pixel (4Y + b, 4X + c) / 255; channels ci >= Ci zero
+ *   H1/<net>            3 planes  [B][15][15][32]   conv1 output (NHWC, after ReLU)
+ *   H2/<net>            3 planes  [B][6][6][64]     conv2 output
+ *   H3/<net>            3 planes  [B][4][4][64]     conv3 output (= cnn_fc1 input row of 1024)
+ *   F/<net>             3 planes  [B][KF]           512 cnn_fc1 features, the actuator value, the n_act actions (values only), zeros
+ *   dz0pi / dz0v        2 planes  [B][H] / [B][3H]  fc0 pre-activation gradients (pi; vf | qf1 | qf2)
+ *   dZ4/<net>           2 planes  [B][512]          cnn_fc1 output gradient, ReLU-masked
+ *   dZ3/<net>           2 planes  [B][1024]         conv3 output gradient [B][4][4][64]
+ *   dZ2/<net>           2 planes  [B][6][6][64]     conv2 output gradient
+ *   dZ1                 2 planes  [B][15][15][2 nets][32]   conv1 output gradient of pi | values
+ *   W1T/online          3 planes  [64 = pi | values][K1]   conv1 kernels transposed, K row of HWIO row r = conv1_krow(r, Ci)
+ *   W1T/target          3 planes  [32][K1]                 (pad rows zero)
+ *   W2T/<net>, W3T/<net>, WfT/<net>   3 planes  [N][K]: cnn2/w [64][512], cnn3/w [64][576], cnn_fc1/w [512][1024] transposed
+ *   K0T/<net>           3 planes  [H or 3H = vf | qf1 | qf2][KF]   fc0 kernels transposed, rows padded with zeros to KF
+ *   W2n/<net>, W3n/<net>, Wfn/<net>   2 planes  the HWIO / [in][out] kernels as stored: [512][64], [576][64], [1024][512]
+ *   K0n/<net>           2 planes  [KF][H] (pi) / [KF][3H] (values: vf | qf1 | qf2), rows beyond each kernel's K zero
+ *   F32/<net>           fp32      [B][FS]            the feature rows the head kernels read (columns as in F)
+ *   z0/pi, z0/target    fp32      [B][H]             fc0 pre-activations without bias
+ *   z0v                 fp32      [B][3H]            the same for vf | qf1 | qf2
+ *   a0/<head>, dz1/<head>  fp32   [B][H]             fc0 activations and fc1 pre-activation gradients; head = pi, vf, qf1, qf2
+ *   dz0_pi / dz0_v3     fp32      [B][H] / [B][3H]   the fp32 values of dz0pi / dz0v */
+int b2g_debug_tensor_info(const b2g_sac* h, const char* name, int64_t* numel, int32_t* planes, int32_t* elem_bytes);
+int b2g_debug_tensor(b2g_sac* h, const char* name, int plane, void* dst, size_t bytes);
+
 #ifdef __cplusplus
 }
 #endif
