@@ -25,6 +25,7 @@ SYMBOLS = [
     "b2g_bdq_create", "b2g_bdq_destroy", "b2g_bdq_param_count", "b2g_bdq_param_info", "b2g_bdq_get_param", "b2g_bdq_set_param",
     "b2g_bdq_get_grad", "b2g_bdq_replay_add", "b2g_bdq_replay_size", "b2g_bdq_set_norm_stats", "b2g_bdq_step",
     "b2g_bdq_step_explicit", "b2g_bdq_act", "b2g_bdq_set_per_beta", "b2g_bdq_get_last_per", "b2g_bdq_state_save", "b2g_bdq_state_load",
+    "b2g_bdq_observe_act", "b2g_bdq_observe_add", "b2g_bdq_obs_rms_set", "b2g_bdq_obs_rms_get", "b2g_bdq_upload_bytes",
     "b2g_encoder_create", "b2g_encoder_destroy", "b2g_encoder_n_layers", "b2g_encoder_layer_shape", "b2g_encoder_set_weights",
     "b2g_encoder_encode", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor",
     "b2g_autoencoder_create", "b2g_autoencoder_destroy", "b2g_autoencoder_n_layers", "b2g_autoencoder_layer_shape",
@@ -160,6 +161,11 @@ def load():
     lib.b2g_bdq_act.argtypes = [vp, fp, C.c_int, C.POINTER(C.c_int32)]
     lib.b2g_bdq_set_per_beta.argtypes = [vp, C.c_float]
     lib.b2g_bdq_get_last_per.argtypes = [vp, C.POINTER(C.c_int32), fp, fp]
+    lib.b2g_bdq_observe_act.argtypes = [vp, fp, C.c_int, C.c_int, C.c_float, C.POINTER(C.c_int32)]
+    lib.b2g_bdq_observe_add.argtypes = [vp, fp, fp, fp, fp, fp, C.c_int, C.c_int]
+    lib.b2g_bdq_obs_rms_set.argtypes = [vp, dp, dp, C.c_double]
+    lib.b2g_bdq_obs_rms_get.argtypes = [vp, dp, dp, dp]
+    lib.b2g_bdq_upload_bytes.argtypes = [vp, i64p, i64p]
     lib.b2g_encoder_create.argtypes = [C.POINTER(EncoderCfg), C.POINTER(vp)]
     lib.b2g_encoder_destroy.argtypes = [vp]
     lib.b2g_encoder_n_layers.argtypes = [vp]

@@ -19,7 +19,7 @@ import numpy as np
 from . import _lib, sb_io, training_state
 from .callbacks import as_callback
 from .learner import _f32, _fp
-from .vec_env import DummyVecEnv
+from .vec_env import DummyVecEnv, VecNormalize
 
 
 class BDQLearner:
@@ -46,6 +46,7 @@ class BDQLearner:
         self.h = C.c_void_p()
         _lib.check(self.lib.b2g_bdq_create(C.byref(cfg), C.byref(self.h)))
         self.obs_dim, self.n_branches, self.n_bins, self.batch_size = obs_dim, n_branches, n_bins, batch_size
+        self.obs_shape = (obs_dim,)          # shape of obs_rms_get's arrays (BDQ sets the env's observation shape)
         self._info = OrderedDict()
         buf = C.create_string_buffer(256)
         rows, cols, nd = C.c_int64(), C.c_int64(), C.c_int32()
@@ -116,8 +117,81 @@ class BDQLearner:
         _lib.check(self.lib.b2g_bdq_state_save(self.h, os.fsencode(path)))
 
     def load_state(self, path: str):
-        """Restores a ``save_state`` file into this learner, which must have the same configuration."""
+        """Restores a ``save_state`` file into this learner, which must have the same configuration (and own a device
+        ``obs_rms`` exactly when the file carries one)."""
         _lib.check(self.lib.b2g_bdq_state_load(self.h, os.fsencode(path)))
+        self.obs_rms_version += 1
+
+    def set_norm_stats(self, obs_mean=None, obs_var=None, ret_var=1.0, clip_obs=10.0, clip_reward=10.0, epsilon=1e-8,
+                       norm_obs=True, norm_reward=True):
+        """VecNormalize's statistics for the gather of the gradient step and act().  ``obs_mean = obs_var = None`` with
+        ``norm_obs``: a learner that owns ``obs_rms`` keeps its device statistics and takes the scalars only."""
+        dp = C.POINTER(C.c_double)
+        mp = vp = None
+        if norm_obs and obs_mean is not None:
+            m = np.ascontiguousarray(obs_mean, np.float64).reshape(-1)
+            v = np.ascontiguousarray(obs_var, np.float64).reshape(-1)
+            assert m.size == self.obs_dim and v.size == self.obs_dim
+            mp, vp = m.ctypes.data_as(dp), v.ctypes.data_as(dp)
+        _lib.check(self.lib.b2g_bdq_set_norm_stats(self.h, mp, vp, float(ret_var), float(clip_obs), float(clip_reward),
+                                                    float(epsilon), int(bool(norm_obs)), int(bool(norm_reward))))
+        if mp is not None:
+            self.obs_rms_version += 1
+
+    # ---- device-resident obs_rms and the actor loop on one upload per frame (include/b200grasp.h: b2g_bdq_observe_*)
+    #: bumped by every call that may change the device statistics (DeviceRunningMeanStd caches against it)
+    obs_rms_version = 0
+
+    def obs_rms_set(self, mean, var, count):
+        """Creates (first call) or overwrites the device ``obs_rms``: float64 mean / var of the observation + count."""
+        dp = C.POINTER(C.c_double)
+        m = np.ascontiguousarray(mean, np.float64).reshape(-1)
+        v = np.ascontiguousarray(var, np.float64).reshape(-1)
+        assert m.size == self.obs_dim and v.size == self.obs_dim
+        _lib.check(self.lib.b2g_bdq_obs_rms_set(self.h, m.ctypes.data_as(dp), v.ctypes.data_as(dp), float(count)))
+        self.obs_rms_version += 1
+
+    def obs_rms_get(self):
+        """(mean, var, count) of the device ``obs_rms`` in ``obs_shape``; waits for the work enqueued on the handle."""
+        dp = C.POINTER(C.c_double)
+        m, v = np.empty(self.obs_shape, np.float64), np.empty(self.obs_shape, np.float64)
+        cnt = C.c_double()
+        _lib.check(self.lib.b2g_bdq_obs_rms_get(self.h, m.ctypes.data_as(dp), v.ctypes.data_as(dp), C.byref(cnt)))
+        return m, v, float(cnt.value)
+
+    def observe_act(self, obs, n=None, update_stats=True, eps=0.0, act=True):
+        """``obs``: n raw observations to upload, merge into ``obs_rms`` (``update_stats``) and stage as the current
+        observation of env i; ``None`` acts on the ones already staged.  Returns the [n, n_branches] epsilon-greedy bin
+        indices, or None with ``act=False``."""
+        if obs is not None:
+            obs = _f32(obs).reshape(-1, self.obs_dim)
+            n = obs.shape[0]
+            self.obs_rms_version += bool(update_stats)
+        out = np.empty((int(n), self.n_branches), np.int32) if act else None
+        _lib.check(self.lib.b2g_bdq_observe_act(self.h, None if obs is None else _fp(obs), int(n), int(bool(update_stats)), float(eps),
+                                                None if out is None else out.ctypes.data_as(C.POINTER(C.c_int32))))
+        return out
+
+    def observe_add(self, act_idx, rew, next_obs, done, reset_obs=None, update_stats=True):
+        """Transition i = (staged obs_i, act_idx_i, rew_i, next_obs_i, done_i); ``reset_obs`` holds, for every finished env,
+        the frame its auto-reset returned (the other rows are not read)."""
+        act, next_obs = _f32(act_idx), _f32(next_obs)
+        rew, done = _f32(np.reshape(rew, -1)), _f32(np.reshape(done, -1))
+        n = rew.shape[0]
+        assert next_obs.size == n * self.obs_dim and act.size == n * self.n_branches and done.size == n
+        if reset_obs is not None:
+            reset_obs = _f32(reset_obs)
+            assert reset_obs.size == next_obs.size
+        _lib.check(self.lib.b2g_bdq_observe_add(self.h, _fp(act), _fp(rew), _fp(next_obs), _fp(done),
+                                                None if reset_obs is None else _fp(reset_obs), n, int(bool(update_stats))))
+        self.obs_rms_version += bool(update_stats)
+
+    def upload_bytes(self) -> dict:
+        """Bytes copied host -> device so far: by ``observe_*`` / ``obs_rms_set``, and by ``act`` + ``replay_add`` +
+        ``set_norm_stats``."""
+        a, b = C.c_int64(), C.c_int64()
+        _lib.check(self.lib.b2g_bdq_upload_bytes(self.h, C.byref(a), C.byref(b)))
+        return {"observe": int(a.value), "other": int(b.value)}
 
     def step(self, n_steps=1, lr=1e-4):
         m = _lib.BdqMetrics()
@@ -162,7 +236,14 @@ class BDQ:
                  exploration_final_eps=0.02, train_freq=1, batch_size=64, learning_starts=1000, target_network_update_freq=1000,
                  num_actions_pad=33, prioritized_replay=False, prioritized_replay_alpha=0.6, prioritized_replay_beta0=0.4,
                  prioritized_replay_beta_iters=None, prioritized_replay_eps=1e-6, epsilon_greedy=True, policy_kwargs=None, verbose=0,
-                 tensorboard_log=None, seed=None, device=0, rank=0, nranks=1, nccl_id=None, _init_setup_model=True, **_ignored):
+                 tensorboard_log=None, seed=None, device=0, rank=0, nranks=1, nccl_id=None, _init_setup_model=True,
+                 device_obs_norm=False, **_ignored):
+        if device_obs_norm and nranks > 1:
+            raise NotImplementedError("device_obs_norm=True keeps VecNormalize's obs_rms on one learner handle; with nranks > 1 every "
+                                      "rank would own different statistics")
+        # learn() stores raw transitions (stable-baselines' rule), feeds the actor, the statistics and the replay from one upload
+        # per frame, and a VecNormalize with norm_obs hands its obs_rms to the device learner (BDQLearner.observe_act / _add)
+        self.device_obs_norm = bool(device_obs_norm)
         self.prioritized_replay = bool(prioritized_replay)
         self.per_alpha, self.per_beta0, self.per_beta_iters, self.per_eps = prioritized_replay_alpha, prioritized_replay_beta0, \
             prioritized_replay_beta_iters, prioritized_replay_eps
@@ -178,9 +259,11 @@ class BDQ:
         self._rng = np.random.default_rng(seed)
         self.learner: Optional[BDQLearner] = None
         self.env = None
+        self._vec_normalize_env = None
         if env is not None:
             self.env = env if hasattr(env, "num_envs") else DummyVecEnv([lambda: env])
             self.observation_space, self.action_space = self.env.observation_space, self.env.action_space
+            self._vec_normalize_env = self.get_vec_normalize_env()
             if _init_setup_model:
                 self.setup_model()
 
@@ -204,7 +287,42 @@ class BDQ:
             else:
                 p[n] = np.zeros(shp, np.float32)
         self.learner.load_parameters(p)
+        self.learner.obs_shape = tuple(self.observation_space.shape)
         self._bins = np.linspace(-1.0, 1.0, self.num_actions_pad).astype(np.float32)
+        self._attach_device_norm()
+
+    def close(self):
+        """Releases the device learner.  Observation statistics it owned go back to the VecNormalize wrapper first."""
+        if self.learner is not None:
+            if self._owns_obs_rms():
+                self._vec_normalize_env.take_obs_rms_back()
+            self.learner.close()
+            self.learner = None
+
+    def _owns_obs_rms(self) -> bool:
+        vn = self._vec_normalize_env
+        return vn is not None and self.learner is not None and getattr(vn, "obs_rms_owner", None) is self.learner
+
+    @property
+    def predict_takes_raw_obs(self) -> bool:
+        """True while a learner owns the statistics of this model's VecNormalize: that wrapper returns raw observations and
+        ``predict`` normalises them on the device."""
+        return bool(getattr(self._vec_normalize_env, "learner_owns_obs_rms", False))
+
+    def _attach_device_norm(self):
+        """device_obs_norm: the wrapper's obs_rms moves to this learner, unless another learner owns it already (a second
+        model on the same env reads the owner's statistics and leaves them where they are)."""
+        vn = self._vec_normalize_env
+        if self.device_obs_norm and isinstance(vn, VecNormalize) and vn.norm_obs and not vn.learner_owns_obs_rms:
+            vn.give_obs_rms_to(self.learner)
+        if self._owns_obs_rms():
+            self._sync_norm_stats()
+
+    def _sync_norm_stats(self):
+        """The owner's reward scalars and clips for the gather (the observation statistics are the learner's own)."""
+        vn = self._vec_normalize_env
+        self.learner.set_norm_stats(None, None, float(vn.ret_rms.var), vn.clip_obs, vn.clip_reward, vn.epsilon,
+                                    norm_obs=vn.norm_obs, norm_reward=vn.norm_reward)
 
     def get_env(self):
         return self.env
@@ -217,18 +335,31 @@ class BDQ:
         callback = as_callback(callback)
         callback.init_callback(self)
         callback.on_training_start({"self": self, "writer": None}, globals())
+        dev = self.device_obs_norm
+        vn = self._vec_normalize_env
+        if dev:
+            if not isinstance(vn, VecNormalize) or not vn.norm_obs:
+                raise RuntimeError("device_obs_norm=True needs the env wrapped in a VecNormalize with norm_obs=True")
+            if not self._owns_obs_rms():
+                raise RuntimeError("learn: the env's VecNormalize statistics are owned by another model's learner (close that model, "
+                                   "or build this one with device_obs_norm=True before it)")
         obs = self.env.reset()
         n_env, D = self.env.num_envs, self.learner.n_branches
         lr = self.learning_rate if not callable(self.learning_rate) else self.learning_rate(1.0)
+        if dev:      # the reset frames: uploaded once, merged (VecNormalize.reset's update), staged as every env's current observation
+            self.learner.observe_act(np.asarray(obs, np.float32), update_stats=vn.training, act=False)
         # reset_num_timesteps=False continues a run: epsilon and beta follow num_timesteps over the schedule of a run that ends
         # total_timesteps from now (the stable-baselines DQN rule)
         resume = not reset_num_timesteps
         horizon = self.num_timesteps + total_timesteps if resume else total_timesteps
         for t in range(0, total_timesteps, n_env):
             eps = self._epsilon(self.num_timesteps if resume else t, horizon)
-            idx = self.learner.act(np.asarray(obs, np.float32))
-            explore = self._rng.random((n_env, D)) < eps                       # independent epsilon-greedy per branch
-            idx = np.where(explore, self._rng.integers(0, self.num_actions_pad, (n_env, D)), idx)
+            if dev:      # the staged frames, current statistics, epsilon-greedy on the device
+                idx = self.learner.observe_act(None, n=n_env, eps=eps)
+            else:
+                idx = self.learner.act(np.asarray(obs, np.float32))
+                explore = self._rng.random((n_env, D)) < eps                   # independent epsilon-greedy per branch
+                idx = np.where(explore, self._rng.integers(0, self.num_actions_pad, (n_env, D)), idx)
             new_obs, rew, done, infos = self.env.step(self._bins[idx])
             self.num_timesteps += n_env
             if callback.on_step() is False:
@@ -236,14 +367,21 @@ class BDQ:
             nxt = np.array(new_obs, np.float32, copy=True)
             for i, info in enumerate(infos):
                 if done[i] and isinstance(info, dict) and "terminal_observation" in info:
-                    nxt[i] = np.asarray(info["terminal_observation"], np.float32).reshape(-1)
-            self.learner.replay_add(np.asarray(obs, np.float32), idx.astype(np.float32), rew, nxt, np.asarray(done, np.float32))
+                    nxt[i] = np.asarray(info["terminal_observation"], np.float32).reshape(nxt[i].shape)
+            if dev:      # raw transitions; next_obs crosses once, a finished env's reset frame is merged and staged
+                self.learner.observe_add(idx.astype(np.float32), vn.get_original_reward(), nxt, np.asarray(done, np.float32),
+                                         reset_obs=np.asarray(new_obs, np.float32) if np.any(done) else None,
+                                         update_stats=vn.training)       # step_wait's update; a callback may switch it
+            else:
+                self.learner.replay_add(np.asarray(obs, np.float32), idx.astype(np.float32), rew, nxt, np.asarray(done, np.float32))
             obs = new_obs
             if self.num_timesteps > self.learning_starts and self.num_timesteps % self.train_freq == 0 and \
                     self.learner.replay_size() >= self.batch_size:
                 if self.prioritized_replay:          # [SB2] LinearSchedule(beta_iters, initial_p=beta0, final_p=1.0)
                     iters = self.per_beta_iters or horizon
                     self.learner.set_per_beta(self.per_beta0 + min(1.0, self.num_timesteps / iters) * (1.0 - self.per_beta0))
+                if dev:      # the sample is normalised with the statistics of this moment: obs_rms on the device, ret_rms here
+                    self._sync_norm_stats()
                 self.learner.step(1, lr)
         callback.on_training_end()
         return self
@@ -290,6 +428,8 @@ class BDQ:
                     prioritized_replay_beta0=self.per_beta0, prioritized_replay_beta_iters=self.per_beta_iters,
                     prioritized_replay_eps=self.per_eps, policy_kwargs=self.policy_kwargs, verbose=self.verbose, seed=self.seed,
                     device=self.device)
+        if self.device_obs_norm:
+            init["device_obs_norm"] = True
         return {"algo": "BDQ", "init": init, "num_timesteps": int(self.num_timesteps), "rng": training_state.rng_state(self._rng)}
 
     def save_training_state(self, path):
@@ -307,6 +447,7 @@ class BDQ:
             raise ValueError(f"{path} holds a {host.get('algo')} training state")
         model = cls("MlpActPolicy", env, **dict(host["init"], **kwargs))
         training_state.restore_vec_normalize(path, model.env)
+        model._attach_device_norm()        # the restored statistics go back to the learner; learner.state carries the same ones
         model.load_parameters(os.path.join(path, training_state.MODEL_FILE))
         model.learner.load_state(os.path.join(path, training_state.STATE_FILE))
         model.num_timesteps = int(host["num_timesteps"])
@@ -336,6 +477,7 @@ class BDQ:
         kw.update(kwargs)
         m = cls("MlpActPolicy", None, _init_setup_model=False, **kw)
         m.env = e if env is not None else None
+        m._vec_normalize_env = m.get_vec_normalize_env() if env is not None else None
         m.observation_space, m.action_space = e.observation_space, e.action_space
         m.setup_model()
         m.learner.load_parameters(params, exact_match=True)

@@ -10,11 +10,15 @@
 // the dueling aggregation, double-Q target, TD loss and backward seeds are one fused per-sample kernel.
 // Output-layer weights are held with their row stride padded to 4 floats (n_bins = 33 -> 36) so every
 // operand row is 16-byte aligned; get/set repack to the zip layout.
+// With device statistics (b2g_bdq_obs_rms_set) the learn loop's actor side runs here too: b2g_bdq_observe_act / _add stage each
+// new frame once, merge it into VecNormalize's obs_rms (obsnorm.cu's kernel), act epsilon-greedily on the device (Philox stream
+// 3) and commit transitions into the replay with a kernel.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <map>
 #include <string>
 #include <vector>
@@ -107,6 +111,49 @@ __global__ void bdq_argmax_kernel(const float* const* A, int n_rows, int D, int 
   float bv = a[0];
   for (int k = 1; k < n; ++k) if (a[k] > bv) { bv = a[k]; best = k; }
   out[i] = best;
+}
+
+// The epsilon-greedy actor of b2g_bdq_observe_act on `rows` evaluated rows (env row0 + b): per branch the greedy bin, and with
+// probability eps a uniform random bin instead, independently per (env, branch).  Philox stream 3 at step counters[7] (the
+// number of earlier acting observe_act calls), block (row0 + b) * D + d: lane x decides, ((x + 0.5) 2^-32 < eps in float64, so
+// eps = 0 never explores and eps = 1 always does), lane y picks the bin (y * n) >> 32.  One CTA; the last chunk of a call
+// advances the counter.
+__global__ void bdq_explore_kernel(const float* const* A, int rows, int row0, int D, int n, int NBS, float eps, unsigned long long seed,
+                                   long long* counters, int advance, int* out) {
+  const unsigned long long step = (unsigned long long)counters[7];
+  const uint2 key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
+  for (int i = threadIdx.x; i < rows * D; i += blockDim.x) {
+    const int b = i / D, d = i - b * D;
+    const float* a = A[d] + (size_t)b * NBS;
+    int best = 0;
+    float bv = a[0];
+    for (int k = 1; k < n; ++k) if (a[k] > bv) { bv = a[k]; best = k; }
+    const unsigned blk = (unsigned)((row0 + b) * D + d);
+    const uint4 r = philox4x32_10(make_uint4((unsigned)step, (unsigned)(step >> 32), blk, 3u), key);
+    const bool explore = ((double)r.x + 0.5) * (1.0 / 4294967296.0) < (double)eps;
+    out[(size_t)(row0 + b) * D + d] = explore ? (int)(((unsigned long long)r.y * (unsigned)n) >> 32) : best;
+  }
+  if (advance) {
+    __syncthreads();
+    if (threadIdx.x == 0) counters[7] = (long long)step + 1;
+  }
+}
+
+// b2g_bdq_observe_add: transition i = (cur[i], act[i], rew[i], nxt[i], done[i]) -> replay slot (first + i) % cap, one CTA per
+// row; CTA 0 also writes the new replay size into counters[5] (what b2g_bdq_replay_add uploads)
+__global__ void bdq_commit_kernel(const float* __restrict__ cur, const float* __restrict__ nxt, const float* __restrict__ act,
+                                  const float* __restrict__ rew, const float* __restrict__ done, int E, int D, long long first, long long cap,
+                                  float* __restrict__ r_obs, float* __restrict__ r_next, float* __restrict__ r_act, float* __restrict__ r_rew,
+                                  float* __restrict__ r_done, long long* counters, long long new_size) {
+  const int i = blockIdx.x;
+  const long long slot = (first + i) % cap;
+  for (int e = threadIdx.x; e < E; e += blockDim.x) {
+    r_obs[slot * E + e] = cur[(size_t)i * E + e];
+    r_next[slot * E + e] = nxt[(size_t)i * E + e];
+  }
+  if (threadIdx.x < D) r_act[slot * D + threadIdx.x] = act[(size_t)i * D + threadIdx.x];
+  if (threadIdx.x == 0) { r_rew[slot] = rew[i]; r_done[slot] = done[i]; }
+  if (i == 0 && threadIdx.x == 0) counters[5] = new_size;
 }
 
 // ------------------------------------------------------------------------------------------------ prioritised replay
@@ -227,6 +274,20 @@ struct b2g_bdq {
   cudaGraphExec_t graph_exec = nullptr;
   bool use_graph = true;
   bool broken = false;         // a training-state load failed after it began writing: only destroy / load are accepted
+  double norm_eps = 1e-8;      // VecNormalize.epsilon of the last b2g_bdq_set_norm_stats
+  // Device-resident VecNormalize observation statistics (created by b2g_bdq_obs_rms_set): float64 mean / var [E]; the count
+  // stays on the host.  b2g_bdq_observe_act / _add staging (allocated on first use): the current observation of env i as a row
+  // of ob_rows[ob_k] (the other buffer takes the next call's next_obs), the reset frames of finished envs, and the call's
+  // actions / rewards / done flags.
+  double *rms_mean = nullptr, *rms_var = nullptr;
+  double rms_count = 0.0;
+  int stage_rows = 0;          // max(batch, 256) envs per observe call
+  float* ob_rows[2]{};         // [stage_rows + B][E] (the actor's gather reads B rows from any chunk start)
+  float* ob_reset = nullptr;   // [stage_rows][E]
+  float *ob_act = nullptr, *ob_rew = nullptr, *ob_done = nullptr;
+  int* ob_idx = nullptr;       // [stage_rows][D] actor output
+  int ob_k = 0, ob_n = 0;
+  int64_t up_observe = 0, up_other = 0;    // host->device bytes: observe_* / obs_rms_set, and act + replay_add + set_norm_stats
   float* p(const std::string& nm) { return P + tensors[tindex.at(nm)].off; }
   float* g(const std::string& nm) { return G + tensors[tindex.at(nm)].off; }
   float* pt(const std::string& nm) { return P + n_train + tensors[tindex.at(nm)].off; }
@@ -454,6 +515,7 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
   h->B = cfg->batch; h->D = cfg->n_branches; h->n = cfg->n_bins; h->NBS = (cfg->n_bins + 3) / 4 * 4;
   h->T0 = cfg->trunk0; h->T1 = cfg->trunk1; h->HB = cfg->branch_hidden; h->E = cfg->obs_dim;
   h->XS = (cfg->obs_dim + cfg->n_branches + 7) / 8 * 8;
+  h->stage_rows = std::max(cfg->batch, 256);
   auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_bdq_destroy(h); g_b2g_err = keep; return rc; };
   if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream"));
   // parameter inventory: same names as the zips (oracle/bdq_ref.py param_specs)
@@ -594,6 +656,7 @@ int b2g_bdq_replay_add(b2g_bdq* h, const float* obs, const float* act_idx, const
     CK(cudaMemcpyAsync(h->r_act + h->r_pos * D, act_idx + done_n * D, chunk * D * sizeof(float), cudaMemcpyDefault, h->stream));
     CK(cudaMemcpyAsync(h->r_rew + h->r_pos, rew + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
     CK(cudaMemcpyAsync(h->r_done + h->r_pos, done + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
+    h->up_other += (int64_t)(chunk * (2 * E + D + 2) * sizeof(float));
     if (h->per) {        // new transitions enter with the running maximum priority ([SB2] PrioritizedReplayBuffer.add)
       PerArgs pr{};
       pr.tsum = h->t_sum; pr.tmin = h->t_min; pr.C = h->per_C; pr.max_prio = h->max_prio; pr.alpha = h->cfg.per_alpha; pr.eps = h->cfg.per_eps;
@@ -608,6 +671,7 @@ int b2g_bdq_replay_add(b2g_bdq* h, const float* obs, const float* act_idx, const
   }
   const long long sz = h->r_size;
   CK(cudaMemcpyAsync(h->counters + 5, &sz, sizeof(long long), cudaMemcpyHostToDevice, h->stream));
+  h->up_other += (int64_t)sizeof(long long);
   CK(cudaStreamSynchronize(h->stream));
   return 0;
 }
@@ -617,17 +681,31 @@ int b2g_bdq_set_norm_stats(b2g_bdq* h, const double* obs_mean, const double* obs
                            int norm_obs, int norm_reward) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  if (norm_obs && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
+  if (norm_obs && !h->rms_mean && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
-  if (norm_obs) {
+  const bool eps_changed = eps != h->norm_eps;
+  h->norm_eps = eps;
+  if (h->rms_mean) {
+    // the handle owns obs_rms: statistics passed here replace it (count kept); the gather's table is derived on the device,
+    // again when only epsilon changed
+    if (obs_mean && obs_var) {
+      if (int rc = b2g_bdq_obs_rms_set(h, obs_mean, obs_var, h->rms_count)) return rc;
+    } else if (eps_changed) {
+      obs_rms_update_launch(nullptr, nullptr, nullptr, 0, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, 0, 0,
+                            h->stream);
+      CK(cudaStreamSynchronize(h->stream));
+    }
+  } else if (norm_obs) {
     std::vector<double> istd(h->E);
     for (int i = 0; i < h->E; ++i) istd[i] = 1.0 / sqrt(obs_var[i] + eps);
     CK(cudaMemcpy(h->d_mean, obs_mean, h->E * sizeof(double), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(h->d_istd, istd.data(), h->E * sizeof(double), cudaMemcpyHostToDevice));
+    h->up_other += (int64_t)(2 * h->E * sizeof(double));
   }
   const double nc[8] = {1.0 / sqrt(ret_var + eps), clip_obs, clip_rew, (double)norm_obs, (double)norm_reward, 0, 0, 0};
   CK(cudaMemcpy(h->d_normc, nc, sizeof(nc), cudaMemcpyHostToDevice));
+  h->up_other += (int64_t)sizeof(nc);
   return 0;
 }
 
@@ -697,6 +775,7 @@ int b2g_bdq_act(b2g_bdq* h, const float* obs, int n, int32_t* act_idx_out) {
   for (int done_n = 0; done_n < n; done_n += h->B) {
     const int chunk = std::min(h->B, n - done_n);
     CK(cudaMemcpyAsync(h->s_obs, obs + (size_t)done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
+    h->up_other += (int64_t)(chunk * E * sizeof(float));
     GatherArgs g = bgather(h, false, false);
     gather_launch(g, h->stream);
     for (auto& gr : h->act) gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
@@ -704,6 +783,160 @@ int b2g_bdq_act(b2g_bdq* h, const float* obs, int n, int32_t* act_idx_out) {
     CK(cudaMemcpyAsync(act_idx_out + (size_t)done_n * D, h->act_idx_out, chunk * D * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
   }
+  CK(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ obs_rms on the device and the
+// actor loop fed from one upload per frame (the BDQ counterpart of obsnorm.cu; the merge is the same kernel, flat layout)
+int b2g_bdq_obs_rms_set(b2g_bdq* h, const double* mean, const double* var, double count) {
+  B2G_USABLE(h);
+  if (!h || !mean || !var) return b2g_fail(B2G_EINVAL, "NULL argument");
+  if (!(count >= 0.0) || !std::isfinite(count)) return b2g_fail(B2G_EINVAL, "obs_rms_set: count must be finite and >= 0");
+  for (int e = 0; e < h->E; ++e)
+    if (!std::isfinite(mean[e]) || !(var[e] >= 0.0) || !std::isfinite(var[e]))
+      return b2g_fail(B2G_EINVAL, "obs_rms_set: mean must be finite and var finite and >= 0 (element " + std::to_string(e) + ")");
+  if (h->cfg.nranks > 1)
+    return b2g_fail(B2G_ESTATE, "device observation statistics are per handle: with nranks > 1 every rank would own different ones");
+  CK(cudaSetDevice(h->cfg.device));
+  if (!h->rms_mean) {     // one allocation for both arrays: it either exists or it does not
+    double* mv = nullptr;
+    if (int rc = dev_alloc(h->allocs, h->stream, &mv, 2 * (size_t)h->E, false)) return rc;
+    h->rms_mean = mv;
+    h->rms_var = mv + h->E;
+  }
+  CK(cudaMemcpyAsync(h->rms_mean, mean, h->E * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(h->rms_var, var, h->E * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  h->up_observe += (int64_t)(2 * h->E * sizeof(double));
+  h->rms_count = count;
+  obs_rms_update_launch(nullptr, nullptr, nullptr, 0, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, 0, 0,
+                        h->stream);
+  CK(cudaStreamSynchronize(h->stream));     // host arrays are caller-owned: copied before return
+  return 0;
+}
+
+int b2g_bdq_obs_rms_get(b2g_bdq* h, double* mean, double* var, double* count) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  if (!h->rms_mean) return b2g_fail(B2G_ESTATE, "the handle has no device statistics: call b2g_bdq_obs_rms_set first");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  if (mean) CK(cudaMemcpy(mean, h->rms_mean, h->E * sizeof(double), cudaMemcpyDeviceToHost));
+  if (var) CK(cudaMemcpy(var, h->rms_var, h->E * sizeof(double), cudaMemcpyDeviceToHost));
+  if (count) *count = h->rms_count;
+  return 0;
+}
+
+int b2g_bdq_upload_bytes(const b2g_bdq* h, int64_t* observe_bytes, int64_t* other_bytes) {
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  if (observe_bytes) *observe_bytes = h->up_observe;
+  if (other_bytes) *other_bytes = h->up_other;
+  return 0;
+}
+
+static int bdq_upload(b2g_bdq* h, void* dst, const void* src, size_t bytes) {
+  CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream));
+  h->up_observe += (int64_t)bytes;
+  return 0;
+}
+
+static void bdq_merge(b2g_bdq* h, const float* a, const float* b, const float* done, int n) {
+  obs_rms_update_launch(a, b, done, n, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, 0, 0, h->stream);
+  h->rms_count += n;
+}
+
+static int bdq_observe_checks(b2g_bdq* h, int n, int update_stats) {
+  if (n < 1 || n > h->stage_rows)
+    return b2g_fail(B2G_EINVAL, "observe: n must be in [1, " + std::to_string(h->stage_rows) + "] (the staging holds max(batch, 256) frames)");
+  if (update_stats && !h->rms_mean) return b2g_fail(B2G_ESTATE, "update_stats needs device statistics: call b2g_bdq_obs_rms_set first");
+  if (h->ob_rows[0]) return 0;
+  const size_t R = h->stage_rows, E = h->E;
+  for (int k = 0; k < 2; ++k)
+    if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_rows[k], (R + h->B) * E)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_reset, R * E)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_act, R * h->D)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_rew, R)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_done, R)) return rc;
+  return dev_alloc(h->allocs, h->stream, &h->ob_idx, R * h->D);
+}
+
+int b2g_bdq_observe_act(b2g_bdq* h, const float* obs, int n, int update_stats, float eps, int32_t* act_idx_out) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  if (!obs && !act_idx_out) return b2g_fail(B2G_EINVAL, "observe_act: nothing to do (obs and act_idx_out are NULL)");
+  if (act_idx_out && !(eps >= 0.f && eps <= 1.f)) return b2g_fail(B2G_EINVAL, "observe_act: eps must be in [0, 1]");
+  CK(cudaSetDevice(h->cfg.device));
+  if (int rc = bdq_observe_checks(h, n, obs ? update_stats : 0)) return rc;
+  if (!obs && h->ob_n == 0) return b2g_fail(B2G_ESTATE, "observe_act: no staged observations (pass obs first)");
+  if (!obs && n != h->ob_n) return b2g_fail(B2G_EINVAL, "observe_act: n differs from the number of staged observations");
+  const size_t E = h->E, D = h->D;
+  float* cur = h->ob_rows[h->ob_k];
+  if (obs) {
+    if (int rc = bdq_upload(h, cur, obs, n * E * sizeof(float))) return rc;
+    if (update_stats) bdq_merge(h, cur, nullptr, nullptr, n);
+    h->ob_n = n;
+  }
+  if (act_idx_out) {
+    const unsigned long long seed = h->cfg.seed + 0x9E3779B97F4A7C15ull * (unsigned long long)h->cfg.rank;
+    for (int k = 0; k < n; k += h->B) {
+      const int chunk = std::min(h->B, n - k);
+      GatherArgs g = bgather(h, false, false);
+      g.obs = cur + (size_t)k * E;
+      gather_launch(g, h->stream);
+      for (auto& gr : h->act) gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
+      bdq_explore_kernel<<<1, 256, 0, h->stream>>>(h->d_Aptr, chunk, k, (int)D, h->n, h->NBS, eps, seed, h->counters, k + chunk >= n, h->ob_idx);
+    }
+    CK(cudaMemcpyAsync(act_idx_out, h->ob_idx, n * D * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+  }
+  CK(cudaStreamSynchronize(h->stream));     // caller-owned arrays are copied, the actions are the result of the call
+  CK(cudaGetLastError());
+  return 0;
+}
+
+int b2g_bdq_observe_add(b2g_bdq* h, const float* act_idx, const float* rew, const float* next_obs, const float* done, const float* reset_obs,
+                        int n, int update_stats) {
+  B2G_USABLE(h);
+  if (!h || !act_idx || !rew || !next_obs || !done) return b2g_fail(B2G_EINVAL, "NULL argument");
+  CK(cudaSetDevice(h->cfg.device));
+  if (int rc = bdq_observe_checks(h, n, update_stats)) return rc;
+  if (h->ob_n == 0) return b2g_fail(B2G_ESTATE, "observe_add: no staged observations (call b2g_bdq_observe_act first)");
+  if (n != h->ob_n) return b2g_fail(B2G_EINVAL, "observe_add: n differs from the number of staged observations");
+  if (n > h->cfg.buffer_capacity) return b2g_fail(B2G_EINVAL, "observe_add: n exceeds buffer_capacity");
+  int n_done = 0;
+  for (int i = 0; i < n; ++i) n_done += done[i] != 0.f;
+  if (n_done && !reset_obs) return b2g_fail(B2G_EINVAL, "observe_add: an env finished but reset_obs is NULL");
+  const size_t E = h->E, D = h->D, fb = E * sizeof(float);
+  float* cur = h->ob_rows[h->ob_k];
+  float* nxt = h->ob_rows[h->ob_k ^ 1];
+  if (int rc = bdq_upload(h, nxt, next_obs, n * fb)) return rc;
+  for (int i = 0; i < n; ++i)         // only the frames of finished envs cross the bus
+    if (done[i] != 0.f)
+      if (int rc = bdq_upload(h, h->ob_reset + i * E, reset_obs + i * E, fb)) return rc;
+  if (int rc = bdq_upload(h, h->ob_act, act_idx, n * D * sizeof(float))) return rc;
+  if (int rc = bdq_upload(h, h->ob_rew, rew, n * sizeof(float))) return rc;
+  if (int rc = bdq_upload(h, h->ob_done, done, n * sizeof(float))) return rc;
+  // the transitions: obs = the staged rows, next_obs = the uploaded rows (a finished env's terminal frame)
+  const int64_t cap = h->cfg.buffer_capacity;
+  const int64_t new_size = std::min<int64_t>(cap, h->r_size + n);
+  bdq_commit_kernel<<<n, 256, 0, h->stream>>>(cur, nxt, h->ob_act, h->ob_rew, h->ob_done, (int)E, (int)D, h->r_pos, cap, h->r_obs, h->r_next,
+                                              h->r_act, h->r_rew, h->r_done, h->counters, new_size);
+  if (h->per) {        // new transitions enter with the running maximum priority, as in b2g_bdq_replay_add
+    PerArgs pr{};
+    pr.tsum = h->t_sum; pr.tmin = h->t_min; pr.C = h->per_C; pr.max_prio = h->max_prio; pr.alpha = h->cfg.per_alpha; pr.eps = h->cfg.per_eps;
+    for (int o = 0; o < n; o += 1024) {
+      const int nn = std::min(1024, n - o);
+      per_write_kernel<<<1, ((nn + 31) / 32) * 32, 0, h->stream>>>(pr, nullptr, h->r_pos + o, cap, nn, 0);
+    }
+  }
+  // VecNormalize's step_wait merges the frames the VecEnv returned: a finished env's reset frame, not its terminal observation
+  if (update_stats) bdq_merge(h, nxt, n_done ? h->ob_reset : nullptr, h->ob_done, n);
+  // the new rows become the current observations; a finished env continues from the frame its reset returned
+  for (int i = 0; i < n; ++i)
+    if (done[i] != 0.f) CK(cudaMemcpyAsync(nxt + i * E, h->ob_reset + i * E, fb, cudaMemcpyDeviceToDevice, h->stream));
+  h->r_pos = (h->r_pos + n) % cap;
+  h->r_size = new_size;
+  h->ob_k ^= 1;
+  CK(cudaStreamSynchronize(h->stream));     // host arrays are caller-owned: copied before return
   CK(cudaGetLastError());
   return 0;
 }
@@ -723,6 +956,14 @@ std::vector<FpField> bdq_fingerprint(const b2g_bdq* h) {
           fp_int("trunk_grad_rescale", c.trunk_grad_rescale), fp_int("seed", (int64_t)c.seed),
           fp_int("prioritized_replay", c.prioritized_replay), fp_real("per_alpha", c.per_alpha), fp_real("per_eps", c.per_eps)};
 }
+// a handle that owns obs_rms writes one more field and one more section (count, mean[E], var[E] as float64); one that does not
+// reads and writes the files it always did
+std::vector<FpField> bdq_fingerprint_rms(const b2g_bdq* h) {
+  std::vector<FpField> fp = bdq_fingerprint(h);
+  if (h->rms_mean) fp.push_back(fp_int("obs_rms", 1));
+  return fp;
+}
+const uint32_t kBdqRmsTag = state_tag("ORMS");
 
 const uint32_t kBdqTags[] = {state_tag("HOST"), state_tag("CNTR"), state_tag("PARM"), state_tag("ADMM"), state_tag("ADMV"),
                              state_tag("ROBS"), state_tag("RNXT"), state_tag("RACT"), state_tag("RREW"), state_tag("RDON"),
@@ -768,7 +1009,14 @@ int b2g_bdq_state_save(b2g_bdq* h, const char* path) {
   secs[0].tag = kBdqTags[0]; secs[0].pieces = {StatePiece{hv, nullptr, sizeof hv}};
   secs[1].tag = kBdqTags[1]; secs[1].pieces = {StatePiece{cnt, nullptr, sizeof cnt}};
   for (auto& s : bdq_device_sections(h, h->r_size)) secs.push_back(std::move(s));
-  return state_write(path, STATE_KIND_BDQ, bdq_fingerprint(h), secs);
+  if (h->rms_mean) {
+    StateSection r;
+    r.tag = kBdqRmsTag;
+    r.pieces = {StatePiece{&h->rms_count, nullptr, sizeof(double)}, bdev(h->rms_mean, h->E * sizeof(double)),
+                bdev(h->rms_var, h->E * sizeof(double))};
+    secs.push_back(std::move(r));
+  }
+  return state_write(path, STATE_KIND_BDQ, bdq_fingerprint_rms(h), secs);
 }
 
 int b2g_bdq_state_load(b2g_bdq* h, const char* path) {
@@ -777,9 +1025,21 @@ int b2g_bdq_state_load(b2g_bdq* h, const char* path) {
   CK(cudaSetDevice(h->cfg.device));
   // ---- everything is checked before the handle changes
   StateReader rd;
-  if (int rc = rd.open(path, STATE_KIND_BDQ, bdq_fingerprint(h))) return rc;
+  if (int rc = rd.open(path, STATE_KIND_BDQ, bdq_fingerprint_rms(h))) {
+    // a file with one fingerprint field more or fewer than this handle: say which side owns obs_rms
+    const std::string msg = g_b2g_err;
+    StateReader other;
+    std::vector<FpField> fp = bdq_fingerprint(h);
+    if (!h->rms_mean) fp.push_back(fp_int("obs_rms", 1));
+    if (other.open(path, STATE_KIND_BDQ, fp) == 0)
+      return b2g_fail(B2G_EINVAL, h->rms_mean ? "the state file has no obs_rms, but this handle owns the observation statistics (b2g_bdq_obs_rms_set)"
+                                              : "the state file carries obs_rms: call b2g_bdq_obs_rms_set on this handle before loading it");
+    return b2g_fail(rc, msg);
+  }
   const int n_sec = (int)(sizeof kBdqTags / sizeof kBdqTags[0]);
-  if (rd.n_sections() != n_sec) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a BDQ learner");
+  const int n_file = n_sec + (h->rms_mean ? 1 : 0);
+  if (rd.n_sections() != n_file || (h->rms_mean && (rd.tag(n_sec) != kBdqRmsTag || rd.bytes(n_sec) != (uint64_t)(2 * h->E + 1) * sizeof(double))))
+    return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a BDQ learner");
   for (int i = 0; i < n_sec; ++i)
     if (rd.tag(i) != kBdqTags[i]) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a BDQ learner");
   int64_t hv[4];
@@ -800,6 +1060,16 @@ int b2g_bdq_state_load(b2g_bdq* h, const char* path) {
   h->broken = true;
   for (int i = 0; i < (int)dev.size(); ++i)
     if (int rc = rd.read_pieces(i + 2, dev[i].pieces)) return rc;
+  if (h->rms_mean) {
+    double count = 0.0;
+    if (int rc = rd.read_pieces(n_sec, {StatePiece{&count, nullptr, sizeof(double)}, bdev(h->rms_mean, h->E * sizeof(double)),
+                                        bdev(h->rms_var, h->E * sizeof(double))})) return rc;
+    h->rms_count = count;
+    obs_rms_update_launch(nullptr, nullptr, nullptr, 0, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, 0, 0,
+                          h->stream);
+    CK(cudaStreamSynchronize(h->stream));
+  }
+  h->ob_n = 0;         // the staged observations are not part of the file: a resumed run starts a fresh episode
   CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
   h->r_size = hv[0]; h->r_pos = hv[1]; h->n_updates = hv[2];
   const uint32_t eps_bits = (uint32_t)hv[3];

@@ -302,6 +302,13 @@ struct GatherArgs {
 };
 void gather_launch(const GatherArgs& a, cudaStream_t s);
 
+// VecNormalize obs_rms merge (obsnorm.cu): the n frames a[i] (b[i] where done[i] != 0 when b != nullptr) -> float64 mean / var
+// [E] by RunningMeanStd.update_from_moments with the prior count, then the gather's table d_mean / d_istd = 1/sqrt(var + eps).
+// Table layout: Cfull > 0 = CNN compact rows of [HW][Cfull] frames (image planes, then the actuator value at index npx);
+// Cfull == 0 = flat, entry e for element e.  n == 0 only derives the table.
+void obs_rms_update_launch(const float* a, const float* b, const float* done, int n, int E, double count, double eps, double* mean,
+                           double* var, double* d_mean, double* d_istd, int Cfull, int npx, cudaStream_t s);
+
 // Philox4x32-10 (counter-based RNG shared by prep_kernel and the in-kernel replay slot draw)
 #ifdef __CUDACC__
 __device__ __forceinline__ void philox_round(uint4& c, uint2& k) {

@@ -1,5 +1,6 @@
 // VecNormalize's observation statistics on the device, and the actor side of the learn loop fed from one upload per frame
-// (b2g_sac_observe_act / b2g_sac_observe_add / b2g_obs_rms_set / b2g_obs_rms_get; contracts in include/b200grasp.h).
+// (b2g_sac_observe_act / b2g_sac_observe_add / b2g_obs_rms_set / b2g_obs_rms_get; contracts in include/b200grasp.h).  The BDQ
+// learner's b2g_bdq_observe_* (bdq.cu) merge into its own obs_rms with the same kernel (obs_rms_update_launch, flat layout).
 //
 // obs_rms = (mean[E], var[E], count) in float64 over the caller's observation layout, the object [SB2]
 // common/running_mean_std.py keeps on the host.  obs_rms_update_kernel merges the n frames of one call into it with the
@@ -39,6 +40,7 @@ __device__ __forceinline__ float frame_value(const float* __restrict__ a, const 
 // values are summed in frame order 0 .. n-1 (mean, then squared deviations from it), so the result does not depend on the
 // grid; consecutive threads read consecutive floats of every frame.  n == 0 only derives the table.
 // Cfull > 0: [HW][Cfull] observations whose compact row keeps the image planes and pixel [0,0] of the last plane (index npx).
+// Cfull == 0: the flat layout, table entry e = element e (SAC's MLP rows, BDQ's [obs_dim] rows).
 template <bool RESET>
 __global__ void __launch_bounds__(256) obs_rms_update_kernel(const float* __restrict__ a, const float* __restrict__ b,
                                                               const float* __restrict__ done, int n, int E, double count, double eps,
@@ -75,11 +77,8 @@ __global__ void __launch_bounds__(256) obs_rms_update_kernel(const float* __rest
 
 void update_launch(b2g_sac* h, const float* a, const float* b, const float* done, int n) {
   const int Cfull = h->cnn ? h->Cimg + 1 : 0, npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0;
-  const dim3 grid((h->E + 255) / 256);
-  if (b) obs_rms_update_kernel<true><<<grid, 256, 0, h->stream>>>(a, b, done, n, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var,
-                                                                 h->d_mean, h->d_istd, Cfull, npx);
-  else obs_rms_update_kernel<false><<<grid, 256, 0, h->stream>>>(a, b, done, n, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var,
-                                                                 h->d_mean, h->d_istd, Cfull, npx);
+  obs_rms_update_launch(a, b, done, n, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, Cfull, npx,
+                        h->stream);
   h->rms_count += n;
 }
 
@@ -140,6 +139,13 @@ int common_checks(b2g_sac* h, int n, int update_stats) {
 }
 
 }  // namespace
+
+void obs_rms_update_launch(const float* a, const float* b, const float* done, int n, int E, double count, double eps, double* mean,
+                           double* var, double* d_mean, double* d_istd, int Cfull, int npx, cudaStream_t s) {
+  const dim3 grid((E + 255) / 256);
+  if (b) obs_rms_update_kernel<true><<<grid, 256, 0, s>>>(a, b, done, n, E, count, eps, mean, var, d_mean, d_istd, Cfull, npx);
+  else obs_rms_update_kernel<false><<<grid, 256, 0, s>>>(a, b, done, n, E, count, eps, mean, var, d_mean, d_istd, Cfull, npx);
+}
 
 void obs_rms_derive(b2g_sac* h) { update_launch(h, nullptr, nullptr, nullptr, 0); }
 

@@ -129,7 +129,7 @@ def train(args):
                     exploration_fraction=c.get("exploration_fraction", 0.1), exploration_final_eps=c.get("exploration_final_eps", 0.02),
                     num_actions_pad=c.get("num_actions_pad", 33), learning_starts=c.get("learning_starts", 1000),
                     target_network_update_freq=c.get("target_network_update_freq", 1000),
-                    prioritized_replay=c.get("prioritized_replay", False))
+                    prioritized_replay=c.get("prioritized_replay", False), device_obs_norm=bool(args.device_norm))
         if args.load_dir:
             model.load_parameters(BDQ.load(args.load_dir, env).get_parameters())
     else:
@@ -266,8 +266,8 @@ def build_parser():
                    help="SAC replay frame budget buffer_size * (1 + F) + n_envs (observations shared between consecutive "
                         "transitions; 0.125 covers episodes down to ~9 steps); default: two frames per replay slot")
     t.add_argument("--device_norm", action="store_true",
-                   help="SAC: keep VecNormalize's observation statistics on the GPU and upload every frame once "
-                        "(SAC(device_obs_norm=True)); --resume takes it from the saved run")
+                   help="keep VecNormalize's observation statistics on the GPU and upload every frame once "
+                        "(SAC / BDQ(device_obs_norm=True)); --resume takes it from the saved run")
     t.add_argument("--eval_freq", type=int, default=50000)
     t.add_argument("--checkpoint_freq", type=int, default=25000)
     t.add_argument("--state_freq", type=int, default=None,

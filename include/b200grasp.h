@@ -279,6 +279,8 @@ int b2g_bdq_get_grad(b2g_bdq* h, const char* name, float* dst, size_t numel);
 int b2g_bdq_replay_add(b2g_bdq* h, const float* obs, const float* act_idx, const float* rew, const float* next_obs,
                        const float* done, int64_t n);
 int64_t b2g_bdq_replay_size(const b2g_bdq* h);
+/* On a handle that owns obs_rms (b2g_bdq_obs_rms_set, below) obs_mean / obs_var may be NULL with norm_obs != 0: the scalars
+ * are set and the device statistics stay; passing them replaces the device statistics (count kept). */
 int b2g_bdq_set_norm_stats(b2g_bdq* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs,
                            double clip_rew, double eps, int norm_obs, int norm_reward);
 /* n_steps x { uniform sample -> forward (online s, online s', target s') -> double-Q TD loss -> backward -> Adam ->
@@ -296,9 +298,37 @@ int b2g_bdq_step_explicit(b2g_bdq* h, const float* obs, const float* act_idx, co
                           float* td_out);
 /* greedy branch indices argmax_n Q_d(s, n) of the online network for n observations */
 int b2g_bdq_act(b2g_bdq* h, const float* obs, int n, int32_t* act_idx_out);
+
+/* ---- VecNormalize's observation statistics on the device and the epsilon-greedy actor fed from one upload per frame: the
+ *      BDQ counterpart of b2g_sac_observe_* (same merge rule and kernel, same rule for which frames are merged, obs_rms over
+ *      the flat [obs_dim] observation).  nranks == 1 only.  Up to max(batch, 256) frames per call; every call returns once the
+ *      handle's stream has run what it enqueued. */
+/* n raw observations (host, caller-owned), or obs == NULL to act on the observations already staged.  update_stats != 0:
+ * merge them into obs_rms first (B2G_ESTATE without b2g_bdq_obs_rms_set).  act_idx_out != NULL: run the online network on
+ * the staged rows normalised with the CURRENT statistics (the gather's rule: b2g_bdq_set_norm_stats's norm_obs and clip_obs),
+ * take the greedy bin of every branch and, independently per (env, branch) with probability eps in [0, 1], a uniform random
+ * bin instead; writes [n][n_branches] bin indices.  The random draws are Philox stream 3 under the training key at step
+ * counters[7] (the number of earlier acting calls, kept in the training-state file), block env * n_branches + branch: lane x
+ * explores when (x + 0.5) 2^-32 < eps (float64), lane y gives bin (y * n_bins) >> 32. */
+int b2g_bdq_observe_act(b2g_bdq* h, const float* obs, int n, int update_stats, float eps, int32_t* act_idx_out);
+/* Transition i = (staged obs_i, act_idx_i, rew_i, next_obs_i, done_i) into the replay (rows as b2g_bdq_replay_add stores them;
+ * new rows enter the prioritised-replay trees at the running maximum priority).  next_obs is uploaded ONCE: it is this
+ * transition's next observation, is merged into obs_rms when update_stats != 0 and becomes the staged observation of env i,
+ * unless done_i: then reset_obs_i (the frame the auto-reset returned; the only rows of reset_obs read) is merged and staged
+ * instead.  B2G_ESTATE before any b2g_bdq_observe_act; n must equal the number of staged observations. */
+int b2g_bdq_observe_add(b2g_bdq* h, const float* act_idx, const float* rew, const float* next_obs, const float* done,
+                        const float* reset_obs /* may be NULL when no env finished */, int n, int update_stats);
+/* obs_rms in and out: float64 [obs_dim] each + count, with the checks of b2g_obs_rms_set / _get */
+int b2g_bdq_obs_rms_set(b2g_bdq* h, const double* mean, const double* var, double count);
+int b2g_bdq_obs_rms_get(b2g_bdq* h, double* mean, double* var, double* count);
+/* bytes copied host -> device so far by b2g_bdq_observe_* and b2g_bdq_obs_rms_set (observe_bytes) and by b2g_bdq_act,
+ * b2g_bdq_replay_add and b2g_bdq_set_norm_stats (other_bytes); either may be NULL */
+int b2g_bdq_upload_bytes(const b2g_bdq* h, int64_t* observe_bytes, int64_t* other_bytes);
 /* training state, as b2g_sac_state_save / _load: online and target parameters, Adam moments, counters, n_updates, the live
- * replay rows, the prioritised-replay sum / min trees, max priority and beta, and bdq/eps.  The fingerprint covers every
- * b2g_bdq_cfg field that decides the layout or the prioritised replay. */
+ * replay rows, the prioritised-replay sum / min trees, max priority and beta, and bdq/eps; and the device obs_rms of a handle
+ * that owns one, behind one more fingerprint field (such a file loads only into a handle that owns obs_rms, and the reverse).
+ * The staged observations of b2g_bdq_observe_* are not saved: a resumed run starts a fresh episode.  The fingerprint covers
+ * every b2g_bdq_cfg field that decides the layout or the prioritised replay. */
 int b2g_bdq_state_save(b2g_bdq* h, const char* path);
 int b2g_bdq_state_load(b2g_bdq* h, const char* path);
 
