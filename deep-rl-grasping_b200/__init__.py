@@ -1,4 +1,4 @@
-"""b200grasp -- H100-native SAC learner behind the stable-baselines model API used by
+"""b200grasp -- H100-native SAC / BDQ / DQN learners behind the stable-baselines model API used by
 BarisYazici/deep-rl-grasping (manipulation_main/training/sb_helper.py:104-128,175).
 
 Import as ``b200grasp`` (``b200grasp.py`` at the repo root aliases this directory, whose name
@@ -17,6 +17,9 @@ _OUT_OF_SCOPE = ("DQN", "DDPG", "TD3", "TRPO", "PPO1", "PPO2", "A2C", "ACER", "A
 
 
 def __getattr__(name):           # sb.DQN / sb.TRPO / ... (sb_helper.py:139-199): the other branches of SBPolicy.learn
+    if name == "DQN":
+        raise NotImplementedError("b200grasp.DQN: the DQN learner is b200grasp.deepq.DQN (stable_baselines.deepq.DQN); "
+                                  "write sb.deepq.DQN at the DQN call sites")
     if name in _OUT_OF_SCOPE:
         raise NotImplementedError(f"b200grasp.{name}: only the SAC and BDQ learners are built (DESIGN.md section 7)")
     raise AttributeError(name)

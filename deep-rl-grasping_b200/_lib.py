@@ -26,6 +26,10 @@ SYMBOLS = [
     "b2g_bdq_get_grad", "b2g_bdq_replay_add", "b2g_bdq_replay_size", "b2g_bdq_set_norm_stats", "b2g_bdq_step",
     "b2g_bdq_step_explicit", "b2g_bdq_act", "b2g_bdq_set_per_beta", "b2g_bdq_get_last_per", "b2g_bdq_state_save", "b2g_bdq_state_load",
     "b2g_bdq_observe_act", "b2g_bdq_observe_add", "b2g_bdq_obs_rms_set", "b2g_bdq_obs_rms_get", "b2g_bdq_upload_bytes",
+    "b2g_dqn_create", "b2g_dqn_destroy", "b2g_dqn_param_count", "b2g_dqn_param_info", "b2g_dqn_get_param", "b2g_dqn_set_param",
+    "b2g_dqn_get_grad", "b2g_dqn_replay_add", "b2g_dqn_replay_size", "b2g_dqn_set_norm_stats", "b2g_dqn_step",
+    "b2g_dqn_step_explicit", "b2g_dqn_set_per_beta", "b2g_dqn_get_last_per", "b2g_dqn_update_target", "b2g_dqn_act",
+    "b2g_dqn_state_save", "b2g_dqn_state_load",
     "b2g_encoder_create", "b2g_encoder_destroy", "b2g_encoder_n_layers", "b2g_encoder_layer_shape", "b2g_encoder_set_weights",
     "b2g_encoder_encode", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor",
     "b2g_autoencoder_create", "b2g_autoencoder_destroy", "b2g_autoencoder_n_layers", "b2g_autoencoder_layer_shape",
@@ -57,6 +61,22 @@ class BdqCfg(C.Structure):
 
 class BdqMetrics(C.Structure):
     _fields_ = [("loss", C.c_float), ("mean_q", C.c_float), ("grad_norm", C.c_float), ("n_updates", C.c_int64)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class DqnCfg(C.Structure):
+    _fields_ = [
+        ("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("hidden0", C.c_int32), ("hidden1", C.c_int32), ("batch", C.c_int32),
+        ("buffer_capacity", C.c_int64), ("gamma", C.c_float), ("seed", C.c_uint64), ("device", C.c_int32),
+        ("prioritized_replay", C.c_int32), ("per_alpha", C.c_float), ("per_eps", C.c_float),
+    ]
+
+
+class DqnMetrics(C.Structure):
+    _fields_ = [("loss", C.c_float), ("mean_q", C.c_float), ("mean_abs_td", C.c_float), ("grad_norm", C.c_float),
+                ("n_clipped", C.c_int32), ("n_updates", C.c_int64)]
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
@@ -144,7 +164,8 @@ def load():
     lib.b2g_last_step_ms.argtypes = [vp]
     lib.b2g_last_step_ms.restype = C.c_float
     lib.b2g_profile_step.argtypes = [vp, C.c_float, C.POINTER(C.c_char_p), fp, C.c_int]
-    for f in ("b2g_sac_state_save", "b2g_sac_state_load", "b2g_bdq_state_save", "b2g_bdq_state_load"):
+    for f in ("b2g_sac_state_save", "b2g_sac_state_load", "b2g_bdq_state_save", "b2g_bdq_state_load", "b2g_dqn_state_save",
+              "b2g_dqn_state_load"):
         getattr(lib, f).argtypes = [vp, C.c_char_p]
     lib.b2g_bdq_create.argtypes = [C.POINTER(BdqCfg), C.POINTER(vp)]
     lib.b2g_bdq_destroy.argtypes = [vp]
@@ -166,6 +187,22 @@ def load():
     lib.b2g_bdq_obs_rms_set.argtypes = [vp, dp, dp, C.c_double]
     lib.b2g_bdq_obs_rms_get.argtypes = [vp, dp, dp, dp]
     lib.b2g_bdq_upload_bytes.argtypes = [vp, i64p, i64p]
+    lib.b2g_dqn_create.argtypes = [C.POINTER(DqnCfg), C.POINTER(vp)]
+    lib.b2g_dqn_destroy.argtypes = [vp]
+    lib.b2g_dqn_param_count.argtypes = [vp]
+    lib.b2g_dqn_param_info.argtypes = [vp, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]
+    for f in ("b2g_dqn_get_param", "b2g_dqn_set_param", "b2g_dqn_get_grad"):
+        getattr(lib, f).argtypes = [vp, C.c_char_p, fp, C.c_size_t]
+    lib.b2g_dqn_replay_add.argtypes = [vp, fp, fp, fp, fp, fp, C.c_int64]
+    lib.b2g_dqn_replay_size.argtypes = [vp]
+    lib.b2g_dqn_replay_size.restype = C.c_int64
+    lib.b2g_dqn_set_norm_stats.argtypes = [vp, dp, dp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int]
+    lib.b2g_dqn_step.argtypes = [vp, C.c_int, C.c_float, C.POINTER(DqnMetrics)]
+    lib.b2g_dqn_step_explicit.argtypes = [vp, fp, fp, fp, fp, fp, fp, C.c_float, C.c_int, C.POINTER(DqnMetrics), fp]
+    lib.b2g_dqn_set_per_beta.argtypes = [vp, C.c_float]
+    lib.b2g_dqn_get_last_per.argtypes = [vp, C.POINTER(C.c_int32), fp, fp]
+    lib.b2g_dqn_update_target.argtypes = [vp]
+    lib.b2g_dqn_act.argtypes = [vp, fp, C.c_int, C.POINTER(C.c_int32), fp]
     lib.b2g_encoder_create.argtypes = [C.POINTER(EncoderCfg), C.POINTER(vp)]
     lib.b2g_encoder_destroy.argtypes = [vp]
     lib.b2g_encoder_n_layers.argtypes = [vp]

@@ -26,6 +26,7 @@
 #include "../../include/b200grasp.h"
 #include "common.cuh"
 #include "host.cuh"
+#include "per.cuh"
 #include "state.cuh"
 
 using namespace b2g;
@@ -154,80 +155,6 @@ __global__ void bdq_commit_kernel(const float* __restrict__ cur, const float* __
   if (threadIdx.x < D) r_act[slot * D + threadIdx.x] = act[(size_t)i * D + threadIdx.x];
   if (threadIdx.x == 0) { r_rew[slot] = rew[i]; r_done[slot] = done[i]; }
   if (i == 0 && threadIdx.x == 0) counters[5] = new_size;
-}
-
-// ------------------------------------------------------------------------------------------------ prioritised replay
-// Proportional prioritisation ([SB2] common/buffers.py PrioritizedReplayBuffer over common/segment_tree.py; Schaul et al.
-// 2016) with the sum / min segment trees resident in HBM: leaves C..2C-1 (C = capacity rounded up to a power of two),
-// node i = f(2i, 2i+1).  Sums are kept in float64 like the Python floats of the reference.
-struct PerArgs {
-  double* tsum; double* tmin; long long C;
-  float* max_prio;                  // running max of the raw priorities (new transitions enter with it)
-  const long long* counters;        // [4] rng step, [5] replay size
-  unsigned long long seed;
-  int B; float alpha, eps; const float* beta;
-  int* indices; float* weights; float* prio_out;
-  const float* td; int D;
-};
-
-// one CTA, B threads: draws B slots proportionally to priority (find_prefixsum_idx descent) and their IS weights
-__global__ void per_sample_kernel(PerArgs a) {
-  const int b = threadIdx.x;
-  if (b >= a.B) return;
-  const unsigned long long step = (unsigned long long)a.counters[4];
-  const long long size = a.counters[5];
-  const uint4 r = philox4x32_10(make_uint4((unsigned)step, (unsigned)(step >> 32), (unsigned)(b >> 2), 2u), make_uint2((unsigned)a.seed, (unsigned)(a.seed >> 32)));
-  const unsigned v = (b & 3) == 0 ? r.x : (b & 3) == 1 ? r.y : (b & 3) == 2 ? r.z : r.w;
-  const double total = a.tsum[1];
-  double mass = ((double)v + 0.5) * (1.0 / 4294967296.0) * total;
-  long long node = 1;
-  while (node < a.C) {
-    const double left = a.tsum[2 * node];
-    if (left > mass) node = 2 * node;
-    else { mass -= left; node = 2 * node + 1; }
-  }
-  long long idx = node - a.C;
-  if (idx >= size) idx = size - 1;                       // (rounding at the right edge of the occupied range)
-  const double beta = (double)a.beta[0];
-  const double p_min = a.tmin[1] / total;
-  const double max_w = pow(p_min * (double)size, -beta);
-  const double p = a.tsum[a.C + idx] / total;
-  a.indices[b] = (int)idx;
-  a.weights[b] = (float)(pow(p * (double)size, -beta) / max_w);
-}
-
-// one CTA: writes `n` leaves and repairs their ancestors level by level (siblings recomputed redundantly: same values)
-__global__ void per_write_kernel(PerArgs a, const int* __restrict__ slots, long long first_slot, long long cap, int n, int from_td) {
-  const int i = threadIdx.x;
-  long long leaf = 0;
-  if (i < n) {
-    const long long slot = slots ? (long long)slots[i] : (first_slot + i) % cap;
-    float raw;
-    if (from_td) {
-      float s = 0.f;
-      for (int d = 0; d < a.D; ++d) s += fabsf(a.td[i * a.D + d]);
-      raw = s + a.eps;
-      atomicMax(reinterpret_cast<int*>(a.max_prio), __float_as_int(raw));      // positive floats order like their bit patterns
-      if (a.prio_out) a.prio_out[i] = raw;
-    } else raw = a.max_prio[0];
-    const double pr = pow((double)raw, (double)a.alpha);
-    leaf = a.C + slot;
-    a.tsum[leaf] = pr; a.tmin[leaf] = pr;
-  }
-  __syncthreads();
-  for (long long span = a.C; span > 1; span >>= 1) {
-    if (i < n) {
-      leaf >>= 1;
-      a.tsum[leaf] = a.tsum[2 * leaf] + a.tsum[2 * leaf + 1];
-      a.tmin[leaf] = fmin(a.tmin[2 * leaf], a.tmin[2 * leaf + 1]);
-    }
-    __syncthreads();
-  }
-}
-
-__global__ void per_init_kernel(double* tsum, double* tmin, long long n2, float* max_prio) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n2; i += (long long)gridDim.x * blockDim.x) { tsum[i] = 0.0; tmin[i] = INFINITY; }
-  if (blockIdx.x == 0 && threadIdx.x == 0) max_prio[0] = 1.0f;
 }
 
 // hard target copy every `freq` updates, decided on the device so that the step can live in a CUDA graph
@@ -437,7 +364,7 @@ int bdq_issue(b2g_bdq* h, bool sampled, bool apply, const float* weights) {
     pr.tsum = h->t_sum; pr.tmin = h->t_min; pr.C = h->per_C; pr.max_prio = h->max_prio; pr.counters = h->counters; pr.seed = pa.seed;
     pr.B = h->B; pr.alpha = h->cfg.per_alpha; pr.eps = h->cfg.per_eps; pr.beta = h->d_beta; pr.indices = h->indices; pr.weights = h->weights;
     pr.prio_out = h->prio_out; pr.td = h->td; pr.D = h->D;
-    if (sampled) { per_sample_kernel<<<1, ((h->B + 31) / 32) * 32, 0, s>>>(pr); weights = h->weights; }   // overwrites the uniform draw
+    if (sampled) { per_sample_launch(pr, s); weights = h->weights; }   // overwrites the uniform draw
   }
   gather_launch(bgather(h, sampled, true), s);
   CK(cudaMemsetAsync(h->G, 0, (size_t)(h->n_train + MET_COUNT) * sizeof(float), s));
@@ -451,7 +378,7 @@ int bdq_issue(b2g_bdq* h, bool sampled, bool apply, const float* weights) {
   t.dV = h->dV; t.td = h->td; t.metrics = h->metrics;
   bdq_tail_kernel<<<(h->B + 127) / 128, 128, 0, s>>>(t);
   for (auto& g : h->bwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
-  if (h->per && sampled) per_write_kernel<<<1, ((h->B + 31) / 32) * 32, 0, s>>>(pr, h->indices, 0, h->cfg.buffer_capacity, h->B, 1);   // update_priorities(|td| + eps)
+  if (h->per && sampled) per_write_launch(pr, h->indices, 0, h->cfg.buffer_capacity, h->B, 1, s);   // update_priorities(|td| + eps)
   if (h->cfg.nranks > 1) {      // gradients + loss scalars averaged over the ranks (each rank sampled its own replay shard)
     CK(cudaMemcpyAsync(h->G + h->n_train, h->metrics, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
     if (int rc = nccl_allreduce_sum_f32(h->nccl_comm, h->G, (size_t)(h->n_train + MET_COUNT), s)) return rc;
@@ -558,7 +485,7 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
     h->per_C = 1;
     while (h->per_C < cap) h->per_C <<= 1;
     BA(h->t_sum, 2 * h->per_C); BA(h->t_min, 2 * h->per_C);
-    per_init_kernel<<<256, 256, 0, h->stream>>>(h->t_sum, h->t_min, 2 * h->per_C, h->max_prio);
+    per_init_launch(h->t_sum, h->t_min, 2 * h->per_C, h->max_prio, h->stream);
     const float beta0 = 0.4f;
     if (cudaMemcpyAsync(h->d_beta, &beta0, sizeof(float), cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "per init"));
   }
@@ -662,7 +589,7 @@ int b2g_bdq_replay_add(b2g_bdq* h, const float* obs, const float* act_idx, const
       pr.tsum = h->t_sum; pr.tmin = h->t_min; pr.C = h->per_C; pr.max_prio = h->max_prio; pr.alpha = h->cfg.per_alpha; pr.eps = h->cfg.per_eps;
       for (int64_t o = 0; o < chunk; o += 1024) {
         const int nn = (int)std::min<int64_t>(1024, chunk - o);
-        per_write_kernel<<<1, ((nn + 31) / 32) * 32, 0, h->stream>>>(pr, nullptr, h->r_pos + o, cap, nn, 0);
+        per_write_launch(pr, nullptr, h->r_pos + o, cap, nn, 0, h->stream);
       }
     }
     h->r_pos = (h->r_pos + chunk) % cap;
@@ -925,7 +852,7 @@ int b2g_bdq_observe_add(b2g_bdq* h, const float* act_idx, const float* rew, cons
     pr.tsum = h->t_sum; pr.tmin = h->t_min; pr.C = h->per_C; pr.max_prio = h->max_prio; pr.alpha = h->cfg.per_alpha; pr.eps = h->cfg.per_eps;
     for (int o = 0; o < n; o += 1024) {
       const int nn = std::min(1024, n - o);
-      per_write_kernel<<<1, ((nn + 31) / 32) * 32, 0, h->stream>>>(pr, nullptr, h->r_pos + o, cap, nn, 0);
+      per_write_launch(pr, nullptr, h->r_pos + o, cap, nn, 0, h->stream);
     }
   }
   // VecNormalize's step_wait merges the frames the VecEnv returned: a finished env's reset frame, not its terminal observation

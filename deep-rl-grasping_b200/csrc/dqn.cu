@@ -1,0 +1,763 @@
+// libb200grasp: dueling double DQN learner -- the `sb.DQN` branch of sb_helper.py:155-165 (stable-baselines 2.10.1 deepq).
+//
+// Network (deepq/policies.py FeedForwardPolicy, dueling=True, layers=[h0, h1], ReLU): two towers on the observation, each with
+// its own first layer, action_value obs -> h0 -> h1 -> n and state_value obs -> h0 -> h1 -> 1, Q = V + (A - mean_n A).  The step
+// (deepq/build_graph.py build_train, double_q=True, grad_norm_clipping=10) is restated in oracle/dqn_ref.py:
+//   a* = argmax Q_online(s'),  y = r + gamma (1 - done) Q_target(s', a*),  td = Q(s, a) - y,  loss = mean_b w_b huber(td_b),
+//   every gradient tensor clipped on its own to L2 norm 10 (tf.clip_by_norm), then TF1 Adam.
+// All layers run on the fp32 gather-GEMM engine (gg_simt.cu) as grouped launches: three forward groups (each layer of both
+// towers for the three evaluations online(s), online(s'), target(s')), one fused per-sample tail, three backward groups.
+// Output-layer weights are held with their row stride padded to 4 floats (n = 1 for the value) so every operand row is 16-byte
+// aligned; get/set repack to the zip layout.  The hard target copy is the caller's (b2g_dqn_update_target): stable-baselines
+// decides it by the environment-step count, which the device never sees.  The replay gather normalises with the statistics of
+// b2g_dqn_set_norm_stats (raw transitions are stored); the actor (b2g_dqn_act) takes observations as the network sees them, the
+// VecNormalize wrapper's output, as stable-baselines' act and predict do.
+#include <cuda_runtime.h>
+#include <math.h>
+#include <string.h>
+
+#include <algorithm>
+#include <map>
+#include <string>
+#include <vector>
+
+#include "../../include/b200grasp.h"
+#include "common.cuh"
+#include "host.cuh"
+#include "per.cuh"
+#include "state.cuh"
+
+using namespace b2g;
+
+namespace {
+
+struct DTensor {
+  std::string name;
+  int rows, cols, stride;   // zip shape [rows, cols] (biases: rows = 1), device row stride
+  int64_t off;              // float offset inside P (online) -- the target copy sits at off + n_train
+  bool is_weight;
+};
+
+// metric slots (prep_kernel zeroes all MET_COUNT; optim_kernel accumulates the post-clip squared norm at MET_GN_PI)
+constexpr int DMET_LOSS = 0, DMET_MEANQ = 1, DMET_ABSTD = 2, DMET_GN2 = 3, DMET_NCLIP = 4;
+constexpr float kGradClip = 10.0f;    // dqn.py passes grad_norm_clipping=10 to build_train
+constexpr int kClipThreads = 512;
+
+struct DqnTailArgs {
+  int B, n, NAS;               // batch, actions, padded action stride
+  float gamma;
+  const float* V[3];           // [B,4] value outputs of the 3 evaluations (col 0)
+  const float* A[3];           // [B,NAS] advantages of the 3 evaluations
+  const float* act; int act_stride;   // action indices (as floats) inside the obs rows
+  const float* rew; const float* done; const float* weights;
+  float* dA;                   // [B,NAS] gradient wrt the advantages
+  float* dV;                   // [B,4]
+  float* td;                   // [B]
+  float* metrics;
+};
+
+__device__ __forceinline__ float row_mean(const float* a, int n) {
+  float m = 0.f;
+  for (int k = 0; k < n; ++k) m += a[k];
+  return m / (float)n;
+}
+
+// first maximal index of Q_k = v + (a_k - mean) (tf.argmax over the dueling output)
+__device__ __forceinline__ int q_argmax(const float* a, float v, float mean, int n) {
+  int best = 0;
+  float bv = v + (a[0] - mean);
+  for (int k = 1; k < n; ++k) {
+    const float q = v + (a[k] - mean);
+    if (q > bv) { bv = q; best = k; }
+  }
+  return best;
+}
+
+// dueling aggregation, double-Q target, Huber loss with IS weights, the backward seeds dA / dV, td and the loss metrics
+__global__ void dqn_tail_kernel(DqnTailArgs t) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  float loss_b = 0.f, q_b = 0.f, atd_b = 0.f;
+  if (b < t.B) {
+    const float invB = 1.0f / (float)t.B;
+    const size_t ra = (size_t)b * t.NAS, rv = (size_t)b * 4;
+    const float* a1 = t.A[1] + ra;                           // online net picks at s'
+    const int best = q_argmax(a1, t.V[1][rv], row_mean(a1, t.n), t.n);
+    const float* a2 = t.A[2] + ra;                           // target net evaluates
+    const float qt = t.V[2][rv] + (a2[best] - row_mean(a2, t.n));
+    const float y = t.rew[b] + t.gamma * (1.f - t.done[b]) * qt;
+    const float* a0 = t.A[0] + ra;
+    const int ai = (int)(t.act[(size_t)b * t.act_stride] + 0.5f);
+    const float q = t.V[0][rv] + (a0[ai] - row_mean(a0, t.n));
+    const float td = q - y;
+    t.td[b] = td;
+    const float w = t.weights ? t.weights[b] : 1.f;
+    const float ad = fabsf(td);
+    loss_b = w * (ad < 1.f ? 0.5f * td * td : ad - 0.5f) * invB;     // tf_util.huber_loss, delta 1
+    q_b = q * invB;
+    atd_b = ad * invB;
+    const float dq = w * fminf(fmaxf(td, -1.f), 1.f) * invB;
+    float* da = t.dA + ra;
+    for (int k = 0; k < t.NAS; ++k) da[k] = k < t.n ? dq * ((k == ai ? 1.f : 0.f) - 1.f / (float)t.n) : 0.f;
+    float* dvp = t.dV + rv;
+    dvp[0] = dq; dvp[1] = dvp[2] = dvp[3] = 0.f;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    loss_b += __shfl_xor_sync(0xffffffffu, loss_b, o);
+    q_b += __shfl_xor_sync(0xffffffffu, q_b, o);
+    atd_b += __shfl_xor_sync(0xffffffffu, atd_b, o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(t.metrics + DMET_LOSS, loss_b); atomicAdd(t.metrics + DMET_MEANQ, q_b); atomicAdd(t.metrics + DMET_ABSTD, atd_b);
+  }
+}
+
+struct ClipJob { long long off; int count; };
+
+// tf.clip_by_norm per variable: one CTA per online tensor, g <- g * clip / max(||g||_2, clip) in place.  Also the squared norm
+// before clipping (summed over the tensors) and the number of tensors the clip scaled.
+__global__ void __launch_bounds__(kClipThreads) dqn_clip_kernel(float* __restrict__ G, const ClipJob* __restrict__ jobs, float clip,
+                                                                float* __restrict__ metrics) {
+  const ClipJob job = jobs[blockIdx.x];
+  float* g = G + job.off;
+  float s = 0.f;
+  for (int i = threadIdx.x; i < job.count; i += blockDim.x) s += g[i] * g[i];
+  __shared__ float red[kClipThreads / 32];
+  __shared__ float s_den;
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float tot = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += red[w];
+    const float norm = sqrtf(tot);
+    atomicAdd(metrics + DMET_GN2, tot);
+    if (norm > clip) atomicAdd(metrics + DMET_NCLIP, 1.f);
+    s_den = fmaxf(norm, clip);
+  }
+  __syncthreads();
+  const float den = s_den;
+  for (int i = threadIdx.x; i < job.count; i += blockDim.x) g[i] = g[i] * clip / den;
+}
+
+// greedy actions of the online net on `rows` evaluated rows, and optionally their Q rows [rows][n]
+__global__ void dqn_act_kernel(const float* __restrict__ A, const float* __restrict__ V, int rows, int n, int NAS, int* __restrict__ out,
+                               float* __restrict__ q_out) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= rows) return;
+  const float* a = A + (size_t)b * NAS;
+  const float v = V[(size_t)b * 4], mean = row_mean(a, n);
+  out[b] = q_argmax(a, v, mean, n);
+  if (q_out)
+    for (int k = 0; k < n; ++k) q_out[(size_t)b * n + k] = v + (a[k] - mean);
+}
+}  // namespace
+
+struct b2g_dqn {
+  b2g_dqn_cfg cfg{};
+  int B = 0, n = 0, NAS = 0, H0 = 0, H1 = 0, XS = 0, E = 0;
+  std::vector<DTensor> tensors;
+  std::map<std::string, int> tindex;
+  int64_t n_train = 0;
+  float *P = nullptr, *Mo = nullptr, *Vo = nullptr, *G = nullptr, *metrics = nullptr;
+  float eps_value = 1.0f;      // deepq/eps (exploration epsilon variable of the zip)
+  cudaStream_t stream = nullptr;
+  std::vector<void*> allocs;
+  float *r_obs = nullptr, *r_next = nullptr, *r_act = nullptr, *r_rew = nullptr, *r_done = nullptr;
+  int64_t r_size = 0, r_pos = 0;
+  double *d_mean = nullptr, *d_istd = nullptr, *d_normc = nullptr;
+  double* d_normc_act = nullptr;   // the actor's gather: observations arrive as the network sees them (no normalisation)
+  float *X = nullptr, *Xn = nullptr, *Xscratch = nullptr;
+  float *h1[3][2]{}, *h2[3][2]{}, *Aout[3]{}, *Vout[3]{};      // [evaluation][tower 0 = action_value, 1 = state_value]
+  float *dA = nullptr, *dV = nullptr, *dh2[2]{}, *dh1[2]{}, *td = nullptr;
+  float *rew_n = nullptr, *done_n = nullptr, *weights = nullptr, *eps_dummy = nullptr;
+  float *s_obs = nullptr, *s_next = nullptr, *s_act = nullptr, *s_rew = nullptr, *s_done = nullptr;
+  int* indices = nullptr;
+  int* act_idx_out = nullptr;
+  float* q_rows = nullptr;
+  ClipJob* clip_jobs = nullptr;
+  int n_clip = 0;
+  long long* counters = nullptr;
+  double* step_consts = nullptr;
+  float* d_lr = nullptr;
+  float cur_lr = -1.f;
+  std::vector<GemmGroup> fwd, bwd, act;
+  long long n_updates = 0;
+  float* h_met = nullptr;
+  bool per = false;
+  double *t_sum = nullptr, *t_min = nullptr;
+  long long per_C = 0;
+  float *max_prio = nullptr, *d_beta = nullptr, *prio_out = nullptr;
+  cudaGraphExec_t graph_exec = nullptr;
+  bool use_graph = true;
+  bool broken = false;         // a training-state load failed after it began writing: only destroy / load are accepted
+  const DTensor& t(const std::string& nm) const { return tensors[tindex.at(nm)]; }
+  float* p(const std::string& nm) { return P + t(nm).off; }
+  float* g(const std::string& nm) { return G + t(nm).off; }
+  float* pt(const std::string& nm) { return P + n_train + t(nm).off; }
+};
+
+namespace {
+const char* const kTower[2] = {"action_value", "state_value"};
+const std::string kOnline = "deepq/model", kTarget = "deepq/target_q_func/model";
+
+std::string fcname(int i) { return i == 0 ? "fully_connected" : "fully_connected_" + std::to_string(i); }
+std::string lname(int tw, int layer) { return kOnline + "/" + kTower[tw] + "/" + fcname(layer); }
+
+void add_t(b2g_dqn* h, const std::string& name, int rows, int cols, bool w, int stride, int64_t& off) {
+  DTensor t{name, rows, cols, stride, off, w};
+  off += ((int64_t)(w ? rows * stride : stride) + 31) / 32 * 32;
+  h->tindex[name] = (int)h->tensors.size();
+  h->tensors.push_back(t);
+}
+
+int build(b2g_dqn* h) {
+  const int B = h->B, NAS = h->NAS, H0 = h->H0, H1 = h->H1, XS = h->XS, obs = h->cfg.obs_dim;
+  const int *iH0, *iH1, *iNAS, *i4, *iobs, *rXS, *rH0, *rH1, *rNAS, *r4, *kH0, *kH1, *kNAS, *k4;
+#define DT(var, vec) if (int rc = upload_table(h->allocs, h->stream, (vec), &var)) return rc;
+  DT(iH0, iota_tab(H0)) DT(iH1, iota_tab(H1)) DT(iNAS, iota_tab(NAS)) DT(i4, iota_tab(4)) DT(iobs, iota_tab(XS))
+  DT(rXS, iota_tab(B, XS)) DT(rH0, iota_tab(B, H0)) DT(rH1, iota_tab(B, H1)) DT(rNAS, iota_tab(B, NAS)) DT(r4, iota_tab(B, 4))
+  DT(kH0, iota_tab(std::max(obs, H0) + 8, H0)) DT(kH1, iota_tab(std::max(H0, H1) + 8, H1)) DT(kNAS, iota_tab(H1 + 8, NAS))
+  DT(k4, iota_tab(H1 + 8, 4))
+#undef DT
+  auto W = [&](int e, int tw, int layer, const char* wb) {
+    const std::string nm = lname(tw, layer) + wb;
+    return e == 2 ? h->pt(nm) : h->p(nm);
+  };
+  // ---------------- forward: each layer of both towers for the 3 evaluations; the act groups hold evaluation 0 only
+  for (int layer = 0; layer < 3; ++layer) {
+    GemmGroup g, a;
+    g.name = "dqn_fwd" + std::to_string(layer); a.name = "act_" + g.name;
+    for (int e = 0; e < 3; ++e)
+      for (int tw = 0; tw < 2; ++tw) {
+        GemmDesc d;
+        if (layer == 0)
+          d = gemm_desc(e == 0 ? h->X : h->Xn, rXS, iobs, W(e, tw, 0, "/weights"), kH0, iH0, h->h1[e][tw], rH0, iH0, B, H0, obs,
+                        GG_A_RVEC | GG_EPI_BIAS_RELU);
+        else if (layer == 1)
+          d = gemm_desc(h->h1[e][tw], rH0, iH0, W(e, tw, 1, "/weights"), kH1, iH1, h->h2[e][tw], rH1, iH1, B, H1, H0, GG_A_RVEC | GG_EPI_BIAS_RELU);
+        else if (tw == 0)
+          d = gemm_desc(h->h2[e][0], rH1, iH1, W(e, 0, 2, "/weights"), kNAS, iNAS, h->Aout[e], rNAS, iNAS, B, NAS, H1, GG_A_RVEC | GG_EPI_BIAS);
+        else
+          d = gemm_desc(h->h2[e][1], rH1, iH1, W(e, 1, 2, "/weights"), k4, i4, h->Vout[e], r4, i4, B, 4, H1, GG_A_RVEC | GG_EPI_BIAS);
+        d.bias = W(e, tw, layer, "/biases");
+        g.host.push_back(d);
+        if (e == 0) a.host.push_back(d);
+      }
+    h->fwd.push_back(g); h->act.push_back(a);
+  }
+  // ---------------- backward (online evaluation 0), both towers per launch; no gradient into the observation
+  {
+    GemmGroup g; g.name = "dqn_out_bwd";
+    for (int tw = 0; tw < 2; ++tw) {
+      const int N = tw == 0 ? NAS : 4;
+      const int *rN = tw == 0 ? rNAS : r4, *iN = tw == 0 ? iNAS : i4, *kN = tw == 0 ? kNAS : k4;
+      const float* dz = tw == 0 ? h->dA : h->dV;
+      GemmDesc w = gemm_desc(h->h2[0][tw], iH1, rH1, dz, rN, iN, h->g(lname(tw, 2) + "/weights"), kN, iN, H1, N, B, GG_COLSUM);
+      w.colsum = h->g(lname(tw, 2) + "/biases");
+      g.host.push_back(w);
+      GemmDesc dg = gemm_desc(dz, rN, iN, h->p(lname(tw, 2) + "/weights"), iN, kN, h->dh2[tw], rH1, iH1, B, H1, N,
+                              GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
+      dg.mask = h->h2[0][tw]; dg.kM = rH1; dg.kN = iH1;
+      g.host.push_back(dg);
+    }
+    h->bwd.push_back(g);
+  }
+  {
+    GemmGroup g; g.name = "dqn_hidden_bwd";
+    for (int tw = 0; tw < 2; ++tw) {
+      GemmDesc w = gemm_desc(h->h1[0][tw], iH0, rH0, h->dh2[tw], rH1, iH1, h->g(lname(tw, 1) + "/weights"), kH1, iH1, H0, H1, B, GG_COLSUM);
+      w.colsum = h->g(lname(tw, 1) + "/biases");
+      g.host.push_back(w);
+      GemmDesc dg = gemm_desc(h->dh2[tw], rH1, iH1, h->p(lname(tw, 1) + "/weights"), iH1, kH1, h->dh1[tw], rH0, iH0, B, H0, H1,
+                              GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
+      dg.mask = h->h1[0][tw]; dg.kM = rH0; dg.kN = iH0;
+      g.host.push_back(dg);
+    }
+    h->bwd.push_back(g);
+  }
+  {
+    GemmGroup g; g.name = "dqn_in_wgrad";
+    for (int tw = 0; tw < 2; ++tw) {
+      GemmDesc w = gemm_desc(h->X, iobs, rXS, h->dh1[tw], rH0, iH0, h->g(lname(tw, 0) + "/weights"), kH0, iH0, obs, H0, B, GG_COLSUM);
+      w.colsum = h->g(lname(tw, 0) + "/biases");
+      g.host.push_back(w);
+    }
+    h->bwd.push_back(g);
+  }
+  for (auto& g : h->fwd) if (int rc = finalize_tiles(g, h->allocs, h->stream)) return rc;
+  for (auto& g : h->bwd) if (int rc = finalize_tiles(g, h->allocs, h->stream)) return rc;
+  for (auto& g : h->act) if (int rc = finalize_tiles(g, h->allocs, h->stream)) return rc;
+  // the clip jobs: every online tensor over its padded rows (pad columns hold zero gradients)
+  std::vector<ClipJob> jobs;
+  for (const DTensor& t : h->tensors) jobs.push_back(ClipJob{(long long)t.off, t.is_weight ? t.rows * t.stride : t.stride});
+  h->n_clip = (int)jobs.size();
+  if (int rc = dev_alloc(h->allocs, h->stream, &h->clip_jobs, jobs.size(), false)) return rc;
+  CK(cudaMemcpyAsync(h->clip_jobs, jobs.data(), jobs.size() * sizeof(ClipJob), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+GatherArgs dgather(b2g_dqn* h, bool from_replay, bool with_next) {
+  GatherArgs g{};
+  g.obs = from_replay ? h->r_obs : h->s_obs;
+  g.next_obs = with_next ? (from_replay ? h->r_next : h->s_next) : nullptr;
+  g.act = with_next ? (from_replay ? h->r_act : h->s_act) : nullptr;
+  g.rew = from_replay ? h->r_rew : h->s_rew;
+  g.done = from_replay ? h->r_done : h->s_done;
+  g.indices = from_replay ? h->indices : nullptr;
+  g.mean = h->d_mean; g.var = h->d_istd; g.normc = h->d_normc;
+  g.B = h->B; g.H = 0; g.W = h->cfg.obs_dim; g.Cimg = 0; g.scale = 1.f;
+  g.F_pi = h->Xscratch; g.F_v = h->X; g.F_t = h->Xn; g.FS = h->XS; g.feat_col = 0;
+  g.rew_out = h->rew_n; g.done_out = h->done_n; g.n_act = 1;
+  return g;
+}
+
+PerArgs dper(b2g_dqn* h, unsigned long long seed) {
+  PerArgs pr{};
+  pr.tsum = h->t_sum; pr.tmin = h->t_min; pr.C = h->per_C; pr.max_prio = h->max_prio; pr.counters = h->counters; pr.seed = seed;
+  pr.B = h->B; pr.alpha = h->cfg.per_alpha; pr.eps = h->cfg.per_eps; pr.beta = h->d_beta; pr.indices = h->indices; pr.weights = h->weights;
+  pr.prio_out = h->prio_out; pr.td = h->td; pr.D = 1;
+  return pr;
+}
+
+int dqn_issue(b2g_dqn* h, bool sampled, bool apply, const float* weights) {
+  cudaStream_t s = h->stream;
+  PrepArgs pa{};
+  pa.counters = h->counters; pa.step_consts = h->step_consts; pa.lr = h->d_lr; pa.metrics = h->metrics;
+  pa.indices = h->indices; pa.eps = h->eps_dummy; pa.B = h->B; pa.A = 1; pa.replay_size = nullptr;
+  pa.seed = h->cfg.seed; pa.gen = sampled ? 1 : 0; pa.apply = apply ? 1 : 0;
+  prep_launch(pa, s);
+  const PerArgs pr = dper(h, pa.seed);
+  if (h->per && sampled) { per_sample_launch(pr, s); weights = h->weights; }   // overwrites the uniform draw
+  gather_launch(dgather(h, sampled, true), s);
+  CK(cudaMemsetAsync(h->G, 0, (size_t)h->n_train * sizeof(float), s));
+  for (auto& g : h->fwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
+  DqnTailArgs t{};
+  t.B = h->B; t.n = h->n; t.NAS = h->NAS; t.gamma = h->cfg.gamma;
+  for (int e = 0; e < 3; ++e) { t.V[e] = h->Vout[e]; t.A[e] = h->Aout[e]; }
+  t.act = h->X + h->cfg.obs_dim; t.act_stride = h->XS;
+  t.rew = h->rew_n; t.done = h->done_n; t.weights = weights;
+  t.dA = h->dA; t.dV = h->dV; t.td = h->td; t.metrics = h->metrics;
+  dqn_tail_kernel<<<(h->B + 127) / 128, 128, 0, s>>>(t);
+  for (auto& g : h->bwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
+  dqn_clip_kernel<<<h->n_clip, kClipThreads, 0, s>>>(h->G, h->clip_jobs, kGradClip, h->metrics);
+  if (h->per && sampled) per_write_launch(pr, h->indices, 0, h->cfg.buffer_capacity, h->B, 1, s);   // update_priorities(|td| + eps)
+  OptimArgs oa{};
+  oa.P = h->P; oa.Mo = h->Mo; oa.Vo = h->Vo; oa.G = h->G; oa.T = h->P + h->n_train;
+  oa.n_pi = (int)h->n_train; oa.n_values = 0; oa.n_ent = 0; oa.n_target = 0;
+  oa.step_consts = h->step_consts; oa.tau = 0.f; oa.grad_scale = 1.0f; oa.metrics = h->metrics; oa.apply = apply ? 1 : 0;
+  optim_launch(oa, s);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+int dfetch(b2g_dqn* h, b2g_dqn_metrics* out) {
+  CK(cudaMemcpyAsync(h->h_met, h->metrics, MET_COUNT * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  if (out) {
+    out->loss = h->h_met[DMET_LOSS]; out->mean_q = h->h_met[DMET_MEANQ]; out->mean_abs_td = h->h_met[DMET_ABSTD];
+    out->grad_norm = sqrtf(h->h_met[DMET_GN2]); out->n_clipped = (int32_t)lrintf(h->h_met[DMET_NCLIP]);
+    out->n_updates = h->n_updates;
+  }
+  return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int b2g_dqn_destroy(b2g_dqn* h) {
+  if (!h) return 0;
+  cudaSetDevice(h->cfg.device);
+  if (h->stream) cudaStreamSynchronize(h->stream);
+  if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
+  for (void* q : h->allocs) cudaFree(q);
+  if (h->h_met) cudaFreeHost(h->h_met);
+  if (h->stream) cudaStreamDestroy(h->stream);
+  delete h;
+  return 0;
+}
+
+int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out) {
+  if (!cfg || !out) return b2g_fail(B2G_EINVAL, "cfg/out is NULL");
+  *out = nullptr;
+  if (cfg->n_actions < 2 || cfg->n_actions > 64) return b2g_fail(B2G_EINVAL, "n_actions must be in [2, 64]");
+  if (cfg->hidden0 % 4 || cfg->hidden1 % 4 || cfg->hidden0 < 4 || cfg->hidden1 < 4 || cfg->hidden0 > 512 || cfg->hidden1 > 512)
+    return b2g_fail(B2G_EINVAL, "hidden widths must be multiples of 4 in [4, 512]");
+  if (cfg->obs_dim < 1 || cfg->batch < 1 || cfg->buffer_capacity < 1) return b2g_fail(B2G_EINVAL, "obs_dim, batch, buffer_capacity must be positive");
+  if (cfg->prioritized_replay && cfg->batch > 1024) return b2g_fail(B2G_EINVAL, "prioritised replay supports batch <= 1024");
+  if (cfg->batch > 65535) return b2g_fail(B2G_EINVAL, "batch must be <= 65535 (one gather CTA row per sample: grid.y)");
+  if (int rc = check_device(cfg->device)) return rc;
+  b2g_dqn* h = new b2g_dqn();
+  h->cfg = *cfg;
+  h->per = cfg->prioritized_replay != 0;
+  const char* ng = getenv("B2G_NO_GRAPH");
+  h->use_graph = !(ng && ng[0] == '1');
+  h->B = cfg->batch; h->n = cfg->n_actions; h->NAS = (cfg->n_actions + 3) / 4 * 4;
+  h->H0 = cfg->hidden0; h->H1 = cfg->hidden1; h->E = cfg->obs_dim;
+  h->XS = (cfg->obs_dim + 1 + 7) / 8 * 8;
+  auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_dqn_destroy(h); g_b2g_err = keep; return rc; };
+  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream"));
+  // parameter inventory in zip order (oracle/dqn_ref.py param_specs)
+  int64_t off = 0;
+  for (int tw = 0; tw < 2; ++tw) {
+    const int no = tw == 0 ? h->n : 1, so = tw == 0 ? h->NAS : 4;
+    add_t(h, lname(tw, 0) + "/weights", h->E, h->H0, true, h->H0, off);
+    add_t(h, lname(tw, 0) + "/biases", 1, h->H0, false, h->H0, off);
+    add_t(h, lname(tw, 1) + "/weights", h->H0, h->H1, true, h->H1, off);
+    add_t(h, lname(tw, 1) + "/biases", 1, h->H1, false, h->H1, off);
+    add_t(h, lname(tw, 2) + "/weights", h->H1, no, true, so, off);
+    add_t(h, lname(tw, 2) + "/biases", 1, no, false, so, off);
+  }
+  h->n_train = off;
+  int rc = 0;
+  const int B = h->B;
+#define DA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
+  DA(h->P, 2 * h->n_train); DA(h->Mo, h->n_train); DA(h->Vo, h->n_train); DA(h->G, h->n_train); DA(h->metrics, MET_COUNT);
+  DA(h->counters, 8); DA(h->step_consts, 4); DA(h->d_lr, 1);
+  const int64_t cap = cfg->buffer_capacity;
+  DA(h->r_obs, cap * h->E); DA(h->r_next, cap * h->E); DA(h->r_act, cap); DA(h->r_rew, cap); DA(h->r_done, cap);
+  DA(h->d_mean, h->E); DA(h->d_istd, h->E); DA(h->d_normc, 8); DA(h->d_normc_act, 8);
+  DA(h->X, (size_t)B * h->XS); DA(h->Xn, (size_t)B * h->XS); DA(h->Xscratch, (size_t)B * h->XS);
+  for (int e = 0; e < 3; ++e) {
+    for (int tw = 0; tw < 2; ++tw) { DA(h->h1[e][tw], B * h->H0); DA(h->h2[e][tw], B * h->H1); }
+    DA(h->Aout[e], B * h->NAS); DA(h->Vout[e], B * 4);
+  }
+  DA(h->dA, B * h->NAS); DA(h->dV, B * 4);
+  for (int tw = 0; tw < 2; ++tw) { DA(h->dh2[tw], B * h->H1); DA(h->dh1[tw], B * h->H0); }
+  DA(h->td, B);
+  DA(h->rew_n, B); DA(h->done_n, B); DA(h->weights, B); DA(h->eps_dummy, B + 8); DA(h->indices, B + 4); DA(h->act_idx_out, B);
+  DA(h->q_rows, B * h->n);
+  DA(h->s_obs, (size_t)B * h->E); DA(h->s_next, (size_t)B * h->E); DA(h->s_act, B); DA(h->s_rew, B); DA(h->s_done, B);
+  DA(h->d_beta, 1); DA(h->max_prio, 1); DA(h->prio_out, B);
+  if (h->per) {
+    h->per_C = 1;
+    while (h->per_C < cap) h->per_C <<= 1;
+    DA(h->t_sum, 2 * h->per_C); DA(h->t_min, 2 * h->per_C);
+    per_init_launch(h->t_sum, h->t_min, 2 * h->per_C, h->max_prio, h->stream);
+    const float beta0 = 0.4f;
+    if (cudaMemcpyAsync(h->d_beta, &beta0, sizeof(float), cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "per init"));
+  }
+#undef DA
+  if (cudaMallocHost((void**)&h->h_met, MET_COUNT * sizeof(float)) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "cudaMallocHost"));
+  {
+    std::vector<double> ones(h->E, 1.0);
+    const double nc[8] = {1.0, 10.0, 10.0, 0.0, 0.0, 0, 0, 0};
+    if (cudaMemcpyAsync(h->d_istd, ones.data(), h->E * sizeof(double), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
+        cudaMemcpyAsync(h->d_normc, nc, sizeof(nc), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
+        cudaMemcpyAsync(h->d_normc_act, nc, sizeof(nc), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
+        cudaStreamSynchronize(h->stream) != cudaSuccess)
+      return bail(b2g_fail(B2G_ECUDA, "init copies"));
+  }
+  if ((rc = build(h))) return bail(rc);
+  if (cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "create sync"));
+  *out = h;
+  return 0;
+}
+
+int b2g_dqn_param_count(const b2g_dqn* h) { B2G_USABLE(h); return h ? 1 + 2 * (int)h->tensors.size() : 0; }
+
+// index 0 = deepq/eps; 1..T = online tensors; T+1..2T = target tensors (names and order as in the zips)
+int b2g_dqn_param_info(const b2g_dqn* h, int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim) {
+  B2G_USABLE(h);
+  if (!h || idx < 0 || idx >= b2g_dqn_param_count(h) || !name) return b2g_fail(B2G_EINVAL, "bad tensor index");
+  std::string nm = "deepq/eps";
+  int64_t r = 1, c = 1;
+  int nd = 0;
+  if (idx > 0) {
+    const int T = (int)h->tensors.size();
+    const DTensor& t = h->tensors[(idx - 1) % T];
+    nm = (idx - 1) < T ? t.name : kTarget + t.name.substr(kOnline.size());
+    r = t.rows; c = t.cols; nd = t.is_weight ? 2 : 1;
+  }
+  snprintf(name, name_cap, "%s", nm.c_str());
+  if (rows) *rows = r;
+  if (cols) *cols = c;
+  if (ndim) *ndim = nd;
+  return 0;
+}
+
+static int dqn_copy(b2g_dqn* h, const char* name, float* arena_online, float* host, size_t numel, bool to_host, bool allow_target) {
+  if (!h || !name || !host) return b2g_fail(B2G_EINVAL, "NULL argument");
+  std::string nm(name);
+  if (nm.size() > 2 && nm.compare(nm.size() - 2, 2, ":0") == 0) nm.resize(nm.size() - 2);
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  if (nm == "deepq/eps") {
+    if (numel != 1) return b2g_fail(B2G_EINVAL, "deepq/eps is a scalar");
+    if (to_host) host[0] = h->eps_value; else h->eps_value = host[0];
+    return 0;
+  }
+  bool target = false;
+  if (nm.compare(0, kTarget.size(), kTarget) == 0) { target = true; nm = kOnline + nm.substr(kTarget.size()); }
+  if (target && !allow_target) return b2g_fail(B2G_EINVAL, "not a trainable variable");
+  auto it = h->tindex.find(nm);
+  if (it == h->tindex.end()) return b2g_fail(B2G_EINVAL, std::string("unknown variable: ") + name);
+  const DTensor& t = h->tensors[it->second];
+  const size_t rows = t.is_weight ? t.rows : 1, cols = t.cols;
+  if (numel != rows * cols) return b2g_fail(B2G_EINVAL, std::string("size mismatch for ") + name);
+  float* dev = arena_online + t.off + (target ? h->n_train : 0);
+  // repack between the zip layout [rows, cols] and the device row stride
+  if (to_host) CK(cudaMemcpy2D(host, cols * sizeof(float), dev, t.stride * sizeof(float), cols * sizeof(float), rows, cudaMemcpyDeviceToHost));
+  else CK(cudaMemcpy2D(dev, t.stride * sizeof(float), host, cols * sizeof(float), cols * sizeof(float), rows, cudaMemcpyHostToDevice));
+  return 0;
+}
+int b2g_dqn_get_param(b2g_dqn* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return dqn_copy(h, name, h ? h->P : nullptr, dst, numel, true, true); }
+int b2g_dqn_set_param(b2g_dqn* h, const char* name, const float* src, size_t numel) {
+  B2G_USABLE(h);
+  return dqn_copy(h, name, h ? h->P : nullptr, const_cast<float*>(src), numel, false, true);
+}
+int b2g_dqn_get_grad(b2g_dqn* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return dqn_copy(h, name, h ? h->G : nullptr, dst, numel, true, false); }
+
+// Every action must be an integer in [0, n_actions): the tail kernel indexes the Q row with it.  The values are read on the host
+// (a device array is copied down first), before anything is stored or launched.
+static int dqn_check_actions(const b2g_dqn* h, const float* act, int64_t n) {
+  cudaPointerAttributes pa{};
+  std::vector<float> tmp;
+  const float* a = act;
+  if (cudaPointerGetAttributes(&pa, act) == cudaSuccess && (pa.type == cudaMemoryTypeDevice)) {
+    tmp.resize(n);
+    CK(cudaMemcpy(tmp.data(), act, n * sizeof(float), cudaMemcpyDeviceToHost));
+    a = tmp.data();
+  }
+  cudaGetLastError();      // a failed attribute query (the pointer is then host memory) leaves no error behind
+  for (int64_t i = 0; i < n; ++i)
+    if (!(a[i] >= 0.f && a[i] < (float)h->n && a[i] == floorf(a[i])))
+      return b2g_fail(B2G_EINVAL, "action " + std::to_string(i) + " = " + std::to_string(a[i]) + " is not an integer in [0, " +
+                                      std::to_string(h->n) + ")");
+  return 0;
+}
+
+int b2g_dqn_replay_add(b2g_dqn* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done, int64_t n) {
+  B2G_USABLE(h);
+  if (!h || !obs || !act || !rew || !next_obs || !done || n < 0) return b2g_fail(B2G_EINVAL, "NULL argument");
+  CK(cudaSetDevice(h->cfg.device));
+  if (int rc = dqn_check_actions(h, act, n)) return rc;
+  const int64_t cap = h->cfg.buffer_capacity;
+  int64_t done_n = 0;
+  while (done_n < n) {
+    const int64_t chunk = std::min(n - done_n, cap - h->r_pos);
+    const size_t E = h->E;
+    CK(cudaMemcpyAsync(h->r_obs + h->r_pos * E, obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
+    CK(cudaMemcpyAsync(h->r_next + h->r_pos * E, next_obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
+    CK(cudaMemcpyAsync(h->r_act + h->r_pos, act + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
+    CK(cudaMemcpyAsync(h->r_rew + h->r_pos, rew + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
+    CK(cudaMemcpyAsync(h->r_done + h->r_pos, done + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
+    if (h->per) {        // new transitions enter with the running maximum priority ([SB2] PrioritizedReplayBuffer.add)
+      const PerArgs pr = dper(h, h->cfg.seed);
+      for (int64_t o = 0; o < chunk; o += 1024)
+        per_write_launch(pr, nullptr, h->r_pos + o, cap, (int)std::min<int64_t>(1024, chunk - o), 0, h->stream);
+    }
+    h->r_pos = (h->r_pos + chunk) % cap;
+    h->r_size = std::min(cap, h->r_size + chunk);
+    done_n += chunk;
+  }
+  const long long sz = h->r_size;
+  CK(cudaMemcpyAsync(h->counters + 5, &sz, sizeof(long long), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+int64_t b2g_dqn_replay_size(const b2g_dqn* h) { B2G_USABLE(h); return h ? h->r_size : 0; }
+
+int b2g_dqn_set_norm_stats(b2g_dqn* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs, double clip_rew, double eps,
+                           int norm_obs, int norm_reward) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  if (norm_obs && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  if (norm_obs) {
+    std::vector<double> istd(h->E);
+    for (int i = 0; i < h->E; ++i) istd[i] = 1.0 / sqrt(obs_var[i] + eps);
+    CK(cudaMemcpy(h->d_mean, obs_mean, h->E * sizeof(double), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->d_istd, istd.data(), h->E * sizeof(double), cudaMemcpyHostToDevice));
+  }
+  const double nc[8] = {1.0 / sqrt(ret_var + eps), clip_obs, clip_rew, (double)norm_obs, (double)norm_reward, 0, 0, 0};
+  CK(cudaMemcpy(h->d_normc, nc, sizeof(nc), cudaMemcpyHostToDevice));
+  return 0;
+}
+
+int b2g_dqn_step(b2g_dqn* h, int n_steps, float lr, b2g_dqn_metrics* out) {
+  B2G_USABLE(h);
+  if (!h || n_steps < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  if (h->r_size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
+  CK(cudaSetDevice(h->cfg.device));
+  if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
+  if (h->use_graph && !h->graph_exec)       // the whole step (~14 launches of tiny layers) replays as one graph
+    if (int rc = capture_graph(h->stream, [&] { return dqn_issue(h, true, true, nullptr); }, &h->graph_exec)) return rc;
+  for (int i = 0; i < n_steps; ++i) {
+    if (h->graph_exec) CK(cudaGraphLaunch(h->graph_exec, h->stream));
+    else if (int rc = dqn_issue(h, true, true, nullptr)) return rc;
+    ++h->n_updates;
+  }
+  return dfetch(h, out);
+}
+
+int b2g_dqn_set_per_beta(b2g_dqn* h, float beta) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  CK(cudaMemcpy(h->d_beta, &beta, sizeof(float), cudaMemcpyHostToDevice));
+  return 0;
+}
+
+int b2g_dqn_get_last_per(b2g_dqn* h, int32_t* slots, float* weights, float* priorities) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  if (slots) CK(cudaMemcpy(slots, h->indices, h->B * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  if (weights) CK(cudaMemcpy(weights, h->weights, h->B * sizeof(float), cudaMemcpyDeviceToHost));
+  if (priorities) CK(cudaMemcpy(priorities, h->prio_out, h->B * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int b2g_dqn_step_explicit(b2g_dqn* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done,
+                          const float* weights, float lr, int apply_update, b2g_dqn_metrics* out, float* td_out) {
+  B2G_USABLE(h);
+  if (!h || !obs || !act || !rew || !next_obs || !done) return b2g_fail(B2G_EINVAL, "NULL argument");
+  CK(cudaSetDevice(h->cfg.device));
+  if (int rc = dqn_check_actions(h, act, h->B)) return rc;
+  if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
+  const size_t B = h->B, E = h->E;
+  CK(cudaMemcpyAsync(h->s_obs, obs, B * E * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->s_next, next_obs, B * E * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->s_act, act, B * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->s_rew, rew, B * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->s_done, done, B * sizeof(float), cudaMemcpyDefault, h->stream));
+  if (weights) CK(cudaMemcpyAsync(h->weights, weights, B * sizeof(float), cudaMemcpyDefault, h->stream));
+  if (int rc = dqn_issue(h, false, apply_update != 0, weights ? h->weights : nullptr)) return rc;
+  if (apply_update) ++h->n_updates;
+  if (td_out) CK(cudaMemcpyAsync(td_out, h->td, B * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  return dfetch(h, out);
+}
+
+int b2g_dqn_update_target(b2g_dqn* h) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaMemcpyAsync(h->P + h->n_train, h->P, (size_t)h->n_train * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+int b2g_dqn_act(b2g_dqn* h, const float* obs, int n, int32_t* act_out, float* q_out) {
+  B2G_USABLE(h);
+  if (!h || !obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  CK(cudaSetDevice(h->cfg.device));
+  const size_t E = h->E;
+  for (int done_n = 0; done_n < n; done_n += h->B) {
+    const int chunk = std::min(h->B, n - done_n);
+    CK(cudaMemcpyAsync(h->s_obs, obs + (size_t)done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
+    GatherArgs g = dgather(h, false, false);
+    g.normc = h->d_normc_act;
+    gather_launch(g, h->stream);
+    for (auto& gr : h->act) gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
+    dqn_act_kernel<<<(chunk + 127) / 128, 128, 0, h->stream>>>(h->Aout[0], h->Vout[0], chunk, h->n, h->NAS, h->act_idx_out,
+                                                               q_out ? h->q_rows : nullptr);
+    CK(cudaMemcpyAsync(act_out + done_n, h->act_idx_out, chunk * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+    if (q_out)
+      CK(cudaMemcpyAsync(q_out + (size_t)done_n * h->n, h->q_rows, (size_t)chunk * h->n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+  }
+  CK(cudaGetLastError());
+  return 0;
+}
+
+}  // extern "C"
+
+// ================================================================================================
+// Training state (b2g_dqn_state_save / _load; container format in state.cuh)
+// ================================================================================================
+namespace {
+
+std::vector<FpField> dqn_fingerprint(const b2g_dqn* h) {
+  const b2g_dqn_cfg& c = h->cfg;
+  return {fp_int("obs_dim", c.obs_dim), fp_int("n_actions", c.n_actions), fp_int("hidden0", c.hidden0), fp_int("hidden1", c.hidden1),
+          fp_int("batch", c.batch), fp_int("buffer_capacity", c.buffer_capacity), fp_real("gamma", c.gamma), fp_int("seed", (int64_t)c.seed),
+          fp_int("prioritized_replay", c.prioritized_replay), fp_real("per_alpha", c.per_alpha), fp_real("per_eps", c.per_eps)};
+}
+
+const uint32_t kDqnTags[] = {state_tag("HOST"), state_tag("CNTR"), state_tag("PARM"), state_tag("ADMM"), state_tag("ADMV"),
+                             state_tag("ROBS"), state_tag("RNXT"), state_tag("RACT"), state_tag("RREW"), state_tag("RDON"),
+                             state_tag("PERT"), state_tag("PERS")};
+
+StatePiece ddev(void* p, size_t bytes) { StatePiece s; s.dev = p; s.bytes = bytes; return s; }
+
+// sections 2.. (parameters .. prioritised-replay scalars) of a handle holding `live` replay rows
+std::vector<StateSection> dqn_device_sections(b2g_dqn* h, int64_t live) {
+  const size_t cap = (size_t)h->cfg.buffer_capacity, E = h->E;
+  std::vector<StateSection> s(10);
+  s[0].pieces = {ddev(h->P, 2 * h->n_train * sizeof(float))};
+  s[1].pieces = {ddev(h->Mo, h->n_train * sizeof(float))};
+  s[2].pieces = {ddev(h->Vo, h->n_train * sizeof(float))};
+  s[3].pieces = {ddev(h->r_obs, live * E * sizeof(float))};       // rows [0, size) are the live ones
+  s[4].pieces = {ddev(h->r_next, live * E * sizeof(float))};
+  s[5].pieces = {ddev(h->r_act, cap * sizeof(float))};
+  s[6].pieces = {ddev(h->r_rew, cap * sizeof(float))};
+  s[7].pieces = {ddev(h->r_done, cap * sizeof(float))};
+  if (h->per) s[8].pieces = {ddev(h->t_sum, 2 * h->per_C * sizeof(double)), ddev(h->t_min, 2 * h->per_C * sizeof(double))};
+  s[9].pieces = {ddev(h->max_prio, sizeof(float)), ddev(h->d_beta, sizeof(float))};
+  for (int i = 0; i < 10; ++i) s[i].tag = kDqnTags[i + 2];
+  return s;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b2g_dqn_state_save(b2g_dqn* h, const char* path) {
+  if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
+  B2G_USABLE(h);
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  long long cnt[8];
+  CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
+  uint32_t eps_bits;
+  memcpy(&eps_bits, &h->eps_value, sizeof eps_bits);
+  int64_t hv[4] = {h->r_size, h->r_pos, h->n_updates, (int64_t)eps_bits};
+  std::vector<StateSection> secs(2);
+  secs[0].tag = kDqnTags[0]; secs[0].pieces = {StatePiece{hv, nullptr, sizeof hv}};
+  secs[1].tag = kDqnTags[1]; secs[1].pieces = {StatePiece{cnt, nullptr, sizeof cnt}};
+  for (auto& s : dqn_device_sections(h, h->r_size)) secs.push_back(std::move(s));
+  return state_write(path, STATE_KIND_DQN, dqn_fingerprint(h), secs);
+}
+
+int b2g_dqn_state_load(b2g_dqn* h, const char* path) {
+  if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
+  CK(cudaSetDevice(h->cfg.device));
+  // ---- everything is checked before the handle changes
+  StateReader rd;
+  if (int rc = rd.open(path, STATE_KIND_DQN, dqn_fingerprint(h))) return rc;
+  const int n_sec = (int)(sizeof kDqnTags / sizeof kDqnTags[0]);
+  if (rd.n_sections() != n_sec) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a DQN learner");
+  for (int i = 0; i < n_sec; ++i)
+    if (rd.tag(i) != kDqnTags[i]) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a DQN learner");
+  int64_t hv[4];
+  long long cnt[8];
+  if (rd.bytes(0) != sizeof hv || rd.bytes(1) != sizeof cnt)
+    return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  if (int rc = rd.read_host(0, hv, sizeof hv)) return rc;
+  const int64_t cap = h->cfg.buffer_capacity;
+  if (hv[0] < 0 || hv[0] > cap || hv[1] < 0 || hv[1] >= cap || (hv[0] < cap && hv[1] != hv[0]) || hv[2] < 0)
+    return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
+  std::vector<StateSection> dev = dqn_device_sections(h, hv[0]);
+  for (int i = 0; i < (int)dev.size(); ++i)
+    if (rd.bytes(i + 2) != dev[i].bytes())
+      return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
+  // ---- from here on a failure leaves the handle unusable until a load succeeds
+  CK(cudaStreamSynchronize(h->stream));
+  h->broken = true;
+  for (int i = 0; i < (int)dev.size(); ++i)
+    if (int rc = rd.read_pieces(i + 2, dev[i].pieces)) return rc;
+  CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
+  h->r_size = hv[0]; h->r_pos = hv[1]; h->n_updates = hv[2];
+  const uint32_t eps_bits = (uint32_t)hv[3];
+  memcpy(&h->eps_value, &eps_bits, sizeof eps_bits);
+  // the captured step graph stays valid: it holds device pointers and configuration; size and Philox step are device counters
+  h->broken = false;
+  return 0;
+}
+
+}  // extern "C"

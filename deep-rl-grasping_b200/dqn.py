@@ -1,0 +1,452 @@
+"""``DQN`` -- the dueling double DQN behind the ``sb.DQN`` call sites of the reference
+(/root/reference/manipulation_main/training/sb_helper.py:155-165,183-199, train_stable_baselines.py:45-48,101-102), i.e.
+stable-baselines 2.10.1 ``deepq`` with its defaults (dueling MLP policy [64, 64], double Q, Huber loss, per-variable gradient
+clipping at 10, prioritised replay).  The learner runs on the GPU (csrc/dqn.cu); the algorithm is restated in
+oracle/dqn_ref.py, which also lists what trained_models/DQN_4pads/DQN_simple_4pads.zip pins.  Import it as
+``b200grasp.deepq.DQN`` (the stable-baselines path ``stable_baselines.deepq.DQN``).
+"""
+from __future__ import annotations
+
+import ctypes as C
+import os
+from collections import OrderedDict
+from typing import Optional
+
+import numpy as np
+
+from . import _lib, sb_io, training_state
+from .callbacks import as_callback
+from .learner import _f32, _fp
+from .vec_env import DummyVecEnv
+
+_ONLINE, _TARGET = "deepq/model/", "deepq/target_q_func/model/"
+
+
+class DQNLearner:
+    """numpy-facing wrapper of one ``b2g_dqn`` handle (maps 1:1 onto the C ABI)."""
+
+    def __init__(self, obs_dim=100, n_actions=12, layers=(64, 64), batch_size=32, buffer_size=50000, gamma=0.99, seed=0, device=0,
+                 prioritized_replay=False, prioritized_replay_alpha=0.6, prioritized_replay_eps=1e-6):
+        self.lib = _lib.load()
+        if len(layers) != 2:
+            raise NotImplementedError(f"layers={list(layers)}: the DQN learner builds two hidden layers")
+        cfg = _lib.DqnCfg(obs_dim, n_actions, int(layers[0]), int(layers[1]), batch_size, buffer_size, gamma, seed, device,
+                          int(bool(prioritized_replay)), float(prioritized_replay_alpha), float(prioritized_replay_eps))
+        self.prioritized_replay = bool(prioritized_replay)
+        self.h = C.c_void_p()
+        _lib.check(self.lib.b2g_dqn_create(C.byref(cfg), C.byref(self.h)))
+        self.obs_dim, self.n_actions, self.batch_size = obs_dim, n_actions, batch_size
+        self._info = OrderedDict()
+        buf = C.create_string_buffer(256)
+        rows, cols, nd = C.c_int64(), C.c_int64(), C.c_int32()
+        for i in range(self.lib.b2g_dqn_param_count(self.h)):
+            _lib.check(self.lib.b2g_dqn_param_info(self.h, i, buf, 256, C.byref(rows), C.byref(cols), C.byref(nd)))
+            shape = () if nd.value == 0 else ((rows.value, cols.value) if nd.value == 2 else (cols.value,))
+            self._info[buf.value.decode()] = shape
+
+    def close(self):
+        if getattr(self, "h", None) is not None and self.h:
+            self.lib.b2g_dqn_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @property
+    def param_shapes(self):
+        return self._info
+
+    def get_parameters(self):
+        out = OrderedDict()
+        for n, shp in self._info.items():
+            a = np.empty(shp, np.float32)
+            _lib.check(self.lib.b2g_dqn_get_param(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
+            out[n] = a
+        return out
+
+    def load_parameters(self, params, exact_match=True):
+        seen = set()
+        for n, a in params.items():
+            key = n[:-2] if n.endswith(":0") else n
+            if key not in self._info:
+                if exact_match:
+                    raise ValueError(f"unknown variable {n}")
+                continue
+            a = _f32(a)
+            if tuple(a.shape) != self._info[key]:
+                raise ValueError(f"shape mismatch for {n}: {a.shape} vs {self._info[key]}")
+            _lib.check(self.lib.b2g_dqn_set_param(self.h, key.encode(), _fp(a.reshape(-1)), a.size))
+            seen.add(key)
+        if exact_match and seen != set(self._info):
+            raise ValueError(f"missing variables: {sorted(set(self._info) - seen)}")
+
+    def get_gradients(self):
+        """The last step's gradients after the per-tensor clip (online tensors)."""
+        out = OrderedDict()
+        for n, shp in self._info.items():
+            if not n.startswith(_ONLINE):
+                continue
+            a = np.empty(shp, np.float32)
+            _lib.check(self.lib.b2g_dqn_get_grad(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
+            out[n] = a
+        return out
+
+    def set_eps(self, eps: float):
+        """deepq/eps: the exploration epsilon the last action was taken with."""
+        a = np.full(1, eps, np.float32)
+        _lib.check(self.lib.b2g_dqn_set_param(self.h, b"deepq/eps", _fp(a), 1))
+
+    def replay_add(self, obs, act, rew, next_obs, done):
+        obs, next_obs = _f32(obs).reshape(-1, self.obs_dim), _f32(next_obs).reshape(-1, self.obs_dim)
+        act, rew, done = _f32(np.reshape(act, -1)), _f32(np.reshape(rew, -1)), _f32(np.reshape(done, -1))
+        n = rew.shape[0]
+        assert obs.shape[0] == n and next_obs.shape[0] == n and act.size == n and done.size == n
+        _lib.check(self.lib.b2g_dqn_replay_add(self.h, _fp(obs), _fp(act), _fp(rew), _fp(next_obs), _fp(done), n))
+
+    def replay_size(self):
+        return int(self.lib.b2g_dqn_replay_size(self.h))
+
+    def set_norm_stats(self, obs_mean=None, obs_var=None, ret_var=1.0, clip_obs=10.0, clip_reward=10.0, epsilon=1e-8, norm_obs=True,
+                       norm_reward=True):
+        """VecNormalize's statistics for the gather of the gradient steps (the replay holds raw transitions); act() takes
+        observations already normalised."""
+        dp = C.POINTER(C.c_double)
+        mp = vp = None
+        if norm_obs:
+            m = np.ascontiguousarray(obs_mean, np.float64).reshape(-1)
+            v = np.ascontiguousarray(obs_var, np.float64).reshape(-1)
+            assert m.size == self.obs_dim and v.size == self.obs_dim
+            mp, vp = m.ctypes.data_as(dp), v.ctypes.data_as(dp)
+        _lib.check(self.lib.b2g_dqn_set_norm_stats(self.h, mp, vp, float(ret_var), float(clip_obs), float(clip_reward), float(epsilon),
+                                                    int(bool(norm_obs)), int(bool(norm_reward))))
+
+    def step(self, n_steps=1, lr=5e-4):
+        m = _lib.DqnMetrics()
+        _lib.check(self.lib.b2g_dqn_step(self.h, n_steps, lr, C.byref(m)))
+        return m.as_dict()
+
+    def set_per_beta(self, beta: float):
+        _lib.check(self.lib.b2g_dqn_set_per_beta(self.h, float(beta)))
+
+    def last_per(self):
+        """Slots, importance weights and new priorities (|td| + eps) of the last sampled step (weights and priorities with
+        prioritised replay only)."""
+        B = self.batch_size
+        idx, w, p = np.empty(B, np.int32), np.empty(B, np.float32), np.empty(B, np.float32)
+        _lib.check(self.lib.b2g_dqn_get_last_per(self.h, idx.ctypes.data_as(C.POINTER(C.c_int32)), _fp(w), _fp(p)))
+        return idx, w, p
+
+    def step_explicit(self, obs, act, rew, next_obs, done, weights=None, lr=5e-4, apply_update=True):
+        B = self.batch_size
+        td = np.empty(B, np.float32)
+        w = _fp(_f32(weights)) if weights is not None else None
+        m = _lib.DqnMetrics()
+        _lib.check(self.lib.b2g_dqn_step_explicit(self.h, _fp(_f32(obs)), _fp(_f32(np.reshape(act, -1))), _fp(_f32(np.reshape(rew, -1))),
+                                                   _fp(_f32(next_obs)), _fp(_f32(np.reshape(done, -1))), w, lr, int(apply_update),
+                                                   C.byref(m), _fp(td)))
+        out = m.as_dict()
+        out["td"] = td
+        return out
+
+    def update_target(self):
+        _lib.check(self.lib.b2g_dqn_update_target(self.h))
+
+    def act(self, obs, with_q=False):
+        """Greedy actions [n] of the online network on observations as the network sees them (a VecNormalize wrapper's
+        output: nothing is normalised here), and with ``with_q`` the Q rows [n, n_actions]."""
+        obs = _f32(obs).reshape(-1, self.obs_dim)
+        n = obs.shape[0]
+        out = np.empty(n, np.int32)
+        q = np.empty((n, self.n_actions), np.float32) if with_q else None
+        _lib.check(self.lib.b2g_dqn_act(self.h, _fp(obs), n, out.ctypes.data_as(C.POINTER(C.c_int32)), None if q is None else _fp(q)))
+        return (out, q) if with_q else out
+
+    def save_state(self, path: str):
+        """Parameters, Adam moments, counters, the live replay rows and the prioritised-replay trees -> ``path``."""
+        _lib.check(self.lib.b2g_dqn_state_save(self.h, os.fsencode(path)))
+
+    def load_state(self, path: str):
+        """Restores a ``save_state`` file into this learner, which must have the same configuration."""
+        _lib.check(self.lib.b2g_dqn_state_load(self.h, os.fsencode(path)))
+
+
+def _linear(t, span, p0, p1):
+    """stable-baselines' LinearSchedule(span, initial_p=p0, final_p=p1).value(t)"""
+    return p0 + min(float(t) / max(1, span), 1.0) * (p1 - p0)
+
+
+def _check_policy_kwargs(policy_kwargs):
+    kw = dict(policy_kwargs or {})
+    unknown = set(kw) - {"layers", "dueling", "layer_norm", "act_fun"}
+    if unknown:
+        raise NotImplementedError(f"policy_kwargs {sorted(unknown)} are not built for DQN")
+    if not kw.get("dueling", True):
+        raise NotImplementedError("dueling=False: only the dueling DQN network is built")
+    if kw.get("layer_norm", False):
+        raise NotImplementedError("layer_norm=True: layer-normalised DQN policies are not built")
+    if kw.get("act_fun") is not None and getattr(kw["act_fun"], "__name__", "") != "relu":
+        raise NotImplementedError("act_fun: only ReLU is built")
+    layers = list(kw.get("layers", [64, 64]))
+    if len(layers) != 2:
+        raise NotImplementedError(f"layers={layers}: the DQN learner builds exactly two hidden layers")
+    return kw, [int(x) for x in layers]
+
+
+class DQN:
+    """stable-baselines 2.10 ``DQN(policy, env, ...)`` with its signature and defaults, plus ``device`` and ``seed``:
+    ``learn / predict / save / load / get_parameters / load_parameters / get_env / get_vec_normalize_env`` and
+    ``save_training_state / load_training_state``.  One environment (stable-baselines' DQN refuses a VecEnv of more)."""
+
+    def __init__(self, policy, env, gamma=0.99, learning_rate=5e-4, buffer_size=50000, exploration_fraction=0.1,
+                 exploration_final_eps=0.02, exploration_initial_eps=1.0, train_freq=1, batch_size=32, double_q=True, learning_starts=1000,
+                 target_network_update_freq=500, prioritized_replay=False, prioritized_replay_alpha=0.6, prioritized_replay_beta0=0.4,
+                 prioritized_replay_beta_iters=None, prioritized_replay_eps=1e-6, param_noise=False, n_cpu_tf_sess=None, verbose=0,
+                 tensorboard_log=None, _init_setup_model=True, policy_kwargs=None, full_tensorboard_log=False, seed=None, device=0):
+        if not double_q:
+            raise NotImplementedError("double_q=False: only the double-Q target is built")
+        if param_noise:
+            raise NotImplementedError("param_noise=True: parameter-noise exploration is not built")
+        if isinstance(policy, str):
+            if policy != "MlpPolicy":
+                raise NotImplementedError(f"policy '{policy}': only the MLP DQN policy is built")
+        else:
+            from .deepq.policies import MlpPolicy
+            if policy is not MlpPolicy:
+                raise NotImplementedError(f"policy {getattr(policy, '__name__', policy)}: only deepq.policies.MlpPolicy is built")
+        self.policy_kwargs, self.layers = _check_policy_kwargs(policy_kwargs)
+        self.gamma, self.learning_rate, self.buffer_size, self.batch_size = gamma, learning_rate, int(buffer_size), int(batch_size)
+        self.exploration_fraction, self.exploration_final_eps = exploration_fraction, exploration_final_eps
+        self.exploration_initial_eps = exploration_initial_eps
+        self.train_freq, self.learning_starts, self.target_network_update_freq = int(train_freq), int(learning_starts), int(target_network_update_freq)
+        self.prioritized_replay = bool(prioritized_replay)
+        self.per_alpha, self.per_beta0, self.per_beta_iters, self.per_eps = prioritized_replay_alpha, prioritized_replay_beta0, \
+            prioritized_replay_beta_iters, prioritized_replay_eps
+        self.verbose, self.seed, self.device = verbose, seed, device
+        self.num_timesteps = 0
+        self.n_target_updates = 0
+        self._rng = np.random.default_rng(seed)            # epsilon-greedy draws of learn()
+        self.predict_rng = np.random.default_rng(seed)     # softmax(Q) draws of predict(deterministic=False)
+        self.learner: Optional[DQNLearner] = None
+        self.env = None
+        self._vec_normalize_env = None
+        if env is not None:
+            self._set_env(env)
+            if _init_setup_model:
+                self.setup_model()
+
+    def _set_env(self, env):
+        env = env if hasattr(env, "num_envs") else DummyVecEnv([lambda: env])
+        if env.num_envs > 1:     # stable-baselines' own refusal (deepq/dqn.py: "...cannot be used with more than one env")
+            raise ValueError("Error: DQN cannot be used with more than one environment (num_envs > 1)")
+        self.env = env
+        self.observation_space, self.action_space = env.observation_space, env.action_space
+        self._vec_normalize_env = self.get_vec_normalize_env()
+
+    def setup_model(self):
+        if not hasattr(self.action_space, "n"):
+            raise NotImplementedError(f"DQN needs a Discrete action space, got {self.action_space}")
+        obs_dim = int(np.prod(self.observation_space.shape))
+        self.learner = DQNLearner(obs_dim, int(self.action_space.n), tuple(self.layers), self.batch_size, self.buffer_size, self.gamma,
+                                  int(self.seed or 0), self.device, prioritized_replay=self.prioritized_replay,
+                                  prioritized_replay_alpha=self.per_alpha, prioritized_replay_eps=self.per_eps)
+        rng = np.random.default_rng(self.seed)
+        p = OrderedDict()
+        for n, shp in self.learner.param_shapes.items():
+            if n == "deepq/eps":
+                p[n] = np.float32(0.0)          # tf.constant_initializer(0) in deepq/build_graph.py build_act
+            elif n.startswith(_TARGET):
+                p[n] = p[n.replace(_TARGET, _ONLINE)].copy()
+            elif len(shp) == 2:                 # tf.contrib.layers.fully_connected: Xavier uniform weights, zero biases
+                lim = np.sqrt(6.0 / (shp[0] + shp[1]))
+                p[n] = rng.uniform(-lim, lim, shp).astype(np.float32)
+            else:
+                p[n] = np.zeros(shp, np.float32)
+        self.learner.load_parameters(p)
+
+    def close(self):
+        if self.learner is not None:
+            self.learner.close()
+            self.learner = None
+
+    def get_env(self):
+        return self.env
+
+    def get_vec_normalize_env(self):
+        from .sac_model import unwrap_vec_normalize
+        return unwrap_vec_normalize(self.env)
+
+    def _sync_norm_stats(self):
+        vn = self._vec_normalize_env
+        self.learner.set_norm_stats(vn.obs_rms.mean, vn.obs_rms.var, float(vn.ret_rms.var), vn.clip_obs, vn.clip_reward, vn.epsilon,
+                                    norm_obs=vn.norm_obs, norm_reward=vn.norm_reward)
+
+    def learn(self, total_timesteps, callback=None, log_interval=100, tb_log_name="DQN", reset_num_timesteps=True, replay_wrapper=None):
+        """stable-baselines 2.10 DQN.learn: per environment step act epsilon-greedily, step, count, call back, store the raw
+        transition, then (past learning_starts, every train_freq steps) one gradient step, and every
+        target_network_update_freq environment steps the hard target copy."""
+        if replay_wrapper is not None:
+            raise NotImplementedError("replay_wrapper: the replay lives on the device")
+        callback = as_callback(callback)
+        callback.init_callback(self)
+        callback.on_training_start({"self": self, "writer": None}, globals())
+        vn = self._vec_normalize_env
+        lr = self.learning_rate if not callable(self.learning_rate) else self.learning_rate(1.0)
+        # reset_num_timesteps=False continues a run: the schedules follow num_timesteps over a run that ends total_timesteps from
+        # now, so an interrupted and resumed run takes the steps of an uninterrupted one
+        t0 = 0 if reset_num_timesteps else self.num_timesteps
+        if reset_num_timesteps:
+            self.num_timesteps = 0
+        horizon = t0 + total_timesteps
+        eps_span = int(self.exploration_fraction * horizon)
+        beta_span = self.per_beta_iters or horizon
+        obs = self.env.reset()
+        raw = vn.get_original_obs() if vn is not None else obs
+        eps = self.exploration_initial_eps
+        for _ in range(total_timesteps):
+            eps = _linear(self.num_timesteps, eps_span, self.exploration_initial_eps, self.exploration_final_eps)
+            greedy = self.learner.act(np.asarray(obs, np.float32))     # the wrapper's output, as stable-baselines' act sees it
+            action = int(self._rng.integers(0, self.learner.n_actions)) if self._rng.random() < eps else int(greedy[0])
+            new_obs, rew, done, infos = self.env.step(np.array([action]))
+            self.num_timesteps += 1
+            if callback.on_step() is False:
+                break
+            new_raw = vn.get_original_obs() if vn is not None else new_obs
+            rew_raw = vn.get_original_reward() if vn is not None else rew
+            nxt = np.array(new_raw, np.float32, copy=True).reshape(1, -1)
+            info = infos[0] if infos else {}
+            if done[0] and isinstance(info, dict) and "terminal_observation" in info and vn is None:
+                nxt[0] = np.asarray(info["terminal_observation"], np.float32).reshape(-1)
+            self.learner.replay_add(np.asarray(raw, np.float32), np.float32(action), rew_raw, nxt, np.asarray(done, np.float32))
+            obs, raw = new_obs, new_raw
+            can_sample = self.learner.replay_size() >= self.batch_size
+            if can_sample and self.num_timesteps > self.learning_starts and self.num_timesteps % self.train_freq == 0:
+                if self.prioritized_replay:
+                    self.learner.set_per_beta(_linear(self.num_timesteps, beta_span, self.per_beta0, 1.0))
+                if vn is not None:       # the sample is normalised with the statistics of this moment
+                    self._sync_norm_stats()
+                self.learner.step(1, lr)
+            if can_sample and self.num_timesteps > self.learning_starts and self.num_timesteps % self.target_network_update_freq == 0:
+                self.learner.update_target()
+                self.n_target_updates += 1
+        self.learner.set_eps(eps)
+        callback.on_training_end()
+        return self
+
+    def predict(self, observation, state=None, mask=None, deterministic=True):
+        """Greedy actions, or with ``deterministic=False`` a draw from softmax(Q) per row (the deepq policy's ``step``; the
+        uniform comes from ``self.predict_rng``).  ``observation`` is what the env hands out: with a VecNormalize wrapper its
+        normalised output, which the network takes as it is."""
+        obs = np.asarray(observation, np.float32).reshape(-1, self.learner.obs_dim)
+        idx, q = self.learner.act(obs, with_q=True)
+        if not deterministic:
+            q = q.astype(np.float64)
+            p = np.exp(q - q.max(1, keepdims=True))
+            p /= p.sum(1, keepdims=True)
+            idx = np.empty(len(q), np.int64)
+            for i in range(len(q)):          # numpy's choice(n, p=p): inverse CDF of one uniform
+                cdf = np.cumsum(p[i])
+                cdf /= cdf[-1]
+                idx[i] = int(np.searchsorted(cdf, self.predict_rng.random(), side="right"))
+        idx = np.asarray(idx, np.int64)
+        single = np.ndim(observation) == len(getattr(self.observation_space, "shape", (self.learner.obs_dim,)))
+        return (int(idx[0]) if single else idx), None
+
+    def get_parameters(self):
+        return OrderedDict((n + ":0", a) for n, a in self.learner.get_parameters().items())
+
+    def load_parameters(self, load_path_or_dict, exact_match=True):
+        params = load_path_or_dict
+        if isinstance(params, str):
+            _, params = sb_io.load_sb_zip(params)
+        self.learner.load_parameters(params, exact_match=exact_match)
+
+    def _data(self):
+        return {"double_q": True, "param_noise": False, "learning_starts": self.learning_starts, "train_freq": self.train_freq,
+                "prioritized_replay": self.prioritized_replay, "prioritized_replay_eps": self.per_eps, "batch_size": self.batch_size,
+                "target_network_update_freq": self.target_network_update_freq, "prioritized_replay_alpha": self.per_alpha,
+                "prioritized_replay_beta0": self.per_beta0, "prioritized_replay_beta_iters": self.per_beta_iters,
+                "exploration_final_eps": self.exploration_final_eps, "exploration_fraction": self.exploration_fraction,
+                "exploration_initial_eps": self.exploration_initial_eps, "learning_rate": self.learning_rate, "gamma": self.gamma,
+                "verbose": self.verbose, "n_envs": 1, "seed": self.seed, "policy_kwargs": dict(self.policy_kwargs)}
+
+    def save(self, save_path, cloudpickle=False):
+        """A stable-baselines zip: ``data`` (hyper-parameters), ``parameter_list`` and ``parameters`` in the zip's order."""
+        d = os.path.dirname(save_path)
+        if d:
+            os.makedirs(d, exist_ok=True)
+        data = self._data()
+        if callable(data["learning_rate"]):
+            data["learning_rate"] = None
+        sb_io.save_sb_zip(save_path, data, self.learner.get_parameters())
+
+    @classmethod
+    def load(cls, load_path, env=None, custom_objects=None, **kwargs):
+        """Reads a stable-baselines DQN zip (the shipped DQN_simple_4pads.zip / best_model.zip unchanged): the number of actions
+        and the widths come from the parameter shapes, the hyper-parameters from ``data``."""
+        from .spaces import Box, Discrete
+        if not os.path.exists(load_path) and os.path.exists(load_path + ".zip"):
+            load_path += ".zip"
+        data, params = sb_io.load_sb_zip(load_path)
+        w0 = params[_ONLINE + "action_value/fully_connected/weights"]
+        w1 = params[_ONLINE + "action_value/fully_connected_1/weights"]
+        w2 = params[_ONLINE + "action_value/fully_connected_2/weights"]
+
+        class _Spaces:
+            num_envs = 1
+            observation_space = Box(-np.inf, np.inf, (w0.shape[0],))
+            action_space = Discrete(w2.shape[1])
+        kw = {k: data[k] for k in ("gamma", "learning_rate", "batch_size", "learning_starts", "train_freq", "target_network_update_freq",
+                                   "exploration_fraction", "exploration_final_eps", "prioritized_replay", "prioritized_replay_alpha",
+                                   "prioritized_replay_beta0", "prioritized_replay_beta_iters", "prioritized_replay_eps", "seed")
+              if k in data and not isinstance(data[k], dict)}
+        kw["policy_kwargs"] = dict(data.get("policy_kwargs") or {}, layers=[int(w0.shape[1]), int(w1.shape[1])])
+        kw.update(kwargs)        # stable-baselines 2.10 does not save buffer_size: its default (50000) unless given here
+        m = cls("MlpPolicy", None, _init_setup_model=False, **kw)
+        if env is not None:
+            m._set_env(env)
+        else:
+            m.observation_space, m.action_space = _Spaces.observation_space, _Spaces.action_space
+        m.setup_model()
+        m.learner.load_parameters(params, exact_match=True)
+        return m
+
+    # ------------------------------------------------------------------ training state (training_state.py)
+    def _host_state(self):
+        if callable(self.learning_rate):
+            raise NotImplementedError("save_training_state needs a constant learning_rate")
+        init = dict(gamma=self.gamma, learning_rate=self.learning_rate, buffer_size=self.buffer_size,
+                    exploration_fraction=self.exploration_fraction, exploration_final_eps=self.exploration_final_eps,
+                    exploration_initial_eps=self.exploration_initial_eps, train_freq=self.train_freq, batch_size=self.batch_size,
+                    learning_starts=self.learning_starts, target_network_update_freq=self.target_network_update_freq,
+                    prioritized_replay=self.prioritized_replay, prioritized_replay_alpha=self.per_alpha,
+                    prioritized_replay_beta0=self.per_beta0, prioritized_replay_beta_iters=self.per_beta_iters,
+                    prioritized_replay_eps=self.per_eps, policy_kwargs=self.policy_kwargs, verbose=self.verbose, seed=self.seed,
+                    device=self.device)
+        return {"algo": "DQN", "init": init, "num_timesteps": int(self.num_timesteps), "n_target_updates": int(self.n_target_updates),
+                "rng": training_state.rng_state(self._rng), "predict_rng": training_state.rng_state(self.predict_rng)}
+
+    def save_training_state(self, path):
+        """Writes directory ``path``: model.zip, learner.state (parameters, Adam moments, counters, the replay and its priority
+        trees), vecnormalize.pkl and host.json."""
+        return training_state.save_training_state(self, path)
+
+    @classmethod
+    def load_training_state(cls, path, env, **kwargs):
+        """Rebuilds the model ``save_training_state`` wrote into ``path`` on ``env``; ``learn(n, reset_num_timesteps=False)``
+        then continues the run."""
+        path = training_state.resolve(path)
+        host = training_state.read_host(path)
+        if host.get("algo") != "DQN":
+            raise ValueError(f"{path} holds a {host.get('algo')} training state")
+        model = cls("MlpPolicy", env, **dict(host["init"], **kwargs))
+        training_state.restore_vec_normalize(path, model.env)
+        model.load_parameters(os.path.join(path, training_state.MODEL_FILE))
+        model.learner.load_state(os.path.join(path, training_state.STATE_FILE))
+        model.num_timesteps = int(host["num_timesteps"])
+        model.n_target_updates = int(host.get("n_target_updates", 0))
+        training_state.set_rng_state(model._rng, host["rng"])
+        training_state.set_rng_state(model.predict_rng, host["predict_rng"])
+        return model

@@ -21,3 +21,25 @@ class Box:
 
     def __repr__(self):
         return f"Box{self.shape}"
+
+
+class Discrete:
+    """Stand-in for gym.spaces.Discrete(n): actions 0 .. n-1 (the DQN learner's action space)."""
+
+    def __init__(self, n, seed=None):
+        self.n = int(n)
+        self.shape = ()
+        self.dtype = np.dtype(np.int64)
+        self._rng = np.random.default_rng(seed)
+
+    def sample(self):
+        return int(self._rng.integers(0, self.n))
+
+    def contains(self, x):
+        return isinstance(x, (int, np.integer)) and 0 <= int(x) < self.n
+
+    def seed(self, seed=None):
+        self._rng = np.random.default_rng(seed)
+
+    def __repr__(self):
+        return f"Discrete({self.n})"

@@ -2,7 +2,7 @@
 
 Mirrors /root/reference/manipulation_main/training/train_stable_baselines.py:26-148 (same sub-commands, flags,
 ``model_dir`` layout: ``config.yaml``, ``best_model/``, ``logs/rl_model_*`` checkpoints, ``vecnormalize.pkl``,
-``log_file.monitor.csv``) and the SAC / BDQ branches of ``SBPolicy.learn`` (sb_helper.py:69-128,175-247).  The
+``log_file.monitor.csv``) and the SAC / DQN / BDQ branches of ``SBPolicy.learn`` (sb_helper.py:69-128,155-165,175-247).  The
 environment itself stays the reference's (PyBullet on host cores): ``--env module:callable`` names a factory
 ``f(config, evaluate=False, validate=False, test=False) -> gym.Env``; the default imports the reference package and
 calls ``gym.make('gripper-env-v0', ...)`` exactly like the original script.
@@ -23,6 +23,8 @@ import yaml
 from . import BDQ, SAC, training_state
 from .bench import Monitor
 from .callbacks import BaseCallback, CheckpointCallback, EvalCallback, TrainingStateCallback
+from .deepq import DQN
+from .deepq.policies import MlpPolicy as DQNMlpPolicy
 from .sac_model import CnnPolicy, MlpPolicy
 from .vec_env import DummyVecEnv, SubprocVecEnv, VecNormalize
 
@@ -67,9 +69,14 @@ def train(args):
     if getattr(args, "resume", None):
         return resume(args)
     config = yaml.safe_load(open(args.config))
+    algo = args.algo
+    if algo == "DQN":          # stable-baselines' DQN takes one environment; its statistics stay with the host VecNormalize
+        if int(args.n_envs) > 1:
+            raise ValueError("--algo DQN: DQN cannot be used with more than one environment (--n_envs 1)")
+        if args.device_norm:
+            raise NotImplementedError("--algo DQN: --device_norm is built for SAC and BDQ only")
     os.mkdir(args.model_dir)                                   # like the reference: refuses to overwrite a run
     os.mkdir(os.path.join(args.model_dir, "best_model"))
-    algo = args.algo
     if args.simple:
         config["simplified"] = True
     if args.shaped:
@@ -132,8 +139,14 @@ def train(args):
                     prioritized_replay=c.get("prioritized_replay", False), device_obs_norm=bool(args.device_norm))
         if args.load_dir:
             model.load_parameters(BDQ.load(args.load_dir, env).get_parameters())
+    elif algo == "DQN":
+        model = DQN(DQNMlpPolicy, env, **dqn_kwargs(config))
+        if args.load_dir:        # every parameter (sb_helper.py:183-199's partial load cannot run: tensorboard_file is undefined there)
+            old = DQN.load(args.load_dir)
+            model.load_parameters(old.get_parameters())
+            old.close()
     else:
-        raise NotImplementedError(f"--algo {algo}: the H100 learner builds the SAC and BDQ branches of SBPolicy.learn (sb_helper.py:85-226)")
+        raise NotImplementedError(f"--algo {algo}: the H100 learner builds the SAC, DQN and BDQ branches of SBPolicy.learn (sb_helper.py:85-226)")
     if args.state_freq:
         callbacks.append(TrainingStateCallback(args.state_freq, os.path.join(args.model_dir, STATE_DIR)))
         _learn_keeping_state(model, int(c["total_timesteps"]), callbacks, os.path.join(args.model_dir, STATE_DIR))
@@ -151,6 +164,13 @@ def train(args):
 STATE_DIR = "training_state"
 
 
+def dqn_kwargs(config):
+    """sb_helper.py:159-165: only gamma, batch_size and prioritized_replay come from the config; every other DQN setting stays at
+    stable-baselines' default (the config's DQN learning_rate is not read there, and the shipped zip holds 5e-4)."""
+    c = config["DQN"]
+    return dict(verbose=2, gamma=config["discount_factor"], batch_size=c["batch_size"], prioritized_replay=c["prioritized_replay"])
+
+
 def _learn_keeping_state(model, total_timesteps, callbacks, state_dir, reset_num_timesteps=True):
     """model.learn; an interrupt (Ctrl-C) writes the training state before the run ends, as sb_helper.py:178-181 does
     for the model."""
@@ -166,7 +186,7 @@ def resume(args):
     model_dir = args.resume
     config = yaml.safe_load(open(os.path.join(model_dir, "config.yaml")))
     algo = config["algorithm"].upper()
-    if algo not in ("SAC", "BDQ"):
+    if algo not in ("SAC", "BDQ", "DQN"):
         raise NotImplementedError(f"--resume: algorithm '{algo}' has no training state")
     state_dir = training_state.resolve(os.path.join(model_dir, STATE_DIR))
     done = int(training_state.read_host(state_dir)["num_timesteps"])
@@ -189,7 +209,7 @@ def resume(args):
     ]
     if args.state_freq:
         callbacks.append(TrainingStateCallback(args.state_freq, os.path.join(model_dir, STATE_DIR)))
-    model = (SAC if algo == "SAC" else BDQ).load_training_state(state_dir, env)
+    model = {"SAC": SAC, "BDQ": BDQ, "DQN": DQN}[algo].load_training_state(state_dir, env)
     remaining = int(config[algo]["total_timesteps"]) - model.num_timesteps
     if remaining > 0:
         _learn_keeping_state(model, remaining, callbacks, os.path.join(model_dir, STATE_DIR), reset_num_timesteps=False)
@@ -238,8 +258,10 @@ def run(args):
             agent._sync_norm_stats()
     elif algo == "bdq":
         agent = BDQ.load(args.model)
+    elif algo == "dqn":
+        agent = DQN.load(args.model)
     else:
-        raise NotImplementedError(f"algorithm '{algo}': only sac / bdq zips run on the H100 learner")
+        raise NotImplementedError(f"algorithm '{algo}': only sac / dqn / bdq zips run on the H100 learner")
     print("Run the agent")
     out = run_agent(task, agent, args.stochastic, n_episodes=args.episodes)
     task.close()
@@ -267,7 +289,7 @@ def build_parser():
                         "transitions; 0.125 covers episodes down to ~9 steps); default: two frames per replay slot")
     t.add_argument("--device_norm", action="store_true",
                    help="keep VecNormalize's observation statistics on the GPU and upload every frame once "
-                        "(SAC / BDQ(device_obs_norm=True)); --resume takes it from the saved run")
+                        "(SAC / BDQ(device_obs_norm=True); not DQN); --resume takes it from the saved run")
     t.add_argument("--eval_freq", type=int, default=50000)
     t.add_argument("--checkpoint_freq", type=int, default=25000)
     t.add_argument("--state_freq", type=int, default=None,

@@ -332,6 +332,76 @@ int b2g_bdq_upload_bytes(const b2g_bdq* h, int64_t* observe_bytes, int64_t* othe
 int b2g_bdq_state_save(b2g_bdq* h, const char* path);
 int b2g_bdq_state_load(b2g_bdq* h, const char* path);
 
+/* ------------------------------------------------------------------------------------------------
+ * Dueling double DQN learner -- the `sb.DQN` object of sb_helper.py:155-165 (stable-baselines 2.10.1 deepq, restated in
+ * oracle/dqn_ref.py).  Variable names / shapes follow trained_models/DQN_4pads/DQN_simple_4pads.zip: two towers
+ * deepq/model/{action_value,state_value}/fully_connected{,_1,_2} (obs -> hidden0 -> hidden1 -> n_actions / 1, ReLU),
+ * Q = V + A - mean(A).  Actions are Discrete indices, stored as floats holding integers.  One step: sample (uniform or
+ * prioritised) -> forward (online s, online s', target s') -> double-Q target, weighted Huber loss -> backward -> every
+ * gradient tensor clipped to L2 norm 10 on its own (tf.clip_by_norm) -> TF1 Adam.  The hard target copy is
+ * b2g_dqn_update_target, called by the host loop (stable-baselines counts environment steps for it, not updates).
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct b2g_dqn b2g_dqn;
+typedef struct b2g_dqn_cfg {
+  int32_t obs_dim;             /* 100 in the shipped zip                                                             */
+  int32_t n_actions;           /* Discrete(n): [2, 64] (12 in the shipped zip)                                       */
+  int32_t hidden0, hidden1;    /* policy layers [hidden0, hidden1]: multiples of 4 in [4, 512] ([64, 64] shipped)    */
+  int32_t batch;               /* <= 1024 with prioritised replay                                                    */
+  int64_t buffer_capacity;
+  float gamma;
+  uint64_t seed;               /* Philox key of the replay draws (streams 0 and 2 of oracle/philox_ref.py)           */
+  int32_t device;
+  int32_t prioritized_replay;  /* 1: proportional prioritised replay on device sum / min segment trees               */
+  float per_alpha, per_eps;    /* priority exponent (0.6) and the epsilon added to |td| (1e-6)                       */
+} b2g_dqn_cfg;
+typedef struct b2g_dqn_metrics {
+  float loss;                  /* mean_b w_b huber(td_b)                                                             */
+  float mean_q, mean_abs_td;   /* mean_b Q(s_b, a_b), mean_b |td_b|                                                  */
+  float grad_norm;             /* global L2 norm of the gradients before the per-tensor clip                        */
+  int32_t n_clipped;           /* number of gradient tensors the clip scaled                                         */
+  int64_t n_updates;
+} b2g_dqn_metrics;
+
+/* B2G_EINVAL naming the limit outside n_actions in [2, 64], widths multiples of 4 in [4, 512], batch <= 65535 (<= 1024 with
+ * PER) */
+int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out);
+int b2g_dqn_destroy(b2g_dqn* h);
+/* index 0 = deepq/eps; then the online tensors, then the target tensors, in the zip's order */
+int b2g_dqn_param_count(const b2g_dqn* h);
+int b2g_dqn_param_info(const b2g_dqn* h, int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim);
+int b2g_dqn_get_param(b2g_dqn* h, const char* name, float* dst, size_t numel);
+int b2g_dqn_set_param(b2g_dqn* h, const char* name, const float* src, size_t numel);
+/* the gradient of the last step after the per-tensor clip (online tensors only) */
+int b2g_dqn_get_grad(b2g_dqn* h, const char* name, float* dst, size_t numel);
+/* raw transitions; every act value must be an integer in [0, n_actions) (B2G_EINVAL naming the first that is not, nothing
+ * stored), as for b2g_dqn_step_explicit's batch */
+int b2g_dqn_replay_add(b2g_dqn* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done,
+                       int64_t n);
+int64_t b2g_dqn_replay_size(const b2g_dqn* h);
+/* VecNormalize's statistics for the gather of the sampled and explicit steps (the replay holds raw transitions); not used by
+ * b2g_dqn_act */
+int b2g_dqn_set_norm_stats(b2g_dqn* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs,
+                           double clip_rew, double eps, int norm_obs, int norm_reward);
+/* n_steps sampled steps, replayed as one captured CUDA graph each */
+int b2g_dqn_step(b2g_dqn* h, int n_steps, float lr, b2g_dqn_metrics* out);
+/* prioritised replay: beta of the NEXT sampled steps; slots / weights / new priorities (|td| + eps) of the last sampled step,
+ * as b2g_bdq_get_last_per */
+int b2g_dqn_set_per_beta(b2g_dqn* h, float beta);
+int b2g_dqn_get_last_per(b2g_dqn* h, int32_t* slots, float* weights, float* priorities);
+/* parity entry point: caller-supplied batch (+ optional importance weights); td_out (may be NULL): [batch] */
+int b2g_dqn_step_explicit(b2g_dqn* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done,
+                          const float* weights, float lr, int apply_update, b2g_dqn_metrics* out, float* td_out);
+/* one device-to-device copy of the online parameters onto the target parameters */
+int b2g_dqn_update_target(b2g_dqn* h);
+/* greedy actions argmax_k Q(s, k) of the online network for n observations as the network sees them (a VecNormalize
+ * wrapper's output: no normalisation is applied here); q_out (may be NULL): the [n, n_actions] Q rows */
+int b2g_dqn_act(b2g_dqn* h, const float* obs, int n, int32_t* act_out, float* q_out);
+/* training state, as b2g_bdq_state_save / _load: parameters, Adam moments, counters, n_updates, the live replay rows, the
+ * prioritised-replay trees, max priority and beta, and deepq/eps.  The fingerprint covers every b2g_dqn_cfg field that
+ * decides the layout or the prioritised replay. */
+int b2g_dqn_state_save(b2g_dqn* h, const char* path);
+int b2g_dqn_state_load(b2g_dqn* h, const char* path);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Row a12: auto-encoder ENCODER forward (perception for the `encoded depth` observation, SURVEY.md section 8).
  * Replaces SimpleAutoEncoder.encode  (/root/reference/manipulation_main/gripperEnv/encoders.py:59-61; graph :87-108)
