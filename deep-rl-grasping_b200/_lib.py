@@ -30,6 +30,9 @@ SYMBOLS = [
     "b2g_dqn_get_grad", "b2g_dqn_replay_add", "b2g_dqn_replay_size", "b2g_dqn_set_norm_stats", "b2g_dqn_step",
     "b2g_dqn_step_explicit", "b2g_dqn_set_per_beta", "b2g_dqn_get_last_per", "b2g_dqn_update_target", "b2g_dqn_act",
     "b2g_dqn_state_save", "b2g_dqn_state_load",
+    "b2g_ppo_create", "b2g_ppo_destroy", "b2g_ppo_param_count", "b2g_ppo_param_info", "b2g_ppo_get_param", "b2g_ppo_set_param",
+    "b2g_ppo_get_grad", "b2g_ppo_rollout_act", "b2g_ppo_rollout_reward", "b2g_ppo_rollout_reset", "b2g_ppo_rollout_get",
+    "b2g_ppo_update", "b2g_ppo_train_step_explicit", "b2g_ppo_act", "b2g_ppo_get_step", "b2g_ppo_state_save", "b2g_ppo_state_load",
     "b2g_encoder_create", "b2g_encoder_destroy", "b2g_encoder_n_layers", "b2g_encoder_layer_shape", "b2g_encoder_set_weights",
     "b2g_encoder_encode", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor",
     "b2g_autoencoder_create", "b2g_autoencoder_destroy", "b2g_autoencoder_n_layers", "b2g_autoencoder_layer_shape",
@@ -77,6 +80,22 @@ class DqnCfg(C.Structure):
 class DqnMetrics(C.Structure):
     _fields_ = [("loss", C.c_float), ("mean_q", C.c_float), ("mean_abs_td", C.c_float), ("grad_norm", C.c_float),
                 ("n_clipped", C.c_int32), ("n_updates", C.c_int64)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class PpoCfg(C.Structure):
+    _fields_ = [
+        ("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("hidden0", C.c_int32), ("hidden1", C.c_int32), ("n_envs", C.c_int32),
+        ("n_steps", C.c_int32), ("nminibatches", C.c_int32), ("noptepochs", C.c_int32), ("gamma", C.c_float), ("lam", C.c_float),
+        ("ent_coef", C.c_float), ("vf_coef", C.c_float), ("max_grad_norm", C.c_float), ("seed", C.c_uint64), ("device", C.c_int32),
+    ]
+
+
+class PpoMetrics(C.Structure):
+    _fields_ = [("policy_loss", C.c_float), ("value_loss", C.c_float), ("entropy", C.c_float), ("approxkl", C.c_float),
+                ("clipfrac", C.c_float), ("grad_norm", C.c_float), ("n_updates", C.c_int64)]
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
@@ -165,7 +184,7 @@ def load():
     lib.b2g_last_step_ms.restype = C.c_float
     lib.b2g_profile_step.argtypes = [vp, C.c_float, C.POINTER(C.c_char_p), fp, C.c_int]
     for f in ("b2g_sac_state_save", "b2g_sac_state_load", "b2g_bdq_state_save", "b2g_bdq_state_load", "b2g_dqn_state_save",
-              "b2g_dqn_state_load"):
+              "b2g_dqn_state_load", "b2g_ppo_state_save", "b2g_ppo_state_load"):
         getattr(lib, f).argtypes = [vp, C.c_char_p]
     lib.b2g_bdq_create.argtypes = [C.POINTER(BdqCfg), C.POINTER(vp)]
     lib.b2g_bdq_destroy.argtypes = [vp]
@@ -203,6 +222,20 @@ def load():
     lib.b2g_dqn_get_last_per.argtypes = [vp, C.POINTER(C.c_int32), fp, fp]
     lib.b2g_dqn_update_target.argtypes = [vp]
     lib.b2g_dqn_act.argtypes = [vp, fp, C.c_int, C.POINTER(C.c_int32), fp]
+    lib.b2g_ppo_create.argtypes = [C.POINTER(PpoCfg), C.POINTER(vp)]
+    lib.b2g_ppo_destroy.argtypes = [vp]
+    lib.b2g_ppo_param_count.argtypes = [vp]
+    lib.b2g_ppo_param_info.argtypes = [vp, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]
+    for f in ("b2g_ppo_get_param", "b2g_ppo_set_param", "b2g_ppo_get_grad"):
+        getattr(lib, f).argtypes = [vp, C.c_char_p, fp, C.c_size_t]
+    lib.b2g_ppo_rollout_act.argtypes = [vp, fp, fp]
+    lib.b2g_ppo_rollout_reward.argtypes = [vp, fp, fp]
+    lib.b2g_ppo_rollout_reset.argtypes = [vp]
+    lib.b2g_ppo_rollout_get.argtypes = [vp, fp, fp, fp, fp, fp]
+    lib.b2g_ppo_update.argtypes = [vp, fp, C.POINTER(C.c_int32), C.c_float, C.c_float, C.c_float, C.POINTER(PpoMetrics)]
+    lib.b2g_ppo_train_step_explicit.argtypes = [vp, fp, fp, fp, fp, fp, C.c_float, C.c_float, C.c_float, C.c_int, C.POINTER(PpoMetrics)]
+    lib.b2g_ppo_act.argtypes = [vp, fp, C.c_int, C.c_int, fp, fp, fp]
+    lib.b2g_ppo_get_step.argtypes = [vp, i64p, i64p, C.POINTER(C.c_int32)]
     lib.b2g_encoder_create.argtypes = [C.POINTER(EncoderCfg), C.POINTER(vp)]
     lib.b2g_encoder_destroy.argtypes = [vp]
     lib.b2g_encoder_n_layers.argtypes = [vp]

@@ -1,8 +1,11 @@
-"""``stable_baselines.common.policies`` names imported by sb_helper.py:11,18 for the TRPO/PPO branches (out of scope)."""
+"""``stable_baselines.common.policies`` names imported by sb_helper.py:11,18 for the TRPO/PPO branches.  ``MlpPolicy`` is the
+actor-critic MLP (tanh, net_arch=[dict(pi=[64, 64], vf=[64, 64])]) that ``ppo2.PPO2`` builds; TRPO stays out of scope."""
 
 
 class MlpPolicy:
-    unsupported = "actor-critic policies (TRPO / PPO branches) are outside the hot-path scope (DESIGN.md section 7)"
+    """A marker: the network itself lives in csrc/ppo.cu."""
+    # ppo2.PPO2 accepts this class by identity; every other learner that reads ``unsupported`` (SAC) refuses it
+    unsupported = "common.policies.MlpPolicy is the actor-critic policy: use it with b200grasp.ppo2.PPO2 (TRPO is not built)"
 
 
 class CnnPolicy(MlpPolicy):

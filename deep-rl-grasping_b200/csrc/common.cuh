@@ -56,6 +56,8 @@ enum GemmFlags : int {
   GG_CN_AFFINE4 = 1 << 8, // host-verified: cN / kN contiguous inside aligned 4-column groups, outputs 16-byte aligned
   GG_EPI_LRELU_GRAD = 1 << 15, // gg_simt_launch_ext: C = acc * g(mask[kM[m] + kN[n]]), g = 1 / alpha / 0 for a post-LeakyReLU value
                                // > 0 / < 0 / == 0 (Keras' relu(x) - alpha * relu(-x) has gradient 0 at x = 0)
+  GG_EPI_BIAS_TANH = 1 << 16,  // gg_simt_launch_tanh: C = tanh(acc + bias[n])
+  GG_EPI_TANH_GRAD = 1 << 17,  // gg_simt_launch_tanh: C = acc * (1 - y^2), y = mask[kM[m] + kN[n]] a stored tanh output
 };
 
 struct GemmDesc {
@@ -98,6 +100,8 @@ void gg_simt_launch(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaS
 // the same engine with GG_EPI_LRELU_GRAD and m-contiguous GG_A_SCALAR gathers, summing in double, with GG_EPI_ATOMIC /
 // GG_COLSUM accumulating into double arrays behind C / colsum (auto-encoder training, autoencoder.cu)
 void gg_simt_launch_ext(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaStream_t s);
+// the plain fp32 engine with the tanh epilogues GG_EPI_BIAS_TANH and GG_EPI_TANH_GRAD (PPO's MLP, ppo.cu)
+void gg_simt_launch_tanh(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaStream_t s);
 constexpr int GG_SIMT_BM = 64, GG_SIMT_BN = 64, GG_SIMT_BK = 16;
 // wgmma engine: 128 x 64 output tile, 64-wide r-chunks; x3 != 0 -> BF16 hi/lo split (3 MMAs)
 cudaError_t gg_tc_launch(const GemmDesc* host_descs, int ndesc, int total_tiles, int mode_flags, int x3, int num_sms, cudaStream_t s);

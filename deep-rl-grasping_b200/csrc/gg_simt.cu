@@ -21,8 +21,9 @@ __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast
 // (a weight or bias gradient over every pixel of a batch) keeps its accuracy; its GG_EPI_ATOMIC and GG_COLSUM destinations
 // are double arrays (C and colsum reinterpreted), accumulated without rounding to fp32.  The plain instantiation is the
 // engine every other path launches, unchanged.
-template <bool EXT>
-__global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict__ descs, int ndesc) {
+// TANH: the PPO variant (fp32 sums, as the plain engine), which adds GG_EPI_BIAS_TANH and GG_EPI_TANH_GRAD (ppo.cu).
+template <bool EXT, bool TANH>
+__device__ __forceinline__ void gg_simt_body(const GemmDesc* __restrict__ descs, int ndesc) {
   __shared__ GemmDesc sd;
   __shared__ __align__(16) float As[BK][BM + PAD];
   __shared__ __align__(16) float Bs[BK][BN + PAD];
@@ -205,7 +206,7 @@ __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict
     const int m = m0 + ty * 4 + i;
     if (m >= d.M) continue;
     const int cm = d.cM[m];
-    const int km = (d.flags & (EXT ? GG_EPI_MASK | GG_EPI_LRELU_GRAD : GG_EPI_MASK)) ? (d.kM ? d.kM[m] : cm) : 0;
+    const int km = (d.flags & (EXT ? GG_EPI_MASK | GG_EPI_LRELU_GRAD : (TANH ? GG_EPI_MASK | GG_EPI_TANH_GRAD : GG_EPI_MASK))) ? (d.kM ? d.kM[m] : cm) : 0;
     float v[4];
     int co[4];
 #pragma unroll
@@ -229,6 +230,11 @@ __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict
         if (EXT && (d.flags & GG_EPI_LRELU_GRAD)) {
           const float a = d.mask[km + (d.kN ? d.kN[n] : cn)];
           v[j] *= a > 0.f ? 1.f : (a < 0.f ? d.alpha : 0.f);
+        }
+        if (TANH && (d.flags & GG_EPI_BIAS_TANH)) v[j] = tanhf(v[j] + d.bias[n]);
+        if (TANH && (d.flags & GG_EPI_TANH_GRAD)) {
+          const float y = d.mask[km + (d.kN ? d.kN[n] : cn)];
+          v[j] *= 1.f - y * y;
         }
         if (d.flags & GG_EPI_SCALE) v[j] *= d.alpha;
       }
@@ -267,6 +273,15 @@ __global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict
     }
   }
 }
+
+template <bool EXT>
+__global__ void __launch_bounds__(256) gg_simt_kernel(const GemmDesc* __restrict__ descs, int ndesc) {
+  gg_simt_body<EXT, false>(descs, ndesc);
+}
+
+__global__ void __launch_bounds__(256) gg_simt_tanh_kernel(const GemmDesc* __restrict__ descs, int ndesc) {
+  gg_simt_body<false, true>(descs, ndesc);
+}
 }  // namespace
 
 void gg_simt_launch(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaStream_t s) {
@@ -277,6 +292,11 @@ void gg_simt_launch(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaS
 void gg_simt_launch_ext(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaStream_t s) {
   if (total_tiles <= 0) return;
   gg_simt_kernel<true><<<total_tiles, 256, 0, s>>>(dev_descs, ndesc);
+}
+
+void gg_simt_launch_tanh(const GemmDesc* dev_descs, int ndesc, int total_tiles, cudaStream_t s) {
+  if (total_tiles <= 0) return;
+  gg_simt_tanh_kernel<<<total_tiles, 256, 0, s>>>(dev_descs, ndesc);
 }
 
 }  // namespace b2g

@@ -1,0 +1,922 @@
+// libb200grasp: PPO2 learner -- the `sb.PPO2` branch of sb_helper.py:137-154 (stable-baselines 2.10.1 ppo2, restated in
+// oracle/ppo_ref.py).
+//
+// Network (common/policies.py FeedForwardPolicy, net_arch=[dict(pi=[h0, h1], vf=[h0, h1])], tanh): two towers on the
+// flattened observation, pi: obs -> h0 -> h1 -> mean [A], vf: obs -> h0 -> h1 -> value, a state-independent pi/logstd [1, A],
+// and the head q (vf latent -> A) that nothing trains.  Both towers' first layers are one [D, 2 h0] matrix (pi columns, then
+// vf columns), so layer 0 is one contraction over the shared input; get / set repack it to the zip's pi_fc0/w and vf_fc0/w.
+//
+// Rollout: b2g_ppo_rollout_act uploads the n_envs observations straight into rollout row t, runs the forward pass and draws
+// mean + std * eps (Philox stream 1 under the caller's key at the device step counter); b2g_ppo_rollout_reward stores row t's
+// rewards and the next episode-start flags.  Observations cross PCIe once.
+//
+// Update (b2g_ppo_update, one CUDA graph): bootstrap value of last_obs, GAE (a thread per env, reverse scan), then for each of
+// noptepochs x nminibatches minibatches, in the caller's permutation:
+//   layer 0   gather-GEMM through the permutation rows, split-R into Z0, then tanh(Z0 + b0)
+//   layer 1   both towers, one grouped launch with the tanh epilogue
+//   tail      one CTA: heads, minibatch advantage normalisation, clipped losses and metrics, head backward, head / logstd
+//             gradients and dZ1 = (dY1)(1 - Y1^2)
+//   layer 1   weight / bias gradients of both towers and dZ0 = dZ1 W1^T (1 - Y0^2), one grouped launch
+//   layer 0   weight / bias gradient X^T dZ0 (D up to 20480 rows)
+//   norm      global L2 norm of the gradient arena (fixed-order partials)
+//   Adam      TF1 Adam, eps 1e-5, on g * min(1, max_grad_norm / norm)   (tf.clip_by_global_norm)
+// q/w and q/b sit behind the trained arena: no gradient, no Adam moments.
+#include <cuda_runtime.h>
+#include <math.h>
+#include <string.h>
+
+#include <algorithm>
+#include <map>
+#include <string>
+#include <vector>
+
+#include "../../include/b200grasp.h"
+#include "common.cuh"
+#include "host.cuh"
+#include "state.cuh"
+
+using namespace b2g;
+
+namespace {
+
+constexpr int kMaxA = 16;            // action components: the tail keeps a row's mean in registers
+constexpr int kMaxWidth = 256;       // hidden widths (multiples of 4: 16-byte rows for the engine)
+constexpr int kMaxMinibatch = 16384; // one tail CTA walks the minibatch
+constexpr int kTailThreads = 1024;
+constexpr int kNormBlocks = 128, kNormThreads = 256;
+constexpr float kAdamEps = 1e-5f;    // ppo2.py: tf.train.AdamOptimizer(learning_rate, epsilon=1e-5)
+
+// metric slots: the last minibatch [0, 8) and the sums over an update's minibatches [8, 16)
+enum : int { PM_PG = 0, PM_VF, PM_ENT, PM_KL, PM_CLIP, PM_GN, PM_N = 8 };
+// device hyper-parameters of the current call: lr, cliprange, cliprange_vf (< 0: no value clipping)
+enum : int { HP_LR = 0, HP_CLIP, HP_CLIPVF, HP_N = 4 };
+
+struct PTensor {
+  std::string name;     // zip name (without the "model/" scope)
+  int rows, cols;       // zip shape (biases and logstd: rows 1)
+  int stride;           // device row stride
+  int64_t off;          // float offset inside P
+  int ndim;
+};
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// kernels
+// ---------------------------------------------------------------------------------------------------------------------------
+
+__device__ __forceinline__ float block_sum(float v, float* red) {   // fixed order: the same value on every call
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float t = 0.f;
+  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
+  return t;
+}
+
+// permutation -> storage rows: flattened (env-major) batch index f = e * n_steps + t lives in rollout row t * n_envs + e
+__global__ void ppo_rows_kernel(const int* __restrict__ perm, int n, int n_steps, int n_envs, int XS, int* __restrict__ rowidx,
+                                int* __restrict__ rowoff) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int f = perm[i], e = f / n_steps, t = f - e * n_steps;
+  const int r = t * n_envs + e;
+  rowidx[i] = r;
+  rowoff[i] = r * XS;
+}
+
+// rowoff[i] = (first + i) * XS for the actor's rows
+__global__ void ppo_iota_rows_kernel(int* __restrict__ rowoff, int first, int n, int XS) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) rowoff[i] = (first + i) * XS;
+}
+
+__global__ void ppo_bias_tanh_kernel(const float* __restrict__ Z, const float* __restrict__ b, float* __restrict__ Y, int n, int N) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n * N) Y[i] = tanhf(Z[i] + b[i % N]);
+}
+
+struct HeadArgs {
+  const float* Y1; int h1;             // [rows, 2 h1]: pi latent | vf latent
+  const float* Wpi; const float* bpi;  // [h1, A], [A]
+  const float* Wvf; const float* bvf;  // [h1, 1], [1]
+  const float* logstd;                 // [A]
+  int A;
+};
+
+// mean and value of row r
+__device__ __forceinline__ void ppo_heads(const HeadArgs& a, int r, float* mu, float& v) {
+  const float* ypi = a.Y1 + (size_t)r * 2 * a.h1;
+  const float* yvf = ypi + a.h1;
+#pragma unroll
+  for (int k = 0; k < kMaxA; ++k) mu[k] = k < a.A ? a.bpi[k] : 0.f;
+  v = a.bvf[0];
+  for (int j = 0; j < a.h1; ++j) {
+    const float yp = ypi[j];
+    const float* w = a.Wpi + (size_t)j * a.A;
+#pragma unroll
+    for (int k = 0; k < kMaxA; ++k)
+      if (k < a.A) mu[k] = fmaf(yp, w[k], mu[k]);
+    v = fmaf(yvf[j], a.Wvf[j], v);
+  }
+}
+
+// Actor over `rows` rows.  mode 0: rollout step t (noise of stream 1, stores action / value / neglogp in row t and the actions
+// in out); mode 1: bootstrap values -> lastv; mode 2: predict (deterministic or stream-1 noise) -> out, values -> vout.
+struct ActArgs {
+  HeadArgs h;
+  int rows, mode, deterministic, t;
+  unsigned long long key;
+  long long* step;                     // stream-1 step counter (advanced by one per drawing call)
+  float* r_act; float* r_val; float* r_nlp;   // rollout rows
+  float* lastv;
+  float* out; float* vout; float* nlpout;
+};
+
+__global__ void __launch_bounds__(kTailThreads) ppo_act_kernel(ActArgs a) {
+  __shared__ unsigned long long s_step;
+  const bool draw = a.mode == 0 || (a.mode == 2 && !a.deterministic);
+  if (threadIdx.x == 0) s_step = (unsigned long long)*a.step;
+  __syncthreads();
+  const int A = a.h.A;
+  const float half_log_2pi = 0.91893853320467274f;
+  for (int r = threadIdx.x; r < a.rows; r += blockDim.x) {
+    float mu[kMaxA], v;
+    ppo_heads(a.h, r, mu, v);
+    if (a.mode == 1) { a.lastv[r] = v; continue; }
+    float z[kMaxA];
+#pragma unroll
+    for (int k = 0; k < kMaxA; ++k) z[k] = 0.f;
+    if (draw) {
+      const uint2 key = make_uint2((unsigned)a.key, (unsigned)(a.key >> 32));
+      // element r * A + k of the flattened [rows, A] noise: lane (i & 3) of block i >> 2 (oracle/philox_ref.py noise)
+#pragma unroll
+      for (int k = 0; k < kMaxA; ++k) {
+        if (k >= A) break;
+        const int i = r * A + k, blk = i >> 2;
+        const uint4 q = philox4x32_10(make_uint4((unsigned)s_step, (unsigned)(s_step >> 32), (unsigned)blk, 1u), key);
+        const int lane = i & 3;
+        const unsigned x0 = lane < 2 ? q.x : q.z, x1 = lane < 2 ? q.y : q.w;
+        const float u0 = ((float)(x0 >> 8) + 0.5f) * (1.0f / 16777216.0f), u1 = ((float)(x1 >> 8) + 0.5f) * (1.0f / 16777216.0f);
+        const float rr = sqrtf(-2.f * logf(u0));
+        float s, c;
+        sincospif(2.f * u1, &s, &c);
+        z[k] = rr * ((lane & 1) ? s : c);
+      }
+    }
+    float nlp = half_log_2pi * (float)A;
+#pragma unroll
+    for (int k = 0; k < kMaxA; ++k) {
+      if (k >= A) break;
+      const float ls = a.h.logstd[k];
+      const float act = mu[k] + expf(ls) * z[k];
+      nlp += 0.5f * z[k] * z[k] + ls;
+      if (a.mode == 0) a.r_act[((size_t)a.t * a.rows + r) * A + k] = act;
+      a.out[(size_t)r * A + k] = act;
+    }
+    if (a.mode == 0) {
+      a.r_val[(size_t)a.t * a.rows + r] = v;
+      a.r_nlp[(size_t)a.t * a.rows + r] = nlp;
+    } else {
+      if (a.vout) a.vout[r] = v;
+      if (a.nlpout) a.nlpout[r] = nlp;
+    }
+  }
+  __syncthreads();
+  if (draw && threadIdx.x == 0) *a.step += 1;
+}
+
+// GAE (ppo2.py Runner._run): a thread per env, reverse over the n_steps rows.  done[t] is the episode-start flag of step t,
+// done[n_steps] the flags after the last step.
+__global__ void ppo_gae_kernel(const float* __restrict__ rew, const float* __restrict__ val, const float* __restrict__ done,
+                               const float* __restrict__ lastv, int T, int E, float gamma, float lam, float* __restrict__ adv,
+                               float* __restrict__ ret) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  float last = 0.f;
+  for (int t = T - 1; t >= 0; --t) {
+    const size_t i = (size_t)t * E + e;
+    const float nnt = 1.f - done[(size_t)(t + 1) * E + e];
+    const float nv = t == T - 1 ? lastv[e] : val[i + E];
+    const float delta = rew[i] + gamma * nv * nnt - val[i];
+    last = delta + gamma * lam * nnt * last;
+    adv[i] = last;
+    ret[i] = last + val[i];
+  }
+}
+
+struct TailArgs2 {
+  HeadArgs h;
+  int M;
+  const int* rowidx;                           // minibatch row -> rollout / staging row
+  const float* act; const float* oval; const float* onlp; const float* ret;
+  const float* hp;                             // HP_* device scalars
+  float ent_coef, vf_coef;
+  float* sz; float* sv; float* snlp; float* sadv; float* sdm; float* sdls; float* sdv;   // scratch [M] / [M, A]
+  float* dZ1;                                  // [M, 2 h1]
+  float* gWpi; float* gbpi; float* gWvf; float* gbvf; float* glogstd;
+  float* met;                                  // PM_* slots [0, 8) last, [8, 16) sums
+};
+
+// ppo2.py _train_step on one minibatch, after layer 1: heads, the clipped losses and their gradients down to dZ1
+__global__ void __launch_bounds__(kTailThreads) ppo_tail_kernel(TailArgs2 a) {
+  __shared__ float red[kTailThreads / 32];
+  const int M = a.M, A = a.h.A, h1 = a.h.h1, tid = threadIdx.x, NT = blockDim.x;
+  const float clip = a.hp[HP_CLIP], clipvf = a.hp[HP_CLIPVF];
+  const float invM = 1.0f / (float)M;
+  // ---- heads, neglogp, raw advantages
+  float s = 0.f;
+  for (int r = tid; r < M; r += NT) {
+    const int q = a.rowidx[r];
+    float mu[kMaxA], v;
+    ppo_heads(a.h, r, mu, v);
+    float nlp = 0.91893853320467274f * (float)A;
+    for (int k = 0; k < A; ++k) {
+      const float ls = a.h.logstd[k];
+      const float z = (a.act[(size_t)q * A + k] - mu[k]) / expf(ls);
+      a.sz[(size_t)r * A + k] = z;
+      nlp += 0.5f * z * z + ls;
+    }
+    const float adv = a.ret[q] - a.oval[q];
+    a.sv[r] = v; a.snlp[r] = nlp; a.sadv[r] = adv;
+    s += adv;
+  }
+  const float mean = block_sum(s, red) * invM;
+  float ss = 0.f;
+  for (int r = tid; r < M; r += NT) { const float d = a.sadv[r] - mean; ss += d * d; }
+  const float stdv = sqrtf(block_sum(ss, red) * invM);        // np.std: population
+  // ---- losses and the gradient seeds
+  float pg_s = 0.f, vf_s = 0.f, kl_s = 0.f, cf_s = 0.f;
+  for (int r = tid; r < M; r += NT) {
+    const int q = a.rowidx[r];
+    const float advn = (a.sadv[r] - mean) / (stdv + 1e-8f);
+    const float onlp = a.onlp[q], nlp = a.snlp[r];
+    const float ratio = expf(onlp - nlp);
+    const float lo = 1.f - clip, hi = 1.f + clip;
+    const float rc = fminf(fmaxf(ratio, lo), hi);
+    const float pg1 = -advn * ratio, pg2 = -advn * rc;
+    pg_s += fmaxf(pg1, pg2);
+    // tf.maximum sends the gradient to its first argument on ties; tf.clip_by_value passes it inside [lo, hi]
+    const float dratio = (pg1 >= pg2 || (ratio >= lo && ratio <= hi)) ? -advn : 0.f;
+    const float g_nlp = -dratio * ratio * invM;
+    const float v = a.sv[r], R = a.ret[q], ov = a.oval[q];
+    float l1 = (v - R) * (v - R), dv = (v - R);
+    if (clipvf >= 0.f) {
+      const float d = v - ov, vc = ov + fminf(fmaxf(d, -clipvf), clipvf);
+      const float l2 = (vc - R) * (vc - R);
+      if (l2 > l1) { l1 = l2; dv = (d >= -clipvf && d <= clipvf) ? (vc - R) : 0.f; }
+    }
+    vf_s += l1;
+    a.sdv[r] = a.vf_coef * dv * invM;
+    kl_s += (nlp - onlp) * (nlp - onlp);
+    cf_s += fabsf(ratio - 1.f) > clip ? 1.f : 0.f;
+    for (int k = 0; k < A; ++k) {
+      const float z = a.sz[(size_t)r * A + k];
+      a.sdm[(size_t)r * A + k] = -g_nlp * z / expf(a.h.logstd[k]);   // d nlp / d mu = -z / sigma
+      a.sdls[(size_t)r * A + k] = g_nlp * (1.f - z * z);             // d nlp / d logstd = 1 - z^2
+    }
+  }
+  const float pg = block_sum(pg_s, red) * invM, vfl = 0.5f * block_sum(vf_s, red) * invM;
+  const float kl = 0.5f * block_sum(kl_s, red) * invM, cf = block_sum(cf_s, red) * invM;
+  __syncthreads();                                                    // sdm / sdls / sdv of every row are written
+  // ---- head backward: dZ1 = dY1 (1 - Y1^2) for both towers
+  for (int i = tid; i < M * h1; i += NT) {
+    const int r = i / h1, k = i - r * h1;
+    const float* dm = a.sdm + (size_t)r * A;
+    const float* w = a.h.Wpi + (size_t)k * A;
+    float d = 0.f;
+    for (int j = 0; j < A; ++j) d = fmaf(dm[j], w[j], d);
+    const float yp = a.h.Y1[(size_t)r * 2 * h1 + k], yv = a.h.Y1[(size_t)r * 2 * h1 + h1 + k];
+    a.dZ1[(size_t)r * 2 * h1 + k] = d * (1.f - yp * yp);
+    a.dZ1[(size_t)r * 2 * h1 + h1 + k] = a.sdv[r] * a.h.Wvf[k] * (1.f - yv * yv);
+  }
+  // ---- head and logstd gradients: sums over the minibatch, one output per thread
+  const int n_wpi = h1 * A, n_jobs = n_wpi + A + h1 + 1 + A;
+  for (int jb = tid; jb < n_jobs; jb += NT) {
+    float g = 0.f;
+    if (jb < n_wpi) {
+      const int k = jb / A, j = jb - k * A;
+      for (int r = 0; r < M; ++r) g = fmaf(a.h.Y1[(size_t)r * 2 * h1 + k], a.sdm[(size_t)r * A + j], g);
+      a.gWpi[jb] = g;
+    } else if (jb < n_wpi + A) {
+      const int j = jb - n_wpi;
+      for (int r = 0; r < M; ++r) g += a.sdm[(size_t)r * A + j];
+      a.gbpi[j] = g;
+    } else if (jb < n_wpi + A + h1) {
+      const int k = jb - n_wpi - A;
+      for (int r = 0; r < M; ++r) g = fmaf(a.h.Y1[(size_t)r * 2 * h1 + h1 + k], a.sdv[r], g);
+      a.gWvf[k] = g;
+    } else if (jb == n_wpi + A + h1) {
+      for (int r = 0; r < M; ++r) g += a.sdv[r];
+      a.gbvf[0] = g;
+    } else {
+      const int j = jb - (n_wpi + A + h1 + 1);
+      for (int r = 0; r < M; ++r) g += a.sdls[(size_t)r * A + j];
+      a.glogstd[j] = g - a.ent_coef;                  // loss = ... - ent_coef * mean sum(logstd + .5 log(2 pi e))
+    }
+  }
+  if (tid == 0) {
+    float ent = 1.4189385332046727f * (float)A;     // 0.5 log(2 pi e) per component
+    for (int k = 0; k < A; ++k) ent += a.h.logstd[k];
+    const float m[5] = {pg, vfl, ent, kl, cf};
+    for (int k = 0; k < 5; ++k) { a.met[k] = m[k]; a.met[PM_N + k] += m[k]; }
+  }
+}
+
+// squared L2 norm of the gradient arena: fixed grid, one partial per CTA; the block also advances the Adam step
+__global__ void __launch_bounds__(kNormThreads) ppo_norm_kernel(const float* __restrict__ G, int n4, float* __restrict__ part,
+                                                                long long* counters) {
+  __shared__ float red[kNormThreads / 32];
+  float s = 0.f;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += gridDim.x * blockDim.x) {
+    const float4 g = reinterpret_cast<const float4*>(G)[i];
+    s += g.x * g.x + g.y * g.y + g.z * g.z + g.w * g.w;
+  }
+  const float t = block_sum(s, red);
+  if (threadIdx.x == 0) {
+    part[blockIdx.x] = t;
+    if (blockIdx.x == 0) counters[0] += 1;
+  }
+}
+
+// TF1 Adam (epsilon 1e-5) on the globally clipped gradient: g * max_norm / max(norm, max_norm) (tf.clip_by_global_norm)
+__global__ void __launch_bounds__(256) ppo_adam_kernel(float* __restrict__ P, float* __restrict__ Mo, float* __restrict__ Vo,
+                                                       float* __restrict__ G, int n4, const float* __restrict__ part,
+                                                       const long long* counters, const float* hp, float max_norm, int apply,
+                                                       float* met) {
+  __shared__ float s_scale;
+  __shared__ float s_lrt;
+  if (threadIdx.x < 32) {
+    float v = 0.f;
+    for (int i = threadIdx.x; i < kNormBlocks; i += 32) v += part[i];
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (threadIdx.x == 0) {
+      const float norm = sqrtf(v);
+      s_scale = max_norm / fmaxf(norm, max_norm);
+      const double t = (double)counters[0];
+      s_lrt = (float)((double)hp[HP_LR] * sqrt(1.0 - pow(0.999, t)) / (1.0 - pow(0.9, t)));
+      if (blockIdx.x == 0) { met[PM_GN] = norm; met[PM_N + PM_GN] += norm; }
+    }
+  }
+  __syncthreads();
+  const float sc = s_scale, lr = s_lrt, b1 = 0.9f, b2 = 0.999f;
+  for (int i4 = blockIdx.x * blockDim.x + threadIdx.x; i4 < n4; i4 += gridDim.x * blockDim.x) {
+    float4 g = reinterpret_cast<float4*>(G)[i4];
+    g.x *= sc; g.y *= sc; g.z *= sc; g.w *= sc;
+    reinterpret_cast<float4*>(G)[i4] = g;                 // b2g_ppo_get_grad reads the clipped gradient
+    if (!apply) continue;
+    float4 m = reinterpret_cast<float4*>(Mo)[i4], v = reinterpret_cast<float4*>(Vo)[i4], p = reinterpret_cast<float4*>(P)[i4];
+#define B2G_PPO_ADAM(c)                              \
+  m.c = b1 * m.c + (1.f - b1) * g.c;                 \
+  v.c = b2 * v.c + (1.f - b2) * (g.c * g.c);         \
+  p.c = p.c - lr * m.c / (sqrtf(v.c) + kAdamEps);
+    B2G_PPO_ADAM(x) B2G_PPO_ADAM(y) B2G_PPO_ADAM(z) B2G_PPO_ADAM(w)
+#undef B2G_PPO_ADAM
+    reinterpret_cast<float4*>(Mo)[i4] = m;
+    reinterpret_cast<float4*>(Vo)[i4] = v;
+    reinterpret_cast<float4*>(P)[i4] = p;
+  }
+}
+
+}  // namespace
+
+// one forward pass (layers 0 and 1) over M rows of an observation arena, and the backward launches of a minibatch
+struct PpoFwd { GemmGroup l0, l1; int M = 0; };
+struct PpoMb { PpoFwd f; GemmGroup b1, b0; const int* rowidx = nullptr; };
+
+struct b2g_ppo {
+  b2g_ppo_cfg cfg{};
+  int D = 0, XS = 0, A = 0, H0 = 0, H1 = 0, E = 0, T = 0, NB = 0, M = 0, NMB = 0, RMAX = 0, P_ROWS = 0;
+  std::vector<PTensor> tensors;
+  std::map<std::string, int> tindex;
+  int64_t n_train = 0, n_total = 0;
+  int64_t oW0 = 0, ob0 = 0, oW1[2]{}, ob1[2]{}, oWvf = 0, obvf = 0, oWpi = 0, obpi = 0, ols = 0;
+  float *P = nullptr, *Mo = nullptr, *Vo = nullptr, *G = nullptr;
+  cudaStream_t stream = nullptr;
+  std::vector<void*> allocs;
+  // rollout
+  float *r_obs = nullptr, *r_act = nullptr, *r_val = nullptr, *r_nlp = nullptr, *r_rew = nullptr, *r_done = nullptr;
+  float *r_adv = nullptr, *r_ret = nullptr, *lastv = nullptr;
+  int t = 0;                    // rollout rows filled
+  // explicit minibatch and predict staging
+  float *s_obs = nullptr, *s_act = nullptr, *s_val = nullptr, *s_nlp = nullptr, *s_ret = nullptr, *p_obs = nullptr;
+  // activations and scratch (RMAX rows)
+  float *Z0 = nullptr, *Y0 = nullptr, *Y1 = nullptr, *dZ1 = nullptr, *dZ0 = nullptr;
+  float *sz = nullptr, *sv = nullptr, *snlp = nullptr, *sadv = nullptr, *sdm = nullptr, *sdls = nullptr, *sdv = nullptr;
+  float *a_out = nullptr, *a_v = nullptr, *a_nlp = nullptr;
+  int *perm = nullptr, *rowidx = nullptr, *rowoff = nullptr, *act_rowoff = nullptr;
+  float *part = nullptr, *met = nullptr, *hp = nullptr;
+  long long* counters = nullptr;  // [0] Adam step, [1] stream-1 step, [2] n_updates
+  float* h_buf = nullptr;         // pinned: metrics, hyper-parameters
+  PpoFwd f_act, f_boot, f_pred;
+  PpoMb mb_explicit;
+  std::vector<PpoMb> mbs;
+  cudaGraphExec_t graph_exec = nullptr;
+  bool use_graph = true;
+  bool broken = false;
+  unsigned long long act_key = 0;
+  long long n_updates = 0;
+  const PTensor& tn(const std::string& nm) const { return tensors[tindex.at(nm)]; }
+};
+
+namespace {
+
+void add_t(b2g_ppo* h, const std::string& name, int rows, int cols, int stride, int64_t off, int ndim) {
+  h->tindex[name] = (int)h->tensors.size();
+  h->tensors.push_back(PTensor{name, rows, cols, stride, off, ndim});
+}
+
+int64_t take(int64_t& off, int64_t n) { const int64_t o = off; off += (n + 31) / 32 * 32; return o; }
+
+int splits_for(int tiles, int R) {   // split-R so a launch covers about two waves of the 132 SMs, >= 64 rows per slice
+  const int want = (264 + tiles - 1) / tiles;
+  return std::max(1, std::min(want, (R + 63) / 64));
+}
+
+// layers 0 and 1 over M rows of `obs` at row offsets rowoff
+int make_fwd(b2g_ppo* h, PpoFwd& f, const float* obs, const int* rowoff, int M, std::map<std::string, const int*>& tab) {
+  const int D = h->D, H0 = h->H0, H1 = h->H1;
+  f.M = M;
+  f.l0 = GemmGroup(); f.l1 = GemmGroup();
+  f.l0.name = "ppo_l0_fwd"; f.l1.name = "ppo_l1_fwd";
+  const int tiles = ((M + 63) / 64) * ((2 * H0 + 63) / 64);
+  GemmDesc d = gemm_desc(obs, rowoff, tab["iD"], h->P + h->oW0, tab["iD_2H0"], tab["i2H0"], h->Z0, tab["rM_2H0"], tab["i2H0"], M, 2 * H0, D,
+                         GG_A_RVEC | GG_EPI_ATOMIC, splits_for(tiles, D));
+  f.l0.host.push_back(d);
+  for (int tw = 0; tw < 2; ++tw) {
+    GemmDesc g = gemm_desc(h->Y0 + tw * H0, tab["rM_2H0"], tab["iH0"], h->P + h->oW1[tw], tab["iH0_H1"], tab["iH1"], h->Y1 + tw * H1,
+                           tab["rM_2H1"], tab["iH1"], M, H1, H0, GG_A_RVEC | GG_EPI_BIAS_TANH);
+    g.bias = h->P + h->ob1[tw];
+    f.l1.host.push_back(g);
+  }
+  if (int rc = finalize_tiles(f.l0, h->allocs, h->stream)) return rc;
+  return finalize_tiles(f.l1, h->allocs, h->stream);
+}
+
+int make_mb(b2g_ppo* h, PpoMb& mb, const float* obs, const int* rowoff, const int* rowidx, std::map<std::string, const int*>& tab) {
+  const int M = h->M, D = h->D, H0 = h->H0, H1 = h->H1;
+  if (int rc = make_fwd(h, mb.f, obs, rowoff, M, tab)) return rc;
+  mb.rowidx = rowidx;
+  mb.b1 = GemmGroup(); mb.b0 = GemmGroup();
+  mb.b1.name = "ppo_l1_bwd"; mb.b0.name = "ppo_l0_wgrad";
+  for (int tw = 0; tw < 2; ++tw) {
+    const int tiles = ((H0 + 63) / 64) * ((H1 + 63) / 64);
+    GemmDesc w = gemm_desc(h->Y0 + tw * H0, tab["iH0"], tab["rM_2H0"], h->dZ1 + tw * H1, tab["rM_2H1"], tab["iH1"], h->G + h->oW1[tw],
+                           tab["iH0_H1"], tab["iH1"], H0, H1, M, GG_COLSUM | GG_EPI_ATOMIC, splits_for(tiles, M));
+    w.colsum = h->G + h->ob1[tw];
+    mb.b1.host.push_back(w);
+    GemmDesc dg = gemm_desc(h->dZ1 + tw * H1, tab["rM_2H1"], tab["iH1"], h->P + h->oW1[tw], tab["iH1"], tab["iH0_H1"], h->dZ0 + tw * H0,
+                            tab["rM_2H0"], tab["iH0"], M, H0, H1, GG_A_RVEC | GG_B_RVEC | GG_EPI_TANH_GRAD);
+    dg.mask = h->Y0 + tw * H0;
+    mb.b1.host.push_back(dg);
+  }
+  const int tiles0 = ((D + 63) / 64) * ((2 * H0 + 63) / 64);
+  GemmDesc w0 = gemm_desc(obs, tab["iD"], rowoff, h->dZ0, tab["rM_2H0"], tab["i2H0"], h->G + h->oW0, tab["iD_2H0"], tab["i2H0"], D, 2 * H0, M,
+                          GG_COLSUM | GG_EPI_ATOMIC, splits_for(tiles0, M));
+  w0.colsum = h->G + h->ob0;
+  mb.b0.host.push_back(w0);
+  if (int rc = finalize_tiles(mb.b1, h->allocs, h->stream)) return rc;
+  return finalize_tiles(mb.b0, h->allocs, h->stream);
+}
+
+HeadArgs heads(b2g_ppo* h) {
+  HeadArgs a{};
+  a.Y1 = h->Y1; a.h1 = h->H1; a.A = h->A;
+  a.Wpi = h->P + h->oWpi; a.bpi = h->P + h->obpi; a.Wvf = h->P + h->oWvf; a.bvf = h->P + h->obvf; a.logstd = h->P + h->ols;
+  return a;
+}
+
+void fwd_issue(b2g_ppo* h, const PpoFwd& f, cudaStream_t s) {
+  cudaMemsetAsync(h->Z0, 0, (size_t)f.M * 2 * h->H0 * sizeof(float), s);
+  gg_simt_launch(f.l0.dev, (int)f.l0.host.size(), f.l0.total_tiles, s);
+  const int n = f.M * 2 * h->H0;
+  ppo_bias_tanh_kernel<<<(n + 255) / 256, 256, 0, s>>>(h->Z0, h->P + h->ob0, h->Y0, f.M, 2 * h->H0);
+  gg_simt_launch_tanh(f.l1.dev, (int)f.l1.host.size(), f.l1.total_tiles, s);
+}
+
+ActArgs act_args(b2g_ppo* h, int rows, int mode) {
+  ActArgs a{};
+  a.h = heads(h); a.rows = rows; a.mode = mode; a.key = h->act_key; a.step = h->counters + 1;
+  a.r_act = h->r_act; a.r_val = h->r_val; a.r_nlp = h->r_nlp; a.lastv = h->lastv;
+  a.out = h->a_out; a.vout = h->a_v; a.nlpout = h->a_nlp;
+  return a;
+}
+
+// one minibatch: forward, tail, backward, global norm, Adam
+void mb_issue(b2g_ppo* h, const PpoMb& mb, const float* act, const float* oval, const float* onlp, const float* ret, bool apply) {
+  cudaStream_t s = h->stream;
+  cudaMemsetAsync(h->G, 0, (size_t)h->n_train * sizeof(float), s);
+  fwd_issue(h, mb.f, s);
+  TailArgs2 t{};
+  t.h = heads(h); t.M = h->M; t.rowidx = mb.rowidx;
+  t.act = act; t.oval = oval; t.onlp = onlp; t.ret = ret; t.hp = h->hp;
+  t.ent_coef = h->cfg.ent_coef; t.vf_coef = h->cfg.vf_coef;
+  t.sz = h->sz; t.sv = h->sv; t.snlp = h->snlp; t.sadv = h->sadv; t.sdm = h->sdm; t.sdls = h->sdls; t.sdv = h->sdv; t.dZ1 = h->dZ1;
+  t.gWpi = h->G + h->oWpi; t.gbpi = h->G + h->obpi; t.gWvf = h->G + h->oWvf; t.gbvf = h->G + h->obvf; t.glogstd = h->G + h->ols;
+  t.met = h->met;
+  ppo_tail_kernel<<<1, kTailThreads, 0, s>>>(t);
+  gg_simt_launch_tanh(mb.b1.dev, (int)mb.b1.host.size(), mb.b1.total_tiles, s);
+  gg_simt_launch(mb.b0.dev, (int)mb.b0.host.size(), mb.b0.total_tiles, s);
+  const int n4 = (int)(h->n_train / 4);
+  ppo_norm_kernel<<<kNormBlocks, kNormThreads, 0, s>>>(h->G, n4, h->part, h->counters);
+  ppo_adam_kernel<<<std::max(1, std::min(264, (n4 + 255) / 256)), 256, 0, s>>>(h->P, h->Mo, h->Vo, h->G, n4, h->part, h->counters, h->hp,
+                                                                               h->cfg.max_grad_norm, apply ? 1 : 0, h->met);
+}
+
+// the whole update after the uploads: row map, bootstrap value, GAE, every minibatch
+int update_issue(b2g_ppo* h) {
+  cudaStream_t s = h->stream;
+  const int n = h->cfg.noptepochs * h->NB;
+  ppo_rows_kernel<<<(n + 255) / 256, 256, 0, s>>>(h->perm, n, h->T, h->E, h->XS, h->rowidx, h->rowoff);
+  fwd_issue(h, h->f_boot, s);
+  ppo_act_kernel<<<1, kTailThreads, 0, s>>>(act_args(h, h->E, 1));
+  ppo_gae_kernel<<<(h->E + 127) / 128, 128, 0, s>>>(h->r_rew, h->r_val, h->r_done, h->lastv, h->T, h->E, h->cfg.gamma, h->cfg.lam,
+                                                    h->r_adv, h->r_ret);
+  cudaMemsetAsync(h->met, 0, 2 * PM_N * sizeof(float), s);
+  for (const PpoMb& mb : h->mbs) mb_issue(h, mb, h->r_act, h->r_val, h->r_nlp, h->r_ret, true);
+  // the flags after the last step are the episode-start flags of the next rollout's first step
+  cudaMemcpyAsync(h->r_done, h->r_done + (size_t)h->T * h->E, h->E * sizeof(float), cudaMemcpyDeviceToDevice, s);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+int upload_hp(b2g_ppo* h, float lr, float clip, float clipvf) {
+  if (!(lr >= 0.f) || !(clip >= 0.f)) return b2g_fail(B2G_EINVAL, "learning rate and cliprange must be >= 0");
+  CK(cudaStreamSynchronize(h->stream));
+  h->h_buf[0] = lr; h->h_buf[1] = clip; h->h_buf[2] = clipvf; h->h_buf[3] = 0.f;
+  CK(cudaMemcpyAsync(h->hp, h->h_buf, HP_N * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  return 0;
+}
+
+int fetch(b2g_ppo* h, b2g_ppo_metrics* out, bool mean_of_update) {
+  CK(cudaMemcpyAsync(h->h_buf, h->met, 2 * PM_N * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  if (out) {
+    const float* m = mean_of_update ? h->h_buf + PM_N : h->h_buf;
+    const float k = mean_of_update ? 1.0f / (float)h->mbs.size() : 1.0f;
+    out->policy_loss = m[PM_PG] * k; out->value_loss = m[PM_VF] * k; out->entropy = m[PM_ENT] * k;
+    out->approxkl = m[PM_KL] * k; out->clipfrac = m[PM_CLIP] * k; out->grad_norm = m[PM_GN] * k;
+    out->n_updates = h->n_updates;
+  }
+  return 0;
+}
+
+int upload_rows(b2g_ppo* h, float* dst, const float* src, int rows) {   // [rows, D] -> rows of stride XS
+  CK(cudaMemcpy2DAsync(dst, h->XS * sizeof(float), src, h->D * sizeof(float), h->D * sizeof(float), rows, cudaMemcpyDefault, h->stream));
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b2g_ppo_destroy(b2g_ppo* h) {
+  if (!h) return 0;
+  cudaSetDevice(h->cfg.device);
+  if (h->stream) cudaStreamSynchronize(h->stream);
+  if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
+  for (void* q : h->allocs) cudaFree(q);
+  if (h->h_buf) cudaFreeHost(h->h_buf);
+  if (h->stream) cudaStreamDestroy(h->stream);
+  delete h;
+  return 0;
+}
+
+int b2g_ppo_create(const b2g_ppo_cfg* cfg, b2g_ppo** out) {
+  if (!cfg || !out) return b2g_fail(B2G_EINVAL, "cfg/out is NULL");
+  *out = nullptr;
+  const b2g_ppo_cfg& c = *cfg;
+  if (c.obs_dim < 1 || c.obs_dim > 65536) return b2g_fail(B2G_EINVAL, "obs_dim must be in [1, 65536]");
+  if (c.n_actions < 1 || c.n_actions > kMaxA) return b2g_fail(B2G_EINVAL, "n_actions must be in [1, 16]");
+  if (c.hidden0 % 4 || c.hidden1 % 4 || c.hidden0 < 4 || c.hidden1 < 4 || c.hidden0 > kMaxWidth || c.hidden1 > kMaxWidth)
+    return b2g_fail(B2G_EINVAL, "hidden widths must be multiples of 4 in [4, 256]");
+  if (c.n_envs < 1 || c.n_envs > 4096) return b2g_fail(B2G_EINVAL, "n_envs must be in [1, 4096]");
+  if (c.n_steps < 1 || c.n_steps > 65536) return b2g_fail(B2G_EINVAL, "n_steps must be in [1, 65536]");
+  if (c.nminibatches < 1 || c.noptepochs < 1) return b2g_fail(B2G_EINVAL, "nminibatches and noptepochs must be positive");
+  const int64_t nb = (int64_t)c.n_steps * c.n_envs;
+  if (nb % c.nminibatches) return b2g_fail(B2G_EINVAL, "n_batch = n_steps * n_envs must be divisible by nminibatches");
+  if (nb / c.nminibatches > kMaxMinibatch) return b2g_fail(B2G_EINVAL, "minibatch n_batch / nminibatches must be <= 16384");
+  if ((int64_t)c.noptepochs * c.nminibatches > 4096) return b2g_fail(B2G_EINVAL, "noptepochs * nminibatches must be <= 4096");
+  const int64_t XS = (c.obs_dim + 3) / 4 * 4;
+  if ((nb + c.n_envs) * XS >= (1LL << 31)) return b2g_fail(B2G_EINVAL, "rollout (n_steps + 1) * n_envs * obs_dim must be < 2^31 floats");
+  if (int rc = check_device(c.device)) return rc;
+  b2g_ppo* h = new b2g_ppo();
+  h->cfg = c;
+  const char* ng = getenv("B2G_NO_GRAPH");
+  h->use_graph = !(ng && ng[0] == '1');
+  h->D = c.obs_dim; h->XS = (int)XS; h->A = c.n_actions; h->H0 = c.hidden0; h->H1 = c.hidden1;
+  h->E = c.n_envs; h->T = c.n_steps; h->NB = (int)nb; h->NMB = c.nminibatches; h->M = (int)(nb / c.nminibatches);
+  h->P_ROWS = std::max(64, h->E);
+  h->RMAX = std::max(h->M, h->P_ROWS);
+  h->act_key = c.seed ^ 0xA5A5A5A5DEADBEEFull;       // oracle/philox_ref.py act_seed
+  auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_ppo_destroy(h); g_b2g_err = keep; return rc; };
+  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream"));
+  // ---- parameter arena: trained tensors, then q (no gradient, no moments)
+  const int D = h->D, A = h->A, H0 = h->H0, H1 = h->H1;
+  int64_t off = 0;
+  h->oW0 = take(off, (int64_t)D * 2 * H0); h->ob0 = take(off, 2 * H0);
+  for (int tw = 0; tw < 2; ++tw) { h->oW1[tw] = take(off, (int64_t)H0 * H1); h->ob1[tw] = take(off, H1); }
+  h->oWvf = take(off, H1); h->obvf = take(off, 1); h->oWpi = take(off, (int64_t)H1 * A); h->obpi = take(off, A); h->ols = take(off, A);
+  h->n_train = off;
+  const int64_t oWq = take(off, (int64_t)H1 * A), obq = take(off, A);
+  h->n_total = off;
+  // zip order (oracle/ppo_ref.py param_specs)
+  add_t(h, "pi_fc0/w", D, H0, 2 * H0, h->oW0, 2); add_t(h, "pi_fc0/b", 1, H0, H0, h->ob0, 1);
+  add_t(h, "vf_fc0/w", D, H0, 2 * H0, h->oW0 + H0, 2); add_t(h, "vf_fc0/b", 1, H0, H0, h->ob0 + H0, 1);
+  add_t(h, "pi_fc1/w", H0, H1, H1, h->oW1[0], 2); add_t(h, "pi_fc1/b", 1, H1, H1, h->ob1[0], 1);
+  add_t(h, "vf_fc1/w", H0, H1, H1, h->oW1[1], 2); add_t(h, "vf_fc1/b", 1, H1, H1, h->ob1[1], 1);
+  add_t(h, "vf/w", H1, 1, 1, h->oWvf, 2); add_t(h, "vf/b", 1, 1, 1, h->obvf, 1);
+  add_t(h, "pi/w", H1, A, A, h->oWpi, 2); add_t(h, "pi/b", 1, A, A, h->obpi, 1);
+  add_t(h, "pi/logstd", 1, A, A, h->ols, 2);
+  add_t(h, "q/w", H1, A, A, oWq, 2); add_t(h, "q/b", 1, A, A, obq, 1);
+  int rc = 0;
+  const int64_t E = h->E, T = h->T, R = h->RMAX;
+#define DA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
+  DA(h->P, h->n_total); DA(h->Mo, h->n_train); DA(h->Vo, h->n_train); DA(h->G, h->n_train);
+  DA(h->r_obs, (T + 1) * E * XS); DA(h->r_act, T * E * A); DA(h->r_val, T * E); DA(h->r_nlp, T * E); DA(h->r_rew, T * E);
+  DA(h->r_done, (T + 1) * E); DA(h->r_adv, T * E); DA(h->r_ret, T * E); DA(h->lastv, E);
+  DA(h->s_obs, (int64_t)h->M * XS); DA(h->s_act, (int64_t)h->M * A); DA(h->s_val, h->M); DA(h->s_nlp, h->M); DA(h->s_ret, h->M);
+  DA(h->p_obs, (int64_t)h->P_ROWS * XS);
+  DA(h->Z0, R * 2 * H0); DA(h->Y0, R * 2 * H0); DA(h->Y1, R * 2 * H1); DA(h->dZ1, R * 2 * H1); DA(h->dZ0, R * 2 * H0);
+  DA(h->sz, R * A); DA(h->sv, R); DA(h->snlp, R); DA(h->sadv, R); DA(h->sdm, R * A); DA(h->sdls, R * A); DA(h->sdv, R);
+  DA(h->a_out, R * A); DA(h->a_v, R); DA(h->a_nlp, R);
+  const int64_t nperm = (int64_t)c.noptepochs * h->NB;
+  DA(h->perm, nperm); DA(h->rowidx, nperm); DA(h->rowoff, nperm); DA(h->act_rowoff, E);
+  DA(h->part, kNormBlocks); DA(h->met, 2 * PM_N); DA(h->hp, HP_N); DA(h->counters, 4);
+#undef DA
+  if (cudaMallocHost((void**)&h->h_buf, 64 * sizeof(float)) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "cudaMallocHost"));
+  // ---- offset tables and descriptor groups
+  std::map<std::string, const int*> tab;
+  auto T_ = [&](const char* nm, const std::vector<int>& v) {
+    const int* p = nullptr;
+    if (int r2 = upload_table(h->allocs, h->stream, v, &p)) return r2;
+    tab[nm] = p;
+    return 0;
+  };
+  if ((rc = T_("iD", iota_tab(D))) || (rc = T_("iH0", iota_tab(H0))) || (rc = T_("iH1", iota_tab(H1))) || (rc = T_("i2H0", iota_tab(2 * H0))) ||
+      (rc = T_("rM_2H0", iota_tab((int)R, 2 * H0))) || (rc = T_("rM_2H1", iota_tab((int)R, 2 * H1))) ||
+      (rc = T_("iH0_H1", iota_tab(H0, H1))) || (rc = T_("iD_2H0", iota_tab(D, 2 * H0))) || (rc = T_("boot", iota_tab((int)E, h->XS, (int)(T * E) * h->XS))) ||
+      (rc = T_("pred", iota_tab(h->P_ROWS, h->XS))) || (rc = T_("sM", iota_tab(h->M, h->XS))) || (rc = T_("iM", iota_tab(h->M))))
+    return bail(rc);
+  if ((rc = make_fwd(h, h->f_act, h->r_obs, h->act_rowoff, (int)E, tab))) return bail(rc);
+  if ((rc = make_fwd(h, h->f_boot, h->r_obs, tab["boot"], (int)E, tab))) return bail(rc);
+  if ((rc = make_fwd(h, h->f_pred, h->p_obs, tab["pred"], h->P_ROWS, tab))) return bail(rc);
+  if ((rc = make_mb(h, h->mb_explicit, h->s_obs, tab["sM"], tab["iM"], tab))) return bail(rc);
+  h->mbs.resize((size_t)c.noptepochs * c.nminibatches);
+  for (size_t k = 0; k < h->mbs.size(); ++k)
+    if ((rc = make_mb(h, h->mbs[k], h->r_obs, h->rowoff + k * h->M, h->rowidx + k * h->M, tab))) return bail(rc);
+  if (cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "create sync"));
+  *out = h;
+  return 0;
+}
+
+int b2g_ppo_param_count(const b2g_ppo* h) { B2G_USABLE(h); return h ? (int)h->tensors.size() : 0; }
+
+int b2g_ppo_param_info(const b2g_ppo* h, int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim) {
+  B2G_USABLE(h);
+  if (!h || idx < 0 || idx >= (int)h->tensors.size() || !name) return b2g_fail(B2G_EINVAL, "bad tensor index");
+  const PTensor& t = h->tensors[idx];
+  snprintf(name, name_cap, "model/%s", t.name.c_str());
+  if (rows) *rows = t.rows;
+  if (cols) *cols = t.cols;
+  if (ndim) *ndim = t.ndim;
+  return 0;
+}
+
+static int ppo_copy(b2g_ppo* h, const char* name, float* arena, float* host, size_t numel, bool to_host, bool grad) {
+  if (!h || !name || !host) return b2g_fail(B2G_EINVAL, "NULL argument");
+  std::string nm(name);
+  if (nm.size() > 2 && nm.compare(nm.size() - 2, 2, ":0") == 0) nm.resize(nm.size() - 2);
+  if (nm.compare(0, 6, "model/") == 0) nm = nm.substr(6);
+  auto it = h->tindex.find(nm);
+  if (it == h->tindex.end()) return b2g_fail(B2G_EINVAL, std::string("unknown variable: ") + name);
+  const PTensor& t = h->tensors[it->second];
+  if (grad && t.off >= h->n_train) return b2g_fail(B2G_EINVAL, std::string("not a trained variable: ") + name);
+  if (numel != (size_t)t.rows * t.cols) return b2g_fail(B2G_EINVAL, std::string("size mismatch for ") + name);
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  float* dev = arena + t.off;
+  const size_t cols = t.cols, rows = t.rows;
+  if (to_host) CK(cudaMemcpy2D(host, cols * sizeof(float), dev, t.stride * sizeof(float), cols * sizeof(float), rows, cudaMemcpyDeviceToHost));
+  else CK(cudaMemcpy2D(dev, t.stride * sizeof(float), host, cols * sizeof(float), cols * sizeof(float), rows, cudaMemcpyHostToDevice));
+  return 0;
+}
+int b2g_ppo_get_param(b2g_ppo* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return ppo_copy(h, name, h ? h->P : nullptr, dst, numel, true, false); }
+int b2g_ppo_set_param(b2g_ppo* h, const char* name, const float* src, size_t numel) {
+  B2G_USABLE(h);
+  return ppo_copy(h, name, h ? h->P : nullptr, const_cast<float*>(src), numel, false, false);
+}
+int b2g_ppo_get_grad(b2g_ppo* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return ppo_copy(h, name, h ? h->G : nullptr, dst, numel, true, true); }
+
+int b2g_ppo_rollout_act(b2g_ppo* h, const float* obs, float* act_out) {
+  B2G_USABLE(h);
+  if (!h || !obs || !act_out) return b2g_fail(B2G_EINVAL, "NULL argument");
+  if (h->t >= h->T) return b2g_fail(B2G_ESTATE, "the rollout holds n_steps rows: call b2g_ppo_update first");
+  CK(cudaSetDevice(h->cfg.device));
+  cudaStream_t s = h->stream;
+  if (int rc = upload_rows(h, h->r_obs + (size_t)h->t * h->E * h->XS, obs, h->E)) return rc;
+  ppo_iota_rows_kernel<<<(h->E + 255) / 256, 256, 0, s>>>(h->act_rowoff, h->t * h->E, h->E, h->XS);
+  fwd_issue(h, h->f_act, s);
+  ActArgs a = act_args(h, h->E, 0);
+  a.t = h->t;
+  ppo_act_kernel<<<1, kTailThreads, 0, s>>>(a);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(act_out, h->a_out, (size_t)h->E * h->A * sizeof(float), cudaMemcpyDefault, s));
+  CK(cudaStreamSynchronize(s));
+  return 0;
+}
+
+int b2g_ppo_rollout_reward(b2g_ppo* h, const float* rew, const float* done) {
+  B2G_USABLE(h);
+  if (!h || !rew || !done) return b2g_fail(B2G_EINVAL, "NULL argument");
+  if (h->t >= h->T) return b2g_fail(B2G_ESTATE, "the rollout holds n_steps rows: call b2g_ppo_update first");
+  CK(cudaSetDevice(h->cfg.device));
+  const size_t E = h->E;
+  CK(cudaMemcpyAsync(h->r_rew + (size_t)h->t * E, rew, E * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->r_done + (size_t)(h->t + 1) * E, done, E * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  h->t += 1;
+  return 0;
+}
+
+int b2g_ppo_rollout_reset(b2g_ppo* h) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaMemsetAsync(h->r_done, 0, (size_t)h->E * sizeof(float), h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  h->t = 0;
+  return 0;
+}
+
+int b2g_ppo_rollout_get(b2g_ppo* h, float* adv, float* ret, float* val, float* nlp, float* act) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  const size_t n = (size_t)h->T * h->E;
+  if (adv) CK(cudaMemcpy(adv, h->r_adv, n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (ret) CK(cudaMemcpy(ret, h->r_ret, n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (val) CK(cudaMemcpy(val, h->r_val, n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (nlp) CK(cudaMemcpy(nlp, h->r_nlp, n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (act) CK(cudaMemcpy(act, h->r_act, n * h->A * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int b2g_ppo_update(b2g_ppo* h, const float* last_obs, const int32_t* perm, float lr, float cliprange, float cliprange_vf,
+                   b2g_ppo_metrics* out) {
+  B2G_USABLE(h);
+  if (!h || !last_obs || !perm) return b2g_fail(B2G_EINVAL, "NULL argument");
+  if (h->t != h->T) return b2g_fail(B2G_ESTATE, "the rollout is not full: n_steps rollout steps come before an update");
+  const int64_t n = (int64_t)h->cfg.noptepochs * h->NB;
+  for (int64_t i = 0; i < n; ++i)
+    if (perm[i] < 0 || perm[i] >= h->NB) return b2g_fail(B2G_EINVAL, "permutation entry " + std::to_string(i) + " is outside [0, n_batch)");
+  CK(cudaSetDevice(h->cfg.device));
+  if (int rc = upload_hp(h, lr, cliprange, cliprange_vf)) return rc;
+  if (int rc = upload_rows(h, h->r_obs + (size_t)h->T * h->E * h->XS, last_obs, h->E)) return rc;
+  CK(cudaMemcpyAsync(h->perm, perm, n * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+  if (h->use_graph && !h->graph_exec)
+    if (int rc = capture_graph(h->stream, [&] { return update_issue(h); }, &h->graph_exec)) return rc;
+  if (h->graph_exec) CK(cudaGraphLaunch(h->graph_exec, h->stream));
+  else if (int rc = update_issue(h)) return rc;
+  h->n_updates += (int64_t)h->mbs.size();
+  h->t = 0;
+  return fetch(h, out, true);
+}
+
+int b2g_ppo_train_step_explicit(b2g_ppo* h, const float* obs, const float* returns, const float* actions, const float* values,
+                                const float* neglogp, float lr, float cliprange, float cliprange_vf, int apply_update,
+                                b2g_ppo_metrics* out) {
+  B2G_USABLE(h);
+  if (!h || !obs || !returns || !actions || !values || !neglogp) return b2g_fail(B2G_EINVAL, "NULL argument");
+  CK(cudaSetDevice(h->cfg.device));
+  if (int rc = upload_hp(h, lr, cliprange, cliprange_vf)) return rc;
+  const size_t M = h->M;
+  if (int rc = upload_rows(h, h->s_obs, obs, h->M)) return rc;
+  CK(cudaMemcpyAsync(h->s_ret, returns, M * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->s_act, actions, M * h->A * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->s_val, values, M * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->s_nlp, neglogp, M * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemsetAsync(h->met, 0, 2 * PM_N * sizeof(float), h->stream));
+  if (!apply_update) {    // the Adam step counter advances only with an applied step
+    long long t0 = 0;
+    CK(cudaMemcpyAsync(&t0, h->counters, sizeof t0, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    mb_issue(h, h->mb_explicit, h->s_act, h->s_val, h->s_nlp, h->s_ret, false);
+    CK(cudaMemcpyAsync(h->counters, &t0, sizeof t0, cudaMemcpyHostToDevice, h->stream));
+  } else {
+    mb_issue(h, h->mb_explicit, h->s_act, h->s_val, h->s_nlp, h->s_ret, true);
+    h->n_updates += 1;
+  }
+  CK(cudaGetLastError());
+  return fetch(h, out, false);
+}
+
+int b2g_ppo_act(b2g_ppo* h, const float* obs, int n, int deterministic, float* act_out, float* value_out, float* neglogp_out) {
+  B2G_USABLE(h);
+  if (!h || !obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  CK(cudaSetDevice(h->cfg.device));
+  cudaStream_t s = h->stream;
+  const int P = h->P_ROWS;
+  for (int done_n = 0; done_n < n; done_n += P) {
+    const int chunk = std::min(P, n - done_n);
+    if (int rc = upload_rows(h, h->p_obs, obs + (size_t)done_n * h->D, chunk)) return rc;
+    fwd_issue(h, h->f_pred, s);
+    ActArgs a = act_args(h, chunk, 2);
+    a.deterministic = deterministic;
+    ppo_act_kernel<<<1, kTailThreads, 0, s>>>(a);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(act_out + (size_t)done_n * h->A, h->a_out, (size_t)chunk * h->A * sizeof(float), cudaMemcpyDefault, s));
+    if (value_out) CK(cudaMemcpyAsync(value_out + done_n, h->a_v, chunk * sizeof(float), cudaMemcpyDefault, s));
+    if (neglogp_out) CK(cudaMemcpyAsync(neglogp_out + done_n, h->a_nlp, chunk * sizeof(float), cudaMemcpyDefault, s));
+    CK(cudaStreamSynchronize(s));
+  }
+  return 0;
+}
+
+int b2g_ppo_get_step(b2g_ppo* h, int64_t* adam_step, int64_t* noise_step, int32_t* rollout_rows) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  long long c[2];
+  CK(cudaMemcpy(c, h->counters, sizeof c, cudaMemcpyDeviceToHost));
+  if (adam_step) *adam_step = c[0];
+  if (noise_step) *noise_step = c[1];
+  if (rollout_rows) *rollout_rows = h->t;
+  return 0;
+}
+
+}  // extern "C"
+
+// ================================================================================================
+// Training state (b2g_ppo_state_save / _load; container format in state.cuh).  An update boundary: the rollout in flight is
+// not saved; a loaded handle starts an empty rollout with cleared episode-start flags (the env starts a fresh episode).
+// ================================================================================================
+namespace {
+
+std::vector<FpField> ppo_fingerprint(const b2g_ppo* h) {
+  const b2g_ppo_cfg& c = h->cfg;
+  return {fp_int("obs_dim", c.obs_dim), fp_int("n_actions", c.n_actions), fp_int("hidden0", c.hidden0), fp_int("hidden1", c.hidden1),
+          fp_int("n_envs", c.n_envs), fp_int("n_steps", c.n_steps), fp_int("nminibatches", c.nminibatches), fp_int("noptepochs", c.noptepochs),
+          fp_int("seed", (int64_t)c.seed)};
+}
+
+const uint32_t kPpoTags[] = {state_tag("HOST"), state_tag("CNTR"), state_tag("PARM"), state_tag("ADMM"), state_tag("ADMV")};
+
+}  // namespace
+
+extern "C" {
+
+int b2g_ppo_state_save(b2g_ppo* h, const char* path) {
+  if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
+  B2G_USABLE(h);
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  long long cnt[4];
+  CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
+  int64_t hv[2] = {h->n_updates, 0};
+  std::vector<StateSection> secs(5);
+  secs[0].pieces = {StatePiece{hv, nullptr, sizeof hv}};
+  secs[1].pieces = {StatePiece{cnt, nullptr, sizeof cnt}};
+  StatePiece p; p.dev = h->P; p.bytes = h->n_total * sizeof(float);
+  StatePiece m; m.dev = h->Mo; m.bytes = h->n_train * sizeof(float);
+  StatePiece v; v.dev = h->Vo; v.bytes = h->n_train * sizeof(float);
+  secs[2].pieces = {p}; secs[3].pieces = {m}; secs[4].pieces = {v};
+  for (int i = 0; i < 5; ++i) secs[i].tag = kPpoTags[i];
+  return state_write(path, STATE_KIND_PPO, ppo_fingerprint(h), secs);
+}
+
+int b2g_ppo_state_load(b2g_ppo* h, const char* path) {
+  if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
+  CK(cudaSetDevice(h->cfg.device));
+  StateReader rd;
+  if (int rc = rd.open(path, STATE_KIND_PPO, ppo_fingerprint(h))) return rc;
+  const int n_sec = (int)(sizeof kPpoTags / sizeof kPpoTags[0]);
+  if (rd.n_sections() != n_sec) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a PPO2 learner");
+  for (int i = 0; i < n_sec; ++i)
+    if (rd.tag(i) != kPpoTags[i]) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a PPO2 learner");
+  int64_t hv[2];
+  long long cnt[4];
+  if (rd.bytes(0) != sizeof hv || rd.bytes(1) != sizeof cnt || rd.bytes(2) != (size_t)h->n_total * sizeof(float) ||
+      rd.bytes(3) != (size_t)h->n_train * sizeof(float) || rd.bytes(4) != (size_t)h->n_train * sizeof(float))
+    return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  if (int rc = rd.read_host(0, hv, sizeof hv)) return rc;
+  if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
+  CK(cudaStreamSynchronize(h->stream));
+  h->broken = true;
+  StatePiece p; p.dev = h->P; p.bytes = h->n_total * sizeof(float);
+  StatePiece m; m.dev = h->Mo; m.bytes = h->n_train * sizeof(float);
+  StatePiece v; v.dev = h->Vo; v.bytes = h->n_train * sizeof(float);
+  std::vector<StatePiece> pp{p}, mm{m}, vv{v};
+  if (int rc = rd.read_pieces(2, pp)) return rc;
+  if (int rc = rd.read_pieces(3, mm)) return rc;
+  if (int rc = rd.read_pieces(4, vv)) return rc;
+  CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
+  CK(cudaMemset(h->r_done, 0, (size_t)h->E * sizeof(float)));
+  h->n_updates = hv[0];
+  h->t = 0;
+  h->broken = false;
+  return 0;
+}
+
+}  // extern "C"

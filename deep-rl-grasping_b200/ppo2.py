@@ -1,0 +1,440 @@
+"""``PPO2`` -- the PPO branch of the reference's training harness (/root/reference/manipulation_main/training/sb_helper.py:137-154,
+train_stable_baselines.py:99-100): stable-baselines 2.10.1 ``PPO2`` with ``common.policies.MlpPolicy`` and its defaults.  The
+rollout buffer, GAE and every minibatch step run on the GPU (csrc/ppo.cu); the algorithm is restated in oracle/ppo_ref.py.
+Import it as ``b200grasp.ppo2.PPO2`` (the stable-baselines path ``stable_baselines.ppo2.PPO2``).
+"""
+from __future__ import annotations
+
+import ctypes as C
+import os
+from collections import OrderedDict
+from typing import Optional
+
+import numpy as np
+
+from . import _lib, sb_io, training_state
+from .callbacks import as_callback
+from .learner import _f32, _fp
+from .vec_env import DummyVecEnv
+
+_SCOPE = "model/"
+
+
+class PPO2Learner:
+    """numpy-facing wrapper of one ``b2g_ppo`` handle (maps 1:1 onto the C ABI)."""
+
+    def __init__(self, obs_dim, n_actions, layers=(64, 64), n_envs=1, n_steps=128, nminibatches=4, noptepochs=4, gamma=0.99, lam=0.95,
+                 ent_coef=0.01, vf_coef=0.5, max_grad_norm=0.5, seed=0, device=0):
+        self.lib = _lib.load()
+        if len(layers) != 2:
+            raise NotImplementedError(f"layers={list(layers)}: the PPO2 learner builds two hidden layers")
+        cfg = _lib.PpoCfg(int(obs_dim), int(n_actions), int(layers[0]), int(layers[1]), int(n_envs), int(n_steps), int(nminibatches),
+                          int(noptepochs), float(gamma), float(lam), float(ent_coef), float(vf_coef), float(max_grad_norm),
+                          int(seed) & 0xFFFFFFFFFFFFFFFF, int(device))
+        self.h = C.c_void_p()
+        _lib.check(self.lib.b2g_ppo_create(C.byref(cfg), C.byref(self.h)))
+        self.obs_dim, self.n_actions, self.n_envs, self.n_steps = int(obs_dim), int(n_actions), int(n_envs), int(n_steps)
+        self.nminibatches, self.noptepochs = int(nminibatches), int(noptepochs)
+        self.n_batch = self.n_envs * self.n_steps
+        self.minibatch = self.n_batch // self.nminibatches
+        self._info = OrderedDict()
+        buf = C.create_string_buffer(256)
+        rows, cols, nd = C.c_int64(), C.c_int64(), C.c_int32()
+        for i in range(self.lib.b2g_ppo_param_count(self.h)):
+            _lib.check(self.lib.b2g_ppo_param_info(self.h, i, buf, 256, C.byref(rows), C.byref(cols), C.byref(nd)))
+            self._info[buf.value.decode()] = (rows.value, cols.value) if nd.value == 2 else (cols.value,)
+
+    def close(self):
+        if getattr(self, "h", None) is not None and self.h:
+            self.lib.b2g_ppo_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @property
+    def param_shapes(self):
+        return self._info
+
+    def get_parameters(self):
+        out = OrderedDict()
+        for n, shp in self._info.items():
+            a = np.empty(shp, np.float32)
+            _lib.check(self.lib.b2g_ppo_get_param(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
+            out[n] = a
+        return out
+
+    def load_parameters(self, params, exact_match=True):
+        seen = set()
+        for n, a in params.items():
+            key = n[:-2] if n.endswith(":0") else n
+            if key not in self._info:
+                if exact_match:
+                    raise ValueError(f"unknown variable {n}")
+                continue
+            a = _f32(a)
+            if tuple(a.shape) != self._info[key]:
+                raise ValueError(f"shape mismatch for {n}: {a.shape} vs {self._info[key]}")
+            _lib.check(self.lib.b2g_ppo_set_param(self.h, key.encode(), _fp(a.reshape(-1)), a.size))
+            seen.add(key)
+        if exact_match and seen != set(self._info):
+            raise ValueError(f"missing variables: {sorted(set(self._info) - seen)}")
+
+    def get_gradients(self):
+        """The last minibatch step's gradients after the global-norm clip (trained variables; q has none)."""
+        out = OrderedDict()
+        for n, shp in self._info.items():
+            if n.startswith(_SCOPE + "q/"):
+                continue
+            a = np.empty(shp, np.float32)
+            _lib.check(self.lib.b2g_ppo_get_grad(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
+            out[n] = a
+        return out
+
+    def rollout_act(self, obs):
+        """Rollout step: obs [n_envs, obs_dim] -> unclipped actions [n_envs, n_actions] (stored with values and neglogp)."""
+        obs = _f32(obs).reshape(self.n_envs, self.obs_dim)
+        out = np.empty((self.n_envs, self.n_actions), np.float32)
+        _lib.check(self.lib.b2g_ppo_rollout_act(self.h, _fp(obs), _fp(out)))
+        return out
+
+    def rollout_reward(self, rew, done):
+        _lib.check(self.lib.b2g_ppo_rollout_reward(self.h, _fp(_f32(np.reshape(rew, -1))), _fp(_f32(np.reshape(done, -1)))))
+
+    def rollout_reset(self):
+        _lib.check(self.lib.b2g_ppo_rollout_reset(self.h))
+
+    def rollout_get(self):
+        """advantages, returns, values, neglogp [n_steps, n_envs] and actions [n_steps, n_envs, n_actions] (time-major)."""
+        T, E = self.n_steps, self.n_envs
+        adv, ret, val, nlp = (np.empty((T, E), np.float32) for _ in range(4))
+        act = np.empty((T, E, self.n_actions), np.float32)
+        _lib.check(self.lib.b2g_ppo_rollout_get(self.h, _fp(adv), _fp(ret), _fp(val), _fp(nlp), _fp(act)))
+        return dict(advantages=adv, returns=ret, values=val, neglogp=nlp, actions=act)
+
+    def update(self, last_obs, perms, lr, cliprange, cliprange_vf):
+        """One update on a full rollout; perms [noptepochs, n_batch] are the epochs' permutations of the env-major batch."""
+        p = np.ascontiguousarray(perms, np.int32).reshape(-1)
+        assert p.size == self.noptepochs * self.n_batch
+        m = _lib.PpoMetrics()
+        _lib.check(self.lib.b2g_ppo_update(self.h, _fp(_f32(last_obs).reshape(self.n_envs, self.obs_dim)),
+                                           p.ctypes.data_as(C.POINTER(C.c_int32)), float(lr), float(cliprange), float(cliprange_vf),
+                                           C.byref(m)))
+        return m.as_dict()
+
+    def train_step_explicit(self, obs, returns, actions, values, neglogp, lr, cliprange, cliprange_vf, apply_update=True):
+        M = self.minibatch
+        m = _lib.PpoMetrics()
+        _lib.check(self.lib.b2g_ppo_train_step_explicit(
+            self.h, _fp(_f32(obs).reshape(M, self.obs_dim)), _fp(_f32(np.reshape(returns, -1))), _fp(_f32(actions).reshape(M, self.n_actions)),
+            _fp(_f32(np.reshape(values, -1))), _fp(_f32(np.reshape(neglogp, -1))), float(lr), float(cliprange), float(cliprange_vf),
+            int(bool(apply_update)), C.byref(m)))
+        return m.as_dict()
+
+    def act(self, obs, deterministic=True):
+        """-> actions [n, n_actions] (mean, or mean + std * noise of stream 1), values [n], neglogp [n]; nothing is stored."""
+        obs = _f32(obs).reshape(-1, self.obs_dim)
+        n = obs.shape[0]
+        a, v, nl = np.empty((n, self.n_actions), np.float32), np.empty(n, np.float32), np.empty(n, np.float32)
+        _lib.check(self.lib.b2g_ppo_act(self.h, _fp(obs), n, int(bool(deterministic)), _fp(a), _fp(v), _fp(nl)))
+        return a, v, nl
+
+    def steps(self):
+        """(Adam step, noise-stream step, rollout rows filled)"""
+        a, b, t = C.c_int64(), C.c_int64(), C.c_int32()
+        _lib.check(self.lib.b2g_ppo_get_step(self.h, C.byref(a), C.byref(b), C.byref(t)))
+        return a.value, b.value, t.value
+
+    def save_state(self, path: str):
+        _lib.check(self.lib.b2g_ppo_state_save(self.h, os.fsencode(path)))
+
+    def load_state(self, path: str):
+        _lib.check(self.lib.b2g_ppo_state_load(self.h, os.fsencode(path)))
+
+
+def _schedule(v):
+    """stable-baselines' get_schedule_fn: a callable of frac, or a constant."""
+    return v if callable(v) else (lambda _frac, _v=v: _v)
+
+
+def _check_policy(policy):
+    from .common.policies import MlpPolicy
+    if isinstance(policy, str):
+        if policy != "MlpPolicy":
+            raise NotImplementedError(f"policy '{policy}': only common.policies.MlpPolicy is built for PPO2")
+    elif policy is not MlpPolicy:
+        raise NotImplementedError(f"policy {getattr(policy, '__name__', policy)}: only common.policies.MlpPolicy is built for PPO2 "
+                                  "(CNN, recurrent and layer-norm policies are not)")
+
+
+def _check_policy_kwargs(policy_kwargs):
+    kw = dict(policy_kwargs or {})
+    unknown = set(kw) - {"layers", "net_arch", "act_fun", "feature_extraction", "layer_norm"}
+    if unknown:
+        raise NotImplementedError(f"policy_kwargs {sorted(unknown)} are not built for PPO2")
+    if kw.get("feature_extraction", "mlp") != "mlp":
+        raise NotImplementedError("feature_extraction: only the MLP extractor is built for PPO2")
+    if kw.get("layer_norm", False):
+        raise NotImplementedError("layer_norm=True: layer-normalised policies are not built")
+    act = kw.get("act_fun")
+    if act is not None and getattr(act, "__name__", str(act)) != "tanh":
+        raise NotImplementedError("act_fun: only tanh is built for PPO2")
+    layers = [int(x) for x in kw.get("layers", None) or [64, 64]]
+    if "net_arch" in kw and kw["net_arch"] is not None:
+        na = list(kw["net_arch"])
+        if len(na) != 1 or not isinstance(na[0], dict):
+            raise NotImplementedError(f"net_arch={na}: shared layers are not built; give net_arch=[dict(pi=[h0, h1], vf=[h0, h1])]")
+        pi, vf = [int(x) for x in na[0].get("pi", [])], [int(x) for x in na[0].get("vf", [])]
+        if pi != vf:
+            raise NotImplementedError(f"net_arch pi={pi} vf={vf}: the towers must have the same widths")
+        layers = pi
+    if len(layers) != 2:
+        raise NotImplementedError(f"layers={layers}: the PPO2 learner builds exactly two hidden layers")
+    return kw, layers
+
+
+class PPO2:
+    """stable-baselines 2.10 ``PPO2(policy, env, ...)`` with its signature and defaults, plus ``device``: ``learn / predict /
+    save / load / get_parameters / load_parameters / get_env / get_vec_normalize_env / close`` and
+    ``save_training_state / load_training_state``.  Box action spaces only, as the reference's configs give."""
+
+    def __init__(self, policy, env, gamma=0.99, n_steps=128, ent_coef=0.01, learning_rate=2.5e-4, vf_coef=0.5, max_grad_norm=0.5,
+                 lam=0.95, nminibatches=4, noptepochs=4, cliprange=0.2, cliprange_vf=None, verbose=0, tensorboard_log=None,
+                 _init_setup_model=True, policy_kwargs=None, full_tensorboard_log=False, seed=None, n_cpu_tf_sess=None, device=0,
+                 **unsupported):
+        if unsupported:
+            if "device_obs_norm" in unsupported:
+                raise NotImplementedError("device_obs_norm: PPO2 stores what a host VecNormalize returns, as stable-baselines does")
+            raise TypeError(f"PPO2 got unexpected keyword arguments {sorted(unsupported)}")
+        _check_policy(policy)
+        self.policy_kwargs, self.layers = _check_policy_kwargs(policy_kwargs)
+        self.gamma, self.n_steps, self.ent_coef, self.learning_rate = gamma, int(n_steps), ent_coef, learning_rate
+        self.vf_coef, self.max_grad_norm, self.lam = vf_coef, max_grad_norm, lam
+        self.nminibatches, self.noptepochs, self.cliprange, self.cliprange_vf = int(nminibatches), int(noptepochs), cliprange, cliprange_vf
+        self.verbose, self.tensorboard_log, self.seed, self.device = verbose, tensorboard_log, seed, device
+        self.num_timesteps = 0
+        self.n_envs = 1
+        self.learner: Optional[PPO2Learner] = None
+        self.env = None
+        self._vec_normalize_env = None
+        self._boundary = None           # (num_timesteps, numpy global state) after the last completed update
+        self.ep_info_buf = []
+        if env is not None:
+            self._set_env(env)
+            if _init_setup_model:
+                self.setup_model()
+
+    def _set_env(self, env):
+        env = env if hasattr(env, "num_envs") else DummyVecEnv([lambda: env])
+        if not hasattr(env.action_space, "low"):
+            raise NotImplementedError(f"PPO2 here needs a Box action space, got {env.action_space} (the reference's PPO branch is continuous)")
+        self.env, self.n_envs = env, int(env.num_envs)
+        self.observation_space, self.action_space = env.observation_space, env.action_space
+        self._vec_normalize_env = self.get_vec_normalize_env()
+        if (self.n_envs * self.n_steps) % self.nminibatches:
+            # ppo2.py's assertion: "The number of minibatches (nminibatches) is not a factor of the total number of samples"
+            raise ValueError(f"nminibatches={self.nminibatches} is not a factor of n_batch = n_envs * n_steps = {self.n_envs * self.n_steps}")
+
+    def setup_model(self):
+        obs_dim = int(np.prod(self.observation_space.shape))
+        A = int(np.prod(self.action_space.shape))
+        self.learner = PPO2Learner(obs_dim, A, tuple(self.layers), self.n_envs, self.n_steps, self.nminibatches, self.noptepochs,
+                                   self.gamma, self.lam, self.ent_coef, self.vf_coef, self.max_grad_norm, int(self.seed or 0), self.device)
+        self.learner.load_parameters(_init_params(obs_dim, A, self.layers, self.seed))
+
+    def close(self):
+        if self.learner is not None:
+            self.learner.close()
+            self.learner = None
+
+    def get_env(self):
+        return self.env
+
+    def get_vec_normalize_env(self):
+        from .sac_model import unwrap_vec_normalize
+        return unwrap_vec_normalize(self.env)
+
+    def learn(self, total_timesteps, callback=None, log_interval=1, tb_log_name="PPO2", reset_num_timesteps=True):
+        """stable-baselines 2.10 PPO2.learn: n_updates = total_timesteps // n_batch rollouts of n_steps steps (clipped actions to
+        the env, num_timesteps += n_envs, callback.on_step() False stops before the update), each followed by noptepochs epochs of
+        np.random.shuffle'd minibatches.  Every call starts from env.reset() with an empty rollout."""
+        callback = as_callback(callback)
+        callback.init_callback(self)
+        if reset_num_timesteps:
+            self.num_timesteps = 0
+        callback.on_training_start({"self": self, "writer": None}, globals())
+        lr_fn, clip_fn = _schedule(self.learning_rate), _schedule(self.cliprange)
+        cvf = self.cliprange_vf
+        cvf_fn = clip_fn if cvf is None else _schedule(cvf)
+        clip_vf_off = isinstance(cvf, (float, int)) and not isinstance(cvf, bool) and cvf < 0
+        L = self.learner
+        n_batch = self.n_envs * self.n_steps
+        n_updates = total_timesteps // n_batch
+        low, high = self.action_space.low.reshape(-1), self.action_space.high.reshape(-1)
+        obs = np.asarray(self.env.reset(), np.float32).reshape(self.n_envs, -1)
+        L.rollout_reset()
+        self.last_metrics = None
+        for update in range(1, n_updates + 1):
+            frac = 1.0 - (update - 1.0) / n_updates
+            lr_now, clip_now = lr_fn(frac), clip_fn(frac)
+            cvf_now = -1.0 if clip_vf_off else cvf_fn(frac)
+            callback.on_rollout_start()
+            stopped = False
+            for _ in range(self.n_steps):
+                actions = L.rollout_act(obs)
+                clipped = np.clip(actions, low, high)
+                new_obs, rew, done, infos = self.env.step(clipped.reshape((self.n_envs,) + tuple(self.action_space.shape)))
+                self.num_timesteps += self.n_envs
+                if callback.on_step() is False:
+                    stopped = True
+                    break
+                for info in infos or []:
+                    ep = info.get("episode") if isinstance(info, dict) else None
+                    if ep is not None:
+                        self.ep_info_buf.append(ep)
+                L.rollout_reward(np.asarray(rew, np.float32), np.asarray(done, np.float32))
+                obs = np.asarray(new_obs, np.float32).reshape(self.n_envs, -1)
+            callback.on_rollout_end()
+            if stopped:
+                L.rollout_reset()
+                break
+            inds = np.arange(n_batch)
+            perms = np.empty((self.noptepochs, n_batch), np.int32)
+            for e in range(self.noptepochs):
+                np.random.shuffle(inds)
+                perms[e] = inds
+            self.last_metrics = L.update(obs, perms, lr_now, clip_now, cvf_now)
+            self._boundary = (self.num_timesteps, np.random.get_state())
+            if self.verbose >= 1 and (update % log_interval == 0 or update == 1):
+                print(f"| ppo2 update {update}/{n_updates} | total_timesteps {self.num_timesteps} | "
+                      + " | ".join(f"{k} {v:.5g}" for k, v in self.last_metrics.items()))
+        callback.on_training_end()
+        return self
+
+    def predict(self, observation, state=None, mask=None, deterministic=False):
+        """The Gaussian mean (deterministic) or a sample of stream 1, clipped to the action space."""
+        obs = np.asarray(observation, np.float32)
+        single = obs.ndim == len(self.observation_space.shape)
+        a, _, _ = self.learner.act(obs.reshape(-1, self.learner.obs_dim), deterministic=deterministic)
+        a = np.clip(a, self.action_space.low.reshape(-1), self.action_space.high.reshape(-1))
+        a = a.reshape((-1,) + tuple(self.action_space.shape))
+        return (a[0] if single else a), None
+
+    def get_parameters(self):
+        return OrderedDict((n + ":0", a) for n, a in self.learner.get_parameters().items())
+
+    def load_parameters(self, load_path_or_dict, exact_match=True):
+        params = load_path_or_dict
+        if isinstance(params, str):
+            _, params = sb_io.load_sb_zip(params)
+        self.learner.load_parameters(params, exact_match=exact_match)
+
+    def _data(self):
+        return {"gamma": self.gamma, "n_steps": self.n_steps, "vf_coef": self.vf_coef, "ent_coef": self.ent_coef,
+                "max_grad_norm": self.max_grad_norm, "learning_rate": self.learning_rate, "lam": self.lam,
+                "nminibatches": self.nminibatches, "noptepochs": self.noptepochs, "cliprange": self.cliprange,
+                "cliprange_vf": self.cliprange_vf, "verbose": self.verbose, "n_envs": self.n_envs, "seed": self.seed,
+                "policy_kwargs": dict(self.policy_kwargs),
+                "observation_shape": list(self.observation_space.shape), "action_shape": list(self.action_space.shape),
+                "action_low": np.asarray(self.action_space.low).reshape(-1).tolist(),
+                "action_high": np.asarray(self.action_space.high).reshape(-1).tolist()}
+
+    def save(self, save_path, cloudpickle=False):
+        """A stable-baselines zip: ``data`` (hyper-parameters, JSON), ``parameter_list`` and ``parameters``."""
+        d = os.path.dirname(save_path)
+        if d:
+            os.makedirs(d, exist_ok=True)
+        data = self._data()
+        for k in ("learning_rate", "cliprange", "cliprange_vf"):
+            if callable(data[k]):
+                data[k] = None
+        sb_io.save_sb_zip(save_path, data, self.learner.get_parameters())
+
+    @classmethod
+    def load(cls, load_path, env=None, custom_objects=None, **kwargs):
+        """Reads a PPO2 zip: widths and sizes from the parameter shapes, hyper-parameters from ``data``."""
+        from .spaces import Box
+        if not os.path.exists(load_path) and os.path.exists(load_path + ".zip"):
+            load_path += ".zip"
+        data, params = sb_io.load_sb_zip(load_path)
+        w0, w1, wpi = params[_SCOPE + "pi_fc0/w"], params[_SCOPE + "pi_fc1/w"], params[_SCOPE + "pi/w"]
+        kw = {k: data[k] for k in ("gamma", "n_steps", "vf_coef", "ent_coef", "max_grad_norm", "learning_rate", "lam", "nminibatches",
+                                   "noptepochs", "cliprange", "cliprange_vf", "seed") if k in data and data[k] is not None}
+        if "cliprange_vf" in data and data["cliprange_vf"] is None:
+            kw["cliprange_vf"] = None
+        kw["policy_kwargs"] = dict(data.get("policy_kwargs") or {}, layers=[int(w0.shape[1]), int(w1.shape[1])])
+        kw.update(kwargs)
+        m = cls("MlpPolicy", None, _init_setup_model=False, **kw)
+        if env is not None:
+            m._set_env(env)
+        else:
+            A = int(wpi.shape[1])
+            m.observation_space = Box(-np.inf, np.inf, tuple(data.get("observation_shape") or (w0.shape[0],)))
+            m.action_space = Box(np.asarray(data.get("action_low", [-1.0] * A), np.float32), np.asarray(data.get("action_high", [1.0] * A), np.float32),
+                                 tuple(data.get("action_shape") or (A,)))
+            m.n_envs = 1
+            if (m.n_envs * m.n_steps) % m.nminibatches:
+                raise ValueError(f"nminibatches={m.nminibatches} is not a factor of n_batch = {m.n_steps}")
+        m.setup_model()
+        m.learner.load_parameters(params, exact_match=True)
+        return m
+
+    # ------------------------------------------------------------------ training state (training_state.py)
+    def _host_state(self):
+        for k in ("learning_rate", "cliprange", "cliprange_vf"):
+            if callable(getattr(self, k)):
+                raise NotImplementedError(f"save_training_state needs a constant {k}")
+        num, np_state = self._boundary if self._boundary is not None else (self.num_timesteps, np.random.get_state())
+        init = dict(gamma=self.gamma, n_steps=self.n_steps, ent_coef=self.ent_coef, learning_rate=self.learning_rate, vf_coef=self.vf_coef,
+                    max_grad_norm=self.max_grad_norm, lam=self.lam, nminibatches=self.nminibatches, noptepochs=self.noptepochs,
+                    cliprange=self.cliprange, cliprange_vf=self.cliprange_vf, verbose=self.verbose, policy_kwargs=self.policy_kwargs,
+                    seed=self.seed, device=self.device)
+        return {"algo": "PPO2", "init": init, "num_timesteps": int(num),
+                "np_random": [np_state[0], np.asarray(np_state[1]).tolist(), int(np_state[2]), int(np_state[3]), float(np_state[4])]}
+
+    def save_training_state(self, path):
+        """Writes directory ``path``: model.zip, learner.state (parameters, Adam moments, counters), vecnormalize.pkl and
+        host.json (num_timesteps and numpy's global generator at the last update boundary: a rollout in flight is not kept)."""
+        return training_state.save_training_state(self, path)
+
+    @classmethod
+    def load_training_state(cls, path, env, **kwargs):
+        """Rebuilds the model ``save_training_state`` wrote into ``path`` on ``env``; ``learn(n, reset_num_timesteps=False)``
+        then continues from the saved update boundary with a fresh episode."""
+        path = training_state.resolve(path)
+        host = training_state.read_host(path)
+        if host.get("algo") != "PPO2":
+            raise ValueError(f"{path} holds a {host.get('algo')} training state")
+        model = cls("MlpPolicy", env, **dict(host["init"], **kwargs))
+        training_state.restore_vec_normalize(path, model.env)
+        model.load_parameters(os.path.join(path, training_state.MODEL_FILE))
+        model.learner.load_state(os.path.join(path, training_state.STATE_FILE))
+        model.num_timesteps = int(host["num_timesteps"])
+        s = host["np_random"]
+        np.random.set_state((s[0], np.asarray(s[1], np.uint32), s[2], s[3], s[4]))
+        model._boundary = (model.num_timesteps, np.random.get_state())
+        return model
+
+
+def _init_params(obs_dim, n_actions, layers, seed):
+    """common/tf_layers.py ortho_init in the variables' creation order: the orthogonal factor of an SVD of a standard normal
+    matrix, scaled sqrt(2) for the hidden layers, 1 for vf, 0.01 for pi and q; zero biases and logstd.  The normal draws come
+    from a generator seeded with ``seed``."""
+    rng = np.random.default_rng(seed)
+    h0, h1 = layers
+    p = OrderedDict()
+    for name, shape in (("pi_fc0/w", (obs_dim, h0)), ("pi_fc0/b", (h0,)), ("vf_fc0/w", (obs_dim, h0)), ("vf_fc0/b", (h0,)),
+                        ("pi_fc1/w", (h0, h1)), ("pi_fc1/b", (h1,)), ("vf_fc1/w", (h0, h1)), ("vf_fc1/b", (h1,)), ("vf/w", (h1, 1)),
+                        ("vf/b", (1,)), ("pi/w", (h1, n_actions)), ("pi/b", (n_actions,)), ("pi/logstd", (1, n_actions)),
+                        ("q/w", (h1, n_actions)), ("q/b", (n_actions,))):
+        if name == "pi/logstd" or len(shape) == 1:
+            p[_SCOPE + name] = np.zeros(shape, np.float32)
+            continue
+        scale = 1.0 if name == "vf/w" else (0.01 if name in ("pi/w", "q/w") else np.sqrt(2.0))
+        u, _, v = np.linalg.svd(rng.normal(0.0, 1.0, shape), full_matrices=False)
+        w = u if u.shape == shape else v
+        p[_SCOPE + name] = (scale * w.reshape(shape)).astype(np.float32)
+    return p

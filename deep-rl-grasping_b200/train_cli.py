@@ -2,7 +2,7 @@
 
 Mirrors /root/reference/manipulation_main/training/train_stable_baselines.py:26-148 (same sub-commands, flags,
 ``model_dir`` layout: ``config.yaml``, ``best_model/``, ``logs/rl_model_*`` checkpoints, ``vecnormalize.pkl``,
-``log_file.monitor.csv``) and the SAC / DQN / BDQ branches of ``SBPolicy.learn`` (sb_helper.py:69-128,155-165,175-247).  The
+``log_file.monitor.csv``) and the SAC / PPO / DQN / BDQ branches of ``SBPolicy.learn`` (sb_helper.py:69-128,137-165,175-247).  The
 environment itself stays the reference's (PyBullet on host cores): ``--env module:callable`` names a factory
 ``f(config, evaluate=False, validate=False, test=False) -> gym.Env``; the default imports the reference package and
 calls ``gym.make('gripper-env-v0', ...)`` exactly like the original script.
@@ -25,6 +25,8 @@ from .bench import Monitor
 from .callbacks import BaseCallback, CheckpointCallback, EvalCallback, TrainingStateCallback
 from .deepq import DQN
 from .deepq.policies import MlpPolicy as DQNMlpPolicy
+from .common.policies import MlpPolicy as PPOMlpPolicy
+from .ppo2 import PPO2
 from .sac_model import CnnPolicy, MlpPolicy
 from .vec_env import DummyVecEnv, SubprocVecEnv, VecNormalize
 
@@ -75,6 +77,11 @@ def train(args):
             raise ValueError("--algo DQN: DQN cannot be used with more than one environment (--n_envs 1)")
         if args.device_norm:
             raise NotImplementedError("--algo DQN: --device_norm is built for SAC and BDQ only")
+    if algo == "PPO":          # PPO2 stores what the host VecNormalize returns, as stable-baselines does
+        if args.device_norm:
+            raise NotImplementedError("--algo PPO: --device_norm is built for SAC and BDQ only")
+        if args.load_dir:
+            raise NotImplementedError("--algo PPO: --load_dir is not read by the reference's PPO branch (sb_helper.py:137-154)")
     os.mkdir(args.model_dir)                                   # like the reference: refuses to overwrite a run
     os.mkdir(os.path.join(args.model_dir, "best_model"))
     if args.simple:
@@ -145,8 +152,11 @@ def train(args):
             old = DQN.load(args.load_dir)
             model.load_parameters(old.get_parameters())
             old.close()
+    elif algo == "PPO":
+        model = PPO2(PPOMlpPolicy, env, **ppo_kwargs(config))
     else:
-        raise NotImplementedError(f"--algo {algo}: the H100 learner builds the SAC, DQN and BDQ branches of SBPolicy.learn (sb_helper.py:85-226)")
+        raise NotImplementedError(f"--algo {algo}: the H100 learner builds the SAC, PPO, DQN and BDQ branches of SBPolicy.learn "
+                                  "(sb_helper.py:85-226)")
     if args.state_freq:
         callbacks.append(TrainingStateCallback(args.state_freq, os.path.join(args.model_dir, STATE_DIR)))
         _learn_keeping_state(model, int(c["total_timesteps"]), callbacks, os.path.join(args.model_dir, STATE_DIR))
@@ -171,6 +181,14 @@ def dqn_kwargs(config):
     return dict(verbose=2, gamma=config["discount_factor"], batch_size=c["batch_size"], prioritized_replay=c["prioritized_replay"])
 
 
+def ppo_kwargs(config):
+    """sb_helper.py:149-154: only gamma (discount_factor) and the PPO learning_rate come from the config, with verbose=2; every
+    other PPO2 setting stays at stable-baselines' default.  The config's PPO ``layers`` and ``n_steps`` are not passed there,
+    and the policy_kwargs sb_helper computes for image observations are dropped before the call, so the policy is always
+    MlpPolicy with [64, 64]."""
+    return dict(verbose=2, gamma=config["discount_factor"], learning_rate=config["PPO"]["learning_rate"])
+
+
 def _learn_keeping_state(model, total_timesteps, callbacks, state_dir, reset_num_timesteps=True):
     """model.learn; an interrupt (Ctrl-C) writes the training state before the run ends, as sb_helper.py:178-181 does
     for the model."""
@@ -186,7 +204,7 @@ def resume(args):
     model_dir = args.resume
     config = yaml.safe_load(open(os.path.join(model_dir, "config.yaml")))
     algo = config["algorithm"].upper()
-    if algo not in ("SAC", "BDQ", "DQN"):
+    if algo not in ("SAC", "BDQ", "DQN", "PPO"):
         raise NotImplementedError(f"--resume: algorithm '{algo}' has no training state")
     state_dir = training_state.resolve(os.path.join(model_dir, STATE_DIR))
     done = int(training_state.read_host(state_dir)["num_timesteps"])
@@ -209,7 +227,7 @@ def resume(args):
     ]
     if args.state_freq:
         callbacks.append(TrainingStateCallback(args.state_freq, os.path.join(model_dir, STATE_DIR)))
-    model = {"SAC": SAC, "BDQ": BDQ, "DQN": DQN}[algo].load_training_state(state_dir, env)
+    model = {"SAC": SAC, "BDQ": BDQ, "DQN": DQN, "PPO": PPO2}[algo].load_training_state(state_dir, env)
     remaining = int(config[algo]["total_timesteps"]) - model.num_timesteps
     if remaining > 0:
         _learn_keeping_state(model, remaining, callbacks, os.path.join(model_dir, STATE_DIR), reset_num_timesteps=False)
@@ -260,8 +278,10 @@ def run(args):
         agent = BDQ.load(args.model)
     elif algo == "dqn":
         agent = DQN.load(args.model)
+    elif algo == "ppo":
+        agent = PPO2.load(args.model)
     else:
-        raise NotImplementedError(f"algorithm '{algo}': only sac / dqn / bdq zips run on the H100 learner")
+        raise NotImplementedError(f"algorithm '{algo}': only sac / ppo / dqn / bdq zips run on the H100 learner")
     print("Run the agent")
     out = run_agent(task, agent, args.stochastic, n_episodes=args.episodes)
     task.close()

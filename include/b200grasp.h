@@ -402,6 +402,73 @@ int b2g_dqn_act(b2g_dqn* h, const float* obs, int n, int32_t* act_out, float* q_
 int b2g_dqn_state_save(b2g_dqn* h, const char* path);
 int b2g_dqn_state_load(b2g_dqn* h, const char* path);
 
+/* ------------------------------------------------------------------------------------------------
+ * PPO2 learner -- the `sb.PPO2` object of sb_helper.py:137-154 (stable-baselines 2.10.1 ppo2 with common.policies.MlpPolicy,
+ * restated in oracle/ppo_ref.py).  Variables model/{pi_fc0,vf_fc0,pi_fc1,vf_fc1,vf,pi}/{w,b}, model/pi/logstd [1, A] and the
+ * untrained head model/q/{w,b}: two tanh towers obs -> hidden0 -> hidden1, a diagonal Gaussian (mean pi, state-independent
+ * logstd) and the value vf.  The rollout lives on the device: b2g_ppo_rollout_act / _reward fill n_steps rows of n_envs
+ * environments, b2g_ppo_update runs GAE and noptepochs x nminibatches clipped-surrogate minibatch steps (global-norm gradient
+ * clip, TF1 Adam with epsilon 1e-5) in the caller's permutation, as one CUDA graph.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct b2g_ppo b2g_ppo;
+typedef struct b2g_ppo_cfg {
+  int32_t obs_dim;             /* flattened observation (float32, no scaling): [1, 65536]                            */
+  int32_t n_actions;           /* Box action size: [1, 16]                                                            */
+  int32_t hidden0, hidden1;    /* net_arch pi = vf = [hidden0, hidden1]: multiples of 4 in [4, 256] ([64, 64] default)  */
+  int32_t n_envs;              /* [1, 4096]                                                                           */
+  int32_t n_steps;             /* rollout length per env (128 default)                                                */
+  int32_t nminibatches;        /* divides n_batch = n_steps * n_envs; minibatch n_batch / nminibatches <= 16384       */
+  int32_t noptepochs;          /* noptepochs * nminibatches <= 4096                                                   */
+  float gamma, lam;            /* discount and GAE lambda (0.99, 0.95)                                                */
+  float ent_coef, vf_coef;     /* 0.01, 0.5                                                                           */
+  float max_grad_norm;         /* tf.clip_by_global_norm bound (0.5)                                                  */
+  uint64_t seed;               /* the actor's noise key is seed ^ 0xA5A5A5A5DEADBEEF (Philox stream 1)               */
+  int32_t device;
+} b2g_ppo_cfg;
+typedef struct b2g_ppo_metrics {
+  float policy_loss, value_loss, entropy, approxkl, clipfrac;   /* ppo2.py's logged losses (update: mean over minibatches) */
+  float grad_norm;             /* global L2 norm of the gradient before the clip                                      */
+  int64_t n_updates;           /* minibatch steps applied so far                                                      */
+} b2g_ppo_metrics;
+
+/* B2G_EINVAL naming the limit outside the ranges above */
+int b2g_ppo_create(const b2g_ppo_cfg* cfg, b2g_ppo** out);
+int b2g_ppo_destroy(b2g_ppo* h);
+/* the 15 variables in the zip's order (model/ prefix); q/w and q/b are never updated */
+int b2g_ppo_param_count(const b2g_ppo* h);
+int b2g_ppo_param_info(const b2g_ppo* h, int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim);
+int b2g_ppo_get_param(b2g_ppo* h, const char* name, float* dst, size_t numel);
+int b2g_ppo_set_param(b2g_ppo* h, const char* name, const float* src, size_t numel);
+/* the gradient of the last minibatch step after the global-norm clip (trained variables only) */
+int b2g_ppo_get_grad(b2g_ppo* h, const char* name, float* dst, size_t numel);
+/* rollout step t: obs [n_envs, obs_dim] -> row t; act_out [n_envs, n_actions] = mean + exp(logstd) * eps, unclipped (the
+ * caller clips for the env); action, value and neglogp stay in row t.  B2G_ESTATE when n_steps rows are filled. */
+int b2g_ppo_rollout_act(b2g_ppo* h, const float* obs, float* act_out);
+/* rewards [n_envs] of step t and the episode-start flags of step t + 1 (the env's done flags) */
+int b2g_ppo_rollout_reward(b2g_ppo* h, const float* rew, const float* done);
+/* empty rollout, episode-start flags cleared (a fresh episode) */
+int b2g_ppo_rollout_reset(b2g_ppo* h);
+/* [n_steps, n_envs] (time-major) advantages and returns of the last update's GAE, values, neglogp, actions [.., n_actions];
+ * any pointer may be NULL */
+int b2g_ppo_rollout_get(b2g_ppo* h, float* adv, float* ret, float* val, float* nlp, float* act);
+/* one update on a full rollout: last_obs [n_envs, obs_dim] bootstraps the GAE; perm [noptepochs * n_batch] holds each epoch's
+ * permutation of the env-major flattened batch; cliprange_vf < 0 turns value clipping off.  out: means over the minibatches. */
+int b2g_ppo_update(b2g_ppo* h, const float* last_obs, const int32_t* perm, float lr, float cliprange, float cliprange_vf,
+                   b2g_ppo_metrics* out);
+/* parity entry point: one minibatch [n_batch / nminibatches] supplied by the caller (advantages = returns - values) */
+int b2g_ppo_train_step_explicit(b2g_ppo* h, const float* obs, const float* returns, const float* actions, const float* values,
+                                const float* neglogp, float lr, float cliprange, float cliprange_vf, int apply_update,
+                                b2g_ppo_metrics* out);
+/* predict: n observations -> mean (deterministic) or mean + std * eps (stream 1, advancing the same counter as the rollout);
+ * nothing is written to the rollout.  value_out / neglogp_out may be NULL. */
+int b2g_ppo_act(b2g_ppo* h, const float* obs, int n, int deterministic, float* act_out, float* value_out, float* neglogp_out);
+/* Adam step, stream-1 step counter, rollout rows filled */
+int b2g_ppo_get_step(b2g_ppo* h, int64_t* adam_step, int64_t* noise_step, int32_t* rollout_rows);
+/* training state at an update boundary: parameters (q included), Adam moments, counters, n_updates.  A load empties the
+ * rollout and clears the episode-start flags. */
+int b2g_ppo_state_save(b2g_ppo* h, const char* path);
+int b2g_ppo_state_load(b2g_ppo* h, const char* path);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Row a12: auto-encoder ENCODER forward (perception for the `encoded depth` observation, SURVEY.md section 8).
  * Replaces SimpleAutoEncoder.encode  (/root/reference/manipulation_main/gripperEnv/encoders.py:59-61; graph :87-108)
