@@ -149,7 +149,7 @@ struct TailArgs {
   float* pi_out;                               // [B,A]
   float* metrics;                              // accumulators (see MET_* in sac.cu)
 };
-cudaError_t tail_launch(const TailArgs& a, cudaStream_t s);
+cudaError_t tail_launch(const TailArgs& a, cudaStream_t s, bool pdl);   // pdl: may start while its predecessor drains
 
 // Weight gradients of the head MLPs (fc0 / fc1 kernels and biases of pi, vf, qf1, qf2) in fp32 on the CUDA cores: 76 MFLOP
 // of [B]-deep reductions, too small for a tensor-engine launch (which would also hold every SM while it runs).

@@ -164,52 +164,74 @@ struct Plane2Job {
   int tile_start;
 };
 
-// 64 (r) x 32 (n) source tile per CTA.  Loads are float4 along n; the transposed copy is written as 16-byte runs of 8
-// consecutive r values per plane (the 2-byte scattered stores of the first version made this the longest leaf kernel).
-__global__ void __launch_bounds__(256) planes2_kernel(const Plane2Job* __restrict__ jobs, const int* __restrict__ cta_job) {
-  __shared__ float tile[64][33];
+// 64 (r) x 32 P2_SUB (n) source strip per CTA, as P2_SUB sub-tiles of 64 x 32 whose loads are all in flight before the first
+// is used: about 30 MB move per step, and 64 x 32 tiles (2 float4 loads per thread) left it latency-bound at under 1 TB/s.
+// Loads are float4 along n; the transposed copy is written as 16-byte runs of 8 consecutive r values per plane (the 2-byte
+// scattered stores of the first version made this the longest leaf kernel).  CTA cta0 + blockIdx.x of the job table.  Jobs
+// narrower than the strip (conv1: N = 32; fc0 at H = 64; conv2 / conv3: N = 64) leave sub-tiles idle: bounds-checked, no loads.
+constexpr int P2_SUB = 4;
+__global__ void __launch_bounds__(256) planes2_kernel(const Plane2Job* __restrict__ jobs, const int* __restrict__ cta_job, int cta0) {
+  __shared__ float tile[P2_SUB][64][33];
   // (the job of a CTA comes from a table: walking the job list cost up to 30 DEPENDENT global loads before the first useful one)
-  const Plane2Job job = jobs[cta_job[blockIdx.x]];
-  const int t = blockIdx.x - job.tile_start;
-  const int tiles_n = (job.N + 31) / 32;
-  const int r0 = (t / tiles_n) * 64, n0 = (t % tiles_n) * 32;
+  const int cta = cta0 + blockIdx.x;
+  const Plane2Job job = jobs[cta_job[cta]];
+  const int t = cta - job.tile_start;
+  const int strips_n = (job.N + 32 * P2_SUB - 1) / (32 * P2_SUB);
+  const int r0 = (t / strips_n) * 64, nb = (t % strips_n) * 32 * P2_SUB;
   const int tid = threadIdx.x;
-  // ---- load 64 x 32 (8 float4 per row, 2 passes of 32 rows)
+  // ---- load P2_SUB x (64 x 32): 8 float4 per row of a sub-tile, 2 passes of 32 rows
   const bool vec_ok = (job.N & 3) == 0;
-  for (int i = tid; i < 64 * 8; i += 256) {
-    const int rr = i >> 3, c4 = i & 7, r = r0 + rr, n = n0 + 4 * c4;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (r < job.R) {
-      const float* sp = job.src + (size_t)r * job.N + n;
-      if (vec_ok && n + 3 < job.N) v = *reinterpret_cast<const float4*>(sp);
-      else { if (n < job.N) v.x = sp[0]; if (n + 1 < job.N) v.y = sp[1]; if (n + 2 < job.N) v.z = sp[2]; if (n + 3 < job.N) v.w = sp[3]; }
-    }
-    tile[rr][4 * c4] = v.x; tile[rr][4 * c4 + 1] = v.y; tile[rr][4 * c4 + 2] = v.z; tile[rr][4 * c4 + 3] = v.w;
-    if (!job.transpose && r < job.R) {      // natural layout: dst[r * ld + off0 + n], 8-byte runs of 4
-      const float x[4] = {v.x, v.y, v.z, v.w};
-      uint16_t p[3][4];
+  float4 v[P2_SUB][2];
 #pragma unroll
-      for (int u = 0; u < 4; ++u) split3(x[u], p[0][u], p[1][u], p[2][u]);
-      for (int k = 0; k < job.np; ++k) {
-        uint16_t* d = job.dst[k] + (size_t)r * job.ld + job.off0 + n;
-        if (n + 3 < job.N && (((size_t)r * job.ld + job.off0 + n) & 3) == 0)
-          *reinterpret_cast<uint2*>(d) = make_uint2((uint32_t)p[k][0] | ((uint32_t)p[k][1] << 16), (uint32_t)p[k][2] | ((uint32_t)p[k][3] << 16));
-        else
-          for (int u = 0; u < 4; ++u) if (n + u < job.N) d[u] = p[k][u];
+  for (int q = 0; q < P2_SUB; ++q)
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int i = tid + 256 * j, r = r0 + (i >> 3), n = nb + 32 * q + 4 * (i & 7);
+      v[q][j] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (r < job.R && n < job.N) {
+        const float* sp = job.src + (size_t)r * job.N + n;
+        if (vec_ok && n + 3 < job.N) v[q][j] = *reinterpret_cast<const float4*>(sp);
+        else { v[q][j].x = sp[0]; if (n + 1 < job.N) v[q][j].y = sp[1]; if (n + 2 < job.N) v[q][j].z = sp[2]; if (n + 3 < job.N) v[q][j].w = sp[3]; }
       }
     }
-  }
+#pragma unroll
+  for (int q = 0; q < P2_SUB; ++q)
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int i = tid + 256 * j, rr = i >> 3, c4 = i & 7, r = r0 + rr, n = nb + 32 * q + 4 * c4;
+      if (job.transpose) {
+        tile[q][rr][4 * c4] = v[q][j].x; tile[q][rr][4 * c4 + 1] = v[q][j].y; tile[q][rr][4 * c4 + 2] = v[q][j].z; tile[q][rr][4 * c4 + 3] = v[q][j].w;
+      } else if (r < job.R && n < job.N) {      // natural layout: dst[r * ld + off0 + n], 8-byte runs of 4
+        const float x[4] = {v[q][j].x, v[q][j].y, v[q][j].z, v[q][j].w};
+        uint16_t p[3][4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) split3(x[u], p[0][u], p[1][u], p[2][u]);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {          // (a constant trip count keeps p[] and job.dst[] in registers)
+          if (k == job.np) break;
+          uint16_t* d = job.dst[k] + (size_t)r * job.ld + job.off0 + n;
+          if (n + 3 < job.N && (((size_t)r * job.ld + job.off0 + n) & 3) == 0)
+            *reinterpret_cast<uint2*>(d) = make_uint2((uint32_t)p[k][0] | ((uint32_t)p[k][1] << 16), (uint32_t)p[k][2] | ((uint32_t)p[k][3] << 16));
+          else
+            for (int u = 0; u < 4; ++u) if (n + u < job.N) d[u] = p[k][u];
+        }
+      }
+    }
   if (!job.transpose) return;
   __syncthreads();
-  // ---- transposed copy: dst[(n + off0) * ld + r]; thread = (n, group of 8 r)
-  {
-    const int nn = tid >> 3, g8 = tid & 7, n = n0 + nn, rb = r0 + 8 * g8;
+  // ---- transposed copy: dst[(n + off0) * ld + r]; thread = (n, group of 8 r) of every sub-tile
+  const int nn = tid >> 3, g8 = tid & 7, rb = r0 + 8 * g8;
+#pragma unroll
+  for (int q = 0; q < P2_SUB; ++q) {
+    const int n = nb + 32 * q + nn;
     if (n < job.N && rb < job.R) {
       uint16_t p[3][8];
 #pragma unroll
-      for (int u = 0; u < 8; ++u) split3(tile[8 * g8 + u][nn], p[0][u], p[1][u], p[2][u]);
+      for (int u = 0; u < 8; ++u) split3(tile[q][8 * g8 + u][nn], p[0][u], p[1][u], p[2][u]);
       const size_t o = (size_t)(n + job.off0) * job.ld + rb;
-      for (int k = 0; k < job.np; ++k) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        if (k == job.np) break;
         uint16_t* d = job.dst[k] + o;
         if (job.k1_ci) {
           for (int u = 0; u < 8; ++u) if (rb + u < job.R) d[conv1_krow(rb + u, job.k1_ci) - rb] = p[k][u];
@@ -457,7 +479,7 @@ int v2_create(b2g_sac* h) {
     Plane2Job j{};
     j.src = src; j.R = R; j.N = N; j.np = np; j.transpose = transpose; j.ld = ld; j.off0 = off0; j.tile_start = start;
     for (int k = 0; k < np; ++k) j.dst[k] = dst[k];
-    start += ((R + 63) / 64) * ((N + 31) / 32);
+    start += ((R + 63) / 64) * ((N + 32 * P2_SUB - 1) / (32 * P2_SUB));
     jobs.push_back(j);
   };
   add_job(h->p("model/pi/cnn1/w"), 64 * Ci, 32, v.W1T[0], 3, 1, K1, 0);
@@ -476,6 +498,7 @@ int v2_create(b2g_sac* h) {
   add_job(h->p("model/values_fn/qf1/fc0/kernel"), h->feat_dim + h->A, H, v.K0T[1], 3, 1, KF, H);
   add_job(h->p("model/values_fn/qf2/fc0/kernel"), h->feat_dim + h->A, H, v.K0T[1], 3, 1, KF, 2 * H);
   add_job(h->p("target/values_fn/vf/fc0/kernel"), h->feat_dim, H, v.K0T[2], 3, 1, KF, 0);
+  v.plane_ctas_fwd = start;      // the forward-layout jobs above, then the backward layouts (first read by bwd_fused)
   for (int n = 0; n < 2; ++n) {
     add_job(h->p(std::string(nets[n]) + "/cnn2/w"), 512, 64, v.W2n[n], 2, 0, 64, 0);
     add_job(h->p(std::string(nets[n]) + "/cnn3/w"), 576, 64, v.W3n[n], 2, 0, 64, 0);
@@ -918,9 +941,10 @@ int v2_create(b2g_sac* h) {
 }
 
 // ================================================================================================ step pieces
-int v2_planes(b2g_sac* h, cudaStream_t s) {
+int v2_planes(b2g_sac* h, bool backward, cudaStream_t s) {
   V2State& v = h->v2;
-  planes2_kernel<<<v.plane_ctas, 256, 0, s>>>((const Plane2Job*)v.plane_jobs, v.plane_cta_job);
+  const int cta0 = backward ? v.plane_ctas_fwd : 0, n = backward ? v.plane_ctas - v.plane_ctas_fwd : v.plane_ctas_fwd;
+  planes2_kernel<<<n, 256, 0, s>>>((const Plane2Job*)v.plane_jobs, v.plane_cta_job, cta0);
   return 0;
 }
 

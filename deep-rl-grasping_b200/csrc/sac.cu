@@ -684,38 +684,50 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
   };
   mark("begin");
   PrepArgs pa = make_prep(h, h->cfg.seed + 0x9E3779B97F4A7C15ull * (unsigned long long)h->cfg.rank, sampled, apply);
-  // Leaf work runs on a second stream (parallel branches once captured in the step graph): zeroing the gradient
-  // arena and refreshing the BF16 weight planes overlap prep + gather; heads_wgrad and the bias column sums overlap
-  // the dgrad chain.  Profiling (per-launch events) keeps everything serial on one stream.
+  // Leaf work runs on two more streams (parallel branches once captured in the step graph).  The fused launches run one
+  // CTA per SM, each owning tiles near the head of its chain, so a leaf CTA still resident when one of them starts holds up
+  // that whole chain: the leaf work goes where no fused launch starts.  Beside the gather, joined before fwd_fused: the
+  // forward-layout weight planes and the z0 / dependency-counter zeroing (aux), the bookkeeping kernel (Adam step sizes,
+  // policy noise, metric accumulators) and the gradient zeroing (aux2).  The planes get SMs only as the gather's CTAs
+  // retire, so fwd_fused starts about 11 us after the gather ends (DESIGN §6).  Alongside the tail: the backward-layout
+  // weight planes, joined before bwd_fused.  heads_wgrad forks after the tail and runs in the backward launch's drain.
+  // Profiling (per-launch events) keeps everything serial on one stream.
   const bool fork = h->fork_leaves && !(prof && prof->on);
   cudaStream_t ax = fork ? h->aux : s;
   GatherArgs ga = make_gather(h, sampled, true);
   if (fork) {
-    // aux branch: weight planes (needed by conv1_fwd), then the bookkeeping kernel (Adam step sizes, policy noise,
-    // metric accumulators) and the gradient zeroing (needed from the tail on).  The gather draws its replay slots
-    // in-kernel from the same Philox stream, so the critical chain starts with the gather itself.
+    // the gather draws its replay slots in-kernel from prep's Philox stream, so the critical chain starts with the gather
     pa.defer_bump = 1; pa.skip_indices = 1;
     if (sampled) { ga.indices = nullptr; ga.rng_counters = h->counters; ga.seed = pa.seed; ga.indices_out = h->indices; }
     CK(cudaEventRecord(h->ev_aux[0], s));
     CK(cudaStreamWaitEvent(ax, h->ev_aux[0], 0));
+    CK(cudaStreamWaitEvent(h->aux2, h->ev_aux[0], 0));
     if (h->use_planes && !h->v2.on) { planes_launch(h->d_jobs, h->n_jobs, h->job_tiles, ax); ++n; }
-    if (h->v2.on) { if (int rc = v2_planes(h, ax)) return rc; ++n; }
+    if (h->v2.on) { if (int rc = v2_planes(h, false, ax)) return rc; ++n; }
     CK(cudaMemsetAsync(h->z0[0], 0, (size_t)5 * h->B * h->H * sizeof(float), ax)); ++n_copy;
-    if (h->v2.on) { CK(cudaMemsetAsync(h->v2.z0v, 0, (size_t)3 * h->B * h->H * sizeof(float), ax)); ++n_copy; }
+    if (h->v2.on) {
+      CK(cudaMemsetAsync(h->v2.z0v, 0, (size_t)3 * h->B * h->H * sizeof(float), ax)); ++n_copy;
+      CK(cudaMemsetAsync(h->v2.dep_ctr, 0, (size_t)h->v2.n_dep_ctr * sizeof(int), ax)); ++n_copy;
+    }
     CK(cudaEventRecord(h->ev_aux[1], ax));
-    prep_launch(pa, ax); ++n;
-    CK(cudaMemsetAsync(h->G, 0, (size_t)(h->n_train + MET_COUNT) * sizeof(float), ax)); ++n_copy;
-    CK(cudaEventRecord(h->ev_aux[6], ax));
+    prep_launch(pa, h->aux2); ++n;
+    CK(cudaMemsetAsync(h->G, 0, (size_t)(h->n_train + MET_COUNT) * sizeof(float), h->aux2)); ++n_copy;
+    CK(cudaEventRecord(h->ev_aux[6], h->aux2));
   } else {
     prep_launch(pa, s); ++n; mark("prep");
   }
   if (h->v2.on) {
-    if (!fork) { if (int rc = v2_planes(h, s)) return rc; ++n; mark("weight_planes_v2"); }
+    if (!fork) {
+      if (int rc = v2_planes(h, false, s)) return rc;
+      ++n; mark("weight_planes_fwd");
+      if (int rc = v2_planes(h, true, s)) return rc;
+      ++n; mark("weight_planes_bwd");
+    }
     if (int rc = v2_gather(h, ga, s)) return rc;
   } else gather_launch(ga, s);
   ++n; mark("gather_normalize");
   if (h->record_after_gather) CK(cudaEventRecord(h->record_after_gather, s));   // staged batch consumed
-  if (fork) CK(cudaStreamWaitEvent(s, h->ev_aux[1], 0));
+  if (fork) { CK(cudaStreamWaitEvent(s, h->ev_aux[1], 0)); CK(cudaStreamWaitEvent(s, h->ev_aux[6], 0)); }
   else {
     CK(cudaMemsetAsync(h->G, 0, (size_t)(h->n_train + MET_COUNT) * sizeof(float), s)); ++n_copy;
     CK(cudaMemsetAsync(h->z0[0], 0, (size_t)5 * h->B * h->H * sizeof(float), s)); ++n_copy;
@@ -730,14 +742,21 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
     return 0;
   };
   if (h->v2.on) {
-    CK(cudaMemsetAsync(h->v2.dep_ctr, 0, (size_t)h->v2.n_dep_ctr * sizeof(int), s)); ++n_copy;
+    if (!fork) { CK(cudaMemsetAsync(h->v2.dep_ctr, 0, (size_t)h->v2.n_dep_ctr * sizeof(int), s)); ++n_copy; }
     if (int rc = v2_launch(h, h->v2.fwd_fused[0], s)) return rc;
     ++n; mark("fwd_fused");
   } else {
     for (auto& g : h->fwd_groups) if (int rc = run_group(g, s)) return rc;
   }
-  if (fork) CK(cudaStreamWaitEvent(s, h->ev_aux[6], 0));
-  CK(tail_launch(make_tail(h, want_per_sample), s)); ++n; mark("heads_tail");
+  if (fork && h->v2.on) {     // the tail does not read the backward-layout planes
+    CK(cudaEventRecord(h->ev_aux[7], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[7], 0));
+    if (int rc = v2_planes(h, true, ax)) return rc;
+    ++n;
+    CK(cudaEventRecord(h->ev_aux[8], ax));
+  }
+  // Not launched early behind fwd_fused: its CTAs would land on the few SMs the draining persistent grid has freed, several
+  // per SM, and the latency-bound tail then ended 30 us after fwd_fused instead of 18 (H100, B = 256).
+  CK(tail_launch(make_tail(h, want_per_sample), s, pdl_enabled() && !h->v2.on)); ++n; mark("heads_tail");
   auto make_optim = [&]() {
     OptimArgs oa{};
     oa.P = h->P; oa.Mo = h->Mo; oa.Vo = h->Vo; oa.G = h->G; oa.T = h->P + h->n_train;
@@ -762,7 +781,13 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
     // on the leaf branch.
     h->v2.sm_reserve = 0;
     cudaStream_t lx = fork ? ax : s;
-    if (fork) { CK(cudaEventRecord(h->ev_aux[2], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[2], 0)); }
+    // heads_wgrad forks from the same point bwd_fused depends on.  It stays off bwd_fused's start because bwd_fused is launched
+    // early (programmatic dependent launch) behind the tail and holds every SM before heads_wgrad is ready; with B2G_PDL=0
+    // the two become ready together and heads_wgrad CTAs can be resident when bwd_fused places its CTAs.
+    if (fork) {
+      CK(cudaStreamWaitEvent(s, h->ev_aux[8], 0));    // the backward-layout planes, read from bwd_fused's first tiles on
+      CK(cudaEventRecord(h->ev_aux[2], s)); CK(cudaStreamWaitEvent(ax, h->ev_aux[2], 0));
+    }
     HeadsWgradArgs wa{};
     const char* hp[4] = {"model/pi", "model/values_fn/vf", "model/values_fn/qf1", "model/values_fn/qf2"};
     for (int q = 0; q < 4; ++q) {
@@ -1149,6 +1174,7 @@ int b2g_sac_destroy(b2g_sac* h) {
   nccl_comm_destroy(h->nccl_comm);
   if (h->side) cudaStreamDestroy(h->side);
   if (h->aux) { cudaStreamSynchronize(h->aux); cudaStreamDestroy(h->aux); }
+  if (h->aux2) { cudaStreamSynchronize(h->aux2); cudaStreamDestroy(h->aux2); }
   for (auto& e : h->ev_aux) if (e) cudaEventDestroy(e);
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   if (h->ev_join) cudaEventDestroy(h->ev_join);
@@ -1329,7 +1355,8 @@ int b2g_sac_create2(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, b2g_sa
   {   // leaf branch of the step (B2G_FORK=0 keeps the step on one stream)
     const char* fk = getenv("B2G_FORK");
     if (!(fk && atoi(fk) == 0)) {
-      if (cudaStreamCreateWithFlags(&h->aux, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "aux stream"));
+      if (cudaStreamCreateWithFlags(&h->aux, cudaStreamNonBlocking) != cudaSuccess ||
+          cudaStreamCreateWithFlags(&h->aux2, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "aux stream"));
       for (auto& e : h->ev_aux)
         if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "aux events"));
       h->fork_leaves = true;
@@ -1951,7 +1978,7 @@ int b2g_sac_state_save(b2g_sac* h, const char* path) {
     return b2g_fail(B2G_ESTATE, "a host-pipelined step is in flight: call b2g_sac_pipeline_flush first (its losses would be lost)");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));     // every enqueued step (b2g_sac_step_async included) has run
-  if (h->aux) CK(cudaStreamSynchronize(h->aux));
+  if (h->aux) { CK(cudaStreamSynchronize(h->aux)); CK(cudaStreamSynchronize(h->aux2)); }
   long long cnt[8];
   CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
   SacHostState hs;
@@ -2025,7 +2052,7 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
   if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
   // ---- from here on a failure leaves the handle unusable until a load succeeds
   CK(cudaStreamSynchronize(h->stream));
-  if (h->aux) CK(cudaStreamSynchronize(h->aux));
+  if (h->aux) { CK(cudaStreamSynchronize(h->aux)); CK(cudaStreamSynchronize(h->aux2)); }
   h->broken = true;
   for (int i = 0; i < (int)dev.size(); ++i)
     if (int rc = rd.read_pieces(i + 2, dev[i].pieces)) return rc;

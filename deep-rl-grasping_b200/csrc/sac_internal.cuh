@@ -62,7 +62,8 @@ struct V2State {
   uint16_t* K0n[2][2]{};         // [0] pi [513 -> 576 rows][H], [1] values packed [576 rows][3H]
   float* z0v = nullptr;          // fc0 pre-activations of vf|q1|q2: [B][3H]
   void* plane_jobs = nullptr; int n_plane_jobs = 0, plane_ctas = 0;
-  const int* plane_cta_job = nullptr;  // job index of every CTA of the planes launch
+  int plane_ctas_fwd = 0;        // CTAs [0, plane_ctas_fwd) write the forward layouts (W1T .. K0T), the rest W2n .. K0n
+  const int* plane_cta_job = nullptr;  // job index of every CTA of the planes launches
   int sm_reserve = 0;           // SMs left to a collective that runs concurrently with the persistent GEMM grids
   std::vector<CUtensorMap> maps; // host copy
   std::vector<char> map_whole;   // per map: the box spans every plane
@@ -84,7 +85,7 @@ struct b2g_sac;
 namespace b2g {
 int v2_alloc(b2g_sac* h);    // plane tensors (before the v1 groups are built: policy inference writes planes 0 / 1 of the activations)
 int v2_create(b2g_sac* h);   // tensor maps + problem groups
-int v2_planes(b2g_sac* h, cudaStream_t s);
+int v2_planes(b2g_sac* h, bool backward, cudaStream_t s);   // the forward-layout or the backward-layout weight planes
 int v2_gather(b2g_sac* h, const GatherArgs& ga, cudaStream_t s);
 int v2_launch(b2g_sac* h, const CgGroup& g, cudaStream_t s);
 // sac.cu hooks of the observe path (obsnorm.cu)
@@ -197,7 +198,8 @@ struct b2g_sac {
   int dp_skip[2][2]{};                 // float4 ranges of the gradient arena pushed by the cnn_fc1 wgrad epilogues
   cudaStream_t side = nullptr;
   cudaStream_t aux = nullptr;              // leaf work off the critical chain (zeroing, weight planes, leaf wgrads, bias sums)
-  cudaEvent_t ev_aux[7]{};
+  cudaStream_t aux2 = nullptr;             // the second leaf branch under the gather (bookkeeping kernel, gradient zeroing)
+  cudaEvent_t ev_aux[9]{};
   bool fork_leaves = false;
   std::map<std::tuple<const void*, const void*, const void*, int>, int> col_ids;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;

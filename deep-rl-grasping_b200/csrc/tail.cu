@@ -838,10 +838,10 @@ cudaError_t smem_optin(K* fn, size_t bytes, unsigned long long& done) {
 }
 
 template <int H>
-cudaError_t tailw_launch(const TailArgs& a, cudaStream_t s) {
+cudaError_t tailw_launch(const TailArgs& a, cudaStream_t s, bool pdl) {
   static unsigned long long done = 0;
   if (cudaError_t e = smem_optin(tailw_kernel<H>, tailw_smem<H>(), done)) return e;
-  return launch_pdl(tailw_kernel<H>, dim3((a.B + TW_G - 1) / TW_G), dim3(H), tailw_smem<H>(), s, pdl_enabled(), a);
+  return launch_pdl(tailw_kernel<H>, dim3((a.B + TW_G - 1) / TW_G), dim3(H), tailw_smem<H>(), s, pdl, a);
 }
 template <int H>
 cudaError_t actw_launch(const TailArgs& t, int n, int deterministic, float* act_out, cudaStream_t s) {
@@ -930,16 +930,16 @@ static size_t tail_smem(int A) {
                           /* tail4 scratch */ 64);
 }
 
-cudaError_t tail_launch(const TailArgs& a, cudaStream_t s) {
+cudaError_t tail_launch(const TailArgs& a, cudaStream_t s, bool pdl) {
   switch (a.H) {
-    case 128: return tailw_launch<128>(a, s);
-    case 192: return tailw_launch<192>(a, s);
-    case 256: return tailw_launch<256>(a, s);
+    case 128: return tailw_launch<128>(a, s, pdl);
+    case 192: return tailw_launch<192>(a, s, pdl);
+    case 256: return tailw_launch<256>(a, s, pdl);
   }
   static unsigned long long done = 0;
   if (cudaError_t e = smem_optin(tail4_kernel, tail_smem(AMAX), done)) return e;
   const int grid = (a.B + 1) / 2;             // four warps per sample, two samples per CTA
-  return launch_pdl(tail4_kernel, dim3(grid), dim3(WARPS * 32), tail_smem(a.A), s, pdl_enabled(), a);
+  return launch_pdl(tail4_kernel, dim3(grid), dim3(WARPS * 32), tail_smem(a.A), s, pdl, a);
 }
 
 }  // namespace b2g
