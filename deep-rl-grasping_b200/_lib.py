@@ -183,51 +183,37 @@ def load():
     lib.b2g_last_step_ms.argtypes = [vp]
     lib.b2g_last_step_ms.restype = C.c_float
     lib.b2g_profile_step.argtypes = [vp, C.c_float, C.POINTER(C.c_char_p), fp, C.c_int]
-    for f in ("b2g_sac_state_save", "b2g_sac_state_load", "b2g_bdq_state_save", "b2g_bdq_state_load", "b2g_dqn_state_save",
-              "b2g_dqn_state_load", "b2g_ppo_state_save", "b2g_ppo_state_load"):
-        getattr(lib, f).argtypes = [vp, C.c_char_p]
+    lib.b2g_sac_state_save.argtypes = lib.b2g_sac_state_load.argtypes = [vp, C.c_char_p]
+    for p in ("bdq", "dqn", "ppo"):          # the handle, named-parameter and training-state calls the three learners share
+        for f in ("destroy", "param_count"):
+            getattr(lib, f"b2g_{p}_{f}").argtypes = [vp]
+        getattr(lib, f"b2g_{p}_param_info").argtypes = [vp, C.c_int, C.c_char_p, C.c_size_t, i64p, i64p, C.POINTER(C.c_int32)]
+        for f in ("get_param", "set_param", "get_grad"):
+            getattr(lib, f"b2g_{p}_{f}").argtypes = [vp, C.c_char_p, fp, C.c_size_t]
+        for f in ("state_save", "state_load"):
+            getattr(lib, f"b2g_{p}_{f}").argtypes = [vp, C.c_char_p]
+    for p in ("bdq", "dqn"):                 # and the transition replay of the two Q learners
+        getattr(lib, f"b2g_{p}_replay_add").argtypes = [vp, fp, fp, fp, fp, fp, C.c_int64]
+        getattr(lib, f"b2g_{p}_replay_size").argtypes = [vp]
+        getattr(lib, f"b2g_{p}_replay_size").restype = C.c_int64
+        getattr(lib, f"b2g_{p}_set_norm_stats").argtypes = [vp, dp, dp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int]
+        getattr(lib, f"b2g_{p}_set_per_beta").argtypes = [vp, C.c_float]
+        getattr(lib, f"b2g_{p}_get_last_per").argtypes = [vp, C.POINTER(C.c_int32), fp, fp]
     lib.b2g_bdq_create.argtypes = [C.POINTER(BdqCfg), C.POINTER(vp)]
-    lib.b2g_bdq_destroy.argtypes = [vp]
-    lib.b2g_bdq_param_count.argtypes = [vp]
-    lib.b2g_bdq_param_info.argtypes = [vp, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]
-    for f in ("b2g_bdq_get_param", "b2g_bdq_set_param", "b2g_bdq_get_grad"):
-        getattr(lib, f).argtypes = [vp, C.c_char_p, fp, C.c_size_t]
-    lib.b2g_bdq_replay_add.argtypes = [vp, fp, fp, fp, fp, fp, C.c_int64]
-    lib.b2g_bdq_replay_size.argtypes = [vp]
-    lib.b2g_bdq_replay_size.restype = C.c_int64
-    lib.b2g_bdq_set_norm_stats.argtypes = [vp, dp, dp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int]
     lib.b2g_bdq_step.argtypes = [vp, C.c_int, C.c_float, C.POINTER(BdqMetrics)]
     lib.b2g_bdq_step_explicit.argtypes = [vp, fp, fp, fp, fp, fp, fp, C.c_float, C.c_int, C.POINTER(BdqMetrics), fp]
     lib.b2g_bdq_act.argtypes = [vp, fp, C.c_int, C.POINTER(C.c_int32)]
-    lib.b2g_bdq_set_per_beta.argtypes = [vp, C.c_float]
-    lib.b2g_bdq_get_last_per.argtypes = [vp, C.POINTER(C.c_int32), fp, fp]
     lib.b2g_bdq_observe_act.argtypes = [vp, fp, C.c_int, C.c_int, C.c_float, C.POINTER(C.c_int32)]
     lib.b2g_bdq_observe_add.argtypes = [vp, fp, fp, fp, fp, fp, C.c_int, C.c_int]
     lib.b2g_bdq_obs_rms_set.argtypes = [vp, dp, dp, C.c_double]
     lib.b2g_bdq_obs_rms_get.argtypes = [vp, dp, dp, dp]
     lib.b2g_bdq_upload_bytes.argtypes = [vp, i64p, i64p]
     lib.b2g_dqn_create.argtypes = [C.POINTER(DqnCfg), C.POINTER(vp)]
-    lib.b2g_dqn_destroy.argtypes = [vp]
-    lib.b2g_dqn_param_count.argtypes = [vp]
-    lib.b2g_dqn_param_info.argtypes = [vp, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]
-    for f in ("b2g_dqn_get_param", "b2g_dqn_set_param", "b2g_dqn_get_grad"):
-        getattr(lib, f).argtypes = [vp, C.c_char_p, fp, C.c_size_t]
-    lib.b2g_dqn_replay_add.argtypes = [vp, fp, fp, fp, fp, fp, C.c_int64]
-    lib.b2g_dqn_replay_size.argtypes = [vp]
-    lib.b2g_dqn_replay_size.restype = C.c_int64
-    lib.b2g_dqn_set_norm_stats.argtypes = [vp, dp, dp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int]
     lib.b2g_dqn_step.argtypes = [vp, C.c_int, C.c_float, C.POINTER(DqnMetrics)]
     lib.b2g_dqn_step_explicit.argtypes = [vp, fp, fp, fp, fp, fp, fp, C.c_float, C.c_int, C.POINTER(DqnMetrics), fp]
-    lib.b2g_dqn_set_per_beta.argtypes = [vp, C.c_float]
-    lib.b2g_dqn_get_last_per.argtypes = [vp, C.POINTER(C.c_int32), fp, fp]
     lib.b2g_dqn_update_target.argtypes = [vp]
     lib.b2g_dqn_act.argtypes = [vp, fp, C.c_int, C.POINTER(C.c_int32), fp]
     lib.b2g_ppo_create.argtypes = [C.POINTER(PpoCfg), C.POINTER(vp)]
-    lib.b2g_ppo_destroy.argtypes = [vp]
-    lib.b2g_ppo_param_count.argtypes = [vp]
-    lib.b2g_ppo_param_info.argtypes = [vp, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]
-    for f in ("b2g_ppo_get_param", "b2g_ppo_set_param", "b2g_ppo_get_grad"):
-        getattr(lib, f).argtypes = [vp, C.c_char_p, fp, C.c_size_t]
     lib.b2g_ppo_rollout_act.argtypes = [vp, fp, fp]
     lib.b2g_ppo_rollout_reward.argtypes = [vp, fp, fp]
     lib.b2g_ppo_rollout_reset.argtypes = [vp]

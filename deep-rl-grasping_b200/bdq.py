@@ -18,12 +18,13 @@ import numpy as np
 
 from . import _lib, sb_io, training_state
 from .callbacks import as_callback
-from .learner import _f32, _fp
+from .learner import HandleLearner, _f32, _fp
 from .vec_env import DummyVecEnv, VecNormalize
 
 
-class BDQLearner:
+class BDQLearner(HandleLearner):
     """numpy-facing wrapper of one ``b2g_bdq`` handle (maps 1:1 onto the C ABI)."""
+    _abi = "bdq"
 
     def __init__(self, obs_dim=100, n_branches=3, n_bins=8, layers=((64, 64), (32,), (32,)), batch_size=64, buffer_size=100000,
                  gamma=0.99, target_network_update_freq=1000, trunk_grad_rescale=True, seed=0, device=0, rank=0, nranks=1, nccl_id=None,
@@ -43,66 +44,12 @@ class BDQLearner:
                           target_network_update_freq, int(trunk_grad_rescale), seed, device, rank, nranks, idp, libp,
                           int(bool(prioritized_replay)), float(prioritized_replay_alpha), float(prioritized_replay_eps))
         self.prioritized_replay = bool(prioritized_replay)
-        self.h = C.c_void_p()
-        _lib.check(self.lib.b2g_bdq_create(C.byref(cfg), C.byref(self.h)))
+        self._create(cfg)
         self.obs_dim, self.n_branches, self.n_bins, self.batch_size = obs_dim, n_branches, n_bins, batch_size
         self.obs_shape = (obs_dim,)          # shape of obs_rms_get's arrays (BDQ sets the env's observation shape)
-        self._info = OrderedDict()
-        buf = C.create_string_buffer(256)
-        rows, cols, nd = C.c_int64(), C.c_int64(), C.c_int32()
-        for i in range(self.lib.b2g_bdq_param_count(self.h)):
-            _lib.check(self.lib.b2g_bdq_param_info(self.h, i, buf, 256, C.byref(rows), C.byref(cols), C.byref(nd)))
-            shape = () if nd.value == 0 else ((rows.value, cols.value) if nd.value == 2 else (cols.value,))
-            self._info[buf.value.decode()] = shape
 
-    def close(self):
-        if getattr(self, "h", None) is not None and self.h:
-            self.lib.b2g_bdq_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    @property
-    def param_shapes(self):
-        return self._info
-
-    def get_parameters(self):
-        out = OrderedDict()
-        for n, shp in self._info.items():
-            a = np.empty(shp, np.float32)
-            _lib.check(self.lib.b2g_bdq_get_param(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
-            out[n] = a
-        return out
-
-    def load_parameters(self, params, exact_match=True):
-        seen = set()
-        for n, a in params.items():
-            key = n[:-2] if n.endswith(":0") else n
-            if key not in self._info:
-                if exact_match:
-                    raise ValueError(f"unknown variable {n}")
-                continue
-            a = _f32(a)
-            if tuple(a.shape) != self._info[key]:
-                raise ValueError(f"shape mismatch for {n}: {a.shape} vs {self._info[key]}")
-            _lib.check(self.lib.b2g_bdq_set_param(self.h, key.encode(), _fp(a.reshape(-1)), a.size))
-            seen.add(key)
-        if exact_match and seen != set(self._info):
-            raise ValueError("missing variables")
-
-    def get_gradients(self):
-        out = OrderedDict()
-        for n, shp in self._info.items():
-            if not n.startswith("bdq/model/"):
-                continue
-            a = np.empty(shp, np.float32)
-            _lib.check(self.lib.b2g_bdq_get_grad(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
-            out[n] = a
-        return out
+    def _has_grad(self, name):
+        return name.startswith("bdq/model/")
 
     def replay_add(self, obs, act_idx, rew, next_obs, done):
         obs, next_obs, act = _f32(obs), _f32(next_obs), _f32(act_idx)
@@ -112,14 +59,10 @@ class BDQLearner:
     def replay_size(self):
         return int(self.lib.b2g_bdq_replay_size(self.h))
 
-    def save_state(self, path: str):
-        """Parameters, Adam moments, counters, the live replay rows and the prioritised-replay trees -> ``path``."""
-        _lib.check(self.lib.b2g_bdq_state_save(self.h, os.fsencode(path)))
-
     def load_state(self, path: str):
         """Restores a ``save_state`` file into this learner, which must have the same configuration (and own a device
         ``obs_rms`` exactly when the file carries one)."""
-        _lib.check(self.lib.b2g_bdq_state_load(self.h, os.fsencode(path)))
+        super().load_state(path)
         self.obs_rms_version += 1
 
     def set_norm_stats(self, obs_mean=None, obs_var=None, ret_var=1.0, clip_obs=10.0, clip_reward=10.0, epsilon=1e-8,

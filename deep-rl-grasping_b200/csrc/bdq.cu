@@ -19,7 +19,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <map>
 #include <string>
 #include <vector>
 
@@ -32,13 +31,6 @@
 using namespace b2g;
 
 namespace {
-
-struct BTensor {
-  std::string name;
-  int rows, cols, stride;   // zip shape [rows, cols] (cols = 1 for biases, rows = 1), device row stride
-  int64_t off;              // float offset inside P (online) -- the target copy sits at off + n_train
-  bool is_weight;
-};
 
 constexpr int BMET_LOSS = 0, BMET_MEANQ = 1, BMET_GN = MET_GN_PI;   // optim_kernel accumulates the squared norm at MET_GN_PI
 
@@ -167,15 +159,13 @@ __global__ void bdq_target_copy_kernel(float* __restrict__ P, long long n_train,
 struct b2g_bdq {
   b2g_bdq_cfg cfg{};
   int B = 0, D = 0, n = 0, NBS = 0, T0 = 0, T1 = 0, HB = 0, XS = 0, E = 0;
-  std::vector<BTensor> tensors;
-  std::map<std::string, int> tindex;
+  ParamTable params;           // bdq/eps, the online tensors, then their target copies at off + n_train
   int64_t n_train = 0;
   float *P = nullptr, *Mo = nullptr, *Vo = nullptr, *G = nullptr, *metrics = nullptr;
   float eps_value = 1.0f;      // bdq/eps (exploration epsilon variable of the zip)
   cudaStream_t stream = nullptr;
   std::vector<void*> allocs;
-  float *r_obs = nullptr, *r_next = nullptr, *r_act = nullptr, *r_rew = nullptr, *r_done = nullptr;
-  int64_t r_size = 0, r_pos = 0;
+  TransitionReplay replay;
   double *d_mean = nullptr, *d_istd = nullptr, *d_normc = nullptr;
   float *X = nullptr, *Xn = nullptr, *Xscratch = nullptr;
   float *h1[3]{}, *h2[3]{}, *hb[3][8]{}, *Aout[3][8]{}, *hv[3]{}, *Vout[3]{};
@@ -193,11 +183,6 @@ struct b2g_bdq {
   long long n_updates = 0;
   float* h_met = nullptr;
   void* nccl_comm = nullptr;
-  // prioritised replay
-  bool per = false;
-  double *t_sum = nullptr, *t_min = nullptr;
-  long long per_C = 0;
-  float *max_prio = nullptr, *d_beta = nullptr, *prio_out = nullptr;
   cudaGraphExec_t graph_exec = nullptr;
   bool use_graph = true;
   bool broken = false;         // a training-state load failed after it began writing: only destroy / load are accepted
@@ -215,19 +200,16 @@ struct b2g_bdq {
   int* ob_idx = nullptr;       // [stage_rows][D] actor output
   int ob_k = 0, ob_n = 0;
   int64_t up_observe = 0, up_other = 0;    // host->device bytes: observe_* / obs_rms_set, and act + replay_add + set_norm_stats
-  float* p(const std::string& nm) { return P + tensors[tindex.at(nm)].off; }
-  float* g(const std::string& nm) { return G + tensors[tindex.at(nm)].off; }
-  float* pt(const std::string& nm) { return P + n_train + tensors[tindex.at(nm)].off; }
+  float* p(const std::string& nm) { return P + params.off(nm); }
+  float* g(const std::string& nm) { return G + params.off(nm); }
 };
 
 namespace {
 std::string fcname(int i) { return i == 0 ? "fully_connected" : "fully_connected_" + std::to_string(i); }
 
+// an online tensor of the zip: weights [rows, cols] at row stride `stride`, biases [cols] padded to `stride`
 void add_t(b2g_bdq* h, const std::string& name, int rows, int cols, bool w, int stride, int64_t& off) {
-  BTensor t{name, rows, cols, stride, off, w};
-  off += ((int64_t)(w ? rows * stride : stride) + 31) / 32 * 32;
-  h->tindex[name] = (int)h->tensors.size();
-  h->tensors.push_back(t);
+  h->params.add(name, w ? rows : 1, cols, w ? 2 : 1, stride, arena_take(off, w ? (int64_t)rows * stride : stride), true);
 }
 
 int build(b2g_bdq* h) {
@@ -241,7 +223,7 @@ int build(b2g_bdq* h) {
   BT(rcat, iota_tab(B, (D + 1) * HB)) BT(icat, iota_tab((D + 1) * HB))
   BT(kT0, iota_tab(std::max(obs, T0) + 8, T0)) BT(kT1, iota_tab(std::max(T0, T1) + 8, T1)) BT(kHB, iota_tab(T1 + 8, HB)) BT(kNBS, iota_tab(HB + 8, NBS)) BT(k4, iota_tab(HB + 8, 4))
   const std::string sc[3] = {"bdq/model", "bdq/model", "bdq/target_q_func/model"};
-  auto W = [&](int e, const std::string& rel) { return e == 2 ? h->pt("bdq/model" + rel) : h->p("bdq/model" + rel); };
+  auto W = [&](int e, const std::string& rel) { return h->p((e == 2 ? "bdq/target_q_func/model" : "bdq/model") + rel); };
   // ---------------- forward (3 evaluations), also the policy-inference groups (evaluation 0 only)
   auto fwd_group = [&](const char* name, int layer) {
     GemmGroup g, a;
@@ -304,7 +286,7 @@ int build(b2g_bdq* h) {
       GemmDesc w = gemm_desc(h->h2[0], iT1, rT1, h->dcat, dzcol, iHB, h->g(rel + "/weights"), kHB, iHB, T1, HB, B, GG_COLSUM);
       w.colsum = h->g(rel + "/biases");
       g.host.push_back(w);
-      for (int r = 0; r < HB; ++r) br[q * HB + r] = (int)h->tensors[h->tindex.at(rel + "/weights")].off + r;
+      for (int r = 0; r < HB; ++r) br[q * HB + r] = (int)h->params.off(rel + "/weights") + r;
     }
     const int* brt; BT(brt, br)
     GemmDesc dg = gemm_desc(h->dcat, rcat, icat, h->P, brt, kHB, h->dh2, rT1, iT1, B, T1, (D + 1) * HB, GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK | GG_EPI_SCALE);
@@ -339,11 +321,11 @@ int build(b2g_bdq* h) {
 
 GatherArgs bgather(b2g_bdq* h, bool from_replay, bool with_next) {
   GatherArgs g{};
-  g.obs = from_replay ? h->r_obs : h->s_obs;
-  g.next_obs = with_next ? (from_replay ? h->r_next : h->s_next) : nullptr;
-  g.act = with_next ? (from_replay ? h->r_act : h->s_act) : nullptr;
-  g.rew = from_replay ? h->r_rew : h->s_rew;
-  g.done = from_replay ? h->r_done : h->s_done;
+  g.obs = from_replay ? h->replay.obs : h->s_obs;
+  g.next_obs = with_next ? (from_replay ? h->replay.next : h->s_next) : nullptr;
+  g.act = with_next ? (from_replay ? h->replay.act : h->s_act) : nullptr;
+  g.rew = from_replay ? h->replay.rew : h->s_rew;
+  g.done = from_replay ? h->replay.done : h->s_done;
   g.indices = from_replay ? h->indices : nullptr;
   g.mean = h->d_mean; g.var = h->d_istd; g.normc = h->d_normc;
   g.B = h->B; g.H = 0; g.W = h->cfg.obs_dim; g.Cimg = 0; g.scale = 1.f;
@@ -359,13 +341,9 @@ int bdq_issue(b2g_bdq* h, bool sampled, bool apply, const float* weights) {
   pa.indices = h->indices; pa.eps = h->eps_dummy; pa.B = h->B; pa.A = 1; pa.replay_size = nullptr;
   pa.seed = h->cfg.seed + 0x9E3779B97F4A7C15ull * (unsigned long long)h->cfg.rank; pa.gen = sampled ? 1 : 0; pa.apply = apply ? 1 : 0;
   prep_launch(pa, s);
-  PerArgs pr{};
-  if (h->per) {
-    pr.tsum = h->t_sum; pr.tmin = h->t_min; pr.C = h->per_C; pr.max_prio = h->max_prio; pr.counters = h->counters; pr.seed = pa.seed;
-    pr.B = h->B; pr.alpha = h->cfg.per_alpha; pr.eps = h->cfg.per_eps; pr.beta = h->d_beta; pr.indices = h->indices; pr.weights = h->weights;
-    pr.prio_out = h->prio_out; pr.td = h->td; pr.D = h->D;
-    if (sampled) { per_sample_launch(pr, s); weights = h->weights; }   // overwrites the uniform draw
-  }
+  const bool per = h->replay.per;
+  const PerArgs pr = h->replay.per_args(h->counters, pa.seed, h->B, h->indices, h->weights, h->td, h->D);
+  if (per && sampled) { per_sample_launch(pr, s); weights = h->weights; }   // overwrites the uniform draw
   gather_launch(bgather(h, sampled, true), s);
   CK(cudaMemsetAsync(h->G, 0, (size_t)(h->n_train + MET_COUNT) * sizeof(float), s));
   for (auto& g : h->fwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
@@ -378,7 +356,7 @@ int bdq_issue(b2g_bdq* h, bool sampled, bool apply, const float* weights) {
   t.dV = h->dV; t.td = h->td; t.metrics = h->metrics;
   bdq_tail_kernel<<<(h->B + 127) / 128, 128, 0, s>>>(t);
   for (auto& g : h->bwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
-  if (h->per && sampled) per_write_launch(pr, h->indices, 0, h->cfg.buffer_capacity, h->B, 1, s);   // update_priorities(|td| + eps)
+  if (per && sampled) per_write_launch(pr, h->indices, 0, h->cfg.buffer_capacity, h->B, 1, s);   // update_priorities(|td| + eps)
   if (h->cfg.nranks > 1) {      // gradients + loss scalars averaged over the ranks (each rank sampled its own replay shard)
     CK(cudaMemcpyAsync(h->G + h->n_train, h->metrics, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
     if (int rc = nccl_allreduce_sum_f32(h->nccl_comm, h->G, (size_t)(h->n_train + MET_COUNT), s)) return rc;
@@ -436,7 +414,6 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
   b2g_bdq* h = new b2g_bdq();
   h->cfg = *cfg;
   h->cfg.nccl_id = nullptr; h->cfg.nccl_lib = nullptr;
-  h->per = cfg->prioritized_replay != 0;
   const char* ng = getenv("B2G_NO_GRAPH");
   h->use_graph = !(ng && ng[0] == '1');
   h->B = cfg->batch; h->D = cfg->n_branches; h->n = cfg->n_bins; h->NBS = (cfg->n_bins + 3) / 4 * 4;
@@ -445,7 +422,8 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
   h->stage_rows = std::max(cfg->batch, 256);
   auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_bdq_destroy(h); g_b2g_err = keep; return rc; };
   if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream"));
-  // parameter inventory: same names as the zips (oracle/bdq_ref.py param_specs)
+  // parameter inventory: same names and order as the zips (oracle/bdq_ref.py all_specs)
+  h->params.add_scalar("bdq/eps", &h->eps_value);
   int64_t off = 0;
   for (int d = 0; d < h->D; ++d) {
     add_t(h, "bdq/model/action_value/" + fcname(2 * d) + "/biases", 1, h->HB, false, h->HB, off);
@@ -462,13 +440,14 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
   add_t(h, "bdq/model/state_value/" + fcname(1) + "/biases", 1, 1, false, 4, off);
   add_t(h, "bdq/model/state_value/" + fcname(1) + "/weights", h->HB, 1, true, 4, off);
   h->n_train = off;
+  h->params.add_copies(1, h->params.count() - 1, "bdq/model", "bdq/target_q_func/model", h->n_train);
   int rc = 0;
   const int B = h->B, D = h->D;
 #define BA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
   BA(h->P, 2 * h->n_train); BA(h->Mo, h->n_train); BA(h->Vo, h->n_train); BA(h->G, h->n_train + MET_COUNT); BA(h->metrics, MET_COUNT);
   BA(h->counters, 8); BA(h->step_consts, 4); BA(h->d_lr, 1);
   const int64_t cap = cfg->buffer_capacity;
-  BA(h->r_obs, cap * h->E); BA(h->r_next, cap * h->E); BA(h->r_act, cap * D); BA(h->r_rew, cap); BA(h->r_done, cap);
+  if ((rc = h->replay.init(h->allocs, h->stream, cap, h->E, D, B, cfg->prioritized_replay != 0, cfg->per_alpha, cfg->per_eps))) return bail(rc);
   BA(h->d_mean, h->E); BA(h->d_istd, h->E); BA(h->d_normc, 8);
   BA(h->X, (size_t)B * h->XS); BA(h->Xn, (size_t)B * h->XS); BA(h->Xscratch, (size_t)B * h->XS);
   for (int e = 0; e < 3; ++e) {
@@ -480,15 +459,6 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
   BA(h->rew_n, B); BA(h->done_n, B); BA(h->weights, B); BA(h->eps_dummy, B + 8); BA(h->indices, B + 4); BA(h->act_idx_out, B * D);
   BA(h->s_obs, (size_t)B * h->E); BA(h->s_next, (size_t)B * h->E); BA(h->s_act, B * D); BA(h->s_rew, B); BA(h->s_done, B);
   BA(h->d_Aptr, 8);
-  BA(h->d_beta, 1); BA(h->max_prio, 1); BA(h->prio_out, B);
-  if (h->per) {
-    h->per_C = 1;
-    while (h->per_C < cap) h->per_C <<= 1;
-    BA(h->t_sum, 2 * h->per_C); BA(h->t_min, 2 * h->per_C);
-    per_init_launch(h->t_sum, h->t_min, 2 * h->per_C, h->max_prio, h->stream);
-    const float beta0 = 0.4f;
-    if (cudaMemcpyAsync(h->d_beta, &beta0, sizeof(float), cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "per init"));
-  }
 #undef BA
   if (cudaMallocHost((void**)&h->h_met, MET_COUNT * sizeof(float)) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "cudaMallocHost"));
   {
@@ -512,97 +482,25 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
   return 0;
 }
 
-int b2g_bdq_param_count(const b2g_bdq* h) { B2G_USABLE(h); return h ? 1 + 2 * (int)h->tensors.size() : 0; }
-
-// index 0 = bdq/eps; 1..T = online tensors; T+1..2T = target tensors (names as in the zips)
+int b2g_bdq_param_count(const b2g_bdq* h) { return param_count(h); }
 int b2g_bdq_param_info(const b2g_bdq* h, int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim) {
-  B2G_USABLE(h);
-  if (!h || idx < 0 || idx >= b2g_bdq_param_count(h) || !name) return b2g_fail(B2G_EINVAL, "bad tensor index");
-  std::string nm = "bdq/eps";
-  int64_t r = 1, c = 1;
-  int nd = 0;
-  if (idx > 0) {
-    const int T = (int)h->tensors.size();
-    const BTensor& t = h->tensors[(idx - 1) % T];
-    nm = (idx - 1) < T ? t.name : std::string("bdq/target_q_func/model") + t.name.substr(strlen("bdq/model"));
-    r = t.rows; c = t.cols; nd = t.is_weight ? 2 : 1;
-  }
-  snprintf(name, name_cap, "%s", nm.c_str());
-  if (rows) *rows = r;
-  if (cols) *cols = c;
-  if (ndim) *ndim = nd;
-  return 0;
+  return param_info(h, idx, name, name_cap, rows, cols, ndim);
 }
-
-static int bdq_copy(b2g_bdq* h, const char* name, float* arena_online, float* host, size_t numel, bool to_host, bool allow_target) {
-  if (!h || !name || !host) return b2g_fail(B2G_EINVAL, "NULL argument");
-  std::string nm(name);
-  if (nm.size() > 2 && nm.compare(nm.size() - 2, 2, ":0") == 0) nm.resize(nm.size() - 2);
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  if (nm == "bdq/eps") {
-    if (numel != 1) return b2g_fail(B2G_EINVAL, "bdq/eps is a scalar");
-    if (to_host) host[0] = h->eps_value; else h->eps_value = host[0];
-    return 0;
-  }
-  bool target = false;
-  const std::string tp = "bdq/target_q_func/model";
-  if (nm.compare(0, tp.size(), tp) == 0) { target = true; nm = "bdq/model" + nm.substr(tp.size()); }
-  if (target && !allow_target) return b2g_fail(B2G_EINVAL, "not a trainable variable");
-  auto it = h->tindex.find(nm);
-  if (it == h->tindex.end()) return b2g_fail(B2G_EINVAL, std::string("unknown variable: ") + name);
-  const BTensor& t = h->tensors[it->second];
-  const size_t rows = t.is_weight ? t.rows : 1, cols = t.is_weight ? t.cols : (size_t)(t.rows * t.cols);
-  const size_t ccount = t.is_weight ? t.cols : (size_t)t.cols;
-  if (numel != rows * ccount) return b2g_fail(B2G_EINVAL, std::string("size mismatch for ") + name);
-  float* dev = arena_online + t.off + (target ? h->n_train : 0);
-  (void)cols;
-  // repack between the zip layout [rows, cols] and the device row stride
-  if (to_host) CK(cudaMemcpy2D(host, ccount * sizeof(float), dev, t.stride * sizeof(float), ccount * sizeof(float), rows, cudaMemcpyDeviceToHost));
-  else CK(cudaMemcpy2D(dev, t.stride * sizeof(float), host, ccount * sizeof(float), ccount * sizeof(float), rows, cudaMemcpyHostToDevice));
-  return 0;
-}
-int b2g_bdq_get_param(b2g_bdq* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return bdq_copy(h, name, h ? h->P : nullptr, dst, numel, true, true); }
+int b2g_bdq_get_param(b2g_bdq* h, const char* name, float* dst, size_t numel) { return param_copy(h, name, ParamCopy::Get, dst, numel); }
 int b2g_bdq_set_param(b2g_bdq* h, const char* name, const float* src, size_t numel) {
-  B2G_USABLE(h);
-  return bdq_copy(h, name, h ? h->P : nullptr, const_cast<float*>(src), numel, false, true);
+  return param_copy(h, name, ParamCopy::Set, const_cast<float*>(src), numel);
 }
-int b2g_bdq_get_grad(b2g_bdq* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return bdq_copy(h, name, h ? h->G : nullptr, dst, numel, true, false); }
+int b2g_bdq_get_grad(b2g_bdq* h, const char* name, float* dst, size_t numel) { return param_copy(h, name, ParamCopy::GetGrad, dst, numel); }
 
 int b2g_bdq_replay_add(b2g_bdq* h, const float* obs, const float* act_idx, const float* rew, const float* next_obs, const float* done, int64_t n) {
   B2G_USABLE(h);
   if (!h || !obs || !act_idx || !rew || !next_obs || !done || n < 0) return b2g_fail(B2G_EINVAL, "NULL argument");
   CK(cudaSetDevice(h->cfg.device));
-  const int64_t cap = h->cfg.buffer_capacity;
-  int64_t done_n = 0;
-  while (done_n < n) {
-    const int64_t chunk = std::min(n - done_n, cap - h->r_pos);
-    const size_t E = h->E, D = h->D;
-    CK(cudaMemcpyAsync(h->r_obs + h->r_pos * E, obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_next + h->r_pos * E, next_obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_act + h->r_pos * D, act_idx + done_n * D, chunk * D * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_rew + h->r_pos, rew + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_done + h->r_pos, done + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
-    h->up_other += (int64_t)(chunk * (2 * E + D + 2) * sizeof(float));
-    if (h->per) {        // new transitions enter with the running maximum priority ([SB2] PrioritizedReplayBuffer.add)
-      PerArgs pr{};
-      pr.tsum = h->t_sum; pr.tmin = h->t_min; pr.C = h->per_C; pr.max_prio = h->max_prio; pr.alpha = h->cfg.per_alpha; pr.eps = h->cfg.per_eps;
-      for (int64_t o = 0; o < chunk; o += 1024) {
-        const int nn = (int)std::min<int64_t>(1024, chunk - o);
-        per_write_launch(pr, nullptr, h->r_pos + o, cap, nn, 0, h->stream);
-      }
-    }
-    h->r_pos = (h->r_pos + chunk) % cap;
-    h->r_size = std::min(cap, h->r_size + chunk);
-    done_n += chunk;
-  }
-  const long long sz = h->r_size;
-  CK(cudaMemcpyAsync(h->counters + 5, &sz, sizeof(long long), cudaMemcpyHostToDevice, h->stream));
-  h->up_other += (int64_t)sizeof(long long);
-  CK(cudaStreamSynchronize(h->stream));
+  if (int rc = h->replay.add(obs, act_idx, rew, next_obs, done, n, h->counters, h->stream)) return rc;
+  h->up_other += (int64_t)(n * (2 * h->E + h->D + 2) * sizeof(float) + sizeof(long long));
   return 0;
 }
-int64_t b2g_bdq_replay_size(const b2g_bdq* h) { B2G_USABLE(h); return h ? h->r_size : 0; }
+int64_t b2g_bdq_replay_size(const b2g_bdq* h) { B2G_USABLE(h); return h ? h->replay.size : 0; }
 
 int b2g_bdq_set_norm_stats(b2g_bdq* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs, double clip_rew, double eps,
                            int norm_obs, int norm_reward) {
@@ -639,7 +537,7 @@ int b2g_bdq_set_norm_stats(b2g_bdq* h, const double* obs_mean, const double* obs
 int b2g_bdq_step(b2g_bdq* h, int n_steps, float lr, b2g_bdq_metrics* out) {
   B2G_USABLE(h);
   if (!h || n_steps < 0) return b2g_fail(B2G_EINVAL, "bad argument");
-  if (h->r_size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
+  if (h->replay.size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
   if (h->use_graph && !h->graph_exec)       // the whole step (~14 launches of tiny layers) replays as one graph
@@ -655,10 +553,7 @@ int b2g_bdq_step(b2g_bdq* h, int n_steps, float lr, b2g_bdq_metrics* out) {
 int b2g_bdq_set_per_beta(b2g_bdq* h, float beta) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  CK(cudaMemcpy(h->d_beta, &beta, sizeof(float), cudaMemcpyHostToDevice));
-  return 0;
+  return h->replay.set_beta(beta, h->cfg.device, h->stream);
 }
 
 // h->indices holds the slots of the last sampled step with uniform replay too (prep_kernel draws them, per_sample_kernel
@@ -666,12 +561,7 @@ int b2g_bdq_set_per_beta(b2g_bdq* h, float beta) {
 int b2g_bdq_get_last_per(b2g_bdq* h, int32_t* slots, float* weights, float* priorities) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  if (slots) CK(cudaMemcpy(slots, h->indices, h->B * sizeof(int32_t), cudaMemcpyDeviceToHost));
-  if (weights) CK(cudaMemcpy(weights, h->weights, h->B * sizeof(float), cudaMemcpyDeviceToHost));
-  if (priorities) CK(cudaMemcpy(priorities, h->prio_out, h->B * sizeof(float), cudaMemcpyDeviceToHost));
-  return 0;
+  return h->replay.get_last(h->indices, h->weights, h->B, slots, weights, priorities, h->cfg.device, h->stream);
 }
 
 int b2g_bdq_step_explicit(b2g_bdq* h, const float* obs, const float* act_idx, const float* rew, const float* next_obs, const float* done,
@@ -843,25 +733,17 @@ int b2g_bdq_observe_add(b2g_bdq* h, const float* act_idx, const float* rew, cons
   if (int rc = bdq_upload(h, h->ob_rew, rew, n * sizeof(float))) return rc;
   if (int rc = bdq_upload(h, h->ob_done, done, n * sizeof(float))) return rc;
   // the transitions: obs = the staged rows, next_obs = the uploaded rows (a finished env's terminal frame)
-  const int64_t cap = h->cfg.buffer_capacity;
-  const int64_t new_size = std::min<int64_t>(cap, h->r_size + n);
-  bdq_commit_kernel<<<n, 256, 0, h->stream>>>(cur, nxt, h->ob_act, h->ob_rew, h->ob_done, (int)E, (int)D, h->r_pos, cap, h->r_obs, h->r_next,
-                                              h->r_act, h->r_rew, h->r_done, h->counters, new_size);
-  if (h->per) {        // new transitions enter with the running maximum priority, as in b2g_bdq_replay_add
-    PerArgs pr{};
-    pr.tsum = h->t_sum; pr.tmin = h->t_min; pr.C = h->per_C; pr.max_prio = h->max_prio; pr.alpha = h->cfg.per_alpha; pr.eps = h->cfg.per_eps;
-    for (int o = 0; o < n; o += 1024) {
-      const int nn = std::min(1024, n - o);
-      per_write_launch(pr, nullptr, h->r_pos + o, cap, nn, 0, h->stream);
-    }
-  }
+  TransitionReplay& rp = h->replay;
+  const int64_t new_size = std::min<int64_t>(rp.cap, rp.size + n);
+  bdq_commit_kernel<<<n, 256, 0, h->stream>>>(cur, nxt, h->ob_act, h->ob_rew, h->ob_done, (int)E, (int)D, rp.pos, rp.cap, rp.obs, rp.next,
+                                              rp.act, rp.rew, rp.done, h->counters, new_size);
+  rp.insert_max_prio(rp.pos, n, h->stream);     // as in b2g_bdq_replay_add
   // VecNormalize's step_wait merges the frames the VecEnv returned: a finished env's reset frame, not its terminal observation
   if (update_stats) bdq_merge(h, nxt, n_done ? h->ob_reset : nullptr, h->ob_done, n);
   // the new rows become the current observations; a finished env continues from the frame its reset returned
   for (int i = 0; i < n; ++i)
     if (done[i] != 0.f) CK(cudaMemcpyAsync(nxt + i * E, h->ob_reset + i * E, fb, cudaMemcpyDeviceToDevice, h->stream));
-  h->r_pos = (h->r_pos + n) % cap;
-  h->r_size = new_size;
+  rp.advance(n);
   h->ob_k ^= 1;
   CK(cudaStreamSynchronize(h->stream));     // host arrays are caller-owned: copied before return
   CK(cudaGetLastError());
@@ -883,36 +765,12 @@ std::vector<FpField> bdq_fingerprint(const b2g_bdq* h) {
           fp_int("trunk_grad_rescale", c.trunk_grad_rescale), fp_int("seed", (int64_t)c.seed),
           fp_int("prioritized_replay", c.prioritized_replay), fp_real("per_alpha", c.per_alpha), fp_real("per_eps", c.per_eps)};
 }
-// a handle that owns obs_rms writes one more field and one more section (count, mean[E], var[E] as float64); one that does not
-// reads and writes the files it always did
-std::vector<FpField> bdq_fingerprint_rms(const b2g_bdq* h) {
-  std::vector<FpField> fp = bdq_fingerprint(h);
-  if (h->rms_mean) fp.push_back(fp_int("obs_rms", 1));
-  return fp;
-}
-const uint32_t kBdqRmsTag = state_tag("ORMS");
-
-const uint32_t kBdqTags[] = {state_tag("HOST"), state_tag("CNTR"), state_tag("PARM"), state_tag("ADMM"), state_tag("ADMV"),
-                             state_tag("ROBS"), state_tag("RNXT"), state_tag("RACT"), state_tag("RREW"), state_tag("RDON"),
-                             state_tag("PERT"), state_tag("PERS")};
-
-StatePiece bdev(void* p, size_t bytes) { StatePiece s; s.dev = p; s.bytes = bytes; return s; }
-
-// sections 2.. (parameters .. prioritised-replay scalars) of a handle holding `live` replay rows
+// sections 2.. (parameters .. prioritised-replay scalars, then obs_rms when the handle owns it) of a handle holding `live`
+// replay rows
 std::vector<StateSection> bdq_device_sections(b2g_bdq* h, int64_t live) {
-  const size_t cap = (size_t)h->cfg.buffer_capacity, E = h->E, D = h->D;
-  std::vector<StateSection> s(10);
-  s[0].pieces = {bdev(h->P, 2 * h->n_train * sizeof(float))};
-  s[1].pieces = {bdev(h->Mo, h->n_train * sizeof(float))};
-  s[2].pieces = {bdev(h->Vo, h->n_train * sizeof(float))};
-  s[3].pieces = {bdev(h->r_obs, live * E * sizeof(float))};       // rows [0, size) are the live ones
-  s[4].pieces = {bdev(h->r_next, live * E * sizeof(float))};
-  s[5].pieces = {bdev(h->r_act, cap * D * sizeof(float))};
-  s[6].pieces = {bdev(h->r_rew, cap * sizeof(float))};
-  s[7].pieces = {bdev(h->r_done, cap * sizeof(float))};
-  if (h->per) s[8].pieces = {bdev(h->t_sum, 2 * h->per_C * sizeof(double)), bdev(h->t_min, 2 * h->per_C * sizeof(double))};
-  s[9].pieces = {bdev(h->max_prio, sizeof(float)), bdev(h->d_beta, sizeof(float))};
-  for (int i = 0; i < 10; ++i) s[i].tag = kBdqTags[i + 2];
+  std::vector<StateSection> s = adam_sections(h->P, 2 * h->n_train, h->Mo, h->Vo, h->n_train);
+  for (auto& r : h->replay.state_sections(live)) s.push_back(std::move(r));
+  if (h->rms_mean) s.push_back(rms_section(&h->rms_count, h->rms_mean, h->rms_var, h->E));
   return s;
 }
 
@@ -931,19 +789,10 @@ int b2g_bdq_state_save(b2g_bdq* h, const char* path) {
   CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
   uint32_t eps_bits;
   memcpy(&eps_bits, &h->eps_value, sizeof eps_bits);
-  int64_t hv[4] = {h->r_size, h->r_pos, h->n_updates, (int64_t)eps_bits};
-  std::vector<StateSection> secs(2);
-  secs[0].tag = kBdqTags[0]; secs[0].pieces = {StatePiece{hv, nullptr, sizeof hv}};
-  secs[1].tag = kBdqTags[1]; secs[1].pieces = {StatePiece{cnt, nullptr, sizeof cnt}};
-  for (auto& s : bdq_device_sections(h, h->r_size)) secs.push_back(std::move(s));
-  if (h->rms_mean) {
-    StateSection r;
-    r.tag = kBdqRmsTag;
-    r.pieces = {StatePiece{&h->rms_count, nullptr, sizeof(double)}, bdev(h->rms_mean, h->E * sizeof(double)),
-                bdev(h->rms_var, h->E * sizeof(double))};
-    secs.push_back(std::move(r));
-  }
-  return state_write(path, STATE_KIND_BDQ, bdq_fingerprint_rms(h), secs);
+  int64_t hv[4] = {h->replay.size, h->replay.pos, h->n_updates, (int64_t)eps_bits};
+  std::vector<StateSection> secs = host_sections(hv, sizeof hv, cnt, sizeof cnt);
+  for (auto& s : bdq_device_sections(h, h->replay.size)) secs.push_back(std::move(s));
+  return state_write(path, STATE_KIND_BDQ, fp_with_rms(bdq_fingerprint(h), h->rms_mean), secs);
 }
 
 int b2g_bdq_state_load(b2g_bdq* h, const char* path) {
@@ -952,58 +801,33 @@ int b2g_bdq_state_load(b2g_bdq* h, const char* path) {
   CK(cudaSetDevice(h->cfg.device));
   // ---- everything is checked before the handle changes
   StateReader rd;
-  if (int rc = rd.open(path, STATE_KIND_BDQ, bdq_fingerprint_rms(h))) {
-    // a file with one fingerprint field more or fewer than this handle: say which side owns obs_rms
-    const std::string msg = g_b2g_err;
-    StateReader other;
-    std::vector<FpField> fp = bdq_fingerprint(h);
-    if (!h->rms_mean) fp.push_back(fp_int("obs_rms", 1));
-    if (other.open(path, STATE_KIND_BDQ, fp) == 0)
-      return b2g_fail(B2G_EINVAL, h->rms_mean ? "the state file has no obs_rms, but this handle owns the observation statistics (b2g_bdq_obs_rms_set)"
-                                              : "the state file carries obs_rms: call b2g_bdq_obs_rms_set on this handle before loading it");
-    return b2g_fail(rc, msg);
-  }
-  const int n_sec = (int)(sizeof kBdqTags / sizeof kBdqTags[0]);
-  const int n_file = n_sec + (h->rms_mean ? 1 : 0);
-  if (rd.n_sections() != n_file || (h->rms_mean && (rd.tag(n_sec) != kBdqRmsTag || rd.bytes(n_sec) != (uint64_t)(2 * h->E + 1) * sizeof(double))))
-    return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a BDQ learner");
-  for (int i = 0; i < n_sec; ++i)
-    if (rd.tag(i) != kBdqTags[i]) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a BDQ learner");
+  if (int rc = state_open_rms(rd, path, STATE_KIND_BDQ, bdq_fingerprint(h), h->rms_mean, "b2g_bdq_obs_rms_set")) return rc;
+  if (int rc = state_check_tags(rd, bdq_device_sections(h, 0), "BDQ")) return rc;
   int64_t hv[4];
   long long cnt[8];
   if (rd.bytes(0) != sizeof hv || rd.bytes(1) != sizeof cnt)
     return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
   if (int rc = rd.read_host(0, hv, sizeof hv)) return rc;
-  const int64_t cap = h->cfg.buffer_capacity;
-  if (hv[0] < 0 || hv[0] > cap || hv[1] < 0 || hv[1] >= cap || (hv[0] < cap && hv[1] != hv[0]) || hv[2] < 0)
-    return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
-  std::vector<StateSection> dev = bdq_device_sections(h, hv[0]);
-  for (int i = 0; i < (int)dev.size(); ++i)
-    if (rd.bytes(i + 2) != dev[i].bytes())
-      return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  if (!h->replay.valid(hv[0], hv[1]) || hv[2] < 0) return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
+  const std::vector<StateSection> dev = bdq_device_sections(h, hv[0]);
+  if (int rc = state_check_lengths(rd, dev)) return rc;
   if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
   // ---- from here on a failure leaves the handle unusable until a load succeeds
   CK(cudaStreamSynchronize(h->stream));
-  h->broken = true;
-  for (int i = 0; i < (int)dev.size(); ++i)
-    if (int rc = rd.read_pieces(i + 2, dev[i].pieces)) return rc;
-  if (h->rms_mean) {
-    double count = 0.0;
-    if (int rc = rd.read_pieces(n_sec, {StatePiece{&count, nullptr, sizeof(double)}, bdev(h->rms_mean, h->E * sizeof(double)),
-                                        bdev(h->rms_var, h->E * sizeof(double))})) return rc;
-    h->rms_count = count;
-    obs_rms_update_launch(nullptr, nullptr, nullptr, 0, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, 0, 0,
-                          h->stream);
-    CK(cudaStreamSynchronize(h->stream));
-  }
-  h->ob_n = 0;         // the staged observations are not part of the file: a resumed run starts a fresh episode
-  CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
-  h->r_size = hv[0]; h->r_pos = hv[1]; h->n_updates = hv[2];
-  const uint32_t eps_bits = (uint32_t)hv[3];
-  memcpy(&h->eps_value, &eps_bits, sizeof eps_bits);
-  // the captured step graph stays valid: it holds device pointers and configuration; size and Philox step are device counters
-  h->broken = false;
-  return 0;
+  return state_read_device(rd, dev, &h->broken, [&] {
+    if (h->rms_mean) {
+      obs_rms_update_launch(nullptr, nullptr, nullptr, 0, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, 0, 0,
+                            h->stream);
+      CK(cudaStreamSynchronize(h->stream));
+    }
+    h->ob_n = 0;       // the staged observations are not part of the file: a resumed run starts a fresh episode
+    CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
+    h->replay.size = hv[0]; h->replay.pos = hv[1]; h->n_updates = hv[2];
+    const uint32_t eps_bits = (uint32_t)hv[3];
+    memcpy(&h->eps_value, &eps_bits, sizeof eps_bits);
+    // the captured step graph stays valid: it holds device pointers and configuration; size and Philox step are device counters
+    return 0;
+  });
 }
 
 }  // extern "C"

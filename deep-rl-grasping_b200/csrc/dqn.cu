@@ -17,7 +17,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <map>
 #include <string>
 #include <vector>
 
@@ -30,13 +29,6 @@
 using namespace b2g;
 
 namespace {
-
-struct DTensor {
-  std::string name;
-  int rows, cols, stride;   // zip shape [rows, cols] (biases: rows = 1), device row stride
-  int64_t off;              // float offset inside P (online) -- the target copy sits at off + n_train
-  bool is_weight;
-};
 
 // metric slots (prep_kernel zeroes all MET_COUNT; optim_kernel accumulates the post-clip squared norm at MET_GN_PI)
 constexpr int DMET_LOSS = 0, DMET_MEANQ = 1, DMET_ABSTD = 2, DMET_GN2 = 3, DMET_NCLIP = 4;
@@ -155,15 +147,13 @@ __global__ void dqn_act_kernel(const float* __restrict__ A, const float* __restr
 struct b2g_dqn {
   b2g_dqn_cfg cfg{};
   int B = 0, n = 0, NAS = 0, H0 = 0, H1 = 0, XS = 0, E = 0;
-  std::vector<DTensor> tensors;
-  std::map<std::string, int> tindex;
+  ParamTable params;           // deepq/eps, the online tensors, then their target copies at off + n_train
   int64_t n_train = 0;
   float *P = nullptr, *Mo = nullptr, *Vo = nullptr, *G = nullptr, *metrics = nullptr;
   float eps_value = 1.0f;      // deepq/eps (exploration epsilon variable of the zip)
   cudaStream_t stream = nullptr;
   std::vector<void*> allocs;
-  float *r_obs = nullptr, *r_next = nullptr, *r_act = nullptr, *r_rew = nullptr, *r_done = nullptr;
-  int64_t r_size = 0, r_pos = 0;
+  TransitionReplay replay;
   double *d_mean = nullptr, *d_istd = nullptr, *d_normc = nullptr;
   double* d_normc_act = nullptr;   // the actor's gather: observations arrive as the network sees them (no normalisation)
   float *X = nullptr, *Xn = nullptr, *Xscratch = nullptr;
@@ -183,17 +173,11 @@ struct b2g_dqn {
   std::vector<GemmGroup> fwd, bwd, act;
   long long n_updates = 0;
   float* h_met = nullptr;
-  bool per = false;
-  double *t_sum = nullptr, *t_min = nullptr;
-  long long per_C = 0;
-  float *max_prio = nullptr, *d_beta = nullptr, *prio_out = nullptr;
   cudaGraphExec_t graph_exec = nullptr;
   bool use_graph = true;
   bool broken = false;         // a training-state load failed after it began writing: only destroy / load are accepted
-  const DTensor& t(const std::string& nm) const { return tensors[tindex.at(nm)]; }
-  float* p(const std::string& nm) { return P + t(nm).off; }
-  float* g(const std::string& nm) { return G + t(nm).off; }
-  float* pt(const std::string& nm) { return P + n_train + t(nm).off; }
+  float* p(const std::string& nm) { return P + params.off(nm); }
+  float* g(const std::string& nm) { return G + params.off(nm); }
 };
 
 namespace {
@@ -201,13 +185,11 @@ const char* const kTower[2] = {"action_value", "state_value"};
 const std::string kOnline = "deepq/model", kTarget = "deepq/target_q_func/model";
 
 std::string fcname(int i) { return i == 0 ? "fully_connected" : "fully_connected_" + std::to_string(i); }
-std::string lname(int tw, int layer) { return kOnline + "/" + kTower[tw] + "/" + fcname(layer); }
+std::string lname(int tw, int layer, const std::string& scope = kOnline) { return scope + "/" + kTower[tw] + "/" + fcname(layer); }
 
+// an online tensor of the zip: weights [rows, cols] at row stride `stride`, biases [cols] padded to `stride`
 void add_t(b2g_dqn* h, const std::string& name, int rows, int cols, bool w, int stride, int64_t& off) {
-  DTensor t{name, rows, cols, stride, off, w};
-  off += ((int64_t)(w ? rows * stride : stride) + 31) / 32 * 32;
-  h->tindex[name] = (int)h->tensors.size();
-  h->tensors.push_back(t);
+  h->params.add(name, w ? rows : 1, cols, w ? 2 : 1, stride, arena_take(off, w ? (int64_t)rows * stride : stride), true);
 }
 
 int build(b2g_dqn* h) {
@@ -219,10 +201,7 @@ int build(b2g_dqn* h) {
   DT(kH0, iota_tab(std::max(obs, H0) + 8, H0)) DT(kH1, iota_tab(std::max(H0, H1) + 8, H1)) DT(kNAS, iota_tab(H1 + 8, NAS))
   DT(k4, iota_tab(H1 + 8, 4))
 #undef DT
-  auto W = [&](int e, int tw, int layer, const char* wb) {
-    const std::string nm = lname(tw, layer) + wb;
-    return e == 2 ? h->pt(nm) : h->p(nm);
-  };
+  auto W = [&](int e, int tw, int layer, const char* wb) { return h->p(lname(tw, layer, e == 2 ? kTarget : kOnline) + wb); };
   // ---------------- forward: each layer of both towers for the 3 evaluations; the act groups hold evaluation 0 only
   for (int layer = 0; layer < 3; ++layer) {
     GemmGroup g, a;
@@ -289,7 +268,8 @@ int build(b2g_dqn* h) {
   for (auto& g : h->act) if (int rc = finalize_tiles(g, h->allocs, h->stream)) return rc;
   // the clip jobs: every online tensor over its padded rows (pad columns hold zero gradients)
   std::vector<ClipJob> jobs;
-  for (const DTensor& t : h->tensors) jobs.push_back(ClipJob{(long long)t.off, t.is_weight ? t.rows * t.stride : t.stride});
+  for (const ParamEntry& t : h->params.entries())
+    if (t.grad) jobs.push_back(ClipJob{(long long)t.off, (int)(t.rows * t.stride)});
   h->n_clip = (int)jobs.size();
   if (int rc = dev_alloc(h->allocs, h->stream, &h->clip_jobs, jobs.size(), false)) return rc;
   CK(cudaMemcpyAsync(h->clip_jobs, jobs.data(), jobs.size() * sizeof(ClipJob), cudaMemcpyHostToDevice, h->stream));
@@ -299,25 +279,17 @@ int build(b2g_dqn* h) {
 
 GatherArgs dgather(b2g_dqn* h, bool from_replay, bool with_next) {
   GatherArgs g{};
-  g.obs = from_replay ? h->r_obs : h->s_obs;
-  g.next_obs = with_next ? (from_replay ? h->r_next : h->s_next) : nullptr;
-  g.act = with_next ? (from_replay ? h->r_act : h->s_act) : nullptr;
-  g.rew = from_replay ? h->r_rew : h->s_rew;
-  g.done = from_replay ? h->r_done : h->s_done;
+  g.obs = from_replay ? h->replay.obs : h->s_obs;
+  g.next_obs = with_next ? (from_replay ? h->replay.next : h->s_next) : nullptr;
+  g.act = with_next ? (from_replay ? h->replay.act : h->s_act) : nullptr;
+  g.rew = from_replay ? h->replay.rew : h->s_rew;
+  g.done = from_replay ? h->replay.done : h->s_done;
   g.indices = from_replay ? h->indices : nullptr;
   g.mean = h->d_mean; g.var = h->d_istd; g.normc = h->d_normc;
   g.B = h->B; g.H = 0; g.W = h->cfg.obs_dim; g.Cimg = 0; g.scale = 1.f;
   g.F_pi = h->Xscratch; g.F_v = h->X; g.F_t = h->Xn; g.FS = h->XS; g.feat_col = 0;
   g.rew_out = h->rew_n; g.done_out = h->done_n; g.n_act = 1;
   return g;
-}
-
-PerArgs dper(b2g_dqn* h, unsigned long long seed) {
-  PerArgs pr{};
-  pr.tsum = h->t_sum; pr.tmin = h->t_min; pr.C = h->per_C; pr.max_prio = h->max_prio; pr.counters = h->counters; pr.seed = seed;
-  pr.B = h->B; pr.alpha = h->cfg.per_alpha; pr.eps = h->cfg.per_eps; pr.beta = h->d_beta; pr.indices = h->indices; pr.weights = h->weights;
-  pr.prio_out = h->prio_out; pr.td = h->td; pr.D = 1;
-  return pr;
 }
 
 int dqn_issue(b2g_dqn* h, bool sampled, bool apply, const float* weights) {
@@ -327,8 +299,9 @@ int dqn_issue(b2g_dqn* h, bool sampled, bool apply, const float* weights) {
   pa.indices = h->indices; pa.eps = h->eps_dummy; pa.B = h->B; pa.A = 1; pa.replay_size = nullptr;
   pa.seed = h->cfg.seed; pa.gen = sampled ? 1 : 0; pa.apply = apply ? 1 : 0;
   prep_launch(pa, s);
-  const PerArgs pr = dper(h, pa.seed);
-  if (h->per && sampled) { per_sample_launch(pr, s); weights = h->weights; }   // overwrites the uniform draw
+  const bool per = h->replay.per;
+  const PerArgs pr = h->replay.per_args(h->counters, pa.seed, h->B, h->indices, h->weights, h->td, 1);
+  if (per && sampled) { per_sample_launch(pr, s); weights = h->weights; }   // overwrites the uniform draw
   gather_launch(dgather(h, sampled, true), s);
   CK(cudaMemsetAsync(h->G, 0, (size_t)h->n_train * sizeof(float), s));
   for (auto& g : h->fwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
@@ -341,7 +314,7 @@ int dqn_issue(b2g_dqn* h, bool sampled, bool apply, const float* weights) {
   dqn_tail_kernel<<<(h->B + 127) / 128, 128, 0, s>>>(t);
   for (auto& g : h->bwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
   dqn_clip_kernel<<<h->n_clip, kClipThreads, 0, s>>>(h->G, h->clip_jobs, kGradClip, h->metrics);
-  if (h->per && sampled) per_write_launch(pr, h->indices, 0, h->cfg.buffer_capacity, h->B, 1, s);   // update_priorities(|td| + eps)
+  if (per && sampled) per_write_launch(pr, h->indices, 0, h->cfg.buffer_capacity, h->B, 1, s);   // update_priorities(|td| + eps)
   OptimArgs oa{};
   oa.P = h->P; oa.Mo = h->Mo; oa.Vo = h->Vo; oa.G = h->G; oa.T = h->P + h->n_train;
   oa.n_pi = (int)h->n_train; oa.n_values = 0; oa.n_ent = 0; oa.n_target = 0;
@@ -389,7 +362,6 @@ int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out) {
   if (int rc = check_device(cfg->device)) return rc;
   b2g_dqn* h = new b2g_dqn();
   h->cfg = *cfg;
-  h->per = cfg->prioritized_replay != 0;
   const char* ng = getenv("B2G_NO_GRAPH");
   h->use_graph = !(ng && ng[0] == '1');
   h->B = cfg->batch; h->n = cfg->n_actions; h->NAS = (cfg->n_actions + 3) / 4 * 4;
@@ -397,7 +369,8 @@ int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out) {
   h->XS = (cfg->obs_dim + 1 + 7) / 8 * 8;
   auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_dqn_destroy(h); g_b2g_err = keep; return rc; };
   if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream"));
-  // parameter inventory in zip order (oracle/dqn_ref.py param_specs)
+  // parameter inventory in zip order (oracle/dqn_ref.py all_specs)
+  h->params.add_scalar("deepq/eps", &h->eps_value);
   int64_t off = 0;
   for (int tw = 0; tw < 2; ++tw) {
     const int no = tw == 0 ? h->n : 1, so = tw == 0 ? h->NAS : 4;
@@ -409,13 +382,14 @@ int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out) {
     add_t(h, lname(tw, 2) + "/biases", 1, no, false, so, off);
   }
   h->n_train = off;
+  h->params.add_copies(1, h->params.count() - 1, kOnline, kTarget, h->n_train);
   int rc = 0;
   const int B = h->B;
 #define DA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
   DA(h->P, 2 * h->n_train); DA(h->Mo, h->n_train); DA(h->Vo, h->n_train); DA(h->G, h->n_train); DA(h->metrics, MET_COUNT);
   DA(h->counters, 8); DA(h->step_consts, 4); DA(h->d_lr, 1);
   const int64_t cap = cfg->buffer_capacity;
-  DA(h->r_obs, cap * h->E); DA(h->r_next, cap * h->E); DA(h->r_act, cap); DA(h->r_rew, cap); DA(h->r_done, cap);
+  if ((rc = h->replay.init(h->allocs, h->stream, cap, h->E, 1, B, cfg->prioritized_replay != 0, cfg->per_alpha, cfg->per_eps))) return bail(rc);
   DA(h->d_mean, h->E); DA(h->d_istd, h->E); DA(h->d_normc, 8); DA(h->d_normc_act, 8);
   DA(h->X, (size_t)B * h->XS); DA(h->Xn, (size_t)B * h->XS); DA(h->Xscratch, (size_t)B * h->XS);
   for (int e = 0; e < 3; ++e) {
@@ -428,15 +402,6 @@ int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out) {
   DA(h->rew_n, B); DA(h->done_n, B); DA(h->weights, B); DA(h->eps_dummy, B + 8); DA(h->indices, B + 4); DA(h->act_idx_out, B);
   DA(h->q_rows, B * h->n);
   DA(h->s_obs, (size_t)B * h->E); DA(h->s_next, (size_t)B * h->E); DA(h->s_act, B); DA(h->s_rew, B); DA(h->s_done, B);
-  DA(h->d_beta, 1); DA(h->max_prio, 1); DA(h->prio_out, B);
-  if (h->per) {
-    h->per_C = 1;
-    while (h->per_C < cap) h->per_C <<= 1;
-    DA(h->t_sum, 2 * h->per_C); DA(h->t_min, 2 * h->per_C);
-    per_init_launch(h->t_sum, h->t_min, 2 * h->per_C, h->max_prio, h->stream);
-    const float beta0 = 0.4f;
-    if (cudaMemcpyAsync(h->d_beta, &beta0, sizeof(float), cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "per init"));
-  }
 #undef DA
   if (cudaMallocHost((void**)&h->h_met, MET_COUNT * sizeof(float)) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "cudaMallocHost"));
   {
@@ -454,59 +419,15 @@ int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out) {
   return 0;
 }
 
-int b2g_dqn_param_count(const b2g_dqn* h) { B2G_USABLE(h); return h ? 1 + 2 * (int)h->tensors.size() : 0; }
-
-// index 0 = deepq/eps; 1..T = online tensors; T+1..2T = target tensors (names and order as in the zips)
+int b2g_dqn_param_count(const b2g_dqn* h) { return param_count(h); }
 int b2g_dqn_param_info(const b2g_dqn* h, int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim) {
-  B2G_USABLE(h);
-  if (!h || idx < 0 || idx >= b2g_dqn_param_count(h) || !name) return b2g_fail(B2G_EINVAL, "bad tensor index");
-  std::string nm = "deepq/eps";
-  int64_t r = 1, c = 1;
-  int nd = 0;
-  if (idx > 0) {
-    const int T = (int)h->tensors.size();
-    const DTensor& t = h->tensors[(idx - 1) % T];
-    nm = (idx - 1) < T ? t.name : kTarget + t.name.substr(kOnline.size());
-    r = t.rows; c = t.cols; nd = t.is_weight ? 2 : 1;
-  }
-  snprintf(name, name_cap, "%s", nm.c_str());
-  if (rows) *rows = r;
-  if (cols) *cols = c;
-  if (ndim) *ndim = nd;
-  return 0;
+  return param_info(h, idx, name, name_cap, rows, cols, ndim);
 }
-
-static int dqn_copy(b2g_dqn* h, const char* name, float* arena_online, float* host, size_t numel, bool to_host, bool allow_target) {
-  if (!h || !name || !host) return b2g_fail(B2G_EINVAL, "NULL argument");
-  std::string nm(name);
-  if (nm.size() > 2 && nm.compare(nm.size() - 2, 2, ":0") == 0) nm.resize(nm.size() - 2);
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  if (nm == "deepq/eps") {
-    if (numel != 1) return b2g_fail(B2G_EINVAL, "deepq/eps is a scalar");
-    if (to_host) host[0] = h->eps_value; else h->eps_value = host[0];
-    return 0;
-  }
-  bool target = false;
-  if (nm.compare(0, kTarget.size(), kTarget) == 0) { target = true; nm = kOnline + nm.substr(kTarget.size()); }
-  if (target && !allow_target) return b2g_fail(B2G_EINVAL, "not a trainable variable");
-  auto it = h->tindex.find(nm);
-  if (it == h->tindex.end()) return b2g_fail(B2G_EINVAL, std::string("unknown variable: ") + name);
-  const DTensor& t = h->tensors[it->second];
-  const size_t rows = t.is_weight ? t.rows : 1, cols = t.cols;
-  if (numel != rows * cols) return b2g_fail(B2G_EINVAL, std::string("size mismatch for ") + name);
-  float* dev = arena_online + t.off + (target ? h->n_train : 0);
-  // repack between the zip layout [rows, cols] and the device row stride
-  if (to_host) CK(cudaMemcpy2D(host, cols * sizeof(float), dev, t.stride * sizeof(float), cols * sizeof(float), rows, cudaMemcpyDeviceToHost));
-  else CK(cudaMemcpy2D(dev, t.stride * sizeof(float), host, cols * sizeof(float), cols * sizeof(float), rows, cudaMemcpyHostToDevice));
-  return 0;
-}
-int b2g_dqn_get_param(b2g_dqn* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return dqn_copy(h, name, h ? h->P : nullptr, dst, numel, true, true); }
+int b2g_dqn_get_param(b2g_dqn* h, const char* name, float* dst, size_t numel) { return param_copy(h, name, ParamCopy::Get, dst, numel); }
 int b2g_dqn_set_param(b2g_dqn* h, const char* name, const float* src, size_t numel) {
-  B2G_USABLE(h);
-  return dqn_copy(h, name, h ? h->P : nullptr, const_cast<float*>(src), numel, false, true);
+  return param_copy(h, name, ParamCopy::Set, const_cast<float*>(src), numel);
 }
-int b2g_dqn_get_grad(b2g_dqn* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return dqn_copy(h, name, h ? h->G : nullptr, dst, numel, true, false); }
+int b2g_dqn_get_grad(b2g_dqn* h, const char* name, float* dst, size_t numel) { return param_copy(h, name, ParamCopy::GetGrad, dst, numel); }
 
 // Every action must be an integer in [0, n_actions): the tail kernel indexes the Q row with it.  The values are read on the host
 // (a device array is copied down first), before anything is stored or launched.
@@ -532,31 +453,9 @@ int b2g_dqn_replay_add(b2g_dqn* h, const float* obs, const float* act, const flo
   if (!h || !obs || !act || !rew || !next_obs || !done || n < 0) return b2g_fail(B2G_EINVAL, "NULL argument");
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = dqn_check_actions(h, act, n)) return rc;
-  const int64_t cap = h->cfg.buffer_capacity;
-  int64_t done_n = 0;
-  while (done_n < n) {
-    const int64_t chunk = std::min(n - done_n, cap - h->r_pos);
-    const size_t E = h->E;
-    CK(cudaMemcpyAsync(h->r_obs + h->r_pos * E, obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_next + h->r_pos * E, next_obs + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_act + h->r_pos, act + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_rew + h->r_pos, rew + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_done + h->r_pos, done + done_n, chunk * sizeof(float), cudaMemcpyDefault, h->stream));
-    if (h->per) {        // new transitions enter with the running maximum priority ([SB2] PrioritizedReplayBuffer.add)
-      const PerArgs pr = dper(h, h->cfg.seed);
-      for (int64_t o = 0; o < chunk; o += 1024)
-        per_write_launch(pr, nullptr, h->r_pos + o, cap, (int)std::min<int64_t>(1024, chunk - o), 0, h->stream);
-    }
-    h->r_pos = (h->r_pos + chunk) % cap;
-    h->r_size = std::min(cap, h->r_size + chunk);
-    done_n += chunk;
-  }
-  const long long sz = h->r_size;
-  CK(cudaMemcpyAsync(h->counters + 5, &sz, sizeof(long long), cudaMemcpyHostToDevice, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return 0;
+  return h->replay.add(obs, act, rew, next_obs, done, n, h->counters, h->stream);
 }
-int64_t b2g_dqn_replay_size(const b2g_dqn* h) { B2G_USABLE(h); return h ? h->r_size : 0; }
+int64_t b2g_dqn_replay_size(const b2g_dqn* h) { B2G_USABLE(h); return h ? h->replay.size : 0; }
 
 int b2g_dqn_set_norm_stats(b2g_dqn* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs, double clip_rew, double eps,
                            int norm_obs, int norm_reward) {
@@ -579,7 +478,7 @@ int b2g_dqn_set_norm_stats(b2g_dqn* h, const double* obs_mean, const double* obs
 int b2g_dqn_step(b2g_dqn* h, int n_steps, float lr, b2g_dqn_metrics* out) {
   B2G_USABLE(h);
   if (!h || n_steps < 0) return b2g_fail(B2G_EINVAL, "bad argument");
-  if (h->r_size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
+  if (h->replay.size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
   if (h->use_graph && !h->graph_exec)       // the whole step (~14 launches of tiny layers) replays as one graph
@@ -595,21 +494,13 @@ int b2g_dqn_step(b2g_dqn* h, int n_steps, float lr, b2g_dqn_metrics* out) {
 int b2g_dqn_set_per_beta(b2g_dqn* h, float beta) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  CK(cudaMemcpy(h->d_beta, &beta, sizeof(float), cudaMemcpyHostToDevice));
-  return 0;
+  return h->replay.set_beta(beta, h->cfg.device, h->stream);
 }
 
 int b2g_dqn_get_last_per(b2g_dqn* h, int32_t* slots, float* weights, float* priorities) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  if (slots) CK(cudaMemcpy(slots, h->indices, h->B * sizeof(int32_t), cudaMemcpyDeviceToHost));
-  if (weights) CK(cudaMemcpy(weights, h->weights, h->B * sizeof(float), cudaMemcpyDeviceToHost));
-  if (priorities) CK(cudaMemcpy(priorities, h->prio_out, h->B * sizeof(float), cudaMemcpyDeviceToHost));
-  return 0;
+  return h->replay.get_last(h->indices, h->weights, h->B, slots, weights, priorities, h->cfg.device, h->stream);
 }
 
 int b2g_dqn_step_explicit(b2g_dqn* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done,
@@ -678,27 +569,10 @@ std::vector<FpField> dqn_fingerprint(const b2g_dqn* h) {
           fp_int("prioritized_replay", c.prioritized_replay), fp_real("per_alpha", c.per_alpha), fp_real("per_eps", c.per_eps)};
 }
 
-const uint32_t kDqnTags[] = {state_tag("HOST"), state_tag("CNTR"), state_tag("PARM"), state_tag("ADMM"), state_tag("ADMV"),
-                             state_tag("ROBS"), state_tag("RNXT"), state_tag("RACT"), state_tag("RREW"), state_tag("RDON"),
-                             state_tag("PERT"), state_tag("PERS")};
-
-StatePiece ddev(void* p, size_t bytes) { StatePiece s; s.dev = p; s.bytes = bytes; return s; }
-
 // sections 2.. (parameters .. prioritised-replay scalars) of a handle holding `live` replay rows
 std::vector<StateSection> dqn_device_sections(b2g_dqn* h, int64_t live) {
-  const size_t cap = (size_t)h->cfg.buffer_capacity, E = h->E;
-  std::vector<StateSection> s(10);
-  s[0].pieces = {ddev(h->P, 2 * h->n_train * sizeof(float))};
-  s[1].pieces = {ddev(h->Mo, h->n_train * sizeof(float))};
-  s[2].pieces = {ddev(h->Vo, h->n_train * sizeof(float))};
-  s[3].pieces = {ddev(h->r_obs, live * E * sizeof(float))};       // rows [0, size) are the live ones
-  s[4].pieces = {ddev(h->r_next, live * E * sizeof(float))};
-  s[5].pieces = {ddev(h->r_act, cap * sizeof(float))};
-  s[6].pieces = {ddev(h->r_rew, cap * sizeof(float))};
-  s[7].pieces = {ddev(h->r_done, cap * sizeof(float))};
-  if (h->per) s[8].pieces = {ddev(h->t_sum, 2 * h->per_C * sizeof(double)), ddev(h->t_min, 2 * h->per_C * sizeof(double))};
-  s[9].pieces = {ddev(h->max_prio, sizeof(float)), ddev(h->d_beta, sizeof(float))};
-  for (int i = 0; i < 10; ++i) s[i].tag = kDqnTags[i + 2];
+  std::vector<StateSection> s = adam_sections(h->P, 2 * h->n_train, h->Mo, h->Vo, h->n_train);
+  for (auto& r : h->replay.state_sections(live)) s.push_back(std::move(r));
   return s;
 }
 
@@ -715,11 +589,9 @@ int b2g_dqn_state_save(b2g_dqn* h, const char* path) {
   CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
   uint32_t eps_bits;
   memcpy(&eps_bits, &h->eps_value, sizeof eps_bits);
-  int64_t hv[4] = {h->r_size, h->r_pos, h->n_updates, (int64_t)eps_bits};
-  std::vector<StateSection> secs(2);
-  secs[0].tag = kDqnTags[0]; secs[0].pieces = {StatePiece{hv, nullptr, sizeof hv}};
-  secs[1].tag = kDqnTags[1]; secs[1].pieces = {StatePiece{cnt, nullptr, sizeof cnt}};
-  for (auto& s : dqn_device_sections(h, h->r_size)) secs.push_back(std::move(s));
+  int64_t hv[4] = {h->replay.size, h->replay.pos, h->n_updates, (int64_t)eps_bits};
+  std::vector<StateSection> secs = host_sections(hv, sizeof hv, cnt, sizeof cnt);
+  for (auto& s : dqn_device_sections(h, h->replay.size)) secs.push_back(std::move(s));
   return state_write(path, STATE_KIND_DQN, dqn_fingerprint(h), secs);
 }
 
@@ -729,35 +601,26 @@ int b2g_dqn_state_load(b2g_dqn* h, const char* path) {
   // ---- everything is checked before the handle changes
   StateReader rd;
   if (int rc = rd.open(path, STATE_KIND_DQN, dqn_fingerprint(h))) return rc;
-  const int n_sec = (int)(sizeof kDqnTags / sizeof kDqnTags[0]);
-  if (rd.n_sections() != n_sec) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a DQN learner");
-  for (int i = 0; i < n_sec; ++i)
-    if (rd.tag(i) != kDqnTags[i]) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a DQN learner");
+  if (int rc = state_check_tags(rd, dqn_device_sections(h, 0), "DQN")) return rc;
   int64_t hv[4];
   long long cnt[8];
   if (rd.bytes(0) != sizeof hv || rd.bytes(1) != sizeof cnt)
     return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
   if (int rc = rd.read_host(0, hv, sizeof hv)) return rc;
-  const int64_t cap = h->cfg.buffer_capacity;
-  if (hv[0] < 0 || hv[0] > cap || hv[1] < 0 || hv[1] >= cap || (hv[0] < cap && hv[1] != hv[0]) || hv[2] < 0)
-    return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
-  std::vector<StateSection> dev = dqn_device_sections(h, hv[0]);
-  for (int i = 0; i < (int)dev.size(); ++i)
-    if (rd.bytes(i + 2) != dev[i].bytes())
-      return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  if (!h->replay.valid(hv[0], hv[1]) || hv[2] < 0) return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
+  const std::vector<StateSection> dev = dqn_device_sections(h, hv[0]);
+  if (int rc = state_check_lengths(rd, dev)) return rc;
   if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
   // ---- from here on a failure leaves the handle unusable until a load succeeds
   CK(cudaStreamSynchronize(h->stream));
-  h->broken = true;
-  for (int i = 0; i < (int)dev.size(); ++i)
-    if (int rc = rd.read_pieces(i + 2, dev[i].pieces)) return rc;
-  CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
-  h->r_size = hv[0]; h->r_pos = hv[1]; h->n_updates = hv[2];
-  const uint32_t eps_bits = (uint32_t)hv[3];
-  memcpy(&h->eps_value, &eps_bits, sizeof eps_bits);
-  // the captured step graph stays valid: it holds device pointers and configuration; size and Philox step are device counters
-  h->broken = false;
-  return 0;
+  return state_read_device(rd, dev, &h->broken, [&] {
+    CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
+    h->replay.size = hv[0]; h->replay.pos = hv[1]; h->n_updates = hv[2];
+    const uint32_t eps_bits = (uint32_t)hv[3];
+    memcpy(&h->eps_value, &eps_bits, sizeof eps_bits);
+    // the captured step graph stays valid: it holds device pointers and configuration; size and Philox step are device counters
+    return 0;
+  });
 }
 
 }  // extern "C"

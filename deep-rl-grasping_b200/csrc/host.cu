@@ -1,7 +1,8 @@
-// libb200grasp: host runtime shared by the SAC, BDQ and encoder handles (declarations and contracts in host.cuh), and the
+// libb200grasp: host runtime shared by the learner and encoder handles (declarations and contracts in host.cuh), and the
 // library-wide part of the C ABI.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
+#include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -87,6 +88,57 @@ int upload_lr(float* d_lr, float* cur_lr, float lr, cudaStream_t s) {
     CK(cudaMemcpy(d_lr, &lr, sizeof(float), cudaMemcpyHostToDevice));
     *cur_lr = lr;
   }
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ named parameters
+void ParamTable::add(const std::string& name, int64_t rows, int64_t cols, int ndim, int stride, int64_t off, bool grad) {
+  index_[name] = (int)entries_.size();
+  entries_.push_back(ParamEntry{name, rows, cols, ndim, stride, off, grad, nullptr});
+}
+
+void ParamTable::add_scalar(const std::string& name, float* v) {
+  index_[name] = (int)entries_.size();
+  entries_.push_back(ParamEntry{name, 1, 1, 0, 1, -1, false, v});
+}
+
+void ParamTable::add_copies(int first, int n, const std::string& from_scope, const std::string& to_scope, int64_t shift) {
+  for (int i = first; i < first + n; ++i) {
+    const ParamEntry e = entries_[i];
+    add(to_scope + e.name.substr(from_scope.size()), e.rows, e.cols, e.ndim, e.stride, e.off + shift, false);
+  }
+}
+
+int ParamTable::info(int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim) const {
+  if (idx < 0 || idx >= count() || !name) return b2g_fail(B2G_EINVAL, "bad tensor index");
+  const ParamEntry& e = entries_[idx];
+  snprintf(name, name_cap, "%s", e.name.c_str());
+  if (rows) *rows = e.rows;
+  if (cols) *cols = e.cols;
+  if (ndim) *ndim = e.ndim;
+  return 0;
+}
+
+int ParamTable::copy(const char* name, ParamCopy mode, float* P, float* G, float* host, size_t numel, int device, cudaStream_t s) const {
+  if (!name || !host) return b2g_fail(B2G_EINVAL, "NULL argument");
+  std::string nm(name);
+  if (nm.size() > 2 && nm.compare(nm.size() - 2, 2, ":0") == 0) nm.resize(nm.size() - 2);
+  CK(cudaSetDevice(device));
+  CK(cudaStreamSynchronize(s));
+  const auto it = index_.find(nm);
+  if (it == index_.end()) return b2g_fail(B2G_EINVAL, std::string("unknown variable: ") + name);
+  const ParamEntry& e = entries_[it->second];
+  if (numel != (size_t)(e.rows * e.cols)) return b2g_fail(B2G_EINVAL, std::string("size mismatch for ") + name);
+  if (e.scalar) {
+    if (mode == ParamCopy::Set) *e.scalar = host[0];
+    else host[0] = *e.scalar;
+    return 0;
+  }
+  if (mode == ParamCopy::GetGrad && !e.grad) return b2g_fail(B2G_EINVAL, std::string("no gradient for ") + name);
+  float* dev = (mode == ParamCopy::GetGrad ? G : P) + e.off;
+  const size_t row = e.cols * sizeof(float), pitch = e.stride * sizeof(float);
+  if (mode == ParamCopy::Set) CK(cudaMemcpy2D(dev, pitch, host, row, row, e.rows, cudaMemcpyHostToDevice));
+  else CK(cudaMemcpy2D(host, row, dev, pitch, row, e.rows, cudaMemcpyDeviceToHost));
   return 0;
 }
 

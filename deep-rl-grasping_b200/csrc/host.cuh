@@ -1,5 +1,6 @@
-// Host runtime shared by the SAC, BDQ and encoder handles (host.cu): error state, device check, tracked device allocations,
-// offset tables, gather-GEMM descriptor groups, CUDA-graph capture, learning-rate upload and NCCL through dlopen.
+// Host runtime shared by the learner and encoder handles (host.cu): error state, device check, tracked device allocations,
+// offset tables, gather-GEMM descriptor groups, CUDA-graph capture, learning-rate upload, the named-parameter table of the BDQ,
+// DQN and PPO2 handles and NCCL through dlopen.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -66,6 +67,56 @@ int capture_graph(cudaStream_t s, const std::function<int()>& issue, cudaGraphEx
 
 // Learning rate -> the device scalar the prep kernel reads; only when it changed (the stream is drained first).
 int upload_lr(float* d_lr, float* cur_lr, float lr, cudaStream_t s);
+
+// ---- named parameters of the BDQ, DQN and PPO2 handles: the variables of the zip, in its order, and where each one lives
+struct ParamEntry {
+  std::string name;            // full zip name
+  int64_t rows, cols;          // zip shape [rows, cols]; rows = 1 for ndim 1, rows = cols = 1 for a scalar
+  int ndim;
+  int stride;                  // device row stride (floats)
+  int64_t off;                 // float offset into the parameter arena, and into the gradient arena when grad
+  bool grad;                   // the gradient arena holds this variable
+  float* scalar;               // a host scalar (bdq/eps, deepq/eps) instead of arena rows
+};
+enum class ParamCopy { Get, Set, GetGrad };
+
+class ParamTable {
+ public:
+  void add(const std::string& name, int64_t rows, int64_t cols, int ndim, int stride, int64_t off, bool grad);
+  void add_scalar(const std::string& name, float* v);
+  // copies of entries [first, first + n) renamed from_scope... -> to_scope..., at off + shift, without gradient (target nets)
+  void add_copies(int first, int n, const std::string& from_scope, const std::string& to_scope, int64_t shift);
+  int count() const { return (int)entries_.size(); }
+  const std::vector<ParamEntry>& entries() const { return entries_; }
+  int64_t off(const std::string& name) const { return entries_[index_.at(name)].off; }
+  // b2g_*_param_info
+  int info(int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim) const;
+  // b2g_*_get_param / _set_param / _get_grad: a trailing ":0" is ignored; the stream is drained, then the rows are repacked
+  // between the zip layout and the device row stride
+  int copy(const char* name, ParamCopy mode, float* P, float* G, float* host, size_t numel, int device, cudaStream_t s) const;
+
+ private:
+  std::vector<ParamEntry> entries_;
+  std::map<std::string, int> index_;
+};
+
+// The next 32-float-aligned arena range of n floats: returns its offset and advances off.
+inline int64_t arena_take(int64_t& off, int64_t n) { const int64_t o = off; off += (n + 31) / 32 * 32; return o; }
+
+// The parameter ABI of handle h (members params, P, G, cfg.device, stream, broken).
+template <class H>
+int param_count(const H* h) { B2G_USABLE(h); return h ? h->params.count() : 0; }
+template <class H>
+int param_info(const H* h, int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim) {
+  B2G_USABLE(h);
+  return h ? h->params.info(idx, name, name_cap, rows, cols, ndim) : b2g_fail(B2G_EINVAL, "bad tensor index");
+}
+template <class H>
+int param_copy(H* h, const char* name, ParamCopy mode, float* host, size_t numel) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL argument");
+  return h->params.copy(name, mode, h->P, h->G, host, numel, h->cfg.device, h->stream);
+}
 
 // ---- NCCL through dlopen (no link-time dependency: the library loads on machines without NCCL or a GPU)
 struct NcclUniqueId { char b[128]; };

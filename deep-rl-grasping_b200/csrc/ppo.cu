@@ -51,14 +51,6 @@ enum : int { PM_PG = 0, PM_VF, PM_ENT, PM_KL, PM_CLIP, PM_GN, PM_N = 8 };
 // device hyper-parameters of the current call: lr, cliprange, cliprange_vf (< 0: no value clipping)
 enum : int { HP_LR = 0, HP_CLIP, HP_CLIPVF, HP_N = 4 };
 
-struct PTensor {
-  std::string name;     // zip name (without the "model/" scope)
-  int rows, cols;       // zip shape (biases and logstd: rows 1)
-  int stride;           // device row stride
-  int64_t off;          // float offset inside P
-  int ndim;
-};
-
 // ---------------------------------------------------------------------------------------------------------------------------
 // kernels
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -386,8 +378,7 @@ struct PpoMb { PpoFwd f; GemmGroup b1, b0; const int* rowidx = nullptr; };
 struct b2g_ppo {
   b2g_ppo_cfg cfg{};
   int D = 0, XS = 0, A = 0, H0 = 0, H1 = 0, E = 0, T = 0, NB = 0, M = 0, NMB = 0, RMAX = 0, P_ROWS = 0;
-  std::vector<PTensor> tensors;
-  std::map<std::string, int> tindex;
+  ParamTable params;            // the zip's variables; q/w and q/b without gradient
   int64_t n_train = 0, n_total = 0;
   int64_t oW0 = 0, ob0 = 0, oW1[2]{}, ob1[2]{}, oWvf = 0, obvf = 0, oWpi = 0, obpi = 0, ols = 0;
   float *P = nullptr, *Mo = nullptr, *Vo = nullptr, *G = nullptr;
@@ -415,17 +406,16 @@ struct b2g_ppo {
   bool broken = false;
   unsigned long long act_key = 0;
   long long n_updates = 0;
-  const PTensor& tn(const std::string& nm) const { return tensors[tindex.at(nm)]; }
 };
 
 namespace {
 
 void add_t(b2g_ppo* h, const std::string& name, int rows, int cols, int stride, int64_t off, int ndim) {
-  h->tindex[name] = (int)h->tensors.size();
-  h->tensors.push_back(PTensor{name, rows, cols, stride, off, ndim});
+  h->params.add("model/" + name, rows, cols, ndim, stride, off, off < h->n_train);
 }
 
-int64_t take(int64_t& off, int64_t n) { const int64_t o = off; off += (n + 31) / 32 * 32; return o; }
+// the zip names carry the model/ scope; the bare names are accepted too
+std::string scoped(const char* name) { return strncmp(name, "model/", 6) == 0 ? name : "model/" + std::string(name); }
 
 int splits_for(int tiles, int R) {   // split-R so a launch covers about two waves of the 132 SMs, >= 64 rows per slice
   const int want = (264 + tiles - 1) / tiles;
@@ -613,11 +603,11 @@ int b2g_ppo_create(const b2g_ppo_cfg* cfg, b2g_ppo** out) {
   // ---- parameter arena: trained tensors, then q (no gradient, no moments)
   const int D = h->D, A = h->A, H0 = h->H0, H1 = h->H1;
   int64_t off = 0;
-  h->oW0 = take(off, (int64_t)D * 2 * H0); h->ob0 = take(off, 2 * H0);
-  for (int tw = 0; tw < 2; ++tw) { h->oW1[tw] = take(off, (int64_t)H0 * H1); h->ob1[tw] = take(off, H1); }
-  h->oWvf = take(off, H1); h->obvf = take(off, 1); h->oWpi = take(off, (int64_t)H1 * A); h->obpi = take(off, A); h->ols = take(off, A);
+  h->oW0 = arena_take(off, (int64_t)D * 2 * H0); h->ob0 = arena_take(off, 2 * H0);
+  for (int tw = 0; tw < 2; ++tw) { h->oW1[tw] = arena_take(off, (int64_t)H0 * H1); h->ob1[tw] = arena_take(off, H1); }
+  h->oWvf = arena_take(off, H1); h->obvf = arena_take(off, 1); h->oWpi = arena_take(off, (int64_t)H1 * A); h->obpi = arena_take(off, A); h->ols = arena_take(off, A);
   h->n_train = off;
-  const int64_t oWq = take(off, (int64_t)H1 * A), obq = take(off, A);
+  const int64_t oWq = arena_take(off, (int64_t)H1 * A), obq = arena_take(off, A);
   h->n_total = off;
   // zip order (oracle/ppo_ref.py param_specs)
   add_t(h, "pi_fc0/w", D, H0, 2 * H0, h->oW0, 2); add_t(h, "pi_fc0/b", 1, H0, H0, h->ob0, 1);
@@ -669,43 +659,19 @@ int b2g_ppo_create(const b2g_ppo_cfg* cfg, b2g_ppo** out) {
   return 0;
 }
 
-int b2g_ppo_param_count(const b2g_ppo* h) { B2G_USABLE(h); return h ? (int)h->tensors.size() : 0; }
-
+int b2g_ppo_param_count(const b2g_ppo* h) { return param_count(h); }
 int b2g_ppo_param_info(const b2g_ppo* h, int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim) {
-  B2G_USABLE(h);
-  if (!h || idx < 0 || idx >= (int)h->tensors.size() || !name) return b2g_fail(B2G_EINVAL, "bad tensor index");
-  const PTensor& t = h->tensors[idx];
-  snprintf(name, name_cap, "model/%s", t.name.c_str());
-  if (rows) *rows = t.rows;
-  if (cols) *cols = t.cols;
-  if (ndim) *ndim = t.ndim;
-  return 0;
+  return param_info(h, idx, name, name_cap, rows, cols, ndim);
 }
-
-static int ppo_copy(b2g_ppo* h, const char* name, float* arena, float* host, size_t numel, bool to_host, bool grad) {
-  if (!h || !name || !host) return b2g_fail(B2G_EINVAL, "NULL argument");
-  std::string nm(name);
-  if (nm.size() > 2 && nm.compare(nm.size() - 2, 2, ":0") == 0) nm.resize(nm.size() - 2);
-  if (nm.compare(0, 6, "model/") == 0) nm = nm.substr(6);
-  auto it = h->tindex.find(nm);
-  if (it == h->tindex.end()) return b2g_fail(B2G_EINVAL, std::string("unknown variable: ") + name);
-  const PTensor& t = h->tensors[it->second];
-  if (grad && t.off >= h->n_train) return b2g_fail(B2G_EINVAL, std::string("not a trained variable: ") + name);
-  if (numel != (size_t)t.rows * t.cols) return b2g_fail(B2G_EINVAL, std::string("size mismatch for ") + name);
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  float* dev = arena + t.off;
-  const size_t cols = t.cols, rows = t.rows;
-  if (to_host) CK(cudaMemcpy2D(host, cols * sizeof(float), dev, t.stride * sizeof(float), cols * sizeof(float), rows, cudaMemcpyDeviceToHost));
-  else CK(cudaMemcpy2D(dev, t.stride * sizeof(float), host, cols * sizeof(float), cols * sizeof(float), rows, cudaMemcpyHostToDevice));
-  return 0;
+int b2g_ppo_get_param(b2g_ppo* h, const char* name, float* dst, size_t numel) {
+  return param_copy(h, name ? scoped(name).c_str() : nullptr, ParamCopy::Get, dst, numel);
 }
-int b2g_ppo_get_param(b2g_ppo* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return ppo_copy(h, name, h ? h->P : nullptr, dst, numel, true, false); }
 int b2g_ppo_set_param(b2g_ppo* h, const char* name, const float* src, size_t numel) {
-  B2G_USABLE(h);
-  return ppo_copy(h, name, h ? h->P : nullptr, const_cast<float*>(src), numel, false, false);
+  return param_copy(h, name ? scoped(name).c_str() : nullptr, ParamCopy::Set, const_cast<float*>(src), numel);
 }
-int b2g_ppo_get_grad(b2g_ppo* h, const char* name, float* dst, size_t numel) { B2G_USABLE(h); return ppo_copy(h, name, h ? h->G : nullptr, dst, numel, true, true); }
+int b2g_ppo_get_grad(b2g_ppo* h, const char* name, float* dst, size_t numel) {
+  return param_copy(h, name ? scoped(name).c_str() : nullptr, ParamCopy::GetGrad, dst, numel);
+}
 
 int b2g_ppo_rollout_act(b2g_ppo* h, const float* obs, float* act_out) {
   B2G_USABLE(h);
@@ -861,7 +827,8 @@ std::vector<FpField> ppo_fingerprint(const b2g_ppo* h) {
           fp_int("seed", (int64_t)c.seed)};
 }
 
-const uint32_t kPpoTags[] = {state_tag("HOST"), state_tag("CNTR"), state_tag("PARM"), state_tag("ADMM"), state_tag("ADMV")};
+// sections 2..: parameters (q included) and the Adam moments
+std::vector<StateSection> ppo_device_sections(b2g_ppo* h) { return adam_sections(h->P, h->n_total, h->Mo, h->Vo, h->n_train); }
 
 }  // namespace
 
@@ -875,14 +842,8 @@ int b2g_ppo_state_save(b2g_ppo* h, const char* path) {
   long long cnt[4];
   CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
   int64_t hv[2] = {h->n_updates, 0};
-  std::vector<StateSection> secs(5);
-  secs[0].pieces = {StatePiece{hv, nullptr, sizeof hv}};
-  secs[1].pieces = {StatePiece{cnt, nullptr, sizeof cnt}};
-  StatePiece p; p.dev = h->P; p.bytes = h->n_total * sizeof(float);
-  StatePiece m; m.dev = h->Mo; m.bytes = h->n_train * sizeof(float);
-  StatePiece v; v.dev = h->Vo; v.bytes = h->n_train * sizeof(float);
-  secs[2].pieces = {p}; secs[3].pieces = {m}; secs[4].pieces = {v};
-  for (int i = 0; i < 5; ++i) secs[i].tag = kPpoTags[i];
+  std::vector<StateSection> secs = host_sections(hv, sizeof hv, cnt, sizeof cnt);
+  for (auto& s : ppo_device_sections(h)) secs.push_back(std::move(s));
   return state_write(path, STATE_KIND_PPO, ppo_fingerprint(h), secs);
 }
 
@@ -891,32 +852,23 @@ int b2g_ppo_state_load(b2g_ppo* h, const char* path) {
   CK(cudaSetDevice(h->cfg.device));
   StateReader rd;
   if (int rc = rd.open(path, STATE_KIND_PPO, ppo_fingerprint(h))) return rc;
-  const int n_sec = (int)(sizeof kPpoTags / sizeof kPpoTags[0]);
-  if (rd.n_sections() != n_sec) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a PPO2 learner");
-  for (int i = 0; i < n_sec; ++i)
-    if (rd.tag(i) != kPpoTags[i]) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a PPO2 learner");
+  const std::vector<StateSection> dev = ppo_device_sections(h);
+  if (int rc = state_check_tags(rd, dev, "PPO2")) return rc;
   int64_t hv[2];
   long long cnt[4];
-  if (rd.bytes(0) != sizeof hv || rd.bytes(1) != sizeof cnt || rd.bytes(2) != (size_t)h->n_total * sizeof(float) ||
-      rd.bytes(3) != (size_t)h->n_train * sizeof(float) || rd.bytes(4) != (size_t)h->n_train * sizeof(float))
+  if (rd.bytes(0) != sizeof hv || rd.bytes(1) != sizeof cnt)
     return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  if (int rc = state_check_lengths(rd, dev)) return rc;
   if (int rc = rd.read_host(0, hv, sizeof hv)) return rc;
   if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
   CK(cudaStreamSynchronize(h->stream));
-  h->broken = true;
-  StatePiece p; p.dev = h->P; p.bytes = h->n_total * sizeof(float);
-  StatePiece m; m.dev = h->Mo; m.bytes = h->n_train * sizeof(float);
-  StatePiece v; v.dev = h->Vo; v.bytes = h->n_train * sizeof(float);
-  std::vector<StatePiece> pp{p}, mm{m}, vv{v};
-  if (int rc = rd.read_pieces(2, pp)) return rc;
-  if (int rc = rd.read_pieces(3, mm)) return rc;
-  if (int rc = rd.read_pieces(4, vv)) return rc;
-  CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
-  CK(cudaMemset(h->r_done, 0, (size_t)h->E * sizeof(float)));
-  h->n_updates = hv[0];
-  h->t = 0;
-  h->broken = false;
-  return 0;
+  return state_read_device(rd, dev, &h->broken, [&] {
+    CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
+    CK(cudaMemset(h->r_done, 0, (size_t)h->E * sizeof(float)));
+    h->n_updates = hv[0];
+    h->t = 0;
+    return 0;
+  });
 }
 
 }  // extern "C"

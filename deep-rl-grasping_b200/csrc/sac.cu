@@ -1904,14 +1904,6 @@ std::vector<FpField> sac_fingerprint(const b2g_sac* h) {
           fp_int("u8_plane_mask", h->u8_mask), fp_real("gamma", c.gamma), fp_real("tau", c.tau),
           fp_real("target_entropy", c.target_entropy), fp_int("seed", (int64_t)c.seed)};
 }
-// a handle that owns obs_rms writes one more field and one more section (count, mean[E], var[E] as float64); one that does not
-// reads and writes the files it always did
-std::vector<FpField> sac_fingerprint_rms(const b2g_sac* h) {
-  std::vector<FpField> fp = sac_fingerprint(h);
-  if (h->rms_mean) fp.push_back(fp_int("obs_rms", 1));
-  return fp;
-}
-const uint32_t kRmsTag = state_tag("ORMS");
 
 // Host replay bookkeeping as stored: r_size, head_seq, tail_seq, next_fid, evicted, |lw|, |prev_next|, lw pairs, prev_next.
 struct SacHostState {
@@ -1929,9 +1921,6 @@ struct SacHostState {
   }
 };
 
-StatePiece host_piece(void* p, size_t bytes) { StatePiece s; s.host = p; s.bytes = bytes; return s; }
-StatePiece dev_piece(void* p, size_t bytes) { StatePiece s; s.dev = p; s.bytes = bytes; return s; }
-
 // frames [lo, hi) of the ring: at most two contiguous ranges, each stored at id % frame_cap
 std::vector<StatePiece> frame_pieces(b2g_sac* h, int64_t lo, int64_t hi) {
   std::vector<StatePiece> v;
@@ -1943,24 +1932,18 @@ std::vector<StatePiece> frame_pieces(b2g_sac* h, int64_t lo, int64_t hi) {
   return v;
 }
 
-const uint32_t kSacTags[] = {state_tag("HOST"), state_tag("CNTR"), state_tag("PARM"), state_tag("ADMM"), state_tag("ADMV"),
-                             state_tag("ROFR"), state_tag("RNFR"), state_tag("RACT"), state_tag("RREW"), state_tag("RDON"),
-                             state_tag("FRMS")};
-
-// the device-resident sections 2..10 (parameters .. frames) of a handle whose frame window is [lo, hi)
+// the sections 2.. (parameters .. frames, then obs_rms when the handle owns it) of a handle whose frame window is [lo, hi)
 std::vector<StateSection> sac_device_sections(b2g_sac* h, int64_t lo, int64_t hi) {
   const size_t cap = (size_t)h->cfg.buffer_capacity;
-  std::vector<StateSection> s(9);
-  s[0].pieces = {dev_piece(h->P, h->n_all * sizeof(float))};
-  s[1].pieces = {dev_piece(h->Mo, h->n_train * sizeof(float))};
-  s[2].pieces = {dev_piece(h->Vo, h->n_train * sizeof(float))};
-  s[3].pieces = {dev_piece(h->r_ofr, cap * sizeof(int))};
-  s[4].pieces = {dev_piece(h->r_nfr, cap * sizeof(int))};
-  s[5].pieces = {dev_piece(h->r_act, cap * h->A * sizeof(float))};
-  s[6].pieces = {dev_piece(h->r_rew, cap * sizeof(float))};
-  s[7].pieces = {dev_piece(h->r_done, cap * sizeof(float))};
-  s[8].pieces = frame_pieces(h, lo, hi);
-  for (int i = 0; i < 9; ++i) s[i].tag = kSacTags[i + 2];
+  std::vector<StateSection> s = adam_sections(h->P, h->n_all, h->Mo, h->Vo, h->n_train);
+  s.resize(9);
+  s[3].tag = state_tag("ROFR"); s[3].pieces = {dev_piece(h->r_ofr, cap * sizeof(int))};
+  s[4].tag = state_tag("RNFR"); s[4].pieces = {dev_piece(h->r_nfr, cap * sizeof(int))};
+  s[5].tag = state_tag("RACT"); s[5].pieces = {dev_piece(h->r_act, cap * h->A * sizeof(float))};
+  s[6].tag = state_tag("RREW"); s[6].pieces = {dev_piece(h->r_rew, cap * sizeof(float))};
+  s[7].tag = state_tag("RDON"); s[7].pieces = {dev_piece(h->r_done, cap * sizeof(float))};
+  s[8].tag = state_tag("FRMS"); s[8].pieces = frame_pieces(h, lo, hi);
+  if (h->rms_mean) s.push_back(rms_section(&h->rms_count, h->rms_mean, h->rms_var, h->E));
   return s;
 }
 
@@ -1988,18 +1971,9 @@ int b2g_sac_state_save(b2g_sac* h, const char* path) {
   std::vector<int64_t> hv = {hs.r_size, hs.head_seq, hs.tail_seq, hs.next_fid, hs.evicted, (int64_t)hs.lw.size(), (int64_t)hs.prev_next.size()};
   for (const auto& q : hs.lw) { hv.push_back(q.first); hv.push_back(q.second); }
   hv.insert(hv.end(), hs.prev_next.begin(), hs.prev_next.end());
-  std::vector<StateSection> secs(2);
-  secs[0].tag = kSacTags[0]; secs[0].pieces = {host_piece(hv.data(), hv.size() * sizeof(int64_t))};
-  secs[1].tag = kSacTags[1]; secs[1].pieces = {host_piece(cnt, sizeof cnt)};
+  std::vector<StateSection> secs = host_sections(hv.data(), hv.size() * sizeof(int64_t), cnt, sizeof cnt);
   for (auto& s : sac_device_sections(h, hs.frame_lo(h->frame_cap), hs.next_fid)) secs.push_back(std::move(s));
-  if (h->rms_mean) {
-    StateSection r;
-    r.tag = kRmsTag;
-    r.pieces = {host_piece(&h->rms_count, sizeof(double)), dev_piece(h->rms_mean, h->E * sizeof(double)),
-                dev_piece(h->rms_var, h->E * sizeof(double))};
-    secs.push_back(std::move(r));
-  }
-  return state_write(path, STATE_KIND_SAC, sac_fingerprint_rms(h), secs);
+  return state_write(path, STATE_KIND_SAC, fp_with_rms(sac_fingerprint(h), h->rms_mean), secs);
 }
 
 int b2g_sac_state_load(b2g_sac* h, const char* path) {
@@ -2011,23 +1985,8 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
   CK(cudaSetDevice(h->cfg.device));
   // ---- everything is checked before the handle changes
   StateReader rd;
-  if (int rc = rd.open(path, STATE_KIND_SAC, sac_fingerprint_rms(h))) {
-    // a file with one fingerprint field more or fewer than this handle: say which side owns obs_rms
-    const std::string msg = g_b2g_err;
-    StateReader other;
-    std::vector<FpField> fp = sac_fingerprint(h);
-    if (!h->rms_mean) fp.push_back(fp_int("obs_rms", 1));
-    if (other.open(path, STATE_KIND_SAC, fp) == 0)
-      return b2g_fail(B2G_EINVAL, h->rms_mean ? "the state file has no obs_rms, but this handle owns the observation statistics (b2g_obs_rms_set)"
-                                              : "the state file carries obs_rms: call b2g_obs_rms_set on this handle before loading it");
-    return b2g_fail(rc, msg);
-  }
-  const int n_sec = (int)(sizeof kSacTags / sizeof kSacTags[0]);
-  const int n_file = n_sec + (h->rms_mean ? 1 : 0);
-  if (rd.n_sections() != n_file || (h->rms_mean && (rd.tag(n_sec) != kRmsTag || rd.bytes(n_sec) != (uint64_t)(2 * h->E + 1) * sizeof(double))))
-    return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a SAC learner");
-  for (int i = 0; i < n_sec; ++i)
-    if (rd.tag(i) != kSacTags[i]) return b2g_fail(B2G_EINVAL, "training-state file has the wrong sections for a SAC learner");
+  if (int rc = state_open_rms(rd, path, STATE_KIND_SAC, sac_fingerprint(h), h->rms_mean, "b2g_obs_rms_set")) return rc;
+  if (int rc = state_check_tags(rd, sac_device_sections(h, 0, 0), "SAC")) return rc;
   const int64_t cap = h->cfg.buffer_capacity, FC = h->frame_cap;
   if (rd.bytes(0) % 8 || rd.bytes(0) < 7 * 8 || rd.bytes(0) > (uint64_t)(7 + 2 * cap + 4 * FC) * 8)
     return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
@@ -2043,37 +2002,27 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
   hs.prev_next.assign(hv.begin() + 7 + 2 * n_lw, hv.end());
   const int64_t lo = hs.frame_lo(FC);
   if (lo < 0 || lo > hs.next_fid || hs.next_fid - lo > FC) return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
-  std::vector<StateSection> dev = sac_device_sections(h, lo, hs.next_fid);
-  for (int i = 0; i < (int)dev.size(); ++i)
-    if (rd.bytes(i + 2) != dev[i].bytes())
-      return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  const std::vector<StateSection> dev = sac_device_sections(h, lo, hs.next_fid);
+  if (int rc = state_check_lengths(rd, dev)) return rc;
   long long cnt[8];
   if (rd.bytes(1) != sizeof cnt) return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
   if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
   // ---- from here on a failure leaves the handle unusable until a load succeeds
   CK(cudaStreamSynchronize(h->stream));
   if (h->aux) { CK(cudaStreamSynchronize(h->aux)); CK(cudaStreamSynchronize(h->aux2)); }
-  h->broken = true;
-  for (int i = 0; i < (int)dev.size(); ++i)
-    if (int rc = rd.read_pieces(i + 2, dev[i].pieces)) return rc;
-  if (h->rms_mean) {
-    double count = 0.0;
-    if (int rc = rd.read_pieces(n_sec, {host_piece(&count, sizeof(double)), dev_piece(h->rms_mean, h->E * sizeof(double)),
-                                        dev_piece(h->rms_var, h->E * sizeof(double))})) return rc;
-    h->rms_count = count;
-    obs_rms_derive(h);
-  }
-  h->ob_n = 0;         // staged observations name frames of the replaced replay: the next b2g_sac_observe_act stages anew
-  CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
-  h->r_size = hs.r_size; h->head_seq = hs.head_seq; h->tail_seq = hs.tail_seq; h->next_fid = hs.next_fid; h->evicted = hs.evicted;
-  h->lw.assign(hs.lw.begin(), hs.lw.end());
-  h->prev_next = hs.prev_next;
-  // The BF16 weight planes follow the restored arena at the next step or act.  The captured step graphs (graph_exec, pipe_graph)
-  // stay valid: their kernel parameters hold device pointers and configuration only, and the replay size, first live slot and
-  // Philox step they depend on are read from the device counters restored above.
-  h->planes_dirty = true;
-  h->broken = false;
-  return 0;
+  return state_read_device(rd, dev, &h->broken, [&] {
+    if (h->rms_mean) obs_rms_derive(h);
+    h->ob_n = 0;       // staged observations name frames of the replaced replay: the next b2g_sac_observe_act stages anew
+    CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
+    h->r_size = hs.r_size; h->head_seq = hs.head_seq; h->tail_seq = hs.tail_seq; h->next_fid = hs.next_fid; h->evicted = hs.evicted;
+    h->lw.assign(hs.lw.begin(), hs.lw.end());
+    h->prev_next = hs.prev_next;
+    // The BF16 weight planes follow the restored arena at the next step or act.  The captured step graphs (graph_exec, pipe_graph)
+    // stay valid: their kernel parameters hold device pointers and configuration only, and the replay size, first live slot and
+    // Philox step they depend on are read from the device counters restored above.
+    h->planes_dirty = true;
+    return 0;
+  });
 }
 
 }  // extern "C"

@@ -285,4 +285,66 @@ int StateReader::read_pieces(int i, const std::vector<StatePiece>& pieces) {
   return 0;
 }
 
+std::vector<StateSection> host_sections(void* host, size_t host_bytes, void* counters, size_t counter_bytes) {
+  std::vector<StateSection> s(2);
+  s[0].tag = state_tag("HOST"); s[0].pieces = {host_piece(host, host_bytes)};
+  s[1].tag = state_tag("CNTR"); s[1].pieces = {host_piece(counters, counter_bytes)};
+  return s;
+}
+
+std::vector<StateSection> adam_sections(float* P, size_t n_param, float* Mo, float* Vo, size_t n_moments) {
+  std::vector<StateSection> s(3);
+  s[0].tag = state_tag("PARM"); s[0].pieces = {dev_piece(P, n_param * sizeof(float))};
+  s[1].tag = state_tag("ADMM"); s[1].pieces = {dev_piece(Mo, n_moments * sizeof(float))};
+  s[2].tag = state_tag("ADMV"); s[2].pieces = {dev_piece(Vo, n_moments * sizeof(float))};
+  return s;
+}
+
+int state_check_tags(const StateReader& rd, const std::vector<StateSection>& dev, const char* learner) {
+  bool ok = rd.n_sections() == 2 + (int)dev.size() && rd.tag(0) == state_tag("HOST") && rd.tag(1) == state_tag("CNTR");
+  for (int i = 0; ok && i < (int)dev.size(); ++i) ok = rd.tag(2 + i) == dev[i].tag;
+  return ok ? 0 : b2g_fail(B2G_EINVAL, std::string("training-state file has the wrong sections for a ") + learner + " learner");
+}
+
+int state_check_lengths(const StateReader& rd, const std::vector<StateSection>& dev) {
+  for (int i = 0; i < (int)dev.size(); ++i)
+    if (rd.bytes(2 + i) != dev[i].bytes())
+      return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  return 0;
+}
+
+int state_read_device(StateReader& rd, const std::vector<StateSection>& dev, bool* broken, const std::function<int()>& restore) {
+  *broken = true;
+  for (int i = 0; i < (int)dev.size(); ++i)
+    if (int rc = rd.read_pieces(2 + i, dev[i].pieces)) return rc;
+  if (int rc = restore()) return rc;
+  *broken = false;
+  return 0;
+}
+
+std::vector<FpField> fp_with_rms(std::vector<FpField> fp, bool owns_rms) {
+  if (owns_rms) fp.push_back(fp_int("obs_rms", 1));
+  return fp;
+}
+
+StateSection rms_section(double* count, double* mean, double* var, int E) {
+  StateSection r;
+  r.tag = state_tag("ORMS");
+  r.pieces = {host_piece(count, sizeof(double)), dev_piece(mean, E * sizeof(double)), dev_piece(var, E * sizeof(double))};
+  return r;
+}
+
+int state_open_rms(StateReader& rd, const char* path, uint32_t kind, const std::vector<FpField>& fp, bool owns_rms, const char* rms_set_call) {
+  const int rc = rd.open(path, kind, fp_with_rms(fp, owns_rms));
+  if (rc == 0) return 0;
+  // a file with one fingerprint field more or fewer than this handle: say which side owns obs_rms
+  const std::string msg = g_b2g_err;
+  StateReader other;
+  if (other.open(path, kind, fp_with_rms(fp, !owns_rms)) == 0)
+    return b2g_fail(B2G_EINVAL, owns_rms ? std::string("the state file has no obs_rms, but this handle owns the observation statistics (") +
+                                               rms_set_call + ")"
+                                         : std::string("the state file carries obs_rms: call ") + rms_set_call + " on this handle before loading it");
+  return b2g_fail(rc, msg);
+}
+
 }  // namespace b2g

@@ -1,4 +1,5 @@
-// Training-state files (state.cu): the container format b2g_sac_state_save / _load and b2g_bdq_state_save / _load share.
+// Training-state files (state.cu): the container format every learner's b2g_*_state_save / _load shares, and the steps of a
+// load they have in common.
 //
 // Layout (little-endian):
 //   StateHeader                  magic "B2GSTATE", format version, handle kind, field / section counts, total file size
@@ -12,6 +13,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -43,6 +45,8 @@ struct StateSection {
   std::vector<StatePiece> pieces;
   size_t bytes() const;
 };
+inline StatePiece host_piece(void* p, size_t bytes) { StatePiece s; s.host = p; s.bytes = bytes; return s; }
+inline StatePiece dev_piece(void* p, size_t bytes) { StatePiece s; s.dev = p; s.bytes = bytes; return s; }
 
 // Writes the whole file.  Device pieces must be quiescent (the caller has synchronised the streams that write them).
 int state_write(const char* path, uint32_t kind, const std::vector<FpField>& fp, const std::vector<StateSection>& secs);
@@ -66,5 +70,27 @@ class StateReader {
   std::vector<uint32_t> tags_;
   std::vector<uint64_t> offs_, lens_, sums_;
 };
+
+// ---- the sections every learner's file starts with: HOST (its host bookkeeping) and CNTR (its device counters), then PARM
+// (n_param floats of the parameter arena), ADMM and ADMV (n_moments floats of the Adam moments)
+std::vector<StateSection> host_sections(void* host, size_t host_bytes, void* counters, size_t counter_bytes);
+std::vector<StateSection> adam_sections(float* P, size_t n_param, float* Mo, float* Vo, size_t n_moments);
+
+// ---- the load steps every learner shares.  A learner's file holds the host sections HOST and CNTR, then its device sections.
+// The file's tags are HOST, CNTR and those of dev, in order (B2G_EINVAL naming the learner otherwise).
+int state_check_tags(const StateReader& rd, const std::vector<StateSection>& dev, const char* learner);
+// Section 2 + i of the file is as long as dev[i], for every i.
+int state_check_lengths(const StateReader& rd, const std::vector<StateSection>& dev);
+// Streams sections 2.. into dev, then runs restore(), which puts back what the handle keeps outside them.  *broken is set before
+// the first write and cleared once restore() has succeeded: a handle that failed part way accepts only destroy and load.
+int state_read_device(StateReader& rd, const std::vector<StateSection>& dev, bool* broken, const std::function<int()>& restore);
+
+// ---- VecNormalize's obs_rms: a handle that owns it writes one more fingerprint field (obs_rms = 1) and one more section (ORMS:
+// count, then mean[E] and var[E] as float64); one that does not reads and writes the files it always did.
+std::vector<FpField> fp_with_rms(std::vector<FpField> fp, bool owns_rms);
+StateSection rms_section(double* count, double* mean, double* var, int E);
+// rd.open() with the fingerprint of a handle that owns obs_rms or not; a file that differs in that alone is refused with a
+// message naming rms_set_call, the call that gives a handle its obs_rms.
+int state_open_rms(StateReader& rd, const char* path, uint32_t kind, const std::vector<FpField>& fp, bool owns_rms, const char* rms_set_call);
 
 }  // namespace b2g

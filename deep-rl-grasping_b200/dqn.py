@@ -16,14 +16,15 @@ import numpy as np
 
 from . import _lib, sb_io, training_state
 from .callbacks import as_callback
-from .learner import _f32, _fp
+from .learner import HandleLearner, _f32, _fp
 from .vec_env import DummyVecEnv
 
 _ONLINE, _TARGET = "deepq/model/", "deepq/target_q_func/model/"
 
 
-class DQNLearner:
+class DQNLearner(HandleLearner):
     """numpy-facing wrapper of one ``b2g_dqn`` handle (maps 1:1 onto the C ABI)."""
+    _abi = "dqn"
 
     def __init__(self, obs_dim=100, n_actions=12, layers=(64, 64), batch_size=32, buffer_size=50000, gamma=0.99, seed=0, device=0,
                  prioritized_replay=False, prioritized_replay_alpha=0.6, prioritized_replay_eps=1e-6):
@@ -33,66 +34,11 @@ class DQNLearner:
         cfg = _lib.DqnCfg(obs_dim, n_actions, int(layers[0]), int(layers[1]), batch_size, buffer_size, gamma, seed, device,
                           int(bool(prioritized_replay)), float(prioritized_replay_alpha), float(prioritized_replay_eps))
         self.prioritized_replay = bool(prioritized_replay)
-        self.h = C.c_void_p()
-        _lib.check(self.lib.b2g_dqn_create(C.byref(cfg), C.byref(self.h)))
+        self._create(cfg)
         self.obs_dim, self.n_actions, self.batch_size = obs_dim, n_actions, batch_size
-        self._info = OrderedDict()
-        buf = C.create_string_buffer(256)
-        rows, cols, nd = C.c_int64(), C.c_int64(), C.c_int32()
-        for i in range(self.lib.b2g_dqn_param_count(self.h)):
-            _lib.check(self.lib.b2g_dqn_param_info(self.h, i, buf, 256, C.byref(rows), C.byref(cols), C.byref(nd)))
-            shape = () if nd.value == 0 else ((rows.value, cols.value) if nd.value == 2 else (cols.value,))
-            self._info[buf.value.decode()] = shape
 
-    def close(self):
-        if getattr(self, "h", None) is not None and self.h:
-            self.lib.b2g_dqn_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    @property
-    def param_shapes(self):
-        return self._info
-
-    def get_parameters(self):
-        out = OrderedDict()
-        for n, shp in self._info.items():
-            a = np.empty(shp, np.float32)
-            _lib.check(self.lib.b2g_dqn_get_param(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
-            out[n] = a
-        return out
-
-    def load_parameters(self, params, exact_match=True):
-        seen = set()
-        for n, a in params.items():
-            key = n[:-2] if n.endswith(":0") else n
-            if key not in self._info:
-                if exact_match:
-                    raise ValueError(f"unknown variable {n}")
-                continue
-            a = _f32(a)
-            if tuple(a.shape) != self._info[key]:
-                raise ValueError(f"shape mismatch for {n}: {a.shape} vs {self._info[key]}")
-            _lib.check(self.lib.b2g_dqn_set_param(self.h, key.encode(), _fp(a.reshape(-1)), a.size))
-            seen.add(key)
-        if exact_match and seen != set(self._info):
-            raise ValueError(f"missing variables: {sorted(set(self._info) - seen)}")
-
-    def get_gradients(self):
-        """The last step's gradients after the per-tensor clip (online tensors)."""
-        out = OrderedDict()
-        for n, shp in self._info.items():
-            if not n.startswith(_ONLINE):
-                continue
-            a = np.empty(shp, np.float32)
-            _lib.check(self.lib.b2g_dqn_get_grad(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
-            out[n] = a
-        return out
+    def _has_grad(self, name):
+        return name.startswith(_ONLINE)
 
     def set_eps(self, eps: float):
         """deepq/eps: the exploration epsilon the last action was taken with."""
@@ -164,13 +110,6 @@ class DQNLearner:
         _lib.check(self.lib.b2g_dqn_act(self.h, _fp(obs), n, out.ctypes.data_as(C.POINTER(C.c_int32)), None if q is None else _fp(q)))
         return (out, q) if with_q else out
 
-    def save_state(self, path: str):
-        """Parameters, Adam moments, counters, the live replay rows and the prioritised-replay trees -> ``path``."""
-        _lib.check(self.lib.b2g_dqn_state_save(self.h, os.fsencode(path)))
-
-    def load_state(self, path: str):
-        """Restores a ``save_state`` file into this learner, which must have the same configuration."""
-        _lib.check(self.lib.b2g_dqn_state_load(self.h, os.fsencode(path)))
 
 
 def _linear(t, span, p0, p1):

@@ -24,6 +24,87 @@ def _f32(a) -> np.ndarray:
     return a if a.flags.c_contiguous else a.copy()
 
 
+class HandleLearner:
+    """What the numpy-facing wrappers of the ``b2g_bdq``, ``b2g_dqn`` and ``b2g_ppo`` handles share: the handle's lifetime,
+    its named parameters (``b2g_<abi>_param_*``, ``_get_param``, ``_set_param``, ``_get_grad``) and its training-state
+    files.  A subclass sets ``_abi`` and ``_has_grad`` and calls ``_create`` with its configuration."""
+    _abi = ""
+
+    def _has_grad(self, name: str) -> bool:
+        raise NotImplementedError
+
+    def _fn(self, name: str):
+        return getattr(self.lib, f"b2g_{self._abi}_{name}")
+
+    def _create(self, cfg):
+        self.h = C.c_void_p()
+        _lib.check(self._fn("create")(C.byref(cfg), C.byref(self.h)))
+        self._info = OrderedDict()
+        buf = C.create_string_buffer(256)
+        rows, cols, nd = C.c_int64(), C.c_int64(), C.c_int32()
+        for i in range(self._fn("param_count")(self.h)):
+            _lib.check(self._fn("param_info")(self.h, i, buf, 256, C.byref(rows), C.byref(cols), C.byref(nd)))
+            self._info[buf.value.decode()] = () if nd.value == 0 else ((rows.value, cols.value) if nd.value == 2 else (cols.value,))
+
+    def close(self):
+        if getattr(self, "h", None) is not None and self.h:
+            self._fn("destroy")(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @property
+    def param_shapes(self):
+        return self._info
+
+    def get_parameters(self):
+        out = OrderedDict()
+        for n, shp in self._info.items():
+            a = np.empty(shp, np.float32)
+            _lib.check(self._fn("get_param")(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
+            out[n] = a
+        return out
+
+    def load_parameters(self, params, exact_match=True):
+        seen = set()
+        for n, a in params.items():
+            key = n[:-2] if n.endswith(":0") else n
+            if key not in self._info:
+                if exact_match:
+                    raise ValueError(f"unknown variable {n}")
+                continue
+            a = _f32(a)
+            if tuple(a.shape) != self._info[key]:
+                raise ValueError(f"shape mismatch for {n}: {a.shape} vs {self._info[key]}")
+            _lib.check(self._fn("set_param")(self.h, key.encode(), _fp(a.reshape(-1)), a.size))
+            seen.add(key)
+        if exact_match and seen != set(self._info):
+            raise ValueError(f"missing variables: {sorted(set(self._info) - seen)}")
+
+    def get_gradients(self):
+        """The last step's gradients of the trained variables, after the learner's gradient clip."""
+        out = OrderedDict()
+        for n, shp in self._info.items():
+            if self._has_grad(n):
+                a = np.empty(shp, np.float32)
+                _lib.check(self._fn("get_grad")(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
+                out[n] = a
+        return out
+
+    def save_state(self, path: str):
+        """Parameters, Adam moments, counters and, for the replay learners, the live replay rows and the prioritised-replay
+        trees -> ``path``."""
+        _lib.check(self._fn("state_save")(self.h, os.fsencode(path)))
+
+    def load_state(self, path: str):
+        """Restores a ``save_state`` file into this learner, which must have the same configuration."""
+        _lib.check(self._fn("state_load")(self.h, os.fsencode(path)))
+
+
 class Learner:
     def __init__(self, obs_shape: Sequence[int], n_act: int = 5, hidden: int = 64, batch_size: int = 64,
                  buffer_size: int = 100000, gamma: float = 0.99, tau: float = 0.005,

@@ -14,14 +14,15 @@ import numpy as np
 
 from . import _lib, sb_io, training_state
 from .callbacks import as_callback
-from .learner import _f32, _fp
+from .learner import HandleLearner, _f32, _fp
 from .vec_env import DummyVecEnv
 
 _SCOPE = "model/"
 
 
-class PPO2Learner:
+class PPO2Learner(HandleLearner):
     """numpy-facing wrapper of one ``b2g_ppo`` handle (maps 1:1 onto the C ABI)."""
+    _abi = "ppo"
 
     def __init__(self, obs_dim, n_actions, layers=(64, 64), n_envs=1, n_steps=128, nminibatches=4, noptepochs=4, gamma=0.99, lam=0.95,
                  ent_coef=0.01, vf_coef=0.5, max_grad_norm=0.5, seed=0, device=0):
@@ -31,68 +32,14 @@ class PPO2Learner:
         cfg = _lib.PpoCfg(int(obs_dim), int(n_actions), int(layers[0]), int(layers[1]), int(n_envs), int(n_steps), int(nminibatches),
                           int(noptepochs), float(gamma), float(lam), float(ent_coef), float(vf_coef), float(max_grad_norm),
                           int(seed) & 0xFFFFFFFFFFFFFFFF, int(device))
-        self.h = C.c_void_p()
-        _lib.check(self.lib.b2g_ppo_create(C.byref(cfg), C.byref(self.h)))
+        self._create(cfg)
         self.obs_dim, self.n_actions, self.n_envs, self.n_steps = int(obs_dim), int(n_actions), int(n_envs), int(n_steps)
         self.nminibatches, self.noptepochs = int(nminibatches), int(noptepochs)
         self.n_batch = self.n_envs * self.n_steps
         self.minibatch = self.n_batch // self.nminibatches
-        self._info = OrderedDict()
-        buf = C.create_string_buffer(256)
-        rows, cols, nd = C.c_int64(), C.c_int64(), C.c_int32()
-        for i in range(self.lib.b2g_ppo_param_count(self.h)):
-            _lib.check(self.lib.b2g_ppo_param_info(self.h, i, buf, 256, C.byref(rows), C.byref(cols), C.byref(nd)))
-            self._info[buf.value.decode()] = (rows.value, cols.value) if nd.value == 2 else (cols.value,)
 
-    def close(self):
-        if getattr(self, "h", None) is not None and self.h:
-            self.lib.b2g_ppo_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    @property
-    def param_shapes(self):
-        return self._info
-
-    def get_parameters(self):
-        out = OrderedDict()
-        for n, shp in self._info.items():
-            a = np.empty(shp, np.float32)
-            _lib.check(self.lib.b2g_ppo_get_param(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
-            out[n] = a
-        return out
-
-    def load_parameters(self, params, exact_match=True):
-        seen = set()
-        for n, a in params.items():
-            key = n[:-2] if n.endswith(":0") else n
-            if key not in self._info:
-                if exact_match:
-                    raise ValueError(f"unknown variable {n}")
-                continue
-            a = _f32(a)
-            if tuple(a.shape) != self._info[key]:
-                raise ValueError(f"shape mismatch for {n}: {a.shape} vs {self._info[key]}")
-            _lib.check(self.lib.b2g_ppo_set_param(self.h, key.encode(), _fp(a.reshape(-1)), a.size))
-            seen.add(key)
-        if exact_match and seen != set(self._info):
-            raise ValueError(f"missing variables: {sorted(set(self._info) - seen)}")
-
-    def get_gradients(self):
-        """The last minibatch step's gradients after the global-norm clip (trained variables; q has none)."""
-        out = OrderedDict()
-        for n, shp in self._info.items():
-            if n.startswith(_SCOPE + "q/"):
-                continue
-            a = np.empty(shp, np.float32)
-            _lib.check(self.lib.b2g_ppo_get_grad(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
-            out[n] = a
-        return out
+    def _has_grad(self, name):
+        return not name.startswith(_SCOPE + "q/")      # q has no gradient
 
     def rollout_act(self, obs):
         """Rollout step: obs [n_envs, obs_dim] -> unclipped actions [n_envs, n_actions] (stored with values and neglogp)."""
@@ -148,11 +95,6 @@ class PPO2Learner:
         _lib.check(self.lib.b2g_ppo_get_step(self.h, C.byref(a), C.byref(b), C.byref(t)))
         return a.value, b.value, t.value
 
-    def save_state(self, path: str):
-        _lib.check(self.lib.b2g_ppo_state_save(self.h, os.fsencode(path)))
-
-    def load_state(self, path: str):
-        _lib.check(self.lib.b2g_ppo_state_load(self.h, os.fsencode(path)))
 
 
 def _schedule(v):
