@@ -34,7 +34,7 @@ SYMBOLS = [
     "b2g_ppo_get_grad", "b2g_ppo_rollout_act", "b2g_ppo_rollout_reward", "b2g_ppo_rollout_reset", "b2g_ppo_rollout_get",
     "b2g_ppo_update", "b2g_ppo_train_step_explicit", "b2g_ppo_act", "b2g_ppo_get_step", "b2g_ppo_state_save", "b2g_ppo_state_load",
     "b2g_encoder_create", "b2g_encoder_destroy", "b2g_encoder_n_layers", "b2g_encoder_layer_shape", "b2g_encoder_set_weights",
-    "b2g_encoder_encode", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor",
+    "b2g_encoder_encode", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor", "b2g_debug_gg_simt",
     "b2g_autoencoder_create", "b2g_autoencoder_destroy", "b2g_autoencoder_n_layers", "b2g_autoencoder_layer_shape",
     "b2g_autoencoder_set_weights", "b2g_autoencoder_get_weights", "b2g_autoencoder_get_grad", "b2g_autoencoder_reset_optimizer",
     "b2g_autoencoder_set_dataset", "b2g_autoencoder_train_epoch", "b2g_autoencoder_evaluate", "b2g_autoencoder_predict",
@@ -123,6 +123,19 @@ class SacMetrics(C.Structure):
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+#: the gather-GEMM flags b2g_debug_gg_simt accepts (B2G_GG_* in include/b200grasp.h)
+GG = dict(A_RVEC=1 << 0, B_RVEC=1 << 1, EPI_BIAS_RELU=1 << 2, EPI_MASK=1 << 3, EPI_ATOMIC=1 << 4, COLSUM=1 << 5,
+          EPI_BIAS=1 << 10, EPI_SCALE=1 << 11, A_SCALAR=1 << 12, EPI_BIAS_LRELU=1 << 13, EPI_LRELU_GRAD=1 << 15,
+          EPI_BIAS_TANH=1 << 16, EPI_TANH_GRAD=1 << 17)
+
+
+class GgProblem(C.Structure):
+    """b2g_debug_gg_problem: arena offsets (-1 = none), extents, flags, splitR and alpha of one gg_simt problem."""
+    _fields_ = [(n, C.c_int64) for n in ("A", "B", "C", "bias", "mask", "colsum", "aM", "aR", "bR", "bN", "cM", "cN", "kM", "kN",
+                                          "C_hi", "C_lo")] + \
+        [(n, C.c_int32) for n in ("M", "N", "R", "flags", "splitR")] + [("alpha", C.c_float)]
 
 
 class B2GError(RuntimeError):
@@ -243,6 +256,8 @@ def load():
     lib.b2g_debug_gemm.argtypes = [C.c_int, C.c_int, C.c_int, fp, fp, fp, C.c_int, C.c_int]
     lib.b2g_debug_tensor_info.argtypes = [vp, C.c_char_p, i64p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     lib.b2g_debug_tensor.argtypes = [vp, C.c_char_p, C.c_int, vp, C.c_size_t]
+    lib.b2g_debug_gg_simt.argtypes = [C.c_int, C.POINTER(GgProblem), C.c_int, fp, C.c_int64, dp, C.c_int64, C.POINTER(C.c_uint16),
+                                      C.c_int64, C.POINTER(C.c_int32), C.c_int64]
     _lib = lib
     return lib
 

@@ -140,3 +140,151 @@ extern "C" int b2g_debug_gemm(int M, int N, int K, const float* A, const float* 
   cudaFree(dA); cudaFree(dB); cudaFree(dC); cudaFree(tabs);
   return ok ? 0 : B2G_ECUDA;
 }
+
+static_assert(B2G_GG_A_RVEC == GG_A_RVEC && B2G_GG_B_RVEC == GG_B_RVEC && B2G_GG_EPI_BIAS_RELU == GG_EPI_BIAS_RELU &&
+                  B2G_GG_EPI_MASK == GG_EPI_MASK && B2G_GG_EPI_ATOMIC == GG_EPI_ATOMIC && B2G_GG_COLSUM == GG_COLSUM &&
+                  B2G_GG_EPI_BIAS == GG_EPI_BIAS && B2G_GG_EPI_SCALE == GG_EPI_SCALE && B2G_GG_A_SCALAR == GG_A_SCALAR &&
+                  B2G_GG_EPI_BIAS_LRELU == GG_EPI_BIAS_LRELU && B2G_GG_EPI_LRELU_GRAD == GG_EPI_LRELU_GRAD &&
+                  B2G_GG_EPI_BIAS_TANH == GG_EPI_BIAS_TANH && B2G_GG_EPI_TANH_GRAD == GG_EPI_TANH_GRAD,
+              "the public gg flag values follow common.cuh");
+
+namespace {
+// The contracts of gg_simt_body that hold only by construction at each call site, checked for one caller-described problem
+// (the refusals are listed with b2g_debug_gg_simt in b200grasp.h).  0, or B2G_EINVAL with the broken contract named.
+int check_gg_problem(int build, int idx, const b2g_debug_gg_problem& p, int64_t n_f32, int64_t n_f64, int64_t n_u16,
+                     const int32_t* tabs, int64_t n_tabs) {
+  const std::string at = "problem " + std::to_string(idx) + ": ";
+  auto fail = [&](const std::string& why) { return b2g_fail(B2G_EINVAL, at + why); };
+  const int f = p.flags;
+  int allowed = GG_A_RVEC | GG_B_RVEC | GG_EPI_BIAS_RELU | GG_EPI_MASK | GG_EPI_ATOMIC | GG_COLSUM | GG_EPI_BIAS | GG_EPI_SCALE |
+                GG_A_SCALAR | GG_EPI_BIAS_LRELU;
+  if (build == 1) allowed |= GG_EPI_LRELU_GRAD;
+  if (build == 2) allowed |= GG_EPI_BIAS_TANH | GG_EPI_TANH_GRAD;
+  if (f & ~allowed) return fail("flags " + std::to_string(f & ~allowed) + " are not flags of build " + std::to_string(build));
+  if ((f & GG_A_SCALAR) && !(f & GG_A_RVEC) && build != 1) return fail("m-direction GG_A_SCALAR exists in build 1 only");
+  if (p.M < 1 || p.N < 1 || p.R < 1) return fail("M, N and R must be >= 1");
+  if (p.splitR < 1 || p.splitR > p.R) return fail("splitR must be in 1..R");
+  if (p.splitR > 1 && !(f & GG_EPI_ATOMIC)) return fail("splitR > 1 needs GG_EPI_ATOMIC (the splits would overwrite each other)");
+  if ((f & GG_COLSUM) && (f & GG_B_RVEC)) return fail("GG_COLSUM sums the n-direction B loads; it cannot take GG_B_RVEC");
+  const bool c64 = build == 1 && (f & GG_EPI_ATOMIC), s64 = build == 1 && (f & GG_COLSUM);
+  const bool need_bias = f & (GG_EPI_BIAS_RELU | GG_EPI_BIAS | GG_EPI_BIAS_LRELU | GG_EPI_BIAS_TANH);
+  const bool need_mask = f & (GG_EPI_MASK | GG_EPI_LRELU_GRAD | GG_EPI_TANH_GRAD);
+  if (p.A < 0 || p.B < 0 || p.C < 0) return fail("A, B and C are required");
+  if (need_bias != (p.bias >= 0)) return fail(need_bias ? "the bias epilogue needs bias" : "bias given without a bias epilogue");
+  if (need_mask != (p.mask >= 0)) return fail(need_mask ? "the mask epilogue needs mask" : "mask given without a mask epilogue");
+  if (((f & GG_COLSUM) != 0) != (p.colsum >= 0)) return fail("colsum goes with GG_COLSUM");
+  if ((p.C_hi >= 0) != (p.C_lo >= 0)) return fail("C_hi and C_lo go together");
+  if ((f & GG_EPI_ATOMIC) && p.C_hi >= 0) return fail("C_hi / C_lo would hold one split's partial under GG_EPI_ATOMIC");
+  if (p.C % 4) return fail("C must be 16-byte aligned (the float4 output store)");
+  // tables
+  struct Tab { const char* name; int64_t off; int len; const int32_t* v = nullptr; int64_t lo = 0, hi = 0; };
+  Tab t[8] = {{"aM", p.aM, p.M}, {"aR", p.aR, p.R}, {"bR", p.bR, p.R}, {"bN", p.bN, p.N},
+              {"cM", p.cM, p.M}, {"cN", p.cN, p.N}, {"kM", p.kM, p.M}, {"kN", p.kN, p.N}};
+  for (int i = 0; i < 8; ++i) {
+    if (t[i].off < 0) {
+      if (i < 6) return fail(std::string(t[i].name) + " is required");
+      t[i] = t[i - 2];          // kM / kN default to cM / cN
+      continue;
+    }
+    if (t[i].off + t[i].len > n_tabs) return fail(std::string(t[i].name) + " runs past the end of tabs");
+    t[i].v = tabs + t[i].off;
+    t[i].lo = *std::min_element(t[i].v, t[i].v + t[i].len);
+    t[i].hi = *std::max_element(t[i].v, t[i].v + t[i].len);
+  }
+  const Tab &aM = t[0], &aR = t[1], &bR = t[2], &bN = t[3], &cM = t[4], &cN = t[5], &kM = t[6], &kN = t[7];
+  auto in = [&](const char* what, int64_t base, int64_t lo, int64_t hi, int64_t n) {
+    return base + lo >= 0 && base + hi < n ? 0 : fail(std::string(what) + " reaches outside its arena");
+  };
+  if (int rc = in("A[aM + aR]", p.A, aM.lo + aR.lo, aM.hi + aR.hi, n_f32)) return rc;
+  if (int rc = in("B[bR + bN]", p.B, bR.lo + bN.lo, bR.hi + bN.hi, n_f32)) return rc;
+  if (int rc = in("C[cM + cN]", p.C, cM.lo + cN.lo, cM.hi + cN.hi, c64 ? n_f64 : n_f32)) return rc;
+  if (p.C_hi >= 0) {
+    if (int rc = in("C_hi[cM + cN]", p.C_hi, cM.lo + cN.lo, cM.hi + cN.hi, n_u16)) return rc;
+    if (int rc = in("C_lo[cM + cN]", p.C_lo, cM.lo + cN.lo, cM.hi + cN.hi, n_u16)) return rc;
+  }
+  if (need_bias) if (int rc = in("bias[n]", p.bias, 0, p.N - 1, n_f32)) return rc;
+  if (need_mask) if (int rc = in("mask[kM + kN]", p.mask, kM.lo + kN.lo, kM.hi + kN.hi, n_f32)) return rc;
+  if (f & GG_COLSUM) if (int rc = in("colsum[n]", p.colsum, 0, p.N - 1, s64 ? n_f64 : n_f32)) return rc;
+  // 4-groups: r-vector loads take r in [4g, 4g + 4) when 4g + 3 < R (splits start at multiples of 16); m- / n-direction loads
+  // take rows (columns) [4g, 4g + 4) when 4g + 3 < M (N).  Each taken group must be contiguous, and base + the group's first
+  // offset + every offset of the other side 16-byte aligned.
+  auto groups = [&](const char* what, int64_t base, const Tab& g, const Tab& other) {
+    for (int i = 0; i + 3 < g.len; i += 4)
+      for (int j = 1; j < 4; ++j)
+        if (g.v[i + j] != g.v[i] + j) return fail(std::string(what) + ": " + g.name + " is not contiguous in the 4-group at " + std::to_string(i));
+    if (g.len < 4) return 0;
+    for (int i = 0; i + 3 < g.len; i += 4)
+      if ((base + g.v[i] + other.v[0]) & 3) return fail(std::string(what) + ": the 4-groups of " + g.name + " are not 16-byte aligned");
+    for (int i = 0; i < other.len; ++i)
+      if ((base + g.v[0] + other.v[i]) & 3) return fail(std::string(what) + ": the 4-groups of " + g.name + " are not 16-byte aligned");
+    return 0;
+  };
+  if (f & GG_A_RVEC) {
+    if (!(f & GG_A_SCALAR)) if (int rc = groups("GG_A_RVEC", p.A, aR, aM)) return rc;
+  } else if (!(build == 1 && (f & GG_A_SCALAR))) {
+    if (int rc = groups("m-direction A", p.A, aM, aR)) return rc;
+  }
+  if (f & GG_B_RVEC) {
+    if (int rc = groups("GG_B_RVEC", p.B, bR, bN)) return rc;
+  } else if (int rc = groups("n-direction B", p.B, bN, bR)) return rc;
+  return 0;
+}
+}  // namespace
+
+extern "C" int b2g_debug_gg_simt(int build, const b2g_debug_gg_problem* p, int n, float* f32, int64_t n_f32, double* f64, int64_t n_f64,
+                                 uint16_t* u16, int64_t n_u16, const int32_t* tabs, int64_t n_tabs) {
+  if (build < 0 || build > 2) return b2g_fail(B2G_EINVAL, "build must be 0 (plain), 1 (ext) or 2 (tanh)");
+  if (!p || n < 1 || n > 16) return b2g_fail(B2G_EINVAL, "1 to 16 problems per launch");
+  const int64_t lim = (int64_t)1 << 31;
+  if (n_f32 < 0 || n_f64 < 0 || n_u16 < 0 || n_tabs < 0 || n_f32 >= lim || n_f64 >= lim || n_u16 >= lim || n_tabs >= lim)
+    return b2g_fail(B2G_EINVAL, "arena lengths must be in 0 .. 2^31 - 1");
+  if ((n_f32 && !f32) || (n_f64 && !f64) || (n_u16 && !u16) || (n_tabs && !tabs)) return b2g_fail(B2G_EINVAL, "NULL arena");
+  for (int i = 0; i < n; ++i)
+    if (int rc = check_gg_problem(build, i, p[i], n_f32, n_f64, n_u16, tabs, n_tabs)) return rc;
+
+  if (int rc = check_device(0)) return rc;
+  cudaStream_t s = nullptr;
+  CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+  std::vector<void*> allocs;
+  const int rc = [&]() -> int {
+    float* d32 = nullptr; double* d64 = nullptr; uint16_t* d16 = nullptr; int32_t* dt = nullptr;
+    if (int rc = dev_alloc(allocs, s, &d32, n_f32, false)) return rc;
+    if (int rc = dev_alloc(allocs, s, &d64, n_f64, false)) return rc;
+    if (int rc = dev_alloc(allocs, s, &d16, n_u16, false)) return rc;
+    if (int rc = dev_alloc(allocs, s, &dt, n_tabs, false)) return rc;
+    if (n_f32) CK(cudaMemcpyAsync(d32, f32, n_f32 * sizeof(float), cudaMemcpyHostToDevice, s));
+    if (n_f64) CK(cudaMemcpyAsync(d64, f64, n_f64 * sizeof(double), cudaMemcpyHostToDevice, s));
+    if (n_u16) CK(cudaMemcpyAsync(d16, u16, n_u16 * sizeof(uint16_t), cudaMemcpyHostToDevice, s));
+    if (n_tabs) CK(cudaMemcpyAsync(dt, tabs, n_tabs * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    GemmGroup g;
+    g.name = "debug_gg_simt";
+    for (int i = 0; i < n; ++i) {
+      const b2g_debug_gg_problem& q = p[i];
+      const bool c64 = build == 1 && (q.flags & GG_EPI_ATOMIC), s64 = build == 1 && (q.flags & GG_COLSUM);
+      GemmDesc d = gemm_desc(d32 + q.A, dt + q.aM, dt + q.aR, d32 + q.B, dt + q.bR, dt + q.bN,
+                             c64 ? reinterpret_cast<float*>(d64 + q.C) : d32 + q.C, dt + q.cM, dt + q.cN, q.M, q.N, q.R, q.flags, q.splitR);
+      if (q.kM >= 0) d.kM = dt + q.kM;
+      if (q.kN >= 0) d.kN = dt + q.kN;
+      if (q.bias >= 0) d.bias = d32 + q.bias;
+      if (q.mask >= 0) d.mask = d32 + q.mask;
+      if (q.colsum >= 0) d.colsum = s64 ? reinterpret_cast<float*>(d64 + q.colsum) : d32 + q.colsum;
+      if (q.C_hi >= 0) { d.C_hi = d16 + q.C_hi; d.C_lo = d16 + q.C_lo; }
+      d.alpha = q.alpha;
+      g.host.push_back(d);
+    }
+    if (int rc = finalize_tiles(g, allocs, s)) return rc;
+    if (build == 0) gg_simt_launch(g.dev, n, g.total_tiles, s);
+    else if (build == 1) gg_simt_launch_ext(g.dev, n, g.total_tiles, s);
+    else gg_simt_launch_tanh(g.dev, n, g.total_tiles, s);
+    CK(cudaGetLastError());
+    if (n_f32) CK(cudaMemcpyAsync(f32, d32, n_f32 * sizeof(float), cudaMemcpyDeviceToHost, s));
+    if (n_f64) CK(cudaMemcpyAsync(f64, d64, n_f64 * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (n_u16) CK(cudaMemcpyAsync(u16, d16, n_u16 * sizeof(uint16_t), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    return 0;
+  }();
+  cudaStreamSynchronize(s);
+  for (void* q : allocs) cudaFree(q);
+  cudaStreamDestroy(s);
+  return rc;
+}

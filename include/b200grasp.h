@@ -548,6 +548,43 @@ int b2g_autoencoder_step(b2g_autoencoder* h, const float* inputs, const float* t
  * ------------------------------------------------------------------------------------------------------------ */
 int b2g_debug_gemm(int M, int N, int K, const float* A, const float* B, float* C, int x3, int split_k);
 
+/* Bring-up hook (not on the product path): one grouped launch of the fp32 gather-GEMM engine (csrc/gg_simt.cu) over problems
+ * the caller describes, through build 0 (plain fp32), 1 (sums in double, GG_EPI_LRELU_GRAD and m-direction GG_A_SCALAR; the
+ * auto-encoder's build) or 2 (GG_EPI_BIAS_TANH / GG_EPI_TANH_GRAD; PPO2's build).  Problem p computes
+ *   C[cM[m] + cN[n]]  (=|+=)  epi( sum_r  A[aM[m] + aR[r]] * B[bR[r] + bN[n]] )
+ * with every operand an element offset into one of four host arenas: A, B, C, bias, mask and colsum into f32 (C and colsum
+ * into f64 under build 1 with GG_EPI_ATOMIC / GG_COLSUM), the tables aM .. kN into tabs (kM / kN = -1: the engine's default
+ * cM / cN), C_hi / C_lo into u16 (-1: none; both or neither).  The f32, f64 and u16 arenas are uploaded, the tiles laid out
+ * as the handles lay them out, the group launched once on a stream of its own, and the three arenas copied back.
+ * Before any CUDA call, B2G_EINVAL (b2g_last_error names the broken contract) refuses: n outside 1..16; M, N, R < 1,
+ * splitR < 1 or > R, splitR > 1 without GG_EPI_ATOMIC; a flag the build does not have; a missing operand; an address any
+ * table can reach outside its arena; GG_A_RVEC / GG_B_RVEC without r contiguous in aligned 4-groups (16-byte addresses),
+ * except A under GG_A_SCALAR; an m- (n-) direction operand whose full aligned 4-groups of rows (columns) are not contiguous
+ * and 16-byte aligned, except A under build 1 with GG_A_SCALAR; GG_COLSUM with GG_B_RVEC (the column sums are taken from the
+ * n-direction B loads); C_hi / C_lo with GG_EPI_ATOMIC; C not 16-byte aligned.  Arena lengths are element counts below 2^31.  Flag values: */
+#define B2G_GG_A_RVEC (1 << 0)
+#define B2G_GG_B_RVEC (1 << 1)
+#define B2G_GG_EPI_BIAS_RELU (1 << 2)
+#define B2G_GG_EPI_MASK (1 << 3)
+#define B2G_GG_EPI_ATOMIC (1 << 4)
+#define B2G_GG_COLSUM (1 << 5)
+#define B2G_GG_EPI_BIAS (1 << 10)
+#define B2G_GG_EPI_SCALE (1 << 11)
+#define B2G_GG_A_SCALAR (1 << 12)
+#define B2G_GG_EPI_BIAS_LRELU (1 << 13)
+#define B2G_GG_EPI_LRELU_GRAD (1 << 15)
+#define B2G_GG_EPI_BIAS_TANH (1 << 16)
+#define B2G_GG_EPI_TANH_GRAD (1 << 17)
+typedef struct {
+  int64_t A, B, C, bias, mask, colsum;       /* offsets into f32 (C / colsum: f64 under build 1 with ATOMIC / COLSUM); -1 = none */
+  int64_t aM, aR, bR, bN, cM, cN, kM, kN;    /* offsets into tabs; kM / kN -1 = cM / cN */
+  int64_t C_hi, C_lo;                        /* offsets into u16, -1 = none */
+  int32_t M, N, R, flags, splitR;
+  float alpha;                               /* GG_EPI_SCALE factor, LeakyReLU slope */
+} b2g_debug_gg_problem;
+int b2g_debug_gg_simt(int build, const b2g_debug_gg_problem* p, int n, float* f32, int64_t n_f32, double* f64, int64_t n_f64,
+                      uint16_t* u16, int64_t n_u16, const int32_t* tabs, int64_t n_tabs);
+
 /* Bring-up hook (not on the product path): one plane of one named device tensor of a SAC handle, copied to the host after the
  * handle's stream is synchronised.  BF16 planes come back as raw uint16 (elem_bytes 2), fp32 buffers as float (elem_bytes 4);
  * bytes must be numel * elem_bytes.  Returns B2G_EINVAL for an unknown name, a plane out of range or a size mismatch, and
