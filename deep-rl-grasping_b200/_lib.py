@@ -34,7 +34,7 @@ SYMBOLS = [
     "b2g_ppo_get_grad", "b2g_ppo_rollout_act", "b2g_ppo_rollout_reward", "b2g_ppo_rollout_reset", "b2g_ppo_rollout_get",
     "b2g_ppo_update", "b2g_ppo_train_step_explicit", "b2g_ppo_act", "b2g_ppo_get_step", "b2g_ppo_state_save", "b2g_ppo_state_load",
     "b2g_encoder_create", "b2g_encoder_destroy", "b2g_encoder_n_layers", "b2g_encoder_layer_shape", "b2g_encoder_set_weights",
-    "b2g_encoder_encode", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor", "b2g_debug_gg_simt",
+    "b2g_encoder_encode", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor", "b2g_debug_gg_simt", "b2g_debug_gg_tc",
     "b2g_autoencoder_create", "b2g_autoencoder_destroy", "b2g_autoencoder_n_layers", "b2g_autoencoder_layer_shape",
     "b2g_autoencoder_set_weights", "b2g_autoencoder_get_weights", "b2g_autoencoder_get_grad", "b2g_autoencoder_reset_optimizer",
     "b2g_autoencoder_set_dataset", "b2g_autoencoder_train_epoch", "b2g_autoencoder_evaluate", "b2g_autoencoder_predict",
@@ -129,6 +129,8 @@ class SacMetrics(C.Structure):
 GG = dict(A_RVEC=1 << 0, B_RVEC=1 << 1, EPI_BIAS_RELU=1 << 2, EPI_MASK=1 << 3, EPI_ATOMIC=1 << 4, COLSUM=1 << 5,
           EPI_BIAS=1 << 10, EPI_SCALE=1 << 11, A_SCALAR=1 << 12, EPI_BIAS_LRELU=1 << 13, EPI_LRELU_GRAD=1 << 15,
           EPI_BIAS_TANH=1 << 16, EPI_TANH_GRAD=1 << 17)
+#: the plane-producer flags of the wgmma engine that b2g_debug_gg_tc accepts besides A_RVEC .. COLSUM
+GG_TC = dict(PLANES=1 << 6, A_ALIGN4=1 << 7, MN_MAJOR=1 << 9, A_ROWLANES=1 << 14)
 
 
 class GgProblem(C.Structure):
@@ -136,6 +138,13 @@ class GgProblem(C.Structure):
     _fields_ = [(n, C.c_int64) for n in ("A", "B", "C", "bias", "mask", "colsum", "aM", "aR", "bR", "bN", "cM", "cN", "kM", "kN",
                                           "C_hi", "C_lo")] + \
         [(n, C.c_int32) for n in ("M", "N", "R", "flags", "splitR")] + [("alpha", C.c_float)]
+
+
+class GgTcProblem(C.Structure):
+    """b2g_debug_gg_tc_problem: arena offsets (-1 = none), extents, flags and splitR of one gg_tc problem."""
+    _fields_ = [(n, C.c_int64) for n in ("A", "B", "C", "bias", "mask", "colsum", "aM", "aR", "bR", "bN", "cM", "cN", "kM", "kN",
+                                          "bR_p", "bN_p", "A_hi", "A_lo", "B_hi", "B_lo", "C_hi", "C_lo")] + \
+        [(n, C.c_int32) for n in ("M", "N", "R", "flags", "splitR")]
 
 
 class B2GError(RuntimeError):
@@ -258,6 +267,8 @@ def load():
     lib.b2g_debug_tensor.argtypes = [vp, C.c_char_p, C.c_int, vp, C.c_size_t]
     lib.b2g_debug_gg_simt.argtypes = [C.c_int, C.POINTER(GgProblem), C.c_int, fp, C.c_int64, dp, C.c_int64, C.POINTER(C.c_uint16),
                                       C.c_int64, C.POINTER(C.c_int32), C.c_int64]
+    lib.b2g_debug_gg_tc.argtypes = [C.c_int, C.POINTER(GgTcProblem), C.c_int, fp, C.c_int64, C.POINTER(C.c_uint16), C.c_int64,
+                                    C.POINTER(C.c_int32), C.c_int64]
     _lib = lib
     return lib
 

@@ -7,6 +7,8 @@
 // buffers) back to the host, so that tests can hold each contraction to a float64 contraction of the inputs it actually read.
 #include <cuda_runtime.h>
 
+#include <algorithm>
+#include <map>
 #include <string>
 #include <vector>
 
@@ -279,6 +281,207 @@ extern "C" int b2g_debug_gg_simt(int build, const b2g_debug_gg_problem* p, int n
     CK(cudaGetLastError());
     if (n_f32) CK(cudaMemcpyAsync(f32, d32, n_f32 * sizeof(float), cudaMemcpyDeviceToHost, s));
     if (n_f64) CK(cudaMemcpyAsync(f64, d64, n_f64 * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (n_u16) CK(cudaMemcpyAsync(u16, d16, n_u16 * sizeof(uint16_t), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    return 0;
+  }();
+  cudaStreamSynchronize(s);
+  for (void* q : allocs) cudaFree(q);
+  cudaStreamDestroy(s);
+  return rc;
+}
+
+static_assert(B2G_GG_PLANES == GG_PLANES && B2G_GG_A_ALIGN4 == GG_A_ALIGN4 && B2G_GG_MN_MAJOR == GG_MN_MAJOR &&
+                  B2G_GG_A_ROWLANES == GG_A_ROWLANES,
+              "the public gg_tc flag values follow common.cuh");
+
+namespace {
+// One offset table of a gg_tc problem: its host values, how many of them the problem uses (len) and how many the kernel reads
+// (reach >= len: the K-major plane producers fetch the r tables a whole 64-row chunk at a time).
+struct TcTab {
+  const char* name = "";
+  int64_t off = -1;
+  int len = 0, reach = 0;
+  const int32_t* v = nullptr;
+};
+
+// The memory contracts of gg_tc_kernel that hold only by construction at each SAC call site, checked for one caller-described
+// problem (the refusals are listed with b2g_debug_gg_tc in b200grasp.h).  0, or B2G_EINVAL with the broken contract named.
+int check_gg_tc_problem(int idx, const b2g_debug_gg_tc_problem& p, int64_t n_f32, int64_t n_u16, const int32_t* tabs, int64_t n_tabs) {
+  const std::string at = "problem " + std::to_string(idx) + ": ";
+  auto fail = [&](const std::string& why) { return b2g_fail(B2G_EINVAL, at + why); };
+  const int f = p.flags;
+  const int allowed = GG_A_RVEC | GG_B_RVEC | GG_EPI_BIAS_RELU | GG_EPI_MASK | GG_EPI_ATOMIC | GG_COLSUM | GG_PLANES | GG_A_ALIGN4 |
+                      GG_MN_MAJOR | GG_A_ROWLANES;
+  if (f & ~allowed)
+    return fail("flags " + std::to_string(f & ~allowed) + " are not implemented by gg_tc (GG_CN_AFFINE4 is derived, not given)");
+  const bool planes = f & GG_PLANES, mn = f & GG_MN_MAJOR, al4 = f & GG_A_ALIGN4;
+  if (!planes && (f & (GG_A_ALIGN4 | GG_MN_MAJOR | GG_A_ROWLANES)))
+    return fail("GG_A_ALIGN4, GG_MN_MAJOR and GG_A_ROWLANES select plane producers; they need GG_PLANES");
+  if ((f & GG_COLSUM) && (f & (GG_B_RVEC | GG_PLANES)))
+    return fail("GG_COLSUM sums the fp32 n-direction B loads; it cannot take GG_B_RVEC or GG_PLANES");
+  if (p.M < 1 || p.N < 1 || p.R < 1) return fail("M, N and R must be >= 1");
+  if (p.splitR < 1 || p.splitR > p.R) return fail("splitR must be in 1..R");
+  if (p.splitR > 1 && !(f & GG_EPI_ATOMIC)) return fail("splitR > 1 needs GG_EPI_ATOMIC (the splits would overwrite each other)");
+  if ((p.C_hi >= 0) != (p.C_lo >= 0)) return fail("C_hi and C_lo go together");
+  if ((f & GG_EPI_ATOMIC) && p.C_hi >= 0) return fail("C_hi / C_lo would hold one split's partial under GG_EPI_ATOMIC");
+  const bool need_bias = f & GG_EPI_BIAS_RELU, need_mask = f & GG_EPI_MASK;
+  if (p.C < 0) return fail("C is required");
+  if (need_bias != (p.bias >= 0)) return fail(need_bias ? "the bias epilogue needs bias" : "bias given without a bias epilogue");
+  if (need_mask != (p.mask >= 0)) return fail(need_mask ? "the mask epilogue needs mask" : "mask given without a mask epilogue");
+  if (((f & GG_COLSUM) != 0) != (p.colsum >= 0)) return fail("colsum goes with GG_COLSUM");
+  const bool have_planes = p.A_hi >= 0 && p.A_lo >= 0 && p.B_hi >= 0 && p.B_lo >= 0;
+  const bool any_plane = p.A_hi >= 0 || p.A_lo >= 0 || p.B_hi >= 0 || p.B_lo >= 0;
+  if (planes && (!have_planes || p.A >= 0 || p.B >= 0)) return fail("GG_PLANES reads A_hi, A_lo, B_hi and B_lo, not A and B");
+  if (!planes && (p.A < 0 || p.B < 0 || any_plane)) return fail("fp32 problems read A and B, not planes");
+  if ((p.bR_p >= 0 || p.bN_p >= 0) && (!planes || mn)) return fail("bR_p / bN_p are read by K-major plane problems only");
+  // vector stores of the epilogue (float4 C and mask, uint2 C_hi / C_lo) start at the region's offset plus multiples of 4
+  if (p.C % 4 || (need_mask && p.mask % 4) || (p.C_hi >= 0 && (p.C_hi % 4 || p.C_lo % 4)))
+    return fail("C, mask, C_hi and C_lo must start 16-byte (C_hi / C_lo: 8-byte) aligned (the vector epilogue stores)");
+  // tables: K-major plane problems read their r tables (aR, and bR_p or bR) up to index 64 ceil(R / 64) - 8
+  const int rk = planes && !mn ? (p.R + GG_TC_BK - 1) / GG_TC_BK * GG_TC_BK - 7 : p.R;
+  TcTab t[10];
+  const int64_t offs[10] = {p.aM, p.aR, p.bR, p.bN, p.cM, p.cN, p.kM, p.kN, p.bR_p, p.bN_p};
+  const char* names[10] = {"aM", "aR", "bR", "bN", "cM", "cN", "kM", "kN", "bR_p", "bN_p"};
+  const int lens[10] = {p.M, p.R, p.R, p.N, p.M, p.N, p.M, p.N, p.R, p.N};
+  for (int i = 0; i < 10; ++i) {
+    t[i].name = names[i]; t[i].off = offs[i]; t[i].len = t[i].reach = lens[i];
+    if (offs[i] < 0) {
+      if (i < 6) return fail(std::string(names[i]) + " is required");
+      continue;
+    }
+    t[i].v = tabs + offs[i];
+  }
+  for (int i : {6, 7}) if (!t[i].v) t[i] = t[i - 2];            // kM / kN default to cM / cN
+  const TcTab &aM = t[0], &aR = t[1], &bR = t[2], &bN = t[3], &cM = t[4], &cN = t[5], &kM = t[6], &kN = t[7];
+  TcTab bRk = t[8].v ? t[8] : bR, bNk = t[9].v ? t[9] : bN;    // the K-major plane B's own tables
+  TcTab aRk = aR;
+  if (planes && !mn) { aRk.reach = rk; bRk.reach = rk; }
+  for (const TcTab* q : std::initializer_list<const TcTab*>{&aM, &aR, &bR, &bN, &cM, &cN, &kM, &kN, &aRk, &bRk, &bNk})
+    if (q->off + q->reach > n_tabs) return fail(std::string(q->name) + " runs past the end of tabs");
+  // [lo, hi] of the elements a table addresses; MN-major plane problems copy 8 elements from every 8-group start of aM / bN
+  auto span = [](const TcTab& q, int g8) {
+    int64_t lo = INT64_MAX, hi = INT64_MIN;
+    for (int i = 0; i < q.len; i += g8 ? 8 : 1) { lo = std::min<int64_t>(lo, q.v[i]); hi = std::max<int64_t>(hi, q.v[i] + (g8 ? 7 : 0)); }
+    return std::make_pair(lo, hi);
+  };
+  auto in = [&](const char* what, int64_t base, std::pair<int64_t, int64_t> x, std::pair<int64_t, int64_t> y, int64_t n) {
+    return base + x.first + y.first >= 0 && base + x.second + y.second < n ? 0 : fail(std::string(what) + " reaches outside its arena");
+  };
+  const auto zero = std::make_pair<int64_t, int64_t>(0, 0);
+  if (!planes) {
+    if (int rc = in("A[aM + aR]", p.A, span(aM, 0), span(aR, 0), n_f32)) return rc;
+    if (int rc = in("B[bR + bN]", p.B, span(bR, 0), span(bN, 0), n_f32)) return rc;
+  } else {
+    const auto sa = span(aM, mn), sb = mn ? span(bN, 1) : span(bNk, 0), ra = span(aR, 0), rb = mn ? span(bR, 0) : span(bRk, 0);
+    for (int64_t base : {p.A_hi, p.A_lo}) if (int rc = in("A_hi / A_lo[aM + aR]", base, sa, ra, n_u16)) return rc;
+    for (int64_t base : {p.B_hi, p.B_lo}) if (int rc = in("B_hi / B_lo[bR + bN]", base, rb, sb, n_u16)) return rc;
+  }
+  if (int rc = in("C[cM + cN]", p.C, span(cM, 0), span(cN, 0), n_f32)) return rc;
+  if (p.C_hi >= 0)
+    for (int64_t base : {p.C_hi, p.C_lo}) if (int rc = in("C_hi / C_lo[cM + cN]", base, span(cM, 0), span(cN, 0), n_u16)) return rc;
+  if (need_bias) if (int rc = in("bias[n]", p.bias, zero, std::make_pair<int64_t, int64_t>(0, p.N - 1), n_f32)) return rc;
+  if (need_mask) if (int rc = in("mask[kM + kN]", p.mask, span(kM, 0), span(kN, 0), n_f32)) return rc;
+  if (f & GG_COLSUM) if (int rc = in("colsum[n]", p.colsum, zero, std::make_pair<int64_t, int64_t>(0, p.N - 1), n_f32)) return rc;
+  // w-groups of table g (entries [w k, w k + w)) read with one vector load: contiguous, and base + the group's first offset + every
+  // offset of the other side a multiple of `align` elements of `eb` bytes.  partial: a last group shorter than w is loaded too
+  // (its valid part).
+  auto groups = [&](const char* what, int64_t base, const TcTab& g, const TcTab& other, int w, int align, int eb, bool partial) {
+    bool any = false;
+    for (int i = 0; i < g.len; i += w) {
+      if (!partial && i + w > g.len) break;
+      any = true;
+      for (int j = 1; j < w && i + j < g.len; ++j)
+        if (g.v[i + j] != g.v[i] + j)
+          return fail(std::string(what) + ": " + g.name + " is not contiguous in the " + std::to_string(w) + "-group at " + std::to_string(i));
+      if ((base + g.v[i] + other.v[0]) % align)
+        return fail(std::string(what) + ": the " + std::to_string(w) + "-groups of " + g.name + " are not " + std::to_string(align * eb) +
+                    "-byte aligned");
+    }
+    if (any)
+      for (int j = 0; j < other.len; ++j)
+        if ((base + g.v[0] + other.v[j]) % align)
+          return fail(std::string(what) + ": the " + std::to_string(w) + "-groups of " + g.name + " are not aligned at every " + other.name);
+    return 0;
+  };
+  if (!planes) {        // float4 loads of full 4-groups (16 bytes of fp32)
+    if (int rc = (f & GG_A_RVEC) ? groups("GG_A_RVEC", p.A, aR, aM, 4, 4, 4, false) : groups("m-direction A", p.A, aM, aR, 4, 4, 4, false))
+      return rc;
+    if (int rc = (f & GG_B_RVEC) ? groups("GG_B_RVEC", p.B, bR, bN, 4, 4, 4, false) : groups("n-direction B", p.B, bN, bR, 4, 4, 4, false))
+      return rc;
+    // int4 loads of the r tables of m- / n-direction operands (and of bR beside an m-direction A)
+    if (!(f & GG_A_RVEC) && p.aR % 4) return fail("aR must start 16-byte aligned (int4 table loads)");
+    if (!((f & GG_A_RVEC) && (f & GG_B_RVEC)) && p.bR % 4) return fail("bR must start 16-byte aligned (int4 table loads)");
+  } else {              // cp.async of 8-groups of BF16 (16 bytes; two 8-byte halves of A under GG_A_ALIGN4)
+    const int aal = al4 ? 4 : 8;
+    for (int64_t base : {p.A_hi, p.A_lo})
+      if (int rc = mn ? groups("MN-major A", base, aM, aR, 8, aal, 2, true) : groups("K-major A", base, aR, aM, 8, aal, 2, true)) return rc;
+    for (int64_t base : {p.B_hi, p.B_lo})
+      if (int rc = mn ? groups("MN-major B", base, bN, bR, 8, 8, 2, true) : groups("K-major B", base, bRk, bNk, 8, 8, 2, true)) return rc;
+  }
+  return 0;
+}
+}  // namespace
+
+extern "C" int b2g_debug_gg_tc(int x3, const b2g_debug_gg_tc_problem* p, int n, float* f32, int64_t n_f32, uint16_t* u16, int64_t n_u16,
+                               const int32_t* tabs, int64_t n_tabs) {
+  if (x3 != 0 && x3 != 1) return b2g_fail(B2G_EINVAL, "x3 must be 0 (hi*hi) or 1 (hi*hi + hi*lo + lo*hi)");
+  if (!p || n < 1 || n > GG_TC_MAX_DESCS) return b2g_fail(B2G_EINVAL, "1 to 16 problems per launch");
+  const int64_t lim = (int64_t)1 << 31;
+  if (n_f32 < 0 || n_u16 < 0 || n_tabs < 0 || n_f32 >= lim || n_u16 >= lim || n_tabs >= lim)
+    return b2g_fail(B2G_EINVAL, "arena lengths must be in 0 .. 2^31 - 1");
+  if ((n_f32 && !f32) || (n_u16 && !u16) || (n_tabs && !tabs)) return b2g_fail(B2G_EINVAL, "NULL arena");
+  auto kernel_of = [](int f) { return (f & GG_PLANES) ? GG_PLANES : f & (GG_A_RVEC | GG_B_RVEC); };
+  for (int i = 1; i < n; ++i)
+    if (kernel_of(p[i].flags) != kernel_of(p[0].flags))
+      return b2g_fail(B2G_EINVAL, "problem " + std::to_string(i) +
+                                      ": its flags select another gg_tc kernel than problem 0's (GG_PLANES, else GG_A_RVEC | GG_B_RVEC)");
+  for (int i = 0; i < n; ++i)
+    if (int rc = check_gg_tc_problem(i, p[i], n_f32, n_u16, tabs, n_tabs)) return rc;
+
+  int num_sms = 0;
+  if (int rc = check_device(0, &num_sms)) return rc;
+  cudaStream_t s = nullptr;
+  CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+  std::vector<void*> allocs;
+  const int rc = [&]() -> int {
+    float* d32 = nullptr; uint16_t* d16 = nullptr; int32_t* dt = nullptr;
+    if (int rc = dev_alloc(allocs, s, &d32, n_f32, false)) return rc;
+    if (int rc = dev_alloc(allocs, s, &d16, n_u16, false)) return rc;
+    if (int rc = dev_alloc(allocs, s, &dt, n_tabs, false)) return rc;
+    if (n_f32) CK(cudaMemcpyAsync(d32, f32, n_f32 * sizeof(float), cudaMemcpyHostToDevice, s));
+    if (n_u16) CK(cudaMemcpyAsync(d16, u16, n_u16 * sizeof(uint16_t), cudaMemcpyHostToDevice, s));
+    if (n_tabs) CK(cudaMemcpyAsync(dt, tabs, n_tabs * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    // host copies of the epilogue tables under their device addresses, as the SAC handle keeps them, for gg_tc_columns
+    std::map<const int*, std::vector<int>> host_tabs;
+    auto keep = [&](int64_t off, int len) {
+      if (off < 0) return;
+      std::vector<int>& v = host_tabs[dt + off];
+      if ((int)v.size() < len) v.assign(tabs + off, tabs + off + len);
+    };
+    ColIds col_ids;
+    GemmGroup g;
+    g.name = "debug_gg_tc";
+    g.tc = true;
+    auto f32p = [&](int64_t off) { return off >= 0 ? d32 + off : nullptr; };
+    auto u16p = [&](int64_t off) { return off >= 0 ? d16 + off : nullptr; };
+    auto tabp = [&](int64_t off) -> const int* { return off >= 0 ? dt + off : nullptr; };
+    for (int i = 0; i < n; ++i) {
+      const b2g_debug_gg_tc_problem& q = p[i];
+      keep(q.cM, q.M); keep(q.cN, q.N); keep(q.kM, q.M); keep(q.kN, q.N);
+      GemmDesc d = gemm_desc(f32p(q.A), tabp(q.aM), tabp(q.aR), f32p(q.B), tabp(q.bR), tabp(q.bN), d32 + q.C, tabp(q.cM), tabp(q.cN),
+                             q.M, q.N, q.R, q.flags, q.splitR);
+      d.kM = tabp(q.kM); d.kN = tabp(q.kN);
+      d.bias = f32p(q.bias); d.mask = f32p(q.mask); d.colsum = f32p(q.colsum);
+      d.A_hi = u16p(q.A_hi); d.A_lo = u16p(q.A_lo); d.B_hi = u16p(q.B_hi); d.B_lo = u16p(q.B_lo);
+      d.bR_p = tabp(q.bR_p); d.bN_p = tabp(q.bN_p);
+      d.C_hi = u16p(q.C_hi); d.C_lo = u16p(q.C_lo);
+      g.host.push_back(d);
+    }
+    for (auto& d : g.host) gg_tc_columns(d, host_tabs, col_ids);
+    if (int rc = finalize_tiles(g, allocs, s, GG_TC_BM, GG_TC_BN)) return rc;
+    CK(gg_tc_launch(g.host.data(), n, g.total_tiles, g.host[0].flags, x3, num_sms, s));
+    if (n_f32) CK(cudaMemcpyAsync(f32, d32, n_f32 * sizeof(float), cudaMemcpyDeviceToHost, s));
     if (n_u16) CK(cudaMemcpyAsync(u16, d16, n_u16 * sizeof(uint16_t), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     return 0;

@@ -67,6 +67,35 @@ int finalize_tiles(GemmGroup& g, std::vector<void*>& allocs, cudaStream_t s, int
   return 0;
 }
 
+void gg_tc_columns(GemmDesc& d, const std::map<const int*, std::vector<int>>& host_tabs, ColIds& col_ids) {
+  {   // GG_CN_AFFINE4: column tables contiguous in aligned groups of 4, row offsets multiples of 4
+    auto grp4 = [&](const int* tab, int n) {
+      auto it = host_tabs.find(tab);
+      if (it == host_tabs.end() || (int)it->second.size() < n) return false;
+      const std::vector<int>& v = it->second;
+      for (int i = 0; i + 3 < n; i += 4)
+        if ((v[i] & 3) || v[i + 1] != v[i] + 1 || v[i + 2] != v[i] + 2 || v[i + 3] != v[i] + 3) return false;
+      return true;
+    };
+    auto mult4 = [&](const int* tab, int n) {
+      auto it = host_tabs.find(tab);
+      if (it == host_tabs.end() || (int)it->second.size() < n) return false;
+      for (int i = 0; i < n; ++i) if (it->second[i] & 3) return false;
+      return true;
+    };
+    bool ok = (d.N % 4 == 0) && grp4(d.cN, d.N) && mult4(d.cM, d.M);
+    if (ok && (d.flags & GG_EPI_MASK)) ok = (!d.kN || grp4(d.kN, d.N)) && (!d.kM || mult4(d.kM, d.M));
+    if (ok) d.flags |= GG_CN_AFFINE4;
+  }
+  {   // column-table identity (gg_tc.cu epilogue): descriptors with the same tables never trigger a re-stage
+    const auto key = std::make_tuple((const void*)d.cN, (const void*)d.kN,
+                                     (const void*)((d.flags & GG_EPI_BIAS_RELU) ? d.bias : nullptr), d.N);
+    auto it = col_ids.find(key);
+    if (it == col_ids.end()) it = col_ids.emplace(key, (int)col_ids.size()).first;
+    d.col_id = it->second;
+  }
+}
+
 int capture_graph(cudaStream_t s, const std::function<int()>& issue, cudaGraphExec_t* exec) {
   cudaGraph_t graph = nullptr;
   CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));

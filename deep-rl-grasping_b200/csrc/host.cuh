@@ -8,6 +8,7 @@
 #include <functional>
 #include <map>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "../../include/b200grasp.h"
@@ -60,6 +61,14 @@ GemmDesc gemm_desc(const float* A, const int* aM, const int* aR, const float* B,
 // Tile grid of every descriptor of a grouped launch (bm x bn output tiles, splitR slices each), their tile_start / tile_count
 // and the group's total_tiles; then the descriptors are copied to g.dev (allocated on the first call), synchronously.
 int finalize_tiles(GemmGroup& g, std::vector<void*>& allocs, cudaStream_t s, int bm = GG_SIMT_BM, int bn = GG_SIMT_BN);
+
+// Identity of the column tables of a wgmma-engine descriptor, (cN, kN, bias under GG_EPI_BIAS_RELU, N) -> id: equal ids share the
+// column tables the gg_tc.cu epilogue stages, so consecutive tiles of such descriptors do not re-stage them.
+using ColIds = std::map<std::tuple<const void*, const void*, const void*, int>, int>;
+// The descriptor fields derived from its tables rather than given by the caller: GG_CN_AFFINE4 (set when the host copies in
+// host_tabs show N % 4 == 0, cN contiguous in aligned groups of 4 and cM a multiple of 4, and under GG_EPI_MASK the same of
+// kN and kM when given) and col_id (new tables take the next id of col_ids).
+void gg_tc_columns(GemmDesc& d, const std::map<const int*, std::vector<int>>& host_tabs, ColIds& col_ids);
 
 // Captures what issue() enqueues on s into a graph and instantiates it into *exec.  A failing issue() ends the capture and
 // returns its code.

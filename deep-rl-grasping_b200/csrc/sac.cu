@@ -118,42 +118,17 @@ void build_params(b2g_sac* h) {
   h->n_all = off;
 }
 
-// SAC's passes over a group before the shared tile layout: GG_CN_AFFINE4, split-R, column-table ids, flops
+// SAC's passes over a group before the shared tile layout: GG_CN_AFFINE4 and column-table ids (gg_tc_columns), split-R, flops
 int finalize_group(b2g_sac* h, GemmGroup& g) {
   g.flops = 0;
   const int bm = g.tc ? GG_TC_BM : GG_SIMT_BM, bn = g.tc ? GG_TC_BN : GG_SIMT_BN, bk = g.tc ? GG_TC_BK : GG_SIMT_BK;
   for (auto& d : g.host) {
-    {   // GG_CN_AFFINE4: column tables contiguous in aligned groups of 4, row offsets multiples of 4
-      auto grp4 = [&](const int* tab, int n) {
-        auto it = h->host_tabs.find(tab);
-        if (it == h->host_tabs.end() || (int)it->second.size() < n) return false;
-        const std::vector<int>& v = it->second;
-        for (int i = 0; i + 3 < n; i += 4)
-          if ((v[i] & 3) || v[i + 1] != v[i] + 1 || v[i + 2] != v[i] + 2 || v[i + 3] != v[i] + 3) return false;
-        return true;
-      };
-      auto mult4 = [&](const int* tab, int n) {
-        auto it = h->host_tabs.find(tab);
-        if (it == h->host_tabs.end() || (int)it->second.size() < n) return false;
-        for (int i = 0; i < n; ++i) if (it->second[i] & 3) return false;
-        return true;
-      };
-      bool ok = (d.N % 4 == 0) && grp4(d.cN, d.N) && mult4(d.cM, d.M);
-      if (ok && (d.flags & GG_EPI_MASK)) ok = (!d.kN || grp4(d.kN, d.N)) && (!d.kM || mult4(d.kM, d.M));
-      if (ok) d.flags |= GG_CN_AFFINE4;
-    }
+    gg_tc_columns(d, h->host_tabs, h->col_ids);
     if (d.flags & GG_EPI_ATOMIC) {     // split-R sized for this engine's tile grid
       const int tiles = ((d.M + bm - 1) / bm) * ((d.N + bn - 1) / bn);
       int sp = std::max(1, h->num_sms / std::max(1, tiles));
       sp = std::min(sp, std::max(1, d.R / (2 * bk)));
       d.splitR = sp;
-    }
-    {   // column-table identity (gg_tc.cu epilogue): descriptors with the same tables never trigger a re-stage
-      const auto key = std::make_tuple((const void*)d.cN, (const void*)d.kN,
-                                       (const void*)((d.flags & GG_EPI_BIAS_RELU) ? d.bias : nullptr), d.N);
-      auto it = h->col_ids.find(key);
-      if (it == h->col_ids.end()) it = h->col_ids.emplace(key, (int)h->col_ids.size()).first;
-      d.col_id = it->second;
     }
     g.flops += 2.0 * d.M * d.N * d.R;
   }

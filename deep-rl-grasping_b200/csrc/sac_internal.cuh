@@ -201,7 +201,7 @@ struct b2g_sac {
   cudaStream_t aux2 = nullptr;             // the second leaf branch under the gather (bookkeeping kernel, gradient zeroing)
   cudaEvent_t ev_aux[9]{};
   bool fork_leaves = false;
-  std::map<std::tuple<const void*, const void*, const void*, int>, int> col_ids;
+  ColIds col_ids;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   bool overlap_ar = false;             // engine v2, N > 1: early all-reduce on the side stream (B2G_AR_OVERLAP=0 disables)
   int ar_sms = 8;

@@ -585,6 +585,39 @@ typedef struct {
 int b2g_debug_gg_simt(int build, const b2g_debug_gg_problem* p, int n, float* f32, int64_t n_f32, double* f64, int64_t n_f64,
                       uint16_t* u16, int64_t n_u16, const int32_t* tabs, int64_t n_tabs);
 
+/* Bring-up hook (not on the product path): one grouped launch of the wgmma gather-GEMM engine (csrc/gg_tc.cu) over 1 to 16
+ * problems the caller describes; x3 = 1 multiplies hi*hi + hi*lo + lo*hi of the BF16 operand splits, x3 = 0 hi*hi only.
+ * Problem p computes C[cM[m] + cN[n]] (=|+=) epi( sum_r A[aM[m] + aR[r]] * B[bR[r] + bN[n]] ) from fp32 A and B (offsets into
+ * f32), or under B2G_GG_PLANES from BF16 planes A_hi / A_lo / B_hi / B_lo (offsets into u16; the plane B of a K-major problem
+ * reads through bR_p / bN_p when given).  C, bias, mask and colsum are offsets into f32, C_hi / C_lo into u16 (-1: none), the
+ * tables into tabs (kM / kN -1: cM / cN).  GG_CN_AFFINE4 and the column-table ids are derived from the tables as the SAC
+ * handle derives them; the tiles are laid out as the handle lays them out (splitR is the caller's).  The arenas are uploaded,
+ * the group launched once on a stream of its own, and f32 and u16 copied back.
+ * Before any CUDA call, B2G_EINVAL (b2g_last_error names the broken contract) refuses: x3 not 0 or 1; n outside 1..16;
+ * problems whose flags select different kernels (B2G_GG_PLANES, else B2G_GG_A_RVEC | B2G_GG_B_RVEC); a flag the engine does not
+ * implement (only A_RVEC, B_RVEC, EPI_BIAS_RELU, EPI_MASK, EPI_ATOMIC, COLSUM, PLANES, A_ALIGN4, MN_MAJOR and A_ROWLANES are);
+ * A_ALIGN4, MN_MAJOR or A_ROWLANES without PLANES; COLSUM with B_RVEC or PLANES (the column sums are taken from the fp32
+ * n-direction B loads); M, N, R < 1, splitR outside 1..R, splitR > 1 without EPI_ATOMIC; C_hi / C_lo with EPI_ATOMIC or one
+ * without the other; an operand missing or given where the problem does not read it; an address any table can reach outside its
+ * arena (the K-major plane producers also read the r tables up to index 64 ceil(R / 64) - 8, and the MN-major ones 8 elements
+ * from every 8-group start of aM / bN); a 16-byte fp32 load (r-, m- or n-direction 4-group), int4 table load, 16-byte plane
+ * copy (8-group; 8 bytes per half under A_ALIGN4) or vector output store whose elements are not contiguous or whose address is
+ * not aligned.  Arena lengths are element counts below 2^31.  Flag values beside B2G_GG_* above: */
+#define B2G_GG_PLANES (1 << 6)
+#define B2G_GG_A_ALIGN4 (1 << 7)
+#define B2G_GG_MN_MAJOR (1 << 9)
+#define B2G_GG_A_ROWLANES (1 << 14)
+typedef struct {
+  int64_t A, B, C, bias, mask, colsum;       /* offsets into f32; -1 = none (A and B are -1 under B2G_GG_PLANES) */
+  int64_t aM, aR, bR, bN, cM, cN, kM, kN;    /* offsets into tabs; kM / kN -1 = cM / cN */
+  int64_t bR_p, bN_p;                        /* offsets into tabs, K-major plane problems only; -1 = bR / bN */
+  int64_t A_hi, A_lo, B_hi, B_lo;            /* offsets into u16, plane problems only; -1 = none */
+  int64_t C_hi, C_lo;                        /* offsets into u16, -1 = none */
+  int32_t M, N, R, flags, splitR;
+} b2g_debug_gg_tc_problem;
+int b2g_debug_gg_tc(int x3, const b2g_debug_gg_tc_problem* p, int n, float* f32, int64_t n_f32, uint16_t* u16, int64_t n_u16,
+                    const int32_t* tabs, int64_t n_tabs);
+
 /* Bring-up hook (not on the product path): one plane of one named device tensor of a SAC handle, copied to the host after the
  * handle's stream is synchronised.  BF16 planes come back as raw uint16 (elem_bytes 2), fp32 buffers as float (elem_bytes 4);
  * bytes must be numel * elem_bytes.  Returns B2G_EINVAL for an unknown name, a plane out of range or a size mismatch, and

@@ -30,6 +30,7 @@ from b200grasp import _lib, synth
 from oracle import sac_ref as R
 from oracle import sac_ref_np as N
 from tests.test_conv1_s2d_cpu import conv1_krow, s2d, w1t
+from tests.gg_tc_ref import SPLIT2, U32, U_TC, Report, bf, bf16_split, gg_gammas
 from tests.test_gpu_configs import vecnorm_for
 from tests.util import load_case, make_batch, make_learner
 
@@ -39,12 +40,8 @@ SCOPES = ("model/pi", "model/values_fn", "target/values_fn")
 HEADS = (("pi", "model/pi"), ("vf", "model/values_fn/vf"), ("qf1", "model/values_fn/qf1"), ("qf2", "model/values_fn/qf2"))
 
 # ------------------------------------------------------------------------------------------------ error model
-U_TC = 2.0 ** -23         # one tensor-core k-step: the products' alignment and the accumulator are truncated, not rounded
-U32 = 2.0 ** -24          # one round-to-nearest fp32 addition or FMA
 # 3 planes, 6 products (p + q <= 2): the missing A_1 B_2 + A_2 B_1 + A_2 B_2, with |A_1| <= 2^-8 (1 + 2^-8) |a|, |A_2| <= 2^-16 |a|
 SPLIT3 = 2 * 2.0 ** -8 * (1 + 2.0 ** -8) * 2.0 ** -16 + 2.0 ** -32
-# 2 planes, 3 products: the missing A_1 B_1
-SPLIT2 = (2.0 ** -8 * (1 + 2.0 ** -8)) ** 2
 R2 = 2.0 ** -16           # a value stored as 2 BF16 planes (3 planes hold an fp32 value exactly)
 
 
@@ -88,21 +85,6 @@ def problem_gammas(B, ci, split_fc1=3, split_dgrad=1):
 
 
 # ------------------------------------------------------------------------------------------------ layouts in float64
-def bf16_split(x, n):
-    """The first n BF16 planes of fp32 x as uint16: plane k = round-to-nearest of the k-th residual (split3 / planes2)."""
-    x = torch.from_numpy(np.ascontiguousarray(x, np.float32))
-    out = []
-    for _ in range(n):
-        h = x.to(torch.bfloat16)
-        out.append(h.view(torch.int16).numpy().view(np.uint16).copy())
-        x = x - h.float()
-    return out
-
-
-def bf(u16):
-    return (np.asarray(u16).astype(np.uint32) << 16).view(np.float32).astype(np.float64)
-
-
 def img_from_s(S, ci):
     """S [B, 16, 16, 4, 4, Cp] -> image [B, 64, 64, ci] (inverse of test_conv1_s2d_cpu.s2d)."""
     B = S.shape[0]
@@ -153,38 +135,6 @@ def mm(a, b):
 
 
 # ------------------------------------------------------------------------------------------------ checks
-class Report:
-    def __init__(self, case):
-        self.case, self.worst, self.fail = case, {}, []
-
-    def hold(self, name, got, ref, mag, gamma, r=0.0):
-        got, ref, mag = (np.asarray(a, np.float64) for a in (got, ref, mag))
-        bar = gamma * mag + r * np.abs(ref)
-        err = np.abs(got - ref)
-        ratio = np.where(bar > 0, err / np.where(bar > 0, bar, 1.0), np.where(err > 0, np.inf, 0.0))
-        worst = float(ratio.max()) if ratio.size else 0.0
-        self.worst[name] = max(worst, self.worst.get(name, 0.0))
-        if worst > 1.0:
-            i = np.unravel_index(int(np.argmax(ratio)), ratio.shape)
-            self.fail.append(f"{name}: err/bar {worst:.3g} at {tuple(int(k) for k in i)} (got {got[i]:.9g}, ref {ref[i]:.9g}, "
-                             f"bar {bar[i]:.3g}); {int((ratio > 1).sum())} of {ratio.size} elements over")
-
-    def exact(self, name, got, want):
-        got, want = np.asarray(got), np.asarray(want)
-        bad = int((got != want).sum())
-        self.worst[name] = max(self.worst.get(name, 0.0), 0.0 if bad == 0 else np.inf)
-        if bad:
-            i = np.unravel_index(int(np.argmax(got != want)), got.shape)
-            self.fail.append(f"{name}: {bad} of {got.size} elements differ (first at {tuple(int(k) for k in i)}: "
-                             f"{got[i]} != {want[i]})")
-
-    def finish(self):
-        print(f"\n[{self.case}] worst err/bar per problem (bit-exact checks: 0 = equal):")
-        for k, v in self.worst.items():
-            print(f"  {k:28s} {v:.3g}")
-        assert not self.fail, "\n".join(self.fail)
-
-
 def read(L, name):
     """All planes of one debug tensor: uint16 [planes][numel] for BF16 planes, float32 [1][numel] for fp32 buffers."""
     n, p, eb = C.c_int64(), C.c_int32(), C.c_int32()
@@ -598,17 +548,6 @@ def test_debug_tensor_refuses_bad_requests():
 
 # ------------------------------------------------------------------------------------------------ gg_tc (b2g_debug_gemm)
 GG_M, GG_N = (1, 127, 128, 129, 300), (1, 16, 17, 33, 64, 65, 130)
-
-
-def gg_gammas(K, split_k, x3):
-    """gg_tc: chunks of 64 K rows, all products of a k-step into ONE accumulator (hi*hi, then hi*lo, lo*hi), split-K partials
-    summed with red.add into the zeroed output."""
-    per = _cdiv(_cdiv(K, split_k), 64) * 64 if split_k > 1 else _cdiv(K, 64) * 64
-    acc = 1.01 * (2 * U_TC * (per // 16) * (3 if x3 else 1) + U32 * split_k)
-    # the split against the exact product: x3 misses lo*lo and each operand's residual below its lo plane; x3 = 0 misses all
-    # but hi*hi
-    split = (SPLIT2 + 2 * 2.0 ** -16 + 2.0 ** -32) if x3 else (2 * 2.0 ** -8 + 2.0 ** -16)
-    return acc, 1.01 * split + acc
 
 
 @pytest.mark.gpu
