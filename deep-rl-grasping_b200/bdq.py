@@ -10,16 +10,16 @@ are branch bin indices, mapped to linspace(-1, 1, n_bins).
 from __future__ import annotations
 
 import ctypes as C
-import os
 from collections import OrderedDict
 from typing import Optional
 
 import numpy as np
 
-from . import _lib, sb_io, training_state
+from . import _lib, training_state
+from .base_model import BaseModel
 from .callbacks import as_callback
-from .learner import HandleLearner, _f32, _fp
-from .vec_env import DummyVecEnv, VecNormalize
+from .learner import HandleLearner, _f32, _fp, nccl_config
+from .vec_env import VecNormalize
 
 
 class BDQLearner(HandleLearner):
@@ -32,20 +32,14 @@ class BDQLearner(HandleLearner):
         self.lib = _lib.load()
         if layers[1][0] != layers[2][0]:
             raise NotImplementedError("branch and state-value hidden widths must match (every shipped zip / config)")
-        self._id_buf, idp, libp = None, None, None
-        if nranks > 1:
-            if nccl_id is None or len(nccl_id) != 128:
-                raise ValueError("nranks > 1 needs the 128-byte nccl_id shared by all ranks")
-            self._id_buf = C.create_string_buffer(bytes(nccl_id), 128)
-            idp = C.cast(self._id_buf, C.c_void_p)
-            lp = _lib.default_nccl_lib()
-            libp = lp.encode() if lp else None
+        self._id_buf, idp, libp = nccl_config(nranks, nccl_id)
         cfg = _lib.BdqCfg(obs_dim, n_branches, n_bins, layers[0][0], layers[0][1], layers[1][0], batch_size, buffer_size, gamma,
                           target_network_update_freq, int(trunk_grad_rescale), seed, device, rank, nranks, idp, libp,
                           int(bool(prioritized_replay)), float(prioritized_replay_alpha), float(prioritized_replay_eps))
         self.prioritized_replay = bool(prioritized_replay)
         self._create(cfg)
-        self.obs_dim, self.n_branches, self.n_bins, self.batch_size = obs_dim, n_branches, n_bins, batch_size
+        self.obs_dim = self.obs_elems = obs_dim
+        self.n_branches, self.n_bins, self.batch_size = n_branches, n_bins, batch_size
         self.obs_shape = (obs_dim,)          # shape of obs_rms_get's arrays (BDQ sets the env's observation shape)
 
     def _has_grad(self, name):
@@ -59,49 +53,7 @@ class BDQLearner(HandleLearner):
     def replay_size(self):
         return int(self.lib.b2g_bdq_replay_size(self.h))
 
-    def load_state(self, path: str):
-        """Restores a ``save_state`` file into this learner, which must have the same configuration (and own a device
-        ``obs_rms`` exactly when the file carries one)."""
-        super().load_state(path)
-        self.obs_rms_version += 1
-
-    def set_norm_stats(self, obs_mean=None, obs_var=None, ret_var=1.0, clip_obs=10.0, clip_reward=10.0, epsilon=1e-8,
-                       norm_obs=True, norm_reward=True):
-        """VecNormalize's statistics for the gather of the gradient step and act().  ``obs_mean = obs_var = None`` with
-        ``norm_obs``: a learner that owns ``obs_rms`` keeps its device statistics and takes the scalars only."""
-        dp = C.POINTER(C.c_double)
-        mp = vp = None
-        if norm_obs and obs_mean is not None:
-            m = np.ascontiguousarray(obs_mean, np.float64).reshape(-1)
-            v = np.ascontiguousarray(obs_var, np.float64).reshape(-1)
-            assert m.size == self.obs_dim and v.size == self.obs_dim
-            mp, vp = m.ctypes.data_as(dp), v.ctypes.data_as(dp)
-        _lib.check(self.lib.b2g_bdq_set_norm_stats(self.h, mp, vp, float(ret_var), float(clip_obs), float(clip_reward),
-                                                    float(epsilon), int(bool(norm_obs)), int(bool(norm_reward))))
-        if mp is not None:
-            self.obs_rms_version += 1
-
-    # ---- device-resident obs_rms and the actor loop on one upload per frame (include/b200grasp.h: b2g_bdq_observe_*)
-    #: bumped by every call that may change the device statistics (DeviceRunningMeanStd caches against it)
-    obs_rms_version = 0
-
-    def obs_rms_set(self, mean, var, count):
-        """Creates (first call) or overwrites the device ``obs_rms``: float64 mean / var of the observation + count."""
-        dp = C.POINTER(C.c_double)
-        m = np.ascontiguousarray(mean, np.float64).reshape(-1)
-        v = np.ascontiguousarray(var, np.float64).reshape(-1)
-        assert m.size == self.obs_dim and v.size == self.obs_dim
-        _lib.check(self.lib.b2g_bdq_obs_rms_set(self.h, m.ctypes.data_as(dp), v.ctypes.data_as(dp), float(count)))
-        self.obs_rms_version += 1
-
-    def obs_rms_get(self):
-        """(mean, var, count) of the device ``obs_rms`` in ``obs_shape``; waits for the work enqueued on the handle."""
-        dp = C.POINTER(C.c_double)
-        m, v = np.empty(self.obs_shape, np.float64), np.empty(self.obs_shape, np.float64)
-        cnt = C.c_double()
-        _lib.check(self.lib.b2g_bdq_obs_rms_get(self.h, m.ctypes.data_as(dp), v.ctypes.data_as(dp), C.byref(cnt)))
-        return m, v, float(cnt.value)
-
+    # ---- the actor loop on one upload per frame (include/b200grasp.h: b2g_bdq_observe_*)
     def observe_act(self, obs, n=None, update_stats=True, eps=0.0, act=True):
         """``obs``: n raw observations to upload, merge into ``obs_rms`` (``update_stats``) and stage as the current
         observation of env i; ``None`` acts on the ones already staged.  Returns the [n, n_branches] epsilon-greedy bin
@@ -128,13 +80,6 @@ class BDQLearner(HandleLearner):
         _lib.check(self.lib.b2g_bdq_observe_add(self.h, _fp(act), _fp(rew), _fp(next_obs), _fp(done),
                                                 None if reset_obs is None else _fp(reset_obs), n, int(bool(update_stats))))
         self.obs_rms_version += bool(update_stats)
-
-    def upload_bytes(self) -> dict:
-        """Bytes copied host -> device so far: by ``observe_*`` / ``obs_rms_set``, and by ``act`` + ``replay_add`` +
-        ``set_norm_stats``."""
-        a, b = C.c_int64(), C.c_int64()
-        _lib.check(self.lib.b2g_bdq_upload_bytes(self.h, C.byref(a), C.byref(b)))
-        return {"observe": int(a.value), "other": int(b.value)}
 
     def step(self, n_steps=1, lr=1e-4):
         m = _lib.BdqMetrics()
@@ -171,9 +116,10 @@ class BDQLearner(HandleLearner):
         return out
 
 
-class BDQ:
+class BDQ(BaseModel):
     """SB-shaped front end: ``BDQ(policy, env, policy_kwargs={'layers': [[64,64],[32],[32]]}, num_actions_pad=33, ...)``
     with ``learn / predict / save / load / get_parameters / load_parameters`` (sb_helper.py:202-226)."""
+    _algo, _policy = "BDQ", "MlpActPolicy"
 
     def __init__(self, policy, env, gamma=0.99, learning_rate=1e-4, buffer_size=1000000, exploration_fraction=0.1,
                  exploration_final_eps=0.02, train_freq=1, batch_size=64, learning_starts=1000, target_network_update_freq=1000,
@@ -201,12 +147,8 @@ class BDQ:
         self.num_timesteps = 0
         self._rng = np.random.default_rng(seed)
         self.learner: Optional[BDQLearner] = None
-        self.env = None
-        self._vec_normalize_env = None
         if env is not None:
-            self.env = env if hasattr(env, "num_envs") else DummyVecEnv([lambda: env])
-            self.observation_space, self.action_space = self.env.observation_space, self.env.action_space
-            self._vec_normalize_env = self.get_vec_normalize_env()
+            self._set_env(env)
             if _init_setup_model:
                 self.setup_model()
 
@@ -234,30 +176,8 @@ class BDQ:
         self._bins = np.linspace(-1.0, 1.0, self.num_actions_pad).astype(np.float32)
         self._attach_device_norm()
 
-    def close(self):
-        """Releases the device learner.  Observation statistics it owned go back to the VecNormalize wrapper first."""
-        if self.learner is not None:
-            if self._owns_obs_rms():
-                self._vec_normalize_env.take_obs_rms_back()
-            self.learner.close()
-            self.learner = None
-
-    def _owns_obs_rms(self) -> bool:
-        vn = self._vec_normalize_env
-        return vn is not None and self.learner is not None and getattr(vn, "obs_rms_owner", None) is self.learner
-
-    @property
-    def predict_takes_raw_obs(self) -> bool:
-        """True while a learner owns the statistics of this model's VecNormalize: that wrapper returns raw observations and
-        ``predict`` normalises them on the device."""
-        return bool(getattr(self._vec_normalize_env, "learner_owns_obs_rms", False))
-
     def _attach_device_norm(self):
-        """device_obs_norm: the wrapper's obs_rms moves to this learner, unless another learner owns it already (a second
-        model on the same env reads the owner's statistics and leaves them where they are)."""
-        vn = self._vec_normalize_env
-        if self.device_obs_norm and isinstance(vn, VecNormalize) and vn.norm_obs and not vn.learner_owns_obs_rms:
-            vn.give_obs_rms_to(self.learner)
+        super()._attach_device_norm()
         if self._owns_obs_rms():
             self._sync_norm_stats()
 
@@ -266,9 +186,6 @@ class BDQ:
         vn = self._vec_normalize_env
         self.learner.set_norm_stats(None, None, float(vn.ret_rms.var), vn.clip_obs, vn.clip_reward, vn.epsilon,
                                     norm_obs=vn.norm_obs, norm_reward=vn.norm_reward)
-
-    def get_env(self):
-        return self.env
 
     def _epsilon(self, t, total):
         frac = min(1.0, t / max(1.0, self.exploration_fraction * total))
@@ -335,29 +252,13 @@ class BDQ:
         act = self._bins[idx]
         return (act[0] if np.ndim(observation) == 1 else act), None
 
-    def get_parameters(self):
-        return OrderedDict((n + ":0", a) for n, a in self.learner.get_parameters().items())
-
-    def load_parameters(self, params, exact_match=True):
-        if isinstance(params, str):
-            _, params = sb_io.load_sb_zip(params)
-        self.learner.load_parameters(params, exact_match=exact_match)
-
-    def save(self, save_path, cloudpickle=False):
-        d = os.path.dirname(save_path)
-        if d:
-            os.makedirs(d, exist_ok=True)
-        data = {"gamma": self.gamma, "learning_rate": float(self.learning_rate), "batch_size": self.batch_size, "buffer_size": self.buffer_size,
+    def _data(self):
+        return {"gamma": self.gamma, "learning_rate": float(self.learning_rate), "batch_size": self.batch_size, "buffer_size": self.buffer_size,
                 "exploration_fraction": self.exploration_fraction, "exploration_final_eps": self.exploration_final_eps,
                 "train_freq": self.train_freq, "learning_starts": self.learning_starts, "num_actions_pad": self.num_actions_pad,
                 "target_network_update_freq": self.target_network_update_freq, "prioritized_replay": self.prioritized_replay,
                 "prioritized_replay_alpha": self.per_alpha, "prioritized_replay_beta0": self.per_beta0, "double_q": True,
                 "epsilon_greedy": True, "policy_kwargs": {"layers": self.layers}}
-        sb_io.save_sb_zip(save_path, data, self.learner.get_parameters())
-
-    def get_vec_normalize_env(self):
-        from .sac_model import unwrap_vec_normalize
-        return unwrap_vec_normalize(self.env)
 
     # ------------------------------------------------------------------ training state (training_state.py)
     def _host_state(self):
@@ -375,53 +276,22 @@ class BDQ:
             init["device_obs_norm"] = True
         return {"algo": "BDQ", "init": init, "num_timesteps": int(self.num_timesteps), "rng": training_state.rng_state(self._rng)}
 
-    def save_training_state(self, path):
-        """Writes directory ``path``: model.zip, learner.state (parameters, Adam moments, counters, the replay and its
-        priority trees), vecnormalize.pkl and host.json.  The previous contents stay loadable until the new one is complete."""
-        return training_state.save_training_state(self, path)
-
-    @classmethod
-    def load_training_state(cls, path, env, **kwargs):
-        """Rebuilds the model ``save_training_state`` wrote into ``path`` on ``env``; ``learn(n, reset_num_timesteps=False)``
-        then continues with epsilon and beta taken from ``num_timesteps``."""
-        path = training_state.resolve(path)
-        host = training_state.read_host(path)
-        if host.get("algo") != "BDQ":
-            raise ValueError(f"{path} holds a {host.get('algo')} training state")
-        model = cls("MlpActPolicy", env, **dict(host["init"], **kwargs))
-        training_state.restore_vec_normalize(path, model.env)
-        model._attach_device_norm()        # the restored statistics go back to the learner; learner.state carries the same ones
-        model.load_parameters(os.path.join(path, training_state.MODEL_FILE))
-        model.learner.load_state(os.path.join(path, training_state.STATE_FILE))
-        model.num_timesteps = int(host["num_timesteps"])
-        training_state.set_rng_state(model._rng, host["rng"])
-        return model
+    def _restore_host_state(self, host):
+        self.num_timesteps = int(host["num_timesteps"])
+        training_state.set_rng_state(self._rng, host["rng"])
 
     @classmethod
     def load(cls, load_path, env=None, **kwargs):
         from .spaces import Box
-        if not os.path.exists(load_path) and os.path.exists(load_path + ".zip"):
-            load_path += ".zip"
-        data, params = sb_io.load_sb_zip(load_path)
+        data, params = cls._read_zip(load_path)
         w0 = params["bdq/model/common_net/fully_connected/weights"]
         w1 = params["bdq/model/common_net/fully_connected_1/weights"]
         wb = params["bdq/model/action_value/fully_connected/weights"]
         wo = params["bdq/model/action_value/fully_connected_1/weights"]
         n_br = sum(1 for n in params if n.startswith("bdq/model/action_value/") and n.endswith("/weights")) // 2
-
-        class _Spaces:
-            num_envs = 1
-            observation_space = Box(-np.inf, np.inf, (w0.shape[0],))
-            action_space = Box(-1.0, 1.0, (n_br,))
-        e = env if env is not None else _Spaces()
         kw = dict(gamma=data.get("gamma", 0.99), batch_size=data.get("batch_size", 64), num_actions_pad=wo.shape[1],
                   policy_kwargs={"layers": [[w0.shape[1], w1.shape[1]], [wb.shape[1]], [wb.shape[1]]]},
                   buffer_size=min(int(data.get("buffer_size", 1000)), 1000) if env is None else data.get("buffer_size", 100000))
         kw.update(kwargs)
         m = cls("MlpActPolicy", None, _init_setup_model=False, **kw)
-        m.env = e if env is not None else None
-        m._vec_normalize_env = m.get_vec_normalize_env() if env is not None else None
-        m.observation_space, m.action_space = e.observation_space, e.action_space
-        m.setup_model()
-        m.learner.load_parameters(params, exact_match=True)
-        return m
+        return m._finish_load(env, Box(-np.inf, np.inf, (w0.shape[0],)), Box(-1.0, 1.0, (n_br,)), params)

@@ -8,16 +8,15 @@ oracle/dqn_ref.py, which also lists what trained_models/DQN_4pads/DQN_simple_4pa
 from __future__ import annotations
 
 import ctypes as C
-import os
 from collections import OrderedDict
 from typing import Optional
 
 import numpy as np
 
-from . import _lib, sb_io, training_state
+from . import _lib, training_state
+from .base_model import BaseModel
 from .callbacks import as_callback
 from .learner import HandleLearner, _f32, _fp
-from .vec_env import DummyVecEnv
 
 _ONLINE, _TARGET = "deepq/model/", "deepq/target_q_func/model/"
 
@@ -35,7 +34,8 @@ class DQNLearner(HandleLearner):
                           int(bool(prioritized_replay)), float(prioritized_replay_alpha), float(prioritized_replay_eps))
         self.prioritized_replay = bool(prioritized_replay)
         self._create(cfg)
-        self.obs_dim, self.n_actions, self.batch_size = obs_dim, n_actions, batch_size
+        self.obs_dim = self.obs_elems = obs_dim
+        self.n_actions, self.batch_size = n_actions, batch_size
 
     def _has_grad(self, name):
         return name.startswith(_ONLINE)
@@ -54,20 +54,6 @@ class DQNLearner(HandleLearner):
 
     def replay_size(self):
         return int(self.lib.b2g_dqn_replay_size(self.h))
-
-    def set_norm_stats(self, obs_mean=None, obs_var=None, ret_var=1.0, clip_obs=10.0, clip_reward=10.0, epsilon=1e-8, norm_obs=True,
-                       norm_reward=True):
-        """VecNormalize's statistics for the gather of the gradient steps (the replay holds raw transitions); act() takes
-        observations already normalised."""
-        dp = C.POINTER(C.c_double)
-        mp = vp = None
-        if norm_obs:
-            m = np.ascontiguousarray(obs_mean, np.float64).reshape(-1)
-            v = np.ascontiguousarray(obs_var, np.float64).reshape(-1)
-            assert m.size == self.obs_dim and v.size == self.obs_dim
-            mp, vp = m.ctypes.data_as(dp), v.ctypes.data_as(dp)
-        _lib.check(self.lib.b2g_dqn_set_norm_stats(self.h, mp, vp, float(ret_var), float(clip_obs), float(clip_reward), float(epsilon),
-                                                    int(bool(norm_obs)), int(bool(norm_reward))))
 
     def step(self, n_steps=1, lr=5e-4):
         m = _lib.DqnMetrics()
@@ -134,10 +120,11 @@ def _check_policy_kwargs(policy_kwargs):
     return kw, [int(x) for x in layers]
 
 
-class DQN:
+class DQN(BaseModel):
     """stable-baselines 2.10 ``DQN(policy, env, ...)`` with its signature and defaults, plus ``device`` and ``seed``:
     ``learn / predict / save / load / get_parameters / load_parameters / get_env / get_vec_normalize_env`` and
     ``save_training_state / load_training_state``.  One environment (stable-baselines' DQN refuses a VecEnv of more)."""
+    _algo = "DQN"
 
     def __init__(self, policy, env, gamma=0.99, learning_rate=5e-4, buffer_size=50000, exploration_fraction=0.1,
                  exploration_final_eps=0.02, exploration_initial_eps=1.0, train_freq=1, batch_size=32, double_q=True, learning_starts=1000,
@@ -169,20 +156,14 @@ class DQN:
         self._rng = np.random.default_rng(seed)            # epsilon-greedy draws of learn()
         self.predict_rng = np.random.default_rng(seed)     # softmax(Q) draws of predict(deterministic=False)
         self.learner: Optional[DQNLearner] = None
-        self.env = None
-        self._vec_normalize_env = None
         if env is not None:
             self._set_env(env)
             if _init_setup_model:
                 self.setup_model()
 
-    def _set_env(self, env):
-        env = env if hasattr(env, "num_envs") else DummyVecEnv([lambda: env])
-        if env.num_envs > 1:     # stable-baselines' own refusal (deepq/dqn.py: "...cannot be used with more than one env")
+    def _check_env(self):
+        if self.n_envs > 1:      # stable-baselines' own refusal (deepq/dqn.py: "...cannot be used with more than one env")
             raise ValueError("Error: DQN cannot be used with more than one environment (num_envs > 1)")
-        self.env = env
-        self.observation_space, self.action_space = env.observation_space, env.action_space
-        self._vec_normalize_env = self.get_vec_normalize_env()
 
     def setup_model(self):
         if not hasattr(self.action_space, "n"):
@@ -204,18 +185,6 @@ class DQN:
             else:
                 p[n] = np.zeros(shp, np.float32)
         self.learner.load_parameters(p)
-
-    def close(self):
-        if self.learner is not None:
-            self.learner.close()
-            self.learner = None
-
-    def get_env(self):
-        return self.env
-
-    def get_vec_normalize_env(self):
-        from .sac_model import unwrap_vec_normalize
-        return unwrap_vec_normalize(self.env)
 
     def _sync_norm_stats(self):
         vn = self._vec_normalize_env
@@ -293,50 +262,27 @@ class DQN:
         single = np.ndim(observation) == len(getattr(self.observation_space, "shape", (self.learner.obs_dim,)))
         return (int(idx[0]) if single else idx), None
 
-    def get_parameters(self):
-        return OrderedDict((n + ":0", a) for n, a in self.learner.get_parameters().items())
-
-    def load_parameters(self, load_path_or_dict, exact_match=True):
-        params = load_path_or_dict
-        if isinstance(params, str):
-            _, params = sb_io.load_sb_zip(params)
-        self.learner.load_parameters(params, exact_match=exact_match)
-
     def _data(self):
-        return {"double_q": True, "param_noise": False, "learning_starts": self.learning_starts, "train_freq": self.train_freq,
+        data = {"double_q": True, "param_noise": False, "learning_starts": self.learning_starts, "train_freq": self.train_freq,
                 "prioritized_replay": self.prioritized_replay, "prioritized_replay_eps": self.per_eps, "batch_size": self.batch_size,
                 "target_network_update_freq": self.target_network_update_freq, "prioritized_replay_alpha": self.per_alpha,
                 "prioritized_replay_beta0": self.per_beta0, "prioritized_replay_beta_iters": self.per_beta_iters,
                 "exploration_final_eps": self.exploration_final_eps, "exploration_fraction": self.exploration_fraction,
                 "exploration_initial_eps": self.exploration_initial_eps, "learning_rate": self.learning_rate, "gamma": self.gamma,
                 "verbose": self.verbose, "n_envs": 1, "seed": self.seed, "policy_kwargs": dict(self.policy_kwargs)}
-
-    def save(self, save_path, cloudpickle=False):
-        """A stable-baselines zip: ``data`` (hyper-parameters), ``parameter_list`` and ``parameters`` in the zip's order."""
-        d = os.path.dirname(save_path)
-        if d:
-            os.makedirs(d, exist_ok=True)
-        data = self._data()
-        if callable(data["learning_rate"]):
+        if callable(self.learning_rate):
             data["learning_rate"] = None
-        sb_io.save_sb_zip(save_path, data, self.learner.get_parameters())
+        return data
 
     @classmethod
     def load(cls, load_path, env=None, custom_objects=None, **kwargs):
         """Reads a stable-baselines DQN zip (the shipped DQN_simple_4pads.zip / best_model.zip unchanged): the number of actions
         and the widths come from the parameter shapes, the hyper-parameters from ``data``."""
         from .spaces import Box, Discrete
-        if not os.path.exists(load_path) and os.path.exists(load_path + ".zip"):
-            load_path += ".zip"
-        data, params = sb_io.load_sb_zip(load_path)
+        data, params = cls._read_zip(load_path)
         w0 = params[_ONLINE + "action_value/fully_connected/weights"]
         w1 = params[_ONLINE + "action_value/fully_connected_1/weights"]
         w2 = params[_ONLINE + "action_value/fully_connected_2/weights"]
-
-        class _Spaces:
-            num_envs = 1
-            observation_space = Box(-np.inf, np.inf, (w0.shape[0],))
-            action_space = Discrete(w2.shape[1])
         kw = {k: data[k] for k in ("gamma", "learning_rate", "batch_size", "learning_starts", "train_freq", "target_network_update_freq",
                                    "exploration_fraction", "exploration_final_eps", "prioritized_replay", "prioritized_replay_alpha",
                                    "prioritized_replay_beta0", "prioritized_replay_beta_iters", "prioritized_replay_eps", "seed")
@@ -344,13 +290,7 @@ class DQN:
         kw["policy_kwargs"] = dict(data.get("policy_kwargs") or {}, layers=[int(w0.shape[1]), int(w1.shape[1])])
         kw.update(kwargs)        # stable-baselines 2.10 does not save buffer_size: its default (50000) unless given here
         m = cls("MlpPolicy", None, _init_setup_model=False, **kw)
-        if env is not None:
-            m._set_env(env)
-        else:
-            m.observation_space, m.action_space = _Spaces.observation_space, _Spaces.action_space
-        m.setup_model()
-        m.learner.load_parameters(params, exact_match=True)
-        return m
+        return m._finish_load(env, Box(-np.inf, np.inf, (w0.shape[0],)), Discrete(w2.shape[1]), params)
 
     # ------------------------------------------------------------------ training state (training_state.py)
     def _host_state(self):
@@ -367,25 +307,8 @@ class DQN:
         return {"algo": "DQN", "init": init, "num_timesteps": int(self.num_timesteps), "n_target_updates": int(self.n_target_updates),
                 "rng": training_state.rng_state(self._rng), "predict_rng": training_state.rng_state(self.predict_rng)}
 
-    def save_training_state(self, path):
-        """Writes directory ``path``: model.zip, learner.state (parameters, Adam moments, counters, the replay and its priority
-        trees), vecnormalize.pkl and host.json."""
-        return training_state.save_training_state(self, path)
-
-    @classmethod
-    def load_training_state(cls, path, env, **kwargs):
-        """Rebuilds the model ``save_training_state`` wrote into ``path`` on ``env``; ``learn(n, reset_num_timesteps=False)``
-        then continues the run."""
-        path = training_state.resolve(path)
-        host = training_state.read_host(path)
-        if host.get("algo") != "DQN":
-            raise ValueError(f"{path} holds a {host.get('algo')} training state")
-        model = cls("MlpPolicy", env, **dict(host["init"], **kwargs))
-        training_state.restore_vec_normalize(path, model.env)
-        model.load_parameters(os.path.join(path, training_state.MODEL_FILE))
-        model.learner.load_state(os.path.join(path, training_state.STATE_FILE))
-        model.num_timesteps = int(host["num_timesteps"])
-        model.n_target_updates = int(host.get("n_target_updates", 0))
-        training_state.set_rng_state(model._rng, host["rng"])
-        training_state.set_rng_state(model.predict_rng, host["predict_rng"])
-        return model
+    def _restore_host_state(self, host):
+        self.num_timesteps = int(host["num_timesteps"])
+        self.n_target_updates = int(host.get("n_target_updates", 0))
+        training_state.set_rng_state(self._rng, host["rng"])
+        training_state.set_rng_state(self.predict_rng, host["predict_rng"])

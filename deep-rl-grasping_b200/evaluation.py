@@ -16,7 +16,7 @@ def evaluate_policy(model, env, n_eval_episodes=10, deterministic=True, render=F
     # predict and normalises them on the device; an evaluation wrapper that normalises on the host hands over its raw copy.
     host_vn = None
     if getattr(model, "predict_takes_raw_obs", False):
-        from .sac_model import unwrap_vec_normalize
+        from .base_model import unwrap_vec_normalize
         host_vn = unwrap_vec_normalize(env)
         if host_vn is not None and (not host_vn.norm_obs or getattr(host_vn, "learner_owns_obs_rms", False)):
             host_vn = None

@@ -1,14 +1,15 @@
-"""Thin numpy-facing wrapper of one ``b2g_sac`` handle (the device-resident learner).
+"""Thin numpy-facing wrappers of the device-resident learners' handles.
 
-``Learner`` is what ``SAC`` (sac.py, the stable-baselines-shaped front end) drives; tests and
-bench.py also use it directly because it maps 1:1 onto the C ABI entry points.
+``HandleLearner`` is what the wrappers of the ``b2g_sac``, ``b2g_bdq``, ``b2g_dqn`` and ``b2g_ppo`` handles share.
+``Learner`` wraps one ``b2g_sac`` handle and is what ``SAC`` (sac_model.py, the stable-baselines-shaped front end) drives;
+tests and bench.py also use it directly because it maps 1:1 onto the C ABI entry points.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
 from collections import OrderedDict
-from typing import Dict, Optional, Sequence
+from typing import Optional, Sequence
 
 import numpy as np
 
@@ -24,17 +25,35 @@ def _f32(a) -> np.ndarray:
     return a if a.flags.c_contiguous else a.copy()
 
 
+def nccl_config(nranks: int, nccl_id: Optional[bytes]):
+    """(id buffer, id pointer, NCCL library path) for a handle's configuration; all None with one rank.  The buffer must
+    outlive the create call that reads the pointer."""
+    if nranks <= 1:
+        return None, None, None
+    if nccl_id is None or len(nccl_id) != 128:
+        raise ValueError("nranks > 1 needs the 128-byte nccl_id shared by all ranks")
+    buf = C.create_string_buffer(bytes(nccl_id), 128)
+    lib_path = _lib.default_nccl_lib()
+    return buf, C.cast(buf, C.c_void_p), lib_path.encode() if lib_path else None
+
+
 class HandleLearner:
-    """What the numpy-facing wrappers of the ``b2g_bdq``, ``b2g_dqn`` and ``b2g_ppo`` handles share: the handle's lifetime,
-    its named parameters (``b2g_<abi>_param_*``, ``_get_param``, ``_set_param``, ``_get_grad``) and its training-state
-    files.  A subclass sets ``_abi`` and ``_has_grad`` and calls ``_create`` with its configuration."""
+    """What the numpy-facing wrappers of the learner handles share: the handle's lifetime, its named parameters
+    (``param_*``, ``get_param``, ``set_param``, ``get_grad``), its training-state files and, for the learners that take
+    VecNormalize's statistics, ``set_norm_stats``, the device ``obs_rms`` and the upload counters.  A subclass sets
+    ``_abi`` and ``_has_grad`` and calls ``_create`` with its configuration, or fills ``_info`` itself.  Entry point
+    ``name`` is ``b2g_<abi>_<name>`` unless ``_names`` maps it to another symbol."""
     _abi = ""
+    _names = {}
+
+    #: bumped by every call that may change the device statistics (DeviceRunningMeanStd caches against it)
+    obs_rms_version = 0
 
     def _has_grad(self, name: str) -> bool:
         raise NotImplementedError
 
     def _fn(self, name: str):
-        return getattr(self.lib, f"b2g_{self._abi}_{name}")
+        return getattr(self.lib, self._names.get(name) or f"b2g_{self._abi}_{name}")
 
     def _create(self, cfg):
         self.h = C.c_void_p()
@@ -97,15 +116,63 @@ class HandleLearner:
 
     def save_state(self, path: str):
         """Parameters, Adam moments, counters and, for the replay learners, the live replay rows and the prioritised-replay
-        trees -> ``path``."""
+        trees -> ``path`` (waits for enqueued steps)."""
         _lib.check(self._fn("state_save")(self.h, os.fsencode(path)))
 
     def load_state(self, path: str):
-        """Restores a ``save_state`` file into this learner, which must have the same configuration."""
+        """Restores a ``save_state`` file into this learner, which must have the same configuration (SAC's precision aside)
+        and own a device ``obs_rms`` exactly when the file carries one.  Other normalisation statistics are not part of the
+        file: set them again with ``set_norm_stats``."""
         _lib.check(self._fn("state_load")(self.h, os.fsencode(path)))
+        self.obs_rms_version += 1
+
+    # ---- VecNormalize's statistics (``obs_elems`` floats per observation)
+    def set_norm_stats(self, obs_mean=None, obs_var=None, ret_var=1.0, clip_obs=10.0, clip_reward=10.0, epsilon=1e-8,
+                       norm_obs=True, norm_reward=True):
+        """The statistics of the gradient step's gather (and of act() where the learner normalises).  ``obs_mean = obs_var
+        = None`` with ``norm_obs``: a learner that owns ``obs_rms`` keeps its device statistics and takes the scalars only."""
+        dp = C.POINTER(C.c_double)
+        mp = vp = None
+        if norm_obs and obs_mean is not None:
+            m = np.ascontiguousarray(obs_mean, np.float64).reshape(-1)
+            v = np.ascontiguousarray(obs_var, np.float64).reshape(-1)
+            assert m.size == self.obs_elems and v.size == self.obs_elems
+            mp, vp = m.ctypes.data_as(dp), v.ctypes.data_as(dp)
+        _lib.check(self._fn("set_norm_stats")(self.h, mp, vp, float(ret_var), float(clip_obs), float(clip_reward), float(epsilon),
+                                               int(bool(norm_obs)), int(bool(norm_reward))))
+        if mp is not None:
+            self.obs_rms_version += 1
+
+    def obs_rms_set(self, mean, var, count):
+        """Creates (first call) or overwrites the device ``obs_rms``: float64 mean / var of the observation + count."""
+        dp = C.POINTER(C.c_double)
+        m = np.ascontiguousarray(mean, np.float64).reshape(-1)
+        v = np.ascontiguousarray(var, np.float64).reshape(-1)
+        assert m.size == self.obs_elems and v.size == self.obs_elems
+        _lib.check(self._fn("obs_rms_set")(self.h, m.ctypes.data_as(dp), v.ctypes.data_as(dp), float(count)))
+        self.obs_rms_version += 1
+
+    def obs_rms_get(self):
+        """(mean, var, count) of the device ``obs_rms`` in ``obs_shape``; waits for the work enqueued on the handle."""
+        dp = C.POINTER(C.c_double)
+        m, v = np.empty(self.obs_shape, np.float64), np.empty(self.obs_shape, np.float64)
+        cnt = C.c_double()
+        _lib.check(self._fn("obs_rms_get")(self.h, m.ctypes.data_as(dp), v.ctypes.data_as(dp), C.byref(cnt)))
+        return m, v, float(cnt.value)
+
+    def upload_bytes(self) -> dict:
+        """Bytes copied host -> device so far: by ``observe_*`` / ``obs_rms_set``, and by ``act`` + ``replay_add`` +
+        ``set_norm_stats``."""
+        a, b = C.c_int64(), C.c_int64()
+        _lib.check(self._fn("upload_bytes")(self.h, C.byref(a), C.byref(b)))
+        return {"observe": int(a.value), "other": int(b.value)}
 
 
-class Learner:
+class Learner(HandleLearner):
+    _abi = "sac"
+    _names = {n: "b2g_" + n for n in ("get_param", "set_param", "get_grad", "set_norm_stats", "obs_rms_set", "obs_rms_get",
+                                      "upload_bytes")}
+
     def __init__(self, obs_shape: Sequence[int], n_act: int = 5, hidden: int = 64, batch_size: int = 64,
                  buffer_size: int = 100000, gamma: float = 0.99, tau: float = 0.005,
                  target_entropy: Optional[float] = None, seed: int = 0, precision: int = _lib.B2G_PREC_FP32_SIMT,
@@ -130,14 +197,7 @@ class Learner:
         cfg.gamma, cfg.tau = gamma, tau
         cfg.target_entropy = float(-n_act if target_entropy is None else target_entropy)
         cfg.seed, cfg.precision, cfg.device, cfg.rank, cfg.nranks = seed, precision, device, rank, nranks
-        self._id_buf = None
-        if nranks > 1:
-            if nccl_id is None or len(nccl_id) != 128:
-                raise ValueError("nranks > 1 needs the 128-byte nccl_id shared by all ranks")
-            self._id_buf = C.create_string_buffer(bytes(nccl_id), 128)
-            cfg.nccl_id = C.cast(self._id_buf, C.c_void_p)
-            lib_path = _lib.default_nccl_lib()
-            cfg.nccl_lib = lib_path.encode() if lib_path else None
+        self._id_buf, cfg.nccl_id, cfg.nccl_lib = nccl_config(nranks, nccl_id)
         self.h = C.c_void_p()
         self.frame_capacity = None if frame_capacity is None else int(frame_capacity)
         self.u8_planes = tuple(int(c) for c in u8_planes)
@@ -155,18 +215,6 @@ class Learner:
         for i in range(self.lib.b2g_param_count(self.h)):
             _lib.check(self.lib.b2g_param_info(self.h, i, C.byref(name), C.byref(numel), C.byref(ndim), shape))
             self._info[name.value.decode()] = tuple(int(shape[k]) for k in range(ndim.value))
-
-    # ---- lifetime
-    def close(self):
-        if getattr(self, "h", None) is not None and self.h:
-            self.lib.b2g_sac_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     # ---- peer-memory data parallelism (include/b200grasp.h: b2g_sac_dp_export / b2g_sac_dp_connect)
     DP_EXPORT_BYTES = 192
@@ -201,44 +249,8 @@ class Learner:
         _lib.check(lib.b2g_nccl_unique_id(C.cast(buf, C.c_void_p), p.encode() if p else None))
         return buf.raw
 
-    # ---- parameters (SB zip names / layouts)
-    @property
-    def param_shapes(self) -> "OrderedDict[str, tuple]":
-        return self._info
-
-    def get_parameters(self) -> "OrderedDict[str, np.ndarray]":
-        out = OrderedDict()
-        for n, shp in self._info.items():
-            a = np.empty(shp, np.float32)
-            _lib.check(self.lib.b2g_get_param(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
-            out[n] = a
-        return out
-
-    def load_parameters(self, params: Dict[str, np.ndarray], exact_match: bool = True):
-        seen = set()
-        for n, a in params.items():
-            key = n[:-2] if n.endswith(":0") else n
-            if key not in self._info:
-                if exact_match:
-                    raise ValueError(f"unknown variable {n}")
-                continue
-            a = _f32(a)
-            if tuple(a.shape) != self._info[key]:
-                raise ValueError(f"shape mismatch for {n}: {a.shape} vs {self._info[key]}")
-            _lib.check(self.lib.b2g_set_param(self.h, key.encode(), _fp(a.reshape(-1)), a.size))
-            seen.add(key)
-        if exact_match and seen != set(self._info):
-            raise ValueError(f"missing variables: {sorted(set(self._info) - seen)[:4]}...")
-
-    def get_gradients(self) -> "OrderedDict[str, np.ndarray]":
-        out = OrderedDict()
-        for n, shp in self._info.items():
-            if n.startswith("target/"):
-                continue
-            a = np.empty(shp, np.float32)
-            _lib.check(self.lib.b2g_get_grad(self.h, n.encode(), _fp(a.reshape(-1)), a.size))
-            out[n] = a
-        return out
+    def _has_grad(self, name):
+        return not name.startswith("target/")
 
     def get_adam(self, name: str):
         shp = self._info[name]
@@ -249,7 +261,7 @@ class Learner:
     def reset_optimizer(self):
         _lib.check(self.lib.b2g_reset_optimizer(self.h))
 
-    # ---- replay + normalisation
+    # ---- replay
     def replay_add(self, obs, act, rew, next_obs, done):
         obs, next_obs, act = _f32(obs), _f32(next_obs), _f32(act)
         rew, done = _f32(np.reshape(rew, -1)), _f32(np.reshape(done, -1))
@@ -286,40 +298,7 @@ class Learner:
             out[k] = ps[i].copy()
         return out
 
-    def set_norm_stats(self, obs_mean=None, obs_var=None, ret_var=1.0, clip_obs=10.0, clip_reward=10.0, epsilon=1e-8,
-                       norm_obs=True, norm_reward=True):
-        dp = C.POINTER(C.c_double)
-        if norm_obs and obs_mean is not None:      # None: a learner that owns obs_rms keeps its device statistics
-            m = np.ascontiguousarray(obs_mean, np.float64).reshape(-1)
-            v = np.ascontiguousarray(obs_var, np.float64).reshape(-1)
-            assert m.size == self.obs_elems and v.size == self.obs_elems
-            mp, vp = m.ctypes.data_as(dp), v.ctypes.data_as(dp)
-        else:
-            mp = vp = None
-        _lib.check(self.lib.b2g_set_norm_stats(self.h, mp, vp, float(ret_var), float(clip_obs), float(clip_reward),
-                                                float(epsilon), int(bool(norm_obs)), int(bool(norm_reward))))
-
-    # ---- device-resident obs_rms and the actor loop on one upload per frame (include/b200grasp.h: b2g_sac_observe_*)
-    #: bumped by every call that may change the device statistics (DeviceRunningMeanStd caches against it)
-    obs_rms_version = 0
-
-    def obs_rms_set(self, mean, var, count):
-        """Creates (first call) or overwrites the device ``obs_rms``: float64 mean / var of the observation shape + count."""
-        dp = C.POINTER(C.c_double)
-        m = np.ascontiguousarray(mean, np.float64).reshape(-1)
-        v = np.ascontiguousarray(var, np.float64).reshape(-1)
-        assert m.size == self.obs_elems and v.size == self.obs_elems
-        _lib.check(self.lib.b2g_obs_rms_set(self.h, m.ctypes.data_as(dp), v.ctypes.data_as(dp), float(count)))
-        self.obs_rms_version += 1
-
-    def obs_rms_get(self):
-        """(mean, var, count) of the device ``obs_rms``; waits for the work enqueued on the handle."""
-        dp = C.POINTER(C.c_double)
-        m, v = np.empty(self.obs_shape, np.float64), np.empty(self.obs_shape, np.float64)
-        cnt = C.c_double()
-        _lib.check(self.lib.b2g_obs_rms_get(self.h, m.ctypes.data_as(dp), v.ctypes.data_as(dp), C.byref(cnt)))
-        return m, v, float(cnt.value)
-
+    # ---- the actor loop on one upload per frame (include/b200grasp.h: b2g_sac_observe_*)
     def observe_act(self, obs, n=None, update_stats=True, deterministic=False, act=True):
         """``obs``: n raw observations to upload, merge into ``obs_rms`` (``update_stats``) and stage as the current
         observation of env i; ``None`` acts on the ones already staged.  Returns the n actions, or None with ``act=False``."""
@@ -345,25 +324,6 @@ class Learner:
         _lib.check(self.lib.b2g_sac_observe_add(self.h, _fp(act), _fp(rew), _fp(next_obs), _fp(done),
                                                 None if reset_obs is None else _fp(reset_obs), n, int(bool(update_stats))))
         self.obs_rms_version += bool(update_stats)
-
-    def upload_bytes(self) -> dict:
-        """Bytes copied host -> device so far: by ``observe_*`` / ``obs_rms_set``, and by ``act`` + ``replay_add`` +
-        ``set_norm_stats``."""
-        a, b = C.c_int64(), C.c_int64()
-        _lib.check(self.lib.b2g_upload_bytes(self.h, C.byref(a), C.byref(b)))
-        return {"observe": int(a.value), "other": int(b.value)}
-
-    # ---- training state (include/b200grasp.h: b2g_sac_state_save / _load)
-    def save_state(self, path: str):
-        """Writes parameters, Adam moments, counters and the whole replay to ``path`` (waits for enqueued steps)."""
-        _lib.check(self.lib.b2g_sac_state_save(self.h, os.fsencode(path)))
-
-    def load_state(self, path: str):
-        """Restores a ``save_state`` file into this learner, which must have the same configuration (precision aside).
-        Normalisation statistics are not part of the file (set them again with ``set_norm_stats``), except the device
-        ``obs_rms`` of a learner that owns one."""
-        _lib.check(self.lib.b2g_sac_state_load(self.h, os.fsencode(path)))
-        self.obs_rms_version += 1
 
     # ---- hot path
     def step(self, n_steps: int = 1, lr: float = 3e-4) -> dict:

@@ -6,16 +6,15 @@ Import it as ``b200grasp.ppo2.PPO2`` (the stable-baselines path ``stable_baselin
 from __future__ import annotations
 
 import ctypes as C
-import os
 from collections import OrderedDict
 from typing import Optional
 
 import numpy as np
 
-from . import _lib, sb_io, training_state
+from . import _lib
+from .base_model import BaseModel
 from .callbacks import as_callback
 from .learner import HandleLearner, _f32, _fp
-from .vec_env import DummyVecEnv
 
 _SCOPE = "model/"
 
@@ -138,10 +137,11 @@ def _check_policy_kwargs(policy_kwargs):
     return kw, layers
 
 
-class PPO2:
+class PPO2(BaseModel):
     """stable-baselines 2.10 ``PPO2(policy, env, ...)`` with its signature and defaults, plus ``device``: ``learn / predict /
     save / load / get_parameters / load_parameters / get_env / get_vec_normalize_env / close`` and
     ``save_training_state / load_training_state``.  Box action spaces only, as the reference's configs give."""
+    _algo = "PPO2"
 
     def __init__(self, policy, env, gamma=0.99, n_steps=128, ent_coef=0.01, learning_rate=2.5e-4, vf_coef=0.5, max_grad_norm=0.5,
                  lam=0.95, nminibatches=4, noptepochs=4, cliprange=0.2, cliprange_vf=None, verbose=0, tensorboard_log=None,
@@ -160,8 +160,6 @@ class PPO2:
         self.num_timesteps = 0
         self.n_envs = 1
         self.learner: Optional[PPO2Learner] = None
-        self.env = None
-        self._vec_normalize_env = None
         self._boundary = None           # (num_timesteps, numpy global state) after the last completed update
         self.ep_info_buf = []
         if env is not None:
@@ -169,13 +167,9 @@ class PPO2:
             if _init_setup_model:
                 self.setup_model()
 
-    def _set_env(self, env):
-        env = env if hasattr(env, "num_envs") else DummyVecEnv([lambda: env])
-        if not hasattr(env.action_space, "low"):
-            raise NotImplementedError(f"PPO2 here needs a Box action space, got {env.action_space} (the reference's PPO branch is continuous)")
-        self.env, self.n_envs = env, int(env.num_envs)
-        self.observation_space, self.action_space = env.observation_space, env.action_space
-        self._vec_normalize_env = self.get_vec_normalize_env()
+    def _check_env(self):
+        if not hasattr(self.action_space, "low"):
+            raise NotImplementedError(f"PPO2 here needs a Box action space, got {self.action_space} (the reference's PPO branch is continuous)")
         if (self.n_envs * self.n_steps) % self.nminibatches:
             # ppo2.py's assertion: "The number of minibatches (nminibatches) is not a factor of the total number of samples"
             raise ValueError(f"nminibatches={self.nminibatches} is not a factor of n_batch = n_envs * n_steps = {self.n_envs * self.n_steps}")
@@ -186,18 +180,6 @@ class PPO2:
         self.learner = PPO2Learner(obs_dim, A, tuple(self.layers), self.n_envs, self.n_steps, self.nminibatches, self.noptepochs,
                                    self.gamma, self.lam, self.ent_coef, self.vf_coef, self.max_grad_norm, int(self.seed or 0), self.device)
         self.learner.load_parameters(_init_params(obs_dim, A, self.layers, self.seed))
-
-    def close(self):
-        if self.learner is not None:
-            self.learner.close()
-            self.learner = None
-
-    def get_env(self):
-        return self.env
-
-    def get_vec_normalize_env(self):
-        from .sac_model import unwrap_vec_normalize
-        return unwrap_vec_normalize(self.env)
 
     def learn(self, total_timesteps, callback=None, log_interval=1, tb_log_name="PPO2", reset_num_timesteps=True):
         """stable-baselines 2.10 PPO2.learn: n_updates = total_timesteps // n_batch rollouts of n_steps steps (clipped actions to
@@ -265,17 +247,8 @@ class PPO2:
         a = a.reshape((-1,) + tuple(self.action_space.shape))
         return (a[0] if single else a), None
 
-    def get_parameters(self):
-        return OrderedDict((n + ":0", a) for n, a in self.learner.get_parameters().items())
-
-    def load_parameters(self, load_path_or_dict, exact_match=True):
-        params = load_path_or_dict
-        if isinstance(params, str):
-            _, params = sb_io.load_sb_zip(params)
-        self.learner.load_parameters(params, exact_match=exact_match)
-
     def _data(self):
-        return {"gamma": self.gamma, "n_steps": self.n_steps, "vf_coef": self.vf_coef, "ent_coef": self.ent_coef,
+        data = {"gamma": self.gamma, "n_steps": self.n_steps, "vf_coef": self.vf_coef, "ent_coef": self.ent_coef,
                 "max_grad_norm": self.max_grad_norm, "learning_rate": self.learning_rate, "lam": self.lam,
                 "nminibatches": self.nminibatches, "noptepochs": self.noptepochs, "cliprange": self.cliprange,
                 "cliprange_vf": self.cliprange_vf, "verbose": self.verbose, "n_envs": self.n_envs, "seed": self.seed,
@@ -283,25 +256,16 @@ class PPO2:
                 "observation_shape": list(self.observation_space.shape), "action_shape": list(self.action_space.shape),
                 "action_low": np.asarray(self.action_space.low).reshape(-1).tolist(),
                 "action_high": np.asarray(self.action_space.high).reshape(-1).tolist()}
-
-    def save(self, save_path, cloudpickle=False):
-        """A stable-baselines zip: ``data`` (hyper-parameters, JSON), ``parameter_list`` and ``parameters``."""
-        d = os.path.dirname(save_path)
-        if d:
-            os.makedirs(d, exist_ok=True)
-        data = self._data()
         for k in ("learning_rate", "cliprange", "cliprange_vf"):
             if callable(data[k]):
                 data[k] = None
-        sb_io.save_sb_zip(save_path, data, self.learner.get_parameters())
+        return data
 
     @classmethod
     def load(cls, load_path, env=None, custom_objects=None, **kwargs):
         """Reads a PPO2 zip: widths and sizes from the parameter shapes, hyper-parameters from ``data``."""
         from .spaces import Box
-        if not os.path.exists(load_path) and os.path.exists(load_path + ".zip"):
-            load_path += ".zip"
-        data, params = sb_io.load_sb_zip(load_path)
+        data, params = cls._read_zip(load_path)
         w0, w1, wpi = params[_SCOPE + "pi_fc0/w"], params[_SCOPE + "pi_fc1/w"], params[_SCOPE + "pi/w"]
         kw = {k: data[k] for k in ("gamma", "n_steps", "vf_coef", "ent_coef", "max_grad_norm", "learning_rate", "lam", "nminibatches",
                                    "noptepochs", "cliprange", "cliprange_vf", "seed") if k in data and data[k] is not None}
@@ -310,19 +274,13 @@ class PPO2:
         kw["policy_kwargs"] = dict(data.get("policy_kwargs") or {}, layers=[int(w0.shape[1]), int(w1.shape[1])])
         kw.update(kwargs)
         m = cls("MlpPolicy", None, _init_setup_model=False, **kw)
-        if env is not None:
-            m._set_env(env)
-        else:
-            A = int(wpi.shape[1])
-            m.observation_space = Box(-np.inf, np.inf, tuple(data.get("observation_shape") or (w0.shape[0],)))
-            m.action_space = Box(np.asarray(data.get("action_low", [-1.0] * A), np.float32), np.asarray(data.get("action_high", [1.0] * A), np.float32),
-                                 tuple(data.get("action_shape") or (A,)))
-            m.n_envs = 1
-            if (m.n_envs * m.n_steps) % m.nminibatches:
-                raise ValueError(f"nminibatches={m.nminibatches} is not a factor of n_batch = {m.n_steps}")
-        m.setup_model()
-        m.learner.load_parameters(params, exact_match=True)
-        return m
+        if env is None and m.n_steps % m.nminibatches:
+            raise ValueError(f"nminibatches={m.nminibatches} is not a factor of n_batch = {m.n_steps}")
+        A = int(wpi.shape[1])
+        return m._finish_load(env, Box(-np.inf, np.inf, tuple(data.get("observation_shape") or (w0.shape[0],))),
+                              Box(np.asarray(data.get("action_low", [-1.0] * A), np.float32),
+                                  np.asarray(data.get("action_high", [1.0] * A), np.float32), tuple(data.get("action_shape") or (A,))),
+                              params)
 
     # ------------------------------------------------------------------ training state (training_state.py)
     def _host_state(self):
@@ -337,28 +295,11 @@ class PPO2:
         return {"algo": "PPO2", "init": init, "num_timesteps": int(num),
                 "np_random": [np_state[0], np.asarray(np_state[1]).tolist(), int(np_state[2]), int(np_state[3]), float(np_state[4])]}
 
-    def save_training_state(self, path):
-        """Writes directory ``path``: model.zip, learner.state (parameters, Adam moments, counters), vecnormalize.pkl and
-        host.json (num_timesteps and numpy's global generator at the last update boundary: a rollout in flight is not kept)."""
-        return training_state.save_training_state(self, path)
-
-    @classmethod
-    def load_training_state(cls, path, env, **kwargs):
-        """Rebuilds the model ``save_training_state`` wrote into ``path`` on ``env``; ``learn(n, reset_num_timesteps=False)``
-        then continues from the saved update boundary with a fresh episode."""
-        path = training_state.resolve(path)
-        host = training_state.read_host(path)
-        if host.get("algo") != "PPO2":
-            raise ValueError(f"{path} holds a {host.get('algo')} training state")
-        model = cls("MlpPolicy", env, **dict(host["init"], **kwargs))
-        training_state.restore_vec_normalize(path, model.env)
-        model.load_parameters(os.path.join(path, training_state.MODEL_FILE))
-        model.learner.load_state(os.path.join(path, training_state.STATE_FILE))
-        model.num_timesteps = int(host["num_timesteps"])
+    def _restore_host_state(self, host):
+        self.num_timesteps = int(host["num_timesteps"])
         s = host["np_random"]
         np.random.set_state((s[0], np.asarray(s[1], np.uint32), s[2], s[3], s[4]))
-        model._boundary = (model.num_timesteps, np.random.get_state())
-        return model
+        self._boundary = (self.num_timesteps, np.random.get_state())
 
 
 def _init_params(obs_dim, n_actions, layers, seed):

@@ -10,17 +10,16 @@ run on the GPU behind the C ABI (include/b200grasp.h).  There is no CPU fallback
 """
 from __future__ import annotations
 
-import os
 import time
 from collections import OrderedDict, deque
 from typing import Optional
 
 import numpy as np
 
-from . import _lib, sb_io, training_state
+from . import _lib, training_state
+from .base_model import BaseModel, unwrap_vec_normalize  # noqa: F401  (unwrap_vec_normalize: also imported from here)
 from .callbacks import as_callback
 from .learner import Learner
-from .vec_env import DummyVecEnv, VecNormalize
 
 
 class CnnPolicy:      # sentinels standing in for stable_baselines.sac.policies.{CnnPolicy,MlpPolicy}
@@ -47,20 +46,9 @@ def _constfn(v):
     return v if callable(v) else (lambda _frac: float(v))
 
 
-def _is_vec(env):
-    return hasattr(env, "num_envs")
+class SAC(BaseModel):
+    _algo = "SAC"
 
-
-def unwrap_vec_normalize(env) -> Optional[VecNormalize]:
-    e = env
-    while e is not None:
-        if isinstance(e, VecNormalize) or type(e).__name__ == "VecNormalize":
-            return e
-        e = getattr(e, "venv", None)
-    return None
-
-
-class SAC:
     def __init__(self, policy, env, gamma=0.99, learning_rate=3e-4, buffer_size=50000, learning_starts=100, train_freq=1,
                  batch_size=64, tau=0.005, ent_coef="auto", target_update_interval=1, gradient_steps=1,
                  target_entropy="auto", action_noise=None, random_exploration=0.0, verbose=0, tensorboard_log=None,
@@ -103,8 +91,6 @@ class SAC:
         self.episode_rewards = [0.0]
         self.ep_info_buf = deque(maxlen=100)
         self.learner: Optional[Learner] = None
-        self.env = None
-        self._vec_normalize_env = None
         self._rng = np.random.default_rng(seed)
         if env is not None:
             self.set_env(env)
@@ -113,21 +99,10 @@ class SAC:
 
     # ------------------------------------------------------------------ env plumbing
     def set_env(self, env):
-        if not _is_vec(env):
-            env = DummyVecEnv([lambda: env])
-        self.env = env
-        self.n_envs = env.num_envs
-        self.observation_space, self.action_space = env.observation_space, env.action_space
-        self._vec_normalize_env = unwrap_vec_normalize(env)
+        self._set_env(env)
         if self.learner is not None:
             self._attach_device_norm()
             self._sync_norm_stats()
-
-    def get_env(self):
-        return self.env
-
-    def get_vec_normalize_env(self):
-        return self._vec_normalize_env
 
     def setup_model(self):
         obs_shape = tuple(self.observation_space.shape)
@@ -167,32 +142,6 @@ class SAC:
             else:
                 p[name] = np.zeros(shape, np.float32)
         self.learner.load_parameters(p)
-
-    def close(self):
-        """Releases the device learner (replay included: Learner.replay_info()["bytes"] of HBM).  Observation statistics this
-        learner owned go back to the VecNormalize wrapper first."""
-        if self.learner is not None:
-            if self._owns_obs_rms():
-                self._vec_normalize_env.take_obs_rms_back()
-            self.learner.close()
-            self.learner = None
-
-    def _owns_obs_rms(self) -> bool:
-        vn = self._vec_normalize_env
-        return vn is not None and getattr(vn, "obs_rms_owner", None) is self.learner and self.learner is not None
-
-    @property
-    def predict_takes_raw_obs(self) -> bool:
-        """True while a learner owns the statistics of this model's VecNormalize: that wrapper returns raw observations and
-        ``predict`` normalises them on the device (``evaluate_policy`` feeds an evaluation wrapper's raw copy accordingly)."""
-        return bool(getattr(self._vec_normalize_env, "learner_owns_obs_rms", False))
-
-    def _attach_device_norm(self):
-        """device_obs_norm: the wrapper's obs_rms moves to this learner, unless another learner owns it already (a second
-        model built on the same env, e.g. a parameter donor: it reads the owner's statistics and leaves them where they are)."""
-        vn = self._vec_normalize_env
-        if self.device_obs_norm and isinstance(vn, VecNormalize) and vn.norm_obs and not vn.learner_owns_obs_rms:
-            vn.give_obs_rms_to(self.learner)
 
     def _sync_norm_stats(self):
         vn = self._vec_normalize_env
@@ -321,16 +270,7 @@ class SAC:
         act = self._unscale_action(act.reshape((-1,) + tuple(self.action_space.shape)))
         return (act[0] if single else act), None
 
-    # ------------------------------------------------------------------ parameters / persistence
-    def get_parameters(self):
-        return OrderedDict((n + ":0", a) for n, a in self.learner.get_parameters().items())
-
-    def load_parameters(self, load_path_or_dict, exact_match=True):
-        params = load_path_or_dict
-        if isinstance(params, str):
-            _, params = sb_io.load_sb_zip(params)
-        self.learner.load_parameters(params, exact_match=exact_match)
-
+    # ------------------------------------------------------------------ persistence
     def _data(self):
         return {
             "gamma": self.gamma, "learning_rate": self.learning_rate if not callable(self.learning_rate) else float(self.learning_rate(1.0)),
@@ -348,12 +288,6 @@ class SAC:
             "b200grasp": {"precision": self.precision, "n_updates": self.n_updates, "replay_frames": self.replay_frames,
                           "replay_u8_planes": list(self.replay_u8_planes), "device_obs_norm": self.device_obs_norm},
         }
-
-    def save(self, save_path, cloudpickle=False):
-        d = os.path.dirname(save_path)
-        if d:
-            os.makedirs(d, exist_ok=True)
-        sb_io.save_sb_zip(save_path, self._data(), self.learner.get_parameters())
 
     # ------------------------------------------------------------------ training state (training_state.py)
     def _host_state(self):
@@ -375,55 +309,27 @@ class SAC:
                 "episode_rewards": [float(r) for r in self.episode_rewards], "ep_info_buf": list(self.ep_info_buf),
                 "rng": training_state.rng_state(self._rng)}
 
-    def save_training_state(self, path):
-        """Writes directory ``path``: model.zip, learner.state (parameters, Adam moments, counters, the whole replay),
-        vecnormalize.pkl and host.json.  The previous contents stay loadable until the new directory is complete."""
-        return training_state.save_training_state(self, path)
-
     @classmethod
-    def load_training_state(cls, path, env, **kwargs):
-        """Rebuilds the model ``save_training_state`` wrote into ``path`` on ``env`` and restores the saved VecNormalize
-        statistics into ``env``'s wrapper.  ``learn(n, reset_num_timesteps=False)`` then continues the run."""
-        path = training_state.resolve(path)
-        host = training_state.read_host(path)
-        if host.get("algo") != "SAC":
-            raise ValueError(f"{path} holds a {host.get('algo')} training state")
-        init = dict(host["init"], **kwargs)
-        model = cls({"CnnPolicy": CnnPolicy, "MlpPolicy": MlpPolicy}[host["policy"]], env, **init)
-        training_state.restore_vec_normalize(path, model.env)
-        model._attach_device_norm()        # the restored statistics go back to the learner; learner.state carries the same ones
-        model.load_parameters(os.path.join(path, training_state.MODEL_FILE))
-        model.learner.load_state(os.path.join(path, training_state.STATE_FILE))
-        model._sync_norm_stats()
-        model.num_timesteps, model.n_updates = int(host["num_timesteps"]), int(host["n_updates"])
-        model.episode_rewards = [float(r) for r in host["episode_rewards"]]
-        model.ep_info_buf = deque(host["ep_info_buf"], maxlen=100)
-        training_state.set_rng_state(model._rng, host["rng"])
-        return model
+    def _policy_from_host(cls, host):
+        return {"CnnPolicy": CnnPolicy, "MlpPolicy": MlpPolicy}[host["policy"]]
+
+    def _restore_host_state(self, host):
+        self._sync_norm_stats()
+        self.num_timesteps, self.n_updates = int(host["num_timesteps"]), int(host["n_updates"])
+        self.episode_rewards = [float(r) for r in host["episode_rewards"]]
+        self.ep_info_buf = deque(host["ep_info_buf"], maxlen=100)
+        training_state.set_rng_state(self._rng, host["rng"])
 
     @classmethod
     def load(cls, load_path, env=None, custom_objects=None, **kwargs):
         """Reads zips written by this class or by stable-baselines 2.10 (e.g.
         trained_models/SAC_depth_1mbuffer/best_model/best_model.zip)."""
         from .spaces import Box
-        if not os.path.exists(load_path) and os.path.exists(load_path + ".zip"):
-            load_path += ".zip"
-        data, params = sb_io.load_sb_zip(load_path)
-        if env is None:
-            if "model/pi/cnn1/w" in params:
-                c = params["model/pi/cnn1/w"].shape[2] + 1
-                obs_space = Box(0.0, 255.0, (64, 64, c))
-            else:
-                obs_space = Box(-np.inf, np.inf, (params["model/pi/fc0/kernel"].shape[0],))
-            n_act = params["model/pi/dense/kernel"].shape[1]
-
-            class _Spaces:
-                num_envs = 1
-                observation_space = obs_space
-                action_space = Box(-1.0, 1.0, (n_act,))
-            env_like = _Spaces()
+        data, params = cls._read_zip(load_path)
+        if "model/pi/cnn1/w" in params:
+            obs_space = Box(0.0, 255.0, (64, 64, params["model/pi/cnn1/w"].shape[2] + 1))
         else:
-            env_like = env if _is_vec(env) else DummyVecEnv([lambda: env])
+            obs_space = Box(-np.inf, np.inf, (params["model/pi/fc0/kernel"].shape[0],))
         kw = {}
         for k in ("gamma", "buffer_size", "learning_starts", "train_freq", "batch_size", "tau"):
             if isinstance(data.get(k), (int, float)):
@@ -445,10 +351,4 @@ class SAC:
         model = cls(policy=data.get("policy", "CnnPolicy"), env=None, _init_setup_model=False,
                     policy_kwargs={"layers": layers}, **kw)
         model._layout_from_zip = True
-        model.env = env_like if env is not None else None
-        model.n_envs = env_like.num_envs
-        model.observation_space, model.action_space = env_like.observation_space, env_like.action_space
-        model._vec_normalize_env = unwrap_vec_normalize(env_like) if env is not None else None
-        model.setup_model()
-        model.learner.load_parameters(params, exact_match=True)
-        return model
+        return model._finish_load(env, obs_space, Box(-1.0, 1.0, (params["model/pi/dense/kernel"].shape[1],)), params)

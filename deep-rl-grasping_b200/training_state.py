@@ -1,4 +1,4 @@
-"""Training-state directories: everything a stopped SAC / BDQ / DQN run needs to continue where it stopped.
+"""Training-state directories: everything a stopped SAC / BDQ / DQN / PPO2 run needs to continue where it stopped.
 
 ``<dir>/`` holds
   model.zip          the stable-baselines zip of ``model.save`` (parameters only, loadable on its own)
@@ -83,7 +83,7 @@ def read_host(path: str) -> dict:
 
 def restore_vec_normalize(path: str, env) -> None:
     """Copies the saved VecNormalize statistics into ``env``'s own VecNormalize wrapper (when both exist)."""
-    from .sac_model import unwrap_vec_normalize
+    from .base_model import unwrap_vec_normalize
     from .vec_env import VecNormalize
     vn = unwrap_vec_normalize(env) if env is not None else None
     f = os.path.join(path, VECNORM_FILE)

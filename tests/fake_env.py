@@ -37,3 +37,26 @@ class FakeGraspEnv:
 def make_env(config, evaluate=False, validate=False, test=False):
     """Factory with the signature train_cli expects (mirrors gym.make('gripper-env-v0', config=..., evaluate=..., ...))."""
     return FakeGraspEnv(seed=1 if evaluate else 0, horizon=20)
+
+
+class FakeFlatEnv:
+    """Flat observations of ``obs_dim`` floats in [0, 1) and a Box(-1, 1)^n_act action space, or Discrete(n_discrete) when
+    that is given: the shape of the BDQ, DQN and PPO2 configurations."""
+
+    def __init__(self, seed=0, horizon=5, obs_dim=6, n_act=3, n_discrete=None):
+        from b200grasp.spaces import Discrete
+        self.observation_space = Box(0.0, 1.0, (obs_dim,))
+        self.action_space = Box(-1.0, 1.0, (n_act,), seed=seed) if n_discrete is None else Discrete(n_discrete, seed=seed)
+        self.rng = np.random.default_rng(seed)
+        self.horizon, self.t, self.obs_dim = horizon, 0, obs_dim
+
+    def reset(self):
+        self.t = 0
+        return self.rng.uniform(0, 1, self.obs_dim).astype(np.float32)
+
+    def step(self, action):
+        self.t += 1
+        return self.rng.uniform(0, 1, self.obs_dim).astype(np.float32), float(self.rng.normal()), self.t >= self.horizon, {}
+
+    def close(self):
+        pass
