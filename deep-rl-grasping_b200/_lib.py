@@ -33,6 +33,10 @@ SYMBOLS = [
     "b2g_ppo_create", "b2g_ppo_destroy", "b2g_ppo_param_count", "b2g_ppo_param_info", "b2g_ppo_get_param", "b2g_ppo_set_param",
     "b2g_ppo_get_grad", "b2g_ppo_rollout_act", "b2g_ppo_rollout_reward", "b2g_ppo_rollout_reset", "b2g_ppo_rollout_get",
     "b2g_ppo_update", "b2g_ppo_train_step_explicit", "b2g_ppo_act", "b2g_ppo_get_step", "b2g_ppo_state_save", "b2g_ppo_state_load",
+    "b2g_trpo_create", "b2g_trpo_destroy", "b2g_trpo_param_count", "b2g_trpo_param_info", "b2g_trpo_get_param", "b2g_trpo_set_param",
+    "b2g_trpo_get_grad", "b2g_trpo_rollout_act", "b2g_trpo_rollout_reward", "b2g_trpo_rollout_reset", "b2g_trpo_rollout_get",
+    "b2g_trpo_update", "b2g_trpo_fvp", "b2g_trpo_step_explicit", "b2g_trpo_act", "b2g_trpo_get_step", "b2g_trpo_state_save",
+    "b2g_trpo_state_load",
     "b2g_encoder_create", "b2g_encoder_destroy", "b2g_encoder_n_layers", "b2g_encoder_layer_shape", "b2g_encoder_set_weights",
     "b2g_encoder_encode", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor", "b2g_debug_gg_simt", "b2g_debug_gg_tc",
     "b2g_autoencoder_create", "b2g_autoencoder_destroy", "b2g_autoencoder_n_layers", "b2g_autoencoder_layer_shape",
@@ -96,6 +100,26 @@ class PpoCfg(C.Structure):
 class PpoMetrics(C.Structure):
     _fields_ = [("policy_loss", C.c_float), ("value_loss", C.c_float), ("entropy", C.c_float), ("approxkl", C.c_float),
                 ("clipfrac", C.c_float), ("grad_norm", C.c_float), ("n_updates", C.c_int64)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class TrpoCfg(C.Structure):
+    _fields_ = [
+        ("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("hidden0", C.c_int32), ("hidden1", C.c_int32),
+        ("timesteps_per_batch", C.c_int32), ("cg_iters", C.c_int32), ("vf_iters", C.c_int32), ("gamma", C.c_float), ("lam", C.c_float),
+        ("max_kl", C.c_float), ("cg_damping", C.c_float), ("entcoeff", C.c_float), ("vf_stepsize", C.c_float), ("seed", C.c_uint64),
+        ("device", C.c_int32),
+    ]
+
+
+class TrpoMetrics(C.Structure):
+    _fields_ = [("optimgain", C.c_float), ("meankl", C.c_float), ("entbonus", C.c_float), ("surrgain", C.c_float), ("entropy", C.c_float),
+                ("optimgain_after", C.c_float), ("meankl_after", C.c_float), ("entbonus_after", C.c_float),
+                ("surrgain_after", C.c_float), ("entropy_after", C.c_float), ("grad_sq", C.c_float), ("shs", C.c_float),
+                ("expected_improve", C.c_float), ("vf_loss", C.c_float), ("cg_iters", C.c_int32), ("accepted", C.c_int32),
+                ("n_iterations", C.c_int64)]
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
@@ -206,7 +230,7 @@ def load():
     lib.b2g_last_step_ms.restype = C.c_float
     lib.b2g_profile_step.argtypes = [vp, C.c_float, C.POINTER(C.c_char_p), fp, C.c_int]
     lib.b2g_sac_state_save.argtypes = lib.b2g_sac_state_load.argtypes = [vp, C.c_char_p]
-    for p in ("bdq", "dqn", "ppo"):          # the handle, named-parameter and training-state calls the three learners share
+    for p in ("bdq", "dqn", "ppo", "trpo"):  # the handle, named-parameter and training-state calls the learners share
         for f in ("destroy", "param_count"):
             getattr(lib, f"b2g_{p}_{f}").argtypes = [vp]
         getattr(lib, f"b2g_{p}_param_info").argtypes = [vp, C.c_int, C.c_char_p, C.c_size_t, i64p, i64p, C.POINTER(C.c_int32)]
@@ -244,6 +268,16 @@ def load():
     lib.b2g_ppo_train_step_explicit.argtypes = [vp, fp, fp, fp, fp, fp, C.c_float, C.c_float, C.c_float, C.c_int, C.POINTER(PpoMetrics)]
     lib.b2g_ppo_act.argtypes = [vp, fp, C.c_int, C.c_int, fp, fp, fp]
     lib.b2g_ppo_get_step.argtypes = [vp, i64p, i64p, C.POINTER(C.c_int32)]
+    lib.b2g_trpo_create.argtypes = [C.POINTER(TrpoCfg), C.POINTER(vp)]
+    lib.b2g_trpo_rollout_act.argtypes = [vp, fp, fp]
+    lib.b2g_trpo_rollout_reward.argtypes = [vp, C.c_float, C.c_float]
+    lib.b2g_trpo_rollout_reset.argtypes = [vp]
+    lib.b2g_trpo_rollout_get.argtypes = [vp, fp, fp, fp, fp]
+    lib.b2g_trpo_update.argtypes = [vp, fp, C.POINTER(C.c_int32), C.POINTER(TrpoMetrics)]
+    lib.b2g_trpo_fvp.argtypes = [vp, fp, fp, fp]
+    lib.b2g_trpo_step_explicit.argtypes = [vp, fp, fp, fp, fp, C.POINTER(C.c_int32), C.POINTER(TrpoMetrics), fp, fp, fp]
+    lib.b2g_trpo_act.argtypes = [vp, fp, C.c_int, C.c_int, fp, fp]
+    lib.b2g_trpo_get_step.argtypes = [vp, i64p, i64p, C.POINTER(C.c_int32)]
     lib.b2g_encoder_create.argtypes = [C.POINTER(EncoderCfg), C.POINTER(vp)]
     lib.b2g_encoder_destroy.argtypes = [vp]
     lib.b2g_encoder_n_layers.argtypes = [vp]

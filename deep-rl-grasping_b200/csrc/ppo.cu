@@ -31,6 +31,7 @@
 #include <vector>
 
 #include "../../include/b200grasp.h"
+#include "actor_critic.cuh"
 #include "common.cuh"
 #include "host.cuh"
 #include "state.cuh"
@@ -39,8 +40,7 @@ using namespace b2g;
 
 namespace {
 
-constexpr int kMaxA = 16;            // action components: the tail keeps a row's mean in registers
-constexpr int kMaxWidth = 256;       // hidden widths (multiples of 4: 16-byte rows for the engine)
+constexpr int kMaxA = kAcMaxA;       // action components: the tail keeps a row's mean in registers
 constexpr int kMaxMinibatch = 16384; // one tail CTA walks the minibatch
 constexpr int kTailThreads = 1024;
 constexpr int kNormBlocks = 128, kNormThreads = 256;
@@ -82,122 +82,8 @@ __global__ void ppo_iota_rows_kernel(int* __restrict__ rowoff, int first, int n,
   if (i < n) rowoff[i] = (first + i) * XS;
 }
 
-__global__ void ppo_bias_tanh_kernel(const float* __restrict__ Z, const float* __restrict__ b, float* __restrict__ Y, int n, int N) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n * N) Y[i] = tanhf(Z[i] + b[i % N]);
-}
-
-struct HeadArgs {
-  const float* Y1; int h1;             // [rows, 2 h1]: pi latent | vf latent
-  const float* Wpi; const float* bpi;  // [h1, A], [A]
-  const float* Wvf; const float* bvf;  // [h1, 1], [1]
-  const float* logstd;                 // [A]
-  int A;
-};
-
-// mean and value of row r
-__device__ __forceinline__ void ppo_heads(const HeadArgs& a, int r, float* mu, float& v) {
-  const float* ypi = a.Y1 + (size_t)r * 2 * a.h1;
-  const float* yvf = ypi + a.h1;
-#pragma unroll
-  for (int k = 0; k < kMaxA; ++k) mu[k] = k < a.A ? a.bpi[k] : 0.f;
-  v = a.bvf[0];
-  for (int j = 0; j < a.h1; ++j) {
-    const float yp = ypi[j];
-    const float* w = a.Wpi + (size_t)j * a.A;
-#pragma unroll
-    for (int k = 0; k < kMaxA; ++k)
-      if (k < a.A) mu[k] = fmaf(yp, w[k], mu[k]);
-    v = fmaf(yvf[j], a.Wvf[j], v);
-  }
-}
-
-// Actor over `rows` rows.  mode 0: rollout step t (noise of stream 1, stores action / value / neglogp in row t and the actions
-// in out); mode 1: bootstrap values -> lastv; mode 2: predict (deterministic or stream-1 noise) -> out, values -> vout.
-struct ActArgs {
-  HeadArgs h;
-  int rows, mode, deterministic, t;
-  unsigned long long key;
-  long long* step;                     // stream-1 step counter (advanced by one per drawing call)
-  float* r_act; float* r_val; float* r_nlp;   // rollout rows
-  float* lastv;
-  float* out; float* vout; float* nlpout;
-};
-
-__global__ void __launch_bounds__(kTailThreads) ppo_act_kernel(ActArgs a) {
-  __shared__ unsigned long long s_step;
-  const bool draw = a.mode == 0 || (a.mode == 2 && !a.deterministic);
-  if (threadIdx.x == 0) s_step = (unsigned long long)*a.step;
-  __syncthreads();
-  const int A = a.h.A;
-  const float half_log_2pi = 0.91893853320467274f;
-  for (int r = threadIdx.x; r < a.rows; r += blockDim.x) {
-    float mu[kMaxA], v;
-    ppo_heads(a.h, r, mu, v);
-    if (a.mode == 1) { a.lastv[r] = v; continue; }
-    float z[kMaxA];
-#pragma unroll
-    for (int k = 0; k < kMaxA; ++k) z[k] = 0.f;
-    if (draw) {
-      const uint2 key = make_uint2((unsigned)a.key, (unsigned)(a.key >> 32));
-      // element r * A + k of the flattened [rows, A] noise: lane (i & 3) of block i >> 2 (oracle/philox_ref.py noise)
-#pragma unroll
-      for (int k = 0; k < kMaxA; ++k) {
-        if (k >= A) break;
-        const int i = r * A + k, blk = i >> 2;
-        const uint4 q = philox4x32_10(make_uint4((unsigned)s_step, (unsigned)(s_step >> 32), (unsigned)blk, 1u), key);
-        const int lane = i & 3;
-        const unsigned x0 = lane < 2 ? q.x : q.z, x1 = lane < 2 ? q.y : q.w;
-        const float u0 = ((float)(x0 >> 8) + 0.5f) * (1.0f / 16777216.0f), u1 = ((float)(x1 >> 8) + 0.5f) * (1.0f / 16777216.0f);
-        const float rr = sqrtf(-2.f * logf(u0));
-        float s, c;
-        sincospif(2.f * u1, &s, &c);
-        z[k] = rr * ((lane & 1) ? s : c);
-      }
-    }
-    float nlp = half_log_2pi * (float)A;
-#pragma unroll
-    for (int k = 0; k < kMaxA; ++k) {
-      if (k >= A) break;
-      const float ls = a.h.logstd[k];
-      const float act = mu[k] + expf(ls) * z[k];
-      nlp += 0.5f * z[k] * z[k] + ls;
-      if (a.mode == 0) a.r_act[((size_t)a.t * a.rows + r) * A + k] = act;
-      a.out[(size_t)r * A + k] = act;
-    }
-    if (a.mode == 0) {
-      a.r_val[(size_t)a.t * a.rows + r] = v;
-      a.r_nlp[(size_t)a.t * a.rows + r] = nlp;
-    } else {
-      if (a.vout) a.vout[r] = v;
-      if (a.nlpout) a.nlpout[r] = nlp;
-    }
-  }
-  __syncthreads();
-  if (draw && threadIdx.x == 0) *a.step += 1;
-}
-
-// GAE (ppo2.py Runner._run): a thread per env, reverse over the n_steps rows.  done[t] is the episode-start flag of step t,
-// done[n_steps] the flags after the last step.
-__global__ void ppo_gae_kernel(const float* __restrict__ rew, const float* __restrict__ val, const float* __restrict__ done,
-                               const float* __restrict__ lastv, int T, int E, float gamma, float lam, float* __restrict__ adv,
-                               float* __restrict__ ret) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= E) return;
-  float last = 0.f;
-  for (int t = T - 1; t >= 0; --t) {
-    const size_t i = (size_t)t * E + e;
-    const float nnt = 1.f - done[(size_t)(t + 1) * E + e];
-    const float nv = t == T - 1 ? lastv[e] : val[i + E];
-    const float delta = rew[i] + gamma * nv * nnt - val[i];
-    last = delta + gamma * lam * nnt * last;
-    adv[i] = last;
-    ret[i] = last + val[i];
-  }
-}
-
 struct TailArgs2 {
-  HeadArgs h;
+  AcHeadArgs h;
   int M;
   const int* rowidx;                           // minibatch row -> rollout / staging row
   const float* act; const float* oval; const float* onlp; const float* ret;
@@ -220,7 +106,7 @@ __global__ void __launch_bounds__(kTailThreads) ppo_tail_kernel(TailArgs2 a) {
   for (int r = tid; r < M; r += NT) {
     const int q = a.rowidx[r];
     float mu[kMaxA], v;
-    ppo_heads(a.h, r, mu, v);
+    ac_heads(a.h, r, mu, v);
     float nlp = 0.91893853320467274f * (float)A;
     for (int k = 0; k < A; ++k) {
       const float ls = a.h.logstd[k];
@@ -372,31 +258,23 @@ __global__ void __launch_bounds__(256) ppo_adam_kernel(float* __restrict__ P, fl
 }  // namespace
 
 // one forward pass (layers 0 and 1) over M rows of an observation arena, and the backward launches of a minibatch
-struct PpoFwd { GemmGroup l0, l1; int M = 0; };
-struct PpoMb { PpoFwd f; GemmGroup b1, b0; const int* rowidx = nullptr; };
+using PpoFwd = AcFwd;
+struct PpoMb { AcFwd f; GemmGroup b1, b0; const int* rowidx = nullptr; };
 
-struct b2g_ppo {
+struct b2g_ppo : ActorCritic {     // network, rollout rows, Z0 / Y0 / Y1, actor outputs, counters [1] (actor_critic.cuh)
   b2g_ppo_cfg cfg{};
-  int D = 0, XS = 0, A = 0, H0 = 0, H1 = 0, E = 0, T = 0, NB = 0, M = 0, NMB = 0, RMAX = 0, P_ROWS = 0;
+  int E = 0, T = 0, NB = 0, M = 0, NMB = 0, RMAX = 0, P_ROWS = 0;
   ParamTable params;            // the zip's variables; q/w and q/b without gradient
   int64_t n_train = 0, n_total = 0;
-  int64_t oW0 = 0, ob0 = 0, oW1[2]{}, ob1[2]{}, oWvf = 0, obvf = 0, oWpi = 0, obpi = 0, ols = 0;
-  float *P = nullptr, *Mo = nullptr, *Vo = nullptr, *G = nullptr;
-  cudaStream_t stream = nullptr;
-  std::vector<void*> allocs;
-  // rollout
-  float *r_obs = nullptr, *r_act = nullptr, *r_val = nullptr, *r_nlp = nullptr, *r_rew = nullptr, *r_done = nullptr;
-  float *r_adv = nullptr, *r_ret = nullptr, *lastv = nullptr;
-  int t = 0;                    // rollout rows filled
+  float *Mo = nullptr, *Vo = nullptr, *G = nullptr;
   // explicit minibatch and predict staging
   float *s_obs = nullptr, *s_act = nullptr, *s_val = nullptr, *s_nlp = nullptr, *s_ret = nullptr, *p_obs = nullptr;
-  // activations and scratch (RMAX rows)
-  float *Z0 = nullptr, *Y0 = nullptr, *Y1 = nullptr, *dZ1 = nullptr, *dZ0 = nullptr;
+  // backward activations and scratch (RMAX rows)
+  float *dZ1 = nullptr, *dZ0 = nullptr;
   float *sz = nullptr, *sv = nullptr, *snlp = nullptr, *sadv = nullptr, *sdm = nullptr, *sdls = nullptr, *sdv = nullptr;
-  float *a_out = nullptr, *a_v = nullptr, *a_nlp = nullptr;
   int *perm = nullptr, *rowidx = nullptr, *rowoff = nullptr, *act_rowoff = nullptr;
   float *part = nullptr, *met = nullptr, *hp = nullptr;
-  long long* counters = nullptr;  // [0] Adam step, [1] stream-1 step, [2] n_updates
+  // counters: [0] Adam step, [1] stream-1 step, [2] n_updates
   float* h_buf = nullptr;         // pinned: metrics, hyper-parameters
   PpoFwd f_act, f_boot, f_pred;
   PpoMb mb_explicit;
@@ -404,7 +282,6 @@ struct b2g_ppo {
   cudaGraphExec_t graph_exec = nullptr;
   bool use_graph = true;
   bool broken = false;
-  unsigned long long act_key = 0;
   long long n_updates = 0;
 };
 
@@ -417,41 +294,16 @@ void add_t(b2g_ppo* h, const std::string& name, int rows, int cols, int stride, 
 // the zip names carry the model/ scope; the bare names are accepted too
 std::string scoped(const char* name) { return strncmp(name, "model/", 6) == 0 ? name : "model/" + std::string(name); }
 
-int splits_for(int tiles, int R) {   // split-R so a launch covers about two waves of the 132 SMs, >= 64 rows per slice
-  const int want = (264 + tiles - 1) / tiles;
-  return std::max(1, std::min(want, (R + 63) / 64));
-}
-
-// layers 0 and 1 over M rows of `obs` at row offsets rowoff
-int make_fwd(b2g_ppo* h, PpoFwd& f, const float* obs, const int* rowoff, int M, std::map<std::string, const int*>& tab) {
-  const int D = h->D, H0 = h->H0, H1 = h->H1;
-  f.M = M;
-  f.l0 = GemmGroup(); f.l1 = GemmGroup();
-  f.l0.name = "ppo_l0_fwd"; f.l1.name = "ppo_l1_fwd";
-  const int tiles = ((M + 63) / 64) * ((2 * H0 + 63) / 64);
-  GemmDesc d = gemm_desc(obs, rowoff, tab["iD"], h->P + h->oW0, tab["iD_2H0"], tab["i2H0"], h->Z0, tab["rM_2H0"], tab["i2H0"], M, 2 * H0, D,
-                         GG_A_RVEC | GG_EPI_ATOMIC, splits_for(tiles, D));
-  f.l0.host.push_back(d);
-  for (int tw = 0; tw < 2; ++tw) {
-    GemmDesc g = gemm_desc(h->Y0 + tw * H0, tab["rM_2H0"], tab["iH0"], h->P + h->oW1[tw], tab["iH0_H1"], tab["iH1"], h->Y1 + tw * H1,
-                           tab["rM_2H1"], tab["iH1"], M, H1, H0, GG_A_RVEC | GG_EPI_BIAS_TANH);
-    g.bias = h->P + h->ob1[tw];
-    f.l1.host.push_back(g);
-  }
-  if (int rc = finalize_tiles(f.l0, h->allocs, h->stream)) return rc;
-  return finalize_tiles(f.l1, h->allocs, h->stream);
-}
-
 int make_mb(b2g_ppo* h, PpoMb& mb, const float* obs, const int* rowoff, const int* rowidx, std::map<std::string, const int*>& tab) {
   const int M = h->M, D = h->D, H0 = h->H0, H1 = h->H1;
-  if (int rc = make_fwd(h, mb.f, obs, rowoff, M, tab)) return rc;
+  if (int rc = ac_make_fwd(h, mb.f, obs, rowoff, M, tab)) return rc;
   mb.rowidx = rowidx;
   mb.b1 = GemmGroup(); mb.b0 = GemmGroup();
   mb.b1.name = "ppo_l1_bwd"; mb.b0.name = "ppo_l0_wgrad";
   for (int tw = 0; tw < 2; ++tw) {
     const int tiles = ((H0 + 63) / 64) * ((H1 + 63) / 64);
     GemmDesc w = gemm_desc(h->Y0 + tw * H0, tab["iH0"], tab["rM_2H0"], h->dZ1 + tw * H1, tab["rM_2H1"], tab["iH1"], h->G + h->oW1[tw],
-                           tab["iH0_H1"], tab["iH1"], H0, H1, M, GG_COLSUM | GG_EPI_ATOMIC, splits_for(tiles, M));
+                           tab["iH0_H1"], tab["iH1"], H0, H1, M, GG_COLSUM | GG_EPI_ATOMIC, ac_splits_for(tiles, M));
     w.colsum = h->G + h->ob1[tw];
     mb.b1.host.push_back(w);
     GemmDesc dg = gemm_desc(h->dZ1 + tw * H1, tab["rM_2H1"], tab["iH1"], h->P + h->oW1[tw], tab["iH1"], tab["iH0_H1"], h->dZ0 + tw * H0,
@@ -461,43 +313,20 @@ int make_mb(b2g_ppo* h, PpoMb& mb, const float* obs, const int* rowoff, const in
   }
   const int tiles0 = ((D + 63) / 64) * ((2 * H0 + 63) / 64);
   GemmDesc w0 = gemm_desc(obs, tab["iD"], rowoff, h->dZ0, tab["rM_2H0"], tab["i2H0"], h->G + h->oW0, tab["iD_2H0"], tab["i2H0"], D, 2 * H0, M,
-                          GG_COLSUM | GG_EPI_ATOMIC, splits_for(tiles0, M));
+                          GG_COLSUM | GG_EPI_ATOMIC, ac_splits_for(tiles0, M));
   w0.colsum = h->G + h->ob0;
   mb.b0.host.push_back(w0);
   if (int rc = finalize_tiles(mb.b1, h->allocs, h->stream)) return rc;
   return finalize_tiles(mb.b0, h->allocs, h->stream);
 }
 
-HeadArgs heads(b2g_ppo* h) {
-  HeadArgs a{};
-  a.Y1 = h->Y1; a.h1 = h->H1; a.A = h->A;
-  a.Wpi = h->P + h->oWpi; a.bpi = h->P + h->obpi; a.Wvf = h->P + h->oWvf; a.bvf = h->P + h->obvf; a.logstd = h->P + h->ols;
-  return a;
-}
-
-void fwd_issue(b2g_ppo* h, const PpoFwd& f, cudaStream_t s) {
-  cudaMemsetAsync(h->Z0, 0, (size_t)f.M * 2 * h->H0 * sizeof(float), s);
-  gg_simt_launch(f.l0.dev, (int)f.l0.host.size(), f.l0.total_tiles, s);
-  const int n = f.M * 2 * h->H0;
-  ppo_bias_tanh_kernel<<<(n + 255) / 256, 256, 0, s>>>(h->Z0, h->P + h->ob0, h->Y0, f.M, 2 * h->H0);
-  gg_simt_launch_tanh(f.l1.dev, (int)f.l1.host.size(), f.l1.total_tiles, s);
-}
-
-ActArgs act_args(b2g_ppo* h, int rows, int mode) {
-  ActArgs a{};
-  a.h = heads(h); a.rows = rows; a.mode = mode; a.key = h->act_key; a.step = h->counters + 1;
-  a.r_act = h->r_act; a.r_val = h->r_val; a.r_nlp = h->r_nlp; a.lastv = h->lastv;
-  a.out = h->a_out; a.vout = h->a_v; a.nlpout = h->a_nlp;
-  return a;
-}
-
 // one minibatch: forward, tail, backward, global norm, Adam
 void mb_issue(b2g_ppo* h, const PpoMb& mb, const float* act, const float* oval, const float* onlp, const float* ret, bool apply) {
   cudaStream_t s = h->stream;
   cudaMemsetAsync(h->G, 0, (size_t)h->n_train * sizeof(float), s);
-  fwd_issue(h, mb.f, s);
+  ac_fwd_issue(h, mb.f, s);
   TailArgs2 t{};
-  t.h = heads(h); t.M = h->M; t.rowidx = mb.rowidx;
+  t.h = ac_head_args(h); t.M = h->M; t.rowidx = mb.rowidx;
   t.act = act; t.oval = oval; t.onlp = onlp; t.ret = ret; t.hp = h->hp;
   t.ent_coef = h->cfg.ent_coef; t.vf_coef = h->cfg.vf_coef;
   t.sz = h->sz; t.sv = h->sv; t.snlp = h->snlp; t.sadv = h->sadv; t.sdm = h->sdm; t.sdls = h->sdls; t.sdv = h->sdv; t.dZ1 = h->dZ1;
@@ -517,10 +346,9 @@ int update_issue(b2g_ppo* h) {
   cudaStream_t s = h->stream;
   const int n = h->cfg.noptepochs * h->NB;
   ppo_rows_kernel<<<(n + 255) / 256, 256, 0, s>>>(h->perm, n, h->T, h->E, h->XS, h->rowidx, h->rowoff);
-  fwd_issue(h, h->f_boot, s);
-  ppo_act_kernel<<<1, kTailThreads, 0, s>>>(act_args(h, h->E, 1));
-  ppo_gae_kernel<<<(h->E + 127) / 128, 128, 0, s>>>(h->r_rew, h->r_val, h->r_done, h->lastv, h->T, h->E, h->cfg.gamma, h->cfg.lam,
-                                                    h->r_adv, h->r_ret);
+  ac_fwd_issue(h, h->f_boot, s);
+  ac_act(ac_act_args(h, h->E, 1), s);
+  ac_gae(h->r_rew, h->r_val, h->r_done, h->lastv, h->T, h->E, h->cfg.gamma, h->cfg.lam, h->r_adv, h->r_ret, s);
   cudaMemsetAsync(h->met, 0, 2 * PM_N * sizeof(float), s);
   for (const PpoMb& mb : h->mbs) mb_issue(h, mb, h->r_act, h->r_val, h->r_nlp, h->r_ret, true);
   // the flags after the last step are the episode-start flags of the next rollout's first step
@@ -577,7 +405,7 @@ int b2g_ppo_create(const b2g_ppo_cfg* cfg, b2g_ppo** out) {
   const b2g_ppo_cfg& c = *cfg;
   if (c.obs_dim < 1 || c.obs_dim > 65536) return b2g_fail(B2G_EINVAL, "obs_dim must be in [1, 65536]");
   if (c.n_actions < 1 || c.n_actions > kMaxA) return b2g_fail(B2G_EINVAL, "n_actions must be in [1, 16]");
-  if (c.hidden0 % 4 || c.hidden1 % 4 || c.hidden0 < 4 || c.hidden1 < 4 || c.hidden0 > kMaxWidth || c.hidden1 > kMaxWidth)
+  if (c.hidden0 % 4 || c.hidden1 % 4 || c.hidden0 < 4 || c.hidden1 < 4 || c.hidden0 > kAcMaxWidth || c.hidden1 > kAcMaxWidth)
     return b2g_fail(B2G_EINVAL, "hidden widths must be multiples of 4 in [4, 256]");
   if (c.n_envs < 1 || c.n_envs > 4096) return b2g_fail(B2G_EINVAL, "n_envs must be in [1, 4096]");
   if (c.n_steps < 1 || c.n_steps > 65536) return b2g_fail(B2G_EINVAL, "n_steps must be in [1, 65536]");
@@ -647,9 +475,9 @@ int b2g_ppo_create(const b2g_ppo_cfg* cfg, b2g_ppo** out) {
       (rc = T_("iH0_H1", iota_tab(H0, H1))) || (rc = T_("iD_2H0", iota_tab(D, 2 * H0))) || (rc = T_("boot", iota_tab((int)E, h->XS, (int)(T * E) * h->XS))) ||
       (rc = T_("pred", iota_tab(h->P_ROWS, h->XS))) || (rc = T_("sM", iota_tab(h->M, h->XS))) || (rc = T_("iM", iota_tab(h->M))))
     return bail(rc);
-  if ((rc = make_fwd(h, h->f_act, h->r_obs, h->act_rowoff, (int)E, tab))) return bail(rc);
-  if ((rc = make_fwd(h, h->f_boot, h->r_obs, tab["boot"], (int)E, tab))) return bail(rc);
-  if ((rc = make_fwd(h, h->f_pred, h->p_obs, tab["pred"], h->P_ROWS, tab))) return bail(rc);
+  if ((rc = ac_make_fwd(h, h->f_act, h->r_obs, h->act_rowoff, (int)E, tab))) return bail(rc);
+  if ((rc = ac_make_fwd(h, h->f_boot, h->r_obs, tab["boot"], (int)E, tab))) return bail(rc);
+  if ((rc = ac_make_fwd(h, h->f_pred, h->p_obs, tab["pred"], h->P_ROWS, tab))) return bail(rc);
   if ((rc = make_mb(h, h->mb_explicit, h->s_obs, tab["sM"], tab["iM"], tab))) return bail(rc);
   h->mbs.resize((size_t)c.noptepochs * c.nminibatches);
   for (size_t k = 0; k < h->mbs.size(); ++k)
@@ -681,10 +509,10 @@ int b2g_ppo_rollout_act(b2g_ppo* h, const float* obs, float* act_out) {
   cudaStream_t s = h->stream;
   if (int rc = upload_rows(h, h->r_obs + (size_t)h->t * h->E * h->XS, obs, h->E)) return rc;
   ppo_iota_rows_kernel<<<(h->E + 255) / 256, 256, 0, s>>>(h->act_rowoff, h->t * h->E, h->E, h->XS);
-  fwd_issue(h, h->f_act, s);
-  ActArgs a = act_args(h, h->E, 0);
+  ac_fwd_issue(h, h->f_act, s);
+  AcActArgs a = ac_act_args(h, h->E, 0);
   a.t = h->t;
-  ppo_act_kernel<<<1, kTailThreads, 0, s>>>(a);
+  ac_act(a, s);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(act_out, h->a_out, (size_t)h->E * h->A * sizeof(float), cudaMemcpyDefault, s));
   CK(cudaStreamSynchronize(s));
@@ -786,10 +614,10 @@ int b2g_ppo_act(b2g_ppo* h, const float* obs, int n, int deterministic, float* a
   for (int done_n = 0; done_n < n; done_n += P) {
     const int chunk = std::min(P, n - done_n);
     if (int rc = upload_rows(h, h->p_obs, obs + (size_t)done_n * h->D, chunk)) return rc;
-    fwd_issue(h, h->f_pred, s);
-    ActArgs a = act_args(h, chunk, 2);
+    ac_fwd_issue(h, h->f_pred, s);
+    AcActArgs a = ac_act_args(h, chunk, 2);
     a.deterministic = deterministic;
-    ppo_act_kernel<<<1, kTailThreads, 0, s>>>(a);
+    ac_act(a, s);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(act_out + (size_t)done_n * h->A, h->a_out, (size_t)chunk * h->A * sizeof(float), cudaMemcpyDefault, s));
     if (value_out) CK(cudaMemcpyAsync(value_out + done_n, h->a_v, chunk * sizeof(float), cudaMemcpyDefault, s));

@@ -19,7 +19,7 @@
 
 namespace b2g {
 
-enum : uint32_t { STATE_KIND_SAC = 1, STATE_KIND_BDQ = 2, STATE_KIND_DQN = 3, STATE_KIND_PPO = 4 };
+enum : uint32_t { STATE_KIND_SAC = 1, STATE_KIND_BDQ = 2, STATE_KIND_DQN = 3, STATE_KIND_PPO = 4, STATE_KIND_TRPO = 5 };
 
 constexpr uint32_t state_tag(const char (&s)[5]) {
   return (uint32_t)(unsigned char)s[0] | (uint32_t)(unsigned char)s[1] << 8 | (uint32_t)(unsigned char)s[2] << 16 |

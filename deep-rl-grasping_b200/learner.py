@@ -1,6 +1,6 @@
 """Thin numpy-facing wrappers of the device-resident learners' handles.
 
-``HandleLearner`` is what the wrappers of the ``b2g_sac``, ``b2g_bdq``, ``b2g_dqn`` and ``b2g_ppo`` handles share.
+``HandleLearner`` is what the wrappers of the ``b2g_sac``, ``b2g_bdq``, ``b2g_dqn``, ``b2g_ppo`` and ``b2g_trpo`` handles share.
 ``Learner`` wraps one ``b2g_sac`` handle and is what ``SAC`` (sac_model.py, the stable-baselines-shaped front end) drives;
 tests and bench.py also use it directly because it maps 1:1 onto the C ABI entry points.
 """

@@ -101,28 +101,28 @@ def _schedule(v):
     return v if callable(v) else (lambda _frac, _v=v: _v)
 
 
-def _check_policy(policy):
+def _check_policy(policy, algo="PPO2"):
     from .common.policies import MlpPolicy
     if isinstance(policy, str):
         if policy != "MlpPolicy":
-            raise NotImplementedError(f"policy '{policy}': only common.policies.MlpPolicy is built for PPO2")
+            raise NotImplementedError(f"policy '{policy}': only common.policies.MlpPolicy is built for {algo}")
     elif policy is not MlpPolicy:
-        raise NotImplementedError(f"policy {getattr(policy, '__name__', policy)}: only common.policies.MlpPolicy is built for PPO2 "
+        raise NotImplementedError(f"policy {getattr(policy, '__name__', policy)}: only common.policies.MlpPolicy is built for {algo} "
                                   "(CNN, recurrent and layer-norm policies are not)")
 
 
-def _check_policy_kwargs(policy_kwargs):
+def _check_policy_kwargs(policy_kwargs, algo="PPO2"):
     kw = dict(policy_kwargs or {})
     unknown = set(kw) - {"layers", "net_arch", "act_fun", "feature_extraction", "layer_norm"}
     if unknown:
-        raise NotImplementedError(f"policy_kwargs {sorted(unknown)} are not built for PPO2")
+        raise NotImplementedError(f"policy_kwargs {sorted(unknown)} are not built for {algo}")
     if kw.get("feature_extraction", "mlp") != "mlp":
-        raise NotImplementedError("feature_extraction: only the MLP extractor is built for PPO2")
+        raise NotImplementedError(f"feature_extraction: only the MLP extractor is built for {algo}")
     if kw.get("layer_norm", False):
         raise NotImplementedError("layer_norm=True: layer-normalised policies are not built")
     act = kw.get("act_fun")
     if act is not None and getattr(act, "__name__", str(act)) != "tanh":
-        raise NotImplementedError("act_fun: only tanh is built for PPO2")
+        raise NotImplementedError(f"act_fun: only tanh is built for {algo}")
     layers = [int(x) for x in kw.get("layers", None) or [64, 64]]
     if "net_arch" in kw and kw["net_arch"] is not None:
         na = list(kw["net_arch"])
@@ -133,7 +133,7 @@ def _check_policy_kwargs(policy_kwargs):
             raise NotImplementedError(f"net_arch pi={pi} vf={vf}: the towers must have the same widths")
         layers = pi
     if len(layers) != 2:
-        raise NotImplementedError(f"layers={layers}: the PPO2 learner builds exactly two hidden layers")
+        raise NotImplementedError(f"layers={layers}: the {algo} learner builds exactly two hidden layers")
     return kw, layers
 
 
@@ -302,11 +302,11 @@ class PPO2(BaseModel):
         self._boundary = (self.num_timesteps, np.random.get_state())
 
 
-def _init_params(obs_dim, n_actions, layers, seed):
+def _init_params(obs_dim, n_actions, layers, seed, rng=None, scope=_SCOPE):
     """common/tf_layers.py ortho_init in the variables' creation order: the orthogonal factor of an SVD of a standard normal
     matrix, scaled sqrt(2) for the hidden layers, 1 for vf, 0.01 for pi and q; zero biases and logstd.  The normal draws come
-    from a generator seeded with ``seed``."""
-    rng = np.random.default_rng(seed)
+    from ``rng``, by default a generator seeded with ``seed``; the names carry ``scope``."""
+    rng = np.random.default_rng(seed) if rng is None else rng
     h0, h1 = layers
     p = OrderedDict()
     for name, shape in (("pi_fc0/w", (obs_dim, h0)), ("pi_fc0/b", (h0,)), ("vf_fc0/w", (obs_dim, h0)), ("vf_fc0/b", (h0,)),
@@ -314,10 +314,10 @@ def _init_params(obs_dim, n_actions, layers, seed):
                         ("vf/b", (1,)), ("pi/w", (h1, n_actions)), ("pi/b", (n_actions,)), ("pi/logstd", (1, n_actions)),
                         ("q/w", (h1, n_actions)), ("q/b", (n_actions,))):
         if name == "pi/logstd" or len(shape) == 1:
-            p[_SCOPE + name] = np.zeros(shape, np.float32)
+            p[scope + name] = np.zeros(shape, np.float32)
             continue
         scale = 1.0 if name == "vf/w" else (0.01 if name in ("pi/w", "q/w") else np.sqrt(2.0))
         u, _, v = np.linalg.svd(rng.normal(0.0, 1.0, shape), full_matrices=False)
         w = u if u.shape == shape else v
-        p[_SCOPE + name] = (scale * w.reshape(shape)).astype(np.float32)
+        p[scope + name] = (scale * w.reshape(shape)).astype(np.float32)
     return p

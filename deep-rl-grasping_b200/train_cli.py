@@ -2,7 +2,7 @@
 
 Mirrors /root/reference/manipulation_main/training/train_stable_baselines.py:26-148 (same sub-commands, flags,
 ``model_dir`` layout: ``config.yaml``, ``best_model/``, ``logs/rl_model_*`` checkpoints, ``vecnormalize.pkl``,
-``log_file.monitor.csv``) and the SAC / PPO / DQN / BDQ branches of ``SBPolicy.learn`` (sb_helper.py:69-128,137-165,175-247).  The
+``log_file.monitor.csv``) and the SAC / TRPO / PPO / DQN / BDQ branches of ``SBPolicy.learn`` (sb_helper.py:69-165,175-247).  The
 environment itself stays the reference's (PyBullet on host cores): ``--env module:callable`` names a factory
 ``f(config, evaluate=False, validate=False, test=False) -> gym.Env``; the default imports the reference package and
 calls ``gym.make('gripper-env-v0', ...)`` exactly like the original script.
@@ -27,6 +27,7 @@ from .deepq import DQN
 from .deepq.policies import MlpPolicy as DQNMlpPolicy
 from .common.policies import MlpPolicy as PPOMlpPolicy
 from .ppo2 import PPO2
+from .trpo_mpi import TRPO
 from .sac_model import CnnPolicy, MlpPolicy
 from .vec_env import DummyVecEnv, SubprocVecEnv, VecNormalize
 
@@ -82,6 +83,14 @@ def train(args):
             raise NotImplementedError("--algo PPO: --device_norm is built for SAC and BDQ only")
         if args.load_dir:
             raise NotImplementedError("--algo PPO: --load_dir is not read by the reference's PPO branch (sb_helper.py:137-154)")
+    if algo == "TRPO":         # TRPO stores what the host VecNormalize returns and trains on one environment
+        if args.device_norm:
+            raise NotImplementedError("--algo TRPO: --device_norm is built for SAC and BDQ only")
+        if args.load_dir:
+            raise NotImplementedError("--algo TRPO: --load_dir is not read by the reference's TRPO branch (sb_helper.py:129-136)")
+        if int(args.n_envs) > 1:
+            raise ValueError("--algo TRPO: the model requires a non vectorized environment or a single vectorized environment "
+                             "(--n_envs 1)")
     os.mkdir(args.model_dir)                                   # like the reference: refuses to overwrite a run
     os.mkdir(os.path.join(args.model_dir, "best_model"))
     if args.simple:
@@ -154,8 +163,10 @@ def train(args):
             old.close()
     elif algo == "PPO":
         model = PPO2(PPOMlpPolicy, env, **ppo_kwargs(config))
+    elif algo == "TRPO":
+        model = TRPO(PPOMlpPolicy, env, **trpo_kwargs(config))
     else:
-        raise NotImplementedError(f"--algo {algo}: the H100 learner builds the SAC, PPO, DQN and BDQ branches of SBPolicy.learn "
+        raise NotImplementedError(f"--algo {algo}: the H100 learner builds the SAC, TRPO, PPO, DQN and BDQ branches of SBPolicy.learn "
                                   "(sb_helper.py:85-226)")
     if args.state_freq:
         callbacks.append(TrainingStateCallback(args.state_freq, os.path.join(args.model_dir, STATE_DIR)))
@@ -189,6 +200,13 @@ def ppo_kwargs(config):
     return dict(verbose=2, gamma=config["discount_factor"], learning_rate=config["PPO"]["learning_rate"])
 
 
+def trpo_kwargs(config):
+    """sb_helper.py:129-136: gamma (discount_factor), timesteps_per_batch (TRPO.max_iters) and vf_stepsize (TRPO.step_size) come
+    from the config, with verbose=2; every other TRPO setting stays at stable-baselines' default."""
+    c = config["TRPO"]
+    return dict(verbose=2, gamma=config["discount_factor"], timesteps_per_batch=c["max_iters"], vf_stepsize=c["step_size"])
+
+
 def _learn_keeping_state(model, total_timesteps, callbacks, state_dir, reset_num_timesteps=True):
     """model.learn; an interrupt (Ctrl-C) writes the training state before the run ends, as sb_helper.py:178-181 does
     for the model."""
@@ -204,7 +222,7 @@ def resume(args):
     model_dir = args.resume
     config = yaml.safe_load(open(os.path.join(model_dir, "config.yaml")))
     algo = config["algorithm"].upper()
-    if algo not in ("SAC", "BDQ", "DQN", "PPO"):
+    if algo not in ("SAC", "BDQ", "DQN", "PPO", "TRPO"):
         raise NotImplementedError(f"--resume: algorithm '{algo}' has no training state")
     state_dir = training_state.resolve(os.path.join(model_dir, STATE_DIR))
     done = int(training_state.read_host(state_dir)["num_timesteps"])
@@ -227,7 +245,7 @@ def resume(args):
     ]
     if args.state_freq:
         callbacks.append(TrainingStateCallback(args.state_freq, os.path.join(model_dir, STATE_DIR)))
-    model = {"SAC": SAC, "BDQ": BDQ, "DQN": DQN, "PPO": PPO2}[algo].load_training_state(state_dir, env)
+    model = {"SAC": SAC, "BDQ": BDQ, "DQN": DQN, "PPO": PPO2, "TRPO": TRPO}[algo].load_training_state(state_dir, env)
     remaining = int(config[algo]["total_timesteps"]) - model.num_timesteps
     if remaining > 0:
         _learn_keeping_state(model, remaining, callbacks, os.path.join(model_dir, STATE_DIR), reset_num_timesteps=False)
@@ -280,8 +298,10 @@ def run(args):
         agent = DQN.load(args.model)
     elif algo == "ppo":
         agent = PPO2.load(args.model)
+    elif algo == "trpo":
+        agent = TRPO.load(args.model)
     else:
-        raise NotImplementedError(f"algorithm '{algo}': only sac / ppo / dqn / bdq zips run on the H100 learner")
+        raise NotImplementedError(f"algorithm '{algo}': only sac / trpo / ppo / dqn / bdq zips run on the H100 learner")
     print("Run the agent")
     out = run_agent(task, agent, args.stochastic, n_episodes=args.episodes)
     task.close()

@@ -1,4 +1,4 @@
-"""Training-state directories: everything a stopped SAC / BDQ / DQN / PPO2 run needs to continue where it stopped.
+"""Training-state directories: everything a stopped SAC / BDQ / DQN / PPO2 / TRPO run needs to continue where it stopped.
 
 ``<dir>/`` holds
   model.zip          the stable-baselines zip of ``model.save`` (parameters only, loadable on its own)

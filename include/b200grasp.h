@@ -469,6 +469,83 @@ int b2g_ppo_get_step(b2g_ppo* h, int64_t* adam_step, int64_t* noise_step, int32_
 int b2g_ppo_state_save(b2g_ppo* h, const char* path);
 int b2g_ppo_state_load(b2g_ppo* h, const char* path);
 
+/* ------------------------------------------------------------------------------------------------
+ * TRPO learner -- the `sb.TRPO` object of sb_helper.py:129-136 (stable-baselines 2.10.1 trpo_mpi with common.policies.MlpPolicy
+ * and one environment, restated in tests/trpo_ref.py).  Variables pi/model/... (the live policy, PPO2's 15 variables under
+ * pi/) then oldpi/model/... (the old policy, the same 15).  The rollout of timesteps_per_batch = N steps lives on the device
+ * (b2g_trpo_rollout_act / _reward); b2g_trpo_update runs, as one CUDA graph: the boundary action and bootstrap value, GAE,
+ * oldpi := pi, the policy gradient at theta_old, cg_iters conjugate-gradient iterations on Fisher-vector products over the
+ * rows [::5], the KL-constrained line search (ten step sizes 0.5^k in one pass), then vf_iters passes of 128-row value
+ * minibatches with MpiAdam (epsilon 1e-8).  Box actions only.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct b2g_trpo b2g_trpo;
+typedef struct b2g_trpo_cfg {
+  int32_t obs_dim;             /* flattened observation (float32, no scaling): [1, 65536]                            */
+  int32_t n_actions;           /* Box action size: [1, 16]                                                            */
+  int32_t hidden0, hidden1;    /* net_arch pi = vf = [hidden0, hidden1]: multiples of 4 in [4, 256] ([64, 64] default)  */
+  int32_t timesteps_per_batch; /* N: [1, 16384] (1024 default)                                                       */
+  int32_t cg_iters;            /* [1, 64] (10)                                                                        */
+  int32_t vf_iters;            /* [0, 64] (3)                                                                         */
+  float gamma, lam;            /* 0.99, 0.98                                                                          */
+  float max_kl;                /* > 0 (0.01)                                                                          */
+  float cg_damping;            /* >= 0 (1e-2)                                                                         */
+  float entcoeff;              /* 0                                                                                   */
+  float vf_stepsize;           /* MpiAdam learning rate (3e-4)                                                        */
+  uint64_t seed;               /* the actor's noise key is seed ^ 0xA5A5A5A5DEADBEEF (Philox stream 1)               */
+  int32_t device;
+} b2g_trpo_cfg;
+typedef struct b2g_trpo_metrics {
+  float optimgain, meankl, entbonus, surrgain, entropy;   /* the losses at theta_old                                   */
+  float optimgain_after, meankl_after, entbonus_after, surrgain_after, entropy_after;  /* at the accepted theta          */
+  float grad_sq;               /* g . g of the policy gradient at theta_old                                          */
+  float shs;                   /* 0.5 stepdir . F stepdir                                                            */
+  float expected_improve;      /* g . fullstep                                                                       */
+  float vf_loss;               /* mean value loss over the value minibatches (0 without any)                         */
+  int32_t cg_iters;            /* conjugate-gradient iterations run                                                  */
+  int32_t accepted;            /* line-search k (step 0.5^k), -1: every candidate rejected, -2: zero gradient       */
+  int64_t n_iterations;        /* policy iterations so far                                                           */
+} b2g_trpo_metrics;
+
+/* B2G_EINVAL naming the limit outside the ranges above, or the device memory the line search needs */
+int b2g_trpo_create(const b2g_trpo_cfg* cfg, b2g_trpo** out);
+int b2g_trpo_destroy(b2g_trpo* h);
+/* the 30 variables in the zip's order: pi/model/... then oldpi/model/...; get_grad returns the policy gradient g at theta_old
+ * of the last step for the policy variables (pi_fc0, pi_fc1, pi and pi/logstd under pi/model/) and refuses the others */
+int b2g_trpo_param_count(const b2g_trpo* h);
+int b2g_trpo_param_info(const b2g_trpo* h, int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim);
+int b2g_trpo_get_param(b2g_trpo* h, const char* name, float* dst, size_t numel);
+int b2g_trpo_set_param(b2g_trpo* h, const char* name, const float* src, size_t numel);
+int b2g_trpo_get_grad(b2g_trpo* h, const char* name, float* dst, size_t numel);
+/* rollout step t: obs [obs_dim] -> row t; act_out [n_actions] = mean + exp(logstd) * eps, unclipped.  After an update, step 0
+ * returns the action drawn for the boundary observation before that update (stable-baselines' traj_segment_generator) and
+ * draws nothing.  B2G_ESTATE when N rows are filled. */
+int b2g_trpo_rollout_act(b2g_trpo* h, const float* obs, float* act_out);
+/* the reward of step t and the env's done flag after it */
+int b2g_trpo_rollout_reward(b2g_trpo* h, float rew, float done);
+/* empty rollout, episode-start flag cleared, no carried action (a fresh env.reset()) */
+int b2g_trpo_rollout_reset(b2g_trpo* h);
+/* [N] advantages, tdlamret, values and [N, n_actions] actions of the rollout; any pointer may be NULL */
+int b2g_trpo_rollout_get(b2g_trpo* h, float* adv, float* ret, float* val, float* act);
+/* one iteration on a full rollout: last_obs [obs_dim] is the boundary observation; perm [vf_iters * N] holds each value pass's
+ * permutation.  B2G_ESTATE when the conjugate-gradient step direction is not finite (metrics are still written). */
+int b2g_trpo_update(b2g_trpo* h, const float* last_obs, const int32_t* perm, b2g_trpo_metrics* out);
+/* test entry points, at the current parameters; both empty the rollout.  fvp: v [n_policy] in var_list order (pi_fc0/w,
+ * pi_fc0/b, pi_fc1/w, pi_fc1/b, pi/w, pi/b, pi/logstd) -> F v over the rows [::5] of obs [N, obs_dim], damping included.
+ * step_explicit: the policy and value step of b2g_trpo_update on obs [N, obs_dim], actions [N, n_actions], raw advantages
+ * [N], tdlamret [N] and perm [vf_iters * N]; grad / stepdir / fullstep [n_policy] in var_list order may be NULL. */
+int b2g_trpo_fvp(b2g_trpo* h, const float* obs, const float* v, float* out);
+int b2g_trpo_step_explicit(b2g_trpo* h, const float* obs, const float* actions, const float* adv, const float* tdlamret,
+                           const int32_t* perm, b2g_trpo_metrics* out, float* grad, float* stepdir, float* fullstep);
+/* predict: n observations -> mean (deterministic) or mean + std * eps (stream 1, advancing the rollout's counter);
+ * value_out may be NULL */
+int b2g_trpo_act(b2g_trpo* h, const float* obs, int n, int deterministic, float* act_out, float* value_out);
+/* value-Adam step, stream-1 step counter, rollout rows filled */
+int b2g_trpo_get_step(b2g_trpo* h, int64_t* adam_step, int64_t* noise_step, int32_t* rollout_rows);
+/* training state at an iteration boundary: parameters (pi and oldpi), the value Adam's moments, counters, iterations.  A load
+ * empties the rollout and clears the episode-start flag. */
+int b2g_trpo_state_save(b2g_trpo* h, const char* path);
+int b2g_trpo_state_load(b2g_trpo* h, const char* path);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Row a12: auto-encoder ENCODER forward (perception for the `encoded depth` observation, SURVEY.md section 8).
  * Replaces SimpleAutoEncoder.encode  (/root/reference/manipulation_main/gripperEnv/encoders.py:59-61; graph :87-108)
