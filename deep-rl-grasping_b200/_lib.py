@@ -17,7 +17,7 @@ B2G_EINVAL, B2G_ECUDA, B2G_ESTATE = -1, -2, -3
 #: every symbol include/b200grasp.h declares (tests check the .so exports each of them)
 SYMBOLS = [
     "b2g_last_error", "b2g_version", "b2g_nccl_unique_id", "b2g_sac_create", "b2g_sac_destroy", "b2g_sac_dp_export", "b2g_sac_dp_connect", "b2g_debug_dp_stamps", "b2g_debug_compact_host", "b2g_sync",
-    "b2g_sac_create2", "b2g_param_count", "b2g_param_info", "b2g_get_param", "b2g_set_param", "b2g_get_grad", "b2g_get_adam",
+    "b2g_sac_create2", "b2g_sac_create3", "b2g_param_count", "b2g_param_info", "b2g_get_param", "b2g_set_param", "b2g_get_grad", "b2g_get_adam",
     "b2g_reset_optimizer", "b2g_replay_add", "b2g_replay_size", "b2g_replay_get", "b2g_replay_info", "b2g_get_last_batch", "b2g_set_norm_stats", "b2g_sac_step",
     "b2g_sac_step_async", "b2g_sac_step_explicit", "b2g_sac_step_host_pipelined", "b2g_sac_pipeline_flush", "b2g_sac_act", "b2g_launches_per_step", "b2g_last_step_ms",
     "b2g_profile_step", "b2g_sac_state_save", "b2g_sac_state_load",
@@ -139,6 +139,15 @@ class ReplayCfg(C.Structure):
     _fields_ = [("frame_capacity", C.c_int64), ("u8_plane_mask", C.c_uint32)]
 
 
+#: b2g_sac_net_cfg.extractor: the CNN policy's feature extractor (include/b200grasp.h)
+B2G_CNN_AUGMENTED, B2G_CNN_NATURE = 0, 1
+EXTRACTORS = {"augmented": B2G_CNN_AUGMENTED, "nature_cnn": B2G_CNN_NATURE}
+
+
+class SacNetCfg(C.Structure):
+    _fields_ = [("extractor", C.c_int32)]
+
+
 class SacMetrics(C.Structure):
     _fields_ = [(n, C.c_float) for n in (
         "policy_loss", "qf1_loss", "qf2_loss", "value_loss", "ent_coef_loss", "entropy", "ent_coef",
@@ -193,6 +202,7 @@ def load():
     lib.b2g_nccl_unique_id.argtypes = [vp, C.c_char_p]
     lib.b2g_sac_create.argtypes = [C.POINTER(SacCfg), C.POINTER(vp)]
     lib.b2g_sac_create2.argtypes = [C.POINTER(SacCfg), C.POINTER(ReplayCfg), C.POINTER(vp)]
+    lib.b2g_sac_create3.argtypes = [C.POINTER(SacCfg), C.POINTER(ReplayCfg), C.POINTER(SacNetCfg), C.POINTER(vp)]
     i64p = C.POINTER(C.c_int64)
     lib.b2g_replay_info.argtypes = [vp, i64p, i64p, i64p, i64p, i64p, i64p]
     lib.b2g_sac_destroy.argtypes = [vp]

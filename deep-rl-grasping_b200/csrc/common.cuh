@@ -241,9 +241,10 @@ void prep_launch(const PrepArgs& a, cudaStream_t s);
 // ---------------------------------------------------------------------------------------------
 // replay row compaction, gather + VecNormalize + /255 (replay.cu)
 // ---------------------------------------------------------------------------------------------
-// full observations [n][HW][Cfull] -> compact rows (first_row + i) % wrap of dst: image planes [HW][Cfull-1] | value at pixel
-// [0,0] of the last plane | 3 zero pads
-void compact_rows(const float* src_full, float* dst, long long first_row, long long wrap, int n, int HW, int Cfull, cudaStream_t s);
+// full observations [n][HW][Cfull] -> compact rows (first_row + i) % wrap of dst: image planes [HW][Ci] | value at pixel [0,0]
+// of plane Ci (Cfull == Ci + 1, the augmented extractor's direct feature; 0 when Cfull == Ci) | 3 zero pads
+void compact_rows(const float* src_full, float* dst, long long first_row, long long wrap, int n, int HW, int Ci, int Cfull,
+                  cudaStream_t s);
 
 // How a replay frame stores one compact row of Ec floats: npx image elements [HW][Ci] (NHWC), then a tail of Ec - npx floats
 // (CNN: the actuator value and 3 pads; MLP: npx = 0 and the tail is the whole observation).  Image channel c lives in the
@@ -298,6 +299,7 @@ struct GatherArgs {
   float* x_obs; float* x_next;   // CNN: [B,H,W,Cimg] image planes (scaled)
   uint16_t* x_obs_hi; uint16_t* x_obs_lo; uint16_t* x_next_hi; uint16_t* x_next_lo;   // optional BF16 planes of x
   float* F_pi; float* F_v; float* F_t; int FS; int feat_col; // feature rows: direct feature -> col feat_col; MLP: whole obs -> cols 0..
+  int act_col;               // CNN: feature-row column of the first replay action (feat_col < 0: no direct feature)
   float* rew_out; float* done_out; int n_act;
   // in-kernel slot draw (indices == nullptr && rng_counters != nullptr): Philox stream 0 of prep_kernel, same values
   const long long* rng_counters;   // [4] = rng step, [5] = replay size, [6] = first live slot (ring_cap > 0)

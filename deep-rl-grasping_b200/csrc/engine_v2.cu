@@ -120,7 +120,7 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
   const bool norm_obs = g.normc[3] != 0.0;
   const float scale = g.scale;
   for (int it = tid; it < 512; it += blockDim.x) s2d_half_block<Ci>(a, src, it, which, b);
-  if (tid == 0) {                                            // direct feature -> column 512 of the feature rows
+  if (tid == 0 && g.feat_col >= 0) {                         // direct feature -> column 512 of the feature rows
     float yy = frame_elem(src, g.fmt, npx, Ci, npx);
     if (norm_obs) yy = (float)fmin(fmax(((double)yy - g.mean[npx]) * g.var[npx], -clip_obs), clip_obs);
     yy = yy / scale;
@@ -135,7 +135,7 @@ __global__ void __launch_bounds__(512) gather2_kernel(Gather2Args a) {
     }
   }
   if (which == 0 && g.act) {
-    const int feat_dim = g.feat_col + 1;
+    const int feat_dim = g.act_col;
     if (tid < g.n_act) {
       const float av = g.act[slot * g.n_act + tid];
       g.F_v[(size_t)b * g.FS + feat_dim + tid] = av;
@@ -482,16 +482,16 @@ int v2_create(b2g_sac* h) {
     start += ((R + 63) / 64) * ((N + 32 * P2_SUB - 1) / (32 * P2_SUB));
     jobs.push_back(j);
   };
-  add_job(h->p("model/pi/cnn1/w"), 64 * Ci, 32, v.W1T[0], 3, 1, K1, 0);
+  add_job(h->p(h->cnn_t("model/pi", 0, "w")), 64 * Ci, 32, v.W1T[0], 3, 1, K1, 0);
   jobs.back().k1_ci = Ci;
-  add_job(h->p("model/values_fn/cnn1/w"), 64 * Ci, 32, v.W1T[0], 3, 1, K1, 32);
+  add_job(h->p(h->cnn_t("model/values_fn", 0, "w")), 64 * Ci, 32, v.W1T[0], 3, 1, K1, 32);
   jobs.back().k1_ci = Ci;
-  add_job(h->p("target/values_fn/cnn1/w"), 64 * Ci, 32, v.W1T[1], 3, 1, K1, 0);
+  add_job(h->p(h->cnn_t("target/values_fn", 0, "w")), 64 * Ci, 32, v.W1T[1], 3, 1, K1, 0);
   jobs.back().k1_ci = Ci;
   for (int n = 0; n < 3; ++n) {
-    add_job(h->p(std::string(nets[n]) + "/cnn2/w"), 512, 64, v.W2T[n], 3, 1, 512, 0);
-    add_job(h->p(std::string(nets[n]) + "/cnn3/w"), 576, 64, v.W3T[n], 3, 1, 576, 0);
-    add_job(h->p(std::string(nets[n]) + "/cnn_fc1/w"), 1024, 512, v.WfT[n], 3, 1, 1024, 0);
+    add_job(h->p(h->cnn_t(nets[n], 1, "w")), 512, 64, v.W2T[n], 3, 1, 512, 0);
+    add_job(h->p(h->cnn_t(nets[n], 2, "w")), 576, 64, v.W3T[n], 3, 1, 576, 0);
+    add_job(h->p(h->cnn_t(nets[n], 3, "w")), 1024, 512, v.WfT[n], 3, 1, 1024, 0);
   }
   add_job(h->p("model/pi/fc0/kernel"), h->feat_dim, H, v.K0T[0], 3, 1, KF, 0);
   add_job(h->p("model/values_fn/vf/fc0/kernel"), h->feat_dim, H, v.K0T[1], 3, 1, KF, 0);
@@ -500,9 +500,9 @@ int v2_create(b2g_sac* h) {
   add_job(h->p("target/values_fn/vf/fc0/kernel"), h->feat_dim, H, v.K0T[2], 3, 1, KF, 0);
   v.plane_ctas_fwd = start;      // the forward-layout jobs above, then the backward layouts (first read by bwd_fused)
   for (int n = 0; n < 2; ++n) {
-    add_job(h->p(std::string(nets[n]) + "/cnn2/w"), 512, 64, v.W2n[n], 2, 0, 64, 0);
-    add_job(h->p(std::string(nets[n]) + "/cnn3/w"), 576, 64, v.W3n[n], 2, 0, 64, 0);
-    add_job(h->p(std::string(nets[n]) + "/cnn_fc1/w"), 1024, 512, v.Wfn[n], 2, 0, 512, 0);
+    add_job(h->p(h->cnn_t(nets[n], 1, "w")), 512, 64, v.W2n[n], 2, 0, 64, 0);
+    add_job(h->p(h->cnn_t(nets[n], 2, "w")), 576, 64, v.W3n[n], 2, 0, 64, 0);
+    add_job(h->p(h->cnn_t(nets[n], 3, "w")), 1024, 512, v.Wfn[n], 2, 0, 512, 0);
   }
   add_job(h->p("model/pi/fc0/kernel"), h->feat_dim, H, v.K0n[0], 2, 0, H, 0);
   add_job(h->p("model/values_fn/vf/fc0/kernel"), h->feat_dim, H, v.K0n[1], 2, 0, 3 * H, 0);
@@ -568,8 +568,8 @@ int v2_create(b2g_sac* h) {
       P.grp_stride = (int)h1_net;
       const int net0 = w == 0 ? 0 : 2;
       for (int p = 0; p < 3; ++p) P.out_p[p] = v.H1[net0][p];
-      P.bias = h->p(std::string(nets[net0]) + "/cnn1/b");
-      P.bias_grp = w == 0 ? (int)(h->p("model/values_fn/cnn1/b") - h->p("model/pi/cnn1/b")) : 32;
+      P.bias = h->p(h->cnn_t(nets[net0], 0, "b"));
+      P.bias_grp = w == 0 ? (int)(h->p(h->cnn_t("model/values_fn", 0, "b")) - h->p(h->cnn_t("model/pi", 0, "b"))) : 32;
       g.host[g.n++] = P;
     }
     if (int rc = push_group(h, v.fwd, g, "conv1_fwd")) return rc;
@@ -589,7 +589,7 @@ int v2_create(b2g_sac* h) {
       P.epi = CG_EPI_ACT; P.rows_tile = 108; P.lim_rows = B * 36;
       P.o_tm = 108 * 64; P.o0 = 64; P.n_valid = 64; P.out_planes = 3;
       for (int p = 0; p < 3; ++p) P.out_p[p] = v.H2[n][p];
-      P.bias = h->p(std::string(nets[n]) + "/cnn2/b"); P.bias_grp = 32;
+      P.bias = h->p(h->cnn_t(nets[n], 1, "b")); P.bias_grp = 32;
       g.host[g.n++] = P;
     }
     if (int rc = push_group(h, v.fwd, g, "conv2_fwd")) return rc;
@@ -609,7 +609,7 @@ int v2_create(b2g_sac* h) {
       P.epi = CG_EPI_ACT; P.rows_tile = 128; P.lim_rows = B * 16;
       P.o_tm = 128 * 64; P.o0 = 64; P.n_valid = 64; P.out_planes = 3;
       for (int p = 0; p < 3; ++p) P.out_p[p] = v.H3[n][p];
-      P.bias = h->p(std::string(nets[n]) + "/cnn3/b"); P.bias_grp = 32;
+      P.bias = h->p(h->cnn_t(nets[n], 2, "b")); P.bias_grp = 32;
       g.host[g.n++] = P;
     }
     if (int rc = push_group(h, v.fwd, g, "conv3_fwd")) return rc;
@@ -629,7 +629,7 @@ int v2_create(b2g_sac* h) {
       P.epi = CG_EPI_ACT; P.rows_tile = 128; P.lim_rows = B;
       P.o_tm = (long long)128 * KF; P.o0 = KF; P.n_valid = 512; P.out_planes = 3;
       for (int p = 0; p < 3; ++p) P.out_p[p] = v.F[n][p];
-      P.bias = h->p(std::string(nets[n]) + "/cnn_fc1/b"); P.bias_grp = 32;
+      P.bias = h->p(h->cnn_t(nets[n], 3, "b")); P.bias_grp = 32;
       P.out_f = h->F[n]; P.f_tm = (long long)128 * FS; P.f0 = FS; P.f_grp = 32;
       if (v.split_fc1 > 1) {
         // 48 tiles of 16 K-chunks would hold 48 of the 132 SMs for the longest stretch of the forward launch: three K-splits per
@@ -686,7 +686,7 @@ int v2_create(b2g_sac* h) {
       P.o_tm = 128 * 512; P.o0 = 512; P.n_valid = 512; P.out_planes = 2;
       for (int p = 0; p < 2; ++p) P.out_p[p] = v.dZ4[n][p];
       P.mask = v.F[n][0]; P.m_tm = (long long)128 * KF; P.m0 = KF;
-      P.colsum = h->g(std::string(nets[n]) + "/cnn_fc1/b"); P.colsum_mask = 511;
+      P.colsum = h->g(h->cnn_t(nets[n], 3, "b")); P.colsum_mask = 511;
       g.host[g.n++] = P;
     }
     if (int rc = push_group(h, v.bwd_groups, g, "heads_dgrad")) return rc;
@@ -708,7 +708,7 @@ int v2_create(b2g_sac* h) {
         P.o_tm = 128 * 1024; P.o0 = 1024; P.n_valid = 1024; P.out_planes = 2;
         for (int p = 0; p < 2; ++p) P.out_p[p] = v.dZ3[n][p];
         P.mask = v.H3[n][0]; P.m_tm = 128 * 1024; P.m0 = 1024;
-        P.colsum = h->g(std::string(nets[n]) + "/cnn3/b"); P.colsum_mask = 63;     // dZ3 row = [16 pixels][64 channels]
+        P.colsum = h->g(h->cnn_t(nets[n], 2, "b")); P.colsum_mask = 63;     // dZ3 row = [16 pixels][64 channels]
         if (v.split_fc1_dgrad > 1) {         // 32 tiles of 8 K-chunks at the head of the backward chain: split-K with finalisation
           P.splits = v.split_fc1_dgrad;
           if (int rc = check_split("B2G_SPLIT_FC1_DGRAD", P.chunks, P.splits)) return rc;
@@ -729,7 +729,7 @@ int v2_create(b2g_sac* h) {
         }
         P.tiles_m = 8; P.tiles_n = 4;
         P.lim_rows = 1024; P.o_tm = 128 * 512; P.o0 = 512; P.n_valid = 512;
-        P.out_f = h->g(std::string(nets[n]) + "/cnn_fc1/w"); P.atomic = 0;
+        P.out_f = h->g(h->cnn_t(nets[n], 3, "w")); P.atomic = 0;
         g.host[g.n++] = P;
       }
     }
@@ -760,7 +760,7 @@ int v2_create(b2g_sac* h) {
         P.o_tm = 108 * 64; P.o0 = 64; P.n_valid = 64; P.out_planes = 2;
         for (int p = 0; p < 2; ++p) P.out_p[p] = v.dZ2[n][p];
         P.mask = v.H2[n][0]; P.m_tm = 108 * 64; P.m0 = 64;
-        P.colsum = h->g(std::string(nets[n]) + "/cnn2/b"); P.colsum_mask = 63;
+        P.colsum = h->g(h->cnn_t(nets[n], 1, "b")); P.colsum_mask = 63;
         g.host[g.n++] = P;
       }
       {
@@ -775,7 +775,7 @@ int v2_create(b2g_sac* h) {
         P.tiles_m = 5; P.tiles_n = 1;
         P.splits = std::max(1, std::min(P.chunks, std::max(14, (P.chunks + 15) / 16)));     // <= 16 chunks (64 k-steps) per accumulator chain
         P.lim_rows = 576; P.o_tm = 128 * 64; P.o0 = 64; P.n_valid = 64;
-        P.out_f = h->g(std::string(nets[n]) + "/cnn3/w"); P.atomic = 1;
+        P.out_f = h->g(h->cnn_t(nets[n], 2, "w")); P.atomic = 1;
         g.host[g.n++] = P;
       }
     }
@@ -815,7 +815,7 @@ int v2_create(b2g_sac* h) {
       P.n_valid = 128; P.out_planes = 2;
       for (int p = 0; p < 2; ++p) P.out_p[p] = v.dZ1[p];
       P.mask = v.H1[n][0];
-      P.colsum = h->g(std::string(nets[n]) + "/cnn1/b"); P.colsum_mask = 31;       // four parity classes x 32 channels
+      P.colsum = h->g(h->cnn_t(nets[n], 0, "b")); P.colsum_mask = 31;       // four parity classes x 32 channels
       g.host[g.n++] = P;
     }
     if (int rc = push_group(h, v.bwd_groups, g, "conv2_dgrad")) return rc;
@@ -834,7 +834,7 @@ int v2_create(b2g_sac* h) {
       P.tiles_m = 4; P.tiles_n = 1;
       P.splits = std::max(1, std::min(P.chunks, std::max(8, (P.chunks + 7) / 8)));           // <= 8 chunks (72 k-steps) per chain
       P.lim_rows = 512; P.o_tm = 128 * 64; P.o0 = 64; P.n_valid = 64;
-      P.out_f = h->g(std::string(nets[n]) + "/cnn2/w"); P.atomic = 1;
+      P.out_f = h->g(h->cnn_t(nets[n], 1, "w")); P.atomic = 1;
       g.host[g.n++] = P;
     }
     {
@@ -877,7 +877,7 @@ int v2_create(b2g_sac* h) {
       P.tiles_n = 1;
       P.splits = std::max(1, std::min(P.chunks, std::max(84 / P.tiles_m, (P.chunks + 15) / 16)));
       P.lim_rows = 64 * Cp; P.n_valid = 64;
-      P.out_f = h->g("model/pi/cnn1/w"); P.f_grp = (long long)(h->g("model/values_fn/cnn1/w") - h->g("model/pi/cnn1/w")); P.atomic = 1;
+      P.out_f = h->g(h->cnn_t("model/pi", 0, "w")); P.f_grp = (long long)(h->g(h->cnn_t("model/values_fn", 0, "w")) - h->g(h->cnn_t("model/pi", 0, "w"))); P.atomic = 1;
       g.host[g.n++] = P;
     }
     if (int rc = push_group(h, v.bwd_groups, g, "conv_wgrad")) return rc;

@@ -76,7 +76,8 @@ __global__ void __launch_bounds__(256) obs_rms_update_kernel(const float* __rest
 }
 
 void update_launch(b2g_sac* h, const float* a, const float* b, const float* done, int n) {
-  const int Cfull = h->cnn ? h->Cimg + 1 : 0, npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0;
+  // the plain nature_cnn's compact image block is the caller's observation itself: the flat layout
+  const int Cfull = h->direct_feature() ? h->Cobs : 0, npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0;
   obs_rms_update_launch(a, b, done, n, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, Cfull, npx,
                         h->stream);
   h->rms_count += n;
@@ -97,7 +98,7 @@ int ensure_staging(b2g_sac* h) {
 // every value of an 8-bit plane is an integer in [0, 255] (what b2g_replay_add refuses on the device, checked here on the
 // host so that nothing is enqueued for a refused call)
 bool u8_values_ok(const b2g_sac* h, const float* frame) {
-  const int Cfull = h->Cimg + 1, HW = h->Hi * h->Wi;
+  const int Cfull = h->Cobs, HW = h->Hi * h->Wi;
   for (int c = 0; c < h->Cimg; ++c) {
     if (!(h->u8_mask >> c & 1)) continue;
     for (int p = 0; p < HW; ++p) {
@@ -124,7 +125,7 @@ int upload(b2g_sac* h, void* dst, const void* src, size_t bytes) {
 
 // caller-layout frames [n][E] -> compact rows [n][Ec]
 int to_rows(b2g_sac* h, const float* full, float* rows, int row0, int n) {
-  if (h->cnn) compact_rows(full, rows, row0, (long long)h->stage_rows + h->B, n, h->Hi * h->Wi, h->Cimg + 1, h->stream);
+  if (h->cnn) compact_rows(full, rows, row0, (long long)h->stage_rows + h->B, n, h->Hi * h->Wi, h->Cimg, h->Cobs, h->stream);
   else CK(cudaMemcpyAsync(rows + (size_t)row0 * h->Ec, full, (size_t)n * h->E * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
   return 0;
 }

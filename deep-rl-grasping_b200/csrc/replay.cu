@@ -3,7 +3,8 @@
 //
 // Row layout.  MLP policy: a row is the observation vector.  CNN policy: a row is COMPACT, Ec = H*W*Ci + 4 floats -- the
 // image planes [H][W][Ci] (NHWC), then the one value of the constant actuator plane the network reads (pixel [0,0] of the last
-// channel, custom_obs_policy.py:28-32), then 3 zero pads.  Callers pass full [H][W][Ci+1] observations; compact_kernel
+// channel, custom_obs_policy.py:28-32; zero for the plain nature_cnn, whose rows hold all Ci planes of the observation), then
+// 3 zero pads.  Callers pass full [H][W][Ci+1] (plain nature_cnn: [H][W][Ci]) observations; compact_kernel
 // writes them into replay_add's staging, the explicit batch and policy inference's staging.  Replay frames hold such rows,
 // optionally with 8-bit image channels (FrameFmt, common.cuh); the gathers decode them into the same fp32 values.
 //
@@ -19,17 +20,16 @@
 namespace b2g {
 namespace {
 
-// full observation [HW][Cfull] -> compact row {image planes [HW][Ci] | value at pixel [0,0] of the last plane | 3 pad}
+// full observation [HW][Cfull] -> compact row {image planes [HW][Ci] | value at pixel [0,0] of plane Ci, or 0 | 3 pad}
 __global__ void __launch_bounds__(256) compact_kernel(const float* __restrict__ src, float* __restrict__ dst, long long first_row, long long wrap,
-                                                       int HW, int Cfull, int Ec) {
-  const int Ci = Cfull - 1;
+                                                       int HW, int Ci, int Cfull, int Ec) {
   const float* s = src + (size_t)blockIdx.x * HW * Cfull;
   float* d = dst + (size_t)((first_row + blockIdx.x) % wrap) * Ec;
   for (int e = threadIdx.x; e < HW * Ci; e += blockDim.x) {
     const int pix = e / Ci, c = e - pix * Ci;
     d[e] = s[(size_t)pix * Cfull + c];
   }
-  if (threadIdx.x < 4) d[HW * Ci + threadIdx.x] = threadIdx.x == 0 ? s[Ci] : 0.f;
+  if (threadIdx.x < 4) d[HW * Ci + threadIdx.x] = threadIdx.x == 0 && Cfull > Ci ? s[Ci] : 0.f;
 }
 
 // float64 VecNormalize of the 4 row elements [e, e + 4) (e % 4 == 0): clip((x - mean) * istd, +-clip_obs)
@@ -96,7 +96,7 @@ __global__ void __launch_bounds__(256) gather_kernel(GatherArgs g) {
         *reinterpret_cast<uint2*>(xlo + o + 4 * e4) = make_uint2((uint32_t)lo[0] | ((uint32_t)lo[1] << 16), (uint32_t)lo[2] | ((uint32_t)lo[3] << 16));
       }
     }
-    if (blockIdx.x == 0 && threadIdx.x == 0) {      // the actuator value -> the direct-feature column of the feature rows
+    if (g.feat_col >= 0 && blockIdx.x == 0 && threadIdx.x == 0) {      // the actuator value -> the direct-feature column
       float y = frame_elem(fsrc, g.fmt, npx, g.Cimg, npx);
       if (norm_obs) y = (float)fmin(fmax(((double)y - g.mean[npx]) * g.var[npx], -clip_obs), clip_obs);
       y = y / inv_scale_denom;
@@ -132,7 +132,7 @@ __global__ void __launch_bounds__(256) gather_kernel(GatherArgs g) {
     }
   }
   if (which == 0 && blockIdx.x == 0 && g.act) {
-    const int feat_dim = cnn ? g.feat_col + 1 : g.W;
+    const int feat_dim = cnn ? g.act_col : g.W;
     if (threadIdx.x < g.n_act) g.F_v[(size_t)b * g.FS + feat_dim + threadIdx.x] = g.act[slot * g.n_act + threadIdx.x];
     if (threadIdx.x == 32) {
       float r = g.rew[slot];
@@ -214,8 +214,9 @@ void frame_commit_launch(const FrameIo& io, const int* plan, long long fid0, lon
   if (m > 0) frame_commit_kernel<<<dim3(m, 2), 256, 0, s>>>(io, plan, fid0, fcap, m, r_ofr, r_nfr, first, cap);
 }
 
-void compact_rows(const float* src_full, float* dst, long long first_row, long long wrap, int n, int HW, int Cfull, cudaStream_t s) {
-  if (n > 0) compact_kernel<<<n, 256, 0, s>>>(src_full, dst, first_row, wrap, HW, Cfull, HW * (Cfull - 1) + 4);
+void compact_rows(const float* src_full, float* dst, long long first_row, long long wrap, int n, int HW, int Ci, int Cfull,
+                  cudaStream_t s) {
+  if (n > 0) compact_kernel<<<n, 256, 0, s>>>(src_full, dst, first_row, wrap, HW, Ci, Cfull, HW * Ci + 4);
 }
 
 void gather_launch(const GatherArgs& a, cudaStream_t s) {

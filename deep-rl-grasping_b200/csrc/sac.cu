@@ -46,6 +46,10 @@ namespace {
 
 int64_t pad32(int64_t n) { return (n + 31) / 32 * 32; }
 
+// layer scopes conv1, conv2, conv3, fc1 of each extractor (b2g_sac_net_cfg): create_augmented_nature_cnn's, and stable-baselines'
+// nature_cnn (common/policies.py: conv(.., 'c1'), 'c2', 'c3', linear(.., 'fc1'))
+const char* const kCnnScopes[2][4] = {{"cnn1", "cnn2", "cnn3", "cnn_fc1"}, {"c1", "c2", "c3", "fc1"}};
+
 void add_tensor(b2g_sac* h, const std::string& name, std::vector<int64_t> shape, int group) {
   Tensor t;
   t.name = name;
@@ -60,20 +64,20 @@ void add_tensor(b2g_sac* h, const std::string& name, std::vector<int64_t> shape,
 }
 
 void add_cnn(b2g_sac* h, const std::string& pre, int group) {
-  add_tensor(h, pre + "/cnn1/w", {8, 8, h->Cimg, 32}, group);
-  add_tensor(h, pre + "/cnn1/b", {1, 32, 1, 1}, group);
-  add_tensor(h, pre + "/cnn2/w", {4, 4, 32, 64}, group);
-  add_tensor(h, pre + "/cnn2/b", {1, 64, 1, 1}, group);
-  add_tensor(h, pre + "/cnn3/w", {3, 3, 64, 64}, group);
-  add_tensor(h, pre + "/cnn3/b", {1, 64, 1, 1}, group);
-  add_tensor(h, pre + "/cnn_fc1/w", {1024, 512}, group);
-  add_tensor(h, pre + "/cnn_fc1/b", {512}, group);
+  add_tensor(h, h->cnn_t(pre, 0, "w"), {8, 8, h->Cimg, 32}, group);
+  add_tensor(h, h->cnn_t(pre, 0, "b"), {1, 32, 1, 1}, group);
+  add_tensor(h, h->cnn_t(pre, 1, "w"), {4, 4, 32, 64}, group);
+  add_tensor(h, h->cnn_t(pre, 1, "b"), {1, 64, 1, 1}, group);
+  add_tensor(h, h->cnn_t(pre, 2, "w"), {3, 3, 64, 64}, group);
+  add_tensor(h, h->cnn_t(pre, 2, "b"), {1, 64, 1, 1}, group);
+  add_tensor(h, h->cnn_t(pre, 3, "w"), {1024, 512}, group);
+  add_tensor(h, h->cnn_t(pre, 3, "b"), {512}, group);
 }
 void add_mlp(b2g_sac* h, const std::string& pre, int in_dim, int group) {
   add_tensor(h, pre + "/fc0/kernel", {in_dim, h->H}, group);
   add_tensor(h, pre + "/fc0/bias", {h->H}, group);
-  add_tensor(h, pre + "/fc1/kernel", {h->H, h->H}, group);
-  add_tensor(h, pre + "/fc1/bias", {h->H}, group);
+  add_tensor(h, h->fc1(pre) + "/kernel", {h->H, h->H}, group);
+  add_tensor(h, h->fc1(pre) + "/bias", {h->H}, group);
 }
 
 // Parameter inventory in SB-zip order (oracle/sac_ref.py param_specs; SURVEY.md Appendix B)
@@ -159,6 +163,7 @@ int build_groups(b2g_sac* h) {
   TAB(kH, iota_tab(std::max(FS, H), H));   // j*H  (fc0 / fc1 kernel rows)
 
   auto nn = [&](int net, const char* s) { return std::string(nets[net]) + s; };
+  auto ct = [&](int net, int layer, const char* wb) { return h->cnn_t(nets[net], layer, wb); };
 
   if (h->cnn) {
     const int Ci = h->Cimg, Hi = h->Hi, Wi = h->Wi, H1 = h->H1, W1 = h->W1, H2 = h->H2, W2 = h->W2, H3 = h->H3, W3 = h->W3;
@@ -194,7 +199,6 @@ int build_groups(b2g_sac* h) {
       }
     }
     // ================= forward groups
-    const char* cname[3] = {"/cnn1", "/cnn2", "/cnn3"};
     for (int l = 0; l < 3; ++l) {
       const Conv& c = cv[l];
       GemmGroup g;
@@ -202,9 +206,9 @@ int build_groups(b2g_sac* h) {
       for (int n = 0; n < 3; ++n) {
         const float* in = l == 0 ? (n == 2 ? h->x_next : h->x_obs) : (l == 1 ? h->h1[n] : h->h2[n]);
         float* out = l == 0 ? h->h1[n] : (l == 1 ? h->h2[n] : h->h3[n]);
-        GemmDesc d = gemm_desc(in, rowoff[l], koff[l], h->p(nn(n, cname[l]) + "/w"), wrow[l], i64, out, crow[l], i64,
+        GemmDesc d = gemm_desc(in, rowoff[l], koff[l], h->p(ct(n, l, "w")), wrow[l], i64, out, crow[l], i64,
                         B * c.Ho * c.Wo, c.Co, c.k * c.k * c.Ci, GG_A_RVEC | GG_EPI_BIAS_RELU);
-        d.bias = h->p(nn(n, cname[l]) + "/b");
+        d.bias = h->p(ct(n, l, "b"));
         if (h->use_planes) {
           uint16_t* const* ip = l == 0 ? h->xp[n == 2 ? 1 : 0] : (l == 1 ? h->h1p[n] : h->h2p[n]);
           uint16_t* const* op = l == 0 ? h->h1p[n] : (l == 1 ? h->h2p[n] : h->h3p[n]);
@@ -222,9 +226,9 @@ int build_groups(b2g_sac* h) {
       GemmGroup g;
       g.name = "fc1_fwd";
       for (int n = 0; n < 3; ++n) {
-        GemmDesc d = gemm_desc(h->h3[n], fcA, i1024, h->p(nn(n, "/cnn_fc1/w")), fcW, i512, h->F[n], rowFS, i512, B, 512, 1024,
+        GemmDesc d = gemm_desc(h->h3[n], fcA, i1024, h->p(ct(n, 3, "w")), fcW, i512, h->F[n], rowFS, i512, B, 512, 1024,
                         GG_A_RVEC | GG_EPI_BIAS_RELU);
-        d.bias = h->p(nn(n, "/cnn_fc1/b"));
+        d.bias = h->p(ct(n, 3, "b"));
         if (h->use_planes) {
           d.flags |= GG_PLANES | GG_B_RVEC;
           d.A_hi = h->h3p[n][0]; d.A_lo = h->h3p[n][1];
@@ -291,15 +295,15 @@ int build_groups(b2g_sac* h) {
         TAB(rowP3, iota_tab(B, P3h * P3w * 64));
         TAB(wfT, iota_tab(1024, 512));
         for (int n = 0; n < 2; ++n) {
-          GemmDesc w = gemm_desc(h->h3[n], i1024, fcA, h->dZ4[n], row512, i512, h->g(nn(n, "/cnn_fc1/w")), fcW, i512, 1024, 512, B,
+          GemmDesc w = gemm_desc(h->h3[n], i1024, fcA, h->dZ4[n], row512, i512, h->g(ct(n, 3, "w")), fcW, i512, 1024, 512, B,
                           GG_COLSUM);
-          w.colsum = h->g(nn(n, "/cnn_fc1/b"));
+          w.colsum = h->g(ct(n, 3, "b"));
           if (h->use_planes) {
             w.flags = (w.flags & ~GG_COLSUM) | GG_PLANES | GG_MN_MAJOR;
             w.A_hi = h->h3p[n][0]; w.A_lo = h->h3p[n][1]; w.B_hi = h->dZ4p[n][0]; w.B_lo = h->dZ4p[n][1];
           }
           f.host.push_back(w);
-          GemmDesc dg = gemm_desc(h->dZ4[n], row512, i512, h->p(nn(n, "/cnn_fc1/w")), i512, wfT, h->dZ3p[n], rowP3, cN3p, B, 1024, 512,
+          GemmDesc dg = gemm_desc(h->dZ4[n], row512, i512, h->p(ct(n, 3, "w")), i512, wfT, h->dZ3p[n], rowP3, cN3p, B, 1024, 512,
                            GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
           dg.mask = h->h3[n]; dg.kM = fcA; dg.kN = i1024;
           if (h->use_planes) {
@@ -333,15 +337,15 @@ int build_groups(b2g_sac* h) {
         TAB(c64, iota_tab(64, 64));
         const int R = B * H3 * W3;
         for (int n = 0; n < 2; ++n) {
-          GemmDesc w = gemm_desc(h->h2[n], koff[2], rowoff[2], h->dZ3p[n], dz3row, i64, h->g(nn(n, "/cnn3/w")), wrow[2], i64, 576, 64, R,
+          GemmDesc w = gemm_desc(h->h2[n], koff[2], rowoff[2], h->dZ3p[n], dz3row, i64, h->g(ct(n, 2, "w")), wrow[2], i64, 576, 64, R,
                           GG_COLSUM | GG_EPI_ATOMIC, split_for(9, R));
-          w.colsum = h->g(nn(n, "/cnn3/b"));
+          w.colsum = h->g(ct(n, 2, "b"));
           if (h->use_planes) {
             w.flags = (w.flags & ~GG_COLSUM) | GG_PLANES | GG_MN_MAJOR;
             w.A_hi = h->h2p[n][0]; w.A_lo = h->h2p[n][1]; w.B_hi = h->dZ3pp[n][0]; w.B_lo = h->dZ3pp[n][1];
           }
           g.host.push_back(w);
-          GemmDesc dg = gemm_desc(h->dZ3p[n], t_am, t_ar, h->p(nn(n, "/cnn3/w")), t_br, c64, h->dZ2p[n], t_cm, i64, B * H2 * W2, 64, 576,
+          GemmDesc dg = gemm_desc(h->dZ3p[n], t_am, t_ar, h->p(ct(n, 2, "w")), t_br, c64, h->dZ2p[n], t_cm, i64, B * H2 * W2, 64, 576,
                            GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
           dg.mask = h->h2[n]; dg.kM = crow[1]; dg.kN = i64;
           if (h->use_planes) {
@@ -361,9 +365,9 @@ int build_groups(b2g_sac* h) {
         const int R = B * H2 * W2;
         TAB(c64, iota_tab(32, 64));
         for (int n = 0; n < 2; ++n) {
-          GemmDesc w = gemm_desc(h->h1[n], koff[1], rowoff[1], h->dZ2p[n], dz2row, i64, h->g(nn(n, "/cnn2/w")), wrow[1], i64, 512, 64, R,
+          GemmDesc w = gemm_desc(h->h1[n], koff[1], rowoff[1], h->dZ2p[n], dz2row, i64, h->g(ct(n, 1, "w")), wrow[1], i64, 512, 64, R,
                           GG_COLSUM | GG_EPI_ATOMIC, split_for(8, R));
-          w.colsum = h->g(nn(n, "/cnn2/b"));
+          w.colsum = h->g(ct(n, 1, "b"));
           if (h->use_planes) {
             w.flags = (w.flags & ~GG_COLSUM) | GG_PLANES | GG_MN_MAJOR;
             w.A_hi = h->h1p[n][0]; w.A_lo = h->h1p[n][1]; w.B_hi = h->dZ2pp[n][0]; w.B_lo = h->dZ2pp[n][1];
@@ -388,7 +392,7 @@ int build_groups(b2g_sac* h) {
                 }
             TAB(t_am, am); TAB(t_ar, ar); TAB(t_br, br); TAB(t_cm, cm);
             for (int n = 0; n < 2; ++n) {
-              GemmDesc dg = gemm_desc(h->dZ2p[n], t_am, t_ar, h->p(nn(n, "/cnn2/w")), t_br, c64, h->dZ1[n], t_cm, i64, B * ny * nx, 32, 256,
+              GemmDesc dg = gemm_desc(h->dZ2p[n], t_am, t_ar, h->p(ct(n, 1, "w")), t_br, c64, h->dZ1[n], t_cm, i64, B * ny * nx, 32, 256,
                                GG_A_RVEC | GG_B_RVEC | GG_EPI_MASK);
               dg.mask = h->h1[n];
               if (h->use_planes) {
@@ -408,9 +412,9 @@ int build_groups(b2g_sac* h) {
         g.name = "conv1_wgrad";
         const int R = B * H1 * W1, M = 64 * Ci;
         for (int n = 0; n < 2; ++n) {
-          GemmDesc w = gemm_desc(h->x_obs, koff[0], rowoff[0], h->dZ1[n], crow[0], i64, h->g(nn(n, "/cnn1/w")), wrow[0], i64, M, 32, R,
+          GemmDesc w = gemm_desc(h->x_obs, koff[0], rowoff[0], h->dZ1[n], crow[0], i64, h->g(ct(n, 0, "w")), wrow[0], i64, M, 32, R,
                           GG_COLSUM | GG_EPI_ATOMIC, split_for((M + 63) / 64, R, 74));
-          w.colsum = h->g(nn(n, "/cnn1/b"));
+          w.colsum = h->g(ct(n, 0, "b"));
           if (h->use_planes) {
             w.flags = (w.flags & ~GG_COLSUM) | GG_PLANES | GG_MN_MAJOR | ((Ci & 1) ? GG_A_ALIGN4 : 0) | GG_A_ROWLANES;
             w.A_hi = h->xp[0][0]; w.A_lo = h->xp[0][1]; w.B_hi = h->dZ1p[n][0]; w.B_lo = h->dZ1p[n][1];
@@ -428,15 +432,14 @@ int build_groups(b2g_sac* h) {
           const int* rows[4] = {crow[0], dz2row, dz3row, row512b};
           const int nrows[4] = {B * H1 * W1, B * H2 * W2, B * H3 * W3, B};
           const int Ns[4] = {32, 64, 64, 512};
-          const char* bn[4] = {"/cnn1/b", "/cnn2/b", "/cnn3/b", "/cnn_fc1/b"};
           for (int l = 0; l < 4; ++l) {
             const int rows_per_cta = 8 * (256 / (Ns[l] / 4));
             const int ctas = (nrows[l] + rows_per_cta - 1) / rows_per_cta;
             if (l == 3) {       // cnn_fc1 bias: ready as soon as dZ4 exists -> part of the early all-reduce range
-              early.push_back(ColsumJob{srcs[l], rows[l], h->g(nn(n, bn[l])), nrows[l], Ns[l], estart});
+              early.push_back(ColsumJob{srcs[l], rows[l], h->g(ct(n, l, "b")), nrows[l], Ns[l], estart});
               estart += ctas;
             } else {
-              jobs.push_back(ColsumJob{srcs[l], rows[l], h->g(nn(n, bn[l])), nrows[l], Ns[l], start});
+              jobs.push_back(ColsumJob{srcs[l], rows[l], h->g(ct(n, l, "b")), nrows[l], Ns[l], start});
               start += ctas;
             }
           }
@@ -490,22 +493,21 @@ int build_groups(b2g_sac* h) {
                        GG_COLSUM);
       w0.colsum = h->g(std::string(hp[q]) + "/fc0/bias");
       g.host.push_back(w0);
-      GemmDesc w1 = gemm_desc(h->a0[q], iH, rowH, h->dz1[q], rowH, iH, h->g(std::string(hp[q]) + "/fc1/kernel"), kH, iH, H, H, B, GG_COLSUM);
-      w1.colsum = h->g(std::string(hp[q]) + "/fc1/bias");
+      GemmDesc w1 = gemm_desc(h->a0[q], iH, rowH, h->dz1[q], rowH, iH, h->g(h->fc1(hp[q]) + "/kernel"), kH, iH, H, H, B, GG_COLSUM);
+      w1.colsum = h->g(h->fc1(hp[q]) + "/bias");
       g.host.push_back(w1);
     }
     // heads_wgrad must run before heads_dgrad? no dependency; keep it first in the backward list
     h->bwd_groups.insert(h->bwd_groups.begin(), g);
   }
   if (h->use_planes) {
-    const char* lname[4] = {"/cnn1/w", "/cnn2/w", "/cnn3/w", "/cnn_fc1/w"};
     const int Rs[4] = {64 * h->Cimg, 512, 576, 1024}, Ns[4] = {32, 64, 64, 512};
     std::vector<PlaneJob> jobs;
     int start = 0;
     for (int n = 0; n < 3; ++n)
       for (int l = 0; l < 4; ++l) {
         PlaneJob j{};
-        j.src = h->p(std::string(nets[n]) + lname[l]);
+        j.src = h->p(h->cnn_t(nets[n], l, "w"));
         j.hi = h->wp[n][l][0]; j.lo = h->wp[n][l][1]; j.hiT = h->wp[n][l][2]; j.loT = h->wp[n][l][3];
         j.R = Rs[l]; j.N = Ns[l]; j.tile_start = start;
         start += ((j.R + 31) / 32) * ((j.N + 31) / 32);
@@ -553,15 +555,15 @@ HeadW head_w(b2g_sac* h, const std::string& pre, const std::string& out) {
   HeadW w;
   w.k0 = h->p(pre + "/fc0/kernel");
   w.b0 = h->p(pre + "/fc0/bias");
-  w.k1 = h->p(pre + "/fc1/kernel");
-  w.b1 = h->p(pre + "/fc1/bias");
+  w.k1 = h->p(h->fc1(pre) + "/kernel");
+  w.b1 = h->p(h->fc1(pre) + "/bias");
   w.ko = h->p(pre + "/" + out + "/kernel");
   w.bo = h->p(pre + "/" + out + "/bias");
   return w;
 }
 HeadG head_g(b2g_sac* h, const std::string& pre, const std::string& out) {
   HeadG g;
-  g.b1 = h->g(pre + "/fc1/bias");
+  g.b1 = h->g(h->fc1(pre) + "/bias");
   g.ko = h->g(pre + "/" + out + "/kernel");
   g.bo = h->g(pre + "/" + out + "/bias");
   return g;
@@ -621,7 +623,8 @@ GatherArgs make_gather(b2g_sac* h, bool from_replay, bool with_next) {
   g.scale = h->cnn ? 255.f : 1.f;
   g.x_obs = h->x_obs; g.x_next = h->x_next;
   g.x_obs_hi = h->xp[0][0]; g.x_obs_lo = h->xp[0][1]; g.x_next_hi = h->xp[1][0]; g.x_next_lo = h->xp[1][1];
-  g.F_pi = h->F[0]; g.F_v = h->F[1]; g.F_t = h->F[2]; g.FS = h->FS; g.feat_col = 512;
+  g.F_pi = h->F[0]; g.F_v = h->F[1]; g.F_t = h->F[2]; g.FS = h->FS;
+  g.feat_col = h->direct_feature() ? 512 : -1; g.act_col = h->feat_dim;
   g.rew_out = h->rew_n; g.done_out = h->done_n; g.n_act = h->A;
   return g;
 }
@@ -744,8 +747,8 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
   // the bytes) are final after cnn_fc1's backward, so their all-reduce runs on a side stream / second communicator underneath the
   // conv backward (the GEMM grids leave ar_sms SMs to it); only the conv ranges (0.6 MB) are reduced on the critical chain.
   const bool overlap = h->overlap_ar && h->cfg.nranks > 1 && !(h->dp_p2p && apply);
-  const int64_t pi_fc1 = h->tensors[h->tindex.at("model/pi/" + std::string(h->cnn ? "cnn_fc1/w" : "fc0/kernel"))].off;
-  const int64_t v_fc1 = h->tensors[h->tindex.at("model/values_fn/" + std::string(h->cnn ? "cnn_fc1/w" : "vf/fc0/kernel"))].off;
+  const int64_t pi_fc1 = h->tensors[h->tindex.at(h->cnn ? h->cnn_t("model/pi", 3, "w") : "model/pi/fc0/kernel")].off;
+  const int64_t v_fc1 = h->tensors[h->tindex.at(h->cnn ? h->cnn_t("model/values_fn", 3, "w") : "model/values_fn/vf/fc0/kernel")].off;
   auto nccl_ck = [&](int rc) -> int {
     if (rc != 0) return b2g_fail(B2G_ENCCL, std::string("nccl: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "?"));
     return 0;
@@ -772,7 +775,7 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
       wa.a0[q] = h->a0[q]; wa.dz1[q] = h->dz1[q];
       wa.M0[q] = q >= 2 ? h->feat_dim + h->A : h->feat_dim;
       wa.g_k0[q] = h->g(std::string(hp[q]) + "/fc0/kernel"); wa.g_b0[q] = h->g(std::string(hp[q]) + "/fc0/bias");
-      wa.g_k1[q] = h->g(std::string(hp[q]) + "/fc1/kernel"); wa.g_b1[q] = h->g(std::string(hp[q]) + "/fc1/bias");
+      wa.g_k1[q] = h->g(h->fc1(hp[q]) + "/kernel"); wa.g_b1[q] = h->g(h->fc1(hp[q]) + "/bias");
     }
     wa.x0_ld = h->FS; wa.B = h->B; wa.H = h->H;
     heads_wgrad_launch(wa, lx); ++n; if (!fork) mark("heads_wgrad");
@@ -934,8 +937,8 @@ int find_tensor(const b2g_sac* h, const char* name) {
 int full_index(const b2g_sac* h, int e) {
   if (!h->cnn) return e;
   const int Ci = h->Cimg, npx = h->Hi * h->Wi * Ci;
-  if (e < npx) return (e / Ci) * (Ci + 1) + e % Ci;
-  return e == npx ? Ci : -1;
+  if (e < npx) return (e / Ci) * h->Cobs + e % Ci;
+  return e == npx && h->direct_feature() ? Ci : -1;
 }
 
 // next frame id; a frame that would overwrite one a live transition references drops the oldest transitions first
@@ -1015,7 +1018,7 @@ int load_rows(b2g_sac* h, const float* src, float* dst, long long first, long lo
   for (long long i = 0; i < n; i += h->stage_rows) {
     const int m = (int)std::min<long long>(h->stage_rows, n - i);
     CK(cudaMemcpyAsync(h->obs_stage, src + i * E, m * E * sizeof(float), cudaMemcpyDefault, h->stream));
-    compact_rows(h->obs_stage, dst, first + i, wrap, m, h->Hi * h->Wi, h->Cimg + 1, h->stream);
+    compact_rows(h->obs_stage, dst, first + i, wrap, m, h->Hi * h->Wi, h->Cimg, h->Cobs, h->stream);
   }
   return 0;
 }
@@ -1113,7 +1116,7 @@ int b2g_sac_dp_connect(b2g_sac* h, const void* all_exports, int nranks) {
   h->dp_skip[0][0] = h->dp_skip[0][1] = h->dp_skip[1][0] = h->dp_skip[1][1] = 0;
   if (h->v2.on) {
     const int n_train4 = (int)((h->n_pi + h->n_values + h->n_ent) >> 2), per4 = (n_train4 + nranks - 1) / nranks;
-    const char* names[2] = {"model/pi/cnn_fc1/w", "model/values_fn/cnn_fc1/w"};
+    const std::string names[2] = {h->cnn_t("model/pi", 3, "w"), h->cnn_t("model/values_fn", 3, "w")};
     for (int k = 0; k < 2; ++k) {
       const float* gp = h->g(names[k]);
       const auto& t = h->tensors[h->tindex.at(names[k])];
@@ -1178,14 +1181,25 @@ int b2g_sac_destroy(b2g_sac* h) {
 int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out) { return b2g_sac_create2(cfg, nullptr, out); }
 
 int b2g_sac_create2(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, b2g_sac** out) {
+  return b2g_sac_create3(cfg, replay, nullptr, out);
+}
+
+int b2g_sac_create3(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, const b2g_sac_net_cfg* net, b2g_sac** out) {
   if (!cfg || !out) return b2g_fail(B2G_EINVAL, "cfg/out is NULL");
   *out = nullptr;
+  const int extractor = net ? net->extractor : B2G_CNN_AUGMENTED;
+  if (extractor != B2G_CNN_AUGMENTED && extractor != B2G_CNN_NATURE)
+    return b2g_fail(B2G_EINVAL, "unknown extractor (B2G_CNN_AUGMENTED or B2G_CNN_NATURE)");
+  if (extractor == B2G_CNN_NATURE && cfg->obs_h <= 0)
+    return b2g_fail(B2G_EINVAL, "B2G_CNN_NATURE is a CNN extractor: the MLP policy (obs_h == 0) has none");
+  const bool nature = extractor == B2G_CNN_NATURE;
+  const int n_img = nature ? cfg->obs_c : cfg->obs_c - 1;      // image planes conv1 reads
   if (replay && replay->frame_capacity < cfg->buffer_capacity + 1)
     return b2g_fail(B2G_EINVAL, "frame_capacity must be at least buffer_capacity + 1");
   if (replay && replay->u8_plane_mask && cfg->obs_h <= 0) return b2g_fail(B2G_EINVAL, "the MLP policy has no 8-bit image planes");
-  if (replay && replay->u8_plane_mask &&
-      (cfg->obs_c < 2 || cfg->obs_c - 1 > 8 || (replay->u8_plane_mask >> (cfg->obs_c - 1)) != 0))
-    return b2g_fail(B2G_EINVAL, "u8_plane_mask may only name image planes, at most 8 (the actuator plane is the last channel)");
+  if (replay && replay->u8_plane_mask && (n_img < 1 || n_img > 8 || (replay->u8_plane_mask >> n_img) != 0))
+    return b2g_fail(B2G_EINVAL, nature ? "u8_plane_mask may only name image planes (below obs_c), at most 8"
+                                       : "u8_plane_mask may only name image planes, at most 8 (the actuator plane is the last channel)");
   if (cfg->hidden != 64 && cfg->hidden != 128 && cfg->hidden != 192 && cfg->hidden != 256)
     return b2g_fail(B2G_EINVAL, "hidden must be 64, 128, 192 or 256 (SAC.layers [H, H])");
   if (cfg->n_act < 1 || cfg->n_act > 8) return b2g_fail(B2G_EINVAL, "n_act must be in [1,8]");
@@ -1201,10 +1215,13 @@ int b2g_sac_create2(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, b2g_sa
   h->num_sms = num_sms;
   h->cfg.nccl_id = nullptr; h->cfg.nccl_lib = nullptr;
   h->cnn = cfg->obs_h > 0;
+  h->extractor = extractor;
+  h->cnn_scope = kCnnScopes[nature ? 1 : 0];
   h->B = cfg->batch; h->A = cfg->n_act; h->H = cfg->hidden;
   if (h->cnn) {
-    if (cfg->obs_c < 2) { delete h; return b2g_fail(B2G_EINVAL, "CNN policy needs obs_c >= 2 (image planes + feature plane)"); }
-    h->Cimg = cfg->obs_c - 1; h->Hi = cfg->obs_h; h->Wi = cfg->obs_w;
+    if (!nature && cfg->obs_c < 2) { delete h; return b2g_fail(B2G_EINVAL, "CNN policy needs obs_c >= 2 (image planes + feature plane)"); }
+    if (nature && (cfg->obs_c < 1 || cfg->obs_c > 8)) { delete h; return b2g_fail(B2G_EINVAL, "nature_cnn needs obs_c in [1, 8]"); }
+    h->Cimg = n_img; h->Cobs = cfg->obs_c; h->Hi = cfg->obs_h; h->Wi = cfg->obs_w;
     h->H1 = (h->Hi - 8) / 4 + 1; h->W1 = (h->Wi - 8) / 4 + 1;
     h->H2 = (h->H1 - 4) / 2 + 1; h->W2 = (h->W1 - 4) / 2 + 1;
     h->H3 = h->H2 - 2; h->W3 = h->W2 - 2;
@@ -1214,7 +1231,7 @@ int b2g_sac_create2(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, b2g_sa
     }
     h->E = h->Hi * h->Wi * cfg->obs_c;
     h->Ec = h->Hi * h->Wi * h->Cimg + 4;
-    h->feat_dim = 513;
+    h->feat_dim = nature ? 512 : 513;
   } else {
     if (cfg->obs_dim < 1) { delete h; return b2g_fail(B2G_EINVAL, "obs_dim must be positive for the MLP policy"); }
     h->E = h->Ec = cfg->obs_dim;
@@ -1687,6 +1704,21 @@ void compact_host(const float* src, float* dst, int n, int HW, int Cfull, int Ec
     d[HW * Ci] = s[Ci]; d[HW * Ci + 1] = 0.f; d[HW * Ci + 2] = 0.f; d[HW * Ci + 3] = 0.f;
   }
 }
+
+// the plain nature_cnn's compact rows: the whole observation [HW][C], then 4 zero floats
+void copy_rows_host(const float* src, float* dst, int n, int E, int Ec, int threads) {
+#pragma omp parallel for num_threads(threads) schedule(static)
+  for (int b = 0; b < n; ++b) {
+    float* d = dst + (size_t)b * Ec;
+    memcpy(d, src + (size_t)b * E, (size_t)E * sizeof(float));
+    d[E] = d[E + 1] = d[E + 2] = d[E + 3] = 0.f;
+  }
+}
+
+void rows_host(const b2g_sac* h, const float* src, float* dst) {
+  if (h->direct_feature()) compact_host(src, dst, h->B, h->Hi * h->Wi, h->Cobs, h->Ec, h->host_threads);
+  else copy_rows_host(src, dst, h->B, h->E, h->Ec, h->host_threads);
+}
 }  // namespace
 
 int b2g_debug_compact_host(const float* src, float* dst, int n, int hw, int cfull, int threads) {
@@ -1757,9 +1789,9 @@ int b2g_sac_step_host_pipelined(b2g_sac* h, const float* obs, const float* act, 
       if (const char* e = getenv("B2G_HOST_THREADS")) h->host_threads = std::max(1, atoi(e));
     }
     if (k >= 2) CK(cudaEventSynchronize(h->ev_h2d[j]));          // the copy out of this staging slot two calls ago
-    compact_host(obs, h->hc_obs[j], (int)B, h->Hi * h->Wi, h->Cimg + 1, h->Ec, h->host_threads);
+    rows_host(h, obs, h->hc_obs[j]);
     CK(cudaMemcpyAsync(h->ps_obs[j], h->hc_obs[j], B * h->Ec * sizeof(float), cudaMemcpyHostToDevice, h->cstream));     // flies while next_obs is compacted
-    compact_host(next_obs, h->hc_next[j], (int)B, h->Hi * h->Wi, h->Cimg + 1, h->Ec, h->host_threads);
+    rows_host(h, next_obs, h->hc_next[j]);
     CK(cudaMemcpyAsync(h->ps_next[j], h->hc_next[j], B * h->Ec * sizeof(float), cudaMemcpyHostToDevice, h->cstream));
   } else {
     CK(cudaMemcpyAsync(h->ps_obs[j], obs, B * E * sizeof(float), cudaMemcpyHostToDevice, h->cstream));
@@ -1880,6 +1912,13 @@ std::vector<FpField> sac_fingerprint(const b2g_sac* h) {
           fp_real("target_entropy", c.target_entropy), fp_int("seed", (int64_t)c.seed)};
 }
 
+// the augmented and MLP fingerprints carry no extractor field, so their files keep the layout they had before nature_cnn existed
+std::vector<FpField> sac_fingerprint(const b2g_sac* h, int extractor) {
+  std::vector<FpField> fp = sac_fingerprint(h);
+  if (extractor == B2G_CNN_NATURE) fp.push_back(fp_int("extractor", extractor));
+  return fp;
+}
+
 // Host replay bookkeeping as stored: r_size, head_seq, tail_seq, next_fid, evicted, |lw|, |prev_next|, lw pairs, prev_next.
 struct SacHostState {
   int64_t r_size = 0, head_seq = 0, tail_seq = 0, next_fid = 0, evicted = 0;
@@ -1948,7 +1987,7 @@ int b2g_sac_state_save(b2g_sac* h, const char* path) {
   hv.insert(hv.end(), hs.prev_next.begin(), hs.prev_next.end());
   std::vector<StateSection> secs = host_sections(hv.data(), hv.size() * sizeof(int64_t), cnt, sizeof cnt);
   for (auto& s : sac_device_sections(h, hs.frame_lo(h->frame_cap), hs.next_fid)) secs.push_back(std::move(s));
-  return state_write(path, STATE_KIND_SAC, fp_with_rms(sac_fingerprint(h), h->rms_mean), secs);
+  return state_write(path, STATE_KIND_SAC, fp_with_rms(sac_fingerprint(h, h->extractor), h->rms_mean), secs);
 }
 
 int b2g_sac_state_load(b2g_sac* h, const char* path) {
@@ -1960,7 +1999,16 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
   CK(cudaSetDevice(h->cfg.device));
   // ---- everything is checked before the handle changes
   StateReader rd;
-  if (int rc = state_open_rms(rd, path, STATE_KIND_SAC, sac_fingerprint(h), h->rms_mean, "b2g_obs_rms_set")) return rc;
+  if (int rc = state_open_rms(rd, path, STATE_KIND_SAC, sac_fingerprint(h, h->extractor), h->rms_mean, "b2g_obs_rms_set")) {
+    const std::string msg = g_b2g_err;
+    StateReader other;      // a file of the other CNN extractor: say so
+    const int ext2 = h->extractor == B2G_CNN_NATURE ? B2G_CNN_AUGMENTED : B2G_CNN_NATURE;
+    if (h->cnn && other.open(path, STATE_KIND_SAC, fp_with_rms(sac_fingerprint(h, ext2), h->rms_mean)) == 0)
+      return b2g_fail(B2G_EINVAL, std::string("the state file was written by a handle of the ") +
+                                      (ext2 == B2G_CNN_NATURE ? "nature_cnn" : "augmented") + " extractor; this handle runs the " +
+                                      (ext2 == B2G_CNN_NATURE ? "augmented" : "nature_cnn") + " one");
+    return b2g_fail(rc, msg);
+  }
   if (int rc = state_check_tags(rd, sac_device_sections(h, 0, 0), "SAC")) return rc;
   const int64_t cap = h->cfg.buffer_capacity, FC = h->frame_cap;
   if (rd.bytes(0) % 8 || rd.bytes(0) < 7 * 8 || rd.bytes(0) > (uint64_t)(7 + 2 * cap + 4 * FC) * 8)

@@ -118,7 +118,7 @@ struct b2g_sac {
   std::vector<void*> allocs;
   // Raw (un-normalised) observations travel as compact rows of Ec floats.  MLP policy: Ec = E.  CNN policy: COMPACT rows
   // (replay.cu), Ec = H*W*Cimg + 4: the image planes, the ONE actuator value the policy reads (pixel [0,0] of the last plane;
-  // augmented_nature_cnn never reads the rest of it, custom_obs_policy.py:28-30) and 3 pad floats.  The explicit batch
+  // augmented_nature_cnn never reads the rest of it, custom_obs_policy.py:28-30; zero under B2G_CNN_NATURE) and 3 pad floats.  The explicit batch
   // (s_obs / s_next) and the pipelined staging (ps_obs / ps_next) hold such rows.
   int Ec = 0;
   // Replay: a ring of cap transition slots {obs frame, next_obs frame, act, rew, done} over a pool of frame_cap frames (one
@@ -234,6 +234,19 @@ struct b2g_sac {
   std::vector<int64_t> ob_fid;
   int ob_n = 0;
   int64_t up_observe = 0, up_other = 0;                   // host->device bytes: observe_* / act + replay_add + set_norm_stats
+
+  // CNN extractor (b2g_sac_net_cfg): B2G_CNN_AUGMENTED reads Cimg = obs_c - 1 planes plus the direct feature at column 512 of
+  // the feature rows; B2G_CNN_NATURE reads Cimg = obs_c planes and has no direct feature.  Cobs = channels of a caller
+  // observation.  cnn_scope: the extractor's layer scopes conv1, conv2, conv3, fc1 (sac.cu).
+  int extractor = 0, Cobs = 0;
+  const char* const* cnn_scope = nullptr;
+  bool direct_feature() const { return cnn && extractor == B2G_CNN_AUGMENTED; }
+  std::string cnn_t(const std::string& net, int layer, const char* wb) const { return net + "/" + cnn_scope[layer] + "/" + wb; }
+  // scope of a head MLP's second layer: nature_cnn opens 'fc1' in model/pi before mlp() creates its dense layers there, so TF1
+  // names the actor's second layer fc1_1 (INTEGRATION.md, "nature_cnn tensor names")
+  std::string fc1(const std::string& head) const {
+    return head + (cnn && extractor == B2G_CNN_NATURE && head == "model/pi" ? "/fc1_1" : "/fc1");
+  }
 
   float* p(const std::string& n) { return P + tensors[tindex.at(n)].off; }
   float* g(const std::string& n) { return G + tensors[tindex.at(n)].off; }

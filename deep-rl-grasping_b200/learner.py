@@ -177,10 +177,15 @@ class Learner(HandleLearner):
                  buffer_size: int = 100000, gamma: float = 0.99, tau: float = 0.005,
                  target_entropy: Optional[float] = None, seed: int = 0, precision: int = _lib.B2G_PREC_FP32_SIMT,
                  device: int = 0, rank: int = 0, nranks: int = 1, nccl_id: Optional[bytes] = None,
-                 frame_capacity: Optional[int] = None, u8_planes: Sequence[int] = ()):
+                 frame_capacity: Optional[int] = None, u8_planes: Sequence[int] = (), extractor: str = "augmented"):
         """frame_capacity / u8_planes: replay storage (include/b200grasp.h, b2g_replay_cfg).  None and () keep two fp32
         frames per replay slot; a smaller frame budget shares each obs with the previous row's next_obs when they are
-        equal, and u8_planes lists image channels stored as one byte per pixel (values must be integers in [0, 255])."""
+        equal, and u8_planes lists image channels stored as one byte per pixel (values must be integers in [0, 255]).
+        extractor: the CNN policy's feature extractor, "augmented" (create_augmented_nature_cnn(1): the last plane is the
+        actuator feature) or "nature_cnn" (stable-baselines' plain nature_cnn over every plane; b2g_sac_net_cfg)."""
+        if extractor not in _lib.EXTRACTORS:
+            raise ValueError(f"extractor must be one of {sorted(_lib.EXTRACTORS)} (got {extractor!r})")
+        self.extractor = extractor
         self.lib = _lib.load()
         self.obs_shape = tuple(int(s) for s in obs_shape)
         self.n_act, self.batch_size = int(n_act), int(batch_size)
@@ -207,7 +212,8 @@ class Learner(HandleLearner):
                 raise ValueError(f"u8_planes must be channel indices (got {self.u8_planes})")
             rcfg = _lib.ReplayCfg(2 * int(buffer_size) if self.frame_capacity is None else self.frame_capacity,
                                   sum(1 << c for c in set(self.u8_planes)))
-        _lib.check(self.lib.b2g_sac_create2(C.byref(cfg), None if rcfg is None else C.byref(rcfg), C.byref(self.h)))
+        ncfg = _lib.SacNetCfg(_lib.EXTRACTORS[extractor])
+        _lib.check(self.lib.b2g_sac_create3(C.byref(cfg), None if rcfg is None else C.byref(rcfg), C.byref(ncfg), C.byref(self.h)))
         self.obs_elems = int(np.prod(self.obs_shape))
         self._info = OrderedDict()
         name, numel, ndim = C.c_char_p(), C.c_int64(), C.c_int32()

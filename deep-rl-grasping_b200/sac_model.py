@@ -16,7 +16,7 @@ from typing import Optional
 
 import numpy as np
 
-from . import _lib, training_state
+from . import _lib, sb_io, training_state
 from .base_model import BaseModel, unwrap_vec_normalize  # noqa: F401  (unwrap_vec_normalize: also imported from here)
 from .callbacks import as_callback
 from .learner import Learner
@@ -40,6 +40,22 @@ def head_width(layers) -> int:
     if len(layers) != 2 or layers[0] != layers[1] or layers[0] not in HEAD_WIDTHS:
         raise NotImplementedError(f"SAC.layers must be [H, H] with H in {list(HEAD_WIDTHS)} (got {layers})")
     return layers[0]
+
+
+def extractor_of(cnn_extractor) -> str:
+    """policy_kwargs['cnn_extractor'] -> the learner's extractor: stable-baselines' plain ``nature_cnn`` (the sentinel
+    ``b200grasp.common.policies.nature_cnn``, or the string "nature_cnn" a training state stores); any other value means
+    ``create_augmented_nature_cnn(1)``."""
+    from .common.policies import nature_cnn
+    return "nature_cnn" if cnn_extractor is nature_cnn or cnn_extractor == "nature_cnn" else "augmented"
+
+
+def zip_extractor(params):
+    """The CNN extractor a parameter dict was written by (conv1's variable name), or None for an MLP policy."""
+    names = {n[:-2] if n.endswith(":0") else n for n in params}
+    if "model/pi/c1/w" in names:
+        return "nature_cnn"
+    return "augmented" if "model/pi/cnn1/w" in names else None
 
 
 def _constfn(v):
@@ -87,6 +103,7 @@ class SAC(BaseModel):
         self.device_obs_norm = bool(device_obs_norm)
         self._dev = dict(device=device, rank=rank, nranks=nranks, nccl_id=nccl_id)
         self._layout_from_zip = False
+        self.extractor = extractor_of(self.policy_kwargs.get("cnn_extractor"))
         self.num_timesteps, self.n_updates = 0, 0
         self.episode_rewards = [0.0]
         self.ep_info_buf = deque(maxlen=100)
@@ -109,19 +126,24 @@ class SAC(BaseModel):
         n_act = int(np.prod(self.action_space.shape))
         if len(obs_shape) == 3 and "cnn_extractor" not in self.policy_kwargs and not self._layout_from_zip:
             # sb_helper.py:93-95: CnnPolicy with policy_kwargs={} means stable-baselines' plain nature_cnn over ALL planes and
-            # no direct feature -- a different network (and different zip variables) from augmented_nature_cnn.  Refuse
-            # instead of silently building the augmented extractor.  (SAC.load knows the layout from the zip itself.)
+            # no direct feature -- a different network (and different zip variables) from augmented_nature_cnn.  The
+            # extractor is asked for by name instead of by omission.  (SAC.load knows the layout from the zip itself.)
             raise NotImplementedError("CnnPolicy without policy_kwargs['cnn_extractor'] selects stable-baselines' plain nature_cnn "
-                                      "(simplified + depth branch, sb_helper.py:93-95), which is not built; pass "
+                                      "(simplified + depth branch, sb_helper.py:93-95); pass cnn_extractor=nature_cnn "
+                                      "(b200grasp.common.policies) for that network, or "
                                       "cnn_extractor=create_augmented_nature_cnn(1) as sb_helper.py:88-91 does")
         tgt = -float(n_act) if self.target_entropy == "auto" else float(self.target_entropy)
         self.learner = Learner(obs_shape, n_act=n_act, hidden=self.hidden, batch_size=self.batch_size, buffer_size=self.buffer_size,
                                gamma=self.gamma, tau=self.tau, target_entropy=tgt, seed=int(self.seed or 0),
                                precision=_PRECISIONS[self.precision], frame_capacity=self.replay_frames,
-                               u8_planes=self.replay_u8_planes, **self._dev)
+                               u8_planes=self.replay_u8_planes, **self._net_kwargs(obs_shape), **self._dev)
         self._init_parameters()
         self._attach_device_norm()
         self._sync_norm_stats()
+
+    def _net_kwargs(self, obs_shape):
+        """Learner's extractor argument: only the plain nature_cnn departs from the default."""
+        return {"extractor": "nature_cnn"} if len(obs_shape) == 3 and self.extractor == "nature_cnn" else {}
 
     def _init_parameters(self):
         """[SB2] ortho_init(sqrt 2) for conv/linear, Glorot-uniform for tf.layers.dense, zero biases,
@@ -142,6 +164,17 @@ class SAC(BaseModel):
             else:
                 p[name] = np.zeros(shape, np.float32)
         self.learner.load_parameters(p)
+
+    def load_parameters(self, load_path_or_dict, exact_match=True):
+        """A donor of the other CNN extractor is refused before any variable is written (its head fc0 kernels differ in
+        shape, so even exact_match=False would leave the learner half loaded)."""
+        params = load_path_or_dict
+        if isinstance(params, str):
+            _, params = sb_io.load_sb_zip(params)
+        theirs = zip_extractor(params)
+        if len(self.observation_space.shape) == 3 and theirs is not None and theirs != self.extractor:
+            raise ValueError(f"the parameters belong to the {theirs} extractor; this model's CNN policy is {self.extractor}")
+        super().load_parameters(params, exact_match=exact_match)
 
     def _sync_norm_stats(self):
         vn = self._vec_normalize_env
@@ -293,8 +326,8 @@ class SAC(BaseModel):
     def _host_state(self):
         kw = self.policy_kwargs.get("cnn_extractor")
         policy_kwargs = dict(self.policy_kwargs)
-        if kw is not None and not isinstance(kw, str):
-            policy_kwargs["cnn_extractor"] = "augmented_nature_cnn"      # the one extractor the learner builds
+        if kw is not None and not isinstance(kw, str):         # the extractor by name (the learner builds these two)
+            policy_kwargs["cnn_extractor"] = "nature_cnn" if self.extractor == "nature_cnn" else "augmented_nature_cnn"
         if callable(self.learning_rate):
             raise NotImplementedError("save_training_state needs a constant learning_rate")
         init = dict(gamma=self.gamma, learning_rate=self.learning_rate, buffer_size=self.buffer_size, learning_starts=self.learning_starts,
@@ -326,7 +359,10 @@ class SAC(BaseModel):
         trained_models/SAC_depth_1mbuffer/best_model/best_model.zip)."""
         from .spaces import Box
         data, params = cls._read_zip(load_path)
-        if "model/pi/cnn1/w" in params:
+        extractor = zip_extractor(params)
+        if extractor == "nature_cnn":         # nature_cnn's conv1 reads every plane
+            obs_space = Box(0.0, 255.0, (64, 64, params["model/pi/c1/w"].shape[2]))
+        elif extractor == "augmented":
             obs_space = Box(0.0, 255.0, (64, 64, params["model/pi/cnn1/w"].shape[2] + 1))
         else:
             obs_space = Box(-np.inf, np.inf, (params["model/pi/fc0/kernel"].shape[0],))
@@ -345,10 +381,14 @@ class SAC(BaseModel):
         kw.update(kwargs)
         # the head widths are the zip's own: the actor's fc0 / fc1 kernels give [H1, H2], and SAC's constructor refuses any
         # layers the learner cannot build (unequal widths included) with the message that names the supported ones
-        layers = [int(params["model/pi/fc0/kernel"].shape[1]), int(params["model/pi/fc1/kernel"].shape[1])]
+        # (nature_cnn's actor names its second layer fc1_1: learner.py, INTEGRATION.md)
+        fc1 = "model/pi/fc1_1/kernel" if extractor == "nature_cnn" else "model/pi/fc1/kernel"
+        layers = [int(params["model/pi/fc0/kernel"].shape[1]), int(params[fc1].shape[1])]
         if "model/pi/fc2/kernel" in params:
             layers.append(int(params["model/pi/fc2/kernel"].shape[1]))
-        model = cls(policy=data.get("policy", "CnnPolicy"), env=None, _init_setup_model=False,
-                    policy_kwargs={"layers": layers}, **kw)
+        pkw = {"layers": layers}
+        if extractor == "nature_cnn":
+            pkw["cnn_extractor"] = "nature_cnn"
+        model = cls(policy=data.get("policy", "CnnPolicy"), env=None, _init_setup_model=False, policy_kwargs=pkw, **kw)
         model._layout_from_zip = True
         return model._finish_load(env, obs_space, Box(-1.0, 1.0, (params["model/pi/dense/kernel"].shape[1],)), params)

@@ -128,7 +128,12 @@ def train(args):
             env = VecNormalize(env, norm_obs=True, norm_reward=True, clip_obs=10.0)
     c = config[algo]
     if algo == "SAC":
-        if _is_image_obs(env):
+        simplified_image = _is_image_obs(env) and bool(config.get("simplified", False))
+        if simplified_image:
+            # sb_helper.py:92-94: CnnPolicy with policy_kwargs={}, i.e. stable-baselines' plain nature_cnn over every plane
+            # and the default [64, 64] head, whatever the config's layers say
+            policy, kw = CnnPolicy, {"cnn_extractor": "nature_cnn"}
+        elif _is_image_obs(env):
             policy, kw = CnnPolicy, {"layers": c["layers"], "cnn_extractor": "augmented_nature_cnn"}
         else:
             policy, kw = MlpPolicy, {"layers": c["layers"], "layer_norm": False}
@@ -136,8 +141,10 @@ def train(args):
         if args.replay_spare is not None:
             # every transition holds one frame of its own plus one per episode end; n_envs more for the rows in flight
             replay["replay_frames"] = int(c["buffer_size"] * (1.0 + args.replay_spare)) + n_envs
-        if _is_image_obs(env) and config.get("full_observation", False):
-            replay["replay_u8_planes"] = (0, 1, 2)        # RGB renders as uint8 (gripperEnv/sensor.py), depth stays fp32
+        if _is_image_obs(env) and config.get("full_observation", False) and not simplified_image:
+            # RGB renders as uint8 (gripperEnv/sensor.py), depth stays fp32; the simplified observation is depth + pad even
+            # under full_observation (robot.py:192-196), so it has no 8-bit planes
+            replay["replay_u8_planes"] = (0, 1, 2)
         if args.device_norm:
             replay["device_obs_norm"] = True
         model = SAC(policy, env, policy_kwargs=kw, verbose=1, gamma=config["discount_factor"], buffer_size=c["buffer_size"],

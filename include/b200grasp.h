@@ -79,7 +79,7 @@ int b2g_nccl_unique_id(void* out128, const char* nccl_lib);
  * episodic streams need about cap * (1 + episode ends / transitions) + n_envs frames.  When a new frame would overwrite one a
  * live transition still references, the oldest transitions are dropped early (b2g_replay_info counts them) and sampling stays
  * uniform over the live ones.
- * u8_plane_mask: bit c declares image channel c (CNN policy, c < obs_c - 1) an 8-bit plane, stored as one byte per pixel;
+ * u8_plane_mask: bit c declares image channel c (CNN policy, c < obs_c - 1; c < obs_c under B2G_CNN_NATURE) an 8-bit plane, stored as one byte per pixel;
  * b2g_replay_add then refuses (B2G_EINVAL, nothing stored) any value there that is not an integer in [0, 255].
  * NULL (the default) = frame_capacity 2 * buffer_capacity and no 8-bit planes.  From 2 * buffer_capacity frames on, every
  * transition keeps two frames of its own (sharing would save nothing): the bytes of two rows per transition, and nothing is
@@ -89,8 +89,22 @@ typedef struct b2g_replay_cfg {
   uint32_t u8_plane_mask;
 } b2g_replay_cfg;
 
+/* The CNN policy's feature extractor.
+ * B2G_CNN_AUGMENTED: create_augmented_nature_cnn(1) (custom_obs_policy.py): conv1 reads the first obs_c - 1 planes, pixel
+ *   [0,0] of the last plane is one direct feature, 513 features; tensors model/pi/cnn1/w .. cnn_fc1/b.
+ * B2G_CNN_NATURE: stable-baselines' plain nature_cnn (common/policies.py), the simplified environment's CnnPolicy: conv1 reads
+ *   all obs_c planes (1 .. 8), no direct feature, 512 features; tensors model/pi/c1/w, c1/b, c2/w, c2/b, c3/w, c3/b, fc1/w (1024,512), fc1/b.
+ *   u8_plane_mask may name any plane below obs_c.  The 4-float tail of a compact replay row is zero. */
+enum { B2G_CNN_AUGMENTED = 0, B2G_CNN_NATURE = 1 };
+typedef struct b2g_sac_net_cfg {
+  int32_t extractor;           /* B2G_CNN_AUGMENTED or B2G_CNN_NATURE (CNN policy only: obs_h > 0)  */
+} b2g_sac_net_cfg;
+
 int b2g_sac_create(const b2g_sac_cfg* cfg, b2g_sac** out);   /* = b2g_sac_create2(cfg, NULL, out) */
-int b2g_sac_create2(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay /* NULL = default */, b2g_sac** out);
+int b2g_sac_create2(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay /* NULL = default */, b2g_sac** out);   /* = create3(.., NULL, ..) */
+/* net == NULL: B2G_CNN_AUGMENTED.  B2G_CNN_NATURE with the MLP policy (obs_h == 0), or an unknown extractor: B2G_EINVAL.
+ * A training-state file records the extractor: b2g_sac_state_load refuses a file of the other extractor. */
+int b2g_sac_create3(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, const b2g_sac_net_cfg* net, b2g_sac** out);
 int b2g_sac_destroy(b2g_sac* h);
 /* Peer-memory data parallelism (nranks > 1, one process per GPU of one NVLink node).  Every rank exports B2G_DP_EXPORT_BYTES
  * (CUDA IPC handles of its parameter arena, gradient receive arena and exchange block), the caller gathers the nranks blobs in rank
