@@ -9,8 +9,10 @@ import os
 from collections import OrderedDict
 from typing import Optional
 
+import numpy as np
+
 from . import sb_io, training_state
-from .vec_env import DummyVecEnv, VecNormalize
+from .vec_env import DummyVecEnv, VecNormalize, unwrap_encode_depth
 
 
 def unwrap_vec_normalize(env) -> Optional[VecNormalize]:
@@ -53,6 +55,9 @@ class BaseModel:
         if self.learner is not None:
             if self._owns_obs_rms():
                 self._vec_normalize_env.take_obs_rms_back()
+            ve = unwrap_encode_depth(self.env)
+            if ve is not None and ve.encoder_owner is self.learner:
+                ve.take_encoder_back()
             self.learner.close()
             self.learner = None
 
@@ -73,6 +78,46 @@ class BaseModel:
         vn = self._vec_normalize_env
         if self.device_obs_norm and isinstance(vn, VecNormalize) and vn.norm_obs and not vn.learner_owns_obs_rms:
             vn.give_obs_rms_to(self.learner)
+
+    # ------------------------------------------------------------------ the perception encoder on the device (VecEncodeDepth)
+    def _attach_obs_encoder(self):
+        """device_obs_norm on a stack with a VecEncodeDepth: the learner takes the encoder and the wrapper passes raw depth rows
+        (one upload per frame, encoded on the device).  It stays in host mode while a host VecNormalize above it needs
+        encoded rows, or while another learner has the encoder."""
+        ve = unwrap_encode_depth(self.env)
+        if ve is None or not self.device_obs_norm or ve.encoder_owner is not None:
+            return
+        if self._vec_normalize_env is not None and not self._owns_obs_rms():
+            return
+        self.learner.set_obs_encoder(ve.encoder, ve.tail)
+        ve.give_encoder_to(self.learner)
+
+    def _check_encoded(self, observation):
+        """``predict`` takes encoded observations: a raw depth row of this model's VecEncodeDepth is refused."""
+        ve = unwrap_encode_depth(self.env)
+        if ve is not None and ve.raw_width != ve.observation_space.shape[0] and np.shape(observation)[-1:] == (ve.raw_width,):
+            raise ValueError(f"predict takes encoded observations of {ve.observation_space.shape[0]} floats, got raw rows of "
+                             f"{ve.raw_width}: wrap the env in a host-mode VecEncodeDepth (as the evaluation env is)")
+
+    def _encoder_host(self):
+        """host.json's record of the encoder a learner encodes with: its directory and weight digest (None without one)."""
+        ve = unwrap_encode_depth(self.env)
+        if ve is None or ve.encoder_owner is not self.learner:
+            return None
+        return {"dir": getattr(ve.encoder, "model_dir", None), "digest": ve.encoder.weights_digest()}
+
+    @staticmethod
+    def _check_encoder_digest(path, host, env):
+        want = host.get("obs_encoder")
+        if want is None:
+            return
+        ve = unwrap_encode_depth(env)
+        if ve is None:
+            raise ValueError(f"{path} was trained on the device encoder of {want['dir']}: wrap the env in a VecEncodeDepth")
+        got = ve.encoder.weights_digest()
+        if got != want["digest"]:
+            raise ValueError(f"{path} was trained through encoder weights {want['digest'][:12]} ({want['dir']}); the env's "
+                             f"VecEncodeDepth holds {got[:12]}")
 
     # ------------------------------------------------------------------ parameters / persistence
     def get_parameters(self):
@@ -125,6 +170,7 @@ class BaseModel:
         host = training_state.read_host(path)
         if host.get("algo") != cls._algo:
             raise ValueError(f"{path} holds a {host.get('algo')} training state")
+        cls._check_encoder_digest(path, host, env)
         model = cls(cls._policy_from_host(host), env, **dict(host["init"], **kwargs))
         training_state.restore_vec_normalize(path, model.env)
         model._attach_device_norm()        # the restored statistics go back to the learner; learner.state carries the same ones

@@ -59,7 +59,7 @@ class BDQLearner(HandleLearner):
         observation of env i; ``None`` acts on the ones already staged.  Returns the [n, n_branches] epsilon-greedy bin
         indices, or None with ``act=False``."""
         if obs is not None:
-            obs = _f32(obs).reshape(-1, self.obs_dim)
+            obs = _f32(obs).reshape(-1, self.frame_elems)
             n = obs.shape[0]
             self.obs_rms_version += bool(update_stats)
         out = np.empty((int(n), self.n_branches), np.int32) if act else None
@@ -73,7 +73,7 @@ class BDQLearner(HandleLearner):
         act, next_obs = _f32(act_idx), _f32(next_obs)
         rew, done = _f32(np.reshape(rew, -1)), _f32(np.reshape(done, -1))
         n = rew.shape[0]
-        assert next_obs.size == n * self.obs_dim and act.size == n * self.n_branches and done.size == n
+        assert next_obs.size == n * self.frame_elems and act.size == n * self.n_branches and done.size == n
         if reset_obs is not None:
             reset_obs = _f32(reset_obs)
             assert reset_obs.size == next_obs.size
@@ -175,6 +175,7 @@ class BDQ(BaseModel):
         self.learner.obs_shape = tuple(self.observation_space.shape)
         self._bins = np.linspace(-1.0, 1.0, self.num_actions_pad).astype(np.float32)
         self._attach_device_norm()
+        self._attach_obs_encoder()
 
     def _attach_device_norm(self):
         super()._attach_device_norm()
@@ -247,6 +248,7 @@ class BDQ(BaseModel):
         return self
 
     def predict(self, observation, state=None, mask=None, deterministic=True):
+        self._check_encoded(observation)
         obs = np.asarray(observation, np.float32).reshape(-1, self.learner.obs_dim)
         idx = self.learner.act(obs)
         act = self._bins[idx]
@@ -274,7 +276,11 @@ class BDQ(BaseModel):
                     device=self.device)
         if self.device_obs_norm:
             init["device_obs_norm"] = True
-        return {"algo": "BDQ", "init": init, "num_timesteps": int(self.num_timesteps), "rng": training_state.rng_state(self._rng)}
+        host = {"algo": "BDQ", "init": init, "num_timesteps": int(self.num_timesteps), "rng": training_state.rng_state(self._rng)}
+        enc = self._encoder_host()
+        if enc is not None:
+            host["obs_encoder"] = enc
+        return host
 
     def _restore_host_state(self, host):
         self.num_timesteps = int(host["num_timesteps"])

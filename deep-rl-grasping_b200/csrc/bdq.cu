@@ -24,6 +24,7 @@
 
 #include "../../include/b200grasp.h"
 #include "common.cuh"
+#include "enc_stage.cuh"
 #include "host.cuh"
 #include "per.cuh"
 #include "state.cuh"
@@ -200,6 +201,7 @@ struct b2g_bdq {
   int* ob_idx = nullptr;       // [stage_rows][D] actor output
   int ob_k = 0, ob_n = 0;
   int64_t up_observe = 0, up_other = 0;    // host->device bytes: observe_* / obs_rms_set, and act + replay_add + set_norm_stats
+  EncStage* enc = nullptr;     // b2g_bdq_set_obs_encoder: observe_* take raw rows and encode them into the staged rows
   float* p(const std::string& nm) { return P + params.off(nm); }
   float* g(const std::string& nm) { return G + params.off(nm); }
 };
@@ -393,6 +395,7 @@ int b2g_bdq_destroy(b2g_bdq* h) {
   if (h->stream) cudaStreamSynchronize(h->stream);
   if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
   nccl_comm_destroy(h->nccl_comm);
+  enc_stage_destroy(h->enc);
   for (void* q : h->allocs) cudaFree(q);
   if (h->h_met) cudaFreeHost(h->h_met);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -662,6 +665,43 @@ static void bdq_merge(b2g_bdq* h, const float* a, const float* b, const float* d
   h->rms_count += n;
 }
 
+// the n frames of a call -> rows [n][E] at dst: uploaded as they are or, with an observation encoder, as raw rows it encodes there
+static int bdq_stage_frames(b2g_bdq* h, float* dst, const float* obs, int n) {
+  if (!h->enc) return bdq_upload(h, dst, obs, (size_t)n * h->E * sizeof(float));
+  if (int rc = bdq_upload(h, enc_stage_raw(h->enc, 0), obs, (size_t)n * enc_stage_row_floats(h->enc) * sizeof(float))) return rc;
+  return enc_stage_encode(h->enc, 0, nullptr, n, 0, dst, h->stream);
+}
+
+// the reset frames of the n_done finished envs -> row i of ob_reset; only those cross the bus and, with an observation encoder,
+// only those are encoded (it reads the flags ob_done, uploaded before)
+static int bdq_stage_reset_frames(b2g_bdq* h, const float* reset_obs, const float* done, int n, int n_done) {
+  const size_t rw = h->enc ? enc_stage_row_floats(h->enc) : h->E;
+  float* dst = h->enc ? enc_stage_raw(h->enc, 1) : h->ob_reset;
+  for (int i = 0; i < n; ++i)
+    if (done[i] != 0.f)
+      if (int rc = bdq_upload(h, dst + i * rw, reset_obs + i * rw, rw * sizeof(float))) return rc;
+  return h->enc ? enc_stage_encode(h->enc, 1, h->ob_done, n, n_done, h->ob_reset, h->stream) : 0;
+}
+
+int b2g_bdq_set_obs_encoder(b2g_bdq* h, const b2g_encoder* enc, int tail) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  if (enc) {
+    if (int rc = enc_stage_check(enc, h->cfg.device, tail, h->E)) return rc;
+    if (h->cfg.nranks > 1)
+      return b2g_fail(B2G_ESTATE, "set_obs_encoder: the observe path is per handle: with nranks > 1 every rank would encode its own");
+  }
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  EncStage* st = nullptr;
+  if (enc)
+    if (int rc = enc_stage_create(enc, h->stage_rows, tail, h->stream, &st)) return rc;
+  enc_stage_destroy(h->enc);
+  h->enc = st;
+  h->ob_n = 0;          // staged observations were in the other layout
+  return 0;
+}
+
 static int bdq_observe_checks(b2g_bdq* h, int n, int update_stats) {
   if (n < 1 || n > h->stage_rows)
     return b2g_fail(B2G_EINVAL, "observe: n must be in [1, " + std::to_string(h->stage_rows) + "] (the staging holds max(batch, 256) frames)");
@@ -689,7 +729,7 @@ int b2g_bdq_observe_act(b2g_bdq* h, const float* obs, int n, int update_stats, f
   const size_t E = h->E, D = h->D;
   float* cur = h->ob_rows[h->ob_k];
   if (obs) {
-    if (int rc = bdq_upload(h, cur, obs, n * E * sizeof(float))) return rc;
+    if (int rc = bdq_stage_frames(h, cur, obs, n)) return rc;
     if (update_stats) bdq_merge(h, cur, nullptr, nullptr, n);
     h->ob_n = n;
   }
@@ -725,13 +765,12 @@ int b2g_bdq_observe_add(b2g_bdq* h, const float* act_idx, const float* rew, cons
   const size_t E = h->E, D = h->D, fb = E * sizeof(float);
   float* cur = h->ob_rows[h->ob_k];
   float* nxt = h->ob_rows[h->ob_k ^ 1];
-  if (int rc = bdq_upload(h, nxt, next_obs, n * fb)) return rc;
-  for (int i = 0; i < n; ++i)         // only the frames of finished envs cross the bus
-    if (done[i] != 0.f)
-      if (int rc = bdq_upload(h, h->ob_reset + i * E, reset_obs + i * E, fb)) return rc;
+  if (int rc = bdq_stage_frames(h, nxt, next_obs, n)) return rc;
   if (int rc = bdq_upload(h, h->ob_act, act_idx, n * D * sizeof(float))) return rc;
   if (int rc = bdq_upload(h, h->ob_rew, rew, n * sizeof(float))) return rc;
   if (int rc = bdq_upload(h, h->ob_done, done, n * sizeof(float))) return rc;
+  if (n_done)
+    if (int rc = bdq_stage_reset_frames(h, reset_obs, done, n, n_done)) return rc;
   // the transitions: obs = the staged rows, next_obs = the uploaded rows (a finished env's terminal frame)
   TransitionReplay& rp = h->replay;
   const int64_t new_size = std::min<int64_t>(rp.cap, rp.size + n);

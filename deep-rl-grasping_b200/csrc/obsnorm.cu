@@ -15,6 +15,9 @@
 //
 // Every copy and kernel of a call is enqueued on the handle's stream and the call synchronises it once before it returns, as
 // b2g_replay_add and b2g_sac_act do: the caller's arrays are free on return.
+//
+// With an observation encoder (b2g_sac_set_obs_encoder) the frames uploaded are raw depth rows; the encoder stage (encoder.cu)
+// turns them into the encoded rows of ob_full on the device, and everything after it runs on those unchanged.
 #include <math.h>
 #include <string.h>
 
@@ -123,6 +126,24 @@ int upload(b2g_sac* h, void* dst, const void* src, size_t bytes) {
   return 0;
 }
 
+// the n frames of a call -> ob_full[0]: uploaded as they are or, with an observation encoder, as raw rows it encodes there
+int stage_frames(b2g_sac* h, const float* obs, int n) {
+  if (!h->enc) return upload(h, h->ob_full[0], obs, (size_t)n * h->E * sizeof(float));
+  if (int rc = upload(h, enc_stage_raw(h->enc, 0), obs, (size_t)n * enc_stage_row_floats(h->enc) * sizeof(float))) return rc;
+  return enc_stage_encode(h->enc, 0, nullptr, n, 0, h->ob_full[0], h->stream);
+}
+
+// the reset frames of the n_done finished envs -> row i of ob_full[1]; only those rows cross the bus and, with an observation
+// encoder, only those are encoded (it reads the flags ob_done, uploaded before)
+int stage_reset_frames(b2g_sac* h, const float* reset_obs, const float* done, int n, int n_done) {
+  const size_t rw = h->enc ? enc_stage_row_floats(h->enc) : h->E;
+  float* dst = h->enc ? enc_stage_raw(h->enc, 1) : h->ob_full[1];
+  for (int i = 0; i < n; ++i)
+    if (done[i] != 0.f)
+      if (int rc = upload(h, dst + i * rw, reset_obs + i * rw, rw * sizeof(float))) return rc;
+  return h->enc ? enc_stage_encode(h->enc, 1, h->ob_done, n, n_done, h->ob_full[1], h->stream) : 0;
+}
+
 // caller-layout frames [n][E] -> compact rows [n][Ec]
 int to_rows(b2g_sac* h, const float* full, float* rows, int row0, int n) {
   if (h->cnn) compact_rows(full, rows, row0, (long long)h->stage_rows + h->B, n, h->Hi * h->Wi, h->Cimg, h->Cobs, h->stream);
@@ -198,6 +219,28 @@ int b2g_upload_bytes(const b2g_sac* h, int64_t* observe_bytes, int64_t* other_by
   return 0;
 }
 
+int b2g_sac_set_obs_encoder(b2g_sac* h, const b2g_encoder* enc, int tail) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  if (enc) {
+    if (h->cnn) return b2g_fail(B2G_EINVAL, "set_obs_encoder: the CNN policy reads images itself; an encoder feeds the MLP policy");
+    if (int rc = enc_stage_check(enc, h->cfg.device, tail, h->E)) return rc;
+    if (h->cfg.nranks > 1)
+      return b2g_fail(B2G_ESTATE, "set_obs_encoder: the observe path is per handle: with nranks > 1 every rank would encode its own");
+  }
+  if (h->pipe_pending) return b2g_fail(B2G_ESTATE, "a host-pipelined step is in flight: call b2g_sac_pipeline_flush first");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  EncStage* st = nullptr;
+  if (enc)
+    if (int rc = enc_stage_create(enc, h->stage_rows, tail, h->stream, &st)) return rc;
+  enc_stage_destroy(h->enc);
+  h->enc = st;
+  h->ob_n = 0;          // staged observations were in the other layout
+  h->ob_fid.clear();
+  return 0;
+}
+
 int b2g_sac_observe_act(b2g_sac* h, const float* obs, int n, int update_stats, int deterministic, float* act_out) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
@@ -210,7 +253,7 @@ int b2g_sac_observe_act(b2g_sac* h, const float* obs, int n, int update_stats, i
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = ensure_staging(h)) return rc;
   if (obs) {
-    if (int rc = upload(h, h->ob_full[0], obs, (size_t)n * h->E * sizeof(float))) return rc;
+    if (int rc = stage_frames(h, obs, n)) return rc;
     if (update_stats) update_launch(h, h->ob_full[0], nullptr, nullptr, n);
     if (int rc = to_rows(h, h->ob_full[0], h->ob_rows[h->ob_k], 0, n)) return rc;
     h->ob_fid.assign((size_t)n, -1);
@@ -245,14 +288,13 @@ int b2g_sac_observe_add(b2g_sac* h, const float* act, const float* rew, const fl
   if (n_done)
     if (int rc = check_frames(h, reset_obs, done, n)) return rc;
   CK(cudaSetDevice(h->cfg.device));
-  const size_t E = h->E, A = h->A, fb = E * sizeof(float);
-  if (int rc = upload(h, h->ob_full[0], next_obs, n * fb)) return rc;
-  for (int i = 0; i < n; ++i)         // only the frames of finished envs cross the bus
-    if (done[i] != 0.f)
-      if (int rc = upload(h, h->ob_full[1] + i * E, reset_obs + i * E, fb)) return rc;
+  const size_t E = h->E, A = h->A;
+  if (int rc = stage_frames(h, next_obs, n)) return rc;
   if (int rc = upload(h, h->ob_act, act, n * A * sizeof(float))) return rc;
   if (int rc = upload(h, h->ob_rew, rew, n * sizeof(float))) return rc;
   if (int rc = upload(h, h->ob_done, done, n * sizeof(float))) return rc;
+  if (n_done)
+    if (int rc = stage_reset_frames(h, reset_obs, done, n, n_done)) return rc;
   // the transitions: obs = the staged rows (linked to their replay frame where one holds them), next_obs = the new rows
   float* cur = h->ob_rows[h->ob_k];
   float* nxt = h->ob_rows[h->ob_k ^ 1];

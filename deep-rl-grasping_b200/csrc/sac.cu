@@ -1156,6 +1156,7 @@ int b2g_sac_destroy(b2g_sac* h) {
   for (auto& e : h->ev_aux) if (e) cudaEventDestroy(e);
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   if (h->ev_join) cudaEventDestroy(h->ev_join);
+  enc_stage_destroy(h->enc);
   for (void* q : h->allocs) cudaFree(q);
   for (int q = 0; q < 2; ++q) { if (h->hc_obs[q]) cudaFreeHost(h->hc_obs[q]); if (h->hc_next[q]) cudaFreeHost(h->hc_next[q]); }
   if (h->h_met) cudaFreeHost(h->h_met);

@@ -11,6 +11,7 @@
 #include "../../include/b200grasp.h"
 #include "cg.cuh"
 #include "common.cuh"
+#include "enc_stage.cuh"
 #include "host.cuh"
 
 namespace b2g {
@@ -234,6 +235,8 @@ struct b2g_sac {
   std::vector<int64_t> ob_fid;
   int ob_n = 0;
   int64_t up_observe = 0, up_other = 0;                   // host->device bytes: observe_* / act + replay_add + set_norm_stats
+  // b2g_sac_set_obs_encoder: observe_* take raw rows and encode them into ob_full (MLP policy only)
+  b2g::EncStage* enc = nullptr;
 
   // CNN extractor (b2g_sac_net_cfg): B2G_CNN_AUGMENTED reads Cimg = obs_c - 1 planes plus the direct feature at column 512 of
   // the feature rows; B2G_CNN_NATURE reads Cimg = obs_c planes and has no direct feature.  Cobs = channels of a caller

@@ -2,7 +2,9 @@
 
 Same names and call shapes as /root/reference/manipulation_main/gripperEnv/encoders.py:
 ``SimpleAutoEncoder(config)`` (:67-136), ``load_weights(model_dir)`` (:27-31), ``encode(imgs)`` (:59-61),
-``encoding_shape`` (:63-65), ``train`` / ``test`` / ``predict`` (:40-57).  ``encode`` runs on the GPU through libb200grasp
+``encoding_shape`` (:63-65), ``train`` / ``test`` / ``predict`` (:40-57).  ``DeferredEncodedDepthImgSensor`` stands in for the
+reference's ``EncodedDepthImgSensor`` (sensor.py:169-230) in env workers that hold no CUDA context: it hands out the filtered
+depth frame, and ``vec_env.VecEncodeDepth`` encodes the frames of every env in the learner's process.  ``encode`` runs on the GPU through libb200grasp
 (csrc/encoder.cu); ``train``, ``test`` and ``predict`` run the whole auto-encoder there (csrc/autoencoder.cu), with the
 bookkeeping of Keras' ``fit`` restated in :func:`fit`.  ``plot`` (pydot) raises ``NotImplementedError``.  ``model.h5`` is read
 and written by ``h5min`` (no h5py/keras needed).
@@ -11,6 +13,7 @@ from __future__ import annotations
 
 import csv
 import ctypes as C
+import hashlib
 import math
 import os
 from typing import Callable, Dict, List, Optional, Sequence, Tuple
@@ -304,15 +307,32 @@ class SimpleAutoEncoder(Encoder):
         if len(arrays) != n:
             raise ValueError(f"expected {n} (kernel, bias) pairs, got {len(arrays)}")
         fp = C.POINTER(C.c_float)
+        loaded = []
         for i, (k, b) in enumerate(arrays):
             k = np.ascontiguousarray(k, np.float32)
             b = np.ascontiguousarray(b, np.float32)
             _lib.check(self._lib.b2g_encoder_set_weights(self._handle, i, k.ctypes.data_as(fp), k.size, b.ctypes.data_as(fp), b.size))
+            loaded.append((k.copy(), b.copy()))
+        self._encoder_arrays = loaded
+
+    def weights_digest(self) -> str:
+        """sha256 over the encoder half's shapes and float32 weights (what a training state records of the encoder it was
+        trained through)."""
+        arrays = getattr(self, "_encoder_arrays", None)
+        if arrays is None:
+            raise ValueError("the encoder has no weights (load_weights first)")
+        h = hashlib.sha256()
+        for k, b in arrays:
+            for a in (k, b):
+                h.update(repr(a.shape).encode())
+                h.update(a.tobytes())
+        return h.hexdigest()
 
     def load_weights(self, model_dir):
         """Loads model.h5; when it also holds the decoder half (the shipped files do), predict / test / train use it."""
         model_dir = os.path.expanduser(model_dir)
         weights = h5min.load_keras_weights(os.path.join(model_dir, "model.h5"))
+        self.model_dir = model_dir
         names = keras_layer_names(len(self.network))
         if all(f"{n}/kernel" in weights and f"{n}/bias" in weights for n in names):
             self.set_model_weights([(weights[f"{n}/kernel"], weights[f"{n}/bias"]) for n in names])
@@ -352,3 +372,42 @@ class SimpleAutoEncoder(Encoder):
             self.close()
         except Exception:
             pass
+
+
+class DeferredEncodedDepthImgSensor:
+    """Drop-in for the reference's ``EncodedDepthImgSensor(config, sensor, robot)`` (sensor.py:169-230) that defers the
+    encoding: ``get_state()`` renders and filters the depth frame exactly as the reference does and returns it flattened in
+    HWC order, NOT encoded.  The env's observation is then ``[H*W depth | tail]``; ``vec_env.VecEncodeDepth`` encodes the
+    frames of all envs at once in the learner's process (or hands them to the learner, which encodes them on its device).
+    It never touches the CUDA library, so ``SubprocVecEnv`` workers hold no CUDA context and no copy of the encoder.
+    ``visualize: true`` is refused: the reconstruction window needs the decoder in the worker."""
+
+    def __init__(self, config, sensor, robot):
+        import yaml
+        from .spaces import Box
+        self.scope = 'encoded_img_sensor'
+        self._sensor = sensor
+        self._robot = robot
+        self.scene_type = config['scene'].get('scene_type', "OnTable")
+        config = config['sensor']
+        if config.get('visualize', False):
+            raise NotImplementedError("DeferredEncodedDepthImgSensor: sensor.visualize needs the decoder in the env worker; use "
+                                      "the reference's EncodedDepthImgSensor to watch reconstructions")
+        self.encoder_dir = os.path.expanduser(config['encoder_dir'])
+        with open(os.path.join(self.encoder_dir, 'config.yaml')) as f:
+            self.encoding_dim = int(yaml.safe_load(f)['encoding_dim'])
+        self.height, self.width = (int(d) for d in sensor.state_space.shape[:2])
+        self.state_space = Box(0.0, np.inf, (self.height * self.width,), np.float32)
+
+    def get_state(self):
+        """The filtered depth frame [H*W] (HWC order, one channel), the input of ``encoder.encode``."""
+        # Render
+        _, img, mask = self._sensor.get_state()
+
+        # Filter (sensor.py:212-219)
+        img[mask == 0] = 0.
+        img[mask == self._robot.robot_id] = 0.
+        if self.scene_type == "OnTable":
+            img[mask == 1] = 0.
+            img[mask == 2] = 0.
+        return np.asarray(img, np.float32).reshape(-1)

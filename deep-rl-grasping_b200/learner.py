@@ -48,6 +48,8 @@ class HandleLearner:
 
     #: bumped by every call that may change the device statistics (DeviceRunningMeanStd caches against it)
     obs_rms_version = 0
+    #: floats of a raw row observe_* take while an observation encoder is attached (set_obs_encoder), else None
+    raw_obs_elems = None
 
     def _has_grad(self, name: str) -> bool:
         raise NotImplementedError
@@ -159,6 +161,24 @@ class HandleLearner:
         cnt = C.c_double()
         _lib.check(self._fn("obs_rms_get")(self.h, m.ctypes.data_as(dp), v.ctypes.data_as(dp), C.byref(cnt)))
         return m, v, float(cnt.value)
+
+    # ---- an observation encoder on the observe path (SAC's MLP policy and BDQ; include/b200grasp.h: b2g_*_set_obs_encoder)
+    def set_obs_encoder(self, encoder, tail: int = 0):
+        """``encoder`` (an ``encoders.SimpleAutoEncoder`` with weights): its geometry and weights are copied into this learner,
+        and from then on ``observe_act`` / ``observe_add`` take raw rows ``[H*W*C depth | tail]`` and encode them on the
+        device into the ``[encoding_dim | tail]`` rows everything else works on.  ``None`` detaches.  Either way the staged
+        observations are cleared."""
+        if encoder is None:
+            _lib.check(self._fn("set_obs_encoder")(self.h, None, 0))
+            self.raw_obs_elems = None
+            return
+        _lib.check(self._fn("set_obs_encoder")(self.h, encoder._handle, int(tail)))
+        self.raw_obs_elems = int(np.prod(encoder.input_shape)) + int(tail)
+
+    @property
+    def frame_elems(self) -> int:
+        """Floats per frame of observe_act / observe_add."""
+        return self.raw_obs_elems or self.obs_elems
 
     def upload_bytes(self) -> dict:
         """Bytes copied host -> device so far: by ``observe_*`` / ``obs_rms_set``, and by ``act`` + ``replay_add`` +
@@ -309,7 +329,7 @@ class Learner(HandleLearner):
         """``obs``: n raw observations to upload, merge into ``obs_rms`` (``update_stats``) and stage as the current
         observation of env i; ``None`` acts on the ones already staged.  Returns the n actions, or None with ``act=False``."""
         if obs is not None:
-            obs = _f32(obs).reshape(-1, self.obs_elems)
+            obs = _f32(obs).reshape(-1, self.frame_elems)
             n = obs.shape[0]
             self.obs_rms_version += bool(update_stats)
         out = np.empty((int(n), self.n_act), np.float32) if act else None
@@ -323,7 +343,7 @@ class Learner(HandleLearner):
         act, next_obs = _f32(act), _f32(next_obs)
         rew, done = _f32(np.reshape(rew, -1)), _f32(np.reshape(done, -1))
         n = rew.shape[0]
-        assert next_obs.size == n * self.obs_elems and act.size == n * self.n_act and done.size == n
+        assert next_obs.size == n * self.frame_elems and act.size == n * self.n_act and done.size == n
         if reset_obs is not None:
             reset_obs = _f32(reset_obs)
             assert reset_obs.size == next_obs.size

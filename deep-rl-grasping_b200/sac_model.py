@@ -119,6 +119,7 @@ class SAC(BaseModel):
         self._set_env(env)
         if self.learner is not None:
             self._attach_device_norm()
+            self._attach_obs_encoder()
             self._sync_norm_stats()
 
     def setup_model(self):
@@ -139,6 +140,7 @@ class SAC(BaseModel):
                                u8_planes=self.replay_u8_planes, **self._net_kwargs(obs_shape), **self._dev)
         self._init_parameters()
         self._attach_device_norm()
+        self._attach_obs_encoder()
         self._sync_norm_stats()
 
     def _net_kwargs(self, obs_shape):
@@ -288,6 +290,7 @@ class SAC(BaseModel):
     # ------------------------------------------------------------------ predict ([SB2] SAC.predict)
     def predict(self, observation, state=None, mask=None, deterministic=True):
         observation = np.asarray(observation, np.float32)
+        self._check_encoded(observation)
         single = observation.shape == tuple(self.observation_space.shape)
         obs = observation.reshape((-1,) + tuple(self.observation_space.shape))
         vn = self._vec_normalize_env
@@ -337,10 +340,14 @@ class SAC(BaseModel):
                     replay_frames=self.replay_frames, replay_u8_planes=list(self.replay_u8_planes))
         if self.device_obs_norm:
             init["device_obs_norm"] = True
-        return {"algo": "SAC", "policy": "CnnPolicy" if len(self.observation_space.shape) == 3 else "MlpPolicy", "init": init,
+        host = {"algo": "SAC", "policy": "CnnPolicy" if len(self.observation_space.shape) == 3 else "MlpPolicy", "init": init,
                 "num_timesteps": int(self.num_timesteps), "n_updates": int(self.n_updates),
                 "episode_rewards": [float(r) for r in self.episode_rewards], "ep_info_buf": list(self.ep_info_buf),
                 "rng": training_state.rng_state(self._rng)}
+        enc = self._encoder_host()
+        if enc is not None:
+            host["obs_encoder"] = enc
+        return host
 
     @classmethod
     def _policy_from_host(cls, host):

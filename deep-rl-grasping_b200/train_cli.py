@@ -29,7 +29,7 @@ from .common.policies import MlpPolicy as PPOMlpPolicy
 from .ppo2 import PPO2
 from .trpo_mpi import TRPO
 from .sac_model import CnnPolicy, MlpPolicy
-from .vec_env import DummyVecEnv, SubprocVecEnv, VecNormalize
+from .vec_env import DummyVecEnv, SubprocVecEnv, VecEncodeDepth, VecNormalize
 
 
 def _default_factory(config, evaluate=False, validate=False, test=False):
@@ -68,11 +68,39 @@ def _is_image_obs(env):
     return len(env.observation_space.shape) == 3
 
 
+def device_encoder(config, n_envs):
+    """The perception encoder of ``config['sensor']['encoder_dir']`` (the directory the reference sensor reads), for the
+    frames and terminal observations of ``n_envs`` envs in one call."""
+    from .encoders import SimpleAutoEncoder
+    model_dir = os.path.expanduser(config["sensor"]["encoder_dir"])
+    with open(os.path.join(model_dir, "config.yaml")) as f:
+        enc = SimpleAutoEncoder(yaml.safe_load(f), max_batch=2 * n_envs)
+    enc.load_weights(model_dir)
+    return enc
+
+
+def encode_depth(env, test_env, config, n_envs):
+    """--device_encode: the training and evaluation envs hand out raw depth rows (encoders.DeferredEncodedDepthImgSensor);
+    one VecEncodeDepth over each encodes them in this process.  A SAC / BDQ model with device_obs_norm then takes the
+    encoder and the training wrapper passes the rows through to the device; the evaluation wrapper stays in host mode."""
+    encoder = device_encoder(config, n_envs)
+    return VecEncodeDepth(env, encoder), VecEncodeDepth(test_env, encoder)
+
+
+def _check_device_encode(config):
+    if config.get("depth_observation", False) or config.get("full_observation", False):
+        raise ValueError("--device_encode: the config observes images (depth_observation / full_observation); the encoder "
+                         "feeds the encoded-depth observation only")
+
+
 def train(args):
     if getattr(args, "resume", None):
         return resume(args)
     config = yaml.safe_load(open(args.config))
     algo = args.algo
+    if args.device_encode:
+        _check_device_encode(config)
+        config["device_encode"] = True          # --resume and run rebuild the same stack
     if algo == "DQN":          # stable-baselines' DQN takes one environment; its statistics stay with the host VecNormalize
         if int(args.n_envs) > 1:
             raise ValueError("--algo DQN: DQN cannot be used with more than one environment (--n_envs 1)")
@@ -111,6 +139,8 @@ def train(args):
     for sub in ("", "best_model"):
         yaml.safe_dump(config, open(os.path.join(args.model_dir, sub, "config.yaml"), "w"))
     test_env = DummyVecEnv([lambda: make(config, evaluate=True, validate=True)])
+    if config.get("device_encode", False):
+        env, test_env = encode_depth(env, test_env, config, n_envs)
     norm = bool(config.get("normalize", False))
     eval_path = os.path.join(args.model_dir, "best_model")
     if norm:
@@ -241,6 +271,8 @@ def resume(args):
     else:
         env = SubprocVecEnv([(lambda i=i: Monitor(make(config), f"{log}_{i}")) for i in range(n_envs)])
     test_env = DummyVecEnv([lambda: make(config, evaluate=True, validate=True)])
+    if config.get("device_encode", False):
+        env, test_env = encode_depth(env, test_env, config, n_envs)
     eval_path = os.path.join(model_dir, "best_model")
     if config.get("normalize", False):
         test_env = VecNormalize(test_env, norm_obs=True, norm_reward=False, clip_obs=10.0)
@@ -290,6 +322,8 @@ def run(args):
     config = yaml.safe_load(open(os.path.join(top, "config.yaml")))
     make = _factory(args.env)
     task = DummyVecEnv([lambda: make(config, evaluate=True, test=args.test)])
+    if config.get("device_encode", False):         # the saved zip takes encoded observations: host mode
+        task = VecEncodeDepth(task, device_encoder(config, 1))
     if config.get("normalize", False):
         task = VecNormalize.load(os.path.join(top, "vecnormalize.pkl"), VecNormalize(task, training=False, norm_obs=True, norm_reward=True, clip_obs=10.0))
         task.training = False
@@ -337,6 +371,9 @@ def build_parser():
     t.add_argument("--device_norm", action="store_true",
                    help="keep VecNormalize's observation statistics on the GPU and upload every frame once "
                         "(SAC / BDQ(device_obs_norm=True); not DQN); --resume takes it from the saved run")
+    t.add_argument("--device_encode", action="store_true",
+                   help="the env's sensor defers the depth encoding (encoders.DeferredEncodedDepthImgSensor): encode the "
+                        "frames of all envs at once in this process, on the learner's device with --device_norm (SAC / BDQ)")
     t.add_argument("--eval_freq", type=int, default=50000)
     t.add_argument("--checkpoint_freq", type=int, default=25000)
     t.add_argument("--state_freq", type=int, default=None,

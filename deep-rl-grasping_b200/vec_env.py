@@ -244,6 +244,116 @@ class SubprocVecEnv(VecEnv):
         self.closed = True
 
 
+class VecEncodeDepth(VecEnv):
+    """Owns the perception encoder of the encoded-depth configuration for a stack of envs whose sensor defers the encoding
+    (``encoders.DeferredEncodedDepthImgSensor``): each raw observation is ``[H*W*C depth | tail]``, ``tail`` floats of actuator
+    state or time feature (default: whatever follows the pixels).  ``observation_space`` is what the reference env reports,
+    ``Box(-1, 1, (encoding_dim,))`` followed by the raw space's last ``tail`` bounds, so a VecNormalize on top keeps the
+    shipped ``obs_rms`` layout.
+
+    Host mode (the default): every ``reset`` / ``step`` makes one ``encoder.encode`` call for the frames of all envs and the
+    terminal observations of the finished ones, and returns encoded rows.  Pass-raw mode: a SAC or BDQ learner built with
+    ``device_obs_norm=True`` took the encoder (``give_encoder_to``) and encodes on its device, so ``reset`` / ``step`` and the
+    terminal observations hand the raw rows through; ``take_encoder_back`` returns to host mode."""
+
+    def __init__(self, venv, encoder, tail=None):
+        from .spaces import Box
+        self.venv, self.encoder = venv, encoder
+        self.num_envs = venv.num_envs
+        self.input_shape = tuple(int(d) for d in encoder.input_shape)
+        self.pixels = int(np.prod(self.input_shape))
+        self.raw_observation_space = raw = venv.observation_space
+        self.raw_width = int(np.prod(raw.shape))
+        self.tail = self.raw_width - self.pixels if tail is None else int(tail)
+        if self.tail < 0 or self.pixels + self.tail != self.raw_width:
+            raise ValueError(f"VecEncodeDepth: raw observations of {self.raw_width} floats are not {self.pixels} pixels "
+                             f"{self.input_shape} + {self.tail} tail floats")
+        dim = int(encoder.encoding_dim)
+        low = np.concatenate([np.full(dim, -1.0), np.ravel(raw.low)[self.pixels:]])
+        high = np.concatenate([np.full(dim, 1.0), np.ravel(raw.high)[self.pixels:]])
+        self.observation_space = Box(low, high, (dim + self.tail,), np.float32)
+        self.action_space = venv.action_space
+        self._owner = None
+
+    # ---- the encoder handed to a device learner (SAC / BDQ with device_obs_norm)
+    @property
+    def pass_raw(self) -> bool:
+        return self._owner is not None
+
+    @property
+    def encoder_owner(self):
+        return self._owner
+
+    def give_encoder_to(self, owner) -> None:
+        """From here on ``owner`` (a learner with the encoder attached) encodes: observations go through raw."""
+        if self._owner is not None and self._owner is not owner:
+            raise RuntimeError("this VecEncodeDepth's encoder is already attached to another learner")
+        self._owner = owner
+
+    def take_encoder_back(self) -> None:
+        """Host mode again (the owner is about to go away)."""
+        self._owner = None
+
+    def encode(self, rows) -> np.ndarray:
+        """Raw rows [n, H*W*C + tail] -> encoded rows [n, encoding_dim + tail] (one ``encoder.encode`` call)."""
+        rows = np.asarray(rows, np.float32).reshape(-1, self.raw_width)
+        enc = np.asarray(self.encoder.encode(rows[:, :self.pixels].reshape((-1,) + self.input_shape)), np.float32)
+        return np.concatenate([enc, rows[:, self.pixels:]], axis=1)
+
+    # ---- VecEnv surface
+    @property
+    def envs(self):
+        return self.venv.envs
+
+    @property
+    def buf_infos(self):
+        return self.venv.buf_infos
+
+    def reset(self):
+        obs = self.venv.reset()
+        return obs if self.pass_raw else self.encode(obs)
+
+    def step_async(self, actions):
+        self.venv.step_async(actions)
+
+    def step_wait(self):
+        obs, rews, dones, infos = self.venv.step_wait()
+        if self.pass_raw:
+            return obs, rews, dones, infos
+        # the reference env encodes the terminal frame too: it joins the same call
+        term = [i for i, info in enumerate(infos) if dones[i] and isinstance(info, dict) and "terminal_observation" in info]
+        n = self.num_envs
+        rows = np.concatenate([np.asarray(obs, np.float32).reshape(n, -1)] +
+                              [np.asarray(infos[i]["terminal_observation"], np.float32).reshape(1, -1) for i in term])
+        enc = self.encode(rows)
+        infos = list(infos)
+        for k, i in enumerate(term):
+            infos[i] = dict(infos[i], terminal_observation=enc[n + k])
+        return enc[:n], rews, dones, infos
+
+    def step(self, actions):
+        self.step_async(actions)
+        return self.step_wait()
+
+    def close(self):
+        self.venv.close()
+
+    def get_attr(self, name, indices=None):
+        return self.venv.get_attr(name, indices)
+
+    def env_method(self, name, *a, **k):
+        return self.venv.env_method(name, *a, **k)
+
+
+def unwrap_encode_depth(env) -> Optional[VecEncodeDepth]:
+    e = env
+    while e is not None:
+        if isinstance(e, VecEncodeDepth):
+            return e
+        e = getattr(e, "venv", None)
+    return None
+
+
 class VecNormalize(VecEnv):
     """[SB2] VecNormalize(venv, training=True, norm_obs=True, norm_reward=True, clip_obs=10.,
     clip_reward=10., gamma=0.99, epsilon=1e-8)."""

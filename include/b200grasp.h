@@ -593,6 +593,20 @@ int b2g_encoder_set_weights(b2g_encoder* h, int layer, const float* kernel, size
 /* imgs: host [n, height, width, channels] fp32 -> out: host [n, encoding_dim]; B2G_ESTATE until every layer is loaded */
 int b2g_encoder_encode(b2g_encoder* h, const float* imgs, int n, float* out);
 
+/* ---- the encoder on a learner's observe path: the env hands out raw depth rows and the learner encodes them on its device.
+ * enc != NULL attaches: the encoder's geometry and weights are copied device to device into a stage the learner handle owns,
+ * on the handle's device and stream, for up to max(batch, 256) rows (the observe calls' limit); the weights are frozen and
+ * the encoder handle may be destroyed afterwards.  enc == NULL detaches.  Either way the staged observations are cleared.
+ * With an encoder attached, b2g_sac_observe_act / _add (and the BDQ pair) take RAW rows [n][H*W*C + tail]: pixels in HWC
+ * order, then `tail` floats (the actuator state, a time feature) copied to columns [encoding_dim, obs_dim) of the encoded
+ * row.  Only the n frames and the reset frames of finished envs cross the bus, and only those are encoded; obs_rms, the actor
+ * and the replay then work on encoded rows [obs_dim] exactly as before, so b2g_sac_act, b2g_replay_add, the step and the
+ * training-state file are unchanged.  The upload counters count the raw bytes.
+ * Before any CUDA call: B2G_EINVAL for a CNN SAC policy, encoding_dim + tail != obs_dim, tail < 0 or an encoder on another
+ * device; B2G_ESTATE for an encoder layer without weights or nranks > 1. */
+int b2g_sac_set_obs_encoder(b2g_sac* h, const b2g_encoder* enc, int tail);
+int b2g_bdq_set_obs_encoder(b2g_bdq* h, const b2g_encoder* enc, int tail);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Auto-encoder TRAINING (encoders.py:40-61 train / test / predict, graph :84-136): the full Keras model
  * encoder -> decoder on one handle, trained with mean_squared_error and Keras Adam (eps 1e-7) in fp32 on the GPU.
