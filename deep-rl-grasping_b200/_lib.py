@@ -43,7 +43,16 @@ SYMBOLS = [
     "b2g_autoencoder_set_weights", "b2g_autoencoder_get_weights", "b2g_autoencoder_get_grad", "b2g_autoencoder_reset_optimizer",
     "b2g_autoencoder_set_dataset", "b2g_autoencoder_train_epoch", "b2g_autoencoder_evaluate", "b2g_autoencoder_predict",
     "b2g_autoencoder_step",
+    "b2g_sac_metrics_log", "b2g_sac_metrics_drain", "b2g_bdq_metrics_log", "b2g_bdq_metrics_drain",
+    "b2g_dqn_metrics_log", "b2g_dqn_metrics_drain",
 ]
+
+#: columns of one per-step metrics-log row (B2G_*_LOG_COLS in include/b200grasp.h), by handle kind
+LOG_COLS = {
+    "sac": ("policy_loss", "qf1_loss", "qf2_loss", "value_loss", "ent_coef_loss", "entropy", "ent_coef", "learning_rate"),
+    "bdq": ("loss", "mean_q", "grad_norm", "learning_rate"),
+    "dqn": ("loss", "mean_q", "mean_abs_td", "grad_norm", "n_clipped", "learning_rate"),
+}
 
 ENC_MAX_LAYERS = 8
 
@@ -248,6 +257,9 @@ def load():
             getattr(lib, f"b2g_{p}_{f}").argtypes = [vp, C.c_char_p, fp, C.c_size_t]
         for f in ("state_save", "state_load"):
             getattr(lib, f"b2g_{p}_{f}").argtypes = [vp, C.c_char_p]
+    for p in ("sac", "bdq", "dqn"):          # the per-step metrics ring of the replay learners
+        getattr(lib, f"b2g_{p}_metrics_log").argtypes = [vp, C.c_int]
+        getattr(lib, f"b2g_{p}_metrics_drain").argtypes = [vp, fp, C.c_int, i64p, C.POINTER(C.c_int), i64p]
     for p in ("bdq", "dqn"):                 # and the transition replay of the two Q learners
         getattr(lib, f"b2g_{p}_replay_add").argtypes = [vp, fp, fp, fp, fp, fp, C.c_int64]
         getattr(lib, f"b2g_{p}_replay_size").argtypes = [vp]

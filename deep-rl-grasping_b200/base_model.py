@@ -11,7 +11,8 @@ from typing import Optional
 
 import numpy as np
 
-from . import sb_io, training_state
+from . import _lib, sb_io, training_state
+from .tensorboard import StepLog, TensorboardWriter
 from .vec_env import DummyVecEnv, VecNormalize, unwrap_encode_depth
 
 
@@ -28,9 +29,30 @@ class BaseModel:
     _algo = ""                     # host.json's "algo"
     _policy = "MlpPolicy"          # what load_training_state passes as the constructor's policy
     device_obs_norm = False
+    tensorboard_log = None
+    #: per-gradient-step summaries of the replay learners: tag -> column of the learner's metrics ring (_lib.LOG_COLS)
+    _step_tags = None
     learner = None
     env = None
     _vec_normalize_env = None
+
+    # ------------------------------------------------------------------ TensorBoard (tensorboard.py)
+    def _learn_logged(self, tb_log_name, reset_num_timesteps, run):
+        """run(writer, step_log) inside stable-baselines' TensorboardWriter: writer is None without tensorboard_log and on
+        ranks other than 0; step_log drains the learner's metrics ring (replay learners) and is drained once more on the
+        way out, also when a callback stops the run or an exception ends it."""
+        dp = getattr(self, "_dev", None) or getattr(self, "_dp", None) or {}
+        path = self.tensorboard_log if int(dp.get("rank", 0)) == 0 else None
+        with TensorboardWriter(path, tb_log_name, new_tb_log=reset_num_timesteps) as writer:
+            steps = None
+            if writer is not None and self._step_tags is not None:
+                cols = _lib.LOG_COLS[self.learner._abi]
+                steps = StepLog(self.learner, writer, list(self._step_tags), [cols.index(c) for c in self._step_tags.values()])
+            try:
+                return run(writer, steps)
+            finally:
+                if steps is not None:
+                    steps.close()
 
     # ------------------------------------------------------------------ env plumbing
     def _set_env(self, env):

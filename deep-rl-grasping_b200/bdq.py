@@ -18,6 +18,7 @@ import numpy as np
 from . import _lib, training_state
 from .base_model import BaseModel
 from .callbacks import as_callback
+from .tensorboard import EpisodeRewardLogger
 from .learner import HandleLearner, _f32, _fp, nccl_config
 from .vec_env import VecNormalize
 
@@ -144,6 +145,7 @@ class BDQ(BaseModel):
         self.train_freq, self.learning_starts = train_freq, learning_starts
         self.target_network_update_freq, self.num_actions_pad = target_network_update_freq, int(num_actions_pad)
         self.verbose, self.seed, self.device = verbose, seed, device
+        self.tensorboard_log = tensorboard_log
         self.num_timesteps = 0
         self._rng = np.random.default_rng(seed)
         self.learner: Optional[BDQLearner] = None
@@ -192,10 +194,17 @@ class BDQ(BaseModel):
         frac = min(1.0, t / max(1.0, self.exploration_fraction * total))
         return 1.0 + frac * (self.exploration_final_eps - 1.0)
 
+    _step_tags = {"loss": "loss", "mean_q": "mean_q", "grad_norm": "grad_norm", "learning_rate": "learning_rate"}
+
     def learn(self, total_timesteps, callback=None, log_interval=100, tb_log_name="BDQ", reset_num_timesteps=True):
+        """With tensorboard_log every gradient step's losses are written from the device metrics ring (tensorboard.py)."""
+        return self._learn_logged(tb_log_name, reset_num_timesteps,
+                                  lambda writer, steps: self._learn(total_timesteps, callback, reset_num_timesteps, writer, steps))
+
+    def _learn(self, total_timesteps, callback, reset_num_timesteps, writer, steps):
         callback = as_callback(callback)
         callback.init_callback(self)
-        callback.on_training_start({"self": self, "writer": None}, globals())
+        callback.on_training_start({"self": self, "writer": writer}, globals())
         dev = self.device_obs_norm
         vn = self._vec_normalize_env
         if dev:
@@ -213,6 +222,7 @@ class BDQ(BaseModel):
         # total_timesteps from now (the stable-baselines DQN rule)
         resume = not reset_num_timesteps
         horizon = self.num_timesteps + total_timesteps if resume else total_timesteps
+        ep_log = EpisodeRewardLogger(n_env) if writer is not None else None
         for t in range(0, total_timesteps, n_env):
             eps = self._epsilon(self.num_timesteps if resume else t, horizon)
             if dev:      # the staged frames, current statistics, epsilon-greedy on the device
@@ -236,6 +246,8 @@ class BDQ(BaseModel):
             else:
                 self.learner.replay_add(np.asarray(obs, np.float32), idx.astype(np.float32), rew, nxt, np.asarray(done, np.float32))
             obs = new_obs
+            if ep_log is not None:
+                ep_log(writer, vn.get_original_reward() if vn is not None else rew, done, self.num_timesteps)
             if self.num_timesteps > self.learning_starts and self.num_timesteps % self.train_freq == 0 and \
                     self.learner.replay_size() >= self.batch_size:
                 if self.prioritized_replay:          # [SB2] LinearSchedule(beta_iters, initial_p=beta0, final_p=1.0)
@@ -244,6 +256,8 @@ class BDQ(BaseModel):
                 if dev:      # the sample is normalised with the statistics of this moment: obs_rms on the device, ret_rms here
                     self._sync_norm_stats()
                 self.learner.step(1, lr)
+                if steps is not None:
+                    steps.queued(1, self.num_timesteps)
         callback.on_training_end()
         return self
 

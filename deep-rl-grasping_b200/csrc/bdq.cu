@@ -26,6 +26,7 @@
 #include "common.cuh"
 #include "enc_stage.cuh"
 #include "host.cuh"
+#include "metrics_log.cuh"
 #include "per.cuh"
 #include "state.cuh"
 
@@ -187,6 +188,7 @@ struct b2g_bdq {
   cudaGraphExec_t graph_exec = nullptr;
   bool use_graph = true;
   bool broken = false;         // a training-state load failed after it began writing: only destroy / load are accepted
+  MetricsLog mlog;             // per-step metrics ring (b2g_bdq_metrics_log); off: the step has no append node
   double norm_eps = 1e-8;      // VecNormalize.epsilon of the last b2g_bdq_set_norm_stats
   // Device-resident VecNormalize observation statistics (created by b2g_bdq_obs_rms_set): float64 mean / var [E]; the count
   // stays on the host.  b2g_bdq_observe_act / _add staging (allocated on first use): the current observation of env i as a row
@@ -371,6 +373,12 @@ int bdq_issue(b2g_bdq* h, bool sampled, bool apply, const float* weights) {
   optim_launch(oa, s);
   CK(cudaGetLastError());
   if (apply) bdq_target_copy_kernel<<<64, 256, 0, s>>>(h->P, h->n_train, h->counters, h->cfg.target_update_freq);   // counters[3] = n_updates (prep)
+  if (apply && h->mlog.on()) {     // loss and mean Q (sums over the ranks), the squared gradient norm, the learning rate
+    MetricsLogSrc m{};
+    m.src[0] = h->metrics + BMET_LOSS; m.src[1] = h->metrics + BMET_MEANQ; m.src[2] = h->metrics + BMET_GN; m.src[3] = h->d_lr;
+    m.K = B2G_BDQ_LOG_COLS;
+    mlog_append(h->mlog, m, h->counters + 3, s);
+  }
   CK(cudaGetLastError());
   return 0;
 }
@@ -396,6 +404,7 @@ int b2g_bdq_destroy(b2g_bdq* h) {
   if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
   nccl_comm_destroy(h->nccl_comm);
   enc_stage_destroy(h->enc);
+  mlog_free(&h->mlog);
   for (void* q : h->allocs) cudaFree(q);
   if (h->h_met) cudaFreeHost(h->h_met);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -865,7 +874,27 @@ int b2g_bdq_state_load(b2g_bdq* h, const char* path) {
     const uint32_t eps_bits = (uint32_t)hv[3];
     memcpy(&h->eps_value, &eps_bits, sizeof eps_bits);
     // the captured step graph stays valid: it holds device pointers and configuration; size and Philox step are device counters
-    return 0;
+    return mlog_rebase(&h->mlog, h->counters + 3, h->stream);     // the restored counter: rows before it are not pending
+  });
+}
+
+int b2g_bdq_metrics_log(b2g_bdq* h, int capacity) {
+  B2G_USABLE(h);
+  if (!h || capacity < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  CK(cudaSetDevice(h->cfg.device));
+  if (int rc = mlog_enable(&h->mlog, capacity, B2G_BDQ_LOG_COLS, h->counters + 3, h->stream)) return rc;
+  // the step gains or loses its append node: capture again at the next step
+  if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
+  return 0;
+}
+
+int b2g_bdq_metrics_drain(b2g_bdq* h, float* rows, int max_rows, int64_t* first_step, int* n_rows, int64_t* lost) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  CK(cudaSetDevice(h->cfg.device));
+  const float inv = 1.0f / (float)h->cfg.nranks;
+  return mlog_drain(&h->mlog, h->counters + 3, h->stream, rows, max_rows, first_step, n_rows, lost, [inv](float* r) {
+    r[0] *= inv; r[1] *= inv; r[2] = sqrtf(r[2]);     // as bfetch
   });
 }
 

@@ -23,6 +23,7 @@
 #include "../../include/b200grasp.h"
 #include "common.cuh"
 #include "host.cuh"
+#include "metrics_log.cuh"
 #include "per.cuh"
 #include "state.cuh"
 
@@ -176,6 +177,7 @@ struct b2g_dqn {
   cudaGraphExec_t graph_exec = nullptr;
   bool use_graph = true;
   bool broken = false;         // a training-state load failed after it began writing: only destroy / load are accepted
+  MetricsLog mlog;             // per-step metrics ring (b2g_dqn_metrics_log); off: the step has no append node
   float* p(const std::string& nm) { return P + params.off(nm); }
   float* g(const std::string& nm) { return G + params.off(nm); }
 };
@@ -320,6 +322,13 @@ int dqn_issue(b2g_dqn* h, bool sampled, bool apply, const float* weights) {
   oa.n_pi = (int)h->n_train; oa.n_values = 0; oa.n_ent = 0; oa.n_target = 0;
   oa.step_consts = h->step_consts; oa.tau = 0.f; oa.grad_scale = 1.0f; oa.metrics = h->metrics; oa.apply = apply ? 1 : 0;
   optim_launch(oa, s);
+  if (apply && h->mlog.on()) {     // the dfetch accumulators (squared gradient norm, clip count as a float), the learning rate
+    MetricsLogSrc m{};
+    m.src[0] = h->metrics + DMET_LOSS; m.src[1] = h->metrics + DMET_MEANQ; m.src[2] = h->metrics + DMET_ABSTD;
+    m.src[3] = h->metrics + DMET_GN2; m.src[4] = h->metrics + DMET_NCLIP; m.src[5] = h->d_lr;
+    m.K = B2G_DQN_LOG_COLS;
+    mlog_append(h->mlog, m, h->counters + 3, s);
+  }
   CK(cudaGetLastError());
   return 0;
 }
@@ -343,6 +352,7 @@ int b2g_dqn_destroy(b2g_dqn* h) {
   cudaSetDevice(h->cfg.device);
   if (h->stream) cudaStreamSynchronize(h->stream);
   if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
+  mlog_free(&h->mlog);
   for (void* q : h->allocs) cudaFree(q);
   if (h->h_met) cudaFreeHost(h->h_met);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -619,7 +629,26 @@ int b2g_dqn_state_load(b2g_dqn* h, const char* path) {
     const uint32_t eps_bits = (uint32_t)hv[3];
     memcpy(&h->eps_value, &eps_bits, sizeof eps_bits);
     // the captured step graph stays valid: it holds device pointers and configuration; size and Philox step are device counters
-    return 0;
+    return mlog_rebase(&h->mlog, h->counters + 3, h->stream);     // the restored counter: rows before it are not pending
+  });
+}
+
+int b2g_dqn_metrics_log(b2g_dqn* h, int capacity) {
+  B2G_USABLE(h);
+  if (!h || capacity < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  CK(cudaSetDevice(h->cfg.device));
+  if (int rc = mlog_enable(&h->mlog, capacity, B2G_DQN_LOG_COLS, h->counters + 3, h->stream)) return rc;
+  // the step gains or loses its append node: capture again at the next step
+  if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
+  return 0;
+}
+
+int b2g_dqn_metrics_drain(b2g_dqn* h, float* rows, int max_rows, int64_t* first_step, int* n_rows, int64_t* lost) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  CK(cudaSetDevice(h->cfg.device));
+  return mlog_drain(&h->mlog, h->counters + 3, h->stream, rows, max_rows, first_step, n_rows, lost, [](float* r) {
+    r[3] = sqrtf(r[3]); r[4] = (float)lrintf(r[4]);     // as dfetch
   });
 }
 

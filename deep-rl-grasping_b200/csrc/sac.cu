@@ -639,6 +639,17 @@ PrepArgs make_prep(b2g_sac* h, unsigned long long seed, bool gen, bool apply) {
   return pa;
 }
 
+// the ring row of one SAC step: the b2g_sac_metrics losses (sums over the ranks), log_ent_coef after the update and the
+// learning rate; sac_mlog_fix turns it into what fill_metrics reports
+MetricsLogSrc sac_mlog_src(b2g_sac* h) {
+  MetricsLogSrc m{};
+  for (int k = 0; k < 6; ++k) m.src[k] = h->metrics + MET_POLICY_LOSS + k;   // policy, qf1, qf2, value, ent_coef losses, entropy
+  m.src[6] = h->p("model/log_ent_coef");
+  m.src[7] = h->d_lr;
+  m.K = B2G_SAC_LOG_COLS;
+  return m;
+}
+
 struct Prof {
   bool on = false;
   std::vector<cudaEvent_t> ev;
@@ -874,6 +885,9 @@ int issue_step(b2g_sac* h, bool sampled, bool apply, bool want_per_sample, Prof*
     mark("adam_polyak_dp");
   } else {     // (a gradient-only step of a connected learner takes the NCCL path above)
     optim_launch(oa, s); ++n; mark("adam_polyak");
+  }
+  if (h->mlog.on() && apply) {     // behind every write of the step's losses, log_ent_coef's update included
+    mlog_append(h->mlog, sac_mlog_src(h), h->counters + 3, s); ++n; mark("metrics_log");
   }
   if (h->use_planes && apply && !h->v2.on) {
     // with fork: refreshed on the aux branch at the head of the next step (the API entry points mark them stale)
@@ -1171,6 +1185,7 @@ int b2g_sac_destroy(b2g_sac* h) {
     if (h->pm_met[j]) cudaFreeHost(h->pm_met[j]);
     if (h->pm_cnt[j]) cudaFreeHost(h->pm_cnt[j]);
   }
+  mlog_free(&h->mlog);
   if (h->cstream) cudaStreamDestroy(h->cstream);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
@@ -2045,7 +2060,32 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
     // stay valid: their kernel parameters hold device pointers and configuration only, and the replay size, first live slot and
     // Philox step they depend on are read from the device counters restored above.
     h->planes_dirty = true;
-    return 0;
+    return mlog_rebase(&h->mlog, h->counters + 3, h->stream);     // the restored counter: rows before it are not pending
+  });
+}
+
+int b2g_sac_metrics_log(b2g_sac* h, int capacity) {
+  B2G_USABLE(h);
+  if (!h || capacity < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  if (h->pipe_pending) return b2g_fail(B2G_ESTATE, "a host-pipelined step is in flight: call b2g_sac_pipeline_flush first");
+  CK(cudaSetDevice(h->cfg.device));
+  if (h->aux) { CK(cudaStreamSynchronize(h->aux)); CK(cudaStreamSynchronize(h->aux2)); }
+  if (int rc = mlog_enable(&h->mlog, capacity, B2G_SAC_LOG_COLS, h->counters + 3, h->stream)) return rc;
+  // the step gains or loses its append node: capture again at the next step
+  if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
+  for (auto& g : h->pipe_graph) if (g) { cudaGraphExecDestroy(g); g = nullptr; }
+  h->launches = 0;
+  return 0;
+}
+
+int b2g_sac_metrics_drain(b2g_sac* h, float* rows, int max_rows, int64_t* first_step, int* n_rows, int64_t* lost) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  CK(cudaSetDevice(h->cfg.device));
+  const float inv = 1.0f / (float)h->cfg.nranks;
+  return mlog_drain(&h->mlog, h->counters + 3, h->stream, rows, max_rows, first_step, n_rows, lost, [inv](float* r) {
+    for (int k = 0; k < 6; ++k) r[k] *= inv;     // as fill_metrics
+    r[6] = expf(r[6]);
   });
 }
 

@@ -13,6 +13,7 @@
 #include "common.cuh"
 #include "enc_stage.cuh"
 #include "host.cuh"
+#include "metrics_log.cuh"
 
 namespace b2g {
 struct Tensor {
@@ -175,6 +176,7 @@ struct b2g_sac {
   long long* pm_cnt[2]{};        // pinned counters
   long long pipe_k = 0;
   bool pipe_pending = false;
+  MetricsLog mlog;               // per-step metrics ring (b2g_sac_metrics_log); off: the step has no append node
   cudaEvent_t record_after_gather = nullptr;
   long long* counters = nullptr;
   double* step_consts = nullptr;

@@ -16,6 +16,7 @@ import numpy as np
 from . import _lib, training_state
 from .base_model import BaseModel
 from .callbacks import as_callback
+from .tensorboard import EpisodeRewardLogger
 from .learner import HandleLearner, _f32, _fp
 
 _ONLINE, _TARGET = "deepq/model/", "deepq/target_q_func/model/"
@@ -151,6 +152,7 @@ class DQN(BaseModel):
         self.per_alpha, self.per_beta0, self.per_beta_iters, self.per_eps = prioritized_replay_alpha, prioritized_replay_beta0, \
             prioritized_replay_beta_iters, prioritized_replay_eps
         self.verbose, self.seed, self.device = verbose, seed, device
+        self.tensorboard_log = tensorboard_log
         self.num_timesteps = 0
         self.n_target_updates = 0
         self._rng = np.random.default_rng(seed)            # epsilon-greedy draws of learn()
@@ -191,15 +193,22 @@ class DQN(BaseModel):
         self.learner.set_norm_stats(vn.obs_rms.mean, vn.obs_rms.var, float(vn.ret_rms.var), vn.clip_obs, vn.clip_reward, vn.epsilon,
                                     norm_obs=vn.norm_obs, norm_reward=vn.norm_reward)
 
+    _step_tags = {"loss": "loss", "mean_q": "mean_q", "mean_abs_td_error": "mean_abs_td", "grad_norm": "grad_norm"}
+
     def learn(self, total_timesteps, callback=None, log_interval=100, tb_log_name="DQN", reset_num_timesteps=True, replay_wrapper=None):
         """stable-baselines 2.10 DQN.learn: per environment step act epsilon-greedily, step, count, call back, store the raw
         transition, then (past learning_starts, every train_freq steps) one gradient step, and every
-        target_network_update_freq environment steps the hard target copy."""
+        target_network_update_freq environment steps the hard target copy.  With tensorboard_log every gradient step's
+        losses are written from the device metrics ring (tensorboard.py)."""
         if replay_wrapper is not None:
             raise NotImplementedError("replay_wrapper: the replay lives on the device")
+        return self._learn_logged(tb_log_name, reset_num_timesteps,
+                                  lambda writer, steps: self._learn(total_timesteps, callback, reset_num_timesteps, writer, steps))
+
+    def _learn(self, total_timesteps, callback, reset_num_timesteps, writer, steps):
         callback = as_callback(callback)
         callback.init_callback(self)
-        callback.on_training_start({"self": self, "writer": None}, globals())
+        callback.on_training_start({"self": self, "writer": writer}, globals())
         vn = self._vec_normalize_env
         lr = self.learning_rate if not callable(self.learning_rate) else self.learning_rate(1.0)
         # reset_num_timesteps=False continues a run: the schedules follow num_timesteps over a run that ends total_timesteps from
@@ -213,6 +222,7 @@ class DQN(BaseModel):
         obs = self.env.reset()
         raw = vn.get_original_obs() if vn is not None else obs
         eps = self.exploration_initial_eps
+        ep_log = EpisodeRewardLogger(1) if writer is not None else None
         for _ in range(total_timesteps):
             eps = _linear(self.num_timesteps, eps_span, self.exploration_initial_eps, self.exploration_final_eps)
             greedy = self.learner.act(np.asarray(obs, np.float32))     # the wrapper's output, as stable-baselines' act sees it
@@ -229,6 +239,8 @@ class DQN(BaseModel):
                 nxt[0] = np.asarray(info["terminal_observation"], np.float32).reshape(-1)
             self.learner.replay_add(np.asarray(raw, np.float32), np.float32(action), rew_raw, nxt, np.asarray(done, np.float32))
             obs, raw = new_obs, new_raw
+            if ep_log is not None:
+                ep_log(writer, rew_raw, done, self.num_timesteps)
             can_sample = self.learner.replay_size() >= self.batch_size
             if can_sample and self.num_timesteps > self.learning_starts and self.num_timesteps % self.train_freq == 0:
                 if self.prioritized_replay:
@@ -236,6 +248,8 @@ class DQN(BaseModel):
                 if vn is not None:       # the sample is normalised with the statistics of this moment
                     self._sync_norm_stats()
                 self.learner.step(1, lr)
+                if steps is not None:
+                    steps.queued(1, self.num_timesteps)
             if can_sample and self.num_timesteps > self.learning_starts and self.num_timesteps % self.target_network_update_freq == 0:
                 self.learner.update_target()
                 self.n_target_updates += 1

@@ -45,6 +45,7 @@ class HandleLearner:
     ``name`` is ``b2g_<abi>_<name>`` unless ``_names`` maps it to another symbol."""
     _abi = ""
     _names = {}
+    log_capacity = 0
 
     #: bumped by every call that may change the device statistics (DeviceRunningMeanStd caches against it)
     obs_rms_version = 0
@@ -53,6 +54,22 @@ class HandleLearner:
 
     def _has_grad(self, name: str) -> bool:
         raise NotImplementedError
+
+    def metrics_log(self, capacity: int):
+        """Per-step metrics ring of ``capacity`` rows on the device (0 turns it off); SAC, BDQ and DQN handles only."""
+        _lib.check(self._fn("metrics_log")(self.h, int(capacity)))
+        self.log_capacity = int(capacity)
+
+    def metrics_drain(self, max_rows: Optional[int] = None):
+        """Rows the steps appended since the last drain: ``(first_step, rows [n, K] float32, lost)``; row i is the metrics of
+        optimiser step ``first_step + i`` (columns ``_lib.LOG_COLS[abi]``) and ``lost`` counts rows overwritten before this
+        drain."""
+        K = len(_lib.LOG_COLS[self._abi])
+        cap = self.log_capacity if max_rows is None else int(max_rows)
+        rows = np.empty((max(cap, 1), K), np.float32)
+        first, n, lost = C.c_int64(), C.c_int(), C.c_int64()
+        _lib.check(self._fn("metrics_drain")(self.h, _fp(rows.reshape(-1)), cap, C.byref(first), C.byref(n), C.byref(lost)))
+        return int(first.value), rows[:n.value].copy(), int(lost.value)
 
     def _fn(self, name: str):
         return getattr(self.lib, self._names.get(name) or f"b2g_{self._abi}_{name}")

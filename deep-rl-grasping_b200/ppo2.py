@@ -14,6 +14,7 @@ import numpy as np
 from . import _lib
 from .base_model import BaseModel
 from .callbacks import as_callback
+from .tensorboard import EpisodeRewardLogger, Summary
 from .learner import HandleLearner, _f32, _fp
 
 _SCOPE = "model/"
@@ -181,15 +182,25 @@ class PPO2(BaseModel):
                                    self.gamma, self.lam, self.ent_coef, self.vf_coef, self.max_grad_norm, int(self.seed or 0), self.device)
         self.learner.load_parameters(_init_params(obs_dim, A, self.layers, self.seed))
 
+    #: TensorBoard tag -> b2g_ppo_metrics field of the per-update summary (tensorboard.py)
+    _update_tags = {"loss/policy_gradient_loss": "policy_loss", "loss/value_function_loss": "value_loss", "loss/entropy_loss": "entropy",
+                    "loss/approximate_kullback-leibler": "approxkl", "loss/clip_factor": "clipfrac"}
+
     def learn(self, total_timesteps, callback=None, log_interval=1, tb_log_name="PPO2", reset_num_timesteps=True):
         """stable-baselines 2.10 PPO2.learn: n_updates = total_timesteps // n_batch rollouts of n_steps steps (clipped actions to
         the env, num_timesteps += n_envs, callback.on_step() False stops before the update), each followed by noptepochs epochs of
-        np.random.shuffle'd minibatches.  Every call starts from env.reset() with an empty rollout."""
+        np.random.shuffle'd minibatches.  Every call starts from env.reset() with an empty rollout.  With tensorboard_log each
+        update's means and every finished episode's reward are written (tensorboard.py)."""
+        return self._learn_logged(tb_log_name, reset_num_timesteps,
+                                  lambda writer, _: self._learn(total_timesteps, callback, log_interval, reset_num_timesteps, writer))
+
+    def _learn(self, total_timesteps, callback, log_interval, reset_num_timesteps, writer):
         callback = as_callback(callback)
         callback.init_callback(self)
         if reset_num_timesteps:
             self.num_timesteps = 0
-        callback.on_training_start({"self": self, "writer": None}, globals())
+        callback.on_training_start({"self": self, "writer": writer}, globals())
+        ep_log = EpisodeRewardLogger(self.n_envs) if writer is not None else None
         lr_fn, clip_fn = _schedule(self.learning_rate), _schedule(self.cliprange)
         cvf = self.cliprange_vf
         cvf_fn = clip_fn if cvf is None else _schedule(cvf)
@@ -220,6 +231,8 @@ class PPO2(BaseModel):
                     if ep is not None:
                         self.ep_info_buf.append(ep)
                 L.rollout_reward(np.asarray(rew, np.float32), np.asarray(done, np.float32))
+                if ep_log is not None:
+                    ep_log(writer, rew, done, self.num_timesteps)
                 obs = np.asarray(new_obs, np.float32).reshape(self.n_envs, -1)
             callback.on_rollout_end()
             if stopped:
@@ -232,6 +245,11 @@ class PPO2(BaseModel):
                 perms[e] = inds
             self.last_metrics = L.update(obs, perms, lr_now, clip_now, cvf_now)
             self._boundary = (self.num_timesteps, np.random.get_state())
+            if writer is not None:
+                m = self.last_metrics
+                vals = [Summary.Value(t, m[k]) for t, k in self._update_tags.items()]
+                vals += [Summary.Value("input_info/learning_rate", lr_now), Summary.Value("input_info/clip_range", clip_now)]
+                writer.add_summary(Summary(vals), self.num_timesteps)
             if self.verbose >= 1 and (update % log_interval == 0 or update == 1):
                 print(f"| ppo2 update {update}/{n_updates} | total_timesteps {self.num_timesteps} | "
                       + " | ".join(f"{k} {v:.5g}" for k, v in self.last_metrics.items()))

@@ -19,6 +19,7 @@ import numpy as np
 from . import _lib, sb_io, training_state
 from .base_model import BaseModel, unwrap_vec_normalize  # noqa: F401  (unwrap_vec_normalize: also imported from here)
 from .callbacks import as_callback
+from .tensorboard import EpisodeRewardLogger
 from .learner import Learner
 
 
@@ -199,9 +200,18 @@ class SAC(BaseModel):
         return low + 0.5 * (a + 1.0) * (high - low)
 
     # ------------------------------------------------------------------ learn
+    _step_tags = {t: t for t in ("policy_loss", "qf1_loss", "qf2_loss", "value_loss", "entropy", "ent_coef_loss", "ent_coef",
+                                 "learning_rate")}
+
     def learn(self, total_timesteps, callback=None, log_interval=4, tb_log_name="SAC", reset_num_timesteps=True,
               replay_wrapper=None):
-        """[SB2] SAC.learn: one env step then (every train_freq steps) gradient_steps minibatch updates."""
+        """[SB2] SAC.learn: one env step then (every train_freq steps) gradient_steps minibatch updates.  With tensorboard_log
+        every gradient step's losses are written from the device metrics ring (tensorboard.py)."""
+        return self._learn_logged(tb_log_name, reset_num_timesteps,
+                                  lambda writer, steps: self._learn(total_timesteps, callback, log_interval, reset_num_timesteps,
+                                                                    writer, steps))
+
+    def _learn(self, total_timesteps, callback, log_interval, reset_num_timesteps, writer, steps):
         if reset_num_timesteps:
             self.num_timesteps = 0
         callback = as_callback(callback)
@@ -221,7 +231,8 @@ class SAC(BaseModel):
         ep_rew = np.zeros(n_env)
         infos_values = {}
         t_start = time.time()
-        self._locals = {"self": self, "writer": None, "total_timesteps": total_timesteps}
+        ep_log = EpisodeRewardLogger(n_env) if writer is not None else None
+        self._locals = {"self": self, "writer": writer, "total_timesteps": total_timesteps}
         callback.on_training_start(self._locals, globals())
         callback.on_rollout_start()
         step = 0
@@ -259,6 +270,8 @@ class SAC(BaseModel):
                                         nxt, np.asarray(done, np.float32))
             obs, obs_ = new_obs, new_obs_
             ep_rew += np.asarray(reward_, np.float64).reshape(-1)
+            if ep_log is not None:
+                ep_log(writer, reward_, done, self.num_timesteps)
             for i in range(n_env):
                 if done[i]:
                     self.episode_rewards.append(float(ep_rew[i]))
@@ -276,9 +289,13 @@ class SAC(BaseModel):
                     self.learner.step_async(self.gradient_steps, lr)
                     self.n_updates += self.gradient_steps
                     self._last_lr = lr
+                    if steps is not None:
+                        steps.queued(self.gradient_steps, self.num_timesteps)
                 callback.on_rollout_start()
             if self.verbose >= 1 and done.any() and log_interval and len(self.episode_rewards) % log_interval == 0:
                 fps = int(step / max(1e-9, time.time() - t_start))
+                if steps is not None:
+                    steps.drain()
                 if self.n_updates:
                     infos_values = self.learner.step(0, getattr(self, "_last_lr", 3e-4))       # 0 steps: just fetch the latest losses
                 print({"episodes": len(self.episode_rewards), "mean 100 episode reward": round(float(np.mean(self.episode_rewards[-101:-1] or [0])), 1),

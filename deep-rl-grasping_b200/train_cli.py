@@ -157,6 +157,7 @@ def train(args):
         else:
             env = VecNormalize(env, norm_obs=True, norm_reward=True, clip_obs=10.0)
     c = config[algo]
+    tb = tensorboard_log(config, algo, args.model_dir)
     if algo == "SAC":
         simplified_image = _is_image_obs(env) and bool(config.get("simplified", False))
         if simplified_image:
@@ -178,7 +179,7 @@ def train(args):
         if args.device_norm:
             replay["device_obs_norm"] = True
         model = SAC(policy, env, policy_kwargs=kw, verbose=1, gamma=config["discount_factor"], buffer_size=c["buffer_size"],
-                    batch_size=c["batch_size"], learning_rate=c["step_size"], precision=args.precision, **replay)
+                    batch_size=c["batch_size"], learning_rate=c["step_size"], precision=args.precision, tensorboard_log=tb, **replay)
         if args.load_dir:
             old = SAC.load(args.load_dir, env, buffer_size=1)
             model.load_parameters(old.get_parameters(), exact_match=False)
@@ -189,19 +190,19 @@ def train(args):
                     exploration_fraction=c.get("exploration_fraction", 0.1), exploration_final_eps=c.get("exploration_final_eps", 0.02),
                     num_actions_pad=c.get("num_actions_pad", 33), learning_starts=c.get("learning_starts", 1000),
                     target_network_update_freq=c.get("target_network_update_freq", 1000),
-                    prioritized_replay=c.get("prioritized_replay", False), device_obs_norm=bool(args.device_norm))
+                    prioritized_replay=c.get("prioritized_replay", False), device_obs_norm=bool(args.device_norm), tensorboard_log=tb)
         if args.load_dir:
             model.load_parameters(BDQ.load(args.load_dir, env).get_parameters())
     elif algo == "DQN":
-        model = DQN(DQNMlpPolicy, env, **dqn_kwargs(config))
+        model = DQN(DQNMlpPolicy, env, tensorboard_log=tb, **dqn_kwargs(config))
         if args.load_dir:        # every parameter (sb_helper.py:183-199's partial load cannot run: tensorboard_file is undefined there)
             old = DQN.load(args.load_dir)
             model.load_parameters(old.get_parameters())
             old.close()
     elif algo == "PPO":
-        model = PPO2(PPOMlpPolicy, env, **ppo_kwargs(config))
+        model = PPO2(PPOMlpPolicy, env, tensorboard_log=tb, **ppo_kwargs(config))
     elif algo == "TRPO":
-        model = TRPO(PPOMlpPolicy, env, **trpo_kwargs(config))
+        model = TRPO(PPOMlpPolicy, env, tensorboard_log=tb, **trpo_kwargs(config))
     else:
         raise NotImplementedError(f"--algo {algo}: the H100 learner builds the SAC, TRPO, PPO, DQN and BDQ branches of SBPolicy.learn "
                                   "(sb_helper.py:85-226)")
@@ -220,6 +221,15 @@ def train(args):
 
 
 STATE_DIR = "training_state"
+
+
+def tensorboard_log(config, algo, model_dir):
+    """sb_helper.py:84: no TensorBoard log when the algorithm's ``tensorboard_logs`` is missing or null, else
+    ``"tensorboard_logs/" + model_dir`` (the directory name only, not the configured path), relative to the working
+    directory."""
+    if (config.get(algo) or {}).get("tensorboard_logs") is None:
+        return None
+    return "tensorboard_logs/" + model_dir
 
 
 def dqn_kwargs(config):
@@ -285,6 +295,8 @@ def resume(args):
     if args.state_freq:
         callbacks.append(TrainingStateCallback(args.state_freq, os.path.join(model_dir, STATE_DIR)))
     model = {"SAC": SAC, "BDQ": BDQ, "DQN": DQN, "PPO": PPO2, "TRPO": TRPO}[algo].load_training_state(state_dir, env)
+    # the continued run writes into the latest run directory of the same log (learn(reset_num_timesteps=False))
+    model.tensorboard_log = tensorboard_log(config, algo, model_dir)
     remaining = int(config[algo]["total_timesteps"]) - model.num_timesteps
     if remaining > 0:
         _learn_keeping_state(model, remaining, callbacks, os.path.join(model_dir, STATE_DIR), reset_num_timesteps=False)

@@ -15,6 +15,7 @@ import numpy as np
 from . import _lib
 from .base_model import BaseModel
 from .callbacks import as_callback
+from .tensorboard import EpisodeRewardLogger, Summary
 from .learner import HandleLearner, _f32, _fp
 from .ppo2 import _check_policy, _check_policy_kwargs, _init_params
 
@@ -170,16 +171,26 @@ class TRPO(BaseModel):
                                    self.device)
         self.learner.load_parameters(init_params(obs_dim, A, self.layers, self.seed))
 
+    #: TensorBoard tag -> b2g_trpo_metrics field of the per-iteration summary (tensorboard.py)
+    _update_tags = {"policy_gradient_loss": "optimgain", "approximate_kullback-leibler": "meankl", "entropy_loss": "entropy",
+                    "value_function_loss": "vf_loss"}
+
     def learn(self, total_timesteps, callback=None, log_interval=100, tb_log_name="TRPO", reset_num_timesteps=True):
         """stable-baselines 2.10 TRPO.learn: iterations while timesteps_so_far < total_timesteps (ceil(total / N) full batches
         of N = timesteps_per_batch steps; clipped actions to the env, num_timesteps += 1, callback.on_step() False stops before
         the update), each followed by the policy step and vf_iters passes of np.random.shuffle'd value minibatches.  Every call
-        starts from env.reset() with an empty rollout."""
+        starts from env.reset() with an empty rollout.  With tensorboard_log each iteration's metrics and every finished
+        episode's reward are written (tensorboard.py)."""
+        return self._learn_logged(tb_log_name, reset_num_timesteps,
+                                  lambda writer, _: self._learn(total_timesteps, callback, log_interval, reset_num_timesteps, writer))
+
+    def _learn(self, total_timesteps, callback, log_interval, reset_num_timesteps, writer):
         callback = as_callback(callback)
         callback.init_callback(self)
         if reset_num_timesteps:
             self.num_timesteps = 0
-        callback.on_training_start({"self": self, "writer": None}, globals())
+        callback.on_training_start({"self": self, "writer": writer}, globals())
+        ep_log = EpisodeRewardLogger(1) if writer is not None else None
         L, N = self.learner, self.timesteps_per_batch
         low, high = self.action_space.low.reshape(-1), self.action_space.high.reshape(-1)
         obs = np.asarray(self.env.reset(), np.float32).reshape(-1)
@@ -202,6 +213,8 @@ class TRPO(BaseModel):
                     if ep is not None:
                         self.ep_info_buf.append(ep)
                 L.rollout_reward(rew, done)
+                if ep_log is not None:
+                    ep_log(writer, rew, done, self.num_timesteps)
                 obs = np.asarray(new_obs, np.float32).reshape(-1)
             callback.on_rollout_end()
             if stopped:
@@ -216,6 +229,9 @@ class TRPO(BaseModel):
             timesteps_so_far += N
             iters_so_far += 1
             self._boundary = (self.num_timesteps, np.random.get_state())
+            if writer is not None:
+                m = self.last_metrics
+                writer.add_summary(Summary([Summary.Value(t, m[k]) for t, k in self._update_tags.items()]), self.num_timesteps)
             if self.verbose >= 1 and (iters_so_far % log_interval == 0 or iters_so_far == 1):
                 print(f"| trpo iteration {iters_so_far} | total_timesteps {self.num_timesteps} | "
                       + " | ".join(f"{k} {v:.5g}" for k, v in self.last_metrics.items()))

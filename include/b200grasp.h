@@ -242,6 +242,21 @@ int b2g_sac_act(b2g_sac* h, const float* obs, int n, int deterministic, float* a
 int b2g_sac_state_save(b2g_sac* h, const char* path);
 int b2g_sac_state_load(b2g_sac* h, const char* path);
 
+/* ---- per-step metrics log (TensorBoard).  With a log enabled every applied gradient step (b2g_sac_step / _async, the
+ *      explicit step with apply_update, b2g_sac_step_host_pipelined; replayed graphs included) appends one row of
+ *      B2G_SAC_LOG_COLS floats to a device ring of `capacity` rows, at row (n_updates - 1) % capacity: policy_loss, qf1_loss,
+ *      qf2_loss, value_loss, ent_coef_loss, entropy, ent_coef (after the update, as b2g_sac_metrics), learning rate.  The
+ *      append is one small kernel inside the step, so the step stays free of host synchronisation.
+ * metrics_log: capacity 0 disables the log (the default); a handle without a log captures and runs the step it always did.
+ *   Enabling (or resizing) empties the ring and recaptures the step graphs; B2G_ESTATE while a host-pipelined step is in flight.
+ * metrics_drain: waits for the handle's stream, then copies up to max_rows of the rows written since the last drain, oldest
+ *   first, to rows[n][B2G_SAC_LOG_COLS]; *first_step = n_updates of the first row (row i is step *first_step + i);
+ *   *lost = rows that were overwritten before this drain (skipped, never silently).  Rows past max_rows stay for the next
+ *   drain.  A training-state load empties the ring.  B2G_ESTATE when the log is off.  Outputs other than rows may be NULL. */
+#define B2G_SAC_LOG_COLS 8
+int b2g_sac_metrics_log(b2g_sac* h, int capacity);
+int b2g_sac_metrics_drain(b2g_sac* h, float* rows, int max_rows, int64_t* first_step, int* n_rows, int64_t* lost);
+
 /* number of kernel launches one gradient step issues (bench.py's gpu_launches) */
 int b2g_launches_per_step(const b2g_sac* h);
 /* device-time of the last b2g_sac_step call measured with CUDA events on the handle's stream (ms) */
@@ -310,6 +325,11 @@ int b2g_bdq_get_last_per(b2g_bdq* h, int32_t* slots, float* weights, float* prio
 int b2g_bdq_step_explicit(b2g_bdq* h, const float* obs, const float* act_idx, const float* rew, const float* next_obs,
                           const float* done, const float* weights, float lr, int apply_update, b2g_bdq_metrics* out,
                           float* td_out);
+/* per-step metrics log, as b2g_sac_metrics_log / _drain: B2G_BDQ_LOG_COLS columns loss, mean_q, grad_norm (as
+ * b2g_bdq_metrics), learning rate; written by b2g_bdq_step and the explicit step with apply_update */
+#define B2G_BDQ_LOG_COLS 4
+int b2g_bdq_metrics_log(b2g_bdq* h, int capacity);
+int b2g_bdq_metrics_drain(b2g_bdq* h, float* rows, int max_rows, int64_t* first_step, int* n_rows, int64_t* lost);
 /* greedy branch indices argmax_n Q_d(s, n) of the online network for n observations */
 int b2g_bdq_act(b2g_bdq* h, const float* obs, int n, int32_t* act_idx_out);
 
@@ -405,6 +425,11 @@ int b2g_dqn_get_last_per(b2g_dqn* h, int32_t* slots, float* weights, float* prio
 /* parity entry point: caller-supplied batch (+ optional importance weights); td_out (may be NULL): [batch] */
 int b2g_dqn_step_explicit(b2g_dqn* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done,
                           const float* weights, float lr, int apply_update, b2g_dqn_metrics* out, float* td_out);
+/* per-step metrics log, as b2g_sac_metrics_log / _drain: B2G_DQN_LOG_COLS columns loss, mean_q, mean_abs_td, grad_norm,
+ * n_clipped (as b2g_dqn_metrics), learning rate; written by b2g_dqn_step and the explicit step with apply_update */
+#define B2G_DQN_LOG_COLS 6
+int b2g_dqn_metrics_log(b2g_dqn* h, int capacity);
+int b2g_dqn_metrics_drain(b2g_dqn* h, float* rows, int max_rows, int64_t* first_step, int* n_rows, int64_t* lost);
 /* one device-to-device copy of the online parameters onto the target parameters */
 int b2g_dqn_update_target(b2g_dqn* h);
 /* greedy actions argmax_k Q(s, k) of the online network for n observations as the network sees them (a VecNormalize
