@@ -1,6 +1,6 @@
-"""``BaseModel`` -- what the SAC, BDQ, DQN and PPO2 front ends share: the env plumbing, the device ownership of VecNormalize's
+"""``BaseModel`` -- what the SAC, BDQ, DQN, PPO2 and TRPO front ends share: the env plumbing, the device ownership of VecNormalize's
 observation statistics, parameters, the stable-baselines zip and training-state directories (training_state.py).  Each
-algorithm keeps its constructor, ``setup_model`` (and with it every parameter-initialisation rule), ``learn``, ``predict``,
+algorithm (PPO2 and TRPO through ``actor_critic.ActorCriticModel``) keeps its constructor, ``setup_model`` (and with it every parameter-initialisation rule), ``learn``, ``predict``,
 ``_data`` (the zip's hyper-parameters) and ``_host_state`` (host.json).
 """
 from __future__ import annotations

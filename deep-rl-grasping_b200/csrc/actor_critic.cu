@@ -1,11 +1,11 @@
-// The actor-critic MLP and rollout kernels the PPO2 and TRPO handles share (actor_critic.cuh).
+// The actor-critic MLP, its rollout and the handle code the PPO2 and TRPO handles share (actor_critic.cuh).
 #include <cuda_runtime.h>
 #include <math.h>
+#include <stdlib.h>
 
 #include <algorithm>
 
 #include "actor_critic.cuh"
-#include "host.cuh"
 
 namespace b2g {
 
@@ -86,14 +86,103 @@ __global__ void ppo_gae_kernel(const float* __restrict__ rew, const float* __res
   }
 }
 
+// rowoff[i] = (first + i) * XS for the actor's rows
+__global__ void ac_iota_rows_kernel(int* __restrict__ rowoff, int first, int n, int XS) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) rowoff[i] = (first + i) * XS;
+}
+
 }  // namespace
+
+int ac_check_net(int obs_dim, int n_actions, int hidden0, int hidden1) {
+  if (obs_dim < 1 || obs_dim > 65536) return b2g_fail(B2G_EINVAL, "obs_dim must be in [1, 65536]");
+  if (n_actions < 1 || n_actions > kAcMaxA) return b2g_fail(B2G_EINVAL, "n_actions must be in [1, 16]");
+  if (hidden0 % 4 || hidden1 % 4 || hidden0 < 4 || hidden1 < 4 || hidden0 > kAcMaxWidth || hidden1 > kAcMaxWidth)
+    return b2g_fail(B2G_EINVAL, "hidden widths must be multiples of 4 in [4, 256]");
+  return 0;
+}
+
+int ac_init(ActorCritic* h, int device, int D, int A, int H0, int H1, int E, int T, int p_rows, uint64_t seed) {
+  h->device = device;
+  h->D = D; h->XS = (int)ac_row_stride(D); h->A = A; h->H0 = H0; h->H1 = H1;
+  h->E = E; h->T = T; h->P_ROWS = p_rows;
+  h->act_key = seed ^ 0xA5A5A5A5DEADBEEFull;       // oracle/philox_ref.py act_seed
+  const char* ng = getenv("B2G_NO_GRAPH");
+  h->use_graph = !(ng && ng[0] == '1');
+  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return b2g_fail(B2G_ECUDA, "stream");
+  return 0;
+}
+
+void ac_layout(ActorCritic* h, const std::string& scope, uint32_t grad_mask, int copies) {
+  const int64_t D = h->D, A = h->A, H0 = h->H0, H1 = h->H1;
+  int64_t off = 0;
+  h->oW0 = arena_take(off, D * 2 * H0); h->ob0 = arena_take(off, 2 * H0);
+  for (int tw = 0; tw < 2; ++tw) { h->oW1[tw] = arena_take(off, H0 * H1); h->ob1[tw] = arena_take(off, H1); }
+  h->oWvf = arena_take(off, H1); h->obvf = arena_take(off, 1); h->oWpi = arena_take(off, H1 * A); h->obpi = arena_take(off, A); h->ols = arena_take(off, A);
+  h->n_train = off;
+  const int64_t oWq = arena_take(off, H1 * A), obq = arena_take(off, A);
+  h->n_total = off;
+  h->n_param = copies * h->n_total;
+  // zip order (oracle/ppo_ref.py param_specs)
+  const struct { const char* name; int64_t rows, cols, stride, off; int ndim; } e[15] = {
+      {"pi_fc0/w", D, H0, 2 * H0, h->oW0, 2},     {"pi_fc0/b", 1, H0, H0, h->ob0, 1},
+      {"vf_fc0/w", D, H0, 2 * H0, h->oW0 + H0, 2}, {"vf_fc0/b", 1, H0, H0, h->ob0 + H0, 1},
+      {"pi_fc1/w", H0, H1, H1, h->oW1[0], 2},     {"pi_fc1/b", 1, H1, H1, h->ob1[0], 1},
+      {"vf_fc1/w", H0, H1, H1, h->oW1[1], 2},     {"vf_fc1/b", 1, H1, H1, h->ob1[1], 1},
+      {"vf/w", H1, 1, 1, h->oWvf, 2},             {"vf/b", 1, 1, 1, h->obvf, 1},
+      {"pi/w", H1, A, A, h->oWpi, 2},             {"pi/b", 1, A, A, h->obpi, 1},
+      {"pi/logstd", 1, A, A, h->ols, 2},
+      {"q/w", H1, A, A, oWq, 2},                  {"q/b", 1, A, A, obq, 1}};
+  for (int i = 0; i < 15; ++i)
+    h->params.add(scope + e[i].name, e[i].rows, e[i].cols, e[i].ndim, (int)e[i].stride, e[i].off, (grad_mask >> i) & 1u);
+}
+
+int ac_alloc(ActorCritic* h, int rows, AcTab& tab) {
+  const int64_t E = h->E, T = h->T, XS = h->XS, A = h->A, H0 = h->H0, H1 = h->H1, R = rows;
+  int rc = 0;
+#define DA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return rc
+  DA(h->P, h->n_param); DA(h->Mo, h->n_train); DA(h->Vo, h->n_train); DA(h->G, h->n_train);
+  DA(h->r_obs, (T + 1) * E * XS); DA(h->r_act, (T + 1) * E * A); DA(h->r_val, (T + 1) * E); DA(h->r_nlp, (T + 1) * E); DA(h->r_rew, T * E);
+  DA(h->r_done, (T + 1) * E); DA(h->r_adv, T * E); DA(h->r_ret, T * E); DA(h->lastv, E);
+  DA(h->p_obs, (int64_t)h->P_ROWS * XS); DA(h->act_rowoff, E);
+  DA(h->Z0, R * 2 * H0); DA(h->Y0, R * 2 * H0); DA(h->Y1, R * 2 * H1);
+  DA(h->a_out, R * A); DA(h->a_v, R); DA(h->a_nlp, R);
+  DA(h->counters, 4);
+#undef DA
+  if (cudaMallocHost((void**)&h->h_buf, kAcHostFloats * sizeof(float)) != cudaSuccess) return b2g_fail(B2G_ECUDA, "cudaMallocHost");
+  auto up = [&](const char* nm, const std::vector<int>& v) {
+    const int* p = nullptr;
+    if (int r2 = upload_table(h->allocs, h->stream, v, &p)) return r2;
+    tab[nm] = p;
+    return 0;
+  };
+  const int D = h->D;
+  if ((rc = up("iD", iota_tab(D))) || (rc = up("iH0", iota_tab((int)H0))) || (rc = up("iH1", iota_tab((int)H1))) ||
+      (rc = up("i2H0", iota_tab(2 * (int)H0))) || (rc = up("rM_2H0", iota_tab(rows, 2 * (int)H0))) ||
+      (rc = up("rM_2H1", iota_tab(rows, 2 * (int)H1))) || (rc = up("iH0_H1", iota_tab((int)H0, (int)H1))) ||
+      (rc = up("iD_2H0", iota_tab(D, 2 * (int)H0))) || (rc = up("boot", iota_tab((int)E, (int)XS, (int)(T * E * XS)))) ||
+      (rc = up("pred", iota_tab(h->P_ROWS, (int)XS))))
+    return rc;
+  if ((rc = ac_make_fwd(h, h->f_act, h->r_obs, h->act_rowoff, (int)E, tab))) return rc;
+  if ((rc = ac_make_fwd(h, h->f_boot, h->r_obs, tab["boot"], (int)E, tab))) return rc;
+  return ac_make_fwd(h, h->f_pred, h->p_obs, tab["pred"], h->P_ROWS, tab);
+}
+
+void ac_release(ActorCritic* h) {
+  cudaSetDevice(h->device);
+  if (h->stream) cudaStreamSynchronize(h->stream);
+  if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
+  for (void* q : h->allocs) cudaFree(q);
+  if (h->h_buf) cudaFreeHost(h->h_buf);
+  if (h->stream) cudaStreamDestroy(h->stream);
+}
 
 int ac_splits_for(int tiles, int R) {
   const int want = (264 + tiles - 1) / tiles;
   return std::max(1, std::min(want, (R + 63) / 64));
 }
 
-int ac_make_fwd(ActorCritic* h, AcFwd& f, const float* obs, const int* rowoff, int M, std::map<std::string, const int*>& tab) {
+int ac_make_fwd(ActorCritic* h, AcFwd& f, const float* obs, const int* rowoff, int M, AcTab& tab) {
   const int D = h->D, H0 = h->H0, H1 = h->H1;
   f.M = M;
   f.l0 = GemmGroup(); f.l1 = GemmGroup();
@@ -144,6 +233,129 @@ void ac_act(const AcActArgs& a, cudaStream_t s) { ppo_act_kernel<<<1, kAcActThre
 void ac_gae(const float* rew, const float* val, const float* done, const float* lastv, int T, int E, float gamma, float lam, float* adv,
             float* ret, cudaStream_t s) {
   ppo_gae_kernel<<<(E + 127) / 128, 128, 0, s>>>(rew, val, done, lastv, T, E, gamma, lam, adv, ret);
+}
+
+int ac_upload_rows(ActorCritic* h, float* dst, const float* src, int rows) {
+  CK(cudaMemcpy2DAsync(dst, h->XS * sizeof(float), src, h->D * sizeof(float), h->D * sizeof(float), rows, cudaMemcpyDefault, h->stream));
+  return 0;
+}
+
+int ac_rollout_act(ActorCritic* h, const float* obs, float* act_out) {
+  CK(cudaSetDevice(h->device));
+  cudaStream_t s = h->stream;
+  if (int rc = ac_upload_rows(h, h->r_obs + (size_t)h->t * h->E * h->XS, obs, h->E)) return rc;
+  ac_iota_rows_kernel<<<(h->E + 255) / 256, 256, 0, s>>>(h->act_rowoff, h->t * h->E, h->E, h->XS);
+  ac_fwd_issue(h, h->f_act, s);
+  AcActArgs a = ac_act_args(h, h->E, 0);
+  a.t = h->t;
+  ac_act(a, s);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(act_out, h->a_out, (size_t)h->E * h->A * sizeof(float), cudaMemcpyDefault, s));
+  CK(cudaStreamSynchronize(s));
+  return 0;
+}
+
+int ac_rollout_reward(ActorCritic* h, const float* rew, const float* done) {
+  CK(cudaSetDevice(h->device));
+  const size_t E = h->E;
+  CK(cudaMemcpyAsync(h->r_rew + (size_t)h->t * E, rew, E * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaMemcpyAsync(h->r_done + (size_t)(h->t + 1) * E, done, E * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaStreamSynchronize(h->stream));      // rew and done may live on the caller's stack
+  h->t += 1;
+  return 0;
+}
+
+int ac_rollout_reset(ActorCritic* h) {
+  CK(cudaSetDevice(h->device));
+  CK(cudaMemsetAsync(h->r_done, 0, (size_t)h->E * sizeof(float), h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  h->t = 0;
+  return 0;
+}
+
+int ac_rollout_get(ActorCritic* h, float* adv, float* ret, float* val, float* nlp, float* act) {
+  CK(cudaSetDevice(h->device));
+  CK(cudaStreamSynchronize(h->stream));
+  const size_t n = (size_t)h->T * h->E;
+  if (adv) CK(cudaMemcpy(adv, h->r_adv, n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (ret) CK(cudaMemcpy(ret, h->r_ret, n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (val) CK(cudaMemcpy(val, h->r_val, n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (nlp) CK(cudaMemcpy(nlp, h->r_nlp, n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (act) CK(cudaMemcpy(act, h->r_act, n * h->A * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int ac_run_update(ActorCritic* h, const std::function<int()>& issue) {
+  if (h->use_graph && !h->graph_exec)
+    if (int rc = capture_graph(h->stream, issue, &h->graph_exec)) return rc;
+  if (h->graph_exec) CK(cudaGraphLaunch(h->graph_exec, h->stream));
+  else if (int rc = issue()) return rc;
+  return 0;
+}
+
+int ac_predict(ActorCritic* h, const float* obs, int n, int deterministic, float* act_out, float* value_out, float* nlp_out) {
+  CK(cudaSetDevice(h->device));
+  cudaStream_t s = h->stream;
+  const int P = h->P_ROWS;
+  for (int done_n = 0; done_n < n; done_n += P) {
+    const int chunk = std::min(P, n - done_n);
+    if (int rc = ac_upload_rows(h, h->p_obs, obs + (size_t)done_n * h->D, chunk)) return rc;
+    ac_fwd_issue(h, h->f_pred, s);
+    AcActArgs a = ac_act_args(h, chunk, 2);
+    a.deterministic = deterministic;
+    ac_act(a, s);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(act_out + (size_t)done_n * h->A, h->a_out, (size_t)chunk * h->A * sizeof(float), cudaMemcpyDefault, s));
+    if (value_out) CK(cudaMemcpyAsync(value_out + done_n, h->a_v, chunk * sizeof(float), cudaMemcpyDefault, s));
+    if (nlp_out) CK(cudaMemcpyAsync(nlp_out + done_n, h->a_nlp, chunk * sizeof(float), cudaMemcpyDefault, s));
+    CK(cudaStreamSynchronize(s));
+  }
+  return 0;
+}
+
+int ac_get_step(ActorCritic* h, int64_t* adam_step, int64_t* noise_step, int32_t* rollout_rows) {
+  CK(cudaSetDevice(h->device));
+  CK(cudaStreamSynchronize(h->stream));
+  long long c[2];
+  CK(cudaMemcpy(c, h->counters, sizeof c, cudaMemcpyDeviceToHost));
+  if (adam_step) *adam_step = c[0];
+  if (noise_step) *noise_step = c[1];
+  if (rollout_rows) *rollout_rows = h->t;
+  return 0;
+}
+
+int ac_state_save(ActorCritic* h, const char* path, uint32_t kind, const std::vector<FpField>& fp) {
+  CK(cudaSetDevice(h->device));
+  CK(cudaStreamSynchronize(h->stream));
+  long long cnt[4];
+  CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
+  int64_t hv[2] = {h->n_updates, 0};
+  std::vector<StateSection> secs = host_sections(hv, sizeof hv, cnt, sizeof cnt);
+  for (auto& s : adam_sections(h->P, h->n_param, h->Mo, h->Vo, h->n_train)) secs.push_back(std::move(s));
+  return state_write(path, kind, fp, secs);
+}
+
+int ac_state_load(ActorCritic* h, const char* path, uint32_t kind, const std::vector<FpField>& fp, const char* learner) {
+  CK(cudaSetDevice(h->device));
+  StateReader rd;
+  if (int rc = rd.open(path, kind, fp)) return rc;
+  const std::vector<StateSection> dev = adam_sections(h->P, h->n_param, h->Mo, h->Vo, h->n_train);
+  if (int rc = state_check_tags(rd, dev, learner)) return rc;
+  int64_t hv[2];
+  long long cnt[4];
+  if (rd.bytes(0) != sizeof hv || rd.bytes(1) != sizeof cnt)
+    return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  if (int rc = state_check_lengths(rd, dev)) return rc;
+  if (int rc = rd.read_host(0, hv, sizeof hv)) return rc;
+  if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
+  CK(cudaStreamSynchronize(h->stream));
+  return state_read_device(rd, dev, &h->broken, [&] {
+    CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
+    CK(cudaMemset(h->r_done, 0, (size_t)h->E * sizeof(float)));
+    h->n_updates = hv[0];
+    h->t = 0;
+    return 0;
+  });
 }
 
 }  // namespace b2g

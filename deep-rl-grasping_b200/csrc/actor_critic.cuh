@@ -1,24 +1,43 @@
 // The actor-critic MLP that the PPO2 (ppo.cu) and TRPO (trpo.cu) handles share (common.policies.MlpPolicy: tanh towers pi and
-// vf of widths [h0, h1] on the flattened observation, a state-independent pi/logstd and the untrained head q), and its
-// single-env-or-more rollout storage: the forward builder, the bias-tanh, actor and GAE kernels (actor_critic.cu).
+// vf of widths [h0, h1] on the flattened observation, a state-independent pi/logstd and the untrained head q), its rollout of
+// T steps of E envs, and what both handles do with them (actor_critic.cu): the parameter arena and the zip's table, the
+// forward builder, the bias-tanh, actor and GAE kernels, the rollout and predict entry points and the training-state file.
+// TRPO's rollout is this rollout with E = 1 and T = timesteps_per_batch.
 //
 // Both towers' first layers are one [D, 2 h0] matrix (pi columns, then vf columns), so layer 0 is one contraction over the
 // shared input.  Arena order: W0, b0, W1 pi, b1 pi, W1 vf, b1 vf, vf/w, vf/b, pi/w, pi/b, pi/logstd (the trained block), then
 // q/w, q/b.
 #pragma once
 #include <cuda_runtime.h>
+#include <stdint.h>
 
 #include <map>
 #include <string>
 #include <vector>
 
 #include "common.cuh"
+#include "host.cuh"
+#include "state.cuh"
 
 namespace b2g {
 
 constexpr int kAcMaxA = 16;           // action components: the kernels keep a row's mean in registers
 constexpr int kAcMaxWidth = 256;      // hidden widths (multiples of 4: 16-byte rows for the engine)
 constexpr int kAcActThreads = 1024;
+constexpr int kAcHostFloats = 64;     // the pinned h_buf
+
+// Sum over the block in a fixed order: the same value on every call.  red holds one T per warp.
+template <class T>
+__device__ __forceinline__ T block_sum_t(T v, T* red) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  T t = 0;
+  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
+  __syncthreads();
+  return t;
+}
 
 struct AcHeadArgs {
   const float* Y1; int h1;             // [rows, 2 h1]: pi latent | vf latent
@@ -57,32 +76,62 @@ struct AcActArgs {
   float* out; float* vout; float* nlpout;
 };
 
-// The network and rollout of one handle.  A handle type derives from it and fills every field at create time.
-struct ActorCritic {
-  int D = 0, XS = 0, A = 0, H0 = 0, H1 = 0;
-  int64_t oW0 = 0, ob0 = 0, oW1[2]{}, ob1[2]{}, oWvf = 0, obvf = 0, oWpi = 0, obpi = 0, ols = 0;
-  float* P = nullptr;                 // parameter arena
-  cudaStream_t stream = nullptr;
-  std::vector<void*> allocs;
-  // rollout: rows of n_envs observations (stride XS), actions, values, neglogp, rewards, episode-start flags, GAE outputs
-  float *r_obs = nullptr, *r_act = nullptr, *r_val = nullptr, *r_nlp = nullptr, *r_rew = nullptr, *r_done = nullptr;
-  float *r_adv = nullptr, *r_ret = nullptr, *lastv = nullptr;
-  int t = 0;                          // rollout rows filled
-  // activations of the forward builder (enough rows for every forward of the handle)
-  float *Z0 = nullptr, *Y0 = nullptr, *Y1 = nullptr;
-  float *a_out = nullptr, *a_v = nullptr, *a_nlp = nullptr;   // actor outputs
-  long long* counters = nullptr;      // [1]: the stream-1 step
-  unsigned long long act_key = 0;
-};
-
 // one forward pass (layers 0 and 1 of both towers) over M rows of an observation arena
 struct AcFwd { GemmGroup l0, l1; int M = 0; };
 
+using AcTab = std::map<std::string, const int*>;
+
+// The network, rollout and bookkeeping of one handle.  A handle type derives from it; ac_init, ac_layout and ac_alloc fill it.
+struct ActorCritic {
+  int device = 0;
+  int D = 0, XS = 0, A = 0, H0 = 0, H1 = 0;
+  int E = 0, T = 0, P_ROWS = 0;       // rollout of T steps of E envs; predict chunks of P_ROWS rows
+  int64_t oW0 = 0, ob0 = 0, oW1[2]{}, ob1[2]{}, oWvf = 0, obvf = 0, oWpi = 0, obpi = 0, ols = 0;
+  int64_t n_train = 0, n_total = 0;   // the trained block; the whole network (q included)
+  int64_t n_param = 0;                // floats of the parameter arena (n_total, or more when the handle keeps copies)
+  ParamTable params;                  // the zip's variables
+  float* P = nullptr;                 // parameter arena
+  float *G = nullptr, *Mo = nullptr, *Vo = nullptr;   // gradient arena and Adam moments, n_train floats each
+  cudaStream_t stream = nullptr;
+  std::vector<void*> allocs;
+  // rollout: rows of E observations (stride XS), actions, values, neglogp, rewards, episode-start flags, GAE outputs; row T
+  // holds the observations after the last step (and the values / actions / neglogp drawn there)
+  float *r_obs = nullptr, *r_act = nullptr, *r_val = nullptr, *r_nlp = nullptr, *r_rew = nullptr, *r_done = nullptr;
+  float *r_adv = nullptr, *r_ret = nullptr, *lastv = nullptr;
+  int t = 0;                          // rollout rows filled
+  float* p_obs = nullptr;             // predict staging, P_ROWS rows
+  int* act_rowoff = nullptr;          // the actor's E row offsets
+  // activations of the forward builder (enough rows for every forward of the handle)
+  float *Z0 = nullptr, *Y0 = nullptr, *Y1 = nullptr;
+  float *a_out = nullptr, *a_v = nullptr, *a_nlp = nullptr;   // actor outputs
+  long long* counters = nullptr;      // [4]: [0] Adam step, [1] the stream-1 step, then the handle's own
+  unsigned long long act_key = 0;
+  float* h_buf = nullptr;             // pinned, kAcHostFloats
+  AcFwd f_act, f_boot, f_pred;        // the rollout step, the bootstrap row T, predict
+  cudaGraphExec_t graph_exec = nullptr;
+  bool use_graph = true;
+  bool broken = false;
+  long long n_updates = 0;
+};
+
+// The configuration checks both handles make first: obs_dim, n_actions and the hidden widths.
+int ac_check_net(int obs_dim, int n_actions, int hidden0, int hidden1);
+inline int64_t ac_row_stride(int obs_dim) { return (obs_dim + 3) / 4 * 4; }
+// Shapes, the actor key (oracle/philox_ref.py act_seed), B2G_NO_GRAPH and the stream.
+int ac_init(ActorCritic* h, int device, int D, int A, int H0, int H1, int E, int T, int p_rows, uint64_t seed);
+// The arena offsets, n_train / n_total / n_param = n_total * copies, and the zip's 15 entries under scope in their order; entry i
+// is in the gradient arena when bit i of grad_mask is set.
+void ac_layout(ActorCritic* h, const std::string& scope, uint32_t grad_mask, int copies);
+// The storage of every ActorCritic field (activations for `rows` rows), the offset tables iD, iH0, iH1, i2H0, rM_2H0, rM_2H1,
+// iH0_H1, iD_2H0, boot and pred into tab, and f_act / f_boot / f_pred.
+int ac_alloc(ActorCritic* h, int rows, AcTab& tab);
+// Frees what the handle holds (not h itself).
+void ac_release(ActorCritic* h);
+
 // split-R so a launch covers about two waves of the 132 SMs, >= 64 rows per slice
 int ac_splits_for(int tiles, int R);
-// Layers 0 and 1 over M rows of `obs` at row offsets rowoff, into Z0 / Y0 / Y1.  tab holds the offset tables iD, iH0, iH1,
-// i2H0, rM_2H0, rM_2H1, iH0_H1 and iD_2H0.
-int ac_make_fwd(ActorCritic* h, AcFwd& f, const float* obs, const int* rowoff, int M, std::map<std::string, const int*>& tab);
+// Layers 0 and 1 over M rows of `obs` at row offsets rowoff, into Z0 / Y0 / Y1, with the tables of ac_alloc.
+int ac_make_fwd(ActorCritic* h, AcFwd& f, const float* obs, const int* rowoff, int M, AcTab& tab);
 void ac_fwd_issue(ActorCritic* h, const AcFwd& f, cudaStream_t s);
 // Y[i] = tanh(Z[i] + b[i % N]) over n rows of N columns
 void ac_bias_tanh(const float* Z, const float* b, float* Y, int n, int N, cudaStream_t s);
@@ -93,5 +142,25 @@ void ac_act(const AcActArgs& a, cudaStream_t s);
 // episode-start flag of step t, done[T] the flags after the last step.
 void ac_gae(const float* rew, const float* val, const float* done, const float* lastv, int T, int E, float gamma, float lam, float* adv,
             float* ret, cudaStream_t s);
+
+// ---- entry-point bodies (the caller has checked the handle and its arguments)
+int ac_upload_rows(ActorCritic* h, float* dst, const float* src, int rows);   // [rows, D] -> rows of stride XS
+// E observations into row t; the forward pass and the actor's draw of step t -> act_out [E, A]
+int ac_rollout_act(ActorCritic* h, const float* obs, float* act_out);
+// row t's E rewards and the next episode-start flags; t += 1
+int ac_rollout_reward(ActorCritic* h, const float* rew, const float* done);
+int ac_rollout_reset(ActorCritic* h);
+int ac_rollout_get(ActorCritic* h, float* adv, float* ret, float* val, float* nlp, float* act);   // nulls are skipped
+// issue() through the update graph (captured on the first call) or directly under B2G_NO_GRAPH=1
+int ac_run_update(ActorCritic* h, const std::function<int()>& issue);
+// in chunks of P_ROWS rows; value_out and nlp_out may be null
+int ac_predict(ActorCritic* h, const float* obs, int n, int deterministic, float* act_out, float* value_out, float* nlp_out);
+int ac_get_step(ActorCritic* h, int64_t* adam_step, int64_t* noise_step, int32_t* rollout_rows);
+
+// ---- training state (container format in state.cuh): HOST {n_updates, 0}, CNTR the 4 counters, then the parameter arena and
+// the Adam moments.  An update boundary: the rollout in flight is not saved; a load leaves an empty rollout with cleared
+// episode-start flags (the env starts a fresh episode).
+int ac_state_save(ActorCritic* h, const char* path, uint32_t kind, const std::vector<FpField>& fp);
+int ac_state_load(ActorCritic* h, const char* path, uint32_t kind, const std::vector<FpField>& fp, const char* learner);
 
 }  // namespace b2g

@@ -1,6 +1,6 @@
 // Host runtime shared by the learner and encoder handles (host.cu): error state, device check, tracked device allocations,
 // offset tables, gather-GEMM descriptor groups, CUDA-graph capture, learning-rate upload, the named-parameter table of the BDQ,
-// DQN and PPO2 handles and NCCL through dlopen.
+// DQN, PPO2 and TRPO handles and NCCL through dlopen.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -77,7 +77,7 @@ int capture_graph(cudaStream_t s, const std::function<int()>& issue, cudaGraphEx
 // Learning rate -> the device scalar the prep kernel reads; only when it changed (the stream is drained first).
 int upload_lr(float* d_lr, float* cur_lr, float lr, cudaStream_t s);
 
-// ---- named parameters of the BDQ, DQN and PPO2 handles: the variables of the zip, in its order, and where each one lives
+// ---- named parameters of the BDQ, DQN, PPO2 and TRPO handles: the variables of the zip, in its order, and where each one lives
 struct ParamEntry {
   std::string name;            // full zip name
   int64_t rows, cols;          // zip shape [rows, cols]; rows = 1 for ndim 1, rows = cols = 1 for a scalar

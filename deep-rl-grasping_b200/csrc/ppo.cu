@@ -55,16 +55,6 @@ enum : int { HP_LR = 0, HP_CLIP, HP_CLIPVF, HP_N = 4 };
 // kernels
 // ---------------------------------------------------------------------------------------------------------------------------
 
-__device__ __forceinline__ float block_sum(float v, float* red) {   // fixed order: the same value on every call
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float t = 0.f;
-  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
-  return t;
-}
-
 // permutation -> storage rows: flattened (env-major) batch index f = e * n_steps + t lives in rollout row t * n_envs + e
 __global__ void ppo_rows_kernel(const int* __restrict__ perm, int n, int n_steps, int n_envs, int XS, int* __restrict__ rowidx,
                                 int* __restrict__ rowoff) {
@@ -74,12 +64,6 @@ __global__ void ppo_rows_kernel(const int* __restrict__ perm, int n, int n_steps
   const int r = t * n_envs + e;
   rowidx[i] = r;
   rowoff[i] = r * XS;
-}
-
-// rowoff[i] = (first + i) * XS for the actor's rows
-__global__ void ppo_iota_rows_kernel(int* __restrict__ rowoff, int first, int n, int XS) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) rowoff[i] = (first + i) * XS;
 }
 
 struct TailArgs2 {
@@ -118,10 +102,10 @@ __global__ void __launch_bounds__(kTailThreads) ppo_tail_kernel(TailArgs2 a) {
     a.sv[r] = v; a.snlp[r] = nlp; a.sadv[r] = adv;
     s += adv;
   }
-  const float mean = block_sum(s, red) * invM;
+  const float mean = block_sum_t(s, red) * invM;
   float ss = 0.f;
   for (int r = tid; r < M; r += NT) { const float d = a.sadv[r] - mean; ss += d * d; }
-  const float stdv = sqrtf(block_sum(ss, red) * invM);        // np.std: population
+  const float stdv = sqrtf(block_sum_t(ss, red) * invM);        // np.std: population
   // ---- losses and the gradient seeds
   float pg_s = 0.f, vf_s = 0.f, kl_s = 0.f, cf_s = 0.f;
   for (int r = tid; r < M; r += NT) {
@@ -153,8 +137,8 @@ __global__ void __launch_bounds__(kTailThreads) ppo_tail_kernel(TailArgs2 a) {
       a.sdls[(size_t)r * A + k] = g_nlp * (1.f - z * z);             // d nlp / d logstd = 1 - z^2
     }
   }
-  const float pg = block_sum(pg_s, red) * invM, vfl = 0.5f * block_sum(vf_s, red) * invM;
-  const float kl = 0.5f * block_sum(kl_s, red) * invM, cf = block_sum(cf_s, red) * invM;
+  const float pg = block_sum_t(pg_s, red) * invM, vfl = 0.5f * block_sum_t(vf_s, red) * invM;
+  const float kl = 0.5f * block_sum_t(kl_s, red) * invM, cf = block_sum_t(cf_s, red) * invM;
   __syncthreads();                                                    // sdm / sdls / sdv of every row are written
   // ---- head backward: dZ1 = dY1 (1 - Y1^2) for both towers
   for (int i = tid; i < M * h1; i += NT) {
@@ -209,7 +193,7 @@ __global__ void __launch_bounds__(kNormThreads) ppo_norm_kernel(const float* __r
     const float4 g = reinterpret_cast<const float4*>(G)[i];
     s += g.x * g.x + g.y * g.y + g.z * g.z + g.w * g.w;
   }
-  const float t = block_sum(s, red);
+  const float t = block_sum_t(s, red);
   if (threadIdx.x == 0) {
     part[blockIdx.x] = t;
     if (blockIdx.x == 0) counters[0] += 1;
@@ -257,44 +241,33 @@ __global__ void __launch_bounds__(256) ppo_adam_kernel(float* __restrict__ P, fl
 
 }  // namespace
 
-// one forward pass (layers 0 and 1) over M rows of an observation arena, and the backward launches of a minibatch
-using PpoFwd = AcFwd;
+// the backward launches of a minibatch after its forward pass
 struct PpoMb { AcFwd f; GemmGroup b1, b0; const int* rowidx = nullptr; };
 
-struct b2g_ppo : ActorCritic {     // network, rollout rows, Z0 / Y0 / Y1, actor outputs, counters [1] (actor_critic.cuh)
+// network, rollout, actor, update graph, counters [0] Adam step, [1] stream-1 step (actor_critic.cuh); h_buf holds metrics and
+// hyper-parameters
+struct b2g_ppo : ActorCritic {
   b2g_ppo_cfg cfg{};
-  int E = 0, T = 0, NB = 0, M = 0, NMB = 0, RMAX = 0, P_ROWS = 0;
-  ParamTable params;            // the zip's variables; q/w and q/b without gradient
-  int64_t n_train = 0, n_total = 0;
-  float *Mo = nullptr, *Vo = nullptr, *G = nullptr;
-  // explicit minibatch and predict staging
-  float *s_obs = nullptr, *s_act = nullptr, *s_val = nullptr, *s_nlp = nullptr, *s_ret = nullptr, *p_obs = nullptr;
+  int NB = 0, M = 0, NMB = 0, RMAX = 0;
+  // explicit minibatch staging
+  float *s_obs = nullptr, *s_act = nullptr, *s_val = nullptr, *s_nlp = nullptr, *s_ret = nullptr;
   // backward activations and scratch (RMAX rows)
   float *dZ1 = nullptr, *dZ0 = nullptr;
   float *sz = nullptr, *sv = nullptr, *snlp = nullptr, *sadv = nullptr, *sdm = nullptr, *sdls = nullptr, *sdv = nullptr;
-  int *perm = nullptr, *rowidx = nullptr, *rowoff = nullptr, *act_rowoff = nullptr;
+  int *perm = nullptr, *rowidx = nullptr, *rowoff = nullptr;
   float *part = nullptr, *met = nullptr, *hp = nullptr;
-  // counters: [0] Adam step, [1] stream-1 step, [2] n_updates
-  float* h_buf = nullptr;         // pinned: metrics, hyper-parameters
-  PpoFwd f_act, f_boot, f_pred;
   PpoMb mb_explicit;
   std::vector<PpoMb> mbs;
-  cudaGraphExec_t graph_exec = nullptr;
-  bool use_graph = true;
-  bool broken = false;
-  long long n_updates = 0;
 };
 
 namespace {
 
-void add_t(b2g_ppo* h, const std::string& name, int rows, int cols, int stride, int64_t off, int ndim) {
-  h->params.add("model/" + name, rows, cols, ndim, stride, off, off < h->n_train);
-}
+constexpr uint32_t kGradMask = (1u << 13) - 1;   // the trained block: every zip entry but q/w and q/b
 
 // the zip names carry the model/ scope; the bare names are accepted too
 std::string scoped(const char* name) { return strncmp(name, "model/", 6) == 0 ? name : "model/" + std::string(name); }
 
-int make_mb(b2g_ppo* h, PpoMb& mb, const float* obs, const int* rowoff, const int* rowidx, std::map<std::string, const int*>& tab) {
+int make_mb(b2g_ppo* h, PpoMb& mb, const float* obs, const int* rowoff, const int* rowidx, AcTab& tab) {
   const int M = h->M, D = h->D, H0 = h->H0, H1 = h->H1;
   if (int rc = ac_make_fwd(h, mb.f, obs, rowoff, M, tab)) return rc;
   mb.rowidx = rowidx;
@@ -378,23 +351,13 @@ int fetch(b2g_ppo* h, b2g_ppo_metrics* out, bool mean_of_update) {
   return 0;
 }
 
-int upload_rows(b2g_ppo* h, float* dst, const float* src, int rows) {   // [rows, D] -> rows of stride XS
-  CK(cudaMemcpy2DAsync(dst, h->XS * sizeof(float), src, h->D * sizeof(float), h->D * sizeof(float), rows, cudaMemcpyDefault, h->stream));
-  return 0;
-}
-
 }  // namespace
 
 extern "C" {
 
 int b2g_ppo_destroy(b2g_ppo* h) {
   if (!h) return 0;
-  cudaSetDevice(h->cfg.device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
-  for (void* q : h->allocs) cudaFree(q);
-  if (h->h_buf) cudaFreeHost(h->h_buf);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  ac_release(h);
   delete h;
   return 0;
 }
@@ -403,10 +366,7 @@ int b2g_ppo_create(const b2g_ppo_cfg* cfg, b2g_ppo** out) {
   if (!cfg || !out) return b2g_fail(B2G_EINVAL, "cfg/out is NULL");
   *out = nullptr;
   const b2g_ppo_cfg& c = *cfg;
-  if (c.obs_dim < 1 || c.obs_dim > 65536) return b2g_fail(B2G_EINVAL, "obs_dim must be in [1, 65536]");
-  if (c.n_actions < 1 || c.n_actions > kMaxA) return b2g_fail(B2G_EINVAL, "n_actions must be in [1, 16]");
-  if (c.hidden0 % 4 || c.hidden1 % 4 || c.hidden0 < 4 || c.hidden1 < 4 || c.hidden0 > kAcMaxWidth || c.hidden1 > kAcMaxWidth)
-    return b2g_fail(B2G_EINVAL, "hidden widths must be multiples of 4 in [4, 256]");
+  if (int rc = ac_check_net(c.obs_dim, c.n_actions, c.hidden0, c.hidden1)) return rc;
   if (c.n_envs < 1 || c.n_envs > 4096) return b2g_fail(B2G_EINVAL, "n_envs must be in [1, 4096]");
   if (c.n_steps < 1 || c.n_steps > 65536) return b2g_fail(B2G_EINVAL, "n_steps must be in [1, 65536]");
   if (c.nminibatches < 1 || c.noptepochs < 1) return b2g_fail(B2G_EINVAL, "nminibatches and noptepochs must be positive");
@@ -414,70 +374,34 @@ int b2g_ppo_create(const b2g_ppo_cfg* cfg, b2g_ppo** out) {
   if (nb % c.nminibatches) return b2g_fail(B2G_EINVAL, "n_batch = n_steps * n_envs must be divisible by nminibatches");
   if (nb / c.nminibatches > kMaxMinibatch) return b2g_fail(B2G_EINVAL, "minibatch n_batch / nminibatches must be <= 16384");
   if ((int64_t)c.noptepochs * c.nminibatches > 4096) return b2g_fail(B2G_EINVAL, "noptepochs * nminibatches must be <= 4096");
-  const int64_t XS = (c.obs_dim + 3) / 4 * 4;
+  const int64_t XS = ac_row_stride(c.obs_dim);
   if ((nb + c.n_envs) * XS >= (1LL << 31)) return b2g_fail(B2G_EINVAL, "rollout (n_steps + 1) * n_envs * obs_dim must be < 2^31 floats");
   if (int rc = check_device(c.device)) return rc;
   b2g_ppo* h = new b2g_ppo();
   h->cfg = c;
-  const char* ng = getenv("B2G_NO_GRAPH");
-  h->use_graph = !(ng && ng[0] == '1');
-  h->D = c.obs_dim; h->XS = (int)XS; h->A = c.n_actions; h->H0 = c.hidden0; h->H1 = c.hidden1;
-  h->E = c.n_envs; h->T = c.n_steps; h->NB = (int)nb; h->NMB = c.nminibatches; h->M = (int)(nb / c.nminibatches);
-  h->P_ROWS = std::max(64, h->E);
-  h->RMAX = std::max(h->M, h->P_ROWS);
-  h->act_key = c.seed ^ 0xA5A5A5A5DEADBEEFull;       // oracle/philox_ref.py act_seed
   auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_ppo_destroy(h); g_b2g_err = keep; return rc; };
-  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream"));
-  // ---- parameter arena: trained tensors, then q (no gradient, no moments)
-  const int D = h->D, A = h->A, H0 = h->H0, H1 = h->H1;
-  int64_t off = 0;
-  h->oW0 = arena_take(off, (int64_t)D * 2 * H0); h->ob0 = arena_take(off, 2 * H0);
-  for (int tw = 0; tw < 2; ++tw) { h->oW1[tw] = arena_take(off, (int64_t)H0 * H1); h->ob1[tw] = arena_take(off, H1); }
-  h->oWvf = arena_take(off, H1); h->obvf = arena_take(off, 1); h->oWpi = arena_take(off, (int64_t)H1 * A); h->obpi = arena_take(off, A); h->ols = arena_take(off, A);
-  h->n_train = off;
-  const int64_t oWq = arena_take(off, (int64_t)H1 * A), obq = arena_take(off, A);
-  h->n_total = off;
-  // zip order (oracle/ppo_ref.py param_specs)
-  add_t(h, "pi_fc0/w", D, H0, 2 * H0, h->oW0, 2); add_t(h, "pi_fc0/b", 1, H0, H0, h->ob0, 1);
-  add_t(h, "vf_fc0/w", D, H0, 2 * H0, h->oW0 + H0, 2); add_t(h, "vf_fc0/b", 1, H0, H0, h->ob0 + H0, 1);
-  add_t(h, "pi_fc1/w", H0, H1, H1, h->oW1[0], 2); add_t(h, "pi_fc1/b", 1, H1, H1, h->ob1[0], 1);
-  add_t(h, "vf_fc1/w", H0, H1, H1, h->oW1[1], 2); add_t(h, "vf_fc1/b", 1, H1, H1, h->ob1[1], 1);
-  add_t(h, "vf/w", H1, 1, 1, h->oWvf, 2); add_t(h, "vf/b", 1, 1, 1, h->obvf, 1);
-  add_t(h, "pi/w", H1, A, A, h->oWpi, 2); add_t(h, "pi/b", 1, A, A, h->obpi, 1);
-  add_t(h, "pi/logstd", 1, A, A, h->ols, 2);
-  add_t(h, "q/w", H1, A, A, oWq, 2); add_t(h, "q/b", 1, A, A, obq, 1);
-  int rc = 0;
-  const int64_t E = h->E, T = h->T, R = h->RMAX;
-#define DA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
-  DA(h->P, h->n_total); DA(h->Mo, h->n_train); DA(h->Vo, h->n_train); DA(h->G, h->n_train);
-  DA(h->r_obs, (T + 1) * E * XS); DA(h->r_act, T * E * A); DA(h->r_val, T * E); DA(h->r_nlp, T * E); DA(h->r_rew, T * E);
-  DA(h->r_done, (T + 1) * E); DA(h->r_adv, T * E); DA(h->r_ret, T * E); DA(h->lastv, E);
-  DA(h->s_obs, (int64_t)h->M * XS); DA(h->s_act, (int64_t)h->M * A); DA(h->s_val, h->M); DA(h->s_nlp, h->M); DA(h->s_ret, h->M);
-  DA(h->p_obs, (int64_t)h->P_ROWS * XS);
-  DA(h->Z0, R * 2 * H0); DA(h->Y0, R * 2 * H0); DA(h->Y1, R * 2 * H1); DA(h->dZ1, R * 2 * H1); DA(h->dZ0, R * 2 * H0);
-  DA(h->sz, R * A); DA(h->sv, R); DA(h->snlp, R); DA(h->sadv, R); DA(h->sdm, R * A); DA(h->sdls, R * A); DA(h->sdv, R);
-  DA(h->a_out, R * A); DA(h->a_v, R); DA(h->a_nlp, R);
-  const int64_t nperm = (int64_t)c.noptepochs * h->NB;
-  DA(h->perm, nperm); DA(h->rowidx, nperm); DA(h->rowoff, nperm); DA(h->act_rowoff, E);
-  DA(h->part, kNormBlocks); DA(h->met, 2 * PM_N); DA(h->hp, HP_N); DA(h->counters, 4);
-#undef DA
-  if (cudaMallocHost((void**)&h->h_buf, 64 * sizeof(float)) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "cudaMallocHost"));
-  // ---- offset tables and descriptor groups
-  std::map<std::string, const int*> tab;
-  auto T_ = [&](const char* nm, const std::vector<int>& v) {
-    const int* p = nullptr;
-    if (int r2 = upload_table(h->allocs, h->stream, v, &p)) return r2;
-    tab[nm] = p;
-    return 0;
-  };
-  if ((rc = T_("iD", iota_tab(D))) || (rc = T_("iH0", iota_tab(H0))) || (rc = T_("iH1", iota_tab(H1))) || (rc = T_("i2H0", iota_tab(2 * H0))) ||
-      (rc = T_("rM_2H0", iota_tab((int)R, 2 * H0))) || (rc = T_("rM_2H1", iota_tab((int)R, 2 * H1))) ||
-      (rc = T_("iH0_H1", iota_tab(H0, H1))) || (rc = T_("iD_2H0", iota_tab(D, 2 * H0))) || (rc = T_("boot", iota_tab((int)E, h->XS, (int)(T * E) * h->XS))) ||
-      (rc = T_("pred", iota_tab(h->P_ROWS, h->XS))) || (rc = T_("sM", iota_tab(h->M, h->XS))) || (rc = T_("iM", iota_tab(h->M))))
+  if (int rc = ac_init(h, c.device, c.obs_dim, c.n_actions, c.hidden0, c.hidden1, c.n_envs, c.n_steps, std::max(64, c.n_envs), c.seed))
     return bail(rc);
-  if ((rc = ac_make_fwd(h, h->f_act, h->r_obs, h->act_rowoff, (int)E, tab))) return bail(rc);
-  if ((rc = ac_make_fwd(h, h->f_boot, h->r_obs, tab["boot"], (int)E, tab))) return bail(rc);
-  if ((rc = ac_make_fwd(h, h->f_pred, h->p_obs, tab["pred"], h->P_ROWS, tab))) return bail(rc);
+  h->NB = (int)nb; h->NMB = c.nminibatches; h->M = (int)(nb / c.nminibatches);
+  h->RMAX = std::max(h->M, h->P_ROWS);
+  ac_layout(h, "model/", kGradMask, 1);
+  AcTab tab;
+  int rc = ac_alloc(h, h->RMAX, tab);
+  if (rc) return bail(rc);
+  const int64_t A = h->A, H0 = h->H0, H1 = h->H1, R = h->RMAX;
+#define DA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
+  DA(h->s_obs, (int64_t)h->M * XS); DA(h->s_act, (int64_t)h->M * A); DA(h->s_val, h->M); DA(h->s_nlp, h->M); DA(h->s_ret, h->M);
+  DA(h->dZ1, R * 2 * H1); DA(h->dZ0, R * 2 * H0);
+  DA(h->sz, R * A); DA(h->sv, R); DA(h->snlp, R); DA(h->sadv, R); DA(h->sdm, R * A); DA(h->sdls, R * A); DA(h->sdv, R);
+  const int64_t nperm = (int64_t)c.noptepochs * h->NB;
+  DA(h->perm, nperm); DA(h->rowidx, nperm); DA(h->rowoff, nperm);
+  DA(h->part, kNormBlocks); DA(h->met, 2 * PM_N); DA(h->hp, HP_N);
+#undef DA
+  for (auto& [nm, v] : {std::make_pair("sM", iota_tab(h->M, h->XS)), std::make_pair("iM", iota_tab(h->M))}) {
+    const int* p = nullptr;
+    if ((rc = upload_table(h->allocs, h->stream, v, &p))) return bail(rc);
+    tab[nm] = p;
+  }
   if ((rc = make_mb(h, h->mb_explicit, h->s_obs, tab["sM"], tab["iM"], tab))) return bail(rc);
   h->mbs.resize((size_t)c.noptepochs * c.nminibatches);
   for (size_t k = 0; k < h->mbs.size(); ++k)
@@ -505,55 +429,26 @@ int b2g_ppo_rollout_act(b2g_ppo* h, const float* obs, float* act_out) {
   B2G_USABLE(h);
   if (!h || !obs || !act_out) return b2g_fail(B2G_EINVAL, "NULL argument");
   if (h->t >= h->T) return b2g_fail(B2G_ESTATE, "the rollout holds n_steps rows: call b2g_ppo_update first");
-  CK(cudaSetDevice(h->cfg.device));
-  cudaStream_t s = h->stream;
-  if (int rc = upload_rows(h, h->r_obs + (size_t)h->t * h->E * h->XS, obs, h->E)) return rc;
-  ppo_iota_rows_kernel<<<(h->E + 255) / 256, 256, 0, s>>>(h->act_rowoff, h->t * h->E, h->E, h->XS);
-  ac_fwd_issue(h, h->f_act, s);
-  AcActArgs a = ac_act_args(h, h->E, 0);
-  a.t = h->t;
-  ac_act(a, s);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(act_out, h->a_out, (size_t)h->E * h->A * sizeof(float), cudaMemcpyDefault, s));
-  CK(cudaStreamSynchronize(s));
-  return 0;
+  return ac_rollout_act(h, obs, act_out);
 }
 
 int b2g_ppo_rollout_reward(b2g_ppo* h, const float* rew, const float* done) {
   B2G_USABLE(h);
   if (!h || !rew || !done) return b2g_fail(B2G_EINVAL, "NULL argument");
   if (h->t >= h->T) return b2g_fail(B2G_ESTATE, "the rollout holds n_steps rows: call b2g_ppo_update first");
-  CK(cudaSetDevice(h->cfg.device));
-  const size_t E = h->E;
-  CK(cudaMemcpyAsync(h->r_rew + (size_t)h->t * E, rew, E * sizeof(float), cudaMemcpyDefault, h->stream));
-  CK(cudaMemcpyAsync(h->r_done + (size_t)(h->t + 1) * E, done, E * sizeof(float), cudaMemcpyDefault, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  h->t += 1;
-  return 0;
+  return ac_rollout_reward(h, rew, done);
 }
 
 int b2g_ppo_rollout_reset(b2g_ppo* h) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaMemsetAsync(h->r_done, 0, (size_t)h->E * sizeof(float), h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  h->t = 0;
-  return 0;
+  return ac_rollout_reset(h);
 }
 
 int b2g_ppo_rollout_get(b2g_ppo* h, float* adv, float* ret, float* val, float* nlp, float* act) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  const size_t n = (size_t)h->T * h->E;
-  if (adv) CK(cudaMemcpy(adv, h->r_adv, n * sizeof(float), cudaMemcpyDeviceToHost));
-  if (ret) CK(cudaMemcpy(ret, h->r_ret, n * sizeof(float), cudaMemcpyDeviceToHost));
-  if (val) CK(cudaMemcpy(val, h->r_val, n * sizeof(float), cudaMemcpyDeviceToHost));
-  if (nlp) CK(cudaMemcpy(nlp, h->r_nlp, n * sizeof(float), cudaMemcpyDeviceToHost));
-  if (act) CK(cudaMemcpy(act, h->r_act, n * h->A * sizeof(float), cudaMemcpyDeviceToHost));
-  return 0;
+  return ac_rollout_get(h, adv, ret, val, nlp, act);
 }
 
 int b2g_ppo_update(b2g_ppo* h, const float* last_obs, const int32_t* perm, float lr, float cliprange, float cliprange_vf,
@@ -566,12 +461,9 @@ int b2g_ppo_update(b2g_ppo* h, const float* last_obs, const int32_t* perm, float
     if (perm[i] < 0 || perm[i] >= h->NB) return b2g_fail(B2G_EINVAL, "permutation entry " + std::to_string(i) + " is outside [0, n_batch)");
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = upload_hp(h, lr, cliprange, cliprange_vf)) return rc;
-  if (int rc = upload_rows(h, h->r_obs + (size_t)h->T * h->E * h->XS, last_obs, h->E)) return rc;
+  if (int rc = ac_upload_rows(h, h->r_obs + (size_t)h->T * h->E * h->XS, last_obs, h->E)) return rc;
   CK(cudaMemcpyAsync(h->perm, perm, n * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
-  if (h->use_graph && !h->graph_exec)
-    if (int rc = capture_graph(h->stream, [&] { return update_issue(h); }, &h->graph_exec)) return rc;
-  if (h->graph_exec) CK(cudaGraphLaunch(h->graph_exec, h->stream));
-  else if (int rc = update_issue(h)) return rc;
+  if (int rc = ac_run_update(h, [&] { return update_issue(h); })) return rc;
   h->n_updates += (int64_t)h->mbs.size();
   h->t = 0;
   return fetch(h, out, true);
@@ -585,7 +477,7 @@ int b2g_ppo_train_step_explicit(b2g_ppo* h, const float* obs, const float* retur
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = upload_hp(h, lr, cliprange, cliprange_vf)) return rc;
   const size_t M = h->M;
-  if (int rc = upload_rows(h, h->s_obs, obs, h->M)) return rc;
+  if (int rc = ac_upload_rows(h, h->s_obs, obs, h->M)) return rc;
   CK(cudaMemcpyAsync(h->s_ret, returns, M * sizeof(float), cudaMemcpyDefault, h->stream));
   CK(cudaMemcpyAsync(h->s_act, actions, M * h->A * sizeof(float), cudaMemcpyDefault, h->stream));
   CK(cudaMemcpyAsync(h->s_val, values, M * sizeof(float), cudaMemcpyDefault, h->stream));
@@ -608,43 +500,19 @@ int b2g_ppo_train_step_explicit(b2g_ppo* h, const float* obs, const float* retur
 int b2g_ppo_act(b2g_ppo* h, const float* obs, int n, int deterministic, float* act_out, float* value_out, float* neglogp_out) {
   B2G_USABLE(h);
   if (!h || !obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
-  CK(cudaSetDevice(h->cfg.device));
-  cudaStream_t s = h->stream;
-  const int P = h->P_ROWS;
-  for (int done_n = 0; done_n < n; done_n += P) {
-    const int chunk = std::min(P, n - done_n);
-    if (int rc = upload_rows(h, h->p_obs, obs + (size_t)done_n * h->D, chunk)) return rc;
-    ac_fwd_issue(h, h->f_pred, s);
-    AcActArgs a = ac_act_args(h, chunk, 2);
-    a.deterministic = deterministic;
-    ac_act(a, s);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(act_out + (size_t)done_n * h->A, h->a_out, (size_t)chunk * h->A * sizeof(float), cudaMemcpyDefault, s));
-    if (value_out) CK(cudaMemcpyAsync(value_out + done_n, h->a_v, chunk * sizeof(float), cudaMemcpyDefault, s));
-    if (neglogp_out) CK(cudaMemcpyAsync(neglogp_out + done_n, h->a_nlp, chunk * sizeof(float), cudaMemcpyDefault, s));
-    CK(cudaStreamSynchronize(s));
-  }
-  return 0;
+  return ac_predict(h, obs, n, deterministic, act_out, value_out, neglogp_out);
 }
 
 int b2g_ppo_get_step(b2g_ppo* h, int64_t* adam_step, int64_t* noise_step, int32_t* rollout_rows) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  long long c[2];
-  CK(cudaMemcpy(c, h->counters, sizeof c, cudaMemcpyDeviceToHost));
-  if (adam_step) *adam_step = c[0];
-  if (noise_step) *noise_step = c[1];
-  if (rollout_rows) *rollout_rows = h->t;
-  return 0;
+  return ac_get_step(h, adam_step, noise_step, rollout_rows);
 }
 
 }  // extern "C"
 
 // ================================================================================================
-// Training state (b2g_ppo_state_save / _load; container format in state.cuh).  An update boundary: the rollout in flight is
-// not saved; a loaded handle starts an empty rollout with cleared episode-start flags (the env starts a fresh episode).
+// Training state (b2g_ppo_state_save / _load; ac_state_save in actor_critic.cuh)
 // ================================================================================================
 namespace {
 
@@ -655,9 +523,6 @@ std::vector<FpField> ppo_fingerprint(const b2g_ppo* h) {
           fp_int("seed", (int64_t)c.seed)};
 }
 
-// sections 2..: parameters (q included) and the Adam moments
-std::vector<StateSection> ppo_device_sections(b2g_ppo* h) { return adam_sections(h->P, h->n_total, h->Mo, h->Vo, h->n_train); }
-
 }  // namespace
 
 extern "C" {
@@ -665,38 +530,12 @@ extern "C" {
 int b2g_ppo_state_save(b2g_ppo* h, const char* path) {
   if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
   B2G_USABLE(h);
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  long long cnt[4];
-  CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
-  int64_t hv[2] = {h->n_updates, 0};
-  std::vector<StateSection> secs = host_sections(hv, sizeof hv, cnt, sizeof cnt);
-  for (auto& s : ppo_device_sections(h)) secs.push_back(std::move(s));
-  return state_write(path, STATE_KIND_PPO, ppo_fingerprint(h), secs);
+  return ac_state_save(h, path, STATE_KIND_PPO, ppo_fingerprint(h));
 }
 
 int b2g_ppo_state_load(b2g_ppo* h, const char* path) {
   if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
-  CK(cudaSetDevice(h->cfg.device));
-  StateReader rd;
-  if (int rc = rd.open(path, STATE_KIND_PPO, ppo_fingerprint(h))) return rc;
-  const std::vector<StateSection> dev = ppo_device_sections(h);
-  if (int rc = state_check_tags(rd, dev, "PPO2")) return rc;
-  int64_t hv[2];
-  long long cnt[4];
-  if (rd.bytes(0) != sizeof hv || rd.bytes(1) != sizeof cnt)
-    return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
-  if (int rc = state_check_lengths(rd, dev)) return rc;
-  if (int rc = rd.read_host(0, hv, sizeof hv)) return rc;
-  if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
-  CK(cudaStreamSynchronize(h->stream));
-  return state_read_device(rd, dev, &h->broken, [&] {
-    CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
-    CK(cudaMemset(h->r_done, 0, (size_t)h->E * sizeof(float)));
-    h->n_updates = hv[0];
-    h->t = 0;
-    return 0;
-  });
+  return ac_state_load(h, path, STATE_KIND_PPO, ppo_fingerprint(h), "PPO2");
 }
 
 }  // extern "C"

@@ -52,20 +52,6 @@ enum : int { TM_BEFORE = 0, TM_AFTER = 5, TM_GG = 10, TM_SHS, TM_EI, TM_VF, TM_N
 // device scalars (double)
 enum : int { SC_RR = 0, SC_ALPHA, SC_BETA, SC_DONE, SC_ZERO, SC_BAD, SC_ITERS, SC_ACC, SC_LM, SC_N = 16 };
 
-template <class T>
-__device__ __forceinline__ T block_sum_t(T v, T* red) {   // fixed order: the same value on every call
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  T t = 0;
-  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
-  __syncthreads();
-  return t;
-}
-
-__global__ void trpo_set_row_kernel(int* rowoff, int v) { *rowoff = v; }
-
 // the value minibatches' storage rows: rowoff[i] = perm[i] * XS
 __global__ void trpo_rows_kernel(const int* __restrict__ perm, int n, int XS, int* __restrict__ rowoff) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -521,37 +507,34 @@ struct VfMb { VfFwd f; TowerBwd b; const int* perm = nullptr; };
 // the tangent launches of the Fisher-vector product
 struct FvpLaunch { GemmGroup t0, t1; TowerBwd b; };
 
-struct b2g_trpo : ActorCritic {     // network, rollout rows, Z0 / Y0 / Y1, actor outputs, counters (actor_critic.cuh)
+// network, rollout of E = 1 env, actor, update graph, counters [0] value-Adam step, [1] stream-1 step (actor_critic.cuh); Mo / Vo
+// are the value Adam's moments, G the policy gradient g; h_buf holds metrics and scalars
+struct b2g_trpo : ActorCritic {
   b2g_trpo_cfg cfg{};
-  int N = 0, NF = 0, RMAX = 0, P_ROWS = 0, NVMB = 0;
-  ParamTable params;
-  int64_t n_train = 0, n_total = 0, n_policy = 0;
-  float *Mo = nullptr, *Vo = nullptr, *G = nullptr, *Gv = nullptr;      // value Adam moments, policy gradient g, value gradient
+  int N = 0, NF = 0, RMAX = 0, NVMB = 0;
+  float* Gv = nullptr;              // value gradient
   float *X = nullptr, *Rv = nullptr, *Pv = nullptr, *Zv = nullptr, *FS = nullptr;   // CG vectors and the full step
-  float *p_obs = nullptr;
   float *atarg = nullptr, *mu_old = nullptr, *nlp_old = nullptr, *sdm = nullptr, *sdls = nullptr, *u = nullptr;
   float *dZ1 = nullptr, *dZ0 = nullptr, *T0 = nullptr, *T1 = nullptr;
   float *dZls = nullptr, *Y0c = nullptr, *Y1c = nullptr, *cand = nullptr;
   float *vZ0 = nullptr, *vY0 = nullptr, *vY1 = nullptr, *vdZ1 = nullptr, *vdZ0 = nullptr;
-  int *perm = nullptr, *vrowoff = nullptr, *act_rowoff = nullptr;
+  int *perm = nullptr, *vrowoff = nullptr;
   double *part = nullptr, *amax = nullptr, *lspart = nullptr, *sc = nullptr;
   float* met = nullptr;
-  float* h_buf = nullptr;           // pinned: metrics and scalars
-  AcFwd f_act, f_boot, f_pred, f_all;
+  AcFwd f_all;
   TowerBwd gbwd;
   FvpLaunch fvp;
   GemmGroup ls_dz, ls_l1;
   std::vector<VfMb> vmbs;
-  cudaGraphExec_t graph_exec = nullptr;
-  bool use_graph = true;
-  bool broken = false;
   bool carried = false;             // rollout row 0 holds the boundary observation and action of the last update
-  long long n_iterations = 0;
 };
 
 namespace {
 
-using Tab = std::map<std::string, const int*>;
+using Tab = AcTab;
+static_assert(TM_N + 2 * SC_N <= kAcHostFloats, "h_buf holds the metrics and the scalars");
+// the policy variables pi_fc0, pi_fc1 and pi (zip entries 0, 1, 4, 5, 10, 11, 12): the gradient arena of the policy step
+constexpr uint32_t kGradMask = (1u << 0) | (1u << 1) | (1u << 4) | (1u << 5) | (1u << 10) | (1u << 11) | (1u << 12);
 
 // tower tw's backward over M rows: obs rows xrows, layer-0 outputs at y0 (rows y0rows, tower column base applied), compact dZ1 /
 // dZ0; gradients into the arena `out`
@@ -783,32 +766,24 @@ int fetch(b2g_trpo* h, b2g_trpo_metrics* out) {
     out->grad_sq = m[TM_GG]; out->shs = m[TM_SHS]; out->expected_improve = m[TM_EI];
     out->vf_loss = h->vmbs.empty() ? 0.f : m[TM_VF] / (float)h->vmbs.size();
     out->cg_iters = (int32_t)hs[SC_ITERS]; out->accepted = (int32_t)hs[SC_ACC];
-    out->n_iterations = h->n_iterations;
+    out->n_iterations = h->n_updates;
   }
   if (hs[SC_BAD] != 0.0) return b2g_fail(B2G_ESTATE, "the conjugate-gradient step direction is not finite");
   return 0;
 }
 
-int upload_rows(b2g_trpo* h, float* dst, const float* src, int rows) {   // [rows, D] -> rows of stride XS
-  CK(cudaMemcpy2DAsync(dst, h->XS * sizeof(float), src, h->D * sizeof(float), h->D * sizeof(float), rows, cudaMemcpyDefault, h->stream));
-  return 0;
-}
-
-// the policy variables (var_list order) <-> the arena layout of the gradient / CG vectors
-const char* const kPolicyVars[7] = {"pi/model/pi_fc0/w", "pi/model/pi_fc0/b", "pi/model/pi_fc1/w", "pi/model/pi_fc1/b",
-                                    "pi/model/pi/w", "pi/model/pi/b", "pi/model/pi/logstd"};
-
+// the policy variables (var_list order: the gradient arena's entries in zip order) <-> the arena layout of the gradient / CG
+// vectors
 void flat_arena(const b2g_trpo* h, float* flat, float* arena, bool to_arena) {
   size_t k = 0;
-  for (const char* nm : kPolicyVars)
-    for (const ParamEntry& e : h->params.entries()) {
-      if (e.name != nm) continue;
-      for (int64_t r = 0; r < e.rows; ++r)
-        for (int64_t c = 0; c < e.cols; ++c, ++k) {
-          float& a = arena[e.off + r * e.stride + c];
-          if (to_arena) a = flat[k]; else flat[k] = a;
-        }
-    }
+  for (const ParamEntry& e : h->params.entries()) {
+    if (!e.grad) continue;
+    for (int64_t r = 0; r < e.rows; ++r)
+      for (int64_t c = 0; c < e.cols; ++c, ++k) {
+        float& a = arena[e.off + r * e.stride + c];
+        if (to_arena) a = flat[k]; else flat[k] = a;
+      }
+  }
 }
 
 int download_flat(b2g_trpo* h, const float* dev, float* flat) {
@@ -819,22 +794,13 @@ int download_flat(b2g_trpo* h, const float* dev, float* flat) {
   return 0;
 }
 
-void add_var(b2g_trpo* h, const std::string& name, int rows, int cols, int stride, int64_t off, int ndim, bool policy) {
-  h->params.add("pi/model/" + name, rows, cols, ndim, stride, off, policy);
-}
-
 }  // namespace
 
 extern "C" {
 
 int b2g_trpo_destroy(b2g_trpo* h) {
   if (!h) return 0;
-  cudaSetDevice(h->cfg.device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
-  for (void* q : h->allocs) cudaFree(q);
-  if (h->h_buf) cudaFreeHost(h->h_buf);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  ac_release(h);
   delete h;
   return 0;
 }
@@ -843,16 +809,13 @@ int b2g_trpo_create(const b2g_trpo_cfg* cfg, b2g_trpo** out) {
   if (!cfg || !out) return b2g_fail(B2G_EINVAL, "cfg/out is NULL");
   *out = nullptr;
   const b2g_trpo_cfg& c = *cfg;
-  if (c.obs_dim < 1 || c.obs_dim > 65536) return b2g_fail(B2G_EINVAL, "obs_dim must be in [1, 65536]");
-  if (c.n_actions < 1 || c.n_actions > kAcMaxA) return b2g_fail(B2G_EINVAL, "n_actions must be in [1, 16]");
-  if (c.hidden0 % 4 || c.hidden1 % 4 || c.hidden0 < 4 || c.hidden1 < 4 || c.hidden0 > kAcMaxWidth || c.hidden1 > kAcMaxWidth)
-    return b2g_fail(B2G_EINVAL, "hidden widths must be multiples of 4 in [4, 256]");
+  if (int rc = ac_check_net(c.obs_dim, c.n_actions, c.hidden0, c.hidden1)) return rc;
   if (c.timesteps_per_batch < 1 || c.timesteps_per_batch > kMaxN) return b2g_fail(B2G_EINVAL, "timesteps_per_batch must be in [1, 16384]");
   if (c.cg_iters < 1 || c.cg_iters > 64) return b2g_fail(B2G_EINVAL, "cg_iters must be in [1, 64]");
   if (c.vf_iters < 0 || c.vf_iters > 64) return b2g_fail(B2G_EINVAL, "vf_iters must be in [0, 64]");
   if (!(c.max_kl > 0.f)) return b2g_fail(B2G_EINVAL, "max_kl must be > 0");
   if (!(c.cg_damping >= 0.f) || !(c.vf_stepsize >= 0.f)) return b2g_fail(B2G_EINVAL, "cg_damping and vf_stepsize must be >= 0");
-  const int64_t XS = (c.obs_dim + 3) / 4 * 4;
+  const int64_t XS = ac_row_stride(c.obs_dim);
   if ((int64_t)(c.timesteps_per_batch + 1) * XS >= (1LL << 31))
     return b2g_fail(B2G_EINVAL, "rollout (timesteps_per_batch + 1) * obs_dim must be < 2^31 floats");
   if (int rc = check_device(c.device)) return rc;
@@ -867,73 +830,42 @@ int b2g_trpo_create(const b2g_trpo_cfg* cfg, b2g_trpo** out) {
   }
   b2g_trpo* h = new b2g_trpo();
   h->cfg = c;
-  const char* ng = getenv("B2G_NO_GRAPH");
-  h->use_graph = !(ng && ng[0] == '1');
-  h->D = c.obs_dim; h->XS = (int)XS; h->A = c.n_actions; h->H0 = c.hidden0; h->H1 = c.hidden1;
-  h->N = (int)N; h->NF = (int)((N + 4) / 5); h->P_ROWS = 64;
+  auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_trpo_destroy(h); g_b2g_err = keep; return rc; };
+  if (int rc = ac_init(h, c.device, c.obs_dim, c.n_actions, c.hidden0, c.hidden1, 1, (int)N, 64, c.seed)) return bail(rc);
+  h->N = (int)N; h->NF = (int)((N + 4) / 5);
   h->RMAX = (int)std::max<int64_t>(N + 1, h->P_ROWS);
   h->NVMB = c.vf_iters * (int)(N / kVfBatch);
-  h->act_key = c.seed ^ 0xA5A5A5A5DEADBEEFull;       // the PPO2 actor's key (stream 1)
-  auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_trpo_destroy(h); g_b2g_err = keep; return rc; };
-  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream"));
-  const int D = h->D, A = h->A;
-  int64_t off = 0;
-  h->oW0 = arena_take(off, (int64_t)D * 2 * H0); h->ob0 = arena_take(off, 2 * H0);
-  for (int tw = 0; tw < 2; ++tw) { h->oW1[tw] = arena_take(off, H0 * H1); h->ob1[tw] = arena_take(off, H1); }
-  h->oWvf = arena_take(off, H1); h->obvf = arena_take(off, 1); h->oWpi = arena_take(off, H1 * A); h->obpi = arena_take(off, A); h->ols = arena_take(off, A);
-  h->n_train = off;
-  const int64_t oWq = arena_take(off, H1 * A), obq = arena_take(off, A);
-  h->n_total = off;
-  h->n_policy = (int64_t)D * H0 + H0 + H0 * H1 + H1 + H1 * A + 2 * A;
-  // zip order: pi/model/... (PPO2's creation order), then the same under oldpi/model/
-  add_var(h, "pi_fc0/w", D, H0, 2 * H0, h->oW0, 2, true); add_var(h, "pi_fc0/b", 1, H0, H0, h->ob0, 1, true);
-  add_var(h, "vf_fc0/w", D, H0, 2 * H0, h->oW0 + H0, 2, false); add_var(h, "vf_fc0/b", 1, H0, H0, h->ob0 + H0, 1, false);
-  add_var(h, "pi_fc1/w", H0, H1, H1, h->oW1[0], 2, true); add_var(h, "pi_fc1/b", 1, H1, H1, h->ob1[0], 1, true);
-  add_var(h, "vf_fc1/w", H0, H1, H1, h->oW1[1], 2, false); add_var(h, "vf_fc1/b", 1, H1, H1, h->ob1[1], 1, false);
-  add_var(h, "vf/w", H1, 1, 1, h->oWvf, 2, false); add_var(h, "vf/b", 1, 1, 1, h->obvf, 1, false);
-  add_var(h, "pi/w", H1, A, A, h->oWpi, 2, true); add_var(h, "pi/b", 1, A, A, h->obpi, 1, true);
-  add_var(h, "pi/logstd", 1, A, A, h->ols, 2, true);
-  add_var(h, "q/w", H1, A, A, oWq, 2, false); add_var(h, "q/b", 1, A, A, obq, 1, false);
+  const int A = h->A;
+  // zip order: pi/model/... (PPO2's creation order), then the same under oldpi/model/ (a second copy of the whole block)
+  ac_layout(h, "pi/model/", kGradMask, 2);
   h->params.add_copies(0, 15, "pi/model/", "oldpi/model/", h->n_total);
-  int rc = 0;
+  Tab tab;
+  int rc = ac_alloc(h, h->RMAX, tab);
+  if (rc) return bail(rc);
   const int64_t R = h->RMAX, NF = h->NF;
 #define DA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
-  DA(h->P, 2 * h->n_total); DA(h->Mo, h->n_train); DA(h->Vo, h->n_train); DA(h->G, h->n_train); DA(h->Gv, h->n_train);
+  DA(h->Gv, h->n_train);
   DA(h->X, h->n_train); DA(h->Rv, h->n_train); DA(h->Pv, h->n_train); DA(h->Zv, h->n_train); DA(h->FS, h->n_train);
-  DA(h->r_obs, (N + 1) * XS); DA(h->r_act, (N + 1) * A); DA(h->r_val, N + 1); DA(h->r_nlp, N + 1); DA(h->r_rew, N);
-  DA(h->r_done, N + 1); DA(h->r_adv, N); DA(h->r_ret, N); DA(h->lastv, 1);
-  DA(h->p_obs, (int64_t)h->P_ROWS * XS);
-  DA(h->Z0, R * 2 * H0); DA(h->Y0, R * 2 * H0); DA(h->Y1, R * 2 * H1);
-  DA(h->a_out, R * A); DA(h->a_v, R); DA(h->a_nlp, R);
   DA(h->atarg, N); DA(h->mu_old, N * A); DA(h->nlp_old, N); DA(h->sdm, N * A); DA(h->sdls, N * A); DA(h->u, NF * A);
   DA(h->dZ1, R * H1); DA(h->dZ0, R * H0); DA(h->T0, NF * H0); DA(h->T1, NF * H1);
   DA(h->dZls, N * H0); DA(h->Y0c, kNcand * N * H0); DA(h->Y1c, kNcand * N * H1);
   DA(h->cand, (int64_t)kNcand * (H0 + H0 * H1 + H1 + H1 * A + 2 * A));
   DA(h->vZ0, kVfBatch * H0); DA(h->vY0, kVfBatch * H0); DA(h->vY1, kVfBatch * H1); DA(h->vdZ1, kVfBatch * H1); DA(h->vdZ0, kVfBatch * H0);
   const int64_t nperm = std::max<int64_t>(1, (int64_t)c.vf_iters * N);
-  DA(h->perm, nperm); DA(h->vrowoff, nperm); DA(h->act_rowoff, 1);
+  DA(h->perm, nperm); DA(h->vrowoff, nperm);
   DA(h->part, kDotBlocks); DA(h->amax, kDotBlocks); DA(h->lspart, kNcand * kLsBlocks * 2); DA(h->sc, SC_N);
-  DA(h->met, TM_N); DA(h->counters, 4);
+  DA(h->met, TM_N);
 #undef DA
-  if (cudaMallocHost((void**)&h->h_buf, (TM_N + 2 * SC_N) * sizeof(float)) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "cudaMallocHost"));
-  Tab tab;
   auto T_ = [&](const char* nm, const std::vector<int>& v) {
     const int* p = nullptr;
     if (int r2 = upload_table(h->allocs, h->stream, v, &p)) return r2;
     tab[nm] = p;
     return 0;
   };
-  if ((rc = T_("iD", iota_tab(D))) || (rc = T_("iH0", iota_tab((int)H0))) || (rc = T_("iH1", iota_tab((int)H1))) ||
-      (rc = T_("i2H0", iota_tab(2 * (int)H0))) || (rc = T_("rM_2H0", iota_tab((int)R, 2 * (int)H0))) ||
-      (rc = T_("rM_2H1", iota_tab((int)R, 2 * (int)H1))) || (rc = T_("rM_H0", iota_tab((int)R, (int)H0))) ||
-      (rc = T_("rM_H1", iota_tab((int)R, (int)H1))) || (rc = T_("iH0_H1", iota_tab((int)H0, (int)H1))) ||
-      (rc = T_("iD_2H0", iota_tab(D, 2 * (int)H0))) || (rc = T_("boot", iota_tab(1, h->XS, (int)N * h->XS))) ||
-      (rc = T_("pred", iota_tab(h->P_ROWS, h->XS))) || (rc = T_("xall", iota_tab((int)N, h->XS))) ||
-      (rc = T_("x5", iota_tab((int)NF, 5 * h->XS))) || (rc = T_("y0_5", iota_tab((int)NF, 5 * 2 * (int)H0))))
+  if ((rc = T_("rM_H0", iota_tab((int)R, (int)H0))) || (rc = T_("rM_H1", iota_tab((int)R, (int)H1))) ||
+      (rc = T_("xall", iota_tab((int)N, h->XS))) || (rc = T_("x5", iota_tab((int)NF, 5 * h->XS))) ||
+      (rc = T_("y0_5", iota_tab((int)NF, 5 * 2 * (int)H0))))
     return bail(rc);
-  if ((rc = ac_make_fwd(h, h->f_act, h->r_obs, h->act_rowoff, 1, tab))) return bail(rc);
-  if ((rc = ac_make_fwd(h, h->f_boot, h->r_obs, tab["boot"], 1, tab))) return bail(rc);
-  if ((rc = ac_make_fwd(h, h->f_pred, h->p_obs, tab["pred"], h->P_ROWS, tab))) return bail(rc);
   if ((rc = ac_make_fwd(h, h->f_all, h->r_obs, tab["xall"], (int)N, tab))) return bail(rc);
   if ((rc = make_tower_bwd(h, h->gbwd, 0, (int)N, h->r_obs, tab["xall"], h->Y0, tab["rM_2H0"], h->dZ1, h->dZ0, h->G, tab))) return bail(rc);
   if ((rc = make_fvp(h, tab))) return bail(rc);
@@ -963,21 +895,12 @@ int b2g_trpo_rollout_act(b2g_trpo* h, const float* obs, float* act_out) {
   B2G_USABLE(h);
   if (!h || !obs || !act_out) return b2g_fail(B2G_EINVAL, "NULL argument");
   if (h->t >= h->N) return b2g_fail(B2G_ESTATE, "the rollout holds timesteps_per_batch rows: call b2g_trpo_update first");
-  CK(cudaSetDevice(h->cfg.device));
-  cudaStream_t s = h->stream;
-  if (int rc = upload_rows(h, h->r_obs + (size_t)h->t * h->XS, obs, 1)) return rc;
-  if (h->t == 0 && h->carried) {     // the boundary action drawn before the last update
-    CK(cudaMemcpyAsync(act_out, h->r_act, (size_t)h->A * sizeof(float), cudaMemcpyDefault, s));
-  } else {
-    trpo_set_row_kernel<<<1, 1, 0, s>>>(h->act_rowoff, h->t * h->XS);
-    ac_fwd_issue(h, h->f_act, s);
-    AcActArgs a = ac_act_args(h, 1, 0);
-    a.t = h->t;
-    ac_act(a, s);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(act_out, h->a_out, (size_t)h->A * sizeof(float), cudaMemcpyDefault, s));
-  }
-  CK(cudaStreamSynchronize(s));
+  if (h->t > 0 || !h->carried) return ac_rollout_act(h, obs, act_out);
+  // row 0 after an update: the boundary action drawn before it
+  CK(cudaSetDevice(h->device));
+  if (int rc = ac_upload_rows(h, h->r_obs, obs, 1)) return rc;
+  CK(cudaMemcpyAsync(act_out, h->r_act, (size_t)h->A * sizeof(float), cudaMemcpyDefault, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   return 0;
 }
 
@@ -985,21 +908,13 @@ int b2g_trpo_rollout_reward(b2g_trpo* h, float rew, float done) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   if (h->t >= h->N) return b2g_fail(B2G_ESTATE, "the rollout holds timesteps_per_batch rows: call b2g_trpo_update first");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaMemcpyAsync(h->r_rew + h->t, &rew, sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  CK(cudaMemcpyAsync(h->r_done + h->t + 1, &done, sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  CK(cudaStreamSynchronize(h->stream));      // rew and done live on this call's stack
-  h->t += 1;
-  return 0;
+  return ac_rollout_reward(h, &rew, &done);
 }
 
 int b2g_trpo_rollout_reset(b2g_trpo* h) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaMemsetAsync(h->r_done, 0, sizeof(float), h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  h->t = 0;
+  if (int rc = ac_rollout_reset(h)) return rc;
   h->carried = false;
   return 0;
 }
@@ -1007,15 +922,7 @@ int b2g_trpo_rollout_reset(b2g_trpo* h) {
 int b2g_trpo_rollout_get(b2g_trpo* h, float* adv, float* ret, float* val, float* act) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  const size_t n = h->N;
-  if (adv) CK(cudaMemcpyAsync(adv, h->r_adv, n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  if (ret) CK(cudaMemcpyAsync(ret, h->r_ret, n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  if (val) CK(cudaMemcpyAsync(val, h->r_val, n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  if (act) CK(cudaMemcpyAsync(act, h->r_act, n * h->A * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return 0;
+  return ac_rollout_get(h, adv, ret, val, nullptr, act);
 }
 
 static int upload_perm(b2g_trpo* h, const int32_t* perm) {
@@ -1033,12 +940,9 @@ int b2g_trpo_update(b2g_trpo* h, const float* last_obs, const int32_t* perm, b2g
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
   if (int rc = upload_perm(h, perm)) return rc;
-  if (int rc = upload_rows(h, h->r_obs + (size_t)h->N * h->XS, last_obs, 1)) return rc;
-  if (h->use_graph && !h->graph_exec)
-    if (int rc = capture_graph(h->stream, [&] { return update_issue(h); }, &h->graph_exec)) return rc;
-  if (h->graph_exec) CK(cudaGraphLaunch(h->graph_exec, h->stream));
-  else if (int rc = update_issue(h)) return rc;
-  h->n_iterations += 1;
+  if (int rc = ac_upload_rows(h, h->r_obs + (size_t)h->N * h->XS, last_obs, 1)) return rc;
+  if (int rc = ac_run_update(h, [&] { return update_issue(h); })) return rc;
+  h->n_updates += 1;
   h->t = 0;
   h->carried = true;
   return fetch(h, out);
@@ -1052,13 +956,13 @@ int b2g_trpo_step_explicit(b2g_trpo* h, const float* obs, const float* actions, 
   CK(cudaStreamSynchronize(h->stream));
   if (int rc = upload_perm(h, perm)) return rc;
   const size_t N = h->N;
-  if (int rc = upload_rows(h, h->r_obs, obs, h->N)) return rc;
+  if (int rc = ac_upload_rows(h, h->r_obs, obs, h->N)) return rc;
   CK(cudaMemcpyAsync(h->r_act, actions, N * h->A * sizeof(float), cudaMemcpyDefault, h->stream));
   CK(cudaMemcpyAsync(h->r_adv, adv, N * sizeof(float), cudaMemcpyDefault, h->stream));
   CK(cudaMemcpyAsync(h->r_ret, tdlamret, N * sizeof(float), cudaMemcpyDefault, h->stream));
   core_issue(h, h->stream);
   CK(cudaGetLastError());
-  h->n_iterations += 1;
+  h->n_updates += 1;
   h->t = 0;
   h->carried = false;
   const int rc = fetch(h, out);
@@ -1076,7 +980,7 @@ int b2g_trpo_fvp(b2g_trpo* h, const float* obs, const float* v, float* out) {
   std::vector<float> arena((size_t)h->n_train, 0.f);
   flat_arena(h, const_cast<float*>(v), arena.data(), true);
   CK(cudaMemcpyAsync(h->Pv, arena.data(), arena.size() * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  if (int rc = upload_rows(h, h->r_obs, obs, h->N)) return rc;
+  if (int rc = ac_upload_rows(h, h->r_obs, obs, h->N)) return rc;
   ac_fwd_issue(h, h->f_all, h->stream);
   fvp_issue(h, h->stream);
   CK(cudaGetLastError());
@@ -1089,43 +993,20 @@ int b2g_trpo_fvp(b2g_trpo* h, const float* obs, const float* v, float* out) {
 int b2g_trpo_act(b2g_trpo* h, const float* obs, int n, int deterministic, float* act_out, float* value_out) {
   B2G_USABLE(h);
   if (!h || !obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
-  CK(cudaSetDevice(h->cfg.device));
-  cudaStream_t s = h->stream;
-  const int P = h->P_ROWS;
-  for (int done_n = 0; done_n < n; done_n += P) {
-    const int chunk = std::min(P, n - done_n);
-    if (int rc = upload_rows(h, h->p_obs, obs + (size_t)done_n * h->D, chunk)) return rc;
-    ac_fwd_issue(h, h->f_pred, s);
-    AcActArgs a = ac_act_args(h, chunk, 2);
-    a.deterministic = deterministic;
-    ac_act(a, s);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(act_out + (size_t)done_n * h->A, h->a_out, (size_t)chunk * h->A * sizeof(float), cudaMemcpyDefault, s));
-    if (value_out) CK(cudaMemcpyAsync(value_out + done_n, h->a_v, chunk * sizeof(float), cudaMemcpyDefault, s));
-    CK(cudaStreamSynchronize(s));
-  }
-  return 0;
+  return ac_predict(h, obs, n, deterministic, act_out, value_out, nullptr);
 }
 
 int b2g_trpo_get_step(b2g_trpo* h, int64_t* adam_step, int64_t* noise_step, int32_t* rollout_rows) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  long long c[2];
-  CK(cudaMemcpyAsync(c, h->counters, sizeof c, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  if (adam_step) *adam_step = c[0];
-  if (noise_step) *noise_step = c[1];
-  if (rollout_rows) *rollout_rows = h->t;
-  return 0;
+  return ac_get_step(h, adam_step, noise_step, rollout_rows);
 }
 
 }  // extern "C"
 
 // ================================================================================================
-// Training state (b2g_trpo_state_save / _load; container format in state.cuh).  An iteration boundary: the rollout in flight
-// and the carried boundary action are not saved (every learn() starts from env.reset()).
+// Training state (b2g_trpo_state_save / _load; ac_state_save in actor_critic.cuh): the parameter arena holds pi and oldpi, the
+// moments are the value Adam's.  The carried boundary action is not saved (every learn() starts from env.reset()).
 // ================================================================================================
 namespace {
 
@@ -1135,9 +1016,6 @@ std::vector<FpField> trpo_fingerprint(const b2g_trpo* h) {
           fp_int("timesteps_per_batch", c.timesteps_per_batch), fp_int("seed", (int64_t)c.seed)};
 }
 
-// sections 2..: parameters (pi and oldpi) and the value Adam's moments
-std::vector<StateSection> trpo_device_sections(b2g_trpo* h) { return adam_sections(h->P, 2 * h->n_total, h->Mo, h->Vo, h->n_train); }
-
 }  // namespace
 
 extern "C" {
@@ -1145,41 +1023,14 @@ extern "C" {
 int b2g_trpo_state_save(b2g_trpo* h, const char* path) {
   if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
   B2G_USABLE(h);
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  long long cnt[4];
-  CK(cudaMemcpyAsync(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  int64_t hv[2] = {h->n_iterations, 0};
-  std::vector<StateSection> secs = host_sections(hv, sizeof hv, cnt, sizeof cnt);
-  for (auto& s : trpo_device_sections(h)) secs.push_back(std::move(s));
-  return state_write(path, STATE_KIND_TRPO, trpo_fingerprint(h), secs);
+  return ac_state_save(h, path, STATE_KIND_TRPO, trpo_fingerprint(h));
 }
 
 int b2g_trpo_state_load(b2g_trpo* h, const char* path) {
   if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
-  CK(cudaSetDevice(h->cfg.device));
-  StateReader rd;
-  if (int rc = rd.open(path, STATE_KIND_TRPO, trpo_fingerprint(h))) return rc;
-  const std::vector<StateSection> dev = trpo_device_sections(h);
-  if (int rc = state_check_tags(rd, dev, "TRPO")) return rc;
-  int64_t hv[2];
-  long long cnt[4];
-  if (rd.bytes(0) != sizeof hv || rd.bytes(1) != sizeof cnt)
-    return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
-  if (int rc = state_check_lengths(rd, dev)) return rc;
-  if (int rc = rd.read_host(0, hv, sizeof hv)) return rc;
-  if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
-  CK(cudaStreamSynchronize(h->stream));
-  return state_read_device(rd, dev, &h->broken, [&] {
-    CK(cudaMemcpyAsync(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemsetAsync(h->r_done, 0, sizeof(float), h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    h->n_iterations = hv[0];
-    h->t = 0;
-    h->carried = false;
-    return 0;
-  });
+  const int rc = ac_state_load(h, path, STATE_KIND_TRPO, trpo_fingerprint(h), "TRPO");
+  if (rc == 0) h->carried = false;
+  return rc;
 }
 
 }  // extern "C"

@@ -6,21 +6,19 @@ Import it as ``b200grasp.ppo2.PPO2`` (the stable-baselines path ``stable_baselin
 from __future__ import annotations
 
 import ctypes as C
-from collections import OrderedDict
 from typing import Optional
 
 import numpy as np
 
 from . import _lib
-from .base_model import BaseModel
-from .callbacks import as_callback
-from .tensorboard import EpisodeRewardLogger, Summary
-from .learner import HandleLearner, _f32, _fp
+from .actor_critic import ActorCriticLearner, ActorCriticModel, check_policy, check_policy_kwargs
+from .actor_critic import init_params as _init_params
+from .learner import _f32, _fp
 
 _SCOPE = "model/"
 
 
-class PPO2Learner(HandleLearner):
+class PPO2Learner(ActorCriticLearner):
     """numpy-facing wrapper of one ``b2g_ppo`` handle (maps 1:1 onto the C ABI)."""
     _abi = "ppo"
 
@@ -50,9 +48,6 @@ class PPO2Learner(HandleLearner):
 
     def rollout_reward(self, rew, done):
         _lib.check(self.lib.b2g_ppo_rollout_reward(self.h, _fp(_f32(np.reshape(rew, -1))), _fp(_f32(np.reshape(done, -1)))))
-
-    def rollout_reset(self):
-        _lib.check(self.lib.b2g_ppo_rollout_reset(self.h))
 
     def rollout_get(self):
         """advantages, returns, values, neglogp [n_steps, n_envs] and actions [n_steps, n_envs, n_actions] (time-major)."""
@@ -89,60 +84,24 @@ class PPO2Learner(HandleLearner):
         _lib.check(self.lib.b2g_ppo_act(self.h, _fp(obs), n, int(bool(deterministic)), _fp(a), _fp(v), _fp(nl)))
         return a, v, nl
 
-    def steps(self):
-        """(Adam step, noise-stream step, rollout rows filled)"""
-        a, b, t = C.c_int64(), C.c_int64(), C.c_int32()
-        _lib.check(self.lib.b2g_ppo_get_step(self.h, C.byref(a), C.byref(b), C.byref(t)))
-        return a.value, b.value, t.value
-
-
 
 def _schedule(v):
     """stable-baselines' get_schedule_fn: a callable of frac, or a constant."""
     return v if callable(v) else (lambda _frac, _v=v: _v)
 
 
-def _check_policy(policy, algo="PPO2"):
-    from .common.policies import MlpPolicy
-    if isinstance(policy, str):
-        if policy != "MlpPolicy":
-            raise NotImplementedError(f"policy '{policy}': only common.policies.MlpPolicy is built for {algo}")
-    elif policy is not MlpPolicy:
-        raise NotImplementedError(f"policy {getattr(policy, '__name__', policy)}: only common.policies.MlpPolicy is built for {algo} "
-                                  "(CNN, recurrent and layer-norm policies are not)")
+def _check_policy_kwargs(policy_kwargs):
+    """check_policy_kwargs with PPO2's messages -> (policy_kwargs as a dict, [h0, h1])"""
+    return check_policy_kwargs(policy_kwargs, "PPO2")
 
 
-def _check_policy_kwargs(policy_kwargs, algo="PPO2"):
-    kw = dict(policy_kwargs or {})
-    unknown = set(kw) - {"layers", "net_arch", "act_fun", "feature_extraction", "layer_norm"}
-    if unknown:
-        raise NotImplementedError(f"policy_kwargs {sorted(unknown)} are not built for {algo}")
-    if kw.get("feature_extraction", "mlp") != "mlp":
-        raise NotImplementedError(f"feature_extraction: only the MLP extractor is built for {algo}")
-    if kw.get("layer_norm", False):
-        raise NotImplementedError("layer_norm=True: layer-normalised policies are not built")
-    act = kw.get("act_fun")
-    if act is not None and getattr(act, "__name__", str(act)) != "tanh":
-        raise NotImplementedError(f"act_fun: only tanh is built for {algo}")
-    layers = [int(x) for x in kw.get("layers", None) or [64, 64]]
-    if "net_arch" in kw and kw["net_arch"] is not None:
-        na = list(kw["net_arch"])
-        if len(na) != 1 or not isinstance(na[0], dict):
-            raise NotImplementedError(f"net_arch={na}: shared layers are not built; give net_arch=[dict(pi=[h0, h1], vf=[h0, h1])]")
-        pi, vf = [int(x) for x in na[0].get("pi", [])], [int(x) for x in na[0].get("vf", [])]
-        if pi != vf:
-            raise NotImplementedError(f"net_arch pi={pi} vf={vf}: the towers must have the same widths")
-        layers = pi
-    if len(layers) != 2:
-        raise NotImplementedError(f"layers={layers}: the {algo} learner builds exactly two hidden layers")
-    return kw, layers
-
-
-class PPO2(BaseModel):
+class PPO2(ActorCriticModel):
     """stable-baselines 2.10 ``PPO2(policy, env, ...)`` with its signature and defaults, plus ``device``: ``learn / predict /
     save / load / get_parameters / load_parameters / get_env / get_vec_normalize_env / close`` and
     ``save_training_state / load_training_state``.  Box action spaces only, as the reference's configs give."""
-    _algo = "PPO2"
+    _algo, _branch, _scope = "PPO2", "PPO", _SCOPE
+    _zip_hyper = ("gamma", "n_steps", "vf_coef", "ent_coef", "max_grad_norm", "learning_rate", "lam", "nminibatches", "noptepochs",
+                  "cliprange", "cliprange_vf", "seed")
 
     def __init__(self, policy, env, gamma=0.99, n_steps=128, ent_coef=0.01, learning_rate=2.5e-4, vf_coef=0.5, max_grad_norm=0.5,
                  lam=0.95, nminibatches=4, noptepochs=4, cliprange=0.2, cliprange_vf=None, verbose=0, tensorboard_log=None,
@@ -152,7 +111,7 @@ class PPO2(BaseModel):
             if "device_obs_norm" in unsupported:
                 raise NotImplementedError("device_obs_norm: PPO2 stores what a host VecNormalize returns, as stable-baselines does")
             raise TypeError(f"PPO2 got unexpected keyword arguments {sorted(unsupported)}")
-        _check_policy(policy)
+        check_policy(policy, "PPO2")
         self.policy_kwargs, self.layers = _check_policy_kwargs(policy_kwargs)
         self.gamma, self.n_steps, self.ent_coef, self.learning_rate = gamma, int(n_steps), ent_coef, learning_rate
         self.vf_coef, self.max_grad_norm, self.lam = vf_coef, max_grad_norm, lam
@@ -161,7 +120,6 @@ class PPO2(BaseModel):
         self.num_timesteps = 0
         self.n_envs = 1
         self.learner: Optional[PPO2Learner] = None
-        self._boundary = None           # (num_timesteps, numpy global state) after the last completed update
         self.ep_info_buf = []
         if env is not None:
             self._set_env(env)
@@ -169,8 +127,7 @@ class PPO2(BaseModel):
                 self.setup_model()
 
     def _check_env(self):
-        if not hasattr(self.action_space, "low"):
-            raise NotImplementedError(f"PPO2 here needs a Box action space, got {self.action_space} (the reference's PPO branch is continuous)")
+        super()._check_env()
         if (self.n_envs * self.n_steps) % self.nminibatches:
             # ppo2.py's assertion: "The number of minibatches (nminibatches) is not a factor of the total number of samples"
             raise ValueError(f"nminibatches={self.nminibatches} is not a factor of n_batch = n_envs * n_steps = {self.n_envs * self.n_steps}")
@@ -195,147 +152,52 @@ class PPO2(BaseModel):
                                   lambda writer, _: self._learn(total_timesteps, callback, log_interval, reset_num_timesteps, writer))
 
     def _learn(self, total_timesteps, callback, log_interval, reset_num_timesteps, writer):
-        callback = as_callback(callback)
-        callback.init_callback(self)
-        if reset_num_timesteps:
-            self.num_timesteps = 0
-        callback.on_training_start({"self": self, "writer": writer}, globals())
-        ep_log = EpisodeRewardLogger(self.n_envs) if writer is not None else None
+        callback, ep_log, obs = self._learn_start(callback, reset_num_timesteps, writer, globals())
         lr_fn, clip_fn = _schedule(self.learning_rate), _schedule(self.cliprange)
         cvf = self.cliprange_vf
         cvf_fn = clip_fn if cvf is None else _schedule(cvf)
         clip_vf_off = isinstance(cvf, (float, int)) and not isinstance(cvf, bool) and cvf < 0
-        L = self.learner
         n_batch = self.n_envs * self.n_steps
         n_updates = total_timesteps // n_batch
-        low, high = self.action_space.low.reshape(-1), self.action_space.high.reshape(-1)
-        obs = np.asarray(self.env.reset(), np.float32).reshape(self.n_envs, -1)
-        L.rollout_reset()
-        self.last_metrics = None
         for update in range(1, n_updates + 1):
             frac = 1.0 - (update - 1.0) / n_updates
             lr_now, clip_now = lr_fn(frac), clip_fn(frac)
             cvf_now = -1.0 if clip_vf_off else cvf_fn(frac)
-            callback.on_rollout_start()
-            stopped = False
-            for _ in range(self.n_steps):
-                actions = L.rollout_act(obs)
-                clipped = np.clip(actions, low, high)
-                new_obs, rew, done, infos = self.env.step(clipped.reshape((self.n_envs,) + tuple(self.action_space.shape)))
-                self.num_timesteps += self.n_envs
-                if callback.on_step() is False:
-                    stopped = True
-                    break
-                for info in infos or []:
-                    ep = info.get("episode") if isinstance(info, dict) else None
-                    if ep is not None:
-                        self.ep_info_buf.append(ep)
-                L.rollout_reward(np.asarray(rew, np.float32), np.asarray(done, np.float32))
-                if ep_log is not None:
-                    ep_log(writer, rew, done, self.num_timesteps)
-                obs = np.asarray(new_obs, np.float32).reshape(self.n_envs, -1)
-            callback.on_rollout_end()
+            obs, stopped = self._rollout(obs, self.n_steps, callback, writer, ep_log)
             if stopped:
-                L.rollout_reset()
                 break
             inds = np.arange(n_batch)
             perms = np.empty((self.noptepochs, n_batch), np.int32)
             for e in range(self.noptepochs):
                 np.random.shuffle(inds)
                 perms[e] = inds
-            self.last_metrics = L.update(obs, perms, lr_now, clip_now, cvf_now)
-            self._boundary = (self.num_timesteps, np.random.get_state())
-            if writer is not None:
-                m = self.last_metrics
-                vals = [Summary.Value(t, m[k]) for t, k in self._update_tags.items()]
-                vals += [Summary.Value("input_info/learning_rate", lr_now), Summary.Value("input_info/clip_range", clip_now)]
-                writer.add_summary(Summary(vals), self.num_timesteps)
+            self._update_done(self.learner.update(obs, perms, lr_now, clip_now, cvf_now), writer,
+                              (("input_info/learning_rate", lr_now), ("input_info/clip_range", clip_now)))
             if self.verbose >= 1 and (update % log_interval == 0 or update == 1):
                 print(f"| ppo2 update {update}/{n_updates} | total_timesteps {self.num_timesteps} | "
                       + " | ".join(f"{k} {v:.5g}" for k, v in self.last_metrics.items()))
         callback.on_training_end()
         return self
 
-    def predict(self, observation, state=None, mask=None, deterministic=False):
-        """The Gaussian mean (deterministic) or a sample of stream 1, clipped to the action space."""
-        obs = np.asarray(observation, np.float32)
-        single = obs.ndim == len(self.observation_space.shape)
-        a, _, _ = self.learner.act(obs.reshape(-1, self.learner.obs_dim), deterministic=deterministic)
-        a = np.clip(a, self.action_space.low.reshape(-1), self.action_space.high.reshape(-1))
-        a = a.reshape((-1,) + tuple(self.action_space.shape))
-        return (a[0] if single else a), None
-
     def _data(self):
         data = {"gamma": self.gamma, "n_steps": self.n_steps, "vf_coef": self.vf_coef, "ent_coef": self.ent_coef,
                 "max_grad_norm": self.max_grad_norm, "learning_rate": self.learning_rate, "lam": self.lam,
                 "nminibatches": self.nminibatches, "noptepochs": self.noptepochs, "cliprange": self.cliprange,
-                "cliprange_vf": self.cliprange_vf, "verbose": self.verbose, "n_envs": self.n_envs, "seed": self.seed,
-                "policy_kwargs": dict(self.policy_kwargs),
-                "observation_shape": list(self.observation_space.shape), "action_shape": list(self.action_space.shape),
-                "action_low": np.asarray(self.action_space.low).reshape(-1).tolist(),
-                "action_high": np.asarray(self.action_space.high).reshape(-1).tolist()}
+                "cliprange_vf": self.cliprange_vf, **self._space_data()}
         for k in ("learning_rate", "cliprange", "cliprange_vf"):
             if callable(data[k]):
                 data[k] = None
         return data
 
-    @classmethod
-    def load(cls, load_path, env=None, custom_objects=None, **kwargs):
-        """Reads a PPO2 zip: widths and sizes from the parameter shapes, hyper-parameters from ``data``."""
-        from .spaces import Box
-        data, params = cls._read_zip(load_path)
-        w0, w1, wpi = params[_SCOPE + "pi_fc0/w"], params[_SCOPE + "pi_fc1/w"], params[_SCOPE + "pi/w"]
-        kw = {k: data[k] for k in ("gamma", "n_steps", "vf_coef", "ent_coef", "max_grad_norm", "learning_rate", "lam", "nminibatches",
-                                   "noptepochs", "cliprange", "cliprange_vf", "seed") if k in data and data[k] is not None}
-        if "cliprange_vf" in data and data["cliprange_vf"] is None:
-            kw["cliprange_vf"] = None
-        kw["policy_kwargs"] = dict(data.get("policy_kwargs") or {}, layers=[int(w0.shape[1]), int(w1.shape[1])])
-        kw.update(kwargs)
-        m = cls("MlpPolicy", None, _init_setup_model=False, **kw)
-        if env is None and m.n_steps % m.nminibatches:
-            raise ValueError(f"nminibatches={m.nminibatches} is not a factor of n_batch = {m.n_steps}")
-        A = int(wpi.shape[1])
-        return m._finish_load(env, Box(-np.inf, np.inf, tuple(data.get("observation_shape") or (w0.shape[0],))),
-                              Box(np.asarray(data.get("action_low", [-1.0] * A), np.float32),
-                                  np.asarray(data.get("action_high", [1.0] * A), np.float32), tuple(data.get("action_shape") or (A,))),
-                              params)
+    def _check_without_env(self):
+        if self.n_steps % self.nminibatches:
+            raise ValueError(f"nminibatches={self.nminibatches} is not a factor of n_batch = {self.n_steps}")
 
-    # ------------------------------------------------------------------ training state (training_state.py)
-    def _host_state(self):
+    def _host_init(self):
         for k in ("learning_rate", "cliprange", "cliprange_vf"):
             if callable(getattr(self, k)):
                 raise NotImplementedError(f"save_training_state needs a constant {k}")
-        num, np_state = self._boundary if self._boundary is not None else (self.num_timesteps, np.random.get_state())
-        init = dict(gamma=self.gamma, n_steps=self.n_steps, ent_coef=self.ent_coef, learning_rate=self.learning_rate, vf_coef=self.vf_coef,
+        return dict(gamma=self.gamma, n_steps=self.n_steps, ent_coef=self.ent_coef, learning_rate=self.learning_rate, vf_coef=self.vf_coef,
                     max_grad_norm=self.max_grad_norm, lam=self.lam, nminibatches=self.nminibatches, noptepochs=self.noptepochs,
                     cliprange=self.cliprange, cliprange_vf=self.cliprange_vf, verbose=self.verbose, policy_kwargs=self.policy_kwargs,
                     seed=self.seed, device=self.device)
-        return {"algo": "PPO2", "init": init, "num_timesteps": int(num),
-                "np_random": [np_state[0], np.asarray(np_state[1]).tolist(), int(np_state[2]), int(np_state[3]), float(np_state[4])]}
-
-    def _restore_host_state(self, host):
-        self.num_timesteps = int(host["num_timesteps"])
-        s = host["np_random"]
-        np.random.set_state((s[0], np.asarray(s[1], np.uint32), s[2], s[3], s[4]))
-        self._boundary = (self.num_timesteps, np.random.get_state())
-
-
-def _init_params(obs_dim, n_actions, layers, seed, rng=None, scope=_SCOPE):
-    """common/tf_layers.py ortho_init in the variables' creation order: the orthogonal factor of an SVD of a standard normal
-    matrix, scaled sqrt(2) for the hidden layers, 1 for vf, 0.01 for pi and q; zero biases and logstd.  The normal draws come
-    from ``rng``, by default a generator seeded with ``seed``; the names carry ``scope``."""
-    rng = np.random.default_rng(seed) if rng is None else rng
-    h0, h1 = layers
-    p = OrderedDict()
-    for name, shape in (("pi_fc0/w", (obs_dim, h0)), ("pi_fc0/b", (h0,)), ("vf_fc0/w", (obs_dim, h0)), ("vf_fc0/b", (h0,)),
-                        ("pi_fc1/w", (h0, h1)), ("pi_fc1/b", (h1,)), ("vf_fc1/w", (h0, h1)), ("vf_fc1/b", (h1,)), ("vf/w", (h1, 1)),
-                        ("vf/b", (1,)), ("pi/w", (h1, n_actions)), ("pi/b", (n_actions,)), ("pi/logstd", (1, n_actions)),
-                        ("q/w", (h1, n_actions)), ("q/b", (n_actions,))):
-        if name == "pi/logstd" or len(shape) == 1:
-            p[scope + name] = np.zeros(shape, np.float32)
-            continue
-        scale = 1.0 if name == "vf/w" else (0.01 if name in ("pi/w", "q/w") else np.sqrt(2.0))
-        u, _, v = np.linalg.svd(rng.normal(0.0, 1.0, shape), full_matrices=False)
-        w = u if u.shape == shape else v
-        p[scope + name] = (scale * w.reshape(shape)).astype(np.float32)
-    return p

@@ -7,17 +7,14 @@ and the value function's MpiAdam run on the GPU (csrc/trpo.cu); the algorithm is
 from __future__ import annotations
 
 import ctypes as C
-from collections import OrderedDict
 from typing import Optional
 
 import numpy as np
 
 from . import _lib
-from .base_model import BaseModel
-from .callbacks import as_callback
-from .tensorboard import EpisodeRewardLogger, Summary
-from .learner import HandleLearner, _f32, _fp
-from .ppo2 import _check_policy, _check_policy_kwargs, _init_params
+from .actor_critic import ActorCriticLearner, ActorCriticModel, check_policy, check_policy_kwargs
+from . import actor_critic
+from .learner import _f32, _fp
 
 PI, OLDPI = "pi/model/", "oldpi/model/"
 #: the policy step's variables, in the flat order of its gradient and step (trpo_mpi.py var_list)
@@ -25,7 +22,7 @@ POLICY_VARS = ("pi_fc0/w", "pi_fc0/b", "pi_fc1/w", "pi_fc1/b", "pi/w", "pi/b", "
 _GAIL = ("expert_dataset", "hidden_size_adversary", "adversary_entcoeff", "g_step", "d_step", "d_stepsize", "using_gail")
 
 
-class TRPOLearner(HandleLearner):
+class TRPOLearner(ActorCriticLearner):
     """numpy-facing wrapper of one ``b2g_trpo`` handle (maps 1:1 onto the C ABI)."""
     _abi = "trpo"
 
@@ -53,9 +50,6 @@ class TRPOLearner(HandleLearner):
 
     def rollout_reward(self, rew, done):
         _lib.check(self.lib.b2g_trpo_rollout_reward(self.h, float(np.ravel(rew)[0]), float(np.ravel(done)[0])))
-
-    def rollout_reset(self):
-        _lib.check(self.lib.b2g_trpo_rollout_reset(self.h))
 
     def rollout_get(self):
         """advantages, tdlamret, values [N] and actions [N, n_actions]."""
@@ -103,18 +97,12 @@ class TRPOLearner(HandleLearner):
         _lib.check(self.lib.b2g_trpo_act(self.h, _fp(obs), n, int(bool(deterministic)), _fp(a), _fp(v)))
         return a, v
 
-    def steps(self):
-        """(value-Adam step, noise-stream step, rollout rows filled)"""
-        a, b, t = C.c_int64(), C.c_int64(), C.c_int32()
-        _lib.check(self.lib.b2g_trpo_get_step(self.h, C.byref(a), C.byref(b), C.byref(t)))
-        return a.value, b.value, t.value
-
 
 def init_params(obs_dim, n_actions, layers, seed):
     """PPO2's initialisation rules for pi/model/... and then oldpi/model/..., drawn from one generator seeded with ``seed``."""
     rng = np.random.default_rng(seed)
-    p = _init_params(obs_dim, n_actions, layers, seed, rng=rng, scope=PI)
-    p.update(_init_params(obs_dim, n_actions, layers, seed, rng=rng, scope=OLDPI))
+    p = actor_critic.init_params(obs_dim, n_actions, layers, seed, rng=rng, scope=PI)
+    p.update(actor_critic.init_params(obs_dim, n_actions, layers, seed, rng=rng, scope=OLDPI))
     return p
 
 
@@ -123,11 +111,12 @@ def value_minibatches(n, batch_size=128):
     return [(s, s + batch_size) for s in range(0, n - batch_size + 1, batch_size)]
 
 
-class TRPO(BaseModel):
+class TRPO(ActorCriticModel):
     """stable-baselines 2.10 ``TRPO(policy, env, ...)`` with its signature and defaults, plus ``device``: ``learn / predict /
     save / load / get_parameters / load_parameters / get_env / get_vec_normalize_env / close`` and
     ``save_training_state / load_training_state``.  One environment with a Box action space, as the reference's configs give."""
-    _algo = "TRPO"
+    _algo, _branch, _scope = "TRPO", "TRPO", PI
+    _zip_hyper = ("gamma", "timesteps_per_batch", "max_kl", "cg_iters", "lam", "entcoeff", "cg_damping", "vf_stepsize", "vf_iters", "seed")
 
     def __init__(self, policy, env, gamma=0.99, timesteps_per_batch=1024, max_kl=0.01, cg_iters=10, lam=0.98, entcoeff=0.0,
                  cg_damping=1e-2, vf_stepsize=3e-4, vf_iters=3, verbose=0, tensorboard_log=None, _init_setup_model=True,
@@ -139,8 +128,8 @@ class TRPO(BaseModel):
             if gail:
                 raise NotImplementedError(f"{gail}: the GAIL path of TRPO is not built")
             raise TypeError(f"TRPO got unexpected keyword arguments {sorted(unsupported)}")
-        _check_policy(policy, "TRPO")
-        self.policy_kwargs, self.layers = _check_policy_kwargs(policy_kwargs, "TRPO")
+        check_policy(policy, "TRPO")
+        self.policy_kwargs, self.layers = check_policy_kwargs(policy_kwargs, "TRPO")
         self.gamma, self.timesteps_per_batch, self.max_kl, self.cg_iters = gamma, int(timesteps_per_batch), max_kl, int(cg_iters)
         self.lam, self.entcoeff, self.cg_damping, self.vf_stepsize, self.vf_iters = lam, entcoeff, cg_damping, vf_stepsize, int(vf_iters)
         self.verbose, self.tensorboard_log, self.full_tensorboard_log = verbose, tensorboard_log, full_tensorboard_log
@@ -148,9 +137,7 @@ class TRPO(BaseModel):
         self.num_timesteps = 0
         self.n_envs = 1
         self.learner: Optional[TRPOLearner] = None
-        self._boundary = None           # (num_timesteps, numpy global state) after the last completed iteration
         self.ep_info_buf = []
-        self.last_metrics = None
         if env is not None:
             self._set_env(env)
             if _init_setup_model:
@@ -159,9 +146,7 @@ class TRPO(BaseModel):
     def _check_env(self):
         if self.n_envs != 1:
             raise ValueError("the model requires a non vectorized environment or a single vectorized environment")
-        if not hasattr(self.action_space, "low"):
-            raise NotImplementedError(f"TRPO here needs a Box action space, got {self.action_space} (the reference's TRPO branch is "
-                                      "continuous)")
+        super()._check_env()
 
     def setup_model(self):
         obs_dim = int(np.prod(self.observation_space.shape))
@@ -185,108 +170,37 @@ class TRPO(BaseModel):
                                   lambda writer, _: self._learn(total_timesteps, callback, log_interval, reset_num_timesteps, writer))
 
     def _learn(self, total_timesteps, callback, log_interval, reset_num_timesteps, writer):
-        callback = as_callback(callback)
-        callback.init_callback(self)
-        if reset_num_timesteps:
-            self.num_timesteps = 0
-        callback.on_training_start({"self": self, "writer": writer}, globals())
-        ep_log = EpisodeRewardLogger(1) if writer is not None else None
-        L, N = self.learner, self.timesteps_per_batch
-        low, high = self.action_space.low.reshape(-1), self.action_space.high.reshape(-1)
-        obs = np.asarray(self.env.reset(), np.float32).reshape(-1)
-        L.rollout_reset()
-        self.last_metrics = None
+        callback, ep_log, obs = self._learn_start(callback, reset_num_timesteps, writer, globals())
+        N = self.timesteps_per_batch
         timesteps_so_far, iters_so_far = 0, 0
         while timesteps_so_far < total_timesteps:
-            callback.on_rollout_start()
-            stopped = False
-            for _ in range(N):
-                action = L.rollout_act(obs)
-                clipped = np.clip(action, low, high)
-                new_obs, rew, done, infos = self.env.step(clipped.reshape((1,) + tuple(self.action_space.shape)))
-                self.num_timesteps += 1
-                if callback.on_step() is False:
-                    stopped = True
-                    break
-                for info in infos or []:
-                    ep = info.get("episode") if isinstance(info, dict) else None
-                    if ep is not None:
-                        self.ep_info_buf.append(ep)
-                L.rollout_reward(rew, done)
-                if ep_log is not None:
-                    ep_log(writer, rew, done, self.num_timesteps)
-                obs = np.asarray(new_obs, np.float32).reshape(-1)
-            callback.on_rollout_end()
+            obs, stopped = self._rollout(obs, N, callback, writer, ep_log)
             if stopped:
-                L.rollout_reset()
                 break
             perms = np.empty((self.vf_iters, N), np.int32)
             for k in range(self.vf_iters):
                 inds = np.arange(N)
                 np.random.shuffle(inds)
                 perms[k] = inds
-            self.last_metrics = L.update(obs, perms)
+            metrics = self.learner.update(obs, perms)
             timesteps_so_far += N
             iters_so_far += 1
-            self._boundary = (self.num_timesteps, np.random.get_state())
-            if writer is not None:
-                m = self.last_metrics
-                writer.add_summary(Summary([Summary.Value(t, m[k]) for t, k in self._update_tags.items()]), self.num_timesteps)
+            self._update_done(metrics, writer)
             if self.verbose >= 1 and (iters_so_far % log_interval == 0 or iters_so_far == 1):
                 print(f"| trpo iteration {iters_so_far} | total_timesteps {self.num_timesteps} | "
                       + " | ".join(f"{k} {v:.5g}" for k, v in self.last_metrics.items()))
         callback.on_training_end()
         return self
 
-    def predict(self, observation, state=None, mask=None, deterministic=False):
-        """The Gaussian mean (deterministic) or a sample of stream 1, clipped to the action space."""
-        obs = np.asarray(observation, np.float32)
-        single = obs.ndim == len(self.observation_space.shape)
-        a, _ = self.learner.act(obs.reshape(-1, self.learner.obs_dim), deterministic=deterministic)
-        a = np.clip(a, self.action_space.low.reshape(-1), self.action_space.high.reshape(-1))
-        a = a.reshape((-1,) + tuple(self.action_space.shape))
-        return (a[0] if single else a), None
-
     def _data(self):
         return {"gamma": self.gamma, "timesteps_per_batch": self.timesteps_per_batch, "max_kl": self.max_kl, "cg_iters": self.cg_iters,
                 "lam": self.lam, "entcoeff": self.entcoeff, "cg_damping": self.cg_damping, "vf_stepsize": self.vf_stepsize,
-                "vf_iters": self.vf_iters, "verbose": self.verbose, "n_envs": self.n_envs, "seed": self.seed,
-                "policy_kwargs": dict(self.policy_kwargs),
-                "observation_shape": list(self.observation_space.shape), "action_shape": list(self.action_space.shape),
-                "action_low": np.asarray(self.action_space.low).reshape(-1).tolist(),
-                "action_high": np.asarray(self.action_space.high).reshape(-1).tolist()}
+                "vf_iters": self.vf_iters, **self._space_data()}
 
-    @classmethod
-    def load(cls, load_path, env=None, custom_objects=None, **kwargs):
-        """Reads a TRPO zip: widths and sizes from the pi/ parameter shapes, hyper-parameters from ``data``."""
-        from .spaces import Box
-        data, params = cls._read_zip(load_path)
-        w0, w1, wpi = params[PI + "pi_fc0/w"], params[PI + "pi_fc1/w"], params[PI + "pi/w"]
-        kw = {k: data[k] for k in ("gamma", "timesteps_per_batch", "max_kl", "cg_iters", "lam", "entcoeff", "cg_damping", "vf_stepsize",
-                                   "vf_iters", "seed") if k in data and data[k] is not None}
-        kw["policy_kwargs"] = dict(data.get("policy_kwargs") or {}, layers=[int(w0.shape[1]), int(w1.shape[1])])
-        kw.update(kwargs)
-        m = cls("MlpPolicy", None, _init_setup_model=False, **kw)
-        A = int(wpi.shape[1])
-        return m._finish_load(env, Box(-np.inf, np.inf, tuple(data.get("observation_shape") or (w0.shape[0],))),
-                              Box(np.asarray(data.get("action_low", [-1.0] * A), np.float32),
-                                  np.asarray(data.get("action_high", [1.0] * A), np.float32), tuple(data.get("action_shape") or (A,))),
-                              params)
-
-    # ------------------------------------------------------------------ training state (training_state.py)
-    def _host_state(self):
-        num, np_state = self._boundary if self._boundary is not None else (self.num_timesteps, np.random.get_state())
-        init = dict(gamma=self.gamma, timesteps_per_batch=self.timesteps_per_batch, max_kl=self.max_kl, cg_iters=self.cg_iters, lam=self.lam,
+    def _host_init(self):
+        return dict(gamma=self.gamma, timesteps_per_batch=self.timesteps_per_batch, max_kl=self.max_kl, cg_iters=self.cg_iters, lam=self.lam,
                     entcoeff=self.entcoeff, cg_damping=self.cg_damping, vf_stepsize=self.vf_stepsize, vf_iters=self.vf_iters,
                     verbose=self.verbose, policy_kwargs=self.policy_kwargs, seed=self.seed, device=self.device)
-        return {"algo": "TRPO", "init": init, "num_timesteps": int(num),
-                "np_random": [np_state[0], np.asarray(np_state[1]).tolist(), int(np_state[2]), int(np_state[3]), float(np_state[4])]}
-
-    def _restore_host_state(self, host):
-        self.num_timesteps = int(host["num_timesteps"])
-        s = host["np_random"]
-        np.random.set_state((s[0], np.asarray(s[1], np.uint32), s[2], s[3], s[4]))
-        self._boundary = (self.num_timesteps, np.random.get_state())
 
 
 __all__ = ["TRPO", "TRPOLearner", "POLICY_VARS", "init_params", "value_minibatches"]

@@ -1,4 +1,4 @@
-"""The SAC, BDQ, DQN and PPO2 front ends on a recording stand-in learner: what each one asks of its learner and what it writes,
+"""The SAC, BDQ, DQN, PPO2 and TRPO front ends on a recording stand-in learner: what each one asks of its learner and what it writes,
 through construction, save / load, training-state directories and close.  Needs no GPU."""
 import hashlib
 import io
@@ -10,7 +10,7 @@ from collections import OrderedDict
 import numpy as np
 import pytest
 
-from b200grasp import bdq, dqn, learner, ppo2, sac_model, sb_io, training_state
+from b200grasp import bdq, dqn, learner, ppo2, sac_model, sb_io, training_state, trpo_mpi
 from b200grasp.vec_env import DummyVecEnv, RunningMeanStd, VecNormalize
 from oracle import bdq_ref, dqn_ref, ppo_ref, sac_ref
 from tests.fake_env import FakeFlatEnv, FakeGraspEnv
@@ -104,10 +104,15 @@ def _ppo_specs(obs_dim, n_actions, layers, *_, **__):
     return ppo_ref.param_specs(obs_dim, n_actions, tuple(layers))
 
 
+def _trpo_specs(obs_dim, n_actions, layers, *_, **__):
+    specs = ppo_ref.param_specs(obs_dim, n_actions, tuple(layers))
+    return [(scope + n[len("model/"):], s) for scope in ("pi/model/", "oldpi/model/") for n, s in specs]
+
+
 @pytest.fixture(autouse=True)
 def fakes(monkeypatch):
     for mod, name, specs in ((sac_model, "Learner", _sac_specs), (bdq, "BDQLearner", _bdq_specs), (dqn, "DQNLearner", _dqn_specs),
-                             (ppo2, "PPO2Learner", _ppo_specs)):
+                             (ppo2, "PPO2Learner", _ppo_specs), (trpo_mpi, "TRPOLearner", _trpo_specs)):
         monkeypatch.setattr(mod, name, type(name, (FakeLearner,), {"specs": staticmethod(specs)}))
     LOG.clear()
     yield
@@ -153,8 +158,17 @@ def _ppo():
     return make, init, lambda: FakeFlatEnv(seed=6, obs_dim=6, n_act=3)
 
 
+def _trpo():
+    make = lambda env, **kw: trpo_mpi.TRPO("MlpPolicy", env, timesteps_per_batch=8, seed=19, policy_kwargs={"layers": [16, 8]}, **kw)
+    rng = np.random.default_rng(19)
+    init = OrderedDict((scope + n[len("model/"):], a) for scope in ("pi/model/", "oldpi/model/")
+                       for n, a in ppo_ref.init_params(6, 3, (16, 8), rng=rng).items())
+    return make, init, lambda: FakeFlatEnv(seed=8, obs_dim=6, n_act=3)
+
+
 CASES = {"sac_mlp": lambda: _sac(False, False), "sac_mlp_dev": lambda: _sac(False, True), "sac_cnn": lambda: _sac(True, False),
-         "sac_cnn_dev": lambda: _sac(True, True), "bdq": lambda: _bdq(False), "bdq_dev": lambda: _bdq(True), "dqn": _dqn, "ppo2": _ppo}
+         "sac_cnn_dev": lambda: _sac(True, True), "bdq": lambda: _bdq(False), "bdq_dev": lambda: _bdq(True), "dqn": _dqn, "ppo2": _ppo,
+         "trpo": _trpo}
 
 
 def _take_log():
@@ -189,7 +203,7 @@ def _advance_host_state(m):
     if isinstance(m, dqn.DQN):
         m.n_target_updates = 2
         m.predict_rng.random(4)
-    if isinstance(m, ppo2.PPO2):
+    if isinstance(m, (ppo2.PPO2, trpo_mpi.TRPO)):
         np.random.seed(23)
         m._boundary = (40, np.random.get_state())
         np.random.random(5)
@@ -203,7 +217,7 @@ def _host_counters(m):
         out.update(n_updates=m.n_updates, episode_rewards=m.episode_rewards, ep_info_buf=list(m.ep_info_buf))
     if isinstance(m, dqn.DQN):
         out.update(n_target_updates=m.n_target_updates, predict_rng=m.predict_rng.bit_generator.state)
-    if isinstance(m, ppo2.PPO2):
+    if isinstance(m, (ppo2.PPO2, trpo_mpi.TRPO)):
         out.update(boundary=[m._boundary[0], np.asarray(m._boundary[1][1]).tolist()])
     if hasattr(m, "_rng"):
         out["rng"] = m._rng.bit_generator.state
@@ -213,7 +227,8 @@ def _host_counters(m):
 _REPLAY = ("gamma", "learning_rate", "batch_size", "buffer_size", "policy_kwargs", "seed")
 HYPER = {"SAC": _REPLAY + ("tau", "n_envs", "device_obs_norm"), "BDQ": _REPLAY + ("num_actions_pad", "device_obs_norm"),
          "DQN": _REPLAY + ("target_network_update_freq",),
-         "PPO2": ("gamma", "learning_rate", "n_steps", "nminibatches", "cliprange_vf", "policy_kwargs", "seed", "n_envs")}
+         "PPO2": ("gamma", "learning_rate", "n_steps", "nminibatches", "cliprange_vf", "policy_kwargs", "seed", "n_envs"),
+         "TRPO": ("gamma", "timesteps_per_batch", "max_kl", "vf_stepsize", "vf_iters", "policy_kwargs", "seed", "n_envs")}
 
 
 def run_case(case, norm, tmp):
@@ -240,13 +255,13 @@ def run_case(case, norm, tmp):
     assert sorted(os.listdir(d)) == sorted(["host.json", "learner.state", "model.zip"] + (["vecnormalize.pkl"] if norm else []))
     host = training_state.read_host(d)
     rec["host"] = {k: v for k, v in host.items() if k not in ("rng", "predict_rng", "np_random")}
-    if isinstance(m, ppo2.PPO2):
+    if isinstance(m, (ppo2.PPO2, trpo_mpi.TRPO)):
         np.random.seed(99)                         # the load must put numpy's generator back
     env2 = _vec(env_fn, norm)
     m2 = type(m).load_training_state(d, env2)
     rec["load_training_state"] = _take_log()
     assert _host_counters(m2) == counters
-    if isinstance(m, ppo2.PPO2):
+    if isinstance(m, (ppo2.PPO2, trpo_mpi.TRPO)):
         np.testing.assert_array_equal(np.random.get_state()[1], m._boundary[1][1])
     assert m2.get_env() is env2 and m2.get_vec_normalize_env() is (env2 if norm else None)
     if norm:
@@ -331,7 +346,8 @@ def _stub(cls, shapes, **attrs):
     return L
 
 
-STUBS = {"sac": (learner.Learner,), "bdq": (bdq.BDQLearner,), "dqn": (dqn.DQNLearner,), "ppo": (ppo2.PPO2Learner,)}   # before any patching
+STUBS = {"sac": (learner.Learner,), "bdq": (bdq.BDQLearner,), "dqn": (dqn.DQNLearner,), "ppo": (ppo2.PPO2Learner,),
+         "trpo": (trpo_mpi.TRPOLearner,)}   # before any patching
 
 
 @pytest.mark.parametrize("abi", list(STUBS))
