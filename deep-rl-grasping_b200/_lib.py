@@ -26,6 +26,8 @@ SYMBOLS = [
     "b2g_bdq_get_grad", "b2g_bdq_replay_add", "b2g_bdq_replay_size", "b2g_bdq_set_norm_stats", "b2g_bdq_step",
     "b2g_bdq_step_explicit", "b2g_bdq_act", "b2g_bdq_set_per_beta", "b2g_bdq_get_last_per", "b2g_bdq_state_save", "b2g_bdq_state_load",
     "b2g_bdq_observe_act", "b2g_bdq_observe_add", "b2g_bdq_obs_rms_set", "b2g_bdq_obs_rms_get", "b2g_bdq_upload_bytes",
+    "b2g_bdq_create2", "b2g_bdq_replay_info", "b2g_bdq_replay_get", "b2g_dqn_create2", "b2g_dqn_replay_info", "b2g_dqn_replay_get",
+    "b2g_transition_replay_bytes",
     "b2g_dqn_create", "b2g_dqn_destroy", "b2g_dqn_param_count", "b2g_dqn_param_info", "b2g_dqn_get_param", "b2g_dqn_set_param",
     "b2g_dqn_get_grad", "b2g_dqn_replay_add", "b2g_dqn_replay_size", "b2g_dqn_set_norm_stats", "b2g_dqn_step",
     "b2g_dqn_step_explicit", "b2g_dqn_set_per_beta", "b2g_dqn_get_last_per", "b2g_dqn_update_target", "b2g_dqn_act",
@@ -267,6 +269,12 @@ def load():
         getattr(lib, f"b2g_{p}_set_norm_stats").argtypes = [vp, dp, dp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int]
         getattr(lib, f"b2g_{p}_set_per_beta").argtypes = [vp, C.c_float]
         getattr(lib, f"b2g_{p}_get_last_per").argtypes = [vp, C.POINTER(C.c_int32), fp, fp]
+        getattr(lib, f"b2g_{p}_replay_info").argtypes = [vp, i64p, i64p, i64p, i64p, i64p, i64p]
+        getattr(lib, f"b2g_{p}_replay_get").argtypes = [vp, C.c_int64, fp, fp, fp, fp, fp, C.POINTER(C.c_int32)]
+    lib.b2g_bdq_create2.argtypes = [C.POINTER(BdqCfg), C.POINTER(ReplayCfg), C.POINTER(vp)]
+    lib.b2g_dqn_create2.argtypes = [C.POINTER(DqnCfg), C.POINTER(ReplayCfg), C.POINTER(vp)]
+    lib.b2g_transition_replay_bytes.argtypes = [C.c_int64, C.c_int, C.c_int, C.c_int64]
+    lib.b2g_transition_replay_bytes.restype = C.c_int64
     lib.b2g_bdq_create.argtypes = [C.POINTER(BdqCfg), C.POINTER(vp)]
     lib.b2g_bdq_step.argtypes = [vp, C.c_int, C.c_float, C.POINTER(BdqMetrics)]
     lib.b2g_bdq_step_explicit.argtypes = [vp, fp, fp, fp, fp, fp, fp, C.c_float, C.c_int, C.POINTER(BdqMetrics), fp]

@@ -36,6 +36,11 @@ class BaseModel:
     env = None
     _vec_normalize_env = None
 
+    def _replay_kwargs(self):
+        """The learner's frame_capacity for BDQ / DQN's ``replay_frames`` (nothing without it: the default layout)."""
+        f = getattr(self, "replay_frames", None)
+        return {} if f is None else {"frame_capacity": f}
+
     # ------------------------------------------------------------------ TensorBoard (tensorboard.py)
     def _learn_logged(self, tb_log_name, reset_num_timesteps, run):
         """run(writer, step_log) inside stable-baselines' TensorboardWriter: writer is None without tensorboard_log and on

@@ -19,17 +19,19 @@ from . import _lib, training_state
 from .base_model import BaseModel
 from .callbacks import as_callback
 from .tensorboard import EpisodeRewardLogger
-from .learner import HandleLearner, _f32, _fp, nccl_config
+from .learner import TransitionReplayLearner, _f32, _fp, nccl_config
 from .vec_env import VecNormalize
 
 
-class BDQLearner(HandleLearner):
+class BDQLearner(TransitionReplayLearner):
     """numpy-facing wrapper of one ``b2g_bdq`` handle (maps 1:1 onto the C ABI)."""
     _abi = "bdq"
 
     def __init__(self, obs_dim=100, n_branches=3, n_bins=8, layers=((64, 64), (32,), (32,)), batch_size=64, buffer_size=100000,
                  gamma=0.99, target_network_update_freq=1000, trunk_grad_rescale=True, seed=0, device=0, rank=0, nranks=1, nccl_id=None,
-                 prioritized_replay=False, prioritized_replay_alpha=0.6, prioritized_replay_eps=1e-6):
+                 prioritized_replay=False, prioritized_replay_alpha=0.6, prioritized_replay_eps=1e-6, frame_capacity=None):
+        """frame_capacity: the replay holds that many observation frames and a slot refers to its obs / next_obs frames
+        (include/b200grasp.h: b2g_bdq_create2); None = two fp32 rows per slot."""
         self.lib = _lib.load()
         if layers[1][0] != layers[2][0]:
             raise NotImplementedError("branch and state-value hidden widths must match (every shipped zip / config)")
@@ -38,9 +40,11 @@ class BDQLearner(HandleLearner):
                           target_network_update_freq, int(trunk_grad_rescale), seed, device, rank, nranks, idp, libp,
                           int(bool(prioritized_replay)), float(prioritized_replay_alpha), float(prioritized_replay_eps))
         self.prioritized_replay = bool(prioritized_replay)
-        self._create(cfg)
+        self.frame_capacity = None if frame_capacity is None else int(frame_capacity)
+        self._create(cfg, self._replay_cfg(self.frame_capacity))
         self.obs_dim = self.obs_elems = obs_dim
         self.n_branches, self.n_bins, self.batch_size = n_branches, n_bins, batch_size
+        self._act_width = n_branches
         self.obs_shape = (obs_dim,)          # shape of obs_rms_get's arrays (BDQ sets the env's observation shape)
 
     def _has_grad(self, name):
@@ -127,13 +131,18 @@ class BDQ(BaseModel):
                  num_actions_pad=33, prioritized_replay=False, prioritized_replay_alpha=0.6, prioritized_replay_beta0=0.4,
                  prioritized_replay_beta_iters=None, prioritized_replay_eps=1e-6, epsilon_greedy=True, policy_kwargs=None, verbose=0,
                  tensorboard_log=None, seed=None, device=0, rank=0, nranks=1, nccl_id=None, _init_setup_model=True,
-                 device_obs_norm=False, **_ignored):
+                 device_obs_norm=False, replay_frames=None, **_ignored):
+        if replay_frames is not None and nranks > 1:
+            raise NotImplementedError("replay_frames with nranks > 1: the frame pool is built for one learner handle")
         if device_obs_norm and nranks > 1:
             raise NotImplementedError("device_obs_norm=True keeps VecNormalize's obs_rms on one learner handle; with nranks > 1 every "
                                       "rank would own different statistics")
         # learn() stores raw transitions (stable-baselines' rule), feeds the actor, the statistics and the replay from one upload
         # per frame, and a VecNormalize with norm_obs hands its obs_rms to the device learner (BDQLearner.observe_act / _add)
         self.device_obs_norm = bool(device_obs_norm)
+        # replay storage: F observation frames, slot s referring to its obs / next_obs frames (BDQLearner: frame_capacity);
+        # None = two fp32 rows per slot
+        self.replay_frames = None if replay_frames is None else int(replay_frames)
         self.prioritized_replay = bool(prioritized_replay)
         self.per_alpha, self.per_beta0, self.per_beta_iters, self.per_eps = prioritized_replay_alpha, prioritized_replay_beta0, \
             prioritized_replay_beta_iters, prioritized_replay_eps
@@ -160,7 +169,7 @@ class BDQ(BaseModel):
         self.learner = BDQLearner(obs_dim, n_br, self.num_actions_pad, tuple(tuple(l) for l in self.layers), self.batch_size,
                                   self.buffer_size, self.gamma, self.target_network_update_freq, True, int(self.seed or 0), self.device,
                                   prioritized_replay=self.prioritized_replay, prioritized_replay_alpha=self.per_alpha,
-                                  prioritized_replay_eps=self.per_eps, **self._dp)
+                                  prioritized_replay_eps=self.per_eps, **self._dp, **self._replay_kwargs())
         rng = np.random.default_rng(self.seed)
         p = OrderedDict()
         for n, shp in self.learner.param_shapes.items():
@@ -290,6 +299,8 @@ class BDQ(BaseModel):
                     device=self.device)
         if self.device_obs_norm:
             init["device_obs_norm"] = True
+        if self.replay_frames is not None:
+            init["replay_frames"] = self.replay_frames
         host = {"algo": "BDQ", "init": init, "num_timesteps": int(self.num_timesteps), "rng": training_state.rng_state(self._rng)}
         enc = self._encoder_host()
         if enc is not None:

@@ -202,6 +202,7 @@ struct b2g_bdq {
   float *ob_act = nullptr, *ob_rew = nullptr, *ob_done = nullptr;
   int* ob_idx = nullptr;       // [stage_rows][D] actor output
   int ob_k = 0, ob_n = 0;
+  std::vector<int64_t> ob_fid;  // replay with frames: frame id holding env i's staged observation (-1: not stored yet)
   int64_t up_observe = 0, up_other = 0;    // host->device bytes: observe_* / obs_rms_set, and act + replay_add + set_norm_stats
   EncStage* enc = nullptr;     // b2g_bdq_set_obs_encoder: observe_* take raw rows and encode them into the staged rows
   float* p(const std::string& nm) { return P + params.off(nm); }
@@ -335,6 +336,7 @@ GatherArgs bgather(b2g_bdq* h, bool from_replay, bool with_next) {
   g.B = h->B; g.H = 0; g.W = h->cfg.obs_dim; g.Cimg = 0; g.scale = 1.f;
   g.F_pi = h->Xscratch; g.F_v = h->X; g.F_t = h->Xn; g.FS = h->XS; g.feat_col = 0;
   g.rew_out = h->rew_n; g.done_out = h->done_n; g.n_act = h->D;
+  if (from_replay) h->replay.gather_args(g, with_next);     // a replay of frames: rows through obs_frame / next_frame
   return g;
 }
 
@@ -344,6 +346,7 @@ int bdq_issue(b2g_bdq* h, bool sampled, bool apply, const float* weights) {
   pa.counters = h->counters; pa.step_consts = h->step_consts; pa.lr = h->d_lr; pa.metrics = h->metrics;
   pa.indices = h->indices; pa.eps = h->eps_dummy; pa.B = h->B; pa.A = 1; pa.replay_size = nullptr;
   pa.seed = h->cfg.seed + 0x9E3779B97F4A7C15ull * (unsigned long long)h->cfg.rank; pa.gen = sampled ? 1 : 0; pa.apply = apply ? 1 : 0;
+  pa.ring_cap = h->replay.ring_cap();
   prep_launch(pa, s);
   const bool per = h->replay.per;
   const PerArgs pr = h->replay.per_args(h->counters, pa.seed, h->B, h->indices, h->weights, h->td, h->D);
@@ -412,7 +415,9 @@ int b2g_bdq_destroy(b2g_bdq* h) {
   return 0;
 }
 
-int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
+int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) { return b2g_bdq_create2(cfg, nullptr, out); }
+
+int b2g_bdq_create2(const b2g_bdq_cfg* cfg, const b2g_replay_cfg* replay, b2g_bdq** out) {
   if (!cfg || !out) return b2g_fail(B2G_EINVAL, "cfg/out is NULL");
   *out = nullptr;
   if (cfg->n_branches < 1 || cfg->n_branches > 8 || cfg->n_bins < 2 || cfg->n_bins > 64) return b2g_fail(B2G_EINVAL, "n_branches in [1,8], n_bins in [2,64]");
@@ -422,6 +427,7 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
   if (cfg->nranks < 1 || cfg->rank < 0 || cfg->rank >= cfg->nranks) return b2g_fail(B2G_EINVAL, "bad rank/nranks");
   if (cfg->nranks > 1 && !cfg->nccl_id) return b2g_fail(B2G_EINVAL, "nranks > 1 needs nccl_id");
   if (cfg->prioritized_replay && cfg->batch > 1024) return b2g_fail(B2G_EINVAL, "prioritised replay supports batch <= 1024");
+  if (int rc = check_replay_cfg(replay, cfg->buffer_capacity, cfg->nranks)) return rc;
   if (int rc = check_device(cfg->device)) return rc;
   b2g_bdq* h = new b2g_bdq();
   h->cfg = *cfg;
@@ -459,7 +465,9 @@ int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out) {
   BA(h->P, 2 * h->n_train); BA(h->Mo, h->n_train); BA(h->Vo, h->n_train); BA(h->G, h->n_train + MET_COUNT); BA(h->metrics, MET_COUNT);
   BA(h->counters, 8); BA(h->step_consts, 4); BA(h->d_lr, 1);
   const int64_t cap = cfg->buffer_capacity;
-  if ((rc = h->replay.init(h->allocs, h->stream, cap, h->E, D, B, cfg->prioritized_replay != 0, cfg->per_alpha, cfg->per_eps))) return bail(rc);
+  if ((rc = h->replay.init(h->allocs, h->stream, cap, h->E, D, B, cfg->prioritized_replay != 0, cfg->per_alpha, cfg->per_eps,
+                           replay ? replay->frame_capacity : 0, h->stage_rows)))
+    return bail(rc);
   BA(h->d_mean, h->E); BA(h->d_istd, h->E); BA(h->d_normc, 8);
   BA(h->X, (size_t)B * h->XS); BA(h->Xn, (size_t)B * h->XS); BA(h->Xscratch, (size_t)B * h->XS);
   for (int e = 0; e < 3; ++e) {
@@ -513,6 +521,20 @@ int b2g_bdq_replay_add(b2g_bdq* h, const float* obs, const float* act_idx, const
   return 0;
 }
 int64_t b2g_bdq_replay_size(const b2g_bdq* h) { B2G_USABLE(h); return h ? h->replay.size : 0; }
+
+int b2g_bdq_replay_info(const b2g_bdq* h, int64_t* capacity, int64_t* size, int64_t* frame_capacity, int64_t* live_frames, int64_t* bytes,
+                        int64_t* evicted_early) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  h->replay.info(capacity, size, frame_capacity, live_frames, bytes, evicted_early);
+  return 0;
+}
+
+int b2g_bdq_replay_get(b2g_bdq* h, int64_t slot, float* obs, float* act_idx, float* rew, float* next_obs, float* done, int32_t* frame_ids) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  return h->replay.get(slot, obs, act_idx, rew, next_obs, done, frame_ids, h->cfg.device, h->stream);
+}
 
 int b2g_bdq_set_norm_stats(b2g_bdq* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs, double clip_rew, double eps,
                            int norm_obs, int norm_reward) {
@@ -741,6 +763,7 @@ int b2g_bdq_observe_act(b2g_bdq* h, const float* obs, int n, int update_stats, f
     if (int rc = bdq_stage_frames(h, cur, obs, n)) return rc;
     if (update_stats) bdq_merge(h, cur, nullptr, nullptr, n);
     h->ob_n = n;
+    h->ob_fid.assign((size_t)n, -1);
   }
   if (act_idx_out) {
     const unsigned long long seed = h->cfg.seed + 0x9E3779B97F4A7C15ull * (unsigned long long)h->cfg.rank;
@@ -768,6 +791,8 @@ int b2g_bdq_observe_add(b2g_bdq* h, const float* act_idx, const float* rew, cons
   if (h->ob_n == 0) return b2g_fail(B2G_ESTATE, "observe_add: no staged observations (call b2g_bdq_observe_act first)");
   if (n != h->ob_n) return b2g_fail(B2G_EINVAL, "observe_add: n differs from the number of staged observations");
   if (n > h->cfg.buffer_capacity) return b2g_fail(B2G_EINVAL, "observe_add: n exceeds buffer_capacity");
+  if (h->replay.ring.dedup && 2 * (int64_t)n > h->replay.ring.frame_cap)
+    return b2g_fail(B2G_EINVAL, "observe_add: 2 n rows exceed frame_capacity (replay_frames)");
   int n_done = 0;
   for (int i = 0; i < n; ++i) n_done += done[i] != 0.f;
   if (n_done && !reset_obs) return b2g_fail(B2G_EINVAL, "observe_add: an env finished but reset_obs is NULL");
@@ -782,16 +807,26 @@ int b2g_bdq_observe_add(b2g_bdq* h, const float* act_idx, const float* rew, cons
     if (int rc = bdq_stage_reset_frames(h, reset_obs, done, n, n_done)) return rc;
   // the transitions: obs = the staged rows, next_obs = the uploaded rows (a finished env's terminal frame)
   TransitionReplay& rp = h->replay;
-  const int64_t new_size = std::min<int64_t>(rp.cap, rp.size + n);
-  bdq_commit_kernel<<<n, 256, 0, h->stream>>>(cur, nxt, h->ob_act, h->ob_rew, h->ob_done, (int)E, (int)D, rp.pos, rp.cap, rp.obs, rp.next,
-                                              rp.act, rp.rew, rp.done, h->counters, new_size);
-  rp.insert_max_prio(rp.pos, n, h->stream);     // as in b2g_bdq_replay_add
+  std::vector<int64_t> next_ids;
+  if (rp.framed()) {
+    // env i's staged row is the frame its previous transition's next_obs took, unless the env was reset since: shared without
+    // comparing; a reset frame (ob_fid -1) takes a frame of its own here, when it is first used as obs
+    next_ids.resize((size_t)n);
+    if (int rc = rp.commit(cur, nxt, n, h->ob_fid.data(), h->ob_act, h->ob_rew, h->ob_done, next_ids.data(), h->stream)) return rc;
+    for (int i = 0; i < n; ++i) h->ob_fid[i] = done[i] != 0.f ? -1 : next_ids[i];
+    if (int rc = rp.finish(next_ids, h->counters, h->stream)) return rc;
+  } else {
+    const int64_t new_size = std::min<int64_t>(rp.cap, rp.size + n);
+    bdq_commit_kernel<<<n, 256, 0, h->stream>>>(cur, nxt, h->ob_act, h->ob_rew, h->ob_done, (int)E, (int)D, rp.pos, rp.cap, rp.obs, rp.next,
+                                                rp.act, rp.rew, rp.done, h->counters, new_size);
+    rp.insert_max_prio(rp.pos, n, h->stream);     // as in b2g_bdq_replay_add
+  }
   // VecNormalize's step_wait merges the frames the VecEnv returned: a finished env's reset frame, not its terminal observation
   if (update_stats) bdq_merge(h, nxt, n_done ? h->ob_reset : nullptr, h->ob_done, n);
   // the new rows become the current observations; a finished env continues from the frame its reset returned
   for (int i = 0; i < n; ++i)
     if (done[i] != 0.f) CK(cudaMemcpyAsync(nxt + i * E, h->ob_reset + i * E, fb, cudaMemcpyDeviceToDevice, h->stream));
-  rp.advance(n);
+  if (!rp.framed()) rp.advance(n);
   h->ob_k ^= 1;
   CK(cudaStreamSynchronize(h->stream));     // host arrays are caller-owned: copied before return
   CK(cudaGetLastError());
@@ -815,9 +850,9 @@ std::vector<FpField> bdq_fingerprint(const b2g_bdq* h) {
 }
 // sections 2.. (parameters .. prioritised-replay scalars, then obs_rms when the handle owns it) of a handle holding `live`
 // replay rows
-std::vector<StateSection> bdq_device_sections(b2g_bdq* h, int64_t live) {
+std::vector<StateSection> bdq_device_sections(b2g_bdq* h, int64_t live, int64_t lo = 0, int64_t hi = 0) {
   std::vector<StateSection> s = adam_sections(h->P, 2 * h->n_train, h->Mo, h->Vo, h->n_train);
-  for (auto& r : h->replay.state_sections(live)) s.push_back(std::move(r));
+  for (auto& r : h->replay.state_sections(live, lo, hi)) s.push_back(std::move(r));
   if (h->rms_mean) s.push_back(rms_section(&h->rms_count, h->rms_mean, h->rms_var, h->E));
   return s;
 }
@@ -837,10 +872,11 @@ int b2g_bdq_state_save(b2g_bdq* h, const char* path) {
   CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
   uint32_t eps_bits;
   memcpy(&eps_bits, &h->eps_value, sizeof eps_bits);
-  int64_t hv[4] = {h->replay.size, h->replay.pos, h->n_updates, (int64_t)eps_bits};
-  std::vector<StateSection> secs = host_sections(hv, sizeof hv, cnt, sizeof cnt);
-  for (auto& s : bdq_device_sections(h, h->replay.size)) secs.push_back(std::move(s));
-  return state_write(path, STATE_KIND_BDQ, fp_with_rms(bdq_fingerprint(h), h->rms_mean), secs);
+  std::vector<int64_t> hv = h->replay.state_host(h->n_updates, (int64_t)eps_bits);
+  const FrameRing& ring = h->replay.ring;
+  std::vector<StateSection> secs = host_sections(hv.data(), hv.size() * sizeof(int64_t), cnt, sizeof cnt);
+  for (auto& s : bdq_device_sections(h, h->replay.size, ring.frame_lo(), ring.next_fid)) secs.push_back(std::move(s));
+  return state_write(path, STATE_KIND_BDQ, fp_with_rms(fp_with_frames(bdq_fingerprint(h), ring.frame_cap), h->rms_mean), secs);
 }
 
 int b2g_bdq_state_load(b2g_bdq* h, const char* path) {
@@ -849,15 +885,15 @@ int b2g_bdq_state_load(b2g_bdq* h, const char* path) {
   CK(cudaSetDevice(h->cfg.device));
   // ---- everything is checked before the handle changes
   StateReader rd;
-  if (int rc = state_open_rms(rd, path, STATE_KIND_BDQ, bdq_fingerprint(h), h->rms_mean, "b2g_bdq_obs_rms_set")) return rc;
+  TransitionReplay& rp = h->replay;
+  if (int rc = state_open_replay(rd, path, STATE_KIND_BDQ, bdq_fingerprint(h), rp.ring.frame_cap, h->rms_mean, "b2g_bdq_obs_rms_set")) return rc;
   if (int rc = state_check_tags(rd, bdq_device_sections(h, 0), "BDQ")) return rc;
-  int64_t hv[4];
   long long cnt[8];
-  if (rd.bytes(0) != sizeof hv || rd.bytes(1) != sizeof cnt)
-    return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
-  if (int rc = rd.read_host(0, hv, sizeof hv)) return rc;
-  if (!h->replay.valid(hv[0], hv[1]) || hv[2] < 0) return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
-  const std::vector<StateSection> dev = bdq_device_sections(h, hv[0]);
+  if (rd.bytes(1) != sizeof cnt) return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  std::vector<int64_t> hv;
+  FrameRing ring;
+  if (int rc = rp.state_host_read(rd, &hv, &ring)) return rc;
+  const std::vector<StateSection> dev = bdq_device_sections(h, hv[0], ring.frame_lo(), ring.next_fid);
   if (int rc = state_check_lengths(rd, dev)) return rc;
   if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
   // ---- from here on a failure leaves the handle unusable until a load succeeds
@@ -870,7 +906,8 @@ int b2g_bdq_state_load(b2g_bdq* h, const char* path) {
     }
     h->ob_n = 0;       // the staged observations are not part of the file: a resumed run starts a fresh episode
     CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
-    h->replay.size = hv[0]; h->replay.pos = hv[1]; h->n_updates = hv[2];
+    rp.ring = ring;
+    rp.size = hv[0]; rp.pos = hv[1]; h->n_updates = hv[2];
     const uint32_t eps_bits = (uint32_t)hv[3];
     memcpy(&h->eps_value, &eps_bits, sizeof eps_bits);
     // the captured step graph stays valid: it holds device pointers and configuration; size and Philox step are device counters

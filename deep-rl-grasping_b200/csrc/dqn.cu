@@ -291,6 +291,7 @@ GatherArgs dgather(b2g_dqn* h, bool from_replay, bool with_next) {
   g.B = h->B; g.H = 0; g.W = h->cfg.obs_dim; g.Cimg = 0; g.scale = 1.f;
   g.F_pi = h->Xscratch; g.F_v = h->X; g.F_t = h->Xn; g.FS = h->XS; g.feat_col = 0;
   g.rew_out = h->rew_n; g.done_out = h->done_n; g.n_act = 1;
+  if (from_replay) h->replay.gather_args(g, with_next);     // a replay of frames: rows through obs_frame / next_frame
   return g;
 }
 
@@ -300,6 +301,7 @@ int dqn_issue(b2g_dqn* h, bool sampled, bool apply, const float* weights) {
   pa.counters = h->counters; pa.step_consts = h->step_consts; pa.lr = h->d_lr; pa.metrics = h->metrics;
   pa.indices = h->indices; pa.eps = h->eps_dummy; pa.B = h->B; pa.A = 1; pa.replay_size = nullptr;
   pa.seed = h->cfg.seed; pa.gen = sampled ? 1 : 0; pa.apply = apply ? 1 : 0;
+  pa.ring_cap = h->replay.ring_cap();
   prep_launch(pa, s);
   const bool per = h->replay.per;
   const PerArgs pr = h->replay.per_args(h->counters, pa.seed, h->B, h->indices, h->weights, h->td, 1);
@@ -360,7 +362,9 @@ int b2g_dqn_destroy(b2g_dqn* h) {
   return 0;
 }
 
-int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out) {
+int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out) { return b2g_dqn_create2(cfg, nullptr, out); }
+
+int b2g_dqn_create2(const b2g_dqn_cfg* cfg, const b2g_replay_cfg* replay, b2g_dqn** out) {
   if (!cfg || !out) return b2g_fail(B2G_EINVAL, "cfg/out is NULL");
   *out = nullptr;
   if (cfg->n_actions < 2 || cfg->n_actions > 64) return b2g_fail(B2G_EINVAL, "n_actions must be in [2, 64]");
@@ -369,6 +373,7 @@ int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out) {
   if (cfg->obs_dim < 1 || cfg->batch < 1 || cfg->buffer_capacity < 1) return b2g_fail(B2G_EINVAL, "obs_dim, batch, buffer_capacity must be positive");
   if (cfg->prioritized_replay && cfg->batch > 1024) return b2g_fail(B2G_EINVAL, "prioritised replay supports batch <= 1024");
   if (cfg->batch > 65535) return b2g_fail(B2G_EINVAL, "batch must be <= 65535 (one gather CTA row per sample: grid.y)");
+  if (int rc = check_replay_cfg(replay, cfg->buffer_capacity, 1)) return rc;
   if (int rc = check_device(cfg->device)) return rc;
   b2g_dqn* h = new b2g_dqn();
   h->cfg = *cfg;
@@ -399,7 +404,9 @@ int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out) {
   DA(h->P, 2 * h->n_train); DA(h->Mo, h->n_train); DA(h->Vo, h->n_train); DA(h->G, h->n_train); DA(h->metrics, MET_COUNT);
   DA(h->counters, 8); DA(h->step_consts, 4); DA(h->d_lr, 1);
   const int64_t cap = cfg->buffer_capacity;
-  if ((rc = h->replay.init(h->allocs, h->stream, cap, h->E, 1, B, cfg->prioritized_replay != 0, cfg->per_alpha, cfg->per_eps))) return bail(rc);
+  if ((rc = h->replay.init(h->allocs, h->stream, cap, h->E, 1, B, cfg->prioritized_replay != 0, cfg->per_alpha, cfg->per_eps,
+                           replay ? replay->frame_capacity : 0, std::max(B, 256))))
+    return bail(rc);
   DA(h->d_mean, h->E); DA(h->d_istd, h->E); DA(h->d_normc, 8); DA(h->d_normc_act, 8);
   DA(h->X, (size_t)B * h->XS); DA(h->Xn, (size_t)B * h->XS); DA(h->Xscratch, (size_t)B * h->XS);
   for (int e = 0; e < 3; ++e) {
@@ -466,6 +473,20 @@ int b2g_dqn_replay_add(b2g_dqn* h, const float* obs, const float* act, const flo
   return h->replay.add(obs, act, rew, next_obs, done, n, h->counters, h->stream);
 }
 int64_t b2g_dqn_replay_size(const b2g_dqn* h) { B2G_USABLE(h); return h ? h->replay.size : 0; }
+
+int b2g_dqn_replay_info(const b2g_dqn* h, int64_t* capacity, int64_t* size, int64_t* frame_capacity, int64_t* live_frames, int64_t* bytes,
+                        int64_t* evicted_early) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  h->replay.info(capacity, size, frame_capacity, live_frames, bytes, evicted_early);
+  return 0;
+}
+
+int b2g_dqn_replay_get(b2g_dqn* h, int64_t slot, float* obs, float* act, float* rew, float* next_obs, float* done, int32_t* frame_ids) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  return h->replay.get(slot, obs, act, rew, next_obs, done, frame_ids, h->cfg.device, h->stream);
+}
 
 int b2g_dqn_set_norm_stats(b2g_dqn* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs, double clip_rew, double eps,
                            int norm_obs, int norm_reward) {
@@ -580,9 +601,9 @@ std::vector<FpField> dqn_fingerprint(const b2g_dqn* h) {
 }
 
 // sections 2.. (parameters .. prioritised-replay scalars) of a handle holding `live` replay rows
-std::vector<StateSection> dqn_device_sections(b2g_dqn* h, int64_t live) {
+std::vector<StateSection> dqn_device_sections(b2g_dqn* h, int64_t live, int64_t lo = 0, int64_t hi = 0) {
   std::vector<StateSection> s = adam_sections(h->P, 2 * h->n_train, h->Mo, h->Vo, h->n_train);
-  for (auto& r : h->replay.state_sections(live)) s.push_back(std::move(r));
+  for (auto& r : h->replay.state_sections(live, lo, hi)) s.push_back(std::move(r));
   return s;
 }
 
@@ -599,10 +620,11 @@ int b2g_dqn_state_save(b2g_dqn* h, const char* path) {
   CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
   uint32_t eps_bits;
   memcpy(&eps_bits, &h->eps_value, sizeof eps_bits);
-  int64_t hv[4] = {h->replay.size, h->replay.pos, h->n_updates, (int64_t)eps_bits};
-  std::vector<StateSection> secs = host_sections(hv, sizeof hv, cnt, sizeof cnt);
-  for (auto& s : dqn_device_sections(h, h->replay.size)) secs.push_back(std::move(s));
-  return state_write(path, STATE_KIND_DQN, dqn_fingerprint(h), secs);
+  std::vector<int64_t> hv = h->replay.state_host(h->n_updates, (int64_t)eps_bits);
+  const FrameRing& ring = h->replay.ring;
+  std::vector<StateSection> secs = host_sections(hv.data(), hv.size() * sizeof(int64_t), cnt, sizeof cnt);
+  for (auto& s : dqn_device_sections(h, h->replay.size, ring.frame_lo(), ring.next_fid)) secs.push_back(std::move(s));
+  return state_write(path, STATE_KIND_DQN, fp_with_frames(dqn_fingerprint(h), ring.frame_cap), secs);
 }
 
 int b2g_dqn_state_load(b2g_dqn* h, const char* path) {
@@ -610,22 +632,23 @@ int b2g_dqn_state_load(b2g_dqn* h, const char* path) {
   CK(cudaSetDevice(h->cfg.device));
   // ---- everything is checked before the handle changes
   StateReader rd;
-  if (int rc = rd.open(path, STATE_KIND_DQN, dqn_fingerprint(h))) return rc;
+  TransitionReplay& rp = h->replay;
+  if (int rc = state_open_replay(rd, path, STATE_KIND_DQN, dqn_fingerprint(h), rp.ring.frame_cap, false, "")) return rc;
   if (int rc = state_check_tags(rd, dqn_device_sections(h, 0), "DQN")) return rc;
-  int64_t hv[4];
   long long cnt[8];
-  if (rd.bytes(0) != sizeof hv || rd.bytes(1) != sizeof cnt)
-    return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
-  if (int rc = rd.read_host(0, hv, sizeof hv)) return rc;
-  if (!h->replay.valid(hv[0], hv[1]) || hv[2] < 0) return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
-  const std::vector<StateSection> dev = dqn_device_sections(h, hv[0]);
+  if (rd.bytes(1) != sizeof cnt) return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  std::vector<int64_t> hv;
+  FrameRing ring;
+  if (int rc = rp.state_host_read(rd, &hv, &ring)) return rc;
+  const std::vector<StateSection> dev = dqn_device_sections(h, hv[0], ring.frame_lo(), ring.next_fid);
   if (int rc = state_check_lengths(rd, dev)) return rc;
   if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
   // ---- from here on a failure leaves the handle unusable until a load succeeds
   CK(cudaStreamSynchronize(h->stream));
   return state_read_device(rd, dev, &h->broken, [&] {
     CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
-    h->replay.size = hv[0]; h->replay.pos = hv[1]; h->n_updates = hv[2];
+    rp.ring = ring;
+    rp.size = hv[0]; rp.pos = hv[1]; h->n_updates = hv[2];
     const uint32_t eps_bits = (uint32_t)hv[3];
     memcpy(&h->eps_value, &eps_bits, sizeof eps_bits);
     // the captured step graph stays valid: it holds device pointers and configuration; size and Philox step are device counters

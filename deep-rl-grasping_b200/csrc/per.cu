@@ -27,7 +27,9 @@ __global__ void per_sample_kernel(PerArgs a) {
     else { mass -= left; node = 2 * node + 1; }
   }
   long long idx = node - a.C;
-  if (idx >= size) idx = size - 1;                       // (rounding at the right edge of the occupied range)
+  if (a.ring_cap > 0) {                                  // live window [counters[6], + size) mod ring_cap; other leaves are 0
+    if (a.tsum[a.C + idx] == 0.0) idx = ring_slot(a.counters[6], (int)(size - 1), a.ring_cap);
+  } else if (idx >= size) idx = size - 1;                // (rounding at the right edge of the occupied range)
   const double beta = (double)a.beta[0];
   const double p_min = a.tmin[1] / total;
   const double max_w = pow(p_min * (double)size, -beta);
@@ -42,17 +44,22 @@ __global__ void per_write_kernel(PerArgs a, const int* __restrict__ slots, long 
   long long leaf = 0;
   if (i < n) {
     const long long slot = slots ? (long long)slots[i] : (first_slot + i) % cap;
-    float raw;
-    if (from_td) {
+    float raw = 0.f;
+    if (from_td == 2) {                                   // the slot left the replay: out of both trees
+      leaf = a.C + slot;
+      a.tsum[leaf] = 0.0; a.tmin[leaf] = INFINITY;
+    } else if (from_td) {
       float s = 0.f;
       for (int d = 0; d < a.D; ++d) s += fabsf(a.td[i * a.D + d]);
       raw = s + a.eps;
       atomicMax(reinterpret_cast<int*>(a.max_prio), __float_as_int(raw));      // positive floats order like their bit patterns
       if (a.prio_out) a.prio_out[i] = raw;
     } else raw = a.max_prio[0];
-    const double pr = pow((double)raw, (double)a.alpha);
-    leaf = a.C + slot;
-    a.tsum[leaf] = pr; a.tmin[leaf] = pr;
+    if (from_td != 2) {
+      const double pr = pow((double)raw, (double)a.alpha);
+      leaf = a.C + slot;
+      a.tsum[leaf] = pr; a.tmin[leaf] = pr;
+    }
   }
   __syncthreads();
   for (long long span = a.C; span > 1; span >>= 1) {
@@ -83,10 +90,23 @@ void per_init_launch(double* tsum, double* tmin, long long n2, float* max_prio, 
 }
 
 int TransitionReplay::init(std::vector<void*>& allocs, cudaStream_t s, int64_t cap_, int E_, int A_, int B, bool per_, float alpha_,
-                           float eps_) {
+                           float eps_, int64_t frame_cap, int stage_rows_) {
   cap = cap_; E = E_; A = A_; per = per_; alpha = alpha_; eps = eps_;
-  if (int rc = dev_alloc(allocs, s, &obs, cap * E)) return rc;
-  if (int rc = dev_alloc(allocs, s, &next, cap * E)) return rc;
+  if (frame_cap > 0) {
+    ring.frame_cap = frame_cap;
+    ring.dedup = frame_cap < 2 * cap;     // at 2 cap every transition has two frames of its own: sharing would save nothing
+    frame_bytes = ((int64_t)E * (int64_t)sizeof(float) + 15) / 16 * 16;   // 16-byte frame stride: the gather's 128-bit loads stay aligned
+    stage_rows = (int)std::min<int64_t>({(int64_t)stage_rows_, cap, frame_cap / 2});
+    if (int rc = dev_alloc(allocs, s, &frames, (size_t)(frame_cap * frame_bytes))) return rc;
+    if (int rc = dev_alloc(allocs, s, &r_ofr, cap)) return rc;
+    if (int rc = dev_alloc(allocs, s, &r_nfr, cap)) return rc;
+    if (int rc = dev_alloc(allocs, s, &c_obs, (size_t)stage_rows * E)) return rc;
+    if (int rc = dev_alloc(allocs, s, &c_next, (size_t)stage_rows * E)) return rc;
+    if (int rc = dev_alloc(allocs, s, &d_plan, 4 * (size_t)stage_rows)) return rc;
+  } else {
+    if (int rc = dev_alloc(allocs, s, &obs, cap * E)) return rc;
+    if (int rc = dev_alloc(allocs, s, &next, cap * E)) return rc;
+  }
   if (int rc = dev_alloc(allocs, s, &act, cap * A)) return rc;
   if (int rc = dev_alloc(allocs, s, &rew, cap)) return rc;
   if (int rc = dev_alloc(allocs, s, &done, cap)) return rc;
@@ -109,7 +129,7 @@ PerArgs TransitionReplay::per_args(const long long* counters, unsigned long long
   PerArgs pr{};
   pr.tsum = t_sum; pr.tmin = t_min; pr.C = per_C; pr.max_prio = max_prio; pr.counters = counters; pr.seed = seed;
   pr.B = B; pr.alpha = alpha; pr.eps = eps; pr.beta = beta; pr.indices = indices; pr.weights = weights;
-  pr.prio_out = prio_out; pr.td = td; pr.D = D;
+  pr.prio_out = prio_out; pr.td = td; pr.D = D; pr.ring_cap = ring_cap();
   return pr;
 }
 
@@ -124,8 +144,83 @@ void TransitionReplay::advance(int64_t n) {
   size = std::min(cap, size + n);
 }
 
+void TransitionReplay::gather_args(GatherArgs& g, bool with_next) const {
+  if (!framed()) return;
+  g.obs = nullptr; g.next_obs = nullptr;
+  g.frames = frames; g.frame_bytes = frame_bytes; g.obs_frame = r_ofr; g.next_frame = with_next ? r_nfr : nullptr;
+}
+
+int TransitionReplay::commit(const float* co, const float* cn, int m, const int64_t* cand, const float* a, const float* r, const float* d,
+                             int64_t* next_ids, cudaStream_t s) {
+  const int64_t FC = ring.frame_cap, first = ring.head_seq, fid0 = ring.next_fid, tail0 = ring.tail_seq;
+  std::vector<int> plan(3 * (size_t)m);
+  for (int i = 0; i < m; ++i) {
+    int64_t of, nf;
+    const bool share = ring.add_transition(cap, cand[i], &of, &nf);
+    plan[i] = (int)(of % FC); plan[m + i] = share ? 0 : 1; plan[2 * m + i] = (int)(nf % FC);
+    next_ids[i] = nf;
+  }
+  if (ring.dedup) CK(cudaMemcpyAsync(d_plan, plan.data(), 3 * m * sizeof(int), cudaMemcpyHostToDevice, s));
+  FrameIo io{};
+  io.c_obs = co; io.c_next = cn; io.frames = frames; io.frame_bytes = frame_bytes; io.npx = 0; io.Ci = 1; io.Ec = E;   // MLP rows: fmt {}
+  frame_commit_launch(io, ring.dedup ? d_plan : nullptr, fid0, FC, m, r_ofr, r_nfr, first, cap, s);
+  for (int64_t k = 0; k < m;) {          // act / rew / done into slots (first + k) % cap, in at most two pieces
+    const int64_t p = (first + k) % cap, len = std::min<int64_t>(m - k, cap - p);
+    CK(cudaMemcpyAsync(act + p * A, a + k * A, len * A * sizeof(float), cudaMemcpyDefault, s));
+    CK(cudaMemcpyAsync(rew + p, r + k, len * sizeof(float), cudaMemcpyDefault, s));
+    CK(cudaMemcpyAsync(done + p, d + k, len * sizeof(float), cudaMemcpyDefault, s));
+    k += len;
+  }
+  insert_max_prio(first % cap, m, s);
+  if (per) {      // transitions dropped early, whose slots no row of this chunk took over, leave the trees (after the insert)
+    const int64_t lo = std::max(tail0, ring.head_seq - cap), hi = ring.tail_seq;
+    const PerArgs pr = per_args(nullptr, 0, 0, nullptr, nullptr, nullptr, 0);
+    for (int64_t o = lo; o < hi; o += 1024) per_write_launch(pr, nullptr, o % cap, cap, (int)std::min<int64_t>(1024, hi - o), 2, s);
+  }
+  return 0;
+}
+
+int TransitionReplay::finish(std::vector<int64_t>& next_ids, long long* counters, cudaStream_t s) {
+  ring.prev_next.swap(next_ids);
+  size = ring.size();
+  pos = ring.head_seq % cap;
+  const long long rc[2] = {size, size == cap ? 0 : ring.tail_seq % cap};    // size, first live slot
+  CK(cudaMemcpyAsync(counters + 5, rc, sizeof rc, cudaMemcpyHostToDevice, s));
+  return 0;
+}
+
 int TransitionReplay::add(const float* o, const float* a, const float* r, const float* nx, const float* d, int64_t n, long long* counters,
                           cudaStream_t s) {
+  if (framed()) {
+    const int64_t R = stage_rows, FC = ring.frame_cap;
+    if (ring.dedup && 2 * n > FC) return b2g_fail(B2G_EINVAL, "replay_add: 2 n rows exceed frame_capacity (replay_frames)");
+    FrameIo io{};
+    io.c_obs = c_obs; io.c_next = c_next; io.frames = frames; io.frame_bytes = frame_bytes; io.npx = 0; io.Ci = 1; io.Ec = E;
+    std::vector<int64_t> next_ids((size_t)n), cand((size_t)R);
+    std::vector<int> hp((size_t)R), flags((size_t)R);
+    for (int64_t c0 = 0; c0 < n; c0 += R) {
+      const int m = (int)std::min<int64_t>(R, n - c0);
+      if (c0 > 0) CK(cudaStreamSynchronize(s));
+      CK(cudaMemcpyAsync(c_obs, o + c0 * E, m * E * sizeof(float), cudaMemcpyDefault, s));
+      CK(cudaMemcpyAsync(c_next, nx + c0 * E, m * E * sizeof(float), cudaMemcpyDefault, s));
+      for (int i = 0; i < m; ++i) cand[i] = -1;
+      if (ring.dedup) {       // row i's obs against the previous call's next_obs frame of row i, while it still exists
+        for (int i = 0; i < m; ++i) {
+          const int64_t p = c0 + i < (int64_t)ring.prev_next.size() ? ring.prev_next[c0 + i] : -1;
+          hp[i] = p >= 0 && p > ring.next_fid - FC ? (int)(p % FC) : -1;
+        }
+        CK(cudaMemcpyAsync(d_plan, hp.data(), m * sizeof(int), cudaMemcpyHostToDevice, s));
+        frame_check_launch(io, d_plan, d_plan + 3 * R, m, s);
+        CK(cudaMemcpyAsync(flags.data(), d_plan + 3 * R, m * sizeof(int), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        for (int i = 0; i < m; ++i) if (flags[i] & 1) cand[i] = ring.prev_next[c0 + i];
+      }
+      if (int rc = commit(c_obs, c_next, m, cand.data(), a + c0 * A, r + c0, d + c0, next_ids.data() + c0, s)) return rc;
+    }
+    if (int rc = finish(next_ids, counters, s)) return rc;
+    CK(cudaStreamSynchronize(s));
+    return 0;
+  }
   for (int64_t done_n = 0; done_n < n;) {
     const int64_t chunk = std::min(n - done_n, cap - pos);
     CK(cudaMemcpyAsync(obs + pos * E, o + done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, s));
@@ -160,8 +255,115 @@ int TransitionReplay::get_last(const int* indices, const float* weights, int B, 
   return 0;
 }
 
-std::vector<StateSection> TransitionReplay::state_sections(int64_t live) const {
+int TransitionReplay::get(int64_t slot, float* o, float* a, float* r, float* nx, float* d, int32_t* frame_ids, int device,
+                          cudaStream_t s) const {
+  const int64_t first = framed() && size < cap ? ring.tail_seq % cap : 0;
+  if (slot < 0 || slot >= cap || ((slot - first) % cap + cap) % cap >= size) return b2g_fail(B2G_EINVAL, "replay slot is not live");
+  CK(cudaSetDevice(device));
+  CK(cudaStreamSynchronize(s));
+  int fr[2] = {-1, -1};
+  if (framed()) {
+    CK(cudaMemcpy(&fr[0], r_ofr + slot, sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(&fr[1], r_nfr + slot, sizeof(int), cudaMemcpyDeviceToHost));
+  }
+  for (int w = 0; w < 2; ++w) {
+    float* dst = w ? nx : o;
+    if (!dst) continue;
+    const void* src = framed() ? (const void*)(frames + (size_t)fr[w] * frame_bytes) : (const void*)((w ? next : obs) + slot * E);
+    CK(cudaMemcpy(dst, src, E * sizeof(float), cudaMemcpyDeviceToHost));
+  }
+  if (a) CK(cudaMemcpy(a, act + slot * A, A * sizeof(float), cudaMemcpyDeviceToHost));
+  if (r) CK(cudaMemcpy(r, rew + slot, sizeof(float), cudaMemcpyDeviceToHost));
+  if (d) CK(cudaMemcpy(d, done + slot, sizeof(float), cudaMemcpyDeviceToHost));
+  if (frame_ids) { frame_ids[0] = fr[0]; frame_ids[1] = fr[1]; }
+  return 0;
+}
+
+void TransitionReplay::info(int64_t* capacity, int64_t* sz, int64_t* frame_capacity, int64_t* live_frames, int64_t* bytes,
+                            int64_t* evicted_early) const {
+  if (capacity) *capacity = cap;
+  if (sz) *sz = size;
+  if (frame_capacity) *frame_capacity = ring.frame_cap;
+  if (live_frames) *live_frames = ring.live_frames();
+  if (bytes) *bytes = transition_replay_bytes(cap, E, A, ring.frame_cap);
+  if (evicted_early) *evicted_early = ring.evicted;
+}
+
+int check_replay_cfg(const b2g_replay_cfg* r, int64_t cap, int nranks) {
+  if (!r) return 0;
+  if (r->frame_capacity < cap + 1) return b2g_fail(B2G_EINVAL, "frame_capacity (replay_frames) must be at least buffer_capacity + 1");
+  if (r->frame_capacity > INT32_MAX) return b2g_fail(B2G_EINVAL, "frame_capacity (replay_frames) must fit in int32 (frame indices)");
+  if (r->u8_plane_mask)
+    return b2g_fail(B2G_EINVAL, "u8_plane_mask: the BDQ / DQN replay stores fp32 observation vectors (8-bit planes are SAC's CNN rows)");
+  if (nranks > 1) return b2g_fail(B2G_EINVAL, "replay frames (replay_frames) are not built for data-parallel learners (nranks > 1)");
+  return 0;
+}
+
+int64_t transition_replay_bytes(int64_t cap, int E, int A, int64_t frame_cap) {
+  const int64_t fb = sizeof(float);
+  const int64_t rows = frame_cap > 0 ? frame_cap * ((E * fb + 15) / 16 * 16) + 2 * cap * (int64_t)sizeof(int) : 2 * cap * E * fb;
+  return rows + cap * (A + 2) * fb;
+}
+
+std::vector<FpField> fp_with_frames(std::vector<FpField> fp, int64_t frame_cap) {
+  if (frame_cap > 0) fp.push_back(fp_int("replay_frames", frame_cap));
+  return fp;
+}
+
+int state_open_replay(StateReader& rd, const char* path, uint32_t kind, const std::vector<FpField>& fp, int64_t frame_cap, bool owns_rms,
+                      const char* rms_set_call) {
+  const int rc = state_open_rms(rd, path, kind, fp_with_frames(fp, frame_cap), owns_rms, rms_set_call);
+  if (rc == 0) return 0;
+  const std::string msg = g_b2g_err;
+  const int has = state_fp_field(path, kind, "replay_frames");
+  if (has == 1 && frame_cap == 0)
+    return b2g_fail(B2G_EINVAL, "the state file holds a replay of frames (replay_frames); this handle was created without them");
+  if (has == 0 && frame_cap > 0)
+    return b2g_fail(B2G_EINVAL, "the state file holds the default replay layout; this handle keeps its replay in " + std::to_string(frame_cap) +
+                                    " frames (replay_frames)");
+  return b2g_fail(rc, msg);
+}
+
+std::vector<int64_t> TransitionReplay::state_host(int64_t n_updates, int64_t eps_bits) const {
+  std::vector<int64_t> hv = {size, pos, n_updates, eps_bits};
+  if (framed()) for (int64_t v : ring.pack()) hv.push_back(v);
+  return hv;
+}
+
+int TransitionReplay::state_host_read(StateReader& rd, std::vector<int64_t>* hv, FrameRing* rg) const {
+  const uint64_t hb = rd.bytes(0);
+  if (framed() ? hb % 8 || hb < 11 * 8 || hb > (uint64_t)(11 + 2 * cap + 4 * ring.frame_cap) * 8 : hb != 4 * 8)
+    return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
+  hv->resize(hb / 8);
+  if (int rc = rd.read_host(0, hv->data(), hb)) return rc;
+  const int64_t* v = hv->data();
+  *rg = ring;
+  const bool ok = framed() ? rg->unpack(v + 4, hv->size() - 4, cap) && v[0] == rg->size() && v[1] == rg->head_seq % cap : valid(v[0], v[1]);
+  if (!ok || v[2] < 0) return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
+  return 0;
+}
+
+std::vector<StateSection> TransitionReplay::state_sections(int64_t live, int64_t lo, int64_t hi) const {
   const size_t fb = sizeof(float);
+  if (framed()) {
+    std::vector<StateSection> s(8);
+    s[0].tag = state_tag("ROFR"); s[0].pieces = {dev_piece(r_ofr, cap * sizeof(int))};
+    s[1].tag = state_tag("RNFR"); s[1].pieces = {dev_piece(r_nfr, cap * sizeof(int))};
+    s[2].tag = state_tag("RACT"); s[2].pieces = {dev_piece(act, cap * A * fb)};
+    s[3].tag = state_tag("RREW"); s[3].pieces = {dev_piece(rew, cap * fb)};
+    s[4].tag = state_tag("RDON"); s[4].pieces = {dev_piece(done, cap * fb)};
+    s[5].tag = state_tag("FRMS");
+    for (int64_t f = lo; f < hi;) {      // frames [lo, hi): at most two contiguous ranges, each stored at id % frame_cap
+      const int64_t p = f % ring.frame_cap, n = std::min(hi - f, ring.frame_cap - p);
+      s[5].pieces.push_back(dev_piece(frames + p * frame_bytes, (size_t)(n * frame_bytes)));
+      f += n;
+    }
+    s[6].tag = state_tag("PERT");
+    if (per) s[6].pieces = {dev_piece(t_sum, 2 * per_C * sizeof(double)), dev_piece(t_min, 2 * per_C * sizeof(double))};
+    s[7].tag = state_tag("PERS"); s[7].pieces = {dev_piece(max_prio, sizeof(float)), dev_piece(beta, sizeof(float))};
+    return s;
+  }
+  (void)lo; (void)hi;
   std::vector<StateSection> s(7);
   s[0].tag = state_tag("ROBS"); s[0].pieces = {dev_piece(obs, live * E * fb)};
   s[1].tag = state_tag("RNXT"); s[1].pieces = {dev_piece(next, live * E * fb)};
@@ -175,3 +377,7 @@ std::vector<StateSection> TransitionReplay::state_sections(int64_t live) const {
 }
 
 }  // namespace b2g
+
+extern "C" int64_t b2g_transition_replay_bytes(int64_t buffer_capacity, int obs_dim, int act_width, int64_t frame_capacity) {
+  return b2g::transition_replay_bytes(buffer_capacity, obs_dim, act_width, frame_capacity);
+}

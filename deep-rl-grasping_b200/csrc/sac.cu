@@ -955,17 +955,6 @@ int full_index(const b2g_sac* h, int e) {
   return e == npx && h->direct_feature() ? Ci : -1;
 }
 
-// next frame id; a frame that would overwrite one a live transition references drops the oldest transitions first
-int64_t alloc_frame(b2g_sac* h) {
-  const int64_t f = h->next_fid++, over = f - h->frame_cap;
-  while (h->head_seq > h->tail_seq) {
-    while (h->lw.front().first < h->tail_seq) h->lw.pop_front();
-    if (h->lw.front().second > over) break;
-    ++h->tail_seq; ++h->evicted;
-  }
-  return f;
-}
-
 FrameIo frame_io(const b2g_sac* h, const float* c_obs, const float* c_next) {
   FrameIo io{};
   io.c_obs = c_obs; io.c_next = c_next; io.frames = h->frames; io.frame_bytes = h->frame_bytes;
@@ -986,13 +975,8 @@ int commit_chunk(b2g_sac* h, const FrameIo& io, int m, const int64_t* cand, cons
   const size_t A = h->A;
   const int64_t first = h->head_seq, fid0 = h->next_fid;
   for (int i = 0; i < m; ++i) {
-    if (h->head_seq - h->tail_seq == cap) ++h->tail_seq;                       // the ring's own replacement
-    const int64_t p = cand[i];
-    const bool share = h->dedup && p >= 0 && p >= h->next_fid + 1 - FC;
-    const int64_t of = share ? p : alloc_frame(h);
-    const int64_t nf = alloc_frame(h);
-    while (!h->lw.empty() && h->lw.back().second >= of) h->lw.pop_back();
-    h->lw.emplace_back(h->head_seq++, of);
+    int64_t of, nf;
+    const bool share = h->add_transition(cap, cand[i], &of, &nf);
     h->h_plan[i] = (int)(of % FC); h->h_plan[m + i] = share ? 0 : 1; h->h_plan[2 * m + i] = (int)(nf % FC);
     next_ids[i] = nf;
   }
@@ -1529,16 +1513,10 @@ int b2g_replay_info(const b2g_sac* h, int64_t* capacity, int64_t* size, int64_t*
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   const int64_t cap = h->cfg.buffer_capacity;
-  int64_t live = 0;
-  if (h->r_size > 0) {
-    int64_t lo = h->next_fid;
-    for (const auto& q : h->lw) if (q.first >= h->tail_seq) { lo = q.second; break; }
-    live = h->next_fid - lo;
-  }
   if (capacity) *capacity = cap;
   if (size) *size = h->r_size;
   if (frame_capacity) *frame_capacity = h->frame_cap;
-  if (live_frames) *live_frames = live;
+  if (live_frames) *live_frames = h->live_frames();
   if (bytes) *bytes = h->frame_cap * h->frame_bytes + cap * (int64_t)(2 * sizeof(int) + (h->A + 2) * sizeof(float));
   if (evicted_early) *evicted_early = h->evicted;
   return 0;
@@ -1935,22 +1913,6 @@ std::vector<FpField> sac_fingerprint(const b2g_sac* h, int extractor) {
   return fp;
 }
 
-// Host replay bookkeeping as stored: r_size, head_seq, tail_seq, next_fid, evicted, |lw|, |prev_next|, lw pairs, prev_next.
-struct SacHostState {
-  int64_t r_size = 0, head_seq = 0, tail_seq = 0, next_fid = 0, evicted = 0;
-  std::vector<std::pair<int64_t, int64_t>> lw;
-  std::vector<int64_t> prev_next;
-  // oldest frame the file must hold: the oldest one a live transition references, or a previous next_obs frame the next
-  // b2g_replay_add may still share
-  int64_t frame_lo(int64_t fcap) const {
-    int64_t lo = next_fid;
-    if (r_size > 0)
-      for (const auto& q : lw) if (q.first >= tail_seq) { lo = q.second; break; }
-    for (int64_t p : prev_next) if (p > next_fid - fcap) lo = std::min(lo, p);
-    return lo;
-  }
-};
-
 // frames [lo, hi) of the ring: at most two contiguous ranges, each stored at id % frame_cap
 std::vector<StatePiece> frame_pieces(b2g_sac* h, int64_t lo, int64_t hi) {
   std::vector<StatePiece> v;
@@ -1994,15 +1956,9 @@ int b2g_sac_state_save(b2g_sac* h, const char* path) {
   if (h->aux) { CK(cudaStreamSynchronize(h->aux)); CK(cudaStreamSynchronize(h->aux2)); }
   long long cnt[8];
   CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
-  SacHostState hs;
-  hs.r_size = h->r_size; hs.head_seq = h->head_seq; hs.tail_seq = h->tail_seq; hs.next_fid = h->next_fid; hs.evicted = h->evicted;
-  hs.lw.assign(h->lw.begin(), h->lw.end());
-  hs.prev_next = h->prev_next;
-  std::vector<int64_t> hv = {hs.r_size, hs.head_seq, hs.tail_seq, hs.next_fid, hs.evicted, (int64_t)hs.lw.size(), (int64_t)hs.prev_next.size()};
-  for (const auto& q : hs.lw) { hv.push_back(q.first); hv.push_back(q.second); }
-  hv.insert(hv.end(), hs.prev_next.begin(), hs.prev_next.end());
+  std::vector<int64_t> hv = h->pack();     // FrameRing's bookkeeping (its size is r_size)
   std::vector<StateSection> secs = host_sections(hv.data(), hv.size() * sizeof(int64_t), cnt, sizeof cnt);
-  for (auto& s : sac_device_sections(h, hs.frame_lo(h->frame_cap), hs.next_fid)) secs.push_back(std::move(s));
+  for (auto& s : sac_device_sections(h, h->frame_lo(), h->next_fid)) secs.push_back(std::move(s));
   return state_write(path, STATE_KIND_SAC, fp_with_rms(sac_fingerprint(h, h->extractor), h->rms_mean), secs);
 }
 
@@ -2031,17 +1987,10 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
     return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
   std::vector<int64_t> hv(rd.bytes(0) / 8);
   if (int rc = rd.read_host(0, hv.data(), hv.size() * 8)) return rc;
-  SacHostState hs;
-  hs.r_size = hv[0]; hs.head_seq = hv[1]; hs.tail_seq = hv[2]; hs.next_fid = hv[3]; hs.evicted = hv[4];
-  const int64_t n_lw = hv[5], n_prev = hv[6];
-  if (n_lw < 0 || n_prev < 0 || (int64_t)hv.size() != 7 + 2 * n_lw + n_prev || hs.r_size != hs.head_seq - hs.tail_seq || hs.r_size < 0 ||
-      hs.r_size > cap || hs.tail_seq < 0 || hs.next_fid < 0 || hs.evicted < 0)
-    return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
-  for (int64_t i = 0; i < n_lw; ++i) hs.lw.emplace_back(hv[7 + 2 * i], hv[8 + 2 * i]);
-  hs.prev_next.assign(hv.begin() + 7 + 2 * n_lw, hv.end());
-  const int64_t lo = hs.frame_lo(FC);
-  if (lo < 0 || lo > hs.next_fid || hs.next_fid - lo > FC) return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
-  const std::vector<StateSection> dev = sac_device_sections(h, lo, hs.next_fid);
+  FrameRing hs;
+  hs.frame_cap = FC; hs.dedup = h->dedup;
+  if (!hs.unpack(hv.data(), hv.size(), cap)) return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
+  const std::vector<StateSection> dev = sac_device_sections(h, hs.frame_lo(), hs.next_fid);
   if (int rc = state_check_lengths(rd, dev)) return rc;
   long long cnt[8];
   if (rd.bytes(1) != sizeof cnt) return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
@@ -2053,9 +2002,8 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
     if (h->rms_mean) obs_rms_derive(h);
     h->ob_n = 0;       // staged observations name frames of the replaced replay: the next b2g_sac_observe_act stages anew
     CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
-    h->r_size = hs.r_size; h->head_seq = hs.head_seq; h->tail_seq = hs.tail_seq; h->next_fid = hs.next_fid; h->evicted = hs.evicted;
-    h->lw.assign(hs.lw.begin(), hs.lw.end());
-    h->prev_next = hs.prev_next;
+    static_cast<FrameRing&>(*h) = hs;
+    h->r_size = hs.size();
     // The BF16 weight planes follow the restored arena at the next step or act.  The captured step graphs (graph_exec, pipe_graph)
     // stay valid: their kernel parameters hold device pointers and configuration only, and the replay size, first live slot and
     // Philox step they depend on are read from the device counters restored above.

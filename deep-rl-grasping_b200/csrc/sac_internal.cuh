@@ -12,6 +12,7 @@
 #include "cg.cuh"
 #include "common.cuh"
 #include "enc_stage.cuh"
+#include "frame_ring.cuh"
 #include "host.cuh"
 #include "metrics_log.cuh"
 
@@ -105,7 +106,7 @@ void obs_rms_derive(b2g_sac* h);
 
 using namespace b2g;   // (internal header: only library translation units include it)
 
-struct b2g_sac {
+struct b2g_sac : FrameRing {         // FrameRing: the replay's frame and transition bookkeeping (frame_ring.cuh)
   b2g_sac_cfg cfg{};
   bool cnn = false;
   int num_sms = 132;
@@ -124,18 +125,14 @@ struct b2g_sac {
   // (s_obs / s_next) and the pipelined staging (ps_obs / ps_next) hold such rows.
   int Ec = 0;
   // Replay: a ring of cap transition slots {obs frame, next_obs frame, act, rew, done} over a pool of frame_cap frames (one
-  // compact row each, stored in format fmt) allocated in FIFO order with monotone 64-bit ids; frame id f sits at f % frame_cap.
-  // Transitions are numbered too: the live ones are [tail_seq, head_seq), transition t sits at slot t % cap.
+  // compact row each, stored in format fmt); the frame and transition numbering is FrameRing's.
   unsigned char* frames = nullptr;
-  int64_t frame_cap = 0, frame_bytes = 0;
+  int64_t frame_bytes = 0;
   FrameFmt fmt{}, row_fmt{};         // frame format; format of an fp32 compact row (explicit batch, staging)
   uint32_t u8_mask = 0;
-  bool dedup = false;                // obs may share the previous call's next_obs frame (frame_cap < 2 cap)
   int *r_ofr = nullptr, *r_nfr = nullptr;
   float *r_act = nullptr, *r_rew = nullptr, *r_done = nullptr;
-  int64_t r_size = 0, head_seq = 0, tail_seq = 0, next_fid = 0, evicted = 0;
-  std::deque<std::pair<int64_t, int64_t>> lw;   // (transition, obs frame id): sliding-window minimum of the live obs frames
-  std::vector<int64_t> prev_next;    // frame ids of the last replay_add's next_obs rows
+  int64_t r_size = 0;
   float *c_obs = nullptr, *c_next = nullptr;    // replay_add staging: compact rows [stage_rows][Ec]
   int *d_plan = nullptr, *h_plan = nullptr;     // [4][stage_rows]: frame plan (3 rows) + check flags; h_plan pinned
   long long* h_rc = nullptr;         // pinned: replay size, first live slot -> counters[5..6]

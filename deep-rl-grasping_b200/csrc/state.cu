@@ -334,6 +334,21 @@ StateSection rms_section(double* count, double* mean, double* var, int E) {
   return r;
 }
 
+int state_fp_field(const char* path, uint32_t kind, const char* name) {
+  FILE* f = path ? fopen(path, "rb") : nullptr;
+  if (!f) return -1;
+  StateHeader hd{};
+  int found = -1;
+  if (fread(&hd, sizeof hd, 1, f) == 1 && memcmp(hd.magic, kMagic, 8) == 0 && hd.kind == kind && hd.n_fp <= 64) {
+    found = 0;
+    FpField fp{};
+    for (uint32_t i = 0; i < hd.n_fp && fread(&fp, sizeof fp, 1, f) == 1; ++i)
+      if (strncmp(fp.name, name, sizeof fp.name) == 0) found = 1;
+  }
+  fclose(f);
+  return found;
+}
+
 int state_open_rms(StateReader& rd, const char* path, uint32_t kind, const std::vector<FpField>& fp, bool owns_rms, const char* rms_set_call) {
   const int rc = rd.open(path, kind, fp_with_rms(fp, owns_rms));
   if (rc == 0) return 0;

@@ -92,5 +92,8 @@ StateSection rms_section(double* count, double* mean, double* var, int E);
 // rd.open() with the fingerprint of a handle that owns obs_rms or not; a file that differs in that alone is refused with a
 // message naming rms_set_call, the call that gives a handle its obs_rms.
 int state_open_rms(StateReader& rd, const char* path, uint32_t kind, const std::vector<FpField>& fp, bool owns_rms, const char* rms_set_call);
+// 1 when the fingerprint of the state file at path has a field of that name, 0 when not, -1 when it is no readable state file
+// of that handle kind
+int state_fp_field(const char* path, uint32_t kind, const char* name);
 
 }  // namespace b2g

@@ -17,26 +17,29 @@ from . import _lib, training_state
 from .base_model import BaseModel
 from .callbacks import as_callback
 from .tensorboard import EpisodeRewardLogger
-from .learner import HandleLearner, _f32, _fp
+from .learner import TransitionReplayLearner, _f32, _fp
 
 _ONLINE, _TARGET = "deepq/model/", "deepq/target_q_func/model/"
 
 
-class DQNLearner(HandleLearner):
+class DQNLearner(TransitionReplayLearner):
     """numpy-facing wrapper of one ``b2g_dqn`` handle (maps 1:1 onto the C ABI)."""
     _abi = "dqn"
 
     def __init__(self, obs_dim=100, n_actions=12, layers=(64, 64), batch_size=32, buffer_size=50000, gamma=0.99, seed=0, device=0,
-                 prioritized_replay=False, prioritized_replay_alpha=0.6, prioritized_replay_eps=1e-6):
+                 prioritized_replay=False, prioritized_replay_alpha=0.6, prioritized_replay_eps=1e-6, frame_capacity=None):
+        """frame_capacity: the replay frame pool of BDQLearner (include/b200grasp.h: b2g_dqn_create2); None = two rows per slot."""
         self.lib = _lib.load()
         if len(layers) != 2:
             raise NotImplementedError(f"layers={list(layers)}: the DQN learner builds two hidden layers")
         cfg = _lib.DqnCfg(obs_dim, n_actions, int(layers[0]), int(layers[1]), batch_size, buffer_size, gamma, seed, device,
                           int(bool(prioritized_replay)), float(prioritized_replay_alpha), float(prioritized_replay_eps))
         self.prioritized_replay = bool(prioritized_replay)
-        self._create(cfg)
+        self.frame_capacity = None if frame_capacity is None else int(frame_capacity)
+        self._create(cfg, self._replay_cfg(self.frame_capacity))
         self.obs_dim = self.obs_elems = obs_dim
         self.n_actions, self.batch_size = n_actions, batch_size
+        self._act_width = 1
 
     def _has_grad(self, name):
         return name.startswith(_ONLINE)
@@ -131,7 +134,8 @@ class DQN(BaseModel):
                  exploration_final_eps=0.02, exploration_initial_eps=1.0, train_freq=1, batch_size=32, double_q=True, learning_starts=1000,
                  target_network_update_freq=500, prioritized_replay=False, prioritized_replay_alpha=0.6, prioritized_replay_beta0=0.4,
                  prioritized_replay_beta_iters=None, prioritized_replay_eps=1e-6, param_noise=False, n_cpu_tf_sess=None, verbose=0,
-                 tensorboard_log=None, _init_setup_model=True, policy_kwargs=None, full_tensorboard_log=False, seed=None, device=0):
+                 tensorboard_log=None, _init_setup_model=True, policy_kwargs=None, full_tensorboard_log=False, seed=None, device=0,
+                 replay_frames=None):
         if not double_q:
             raise NotImplementedError("double_q=False: only the double-Q target is built")
         if param_noise:
@@ -151,6 +155,7 @@ class DQN(BaseModel):
         self.prioritized_replay = bool(prioritized_replay)
         self.per_alpha, self.per_beta0, self.per_beta_iters, self.per_eps = prioritized_replay_alpha, prioritized_replay_beta0, \
             prioritized_replay_beta_iters, prioritized_replay_eps
+        self.replay_frames = None if replay_frames is None else int(replay_frames)    # DQNLearner's frame_capacity
         self.verbose, self.seed, self.device = verbose, seed, device
         self.tensorboard_log = tensorboard_log
         self.num_timesteps = 0
@@ -173,7 +178,8 @@ class DQN(BaseModel):
         obs_dim = int(np.prod(self.observation_space.shape))
         self.learner = DQNLearner(obs_dim, int(self.action_space.n), tuple(self.layers), self.batch_size, self.buffer_size, self.gamma,
                                   int(self.seed or 0), self.device, prioritized_replay=self.prioritized_replay,
-                                  prioritized_replay_alpha=self.per_alpha, prioritized_replay_eps=self.per_eps)
+                                  prioritized_replay_alpha=self.per_alpha, prioritized_replay_eps=self.per_eps,
+                                  **self._replay_kwargs())
         rng = np.random.default_rng(self.seed)
         p = OrderedDict()
         for n, shp in self.learner.param_shapes.items():
@@ -318,6 +324,8 @@ class DQN(BaseModel):
                     prioritized_replay_beta0=self.per_beta0, prioritized_replay_beta_iters=self.per_beta_iters,
                     prioritized_replay_eps=self.per_eps, policy_kwargs=self.policy_kwargs, verbose=self.verbose, seed=self.seed,
                     device=self.device)
+        if self.replay_frames is not None:
+            init["replay_frames"] = self.replay_frames
         return {"algo": "DQN", "init": init, "num_timesteps": int(self.num_timesteps), "n_target_updates": int(self.n_target_updates),
                 "rng": training_state.rng_state(self._rng), "predict_rng": training_state.rng_state(self.predict_rng)}
 

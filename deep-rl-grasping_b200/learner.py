@@ -74,9 +74,13 @@ class HandleLearner:
     def _fn(self, name: str):
         return getattr(self.lib, self._names.get(name) or f"b2g_{self._abi}_{name}")
 
-    def _create(self, cfg):
+    def _create(self, cfg, replay=None):
+        """``replay``: an ``_lib.ReplayCfg`` for the ``create2`` call (BDQ / DQN replay frames); None = ``create``."""
         self.h = C.c_void_p()
-        _lib.check(self._fn("create")(C.byref(cfg), C.byref(self.h)))
+        if replay is None:
+            _lib.check(self._fn("create")(C.byref(cfg), C.byref(self.h)))
+        else:
+            _lib.check(self._fn("create2")(C.byref(cfg), C.byref(replay), C.byref(self.h)))
         self._info = OrderedDict()
         buf = C.create_string_buffer(256)
         rows, cols, nd = C.c_int64(), C.c_int64(), C.c_int32()
@@ -203,6 +207,40 @@ class HandleLearner:
         a, b = C.c_int64(), C.c_int64()
         _lib.check(self._fn("upload_bytes")(self.h, C.byref(a), C.byref(b)))
         return {"observe": int(a.value), "other": int(b.value)}
+
+
+class TransitionReplayLearner(HandleLearner):
+    """The transition replay the BDQ and DQN handles share (include/b200grasp.h: b2g_bdq_create2, b2g_*_replay_info)."""
+
+    @staticmethod
+    def _replay_cfg(frame_capacity: Optional[int]):
+        """``frame_capacity``: keep obs / next_obs in a pool of that many frames (at least buffer_size + 1); None = two rows
+        per slot."""
+        return None if frame_capacity is None else _lib.ReplayCfg(int(frame_capacity), 0)
+
+    def replay_info(self) -> dict:
+        """capacity, size, frame_capacity and live_frames (0 without frames), bytes (device memory of the replay: rows or
+        frames and frame indices, actions, rewards, dones), evicted_early."""
+        keys = ("capacity", "size", "frame_capacity", "live_frames", "bytes", "evicted_early")
+        vals = [C.c_int64() for _ in keys]
+        _lib.check(self._fn("replay_info")(self.h, *[C.byref(v) for v in vals]))
+        return {k: int(v.value) for k, v in zip(keys, vals)}
+
+    def replay_get(self, slot: int) -> dict:
+        """The stored transition of a live slot: obs, act, rew, next_obs, done, and frames = its (obs, next_obs) frame ids
+        (-1 without frames)."""
+        o, nx = np.empty(self.obs_dim, np.float32), np.empty(self.obs_dim, np.float32)
+        a = np.empty(self._act_width, np.float32)
+        r, d = np.empty(1, np.float32), np.empty(1, np.float32)
+        fr = np.empty(2, np.int32)
+        _lib.check(self._fn("replay_get")(self.h, int(slot), _fp(o), _fp(a), _fp(r), _fp(nx), _fp(d), fr.ctypes.data_as(C.POINTER(C.c_int32))))
+        return {"obs": o, "act": a, "rew": float(r[0]), "next_obs": nx, "done": float(d[0]), "frames": (int(fr[0]), int(fr[1]))}
+
+
+def transition_replay_bytes(buffer_size: int, obs_dim: int, act_width: int, frame_capacity: Optional[int] = None) -> int:
+    """Device bytes of the BDQ / DQN replay of that shape without allocating it (``act_width``: n_branches, 1 for DQN;
+    ``frame_capacity`` None = two rows per slot); the prioritised-replay trees are not counted."""
+    return int(_lib.load().b2g_transition_replay_bytes(int(buffer_size), int(obs_dim), int(act_width), int(frame_capacity or 0)))
 
 
 class Learner(HandleLearner):

@@ -14,6 +14,7 @@ from __future__ import annotations
 
 import argparse
 import importlib
+import inspect
 import logging
 import os
 
@@ -168,10 +169,7 @@ def train(args):
             policy, kw = CnnPolicy, {"layers": c["layers"], "cnn_extractor": "augmented_nature_cnn"}
         else:
             policy, kw = MlpPolicy, {"layers": c["layers"], "layer_norm": False}
-        replay = {}
-        if args.replay_spare is not None:
-            # every transition holds one frame of its own plus one per episode end; n_envs more for the rows in flight
-            replay["replay_frames"] = int(c["buffer_size"] * (1.0 + args.replay_spare)) + n_envs
+        replay = replay_frames_kwargs(args, c["buffer_size"], n_envs)
         if _is_image_obs(env) and config.get("full_observation", False) and not simplified_image:
             # RGB renders as uint8 (gripperEnv/sensor.py), depth stays fp32; the simplified observation is depth + pad even
             # under full_observation (robot.py:192-196), so it has no 8-bit planes
@@ -190,11 +188,15 @@ def train(args):
                     exploration_fraction=c.get("exploration_fraction", 0.1), exploration_final_eps=c.get("exploration_final_eps", 0.02),
                     num_actions_pad=c.get("num_actions_pad", 33), learning_starts=c.get("learning_starts", 1000),
                     target_network_update_freq=c.get("target_network_update_freq", 1000),
-                    prioritized_replay=c.get("prioritized_replay", False), device_obs_norm=bool(args.device_norm), tensorboard_log=tb)
+                    prioritized_replay=c.get("prioritized_replay", False), device_obs_norm=bool(args.device_norm), tensorboard_log=tb,
+                    **replay_frames_kwargs(args, c["buffer_size"], n_envs))
         if args.load_dir:
             model.load_parameters(BDQ.load(args.load_dir, env).get_parameters())
     elif algo == "DQN":
-        model = DQN(DQNMlpPolicy, env, tensorboard_log=tb, **dqn_kwargs(config))
+        kw = dqn_kwargs(config)
+        # sb_helper leaves DQN's buffer_size at stable-baselines' default, which DQN's signature holds
+        kw.update(replay_frames_kwargs(args, inspect.signature(DQN).parameters["buffer_size"].default, n_envs))
+        model = DQN(DQNMlpPolicy, env, tensorboard_log=tb, **kw)
         if args.load_dir:        # every parameter (sb_helper.py:183-199's partial load cannot run: tensorboard_file is undefined there)
             old = DQN.load(args.load_dir)
             model.load_parameters(old.get_parameters())
@@ -230,6 +232,14 @@ def tensorboard_log(config, algo, model_dir):
     if (config.get(algo) or {}).get("tensorboard_logs") is None:
         return None
     return "tensorboard_logs/" + model_dir
+
+
+def replay_frames_kwargs(args, buffer_size, n_envs):
+    """train --replay_spare F (SAC, BDQ, DQN): {"replay_frames": buffer_size * (1 + F) + n_envs}, or {} without the flag.  Every
+    transition holds one frame of its own plus one per episode end; n_envs more for the rows in flight."""
+    if args.replay_spare is None:
+        return {}
+    return {"replay_frames": int(buffer_size * (1.0 + args.replay_spare)) + n_envs}
 
 
 def dqn_kwargs(config):
@@ -378,8 +388,9 @@ def build_parser():
     t.add_argument("--n_envs", type=int, default=1, help=">1: SubprocVecEnv actor loop on host cores feeding the device replay")
     t.add_argument("--precision", default="bf16x3", choices=["fp32", "bf16x3", "bf16"])
     t.add_argument("--replay_spare", type=float, default=None,
-                   help="SAC replay frame budget buffer_size * (1 + F) + n_envs (observations shared between consecutive "
-                        "transitions; 0.125 covers episodes down to ~9 steps); default: two frames per replay slot")
+                   help="SAC / BDQ / DQN replay frame budget buffer_size * (1 + F) + n_envs (observations shared between "
+                        "consecutive transitions; 0.125 covers episodes down to ~9 steps); default: two frames per replay slot; "
+                        "--resume takes it from the saved run")
     t.add_argument("--device_norm", action="store_true",
                    help="keep VecNormalize's observation statistics on the GPU and upload every frame once "
                         "(SAC / BDQ(device_obs_norm=True); not DQN); --resume takes it from the saved run")

@@ -298,7 +298,15 @@ typedef struct b2g_bdq_metrics {
   int64_t n_updates;
 } b2g_bdq_metrics;
 
-int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out);
+int b2g_bdq_create(const b2g_bdq_cfg* cfg, b2g_bdq** out);   /* = b2g_bdq_create2(cfg, NULL, out) */
+/* replay != NULL: the transition replay keeps obs / next_obs in a pool of frame_capacity fp32 frames (frame_capacity >=
+ * buffer_capacity + 1, u8_plane_mask 0, nranks 1; B2G_EINVAL otherwise), as b2g_sac_create2's replay does: every next_obs
+ * takes a new frame, and row i's obs shares the frame of the previous call's next_obs of row i when the two are bitwise equal
+ * (b2g_bdq_replay_add) or by construction (b2g_bdq_observe_add, unless env i was reset).  When frames run out before slots do,
+ * the oldest transitions go early (b2g_bdq_replay_info counts them); sampling, uniform or prioritised, draws live slots only.
+ * A training-state file records the layout: a file of the other one is refused naming replay_frames.  NULL: two fp32 rows per
+ * slot, as b2g_bdq_create. */
+int b2g_bdq_create2(const b2g_bdq_cfg* cfg, const b2g_replay_cfg* replay, b2g_bdq** out);
 int b2g_bdq_destroy(b2g_bdq* h);
 int b2g_bdq_param_count(const b2g_bdq* h);
 int b2g_bdq_param_info(const b2g_bdq* h, int idx, char* name, size_t name_cap, int64_t* rows, int64_t* cols, int32_t* ndim);
@@ -308,6 +316,13 @@ int b2g_bdq_get_grad(b2g_bdq* h, const char* name, float* dst, size_t numel);
 int b2g_bdq_replay_add(b2g_bdq* h, const float* obs, const float* act_idx, const float* rew, const float* next_obs,
                        const float* done, int64_t n);
 int64_t b2g_bdq_replay_size(const b2g_bdq* h);
+/* as b2g_replay_info: frame_capacity and live_frames are 0 without frames; bytes = b2g_transition_replay_bytes of the handle */
+int b2g_bdq_replay_info(const b2g_bdq* h, int64_t* capacity, int64_t* size, int64_t* frame_capacity, int64_t* live_frames,
+                        int64_t* bytes, int64_t* evicted_early);
+/* the stored transition of a live slot (any output may be NULL); frame_ids[2]: the frames of its obs and next_obs (-1 without
+ * frames).  B2G_EINVAL for a slot that is not live. */
+int b2g_bdq_replay_get(b2g_bdq* h, int64_t slot, float* obs, float* act_idx, float* rew, float* next_obs, float* done,
+                       int32_t* frame_ids);
 /* On a handle that owns obs_rms (b2g_bdq_obs_rms_set, below) obs_mean / obs_var may be NULL with norm_obs != 0: the scalars
  * are set and the device statistics stay; passing them replaces the device statistics (count kept). */
 int b2g_bdq_set_norm_stats(b2g_bdq* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs,
@@ -398,7 +413,9 @@ typedef struct b2g_dqn_metrics {
 
 /* B2G_EINVAL naming the limit outside n_actions in [2, 64], widths multiples of 4 in [4, 512], batch <= 65535 (<= 1024 with
  * PER) */
-int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out);
+int b2g_dqn_create(const b2g_dqn_cfg* cfg, b2g_dqn** out);   /* = b2g_dqn_create2(cfg, NULL, out) */
+/* replay: the frame pool of b2g_bdq_create2, with the same rules */
+int b2g_dqn_create2(const b2g_dqn_cfg* cfg, const b2g_replay_cfg* replay, b2g_dqn** out);
 int b2g_dqn_destroy(b2g_dqn* h);
 /* index 0 = deepq/eps; then the online tensors, then the target tensors, in the zip's order */
 int b2g_dqn_param_count(const b2g_dqn* h);
@@ -412,6 +429,14 @@ int b2g_dqn_get_grad(b2g_dqn* h, const char* name, float* dst, size_t numel);
 int b2g_dqn_replay_add(b2g_dqn* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done,
                        int64_t n);
 int64_t b2g_dqn_replay_size(const b2g_dqn* h);
+int b2g_dqn_replay_info(const b2g_dqn* h, int64_t* capacity, int64_t* size, int64_t* frame_capacity, int64_t* live_frames,
+                        int64_t* bytes, int64_t* evicted_early);
+int b2g_dqn_replay_get(b2g_dqn* h, int64_t slot, float* obs, float* act, float* rew, float* next_obs, float* done, int32_t* frame_ids);
+/* Device bytes of the BDQ / DQN transition replay of buffer_capacity slots of obs_dim floats and act_width action floats
+ * (n_branches, or 1 for DQN), without allocating it: frame_capacity * round_up(4 obs_dim, 16) + 8 buffer_capacity (frame
+ * indices) with frames (frame_capacity > 0), 8 obs_dim buffer_capacity without; plus 4 (act_width + 2) buffer_capacity
+ * (actions, rewards, dones).  The prioritised-replay trees are not counted. */
+int64_t b2g_transition_replay_bytes(int64_t buffer_capacity, int obs_dim, int act_width, int64_t frame_capacity);
 /* VecNormalize's statistics for the gather of the sampled and explicit steps (the replay holds raw transitions); not used by
  * b2g_dqn_act */
 int b2g_dqn_set_norm_stats(b2g_dqn* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs,
