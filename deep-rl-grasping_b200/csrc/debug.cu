@@ -74,6 +74,13 @@ int find_debug_tensor(const b2g_sac* h, const std::string& name, DebugTensor& t)
   }
   if (name == "z0/pi") return f32(h->z0[0], B * H);
   if (name == "z0/target") return f32(h->z0[4], B * H);
+  for (int q = 1; q < 4; ++q)      // separate buffers only without engine v2 (which writes them into z0v)
+    if (name == "z0/" + head[q]) {
+      if (v.on) return b2g_fail(B2G_ESTATE, name + ": engine v2 writes the value heads' fc0 outputs into z0v");
+      return f32(h->z0[q], B * H);
+    }
+  if (name == "rew_n") return f32(h->rew_n, B);
+  if (name == "done_n") return f32(h->done_n, B);
   if (name == "z0v") { t.v2 = true; t.planes[0] = v.z0v; t.np = 1; t.elem_bytes = 4; t.numel = B * 3 * H; return 0; }
   if (name == "dz0_pi") return f32(h->dz0_pi, B * H);
   if (name == "dz0_v3") return f32(h->dz0_v3, B * 3 * H);

@@ -800,6 +800,9 @@ int b2g_debug_gg_tc(int x3, const b2g_debug_gg_tc_problem* p, int n, float* f32,
  *   F32/<net>           fp32      [B][FS]            the feature rows the head kernels read (columns as in F)
  *   z0/pi, z0/target    fp32      [B][H]             fc0 pre-activations without bias
  *   z0v                 fp32      [B][3H]            the same for vf | qf1 | qf2
+ *   z0/vf, z0/qf1, z0/qf2  fp32   [B][H]             the same as separate buffers, on a handle WITHOUT engine v2 (B2G_ESTATE on
+ *                                                    one with it: use z0v)
+ *   rew_n, done_n       fp32      [B]                the reward and done the tail read (after the gather's normalisation and clip)
  *   a0/<head>, dz1/<head>  fp32   [B][H]             fc0 activations and fc1 pre-activation gradients; head = pi, vf, qf1, qf2
  *   dz0_pi / dz0_v3     fp32      [B][H] / [B][3H]   the fp32 values of dz0pi / dz0v */
 int b2g_debug_tensor_info(const b2g_sac* h, const char* name, int64_t* numel, int32_t* planes, int32_t* elem_bytes);

@@ -535,6 +535,10 @@ def test_debug_tensor_refuses_bad_requests():
         assert L.lib.b2g_debug_tensor(L.h, b"dZ4/pi", 2, vp, 4 * 512 * 2) == _lib.B2G_EINVAL        # 2 planes
         assert L.lib.b2g_debug_tensor(L.h, b"dZ4/pi", 0, vp, 4 * 512 * 2 - 2) == _lib.B2G_EINVAL
         assert L.lib.b2g_debug_tensor(L.h, b"dZ4/target", 0, vp, 4 * 512 * 2) == _lib.B2G_EINVAL    # no target backward
+        for q in (b"z0/vf", b"z0/qf1", b"z0/qf2"):                       # engine v2 writes them into z0v
+            assert L.lib.b2g_debug_tensor(L.h, q, 0, vp, 4 * 64 * 4) == _lib.B2G_ESTATE
+        assert L.lib.b2g_debug_tensor(L.h, b"rew_n", 0, vp, 4 * 4 - 4) == _lib.B2G_EINVAL          # [B] fp32
+        assert L.lib.b2g_debug_tensor(L.h, b"done_n", 1, vp, 4 * 4) == _lib.B2G_EINVAL             # one plane
     finally:
         L.close()
     L0 = make_learner(cfg, vn, 4, params, buffer_size=64, precision=0)
@@ -542,6 +546,8 @@ def test_debug_tensor_refuses_bad_requests():
         assert L0.lib.b2g_debug_tensor(L0.h, b"dZ4/pi", 0, vp, 4 * 512 * 2) == _lib.B2G_ESTATE
         n = C.c_int64()
         assert L0.lib.b2g_debug_tensor_info(L0.h, b"F32/pi", C.byref(n), None, None) == 0
+        for q in (b"z0/vf", b"z0/qf1", b"z0/qf2"):                       # separate buffers without engine v2
+            assert L0.lib.b2g_debug_tensor_info(L0.h, q, C.byref(n), None, None) == 0 and n.value == 4 * 64
     finally:
         L0.close()
 
