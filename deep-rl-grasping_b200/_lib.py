@@ -40,7 +40,7 @@ SYMBOLS = [
     "b2g_trpo_update", "b2g_trpo_fvp", "b2g_trpo_step_explicit", "b2g_trpo_act", "b2g_trpo_get_step", "b2g_trpo_state_save",
     "b2g_trpo_state_load",
     "b2g_encoder_create", "b2g_encoder_destroy", "b2g_encoder_n_layers", "b2g_encoder_layer_shape", "b2g_encoder_set_weights",
-    "b2g_encoder_encode", "b2g_sac_set_obs_encoder", "b2g_bdq_set_obs_encoder", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor", "b2g_debug_gg_simt", "b2g_debug_gg_tc",
+    "b2g_encoder_encode", "b2g_encoder_create2", "b2g_debug_encoder_layers", "b2g_sac_set_obs_encoder", "b2g_bdq_set_obs_encoder", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor", "b2g_debug_gg_simt", "b2g_debug_gg_tc",
     "b2g_autoencoder_create", "b2g_autoencoder_destroy", "b2g_autoencoder_n_layers", "b2g_autoencoder_layer_shape",
     "b2g_autoencoder_set_weights", "b2g_autoencoder_get_weights", "b2g_autoencoder_get_grad", "b2g_autoencoder_reset_optimizer",
     "b2g_autoencoder_set_dataset", "b2g_autoencoder_train_epoch", "b2g_autoencoder_evaluate", "b2g_autoencoder_predict",
@@ -314,6 +314,8 @@ def load():
     lib.b2g_encoder_layer_shape.argtypes = [vp, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     lib.b2g_encoder_set_weights.argtypes = [vp, C.c_int, fp, C.c_size_t, fp, C.c_size_t]
     lib.b2g_encoder_encode.argtypes = [vp, fp, C.c_int, fp]
+    lib.b2g_encoder_create2.argtypes = [C.POINTER(EncoderCfg), C.c_int32, C.POINTER(vp)]
+    lib.b2g_debug_encoder_layers.argtypes = [vp, fp, C.c_int, fp, C.c_int64]
     lib.b2g_sac_set_obs_encoder.argtypes = [vp, vp, C.c_int]
     lib.b2g_bdq_set_obs_encoder.argtypes = [vp, vp, C.c_int]
     lib.b2g_autoencoder_create.argtypes = [C.POINTER(EncoderCfg), C.POINTER(vp)]

@@ -127,11 +127,13 @@ class BaseModel:
                              f"{ve.raw_width}: wrap the env in a host-mode VecEncodeDepth (as the evaluation env is)")
 
     def _encoder_host(self):
-        """host.json's record of the encoder a learner encodes with: its directory and weight digest (None without one)."""
+        """host.json's record of the encoder a learner encodes with: its directory, weight digest and precision (None
+        without one)."""
         ve = unwrap_encode_depth(self.env)
         if ve is None or ve.encoder_owner is not self.learner:
             return None
-        return {"dir": getattr(ve.encoder, "model_dir", None), "digest": ve.encoder.weights_digest()}
+        return {"dir": getattr(ve.encoder, "model_dir", None), "digest": ve.encoder.weights_digest(),
+                "precision": getattr(ve.encoder, "precision", "fp32")}
 
     @staticmethod
     def _check_encoder_digest(path, host, env):
@@ -141,6 +143,10 @@ class BaseModel:
         ve = unwrap_encode_depth(env)
         if ve is None:
             raise ValueError(f"{path} was trained on the device encoder of {want['dir']}: wrap the env in a VecEncodeDepth")
+        want_prec, got_prec = want.get("precision", "fp32"), getattr(ve.encoder, "precision", "fp32")   # older files: fp32
+        if got_prec != want_prec:
+            raise ValueError(f"{path} was trained through the {want_prec} encoder of {want['dir']}; the env's VecEncodeDepth "
+                             f"encodes in {got_prec}")
         got = ve.encoder.weights_digest()
         if got != want["digest"]:
             raise ValueError(f"{path} was trained through encoder weights {want['digest'][:12]} ({want['dir']}); the env's "

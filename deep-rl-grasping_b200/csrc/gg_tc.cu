@@ -165,7 +165,10 @@ __device__ __forceinline__ TileInfo tile_info(const DescPack& pk, int tile) {
   return ti;
 }
 
-template <bool a_rvec, bool b_rvec, bool planes>
+// enc: the encoder forward's instantiation (planes only, encoder.cu): adds the GG_EPI_BIAS_LRELU epilogue and lets a descriptor
+// without C write only its BF16 planes (C_hi / C_lo: the next layer's input).  Every other launch runs enc = false, whose code
+// is the engine as it was before the flag existed.
+template <bool a_rvec, bool b_rvec, bool planes, bool enc = false>
 __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const __grid_constant__ DescPack pk, int x3) {
   constexpr int NPROD = Roles<planes>::NPROD, MMA_WARP = Roles<planes>::MMA_WARP, NEPI = Roles<planes>::NEPI;
   constexpr int EPI_COLS = Roles<planes>::EPI_COLS;
@@ -550,6 +553,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
     uint32_t gcm = 0;                              // ring chunk counter, continuous across tiles
     int pinned_p = -1, dflags = 0, dN = 0;
     float* dC = nullptr; uint16_t* dChi = nullptr; uint16_t* dClo = nullptr; const float* dmask = nullptr;
+    float dalpha = 0.f;                            // enc: LeakyReLU slope
     const uint32_t stg = ring + STAGES * STAGE_BYTES + (uint32_t)ew * (32 * EPI_COLS * 4);
     int staged_n0 = -1, st_col = -2;               // which (column tables, column block) the staged copies belong to
     // Everything a tile's epilogue needs from global memory besides the mask -- tile coordinates, this lane's row
@@ -587,7 +591,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
         }
       } else if (et < 2 * TN) {
         const int n = e.ti.n0 + et - TN;
-        if ((fl & GG_EPI_BIAS_RELU) && n < d2.N) e.t_bias = d2.bias[n];
+        if ((fl & (enc ? GG_EPI_BIAS_RELU | GG_EPI_BIAS_LRELU : GG_EPI_BIAS_RELU)) && n < d2.N) e.t_bias = d2.bias[n];
       }
       return e;
     };
@@ -614,6 +618,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
       if (ti.p != pinned_p) {      // register copies of everything the store loops need from the descriptor
         dflags = pin(d.flags); dN = pin(d.N);
         dC = pin(d.C); dChi = pin(d.C_hi); dClo = pin(d.C_lo); dmask = pin(d.mask);
+        if (enc) dalpha = d.alpha;
         pinned_p = ti.p;
       }
       // column split between the two warps of a row quarter (8 epilogue warps, planes mode): 32 + 32 columns,
@@ -698,6 +703,12 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
               const float4 bb = *reinterpret_cast<const float4*>(&s_bias[cb + 4 * g]);
               o.x = fmaxf(o.x + bb.x, 0.f); o.y = fmaxf(o.y + bb.y, 0.f); o.z = fmaxf(o.z + bb.z, 0.f); o.w = fmaxf(o.w + bb.w, 0.f);
             }
+            if (enc && (dflags & GG_EPI_BIAS_LRELU)) {     // gg_simt's order: v + bias, then v > 0 ? v : alpha * v
+              const float4 bb = *reinterpret_cast<const float4*>(&s_bias[cb + 4 * g]);
+              o.x += bb.x; o.y += bb.y; o.z += bb.z; o.w += bb.w;
+              o.x = o.x > 0.f ? o.x : dalpha * o.x; o.y = o.y > 0.f ? o.y : dalpha * o.y;
+              o.z = o.z > 0.f ? o.z : dalpha * o.z; o.w = o.w > 0.f ? o.w : dalpha * o.w;
+            }
             const int c = ((cb - col0) >> 2) + g;
             const uint32_t a = stg + (uint32_t)lane * (EPI_COLS * 4) + (uint32_t)((c ^ (lane & 7)) << 4);
             asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(a), "f"(o.x), "f"(o.y), "f"(o.z), "f"(o.w) : "memory");
@@ -711,9 +722,10 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
             float o = __uint_as_float(v[j]);
             const int cnj = s_cn[cb + j];
             if (dflags & GG_EPI_BIAS_RELU) o = fmaxf(o + s_bias[cb + j], 0.f);
+            if (enc && (dflags & GG_EPI_BIAS_LRELU)) { o += s_bias[cb + j]; o = o > 0.f ? o : dalpha * o; }
             if (dflags & GG_EPI_MASK) o = dmask[km + s_kn[cb + j]] > 0.f ? o : 0.f;
             if (dflags & GG_EPI_ATOMIC) atomicAdd(dC + cm + cnj, o);
-            else dC[cm + cnj] = o;
+            else if (!enc || dC) dC[cm + cnj] = o;
             if (dChi) {
               const __nv_bfloat16 h = __float2bfloat16_rn(o);
               dChi[cm + cnj] = __bfloat16_as_ushort(h);
@@ -757,7 +769,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
             if (dflags & GG_EPI_ATOMIC) {
               float* cp = dC + cmr[u] + cn;
               atomicAdd(cp + 0, v4.x); atomicAdd(cp + 1, v4.y); atomicAdd(cp + 2, v4.z); atomicAdd(cp + 3, v4.w);
-            } else {
+            } else if (!enc || dC) {
               *reinterpret_cast<float4*>(dC + cmr[u] + cn) = v4;
             }
             if (dChi) {
@@ -775,22 +787,23 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
   }
 }
 
-template <bool AR, bool BR, bool PL>
+template <bool AR, bool BR, bool PL, bool ENC = false>
 cudaError_t launch_mode(const DescPack& pk, int x3, int num_sms, cudaStream_t s) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gg_tc_kernel<AR, BR, PL>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(gg_tc_kernel<AR, BR, PL, ENC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
   const int grid = pk.total_tiles < num_sms ? pk.total_tiles : num_sms;
-  return launch_pdl(gg_tc_kernel<AR, BR, PL>, dim3(grid), dim3(Roles<PL>::NTHREADS), SMEM_BYTES, s, pdl_enabled(), pk, x3);
+  return launch_pdl(gg_tc_kernel<AR, BR, PL, ENC>, dim3(grid), dim3(Roles<PL>::NTHREADS), SMEM_BYTES, s, pdl_enabled(), pk, x3);
 }
 }  // namespace
 
 int gg_tc_smem_bytes() { return SMEM_BYTES; }
 
-// All problems of one launch share the operand-contiguity mode (flags & (GG_A_RVEC | GG_B_RVEC)).
+// All problems of one launch share the operand-contiguity mode (flags & (GG_A_RVEC | GG_B_RVEC)).  GG_PLANES | GG_EPI_BIAS_LRELU
+// selects the encoder forward's instantiation.
 // host_descs: the group's descriptors (at most GG_TC_MAX_DESCS), passed as a __grid_constant__ pack.
 cudaError_t gg_tc_launch(const GemmDesc* host_descs, int ndesc, int total_tiles, int mode_flags, int x3, int num_sms, cudaStream_t s) {
   if (total_tiles <= 0) return cudaSuccess;
@@ -800,6 +813,7 @@ cudaError_t gg_tc_launch(const GemmDesc* host_descs, int ndesc, int total_tiles,
   pk.n = ndesc;
   pk.total_tiles = total_tiles;
   const bool ar = mode_flags & GG_A_RVEC, br = mode_flags & GG_B_RVEC;
+  if ((mode_flags & GG_PLANES) && (mode_flags & GG_EPI_BIAS_LRELU)) return launch_mode<true, true, true, true>(pk, x3, num_sms, s);
   if (mode_flags & GG_PLANES) return launch_mode<true, true, true>(pk, x3, num_sms, s);
   if (ar && br) return launch_mode<true, true, false>(pk, x3, num_sms, s);
   if (ar) return launch_mode<true, false, false>(pk, x3, num_sms, s);

@@ -118,10 +118,20 @@ def fit(n: int, batch_size: int, epochs: int, train_epoch: Callable[[np.ndarray,
     return history
 
 
-class Encoder(object):
-    """Base class for learning abstract representations of image observations."""
+ENCODER_PRECISIONS = {"fp32": _lib.B2G_PREC_FP32_SIMT, "bf16x3": _lib.B2G_PREC_BF16X3}
 
-    def __init__(self, config, max_batch: int = 1, device: int = 0, seed: Optional[int] = None):
+
+class Encoder(object):
+    """Base class for learning abstract representations of image observations.
+
+    ``precision`` is the arithmetic of ``encode`` and of the observe-path stage a learner copies from this encoder: "fp32"
+    (fp32 FFMA on the CUDA cores, the default) or "bf16x3" (the tensor-core engine, BF16 hi/lo operand splits summed in fp32:
+    about 2^-16 relative per layer).  ``train``, ``test`` and ``predict`` run in fp32 either way."""
+
+    def __init__(self, config, max_batch: int = 1, device: int = 0, seed: Optional[int] = None, precision: str = "fp32"):
+        if precision not in ENCODER_PRECISIONS:
+            raise ValueError(f"precision must be one of {sorted(ENCODER_PRECISIONS)}, got {precision!r}")
+        self.precision = precision
         self._handle = C.c_void_p()
         self._ae = C.c_void_p()
         self._ae_batch = 0
@@ -159,7 +169,7 @@ class SimpleAutoEncoder(Encoder):
         self._learning_rate = float(config.get("learning_rate", 2e-4))
         self._train_batch = int(config.get("batch_size", 128))
         self._weights = None            # [(kernel, bias)] of all 2L+2 layers once the decoder half is known
-        _lib.check(self._lib.b2g_encoder_create(C.byref(cfg), C.byref(self._handle)))
+        _lib.check(self._lib.b2g_encoder_create2(C.byref(cfg), ENCODER_PRECISIONS[self.precision], C.byref(self._handle)))
 
     # ---- whole auto-encoder (csrc/autoencoder.cu)
     def _shapes(self):

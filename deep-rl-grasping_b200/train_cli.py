@@ -71,11 +71,12 @@ def _is_image_obs(env):
 
 def device_encoder(config, n_envs):
     """The perception encoder of ``config['sensor']['encoder_dir']`` (the directory the reference sensor reads), for the
-    frames and terminal observations of ``n_envs`` envs in one call."""
+    frames and terminal observations of ``n_envs`` envs in one call, at the run's ``device_encode_precision`` (fp32 when
+    the config has none)."""
     from .encoders import SimpleAutoEncoder
     model_dir = os.path.expanduser(config["sensor"]["encoder_dir"])
     with open(os.path.join(model_dir, "config.yaml")) as f:
-        enc = SimpleAutoEncoder(yaml.safe_load(f), max_batch=2 * n_envs)
+        enc = SimpleAutoEncoder(yaml.safe_load(f), max_batch=2 * n_envs, precision=config.get("device_encode_precision", "fp32"))
     enc.load_weights(model_dir)
     return enc
 
@@ -102,6 +103,7 @@ def train(args):
     if args.device_encode:
         _check_device_encode(config)
         config["device_encode"] = True          # --resume and run rebuild the same stack
+        config["device_encode_precision"] = args.encoder_precision or "fp32"
     if algo == "DQN":          # stable-baselines' DQN takes one environment; its statistics stay with the host VecNormalize
         if int(args.n_envs) > 1:
             raise ValueError("--algo DQN: DQN cannot be used with more than one environment (--n_envs 1)")
@@ -397,6 +399,9 @@ def build_parser():
     t.add_argument("--device_encode", action="store_true",
                    help="the env's sensor defers the depth encoding (encoders.DeferredEncodedDepthImgSensor): encode the "
                         "frames of all envs at once in this process, on the learner's device with --device_norm (SAC / BDQ)")
+    t.add_argument("--encoder_precision", default=None, choices=["fp32", "bf16x3"],
+                   help="with --device_encode: the encoder's arithmetic, fp32 on the CUDA cores (default) or bf16x3 on the tensor "
+                        "cores (about 2^-16 relative per layer); recorded in config.yaml as device_encode_precision")
     t.add_argument("--eval_freq", type=int, default=50000)
     t.add_argument("--checkpoint_freq", type=int, default=25000)
     t.add_argument("--state_freq", type=int, default=None,
@@ -424,6 +429,8 @@ def main(argv=None):
     if not hasattr(args, "func"):
         build_parser().print_help()
         return None
+    if args.func is train and args.encoder_precision is not None and not args.device_encode:
+        parser._subparsers._group_actions[0].choices["train"].error("--encoder_precision needs --device_encode")
     if args.func is train and not args.resume:
         missing = [f"--{k}" for k in ("config", "algo", "model_dir") if getattr(args, k) is None]
         if missing:

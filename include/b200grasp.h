@@ -634,7 +634,16 @@ typedef struct b2g_encoder_cfg {
   int32_t max_batch;
   int32_t device;
 } b2g_encoder_cfg;
-int b2g_encoder_create(const b2g_encoder_cfg* cfg, b2g_encoder** out);
+int b2g_encoder_create(const b2g_encoder_cfg* cfg, b2g_encoder** out);      /* = create2(cfg, B2G_PREC_FP32_SIMT, out) */
+/* The encoder at a chosen precision (b2g_encoder_encode, and the stage b2g_*_set_obs_encoder copies from it, run at it):
+ *   B2G_PREC_FP32_SIMT  fp32 FFMA gather-GEMMs on the CUDA cores (the default; what b2g_encoder_create builds);
+ *   B2G_PREC_BF16X3     the four contractions on the wgmma engine: operands split into BF16 hi + lo, hi*hi + hi*lo + lo*hi
+ *                       summed in fp32 (about 2^-16 relative per layer, the SAC learner's bf16x3 contract).  Layer 0 reads an
+ *                       x-unfolded copy of the image whose kernel rows are padded to a multiple of 8 taps; every conv but the
+ *                       last needs filters % 8 == 0.  A frame's encoding does not depend on its batch or its row in it.
+ * B2G_EINVAL before any CUDA call for B2G_PREC_BF16 (single-pass BF16 encodings are not offered as policy inputs), any other
+ * value, a geometry b2g_encoder_create refuses, and a bf16x3 geometry the engine cannot take (the message names the reason). */
+int b2g_encoder_create2(const b2g_encoder_cfg* cfg, int32_t precision, b2g_encoder** out);
 int b2g_encoder_destroy(b2g_encoder* h);
 int b2g_encoder_n_layers(const b2g_encoder* h);                      /* conv layers + 1 (dense) */
 int b2g_encoder_layer_shape(const b2g_encoder* h, int layer, int64_t* kernel_numel, int64_t* bias_numel);
@@ -642,6 +651,9 @@ int b2g_encoder_set_weights(b2g_encoder* h, int layer, const float* kernel, size
                             size_t bias_numel);
 /* imgs: host [n, height, width, channels] fp32 -> out: host [n, encoding_dim]; B2G_ESTATE until every layer is loaded */
 int b2g_encoder_encode(b2g_encoder* h, const float* imgs, int n, float* out);
+/* debug: b2g_encoder_encode of imgs, then every layer's output as the next layer reads it (bf16x3: hi + lo of its planes):
+ * out = [conv 0 [n][out_h][out_w][f] | conv 1 ... | dense [n][encoding_dim]], out_numel their total */
+int b2g_debug_encoder_layers(b2g_encoder* h, const float* imgs, int n, float* out, int64_t out_numel);
 
 /* ---- the encoder on a learner's observe path: the env hands out raw depth rows and the learner encodes them on its device.
  * enc != NULL attaches: the encoder's geometry and weights are copied device to device into a stage the learner handle owns,
