@@ -10,25 +10,22 @@
 // the dueling aggregation, double-Q target, TD loss and backward seeds are one fused per-sample kernel.
 // Output-layer weights are held with their row stride padded to 4 floats (n_bins = 33 -> 36) so every
 // operand row is 16-byte aligned; get/set repack to the zip layout.
+// The replay, normalisation, step, training-state and metrics-log plumbing is the QLearner base shared with DQN (q_learner.cu).
 // With device statistics (b2g_bdq_obs_rms_set) the learn loop's actor side runs here too: b2g_bdq_observe_act / _add stage each
-// new frame once, merge it into VecNormalize's obs_rms (obsnorm.cu's kernel), act epsilon-greedily on the device (Philox stream
-// 3) and commit transitions into the replay with a kernel.
+// new frame once, merge it into VecNormalize's obs_rms (ObsRms, obsnorm.cuh, shared with SAC), act epsilon-greedily on the
+// device (Philox stream 3) and commit transitions into the replay with a kernel.
 #include <cuda_runtime.h>
 #include <math.h>
-#include <string.h>
 
 #include <algorithm>
-#include <cmath>
 #include <string>
 #include <vector>
 
 #include "../../include/b200grasp.h"
 #include "common.cuh"
-#include "enc_stage.cuh"
 #include "host.cuh"
-#include "metrics_log.cuh"
-#include "per.cuh"
-#include "state.cuh"
+#include "obsnorm.cuh"
+#include "q_learner.cuh"
 
 using namespace b2g;
 
@@ -158,44 +155,16 @@ __global__ void bdq_target_copy_kernel(float* __restrict__ P, long long n_train,
 }
 }  // namespace
 
-struct b2g_bdq {
+struct b2g_bdq : QLearner {     // A = D: one bin per branch
   b2g_bdq_cfg cfg{};
-  int B = 0, D = 0, n = 0, NBS = 0, T0 = 0, T1 = 0, HB = 0, XS = 0, E = 0;
-  ParamTable params;           // bdq/eps, the online tensors, then their target copies at off + n_train
-  int64_t n_train = 0;
-  float *P = nullptr, *Mo = nullptr, *Vo = nullptr, *G = nullptr, *metrics = nullptr;
-  float eps_value = 1.0f;      // bdq/eps (exploration epsilon variable of the zip)
-  cudaStream_t stream = nullptr;
-  std::vector<void*> allocs;
-  TransitionReplay replay;
-  double *d_mean = nullptr, *d_istd = nullptr, *d_normc = nullptr;
-  float *X = nullptr, *Xn = nullptr, *Xscratch = nullptr;
+  int D = 0, n = 0, NBS = 0, T0 = 0, T1 = 0, HB = 0;
   float *h1[3]{}, *h2[3]{}, *hb[3][8]{}, *Aout[3][8]{}, *hv[3]{}, *Vout[3]{};
-  float *dA[8]{}, *dV = nullptr, *dcat = nullptr, *dh2 = nullptr, *dh1 = nullptr, *td = nullptr;
-  float *rew_n = nullptr, *done_n = nullptr, *weights = nullptr, *eps_dummy = nullptr;
-  float *s_obs = nullptr, *s_next = nullptr, *s_act = nullptr, *s_rew = nullptr, *s_done = nullptr;
-  int* indices = nullptr;
-  int* act_idx_out = nullptr;
+  float *dA[8]{}, *dV = nullptr, *dcat = nullptr, *dh2 = nullptr, *dh1 = nullptr;
   const float** d_Aptr = nullptr;
-  long long* counters = nullptr;
-  double* step_consts = nullptr;
-  float* d_lr = nullptr;
-  float cur_lr = -1.f;
-  std::vector<GemmGroup> fwd, bwd, act;
-  long long n_updates = 0;
-  float* h_met = nullptr;
   void* nccl_comm = nullptr;
-  cudaGraphExec_t graph_exec = nullptr;
-  bool use_graph = true;
-  bool broken = false;         // a training-state load failed after it began writing: only destroy / load are accepted
-  MetricsLog mlog;             // per-step metrics ring (b2g_bdq_metrics_log); off: the step has no append node
-  double norm_eps = 1e-8;      // VecNormalize.epsilon of the last b2g_bdq_set_norm_stats
-  // Device-resident VecNormalize observation statistics (created by b2g_bdq_obs_rms_set): float64 mean / var [E]; the count
-  // stays on the host.  b2g_bdq_observe_act / _add staging (allocated on first use): the current observation of env i as a row
-  // of ob_rows[ob_k] (the other buffer takes the next call's next_obs), the reset frames of finished envs, and the call's
-  // actions / rewards / done flags.
-  double *rms_mean = nullptr, *rms_var = nullptr;
-  double rms_count = 0.0;
+  ObsRms rms;                  // device VecNormalize statistics (b2g_bdq_obs_rms_set), upload counts, observation encoder
+  // b2g_bdq_observe_act / _add staging (allocated on first use): the current observation of env i as a row of ob_rows[ob_k] (the
+  // other buffer takes the next call's next_obs), the reset frames of finished envs, and the call's actions / rewards / done flags.
   int stage_rows = 0;          // max(batch, 256) envs per observe call
   float* ob_rows[2]{};         // [stage_rows + B][E] (the actor's gather reads B rows from any chunk start)
   float* ob_reset = nullptr;   // [stage_rows][E]
@@ -203,10 +172,6 @@ struct b2g_bdq {
   int* ob_idx = nullptr;       // [stage_rows][D] actor output
   int ob_k = 0, ob_n = 0;
   std::vector<int64_t> ob_fid;  // replay with frames: frame id holding env i's staged observation (-1: not stored yet)
-  int64_t up_observe = 0, up_other = 0;    // host->device bytes: observe_* / obs_rms_set, and act + replay_add + set_norm_stats
-  EncStage* enc = nullptr;     // b2g_bdq_set_obs_encoder: observe_* take raw rows and encode them into the staged rows
-  float* p(const std::string& nm) { return P + params.off(nm); }
-  float* g(const std::string& nm) { return G + params.off(nm); }
 };
 
 namespace {
@@ -218,7 +183,7 @@ void add_t(b2g_bdq* h, const std::string& name, int rows, int cols, bool w, int 
 }
 
 int build(b2g_bdq* h) {
-  const int B = h->B, D = h->D, NBS = h->NBS, T0 = h->T0, T1 = h->T1, HB = h->HB, XS = h->XS, obs = h->cfg.obs_dim;
+  const int B = h->B, D = h->D, NBS = h->NBS, T0 = h->T0, T1 = h->T1, HB = h->HB, XS = h->XS, obs = h->E;
   const int* iT0; const int* iT1; const int* iHB; const int* iNBS; const int* i4; const int* iobs;
   const int* rXS; const int* rT0; const int* rT1; const int* rHB; const int* rNBS; const int* r4; const int* rcat;
   const int* kT0; const int* kT1; const int* kHB; const int* kNBS; const int* k4; const int* icat;
@@ -324,56 +289,26 @@ int build(b2g_bdq* h) {
   return 0;
 }
 
-GatherArgs bgather(b2g_bdq* h, bool from_replay, bool with_next) {
-  GatherArgs g{};
-  g.obs = from_replay ? h->replay.obs : h->s_obs;
-  g.next_obs = with_next ? (from_replay ? h->replay.next : h->s_next) : nullptr;
-  g.act = with_next ? (from_replay ? h->replay.act : h->s_act) : nullptr;
-  g.rew = from_replay ? h->replay.rew : h->s_rew;
-  g.done = from_replay ? h->replay.done : h->s_done;
-  g.indices = from_replay ? h->indices : nullptr;
-  g.mean = h->d_mean; g.var = h->d_istd; g.normc = h->d_normc;
-  g.B = h->B; g.H = 0; g.W = h->cfg.obs_dim; g.Cimg = 0; g.scale = 1.f;
-  g.F_pi = h->Xscratch; g.F_v = h->X; g.F_t = h->Xn; g.FS = h->XS; g.feat_col = 0;
-  g.rew_out = h->rew_n; g.done_out = h->done_n; g.n_act = h->D;
-  if (from_replay) h->replay.gather_args(g, with_next);     // a replay of frames: rows through obs_frame / next_frame
-  return g;
-}
-
 int bdq_issue(b2g_bdq* h, bool sampled, bool apply, const float* weights) {
   cudaStream_t s = h->stream;
-  PrepArgs pa{};
-  pa.counters = h->counters; pa.step_consts = h->step_consts; pa.lr = h->d_lr; pa.metrics = h->metrics;
-  pa.indices = h->indices; pa.eps = h->eps_dummy; pa.B = h->B; pa.A = 1; pa.replay_size = nullptr;
-  pa.seed = h->cfg.seed + 0x9E3779B97F4A7C15ull * (unsigned long long)h->cfg.rank; pa.gen = sampled ? 1 : 0; pa.apply = apply ? 1 : 0;
-  pa.ring_cap = h->replay.ring_cap();
-  prep_launch(pa, s);
-  const bool per = h->replay.per;
-  const PerArgs pr = h->replay.per_args(h->counters, pa.seed, h->B, h->indices, h->weights, h->td, h->D);
-  if (per && sampled) { per_sample_launch(pr, s); weights = h->weights; }   // overwrites the uniform draw
-  gather_launch(bgather(h, sampled, true), s);
-  CK(cudaMemsetAsync(h->G, 0, (size_t)(h->n_train + MET_COUNT) * sizeof(float), s));
-  for (auto& g : h->fwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
+  PerArgs pr;
+  if (int rc = ql_issue_prologue(h, sampled, apply, (size_t)(h->n_train + MET_COUNT), &weights, &pr)) return rc;
   BdqTailArgs t{};
-  t.B = h->B; t.D = h->D; t.n = h->n; t.NBS = h->NBS; t.gamma = h->cfg.gamma;
+  t.B = h->B; t.D = h->D; t.n = h->n; t.NBS = h->NBS; t.gamma = h->gamma;
   for (int e = 0; e < 3; ++e) { t.V[e] = h->Vout[e]; for (int d = 0; d < h->D; ++d) t.A[e][d] = h->Aout[e][d]; }
-  t.act = h->X + h->cfg.obs_dim; t.act_stride = h->XS;
+  t.act = h->X + h->E; t.act_stride = h->XS;
   t.rew = h->rew_n; t.done = h->done_n; t.weights = weights;
   for (int d = 0; d < h->D; ++d) t.dA[d] = h->dA[d];
   t.dV = h->dV; t.td = h->td; t.metrics = h->metrics;
   bdq_tail_kernel<<<(h->B + 127) / 128, 128, 0, s>>>(t);
   for (auto& g : h->bwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
-  if (per && sampled) per_write_launch(pr, h->indices, 0, h->cfg.buffer_capacity, h->B, 1, s);   // update_priorities(|td| + eps)
-  if (h->cfg.nranks > 1) {      // gradients + loss scalars averaged over the ranks (each rank sampled its own replay shard)
+  ql_issue_priorities(h, sampled, pr);
+  if (h->nranks > 1) {      // gradients + loss scalars averaged over the ranks (each rank sampled its own replay shard)
     CK(cudaMemcpyAsync(h->G + h->n_train, h->metrics, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
     if (int rc = nccl_allreduce_sum_f32(h->nccl_comm, h->G, (size_t)(h->n_train + MET_COUNT), s)) return rc;
     CK(cudaMemcpyAsync(h->metrics, h->G + h->n_train, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
   }
-  OptimArgs oa{};
-  oa.P = h->P; oa.Mo = h->Mo; oa.Vo = h->Vo; oa.G = h->G; oa.T = h->P + h->n_train;
-  oa.n_pi = (int)h->n_train; oa.n_values = 0; oa.n_ent = 0; oa.n_target = 0;
-  oa.step_consts = h->step_consts; oa.tau = 0.f; oa.grad_scale = 1.0f / (float)h->cfg.nranks; oa.metrics = h->metrics; oa.apply = apply ? 1 : 0;
-  optim_launch(oa, s);
+  optim_launch(ql_optim_args(h, apply), s);
   CK(cudaGetLastError());
   if (apply) bdq_target_copy_kernel<<<64, 256, 0, s>>>(h->P, h->n_train, h->counters, h->cfg.target_update_freq);   // counters[3] = n_updates (prep)
   if (apply && h->mlog.on()) {     // loss and mean Q (sums over the ranks), the squared gradient norm, the learning rate
@@ -387,10 +322,9 @@ int bdq_issue(b2g_bdq* h, bool sampled, bool apply, const float* weights) {
 }
 
 int bfetch(b2g_bdq* h, b2g_bdq_metrics* out) {
-  CK(cudaMemcpyAsync(h->h_met, h->metrics, MET_COUNT * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  if (int rc = ql_fetch(h)) return rc;
   if (out) {
-    const float inv = 1.0f / (float)h->cfg.nranks;
+    const float inv = 1.0f / (float)h->nranks;
     out->loss = h->h_met[BMET_LOSS] * inv; out->mean_q = h->h_met[BMET_MEANQ] * inv; out->grad_norm = sqrtf(h->h_met[BMET_GN]);
     out->n_updates = h->n_updates;
   }
@@ -402,15 +336,13 @@ extern "C" {
 
 int b2g_bdq_destroy(b2g_bdq* h) {
   if (!h) return 0;
-  cudaSetDevice(h->cfg.device);
+  cudaSetDevice(h->device);
   if (h->stream) cudaStreamSynchronize(h->stream);
-  if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
+  // the step graph first: with nranks > 1 it holds a captured all-reduce, whose resources NCCL reclaims through the communicator
+  if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
   nccl_comm_destroy(h->nccl_comm);
-  enc_stage_destroy(h->enc);
-  mlog_free(&h->mlog);
-  for (void* q : h->allocs) cudaFree(q);
-  if (h->h_met) cudaFreeHost(h->h_met);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  enc_stage_destroy(h->rms.enc);
+  ql_release(h);
   delete h;
   return 0;
 }
@@ -432,14 +364,14 @@ int b2g_bdq_create2(const b2g_bdq_cfg* cfg, const b2g_replay_cfg* replay, b2g_bd
   b2g_bdq* h = new b2g_bdq();
   h->cfg = *cfg;
   h->cfg.nccl_id = nullptr; h->cfg.nccl_lib = nullptr;
-  const char* ng = getenv("B2G_NO_GRAPH");
-  h->use_graph = !(ng && ng[0] == '1');
-  h->B = cfg->batch; h->D = cfg->n_branches; h->n = cfg->n_bins; h->NBS = (cfg->n_bins + 3) / 4 * 4;
-  h->T0 = cfg->trunk0; h->T1 = cfg->trunk1; h->HB = cfg->branch_hidden; h->E = cfg->obs_dim;
-  h->XS = (cfg->obs_dim + cfg->n_branches + 7) / 8 * 8;
+  h->device = cfg->device; h->rank = cfg->rank; h->nranks = cfg->nranks; h->seed = cfg->seed; h->gamma = cfg->gamma;
+  h->B = cfg->batch; h->E = cfg->obs_dim; h->XS = (cfg->obs_dim + cfg->n_branches + 7) / 8 * 8; h->A = cfg->n_branches;
+  h->buffer_capacity = cfg->buffer_capacity; h->prioritized = cfg->prioritized_replay != 0;
+  h->per_alpha = cfg->per_alpha; h->per_eps = cfg->per_eps;
+  h->D = cfg->n_branches; h->n = cfg->n_bins; h->NBS = (cfg->n_bins + 3) / 4 * 4;
+  h->T0 = cfg->trunk0; h->T1 = cfg->trunk1; h->HB = cfg->branch_hidden;
   h->stage_rows = std::max(cfg->batch, 256);
   auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_bdq_destroy(h); g_b2g_err = keep; return rc; };
-  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream"));
   // parameter inventory: same names and order as the zips (oracle/bdq_ref.py all_specs)
   h->params.add_scalar("bdq/eps", &h->eps_value);
   int64_t off = 0;
@@ -461,37 +393,24 @@ int b2g_bdq_create2(const b2g_bdq_cfg* cfg, const b2g_replay_cfg* replay, b2g_bd
   h->params.add_copies(1, h->params.count() - 1, "bdq/model", "bdq/target_q_func/model", h->n_train);
   int rc = 0;
   const int B = h->B, D = h->D;
+  if ((rc = ql_init(h, MET_COUNT, replay, h->stage_rows))) return bail(rc);     // the metrics ride the all-reduce in G
 #define BA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
-  BA(h->P, 2 * h->n_train); BA(h->Mo, h->n_train); BA(h->Vo, h->n_train); BA(h->G, h->n_train + MET_COUNT); BA(h->metrics, MET_COUNT);
-  BA(h->counters, 8); BA(h->step_consts, 4); BA(h->d_lr, 1);
-  const int64_t cap = cfg->buffer_capacity;
-  if ((rc = h->replay.init(h->allocs, h->stream, cap, h->E, D, B, cfg->prioritized_replay != 0, cfg->per_alpha, cfg->per_eps,
-                           replay ? replay->frame_capacity : 0, h->stage_rows)))
-    return bail(rc);
-  BA(h->d_mean, h->E); BA(h->d_istd, h->E); BA(h->d_normc, 8);
-  BA(h->X, (size_t)B * h->XS); BA(h->Xn, (size_t)B * h->XS); BA(h->Xscratch, (size_t)B * h->XS);
   for (int e = 0; e < 3; ++e) {
     BA(h->h1[e], B * h->T0); BA(h->h2[e], B * h->T1); BA(h->hv[e], B * h->HB); BA(h->Vout[e], B * 4);
     for (int d = 0; d < D; ++d) { BA(h->hb[e][d], B * h->HB); BA(h->Aout[e][d], B * h->NBS); }
   }
   for (int d = 0; d < D; ++d) BA(h->dA[d], B * h->NBS);
-  BA(h->dV, B * 4); BA(h->dcat, (size_t)B * (D + 1) * h->HB); BA(h->dh2, B * h->T1); BA(h->dh1, B * h->T0); BA(h->td, B * D);
-  BA(h->rew_n, B); BA(h->done_n, B); BA(h->weights, B); BA(h->eps_dummy, B + 8); BA(h->indices, B + 4); BA(h->act_idx_out, B * D);
-  BA(h->s_obs, (size_t)B * h->E); BA(h->s_next, (size_t)B * h->E); BA(h->s_act, B * D); BA(h->s_rew, B); BA(h->s_done, B);
+  BA(h->dV, B * 4); BA(h->dcat, (size_t)B * (D + 1) * h->HB); BA(h->dh2, B * h->T1); BA(h->dh1, B * h->T0);
   BA(h->d_Aptr, 8);
 #undef BA
-  if (cudaMallocHost((void**)&h->h_met, MET_COUNT * sizeof(float)) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "cudaMallocHost"));
   {
-    std::vector<double> ones(h->E, 1.0);
-    const double nc[8] = {1.0, 10.0, 10.0, 0.0, 0.0, 0, 0, 0};
     const float* ap[8] = {};
     for (int d = 0; d < D; ++d) ap[d] = h->Aout[0][d];
-    if (cudaMemcpyAsync(h->d_istd, ones.data(), h->E * sizeof(double), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
-        cudaMemcpyAsync(h->d_normc, nc, sizeof(nc), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
-        cudaMemcpyAsync(h->d_Aptr, ap, sizeof(ap), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
+    if (cudaMemcpyAsync(h->d_Aptr, ap, sizeof(ap), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
         cudaStreamSynchronize(h->stream) != cudaSuccess)
       return bail(b2g_fail(B2G_ECUDA, "init copies"));
   }
+  h->rms.E = h->E; h->rms.d_mean = h->d_mean; h->rms.d_istd = h->d_istd; h->rms.set_call = "b2g_bdq_obs_rms_set";
   if ((rc = build(h))) return bail(rc);
   if (cfg->nranks > 1) {
     if ((rc = nccl_comm_init(&h->nccl_comm, cfg->nranks, cfg->nccl_id, cfg->rank, cfg->nccl_lib))) return bail(rc);
@@ -513,107 +432,33 @@ int b2g_bdq_set_param(b2g_bdq* h, const char* name, const float* src, size_t num
 int b2g_bdq_get_grad(b2g_bdq* h, const char* name, float* dst, size_t numel) { return param_copy(h, name, ParamCopy::GetGrad, dst, numel); }
 
 int b2g_bdq_replay_add(b2g_bdq* h, const float* obs, const float* act_idx, const float* rew, const float* next_obs, const float* done, int64_t n) {
-  B2G_USABLE(h);
-  if (!h || !obs || !act_idx || !rew || !next_obs || !done || n < 0) return b2g_fail(B2G_EINVAL, "NULL argument");
-  CK(cudaSetDevice(h->cfg.device));
-  if (int rc = h->replay.add(obs, act_idx, rew, next_obs, done, n, h->counters, h->stream)) return rc;
-  h->up_other += (int64_t)(n * (2 * h->E + h->D + 2) * sizeof(float) + sizeof(long long));
+  if (int rc = ql_replay_add(h, obs, act_idx, rew, next_obs, done, n, nullptr)) return rc;
+  h->rms.up_other += (int64_t)(n * (2 * h->E + h->D + 2) * sizeof(float) + sizeof(long long));
   return 0;
 }
-int64_t b2g_bdq_replay_size(const b2g_bdq* h) { B2G_USABLE(h); return h ? h->replay.size : 0; }
-
+int64_t b2g_bdq_replay_size(const b2g_bdq* h) { return ql_replay_size(h); }
 int b2g_bdq_replay_info(const b2g_bdq* h, int64_t* capacity, int64_t* size, int64_t* frame_capacity, int64_t* live_frames, int64_t* bytes,
                         int64_t* evicted_early) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  h->replay.info(capacity, size, frame_capacity, live_frames, bytes, evicted_early);
-  return 0;
+  return ql_replay_info(h, capacity, size, frame_capacity, live_frames, bytes, evicted_early);
 }
-
 int b2g_bdq_replay_get(b2g_bdq* h, int64_t slot, float* obs, float* act_idx, float* rew, float* next_obs, float* done, int32_t* frame_ids) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  return h->replay.get(slot, obs, act_idx, rew, next_obs, done, frame_ids, h->cfg.device, h->stream);
+  return ql_replay_get(h, slot, obs, act_idx, rew, next_obs, done, frame_ids);
 }
-
 int b2g_bdq_set_norm_stats(b2g_bdq* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs, double clip_rew, double eps,
                            int norm_obs, int norm_reward) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  if (norm_obs && !h->rms_mean && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  const bool eps_changed = eps != h->norm_eps;
-  h->norm_eps = eps;
-  if (h->rms_mean) {
-    // the handle owns obs_rms: statistics passed here replace it (count kept); the gather's table is derived on the device,
-    // again when only epsilon changed
-    if (obs_mean && obs_var) {
-      if (int rc = b2g_bdq_obs_rms_set(h, obs_mean, obs_var, h->rms_count)) return rc;
-    } else if (eps_changed) {
-      obs_rms_update_launch(nullptr, nullptr, nullptr, 0, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, 0, 0,
-                            h->stream);
-      CK(cudaStreamSynchronize(h->stream));
-    }
-  } else if (norm_obs) {
-    std::vector<double> istd(h->E);
-    for (int i = 0; i < h->E; ++i) istd[i] = 1.0 / sqrt(obs_var[i] + eps);
-    CK(cudaMemcpy(h->d_mean, obs_mean, h->E * sizeof(double), cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(h->d_istd, istd.data(), h->E * sizeof(double), cudaMemcpyHostToDevice));
-    h->up_other += (int64_t)(2 * h->E * sizeof(double));
-  }
-  const double nc[8] = {1.0 / sqrt(ret_var + eps), clip_obs, clip_rew, (double)norm_obs, (double)norm_reward, 0, 0, 0};
-  CK(cudaMemcpy(h->d_normc, nc, sizeof(nc), cudaMemcpyHostToDevice));
-  h->up_other += (int64_t)sizeof(nc);
-  return 0;
+  return ql_set_norm_stats(h, h ? &h->rms : nullptr, obs_mean, obs_var, ret_var, clip_obs, clip_rew, eps, norm_obs, norm_reward);
 }
-
 int b2g_bdq_step(b2g_bdq* h, int n_steps, float lr, b2g_bdq_metrics* out) {
-  B2G_USABLE(h);
-  if (!h || n_steps < 0) return b2g_fail(B2G_EINVAL, "bad argument");
-  if (h->replay.size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
-  CK(cudaSetDevice(h->cfg.device));
-  if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
-  if (h->use_graph && !h->graph_exec)       // the whole step (~14 launches of tiny layers) replays as one graph
-    if (int rc = capture_graph(h->stream, [&] { return bdq_issue(h, true, true, nullptr); }, &h->graph_exec)) return rc;
-  for (int i = 0; i < n_steps; ++i) {
-    if (h->graph_exec) CK(cudaGraphLaunch(h->graph_exec, h->stream));
-    else if (int rc = bdq_issue(h, true, true, nullptr)) return rc;
-    ++h->n_updates;
-  }
+  if (int rc = ql_step(h, n_steps, lr, [h] { return bdq_issue(h, true, true, nullptr); })) return rc;
   return bfetch(h, out);
 }
-
-int b2g_bdq_set_per_beta(b2g_bdq* h, float beta) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  return h->replay.set_beta(beta, h->cfg.device, h->stream);
-}
-
-// h->indices holds the slots of the last sampled step with uniform replay too (prep_kernel draws them, per_sample_kernel
-// overwrites them with PER); weights and prio_out are written by PER steps only
-int b2g_bdq_get_last_per(b2g_bdq* h, int32_t* slots, float* weights, float* priorities) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  return h->replay.get_last(h->indices, h->weights, h->B, slots, weights, priorities, h->cfg.device, h->stream);
-}
-
+int b2g_bdq_set_per_beta(b2g_bdq* h, float beta) { return ql_set_per_beta(h, beta); }
+int b2g_bdq_get_last_per(b2g_bdq* h, int32_t* slots, float* weights, float* priorities) { return ql_get_last_per(h, slots, weights, priorities); }
 int b2g_bdq_step_explicit(b2g_bdq* h, const float* obs, const float* act_idx, const float* rew, const float* next_obs, const float* done,
                           const float* weights, float lr, int apply_update, b2g_bdq_metrics* out, float* td_out) {
-  B2G_USABLE(h);
-  if (!h || !obs || !act_idx || !rew || !next_obs || !done) return b2g_fail(B2G_EINVAL, "NULL argument");
-  CK(cudaSetDevice(h->cfg.device));
-  if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
-  const size_t B = h->B, E = h->E, D = h->D;
-  CK(cudaMemcpyAsync(h->s_obs, obs, B * E * sizeof(float), cudaMemcpyDefault, h->stream));
-  CK(cudaMemcpyAsync(h->s_next, next_obs, B * E * sizeof(float), cudaMemcpyDefault, h->stream));
-  CK(cudaMemcpyAsync(h->s_act, act_idx, B * D * sizeof(float), cudaMemcpyDefault, h->stream));
-  CK(cudaMemcpyAsync(h->s_rew, rew, B * sizeof(float), cudaMemcpyDefault, h->stream));
-  CK(cudaMemcpyAsync(h->s_done, done, B * sizeof(float), cudaMemcpyDefault, h->stream));
-  if (weights) CK(cudaMemcpyAsync(h->weights, weights, B * sizeof(float), cudaMemcpyDefault, h->stream));
-  if (int rc = bdq_issue(h, false, apply_update != 0, weights ? h->weights : nullptr)) return rc;
-  if (apply_update) ++h->n_updates;
-  if (td_out) CK(cudaMemcpyAsync(td_out, h->td, B * D * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  if (int rc = ql_step_explicit(h, obs, act_idx, rew, next_obs, done, weights, lr, apply_update, td_out, nullptr,
+                                [h](bool apply, const float* w) { return bdq_issue(h, false, apply, w); }))
+    return rc;
   return bfetch(h, out);
 }
 
@@ -621,13 +466,13 @@ int b2g_bdq_step_explicit(b2g_bdq* h, const float* obs, const float* act_idx, co
 int b2g_bdq_act(b2g_bdq* h, const float* obs, int n, int32_t* act_idx_out) {
   B2G_USABLE(h);
   if (!h || !obs || !act_idx_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
-  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaSetDevice(h->device));
   const size_t E = h->E, D = h->D;
   for (int done_n = 0; done_n < n; done_n += h->B) {
     const int chunk = std::min(h->B, n - done_n);
     CK(cudaMemcpyAsync(h->s_obs, obs + (size_t)done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-    h->up_other += (int64_t)(chunk * E * sizeof(float));
-    GatherArgs g = bgather(h, false, false);
+    h->rms.up_other += (int64_t)(chunk * E * sizeof(float));
+    GatherArgs g = ql_gather(h, false, false);
     gather_launch(g, h->stream);
     for (auto& gr : h->act) gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
     bdq_argmax_kernel<<<(chunk * (int)D + 127) / 128, 128, 0, h->stream>>>(h->d_Aptr, chunk, (int)D, h->n, h->NBS, h->act_idx_out);
@@ -639,104 +484,25 @@ int b2g_bdq_act(b2g_bdq* h, const float* obs, int n, int32_t* act_idx_out) {
 }
 
 // ------------------------------------------------------------------------------------------------ obs_rms on the device and the
-// actor loop fed from one upload per frame (the BDQ counterpart of obsnorm.cu; the merge is the same kernel, flat layout)
-int b2g_bdq_obs_rms_set(b2g_bdq* h, const double* mean, const double* var, double count) {
-  B2G_USABLE(h);
-  if (!h || !mean || !var) return b2g_fail(B2G_EINVAL, "NULL argument");
-  if (!(count >= 0.0) || !std::isfinite(count)) return b2g_fail(B2G_EINVAL, "obs_rms_set: count must be finite and >= 0");
-  for (int e = 0; e < h->E; ++e)
-    if (!std::isfinite(mean[e]) || !(var[e] >= 0.0) || !std::isfinite(var[e]))
-      return b2g_fail(B2G_EINVAL, "obs_rms_set: mean must be finite and var finite and >= 0 (element " + std::to_string(e) + ")");
-  if (h->cfg.nranks > 1)
-    return b2g_fail(B2G_ESTATE, "device observation statistics are per handle: with nranks > 1 every rank would own different ones");
-  CK(cudaSetDevice(h->cfg.device));
-  if (!h->rms_mean) {     // one allocation for both arrays: it either exists or it does not
-    double* mv = nullptr;
-    if (int rc = dev_alloc(h->allocs, h->stream, &mv, 2 * (size_t)h->E, false)) return rc;
-    h->rms_mean = mv;
-    h->rms_var = mv + h->E;
-  }
-  CK(cudaMemcpyAsync(h->rms_mean, mean, h->E * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  CK(cudaMemcpyAsync(h->rms_var, var, h->E * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  h->up_observe += (int64_t)(2 * h->E * sizeof(double));
-  h->rms_count = count;
-  obs_rms_update_launch(nullptr, nullptr, nullptr, 0, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, 0, 0,
-                        h->stream);
-  CK(cudaStreamSynchronize(h->stream));     // host arrays are caller-owned: copied before return
-  return 0;
-}
-
-int b2g_bdq_obs_rms_get(b2g_bdq* h, double* mean, double* var, double* count) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  if (!h->rms_mean) return b2g_fail(B2G_ESTATE, "the handle has no device statistics: call b2g_bdq_obs_rms_set first");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  if (mean) CK(cudaMemcpy(mean, h->rms_mean, h->E * sizeof(double), cudaMemcpyDeviceToHost));
-  if (var) CK(cudaMemcpy(var, h->rms_var, h->E * sizeof(double), cudaMemcpyDeviceToHost));
-  if (count) *count = h->rms_count;
-  return 0;
-}
-
+// actor loop fed from one upload per frame (ObsRms, obsnorm.cuh; the merge is obsnorm.cu's kernel over the flat layout)
+int b2g_bdq_obs_rms_set(b2g_bdq* h, const double* mean, const double* var, double count) { return obs_rms_set(h, mean, var, count); }
+int b2g_bdq_obs_rms_get(b2g_bdq* h, double* mean, double* var, double* count) { return obs_rms_get(h, mean, var, count); }
 int b2g_bdq_upload_bytes(const b2g_bdq* h, int64_t* observe_bytes, int64_t* other_bytes) {
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  if (observe_bytes) *observe_bytes = h->up_observe;
-  if (other_bytes) *other_bytes = h->up_other;
-  return 0;
-}
-
-static int bdq_upload(b2g_bdq* h, void* dst, const void* src, size_t bytes) {
-  CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream));
-  h->up_observe += (int64_t)bytes;
-  return 0;
-}
-
-static void bdq_merge(b2g_bdq* h, const float* a, const float* b, const float* done, int n) {
-  obs_rms_update_launch(a, b, done, n, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, 0, 0, h->stream);
-  h->rms_count += n;
-}
-
-// the n frames of a call -> rows [n][E] at dst: uploaded as they are or, with an observation encoder, as raw rows it encodes there
-static int bdq_stage_frames(b2g_bdq* h, float* dst, const float* obs, int n) {
-  if (!h->enc) return bdq_upload(h, dst, obs, (size_t)n * h->E * sizeof(float));
-  if (int rc = bdq_upload(h, enc_stage_raw(h->enc, 0), obs, (size_t)n * enc_stage_row_floats(h->enc) * sizeof(float))) return rc;
-  return enc_stage_encode(h->enc, 0, nullptr, n, 0, dst, h->stream);
-}
-
-// the reset frames of the n_done finished envs -> row i of ob_reset; only those cross the bus and, with an observation encoder,
-// only those are encoded (it reads the flags ob_done, uploaded before)
-static int bdq_stage_reset_frames(b2g_bdq* h, const float* reset_obs, const float* done, int n, int n_done) {
-  const size_t rw = h->enc ? enc_stage_row_floats(h->enc) : h->E;
-  float* dst = h->enc ? enc_stage_raw(h->enc, 1) : h->ob_reset;
-  for (int i = 0; i < n; ++i)
-    if (done[i] != 0.f)
-      if (int rc = bdq_upload(h, dst + i * rw, reset_obs + i * rw, rw * sizeof(float))) return rc;
-  return h->enc ? enc_stage_encode(h->enc, 1, h->ob_done, n, n_done, h->ob_reset, h->stream) : 0;
+  return obs_rms_upload_bytes(h, observe_bytes, other_bytes);
 }
 
 int b2g_bdq_set_obs_encoder(b2g_bdq* h, const b2g_encoder* enc, int tail) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  if (enc) {
-    if (int rc = enc_stage_check(enc, h->cfg.device, tail, h->E)) return rc;
-    if (h->cfg.nranks > 1)
-      return b2g_fail(B2G_ESTATE, "set_obs_encoder: the observe path is per handle: with nranks > 1 every rank would encode its own");
-  }
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  EncStage* st = nullptr;
   if (enc)
-    if (int rc = enc_stage_create(enc, h->stage_rows, tail, h->stream, &st)) return rc;
-  enc_stage_destroy(h->enc);
-  h->enc = st;
-  h->ob_n = 0;          // staged observations were in the other layout
-  return 0;
+    if (int rc = obs_rms_check_encoder(h, enc, tail)) return rc;
+  return obs_rms_attach_encoder(h, enc, tail);
 }
 
 static int bdq_observe_checks(b2g_bdq* h, int n, int update_stats) {
   if (n < 1 || n > h->stage_rows)
     return b2g_fail(B2G_EINVAL, "observe: n must be in [1, " + std::to_string(h->stage_rows) + "] (the staging holds max(batch, 256) frames)");
-  if (update_stats && !h->rms_mean) return b2g_fail(B2G_ESTATE, "update_stats needs device statistics: call b2g_bdq_obs_rms_set first");
+  if (update_stats && !h->rms.on()) return b2g_fail(B2G_ESTATE, "update_stats needs device statistics: call b2g_bdq_obs_rms_set first");
   if (h->ob_rows[0]) return 0;
   const size_t R = h->stage_rows, E = h->E;
   for (int k = 0; k < 2; ++k)
@@ -753,23 +519,23 @@ int b2g_bdq_observe_act(b2g_bdq* h, const float* obs, int n, int update_stats, f
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   if (!obs && !act_idx_out) return b2g_fail(B2G_EINVAL, "observe_act: nothing to do (obs and act_idx_out are NULL)");
   if (act_idx_out && !(eps >= 0.f && eps <= 1.f)) return b2g_fail(B2G_EINVAL, "observe_act: eps must be in [0, 1]");
-  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaSetDevice(h->device));
   if (int rc = bdq_observe_checks(h, n, obs ? update_stats : 0)) return rc;
   if (!obs && h->ob_n == 0) return b2g_fail(B2G_ESTATE, "observe_act: no staged observations (pass obs first)");
   if (!obs && n != h->ob_n) return b2g_fail(B2G_EINVAL, "observe_act: n differs from the number of staged observations");
   const size_t E = h->E, D = h->D;
   float* cur = h->ob_rows[h->ob_k];
   if (obs) {
-    if (int rc = bdq_stage_frames(h, cur, obs, n)) return rc;
-    if (update_stats) bdq_merge(h, cur, nullptr, nullptr, n);
+    if (int rc = h->rms.stage_frames(cur, obs, n, h->stream)) return rc;
+    if (update_stats) h->rms.merge(cur, nullptr, nullptr, n, h->stream);
     h->ob_n = n;
     h->ob_fid.assign((size_t)n, -1);
   }
   if (act_idx_out) {
-    const unsigned long long seed = h->cfg.seed + 0x9E3779B97F4A7C15ull * (unsigned long long)h->cfg.rank;
+    const unsigned long long seed = h->philox_key();
     for (int k = 0; k < n; k += h->B) {
       const int chunk = std::min(h->B, n - k);
-      GatherArgs g = bgather(h, false, false);
+      GatherArgs g = ql_gather(h, false, false);
       g.obs = cur + (size_t)k * E;
       gather_launch(g, h->stream);
       for (auto& gr : h->act) gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
@@ -786,11 +552,11 @@ int b2g_bdq_observe_add(b2g_bdq* h, const float* act_idx, const float* rew, cons
                         int n, int update_stats) {
   B2G_USABLE(h);
   if (!h || !act_idx || !rew || !next_obs || !done) return b2g_fail(B2G_EINVAL, "NULL argument");
-  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaSetDevice(h->device));
   if (int rc = bdq_observe_checks(h, n, update_stats)) return rc;
   if (h->ob_n == 0) return b2g_fail(B2G_ESTATE, "observe_add: no staged observations (call b2g_bdq_observe_act first)");
   if (n != h->ob_n) return b2g_fail(B2G_EINVAL, "observe_add: n differs from the number of staged observations");
-  if (n > h->cfg.buffer_capacity) return b2g_fail(B2G_EINVAL, "observe_add: n exceeds buffer_capacity");
+  if (n > h->buffer_capacity) return b2g_fail(B2G_EINVAL, "observe_add: n exceeds buffer_capacity");
   if (h->replay.ring.dedup && 2 * (int64_t)n > h->replay.ring.frame_cap)
     return b2g_fail(B2G_EINVAL, "observe_add: 2 n rows exceed frame_capacity (replay_frames)");
   int n_done = 0;
@@ -799,12 +565,12 @@ int b2g_bdq_observe_add(b2g_bdq* h, const float* act_idx, const float* rew, cons
   const size_t E = h->E, D = h->D, fb = E * sizeof(float);
   float* cur = h->ob_rows[h->ob_k];
   float* nxt = h->ob_rows[h->ob_k ^ 1];
-  if (int rc = bdq_stage_frames(h, nxt, next_obs, n)) return rc;
-  if (int rc = bdq_upload(h, h->ob_act, act_idx, n * D * sizeof(float))) return rc;
-  if (int rc = bdq_upload(h, h->ob_rew, rew, n * sizeof(float))) return rc;
-  if (int rc = bdq_upload(h, h->ob_done, done, n * sizeof(float))) return rc;
+  if (int rc = h->rms.stage_frames(nxt, next_obs, n, h->stream)) return rc;
+  if (int rc = h->rms.upload(h->ob_act, act_idx, n * D * sizeof(float), h->stream)) return rc;
+  if (int rc = h->rms.upload(h->ob_rew, rew, n * sizeof(float), h->stream)) return rc;
+  if (int rc = h->rms.upload(h->ob_done, done, n * sizeof(float), h->stream)) return rc;
   if (n_done)
-    if (int rc = bdq_stage_reset_frames(h, reset_obs, done, n, n_done)) return rc;
+    if (int rc = h->rms.stage_reset_frames(h->ob_reset, reset_obs, done, h->ob_done, n, n_done, h->stream)) return rc;
   // the transitions: obs = the staged rows, next_obs = the uploaded rows (a finished env's terminal frame)
   TransitionReplay& rp = h->replay;
   std::vector<int64_t> next_ids;
@@ -822,7 +588,7 @@ int b2g_bdq_observe_add(b2g_bdq* h, const float* act_idx, const float* rew, cons
     rp.insert_max_prio(rp.pos, n, h->stream);     // as in b2g_bdq_replay_add
   }
   // VecNormalize's step_wait merges the frames the VecEnv returned: a finished env's reset frame, not its terminal observation
-  if (update_stats) bdq_merge(h, nxt, n_done ? h->ob_reset : nullptr, h->ob_done, n);
+  if (update_stats) h->rms.merge(nxt, n_done ? h->ob_reset : nullptr, h->ob_done, n, h->stream);
   // the new rows become the current observations; a finished env continues from the frame its reset returned
   for (int i = 0; i < n; ++i)
     if (done[i] != 0.f) CK(cudaMemcpyAsync(nxt + i * E, h->ob_reset + i * E, fb, cudaMemcpyDeviceToDevice, h->stream));
@@ -848,89 +614,28 @@ std::vector<FpField> bdq_fingerprint(const b2g_bdq* h) {
           fp_int("trunk_grad_rescale", c.trunk_grad_rescale), fp_int("seed", (int64_t)c.seed),
           fp_int("prioritized_replay", c.prioritized_replay), fp_real("per_alpha", c.per_alpha), fp_real("per_eps", c.per_eps)};
 }
-// sections 2.. (parameters .. prioritised-replay scalars, then obs_rms when the handle owns it) of a handle holding `live`
-// replay rows
-std::vector<StateSection> bdq_device_sections(b2g_bdq* h, int64_t live, int64_t lo = 0, int64_t hi = 0) {
-  std::vector<StateSection> s = adam_sections(h->P, 2 * h->n_train, h->Mo, h->Vo, h->n_train);
-  for (auto& r : h->replay.state_sections(live, lo, hi)) s.push_back(std::move(r));
-  if (h->rms_mean) s.push_back(rms_section(&h->rms_count, h->rms_mean, h->rms_var, h->E));
-  return s;
-}
-
 }  // namespace
 
 extern "C" {
 
 int b2g_bdq_state_save(b2g_bdq* h, const char* path) {
-  if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
-  B2G_USABLE(h);
-  if (h->cfg.nranks > 1)
-    return b2g_fail(B2G_ESTATE, "training-state files of data-parallel learners (nranks > 1) are not built: each rank holds its own replay shard");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  long long cnt[8];
-  CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
-  uint32_t eps_bits;
-  memcpy(&eps_bits, &h->eps_value, sizeof eps_bits);
-  std::vector<int64_t> hv = h->replay.state_host(h->n_updates, (int64_t)eps_bits);
-  const FrameRing& ring = h->replay.ring;
-  std::vector<StateSection> secs = host_sections(hv.data(), hv.size() * sizeof(int64_t), cnt, sizeof cnt);
-  for (auto& s : bdq_device_sections(h, h->replay.size, ring.frame_lo(), ring.next_fid)) secs.push_back(std::move(s));
-  return state_write(path, STATE_KIND_BDQ, fp_with_rms(fp_with_frames(bdq_fingerprint(h), ring.frame_cap), h->rms_mean), secs);
+  return ql_state_save(h, path, STATE_KIND_BDQ, h ? bdq_fingerprint(h) : std::vector<FpField>{}, h ? &h->rms : nullptr,
+                       h && h->nranks > 1 ? "training-state files of data-parallel learners (nranks > 1) are not built: each rank "
+                                                "holds its own replay shard"
+                                              : nullptr);
 }
 
 int b2g_bdq_state_load(b2g_bdq* h, const char* path) {
-  if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
-  if (h->cfg.nranks > 1) return b2g_fail(B2G_ESTATE, "training-state files of data-parallel learners (nranks > 1) are not built");
-  CK(cudaSetDevice(h->cfg.device));
-  // ---- everything is checked before the handle changes
-  StateReader rd;
-  TransitionReplay& rp = h->replay;
-  if (int rc = state_open_replay(rd, path, STATE_KIND_BDQ, bdq_fingerprint(h), rp.ring.frame_cap, h->rms_mean, "b2g_bdq_obs_rms_set")) return rc;
-  if (int rc = state_check_tags(rd, bdq_device_sections(h, 0), "BDQ")) return rc;
-  long long cnt[8];
-  if (rd.bytes(1) != sizeof cnt) return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
-  std::vector<int64_t> hv;
-  FrameRing ring;
-  if (int rc = rp.state_host_read(rd, &hv, &ring)) return rc;
-  const std::vector<StateSection> dev = bdq_device_sections(h, hv[0], ring.frame_lo(), ring.next_fid);
-  if (int rc = state_check_lengths(rd, dev)) return rc;
-  if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
-  // ---- from here on a failure leaves the handle unusable until a load succeeds
-  CK(cudaStreamSynchronize(h->stream));
-  return state_read_device(rd, dev, &h->broken, [&] {
-    if (h->rms_mean) {
-      obs_rms_update_launch(nullptr, nullptr, nullptr, 0, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, 0, 0,
-                            h->stream);
-      CK(cudaStreamSynchronize(h->stream));
-    }
-    h->ob_n = 0;       // the staged observations are not part of the file: a resumed run starts a fresh episode
-    CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
-    rp.ring = ring;
-    rp.size = hv[0]; rp.pos = hv[1]; h->n_updates = hv[2];
-    const uint32_t eps_bits = (uint32_t)hv[3];
-    memcpy(&h->eps_value, &eps_bits, sizeof eps_bits);
-    // the captured step graph stays valid: it holds device pointers and configuration; size and Philox step are device counters
-    return mlog_rebase(&h->mlog, h->counters + 3, h->stream);     // the restored counter: rows before it are not pending
-  });
+  return ql_state_load(h, path, STATE_KIND_BDQ, h ? bdq_fingerprint(h) : std::vector<FpField>{}, h ? &h->rms : nullptr,
+                       h && h->nranks > 1 ? "training-state files of data-parallel learners (nranks > 1) are not built" : nullptr,
+                       "BDQ", [h] { h->ob_n = 0; });     // the staged observations are not part of the file: a fresh episode
 }
 
-int b2g_bdq_metrics_log(b2g_bdq* h, int capacity) {
-  B2G_USABLE(h);
-  if (!h || capacity < 0) return b2g_fail(B2G_EINVAL, "bad argument");
-  CK(cudaSetDevice(h->cfg.device));
-  if (int rc = mlog_enable(&h->mlog, capacity, B2G_BDQ_LOG_COLS, h->counters + 3, h->stream)) return rc;
-  // the step gains or loses its append node: capture again at the next step
-  if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
-  return 0;
-}
+int b2g_bdq_metrics_log(b2g_bdq* h, int capacity) { return ql_metrics_log(h, capacity, B2G_BDQ_LOG_COLS); }
 
 int b2g_bdq_metrics_drain(b2g_bdq* h, float* rows, int max_rows, int64_t* first_step, int* n_rows, int64_t* lost) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
-  const float inv = 1.0f / (float)h->cfg.nranks;
-  return mlog_drain(&h->mlog, h->counters + 3, h->stream, rows, max_rows, first_step, n_rows, lost, [inv](float* r) {
+  const float inv = h ? 1.0f / (float)h->nranks : 1.0f;
+  return ql_metrics_drain(h, rows, max_rows, first_step, n_rows, lost, [inv](float* r) {
     r[0] *= inv; r[1] *= inv; r[2] = sqrtf(r[2]);     // as bfetch
   });
 }

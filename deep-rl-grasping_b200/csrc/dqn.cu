@@ -11,10 +11,10 @@
 // aligned; get/set repack to the zip layout.  The hard target copy is the caller's (b2g_dqn_update_target): stable-baselines
 // decides it by the environment-step count, which the device never sees.  The replay gather normalises with the statistics of
 // b2g_dqn_set_norm_stats (raw transitions are stored); the actor (b2g_dqn_act) takes observations as the network sees them, the
-// VecNormalize wrapper's output, as stable-baselines' act and predict do.
+// VecNormalize wrapper's output, as stable-baselines' act and predict do.  The replay, normalisation, step, training-state and
+// metrics-log plumbing is the QLearner base shared with BDQ (q_learner.cu).
 #include <cuda_runtime.h>
 #include <math.h>
-#include <string.h>
 
 #include <algorithm>
 #include <string>
@@ -23,9 +23,7 @@
 #include "../../include/b200grasp.h"
 #include "common.cuh"
 #include "host.cuh"
-#include "metrics_log.cuh"
-#include "per.cuh"
-#include "state.cuh"
+#include "q_learner.cuh"
 
 using namespace b2g;
 
@@ -145,41 +143,15 @@ __global__ void dqn_act_kernel(const float* __restrict__ A, const float* __restr
 }
 }  // namespace
 
-struct b2g_dqn {
+struct b2g_dqn : QLearner {     // A = 1
   b2g_dqn_cfg cfg{};
-  int B = 0, n = 0, NAS = 0, H0 = 0, H1 = 0, XS = 0, E = 0;
-  ParamTable params;           // deepq/eps, the online tensors, then their target copies at off + n_train
-  int64_t n_train = 0;
-  float *P = nullptr, *Mo = nullptr, *Vo = nullptr, *G = nullptr, *metrics = nullptr;
-  float eps_value = 1.0f;      // deepq/eps (exploration epsilon variable of the zip)
-  cudaStream_t stream = nullptr;
-  std::vector<void*> allocs;
-  TransitionReplay replay;
-  double *d_mean = nullptr, *d_istd = nullptr, *d_normc = nullptr;
+  int n = 0, NAS = 0, H0 = 0, H1 = 0;
   double* d_normc_act = nullptr;   // the actor's gather: observations arrive as the network sees them (no normalisation)
-  float *X = nullptr, *Xn = nullptr, *Xscratch = nullptr;
   float *h1[3][2]{}, *h2[3][2]{}, *Aout[3]{}, *Vout[3]{};      // [evaluation][tower 0 = action_value, 1 = state_value]
-  float *dA = nullptr, *dV = nullptr, *dh2[2]{}, *dh1[2]{}, *td = nullptr;
-  float *rew_n = nullptr, *done_n = nullptr, *weights = nullptr, *eps_dummy = nullptr;
-  float *s_obs = nullptr, *s_next = nullptr, *s_act = nullptr, *s_rew = nullptr, *s_done = nullptr;
-  int* indices = nullptr;
-  int* act_idx_out = nullptr;
+  float *dA = nullptr, *dV = nullptr, *dh2[2]{}, *dh1[2]{};
   float* q_rows = nullptr;
   ClipJob* clip_jobs = nullptr;
   int n_clip = 0;
-  long long* counters = nullptr;
-  double* step_consts = nullptr;
-  float* d_lr = nullptr;
-  float cur_lr = -1.f;
-  std::vector<GemmGroup> fwd, bwd, act;
-  long long n_updates = 0;
-  float* h_met = nullptr;
-  cudaGraphExec_t graph_exec = nullptr;
-  bool use_graph = true;
-  bool broken = false;         // a training-state load failed after it began writing: only destroy / load are accepted
-  MetricsLog mlog;             // per-step metrics ring (b2g_dqn_metrics_log); off: the step has no append node
-  float* p(const std::string& nm) { return P + params.off(nm); }
-  float* g(const std::string& nm) { return G + params.off(nm); }
 };
 
 namespace {
@@ -195,7 +167,7 @@ void add_t(b2g_dqn* h, const std::string& name, int rows, int cols, bool w, int 
 }
 
 int build(b2g_dqn* h) {
-  const int B = h->B, NAS = h->NAS, H0 = h->H0, H1 = h->H1, XS = h->XS, obs = h->cfg.obs_dim;
+  const int B = h->B, NAS = h->NAS, H0 = h->H0, H1 = h->H1, XS = h->XS, obs = h->E;
   const int *iH0, *iH1, *iNAS, *i4, *iobs, *rXS, *rH0, *rH1, *rNAS, *r4, *kH0, *kH1, *kNAS, *k4;
 #define DT(var, vec) if (int rc = upload_table(h->allocs, h->stream, (vec), &var)) return rc;
   DT(iH0, iota_tab(H0)) DT(iH1, iota_tab(H1)) DT(iNAS, iota_tab(NAS)) DT(i4, iota_tab(4)) DT(iobs, iota_tab(XS))
@@ -279,51 +251,21 @@ int build(b2g_dqn* h) {
   return 0;
 }
 
-GatherArgs dgather(b2g_dqn* h, bool from_replay, bool with_next) {
-  GatherArgs g{};
-  g.obs = from_replay ? h->replay.obs : h->s_obs;
-  g.next_obs = with_next ? (from_replay ? h->replay.next : h->s_next) : nullptr;
-  g.act = with_next ? (from_replay ? h->replay.act : h->s_act) : nullptr;
-  g.rew = from_replay ? h->replay.rew : h->s_rew;
-  g.done = from_replay ? h->replay.done : h->s_done;
-  g.indices = from_replay ? h->indices : nullptr;
-  g.mean = h->d_mean; g.var = h->d_istd; g.normc = h->d_normc;
-  g.B = h->B; g.H = 0; g.W = h->cfg.obs_dim; g.Cimg = 0; g.scale = 1.f;
-  g.F_pi = h->Xscratch; g.F_v = h->X; g.F_t = h->Xn; g.FS = h->XS; g.feat_col = 0;
-  g.rew_out = h->rew_n; g.done_out = h->done_n; g.n_act = 1;
-  if (from_replay) h->replay.gather_args(g, with_next);     // a replay of frames: rows through obs_frame / next_frame
-  return g;
-}
-
 int dqn_issue(b2g_dqn* h, bool sampled, bool apply, const float* weights) {
   cudaStream_t s = h->stream;
-  PrepArgs pa{};
-  pa.counters = h->counters; pa.step_consts = h->step_consts; pa.lr = h->d_lr; pa.metrics = h->metrics;
-  pa.indices = h->indices; pa.eps = h->eps_dummy; pa.B = h->B; pa.A = 1; pa.replay_size = nullptr;
-  pa.seed = h->cfg.seed; pa.gen = sampled ? 1 : 0; pa.apply = apply ? 1 : 0;
-  pa.ring_cap = h->replay.ring_cap();
-  prep_launch(pa, s);
-  const bool per = h->replay.per;
-  const PerArgs pr = h->replay.per_args(h->counters, pa.seed, h->B, h->indices, h->weights, h->td, 1);
-  if (per && sampled) { per_sample_launch(pr, s); weights = h->weights; }   // overwrites the uniform draw
-  gather_launch(dgather(h, sampled, true), s);
-  CK(cudaMemsetAsync(h->G, 0, (size_t)h->n_train * sizeof(float), s));
-  for (auto& g : h->fwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
+  PerArgs pr;
+  if (int rc = ql_issue_prologue(h, sampled, apply, (size_t)h->n_train, &weights, &pr)) return rc;
   DqnTailArgs t{};
-  t.B = h->B; t.n = h->n; t.NAS = h->NAS; t.gamma = h->cfg.gamma;
+  t.B = h->B; t.n = h->n; t.NAS = h->NAS; t.gamma = h->gamma;
   for (int e = 0; e < 3; ++e) { t.V[e] = h->Vout[e]; t.A[e] = h->Aout[e]; }
-  t.act = h->X + h->cfg.obs_dim; t.act_stride = h->XS;
+  t.act = h->X + h->E; t.act_stride = h->XS;
   t.rew = h->rew_n; t.done = h->done_n; t.weights = weights;
   t.dA = h->dA; t.dV = h->dV; t.td = h->td; t.metrics = h->metrics;
   dqn_tail_kernel<<<(h->B + 127) / 128, 128, 0, s>>>(t);
   for (auto& g : h->bwd) gg_simt_launch(g.dev, (int)g.host.size(), g.total_tiles, s);
   dqn_clip_kernel<<<h->n_clip, kClipThreads, 0, s>>>(h->G, h->clip_jobs, kGradClip, h->metrics);
-  if (per && sampled) per_write_launch(pr, h->indices, 0, h->cfg.buffer_capacity, h->B, 1, s);   // update_priorities(|td| + eps)
-  OptimArgs oa{};
-  oa.P = h->P; oa.Mo = h->Mo; oa.Vo = h->Vo; oa.G = h->G; oa.T = h->P + h->n_train;
-  oa.n_pi = (int)h->n_train; oa.n_values = 0; oa.n_ent = 0; oa.n_target = 0;
-  oa.step_consts = h->step_consts; oa.tau = 0.f; oa.grad_scale = 1.0f; oa.metrics = h->metrics; oa.apply = apply ? 1 : 0;
-  optim_launch(oa, s);
+  ql_issue_priorities(h, sampled, pr);
+  optim_launch(ql_optim_args(h, apply), s);
   if (apply && h->mlog.on()) {     // the dfetch accumulators (squared gradient norm, clip count as a float), the learning rate
     MetricsLogSrc m{};
     m.src[0] = h->metrics + DMET_LOSS; m.src[1] = h->metrics + DMET_MEANQ; m.src[2] = h->metrics + DMET_ABSTD;
@@ -336,8 +278,7 @@ int dqn_issue(b2g_dqn* h, bool sampled, bool apply, const float* weights) {
 }
 
 int dfetch(b2g_dqn* h, b2g_dqn_metrics* out) {
-  CK(cudaMemcpyAsync(h->h_met, h->metrics, MET_COUNT * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  if (int rc = ql_fetch(h)) return rc;
   if (out) {
     out->loss = h->h_met[DMET_LOSS]; out->mean_q = h->h_met[DMET_MEANQ]; out->mean_abs_td = h->h_met[DMET_ABSTD];
     out->grad_norm = sqrtf(h->h_met[DMET_GN2]); out->n_clipped = (int32_t)lrintf(h->h_met[DMET_NCLIP]);
@@ -351,13 +292,7 @@ extern "C" {
 
 int b2g_dqn_destroy(b2g_dqn* h) {
   if (!h) return 0;
-  cudaSetDevice(h->cfg.device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
-  mlog_free(&h->mlog);
-  for (void* q : h->allocs) cudaFree(q);
-  if (h->h_met) cudaFreeHost(h->h_met);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  ql_release(h);
   delete h;
   return 0;
 }
@@ -377,13 +312,13 @@ int b2g_dqn_create2(const b2g_dqn_cfg* cfg, const b2g_replay_cfg* replay, b2g_dq
   if (int rc = check_device(cfg->device)) return rc;
   b2g_dqn* h = new b2g_dqn();
   h->cfg = *cfg;
-  const char* ng = getenv("B2G_NO_GRAPH");
-  h->use_graph = !(ng && ng[0] == '1');
-  h->B = cfg->batch; h->n = cfg->n_actions; h->NAS = (cfg->n_actions + 3) / 4 * 4;
-  h->H0 = cfg->hidden0; h->H1 = cfg->hidden1; h->E = cfg->obs_dim;
-  h->XS = (cfg->obs_dim + 1 + 7) / 8 * 8;
+  h->device = cfg->device; h->seed = cfg->seed; h->gamma = cfg->gamma;
+  h->B = cfg->batch; h->E = cfg->obs_dim; h->XS = (cfg->obs_dim + 1 + 7) / 8 * 8;
+  h->buffer_capacity = cfg->buffer_capacity; h->prioritized = cfg->prioritized_replay != 0;
+  h->per_alpha = cfg->per_alpha; h->per_eps = cfg->per_eps;
+  h->n = cfg->n_actions; h->NAS = (cfg->n_actions + 3) / 4 * 4;
+  h->H0 = cfg->hidden0; h->H1 = cfg->hidden1;
   auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_dqn_destroy(h); g_b2g_err = keep; return rc; };
-  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "stream"));
   // parameter inventory in zip order (oracle/dqn_ref.py all_specs)
   h->params.add_scalar("deepq/eps", &h->eps_value);
   int64_t off = 0;
@@ -400,33 +335,20 @@ int b2g_dqn_create2(const b2g_dqn_cfg* cfg, const b2g_replay_cfg* replay, b2g_dq
   h->params.add_copies(1, h->params.count() - 1, kOnline, kTarget, h->n_train);
   int rc = 0;
   const int B = h->B;
+  if ((rc = ql_init(h, 0, replay, std::max(B, 256)))) return bail(rc);
 #define DA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
-  DA(h->P, 2 * h->n_train); DA(h->Mo, h->n_train); DA(h->Vo, h->n_train); DA(h->G, h->n_train); DA(h->metrics, MET_COUNT);
-  DA(h->counters, 8); DA(h->step_consts, 4); DA(h->d_lr, 1);
-  const int64_t cap = cfg->buffer_capacity;
-  if ((rc = h->replay.init(h->allocs, h->stream, cap, h->E, 1, B, cfg->prioritized_replay != 0, cfg->per_alpha, cfg->per_eps,
-                           replay ? replay->frame_capacity : 0, std::max(B, 256))))
-    return bail(rc);
-  DA(h->d_mean, h->E); DA(h->d_istd, h->E); DA(h->d_normc, 8); DA(h->d_normc_act, 8);
-  DA(h->X, (size_t)B * h->XS); DA(h->Xn, (size_t)B * h->XS); DA(h->Xscratch, (size_t)B * h->XS);
+  DA(h->d_normc_act, 8);
   for (int e = 0; e < 3; ++e) {
     for (int tw = 0; tw < 2; ++tw) { DA(h->h1[e][tw], B * h->H0); DA(h->h2[e][tw], B * h->H1); }
     DA(h->Aout[e], B * h->NAS); DA(h->Vout[e], B * 4);
   }
   DA(h->dA, B * h->NAS); DA(h->dV, B * 4);
   for (int tw = 0; tw < 2; ++tw) { DA(h->dh2[tw], B * h->H1); DA(h->dh1[tw], B * h->H0); }
-  DA(h->td, B);
-  DA(h->rew_n, B); DA(h->done_n, B); DA(h->weights, B); DA(h->eps_dummy, B + 8); DA(h->indices, B + 4); DA(h->act_idx_out, B);
   DA(h->q_rows, B * h->n);
-  DA(h->s_obs, (size_t)B * h->E); DA(h->s_next, (size_t)B * h->E); DA(h->s_act, B); DA(h->s_rew, B); DA(h->s_done, B);
 #undef DA
-  if (cudaMallocHost((void**)&h->h_met, MET_COUNT * sizeof(float)) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "cudaMallocHost"));
   {
-    std::vector<double> ones(h->E, 1.0);
     const double nc[8] = {1.0, 10.0, 10.0, 0.0, 0.0, 0, 0, 0};
-    if (cudaMemcpyAsync(h->d_istd, ones.data(), h->E * sizeof(double), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
-        cudaMemcpyAsync(h->d_normc, nc, sizeof(nc), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
-        cudaMemcpyAsync(h->d_normc_act, nc, sizeof(nc), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
+    if (cudaMemcpyAsync(h->d_normc_act, nc, sizeof(nc), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
         cudaStreamSynchronize(h->stream) != cudaSuccess)
       return bail(b2g_fail(B2G_ECUDA, "init copies"));
   }
@@ -466,98 +388,39 @@ static int dqn_check_actions(const b2g_dqn* h, const float* act, int64_t n) {
 }
 
 int b2g_dqn_replay_add(b2g_dqn* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done, int64_t n) {
-  B2G_USABLE(h);
-  if (!h || !obs || !act || !rew || !next_obs || !done || n < 0) return b2g_fail(B2G_EINVAL, "NULL argument");
-  CK(cudaSetDevice(h->cfg.device));
-  if (int rc = dqn_check_actions(h, act, n)) return rc;
-  return h->replay.add(obs, act, rew, next_obs, done, n, h->counters, h->stream);
+  return ql_replay_add(h, obs, act, rew, next_obs, done, n, [&] { return dqn_check_actions(h, act, n); });
 }
-int64_t b2g_dqn_replay_size(const b2g_dqn* h) { B2G_USABLE(h); return h ? h->replay.size : 0; }
-
+int64_t b2g_dqn_replay_size(const b2g_dqn* h) { return ql_replay_size(h); }
 int b2g_dqn_replay_info(const b2g_dqn* h, int64_t* capacity, int64_t* size, int64_t* frame_capacity, int64_t* live_frames, int64_t* bytes,
                         int64_t* evicted_early) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  h->replay.info(capacity, size, frame_capacity, live_frames, bytes, evicted_early);
-  return 0;
+  return ql_replay_info(h, capacity, size, frame_capacity, live_frames, bytes, evicted_early);
 }
-
 int b2g_dqn_replay_get(b2g_dqn* h, int64_t slot, float* obs, float* act, float* rew, float* next_obs, float* done, int32_t* frame_ids) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  return h->replay.get(slot, obs, act, rew, next_obs, done, frame_ids, h->cfg.device, h->stream);
+  return ql_replay_get(h, slot, obs, act, rew, next_obs, done, frame_ids);
 }
-
 int b2g_dqn_set_norm_stats(b2g_dqn* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs, double clip_rew, double eps,
                            int norm_obs, int norm_reward) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  if (norm_obs && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  if (norm_obs) {
-    std::vector<double> istd(h->E);
-    for (int i = 0; i < h->E; ++i) istd[i] = 1.0 / sqrt(obs_var[i] + eps);
-    CK(cudaMemcpy(h->d_mean, obs_mean, h->E * sizeof(double), cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(h->d_istd, istd.data(), h->E * sizeof(double), cudaMemcpyHostToDevice));
-  }
-  const double nc[8] = {1.0 / sqrt(ret_var + eps), clip_obs, clip_rew, (double)norm_obs, (double)norm_reward, 0, 0, 0};
-  CK(cudaMemcpy(h->d_normc, nc, sizeof(nc), cudaMemcpyHostToDevice));
-  return 0;
+  return ql_set_norm_stats(h, nullptr, obs_mean, obs_var, ret_var, clip_obs, clip_rew, eps, norm_obs, norm_reward);
 }
-
 int b2g_dqn_step(b2g_dqn* h, int n_steps, float lr, b2g_dqn_metrics* out) {
-  B2G_USABLE(h);
-  if (!h || n_steps < 0) return b2g_fail(B2G_EINVAL, "bad argument");
-  if (h->replay.size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
-  CK(cudaSetDevice(h->cfg.device));
-  if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
-  if (h->use_graph && !h->graph_exec)       // the whole step (~14 launches of tiny layers) replays as one graph
-    if (int rc = capture_graph(h->stream, [&] { return dqn_issue(h, true, true, nullptr); }, &h->graph_exec)) return rc;
-  for (int i = 0; i < n_steps; ++i) {
-    if (h->graph_exec) CK(cudaGraphLaunch(h->graph_exec, h->stream));
-    else if (int rc = dqn_issue(h, true, true, nullptr)) return rc;
-    ++h->n_updates;
-  }
+  if (int rc = ql_step(h, n_steps, lr, [h] { return dqn_issue(h, true, true, nullptr); })) return rc;
   return dfetch(h, out);
 }
-
-int b2g_dqn_set_per_beta(b2g_dqn* h, float beta) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  return h->replay.set_beta(beta, h->cfg.device, h->stream);
-}
-
-int b2g_dqn_get_last_per(b2g_dqn* h, int32_t* slots, float* weights, float* priorities) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  return h->replay.get_last(h->indices, h->weights, h->B, slots, weights, priorities, h->cfg.device, h->stream);
-}
-
+int b2g_dqn_set_per_beta(b2g_dqn* h, float beta) { return ql_set_per_beta(h, beta); }
+int b2g_dqn_get_last_per(b2g_dqn* h, int32_t* slots, float* weights, float* priorities) { return ql_get_last_per(h, slots, weights, priorities); }
 int b2g_dqn_step_explicit(b2g_dqn* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done,
                           const float* weights, float lr, int apply_update, b2g_dqn_metrics* out, float* td_out) {
-  B2G_USABLE(h);
-  if (!h || !obs || !act || !rew || !next_obs || !done) return b2g_fail(B2G_EINVAL, "NULL argument");
-  CK(cudaSetDevice(h->cfg.device));
-  if (int rc = dqn_check_actions(h, act, h->B)) return rc;
-  if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
-  const size_t B = h->B, E = h->E;
-  CK(cudaMemcpyAsync(h->s_obs, obs, B * E * sizeof(float), cudaMemcpyDefault, h->stream));
-  CK(cudaMemcpyAsync(h->s_next, next_obs, B * E * sizeof(float), cudaMemcpyDefault, h->stream));
-  CK(cudaMemcpyAsync(h->s_act, act, B * sizeof(float), cudaMemcpyDefault, h->stream));
-  CK(cudaMemcpyAsync(h->s_rew, rew, B * sizeof(float), cudaMemcpyDefault, h->stream));
-  CK(cudaMemcpyAsync(h->s_done, done, B * sizeof(float), cudaMemcpyDefault, h->stream));
-  if (weights) CK(cudaMemcpyAsync(h->weights, weights, B * sizeof(float), cudaMemcpyDefault, h->stream));
-  if (int rc = dqn_issue(h, false, apply_update != 0, weights ? h->weights : nullptr)) return rc;
-  if (apply_update) ++h->n_updates;
-  if (td_out) CK(cudaMemcpyAsync(td_out, h->td, B * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  if (int rc = ql_step_explicit(h, obs, act, rew, next_obs, done, weights, lr, apply_update, td_out,
+                                [&] { return dqn_check_actions(h, act, h->B); },
+                                [h](bool apply, const float* w) { return dqn_issue(h, false, apply, w); }))
+    return rc;
   return dfetch(h, out);
 }
 
 int b2g_dqn_update_target(b2g_dqn* h) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaSetDevice(h->device));
   CK(cudaMemcpyAsync(h->P + h->n_train, h->P, (size_t)h->n_train * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return 0;
@@ -566,12 +429,12 @@ int b2g_dqn_update_target(b2g_dqn* h) {
 int b2g_dqn_act(b2g_dqn* h, const float* obs, int n, int32_t* act_out, float* q_out) {
   B2G_USABLE(h);
   if (!h || !obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
-  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaSetDevice(h->device));
   const size_t E = h->E;
   for (int done_n = 0; done_n < n; done_n += h->B) {
     const int chunk = std::min(h->B, n - done_n);
     CK(cudaMemcpyAsync(h->s_obs, obs + (size_t)done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
-    GatherArgs g = dgather(h, false, false);
+    GatherArgs g = ql_gather(h, false, false);
     g.normc = h->d_normc_act;
     gather_launch(g, h->stream);
     for (auto& gr : h->act) gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
@@ -600,77 +463,22 @@ std::vector<FpField> dqn_fingerprint(const b2g_dqn* h) {
           fp_int("prioritized_replay", c.prioritized_replay), fp_real("per_alpha", c.per_alpha), fp_real("per_eps", c.per_eps)};
 }
 
-// sections 2.. (parameters .. prioritised-replay scalars) of a handle holding `live` replay rows
-std::vector<StateSection> dqn_device_sections(b2g_dqn* h, int64_t live, int64_t lo = 0, int64_t hi = 0) {
-  std::vector<StateSection> s = adam_sections(h->P, 2 * h->n_train, h->Mo, h->Vo, h->n_train);
-  for (auto& r : h->replay.state_sections(live, lo, hi)) s.push_back(std::move(r));
-  return s;
-}
-
 }  // namespace
 
 extern "C" {
 
 int b2g_dqn_state_save(b2g_dqn* h, const char* path) {
-  if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
-  B2G_USABLE(h);
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  long long cnt[8];
-  CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
-  uint32_t eps_bits;
-  memcpy(&eps_bits, &h->eps_value, sizeof eps_bits);
-  std::vector<int64_t> hv = h->replay.state_host(h->n_updates, (int64_t)eps_bits);
-  const FrameRing& ring = h->replay.ring;
-  std::vector<StateSection> secs = host_sections(hv.data(), hv.size() * sizeof(int64_t), cnt, sizeof cnt);
-  for (auto& s : dqn_device_sections(h, h->replay.size, ring.frame_lo(), ring.next_fid)) secs.push_back(std::move(s));
-  return state_write(path, STATE_KIND_DQN, fp_with_frames(dqn_fingerprint(h), ring.frame_cap), secs);
+  return ql_state_save(h, path, STATE_KIND_DQN, h ? dqn_fingerprint(h) : std::vector<FpField>{}, nullptr, nullptr);
 }
 
 int b2g_dqn_state_load(b2g_dqn* h, const char* path) {
-  if (!h || !path) return b2g_fail(B2G_EINVAL, "NULL argument");
-  CK(cudaSetDevice(h->cfg.device));
-  // ---- everything is checked before the handle changes
-  StateReader rd;
-  TransitionReplay& rp = h->replay;
-  if (int rc = state_open_replay(rd, path, STATE_KIND_DQN, dqn_fingerprint(h), rp.ring.frame_cap, false, "")) return rc;
-  if (int rc = state_check_tags(rd, dqn_device_sections(h, 0), "DQN")) return rc;
-  long long cnt[8];
-  if (rd.bytes(1) != sizeof cnt) return b2g_fail(B2G_EINVAL, "training-state section lengths do not match this handle's configuration");
-  std::vector<int64_t> hv;
-  FrameRing ring;
-  if (int rc = rp.state_host_read(rd, &hv, &ring)) return rc;
-  const std::vector<StateSection> dev = dqn_device_sections(h, hv[0], ring.frame_lo(), ring.next_fid);
-  if (int rc = state_check_lengths(rd, dev)) return rc;
-  if (int rc = rd.read_host(1, cnt, sizeof cnt)) return rc;
-  // ---- from here on a failure leaves the handle unusable until a load succeeds
-  CK(cudaStreamSynchronize(h->stream));
-  return state_read_device(rd, dev, &h->broken, [&] {
-    CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
-    rp.ring = ring;
-    rp.size = hv[0]; rp.pos = hv[1]; h->n_updates = hv[2];
-    const uint32_t eps_bits = (uint32_t)hv[3];
-    memcpy(&h->eps_value, &eps_bits, sizeof eps_bits);
-    // the captured step graph stays valid: it holds device pointers and configuration; size and Philox step are device counters
-    return mlog_rebase(&h->mlog, h->counters + 3, h->stream);     // the restored counter: rows before it are not pending
-  });
+  return ql_state_load(h, path, STATE_KIND_DQN, h ? dqn_fingerprint(h) : std::vector<FpField>{}, nullptr, nullptr, "DQN", nullptr);
 }
 
-int b2g_dqn_metrics_log(b2g_dqn* h, int capacity) {
-  B2G_USABLE(h);
-  if (!h || capacity < 0) return b2g_fail(B2G_EINVAL, "bad argument");
-  CK(cudaSetDevice(h->cfg.device));
-  if (int rc = mlog_enable(&h->mlog, capacity, B2G_DQN_LOG_COLS, h->counters + 3, h->stream)) return rc;
-  // the step gains or loses its append node: capture again at the next step
-  if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
-  return 0;
-}
+int b2g_dqn_metrics_log(b2g_dqn* h, int capacity) { return ql_metrics_log(h, capacity, B2G_DQN_LOG_COLS); }
 
 int b2g_dqn_metrics_drain(b2g_dqn* h, float* rows, int max_rows, int64_t* first_step, int* n_rows, int64_t* lost) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  CK(cudaSetDevice(h->cfg.device));
-  return mlog_drain(&h->mlog, h->counters + 3, h->stream, rows, max_rows, first_step, n_rows, lost, [](float* r) {
+  return ql_metrics_drain(h, rows, max_rows, first_step, n_rows, lost, [](float* r) {
     r[3] = sqrtf(r[3]); r[4] = (float)lrintf(r[4]);     // as dfetch
   });
 }

@@ -1,6 +1,7 @@
 // VecNormalize's observation statistics on the device, and the actor side of the learn loop fed from one upload per frame
-// (b2g_sac_observe_act / b2g_sac_observe_add / b2g_obs_rms_set / b2g_obs_rms_get; contracts in include/b200grasp.h).  The BDQ
-// learner's b2g_bdq_observe_* (bdq.cu) merge into its own obs_rms with the same kernel (obs_rms_update_launch, flat layout).
+// (b2g_sac_observe_act / b2g_sac_observe_add / b2g_obs_rms_set / b2g_obs_rms_get; contracts in include/b200grasp.h).  The
+// statistics, their staging and their entry-point bodies are ObsRms (obsnorm.cuh), which the BDQ learner's b2g_bdq_observe_*
+// (bdq.cu) use too, over the flat layout.
 //
 // obs_rms = (mean[E], var[E], count) in float64 over the caller's observation layout, the object [SB2]
 // common/running_mean_std.py keeps on the host.  obs_rms_update_kernel merges the n frames of one call into it with the
@@ -25,6 +26,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "obsnorm.cuh"
 #include "sac_internal.cuh"
 
 namespace b2g {
@@ -78,14 +80,6 @@ __global__ void __launch_bounds__(256) obs_rms_update_kernel(const float* __rest
   }
 }
 
-void update_launch(b2g_sac* h, const float* a, const float* b, const float* done, int n) {
-  // the plain nature_cnn's compact image block is the caller's observation itself: the flat layout
-  const int Cfull = h->direct_feature() ? h->Cobs : 0, npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0;
-  obs_rms_update_launch(a, b, done, n, h->E, h->rms_count, h->norm_eps, h->rms_mean, h->rms_var, h->d_mean, h->d_istd, Cfull, npx,
-                        h->stream);
-  h->rms_count += n;
-}
-
 int ensure_staging(b2g_sac* h) {
   if (h->ob_act) return 0;
   const size_t R = h->stage_rows;
@@ -120,30 +114,6 @@ int check_frames(const b2g_sac* h, const float* frames, const float* only_where,
   return 0;
 }
 
-int upload(b2g_sac* h, void* dst, const void* src, size_t bytes) {
-  CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream));
-  h->up_observe += (int64_t)bytes;
-  return 0;
-}
-
-// the n frames of a call -> ob_full[0]: uploaded as they are or, with an observation encoder, as raw rows it encodes there
-int stage_frames(b2g_sac* h, const float* obs, int n) {
-  if (!h->enc) return upload(h, h->ob_full[0], obs, (size_t)n * h->E * sizeof(float));
-  if (int rc = upload(h, enc_stage_raw(h->enc, 0), obs, (size_t)n * enc_stage_row_floats(h->enc) * sizeof(float))) return rc;
-  return enc_stage_encode(h->enc, 0, nullptr, n, 0, h->ob_full[0], h->stream);
-}
-
-// the reset frames of the n_done finished envs -> row i of ob_full[1]; only those rows cross the bus and, with an observation
-// encoder, only those are encoded (it reads the flags ob_done, uploaded before)
-int stage_reset_frames(b2g_sac* h, const float* reset_obs, const float* done, int n, int n_done) {
-  const size_t rw = h->enc ? enc_stage_row_floats(h->enc) : h->E;
-  float* dst = h->enc ? enc_stage_raw(h->enc, 1) : h->ob_full[1];
-  for (int i = 0; i < n; ++i)
-    if (done[i] != 0.f)
-      if (int rc = upload(h, dst + i * rw, reset_obs + i * rw, rw * sizeof(float))) return rc;
-  return h->enc ? enc_stage_encode(h->enc, 1, h->ob_done, n, n_done, h->ob_full[1], h->stream) : 0;
-}
-
 // caller-layout frames [n][E] -> compact rows [n][Ec]
 int to_rows(b2g_sac* h, const float* full, float* rows, int row0, int n) {
   if (h->cnn) compact_rows(full, rows, row0, (long long)h->stage_rows + h->B, n, h->Hi * h->Wi, h->Cimg, h->Cobs, h->stream);
@@ -155,7 +125,7 @@ int common_checks(b2g_sac* h, int n, int update_stats) {
   if (h->pipe_pending) return b2g_fail(B2G_ESTATE, "a host-pipelined step is in flight: call b2g_sac_pipeline_flush first");
   if (n < 1 || n > h->stage_rows)
     return b2g_fail(B2G_EINVAL, "observe: n must be in [1, " + std::to_string(h->stage_rows) + "] (the staging holds max(batch, 256) frames)");
-  if (update_stats && !h->rms_mean)
+  if (update_stats && !h->rms.on())
     return b2g_fail(B2G_ESTATE, "update_stats needs device statistics: call b2g_obs_rms_set first");
   return 0;
 }
@@ -169,54 +139,73 @@ void obs_rms_update_launch(const float* a, const float* b, const float* done, in
   else obs_rms_update_kernel<false><<<grid, 256, 0, s>>>(a, b, done, n, E, count, eps, mean, var, d_mean, d_istd, Cfull, npx);
 }
 
-void obs_rms_derive(b2g_sac* h) { update_launch(h, nullptr, nullptr, nullptr, 0); }
+void ObsRms::merge(const float* a, const float* b, const float* done, int n, cudaStream_t s) {
+  obs_rms_update_launch(a, b, done, n, E, count, eps, mean, var, d_mean, d_istd, Cfull, npx, s);
+  count += n;
+}
+
+int ObsRms::set(const double* m, const double* v, double c, int device, int nranks, std::vector<void*>& allocs, cudaStream_t s) {
+  if (!(c >= 0.0) || !std::isfinite(c)) return b2g_fail(B2G_EINVAL, "obs_rms_set: count must be finite and >= 0");
+  for (int e = 0; e < E; ++e)
+    if (!std::isfinite(m[e]) || !(v[e] >= 0.0) || !std::isfinite(v[e]))
+      return b2g_fail(B2G_EINVAL, "obs_rms_set: mean must be finite and var finite and >= 0 (element " + std::to_string(e) + ")");
+  if (nranks > 1)
+    return b2g_fail(B2G_ESTATE, "device observation statistics are per handle: with nranks > 1 every rank would own different ones");
+  CK(cudaSetDevice(device));
+  if (!mean) {     // one allocation for both arrays: it either exists or it does not
+    double* mv = nullptr;
+    if (int rc = dev_alloc(allocs, s, &mv, 2 * (size_t)E, false)) return rc;
+    mean = mv;
+    var = mv + E;
+  }
+  CK(cudaMemcpyAsync(mean, m, E * sizeof(double), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(var, v, E * sizeof(double), cudaMemcpyHostToDevice, s));
+  up_observe += (int64_t)(2 * E * sizeof(double));
+  count = c;
+  derive(s);
+  CK(cudaStreamSynchronize(s));     // host arrays are caller-owned: copied before return
+  return 0;
+}
+
+int ObsRms::norm_stats(const double* m, const double* v, double eps_, int device, int nranks, std::vector<void*>& allocs, cudaStream_t s) {
+  const bool eps_changed = eps_ != eps;
+  eps = eps_;
+  if (!on()) return 0;
+  if (m && v) return set(m, v, count, device, nranks, allocs, s);
+  if (eps_changed) derive(s);
+  return 0;
+}
+
+int ObsRms::upload(void* dst, const void* src, size_t bytes, cudaStream_t s) {
+  CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s));
+  up_observe += (int64_t)bytes;
+  return 0;
+}
+
+int ObsRms::stage_frames(float* dst, const float* obs, int n, cudaStream_t s) {
+  if (!enc) return upload(dst, obs, (size_t)n * E * sizeof(float), s);
+  if (int rc = upload(enc_stage_raw(enc, 0), obs, (size_t)n * enc_stage_row_floats(enc) * sizeof(float), s)) return rc;
+  return enc_stage_encode(enc, 0, nullptr, n, 0, dst, s);
+}
+
+int ObsRms::stage_reset_frames(float* dst, const float* reset_obs, const float* done, const float* d_done, int n, int n_done,
+                               cudaStream_t s) {
+  const size_t rw = enc ? enc_stage_row_floats(enc) : E;
+  float* up = enc ? enc_stage_raw(enc, 1) : dst;
+  for (int i = 0; i < n; ++i)
+    if (done[i] != 0.f)
+      if (int rc = upload(up + i * rw, reset_obs + i * rw, rw * sizeof(float), s)) return rc;
+  return enc ? enc_stage_encode(enc, 1, d_done, n, n_done, dst, s) : 0;
+}
 
 }  // namespace b2g
 
 extern "C" {
 
-int b2g_obs_rms_set(b2g_sac* h, const double* mean, const double* var, double count) {
-  B2G_USABLE(h);
-  if (!h || !mean || !var) return b2g_fail(B2G_EINVAL, "NULL argument");
-  if (!(count >= 0.0) || !std::isfinite(count)) return b2g_fail(B2G_EINVAL, "obs_rms_set: count must be finite and >= 0");
-  for (int e = 0; e < h->E; ++e)
-    if (!std::isfinite(mean[e]) || !(var[e] >= 0.0) || !std::isfinite(var[e]))
-      return b2g_fail(B2G_EINVAL, "obs_rms_set: mean must be finite and var finite and >= 0 (element " + std::to_string(e) + ")");
-  if (h->cfg.nranks > 1)
-    return b2g_fail(B2G_ESTATE, "device observation statistics are per handle: with nranks > 1 every rank would own different ones");
-  CK(cudaSetDevice(h->cfg.device));
-  if (!h->rms_mean) {     // one allocation for both arrays: it either exists or it does not
-    double* mv = nullptr;
-    if (int rc = dev_alloc(h->allocs, h->stream, &mv, 2 * (size_t)h->E, false)) return rc;
-    h->rms_mean = mv;
-    h->rms_var = mv + h->E;
-  }
-  CK(cudaMemcpyAsync(h->rms_mean, mean, h->E * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  CK(cudaMemcpyAsync(h->rms_var, var, h->E * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  h->up_observe += (int64_t)(2 * h->E * sizeof(double));
-  h->rms_count = count;
-  obs_rms_derive(h);
-  CK(cudaStreamSynchronize(h->stream));     // host arrays are caller-owned: copied before return
-  return 0;
-}
-
-int b2g_obs_rms_get(b2g_sac* h, double* mean, double* var, double* count) {
-  B2G_USABLE(h);
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  if (!h->rms_mean) return b2g_fail(B2G_ESTATE, "the handle has no device statistics: call b2g_obs_rms_set first");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  if (mean) CK(cudaMemcpy(mean, h->rms_mean, h->E * sizeof(double), cudaMemcpyDeviceToHost));
-  if (var) CK(cudaMemcpy(var, h->rms_var, h->E * sizeof(double), cudaMemcpyDeviceToHost));
-  if (count) *count = h->rms_count;
-  return 0;
-}
-
+int b2g_obs_rms_set(b2g_sac* h, const double* mean, const double* var, double count) { return obs_rms_set(h, mean, var, count); }
+int b2g_obs_rms_get(b2g_sac* h, double* mean, double* var, double* count) { return obs_rms_get(h, mean, var, count); }
 int b2g_upload_bytes(const b2g_sac* h, int64_t* observe_bytes, int64_t* other_bytes) {
-  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  if (observe_bytes) *observe_bytes = h->up_observe;
-  if (other_bytes) *other_bytes = h->up_other;
-  return 0;
+  return obs_rms_upload_bytes(h, observe_bytes, other_bytes);
 }
 
 int b2g_sac_set_obs_encoder(b2g_sac* h, const b2g_encoder* enc, int tail) {
@@ -224,19 +213,10 @@ int b2g_sac_set_obs_encoder(b2g_sac* h, const b2g_encoder* enc, int tail) {
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   if (enc) {
     if (h->cnn) return b2g_fail(B2G_EINVAL, "set_obs_encoder: the CNN policy reads images itself; an encoder feeds the MLP policy");
-    if (int rc = enc_stage_check(enc, h->cfg.device, tail, h->E)) return rc;
-    if (h->cfg.nranks > 1)
-      return b2g_fail(B2G_ESTATE, "set_obs_encoder: the observe path is per handle: with nranks > 1 every rank would encode its own");
+    if (int rc = obs_rms_check_encoder(h, enc, tail)) return rc;
   }
   if (h->pipe_pending) return b2g_fail(B2G_ESTATE, "a host-pipelined step is in flight: call b2g_sac_pipeline_flush first");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  EncStage* st = nullptr;
-  if (enc)
-    if (int rc = enc_stage_create(enc, h->stage_rows, tail, h->stream, &st)) return rc;
-  enc_stage_destroy(h->enc);
-  h->enc = st;
-  h->ob_n = 0;          // staged observations were in the other layout
+  if (int rc = obs_rms_attach_encoder(h, enc, tail)) return rc;
   h->ob_fid.clear();
   return 0;
 }
@@ -253,8 +233,8 @@ int b2g_sac_observe_act(b2g_sac* h, const float* obs, int n, int update_stats, i
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = ensure_staging(h)) return rc;
   if (obs) {
-    if (int rc = stage_frames(h, obs, n)) return rc;
-    if (update_stats) update_launch(h, h->ob_full[0], nullptr, nullptr, n);
+    if (int rc = h->rms.stage_frames(h->ob_full[0], obs, n, h->stream)) return rc;
+    if (update_stats) h->rms.merge(h->ob_full[0], nullptr, nullptr, n, h->stream);
     if (int rc = to_rows(h, h->ob_full[0], h->ob_rows[h->ob_k], 0, n)) return rc;
     h->ob_fid.assign((size_t)n, -1);
     h->ob_n = n;
@@ -289,19 +269,19 @@ int b2g_sac_observe_add(b2g_sac* h, const float* act, const float* rew, const fl
     if (int rc = check_frames(h, reset_obs, done, n)) return rc;
   CK(cudaSetDevice(h->cfg.device));
   const size_t E = h->E, A = h->A;
-  if (int rc = stage_frames(h, next_obs, n)) return rc;
-  if (int rc = upload(h, h->ob_act, act, n * A * sizeof(float))) return rc;
-  if (int rc = upload(h, h->ob_rew, rew, n * sizeof(float))) return rc;
-  if (int rc = upload(h, h->ob_done, done, n * sizeof(float))) return rc;
+  if (int rc = h->rms.stage_frames(h->ob_full[0], next_obs, n, h->stream)) return rc;
+  if (int rc = h->rms.upload(h->ob_act, act, n * A * sizeof(float), h->stream)) return rc;
+  if (int rc = h->rms.upload(h->ob_rew, rew, n * sizeof(float), h->stream)) return rc;
+  if (int rc = h->rms.upload(h->ob_done, done, n * sizeof(float), h->stream)) return rc;
   if (n_done)
-    if (int rc = stage_reset_frames(h, reset_obs, done, n, n_done)) return rc;
+    if (int rc = h->rms.stage_reset_frames(h->ob_full[1], reset_obs, done, h->ob_done, n, n_done, h->stream)) return rc;
   // the transitions: obs = the staged rows (linked to their replay frame where one holds them), next_obs = the new rows
   float* cur = h->ob_rows[h->ob_k];
   float* nxt = h->ob_rows[h->ob_k ^ 1];
   if (int rc = to_rows(h, h->ob_full[0], nxt, 0, n)) return rc;
   std::vector<int64_t> next_fid((size_t)n);
   if (int rc = sac_replay_add_linked(h, cur, nxt, h->ob_fid.data(), h->ob_act, h->ob_rew, h->ob_done, n, next_fid.data())) return rc;
-  if (update_stats) update_launch(h, h->ob_full[0], n_done ? h->ob_full[1] : nullptr, h->ob_done, n);
+  if (update_stats) h->rms.merge(h->ob_full[0], n_done ? h->ob_full[1] : nullptr, h->ob_done, n, h->stream);
   // the new rows become the current observations; a finished env continues from the frame its reset returned
   for (int i = 0; i < n; ++i) {
     h->ob_fid[i] = next_fid[i];

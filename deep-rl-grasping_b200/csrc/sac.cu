@@ -1154,7 +1154,7 @@ int b2g_sac_destroy(b2g_sac* h) {
   for (auto& e : h->ev_aux) if (e) cudaEventDestroy(e);
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   if (h->ev_join) cudaEventDestroy(h->ev_join);
-  enc_stage_destroy(h->enc);
+  enc_stage_destroy(h->rms.enc);
   for (void* q : h->allocs) cudaFree(q);
   for (int q = 0; q < 2; ++q) { if (h->hc_obs[q]) cudaFreeHost(h->hc_obs[q]); if (h->hc_next[q]) cudaFreeHost(h->hc_next[q]); }
   if (h->h_met) cudaFreeHost(h->h_met);
@@ -1280,6 +1280,9 @@ int b2g_sac_create3(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, const 
       cudaMallocHost((void**)&h->h_rc, 2 * sizeof(long long)) != cudaSuccess)
     return bail(b2g_fail(B2G_ECUDA, "replay staging"));
   DA(h->d_mean, h->Ec); DA(h->d_istd, h->Ec); DA(h->d_normc, 8);
+  // obs_rms over the caller's layout; the plain nature_cnn's compact image block is the caller's observation itself: the flat table
+  h->rms.E = h->E; h->rms.Cfull = h->direct_feature() ? h->Cobs : 0; h->rms.npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0;
+  h->rms.d_mean = h->d_mean; h->rms.d_istd = h->d_istd; h->rms.set_call = "b2g_obs_rms_set";
   for (int k = 0; k < 2; ++k) {
     if (cudaMallocHost((void**)&h->hp_stats[k], (size_t)(2 * h->Ec + 8) * sizeof(double)) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->ev_stats[k], cudaEventDisableTiming) != cudaSuccess)
@@ -1500,7 +1503,7 @@ int b2g_replay_add(b2g_sac* h, const float* obs, const float* act, const float* 
     }
     if (int rc = commit_chunk(h, io, m, cand.data(), act + c0 * A, rew + c0, done + c0, next_ids.data() + c0)) return rc;
   }
-  h->up_other += (int64_t)(n * (2 * E + A + 2) * sizeof(float));
+  h->rms.up_other += (int64_t)(n * (2 * E + A + 2) * sizeof(float));
   if (int rc = commit_finish(h, next_ids)) return rc;
   CK(cudaStreamSynchronize(h->stream));     // host arrays are caller-owned: copied before return
   return 0;
@@ -1579,20 +1582,10 @@ int b2g_set_norm_stats(b2g_sac* h, const double* obs_mean, const double* obs_var
                        double eps, int norm_obs, int norm_reward) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  if (norm_obs && !h->rms_mean && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
+  if (norm_obs && !h->rms.on() && (!obs_mean || !obs_var)) return b2g_fail(B2G_EINVAL, "norm_obs needs obs_mean/obs_var");
   CK(cudaSetDevice(h->cfg.device));
-  const bool eps_changed = eps != h->norm_eps;
-  h->norm_eps = eps;
-  if (h->rms_mean) {
-    // the handle owns obs_rms: statistics passed here replace it (count kept), and the table the gather reads is derived on
-    // the device, again when only epsilon changed
-    if (obs_mean && obs_var) {
-      if (int rc = b2g_obs_rms_set(h, obs_mean, obs_var, h->rms_count)) return rc;
-    } else if (eps_changed) {
-      obs_rms_derive(h);
-    }
-    obs_mean = obs_var = nullptr;
-  }
+  if (int rc = h->rms.norm_stats(obs_mean, obs_var, eps, h->cfg.device, h->cfg.nranks, h->allocs, h->stream)) return rc;
+  if (h->rms.on()) obs_mean = obs_var = nullptr;
   // Called once per environment step by the learn loop (VecNormalize statistics move with every observation): the values
   // are staged in one of two pinned buffers and uploaded asynchronously IN STREAM ORDER -- no stream synchronisation, the
   // next gradient step simply sees them.  A buffer is reused only after its previous upload has completed.
@@ -1609,14 +1602,14 @@ int b2g_set_norm_stats(b2g_sac* h, const double* obs_mean, const double* obs_var
     }
     CK(cudaMemcpyAsync(h->d_mean, m, Ec * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_istd, is, Ec * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    h->up_other += (int64_t)(2 * h->E * sizeof(double));
+    h->rms.up_other += (int64_t)(2 * h->E * sizeof(double));
   }
   h->ret_istd = 1.0 / sqrt(ret_var + eps);
   h->clip_obs = clip_obs; h->clip_rew = clip_rew; h->norm_obs = norm_obs; h->norm_rew = norm_reward;
   double* nc = st + 2 * Ec;
   nc[0] = h->ret_istd; nc[1] = clip_obs; nc[2] = clip_rew; nc[3] = (double)norm_obs; nc[4] = (double)norm_reward; nc[5] = nc[6] = nc[7] = 0.0;
   CK(cudaMemcpyAsync(h->d_normc, nc, 8 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  h->up_other += 8 * sizeof(double);
+  h->rms.up_other += 8 * sizeof(double);
   CK(cudaEventRecord(h->ev_stats[k], h->stream));
   return 0;
 }
@@ -1849,7 +1842,7 @@ int b2g_sac_act(b2g_sac* h, const float* obs, int n, int deterministic, float* a
   for (int done_n = 0; done_n < n; done_n += h->B) {
     const int chunk = std::min(h->B, n - done_n);
     if (int rc = load_rows(h, obs + (size_t)done_n * E, h->s_obs, 0, h->B, chunk)) return rc;
-    h->up_other += (int64_t)(chunk * E * sizeof(float));
+    h->rms.up_other += (int64_t)(chunk * E * sizeof(float));
     if (int rc = sac_act_rows(h, h->s_obs, chunk, deterministic)) return rc;
     CK(cudaMemcpyAsync(act_out + (size_t)done_n * A, h->pi_out, chunk * A * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
@@ -1935,7 +1928,7 @@ std::vector<StateSection> sac_device_sections(b2g_sac* h, int64_t lo, int64_t hi
   s[6].tag = state_tag("RREW"); s[6].pieces = {dev_piece(h->r_rew, cap * sizeof(float))};
   s[7].tag = state_tag("RDON"); s[7].pieces = {dev_piece(h->r_done, cap * sizeof(float))};
   s[8].tag = state_tag("FRMS"); s[8].pieces = frame_pieces(h, lo, hi);
-  if (h->rms_mean) s.push_back(rms_section(&h->rms_count, h->rms_mean, h->rms_var, h->E));
+  if (h->rms.on()) s.push_back(rms_section(&h->rms.count, h->rms.mean, h->rms.var, h->E));
   return s;
 }
 
@@ -1959,7 +1952,7 @@ int b2g_sac_state_save(b2g_sac* h, const char* path) {
   std::vector<int64_t> hv = h->pack();     // FrameRing's bookkeeping (its size is r_size)
   std::vector<StateSection> secs = host_sections(hv.data(), hv.size() * sizeof(int64_t), cnt, sizeof cnt);
   for (auto& s : sac_device_sections(h, h->frame_lo(), h->next_fid)) secs.push_back(std::move(s));
-  return state_write(path, STATE_KIND_SAC, fp_with_rms(sac_fingerprint(h, h->extractor), h->rms_mean), secs);
+  return state_write(path, STATE_KIND_SAC, fp_with_rms(sac_fingerprint(h, h->extractor), h->rms.on()), secs);
 }
 
 int b2g_sac_state_load(b2g_sac* h, const char* path) {
@@ -1971,11 +1964,11 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
   CK(cudaSetDevice(h->cfg.device));
   // ---- everything is checked before the handle changes
   StateReader rd;
-  if (int rc = state_open_rms(rd, path, STATE_KIND_SAC, sac_fingerprint(h, h->extractor), h->rms_mean, "b2g_obs_rms_set")) {
+  if (int rc = state_open_rms(rd, path, STATE_KIND_SAC, sac_fingerprint(h, h->extractor), h->rms.on(), h->rms.set_call)) {
     const std::string msg = g_b2g_err;
     StateReader other;      // a file of the other CNN extractor: say so
     const int ext2 = h->extractor == B2G_CNN_NATURE ? B2G_CNN_AUGMENTED : B2G_CNN_NATURE;
-    if (h->cnn && other.open(path, STATE_KIND_SAC, fp_with_rms(sac_fingerprint(h, ext2), h->rms_mean)) == 0)
+    if (h->cnn && other.open(path, STATE_KIND_SAC, fp_with_rms(sac_fingerprint(h, ext2), h->rms.on())) == 0)
       return b2g_fail(B2G_EINVAL, std::string("the state file was written by a handle of the ") +
                                       (ext2 == B2G_CNN_NATURE ? "nature_cnn" : "augmented") + " extractor; this handle runs the " +
                                       (ext2 == B2G_CNN_NATURE ? "augmented" : "nature_cnn") + " one");
@@ -1999,7 +1992,7 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
   CK(cudaStreamSynchronize(h->stream));
   if (h->aux) { CK(cudaStreamSynchronize(h->aux)); CK(cudaStreamSynchronize(h->aux2)); }
   return state_read_device(rd, dev, &h->broken, [&] {
-    if (h->rms_mean) obs_rms_derive(h);
+    if (h->rms.on()) h->rms.derive(h->stream);
     h->ob_n = 0;       // staged observations name frames of the replaced replay: the next b2g_sac_observe_act stages anew
     CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
     static_cast<FrameRing&>(*h) = hs;

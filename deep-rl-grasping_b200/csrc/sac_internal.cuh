@@ -15,6 +15,7 @@
 #include "frame_ring.cuh"
 #include "host.cuh"
 #include "metrics_log.cuh"
+#include "obsnorm.cuh"
 
 namespace b2g {
 struct Tensor {
@@ -100,8 +101,6 @@ int sac_act_rows(b2g_sac* h, const float* rows, int chunk, int deterministic);
 // h_rc are pinned and read by the copies enqueued here).
 int sac_replay_add_linked(b2g_sac* h, const float* c_obs, const float* c_next, const int64_t* obs_fid, const float* act,
                           const float* rew, const float* done, int n, int64_t* next_fid);
-// obsnorm.cu: refreshes d_mean / d_istd from the handle's obs_rms and norm_eps (enqueued on h->stream)
-void obs_rms_derive(b2g_sac* h);
 }  // namespace b2g
 
 using namespace b2g;   // (internal header: only library translation units include it)
@@ -219,12 +218,10 @@ struct b2g_sac : FrameRing {         // FrameRing: the replay's frame and transi
   double* hp_stats[2]{};             // pinned staging of set_norm_stats (asynchronous upload, no stream sync)
   cudaEvent_t ev_stats[2]{};
   int stats_k = 0;
-  double norm_eps = 1e-8;            // VecNormalize.epsilon of the last b2g_set_norm_stats
 
-  // Device-resident VecNormalize observation statistics (obsnorm.cu; created by b2g_obs_rms_set): float64 mean / var over the
-  // caller's observation layout [E].  The count stays on the host: count + n is the same float64 sum there.
-  double *rms_mean = nullptr, *rms_var = nullptr;
-  double rms_count = 0.0;
+  // Device-resident VecNormalize observation statistics (created by b2g_obs_rms_set), their upload counts and the observation
+  // encoder of b2g_sac_set_obs_encoder (MLP policy only: observe_* take raw rows and encode them into ob_full)
+  ObsRms rms;
   // b2g_sac_observe_act / _add staging (allocated on first use): the frames of one call in the caller's layout, the current
   // observation of env i as a compact row, and the replay frame that already holds it (-1: none yet).
   float* ob_full[2]{};               // [stage_rows][E]: 0 = obs / next_obs, 1 = reset_obs
@@ -233,9 +230,6 @@ struct b2g_sac : FrameRing {         // FrameRing: the replay's frame and transi
   float *ob_act = nullptr, *ob_rew = nullptr, *ob_done = nullptr;
   std::vector<int64_t> ob_fid;
   int ob_n = 0;
-  int64_t up_observe = 0, up_other = 0;                   // host->device bytes: observe_* / act + replay_add + set_norm_stats
-  // b2g_sac_set_obs_encoder: observe_* take raw rows and encode them into ob_full (MLP policy only)
-  b2g::EncStage* enc = nullptr;
 
   // CNN extractor (b2g_sac_net_cfg): B2G_CNN_AUGMENTED reads Cimg = obs_c - 1 planes plus the direct feature at column 512 of
   // the feature rows; B2G_CNN_NATURE reads Cimg = obs_c planes and has no direct feature.  Cobs = channels of a caller

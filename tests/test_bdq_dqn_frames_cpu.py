@@ -68,7 +68,7 @@ def test_touched_sources_compile_for_sm90a_without_spills(tmp_path):
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     if not shutil.which(nvcc):
         pytest.skip("nvcc not found")
-    for f in ("per.cu", "bdq.cu", "dqn.cu"):          # (state.cu, also touched, holds no kernels)
+    for f in ("per.cu", "bdq.cu", "dqn.cu"):          # (state.cu and q_learner.cu, also touched, hold no kernels)
         src = os.path.join(ROOT, "deep-rl-grasping_b200", "csrc", f)
         r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
                             "-Xptxas", "-v", "-c", src, "-o", str(tmp_path / (f + ".o"))], capture_output=True, text=True)

@@ -248,3 +248,137 @@ def test_state_layout_and_refusals(case, tmp_path):
     assert_same(saved, bits(R.L.get_parameters()))
     R.step()
     R.L.close()
+
+
+# ---- the replay, normalisation, step and metrics-log entry points of the BDQ and DQN handles (one QLearner base)
+Q_KINDS = ("bdq", "bdq_per", "dqn", "dqn_per")
+
+
+@pytest.fixture(params=Q_KINDS)
+def qcase(request):
+    c = Case(request.param)
+    yield c
+    c.L.close()
+
+
+@pytest.mark.parametrize("frames", [False, True])
+@pytest.mark.parametrize("kind", Q_KINDS)
+def test_replay_info_and_get(kind, frames):
+    c = Case(kind)
+    if frames:      # the same learner over a pool of frames
+        c.L.close()
+        per = c.per
+        if c.kind == "bdq":
+            c.L = BDQLearner(OBS, c.D, c.n, ((c.T0, c.T1), (c.HB,), (c.HB,)), batch_size=B, buffer_size=CAP, prioritized_replay=per,
+                             frame_capacity=CAP + 16)
+        else:
+            c.L = DQNLearner(OBS, c.n, (c.H0, c.H1), batch_size=B, buffer_size=CAP, prioritized_replay=per, frame_capacity=CAP + 16)
+    rows = [c.batch() for _ in range(3)]
+    for r in rows:
+        c.L.replay_add(*r)
+    info = c.L.replay_info()
+    assert info["capacity"] == CAP and info["size"] == 3 * B and info["evicted_early"] == 0 and info["bytes"] > 0
+    if frames:
+        assert info["frame_capacity"] == CAP + 16 and 0 < info["live_frames"] <= CAP + 16
+    else:
+        assert info["frame_capacity"] == 0 and info["live_frames"] == 0
+    for k, (obs, act, rew, nxt, done) in enumerate(rows):
+        for i in range(B):
+            got = c.L.replay_get(k * B + i)
+            assert np.array_equal(got["obs"], obs[i]) and np.array_equal(got["next_obs"], nxt[i])
+            assert np.array_equal(got["act"], np.reshape(act[i], -1))
+            assert got["rew"] == rew[i] and got["done"] == done[i]
+            assert (min(got["frames"]) >= 0) if frames else got["frames"] == (-1, -1)
+    c.L.close()
+
+
+def test_q_refusals(qcase):
+    L = qcase.L
+    with pytest.raises(_lib.B2GError, match="replay buffer is empty") as e:
+        L.step()
+    assert e.value.code == _lib.B2G_ESTATE
+    with pytest.raises(_lib.B2GError, match="norm_obs needs obs_mean/obs_var") as e:
+        _lib.check(qcase.fn("set_norm_stats")(L.h, None, None, 1.0, 10.0, 10.0, 1e-8, 1, 0))
+    assert e.value.code == _lib.B2G_EINVAL
+    with pytest.raises(_lib.B2GError, match="bad argument") as e:
+        L.metrics_log(-1)
+    assert e.value.code == _lib.B2G_EINVAL
+
+
+def test_last_per_after_sampled_step(qcase):
+    qcase.fill(3 * B)
+    qcase.L.step(1)
+    slots, w, p = qcase.L.last_per()
+    assert ((slots >= 0) & (slots < qcase.live)).all()
+    if qcase.per:
+        assert (np.isfinite(w) & (w > 0) & (w <= 1)).all()
+        assert (np.isfinite(p) & (p > 0)).all()
+
+
+@pytest.mark.parametrize("kind", Q_KINDS)
+def test_sampled_step_matches_explicit_step_on_its_slots(kind):
+    """A sampled step at learning rate 0 leaves the weights as they were; the explicit step on the slots it drew (and, with
+    PER, on the importance weights it used) gives the same losses, bit for bit (one warp of samples: the loss sums have one
+    order).  The sampled step's TD is read back only through PER's new priorities, sum_d |td_d| + eps in float32: with PER
+    they must equal those of the explicit step's TD; with uniform replay no TD of a sampled step is readable."""
+    c = Case(kind)
+    c.fill(3 * B)
+    m = c.L.step(1, lr=0.0)
+    slots, w, prio = c.L.last_per()
+    rows = [c.L.replay_get(int(s)) for s in slots]
+    obs = np.stack([r["obs"] for r in rows])
+    nxt = np.stack([r["next_obs"] for r in rows])
+    act = np.stack([r["act"] for r in rows]).reshape((B, c.D) if c.kind == "bdq" else (B,))
+    rew = np.array([r["rew"] for r in rows], np.float32)
+    done = np.array([r["done"] for r in rows], np.float32)
+    e = c.L.step_explicit(obs, act, rew, nxt, done, weights=w if c.per else None, lr=0.0, apply_update=False)
+    keys = ("loss", "mean_q") + (("mean_abs_td",) if c.kind == "dqn" else ())
+    for k in keys:
+        assert np.float32(e[k]) == np.float32(m[k]), (k, e[k], m[k])
+    td = np.asarray(e["td"], np.float32).reshape(B, -1)
+    assert np.isfinite(td).all()
+    if c.per:       # per_write_kernel's order: |td_0| + |td_1| + ... in float32, then + eps
+        want = np.empty(B, np.float32)
+        for i in range(B):
+            s = np.float32(0)
+            for v in td[i]:
+                s = np.float32(s + np.abs(v))
+            want[i] = np.float32(s + np.float32(1e-6))
+        assert np.array_equal(want, prio), (want, prio)
+    c.L.close()
+
+
+def test_bdq_upload_bytes():
+    c = Case("bdq")
+    L, D, E, f, d = c.L, c.D, OBS, 4, 8
+    up = lambda: (L.upload_bytes()["observe"], L.upload_bytes()["other"])
+    assert up() == (0, 0)
+    L.replay_add(*c.batch())
+    other = B * (2 * E + D + 2) * f + 8
+    assert up() == (0, other)
+    L.set_norm_stats(np.zeros(E), np.ones(E))
+    other += 2 * E * d + 8 * d
+    assert up() == (0, other)
+    L.set_norm_stats(norm_obs=False)
+    other += 8 * d
+    assert up() == (0, other)
+    L.act(np.zeros((3, E), np.float32))
+    other += 3 * E * f
+    assert up() == (0, other)
+    L.obs_rms_set(np.zeros(E), np.ones(E), 1.0)
+    observe = 2 * E * d
+    assert up() == (observe, other)
+    L.set_norm_stats(np.zeros(E), np.ones(E))     # replaces the device statistics
+    observe += 2 * E * d
+    other += 8 * d
+    assert up() == (observe, other)
+    n = 5
+    L.observe_act(np.ones((n, E), np.float32), eps=0.5)
+    observe += n * E * f
+    assert up() == (observe, other)
+    done = np.array([0, 1, 0, 1, 0], np.float32)
+    L.observe_add(np.zeros((n, D), np.float32), np.ones(n, np.float32), np.ones((n, E), np.float32), done,
+                  reset_obs=np.zeros((n, E), np.float32))
+    observe += n * E * f + n * D * f + 2 * n * f + 2 * E * f
+    assert up() == (observe, other)
+    L.close()
