@@ -41,6 +41,8 @@ SYMBOLS = [
     "b2g_trpo_state_load",
     "b2g_encoder_create", "b2g_encoder_destroy", "b2g_encoder_n_layers", "b2g_encoder_layer_shape", "b2g_encoder_set_weights",
     "b2g_encoder_encode", "b2g_encoder_create2", "b2g_debug_encoder_layers", "b2g_sac_set_obs_encoder", "b2g_bdq_set_obs_encoder", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor", "b2g_debug_gg_simt", "b2g_debug_gg_tc",
+    "b2g_debug_ppo_tensor_info", "b2g_debug_ppo_tensor", "b2g_debug_trpo_tensor_info", "b2g_debug_trpo_tensor",
+    "b2g_debug_trpo_cg",
     "b2g_autoencoder_create", "b2g_autoencoder_destroy", "b2g_autoencoder_n_layers", "b2g_autoencoder_layer_shape",
     "b2g_autoencoder_set_weights", "b2g_autoencoder_get_weights", "b2g_autoencoder_get_grad", "b2g_autoencoder_reset_optimizer",
     "b2g_autoencoder_set_dataset", "b2g_autoencoder_train_epoch", "b2g_autoencoder_evaluate", "b2g_autoencoder_predict",
@@ -333,6 +335,10 @@ def load():
     lib.b2g_debug_gemm.argtypes = [C.c_int, C.c_int, C.c_int, fp, fp, fp, C.c_int, C.c_int]
     lib.b2g_debug_tensor_info.argtypes = [vp, C.c_char_p, i64p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     lib.b2g_debug_tensor.argtypes = [vp, C.c_char_p, C.c_int, vp, C.c_size_t]
+    for k in ("ppo", "trpo"):
+        getattr(lib, f"b2g_debug_{k}_tensor_info").argtypes = [vp, C.c_char_p, i64p, C.POINTER(C.c_int32)]
+        getattr(lib, f"b2g_debug_{k}_tensor").argtypes = [vp, C.c_char_p, vp, C.c_size_t]
+    lib.b2g_debug_trpo_cg.argtypes = [vp, fp, fp, fp, C.c_int, fp]
     lib.b2g_debug_gg_simt.argtypes = [C.c_int, C.POINTER(GgProblem), C.c_int, fp, C.c_int64, dp, C.c_int64, C.POINTER(C.c_uint16),
                                       C.c_int64, C.POINTER(C.c_int32), C.c_int64]
     lib.b2g_debug_gg_tc.argtypes = [C.c_int, C.POINTER(GgTcProblem), C.c_int, fp, C.c_int64, C.POINTER(C.c_uint16), C.c_int64,

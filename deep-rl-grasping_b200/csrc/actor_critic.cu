@@ -324,6 +324,35 @@ int ac_get_step(ActorCritic* h, int64_t* adam_step, int64_t* noise_step, int32_t
   return 0;
 }
 
+bool ac_debug_base(const ActorCritic* h, int rows, const std::string& name, AcDebugBuf& b) {
+  const int64_t E = h->E, T = h->T, A = h->A, R = rows;
+  const struct { const char* nm; const void* p; int64_t n; int eb; } t[] = {
+      {"P", h->P, h->n_param, 4},          {"G", h->G, h->n_train, 4},           {"Mo", h->Mo, h->n_train, 4},
+      {"Vo", h->Vo, h->n_train, 4},        {"Z0", h->Z0, R * 2 * h->H0, 4},      {"Y0", h->Y0, R * 2 * h->H0, 4},
+      {"Y1", h->Y1, R * 2 * h->H1, 4},     {"r_obs", h->r_obs, (T + 1) * E * h->XS, 4}, {"r_act", h->r_act, (T + 1) * E * A, 4},
+      {"r_val", h->r_val, (T + 1) * E, 4}, {"r_nlp", h->r_nlp, (T + 1) * E, 4},  {"r_rew", h->r_rew, T * E, 4},
+      {"r_done", h->r_done, (T + 1) * E, 4}, {"r_adv", h->r_adv, T * E, 4},      {"r_ret", h->r_ret, T * E, 4},
+      {"lastv", h->lastv, E, 4},           {"a_out", h->a_out, R * A, 4},        {"a_v", h->a_v, R, 4},
+      {"a_nlp", h->a_nlp, R, 4},           {"act_rowoff", h->act_rowoff, E, 4},  {"counters", h->counters, 4, 8}};
+  for (const auto& e : t)
+    if (name == e.nm) { b.p = e.p; b.numel = e.n; b.elem_bytes = e.eb; return true; }
+  return false;
+}
+
+int ac_debug_info(const AcDebugBuf& b, int64_t* numel, int32_t* elem_bytes) {
+  if (numel) *numel = b.numel;
+  if (elem_bytes) *elem_bytes = b.elem_bytes;
+  return 0;
+}
+
+int ac_debug_read(ActorCritic* h, const AcDebugBuf& b, const char* name, void* dst, size_t bytes) {
+  if (bytes != (size_t)b.numel * b.elem_bytes) return b2g_fail(B2G_EINVAL, std::string(name) + ": size mismatch");
+  CK(cudaSetDevice(h->device));
+  CK(cudaStreamSynchronize(h->stream));
+  CK(cudaMemcpy(dst, b.p, bytes, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
 int ac_state_save(ActorCritic* h, const char* path, uint32_t kind, const std::vector<FpField>& fp) {
   CK(cudaSetDevice(h->device));
   CK(cudaStreamSynchronize(h->stream));

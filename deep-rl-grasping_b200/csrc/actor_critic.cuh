@@ -157,6 +157,15 @@ int ac_run_update(ActorCritic* h, const std::function<int()>& issue);
 int ac_predict(ActorCritic* h, const float* obs, int n, int deterministic, float* act_out, float* value_out, float* nlp_out);
 int ac_get_step(ActorCritic* h, int64_t* adam_step, int64_t* noise_step, int32_t* rollout_rows);
 
+// ---- debug read-back (b2g_debug_ppo_tensor / b2g_debug_trpo_tensor): one named device buffer, its element count and size
+struct AcDebugBuf { const void* p = nullptr; int64_t numel = 0; int elem_bytes = 4; };
+// The ActorCritic fields (activations of `rows` rows): P G Mo Vo Z0 Y0 Y1 r_obs r_act r_val r_nlp r_rew r_done r_adv r_ret
+// lastv a_out a_v a_nlp act_rowoff counters.  false for any other name.
+bool ac_debug_base(const ActorCritic* h, int rows, const std::string& name, AcDebugBuf& b);
+// The bodies of the _info and read entry points; find fills b or fails with the unknown name.  The read syncs the handle's stream.
+int ac_debug_info(const AcDebugBuf& b, int64_t* numel, int32_t* elem_bytes);
+int ac_debug_read(ActorCritic* h, const AcDebugBuf& b, const char* name, void* dst, size_t bytes);
+
 // ---- training state (container format in state.cuh): HOST {n_updates, 0}, CNTR the 4 counters, then the parameter arena and
 // the Adam moments.  An update boundary: the rollout in flight is not saved; a load leaves an empty rollout with cleared
 // episode-start flags (the env starts a fresh episode).

@@ -539,3 +539,43 @@ int b2g_ppo_state_load(b2g_ppo* h, const char* path) {
 }
 
 }  // extern "C"
+
+// ================================================================================================
+// Debug read-back of the handle's device buffers (b2g_debug_ppo_tensor; layouts in b200grasp.h)
+// ================================================================================================
+namespace {
+
+int find_ppo_tensor(const b2g_ppo* h, const char* name, AcDebugBuf& b) {
+  if (ac_debug_base(h, h->RMAX, name, b)) return 0;
+  const int64_t R = h->RMAX, A = h->A, np = (int64_t)h->cfg.noptepochs * h->NB;
+  const struct { const char* nm; const void* p; int64_t n; } t[] = {
+      {"sz", h->sz, R * A},       {"sv", h->sv, R},           {"snlp", h->snlp, R},      {"sadv", h->sadv, R},
+      {"sdm", h->sdm, R * A},     {"sdls", h->sdls, R * A},   {"sdv", h->sdv, R},        {"dZ1", h->dZ1, R * 2 * h->H1},
+      {"dZ0", h->dZ0, R * 2 * h->H0}, {"part", h->part, kNormBlocks}, {"met", h->met, 2 * PM_N}, {"hp", h->hp, HP_N},
+      {"rowidx", h->rowidx, np},  {"rowoff", h->rowoff, np},  {"perm", h->perm, np}};
+  for (const auto& e : t)
+    if (!strcmp(name, e.nm)) { b.p = e.p; b.numel = e.n; b.elem_bytes = 4; return 0; }
+  return b2g_fail(B2G_EINVAL, std::string("unknown PPO2 debug tensor: ") + name);
+}
+
+}  // namespace
+
+extern "C" {
+
+int b2g_debug_ppo_tensor_info(const b2g_ppo* h, const char* name, int64_t* numel, int32_t* elem_bytes) {
+  B2G_USABLE(h);
+  if (!h || !name) return b2g_fail(B2G_EINVAL, "NULL argument");
+  AcDebugBuf b;
+  if (int rc = find_ppo_tensor(h, name, b)) return rc;
+  return ac_debug_info(b, numel, elem_bytes);
+}
+
+int b2g_debug_ppo_tensor(b2g_ppo* h, const char* name, void* dst, size_t bytes) {
+  B2G_USABLE(h);
+  if (!h || !name || !dst) return b2g_fail(B2G_EINVAL, "NULL argument");
+  AcDebugBuf b;
+  if (int rc = find_ppo_tensor(h, name, b)) return rc;
+  return ac_debug_read(h, b, name, dst, bytes);
+}
+
+}  // extern "C"

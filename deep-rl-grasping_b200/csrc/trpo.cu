@@ -650,10 +650,9 @@ void fvp_issue(b2g_trpo* h, cudaStream_t s) {
   trpo_fvp_finish_kernel<<<grid_for(h->n_train), 256, 0, s>>>(h->Zv, h->Pv, (int)h->n_train, h->ols, A, h->cfg.cg_damping);
 }
 
-// the policy and value step on rollout rows 0..N-1 (obs, actions, raw advantages r_adv, tdlamret r_ret) and the uploaded
-// permutation
-void core_issue(b2g_trpo* h, cudaStream_t s) {
-  const int N = h->N, H0 = h->H0, H1 = h->H1, A = h->A;
+// oldpi := pi, the policy gradient g at theta_old over rollout rows 0..N-1, and CG's start: x = 0, r = p = g
+void policy_grad_issue(b2g_trpo* h, cudaStream_t s) {
+  const int N = h->N, H1 = h->H1, A = h->A;
   const b2g_trpo_cfg& c = h->cfg;
   // oldpi := pi
   cudaMemcpyAsync(h->P + h->n_total, h->P, (size_t)h->n_total * sizeof(float), cudaMemcpyDeviceToDevice, s);
@@ -673,15 +672,26 @@ void core_issue(b2g_trpo* h, cudaStream_t s) {
   dot_issue(h, h->G, h->G, true, s);
   cg_stage(h, CG_INIT, s);
   vec_issue(h, 0, s);
-  for (int it = 0; it < c.cg_iters; ++it) {
-    fvp_issue(h, s);
-    dot_issue(h, h->Pv, h->Zv, false, s);
-    cg_stage(h, CG_ALPHA, s);
-    vec_issue(h, 1, s);
-    dot_issue(h, h->Rv, h->Rv, false, s);
-    cg_stage(h, CG_BETA, s);
-    vec_issue(h, 2, s);
-  }
+}
+
+// one CG iteration: z = F p, alpha, x += alpha p, r -= alpha z, beta, p = r + beta p
+void cg_iteration_issue(b2g_trpo* h, cudaStream_t s) {
+  fvp_issue(h, s);
+  dot_issue(h, h->Pv, h->Zv, false, s);
+  cg_stage(h, CG_ALPHA, s);
+  vec_issue(h, 1, s);
+  dot_issue(h, h->Rv, h->Rv, false, s);
+  cg_stage(h, CG_BETA, s);
+  vec_issue(h, 2, s);
+}
+
+// the policy and value step on rollout rows 0..N-1 (obs, actions, raw advantages r_adv, tdlamret r_ret) and the uploaded
+// permutation
+void core_issue(b2g_trpo* h, cudaStream_t s) {
+  const int N = h->N, H0 = h->H0, H1 = h->H1, A = h->A;
+  const b2g_trpo_cfg& c = h->cfg;
+  policy_grad_issue(h, s);
+  for (int it = 0; it < c.cg_iters; ++it) cg_iteration_issue(h, s);
   dot_issue(h, h->X, h->X, false, s);
   cg_stage(h, CG_CHECK, s);
   cudaMemcpyAsync(h->Pv, h->X, (size_t)h->n_train * sizeof(float), cudaMemcpyDeviceToDevice, s);
@@ -1031,6 +1041,78 @@ int b2g_trpo_state_load(b2g_trpo* h, const char* path) {
   const int rc = ac_state_load(h, path, STATE_KIND_TRPO, trpo_fingerprint(h), "TRPO");
   if (rc == 0) h->carried = false;
   return rc;
+}
+
+}  // extern "C"
+
+// ================================================================================================
+// Debug read-back of the handle's device buffers (b2g_debug_trpo_tensor; layouts in b200grasp.h)
+// ================================================================================================
+namespace {
+
+int find_trpo_tensor(const b2g_trpo* h, const char* name, AcDebugBuf& b) {
+  if (ac_debug_base(h, h->RMAX, name, b)) return 0;
+  const int64_t N = h->N, NF = h->NF, R = h->RMAX, A = h->A, H0 = h->H0, H1 = h->H1, n = h->n_train, V = kVfBatch;
+  const int64_t np = std::max<int64_t>(1, (int64_t)h->cfg.vf_iters * N);
+  const struct { const char* nm; const void* p; int64_t n; int eb; } t[] = {
+      {"atarg", h->atarg, N, 4},     {"mu_old", h->mu_old, N * A, 4}, {"nlp_old", h->nlp_old, N, 4}, {"sdm", h->sdm, N * A, 4},
+      {"sdls", h->sdls, N * A, 4},   {"u", h->u, NF * A, 4},          {"T0", h->T0, NF * H0, 4},      {"T1", h->T1, NF * H1, 4},
+      {"dZ1", h->dZ1, R * H1, 4},    {"dZ0", h->dZ0, R * H0, 4},      {"X", h->X, n, 4},              {"Rv", h->Rv, n, 4},
+      {"Pv", h->Pv, n, 4},           {"Zv", h->Zv, n, 4},             {"FS", h->FS, n, 4},            {"Gv", h->Gv, n, 4},
+      {"part", h->part, kDotBlocks, 8}, {"amax", h->amax, kDotBlocks, 8}, {"lspart", h->lspart, kNcand * kLsBlocks * 2, 8},
+      {"sc", h->sc, SC_N, 8},        {"met", h->met, TM_N, 4},
+      {"cand", h->cand, kNcand * (H0 + H0 * H1 + H1 + H1 * A + 2 * A), 4},
+      {"Y0c", h->Y0c, kNcand * N * H0, 4}, {"Y1c", h->Y1c, kNcand * N * H1, 4}, {"dZls", h->dZls, N * H0, 4},
+      {"vZ0", h->vZ0, V * H0, 4},    {"vY0", h->vY0, V * H0, 4},      {"vY1", h->vY1, V * H1, 4},     {"vdZ1", h->vdZ1, V * H1, 4},
+      {"vdZ0", h->vdZ0, V * H0, 4},  {"perm", h->perm, np, 4},        {"vrowoff", h->vrowoff, np, 4}};
+  for (const auto& e : t)
+    if (!strcmp(name, e.nm)) { b.p = e.p; b.numel = e.n; b.elem_bytes = e.eb; return 0; }
+  return b2g_fail(B2G_EINVAL, std::string("unknown TRPO debug tensor: ") + name);
+}
+
+}  // namespace
+
+extern "C" {
+
+int b2g_debug_trpo_tensor_info(const b2g_trpo* h, const char* name, int64_t* numel, int32_t* elem_bytes) {
+  B2G_USABLE(h);
+  if (!h || !name) return b2g_fail(B2G_EINVAL, "NULL argument");
+  AcDebugBuf b;
+  if (int rc = find_trpo_tensor(h, name, b)) return rc;
+  return ac_debug_info(b, numel, elem_bytes);
+}
+
+int b2g_debug_trpo_cg(b2g_trpo* h, const float* obs, const float* actions, const float* adv, int iters, float* prev) {
+  B2G_USABLE(h);
+  if (!h || !obs || !actions || !adv || !prev) return b2g_fail(B2G_EINVAL, "NULL argument");
+  if (iters < 1 || iters > 64) return b2g_fail(B2G_EINVAL, "iters must be in [1, 64]");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  cudaStream_t s = h->stream;
+  const size_t N = h->N, n = (size_t)h->n_train;
+  if (int rc = ac_upload_rows(h, h->r_obs, obs, h->N)) return rc;
+  CK(cudaMemcpyAsync(h->r_act, actions, N * h->A * sizeof(float), cudaMemcpyDefault, s));
+  CK(cudaMemcpyAsync(h->r_adv, adv, N * sizeof(float), cudaMemcpyDefault, s));
+  policy_grad_issue(h, s);
+  for (int it = 0; it + 1 < iters; ++it) cg_iteration_issue(h, s);
+  CK(cudaMemcpyAsync(prev, h->X, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(prev + n, h->Rv, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(prev + 2 * n, h->Pv, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(prev + 3 * n, h->sc, SC_N * sizeof(double), cudaMemcpyDeviceToHost, s));
+  cg_iteration_issue(h, s);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(s));
+  h->t = 0;
+  h->carried = false;
+  return 0;
+}
+
+int b2g_debug_trpo_tensor(b2g_trpo* h, const char* name, void* dst, size_t bytes) {
+  B2G_USABLE(h);
+  if (!h || !name || !dst) return b2g_fail(B2G_EINVAL, "NULL argument");
+  AcDebugBuf b;
+  if (int rc = find_trpo_tensor(h, name, b)) return rc;
+  return ac_debug_read(h, b, name, dst, bytes);
 }
 
 }  // extern "C"

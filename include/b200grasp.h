@@ -820,6 +820,36 @@ int b2g_debug_gg_tc(int x3, const b2g_debug_gg_tc_problem* p, int n, float* f32,
 int b2g_debug_tensor_info(const b2g_sac* h, const char* name, int64_t* numel, int32_t* planes, int32_t* elem_bytes);
 int b2g_debug_tensor(b2g_sac* h, const char* name, int plane, void* dst, size_t bytes);
 
+/* One named device buffer of a PPO2 / TRPO handle back to the host, after syncing the handle's stream, so that tests can hold
+ * each actor-critic kernel to float64 of the inputs it read.  _info gives the element count and size (4: fp32, or int32 for
+ * the row tables; 8: the int64 counters, and float64 for TRPO's part, amax, lspart and sc); bytes must be numel * elem_bytes.
+ * B2G_EINVAL for an unknown name or a size mismatch.  The buffers hold what the LAST call left.  R = activation rows (PPO2:
+ * max(minibatch, max(64, n_envs)); TRPO: max(N + 1, 64)), E = n_envs (TRPO 1), T = n_steps (TRPO N), XS = obs_dim rounded up
+ * to 4, n_train / n_param = floats of the trained block / of the arena, D, A, H0, H1 as configured.
+ * Both handles:
+ *   P [n_param], G Mo Vo [n_train]     parameter arena (actor_critic.cuh order), gradient arena and Adam moments
+ *   Z0 Y0 [R][2 H0], Y1 [R][2 H1]       layer-0 pre-activations (no bias) and both layers' tanh outputs: pi | vf columns
+ *   r_obs [T + 1][E][XS], r_act [T + 1][E][A], r_val r_nlp r_done [T + 1][E], r_rew r_adv r_ret [T][E], lastv [E]
+ *   a_out [R][A], a_v a_nlp [R]         the actor's predict outputs; act_rowoff int32 [E]; counters int64 [4]
+ * PPO2 (M = minibatch, NP = noptepochs * n_batch):
+ *   sz sdm sdls [R][A], sv snlp sadv sdv [R], dZ1 [R][2 H1], dZ0 [R][2 H0]   the tail's scratch and outputs
+ *   part [128] (norm partials), met [16], hp [4], rowidx rowoff perm int32 [NP]
+ * TRPO (NF = ceil(N / 5), V = 128, K = 10 line-search candidates):
+ *   atarg nlp_old [N], mu_old sdm sdls [N][A], u [NF][A], T0 [NF][H0], T1 [NF][H1], dZ1 [R][H1], dZ0 [R][H0]
+ *   X Rv Pv Zv FS Gv [n_train]          CG vectors, the full step and the value gradient, in the arena layout
+ *   part amax [128], lspart [K][64][2], sc [16] (float64), met [16]
+ *   cand [K][H0 + H0 H1 + H1 + H1 A + 2 A] (b0, W1, b1, pi/w, pi/b, logstd blocks of all K, block after block)
+ *   Y0c [K][N][H0], Y1c [K][N][H1], dZls [N][H0], vZ0 vY0 vdZ0 [V][H0], vY1 vdZ1 [V][H1], perm vrowoff int32 [max(1, vf_iters N)] */
+int b2g_debug_ppo_tensor_info(const b2g_ppo* h, const char* name, int64_t* numel, int32_t* elem_bytes);
+int b2g_debug_ppo_tensor(b2g_ppo* h, const char* name, void* dst, size_t bytes);
+int b2g_debug_trpo_tensor_info(const b2g_trpo* h, const char* name, int64_t* numel, int32_t* elem_bytes);
+int b2g_debug_trpo_tensor(b2g_trpo* h, const char* name, void* dst, size_t bytes);
+/* The policy gradient of b2g_trpo_step_explicit on obs [N, obs_dim], actions [N, n_actions] and raw advantages [N], then
+ * `iters` (1..64) conjugate-gradient iterations and nothing after them.  prev [3 n_train + 2 * SC_N(16)] receives x, r and p
+ * (arena layout) and the 16 float64 CG scalars as they stood before the last iteration; the debug tensors then hold that
+ * iteration's z = F p_prev (Zv), x, r, p after its p update (X, Rv, Pv) and scalars (sc). */
+int b2g_debug_trpo_cg(b2g_trpo* h, const float* obs, const float* actions, const float* adv, int iters, float* prev);
+
 #ifdef __cplusplus
 }
 #endif
