@@ -39,6 +39,9 @@ SYMBOLS = [
     "b2g_trpo_get_grad", "b2g_trpo_rollout_act", "b2g_trpo_rollout_reward", "b2g_trpo_rollout_reset", "b2g_trpo_rollout_get",
     "b2g_trpo_update", "b2g_trpo_fvp", "b2g_trpo_step_explicit", "b2g_trpo_act", "b2g_trpo_get_step", "b2g_trpo_state_save",
     "b2g_trpo_state_load",
+    "b2g_ppo_obs_rms_set", "b2g_ppo_obs_rms_get", "b2g_ppo_upload_bytes", "b2g_ppo_set_norm_stats", "b2g_ppo_set_obs_encoder",
+    "b2g_ppo_observe_act", "b2g_ppo_act_raw", "b2g_trpo_obs_rms_set", "b2g_trpo_obs_rms_get", "b2g_trpo_upload_bytes",
+    "b2g_trpo_set_norm_stats", "b2g_trpo_set_obs_encoder", "b2g_trpo_observe_act", "b2g_trpo_act_raw",
     "b2g_encoder_create", "b2g_encoder_destroy", "b2g_encoder_n_layers", "b2g_encoder_layer_shape", "b2g_encoder_set_weights",
     "b2g_encoder_encode", "b2g_encoder_create2", "b2g_debug_encoder_layers", "b2g_sac_set_obs_encoder", "b2g_bdq_set_obs_encoder", "b2g_debug_gemm", "b2g_debug_tensor_info", "b2g_debug_tensor", "b2g_debug_gg_simt", "b2g_debug_gg_tc",
     "b2g_debug_ppo_tensor_info", "b2g_debug_ppo_tensor", "b2g_debug_trpo_tensor_info", "b2g_debug_trpo_tensor",
@@ -310,6 +313,15 @@ def load():
     lib.b2g_trpo_step_explicit.argtypes = [vp, fp, fp, fp, fp, C.POINTER(C.c_int32), C.POINTER(TrpoMetrics), fp, fp, fp]
     lib.b2g_trpo_act.argtypes = [vp, fp, C.c_int, C.c_int, fp, fp]
     lib.b2g_trpo_get_step.argtypes = [vp, i64p, i64p, C.POINTER(C.c_int32)]
+    for p in ("ppo", "trpo"):                # VecNormalize's obs_rms on the device and the observe path of the two
+        getattr(lib, f"b2g_{p}_obs_rms_set").argtypes = [vp, dp, dp, C.c_double]
+        getattr(lib, f"b2g_{p}_obs_rms_get").argtypes = [vp, dp, dp, dp]
+        getattr(lib, f"b2g_{p}_upload_bytes").argtypes = [vp, i64p, i64p]
+        getattr(lib, f"b2g_{p}_set_norm_stats").argtypes = [vp, C.c_double, C.c_double, C.c_int]
+        getattr(lib, f"b2g_{p}_set_obs_encoder").argtypes = [vp, vp, C.c_int]
+        getattr(lib, f"b2g_{p}_observe_act").argtypes = [vp, fp, C.c_int, C.c_int, fp]
+    lib.b2g_ppo_act_raw.argtypes = [vp, fp, C.c_int, C.c_int, fp, fp, fp]
+    lib.b2g_trpo_act_raw.argtypes = [vp, fp, C.c_int, C.c_int, fp, fp]
     lib.b2g_encoder_create.argtypes = [C.POINTER(EncoderCfg), C.POINTER(vp)]
     lib.b2g_encoder_destroy.argtypes = [vp]
     lib.b2g_encoder_n_layers.argtypes = [vp]

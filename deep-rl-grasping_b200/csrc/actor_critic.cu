@@ -4,6 +4,8 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <cmath>
+#include <string>
 
 #include "actor_critic.cuh"
 
@@ -92,6 +94,29 @@ __global__ void ac_iota_rows_kernel(int* __restrict__ rowoff, int first, int n, 
   if (i < n) rowoff[i] = (first + i) * XS;
 }
 
+// VecNormalize.normalize_obs of n rows [n][D] into rows of stride XS, one thread per destination element: the float64
+// subtract, sqrt, divide and clip in numpy's order, then one rounding to fp32 (NaN passes the clip as np.clip passes it).
+// mean == nullptr copies.  The pad columns [D, XS) are written 0.
+__global__ void __launch_bounds__(256) ac_obs_norm_kernel(const float* __restrict__ x, int n, int D, int XS,
+                                                          const double* __restrict__ mean, const double* __restrict__ var,
+                                                          double eps, double clip, float* __restrict__ dst) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)n * XS) return;
+  const int r = (int)(i / XS), j = (int)(i - (long long)r * XS);
+  float out = 0.f;
+  if (j < D) {
+    const float v = x[(size_t)r * D + j];
+    if (mean) {
+      double y = __ddiv_rn(__dsub_rn((double)v, mean[j]), __dsqrt_rn(__dadd_rn(var[j], eps)));
+      y = y < -clip ? -clip : (y > clip ? clip : y);
+      out = __double2float_rn(y);
+    } else {
+      out = v;
+    }
+  }
+  dst[i] = out;
+}
+
 }  // namespace
 
 int ac_check_net(int obs_dim, int n_actions, int hidden0, int hidden1) {
@@ -107,6 +132,9 @@ int ac_init(ActorCritic* h, int device, int D, int A, int H0, int H1, int E, int
   h->D = D; h->XS = (int)ac_row_stride(D); h->A = A; h->H0 = H0; h->H1 = H1;
   h->E = E; h->T = T; h->P_ROWS = p_rows;
   h->act_key = seed ^ 0xA5A5A5A5DEADBEEFull;       // oracle/philox_ref.py act_seed
+  h->cfg.device = device;
+  h->stage_rows = E;
+  h->rms.E = D;
   const char* ng = getenv("B2G_NO_GRAPH");
   h->use_graph = !(ng && ng[0] == '1');
   if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return b2g_fail(B2G_ECUDA, "stream");
@@ -172,6 +200,7 @@ void ac_release(ActorCritic* h) {
   cudaSetDevice(h->device);
   if (h->stream) cudaStreamSynchronize(h->stream);
   if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
+  enc_stage_destroy(h->rms.enc);
   for (void* q : h->allocs) cudaFree(q);
   if (h->h_buf) cudaFreeHost(h->h_buf);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -240,10 +269,11 @@ int ac_upload_rows(ActorCritic* h, float* dst, const float* src, int rows) {
   return 0;
 }
 
-int ac_rollout_act(ActorCritic* h, const float* obs, float* act_out) {
-  CK(cudaSetDevice(h->device));
+namespace {
+
+// the forward pass and the stream-1 draw of rollout row t (its observations in place) -> act_out, enqueued
+int act_row(ActorCritic* h, float* act_out) {
   cudaStream_t s = h->stream;
-  if (int rc = ac_upload_rows(h, h->r_obs + (size_t)h->t * h->E * h->XS, obs, h->E)) return rc;
   ac_iota_rows_kernel<<<(h->E + 255) / 256, 256, 0, s>>>(h->act_rowoff, h->t * h->E, h->E, h->XS);
   ac_fwd_issue(h, h->f_act, s);
   AcActArgs a = ac_act_args(h, h->E, 0);
@@ -251,7 +281,23 @@ int ac_rollout_act(ActorCritic* h, const float* obs, float* act_out) {
   ac_act(a, s);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(act_out, h->a_out, (size_t)h->E * h->A * sizeof(float), cudaMemcpyDefault, s));
-  CK(cudaStreamSynchronize(s));
+  h->acted = true;
+  return 0;
+}
+
+int ensure_stage(ActorCritic* h) {
+  if (h->ob_stage) return 0;
+  return dev_alloc(h->allocs, h->stream, &h->ob_stage, (size_t)std::max(h->E, h->P_ROWS) * h->D);
+}
+
+}  // namespace
+
+int ac_rollout_act(ActorCritic* h, const float* obs, float* act_out) {
+  CK(cudaSetDevice(h->device));
+  if (int rc = ac_upload_rows(h, h->r_obs + (size_t)h->t * h->E * h->XS, obs, h->E)) return rc;
+  h->ob_n = 0;
+  if (int rc = act_row(h, act_out)) return rc;
+  CK(cudaStreamSynchronize(h->stream));
   return 0;
 }
 
@@ -262,6 +308,7 @@ int ac_rollout_reward(ActorCritic* h, const float* rew, const float* done) {
   CK(cudaMemcpyAsync(h->r_done + (size_t)(h->t + 1) * E, done, E * sizeof(float), cudaMemcpyDefault, h->stream));
   CK(cudaStreamSynchronize(h->stream));      // rew and done may live on the caller's stack
   h->t += 1;
+  h->acted = false;
   return 0;
 }
 
@@ -270,6 +317,109 @@ int ac_rollout_reset(ActorCritic* h) {
   CK(cudaMemsetAsync(h->r_done, 0, (size_t)h->E * sizeof(float), h->stream));
   CK(cudaStreamSynchronize(h->stream));
   h->t = 0;
+  h->acted = false;
+  h->ob_n = 0;
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// obs_rms on the device and the observe path
+// ---------------------------------------------------------------------------------------------------------------------------
+void ac_obs_normalize(const ActorCritic* h, const float* x, int n, float* dst, cudaStream_t s) {
+  const bool norm = h->rms.on() && h->norm_obs;
+  const long long total = (long long)n * h->XS;
+  ac_obs_norm_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(x, n, h->D, h->XS, norm ? h->rms.mean : nullptr,
+                                                                     norm ? h->rms.var : nullptr, h->rms.eps, h->clip_obs, dst);
+}
+
+int ac_obs_rms_set(ActorCritic* h, const double* mean, const double* var, double count) {
+  if (h && !h->rms_tab) {      // ObsRms::merge rewrites a table as it merges; allocated with obs_rms
+    CK(cudaSetDevice(h->device));
+    if (int rc = dev_alloc(h->allocs, h->stream, &h->rms_tab, 2 * (size_t)h->D)) return rc;
+    h->rms.d_mean = h->rms_tab;
+    h->rms.d_istd = h->rms_tab + h->D;
+  }
+  return obs_rms_set(h, mean, var, count);
+}
+
+int ac_obs_rms_get(ActorCritic* h, double* mean, double* var, double* count) { return obs_rms_get(h, mean, var, count); }
+
+int ac_upload_bytes(const ActorCritic* h, int64_t* observe_bytes, int64_t* other_bytes) {
+  return obs_rms_upload_bytes(h, observe_bytes, other_bytes);
+}
+
+int ac_set_norm_stats(ActorCritic* h, double clip_obs, double eps, int norm_obs) {
+  if (!(clip_obs >= 0.0) || !std::isfinite(clip_obs) || !(eps >= 0.0) || !std::isfinite(eps))
+    return b2g_fail(B2G_EINVAL, "set_norm_stats: clip_obs and epsilon must be finite and >= 0");
+  CK(cudaSetDevice(h->device));
+  if (int rc = h->rms.norm_stats(nullptr, nullptr, eps, h->cfg.device, h->cfg.nranks, h->allocs, h->stream)) return rc;
+  h->clip_obs = clip_obs;      // a kernel argument: observe calls enqueued later read the new value
+  h->norm_obs = norm_obs != 0;
+  return 0;
+}
+
+int ac_set_obs_encoder(ActorCritic* h, const b2g_encoder* enc, int tail) {
+  if (enc)
+    if (int rc = obs_rms_check_encoder(h, enc, tail)) return rc;
+  return obs_rms_attach_encoder(h, enc, tail);
+}
+
+int ac_observe_act(ActorCritic* h, const float* obs, int n, int update_stats, float* act_out, bool carried) {
+  if (!obs && !act_out) return b2g_fail(B2G_EINVAL, "observe_act: nothing to do (obs and act_out are NULL)");
+  if (n != h->E) return b2g_fail(B2G_EINVAL, "observe_act: n must be the handle's n_envs (" + std::to_string(h->E) + ")");
+  if (obs && update_stats && !h->rms.on())
+    return b2g_fail(B2G_ESTATE, std::string("update_stats needs device statistics: call ") + h->rms.set_call + " first");
+  const int row = h->t + (h->acted ? 1 : 0);     // the row an observation staged now belongs to
+  if (act_out) {
+    if (h->t >= h->T) return b2g_fail(B2G_ESTATE, "observe_act: the rollout is full: update first");
+    if (h->acted) return b2g_fail(B2G_ESTATE, "observe_act: row t's action is drawn: pass its rewards (rollout_reward) first");
+    if (!obs && !(h->ob_n && h->ob_row == h->t))
+      return b2g_fail(B2G_ESTATE, "observe_act: no observation staged in the current row (pass obs first)");
+  } else if (row > h->T) {
+    return b2g_fail(B2G_ESTATE, "observe_act: the rollout is full: update first");
+  }
+  CK(cudaSetDevice(h->device));
+  cudaStream_t s = h->stream;
+  if (obs) {
+    if (int rc = ensure_stage(h)) return rc;
+    if (int rc = h->rms.stage_frames(h->ob_stage, obs, n, s)) return rc;
+    if (update_stats) h->rms.merge(h->ob_stage, nullptr, nullptr, n, s);
+    ac_obs_normalize(h, h->ob_stage, n, h->r_obs + (size_t)row * h->E * h->XS, s);
+    h->ob_n = n;
+    h->ob_row = row;
+  }
+  if (act_out) {
+    if (carried && h->t == 0) {      // the action drawn for this row before the last update
+      CK(cudaMemcpyAsync(act_out, h->r_act, (size_t)h->E * h->A * sizeof(float), cudaMemcpyDefault, s));
+      h->acted = true;
+    } else if (int rc = act_row(h, act_out)) {
+      return rc;
+    }
+  }
+  CK(cudaStreamSynchronize(s));      // caller-owned arrays are copied, the actions are the result of the call
+  CK(cudaGetLastError());
+  return 0;
+}
+
+int ac_check_last_obs(const ActorCritic* h, const float* last_obs) {
+  if (last_obs || (h->ob_n && h->ob_row == h->T)) return 0;
+  return b2g_fail(B2G_EINVAL, "update: last_obs is NULL and no observation is staged in the bootstrap row (observe_act after the "
+                              "last step)");
+}
+
+int ac_update_last_obs(ActorCritic* h, const float* last_obs) {
+  if (!last_obs) return 0;
+  h->ob_n = 0;
+  return ac_upload_rows(h, h->r_obs + (size_t)h->T * h->E * h->XS, last_obs, h->E);
+}
+
+int ac_update_finish(ActorCritic* h, const float* last_obs, bool copy_row0) {
+  h->acted = false;
+  if (last_obs) return 0;
+  if (copy_row0)
+    CK(cudaMemcpyAsync(h->r_obs, h->r_obs + (size_t)h->T * h->E * h->XS, (size_t)h->E * h->XS * sizeof(float), cudaMemcpyDeviceToDevice,
+                       h->stream));
+  h->ob_row = 0;
   return 0;
 }
 
@@ -293,13 +443,22 @@ int ac_run_update(ActorCritic* h, const std::function<int()>& issue) {
   return 0;
 }
 
-int ac_predict(ActorCritic* h, const float* obs, int n, int deterministic, float* act_out, float* value_out, float* nlp_out) {
+int ac_predict(ActorCritic* h, const float* obs, int n, int deterministic, float* act_out, float* value_out, float* nlp_out, bool raw) {
   CK(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
   const int P = h->P_ROWS;
+  if (raw)
+    if (int rc = ensure_stage(h)) return rc;
   for (int done_n = 0; done_n < n; done_n += P) {
     const int chunk = std::min(P, n - done_n);
-    if (int rc = ac_upload_rows(h, h->p_obs, obs + (size_t)done_n * h->D, chunk)) return rc;
+    if (raw) {
+      const size_t bytes = (size_t)chunk * h->D * sizeof(float);
+      CK(cudaMemcpyAsync(h->ob_stage, obs + (size_t)done_n * h->D, bytes, cudaMemcpyDefault, s));
+      h->rms.up_other += (int64_t)bytes;
+      ac_obs_normalize(h, h->ob_stage, chunk, h->p_obs, s);
+    } else if (int rc = ac_upload_rows(h, h->p_obs, obs + (size_t)done_n * h->D, chunk)) {
+      return rc;
+    }
     ac_fwd_issue(h, h->f_pred, s);
     AcActArgs a = ac_act_args(h, chunk, 2);
     a.deterministic = deterministic;
@@ -353,6 +512,15 @@ int ac_debug_read(ActorCritic* h, const AcDebugBuf& b, const char* name, void* d
   return 0;
 }
 
+namespace {
+// sections 2..: the parameter arena and the Adam moments, then obs_rms when the handle owns it
+std::vector<StateSection> ac_device_sections(ActorCritic* h) {
+  std::vector<StateSection> s = adam_sections(h->P, h->n_param, h->Mo, h->Vo, h->n_train);
+  if (h->rms.on()) s.push_back(rms_section(&h->rms.count, h->rms.mean, h->rms.var, h->D));
+  return s;
+}
+}  // namespace
+
 int ac_state_save(ActorCritic* h, const char* path, uint32_t kind, const std::vector<FpField>& fp) {
   CK(cudaSetDevice(h->device));
   CK(cudaStreamSynchronize(h->stream));
@@ -360,15 +528,15 @@ int ac_state_save(ActorCritic* h, const char* path, uint32_t kind, const std::ve
   CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
   int64_t hv[2] = {h->n_updates, 0};
   std::vector<StateSection> secs = host_sections(hv, sizeof hv, cnt, sizeof cnt);
-  for (auto& s : adam_sections(h->P, h->n_param, h->Mo, h->Vo, h->n_train)) secs.push_back(std::move(s));
-  return state_write(path, kind, fp, secs);
+  for (auto& s : ac_device_sections(h)) secs.push_back(std::move(s));
+  return state_write(path, kind, fp_with_rms(fp, h->rms.on()), secs);
 }
 
 int ac_state_load(ActorCritic* h, const char* path, uint32_t kind, const std::vector<FpField>& fp, const char* learner) {
   CK(cudaSetDevice(h->device));
   StateReader rd;
-  if (int rc = rd.open(path, kind, fp)) return rc;
-  const std::vector<StateSection> dev = adam_sections(h->P, h->n_param, h->Mo, h->Vo, h->n_train);
+  if (int rc = state_open_rms(rd, path, kind, fp, h->rms.on(), h->rms.set_call)) return rc;
+  const std::vector<StateSection> dev = ac_device_sections(h);
   if (int rc = state_check_tags(rd, dev, learner)) return rc;
   int64_t hv[2];
   long long cnt[4];
@@ -381,8 +549,14 @@ int ac_state_load(ActorCritic* h, const char* path, uint32_t kind, const std::ve
   return state_read_device(rd, dev, &h->broken, [&] {
     CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
     CK(cudaMemset(h->r_done, 0, (size_t)h->E * sizeof(float)));
+    if (h->rms.on()) {      // the table ObsRms keeps beside obs_rms
+      h->rms.derive(h->stream);
+      CK(cudaStreamSynchronize(h->stream));
+    }
     h->n_updates = hv[0];
     h->t = 0;
+    h->acted = false;
+    h->ob_n = 0;
     return 0;
   });
 }

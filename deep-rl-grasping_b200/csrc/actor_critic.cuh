@@ -17,6 +17,7 @@
 
 #include "common.cuh"
 #include "host.cuh"
+#include "obsnorm.cuh"
 #include "state.cuh"
 
 namespace b2g {
@@ -112,6 +113,18 @@ struct ActorCritic {
   bool use_graph = true;
   bool broken = false;
   long long n_updates = 0;
+  bool acted = false;                 // row t's action is drawn: an observation staged now belongs to row t + 1
+  // VecNormalize's obs_rms on the device (ObsRms, obsnorm.cuh) and the observe path that normalises each frame once into the
+  // rollout.  The obsnorm.cuh templates are instantiated on ActorCritic and read cfg, allocs, stream, stage_rows and ob_n (a
+  // handle's own cfg hides this one).
+  ObsRms rms;
+  struct { int device = 0, nranks = 1; } cfg;
+  double clip_obs = 10.0;             // VecNormalize.clip_obs of the last set_norm_stats
+  bool norm_obs = true;               // VecNormalize.norm_obs: false copies the rows as they are
+  int stage_rows = 0;                 // E: the rows of an observe call (and of the encoder stage)
+  int ob_n = 0, ob_row = -1;          // ob_n observations staged (0 or E), normalised into rollout row ob_row
+  float* ob_stage = nullptr;          // [max(E, P_ROWS)][D] frames as uploaded or encoded, before the normalisation
+  double* rms_tab = nullptr;          // [2][D]: the d_mean / d_istd table ObsRms::merge rewrites (nothing here reads it)
 };
 
 // The configuration checks both handles make first: obs_dim, n_actions and the hidden widths.
@@ -153,9 +166,31 @@ int ac_rollout_reset(ActorCritic* h);
 int ac_rollout_get(ActorCritic* h, float* adv, float* ret, float* val, float* nlp, float* act);   // nulls are skipped
 // issue() through the update graph (captured on the first call) or directly under B2G_NO_GRAPH=1
 int ac_run_update(ActorCritic* h, const std::function<int()>& issue);
-// in chunks of P_ROWS rows; value_out and nlp_out may be null
-int ac_predict(ActorCritic* h, const float* obs, int n, int deterministic, float* act_out, float* value_out, float* nlp_out);
+// in chunks of P_ROWS rows; value_out and nlp_out may be null.  raw: the rows are normalised with the current obs_rms first
+// (nothing is merged)
+int ac_predict(ActorCritic* h, const float* obs, int n, int deterministic, float* act_out, float* value_out, float* nlp_out,
+               bool raw = false);
 int ac_get_step(ActorCritic* h, int64_t* adam_step, int64_t* noise_step, int32_t* rollout_rows);
+
+// ---- VecNormalize's obs_rms on the device and the observe path (b2g_ppo_* / b2g_trpo_* forward to these)
+// n rows [n][D] at x -> rows of stride XS at dst: float(clip((double(x) - mean) / sqrt(var + eps), -clip_obs, clip_obs)) in
+// float64, numpy's order, rounded once; a copy without obs_rms or with norm_obs off; the pad columns [D, XS) are zero
+void ac_obs_normalize(const ActorCritic* h, const float* x, int n, float* dst, cudaStream_t s);
+int ac_obs_rms_set(ActorCritic* h, const double* mean, const double* var, double count);
+int ac_obs_rms_get(ActorCritic* h, double* mean, double* var, double* count);
+int ac_upload_bytes(const ActorCritic* h, int64_t* observe_bytes, int64_t* other_bytes);
+int ac_set_norm_stats(ActorCritic* h, double clip_obs, double eps, int norm_obs);
+int ac_set_obs_encoder(ActorCritic* h, const b2g_encoder* enc, int tail);
+// obs: n = E raw frames uploaded once, merged when update_stats, normalised into the current row (t, or t + 1 once row t's
+// action is drawn); act_out: the rollout step on row t.  carried: row 0 holds an action drawn before the last update (TRPO's
+// boundary), returned without a draw.  One stream synchronise.
+int ac_observe_act(ActorCritic* h, const float* obs, int n, int update_stats, float* act_out, bool carried);
+// update's last_obs: uploaded into row T, or NULL: the row observe_act staged there (the check: B2G_EINVAL without one)
+int ac_check_last_obs(const ActorCritic* h, const float* last_obs);
+int ac_update_last_obs(ActorCritic* h, const float* last_obs);
+// after an update's launch: with a staged row T it is the first observation of the next rollout, in row 0 (copy_row0: the
+// update did not copy it there itself)
+int ac_update_finish(ActorCritic* h, const float* last_obs, bool copy_row0);
 
 // ---- debug read-back (b2g_debug_ppo_tensor / b2g_debug_trpo_tensor): one named device buffer, its element count and size
 struct AcDebugBuf { const void* p = nullptr; int64_t numel = 0; int elem_bytes = 4; };
@@ -167,8 +202,9 @@ int ac_debug_info(const AcDebugBuf& b, int64_t* numel, int32_t* elem_bytes);
 int ac_debug_read(ActorCritic* h, const AcDebugBuf& b, const char* name, void* dst, size_t bytes);
 
 // ---- training state (container format in state.cuh): HOST {n_updates, 0}, CNTR the 4 counters, then the parameter arena and
-// the Adam moments.  An update boundary: the rollout in flight is not saved; a load leaves an empty rollout with cleared
-// episode-start flags (the env starts a fresh episode).
+// the Adam moments, then ORMS (obs_rms) behind the obs_rms fingerprint field when the handle owns device statistics.  An
+// update boundary: the rollout in flight is not saved; a load leaves an empty rollout with cleared episode-start flags and
+// nothing staged (the env starts a fresh episode).
 int ac_state_save(ActorCritic* h, const char* path, uint32_t kind, const std::vector<FpField>& fp);
 int ac_state_load(ActorCritic* h, const char* path, uint32_t kind, const std::vector<FpField>& fp, const char* learner);
 

@@ -382,6 +382,7 @@ int b2g_ppo_create(const b2g_ppo_cfg* cfg, b2g_ppo** out) {
   auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_ppo_destroy(h); g_b2g_err = keep; return rc; };
   if (int rc = ac_init(h, c.device, c.obs_dim, c.n_actions, c.hidden0, c.hidden1, c.n_envs, c.n_steps, std::max(64, c.n_envs), c.seed))
     return bail(rc);
+  h->rms.set_call = "b2g_ppo_obs_rms_set";
   h->NB = (int)nb; h->NMB = c.nminibatches; h->M = (int)(nb / c.nminibatches);
   h->RMAX = std::max(h->M, h->P_ROWS);
   ac_layout(h, "model/", kGradMask, 1);
@@ -454,18 +455,20 @@ int b2g_ppo_rollout_get(b2g_ppo* h, float* adv, float* ret, float* val, float* n
 int b2g_ppo_update(b2g_ppo* h, const float* last_obs, const int32_t* perm, float lr, float cliprange, float cliprange_vf,
                    b2g_ppo_metrics* out) {
   B2G_USABLE(h);
-  if (!h || !last_obs || !perm) return b2g_fail(B2G_EINVAL, "NULL argument");
+  if (!h || !perm) return b2g_fail(B2G_EINVAL, "NULL argument");
   if (h->t != h->T) return b2g_fail(B2G_ESTATE, "the rollout is not full: n_steps rollout steps come before an update");
+  if (int rc = ac_check_last_obs(h, last_obs)) return rc;
   const int64_t n = (int64_t)h->cfg.noptepochs * h->NB;
   for (int64_t i = 0; i < n; ++i)
     if (perm[i] < 0 || perm[i] >= h->NB) return b2g_fail(B2G_EINVAL, "permutation entry " + std::to_string(i) + " is outside [0, n_batch)");
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = upload_hp(h, lr, cliprange, cliprange_vf)) return rc;
-  if (int rc = ac_upload_rows(h, h->r_obs + (size_t)h->T * h->E * h->XS, last_obs, h->E)) return rc;
+  if (int rc = ac_update_last_obs(h, last_obs)) return rc;
   CK(cudaMemcpyAsync(h->perm, perm, n * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
   if (int rc = ac_run_update(h, [&] { return update_issue(h); })) return rc;
   h->n_updates += (int64_t)h->mbs.size();
   h->t = 0;
+  if (int rc = ac_update_finish(h, last_obs, true)) return rc;
   return fetch(h, out, true);
 }
 
@@ -508,6 +511,24 @@ int b2g_ppo_get_step(b2g_ppo* h, int64_t* adam_step, int64_t* noise_step, int32_
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   return ac_get_step(h, adam_step, noise_step, rollout_rows);
 }
+
+// ---- VecNormalize's obs_rms on the device and the observe path (bodies in actor_critic.cu)
+#define B2G_PPO_HANDLE(h) B2G_USABLE(h); if (!h) return b2g_fail(B2G_EINVAL, "NULL handle")
+int b2g_ppo_obs_rms_set(b2g_ppo* h, const double* mean, const double* var, double count) { return ac_obs_rms_set(h, mean, var, count); }
+int b2g_ppo_obs_rms_get(b2g_ppo* h, double* mean, double* var, double* count) { return ac_obs_rms_get(h, mean, var, count); }
+int b2g_ppo_upload_bytes(const b2g_ppo* h, int64_t* observe_bytes, int64_t* other_bytes) { return ac_upload_bytes(h, observe_bytes, other_bytes); }
+int b2g_ppo_set_norm_stats(b2g_ppo* h, double clip_obs, double eps, int norm_obs) { B2G_PPO_HANDLE(h); return ac_set_norm_stats(h, clip_obs, eps, norm_obs); }
+int b2g_ppo_set_obs_encoder(b2g_ppo* h, const b2g_encoder* enc, int tail) { B2G_PPO_HANDLE(h); return ac_set_obs_encoder(h, enc, tail); }
+int b2g_ppo_observe_act(b2g_ppo* h, const float* obs, int n, int update_stats, float* act_out) {
+  B2G_PPO_HANDLE(h);
+  return ac_observe_act(h, obs, n, update_stats, act_out, false);
+}
+int b2g_ppo_act_raw(b2g_ppo* h, const float* obs, int n, int deterministic, float* act_out, float* value_out, float* neglogp_out) {
+  B2G_PPO_HANDLE(h);
+  if (!obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  return ac_predict(h, obs, n, deterministic, act_out, value_out, neglogp_out, true);
+}
+#undef B2G_PPO_HANDLE
 
 }  // extern "C"
 

@@ -842,6 +842,7 @@ int b2g_trpo_create(const b2g_trpo_cfg* cfg, b2g_trpo** out) {
   h->cfg = c;
   auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_trpo_destroy(h); g_b2g_err = keep; return rc; };
   if (int rc = ac_init(h, c.device, c.obs_dim, c.n_actions, c.hidden0, c.hidden1, 1, (int)N, 64, c.seed)) return bail(rc);
+  h->rms.set_call = "b2g_trpo_obs_rms_set";
   h->N = (int)N; h->NF = (int)((N + 4) / 5);
   h->RMAX = (int)std::max<int64_t>(N + 1, h->P_ROWS);
   h->NVMB = c.vf_iters * (int)(N / kVfBatch);
@@ -911,6 +912,8 @@ int b2g_trpo_rollout_act(b2g_trpo* h, const float* obs, float* act_out) {
   if (int rc = ac_upload_rows(h, h->r_obs, obs, 1)) return rc;
   CK(cudaMemcpyAsync(act_out, h->r_act, (size_t)h->A * sizeof(float), cudaMemcpyDefault, h->stream));
   CK(cudaStreamSynchronize(h->stream));
+  h->acted = true;
+  h->ob_n = 0;
   return 0;
 }
 
@@ -945,16 +948,18 @@ static int upload_perm(b2g_trpo* h, const int32_t* perm) {
 
 int b2g_trpo_update(b2g_trpo* h, const float* last_obs, const int32_t* perm, b2g_trpo_metrics* out) {
   B2G_USABLE(h);
-  if (!h || !last_obs || (!perm && h->cfg.vf_iters > 0)) return b2g_fail(B2G_EINVAL, "NULL argument");
+  if (!h || (!perm && h->cfg.vf_iters > 0)) return b2g_fail(B2G_EINVAL, "NULL argument");
   if (h->t != h->N) return b2g_fail(B2G_ESTATE, "the rollout is not full: timesteps_per_batch rollout steps come before an update");
+  if (int rc = ac_check_last_obs(h, last_obs)) return rc;
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
   if (int rc = upload_perm(h, perm)) return rc;
-  if (int rc = ac_upload_rows(h, h->r_obs + (size_t)h->N * h->XS, last_obs, 1)) return rc;
+  if (int rc = ac_update_last_obs(h, last_obs)) return rc;
   if (int rc = ac_run_update(h, [&] { return update_issue(h); })) return rc;
   h->n_updates += 1;
   h->t = 0;
   h->carried = true;
+  if (int rc = ac_update_finish(h, last_obs, false)) return rc;     // the update carried row N into row 0 itself
   return fetch(h, out);
 }
 
@@ -975,6 +980,8 @@ int b2g_trpo_step_explicit(b2g_trpo* h, const float* obs, const float* actions, 
   h->n_updates += 1;
   h->t = 0;
   h->carried = false;
+  h->acted = false;
+  h->ob_n = 0;
   const int rc = fetch(h, out);
   if (grad) if (int r2 = download_flat(h, h->G, grad)) return r2;
   if (stepdir) if (int r2 = download_flat(h, h->X, stepdir)) return r2;
@@ -997,6 +1004,8 @@ int b2g_trpo_fvp(b2g_trpo* h, const float* obs, const float* v, float* out) {
   CK(cudaStreamSynchronize(h->stream));
   h->t = 0;
   h->carried = false;
+  h->acted = false;
+  h->ob_n = 0;
   return download_flat(h, h->Zv, out);
 }
 
@@ -1011,6 +1020,25 @@ int b2g_trpo_get_step(b2g_trpo* h, int64_t* adam_step, int64_t* noise_step, int3
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   return ac_get_step(h, adam_step, noise_step, rollout_rows);
 }
+
+// ---- VecNormalize's obs_rms on the device and the observe path (bodies in actor_critic.cu); the boundary row carried into
+// row 0 is the normalised row as it was staged
+#define B2G_TRPO_HANDLE(h) B2G_USABLE(h); if (!h) return b2g_fail(B2G_EINVAL, "NULL handle")
+int b2g_trpo_obs_rms_set(b2g_trpo* h, const double* mean, const double* var, double count) { return ac_obs_rms_set(h, mean, var, count); }
+int b2g_trpo_obs_rms_get(b2g_trpo* h, double* mean, double* var, double* count) { return ac_obs_rms_get(h, mean, var, count); }
+int b2g_trpo_upload_bytes(const b2g_trpo* h, int64_t* observe_bytes, int64_t* other_bytes) { return ac_upload_bytes(h, observe_bytes, other_bytes); }
+int b2g_trpo_set_norm_stats(b2g_trpo* h, double clip_obs, double eps, int norm_obs) { B2G_TRPO_HANDLE(h); return ac_set_norm_stats(h, clip_obs, eps, norm_obs); }
+int b2g_trpo_set_obs_encoder(b2g_trpo* h, const b2g_encoder* enc, int tail) { B2G_TRPO_HANDLE(h); return ac_set_obs_encoder(h, enc, tail); }
+int b2g_trpo_observe_act(b2g_trpo* h, const float* obs, int n, int update_stats, float* act_out) {
+  B2G_TRPO_HANDLE(h);
+  return ac_observe_act(h, obs, n, update_stats, act_out, h->carried);
+}
+int b2g_trpo_act_raw(b2g_trpo* h, const float* obs, int n, int deterministic, float* act_out, float* value_out) {
+  B2G_TRPO_HANDLE(h);
+  if (!obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  return ac_predict(h, obs, n, deterministic, act_out, value_out, nullptr, true);
+}
+#undef B2G_TRPO_HANDLE
 
 }  // extern "C"
 
@@ -1104,6 +1132,8 @@ int b2g_debug_trpo_cg(b2g_trpo* h, const float* obs, const float* actions, const
   CK(cudaStreamSynchronize(s));
   h->t = 0;
   h->carried = false;
+  h->acted = false;
+  h->ob_n = 0;
   return 0;
 }
 

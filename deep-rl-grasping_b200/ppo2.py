@@ -58,11 +58,12 @@ class PPO2Learner(ActorCriticLearner):
         return dict(advantages=adv, returns=ret, values=val, neglogp=nlp, actions=act)
 
     def update(self, last_obs, perms, lr, cliprange, cliprange_vf):
-        """One update on a full rollout; perms [noptepochs, n_batch] are the epochs' permutations of the env-major batch."""
+        """One update on a full rollout; perms [noptepochs, n_batch] are the epochs' permutations of the env-major batch.
+        ``last_obs=None`` bootstraps from the row observe_act staged after the last step."""
         p = np.ascontiguousarray(perms, np.int32).reshape(-1)
         assert p.size == self.noptepochs * self.n_batch
         m = _lib.PpoMetrics()
-        _lib.check(self.lib.b2g_ppo_update(self.h, _fp(_f32(last_obs).reshape(self.n_envs, self.obs_dim)),
+        _lib.check(self.lib.b2g_ppo_update(self.h, None if last_obs is None else _fp(_f32(last_obs).reshape(self.n_envs, self.obs_dim)),
                                            p.ctypes.data_as(C.POINTER(C.c_int32)), float(lr), float(cliprange), float(cliprange_vf),
                                            C.byref(m)))
         return m.as_dict()
@@ -76,12 +77,14 @@ class PPO2Learner(ActorCriticLearner):
             int(bool(apply_update)), C.byref(m)))
         return m.as_dict()
 
-    def act(self, obs, deterministic=True):
-        """-> actions [n, n_actions] (mean, or mean + std * noise of stream 1), values [n], neglogp [n]; nothing is stored."""
+    def act(self, obs, deterministic=True, raw=False):
+        """-> actions [n, n_actions] (mean, or mean + std * noise of stream 1), values [n], neglogp [n]; nothing is stored.
+        ``raw``: the observations are normalised with the device obs_rms first (b2g_ppo_act_raw)."""
         obs = _f32(obs).reshape(-1, self.obs_dim)
         n = obs.shape[0]
         a, v, nl = np.empty((n, self.n_actions), np.float32), np.empty(n, np.float32), np.empty(n, np.float32)
-        _lib.check(self.lib.b2g_ppo_act(self.h, _fp(obs), n, int(bool(deterministic)), _fp(a), _fp(v), _fp(nl)))
+        fn = self.lib.b2g_ppo_act_raw if raw else self.lib.b2g_ppo_act
+        _lib.check(fn(self.h, _fp(obs), n, int(bool(deterministic)), _fp(a), _fp(v), _fp(nl)))
         return a, v, nl
 
 
@@ -106,11 +109,13 @@ class PPO2(ActorCriticModel):
     def __init__(self, policy, env, gamma=0.99, n_steps=128, ent_coef=0.01, learning_rate=2.5e-4, vf_coef=0.5, max_grad_norm=0.5,
                  lam=0.95, nminibatches=4, noptepochs=4, cliprange=0.2, cliprange_vf=None, verbose=0, tensorboard_log=None,
                  _init_setup_model=True, policy_kwargs=None, full_tensorboard_log=False, seed=None, n_cpu_tf_sess=None, device=0,
-                 **unsupported):
+                 device_obs_norm=False, **unsupported):
         if unsupported:
-            if "device_obs_norm" in unsupported:
-                raise NotImplementedError("device_obs_norm: PPO2 stores what a host VecNormalize returns, as stable-baselines does")
             raise TypeError(f"PPO2 got unexpected keyword arguments {sorted(unsupported)}")
+        # learn() uploads each raw frame once: a VecNormalize with norm_obs hands its obs_rms to the learner, which merges the
+        # frame and stores it in the rollout normalised as the wrapper would have returned it (PPO2Learner.observe_act)
+        self.device_obs_norm = bool(device_obs_norm)
+        self._refuse_device_obs_norm_without_wrapper(env)
         check_policy(policy, "PPO2")
         self.policy_kwargs, self.layers = _check_policy_kwargs(policy_kwargs)
         self.gamma, self.n_steps, self.ent_coef, self.learning_rate = gamma, int(n_steps), ent_coef, learning_rate
@@ -138,6 +143,7 @@ class PPO2(ActorCriticModel):
         self.learner = PPO2Learner(obs_dim, A, tuple(self.layers), self.n_envs, self.n_steps, self.nminibatches, self.noptepochs,
                                    self.gamma, self.lam, self.ent_coef, self.vf_coef, self.max_grad_norm, int(self.seed or 0), self.device)
         self.learner.load_parameters(_init_params(obs_dim, A, self.layers, self.seed))
+        self._attach_device()
 
     #: TensorBoard tag -> b2g_ppo_metrics field of the per-update summary (tensorboard.py)
     _update_tags = {"loss/policy_gradient_loss": "policy_loss", "loss/value_function_loss": "value_loss", "loss/entropy_loss": "entropy",
@@ -171,7 +177,8 @@ class PPO2(ActorCriticModel):
             for e in range(self.noptepochs):
                 np.random.shuffle(inds)
                 perms[e] = inds
-            self._update_done(self.learner.update(obs, perms, lr_now, clip_now, cvf_now), writer,
+            last_obs = None if self.device_obs_norm else obs          # None: the row observed after the last step
+            self._update_done(self.learner.update(last_obs, perms, lr_now, clip_now, cvf_now), writer,
                               (("input_info/learning_rate", lr_now), ("input_info/clip_range", clip_now)))
             if self.verbose >= 1 and (update % log_interval == 0 or update == 1):
                 print(f"| ppo2 update {update}/{n_updates} | total_timesteps {self.num_timesteps} | "

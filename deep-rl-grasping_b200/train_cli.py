@@ -83,7 +83,7 @@ def device_encoder(config, n_envs):
 
 def encode_depth(env, test_env, config, n_envs):
     """--device_encode: the training and evaluation envs hand out raw depth rows (encoders.DeferredEncodedDepthImgSensor);
-    one VecEncodeDepth over each encodes them in this process.  A SAC / BDQ model with device_obs_norm then takes the
+    one VecEncodeDepth over each encodes them in this process.  A SAC / BDQ / PPO2 / TRPO model with device_obs_norm then takes the
     encoder and the training wrapper passes the rows through to the device; the evaluation wrapper stays in host mode."""
     encoder = device_encoder(config, n_envs)
     return VecEncodeDepth(env, encoder), VecEncodeDepth(test_env, encoder)
@@ -108,15 +108,15 @@ def train(args):
         if int(args.n_envs) > 1:
             raise ValueError("--algo DQN: DQN cannot be used with more than one environment (--n_envs 1)")
         if args.device_norm:
-            raise NotImplementedError("--algo DQN: --device_norm is built for SAC and BDQ only")
-    if algo == "PPO":          # PPO2 stores what the host VecNormalize returns, as stable-baselines does
-        if args.device_norm:
-            raise NotImplementedError("--algo PPO: --device_norm is built for SAC and BDQ only")
+            raise NotImplementedError("--algo DQN: --device_norm is built for SAC, BDQ, PPO and TRPO only")
+    if algo in ("PPO", "TRPO") and args.device_norm and not config.get("normalize", False):
+        # PPO2 and TRPO store what VecNormalize returns: --device_norm moves its statistics to the learner, so it needs them
+        raise NotImplementedError(f"--algo {algo}: --device_norm keeps VecNormalize's observation statistics on the GPU; the "
+                                  "config has no normalize: true")
+    if algo == "PPO":
         if args.load_dir:
             raise NotImplementedError("--algo PPO: --load_dir is not read by the reference's PPO branch (sb_helper.py:137-154)")
-    if algo == "TRPO":         # TRPO stores what the host VecNormalize returns and trains on one environment
-        if args.device_norm:
-            raise NotImplementedError("--algo TRPO: --device_norm is built for SAC and BDQ only")
+    if algo == "TRPO":         # TRPO trains on one environment
         if args.load_dir:
             raise NotImplementedError("--algo TRPO: --load_dir is not read by the reference's TRPO branch (sb_helper.py:129-136)")
         if int(args.n_envs) > 1:
@@ -204,9 +204,9 @@ def train(args):
             model.load_parameters(old.get_parameters())
             old.close()
     elif algo == "PPO":
-        model = PPO2(PPOMlpPolicy, env, tensorboard_log=tb, **ppo_kwargs(config))
+        model = PPO2(PPOMlpPolicy, env, tensorboard_log=tb, device_obs_norm=bool(args.device_norm), **ppo_kwargs(config))
     elif algo == "TRPO":
-        model = TRPO(PPOMlpPolicy, env, tensorboard_log=tb, **trpo_kwargs(config))
+        model = TRPO(PPOMlpPolicy, env, tensorboard_log=tb, device_obs_norm=bool(args.device_norm), **trpo_kwargs(config))
     else:
         raise NotImplementedError(f"--algo {algo}: the H100 learner builds the SAC, TRPO, PPO, DQN and BDQ branches of SBPolicy.learn "
                                   "(sb_helper.py:85-226)")
@@ -395,10 +395,11 @@ def build_parser():
                         "--resume takes it from the saved run")
     t.add_argument("--device_norm", action="store_true",
                    help="keep VecNormalize's observation statistics on the GPU and upload every frame once "
-                        "(SAC / BDQ(device_obs_norm=True); not DQN); --resume takes it from the saved run")
+                        "(SAC / BDQ / PPO / TRPO(device_obs_norm=True); not DQN); --resume takes it from the saved run")
     t.add_argument("--device_encode", action="store_true",
                    help="the env's sensor defers the depth encoding (encoders.DeferredEncodedDepthImgSensor): encode the "
-                        "frames of all envs at once in this process, on the learner's device with --device_norm (SAC / BDQ)")
+                        "frames of all envs at once in this process, on the learner's device with --device_norm (SAC / BDQ / "
+                        "PPO / TRPO)")
     t.add_argument("--encoder_precision", default=None, choices=["fp32", "bf16x3"],
                    help="with --device_encode: the encoder's arithmetic, fp32 on the CUDA cores (default) or bf16x3 on the tensor "
                         "cores (about 2^-16 relative per layer); recorded in config.yaml as device_encode_precision")

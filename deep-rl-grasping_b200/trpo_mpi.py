@@ -64,11 +64,12 @@ class TRPOLearner(ActorCriticLearner):
         return p
 
     def update(self, last_obs, perms):
-        """One iteration on a full rollout; perms [vf_iters, N] are the value passes' permutations."""
+        """One iteration on a full rollout; perms [vf_iters, N] are the value passes' permutations.  ``last_obs=None``:
+        the row observe_act staged after the last step is the boundary observation."""
         p = self._perm(perms)
         m = _lib.TrpoMetrics()
-        _lib.check(self.lib.b2g_trpo_update(self.h, _fp(_f32(last_obs).reshape(self.obs_dim)), p.ctypes.data_as(C.POINTER(C.c_int32)),
-                                            C.byref(m)))
+        lo = None if last_obs is None else _fp(_f32(last_obs).reshape(self.obs_dim))
+        _lib.check(self.lib.b2g_trpo_update(self.h, lo, p.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(m)))
         return m.as_dict()
 
     def step_explicit(self, obs, actions, adv, tdlamret, perms):
@@ -89,12 +90,14 @@ class TRPOLearner(ActorCriticLearner):
                                          _fp(out)))
         return out
 
-    def act(self, obs, deterministic=True):
-        """-> actions [n, n_actions] (mean, or mean + std * noise of stream 1), values [n]; nothing is stored."""
+    def act(self, obs, deterministic=True, raw=False):
+        """-> actions [n, n_actions] (mean, or mean + std * noise of stream 1), values [n]; nothing is stored.  ``raw``: the
+        observations are normalised with the device obs_rms first (b2g_trpo_act_raw)."""
         obs = _f32(obs).reshape(-1, self.obs_dim)
         n = obs.shape[0]
         a, v = np.empty((n, self.n_actions), np.float32), np.empty(n, np.float32)
-        _lib.check(self.lib.b2g_trpo_act(self.h, _fp(obs), n, int(bool(deterministic)), _fp(a), _fp(v)))
+        fn = self.lib.b2g_trpo_act_raw if raw else self.lib.b2g_trpo_act
+        _lib.check(fn(self.h, _fp(obs), n, int(bool(deterministic)), _fp(a), _fp(v)))
         return a, v
 
 
@@ -120,14 +123,16 @@ class TRPO(ActorCriticModel):
 
     def __init__(self, policy, env, gamma=0.99, timesteps_per_batch=1024, max_kl=0.01, cg_iters=10, lam=0.98, entcoeff=0.0,
                  cg_damping=1e-2, vf_stepsize=3e-4, vf_iters=3, verbose=0, tensorboard_log=None, _init_setup_model=True,
-                 policy_kwargs=None, full_tensorboard_log=False, seed=None, n_cpu_tf_sess=1, device=0, **unsupported):
+                 policy_kwargs=None, full_tensorboard_log=False, seed=None, n_cpu_tf_sess=1, device=0, device_obs_norm=False,
+                 **unsupported):
         if unsupported:
-            if "device_obs_norm" in unsupported:
-                raise NotImplementedError("device_obs_norm: TRPO stores what a host VecNormalize returns, as stable-baselines does")
             gail = sorted(set(unsupported) & set(_GAIL))
             if gail:
                 raise NotImplementedError(f"{gail}: the GAIL path of TRPO is not built")
             raise TypeError(f"TRPO got unexpected keyword arguments {sorted(unsupported)}")
+        # PPO2's observe path on one env (TRPOLearner.observe_act): the carried boundary row is the row as it was normalised
+        self.device_obs_norm = bool(device_obs_norm)
+        self._refuse_device_obs_norm_without_wrapper(env)
         check_policy(policy, "TRPO")
         self.policy_kwargs, self.layers = check_policy_kwargs(policy_kwargs, "TRPO")
         self.gamma, self.timesteps_per_batch, self.max_kl, self.cg_iters = gamma, int(timesteps_per_batch), max_kl, int(cg_iters)
@@ -155,6 +160,7 @@ class TRPO(ActorCriticModel):
                                    self.cg_iters, self.cg_damping, self.entcoeff, self.vf_stepsize, self.vf_iters, int(self.seed or 0),
                                    self.device)
         self.learner.load_parameters(init_params(obs_dim, A, self.layers, self.seed))
+        self._attach_device()
 
     #: TensorBoard tag -> b2g_trpo_metrics field of the per-iteration summary (tensorboard.py)
     _update_tags = {"policy_gradient_loss": "optimgain", "approximate_kullback-leibler": "meankl", "entropy_loss": "entropy",
@@ -182,7 +188,7 @@ class TRPO(ActorCriticModel):
                 inds = np.arange(N)
                 np.random.shuffle(inds)
                 perms[k] = inds
-            metrics = self.learner.update(obs, perms)
+            metrics = self.learner.update(None if self.device_obs_norm else obs, perms)
             timesteps_so_far += N
             iters_so_far += 1
             self._update_done(metrics, writer)

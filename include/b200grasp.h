@@ -533,6 +533,31 @@ int b2g_ppo_get_step(b2g_ppo* h, int64_t* adam_step, int64_t* noise_step, int32_
 int b2g_ppo_state_save(b2g_ppo* h, const char* path);
 int b2g_ppo_state_load(b2g_ppo* h, const char* path);
 
+/* ---- VecNormalize's observation statistics on the device and the rollout fed from one upload per frame (PPO2 and TRPO
+ *      share these bodies; nranks is 1).  obs_rms is float64 [obs_dim] mean / var + count with the merge rule, kernel and
+ *      checks of b2g_obs_rms_set / _get.  Each observation is normalised ONCE, right after its merge, and stored in the rollout
+ *      as VecNormalize returns it: float(clip((double(x) - mean) / sqrt(var + epsilon), -clip_obs, clip_obs)), evaluated in
+ *      float64 in numpy's order and rounded once (bit-identical to VecNormalize.normalize_obs on the same statistics); without
+ *      obs_rms, or with norm_obs 0, the rows are stored as given.  The statistics also ride the training-state file (an ORMS
+ *      section behind the obs_rms fingerprint field; a file of the other kind is refused naming obs_rms). */
+int b2g_ppo_obs_rms_set(b2g_ppo* h, const double* mean, const double* var, double count);
+int b2g_ppo_obs_rms_get(b2g_ppo* h, double* mean, double* var, double* count);
+/* bytes copied host -> device by b2g_ppo_observe_act and b2g_ppo_obs_rms_set (observe_bytes) and by b2g_ppo_act_raw (other) */
+int b2g_ppo_upload_bytes(const b2g_ppo* h, int64_t* observe_bytes, int64_t* other_bytes);
+/* VecNormalize's clip_obs, epsilon and norm_obs for the normalisation (defaults 10, 1e-8, 1); B2G_EINVAL unless clip_obs and
+ * epsilon are finite and >= 0 */
+int b2g_ppo_set_norm_stats(b2g_ppo* h, double clip_obs, double eps, int norm_obs);
+/* obs != NULL: n = n_envs raw frames (host, caller-owned) are uploaded once, merged into obs_rms when update_stats != 0
+ * (B2G_ESTATE without b2g_ppo_obs_rms_set) and normalised into the current rollout row: row t, or row t + 1 once row t's action
+ * is drawn (so the frames the env returns after step t go to row t + 1, and after the last step to row n_steps, the bootstrap
+ * row).  act_out != NULL: rollout step t on that row (b2g_ppo_rollout_act without the upload; B2G_ESTATE when row t holds no
+ * staged observation or its action is drawn).  Both NULL: B2G_EINVAL.  n != n_envs: B2G_EINVAL.  One stream synchronise.
+ * b2g_ppo_update with last_obs == NULL bootstraps from the staged row n_steps and starts the next rollout from it (row 0);
+ * without one it is refused with B2G_EINVAL. */
+int b2g_ppo_observe_act(b2g_ppo* h, const float* obs, int n, int update_stats, float* act_out);
+/* b2g_ppo_act on raw observations: normalised with the current statistics first (nothing is merged) */
+int b2g_ppo_act_raw(b2g_ppo* h, const float* obs, int n, int deterministic, float* act_out, float* value_out, float* neglogp_out);
+
 /* ------------------------------------------------------------------------------------------------
  * TRPO learner -- the `sb.TRPO` object of sb_helper.py:129-136 (stable-baselines 2.10.1 trpo_mpi with common.policies.MlpPolicy
  * and one environment, restated in tests/trpo_ref.py).  Variables pi/model/... (the live policy, PPO2's 15 variables under
@@ -609,6 +634,14 @@ int b2g_trpo_get_step(b2g_trpo* h, int64_t* adam_step, int64_t* noise_step, int3
  * empties the rollout and clears the episode-start flag. */
 int b2g_trpo_state_save(b2g_trpo* h, const char* path);
 int b2g_trpo_state_load(b2g_trpo* h, const char* path);
+/* the PPO2 observe path above on the TRPO handle (n = 1).  After an update, step 0 acts on the carried boundary row: the
+ * normalised row as it was staged, and the action drawn for it before the update. */
+int b2g_trpo_obs_rms_set(b2g_trpo* h, const double* mean, const double* var, double count);
+int b2g_trpo_obs_rms_get(b2g_trpo* h, double* mean, double* var, double* count);
+int b2g_trpo_upload_bytes(const b2g_trpo* h, int64_t* observe_bytes, int64_t* other_bytes);
+int b2g_trpo_set_norm_stats(b2g_trpo* h, double clip_obs, double eps, int norm_obs);
+int b2g_trpo_observe_act(b2g_trpo* h, const float* obs, int n, int update_stats, float* act_out);
+int b2g_trpo_act_raw(b2g_trpo* h, const float* obs, int n, int deterministic, float* act_out, float* value_out);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Row a12: auto-encoder ENCODER forward (perception for the `encoded depth` observation, SURVEY.md section 8).
@@ -668,6 +701,10 @@ int b2g_debug_encoder_layers(b2g_encoder* h, const float* imgs, int n, float* ou
  * device; B2G_ESTATE for an encoder layer without weights or nranks > 1. */
 int b2g_sac_set_obs_encoder(b2g_sac* h, const b2g_encoder* enc, int tail);
 int b2g_bdq_set_obs_encoder(b2g_bdq* h, const b2g_encoder* enc, int tail);
+/* the same on the PPO2 and TRPO handles: b2g_ppo_observe_act / b2g_trpo_observe_act take raw rows, encode them into the
+ * staged rows and normalise those into the rollout */
+int b2g_ppo_set_obs_encoder(b2g_ppo* h, const b2g_encoder* enc, int tail);
+int b2g_trpo_set_obs_encoder(b2g_trpo* h, const b2g_encoder* enc, int tail);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Auto-encoder TRAINING (encoders.py:40-61 train / test / predict, graph :84-136): the full Keras model
