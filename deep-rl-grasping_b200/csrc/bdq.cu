@@ -573,14 +573,13 @@ int b2g_bdq_observe_add(b2g_bdq* h, const float* act_idx, const float* rew, cons
     if (int rc = h->rms.stage_reset_frames(h->ob_reset, reset_obs, done, h->ob_done, n, n_done, h->stream)) return rc;
   // the transitions: obs = the staged rows, next_obs = the uploaded rows (a finished env's terminal frame)
   TransitionReplay& rp = h->replay;
-  std::vector<int64_t> next_ids;
   if (rp.framed()) {
     // env i's staged row is the frame its previous transition's next_obs took, unless the env was reset since: shared without
     // comparing; a reset frame (ob_fid -1) takes a frame of its own here, when it is first used as obs
-    next_ids.resize((size_t)n);
-    if (int rc = rp.commit(cur, nxt, n, h->ob_fid.data(), h->ob_act, h->ob_rew, h->ob_done, next_ids.data(), h->stream)) return rc;
+    std::vector<int64_t> next_ids((size_t)n);
+    if (int rc = rp.add_linked(cur, nxt, h->ob_fid.data(), h->ob_act, h->ob_rew, h->ob_done, n, next_ids.data(), h->counters, h->stream))
+      return rc;
     for (int i = 0; i < n; ++i) h->ob_fid[i] = done[i] != 0.f ? -1 : next_ids[i];
-    if (int rc = rp.finish(next_ids, h->counters, h->stream)) return rc;
   } else {
     const int64_t new_size = std::min<int64_t>(rp.cap, rp.size + n);
     bdq_commit_kernel<<<n, 256, 0, h->stream>>>(cur, nxt, h->ob_act, h->ob_rew, h->ob_done, (int)E, (int)D, rp.pos, rp.cap, rp.obs, rp.next,

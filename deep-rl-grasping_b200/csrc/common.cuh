@@ -256,8 +256,9 @@ struct FrameFmt {
   signed char ch[8];
 };
 #ifdef __CUDACC__
-// element e of the compact row stored in frame f (decoded values are exactly the values the caller passed)
-__device__ __forceinline__ float frame_elem(const unsigned char* __restrict__ f, const FrameFmt& m, int npx, int Ci, int e) {
+// element e of the compact row stored in frame f (decoded values are exactly the values the caller passed); the host decodes
+// a frame it read back the same way (TransitionReplay::get)
+__host__ __device__ __forceinline__ float frame_elem(const unsigned char* __restrict__ f, const FrameFmt& m, int npx, int Ci, int e) {
   if (e >= npx) return reinterpret_cast<const float*>(f + m.tail)[e - npx];
   if (m.n8 == 0) return reinterpret_cast<const float*>(f)[e];
   const int pix = e / Ci, k = m.ch[e - pix * Ci];

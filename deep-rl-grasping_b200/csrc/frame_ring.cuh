@@ -1,5 +1,5 @@
-// Host bookkeeping of a replay whose transitions reference observation frames of a pool: SAC's replay (sac.cu) and the BDQ /
-// DQN transition replay built with frames (per.cu).  The frame rows themselves, and the kernels that check and write them, are
+// Host bookkeeping of a replay whose transitions reference observation frames of a pool: the transition replay (per.cuh) of
+// SAC, and of BDQ / DQN built with frames.  The frame rows themselves, and the kernels that check and write them, are
 // FrameFmt / frame_check / frame_commit (common.cuh, replay.cu).
 //
 // Frames are allocated in FIFO order with monotone 64-bit ids; frame id f sits at f % frame_cap.  Transitions are numbered

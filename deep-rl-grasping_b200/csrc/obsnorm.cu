@@ -260,7 +260,8 @@ int b2g_sac_observe_add(b2g_sac* h, const float* act, const float* rew, const fl
   if (int rc = common_checks(h, n, update_stats)) return rc;
   if (h->ob_n == 0) return b2g_fail(B2G_ESTATE, "observe_add: no staged observations (call b2g_sac_observe_act first)");
   if (n != h->ob_n) return b2g_fail(B2G_EINVAL, "observe_add: n differs from the number of staged observations");
-  if (h->dedup && 2 * (int64_t)n > h->frame_cap) return b2g_fail(B2G_EINVAL, "observe_add: 2 n rows exceed frame_capacity");
+  if (h->replay.ring.dedup && 2 * (int64_t)n > h->replay.ring.frame_cap)
+    return b2g_fail(B2G_EINVAL, "observe_add: 2 n rows exceed frame_capacity");
   int n_done = 0;
   for (int i = 0; i < n; ++i) n_done += done[i] != 0.f;
   if (n_done && !reset_obs) return b2g_fail(B2G_EINVAL, "observe_add: an env finished but reset_obs is NULL");
@@ -280,7 +281,9 @@ int b2g_sac_observe_add(b2g_sac* h, const float* act, const float* rew, const fl
   float* nxt = h->ob_rows[h->ob_k ^ 1];
   if (int rc = to_rows(h, h->ob_full[0], nxt, 0, n)) return rc;
   std::vector<int64_t> next_fid((size_t)n);
-  if (int rc = sac_replay_add_linked(h, cur, nxt, h->ob_fid.data(), h->ob_act, h->ob_rew, h->ob_done, n, next_fid.data())) return rc;
+  if (int rc = h->replay.add_linked(cur, nxt, h->ob_fid.data(), h->ob_act, h->ob_rew, h->ob_done, n, next_fid.data(), h->counters,
+                                    h->stream))
+    return rc;
   if (update_stats) h->rms.merge(h->ob_full[0], n_done ? h->ob_full[1] : nullptr, h->ob_done, n, h->stream);
   // the new rows become the current observations; a finished env continues from the frame its reset returned
   for (int i = 0; i < n; ++i) {

@@ -89,20 +89,30 @@ void per_init_launch(double* tsum, double* tmin, long long n2, float* max_prio, 
   per_init_kernel<<<256, 256, 0, s>>>(tsum, tmin, n2, max_prio);
 }
 
+FrameIo plain_frames(int E) {
+  FrameIo f{};
+  f.npx = 0; f.Ci = 1; f.Ec = E;         // fmt {}: the whole row is the fp32 tail
+  f.frame_bytes = ((int64_t)E * (int64_t)sizeof(float) + 15) / 16 * 16;
+  return f;
+}
+
 int TransitionReplay::init(std::vector<void*>& allocs, cudaStream_t s, int64_t cap_, int E_, int A_, int B, bool per_, float alpha_,
-                           float eps_, int64_t frame_cap, int stage_rows_) {
+                           float eps_, int64_t frame_cap, const FrameIo& layout, int stage_rows_) {
   cap = cap_; E = E_; A = A_; per = per_; alpha = alpha_; eps = eps_;
+  if (cudaMallocHost((void**)&h_rc, 2 * sizeof(long long)) != cudaSuccess) return b2g_fail(B2G_ECUDA, "replay staging");
   if (frame_cap > 0) {
     ring.frame_cap = frame_cap;
     ring.dedup = frame_cap < 2 * cap;     // at 2 cap every transition has two frames of its own: sharing would save nothing
-    frame_bytes = ((int64_t)E * (int64_t)sizeof(float) + 15) / 16 * 16;   // 16-byte frame stride: the gather's 128-bit loads stay aligned
+    io = layout;
+    // one commit launch writes distinct transition slots and distinct frames
     stage_rows = (int)std::min<int64_t>({(int64_t)stage_rows_, cap, frame_cap / 2});
-    if (int rc = dev_alloc(allocs, s, &frames, (size_t)(frame_cap * frame_bytes))) return rc;
+    if (int rc = dev_alloc(allocs, s, &io.frames, (size_t)(frame_cap * io.frame_bytes))) return rc;
     if (int rc = dev_alloc(allocs, s, &r_ofr, cap)) return rc;
     if (int rc = dev_alloc(allocs, s, &r_nfr, cap)) return rc;
-    if (int rc = dev_alloc(allocs, s, &c_obs, (size_t)stage_rows * E)) return rc;
-    if (int rc = dev_alloc(allocs, s, &c_next, (size_t)stage_rows * E)) return rc;
+    if (int rc = dev_alloc(allocs, s, &c_obs, (size_t)stage_rows * io.Ec)) return rc;
+    if (int rc = dev_alloc(allocs, s, &c_next, (size_t)stage_rows * io.Ec)) return rc;
     if (int rc = dev_alloc(allocs, s, &d_plan, 4 * (size_t)stage_rows)) return rc;
+    if (cudaMallocHost((void**)&h_plan, 4 * (size_t)stage_rows * sizeof(int)) != cudaSuccess) return b2g_fail(B2G_ECUDA, "replay staging");
   } else {
     if (int rc = dev_alloc(allocs, s, &obs, cap * E)) return rc;
     if (int rc = dev_alloc(allocs, s, &next, cap * E)) return rc;
@@ -122,6 +132,12 @@ int TransitionReplay::init(std::vector<void*>& allocs, cudaStream_t s, int64_t c
   const float beta0 = 0.4f;
   CK(cudaMemcpyAsync(beta, &beta0, sizeof(float), cudaMemcpyHostToDevice, s));
   return 0;
+}
+
+void TransitionReplay::release() {
+  if (h_plan) cudaFreeHost(h_plan);
+  if (h_rc) cudaFreeHost(h_rc);
+  h_plan = nullptr; h_rc = nullptr;
 }
 
 PerArgs TransitionReplay::per_args(const long long* counters, unsigned long long seed, int B, int* indices, float* weights, const float* td,
@@ -145,25 +161,27 @@ void TransitionReplay::advance(int64_t n) {
 }
 
 void TransitionReplay::gather_args(GatherArgs& g, bool with_next) const {
-  if (!framed()) return;
+  g.act = with_next ? act : nullptr; g.rew = rew; g.done = done;
+  if (!framed()) {
+    g.obs = obs; g.next_obs = with_next ? next : nullptr;
+    return;
+  }
   g.obs = nullptr; g.next_obs = nullptr;
-  g.frames = frames; g.frame_bytes = frame_bytes; g.obs_frame = r_ofr; g.next_frame = with_next ? r_nfr : nullptr;
+  g.frames = io.frames; g.frame_bytes = io.frame_bytes; g.obs_frame = r_ofr; g.next_frame = with_next ? r_nfr : nullptr;
+  g.fmt = io.fmt; g.ring_cap = cap;
 }
 
 int TransitionReplay::commit(const float* co, const float* cn, int m, const int64_t* cand, const float* a, const float* r, const float* d,
                              int64_t* next_ids, cudaStream_t s) {
   const int64_t FC = ring.frame_cap, first = ring.head_seq, fid0 = ring.next_fid, tail0 = ring.tail_seq;
-  std::vector<int> plan(3 * (size_t)m);
   for (int i = 0; i < m; ++i) {
     int64_t of, nf;
     const bool share = ring.add_transition(cap, cand[i], &of, &nf);
-    plan[i] = (int)(of % FC); plan[m + i] = share ? 0 : 1; plan[2 * m + i] = (int)(nf % FC);
+    h_plan[i] = (int)(of % FC); h_plan[m + i] = share ? 0 : 1; h_plan[2 * m + i] = (int)(nf % FC);
     next_ids[i] = nf;
   }
-  if (ring.dedup) CK(cudaMemcpyAsync(d_plan, plan.data(), 3 * m * sizeof(int), cudaMemcpyHostToDevice, s));
-  FrameIo io{};
-  io.c_obs = co; io.c_next = cn; io.frames = frames; io.frame_bytes = frame_bytes; io.npx = 0; io.Ci = 1; io.Ec = E;   // MLP rows: fmt {}
-  frame_commit_launch(io, ring.dedup ? d_plan : nullptr, fid0, FC, m, r_ofr, r_nfr, first, cap, s);
+  if (ring.dedup) CK(cudaMemcpyAsync(d_plan, h_plan, 3 * m * sizeof(int), cudaMemcpyHostToDevice, s));
+  frame_commit_launch(frame_io(co, cn), ring.dedup ? d_plan : nullptr, fid0, FC, m, r_ofr, r_nfr, first, cap, s);
   for (int64_t k = 0; k < m;) {          // act / rew / done into slots (first + k) % cap, in at most two pieces
     const int64_t p = (first + k) % cap, len = std::min<int64_t>(m - k, cap - p);
     CK(cudaMemcpyAsync(act + p * A, a + k * A, len * A * sizeof(float), cudaMemcpyDefault, s));
@@ -184,37 +202,66 @@ int TransitionReplay::finish(std::vector<int64_t>& next_ids, long long* counters
   ring.prev_next.swap(next_ids);
   size = ring.size();
   pos = ring.head_seq % cap;
-  const long long rc[2] = {size, size == cap ? 0 : ring.tail_seq % cap};    // size, first live slot
-  CK(cudaMemcpyAsync(counters + 5, rc, sizeof rc, cudaMemcpyHostToDevice, s));
+  h_rc[0] = size;
+  h_rc[1] = size == cap ? 0 : ring.tail_seq % cap;     // the first live slot
+  CK(cudaMemcpyAsync(counters + 5, h_rc, 2 * sizeof(long long), cudaMemcpyHostToDevice, s));
   return 0;
 }
 
+int TransitionReplay::add_linked(const float* co, const float* cn, const int64_t* cand, const float* a, const float* r, const float* d, int n,
+                                 int64_t* next_fid, long long* counters, cudaStream_t s) {
+  std::vector<int64_t> next_ids((size_t)n);
+  for (int64_t c0 = 0; c0 < n; c0 += stage_rows) {
+    const int m = (int)std::min<int64_t>(stage_rows, n - c0);
+    if (c0 > 0) CK(cudaStreamSynchronize(s));        // the previous chunk's plan upload has left h_plan
+    if (int rc = commit(co + c0 * io.Ec, cn + c0 * io.Ec, m, cand + c0, a + c0 * A, r + c0, d + c0, next_ids.data() + c0, s)) return rc;
+  }
+  std::copy(next_ids.begin(), next_ids.end(), next_fid);
+  return finish(next_ids, counters, s);
+}
+
 int TransitionReplay::add(const float* o, const float* a, const float* r, const float* nx, const float* d, int64_t n, long long* counters,
-                          cudaStream_t s) {
+                          cudaStream_t s, const RowLoader& load) {
   if (framed()) {
     const int64_t R = stage_rows, FC = ring.frame_cap;
-    if (ring.dedup && 2 * n > FC) return b2g_fail(B2G_EINVAL, "replay_add: 2 n rows exceed frame_capacity (replay_frames)");
-    FrameIo io{};
-    io.c_obs = c_obs; io.c_next = c_next; io.frames = frames; io.frame_bytes = frame_bytes; io.npx = 0; io.Ci = 1; io.Ec = E;
+    if (ring.dedup && 2 * n > FC) return b2g_fail(B2G_EINVAL, std::string("replay_add: 2 n rows exceed ") + frames_name);
+    const bool u8 = io.fmt.n8 > 0;
+    const FrameIo fio = frame_io(c_obs, c_next);
+    int* flags = h_plan + 3 * R;
+    // rows [c0, c0 + m) -> the compact staging, then (when sharing frames or checking 8-bit values) frame_check -> flags,
+    // synchronised
+    auto stage = [&](int64_t c0, int m, bool check) -> int {
+      if (c0 > 0) CK(cudaStreamSynchronize(s));        // the previous chunk's plan upload has left h_plan
+      for (int w = 0; w < 2; ++w) {
+        const float* src = (w ? nx : o) + c0 * E;
+        float* dst = w ? c_next : c_obs;
+        if (load) {
+          if (int rc = load(src, dst, m)) return rc;
+        } else CK(cudaMemcpyAsync(dst, src, m * io.Ec * sizeof(float), cudaMemcpyDefault, s));
+      }
+      if (!check) return 0;
+      for (int i = 0; i < m; ++i) {      // candidate frame of row i: the previous call's next_obs of row i, while it still exists
+        const int64_t p = c0 + i < (int64_t)ring.prev_next.size() ? ring.prev_next[c0 + i] : -1;
+        h_plan[i] = ring.dedup && p >= 0 && p > ring.next_fid - FC ? (int)(p % FC) : -1;
+      }
+      CK(cudaMemcpyAsync(d_plan, h_plan, m * sizeof(int), cudaMemcpyHostToDevice, s));
+      frame_check_launch(fio, d_plan, d_plan + 3 * R, m, s);
+      CK(cudaMemcpyAsync(flags, d_plan + 3 * R, m * sizeof(int), cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      for (int i = 0; i < m; ++i)
+        if (flags[i] & 2) return b2g_fail(B2G_EINVAL, "replay_add: a value of an 8-bit plane is not an integer in [0, 255]");
+      return 0;
+    };
+    // a call larger than the staging validates every row before it stores the first one
+    if (u8 && n > R)
+      for (int64_t c0 = 0; c0 < n; c0 += R)
+        if (int rc = stage(c0, (int)std::min<int64_t>(R, n - c0), true)) return rc;
     std::vector<int64_t> next_ids((size_t)n), cand((size_t)R);
-    std::vector<int> hp((size_t)R), flags((size_t)R);
     for (int64_t c0 = 0; c0 < n; c0 += R) {
       const int m = (int)std::min<int64_t>(R, n - c0);
-      if (c0 > 0) CK(cudaStreamSynchronize(s));
-      CK(cudaMemcpyAsync(c_obs, o + c0 * E, m * E * sizeof(float), cudaMemcpyDefault, s));
-      CK(cudaMemcpyAsync(c_next, nx + c0 * E, m * E * sizeof(float), cudaMemcpyDefault, s));
-      for (int i = 0; i < m; ++i) cand[i] = -1;
-      if (ring.dedup) {       // row i's obs against the previous call's next_obs frame of row i, while it still exists
-        for (int i = 0; i < m; ++i) {
-          const int64_t p = c0 + i < (int64_t)ring.prev_next.size() ? ring.prev_next[c0 + i] : -1;
-          hp[i] = p >= 0 && p > ring.next_fid - FC ? (int)(p % FC) : -1;
-        }
-        CK(cudaMemcpyAsync(d_plan, hp.data(), m * sizeof(int), cudaMemcpyHostToDevice, s));
-        frame_check_launch(io, d_plan, d_plan + 3 * R, m, s);
-        CK(cudaMemcpyAsync(flags.data(), d_plan + 3 * R, m * sizeof(int), cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        for (int i = 0; i < m; ++i) if (flags[i] & 1) cand[i] = ring.prev_next[c0 + i];
-      }
+      if (int rc = stage(c0, m, ring.dedup || (u8 && n <= R))) return rc;
+      for (int i = 0; i < m; ++i)        // the previous call's next_obs of row i, where frame_check found it equal bit for bit
+        cand[i] = ring.dedup && (flags[i] & 1) ? ring.prev_next[c0 + i] : -1;
       if (int rc = commit(c_obs, c_next, m, cand.data(), a + c0 * A, r + c0, d + c0, next_ids.data() + c0, s)) return rc;
     }
     if (int rc = finish(next_ids, counters, s)) return rc;
@@ -232,8 +279,8 @@ int TransitionReplay::add(const float* o, const float* a, const float* r, const 
     advance(chunk);
     done_n += chunk;
   }
-  const long long sz = size;
-  CK(cudaMemcpyAsync(counters + 5, &sz, sizeof(long long), cudaMemcpyHostToDevice, s));
+  h_rc[0] = size;
+  CK(cudaMemcpyAsync(counters + 5, h_rc, sizeof(long long), cudaMemcpyHostToDevice, s));
   CK(cudaStreamSynchronize(s));
   return 0;
 }
@@ -266,11 +313,17 @@ int TransitionReplay::get(int64_t slot, float* o, float* a, float* r, float* nx,
     CK(cudaMemcpy(&fr[0], r_ofr + slot, sizeof(int), cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(&fr[1], r_nfr + slot, sizeof(int), cudaMemcpyDeviceToHost));
   }
+  std::vector<float> frame(framed() ? io.frame_bytes / sizeof(float) : 0);    // frame strides are whole floats
   for (int w = 0; w < 2; ++w) {
     float* dst = w ? nx : o;
     if (!dst) continue;
-    const void* src = framed() ? (const void*)(frames + (size_t)fr[w] * frame_bytes) : (const void*)((w ? next : obs) + slot * E);
-    CK(cudaMemcpy(dst, src, E * sizeof(float), cudaMemcpyDeviceToHost));
+    if (!framed()) {
+      CK(cudaMemcpy(dst, (w ? next : obs) + slot * E, E * sizeof(float), cudaMemcpyDeviceToHost));
+      continue;
+    }
+    CK(cudaMemcpy(frame.data(), io.frames + (size_t)fr[w] * io.frame_bytes, io.frame_bytes, cudaMemcpyDeviceToHost));
+    const unsigned char* f = reinterpret_cast<const unsigned char*>(frame.data());
+    for (int e = 0; e < io.Ec; ++e) dst[e] = frame_elem(f, io.fmt, io.npx, io.Ci, e);
   }
   if (a) CK(cudaMemcpy(a, act + slot * A, A * sizeof(float), cudaMemcpyDeviceToHost));
   if (r) CK(cudaMemcpy(r, rew + slot, sizeof(float), cudaMemcpyDeviceToHost));
@@ -285,14 +338,22 @@ void TransitionReplay::info(int64_t* capacity, int64_t* sz, int64_t* frame_capac
   if (sz) *sz = size;
   if (frame_capacity) *frame_capacity = ring.frame_cap;
   if (live_frames) *live_frames = ring.live_frames();
-  if (bytes) *bytes = transition_replay_bytes(cap, E, A, ring.frame_cap);
+  if (bytes) {
+    const int64_t fb = sizeof(float);
+    *bytes = (framed() ? ring.frame_cap * io.frame_bytes + 2 * cap * (int64_t)sizeof(int) : 2 * cap * E * fb) + cap * (A + 2) * fb;
+  }
   if (evicted_early) *evicted_early = ring.evicted;
+}
+
+int check_frame_capacity(int64_t frame_cap, int64_t cap, const char* name) {
+  if (frame_cap < cap + 1) return b2g_fail(B2G_EINVAL, std::string(name) + " must be at least buffer_capacity + 1");
+  if (frame_cap > INT32_MAX) return b2g_fail(B2G_EINVAL, std::string(name) + " must fit in int32 (frame indices)");
+  return 0;
 }
 
 int check_replay_cfg(const b2g_replay_cfg* r, int64_t cap, int nranks) {
   if (!r) return 0;
-  if (r->frame_capacity < cap + 1) return b2g_fail(B2G_EINVAL, "frame_capacity (replay_frames) must be at least buffer_capacity + 1");
-  if (r->frame_capacity > INT32_MAX) return b2g_fail(B2G_EINVAL, "frame_capacity (replay_frames) must fit in int32 (frame indices)");
+  if (int rc = check_frame_capacity(r->frame_capacity, cap, "frame_capacity (replay_frames)")) return rc;
   if (r->u8_plane_mask)
     return b2g_fail(B2G_EINVAL, "u8_plane_mask: the BDQ / DQN replay stores fp32 observation vectors (8-bit planes are SAC's CNN rows)");
   if (nranks > 1) return b2g_fail(B2G_EINVAL, "replay frames (replay_frames) are not built for data-parallel learners (nranks > 1)");
@@ -301,7 +362,7 @@ int check_replay_cfg(const b2g_replay_cfg* r, int64_t cap, int nranks) {
 
 int64_t transition_replay_bytes(int64_t cap, int E, int A, int64_t frame_cap) {
   const int64_t fb = sizeof(float);
-  const int64_t rows = frame_cap > 0 ? frame_cap * ((E * fb + 15) / 16 * 16) + 2 * cap * (int64_t)sizeof(int) : 2 * cap * E * fb;
+  const int64_t rows = frame_cap > 0 ? frame_cap * plain_frames(E).frame_bytes + 2 * cap * (int64_t)sizeof(int) : 2 * cap * E * fb;
   return rows + cap * (A + 2) * fb;
 }
 
@@ -346,7 +407,7 @@ int TransitionReplay::state_host_read(StateReader& rd, std::vector<int64_t>* hv,
 std::vector<StateSection> TransitionReplay::state_sections(int64_t live, int64_t lo, int64_t hi) const {
   const size_t fb = sizeof(float);
   if (framed()) {
-    std::vector<StateSection> s(8);
+    std::vector<StateSection> s(6);
     s[0].tag = state_tag("ROFR"); s[0].pieces = {dev_piece(r_ofr, cap * sizeof(int))};
     s[1].tag = state_tag("RNFR"); s[1].pieces = {dev_piece(r_nfr, cap * sizeof(int))};
     s[2].tag = state_tag("RACT"); s[2].pieces = {dev_piece(act, cap * A * fb)};
@@ -355,24 +416,26 @@ std::vector<StateSection> TransitionReplay::state_sections(int64_t live, int64_t
     s[5].tag = state_tag("FRMS");
     for (int64_t f = lo; f < hi;) {      // frames [lo, hi): at most two contiguous ranges, each stored at id % frame_cap
       const int64_t p = f % ring.frame_cap, n = std::min(hi - f, ring.frame_cap - p);
-      s[5].pieces.push_back(dev_piece(frames + p * frame_bytes, (size_t)(n * frame_bytes)));
+      s[5].pieces.push_back(dev_piece(io.frames + p * io.frame_bytes, (size_t)(n * io.frame_bytes)));
       f += n;
     }
-    s[6].tag = state_tag("PERT");
-    if (per) s[6].pieces = {dev_piece(t_sum, 2 * per_C * sizeof(double)), dev_piece(t_min, 2 * per_C * sizeof(double))};
-    s[7].tag = state_tag("PERS"); s[7].pieces = {dev_piece(max_prio, sizeof(float)), dev_piece(beta, sizeof(float))};
     return s;
   }
   (void)lo; (void)hi;
-  std::vector<StateSection> s(7);
+  std::vector<StateSection> s(5);
   s[0].tag = state_tag("ROBS"); s[0].pieces = {dev_piece(obs, live * E * fb)};
   s[1].tag = state_tag("RNXT"); s[1].pieces = {dev_piece(next, live * E * fb)};
   s[2].tag = state_tag("RACT"); s[2].pieces = {dev_piece(act, cap * A * fb)};
   s[3].tag = state_tag("RREW"); s[3].pieces = {dev_piece(rew, cap * fb)};
   s[4].tag = state_tag("RDON"); s[4].pieces = {dev_piece(done, cap * fb)};
-  s[5].tag = state_tag("PERT");
-  if (per) s[5].pieces = {dev_piece(t_sum, 2 * per_C * sizeof(double)), dev_piece(t_min, 2 * per_C * sizeof(double))};
-  s[6].tag = state_tag("PERS"); s[6].pieces = {dev_piece(max_prio, sizeof(float)), dev_piece(beta, sizeof(float))};
+  return s;
+}
+
+std::vector<StateSection> TransitionReplay::per_sections() const {
+  std::vector<StateSection> s(2);
+  s[0].tag = state_tag("PERT");
+  if (per) s[0].pieces = {dev_piece(t_sum, 2 * per_C * sizeof(double)), dev_piece(t_min, 2 * per_C * sizeof(double))};
+  s[1].tag = state_tag("PERS"); s[1].pieces = {dev_piece(max_prio, sizeof(float)), dev_piece(beta, sizeof(float))};
   return s;
 }
 

@@ -20,7 +20,7 @@ int ql_init(QLearner* h, int64_t g_extra, const b2g_replay_cfg* replay, int stag
   QA(h->P, 2 * h->n_train); QA(h->Mo, h->n_train); QA(h->Vo, h->n_train); QA(h->G, h->n_train + g_extra); QA(h->metrics, MET_COUNT);
   QA(h->counters, 8); QA(h->step_consts, 4); QA(h->d_lr, 1);
   if (int rc = h->replay.init(h->allocs, h->stream, h->buffer_capacity, E, A, B, h->prioritized, h->per_alpha, h->per_eps,
-                              replay ? replay->frame_capacity : 0, stage_rows))
+                              replay ? replay->frame_capacity : 0, plain_frames(E), stage_rows))
     return rc;
   QA(h->d_mean, E); QA(h->d_istd, E); QA(h->d_normc, 8);
   QA(h->X, (size_t)B * h->XS); QA(h->Xn, (size_t)B * h->XS); QA(h->Xscratch, (size_t)B * h->XS);
@@ -44,23 +44,23 @@ void ql_release(QLearner* h) {
   if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
   mlog_free(&h->mlog);
   for (void* q : h->allocs) cudaFree(q);
+  h->replay.release();
   if (h->h_met) cudaFreeHost(h->h_met);
   if (h->stream) cudaStreamDestroy(h->stream);
 }
 
 GatherArgs ql_gather(QLearner* h, bool from_replay, bool with_next) {
   GatherArgs g{};
-  g.obs = from_replay ? h->replay.obs : h->s_obs;
-  g.next_obs = with_next ? (from_replay ? h->replay.next : h->s_next) : nullptr;
-  g.act = with_next ? (from_replay ? h->replay.act : h->s_act) : nullptr;
-  g.rew = from_replay ? h->replay.rew : h->s_rew;
-  g.done = from_replay ? h->replay.done : h->s_done;
-  g.indices = from_replay ? h->indices : nullptr;
+  g.obs = h->s_obs; g.next_obs = with_next ? h->s_next : nullptr;
+  g.act = with_next ? h->s_act : nullptr; g.rew = h->s_rew; g.done = h->s_done;
+  if (from_replay) {
+    h->replay.gather_args(g, with_next);
+    g.indices = h->indices;
+  }
   g.mean = h->d_mean; g.var = h->d_istd; g.normc = h->d_normc;
   g.B = h->B; g.H = 0; g.W = h->E; g.Cimg = 0; g.scale = 1.f;
   g.F_pi = h->Xscratch; g.F_v = h->X; g.F_t = h->Xn; g.FS = h->XS; g.feat_col = 0;
   g.rew_out = h->rew_n; g.done_out = h->done_n; g.n_act = h->A;
-  if (from_replay) h->replay.gather_args(g, with_next);     // a replay of frames: rows through obs_frame / next_frame
   return g;
 }
 
@@ -208,6 +208,7 @@ namespace {
 std::vector<StateSection> ql_device_sections(QLearner* h, ObsRms* rms, int64_t live, int64_t lo = 0, int64_t hi = 0) {
   std::vector<StateSection> s = adam_sections(h->P, 2 * h->n_train, h->Mo, h->Vo, h->n_train);
   for (auto& r : h->replay.state_sections(live, lo, hi)) s.push_back(std::move(r));
+  for (auto& r : h->replay.per_sections()) s.push_back(std::move(r));
   if (rms && rms->on()) s.push_back(rms_section(&rms->count, rms->mean, rms->var, h->E));
   return s;
 }

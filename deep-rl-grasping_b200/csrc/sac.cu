@@ -605,17 +605,12 @@ TailArgs make_tail(b2g_sac* h, bool want_per_sample) {
 
 GatherArgs make_gather(b2g_sac* h, bool from_replay, bool with_next) {
   GatherArgs g{};
-  g.obs = from_replay ? nullptr : h->s_obs;
-  g.next_obs = with_next ? (from_replay ? nullptr : h->s_next) : nullptr;
+  g.obs = h->s_obs; g.next_obs = with_next ? h->s_next : nullptr; g.fmt = h->row_fmt;
+  g.act = with_next ? h->s_act : nullptr; g.rew = h->s_rew; g.done = h->s_done;
   if (from_replay) {
-    g.frames = h->frames; g.frame_bytes = h->frame_bytes; g.obs_frame = h->r_ofr; g.next_frame = with_next ? h->r_nfr : nullptr;
-    g.ring_cap = h->cfg.buffer_capacity;
+    h->replay.gather_args(g, with_next);      // frames through the slots' frame indices
+    g.indices = h->indices;
   }
-  g.fmt = from_replay ? h->fmt : h->row_fmt;
-  g.act = with_next ? (from_replay ? h->r_act : h->s_act) : nullptr;
-  g.rew = from_replay ? h->r_rew : h->s_rew;
-  g.done = from_replay ? h->r_done : h->s_done;
-  g.indices = from_replay ? h->indices : nullptr;
   g.mean = h->d_mean; g.var = h->d_istd;
   g.normc = h->d_normc;
   g.B = h->B;
@@ -955,55 +950,6 @@ int full_index(const b2g_sac* h, int e) {
   return e == npx && h->direct_feature() ? Ci : -1;
 }
 
-FrameIo frame_io(const b2g_sac* h, const float* c_obs, const float* c_next) {
-  FrameIo io{};
-  io.c_obs = c_obs; io.c_next = c_next; io.frames = h->frames; io.frame_bytes = h->frame_bytes;
-  io.fmt = h->fmt; io.npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0; io.Ci = h->cnn ? h->Cimg : 1; io.Ec = h->Ec;
-  return io;
-}
-
-// rows per commit launch: one launch writes distinct transition slots and distinct frames
-int64_t commit_rows(const b2g_sac* h) { return std::min<int64_t>({(int64_t)h->stage_rows, h->cfg.buffer_capacity, h->frame_cap / 2}); }
-
-// Stores m <= commit_rows(h) transitions whose compact rows sit at io.c_obs / io.c_next: plans their frames, commits them and
-// copies act / rew / done (host or device memory) into the ring.  cand[i] >= 0 names a frame that already holds c_obs[i]: it
-// is shared while it outlives the allocation of this row's next_obs frame.  next_ids[i] receives the frame id of c_next[i].
-// h_plan must be free (the previous chunk's upload has run); everything is enqueued on h->stream.
-int commit_chunk(b2g_sac* h, const FrameIo& io, int m, const int64_t* cand, const float* act, const float* rew, const float* done,
-                 int64_t* next_ids) {
-  const int64_t cap = h->cfg.buffer_capacity, FC = h->frame_cap;
-  const size_t A = h->A;
-  const int64_t first = h->head_seq, fid0 = h->next_fid;
-  for (int i = 0; i < m; ++i) {
-    int64_t of, nf;
-    const bool share = h->add_transition(cap, cand[i], &of, &nf);
-    h->h_plan[i] = (int)(of % FC); h->h_plan[m + i] = share ? 0 : 1; h->h_plan[2 * m + i] = (int)(nf % FC);
-    next_ids[i] = nf;
-  }
-  if (h->dedup) CK(cudaMemcpyAsync(h->d_plan, h->h_plan, 3 * m * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  frame_commit_launch(io, h->dedup ? h->d_plan : nullptr, fid0, FC, m, h->r_ofr, h->r_nfr, first, cap, h->stream);
-  for (int64_t k = 0; k < m;) {          // act / rew / done into slots (first + k) % cap, in at most two pieces
-    const int64_t pos = (first + k) % cap, len = std::min<int64_t>(m - k, cap - pos);
-    CK(cudaMemcpyAsync(h->r_act + pos * A, act + k * A, len * A * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_rew + pos, rew + k, len * sizeof(float), cudaMemcpyDefault, h->stream));
-    CK(cudaMemcpyAsync(h->r_done + pos, done + k, len * sizeof(float), cudaMemcpyDefault, h->stream));
-    k += len;
-  }
-  return 0;
-}
-
-// After the last chunk of a call: the next call's sharing candidates, and the replay size / first live slot the sampler reads
-// (it draws u in [0, size) and reads slot (first live + u) % cap; the first live slot is 0 unless transitions went early).
-int commit_finish(b2g_sac* h, std::vector<int64_t>& next_ids) {
-  const int64_t cap = h->cfg.buffer_capacity;
-  h->prev_next.swap(next_ids);
-  h->r_size = h->head_seq - h->tail_seq;
-  h->h_rc[0] = h->r_size;
-  h->h_rc[1] = h->r_size == cap ? 0 : h->tail_seq % cap;
-  CK(cudaMemcpyAsync(h->counters + 5, h->h_rc, 2 * sizeof(long long), cudaMemcpyHostToDevice, h->stream));
-  return 0;
-}
-
 // n caller observations (host or device memory) -> rows (first + i) % wrap of dst in the ring layout, on h->stream.  CNN: copied in
 // pieces through the full-layout staging buffer and compacted (stream order frees the buffer for the next piece); MLP: a plain
 // copy, for which first + n <= wrap.
@@ -1040,21 +986,6 @@ int sac_act_rows(b2g_sac* h, const float* rows, int chunk, int deterministic) {
   }
   CK(b2g::act_launch(make_tail(h, false), chunk, deterministic, h->pi_out, h->stream));
   return 0;
-}
-
-int sac_replay_add_linked(b2g_sac* h, const float* c_obs, const float* c_next, const int64_t* obs_fid, const float* act,
-                          const float* rew, const float* done, int n, int64_t* next_fid) {
-  const int64_t R = commit_rows(h);
-  const size_t A = h->A, Ec = h->Ec;
-  std::vector<int64_t> next_ids((size_t)n);
-  for (int64_t c0 = 0; c0 < n; c0 += R) {
-    const int m = (int)std::min<int64_t>(R, n - c0);
-    if (c0 > 0) CK(cudaStreamSynchronize(h->stream));        // the previous chunk's plan upload has left h_plan
-    if (int rc = commit_chunk(h, frame_io(h, c_obs + c0 * Ec, c_next + c0 * Ec), m, obs_fid + c0, act + c0 * A, rew + c0, done + c0,
-                              next_ids.data() + c0)) return rc;
-  }
-  std::copy(next_ids.begin(), next_ids.end(), next_fid);
-  return commit_finish(h, next_ids);
 }
 
 }  // namespace b2g
@@ -1159,8 +1090,7 @@ int b2g_sac_destroy(b2g_sac* h) {
   for (int q = 0; q < 2; ++q) { if (h->hc_obs[q]) cudaFreeHost(h->hc_obs[q]); if (h->hc_next[q]) cudaFreeHost(h->hc_next[q]); }
   if (h->h_met) cudaFreeHost(h->h_met);
   if (h->h_cnt) cudaFreeHost(h->h_cnt);
-  if (h->h_plan) cudaFreeHost(h->h_plan);
-  if (h->h_rc) cudaFreeHost(h->h_rc);
+  h->replay.release();
   for (int k = 0; k < 2; ++k) { if (h->hp_stats[k]) cudaFreeHost(h->hp_stats[k]); if (h->ev_stats[k]) cudaEventDestroy(h->ev_stats[k]); }
   for (int j = 0; j < 2; ++j) {
     if (h->ev_h2d[j]) cudaEventDestroy(h->ev_h2d[j]);
@@ -1194,8 +1124,6 @@ int b2g_sac_create3(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, const 
     return b2g_fail(B2G_EINVAL, "B2G_CNN_NATURE is a CNN extractor: the MLP policy (obs_h == 0) has none");
   const bool nature = extractor == B2G_CNN_NATURE;
   const int n_img = nature ? cfg->obs_c : cfg->obs_c - 1;      // image planes conv1 reads
-  if (replay && replay->frame_capacity < cfg->buffer_capacity + 1)
-    return b2g_fail(B2G_EINVAL, "frame_capacity must be at least buffer_capacity + 1");
   if (replay && replay->u8_plane_mask && cfg->obs_h <= 0) return b2g_fail(B2G_EINVAL, "the MLP policy has no 8-bit image planes");
   if (replay && replay->u8_plane_mask && (n_img < 1 || n_img > 8 || (replay->u8_plane_mask >> n_img) != 0))
     return b2g_fail(B2G_EINVAL, nature ? "u8_plane_mask may only name image planes (below obs_c), at most 8"
@@ -1204,6 +1132,8 @@ int b2g_sac_create3(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, const 
     return b2g_fail(B2G_EINVAL, "hidden must be 64, 128, 192 or 256 (SAC.layers [H, H])");
   if (cfg->n_act < 1 || cfg->n_act > 8) return b2g_fail(B2G_EINVAL, "n_act must be in [1,8]");
   if (cfg->batch < 1 || cfg->buffer_capacity < 1) return b2g_fail(B2G_EINVAL, "batch and buffer_capacity must be positive");
+  const int64_t frame_cap = replay ? replay->frame_capacity : 2 * cfg->buffer_capacity;
+  if (int rc = check_frame_capacity(frame_cap, cfg->buffer_capacity, "frame_capacity")) return rc;
   if (cfg->nranks < 1 || cfg->rank < 0 || cfg->rank >= cfg->nranks) return b2g_fail(B2G_EINVAL, "bad rank/nranks");
   if (cfg->precision < B2G_PREC_FP32_SIMT || cfg->precision > B2G_PREC_BF16)
     return b2g_fail(B2G_EINVAL, "unknown precision mode");
@@ -1252,33 +1182,27 @@ int b2g_sac_create3(const b2g_sac_cfg* cfg, const b2g_replay_cfg* replay, const 
     h->v2.on = h->cnn && cfg->precision == B2G_PREC_BF16X3 && h->Hi == 64 && h->Wi == 64 && h->Cimg <= 4;
     if (const char* dbg = getenv("B2G_CG_DEBUG")) h->v2.dbg = atoi(dbg);
   }
+  h->stage_rows = std::max(B, 256);
   {   // frame formats: the fp32 compact row, and the replay frames (8-bit planes first, then the fp32 planes, then the tail)
     const int npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0, HW = h->Hi * h->Wi;
     h->row_fmt.n32 = h->Cimg; h->row_fmt.tail = 4 * npx;
     h->u8_mask = replay ? replay->u8_plane_mask : 0;
-    h->fmt = h->row_fmt;
-    h->frame_bytes = (int64_t)h->Ec * 4;
+    FrameIo lay{};
+    lay.fmt = h->row_fmt; lay.npx = npx; lay.Ci = h->cnn ? h->Cimg : 1; lay.Ec = h->Ec;
+    lay.frame_bytes = (int64_t)h->Ec * 4;       // the compact row itself (replay_budget.frame_bytes)
     if (h->u8_mask) {
-      FrameFmt& f = h->fmt;
+      FrameFmt& f = lay.fmt;
       f.n8 = f.n32 = 0;
       for (int c = 0; c < h->Cimg; ++c) f.ch[c] = (h->u8_mask >> c & 1) ? (signed char)f.n8++ : (signed char)(-1 - f.n32++);
       f.f32_off = HW * f.n8;
       f.tail = f.f32_off + 4 * HW * f.n32;
       if (f.f32_off % 16 != 0) return bail(b2g_fail(B2G_EINVAL, "8-bit planes need H * W * (8-bit planes) to be a multiple of 16"));
-      h->frame_bytes = (f.tail + 16 + 15) / 16 * 16;      // 16-byte frame stride: the gathers' 128-bit loads stay aligned
+      lay.frame_bytes = (f.tail + 16 + 15) / 16 * 16;      // 16-byte frame stride: the gathers' 128-bit loads stay aligned
     }
-    h->frame_cap = replay ? replay->frame_capacity : 2 * cap;
-    if (h->frame_cap > INT32_MAX) return bail(b2g_fail(B2G_EINVAL, "frame_capacity must fit in int32 (frame indices)"));
-    h->dedup = h->frame_cap < 2 * cap;     // at 2 cap every transition has two frames of its own: sharing would save nothing
+    h->replay.frames_name = "frame_capacity";
+    if ((rc = h->replay.init(h->allocs, h->stream, cap, h->E, h->A, B, false, 0.f, 0.f, frame_cap, lay, h->stage_rows))) return bail(rc);
   }
-  if ((rc = dev_alloc(h->allocs, h->stream, &h->frames, (size_t)(h->frame_cap * h->frame_bytes)))) return bail(rc);
-  DA(h->r_ofr, cap); DA(h->r_nfr, cap); DA(h->r_act, cap * h->A); DA(h->r_rew, cap); DA(h->r_done, cap);
-  h->stage_rows = std::max(B, 256);
   if (h->cnn) DA(h->obs_stage, (size_t)h->stage_rows * h->E);
-  DA(h->c_obs, (size_t)h->stage_rows * h->Ec); DA(h->c_next, (size_t)h->stage_rows * h->Ec); DA(h->d_plan, 4 * h->stage_rows);
-  if (cudaMallocHost((void**)&h->h_plan, 4 * h->stage_rows * sizeof(int)) != cudaSuccess ||
-      cudaMallocHost((void**)&h->h_rc, 2 * sizeof(long long)) != cudaSuccess)
-    return bail(b2g_fail(B2G_ECUDA, "replay staging"));
   DA(h->d_mean, h->Ec); DA(h->d_istd, h->Ec); DA(h->d_normc, 8);
   // obs_rms over the caller's layout; the plain nature_cnn's compact image block is the caller's observation itself: the flat table
   h->rms.E = h->E; h->rms.Cfull = h->direct_feature() ? h->Cobs : 0; h->rms.npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0;
@@ -1464,104 +1388,38 @@ int b2g_replay_add(b2g_sac* h, const float* obs, const float* act, const float* 
                    int64_t n) {
   B2G_USABLE(h);
   if (!h || !obs || !act || !rew || !next_obs || !done || n < 0) return b2g_fail(B2G_EINVAL, "NULL argument");
-  if (h->dedup && 2 * n > h->frame_cap) return b2g_fail(B2G_EINVAL, "replay_add: 2 n rows exceed frame_capacity");
   CK(cudaSetDevice(h->cfg.device));
-  const int64_t FC = h->frame_cap;
-  const int64_t R = commit_rows(h);
-  const size_t E = h->E, A = h->A;
-  const FrameIo io = frame_io(h, h->c_obs, h->c_next);
-  int* flags = h->h_plan + 3 * R;
-  // rows [c0, c0 + m) -> compact staging, then (when sharing frames or checking 8-bit values) frame_check -> flags, synchronised
-  auto stage_check = [&](int64_t c0, int m, bool check) -> int {
-    if (c0 > 0) CK(cudaStreamSynchronize(h->stream));        // the previous chunk's plan upload has left h_plan
-    if (int rc = load_rows(h, obs + c0 * E, h->c_obs, 0, R, m)) return rc;
-    if (int rc = load_rows(h, next_obs + c0 * E, h->c_next, 0, R, m)) return rc;
-    if (!check) return 0;
-    for (int i = 0; i < m; ++i) {      // candidate frame of row i: the previous call's next_obs of row i, while it still exists
-      const int64_t p = c0 + i < (int64_t)h->prev_next.size() ? h->prev_next[c0 + i] : -1;
-      h->h_plan[i] = h->dedup && p >= 0 && p > h->next_fid - FC ? (int)(p % FC) : -1;
-    }
-    CK(cudaMemcpyAsync(h->d_plan, h->h_plan, m * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    frame_check_launch(io, h->d_plan, h->d_plan + 3 * R, m, h->stream);
-    CK(cudaMemcpyAsync(flags, h->d_plan + 3 * R, m * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    for (int i = 0; i < m; ++i)
-      if (flags[i] & 2) return b2g_fail(B2G_EINVAL, "replay_add: a value of an 8-bit plane is not an integer in [0, 255]");
-    return 0;
-  };
-  // a call larger than the staging validates every row before it stores the first one
-  if (h->u8_mask && n > R)
-    for (int64_t c0 = 0; c0 < n; c0 += R)
-      if (int rc = stage_check(c0, (int)std::min<int64_t>(R, n - c0), true)) return rc;
-  std::vector<int64_t> next_ids((size_t)n), cand((size_t)R);
-  for (int64_t c0 = 0; c0 < n; c0 += R) {
-    const int m = (int)std::min<int64_t>(R, n - c0);
-    if (int rc = stage_check(c0, m, h->dedup || (h->u8_mask && n <= R))) return rc;
-    for (int i = 0; i < m; ++i) {      // the previous call's next_obs of row i, where frame_check found it equal bit for bit
-      const int64_t p = c0 + i < (int64_t)h->prev_next.size() ? h->prev_next[c0 + i] : -1;
-      cand[i] = h->dedup && (flags[i] & 1) ? p : -1;
-    }
-    if (int rc = commit_chunk(h, io, m, cand.data(), act + c0 * A, rew + c0, done + c0, next_ids.data() + c0)) return rc;
-  }
-  h->rms.up_other += (int64_t)(n * (2 * E + A + 2) * sizeof(float));
-  if (int rc = commit_finish(h, next_ids)) return rc;
-  CK(cudaStreamSynchronize(h->stream));     // host arrays are caller-owned: copied before return
+  auto load = [h](const float* src, float* dst, int m) { return load_rows(h, src, dst, 0, h->stage_rows, m); };
+  if (int rc = h->replay.add(obs, act, rew, next_obs, done, n, h->counters, h->stream, load)) return rc;
+  h->rms.up_other += (int64_t)(n * (2 * h->E + h->A + 2) * sizeof(float));
   return 0;
 }
 
-int64_t b2g_replay_size(const b2g_sac* h) { B2G_USABLE(h); return h ? h->r_size : 0; }
+int64_t b2g_replay_size(const b2g_sac* h) { B2G_USABLE(h); return h ? h->replay.size : 0; }
 
 int b2g_replay_info(const b2g_sac* h, int64_t* capacity, int64_t* size, int64_t* frame_capacity, int64_t* live_frames,
                     int64_t* bytes, int64_t* evicted_early) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  const int64_t cap = h->cfg.buffer_capacity;
-  if (capacity) *capacity = cap;
-  if (size) *size = h->r_size;
-  if (frame_capacity) *frame_capacity = h->frame_cap;
-  if (live_frames) *live_frames = h->live_frames();
-  if (bytes) *bytes = h->frame_cap * h->frame_bytes + cap * (int64_t)(2 * sizeof(int) + (h->A + 2) * sizeof(float));
-  if (evicted_early) *evicted_early = h->evicted;
+  h->replay.info(capacity, size, frame_capacity, live_frames, bytes, evicted_early);
   return 0;
 }
 
 int b2g_replay_get(b2g_sac* h, int64_t slot, float* obs, float* act, float* rew, float* next_obs, float* done) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  const int64_t cap = h->cfg.buffer_capacity;
-  if (slot < 0 || slot >= cap || ((slot - h->tail_seq % cap) % cap + cap) % cap >= h->r_size)
-    return b2g_fail(B2G_EINVAL, "replay slot is not live");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  const size_t A = h->A;
-  // expand the frames: for the CNN policy the actuator plane comes back as zeros except pixel [0,0] (all the policy reads of it)
-  std::vector<unsigned char> fr(h->frame_bytes);
-  const FrameFmt& fm = h->fmt;
-  const int npx = h->cnn ? h->Hi * h->Wi * h->Cimg : 0;
+  std::vector<float> row[2] = {std::vector<float>(obs ? h->Ec : 0), std::vector<float>(next_obs ? h->Ec : 0)};
+  if (int rc = h->replay.get(slot, obs ? row[0].data() : nullptr, act, rew, next_obs ? row[1].data() : nullptr, done, nullptr,
+                             h->cfg.device, h->stream))
+    return rc;
+  // the caller's layout: for the CNN policy the actuator plane comes back as zeros except pixel [0,0] (all the policy reads of it)
   for (int w = 0; w < 2; ++w) {
     float* dst = w ? next_obs : obs;
     if (!dst) continue;
-    int fi = 0;
-    CK(cudaMemcpy(&fi, (w ? h->r_nfr : h->r_ofr) + slot, sizeof(int), cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(fr.data(), h->frames + (size_t)fi * h->frame_bytes, h->frame_bytes, cudaMemcpyDeviceToHost));
     std::fill(dst, dst + h->E, 0.f);
-    for (int e = 0; e < h->Ec; ++e) {
-      const int f = full_index(h, e);
-      if (f < 0) continue;
-      float v;
-      if (e >= npx) memcpy(&v, fr.data() + fm.tail + 4 * (e - npx), 4);
-      else if (fm.n8 == 0) memcpy(&v, fr.data() + 4 * e, 4);
-      else {
-        const int pix = e / h->Cimg, k = fm.ch[e % h->Cimg];
-        if (k >= 0) v = (float)fr[pix * fm.n8 + k];
-        else memcpy(&v, fr.data() + fm.f32_off + 4 * (pix * fm.n32 - 1 - k), 4);
-      }
-      dst[f] = v;
-    }
+    for (int e = 0; e < h->Ec; ++e)
+      if (const int f = full_index(h, e); f >= 0) dst[f] = row[w][e];
   }
-  if (act) CK(cudaMemcpy(act, h->r_act + slot * A, A * sizeof(float), cudaMemcpyDeviceToHost));
-  if (rew) CK(cudaMemcpy(rew, h->r_rew + slot, sizeof(float), cudaMemcpyDeviceToHost));
-  if (done) CK(cudaMemcpy(done, h->r_done + slot, sizeof(float), cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -1625,7 +1483,7 @@ static int ensure_graph(b2g_sac* h) {
 int b2g_sac_step_async(b2g_sac* h, int n_steps, float lr) {
   B2G_USABLE(h);
   if (!h || n_steps < 0) return b2g_fail(B2G_EINVAL, "bad argument");
-  if (h->r_size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
+  if (h->replay.size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
   refresh_planes(h, true);
@@ -1864,7 +1722,7 @@ float b2g_last_step_ms(const b2g_sac* h) { B2G_USABLE(h); return h ? h->last_ms 
 int b2g_profile_step(b2g_sac* h, float lr, const char** names, float* ms, int cap) {
   B2G_USABLE(h);
   if (!h || !names || !ms) return b2g_fail(B2G_EINVAL, "NULL argument");
-  if (h->r_size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
+  if (h->replay.size < 1) return b2g_fail(B2G_ESTATE, "replay buffer is empty");
   CK(cudaSetDevice(h->cfg.device));
   if (int rc = upload_lr(h->d_lr, &h->cur_lr, lr, h->stream)) return rc;
   refresh_planes(h);
@@ -1894,7 +1752,7 @@ std::vector<FpField> sac_fingerprint(const b2g_sac* h) {
   const b2g_sac_cfg& c = h->cfg;
   return {fp_int("obs_h", c.obs_h), fp_int("obs_w", c.obs_w), fp_int("obs_c", c.obs_c), fp_int("obs_dim", c.obs_dim),
           fp_int("n_act", c.n_act), fp_int("hidden", c.hidden), fp_int("batch", c.batch),
-          fp_int("buffer_capacity", c.buffer_capacity), fp_int("frame_capacity", h->frame_cap),
+          fp_int("buffer_capacity", c.buffer_capacity), fp_int("frame_capacity", h->replay.ring.frame_cap),
           fp_int("u8_plane_mask", h->u8_mask), fp_real("gamma", c.gamma), fp_real("tau", c.tau),
           fp_real("target_entropy", c.target_entropy), fp_int("seed", (int64_t)c.seed)};
 }
@@ -1906,28 +1764,10 @@ std::vector<FpField> sac_fingerprint(const b2g_sac* h, int extractor) {
   return fp;
 }
 
-// frames [lo, hi) of the ring: at most two contiguous ranges, each stored at id % frame_cap
-std::vector<StatePiece> frame_pieces(b2g_sac* h, int64_t lo, int64_t hi) {
-  std::vector<StatePiece> v;
-  for (int64_t f = lo; f < hi;) {
-    const int64_t pos = f % h->frame_cap, n = std::min(hi - f, h->frame_cap - pos);
-    v.push_back(dev_piece(h->frames + pos * h->frame_bytes, (size_t)(n * h->frame_bytes)));
-    f += n;
-  }
-  return v;
-}
-
 // the sections 2.. (parameters .. frames, then obs_rms when the handle owns it) of a handle whose frame window is [lo, hi)
 std::vector<StateSection> sac_device_sections(b2g_sac* h, int64_t lo, int64_t hi) {
-  const size_t cap = (size_t)h->cfg.buffer_capacity;
   std::vector<StateSection> s = adam_sections(h->P, h->n_all, h->Mo, h->Vo, h->n_train);
-  s.resize(9);
-  s[3].tag = state_tag("ROFR"); s[3].pieces = {dev_piece(h->r_ofr, cap * sizeof(int))};
-  s[4].tag = state_tag("RNFR"); s[4].pieces = {dev_piece(h->r_nfr, cap * sizeof(int))};
-  s[5].tag = state_tag("RACT"); s[5].pieces = {dev_piece(h->r_act, cap * h->A * sizeof(float))};
-  s[6].tag = state_tag("RREW"); s[6].pieces = {dev_piece(h->r_rew, cap * sizeof(float))};
-  s[7].tag = state_tag("RDON"); s[7].pieces = {dev_piece(h->r_done, cap * sizeof(float))};
-  s[8].tag = state_tag("FRMS"); s[8].pieces = frame_pieces(h, lo, hi);
+  for (auto& r : h->replay.state_sections(0, lo, hi)) s.push_back(std::move(r));     // ROFR RNFR RACT RREW RDON FRMS
   if (h->rms.on()) s.push_back(rms_section(&h->rms.count, h->rms.mean, h->rms.var, h->E));
   return s;
 }
@@ -1949,9 +1789,10 @@ int b2g_sac_state_save(b2g_sac* h, const char* path) {
   if (h->aux) { CK(cudaStreamSynchronize(h->aux)); CK(cudaStreamSynchronize(h->aux2)); }
   long long cnt[8];
   CK(cudaMemcpy(cnt, h->counters, sizeof cnt, cudaMemcpyDeviceToHost));
-  std::vector<int64_t> hv = h->pack();     // FrameRing's bookkeeping (its size is r_size)
+  const FrameRing& ring = h->replay.ring;
+  std::vector<int64_t> hv = ring.pack();     // the replay's bookkeeping (its size is replay.size)
   std::vector<StateSection> secs = host_sections(hv.data(), hv.size() * sizeof(int64_t), cnt, sizeof cnt);
-  for (auto& s : sac_device_sections(h, h->frame_lo(), h->next_fid)) secs.push_back(std::move(s));
+  for (auto& s : sac_device_sections(h, ring.frame_lo(), ring.next_fid)) secs.push_back(std::move(s));
   return state_write(path, STATE_KIND_SAC, fp_with_rms(sac_fingerprint(h, h->extractor), h->rms.on()), secs);
 }
 
@@ -1975,13 +1816,12 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
     return b2g_fail(rc, msg);
   }
   if (int rc = state_check_tags(rd, sac_device_sections(h, 0, 0), "SAC")) return rc;
-  const int64_t cap = h->cfg.buffer_capacity, FC = h->frame_cap;
+  const int64_t cap = h->cfg.buffer_capacity, FC = h->replay.ring.frame_cap;
   if (rd.bytes(0) % 8 || rd.bytes(0) < 7 * 8 || rd.bytes(0) > (uint64_t)(7 + 2 * cap + 4 * FC) * 8)
     return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
   std::vector<int64_t> hv(rd.bytes(0) / 8);
   if (int rc = rd.read_host(0, hv.data(), hv.size() * 8)) return rc;
-  FrameRing hs;
-  hs.frame_cap = FC; hs.dedup = h->dedup;
+  FrameRing hs = h->replay.ring;
   if (!hs.unpack(hv.data(), hv.size(), cap)) return b2g_fail(B2G_EINVAL, "corrupt replay bookkeeping in the training-state file");
   const std::vector<StateSection> dev = sac_device_sections(h, hs.frame_lo(), hs.next_fid);
   if (int rc = state_check_lengths(rd, dev)) return rc;
@@ -1995,8 +1835,9 @@ int b2g_sac_state_load(b2g_sac* h, const char* path) {
     if (h->rms.on()) h->rms.derive(h->stream);
     h->ob_n = 0;       // staged observations name frames of the replaced replay: the next b2g_sac_observe_act stages anew
     CK(cudaMemcpy(h->counters, cnt, sizeof cnt, cudaMemcpyHostToDevice));
-    static_cast<FrameRing&>(*h) = hs;
-    h->r_size = hs.size();
+    h->replay.ring = hs;
+    h->replay.size = hs.size();
+    h->replay.pos = hs.head_seq % cap;
     // The BF16 weight planes follow the restored arena at the next step or act.  The captured step graphs (graph_exec, pipe_graph)
     // stay valid: their kernel parameters hold device pointers and configuration only, and the replay size, first live slot and
     // Philox step they depend on are read from the device counters restored above.

@@ -12,10 +12,10 @@
 #include "cg.cuh"
 #include "common.cuh"
 #include "enc_stage.cuh"
-#include "frame_ring.cuh"
 #include "host.cuh"
 #include "metrics_log.cuh"
 #include "obsnorm.cuh"
+#include "per.cuh"
 
 namespace b2g {
 struct Tensor {
@@ -95,17 +95,11 @@ int v2_launch(b2g_sac* h, const CgGroup& g, cudaStream_t s);
 // sac.cu hooks of the observe path (obsnorm.cu)
 // policy forward on `chunk` <= batch compact rows at `rows` (device), enqueued on h->stream; the actions land in h->pi_out
 int sac_act_rows(b2g_sac* h, const float* rows, int chunk, int deterministic);
-// n <= stage_rows transitions from device memory: compact rows c_obs / c_next, act / rew / done.  obs_fid[i] >= 0 names the
-// replay frame that already holds c_obs[i] (linked instead of stored while it is live and frames are shared); next_fid[i]
-// receives the frame id given to c_next[i].  Enqueues on h->stream; the caller synchronises it before it returns (h_plan and
-// h_rc are pinned and read by the copies enqueued here).
-int sac_replay_add_linked(b2g_sac* h, const float* c_obs, const float* c_next, const int64_t* obs_fid, const float* act,
-                          const float* rew, const float* done, int n, int64_t* next_fid);
 }  // namespace b2g
 
 using namespace b2g;   // (internal header: only library translation units include it)
 
-struct b2g_sac : FrameRing {         // FrameRing: the replay's frame and transition bookkeeping (frame_ring.cuh)
+struct b2g_sac {
   b2g_sac_cfg cfg{};
   bool cnn = false;
   int num_sms = 132;
@@ -123,18 +117,11 @@ struct b2g_sac : FrameRing {         // FrameRing: the replay's frame and transi
   // augmented_nature_cnn never reads the rest of it, custom_obs_policy.py:28-30; zero under B2G_CNN_NATURE) and 3 pad floats.  The explicit batch
   // (s_obs / s_next) and the pipelined staging (ps_obs / ps_next) hold such rows.
   int Ec = 0;
-  // Replay: a ring of cap transition slots {obs frame, next_obs frame, act, rew, done} over a pool of frame_cap frames (one
-  // compact row each, stored in format fmt); the frame and transition numbering is FrameRing's.
-  unsigned char* frames = nullptr;
-  int64_t frame_bytes = 0;
-  FrameFmt fmt{}, row_fmt{};         // frame format; format of an fp32 compact row (explicit batch, staging)
+  // Replay: a ring of cap transition slots {obs frame, next_obs frame, act, rew, done} over a pool of frames, one compact row
+  // each (per.cuh)
+  TransitionReplay replay;
+  FrameFmt row_fmt{};                // format of an fp32 compact row (explicit batch, staging)
   uint32_t u8_mask = 0;
-  int *r_ofr = nullptr, *r_nfr = nullptr;
-  float *r_act = nullptr, *r_rew = nullptr, *r_done = nullptr;
-  int64_t r_size = 0;
-  float *c_obs = nullptr, *c_next = nullptr;    // replay_add staging: compact rows [stage_rows][Ec]
-  int *d_plan = nullptr, *h_plan = nullptr;     // [4][stage_rows]: frame plan (3 rows) + check flags; h_plan pinned
-  long long* h_rc = nullptr;         // pinned: replay size, first live slot -> counters[5..6]
   float* obs_stage = nullptr;        // CNN: caller observations in the full layout [stage_rows][E] on their way to compact rows
   int stage_rows = 0;
   // normalisation, in the ring layout (pads: mean 0, istd 1)

@@ -208,6 +208,14 @@ class HandleLearner:
         _lib.check(self._fn("upload_bytes")(self.h, C.byref(a), C.byref(b)))
         return {"observe": int(a.value), "other": int(b.value)}
 
+    def replay_info(self) -> dict:
+        """SAC, BDQ and DQN handles: capacity, size, frame_capacity and live_frames (0 without frames), bytes (device memory
+        of the replay: rows or frames and frame indices, actions, rewards, dones), evicted_early."""
+        keys = ("capacity", "size", "frame_capacity", "live_frames", "bytes", "evicted_early")
+        vals = [C.c_int64() for _ in keys]
+        _lib.check(self._fn("replay_info")(self.h, *[C.byref(v) for v in vals]))
+        return {k: int(v.value) for k, v in zip(keys, vals)}
+
 
 class TransitionReplayLearner(HandleLearner):
     """The transition replay the BDQ and DQN handles share (include/b200grasp.h: b2g_bdq_create2, b2g_*_replay_info)."""
@@ -217,14 +225,6 @@ class TransitionReplayLearner(HandleLearner):
         """``frame_capacity``: keep obs / next_obs in a pool of that many frames (at least buffer_size + 1); None = two rows
         per slot."""
         return None if frame_capacity is None else _lib.ReplayCfg(int(frame_capacity), 0)
-
-    def replay_info(self) -> dict:
-        """capacity, size, frame_capacity and live_frames (0 without frames), bytes (device memory of the replay: rows or
-        frames and frame indices, actions, rewards, dones), evicted_early."""
-        keys = ("capacity", "size", "frame_capacity", "live_frames", "bytes", "evicted_early")
-        vals = [C.c_int64() for _ in keys]
-        _lib.check(self._fn("replay_info")(self.h, *[C.byref(v) for v in vals]))
-        return {k: int(v.value) for k, v in zip(keys, vals)}
 
     def replay_get(self, slot: int) -> dict:
         """The stored transition of a live slot: obs, act, rew, next_obs, done, and frames = its (obs, next_obs) frame ids
@@ -246,7 +246,7 @@ def transition_replay_bytes(buffer_size: int, obs_dim: int, act_width: int, fram
 class Learner(HandleLearner):
     _abi = "sac"
     _names = {n: "b2g_" + n for n in ("get_param", "set_param", "get_grad", "set_norm_stats", "obs_rms_set", "obs_rms_get",
-                                      "upload_bytes")}
+                                      "upload_bytes", "replay_info")}
 
     def __init__(self, obs_shape: Sequence[int], n_act: int = 5, hidden: int = 64, batch_size: int = 64,
                  buffer_size: int = 100000, gamma: float = 0.99, tau: float = 0.005,
@@ -352,13 +352,6 @@ class Learner(HandleLearner):
 
     def replay_size(self) -> int:
         return int(self.lib.b2g_replay_size(self.h))
-
-    def replay_info(self) -> dict:
-        """capacity, size, frame_capacity, live_frames, bytes (device memory of the replay), evicted_early."""
-        keys = ("capacity", "size", "frame_capacity", "live_frames", "bytes", "evicted_early")
-        vals = [C.c_int64() for _ in keys]
-        _lib.check(self.lib.b2g_replay_info(self.h, *[C.byref(v) for v in vals]))
-        return {k: int(v.value) for k, v in zip(keys, vals)}
 
     def replay_get(self, slot: int) -> dict:
         """One stored (raw) transition, like ``ReplayBuffer.storage[slot]``."""
