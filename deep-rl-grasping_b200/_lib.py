@@ -32,6 +32,8 @@ SYMBOLS = [
     "b2g_dqn_get_grad", "b2g_dqn_replay_add", "b2g_dqn_replay_size", "b2g_dqn_set_norm_stats", "b2g_dqn_step",
     "b2g_dqn_step_explicit", "b2g_dqn_set_per_beta", "b2g_dqn_get_last_per", "b2g_dqn_update_target", "b2g_dqn_act",
     "b2g_dqn_state_save", "b2g_dqn_state_load",
+    "b2g_dqn_observe_act", "b2g_dqn_observe_add", "b2g_dqn_act_raw", "b2g_dqn_obs_rms_set", "b2g_dqn_obs_rms_get",
+    "b2g_dqn_upload_bytes", "b2g_dqn_set_obs_encoder",
     "b2g_ppo_create", "b2g_ppo_destroy", "b2g_ppo_param_count", "b2g_ppo_param_info", "b2g_ppo_get_param", "b2g_ppo_set_param",
     "b2g_ppo_get_grad", "b2g_ppo_rollout_act", "b2g_ppo_rollout_reward", "b2g_ppo_rollout_reset", "b2g_ppo_rollout_get",
     "b2g_ppo_update", "b2g_ppo_train_step_explicit", "b2g_ppo_act", "b2g_ppo_get_step", "b2g_ppo_state_save", "b2g_ppo_state_load",
@@ -293,7 +295,13 @@ def load():
     lib.b2g_dqn_step.argtypes = [vp, C.c_int, C.c_float, C.POINTER(DqnMetrics)]
     lib.b2g_dqn_step_explicit.argtypes = [vp, fp, fp, fp, fp, fp, fp, C.c_float, C.c_int, C.POINTER(DqnMetrics), fp]
     lib.b2g_dqn_update_target.argtypes = [vp]
-    lib.b2g_dqn_act.argtypes = [vp, fp, C.c_int, C.POINTER(C.c_int32), fp]
+    lib.b2g_dqn_act.argtypes = lib.b2g_dqn_act_raw.argtypes = [vp, fp, C.c_int, C.POINTER(C.c_int32), fp]
+    lib.b2g_dqn_observe_act.argtypes = [vp, fp, C.c_int, C.c_int, C.c_float, C.POINTER(C.c_int32)]
+    lib.b2g_dqn_observe_add.argtypes = [vp, fp, fp, fp, fp, fp, C.c_int, C.c_int]
+    lib.b2g_dqn_obs_rms_set.argtypes = [vp, dp, dp, C.c_double]
+    lib.b2g_dqn_obs_rms_get.argtypes = [vp, dp, dp, dp]
+    lib.b2g_dqn_upload_bytes.argtypes = [vp, i64p, i64p]
+    lib.b2g_dqn_set_obs_encoder.argtypes = [vp, vp, C.c_int]
     lib.b2g_ppo_create.argtypes = [C.POINTER(PpoCfg), C.POINTER(vp)]
     lib.b2g_ppo_rollout_act.argtypes = [vp, fp, fp]
     lib.b2g_ppo_rollout_reward.argtypes = [vp, fp, fp]

@@ -11,9 +11,10 @@
 // Output-layer weights are held with their row stride padded to 4 floats (n_bins = 33 -> 36) so every
 // operand row is 16-byte aligned; get/set repack to the zip layout.
 // The replay, normalisation, step, training-state and metrics-log plumbing is the QLearner base shared with DQN (q_learner.cu).
-// With device statistics (b2g_bdq_obs_rms_set) the learn loop's actor side runs here too: b2g_bdq_observe_act / _add stage each
-// new frame once, merge it into VecNormalize's obs_rms (ObsRms, obsnorm.cuh, shared with SAC), act epsilon-greedily on the
-// device (Philox stream 3) and commit transitions into the replay with a kernel.
+// With device statistics (b2g_bdq_obs_rms_set) the learn loop's actor side runs here too, on the observe path of the QLearner
+// base (q_learner.cu, shared with DQN): b2g_bdq_observe_act / _add stage each new frame once, merge it into VecNormalize's
+// obs_rms (ObsRms, obsnorm.cuh, shared with SAC), act epsilon-greedily on the device (Philox stream 3, bdq_explore_kernel) and
+// commit transitions into the replay with a kernel.
 #include <cuda_runtime.h>
 #include <math.h>
 
@@ -131,23 +132,6 @@ __global__ void bdq_explore_kernel(const float* const* A, int rows, int row0, in
   }
 }
 
-// b2g_bdq_observe_add: transition i = (cur[i], act[i], rew[i], nxt[i], done[i]) -> replay slot (first + i) % cap, one CTA per
-// row; CTA 0 also writes the new replay size into counters[5] (what b2g_bdq_replay_add uploads)
-__global__ void bdq_commit_kernel(const float* __restrict__ cur, const float* __restrict__ nxt, const float* __restrict__ act,
-                                  const float* __restrict__ rew, const float* __restrict__ done, int E, int D, long long first, long long cap,
-                                  float* __restrict__ r_obs, float* __restrict__ r_next, float* __restrict__ r_act, float* __restrict__ r_rew,
-                                  float* __restrict__ r_done, long long* counters, long long new_size) {
-  const int i = blockIdx.x;
-  const long long slot = (first + i) % cap;
-  for (int e = threadIdx.x; e < E; e += blockDim.x) {
-    r_obs[slot * E + e] = cur[(size_t)i * E + e];
-    r_next[slot * E + e] = nxt[(size_t)i * E + e];
-  }
-  if (threadIdx.x < D) r_act[slot * D + threadIdx.x] = act[(size_t)i * D + threadIdx.x];
-  if (threadIdx.x == 0) { r_rew[slot] = rew[i]; r_done[slot] = done[i]; }
-  if (i == 0 && threadIdx.x == 0) counters[5] = new_size;
-}
-
 // hard target copy every `freq` updates, decided on the device so that the step can live in a CUDA graph
 __global__ void bdq_target_copy_kernel(float* __restrict__ P, long long n_train, const long long* __restrict__ counters, int freq) {
   if (freq <= 0 || counters[3] % freq != 0) return;
@@ -162,16 +146,6 @@ struct b2g_bdq : QLearner {     // A = D: one bin per branch
   float *dA[8]{}, *dV = nullptr, *dcat = nullptr, *dh2 = nullptr, *dh1 = nullptr;
   const float** d_Aptr = nullptr;
   void* nccl_comm = nullptr;
-  ObsRms rms;                  // device VecNormalize statistics (b2g_bdq_obs_rms_set), upload counts, observation encoder
-  // b2g_bdq_observe_act / _add staging (allocated on first use): the current observation of env i as a row of ob_rows[ob_k] (the
-  // other buffer takes the next call's next_obs), the reset frames of finished envs, and the call's actions / rewards / done flags.
-  int stage_rows = 0;          // max(batch, 256) envs per observe call
-  float* ob_rows[2]{};         // [stage_rows + B][E] (the actor's gather reads B rows from any chunk start)
-  float* ob_reset = nullptr;   // [stage_rows][E]
-  float *ob_act = nullptr, *ob_rew = nullptr, *ob_done = nullptr;
-  int* ob_idx = nullptr;       // [stage_rows][D] actor output
-  int ob_k = 0, ob_n = 0;
-  std::vector<int64_t> ob_fid;  // replay with frames: frame id holding env i's staged observation (-1: not stored yet)
 };
 
 namespace {
@@ -341,7 +315,6 @@ int b2g_bdq_destroy(b2g_bdq* h) {
   // the step graph first: with nranks > 1 it holds a captured all-reduce, whose resources NCCL reclaims through the communicator
   if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
   nccl_comm_destroy(h->nccl_comm);
-  enc_stage_destroy(h->rms.enc);
   ql_release(h);
   delete h;
   return 0;
@@ -370,7 +343,7 @@ int b2g_bdq_create2(const b2g_bdq_cfg* cfg, const b2g_replay_cfg* replay, b2g_bd
   h->per_alpha = cfg->per_alpha; h->per_eps = cfg->per_eps;
   h->D = cfg->n_branches; h->n = cfg->n_bins; h->NBS = (cfg->n_bins + 3) / 4 * 4;
   h->T0 = cfg->trunk0; h->T1 = cfg->trunk1; h->HB = cfg->branch_hidden;
-  h->stage_rows = std::max(cfg->batch, 256);
+  h->abi = "bdq";
   auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_bdq_destroy(h); g_b2g_err = keep; return rc; };
   // parameter inventory: same names and order as the zips (oracle/bdq_ref.py all_specs)
   h->params.add_scalar("bdq/eps", &h->eps_value);
@@ -393,7 +366,7 @@ int b2g_bdq_create2(const b2g_bdq_cfg* cfg, const b2g_replay_cfg* replay, b2g_bd
   h->params.add_copies(1, h->params.count() - 1, "bdq/model", "bdq/target_q_func/model", h->n_train);
   int rc = 0;
   const int B = h->B, D = h->D;
-  if ((rc = ql_init(h, MET_COUNT, replay, h->stage_rows))) return bail(rc);     // the metrics ride the all-reduce in G
+  if ((rc = ql_init(h, MET_COUNT, replay, std::max(cfg->batch, 256)))) return bail(rc);     // the metrics ride the all-reduce in G
 #define BA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
   for (int e = 0; e < 3; ++e) {
     BA(h->h1[e], B * h->T0); BA(h->h2[e], B * h->T1); BA(h->hv[e], B * h->HB); BA(h->Vout[e], B * 4);
@@ -410,7 +383,7 @@ int b2g_bdq_create2(const b2g_bdq_cfg* cfg, const b2g_replay_cfg* replay, b2g_bd
         cudaStreamSynchronize(h->stream) != cudaSuccess)
       return bail(b2g_fail(B2G_ECUDA, "init copies"));
   }
-  h->rms.E = h->E; h->rms.d_mean = h->d_mean; h->rms.d_istd = h->d_istd; h->rms.set_call = "b2g_bdq_obs_rms_set";
+  h->rms.set_call = "b2g_bdq_obs_rms_set";
   if ((rc = build(h))) return bail(rc);
   if (cfg->nranks > 1) {
     if ((rc = nccl_comm_init(&h->nccl_comm, cfg->nranks, cfg->nccl_id, cfg->rank, cfg->nccl_lib))) return bail(rc);
@@ -494,24 +467,7 @@ int b2g_bdq_upload_bytes(const b2g_bdq* h, int64_t* observe_bytes, int64_t* othe
 int b2g_bdq_set_obs_encoder(b2g_bdq* h, const b2g_encoder* enc, int tail) {
   B2G_USABLE(h);
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
-  if (enc)
-    if (int rc = obs_rms_check_encoder(h, enc, tail)) return rc;
-  return obs_rms_attach_encoder(h, enc, tail);
-}
-
-static int bdq_observe_checks(b2g_bdq* h, int n, int update_stats) {
-  if (n < 1 || n > h->stage_rows)
-    return b2g_fail(B2G_EINVAL, "observe: n must be in [1, " + std::to_string(h->stage_rows) + "] (the staging holds max(batch, 256) frames)");
-  if (update_stats && !h->rms.on()) return b2g_fail(B2G_ESTATE, "update_stats needs device statistics: call b2g_bdq_obs_rms_set first");
-  if (h->ob_rows[0]) return 0;
-  const size_t R = h->stage_rows, E = h->E;
-  for (int k = 0; k < 2; ++k)
-    if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_rows[k], (R + h->B) * E)) return rc;
-  if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_reset, R * E)) return rc;
-  if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_act, R * h->D)) return rc;
-  if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_rew, R)) return rc;
-  if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_done, R)) return rc;
-  return dev_alloc(h->allocs, h->stream, &h->ob_idx, R * h->D);
+  return ql_set_obs_encoder(h, enc, tail);
 }
 
 int b2g_bdq_observe_act(b2g_bdq* h, const float* obs, int n, int update_stats, float eps, int32_t* act_idx_out) {
@@ -519,19 +475,8 @@ int b2g_bdq_observe_act(b2g_bdq* h, const float* obs, int n, int update_stats, f
   if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
   if (!obs && !act_idx_out) return b2g_fail(B2G_EINVAL, "observe_act: nothing to do (obs and act_idx_out are NULL)");
   if (act_idx_out && !(eps >= 0.f && eps <= 1.f)) return b2g_fail(B2G_EINVAL, "observe_act: eps must be in [0, 1]");
-  CK(cudaSetDevice(h->device));
-  if (int rc = bdq_observe_checks(h, n, obs ? update_stats : 0)) return rc;
-  if (!obs && h->ob_n == 0) return b2g_fail(B2G_ESTATE, "observe_act: no staged observations (pass obs first)");
-  if (!obs && n != h->ob_n) return b2g_fail(B2G_EINVAL, "observe_act: n differs from the number of staged observations");
-  const size_t E = h->E, D = h->D;
-  float* cur = h->ob_rows[h->ob_k];
-  if (obs) {
-    if (int rc = h->rms.stage_frames(cur, obs, n, h->stream)) return rc;
-    if (update_stats) h->rms.merge(cur, nullptr, nullptr, n, h->stream);
-    h->ob_n = n;
-    h->ob_fid.assign((size_t)n, -1);
-  }
-  if (act_idx_out) {
+  return ql_observe_act(h, obs, n, update_stats, act_idx_out != nullptr, [&](const float* cur) {
+    const size_t E = h->E, D = h->D;
     const unsigned long long seed = h->philox_key();
     for (int k = 0; k < n; k += h->B) {
       const int chunk = std::min(h->B, n - k);
@@ -542,60 +487,15 @@ int b2g_bdq_observe_act(b2g_bdq* h, const float* obs, int n, int update_stats, f
       bdq_explore_kernel<<<1, 256, 0, h->stream>>>(h->d_Aptr, chunk, k, (int)D, h->n, h->NBS, eps, seed, h->counters, k + chunk >= n, h->ob_idx);
     }
     CK(cudaMemcpyAsync(act_idx_out, h->ob_idx, n * D * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
-  }
-  CK(cudaStreamSynchronize(h->stream));     // caller-owned arrays are copied, the actions are the result of the call
-  CK(cudaGetLastError());
-  return 0;
+    return 0;
+  });
 }
 
 int b2g_bdq_observe_add(b2g_bdq* h, const float* act_idx, const float* rew, const float* next_obs, const float* done, const float* reset_obs,
                         int n, int update_stats) {
   B2G_USABLE(h);
   if (!h || !act_idx || !rew || !next_obs || !done) return b2g_fail(B2G_EINVAL, "NULL argument");
-  CK(cudaSetDevice(h->device));
-  if (int rc = bdq_observe_checks(h, n, update_stats)) return rc;
-  if (h->ob_n == 0) return b2g_fail(B2G_ESTATE, "observe_add: no staged observations (call b2g_bdq_observe_act first)");
-  if (n != h->ob_n) return b2g_fail(B2G_EINVAL, "observe_add: n differs from the number of staged observations");
-  if (n > h->buffer_capacity) return b2g_fail(B2G_EINVAL, "observe_add: n exceeds buffer_capacity");
-  if (h->replay.ring.dedup && 2 * (int64_t)n > h->replay.ring.frame_cap)
-    return b2g_fail(B2G_EINVAL, "observe_add: 2 n rows exceed frame_capacity (replay_frames)");
-  int n_done = 0;
-  for (int i = 0; i < n; ++i) n_done += done[i] != 0.f;
-  if (n_done && !reset_obs) return b2g_fail(B2G_EINVAL, "observe_add: an env finished but reset_obs is NULL");
-  const size_t E = h->E, D = h->D, fb = E * sizeof(float);
-  float* cur = h->ob_rows[h->ob_k];
-  float* nxt = h->ob_rows[h->ob_k ^ 1];
-  if (int rc = h->rms.stage_frames(nxt, next_obs, n, h->stream)) return rc;
-  if (int rc = h->rms.upload(h->ob_act, act_idx, n * D * sizeof(float), h->stream)) return rc;
-  if (int rc = h->rms.upload(h->ob_rew, rew, n * sizeof(float), h->stream)) return rc;
-  if (int rc = h->rms.upload(h->ob_done, done, n * sizeof(float), h->stream)) return rc;
-  if (n_done)
-    if (int rc = h->rms.stage_reset_frames(h->ob_reset, reset_obs, done, h->ob_done, n, n_done, h->stream)) return rc;
-  // the transitions: obs = the staged rows, next_obs = the uploaded rows (a finished env's terminal frame)
-  TransitionReplay& rp = h->replay;
-  if (rp.framed()) {
-    // env i's staged row is the frame its previous transition's next_obs took, unless the env was reset since: shared without
-    // comparing; a reset frame (ob_fid -1) takes a frame of its own here, when it is first used as obs
-    std::vector<int64_t> next_ids((size_t)n);
-    if (int rc = rp.add_linked(cur, nxt, h->ob_fid.data(), h->ob_act, h->ob_rew, h->ob_done, n, next_ids.data(), h->counters, h->stream))
-      return rc;
-    for (int i = 0; i < n; ++i) h->ob_fid[i] = done[i] != 0.f ? -1 : next_ids[i];
-  } else {
-    const int64_t new_size = std::min<int64_t>(rp.cap, rp.size + n);
-    bdq_commit_kernel<<<n, 256, 0, h->stream>>>(cur, nxt, h->ob_act, h->ob_rew, h->ob_done, (int)E, (int)D, rp.pos, rp.cap, rp.obs, rp.next,
-                                                rp.act, rp.rew, rp.done, h->counters, new_size);
-    rp.insert_max_prio(rp.pos, n, h->stream);     // as in b2g_bdq_replay_add
-  }
-  // VecNormalize's step_wait merges the frames the VecEnv returned: a finished env's reset frame, not its terminal observation
-  if (update_stats) h->rms.merge(nxt, n_done ? h->ob_reset : nullptr, h->ob_done, n, h->stream);
-  // the new rows become the current observations; a finished env continues from the frame its reset returned
-  for (int i = 0; i < n; ++i)
-    if (done[i] != 0.f) CK(cudaMemcpyAsync(nxt + i * E, h->ob_reset + i * E, fb, cudaMemcpyDeviceToDevice, h->stream));
-  if (!rp.framed()) rp.advance(n);
-  h->ob_k ^= 1;
-  CK(cudaStreamSynchronize(h->stream));     // host arrays are caller-owned: copied before return
-  CK(cudaGetLastError());
-  return 0;
+  return ql_observe_add(h, act_idx, rew, next_obs, done, reset_obs, n, update_stats, nullptr);
 }
 
 }  // extern "C"

@@ -13,6 +13,9 @@
 // b2g_dqn_set_norm_stats (raw transitions are stored); the actor (b2g_dqn_act) takes observations as the network sees them, the
 // VecNormalize wrapper's output, as stable-baselines' act and predict do.  The replay, normalisation, step, training-state and
 // metrics-log plumbing is the QLearner base shared with BDQ (q_learner.cu).
+// With device statistics (b2g_dqn_obs_rms_set) the learn loop's actor side runs here too, on the observe path BDQ shares
+// (q_learner.cu): b2g_dqn_observe_act / _add stage each new frame once, merge it into VecNormalize's obs_rms, act
+// epsilon-greedily on the device (Philox stream 3, dqn_explore_kernel) and commit the transitions into the replay.
 #include <cuda_runtime.h>
 #include <math.h>
 
@@ -140,6 +143,27 @@ __global__ void dqn_act_kernel(const float* __restrict__ A, const float* __restr
   out[b] = q_argmax(a, v, mean, n);
   if (q_out)
     for (int k = 0; k < n; ++k) q_out[(size_t)b * n + k] = v + (a[k] - mean);
+}
+// The epsilon-greedy actor of b2g_dqn_observe_act on `rows` evaluated rows (env row0 + b): the greedy action of dqn_act_kernel
+// and, with probability eps, a uniform random action instead.  Philox stream 3 at step counters[7] (the number of earlier
+// acting observe_act calls), block row0 + b: lane x decides ((x + 0.5) 2^-32 < eps in float64, so eps = 0 never explores and
+// eps = 1 always does), lane y picks the action (y * n) >> 32 -- bdq_explore_kernel's rule with one branch.  One CTA; the last
+// chunk of a call advances the counter.
+__global__ void dqn_explore_kernel(const float* __restrict__ A, const float* __restrict__ V, int rows, int row0, int n, int NAS, float eps,
+                                   unsigned long long seed, long long* counters, int advance, int* __restrict__ out) {
+  const unsigned long long step = (unsigned long long)counters[7];
+  const uint2 key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
+  for (int b = threadIdx.x; b < rows; b += blockDim.x) {
+    const float* a = A + (size_t)b * NAS;
+    const int best = q_argmax(a, V[(size_t)b * 4], row_mean(a, n), n);
+    const uint4 r = philox4x32_10(make_uint4((unsigned)step, (unsigned)(step >> 32), (unsigned)(row0 + b), 3u), key);
+    const bool explore = ((double)r.x + 0.5) * (1.0 / 4294967296.0) < (double)eps;
+    out[row0 + b] = explore ? (int)(((unsigned long long)r.y * (unsigned)n) >> 32) : best;
+  }
+  if (advance) {
+    __syncthreads();
+    if (threadIdx.x == 0) counters[7] = (long long)step + 1;
+  }
 }
 }  // namespace
 
@@ -318,6 +342,7 @@ int b2g_dqn_create2(const b2g_dqn_cfg* cfg, const b2g_replay_cfg* replay, b2g_dq
   h->per_alpha = cfg->per_alpha; h->per_eps = cfg->per_eps;
   h->n = cfg->n_actions; h->NAS = (cfg->n_actions + 3) / 4 * 4;
   h->H0 = cfg->hidden0; h->H1 = cfg->hidden1;
+  h->abi = "dqn";
   auto bail = [&](int rc) { std::string keep = g_b2g_err; b2g_dqn_destroy(h); g_b2g_err = keep; return rc; };
   // parameter inventory in zip order (oracle/dqn_ref.py all_specs)
   h->params.add_scalar("deepq/eps", &h->eps_value);
@@ -336,6 +361,7 @@ int b2g_dqn_create2(const b2g_dqn_cfg* cfg, const b2g_replay_cfg* replay, b2g_dq
   int rc = 0;
   const int B = h->B;
   if ((rc = ql_init(h, 0, replay, std::max(B, 256)))) return bail(rc);
+  h->rms.set_call = "b2g_dqn_obs_rms_set";
 #define DA(ptr, count) if ((rc = dev_alloc(h->allocs, h->stream, &(ptr), (size_t)(count)))) return bail(rc)
   DA(h->d_normc_act, 8);
   for (int e = 0; e < 3; ++e) {
@@ -388,7 +414,9 @@ static int dqn_check_actions(const b2g_dqn* h, const float* act, int64_t n) {
 }
 
 int b2g_dqn_replay_add(b2g_dqn* h, const float* obs, const float* act, const float* rew, const float* next_obs, const float* done, int64_t n) {
-  return ql_replay_add(h, obs, act, rew, next_obs, done, n, [&] { return dqn_check_actions(h, act, n); });
+  if (int rc = ql_replay_add(h, obs, act, rew, next_obs, done, n, [&] { return dqn_check_actions(h, act, n); })) return rc;
+  h->rms.up_other += (int64_t)(n * (2 * h->E + 3) * sizeof(float) + sizeof(long long));
+  return 0;
 }
 int64_t b2g_dqn_replay_size(const b2g_dqn* h) { return ql_replay_size(h); }
 int b2g_dqn_replay_info(const b2g_dqn* h, int64_t* capacity, int64_t* size, int64_t* frame_capacity, int64_t* live_frames, int64_t* bytes,
@@ -400,7 +428,7 @@ int b2g_dqn_replay_get(b2g_dqn* h, int64_t slot, float* obs, float* act, float* 
 }
 int b2g_dqn_set_norm_stats(b2g_dqn* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs, double clip_rew, double eps,
                            int norm_obs, int norm_reward) {
-  return ql_set_norm_stats(h, nullptr, obs_mean, obs_var, ret_var, clip_obs, clip_rew, eps, norm_obs, norm_reward);
+  return ql_set_norm_stats(h, h ? &h->rms : nullptr, obs_mean, obs_var, ret_var, clip_obs, clip_rew, eps, norm_obs, norm_reward);
 }
 int b2g_dqn_step(b2g_dqn* h, int n_steps, float lr, b2g_dqn_metrics* out) {
   if (int rc = ql_step(h, n_steps, lr, [h] { return dqn_issue(h, true, true, nullptr); })) return rc;
@@ -426,16 +454,17 @@ int b2g_dqn_update_target(b2g_dqn* h) {
   return 0;
 }
 
-int b2g_dqn_act(b2g_dqn* h, const float* obs, int n, int32_t* act_out, float* q_out) {
-  B2G_USABLE(h);
-  if (!h || !obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+namespace {
+// b2g_dqn_act (normc = the identity d_normc_act) and b2g_dqn_act_raw (normc = the gather's d_normc over obs_rms's table)
+int dqn_act_rows(b2g_dqn* h, const float* obs, int n, int32_t* act_out, float* q_out, const double* normc) {
   CK(cudaSetDevice(h->device));
   const size_t E = h->E;
   for (int done_n = 0; done_n < n; done_n += h->B) {
     const int chunk = std::min(h->B, n - done_n);
     CK(cudaMemcpyAsync(h->s_obs, obs + (size_t)done_n * E, chunk * E * sizeof(float), cudaMemcpyDefault, h->stream));
+    h->rms.up_other += (int64_t)(chunk * E * sizeof(float));
     GatherArgs g = ql_gather(h, false, false);
-    g.normc = h->d_normc_act;
+    g.normc = normc;
     gather_launch(g, h->stream);
     for (auto& gr : h->act) gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
     dqn_act_kernel<<<(chunk + 127) / 128, 128, 0, h->stream>>>(h->Aout[0], h->Vout[0], chunk, h->n, h->NAS, h->act_idx_out,
@@ -447,6 +476,65 @@ int b2g_dqn_act(b2g_dqn* h, const float* obs, int n, int32_t* act_out, float* q_
   }
   CK(cudaGetLastError());
   return 0;
+}
+}  // namespace
+
+int b2g_dqn_act(b2g_dqn* h, const float* obs, int n, int32_t* act_out, float* q_out) {
+  B2G_USABLE(h);
+  if (!h || !obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  return dqn_act_rows(h, obs, n, act_out, q_out, h->d_normc_act);
+}
+
+int b2g_dqn_act_raw(b2g_dqn* h, const float* obs, int n, int32_t* act_out, float* q_out) {
+  B2G_USABLE(h);
+  if (!h || !obs || !act_out || n < 0) return b2g_fail(B2G_EINVAL, "bad argument");
+  if (!h->rms.on()) return b2g_fail(B2G_ESTATE, "act_raw normalises with the device statistics: call b2g_dqn_obs_rms_set first");
+  return dqn_act_rows(h, obs, n, act_out, q_out, h->d_normc);
+}
+
+// ------------------------------------------------------------------------------------------------ obs_rms on the device and the
+// actor loop fed from one upload per frame (the QLearner observe path, q_learner.cu; the templates of obsnorm.cuh read the
+// QLearner view of device and nranks)
+int b2g_dqn_obs_rms_set(b2g_dqn* h, const double* mean, const double* var, double count) {
+  return obs_rms_set(static_cast<QLearner*>(h), mean, var, count);
+}
+int b2g_dqn_obs_rms_get(b2g_dqn* h, double* mean, double* var, double* count) { return obs_rms_get(static_cast<QLearner*>(h), mean, var, count); }
+int b2g_dqn_upload_bytes(const b2g_dqn* h, int64_t* observe_bytes, int64_t* other_bytes) {
+  return obs_rms_upload_bytes(static_cast<const QLearner*>(h), observe_bytes, other_bytes);
+}
+
+int b2g_dqn_set_obs_encoder(b2g_dqn* h, const b2g_encoder* enc, int tail) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  return ql_set_obs_encoder(h, enc, tail);
+}
+
+int b2g_dqn_observe_act(b2g_dqn* h, const float* obs, int n, int update_stats, float eps, int32_t* act_out) {
+  B2G_USABLE(h);
+  if (!h) return b2g_fail(B2G_EINVAL, "NULL handle");
+  if (!obs && !act_out) return b2g_fail(B2G_EINVAL, "observe_act: nothing to do (obs and act_out are NULL)");
+  if (act_out && !(eps >= 0.f && eps <= 1.f)) return b2g_fail(B2G_EINVAL, "observe_act: eps must be in [0, 1]");
+  return ql_observe_act(h, obs, n, update_stats, act_out != nullptr, [&](const float* cur) {
+    const unsigned long long seed = h->philox_key();
+    for (int k = 0; k < n; k += h->B) {      // the act groups in chunks of batch rows, normalised with the gather's table
+      const int chunk = std::min(h->B, n - k);
+      GatherArgs g = ql_gather(h, false, false);
+      g.obs = cur + (size_t)k * h->E;
+      gather_launch(g, h->stream);
+      for (auto& gr : h->act) gg_simt_launch(gr.dev, (int)gr.host.size(), gr.total_tiles, h->stream);
+      dqn_explore_kernel<<<1, 256, 0, h->stream>>>(h->Aout[0], h->Vout[0], chunk, k, h->n, h->NAS, eps, seed, h->counters, k + chunk >= n,
+                                                   h->ob_idx);
+    }
+    CK(cudaMemcpyAsync(act_out, h->ob_idx, n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+    return 0;
+  });
+}
+
+int b2g_dqn_observe_add(b2g_dqn* h, const float* act, const float* rew, const float* next_obs, const float* done, const float* reset_obs,
+                        int n, int update_stats) {
+  B2G_USABLE(h);
+  if (!h || !act || !rew || !next_obs || !done) return b2g_fail(B2G_EINVAL, "NULL argument");
+  return ql_observe_add(h, act, rew, next_obs, done, reset_obs, n, update_stats, [&] { return dqn_check_actions(h, act, n); });
 }
 
 }  // extern "C"
@@ -468,11 +556,12 @@ std::vector<FpField> dqn_fingerprint(const b2g_dqn* h) {
 extern "C" {
 
 int b2g_dqn_state_save(b2g_dqn* h, const char* path) {
-  return ql_state_save(h, path, STATE_KIND_DQN, h ? dqn_fingerprint(h) : std::vector<FpField>{}, nullptr, nullptr);
+  return ql_state_save(h, path, STATE_KIND_DQN, h ? dqn_fingerprint(h) : std::vector<FpField>{}, h ? &h->rms : nullptr, nullptr);
 }
 
 int b2g_dqn_state_load(b2g_dqn* h, const char* path) {
-  return ql_state_load(h, path, STATE_KIND_DQN, h ? dqn_fingerprint(h) : std::vector<FpField>{}, nullptr, nullptr, "DQN", nullptr);
+  return ql_state_load(h, path, STATE_KIND_DQN, h ? dqn_fingerprint(h) : std::vector<FpField>{}, h ? &h->rms : nullptr, nullptr, "DQN",
+                       [h] { h->ob_n = 0; });     // the staged observations are not part of the file: a fresh episode
 }
 
 int b2g_dqn_metrics_log(b2g_dqn* h, int capacity) { return ql_metrics_log(h, capacity, B2G_DQN_LOG_COLS); }

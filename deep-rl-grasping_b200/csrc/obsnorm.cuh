@@ -1,7 +1,7 @@
 // VecNormalize's observation statistics on the device (obs_rms) and the frame staging of the observe path, one implementation
-// for the SAC (obsnorm.cu) and BDQ (bdq.cu) handles.  A handle owns one ObsRms as its member `rms`; the templates below are the
-// bodies of its b2g_*obs_rms_set / _get and b2g_*upload_bytes, and the checks and attach of b2g_*_set_obs_encoder.  They read the
-// handle's cfg.device, cfg.nranks, allocs, stream, stage_rows and ob_n.
+// for the SAC (obsnorm.cu), BDQ / DQN (q_learner.cu) and PPO2 / TRPO (actor_critic.cu) handles.  A handle owns one ObsRms as its
+// member `rms`; the templates below are the bodies of its b2g_*obs_rms_set / _get and b2g_*upload_bytes, and the checks and
+// attach of b2g_*_set_obs_encoder.  They read the handle's cfg.device, cfg.nranks, allocs, stream, stage_rows and ob_n.
 #pragma once
 #include <cuda_runtime.h>
 

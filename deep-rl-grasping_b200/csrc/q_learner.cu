@@ -3,6 +3,7 @@
 #include <math.h>
 #include <string.h>
 
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -10,6 +11,25 @@
 #include "q_learner.cuh"
 
 namespace b2g {
+
+namespace {
+// observe_add without frames: transition i = (cur[i], act[i][A], rew[i], nxt[i], done[i]) -> replay slot (first + i) % cap, one
+// CTA per row; CTA 0 also writes the new replay size into counters[5] (what replay_add uploads)
+__global__ void ql_commit_kernel(const float* __restrict__ cur, const float* __restrict__ nxt, const float* __restrict__ act,
+                                 const float* __restrict__ rew, const float* __restrict__ done, int E, int A, long long first, long long cap,
+                                 float* __restrict__ r_obs, float* __restrict__ r_next, float* __restrict__ r_act, float* __restrict__ r_rew,
+                                 float* __restrict__ r_done, long long* counters, long long new_size) {
+  const int i = blockIdx.x;
+  const long long slot = (first + i) % cap;
+  for (int e = threadIdx.x; e < E; e += blockDim.x) {
+    r_obs[slot * E + e] = cur[(size_t)i * E + e];
+    r_next[slot * E + e] = nxt[(size_t)i * E + e];
+  }
+  if (threadIdx.x < A) r_act[slot * A + threadIdx.x] = act[(size_t)i * A + threadIdx.x];
+  if (threadIdx.x == 0) { r_rew[slot] = rew[i]; r_done[slot] = done[i]; }
+  if (i == 0 && threadIdx.x == 0) counters[5] = new_size;
+}
+}  // namespace
 
 int ql_init(QLearner* h, int64_t g_extra, const b2g_replay_cfg* replay, int stage_rows) {
   const char* ng = getenv("B2G_NO_GRAPH");
@@ -29,6 +49,9 @@ int ql_init(QLearner* h, int64_t g_extra, const b2g_replay_cfg* replay, int stag
   QA(h->s_obs, (size_t)B * E); QA(h->s_next, (size_t)B * E); QA(h->s_act, B * A); QA(h->s_rew, B); QA(h->s_done, B);
 #undef QA
   if (cudaMallocHost((void**)&h->h_met, MET_COUNT * sizeof(float)) != cudaSuccess) return b2g_fail(B2G_ECUDA, "cudaMallocHost");
+  h->cfg.device = h->device; h->cfg.nranks = h->nranks;
+  h->stage_rows = stage_rows;
+  h->rms.E = E; h->rms.d_mean = h->d_mean; h->rms.d_istd = h->d_istd;
   std::vector<double> ones(E, 1.0);
   const double nc[8] = {1.0, 10.0, 10.0, 0.0, 0.0, 0, 0, 0};
   if (cudaMemcpyAsync(h->d_istd, ones.data(), E * sizeof(double), cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
@@ -42,6 +65,8 @@ void ql_release(QLearner* h) {
   cudaSetDevice(h->device);
   if (h->stream) cudaStreamSynchronize(h->stream);
   if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
+  enc_stage_destroy(h->rms.enc);
+  h->rms.enc = nullptr;
   mlog_free(&h->mlog);
   for (void* q : h->allocs) cudaFree(q);
   h->replay.release();
@@ -199,6 +224,109 @@ int ql_step_explicit(QLearner* h, const float* obs, const float* act, const floa
   if (apply_update) ++h->n_updates;
   if (td_out) CK(cudaMemcpyAsync(td_out, h->td, B * A * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   return 0;
+}
+
+// ------------------------------------------------------------------------------------------------------------- observe path
+namespace {
+// the refusals every observe call makes
+int ql_observe_checks(const QLearner* h, int n, int update_stats) {
+  if (n < 1 || n > h->stage_rows)
+    return b2g_fail(B2G_EINVAL, "observe: n must be in [1, " + std::to_string(h->stage_rows) + "] (the staging holds max(batch, 256) frames)");
+  if (update_stats && !h->rms.on())
+    return b2g_fail(B2G_ESTATE, std::string("update_stats needs device statistics: call ") + h->rms.set_call + " first");
+  return 0;
+}
+
+// the staging buffers, on first use
+int ql_observe_alloc(QLearner* h) {
+  if (h->ob_rows[0]) return 0;
+  const size_t R = h->stage_rows, E = h->E;
+  for (int k = 0; k < 2; ++k)
+    if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_rows[k], (R + h->B) * E)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_reset, R * E)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_act, R * h->A)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_rew, R)) return rc;
+  if (int rc = dev_alloc(h->allocs, h->stream, &h->ob_done, R)) return rc;
+  return dev_alloc(h->allocs, h->stream, &h->ob_idx, R * h->A);
+}
+}  // namespace
+
+int ql_observe_act(QLearner* h, const float* obs, int n, int update_stats, bool acting, const std::function<int(const float*)>& act) {
+  if (int rc = ql_observe_checks(h, n, obs ? update_stats : 0)) return rc;
+  if (!obs && h->ob_n == 0) return b2g_fail(B2G_ESTATE, "observe_act: no staged observations (pass obs first)");
+  if (!obs && n != h->ob_n) return b2g_fail(B2G_EINVAL, "observe_act: n differs from the number of staged observations");
+  CK(cudaSetDevice(h->device));
+  if (int rc = ql_observe_alloc(h)) return rc;
+  float* cur = h->ob_rows[h->ob_k];
+  if (obs) {
+    if (int rc = h->rms.stage_frames(cur, obs, n, h->stream)) return rc;
+    if (update_stats) h->rms.merge(cur, nullptr, nullptr, n, h->stream);
+    h->ob_n = n;
+    h->ob_fid.assign((size_t)n, -1);
+  }
+  if (acting)
+    if (int rc = act(cur)) return rc;
+  CK(cudaStreamSynchronize(h->stream));     // caller-owned arrays are copied, the actions are the result of the call
+  CK(cudaGetLastError());
+  return 0;
+}
+
+int ql_observe_add(QLearner* h, const float* act, const float* rew, const float* next_obs, const float* done, const float* reset_obs,
+                   int n, int update_stats, const std::function<int()>& check) {
+  if (int rc = ql_observe_checks(h, n, update_stats)) return rc;
+  if (h->ob_n == 0)
+    return b2g_fail(B2G_ESTATE, std::string("observe_add: no staged observations (call b2g_") + h->abi + "_observe_act first)");
+  if (n != h->ob_n) return b2g_fail(B2G_EINVAL, "observe_add: n differs from the number of staged observations");
+  if (n > h->buffer_capacity) return b2g_fail(B2G_EINVAL, "observe_add: n exceeds buffer_capacity");
+  if (h->replay.ring.dedup && 2 * (int64_t)n > h->replay.ring.frame_cap)
+    return b2g_fail(B2G_EINVAL, "observe_add: 2 n rows exceed frame_capacity (replay_frames)");
+  int n_done = 0;
+  for (int i = 0; i < n; ++i) n_done += done[i] != 0.f;
+  if (n_done && !reset_obs) return b2g_fail(B2G_EINVAL, "observe_add: an env finished but reset_obs is NULL");
+  if (check)
+    if (int rc = check()) return rc;
+  CK(cudaSetDevice(h->device));
+  if (int rc = ql_observe_alloc(h)) return rc;
+  const size_t E = h->E, A = h->A, fb = E * sizeof(float);
+  float* cur = h->ob_rows[h->ob_k];
+  float* nxt = h->ob_rows[h->ob_k ^ 1];
+  if (int rc = h->rms.stage_frames(nxt, next_obs, n, h->stream)) return rc;
+  if (int rc = h->rms.upload(h->ob_act, act, n * A * sizeof(float), h->stream)) return rc;
+  if (int rc = h->rms.upload(h->ob_rew, rew, n * sizeof(float), h->stream)) return rc;
+  if (int rc = h->rms.upload(h->ob_done, done, n * sizeof(float), h->stream)) return rc;
+  if (n_done)
+    if (int rc = h->rms.stage_reset_frames(h->ob_reset, reset_obs, done, h->ob_done, n, n_done, h->stream)) return rc;
+  // the transitions: obs = the staged rows, next_obs = the uploaded rows (what the caller passes as a finished env's next_obs)
+  TransitionReplay& rp = h->replay;
+  if (rp.framed()) {
+    // env i's staged row is the frame its previous transition's next_obs took, unless the env was reset since: shared without
+    // comparing; a reset frame (ob_fid -1) takes a frame of its own here, when it is first used as obs
+    std::vector<int64_t> next_ids((size_t)n);
+    if (int rc = rp.add_linked(cur, nxt, h->ob_fid.data(), h->ob_act, h->ob_rew, h->ob_done, n, next_ids.data(), h->counters, h->stream))
+      return rc;
+    for (int i = 0; i < n; ++i) h->ob_fid[i] = done[i] != 0.f ? -1 : next_ids[i];
+  } else {
+    const int64_t new_size = std::min<int64_t>(rp.cap, rp.size + n);
+    ql_commit_kernel<<<n, 256, 0, h->stream>>>(cur, nxt, h->ob_act, h->ob_rew, h->ob_done, (int)E, (int)A, rp.pos, rp.cap, rp.obs, rp.next,
+                                               rp.act, rp.rew, rp.done, h->counters, new_size);
+    rp.insert_max_prio(rp.pos, n, h->stream);     // as in replay_add
+  }
+  // VecNormalize's step_wait merges the frames the VecEnv returned: a finished env's reset frame, not its terminal observation
+  if (update_stats) h->rms.merge(nxt, n_done ? h->ob_reset : nullptr, h->ob_done, n, h->stream);
+  // the new rows become the current observations; a finished env continues from the frame its reset returned
+  for (int i = 0; i < n; ++i)
+    if (done[i] != 0.f) CK(cudaMemcpyAsync(nxt + i * E, h->ob_reset + i * E, fb, cudaMemcpyDeviceToDevice, h->stream));
+  if (!rp.framed()) rp.advance(n);
+  h->ob_k ^= 1;
+  CK(cudaStreamSynchronize(h->stream));     // host arrays are caller-owned: copied before return
+  CK(cudaGetLastError());
+  return 0;
+}
+
+int ql_set_obs_encoder(QLearner* h, const b2g_encoder* enc, int tail) {
+  if (enc)
+    if (int rc = obs_rms_check_encoder(h, enc, tail)) return rc;
+  return obs_rms_attach_encoder(h, enc, tail);
 }
 
 // ------------------------------------------------------------------------------------------------------------- training state

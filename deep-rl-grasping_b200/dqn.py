@@ -18,6 +18,7 @@ from .base_model import BaseModel
 from .callbacks import as_callback
 from .tensorboard import EpisodeRewardLogger
 from .learner import TransitionReplayLearner, _f32, _fp
+from .vec_env import VecNormalize
 
 _ONLINE, _TARGET = "deepq/model/", "deepq/target_q_func/model/"
 
@@ -40,6 +41,7 @@ class DQNLearner(TransitionReplayLearner):
         self.obs_dim = self.obs_elems = obs_dim
         self.n_actions, self.batch_size = n_actions, batch_size
         self._act_width = 1
+        self.obs_shape = (obs_dim,)          # shape of obs_rms_get's arrays (DQN sets the env's observation shape)
 
     def _has_grad(self, name):
         return name.startswith(_ONLINE)
@@ -100,6 +102,44 @@ class DQNLearner(TransitionReplayLearner):
         _lib.check(self.lib.b2g_dqn_act(self.h, _fp(obs), n, out.ctypes.data_as(C.POINTER(C.c_int32)), None if q is None else _fp(q)))
         return (out, q) if with_q else out
 
+    def act_raw(self, obs, with_q=False):
+        """``act`` on raw observations, normalised on the device with the learner's ``obs_rms`` (predict while the learner
+        owns VecNormalize's statistics)."""
+        obs = _f32(obs).reshape(-1, self.obs_dim)
+        n = obs.shape[0]
+        out = np.empty(n, np.int32)
+        q = np.empty((n, self.n_actions), np.float32) if with_q else None
+        _lib.check(self.lib.b2g_dqn_act_raw(self.h, _fp(obs), n, out.ctypes.data_as(C.POINTER(C.c_int32)), None if q is None else _fp(q)))
+        return (out, q) if with_q else out
+
+    # ---- the actor loop on one upload per frame (include/b200grasp.h: b2g_dqn_observe_*)
+    def observe_act(self, obs, n=None, update_stats=True, eps=0.0, act=True):
+        """``obs``: n raw observations to upload, merge into ``obs_rms`` (``update_stats``) and stage as the current
+        observation of env i; ``None`` acts on the ones already staged.  Returns the [n] epsilon-greedy actions, or None
+        with ``act=False``."""
+        if obs is not None:
+            obs = _f32(obs).reshape(-1, self.frame_elems)
+            n = obs.shape[0]
+            self.obs_rms_version += bool(update_stats)
+        out = np.empty(int(n), np.int32) if act else None
+        _lib.check(self.lib.b2g_dqn_observe_act(self.h, None if obs is None else _fp(obs), int(n), int(bool(update_stats)), float(eps),
+                                                None if out is None else out.ctypes.data_as(C.POINTER(C.c_int32))))
+        return out
+
+    def observe_add(self, act, rew, next_obs, done, reset_obs=None, update_stats=True):
+        """Transition i = (staged obs_i, act_i, rew_i, next_obs_i, done_i); ``reset_obs`` holds, for every finished env,
+        the frame its auto-reset returned (the other rows are not read)."""
+        act, next_obs = _f32(np.reshape(act, -1)), _f32(next_obs)
+        rew, done = _f32(np.reshape(rew, -1)), _f32(np.reshape(done, -1))
+        n = rew.shape[0]
+        assert next_obs.size == n * self.frame_elems and act.size == n and done.size == n
+        if reset_obs is not None:
+            reset_obs = _f32(reset_obs)
+            assert reset_obs.size == next_obs.size
+        _lib.check(self.lib.b2g_dqn_observe_add(self.h, _fp(act), _fp(rew), _fp(next_obs), _fp(done),
+                                                None if reset_obs is None else _fp(reset_obs), n, int(bool(update_stats))))
+        self.obs_rms_version += bool(update_stats)
+
 
 
 def _linear(t, span, p0, p1):
@@ -135,7 +175,7 @@ class DQN(BaseModel):
                  target_network_update_freq=500, prioritized_replay=False, prioritized_replay_alpha=0.6, prioritized_replay_beta0=0.4,
                  prioritized_replay_beta_iters=None, prioritized_replay_eps=1e-6, param_noise=False, n_cpu_tf_sess=None, verbose=0,
                  tensorboard_log=None, _init_setup_model=True, policy_kwargs=None, full_tensorboard_log=False, seed=None, device=0,
-                 replay_frames=None):
+                 replay_frames=None, device_obs_norm=False):
         if not double_q:
             raise NotImplementedError("double_q=False: only the double-Q target is built")
         if param_noise:
@@ -156,6 +196,9 @@ class DQN(BaseModel):
         self.per_alpha, self.per_beta0, self.per_beta_iters, self.per_eps = prioritized_replay_alpha, prioritized_replay_beta0, \
             prioritized_replay_beta_iters, prioritized_replay_eps
         self.replay_frames = None if replay_frames is None else int(replay_frames)    # DQNLearner's frame_capacity
+        # learn() feeds the actor, the statistics and the replay from one upload per frame (DQNLearner.observe_act / _add), a
+        # VecNormalize with norm_obs hands its obs_rms to the device learner and a VecEncodeDepth its encoder
+        self.device_obs_norm = bool(device_obs_norm)
         self.verbose, self.seed, self.device = verbose, seed, device
         self.tensorboard_log = tensorboard_log
         self.num_timesteps = 0
@@ -167,6 +210,12 @@ class DQN(BaseModel):
             self._set_env(env)
             if _init_setup_model:
                 self.setup_model()
+
+    def set_env(self, env):
+        self._set_env(env)
+        if self.learner is not None:
+            self._attach_device_norm()
+            self._attach_obs_encoder()
 
     def _check_env(self):
         if self.n_envs > 1:      # stable-baselines' own refusal (deepq/dqn.py: "...cannot be used with more than one env")
@@ -193,9 +242,23 @@ class DQN(BaseModel):
             else:
                 p[n] = np.zeros(shp, np.float32)
         self.learner.load_parameters(p)
+        self.learner.obs_shape = tuple(self.observation_space.shape)
+        self._attach_device_norm()
+        self._attach_obs_encoder()
+
+    def _attach_device_norm(self):
+        super()._attach_device_norm()
+        if self._owns_obs_rms():
+            self._sync_norm_stats()
 
     def _sync_norm_stats(self):
+        """The wrapper's statistics for the gather of the sampled step; a learner that owns obs_rms takes the reward scalars
+        and clips only (the observation statistics are its own)."""
         vn = self._vec_normalize_env
+        if self._owns_obs_rms():
+            self.learner.set_norm_stats(None, None, float(vn.ret_rms.var), vn.clip_obs, vn.clip_reward, vn.epsilon,
+                                        norm_obs=vn.norm_obs, norm_reward=vn.norm_reward)
+            return
         self.learner.set_norm_stats(vn.obs_rms.mean, vn.obs_rms.var, float(vn.ret_rms.var), vn.clip_obs, vn.clip_reward, vn.epsilon,
                                     norm_obs=vn.norm_obs, norm_reward=vn.norm_reward)
 
@@ -225,14 +288,27 @@ class DQN(BaseModel):
         horizon = t0 + total_timesteps
         eps_span = int(self.exploration_fraction * horizon)
         beta_span = self.per_beta_iters or horizon
+        dev = self.device_obs_norm
+        if dev and vn is not None:
+            if not isinstance(vn, VecNormalize) or not vn.norm_obs:
+                raise RuntimeError("device_obs_norm=True needs the env's VecNormalize to have norm_obs=True")
+            if not self._owns_obs_rms():
+                raise RuntimeError("learn: the env's VecNormalize statistics are owned by another model's learner (close that model, "
+                                   "or build this one with device_obs_norm=True before it)")
         obs = self.env.reset()
         raw = vn.get_original_obs() if vn is not None else obs
+        stats = dev and vn is not None
+        if dev:      # the reset frames: uploaded once, merged (VecNormalize.reset's update), staged as the current observation
+            self.learner.observe_act(np.asarray(raw, np.float32), update_stats=stats and vn.training, act=False)
         eps = self.exploration_initial_eps
         ep_log = EpisodeRewardLogger(1) if writer is not None else None
         for _ in range(total_timesteps):
             eps = _linear(self.num_timesteps, eps_span, self.exploration_initial_eps, self.exploration_final_eps)
-            greedy = self.learner.act(np.asarray(obs, np.float32))     # the wrapper's output, as stable-baselines' act sees it
-            action = int(self._rng.integers(0, self.learner.n_actions)) if self._rng.random() < eps else int(greedy[0])
+            if dev:      # the staged frame, current statistics, epsilon-greedy on the device (Philox stream 3)
+                action = int(self.learner.observe_act(None, n=1, eps=eps)[0])
+            else:
+                greedy = self.learner.act(np.asarray(obs, np.float32))     # the wrapper's output, as stable-baselines' act sees it
+                action = int(self._rng.integers(0, self.learner.n_actions)) if self._rng.random() < eps else int(greedy[0])
             new_obs, rew, done, infos = self.env.step(np.array([action]))
             self.num_timesteps += 1
             if callback.on_step() is False:
@@ -243,7 +319,12 @@ class DQN(BaseModel):
             info = infos[0] if infos else {}
             if done[0] and isinstance(info, dict) and "terminal_observation" in info and vn is None:
                 nxt[0] = np.asarray(info["terminal_observation"], np.float32).reshape(-1)
-            self.learner.replay_add(np.asarray(raw, np.float32), np.float32(action), rew_raw, nxt, np.asarray(done, np.float32))
+            if dev:      # next_obs crosses once; a finished env's reset frame is merged and staged
+                self.learner.observe_add(np.float32(action), rew_raw, nxt, np.asarray(done, np.float32),
+                                         reset_obs=np.asarray(new_raw, np.float32).reshape(1, -1) if done[0] else None,
+                                         update_stats=stats and vn.training)       # step_wait's update; a callback may switch it
+            else:
+                self.learner.replay_add(np.asarray(raw, np.float32), np.float32(action), rew_raw, nxt, np.asarray(done, np.float32))
             obs, raw = new_obs, new_raw
             if ep_log is not None:
                 ep_log(writer, rew_raw, done, self.num_timesteps)
@@ -266,9 +347,12 @@ class DQN(BaseModel):
     def predict(self, observation, state=None, mask=None, deterministic=True):
         """Greedy actions, or with ``deterministic=False`` a draw from softmax(Q) per row (the deepq policy's ``step``; the
         uniform comes from ``self.predict_rng``).  ``observation`` is what the env hands out: with a VecNormalize wrapper its
-        normalised output, which the network takes as it is."""
+        normalised output, which the network takes as it is, or its raw output while this model's learner owns the
+        statistics (``predict_takes_raw_obs``), which the learner normalises on the device."""
+        self._check_encoded(observation)
         obs = np.asarray(observation, np.float32).reshape(-1, self.learner.obs_dim)
-        idx, q = self.learner.act(obs, with_q=True)
+        act = self.learner.act_raw if self.predict_takes_raw_obs else self.learner.act
+        idx, q = act(obs, with_q=True)
         if not deterministic:
             q = q.astype(np.float64)
             p = np.exp(q - q.max(1, keepdims=True))
@@ -326,8 +410,14 @@ class DQN(BaseModel):
                     device=self.device)
         if self.replay_frames is not None:
             init["replay_frames"] = self.replay_frames
-        return {"algo": "DQN", "init": init, "num_timesteps": int(self.num_timesteps), "n_target_updates": int(self.n_target_updates),
+        if self.device_obs_norm:
+            init["device_obs_norm"] = True
+        host = {"algo": "DQN", "init": init, "num_timesteps": int(self.num_timesteps), "n_target_updates": int(self.n_target_updates),
                 "rng": training_state.rng_state(self._rng), "predict_rng": training_state.rng_state(self.predict_rng)}
+        enc = self._encoder_host()
+        if enc is not None:
+            host["obs_encoder"] = enc
+        return host
 
     def _restore_host_state(self, host):
         self.num_timesteps = int(host["num_timesteps"])

@@ -438,7 +438,8 @@ int b2g_dqn_replay_get(b2g_dqn* h, int64_t slot, float* obs, float* act, float* 
  * (actions, rewards, dones).  The prioritised-replay trees are not counted. */
 int64_t b2g_transition_replay_bytes(int64_t buffer_capacity, int obs_dim, int act_width, int64_t frame_capacity);
 /* VecNormalize's statistics for the gather of the sampled and explicit steps (the replay holds raw transitions); not used by
- * b2g_dqn_act */
+ * b2g_dqn_act.  On a handle that owns obs_rms (b2g_dqn_obs_rms_set, below) obs_mean / obs_var may be NULL with norm_obs != 0:
+ * the scalars are set and the device statistics stay; passing them replaces the device statistics (count kept). */
 int b2g_dqn_set_norm_stats(b2g_dqn* h, const double* obs_mean, const double* obs_var, double ret_var, double clip_obs,
                            double clip_rew, double eps, int norm_obs, int norm_reward);
 /* n_steps sampled steps, replayed as one captured CUDA graph each */
@@ -460,9 +461,42 @@ int b2g_dqn_update_target(b2g_dqn* h);
 /* greedy actions argmax_k Q(s, k) of the online network for n observations as the network sees them (a VecNormalize
  * wrapper's output: no normalisation is applied here); q_out (may be NULL): the [n, n_actions] Q rows */
 int b2g_dqn_act(b2g_dqn* h, const float* obs, int n, int32_t* act_out, float* q_out);
+
+/* ---- VecNormalize's observation statistics on the device and the epsilon-greedy actor fed from one upload per frame: the
+ *      DQN counterpart of b2g_bdq_observe_* (the same observe path, merge rule and refusals, obs_rms over the flat [obs_dim]
+ *      observation).  Up to max(batch, 256) frames per call; every call returns once the handle's stream has run what it
+ *      enqueued.  Before any CUDA work: B2G_EINVAL for eps outside [0, 1] or an n other than the number of staged
+ *      observations, B2G_ESTATE for update_stats without b2g_dqn_obs_rms_set and for b2g_dqn_observe_add before any
+ *      b2g_dqn_observe_act. */
+/* n raw observations (host, caller-owned), or obs == NULL to act on the observations already staged.  update_stats != 0:
+ * merge them into obs_rms first.  act_out != NULL: run the online network on the staged rows normalised with the CURRENT
+ * statistics (the gather's rule: b2g_dqn_set_norm_stats's norm_obs and clip_obs), take the greedy action (b2g_dqn_act's
+ * argmax of Q = V + A - mean A, first maximum) and, with probability eps in [0, 1] per env, a uniform random action instead;
+ * writes [n] actions.  The random draws are Philox stream 3 under the training key at step counters[7] (the number of earlier
+ * acting calls, kept in the training-state file), block env: lane x explores when (x + 0.5) 2^-32 < eps (float64), lane y
+ * gives action (y * n_actions) >> 32 -- b2g_bdq_observe_act's rule with one branch. */
+int b2g_dqn_observe_act(b2g_dqn* h, const float* obs, int n, int update_stats, float eps, int32_t* act_out);
+/* Transition i = (staged obs_i, act_i, rew_i, next_obs_i, done_i) into the replay (rows as b2g_dqn_replay_add stores them;
+ * every act value must be an integer in [0, n_actions), checked before anything is stored; new rows enter the
+ * prioritised-replay trees at the running maximum priority).  next_obs is uploaded ONCE: it is this transition's next
+ * observation, is merged into obs_rms when update_stats != 0 and becomes the staged observation of env i, unless done_i:
+ * then reset_obs_i (the frame the auto-reset returned; the only rows of reset_obs read) is merged and staged instead. */
+int b2g_dqn_observe_add(b2g_dqn* h, const float* act, const float* rew, const float* next_obs, const float* done,
+                        const float* reset_obs /* may be NULL when no env finished */, int n, int update_stats);
+/* b2g_dqn_act on RAW observations, normalised on the device with obs_rms's table and the clip_obs / norm_obs of
+ * b2g_dqn_set_norm_stats: predict while the learner owns the statistics.  B2G_ESTATE without b2g_dqn_obs_rms_set. */
+int b2g_dqn_act_raw(b2g_dqn* h, const float* obs, int n, int32_t* act_out, float* q_out);
+/* obs_rms in and out: float64 [obs_dim] each + count, with the checks of b2g_obs_rms_set / _get */
+int b2g_dqn_obs_rms_set(b2g_dqn* h, const double* mean, const double* var, double count);
+int b2g_dqn_obs_rms_get(b2g_dqn* h, double* mean, double* var, double* count);
+/* bytes copied host -> device so far by b2g_dqn_observe_* and b2g_dqn_obs_rms_set (observe_bytes) and by b2g_dqn_act /
+ * _act_raw, b2g_dqn_replay_add and b2g_dqn_set_norm_stats (other_bytes); either may be NULL */
+int b2g_dqn_upload_bytes(const b2g_dqn* h, int64_t* observe_bytes, int64_t* other_bytes);
 /* training state, as b2g_bdq_state_save / _load: parameters, Adam moments, counters, n_updates, the live replay rows, the
- * prioritised-replay trees, max priority and beta, and deepq/eps.  The fingerprint covers every b2g_dqn_cfg field that
- * decides the layout or the prioritised replay. */
+ * prioritised-replay trees, max priority and beta, and deepq/eps; and the device obs_rms of a handle that owns one, behind
+ * one more fingerprint field (such a file loads only into a handle that owns obs_rms, and the reverse; a handle without
+ * device statistics writes the files it wrote before).  The staged observations of b2g_dqn_observe_* are not saved.  The
+ * fingerprint covers every b2g_dqn_cfg field that decides the layout or the prioritised replay. */
 int b2g_dqn_state_save(b2g_dqn* h, const char* path);
 int b2g_dqn_state_load(b2g_dqn* h, const char* path);
 
@@ -701,6 +735,8 @@ int b2g_debug_encoder_layers(b2g_encoder* h, const float* imgs, int n, float* ou
  * device; B2G_ESTATE for an encoder layer without weights or nranks > 1. */
 int b2g_sac_set_obs_encoder(b2g_sac* h, const b2g_encoder* enc, int tail);
 int b2g_bdq_set_obs_encoder(b2g_bdq* h, const b2g_encoder* enc, int tail);
+/* the same on the DQN handle: b2g_dqn_observe_act / _add take raw rows */
+int b2g_dqn_set_obs_encoder(b2g_dqn* h, const b2g_encoder* enc, int tail);
 /* the same on the PPO2 and TRPO handles: b2g_ppo_observe_act / b2g_trpo_observe_act take raw rows, encode them into the
  * staged rows and normalise those into the rollout */
 int b2g_ppo_set_obs_encoder(b2g_ppo* h, const b2g_encoder* enc, int tail);
