@@ -51,7 +51,7 @@ SYMBOLS = [
     "b2g_autoencoder_create", "b2g_autoencoder_destroy", "b2g_autoencoder_n_layers", "b2g_autoencoder_layer_shape",
     "b2g_autoencoder_set_weights", "b2g_autoencoder_get_weights", "b2g_autoencoder_get_grad", "b2g_autoencoder_reset_optimizer",
     "b2g_autoencoder_set_dataset", "b2g_autoencoder_train_epoch", "b2g_autoencoder_evaluate", "b2g_autoencoder_predict",
-    "b2g_autoencoder_step",
+    "b2g_autoencoder_step", "b2g_autoencoder_create2", "b2g_debug_autoencoder_tensor", "b2g_debug_autoencoder_tensor_numel",
     "b2g_sac_metrics_log", "b2g_sac_metrics_drain", "b2g_bdq_metrics_log", "b2g_bdq_metrics_drain",
     "b2g_dqn_metrics_log", "b2g_dqn_metrics_drain",
 ]
@@ -341,6 +341,10 @@ def load():
     lib.b2g_sac_set_obs_encoder.argtypes = [vp, vp, C.c_int]
     lib.b2g_bdq_set_obs_encoder.argtypes = [vp, vp, C.c_int]
     lib.b2g_autoencoder_create.argtypes = [C.POINTER(EncoderCfg), C.POINTER(vp)]
+    lib.b2g_autoencoder_create2.argtypes = [C.POINTER(EncoderCfg), C.c_int32, C.POINTER(vp)]
+    lib.b2g_debug_autoencoder_tensor.argtypes = [vp, C.c_int, C.c_int, fp, C.c_int64, C.POINTER(C.c_int32)]
+    lib.b2g_debug_autoencoder_tensor_numel.argtypes = [vp, C.c_int, C.c_int]
+    lib.b2g_debug_autoencoder_tensor_numel.restype = C.c_int64
     lib.b2g_autoencoder_destroy.argtypes = [vp]
     lib.b2g_autoencoder_n_layers.argtypes = [vp]
     lib.b2g_autoencoder_layer_shape.argtypes = [vp, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]

@@ -1,6 +1,6 @@
 // libb200grasp: convolutional auto-encoder TRAINING -- SURVEY.md section 8 row a12 (encoders.py:40-61 train / test / predict).
 //
-// The whole Keras model (encoders.py:84-136) on one handle, in fp32 on the CUDA cores.  One training step is
+// The whole Keras model (encoders.py:84-136) on one handle, in fp32 on the CUDA cores (or bf16x3, below).  One training step is
 //   forward of the 2L+2 layers -> MSE seed -> backward (input gradient of every layer but the first conv, weight and bias
 //   gradient of every layer) -> Keras Adam.
 // Every conv and dense contraction runs on the gather-GEMM engine (gg_simt.cu) from offset tables; the encoder half's
@@ -20,6 +20,18 @@
 // The one-filter output conv would waste 63 of 64 tile columns on the engine, so its forward (fused with the MSE seed and
 // the bias gradient) and its weight gradient are direct-convolution kernels over 8x8 pixel tiles staged in shared memory.
 // Its input gradient (N = filters_0) runs on the engine.
+//
+// Precision B2G_PREC_BF16X3 (b2g_autoencoder_create2) runs every contraction whose operands the wgmma engine's
+// register-staged producer can read on that engine (gg_tc.cu, GG_ACC64 instantiations, x3 = 1): the producer gathers the same
+// fp32 tensors through the same offset tables in 16-byte groups of 4 consecutive values, splits each value into BF16 hi + lo in
+// registers and the tensor cores sum hi*hi + hi*lo + lo*hi in fp32.  That covers the forward of every conv but the first and
+// of both dense layers (bias + LeakyReLU epilogue), every input gradient but the output conv's (LeakyReLU-derivative epilogue
+// into the previous layer's D) and every weight and bias gradient but the first conv's and the output conv's.  A weight
+// gradient's split-R partial sums (the tensor cores' fp32 accumulators over one split's r-range; the bias: each producer
+// thread's fp32 running sum of D over its share of that range) are added into the double arena with double atomics.
+// conv1's forward and weight gradient (one input channel) and the output conv's input gradient (one filter) have no 4-element
+// groups along their reduction or output rows, so they stay on gg_simt, as do the output conv's direct kernels and Adam.
+// Nothing is kept as planes in HBM: the weights change every step and each activation and gradient is read once or twice.
 //
 // Training epochs keep the dataset on the device: each step gathers its batch rows through the epoch's permutation and a
 // device cursor, so one captured graph per batch size replays every step (the partial last batch has its own graph).
@@ -71,6 +83,7 @@ struct AeGemm {
   GemmDesc d;
   int m_per = 0, r_per = 0;  // M or R per sample (the other extent is fixed)
   bool wgrad = false;
+  bool tc = false;           // bf16x3: runs on the wgmma engine
 };
 
 struct AePlan {
@@ -256,6 +269,7 @@ __global__ void ae_adam(float4* __restrict__ P, float4* __restrict__ Mo, float4*
 
 struct b2g_autoencoder {
   b2g_encoder_cfg cfg{};
+  int precision = B2G_PREC_FP32_SIMT;
   cudaStream_t stream = nullptr;
   int num_sms = 132;
   std::vector<void*> allocs;
@@ -279,6 +293,7 @@ struct b2g_autoencoder {
   std::vector<AeGemm> fwd_g, bwd_g;                  // contractions at max_batch, in issue order
   std::map<int, AePlan> plans;
   size_t out_smem_fwd = 0, out_smem_wg = 0;
+  ColIds col_ids;                                    // bf16x3: column-table identities of the wgmma descriptors
 };
 
 namespace {
@@ -294,14 +309,19 @@ int add_gemm(b2g_autoencoder* h, std::vector<AeGemm>& list, const float* A, cons
   e.d = gemm_desc(A, nullptr, nullptr, B, nullptr, nullptr, C, nullptr, nullptr, M, N, R, flags);
   e.d.bias = bias; e.d.mask = mask; e.d.colsum = colsum; e.d.alpha = h->cfg.alpha;
   e.m_per = m_per; e.r_per = r_per; e.wgrad = (flags & GG_EPI_ATOMIC) != 0;
+  // GG_A_SCALAR marks the operands without 4-element groups (one channel / one filter): gg_simt only
+  e.tc = h->precision == B2G_PREC_BF16X3 && !(flags & GG_A_SCALAR);
+  std::map<const int*, std::vector<int>> host;       // the column-side tables, for gg_tc_columns
+  auto* hc = e.tc ? &host : nullptr;
   if (int rc = ae_upload(h, aM, &e.d.aM)) return rc;
   if (int rc = ae_upload(h, aR, &e.d.aR)) return rc;
   if (int rc = ae_upload(h, bN, &e.d.bN)) return rc;
   if (int rc = ae_upload(h, bR, &e.d.bR)) return rc;
-  if (int rc = ae_upload(h, cM, &e.d.cM)) return rc;
-  if (int rc = ae_upload(h, cN, &e.d.cN)) return rc;
-  if (kM) if (int rc = ae_upload(h, *kM, &e.d.kM)) return rc;
-  if (kN) if (int rc = ae_upload(h, *kN, &e.d.kN)) return rc;
+  if (int rc = upload_table(h->allocs, h->stream, cM, &e.d.cM, hc)) return rc;
+  if (int rc = upload_table(h->allocs, h->stream, cN, &e.d.cN, hc)) return rc;
+  if (kM) if (int rc = upload_table(h->allocs, h->stream, *kM, &e.d.kM, hc)) return rc;
+  if (kN) if (int rc = upload_table(h->allocs, h->stream, *kN, &e.d.kN, hc)) return rc;
+  if (e.tc) gg_tc_columns(e.d, host, h->col_ids);
   list.push_back(e);
   return 0;
 }
@@ -468,6 +488,19 @@ int get_plan(b2g_autoencoder* h, int n, AePlan** out) {
       GemmDesc d = e.d;
       if (e.m_per) d.M = e.m_per * n;
       if (e.r_per) d.R = e.r_per * n;
+      if (e.tc) {
+        // persistent grid of min(tiles, SMs) CTAs: a weight gradient splits R so that its tiles fill the SMs once
+        d.tiles_m = (d.M + GG_TC_BM - 1) / GG_TC_BM;
+        d.tiles_n = (d.N + GG_TC_BN - 1) / GG_TC_BN;
+        if (e.wgrad) d.splitR = std::max(1, std::min(h->num_sms / (d.tiles_m * d.tiles_n), d.R / 512));
+        d.tile_start = 0;
+        d.tile_count = d.tiles_m * d.tiles_n * d.splitR;
+        g.host = {d};
+        g.total_tiles = d.tile_count;
+        g.tc = true;
+        p.g.push_back(g);
+        continue;
+      }
       if (e.wgrad) {
         const int tiles = ((d.M + GG_SIMT_BM - 1) / GG_SIMT_BM) * ((d.N + GG_SIMT_BN - 1) / GG_SIMT_BN);
         d.splitR = std::max(1, std::min((2 * h->num_sms + tiles - 1) / tiles, d.R / 256));
@@ -478,6 +511,13 @@ int get_plan(b2g_autoencoder* h, int n, AePlan** out) {
     }
   *out = &(h->plans[n] = p);
   return 0;
+}
+
+// one contraction: gg_tc (GG_ACC64, x3 = 1) or gg_simt_launch_ext; a failed launch shows in cudaGetLastError
+void launch_group(b2g_autoencoder* h, const GemmGroup& g) {
+  if (!g.tc) { gg_simt_launch_ext(g.dev, 1, g.total_tiles, h->stream); return; }
+  const GemmDesc& d = g.host[0];
+  gg_tc_launch(g.host.data(), 1, g.total_tiles, (d.flags & (GG_A_RVEC | GG_B_RVEC)) | GG_ACC64, 1, h->num_sms, h->stream);
 }
 
 int grid_for(long long work) { return (int)std::max<long long>(1, std::min<long long>((work + 255) / 256, 132 * 8)); }
@@ -493,15 +533,14 @@ void issue_gather(b2g_autoencoder* h, int n, const float* src, const float* tgt,
 void issue_forward(b2g_autoencoder* h, AePlan& p, int n, bool grad, float* Y) {
   const int Lc = h->cfg.n_layers, nL = (int)h->L.size();
   int k = 0;
-  for (int l = 0; l <= Lc + 1; ++l) { const GemmGroup& g = p.g[k++]; gg_simt_launch_ext(g.dev, 1, g.total_tiles, h->stream); }
+  for (int l = 0; l <= Lc + 1; ++l) launch_group(h, p.g[k++]);
   for (int j = Lc + 2; j < nL; ++j) {
     const AeLayer& pv = h->L[j - 1];
     const AeLayer& cur = h->L[j];
     ae_upsample<<<grid_for((long long)n * cur.g.in_h * cur.g.in_w * pv.map_c / 4), 256, 0, h->stream>>>(
         pv.act, n, pv.map_h, pv.map_w, pv.map_c, cur.up, cur.in, cur.g.hp, cur.g.wp, cur.g.pad_t, cur.g.pad_l);
     if (cur.kind == DEC_CONV) {
-      const GemmGroup& g = p.g[k++];
-      gg_simt_launch_ext(g.dev, 1, g.total_tiles, h->stream);
+      launch_group(h, p.g[k++]);
     } else {
       const int H = h->cfg.height, W = h->cfg.width;
       const int tiles = ((H + AE_TILE - 1) / AE_TILE) * ((W + AE_TILE - 1) / AE_TILE);
@@ -518,7 +557,7 @@ void issue_backward(b2g_autoencoder* h, AePlan& p, int n) {
   const int tiles = n * ((H + AE_TILE - 1) / AE_TILE) * ((W + AE_TILE - 1) / AE_TILE);
   ae_out_wgrad<<<std::min(tiles, 2 * h->num_sms), 256, h->out_smem_wg, h->stream>>>(o.in, o.g.hp, o.g.wp, o.g.in_c, o.g.k, H, W, n, o.D,
                                                                                    o.dh, o.dw, h->G64 + o.w_off);
-  for (size_t k = h->fwd_g.size(); k < p.g.size(); ++k) gg_simt_launch_ext(p.g[k].dev, 1, p.g[k].total_tiles, h->stream);
+  for (size_t k = h->fwd_g.size(); k < p.g.size(); ++k) launch_group(h, p.g[k]);
   ae_round_grads<<<grid_for((long long)h->n_par), 256, 0, h->stream>>>(h->G64, h->G, (int)h->n_par);
 }
 
@@ -583,7 +622,17 @@ int stage_batch(b2g_autoencoder* h, const float* in, const float* tg, int n) {
 extern "C" {
 
 int b2g_autoencoder_create(const b2g_encoder_cfg* cfg, b2g_autoencoder** out) {
+  return b2g_autoencoder_create2(cfg, B2G_PREC_FP32_SIMT, out);
+}
+
+int b2g_autoencoder_create2(const b2g_encoder_cfg* cfg, int32_t precision, b2g_autoencoder** out) {
   if (!cfg || !out) return b2g_fail(B2G_EINVAL, "null argument");
+  if (precision == B2G_PREC_BF16)
+    return b2g_fail(B2G_EINVAL, "auto-encoder precision B2G_PREC_BF16: single-pass BF16 training is not offered; use "
+                                "B2G_PREC_FP32_SIMT or B2G_PREC_BF16X3");
+  if (precision != B2G_PREC_FP32_SIMT && precision != B2G_PREC_BF16X3)
+    return b2g_fail(B2G_EINVAL, "auto-encoder precision " + std::to_string(precision) +
+                                    ": expected B2G_PREC_FP32_SIMT (0) or B2G_PREC_BF16X3 (1)");
   if (cfg->n_layers < 1 || cfg->n_layers > B2G_ENC_MAX_LAYERS) return b2g_fail(B2G_EINVAL, "n_layers out of range");
   if (cfg->height < 1 || cfg->width < 1 || cfg->encoding_dim < 1 || cfg->max_batch < 1)
     return b2g_fail(B2G_EINVAL, "non-positive dimension");
@@ -646,6 +695,7 @@ int b2g_autoencoder_create(const b2g_encoder_cfg* cfg, b2g_autoencoder** out) {
 
   b2g_autoencoder* h = new b2g_autoencoder();
   h->cfg = *cfg;
+  h->precision = precision;
   h->L = L;
   h->out_smem_fwd = smem_fwd; h->out_smem_wg = smem_wg;
   auto bail = [&](int rc) { b2g_autoencoder_destroy(h); return rc; };
@@ -706,6 +756,8 @@ int b2g_autoencoder_create(const b2g_encoder_cfg* cfg, b2g_autoencoder** out) {
     return bail(b2g_fail(B2G_ECUDA, "output conv shared memory"));
   if (smem_wg > 48 * 1024 && cudaFuncSetAttribute(ae_out_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_wg) != cudaSuccess)
     return bail(b2g_fail(B2G_ECUDA, "output conv shared memory"));
+  if (precision == B2G_PREC_BF16X3 && gg_tc_acc64_init() != cudaSuccess)
+    return bail(b2g_fail(B2G_ECUDA, "wgmma engine shared memory"));
   if ((rc = build(h))) return bail(rc);
   if (cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(b2g_fail(B2G_ECUDA, "auto-encoder create sync"));
   *out = h;
@@ -868,6 +920,53 @@ int b2g_autoencoder_predict(b2g_autoencoder* h, const float* imgs, int n, float*
     memcpy(out + s * HW, h->pin, m * HW * sizeof(float));
   }
   return 0;
+}
+
+int b2g_debug_autoencoder_tensor(b2g_autoencoder* h, int layer, int which, float* out, int64_t numel, int32_t* on_tc) {
+  if (!h) return b2g_fail(B2G_EINVAL, "null handle");
+  if (layer < 0 || layer >= (int)h->L.size()) return b2g_fail(B2G_EINVAL, "layer out of range");
+  const AeLayer& y = h->L[layer];
+  const size_t N = h->cfg.max_batch;
+  const float* src = nullptr;
+  size_t n = 0;
+  const bool conv = y.kind == ENC_CONV || y.kind == DEC_CONV || y.kind == OUT_CONV;
+  switch (which) {
+    case 0: src = y.in; n = conv ? N * y.g.hp * y.g.wp * y.g.in_c : N * y.in_ld; break;
+    case 1:
+      src = y.act;
+      n = y.kind == DEC_CONV ? N * y.g.out_h * y.g.out_w * y.g.f : y.kind == ENC_DENSE ? N * h->zs : y.kind == DEC_DENSE ? N * y.g.f : 0;
+      break;
+    case 2: src = y.D; n = conv ? N * y.dh * y.dw * y.g.f : N * y.dw; break;
+    default: return b2g_fail(B2G_EINVAL, "which must be 0 (input), 1 (activation) or 2 (pre-activation gradient)");
+  }
+  if (!src || n == 0) return b2g_fail(B2G_EINVAL, "layer " + std::to_string(layer) + " keeps no tensor " + std::to_string(which));
+  if (on_tc) {   // which engine runs the layer's forward, input gradient and weight gradient (-1: none)
+    on_tc[0] = on_tc[1] = on_tc[2] = -1;
+    for (const AeGemm& e : h->fwd_g) if (e.d.A == y.in && e.d.B == h->P + y.w_off) on_tc[0] = e.tc;
+    for (const AeGemm& e : h->bwd_g) {
+      if (e.d.A == y.D && e.d.B == h->P + y.w_off) on_tc[1] = e.tc;
+      if (e.wgrad && e.d.A == y.in && e.d.B == y.D) on_tc[2] = e.tc;
+    }
+  }
+  if (!out) return 0;
+  if (numel != (int64_t)n) return b2g_fail(B2G_EINVAL, "numel " + std::to_string(numel) + " != " + std::to_string(n));
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  CK(cudaMemcpy(out, src, n * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int64_t b2g_debug_autoencoder_tensor_numel(b2g_autoencoder* h, int layer, int which) {
+  if (!h || layer < 0 || layer >= (int)h->L.size()) return -1;
+  const AeLayer& y = h->L[layer];
+  const size_t N = h->cfg.max_batch;
+  const bool conv = y.kind == ENC_CONV || y.kind == DEC_CONV || y.kind == OUT_CONV;
+  if (which == 0) return (int64_t)(conv ? N * y.g.hp * y.g.wp * y.g.in_c : N * y.in_ld);
+  if (which == 1)
+    return (int64_t)(y.kind == DEC_CONV ? N * y.g.out_h * y.g.out_w * y.g.f : y.kind == ENC_DENSE ? N * h->zs
+                                                                              : y.kind == DEC_DENSE ? N * y.g.f : 0);
+  if (which == 2) return (int64_t)(conv ? N * y.dh * y.dw * y.g.f : N * y.dw);
+  return -1;
 }
 
 int b2g_autoencoder_step(b2g_autoencoder* h, const float* inputs, const float* targets, int n, float lr, int apply_update,

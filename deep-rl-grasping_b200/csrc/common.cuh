@@ -58,6 +58,8 @@ enum GemmFlags : int {
                                // > 0 / < 0 / == 0 (Keras' relu(x) - alpha * relu(-x) has gradient 0 at x = 0)
   GG_EPI_BIAS_TANH = 1 << 16,  // gg_simt_launch_tanh: C = tanh(acc + bias[n])
   GG_EPI_TANH_GRAD = 1 << 17,  // gg_simt_launch_tanh: C = acc * (1 - y^2), y = mask[kM[m] + kN[n]] a stored tanh output
+  GG_ACC64 = 1 << 18,          // gg_tc_launch: the auto-encoder training instantiations (GG_EPI_BIAS_LRELU, GG_EPI_LRELU_GRAD, and
+                               // GG_EPI_ATOMIC / GG_COLSUM adding fp32 split partials into double arrays behind C / colsum)
 };
 
 struct GemmDesc {
@@ -107,6 +109,8 @@ constexpr int GG_SIMT_BM = 64, GG_SIMT_BN = 64, GG_SIMT_BK = 16;
 cudaError_t gg_tc_launch(const GemmDesc* host_descs, int ndesc, int total_tiles, int mode_flags, int x3, int num_sms, cudaStream_t s);
 constexpr int GG_TC_MAX_DESCS = 16;
 int gg_tc_smem_bytes();
+// sets the shared-memory opt-in of the GG_ACC64 instantiations (before a graph capture launches them)
+cudaError_t gg_tc_acc64_init();
 constexpr int GG_TC_BM = 128, GG_TC_BN = 64, GG_TC_BK = 64;
 
 // ---------------------------------------------------------------------------------------------

@@ -166,12 +166,17 @@ __device__ __forceinline__ TileInfo tile_info(const DescPack& pk, int tile) {
 }
 
 // enc: the encoder forward's instantiation (planes only, encoder.cu): adds the GG_EPI_BIAS_LRELU epilogue and lets a descriptor
-// without C write only its BF16 planes (C_hi / C_lo: the next layer's input).  Every other launch runs enc = false, whose code
-// is the engine as it was before the flag existed.
-template <bool a_rvec, bool b_rvec, bool planes, bool enc = false>
+// without C write only its BF16 planes (C_hi / C_lo: the next layer's input).
+// ae: the auto-encoder training instantiations (register-staged fp32 operands only, autoencoder.cu, GG_ACC64): the
+// GG_EPI_BIAS_LRELU epilogue, the LeakyReLU-derivative epilogue GG_EPI_LRELU_GRAD (C = acc * g(mask), g = 1 / alpha / 0 for a
+// stored LeakyReLU output > 0 / < 0 / == 0), and GG_EPI_ATOMIC / GG_COLSUM adding each split's fp32 partial sums into DOUBLE
+// arrays behind C / colsum with double atomics.  Every other launch runs enc = ae = false, whose code is the engine as it was
+// before the flags existed.
+template <bool a_rvec, bool b_rvec, bool planes, bool enc = false, bool ae = false>
 __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const __grid_constant__ DescPack pk, int x3) {
   constexpr int NPROD = Roles<planes>::NPROD, MMA_WARP = Roles<planes>::MMA_WARP, NEPI = Roles<planes>::NEPI;
   constexpr int EPI_COLS = Roles<planes>::EPI_COLS;
+  constexpr int MASKF = ae ? (GG_EPI_MASK | GG_EPI_LRELU_GRAD) : GG_EPI_MASK;   // flags that read mask[kM[m] + kN[n]]
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_full[STAGES], bar_empty[STAGES];
   __shared__ int s_cn[TN], s_kn[TN];
@@ -529,10 +534,18 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
       }
       if (do_colsum && b_thread) {           // bias gradients: column sums of the B operand rows of this r-range
         const int nb = ti.n0 + 4 * qb;
-        if (nb + 0 < d.N) atomicAdd(d.colsum + nb + 0, csum.x);
-        if (nb + 1 < d.N) atomicAdd(d.colsum + nb + 1, csum.y);
-        if (nb + 2 < d.N) atomicAdd(d.colsum + nb + 2, csum.z);
-        if (nb + 3 < d.N) atomicAdd(d.colsum + nb + 3, csum.w);
+        if (ae) {
+          double* cs = reinterpret_cast<double*>(d.colsum);
+          if (nb + 0 < d.N) atomicAdd(cs + nb + 0, (double)csum.x);
+          if (nb + 1 < d.N) atomicAdd(cs + nb + 1, (double)csum.y);
+          if (nb + 2 < d.N) atomicAdd(cs + nb + 2, (double)csum.z);
+          if (nb + 3 < d.N) atomicAdd(cs + nb + 3, (double)csum.w);
+        } else {
+          if (nb + 0 < d.N) atomicAdd(d.colsum + nb + 0, csum.x);
+          if (nb + 1 < d.N) atomicAdd(d.colsum + nb + 1, csum.y);
+          if (nb + 2 < d.N) atomicAdd(d.colsum + nb + 2, csum.z);
+          if (nb + 3 < d.N) atomicAdd(d.colsum + nb + 3, csum.w);
+        }
       }
     }
   } else {
@@ -553,7 +566,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
     uint32_t gcm = 0;                              // ring chunk counter, continuous across tiles
     int pinned_p = -1, dflags = 0, dN = 0;
     float* dC = nullptr; uint16_t* dChi = nullptr; uint16_t* dClo = nullptr; const float* dmask = nullptr;
-    float dalpha = 0.f;                            // enc: LeakyReLU slope
+    float dalpha = 0.f;                            // enc, ae: LeakyReLU slope
     const uint32_t stg = ring + STAGES * STAGE_BYTES + (uint32_t)ew * (32 * EPI_COLS * 4);
     int staged_n0 = -1, st_col = -2;               // which (column tables, column block) the staged copies belong to
     // Everything a tile's epilogue needs from global memory besides the mask -- tile coordinates, this lane's row
@@ -579,7 +592,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
       e.ok = m2 < d2.M;
       if (e.ok) e.cm = d2.cM[m2];
       const int* kMp = d2.kM;
-      e.km_same = !((fl & GG_EPI_MASK) && kMp);
+      e.km_same = !((fl & MASKF) && kMp);
       if (e.ok && !e.km_same) e.km = kMp[m2];
       if (et < TN) {
         const int n = e.ti.n0 + et;
@@ -591,7 +604,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
         }
       } else if (et < 2 * TN) {
         const int n = e.ti.n0 + et - TN;
-        if ((fl & (enc ? GG_EPI_BIAS_RELU | GG_EPI_BIAS_LRELU : GG_EPI_BIAS_RELU)) && n < d2.N) e.t_bias = d2.bias[n];
+        if ((fl & (enc || ae ? GG_EPI_BIAS_RELU | GG_EPI_BIAS_LRELU : GG_EPI_BIAS_RELU)) && n < d2.N) e.t_bias = d2.bias[n];
       }
       return e;
     };
@@ -618,7 +631,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
       if (ti.p != pinned_p) {      // register copies of everything the store loops need from the descriptor
         dflags = pin(d.flags); dN = pin(d.N);
         dC = pin(d.C); dChi = pin(d.C_hi); dClo = pin(d.C_lo); dmask = pin(d.mask);
-        if (enc) dalpha = d.alpha;
+        if (enc || ae) dalpha = d.alpha;
         pinned_p = ti.p;
       }
       // column split between the two warps of a row quarter (8 epilogue warps, planes mode): 32 + 32 columns,
@@ -703,7 +716,7 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
               const float4 bb = *reinterpret_cast<const float4*>(&s_bias[cb + 4 * g]);
               o.x = fmaxf(o.x + bb.x, 0.f); o.y = fmaxf(o.y + bb.y, 0.f); o.z = fmaxf(o.z + bb.z, 0.f); o.w = fmaxf(o.w + bb.w, 0.f);
             }
-            if (enc && (dflags & GG_EPI_BIAS_LRELU)) {     // gg_simt's order: v + bias, then v > 0 ? v : alpha * v
+            if ((enc || ae) && (dflags & GG_EPI_BIAS_LRELU)) {     // gg_simt's order: v + bias, then v > 0 ? v : alpha * v
               const float4 bb = *reinterpret_cast<const float4*>(&s_bias[cb + 4 * g]);
               o.x += bb.x; o.y += bb.y; o.z += bb.z; o.w += bb.w;
               o.x = o.x > 0.f ? o.x : dalpha * o.x; o.y = o.y > 0.f ? o.y : dalpha * o.y;
@@ -722,9 +735,14 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
             float o = __uint_as_float(v[j]);
             const int cnj = s_cn[cb + j];
             if (dflags & GG_EPI_BIAS_RELU) o = fmaxf(o + s_bias[cb + j], 0.f);
-            if (enc && (dflags & GG_EPI_BIAS_LRELU)) { o += s_bias[cb + j]; o = o > 0.f ? o : dalpha * o; }
+            if ((enc || ae) && (dflags & GG_EPI_BIAS_LRELU)) { o += s_bias[cb + j]; o = o > 0.f ? o : dalpha * o; }
             if (dflags & GG_EPI_MASK) o = dmask[km + s_kn[cb + j]] > 0.f ? o : 0.f;
-            if (dflags & GG_EPI_ATOMIC) atomicAdd(dC + cm + cnj, o);
+            if (ae && (dflags & GG_EPI_LRELU_GRAD)) {
+              const float mv = dmask[km + s_kn[cb + j]];
+              o = mv > 0.f ? o : (mv < 0.f ? o * dalpha : 0.f);
+            }
+            if (ae && (dflags & GG_EPI_ATOMIC)) atomicAdd(reinterpret_cast<double*>(dC) + cm + cnj, (double)o);
+            else if (dflags & GG_EPI_ATOMIC) atomicAdd(dC + cm + cnj, o);
             else if (!enc || dC) dC[cm + cnj] = o;
             if (dChi) {
               const __nv_bfloat16 h = __float2bfloat16_rn(o);
@@ -757,16 +775,27 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
             if (okr[u]) {
               const uint32_t a = stg + (uint32_t)row * (EPI_COLS * 4) + (uint32_t)((c ^ (row & 7)) << 4);
               asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(o[u].x), "=f"(o[u].y), "=f"(o[u].z), "=f"(o[u].w) : "r"(a));
-              if (dflags & GG_EPI_MASK) mk[u] = (planes && rr0 == 0) ? mk0[u] : ldg4(dmask + km_r + kn);
+              if (dflags & MASKF) mk[u] = (planes && rr0 == 0) ? mk0[u] : ldg4(dmask + km_r + kn);
             }
           }
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
             if (!okr[u]) continue;
             float4 v4 = o[u];
-            v4.x = mk[u].x > 0.f ? v4.x : 0.f; v4.y = mk[u].y > 0.f ? v4.y : 0.f;
-            v4.z = mk[u].z > 0.f ? v4.z : 0.f; v4.w = mk[u].w > 0.f ? v4.w : 0.f;
-            if (dflags & GG_EPI_ATOMIC) {
+            if (ae && (dflags & GG_EPI_LRELU_GRAD)) {
+              v4.x = mk[u].x > 0.f ? v4.x : (mk[u].x < 0.f ? v4.x * dalpha : 0.f);
+              v4.y = mk[u].y > 0.f ? v4.y : (mk[u].y < 0.f ? v4.y * dalpha : 0.f);
+              v4.z = mk[u].z > 0.f ? v4.z : (mk[u].z < 0.f ? v4.z * dalpha : 0.f);
+              v4.w = mk[u].w > 0.f ? v4.w : (mk[u].w < 0.f ? v4.w * dalpha : 0.f);
+            } else {
+              v4.x = mk[u].x > 0.f ? v4.x : 0.f; v4.y = mk[u].y > 0.f ? v4.y : 0.f;
+              v4.z = mk[u].z > 0.f ? v4.z : 0.f; v4.w = mk[u].w > 0.f ? v4.w : 0.f;
+            }
+            if (ae && (dflags & GG_EPI_ATOMIC)) {
+              double* cp = reinterpret_cast<double*>(dC) + cmr[u] + cn;
+              atomicAdd(cp + 0, (double)v4.x); atomicAdd(cp + 1, (double)v4.y); atomicAdd(cp + 2, (double)v4.z);
+              atomicAdd(cp + 3, (double)v4.w);
+            } else if (dflags & GG_EPI_ATOMIC) {
               float* cp = dC + cmr[u] + cn;
               atomicAdd(cp + 0, v4.x); atomicAdd(cp + 1, v4.y); atomicAdd(cp + 2, v4.z); atomicAdd(cp + 3, v4.w);
             } else if (!enc || dC) {
@@ -787,23 +816,36 @@ __global__ void __launch_bounds__(Roles<planes>::NTHREADS, 1) gg_tc_kernel(const
   }
 }
 
-template <bool AR, bool BR, bool PL, bool ENC = false>
-cudaError_t launch_mode(const DescPack& pk, int x3, int num_sms, cudaStream_t s) {
+template <bool AR, bool BR, bool PL, bool ENC = false, bool AE = false>
+cudaError_t set_smem_attr() {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gg_tc_kernel<AR, BR, PL, ENC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(gg_tc_kernel<AR, BR, PL, ENC, AE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
+  return cudaSuccess;
+}
+
+template <bool AR, bool BR, bool PL, bool ENC = false, bool AE = false>
+cudaError_t launch_mode(const DescPack& pk, int x3, int num_sms, cudaStream_t s) {
+  if (cudaError_t e = set_smem_attr<AR, BR, PL, ENC, AE>()) return e;
   const int grid = pk.total_tiles < num_sms ? pk.total_tiles : num_sms;
-  return launch_pdl(gg_tc_kernel<AR, BR, PL, ENC>, dim3(grid), dim3(Roles<PL>::NTHREADS), SMEM_BYTES, s, pdl_enabled(), pk, x3);
+  return launch_pdl(gg_tc_kernel<AR, BR, PL, ENC, AE>, dim3(grid), dim3(Roles<PL>::NTHREADS), SMEM_BYTES, s, pdl_enabled(), pk, x3);
 }
 }  // namespace
 
 int gg_tc_smem_bytes() { return SMEM_BYTES; }
 
+cudaError_t gg_tc_acc64_init() {
+  if (cudaError_t e = set_smem_attr<true, false, false, false, true>()) return e;
+  if (cudaError_t e = set_smem_attr<true, true, false, false, true>()) return e;
+  return set_smem_attr<false, false, false, false, true>();
+}
+
 // All problems of one launch share the operand-contiguity mode (flags & (GG_A_RVEC | GG_B_RVEC)).  GG_PLANES | GG_EPI_BIAS_LRELU
-// selects the encoder forward's instantiation.
+// selects the encoder forward's instantiation, GG_ACC64 the auto-encoder training's (A r-contiguous, or both operands
+// m- / n-contiguous: the weight gradients).
 // host_descs: the group's descriptors (at most GG_TC_MAX_DESCS), passed as a __grid_constant__ pack.
 cudaError_t gg_tc_launch(const GemmDesc* host_descs, int ndesc, int total_tiles, int mode_flags, int x3, int num_sms, cudaStream_t s) {
   if (total_tiles <= 0) return cudaSuccess;
@@ -814,6 +856,12 @@ cudaError_t gg_tc_launch(const GemmDesc* host_descs, int ndesc, int total_tiles,
   pk.total_tiles = total_tiles;
   const bool ar = mode_flags & GG_A_RVEC, br = mode_flags & GG_B_RVEC;
   if ((mode_flags & GG_PLANES) && (mode_flags & GG_EPI_BIAS_LRELU)) return launch_mode<true, true, true, true>(pk, x3, num_sms, s);
+  if (mode_flags & GG_ACC64) {
+    if (ar && br) return launch_mode<true, true, false, false, true>(pk, x3, num_sms, s);
+    if (ar) return launch_mode<true, false, false, false, true>(pk, x3, num_sms, s);
+    if (!br) return launch_mode<false, false, false, false, true>(pk, x3, num_sms, s);
+    return cudaErrorInvalidValue;
+  }
   if (mode_flags & GG_PLANES) return launch_mode<true, true, true>(pk, x3, num_sms, s);
   if (ar && br) return launch_mode<true, true, false>(pk, x3, num_sms, s);
   if (ar) return launch_mode<true, false, false>(pk, x3, num_sms, s);

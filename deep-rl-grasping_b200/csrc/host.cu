@@ -84,7 +84,7 @@ void gg_tc_columns(GemmDesc& d, const std::map<const int*, std::vector<int>>& ho
       return true;
     };
     bool ok = (d.N % 4 == 0) && grp4(d.cN, d.N) && mult4(d.cM, d.M);
-    if (ok && (d.flags & GG_EPI_MASK)) ok = (!d.kN || grp4(d.kN, d.N)) && (!d.kM || mult4(d.kM, d.M));
+    if (ok && (d.flags & (GG_EPI_MASK | GG_EPI_LRELU_GRAD))) ok = (!d.kN || grp4(d.kN, d.N)) && (!d.kM || mult4(d.kM, d.M));
     if (ok) d.flags |= GG_CN_AFFINE4;
   }
   {   // column-table identity (gg_tc.cu epilogue): descriptors with the same tables never trigger a re-stage

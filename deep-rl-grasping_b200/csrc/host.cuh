@@ -66,8 +66,8 @@ int finalize_tiles(GemmGroup& g, std::vector<void*>& allocs, cudaStream_t s, int
 // column tables the gg_tc.cu epilogue stages, so consecutive tiles of such descriptors do not re-stage them.
 using ColIds = std::map<std::tuple<const void*, const void*, const void*, int>, int>;
 // The descriptor fields derived from its tables rather than given by the caller: GG_CN_AFFINE4 (set when the host copies in
-// host_tabs show N % 4 == 0, cN contiguous in aligned groups of 4 and cM a multiple of 4, and under GG_EPI_MASK the same of
-// kN and kM when given) and col_id (new tables take the next id of col_ids).
+// host_tabs show N % 4 == 0, cN contiguous in aligned groups of 4 and cM a multiple of 4, and under GG_EPI_MASK or
+// GG_EPI_LRELU_GRAD the same of kN and kM when given) and col_id (new tables take the next id of col_ids).
 void gg_tc_columns(GemmDesc& d, const std::map<const int*, std::vector<int>>& host_tabs, ColIds& col_ids);
 
 // Captures what issue() enqueues on s into a graph and instantiates it into *exec.  A failing issue() ends the capture and

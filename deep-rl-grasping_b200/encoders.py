@@ -126,12 +126,22 @@ class Encoder(object):
 
     ``precision`` is the arithmetic of ``encode`` and of the observe-path stage a learner copies from this encoder: "fp32"
     (fp32 FFMA on the CUDA cores, the default) or "bf16x3" (the tensor-core engine, BF16 hi/lo operand splits summed in fp32:
-    about 2^-16 relative per layer).  ``train``, ``test`` and ``predict`` run in fp32 either way."""
+    about 2^-16 relative per layer).
 
-    def __init__(self, config, max_batch: int = 1, device: int = 0, seed: Optional[int] = None, precision: str = "fp32"):
+    ``train_precision`` is the arithmetic of the training handle behind ``train``, ``test``, ``predict`` and ``step``:
+    "fp32" (every product exact in fp32, summed in double on the CUDA cores, the default) or "bf16x3" (every conv and dense
+    contraction but conv1's forward and weight gradient and the one-filter output conv on the tensor-core engine: each
+    element within about 2^-15 of the sum of |products| of its contraction).  The two keywords are independent: a
+    ``precision="bf16x3"`` encoder still trains in fp32 unless ``train_precision`` says otherwise."""
+
+    def __init__(self, config, max_batch: int = 1, device: int = 0, seed: Optional[int] = None, precision: str = "fp32",
+                 train_precision: str = "fp32"):
         if precision not in ENCODER_PRECISIONS:
             raise ValueError(f"precision must be one of {sorted(ENCODER_PRECISIONS)}, got {precision!r}")
+        if train_precision not in ENCODER_PRECISIONS:
+            raise ValueError(f"train_precision must be one of {sorted(ENCODER_PRECISIONS)}, got {train_precision!r}")
         self.precision = precision
+        self.train_precision = train_precision
         self._handle = C.c_void_p()
         self._ae = C.c_void_p()
         self._ae_batch = 0
@@ -183,7 +193,7 @@ class SimpleAutoEncoder(Encoder):
             self._close_ae()
             cfg = _lib.EncoderCfg.from_buffer_copy(self._cfg)
             cfg.max_batch = max(batch, self._train_batch)
-            _lib.check(self._lib.b2g_autoencoder_create(C.byref(cfg), C.byref(self._ae)))
+            _lib.check(self._lib.b2g_autoencoder_create2(C.byref(cfg), ENCODER_PRECISIONS[self.train_precision], C.byref(self._ae)))
             self._ae_batch = cfg.max_batch
             self._push_weights()
         return self._ae

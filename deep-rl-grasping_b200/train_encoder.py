@@ -1,8 +1,11 @@
 """Command line of the reference's encoder training script (manipulation_main/training/train_encoder.py:30-65), with the
 model on the GPU (``b200grasp.encoders.SimpleAutoEncoder``).
 
-    python -m b200grasp.train_encoder <model_dir> train --config <config.yaml>
-    python -m b200grasp.train_encoder <model_dir> test
+    python -m b200grasp.train_encoder <model_dir> train --config <config.yaml> [--train_precision {fp32,bf16x3}]
+    python -m b200grasp.train_encoder <model_dir> test [--train_precision {fp32,bf16x3}]
+
+``--train_precision`` picks the arithmetic of the training handle (``SimpleAutoEncoder(train_precision=...)``): fp32 (the
+default) or bf16x3 (the tensor-core engine).
 
 The dataset is the reference's pickle ``{'train' | 'test': {'rgb', 'depth', 'masks'}}`` at the config's ``data_path``.
 ``plot_history`` and ``visualize`` (matplotlib) are not provided.
@@ -46,7 +49,7 @@ def train(args):
     config = _load_yaml(args.config)
     model_dir = os.path.expanduser(args.model_dir)
     os.makedirs(model_dir, exist_ok=True)
-    model = encoders.SimpleAutoEncoder(config, seed=args.seed)
+    model = encoders.SimpleAutoEncoder(config, seed=args.seed, train_precision=args.train_precision)
     with open(os.path.join(model_dir, "config.yaml"), "w") as f:
         yaml.safe_dump(config, f, default_flow_style=False)
     train_imgs = _preprocess_depth(_load_data_set(config["data_path"], test=False))
@@ -55,7 +58,7 @@ def train(args):
 
 def test(args):
     config = _load_yaml(os.path.join(os.path.expanduser(args.model_dir), "config.yaml"))
-    model = encoders.SimpleAutoEncoder(config)
+    model = encoders.SimpleAutoEncoder(config, train_precision=args.train_precision)
     model.load_weights(args.model_dir)
     test_imgs = _preprocess_depth(_load_data_set(config["data_path"], test=True))
     loss = model.test(test_imgs, test_imgs)
@@ -73,6 +76,9 @@ def main(argv=None):
     train_parser.set_defaults(func=train)
     test_parser = subparsers.add_parser("test")
     test_parser.set_defaults(func=test)
+    for p in (train_parser, test_parser):
+        p.add_argument("--train_precision", choices=sorted(encoders.ENCODER_PRECISIONS), default="fp32",
+                       help="arithmetic of the training handle: fp32 (CUDA cores) or bf16x3 (tensor cores)")
     args = parser.parse_args(argv)
     if not hasattr(args, "func"):
         parser.error("choose a sub-command: train or test")

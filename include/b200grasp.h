@@ -757,7 +757,19 @@ int b2g_trpo_set_obs_encoder(b2g_trpo* h, const b2g_encoder* enc, int tail);
  * batch of any call.  Calls that run the model return B2G_ESTATE until every layer has weights.
  * ------------------------------------------------------------------------------------------------------------ */
 typedef struct b2g_autoencoder b2g_autoencoder;
-int b2g_autoencoder_create(const b2g_encoder_cfg* cfg, b2g_autoencoder** out);
+int b2g_autoencoder_create(const b2g_encoder_cfg* cfg, b2g_autoencoder** out);     /* = create2(cfg, B2G_PREC_FP32_SIMT, out) */
+/* The training handle at a chosen precision (b2g_autoencoder_step, _train_epoch, _evaluate and _predict all run at it):
+ *   B2G_PREC_FP32_SIMT  every contraction's exact fp32 products summed in double on the CUDA cores (what _create builds);
+ *   B2G_PREC_BF16X3     every conv and dense contraction whose operands come in 16-byte groups of 4 values on the wgmma
+ *                       engine: operands split into BF16 hi + lo in registers, hi*hi + hi*lo + lo*hi summed in fp32 per
+ *                       64-row chunk; weight-gradient split-R partials (and the bias gradients' fp32 partial column sums)
+ *                       added into the double gradient arena with double atomics.  conv1's forward and weight gradient (one
+ *                       input channel) and the output conv (one filter) stay on the CUDA cores.  Each element is within
+ *                       about 2^-15 of the sum of |products| of its contraction, not of its value: conv1's kernel gradient,
+ *                       a sum whose terms cancel by a factor of several hundred, is correspondingly less precise.
+ * B2G_EINVAL before any CUDA call for B2G_PREC_BF16 (single-pass BF16 training is not offered), any other value and every
+ * geometry _create refuses; bf16x3 accepts every geometry _create accepts (filters % 4 == 0 gives the 4-value groups). */
+int b2g_autoencoder_create2(const b2g_encoder_cfg* cfg, int32_t precision, b2g_autoencoder** out);
 int b2g_autoencoder_destroy(b2g_autoencoder* h);
 int b2g_autoencoder_n_layers(const b2g_autoencoder* h);
 int b2g_autoencoder_layer_shape(const b2g_autoencoder* h, int layer, int64_t* kernel_numel, int64_t* bias_numel);
@@ -780,6 +792,16 @@ int b2g_autoencoder_predict(b2g_autoencoder* h, const float* imgs, int n, float*
 /* one step on a host batch (targets == NULL: the inputs); apply_update == 0 only computes loss and gradients */
 int b2g_autoencoder_step(b2g_autoencoder* h, const float* inputs, const float* targets, int n, float lr, int apply_update,
                          double* loss);
+/* debug: a device tensor of layer `layer` as the last call left it, the whole max_batch buffer copied to out (numel elements):
+ * which = 0 the input the layer's contractions read (convs: the zero-bordered NHWC buffer [N][hp][wp][in_c], a decoder conv's
+ * holding the upsampled map; dense: rows [N][in_ld]), 1 the stored LeakyReLU output where no bordered buffer holds it
+ * (encoder dense [N][round4(encoding_dim)], decoder dense [N][h*w*c], decoder convs [N][out_h][out_w][f]), 2 the gradient of
+ * the pre-activation (convs: [N][in_h + pad_t + k - 1][in_w + pad_l + k - 1][f] with output (oy, ox) at (oy*s + k-1,
+ * ox*s + k-1); dense: rows [N][round4(f)]).  on_tc (optional, 3 ints) receives whether the layer's forward, input gradient and
+ * weight gradient run on the wgmma engine (1), on the CUDA cores (0) or not as a contraction (-1).  out == NULL only fills
+ * on_tc.  b2g_debug_autoencoder_tensor_numel gives numel (-1: no such tensor). */
+int b2g_debug_autoencoder_tensor(b2g_autoencoder* h, int layer, int which, float* out, int64_t numel, int32_t* on_tc);
+int64_t b2g_debug_autoencoder_tensor_numel(b2g_autoencoder* h, int layer, int which);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Bring-up hook (not on the product path): C[M,N] = A[M,K] * B[N,K]^T through the wgmma engine; host pointers,
